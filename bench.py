@@ -21,6 +21,9 @@ N > 1   ONE planning problem on all ranks: the same nominal policy everywhere, N
              with the reference's own thread rule (nproc - 3) and the fp32 instantiation beside it.
 
 --impl reference times that CPU path as its own arm.
+--dump-outputs DIR writes what the timed path returned in its last step (returns, failure flags, ranking and, at N = 1,
+             every candidate's trajectory; the winner trajectory of the end-to-end call) plus the inputs of that step as
+             DIR/<name>.npy (float32 / float64), so that two builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -98,7 +101,7 @@ def algorithmic_bytes_per_env_step(m, P):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
     Q = "clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown," \
         "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
 
@@ -316,10 +319,30 @@ def model_fidelity(m):
 
 
 def hbm_peak():
-    peaks_path = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(peaks_path):
-        return json.load(open(peaks_path))["hbm_gbs"], "measured (MEASURED_PEAKS.json hbm_gbs, burst copy)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "NVIDIA H100 SXM data sheet (HBM3, 3.35 TB/s), not a measured copy rate"
+
+
+def gpu_identity(index):
+    """Name and power limit of the card the numbers were measured on (part of every absolute number)."""
+    import torch
+    out = {"name": torch.cuda.get_device_name(index), "power_limit_w": None}
+    try:
+        r = subprocess.run(["nvidia-smi", "-i", str(index), "--query-gpu=power.limit", "--format=csv,noheader,nounits"],
+                           capture_output=True, text=True, timeout=30)
+        out["power_limit_w"] = float(r.stdout.strip().splitlines()[0])
+    except (OSError, ValueError, IndexError, subprocess.SubprocessError):
+        pass
+    return out
+
+
+def dump_outputs(d, arrays):
+    """arrays: name -> array; integer / flag arrays are stored as float64 / float32 (exact), everything as .npy."""
+    os.makedirs(d, exist_ok=True)
+    for name, a in arrays.items():
+        a = np.asarray(a)
+        if a.dtype not in (np.float32, np.float64):
+            a = a.astype(np.float64 if a.dtype.itemsize >= 4 else np.float32)
+        np.save(os.path.join(d, name + ".npy"), a)
 
 
 def run_reference(args, rank, world):
@@ -359,7 +382,10 @@ def main():
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-probes", action="store_true", help="skip the iLQG / Humanoid Track probes (profiling runs)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's outputs and inputs as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     args.warmup = max(args.warmup, 3)
     rank = int(os.environ.get("RANK", 0)); local = int(os.environ.get("LOCAL_RANK", 0))
     world = int(os.environ.get("WORLD_SIZE", 1))
@@ -390,7 +416,7 @@ def main():
     # the burn-in runs on this rank's GPU alone with 256 candidates: deterministic, so every rank holds the same nominal
     m, state, mocap, knots, kt, nominal_return = load_inputs(eng, n_iter, n_cand=n_total)
     P = knots[0].shape[1]
-    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device="cuda")  # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device="cuda")  # > 50 MB L2
 
     def barrier():
         torch.cuda.synchronize()
@@ -422,11 +448,18 @@ def main():
             eng.launch_resident()
             eng.sync()
         else:
-            eng.rollout_spline_sharded(state, 0.0, mocap, knots[it], kt, INTERP, HORIZON)
+            dev_out = eng.rollout_spline_sharded(state, 0.0, mocap, knots[it], kt, INTERP, HORIZON)
         if it >= args.warmup:
             kern_ms.append(eng.last_kernel_ms)
     barrier()
     wall = time.perf_counter() - t_wall0
+    dumps = {}
+    if args.dump_outputs:                 # the device-timed path's last step (the resident inputs are knots[0] at N = 1)
+        if world == 1:
+            dev_out = eng.read_returns()
+            dumps.update({"device_" + k: v for k, v in eng.fetch_all().items()})
+            dumps.update(input_device_knots=knots[0])
+        dumps.update(device_returns=dev_out[0], device_failure=dev_out[1], device_order=dev_out[2])
     gpu_launches = eng.launch_count - launches0
     ms_per_step = max_over_ranks(float(np.sum(kern_ms))) / args.steps
     value = n_total * HORIZON / (ms_per_step * 1e-3)
@@ -452,6 +485,10 @@ def main():
         ret, order, best = e2e_step(args.warmup + it)
     barrier()
     e2e_value = n_total * HORIZON / max_over_ranks((time.perf_counter() - t0) / args.steps)
+    if args.dump_outputs:
+        dumps.update(e2e_returns=ret, e2e_order=order, input_state=state, input_mocap=mocap, input_knot_times=kt,
+                     input_e2e_knots=knots[args.warmup + args.steps - 1])
+        dumps.update({"e2e_winner_" + k: v for k, v in best.items()})
     clk = clocks.stop()      # samples cover both timed regions (device-timed and end-to-end), 50 ms apart
 
     # ---------------- N > 1: one-problem evidence + strong scaling of the 256-candidate problem
@@ -498,17 +535,6 @@ def main():
                 "algorithmic_bytes_per_env_step": algorithmic_bytes_per_env_step(m, P),
                 "note": "latency/occupancy-bound by construction: 256 candidates, 64 dependent steps each; one main warp per candidate plus helper warps for the wide phases (DESIGN.md section 5)",
                 "kernel_shape": int(eng.last_kernel_shape)}
-    for prof in ("traffic_r02.json", "traffic_r01.json"):
-        pp = os.path.join(ROOT, "profiles", prof)
-        if os.path.exists(pp):
-            pj = json.load(open(pp))
-            roofline["traffic"] = pj.get("dram_bytes_per_launch")
-            # what actually bounds the kernel (from the committed ncu capture of the same launch): issue-slot use and stalls
-            roofline["latency_bound_evidence"] = {k: pj[k] for k in ("smsp__issue_active_pct", "sm__warps_active_pct_of_peak",
-                                                                     "warp_instructions_per_env_step", "warp_instructions_per_env_step_main_warp",
-                                                                     "stall_mix_pct", "stall_mix_pct_main_warp",
-                                                                     "counters_from") if k in pj}
-            break
     cores = usable_cores()
     probes = world == 1 and not args.no_probes
     ilqg = ilqg_probe(m, eng, mocap, cores) if probes else None
@@ -581,7 +607,9 @@ def main():
                                     "fetch_trajectory_sharded(winner: ncclBroadcast), host buffers")},
             "clocks": clk, "e2e": {"value": e2e_value, "unit": UNIT, "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h},
             "gpu_launches": int(gpu_launches), "roofline": roofline, "cpu_baseline": cpu, "parity": parity, "ilqg": ilqg, "humanoid_track": config3, "shadow_reorient_standin": config5,
-            "multi_gpu": multi, "wall_s_timed_region": wall}
+            "multi_gpu": multi, "wall_s_timed_region": wall, "gpu": gpu_identity(local)}
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, dumps)
     print(json.dumps(line), flush=True)
     if world > 1:
         dist.destroy_process_group()

@@ -1,4 +1,4 @@
-/* mjpc_b200.h - C ABI of the B200 rollout engine (libmjpc_b200.so).
+/* mjpc_b200.h - C ABI of the H100 (sm_90a) rollout engine (libmjpc_b200.so).
  *
  * The engine replaces the data-parallel hot path of MJPC and nothing else.  std::function policies and
  * virtual ResidualFn objects cannot cross to the device, so every entry point takes *data* and sits exactly

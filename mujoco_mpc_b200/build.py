@@ -1,4 +1,4 @@
-"""Build the CUDA engine in-tree: nvcc -> mujoco_mpc_b200/csrc/libmjpc_b200.so (sm_100a only)."""
+"""Build the CUDA engine in-tree: nvcc -> mujoco_mpc_b200/csrc/libmjpc_b200.so (sm_90a, H100, only)."""
 from __future__ import annotations
 
 import os
@@ -8,8 +8,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 SO = os.environ.get("MJPC_B200_SO") or os.path.join(CSRC, "libmjpc_b200.so")  # override: perf experiments only
 # -use_fast_math (approximate division / sqrt / sincos, flush-to-zero): the parity ablation with and without it is
-# profiles/parity_ablation.py -> profiles/r02_fast_math_ablation.txt; MJPC_B200_NO_FAST_MATH=1 builds the IEEE variant
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17"] + \
+# profiles/parity_ablation.py; MJPC_B200_NO_FAST_MATH=1 builds the IEEE variant
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17"] + \
              ([] if os.environ.get("MJPC_B200_NO_FAST_MATH") == "1" else ["-use_fast_math"]) + \
              os.environ.get("MJPC_B200_NVCC_EXTRA", "").split() + ["-Xcompiler", "-fPIC", "-shared"]
 

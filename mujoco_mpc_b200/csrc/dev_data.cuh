@@ -8,10 +8,10 @@
 
 #include "dev_model.h"
 
-// Code-footprint control (profiles/README.md "code footprint"): with one warp per scheduler every instruction-cache
+// Code-footprint control: with one warp per scheduler every instruction-cache
 // miss is exposed, and the Newton loop's straight-line code (fully unrolled by default) streams from L2 on every
 // iteration.  MJPC_ROLL marks loops whose unrolling buys no ILP worth its code size.
-#ifndef MJPC_NO_COMPACT   // -DMJPC_NO_COMPACT restores the fully unrolled build (profiles/r02_code_footprint.txt compares them)
+#ifndef MJPC_NO_COMPACT   // -DMJPC_NO_COMPACT restores the fully unrolled build (profiles/footprint.py measures the executed code)
 #define MJPC_COMPACT 1
 #endif
 #ifdef MJPC_COMPACT
@@ -87,7 +87,7 @@ enum { STATE_SATISFIED = 0, STATE_QUADRATIC, STATE_LINEARNEG, STATE_LINEARPOS, S
 //   [model floats nf][model ints ni][DevModel header][DevLayout][warp 0 state][warp 1 state] ...
 // All accessors derive their pointers from the g_smem symbol with 32-bit float indices, so the compiler emits
 // LDS/STS with shared-window addressing (pointers kept in a struct degrade to generic LD + 64-bit address
-// arithmetic: that was ~45 % of the executed instructions in the first profile, profiles/r01_v4_rollout_ncu.txt).
+// arithmetic: that was ~45 % of the executed instructions in the first profile).
 extern __shared__ __align__(16) float g_smem[];
 
 struct Ctx {
@@ -205,7 +205,7 @@ __device__ __forceinline__ void wide_post(const Ctx& c, int cmd) {
 }
 
 // ---------------------------------------------------------------------------------------- co-resident pairs
-// At 256 candidates 108 of the 148 SMs run two candidates, and the measured cost of sharing an SM is instruction
+// At 256 candidates 124 of the H100's 132 SMs run two candidates, and the measured cost of sharing an SM is instruction
 // fetch: two candidates at different places of the 124 KB-per-step code evict each other's lines, while two that
 // run the SAME code at the same time cost each other almost nothing (profiles/icache_probe.py).  The main warps of
 // the two candidates of an SM therefore keep in step through a 128-byte record in HBM (they are different CTAs):

@@ -46,7 +46,7 @@ struct mjpc_b200 {
   ModelPack pack;
   int maxN = 0, maxH = 0, maxP = 64;
   int warps_per_cta = 1;
-  int num_sms = 148;
+  int num_sms = 132;
   int static_spec = 0;   // 1 / 2: the model equals spec_quadruped.h / spec_humanoid_track.h -> static rollout kernel
   float* d_pack = nullptr;
   // inputs
@@ -274,7 +274,7 @@ __global__ void pack_slot_kernel(const float* __restrict__ ret, const unsigned c
 
 extern "C" {
 
-const char* mjpc_b200_version(void) { return "mjpc_b200 0.1.0 (sm_100a)"; }
+const char* mjpc_b200_version(void) { return "mjpc_b200 0.1.0 (sm_90a)"; }
 const char* mjpc_b200_last_error(void) { return g_last_error.c_str(); }
 
 // inside create(): a failing CUDA call must not leak the half-built handle

@@ -16,7 +16,7 @@ namespace mjpc_b200_host {
 struct iLQGSettings {                    // mjpc/planners/ilqg/settings.h:21-36
   double min_linesearch_step = 1.0e-3;
   // The reference's settings are 1e-6, one-sided, in fp64.  In fp32 that is below the rounding of the states; measured on
-  // the device (profiles/fd_gradient_check.py, profiles/r02_fd_gradient.txt): with 1e-3 one-sided iLQG does not improve the
+  // the device (profiles/fd_gradient_check.py): with 1e-3 one-sided iLQG does not improve the
   // Quadruped return at all, with CENTRED 3e-4 it follows the fp64 reference (0.124 vs 0.115 after 8 iterations from 0.324).
   double fd_tolerance = 3.0e-4;
   double min_regularization = 1.0e-6;

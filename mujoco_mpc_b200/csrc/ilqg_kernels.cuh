@@ -9,7 +9,7 @@
 //   backward_pass_kernel                  RiccatiStep recursion (mjpc/planners/ilqg/backward_pass.cc:65-250,
 //       mjpc/planners/ilqg/planner.cc:429-520): ONE CTA, strictly sequential in t (value function dependence),
 //       matrices resident in shared memory, box-QP ([EXT] mju_boxQP restated: projected Newton) on one warp.
-//       The n=36, m=12 products are fp32 CUDA-core FMAs: a tcgen05 tile is at least 64x8x8 per instruction with
+//       The n=36, m=12 products are fp32 CUDA-core FMAs: a Hopper wgmma tile is at least 64x8x8 per warpgroup with
 //       operands in swizzled shared-memory tiles and TF32 inputs, which for 36x36x36 products costs more in
 //       staging than the ~0.3 MFLOP per step it would accelerate, and TF32's 10-bit mantissa breaks the
 //       Riccati recursion's accuracy (DESIGN.md "tensor cores").
@@ -498,7 +498,7 @@ __device__ inline int box_qp_serial(float* res, float* R, int* index, const floa
 // ---- warp-parallel versions (warp 0 of the CTA; n <= 32; lane i owns element / row i).  Same algorithm and
 // constants as the serial code above; the left-looking Cholesky and the forward substitution subtract in the
 // same order as the serial loops, reductions are butterfly sums (identical in every lane, so control flow stays
-// warp-uniform).  The serial box-QP was 59 % of the backward pass (profiles/README.md, prof_r01_bp).
+// warp-uniform).  The serial box-QP dominated the backward pass before.
 __device__ inline float chol_warp(float* A, int n, int lane) {
   float minp = 3.4e38f;
   for (int j = 0; j < n; j++) {
@@ -606,8 +606,8 @@ __device__ inline int box_qp_warp(float* res, float* R, int* index, const float*
 //   K[m*n] Wx[n] Qx[n] Qu[m] du[m] Qd[m] qp_res[m] qp_R[m*m] qp_lo[m] qp_hi[m] scratch[8m] + index[m] ints
 // One CTA walks the 63 dependent Riccati steps; within a step the 36x36x36 products are spread over all threads.  The
 // thread count is a latency knob, not a throughput one: with 8 warps (2 per scheduler) the shared-memory load -> FMA
-// chains of the products were exposed (68.7 k cycles per step, profiles/r02_ilqg_ncu.txt); measured 256 / 512 / 1024
-// threads: 2.28 / 2.06 / 2.16 ms per sweep - the rest is the serial box-QP and gain solves between the barriers.
+// chains of the products were exposed; 512 threads measured faster than 256 and 1024 - the rest is the serial box-QP
+// and gain solves between the barriers.
 #ifndef MJPC_BP_THREADS
 #define MJPC_BP_THREADS 512
 #endif

@@ -1,4 +1,4 @@
-// rollout_kernels.cuh - the CUDA kernels of the hot path (sm_100a).
+// rollout_kernels.cuh - the CUDA kernels of the hot path (sm_90a).
 //
 //   rollout_kernel      one candidate trajectory per warp (generic) or per CTA of main + helper warps (static instances)
 //                       (Trajectory::Rollout / RolloutDiscrete,

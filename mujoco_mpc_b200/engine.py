@@ -1,7 +1,7 @@
 """ctypes binding of libmjpc_b200.so - the reference-facing call a user makes.
 
 Every method goes through the C ABI in include/mjpc_b200.h; there is no Python/NumPy compute path and no
-CPU fallback: if the library is missing or no B200 is visible, construction raises.
+CPU fallback: if the library is missing or no CUDA device is visible, construction raises.
 """
 from __future__ import annotations
 

@@ -10,7 +10,7 @@ Host-side, offline: nothing here runs per planning iteration.  The compiled
 model is serialised by :mod:`mujoco_mpc_b200.blob` and consumed by the CPU
 oracle (``oracle/``) and by the CUDA engine (``csrc/``) through the C ABI.
 
-Reference semantics followed (files under /root/reference):
+Reference semantics followed (files of google-deepmind/mujoco_mpc):
   * cost terms from leading ``<sensor><user>`` entries: mjpc/task.cc:147-248
   * ``residual_*`` numerics -> task parameters:        mjpc/task.cc:38-64
   * trace sensors named ``trace%d``:                   mjpc/task.cc:190-198

@@ -695,8 +695,8 @@ def synth_mocap(m, seed=0):
 def track_keyframes(keyframes_dir=None, synthetic=False):
     """The Humanoid Track mocap clips (mjpc/tasks/humanoid/tracking/keyframes/*.xml, tracking.cc:43-54).  Order of
     preference: an explicit directory (or $MJPC_B200_TRACK_KEYFRAMES) holding the reference's XML files, parsed here;
-    the committed fixture models/data/humanoid_track_keyframes.npz (the same data parsed by make_track_keyframes.py -
-    /root/reference does not exist on the GPU box); None -> the caller falls back to synth_mocap.
+    the committed fixture tests/golden/humanoid_track_keyframes.npz (the same data parsed by make_track_keyframes.py, so
+    that the task runs without the reference tree); None -> the caller falls back to synth_mocap.
     Returns (dict(mpos, qpos, qvel) | None, source string)."""
     import os
     if synthetic:
@@ -705,11 +705,12 @@ def track_keyframes(keyframes_dir=None, synthetic=False):
     if d:
         from .make_track_keyframes import parse_keyframes
         return parse_keyframes(d), "reference keyframes parsed from " + d
-    fx = os.path.join(os.path.dirname(os.path.abspath(__file__)), "data", "humanoid_track_keyframes.npz")
+    fx = os.path.join(os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))), "tests", "golden",
+                      "humanoid_track_keyframes.npz")
     if os.path.exists(fx):
         z = np.load(fx)
         return dict(mpos=z["mpos"].astype(float), qpos=z["qpos"].astype(float), qvel=z["qvel"].astype(float)), \
-            "reference keyframes (1889 CMU frames, fixture models/data/humanoid_track_keyframes.npz)"
+            "reference keyframes (1889 CMU frames, fixture tests/golden/humanoid_track_keyframes.npz)"
     return None, "synthetic clips (synth_mocap): fixture missing"
 
 

@@ -18,8 +18,8 @@ for rep in range(12):
         ret[on] = r
         if rep >= 2: ms[on].append(e.last_kernel_ms)
     if rep == 11:
-        st = e.fetch_stats(); c = st[:, 0] / 1.965e6
-        print("   (sync on) per-candidate ms min %.2f median %.2f max %.2f" % (c.min(), np.median(c), c.max()))
+        st = e.fetch_stats(); c = st[:, 0] / 1e6
+        print("   (last mode) per-candidate M cycles min %.2f median %.2f max %.2f" % (c.min(), np.median(c), c.max()))
 for k, v in ms.items():
     print("N=%d pair sync %s: kernel ms min %.3f median %.3f max %.3f" % (N, k, min(v), np.median(v), max(v)))
 print("returns bitwise equal:", all(np.array_equal(ret[modes[0]], ret[k]) for k in modes))

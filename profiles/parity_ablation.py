@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Parity of the library selected by MJPC_B200_SO (default: the in-tree build) on BASELINE config 2 inputs:
 teacher-forced per-step error, 256x64 return parity, Newton iterations, kernel time.  One JSON line.
-Used for the -use_fast_math ablation (profiles/r02_fast_math_ablation.txt):
+Used for the -use_fast_math ablation:
   MJPC_B200_NO_FAST_MATH=1 MJPC_B200_SO=$PWD/mujoco_mpc_b200/csrc/libmjpc_b200_ieee.so python -m mujoco_mpc_b200.build
   MJPC_B200_SO=... python profiles/parity_ablation.py <label>
 """

@@ -12,7 +12,7 @@ kn = np.concatenate([d["knots"]] * ((N + 255) // 256))[:N]
 for i in range(3):
     e.rollout_spline(d["state"], 0.0, d["mocap"], kn, d["kt"], 2, 64)
 st = e.fetch_stats()
-ms = st[:, 0] / 1.965e6; sm = st[:, 4]; slot = st[:, 5]; it = st[:, 1] / 64
+ms = st[:, 0] / 1e6; sm = st[:, 4]; slot = st[:, 5]; it = st[:, 1] / 64   # ms: M SM cycles
 print("kernel %.2f ms; SMs used %d; slots seen %s" % (e.last_kernel_ms, len(set(sm)), sorted(set(slot))))
 alone = np.array([np.sum(sm == s) == 1 for s in sm])
 same_sched = np.zeros(N, bool)
@@ -25,4 +25,4 @@ for s in set(sm):
 per_iter = ms / it
 for name, mask in (("alone on its SM", alone), ("shares SM, own scheduler", ~alone & ~same_sched), ("shares SM and scheduler", same_sched)):
     if mask.any():
-        print("%-28s n=%3d  ms median %.2f max %.2f | ms per (Newton iteration/step) median %.3f" % (name, mask.sum(), np.median(ms[mask]), ms[mask].max(), np.median(per_iter[mask])))
+        print("%-28s n=%3d  M cycles median %.2f max %.2f | M cycles per (Newton iteration/step) median %.3f" % (name, mask.sum(), np.median(ms[mask]), ms[mask].max(), np.median(per_iter[mask])))

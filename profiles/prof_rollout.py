@@ -16,6 +16,6 @@ print("kernel ms", ms[-1], "min", min(ms), "static", e.last_kernel_static)
 if len(sys.argv) > 2:
     np.save(sys.argv[2], ret)   # returns of this build (compared across experiment builds)
 st = e.fetch_stats()
-cyc = st[:, 0] / 1.965e6
-print("per-candidate ms: min %.2f median %.2f max %.2f ; newton iters/step mean %.2f max-cand %.2f ; ncon/step %.2f nefc/step %.2f" % (
+cyc = st[:, 0] / 1e6
+print("per-candidate M cycles: min %.2f median %.2f max %.2f ; newton iters/step mean %.2f max-cand %.2f ; ncon/step %.2f nefc/step %.2f" % (
     cyc.min(), np.median(cyc), cyc.max(), st[:, 1].mean() / 64, st[:, 1].max() / 64, st[:, 2].mean() / 64, st[:, 3].mean() / 64))

@@ -1,6 +1,6 @@
 """testspeed-style closed loop (mjpc/testspeed.cc:44-128): plan, act, step the plant, report wall time, x realtime and
 the average cost per step.  The plant is the fp64 oracle (test infrastructure - which is why this tool lives under
-profiles/ and not in the product package); the planner runs on the B200 engine (--backend b200) or on the oracle
+profiles/ and not in the product package); the planner runs on the CUDA engine (--backend b200) or on the oracle
 ThreadPool path (--backend oracle, CPU only).
 
   python profiles/testspeed.py --task quadruped --planner sampling --steps 200 --backend b200

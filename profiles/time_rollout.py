@@ -21,6 +21,6 @@ k2 = candidate_knots(pl.values, pl.sigma, pl.ctrlrange, 99, 256)
 for i in range(3):
     ret, fail, order = e.rollout_spline(state, 0.0, mocap, k2, pl.times, 2, 64)
 st = e.fetch_stats()
-cyc = st[:, 0] / 1.965e6
-print("   steady-nominal: kernel %.2f ms  newton/step %.2f  per-cand ms min/med/max %.1f/%.1f/%.1f  best return %.4f" % (
+cyc = st[:, 0] / 1e6
+print("   steady-nominal: kernel %.2f ms  newton/step %.2f  per-cand M cycles min/med/max %.1f/%.1f/%.1f  best return %.4f" % (
     e.last_kernel_ms, st[:, 1].mean() / 64, cyc.min(), np.median(cyc), cyc.max(), float(ret.min())))

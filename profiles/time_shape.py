@@ -13,5 +13,5 @@ ms = []
 for rep in range(12):
     e.rollout_spline(d["state"], 0.0, d["mocap"], kn, d["kt"], 2, 64)
     if rep >= 2: ms.append(e.last_kernel_ms)
-st = e.fetch_stats(); c = st[:, 0] / 1.965e6
-print("%s N=%d %s: kernel ms min %.3f median %.3f | per-candidate min %.2f median %.2f max %.2f" % (os.environ.get("MJPC_B200_SO", "default")[-12:], N, sys.argv[1], min(ms), np.median(ms), c.min(), np.median(c), c.max()))
+st = e.fetch_stats(); c = st[:, 0] / 1e6
+print("%s N=%d %s: kernel ms min %.3f median %.3f | per-candidate M cycles min %.2f median %.2f max %.2f" % (os.environ.get("MJPC_B200_SO", "default")[-12:], N, sys.argv[1], min(ms), np.median(ms), c.min(), np.median(c), c.max()))

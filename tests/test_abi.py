@@ -18,7 +18,7 @@ def test_header_symbols_exported():
         assert hasattr(lib, name), f"{name} declared in the header but not exported"
     assert sorted(EXPORTS) == declared
     lib.mjpc_b200_version.restype = ctypes.c_char_p
-    assert b"sm_100a" in lib.mjpc_b200_version()
+    assert b"sm_90a" in lib.mjpc_b200_version()
 
 
 def test_no_cpu_fallback():

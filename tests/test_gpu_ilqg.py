@@ -250,7 +250,7 @@ def test_ilqg_quadruped_iteration_improves(ctx):
     """BASELINE config 4 (Quadruped, iLQG, H=64, MakeDifferentiable on): the planner must actually descend.  With the
     engine's FD settings (centred, 3e-4; csrc/host/ilqg_planner.h) eight iterations from the home keyframe take the
     return from 0.324 to 0.124 on the device; the fp64 oracle with the reference's own settings (1e-6, one-sided) reaches
-    0.115 (profiles/r02_fd_gradient.txt).  One-sided 1e-3 - the round-1 setting - does not improve it at all: the
+    0.115.  One-sided 1e-3 - the round-1 setting - does not improve it at all: the
     perturbation crosses contact kinks and the gradient is noise (profiles/fd_gradient_check.py)."""
     from mujoco_mpc_b200.ilqg import ILQGPlanner
     m, e, _ = ctx["quadruped"]
