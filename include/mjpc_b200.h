@@ -255,6 +255,28 @@ void mjpc_b200_ce_planner_action_from_policy(void* planner, double* action, doub
 int mjpc_b200_ce_planner_get_result(void* planner, double* improvement, float* returns, int* order, double* knots,
                                     double* knot_times, double* variance);
 
+/* ---- Sample Gradient planner (csrc/host/sample_gradient_planner.{h,cc}; mjpc/planners/sample_gradient/planner.cc).
+ * One rollout launch covers candidate 0 (the resampled nominal), the noisy samples 1 .. N-G-1 (knot += exploration * z,
+ * not scaled by the control range) and the G gradient candidates N-G .. N-1 computed by the previous iteration; the
+ * fitness-shaped gradient estimate and the log-spaced steps (1e-3 .. 2) along it are host arithmetic in double.
+ * num_gradient is clamped to N - 1 on every optimize_policy.  Requires num_trajectory >= 1, num_spline_points >= 2. */
+int mjpc_b200_sg_planner_create(const mjpc_model_blob* model, int num_trajectory, int num_gradient, int num_spline_points,
+                                int interpolation, double exploration, double gradient_filter, double timestep,
+                                const double* ctrlrange, uint32_t seed, int max_horizon, int device, void** out);
+void mjpc_b200_sg_planner_destroy(void* planner);
+void mjpc_b200_sg_planner_reset(void* planner, int horizon, const double* initial_repeated_action);
+void mjpc_b200_sg_planner_set_state(void* planner, const double* state, double time, const double* mocap);
+int mjpc_b200_sg_planner_optimize_policy(void* planner, int horizon);       /* SampleGradientPlanner::OptimizePolicy */
+int mjpc_b200_sg_planner_nominal_trajectory(void* planner, int horizon);    /* rolls out the resampled nominal alone */
+void mjpc_b200_sg_planner_action_from_policy(void* planner, double* action, double time, int use_previous);
+/* winner, winner_type (0 nominal, 1 noisy, 2 gradient), improvement, returns [N], order [N] (as trajectory_order holds
+ * it: the ranking of all N, or of the N-G noisy samples in its first N-G entries on the call that computed the
+ * fitness weights), installed knots [P][nu] / times [P], gradient candidates' knots [G][P][nu] as the next iteration
+ * resamples and rolls them out, gradient [P][nu].  Any pointer may be NULL; returns the number of installed knots. */
+int mjpc_b200_sg_planner_get_result(void* planner, int* winner, int* winner_type, double* improvement, float* returns,
+                                    int* order, double* knots, double* knot_times, double* gradient_knots,
+                                    double* gradient);
+
 /* ---- Robust planner (csrc/host/robust_planner.{h,cc}; mjpc/planners/robust/robust_planner.cc:40-160) over the
  * sampling planner: the best `ncandidates` of the clean launch are re-rolled `nrepetitions` times each with
  * NoisyRollout force perturbations (one launch on a second handle) and the best mean score is installed.
@@ -367,6 +389,9 @@ int mjpc_b200_ilqs_planner_get_result(void* planner, double* scalars);
  * settings[20] = {planner, horizon, timestep, integrator, differentiable (-1 = the reference default), num_trajectory,
  *   num_spline_points, representation, exploration, ilqg_num_rollouts, ilqg_representation, fd_tolerance, n_elite, std_min,
  *   explore_fraction, robust_candidates, robust_repetitions, robust_xfrc, robust_xfrc_rate, seed} */
+/* agent_planner 6 is the Sample Gradient planner (above).  It takes settings[22]: the twenty entries above, then
+ * settings[20] = sample_gradient_trajectories and settings[21] = sample_gradient_filter.  Those two are read only when
+ * settings[0] == 6, so a caller of planners 0-5 may keep passing 20 values. */
 int mjpc_b200_agent_steps(double horizon, double timestep);
 int mjpc_b200_agent_create(const mjpc_model_blob* model, const double* settings, const double* ctrlrange, int device, void** out);
 void mjpc_b200_agent_destroy(void* agent);

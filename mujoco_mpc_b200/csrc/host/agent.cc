@@ -60,8 +60,13 @@ int Agent::Initialize(const mjpc_model_blob* model, const AgentSettings& s, cons
                            s.num_spline_points, s.representation, s.exploration, s.std_min, s.explore_fraction, s.timestep,
                            ctrlrange, s.seed, Hmax, device);
       break;
+    case kSampleGradientPlanner:   // not gradient-based for MakeDifferentiable (agent.cc:155-163)
+      sg_.reset(new SampleGradientPlanner);
+      rc = sg_->Initialize(model, s.num_trajectory, s.num_gradient, s.num_spline_points, s.representation, s.exploration,
+                           s.gradient_filter, s.timestep, ctrlrange, s.seed, Hmax, device);
+      break;
     default:
-      return MJPC_B200_ERR_UNSUPPORTED;   // SampleGradient: not built
+      return MJPC_B200_ERR_UNSUPPORTED;
   }
   if (rc) return rc;
   std::vector<mjpc_b200_t*> hs = Handles();
@@ -82,6 +87,7 @@ std::vector<mjpc_b200_t*> Agent::Handles() {
   if (ilqs_) { hs.push_back(ilqs_->sampling.gpu()); hs.push_back(ilqs_->ilqg.gpu()); }
   if (robust_) { hs.push_back(robust_->delegate()->gpu()); hs.push_back(robust_->noisy()); }
   if (ce_) hs.push_back(ce_->gpu());
+  if (sg_) hs.push_back(sg_->gpu());
   return hs;
 }
 
@@ -92,6 +98,7 @@ void Agent::Reset(const double* a) {
   if (ilqs_) ilqs_->Reset(steps_, a);
   if (robust_) robust_->Reset(steps_, a);
   if (ce_) ce_->Reset(steps_, a);
+  if (sg_) sg_->Reset(steps_, a);
 }
 
 void Agent::SetState(const double* state, double time, const double* mocap) {
@@ -123,6 +130,7 @@ int Agent::PlanIteration() {
   if (ilqs_) ilqs_->SetState(state_.data(), time_, mc);
   if (robust_) robust_->SetState(state_.data(), time_, mc);
   if (ce_) ce_->SetState(state_.data(), time_, mc);
+  if (sg_) sg_->SetState(state_.data(), time_, mc);
   if (have_task_) {   // residual_fn_ = ActiveTask()->Residual(): the snapshot stays constant during planning (agent.cc:316-319)
     mjpc_task_desc td{weight_.empty() ? nullptr : weight_.data(), parameters_.empty() ? nullptr : parameters_.data(),
                       task_state_.empty() ? nullptr : task_state_.data(), risk_};
@@ -137,9 +145,11 @@ int Agent::PlanIteration() {
     if (ilqs_) rc = ilqs_->OptimizePolicy(steps_);
     if (robust_) rc = robust_->OptimizePolicy(steps_);
     if (ce_) rc = ce_->OptimizePolicy(steps_);
+    if (sg_) rc = sg_->OptimizePolicy(steps_);
   } else {
     if (ilqg_) rc = ilqg_->NominalTrajectory(steps_);
     if (ilqs_) rc = ilqs_->NominalTrajectory(steps_);
+    if (sg_) rc = sg_->NominalTrajectory(steps_);
     if (sampling_) { sampling_->UpdateNominalPolicy(steps_); rc = sampling_->Rollouts(1, steps_); }
   }
   for (mjpc_b200_t* h : hs) mjpc_b200_set_differentiable(h, 0);            // restore solimp defaults (agent.cc:346-356)
@@ -153,6 +163,7 @@ void Agent::ActionFromPolicy(double* action, const double* state, double time, b
   if (ilqs_) ilqs_->ActionFromPolicy(action, state, time, use_previous);
   if (robust_) robust_->ActionFromPolicy(action, time, use_previous);
   if (ce_) ce_->ActionFromPolicy(action, time, use_previous);
+  if (sg_) sg_->ActionFromPolicy(action, time, use_previous);
 }
 
 }  // namespace mjpc_b200_host
@@ -168,6 +179,8 @@ int mjpc_b200_agent_steps(double horizon, double timestep) { return Agent::Steps
 // settings[20] = {planner, horizon, timestep, integrator, differentiable (-1 default), num_trajectory, num_spline_points,
 //                 representation, exploration, ilqg_num_rollouts, ilqg_representation, fd_tolerance, n_elite, std_min,
 //                 explore_fraction, robust_candidates, robust_repetitions, robust_xfrc, robust_xfrc_rate, seed}
+// settings[22] for the Sample Gradient planner (planner 6): settings[20] = sample_gradient_trajectories,
+//                 settings[21] = sample_gradient_filter; read only for planner 6, so the other planners may pass 20
 int mjpc_b200_agent_create(const mjpc_model_blob* model, const double* settings, const double* ctrlrange, int device, void** out) {
   if (!model || !settings || !ctrlrange || !out) return MJPC_B200_ERR_BAD_ARGUMENT;
   AgentSettings s;
@@ -178,6 +191,7 @@ int mjpc_b200_agent_create(const mjpc_model_blob* model, const double* settings,
   s.std_min = settings[13]; s.explore_fraction = settings[14]; s.robust_candidates = (int)settings[15];
   s.robust_repetitions = (int)settings[16]; s.robust_xfrc = settings[17]; s.robust_xfrc_rate = settings[18];
   s.seed = (unsigned)settings[19];
+  if (s.planner == mjpc_b200_host::kSampleGradientPlanner) { s.num_gradient = (int)settings[20]; s.gradient_filter = settings[21]; }
   auto* a = new Agent;
   int rc = a->Initialize(model, s, ctrlrange, device);
   if (rc) { delete a; *out = nullptr; return rc; }

@@ -14,6 +14,7 @@
 #include "gradient_planner.h"
 #include "ilqg_planner.h"
 #include "robust_planner.h"
+#include "sample_gradient_planner.h"
 #include "sampling_planner.h"
 
 namespace mjpc_b200_host {
@@ -37,6 +38,7 @@ struct AgentSettings {              // what the reference reads from the task XM
   double fd_tolerance = 3.0e-4;     // with centred differences (ilqg_planner.h)
   int n_elite = 0; double std_min = 0.01, explore_fraction = 0.0;
   int robust_candidates = -1, robust_repetitions = 5; double robust_xfrc = 0.1, robust_xfrc_rate = 0.1;
+  int num_gradient = 0; double gradient_filter = 1.0;   // sample_gradient_trajectories / sample_gradient_filter
   unsigned seed = 0x5EED;
 };
 
@@ -62,6 +64,7 @@ class Agent {
   std::unique_ptr<iLQSPlanner> ilqs_;
   std::unique_ptr<RobustPlanner> robust_;
   std::unique_ptr<CrossEntropyPlanner> ce_;
+  std::unique_ptr<SampleGradientPlanner> sg_;
   std::vector<double> state_, mocap_, weight_, parameters_, task_state_;
   double time_ = 0, risk_ = 0;
   bool have_task_ = false;

@@ -25,11 +25,7 @@ struct DifferentiableScope {          // MakeDifferentiable while planning (agen
 std::vector<double> LogScaleSteps(int K, double min_step) {   // LogScale (utilities.cc:819-825) + trailing 0
   std::vector<double> s(K, 0.0);
   const int steps = K - 1;
-  if (steps > 0) {
-    const double lo = std::log(min_step), hi = std::log(1.0);
-    const double step = (hi - lo) / std::max(steps - 1, 1);
-    for (int i = 0; i < steps; i++) s[i] = std::exp(lo + i * step);
-  }
+  if (steps > 0) LogScale(s.data(), 1.0, min_step, steps);
   s[K - 1] = 0.0;
   return s;
 }

@@ -159,9 +159,9 @@ std::vector<float> iLQGPlanner::StepSizes() const {
   std::vector<float> s(K_, 0.f);
   const int steps = K_ - 1;
   if (steps > 0) {
-    const double lo = std::log(settings.min_linesearch_step), hi = std::log(1.0);
-    const double step = (hi - lo) / std::max(steps - 1, 1);
-    for (int i = 0; i < steps; i++) s[i] = (float)std::exp(lo + i * step);
+    std::vector<double> d(steps);
+    LogScale(d.data(), 1.0, settings.min_linesearch_step, steps);
+    for (int i = 0; i < steps; i++) s[i] = (float)d[i];
   }
   s[K_ - 1] = 0.f;
   return s;

@@ -74,6 +74,11 @@ double PhiloxNormal(uint32_t seed, uint32_t iteration, uint32_t candidate, uint3
   return std::sqrt(-2.0 * std::log(u1)) * std::cos(2.0 * M_PI * u2);
 }
 
+void LogScale(double* values, double max_value, double min_value, int steps) {
+  const double step = (std::log(max_value) - std::log(min_value)) / std::max(steps - 1, 1);
+  for (int i = 0; i < steps; i++) values[i] = std::exp(std::log(min_value) + i * step);
+}
+
 // ------------------------------------------------------------------------------------------ SamplingPlanner
 SamplingPlanner::~SamplingPlanner() {
   if (gpu_) mjpc_b200_destroy(gpu_);

@@ -48,6 +48,9 @@ struct SamplingPolicy {
 void Philox4x32(const uint32_t ctr[4], const uint32_t key[2], uint32_t out[4]);
 double PhiloxNormal(uint32_t seed, uint32_t iteration, uint32_t candidate, uint32_t knot, uint32_t dof);
 
+// LogScale (utilities.cc:819-825): `steps` values ascending from min_value to max_value, evenly spaced in log
+void LogScale(double* values, double max_value, double min_value, int steps);
+
 struct Trajectory {                                   // mjpc/trajectory.h:74-86 (device arithmetic: float)
   int horizon = 0, dim_state = 0, dim_action = 0, dim_residual = 0, dim_trace = 0;
   std::vector<float> states, actions, residual, costs, trace;

@@ -33,6 +33,10 @@ EXPORTS = ["mjpc_b200_version", "mjpc_b200_last_error", "mjpc_b200_create", "mjp
            "mjpc_b200_ce_planner_create", "mjpc_b200_ce_planner_destroy", "mjpc_b200_ce_planner_reset",
            "mjpc_b200_ce_planner_set_state", "mjpc_b200_ce_planner_optimize_policy",
            "mjpc_b200_ce_planner_action_from_policy", "mjpc_b200_ce_planner_get_result",
+           "mjpc_b200_sg_planner_create", "mjpc_b200_sg_planner_destroy", "mjpc_b200_sg_planner_reset",
+           "mjpc_b200_sg_planner_set_state", "mjpc_b200_sg_planner_optimize_policy",
+           "mjpc_b200_sg_planner_nominal_trajectory", "mjpc_b200_sg_planner_action_from_policy",
+           "mjpc_b200_sg_planner_get_result",
            "mjpc_b200_ilqg_planner_create", "mjpc_b200_ilqg_planner_destroy", "mjpc_b200_ilqg_planner_set_fd",
            "mjpc_b200_gradient_planner_set_fd", "mjpc_b200_ilqs_planner_set_fd", "mjpc_b200_ilqg_planner_reset",
            "mjpc_b200_ilqg_planner_set_state", "mjpc_b200_ilqg_planner_nominal_trajectory",
@@ -90,6 +94,7 @@ def load_library():
         lib.mjpc_b200_planner_destroy.argtypes = [C.c_void_p]
         lib.mjpc_b200_planner_set_exploration.argtypes = [C.c_void_p, C.c_double, C.c_double]
         lib.mjpc_b200_ce_planner_destroy.argtypes = [C.c_void_p]
+        lib.mjpc_b200_sg_planner_destroy.argtypes = [C.c_void_p]
         lib.mjpc_b200_ilqg_planner_destroy.argtypes = [C.c_void_p]
         for n in ("mjpc_b200_ilqg_planner_set_fd", "mjpc_b200_gradient_planner_set_fd", "mjpc_b200_ilqs_planner_set_fd"):
             getattr(lib, n).argtypes = [C.c_void_p, C.c_double, C.c_int, C.c_int]
@@ -516,6 +521,74 @@ class CppCrossEntropyPlanner:
         return a
 
 
+class CppSampleGradientPlanner:
+    """The C++ Sample Gradient planner (csrc/host/sample_gradient_planner.cc) through its C wrappers."""
+
+    def __init__(self, model, num_trajectory, horizon, num_gradient=None, gradient_filter=None, seed=0x5EED, device=0):
+        self.lib = load_library()
+        m = self.m = model
+        self._blob = to_blob(model)
+        self._buf = C.create_string_buffer(self._blob, len(self._blob))
+        mb = ModelBlob(C.cast(self._buf, C.c_void_p), len(self._blob))
+        num = m.numeric
+        self.P = int(num.get("sampling_spline_points", [3])[0])
+        self.horizon, self.N, self.nu = int(horizon), int(num_trajectory), m.nu
+        G = int(num_gradient if num_gradient is not None else num.get("sample_gradient_trajectories", [0])[0])
+        self.G = max(min(G, self.N - 1), 0)                  # the clamp OptimizePolicy applies
+        f = float(gradient_filter if gradient_filter is not None else num.get("sample_gradient_filter", [1.0])[0])
+        cr = _d(np.asarray(m.actuator_ctrlrange, float).reshape(-1))
+        h = C.c_void_p()
+        rc = self.lib.mjpc_b200_sg_planner_create(
+            C.byref(mb), self.N, G, self.P, int(num.get("sampling_representation", [2])[0]),
+            C.c_double(float(num.get("sampling_exploration", [0.1])[0])), C.c_double(f), C.c_double(float(m.opt_timestep)),
+            _pd(cr), C.c_uint32(seed), self.horizon, int(device), C.byref(h))
+        if rc != 0:
+            raise EngineError(f"mjpc_b200_sg_planner_create failed ({rc}): {self.lib.mjpc_b200_last_error().decode()}")
+        self.h = h
+
+    def close(self):
+        if getattr(self, "h", None):
+            self.lib.mjpc_b200_sg_planner_destroy(self.h)
+            self.h = None
+
+    __del__ = close
+
+    def reset(self, initial_repeated_action=None):
+        a = _d(initial_repeated_action)
+        self.lib.mjpc_b200_sg_planner_reset(self.h, self.horizon, _pd(a))
+
+    def set_state(self, state, time, mocap):
+        s, mc = _d(state), _d(mocap)
+        self.lib.mjpc_b200_sg_planner_set_state(self.h, _pd(s), C.c_double(time), _pd(mc))
+
+    def optimize_policy(self):
+        rc = self.lib.mjpc_b200_sg_planner_optimize_policy(self.h, self.horizon)
+        if rc != 0:
+            raise EngineError(f"sg_planner_optimize_policy failed: {self.lib.mjpc_b200_last_error().decode()}")
+        return self.result()
+
+    def nominal_trajectory(self):
+        rc = self.lib.mjpc_b200_sg_planner_nominal_trajectory(self.h, self.horizon)
+        if rc != 0:
+            raise EngineError(f"sg_planner_nominal_trajectory failed: {self.lib.mjpc_b200_last_error().decode()}")
+
+    def result(self):
+        winner, wtype, imp = C.c_int(), C.c_int(), C.c_double()
+        ret = np.zeros(self.N, np.float32); order = np.zeros(self.N, np.int32)
+        knots = np.zeros((self.P, self.nu)); kt = np.zeros(self.P)
+        gk = np.zeros((self.G, self.P, self.nu)); grad = np.zeros((self.P, self.nu))
+        n = self.lib.mjpc_b200_sg_planner_get_result(self.h, C.byref(winner), C.byref(wtype), C.byref(imp), _pf(ret),
+                                                     order.ctypes.data_as(_ip), _pd(knots), _pd(kt),
+                                                     _pd(gk) if self.G else None, _pd(grad))
+        return dict(winner=winner.value, winner_type=wtype.value, improvement=imp.value, returns=ret, order=order,
+                    knots=knots[:n], knot_times=kt[:n], gradient_knots=gk, gradient=grad)
+
+    def action_from_policy(self, time, use_previous=False):
+        a = np.zeros(self.nu)
+        self.lib.mjpc_b200_sg_planner_action_from_policy(self.h, _pd(a), C.c_double(time), int(use_previous))
+        return a
+
+
 class CppILQGPlanner:
     """The C++ iLQG planner (csrc/host/ilqg_planner.cc) through its C wrappers."""
 
@@ -754,11 +827,11 @@ class CppILQSPlanner:
 
 class CppAgent:
     """Agent::PlanIteration glue (csrc/host/agent.cc) through its C wrappers; settings mirror the task XML numerics."""
-    PLANNERS = {"sampling": 0, "gradient": 1, "ilqg": 2, "ilqs": 3, "robust": 4, "cross_entropy": 5}
+    PLANNERS = {"sampling": 0, "gradient": 1, "ilqg": 2, "ilqs": 3, "robust": 4, "cross_entropy": 5, "sample_gradient": 6}
 
     def __init__(self, model, planner="sampling", horizon=None, timestep=None, integrator=0, differentiable=-1, num_trajectory=None,
                  num_spline_points=None, representation=None, exploration=None, ilqg_num_rollouts=10, ilqg_representation=1,
-                 fd_tolerance=3e-4, seed=0x5EED, device=0):
+                 fd_tolerance=3e-4, seed=0x5EED, device=0, num_gradient=None, gradient_filter=None):
         self.lib = load_library()
         m = self.m = model
         num = m.numeric
@@ -775,7 +848,9 @@ class CppAgent:
                        g("sampling_exploration", 0.1) if exploration is None else exploration,
                        ilqg_num_rollouts, ilqg_representation, fd_tolerance, 0, g("std_min", 0.01), g("explore_fraction", 0.0),
                        g("robust_candidates", -1), g("robust_repetitions", 5), g("robust_xfrc", 0.1), g("robust_xfrc_rate", 0.1),
-                       seed], float)
+                       seed,
+                       g("sample_gradient_trajectories", 0) if num_gradient is None else num_gradient,
+                       g("sample_gradient_filter", 1.0) if gradient_filter is None else gradient_filter], float)
         cr = _d(np.asarray(m.actuator_ctrlrange, float).reshape(-1))
         h = C.c_void_p()
         rc = self.lib.mjpc_b200_agent_create(C.byref(mb), _pd(st), _pd(cr), int(device), C.byref(h))

@@ -6,10 +6,13 @@ Mirrors mjpc/planners/sampling/planner.cc:
     seed 0x5EED, counter = (iteration, candidate, knot, dof): the reference's absl::BitGen is unseedable,
     SURVEY.md section 0 finding 4)
   * OptimizePolicy / CopyCandidateToPolicy      :197-212, 534-543 -> SamplingPlanner.optimize_policy
+and, on the same rollout backend, the Cross-Entropy, Sample Gradient and Robust planners.
 The spline itself (mjpc/spline/spline.cc:103-156, 250-287) is restated in sample_spline for the host-side
 resampling; the device evaluates the same formula per step.
 """
 from __future__ import annotations
+
+import math
 
 import numpy as np
 
@@ -228,6 +231,143 @@ class CrossEntropyPlanner:
         self.order = order
         self.returns = ret
         self.iteration += 1
+        return ret, fail
+
+    def action_from_policy(self, time):
+        return clamp(sample_spline(self.times, self.values, self.interp, time), self.ctrlrange)
+
+
+def log_scale(max_value, min_value, steps):
+    """LogScale (utilities.cc:819-825): `steps` values ascending from min_value to max_value, evenly spaced in log."""
+    step = (math.log(max_value) - math.log(min_value)) / max(steps - 1, 1)
+    return np.array([math.exp(math.log(min_value) + i * step) for i in range(steps)])
+
+
+class SampleGradientPlanner:
+    """Sample Gradient planner (mjpc/planners/sample_gradient/planner.cc) on the same rollout backend.
+
+    One launch of N candidates per OptimizePolicy (:169-273): 0 = the resampled nominal, 1 .. N-G-1 = noisy samples
+    clamp(nominal + sigma * z) (not scaled by the control range; z from the injected Philox stream), N-G .. N-1 = the
+    gradient candidates of the previous iteration resampled onto this iteration's knot times (an empty plan after
+    Reset is the clamped zero plan).  The winner is the best candidate if it beats the nominal strictly.
+    GradientCandidates (:401-493) then forms a fitness-shaped gradient estimate from the noise and puts candidate j at
+    clamp(nominal - (s_j / sigma) (f * gradient + (1 - f) * gradient_previous)), s = LogScale(2, 1e-3, G).  The
+    reference's quirks are kept (DESIGN.md section 8): the weights are cached by size and, on the call that computes
+    them, indexed by candidate index rather than rank; later calls pair them with the ranking of all N candidates.
+    """
+    GRADIENT_MAX_STEP_SIZE, GRADIENT_MIN_STEP_SIZE = 2.0, 1.0e-3
+
+    def __init__(self, model, backend, num_trajectory=None, horizon=None, num_gradient=None, gradient_filter=None,
+                 seed=0x5EED):
+        m = self.model = model
+        self.backend = backend
+        num = m.numeric
+        self.num_trajectory = int(num_trajectory or num.get("sampling_trajectories", [10])[0])
+        self.num_gradient = int(num_gradient if num_gradient is not None else num.get("sample_gradient_trajectories", [0])[0])
+        self.gradient_filter = float(gradient_filter if gradient_filter is not None else
+                                     num.get("sample_gradient_filter", [1.0])[0])
+        self.P = int(num.get("sampling_spline_points", [3])[0])
+        self.sigma = float(num.get("sampling_exploration", [0.1])[0])
+        self.interp = int(num.get("sampling_representation", [2])[0])
+        self.timestep = float(m.opt_timestep)
+        self.horizon = int(horizon or max(min(num.get("agent_horizon", [0.5])[0] / self.timestep + 1, 512), 1))
+        self.ctrlrange = np.asarray(m.actuator_ctrlrange, float).reshape(-1, 2)
+        self.seed = seed
+        self.return_weight = None                 # cached by size; Reset keeps them (planner.cc:419, 462)
+        self.step_size = None
+        self.order = np.arange(self.num_trajectory)
+        self.reset()
+
+    def reset(self, initial_repeated_action=None):
+        nu = self.model.nu
+        self.times = np.zeros(1)
+        self.values = np.zeros((1, nu)) if initial_repeated_action is None else \
+            np.asarray(initial_repeated_action, float)[None]
+        self.resampled = (self.times, self.values)
+        # gradient candidates' plans: empty after Reset
+        self.candidates = [(np.zeros(0), np.zeros((0, nu))) for _ in range(self.num_trajectory)]
+        self.noise = np.zeros((self.num_trajectory, self.P, nu))
+        self.gradient = np.zeros((self.P, nu))
+        self.gradient_previous = np.zeros((self.P, nu))
+        self.winner, self.winner_type, self.improvement, self.iteration = 0, 0, 0.0, 0
+
+    def set_state(self, state, time, mocap):
+        self.state, self.time, self.mocap = np.asarray(state, float), float(time), np.asarray(mocap, float)
+
+    def resample(self, times, values):
+        """ResamplePolicy (:302-326): P knots at time + k (H-1) dt / (P-1), for every interpolation."""
+        shift = max((self.horizon - 1) * self.timestep / (self.P - 1), 1e-5)
+        new_t = self.time + shift * np.arange(self.P)
+        new_v = np.stack([clamp(sample_spline(times, values, self.interp, tt), self.ctrlrange) for tt in new_t])
+        return new_t, new_v
+
+    def optimize_policy(self):
+        N = self.num_trajectory
+        G = self.num_gradient = min(self.num_gradient, N - 1)
+        n = N - G
+        times, nominal = self.resample(self.times, self.values)
+        self.resampled = (times, nominal)
+        knots = np.empty((N, self.P, self.model.nu))
+        knots[0] = nominal
+        z = philox_normal(self.iteration, N, self.P, self.model.nu, self.seed)
+        self.noise[1:n] = z[1:n]
+        knots[1:n] = np.clip(nominal[None] + z[1:n] * self.sigma, self.ctrlrange[:, 0], self.ctrlrange[:, 1])
+        for i in range(n, N):
+            knots[i] = self.resample(*self.candidates[i])[1]
+        ret, fail, order = self.backend.rollout_spline(self.state, self.time, self.mocap, knots, times, self.interp,
+                                                       self.horizon)
+        ret = np.asarray(ret)
+        self.order = np.array(order if order is not None else np.argsort(ret, kind="stable"))
+        self.winner = int(self.order[0]) if ret[self.order[0]] < ret[0] else 0
+        self.winner_type = 0 if self.winner == 0 else (1 if self.winner < n else 2)
+        self.times, self.values = times, knots[self.winner].copy()
+        self.improvement = max(float(ret[0]) - float(ret[self.winner]), 0.0)
+        self.knots, self.returns = knots, ret
+        self.gradient_candidates(ret, times, nominal)
+        self.iteration += 1
+        return ret, fail
+
+    def gradient_candidates(self, ret, times, nominal):
+        N, G = self.num_trajectory, self.num_gradient
+        n = N - G
+        if G < 1:
+            return
+        self.gradient_previous = self.gradient.copy()
+        if self.return_weight is None or len(self.return_weight) != n:
+            self.order[:n] = np.argsort(ret[:n], kind="stable")
+            f0 = math.log(0.5 * n + 1.0)
+            shaped = [max(0.0, f0 - math.log(int(self.order[i]) + 1)) for i in range(n)]
+            den = 0.0
+            for s in shaped:
+                den += s
+            self.return_weight = np.array([s / den - 1.0 / n for s in shaped])
+        g = np.zeros_like(self.gradient)
+        for i in range(n):
+            g += self.noise[self.order[i]] * (self.return_weight[i] / n)
+        self.gradient = g
+        if self.step_size is None or len(self.step_size) != G:
+            self.step_size = log_scale(self.GRADIENT_MAX_STEP_SIZE, self.GRADIENT_MIN_STEP_SIZE, G)
+        f = self.gradient_filter
+        for j in range(G):
+            scaling = self.step_size[j] / self.sigma
+            v = nominal + self.gradient * (-scaling * f)
+            v = v + self.gradient_previous * (-scaling * (1.0 - f))
+            self.candidates[n + j] = (times, np.clip(v, self.ctrlrange[:, 0], self.ctrlrange[:, 1]))
+
+    @property
+    def gradient_knots(self):
+        """The gradient candidates' knots [G][P][nu] as the next iteration resamples and rolls them out."""
+        n = self.num_trajectory - self.num_gradient
+        return np.stack([self.candidates[i][1] for i in range(n, self.num_trajectory)]) if self.num_gradient else \
+            np.zeros((0, self.P, self.model.nu))
+
+    def nominal_trajectory(self):
+        """NominalTrajectory (:276-287): the resampled nominal as one candidate (an empty plan = the clamped zero)."""
+        times, values = self.resampled
+        if len(times) == 0:
+            times, values = np.array([self.time]), clamp(np.zeros(self.model.nu), self.ctrlrange)[None]
+        ret, fail, _ = self.backend.rollout_spline(self.state, self.time, self.mocap, values[None], times, self.interp,
+                                                   self.horizon)
         return ret, fail
 
     def action_from_policy(self, time):

@@ -14,7 +14,7 @@ from conftest import OracleBackend, get_model, mocap_of
 def main(argv=None):
     ap = argparse.ArgumentParser()
     ap.add_argument("--task", default="quadruped", choices=["quadruped", "humanoid", "humanoid_track", "cartpole", "particle"])
-    ap.add_argument("--planner", default="sampling", choices=["sampling", "cross_entropy", "robust"])
+    ap.add_argument("--planner", default="sampling", choices=["sampling", "cross_entropy", "robust", "sample_gradient"])
     ap.add_argument("--backend", default="b200", choices=["b200", "oracle"])
     ap.add_argument("--steps", type=int, default=100)
     ap.add_argument("--candidates", type=int, default=0)
@@ -34,7 +34,8 @@ def main(argv=None):
         backend = Engine(m, N + extra, H)
     else:
         backend = OracleBackend(m, threads=a.threads)
-    cls = {"sampling": P.SamplingPlanner, "cross_entropy": P.CrossEntropyPlanner, "robust": P.RobustPlanner}[a.planner]
+    cls = {"sampling": P.SamplingPlanner, "cross_entropy": P.CrossEntropyPlanner, "robust": P.RobustPlanner,
+           "sample_gradient": P.SampleGradientPlanner}[a.planner]
     pl = cls(m, backend, num_trajectory=N, horizon=H)
     pl.reset(np.zeros(m.nu)) if a.planner != "cross_entropy" else pl.reset()
     transition = None
