@@ -105,6 +105,25 @@ int mjpc_b200_rollout_spline(mjpc_b200_t* h, const float* state, double time, co
                              const float* userdata, const float* knots, const double* knot_times, int interp,
                              int P, int N, int H, float* returns, uint8_t* failure, int* order);
 
+/* B independent planning problems of N candidates each in ONE rollout launch (mjpc_b200_rollout_spline is the case
+ * B = 1).  Every problem has its own start state, absolute start time, mocap, task snapshot and knots; N, P, interp and
+ * H are common.  Candidate i of problem b has the flat index b*N + i.
+ *   states [B][dim_state], times [B] (absolute), mocaps [B][7 nmocap], knots [B][N][P][nu], knot_times [B][P] (absolute)
+ *   weights [B][num_term], parameters [B][num_parameters], task_states [B][task_state_size]: each may be NULL, which
+ *     stands for the handle's set_task value in every problem; the time-like task-state entries are rebased by times[b].
+ *     Risk is the handle's (Task::risk).
+ *   returns [B][N], failure [B][N]; order [B][N] (may be NULL): order[b] ranks problem b's candidates by return with
+ *     indices local to the problem (0..N-1, ties: lower index first).
+ * B*N must not exceed max_candidates (MJPC_B200_ERR_CAPACITY); B, N, H >= 1, H <= max_horizon and P <= 64, otherwise an
+ * error is returned and the handle stays usable.  With MJPC_B200_WARPS_PER_CTA > 1 and B > 1, N must be a multiple of it
+ * (MJPC_B200_ERR_UNSUPPORTED).  After a batched launch, fetch_trajectory, fetch_all and fetch_stats take the flat index,
+ * last_kernel_ms / last_kernel_static describe the one launch, and NoisyRollout force noise (set_xfrc_noise) draws
+ * with the flat index as its candidate counter. */
+int mjpc_b200_rollout_spline_batched(mjpc_b200_t* h, int B, const float* states, const double* times, const float* mocaps,
+                                     const double* weights, const double* parameters, const double* task_states,
+                                     const float* knots, const double* knot_times, int interp, int P, int N, int H,
+                                     float* returns, uint8_t* failure, int* order);
+
 /* NoisyRollout (mjpc/trajectory.cc:100-210, used by the Robust planner): the following rollouts of this handle add
  * Ornstein-Uhlenbeck noise to xfrc_applied of every body (stationary std xfrc_std, correlation time xfrc_rate
  * seconds), drawn from Philox4x32-10 with key (seed, 1) and counter (step, candidate, element, 'XFRC') - the
@@ -236,6 +255,26 @@ int mjpc_b200_planner_optimize_policy(void* planner, int horizon);          /* S
 void mjpc_b200_planner_action_from_policy(void* planner, double* action, double time, int use_previous);
 int mjpc_b200_planner_get_result(void* planner, int* winner, double* improvement, float* returns, double* knots,
                                  double* knot_times);
+
+/* ---- Batched Predictive Sampling (csrc/host/batch_sampling_planner.{h,cc}): num_problems independent SamplingPlanners
+ * (each with its own seed, state, mocap, task snapshot and policy) on ONE engine handle; optimize_policy makes one
+ * mjpc_b200_rollout_spline_batched launch for all of them, and each problem's result equals that of a SamplingPlanner
+ * with the same seed and inputs.  seeds [num_problems].  The task snapshot of every problem starts as the model's
+ * (weight, parameters, task state); set_task replaces its non-NULL members.  Calls that take a problem index return
+ * MJPC_B200_ERR_BAD_ARGUMENT when it is outside [0, num_problems). */
+int mjpc_b200_batch_planner_create(const mjpc_model_blob* model, int num_problems, int num_trajectory, int num_spline_points,
+                                   int interpolation, double exploration, double timestep, const double* ctrlrange,
+                                   const uint32_t* seeds, int max_horizon, int device, void** out);
+void mjpc_b200_batch_planner_destroy(void* planner);
+int mjpc_b200_batch_planner_reset(void* planner, int problem, int horizon, const double* initial_repeated_action);
+int mjpc_b200_batch_planner_set_state(void* planner, int problem, const double* state, double time, const double* mocap);
+int mjpc_b200_batch_planner_set_task(void* planner, int problem, const double* weight, const double* parameters,
+                                     const double* task_state);
+int mjpc_b200_batch_planner_optimize_policy(void* planner, int horizon);   /* every problem: SamplingPlanner::OptimizePolicy */
+int mjpc_b200_batch_planner_action_from_policy(void* planner, int problem, double* action, double time, int use_previous);
+/* as mjpc_b200_planner_get_result for one problem (returns [num_trajectory]); returns the number of installed knots */
+int mjpc_b200_batch_planner_get_result(void* planner, int problem, int* winner, double* improvement, float* returns,
+                                       double* knots, double* knot_times);
 
 /* ---- Cross-Entropy planner (csrc/host/cross_entropy_planner.{h,cc}; mjpc/planners/cross_entropy/planner.h:35-146).
  * One rollout launch covers the N noisy candidates and the un-noised nominal (candidate N); the elite mean and

@@ -49,8 +49,8 @@ struct mjpc_b200 {
   int num_sms = 132;
   int static_spec = 0;   // 1 / 2: the model equals spec_quadruped.h / spec_humanoid_track.h -> static rollout kernel
   float* d_pack = nullptr;
-  // inputs
-  float *d_state = nullptr, *d_mocap = nullptr, *d_task_state = nullptr, *d_knots = nullptr, *d_knot_times = nullptr;
+  // inputs: d_in holds the per-problem inputs and the knots of the last rollout launch (stage_problems)
+  float *d_in = nullptr, *d_task_state = nullptr;
   float *d_unom = nullptr, *d_xnom = nullptr, *d_tnom = nullptr, *d_gains = nullptr, *d_du = nullptr, *d_steps = nullptr;
   // outputs
   float *d_states = nullptr, *d_actions = nullptr, *d_residual = nullptr, *d_costs = nullptr, *d_trace = nullptr,
@@ -124,23 +124,58 @@ int set_smem(const void* fn, size_t bytes) {
   return 0;
 }
 
-// fill the pinned staging buffer with the per-iteration inputs shared by both rollout flavours
-struct Staged { size_t state, mocap, tstate, end; };
-Staged stage_common(mjpc_b200* h, const float* state, double time, const float* mocap) {
+// floats of the per-problem block of stage_problems for B problems and P knots (knots excluded)
+size_t problem_floats(const DevModel& M, int B, int P) {
+  return (size_t)B * (2 + M.nq + M.nv + 7 * M.nmocap + M.task_state_size + M.num_term + M.num_parameters + P);
+}
+
+// Stage the inputs of a rollout launch of B problems back to back in the pinned buffer and upload them with ONE copy
+// into d_in; point A's per-problem inputs at them.  Layout (floats):
+//   [time0: B doubles][state B x ds][mocap B x 7 nmocap][task_state B x size][weight B x num_term, if given]
+//   [parameters B x num_parameters, if given][knot_times B x P][knots B x N x P x nu]   (knot blocks: spline launches)
+// A NULL task_states / weights / parameters stands for the handle's set_task values; the time-like task-state entries
+// and the knot times are made relative to each problem's own start time.  *end: the first h_in float after the block.
+int stage_problems(mjpc_b200* h, int B, const float* states, const double* times, const float* mocaps,
+                   const double* weights, const double* parameters, const double* task_states, const float* knots,
+                   const double* knot_times, int P, int N, RolloutArgs* A, size_t* end) {
   const DevModel& M = h->pack.M;
-  Staged s;
-  size_t o = 0;
-  s.state = o; std::memcpy(h->h_in + o, state, (M.nq + M.nv) * 4); o += M.nq + M.nv;
-  s.mocap = o; if (M.nmocap) std::memcpy(h->h_in + o, mocap, 7 * M.nmocap * 4); o += 7 * M.nmocap;
-  s.tstate = o;
-  for (int i = 0; i < M.task_state_size; i++) {
-    double v = h->task_state[i];
-    if (std::find(h->time_idx.begin(), h->time_idx.end(), i) != h->time_idx.end()) v -= time;
-    h->h_in[o + i] = (float)v;
+  const size_t ds = M.nq + M.nv, nm = 7 * (size_t)M.nmocap, nts = M.task_state_size, nw = M.num_term,
+               np = M.num_parameters;
+  float* in = h->h_in;
+  std::memcpy(in, times, (size_t)B * sizeof(double));
+  size_t o = 2 * (size_t)B;
+  const size_t o_state = o; std::memcpy(in + o, states, B * ds * 4); o += B * ds;
+  const size_t o_mocap = o; if (nm) std::memcpy(in + o, mocaps, B * nm * 4); o += B * nm;
+  const size_t o_ts = o;
+  for (int b = 0; b < B; b++) {
+    const double* src = task_states ? task_states + b * nts : h->task_state.data();
+    for (size_t i = 0; i < nts; i++) {
+      double v = src[i];
+      if (std::find(h->time_idx.begin(), h->time_idx.end(), (int)i) != h->time_idx.end()) v -= times[b];
+      in[o + i] = (float)v;
+    }
+    o += nts;
   }
-  o += M.task_state_size;
-  s.end = o;
-  return s;
+  const size_t o_w = o;
+  if (weights) for (size_t i = 0; i < B * nw; i++) in[o++] = (float)weights[i];
+  const size_t o_p = o;
+  if (parameters) for (size_t i = 0; i < B * np; i++) in[o++] = (float)parameters[i];
+  const size_t o_kt = o;
+  if (knots) {
+    for (int b = 0; b < B; b++)
+      for (int k = 0; k < P; k++) in[o++] = (float)(knot_times[(size_t)b * P + k] - times[b]);
+  }
+  const size_t o_k = o;
+  if (knots) { std::memcpy(in + o, knots, (size_t)B * N * P * M.nu * 4); o += (size_t)B * N * P * M.nu; }
+  CUDA_TRY(cudaMemcpyAsync(h->d_in, in, o * 4, cudaMemcpyHostToDevice, h->stream));
+  float* d = h->d_in;
+  A->nprob = B; A->nper = N;
+  A->time0 = reinterpret_cast<const double*>(d);
+  A->state = d + o_state; A->mocap = d + o_mocap; A->task_state = d + o_ts;
+  A->weight = weights ? d + o_w : nullptr; A->parameters = parameters ? d + o_p : nullptr;
+  A->knot_times = knots ? d + o_kt : nullptr; A->knots = knots ? d + o_k : nullptr;
+  *end = o;
+  return 0;
 }
 
 int launch_rollout(mjpc_b200* h, const RolloutArgs& A_in) {
@@ -174,7 +209,7 @@ int launch_rollout(mjpc_b200* h, const RolloutArgs& A_in) {
     rollout_kernel<<<grid, 32 * wpc, smem, h->stream>>>(A);
   }
   h->last_static = use_static ? (plain ? 2 : 1) : 0;
-  rank_kernel<<<(A.N + 255) / 256, 256, 0, h->stream>>>(A.returns, A.N, h->d_order);
+  rank_kernel<<<(A.N + 255) / 256, 256, 0, h->stream>>>(A.returns, A.nper, A.nprob, h->d_order);
   CUDA_TRY(cudaEventRecord(h->ev1, h->stream));
   CUDA_TRY(cudaGetLastError());
   h->launches += 2;
@@ -182,13 +217,12 @@ int launch_rollout(mjpc_b200* h, const RolloutArgs& A_in) {
   return 0;
 }
 
-RolloutArgs base_args(mjpc_b200* h, double time, int N, int H) {
+RolloutArgs base_args(mjpc_b200* h, int N, int H) {
   RolloutArgs A;
   std::memset(&A, 0, sizeof(A));
   A.M = h->pack.M;
   A.pack = h->d_pack;
-  A.state = h->d_state; A.mocap = h->d_mocap; A.task_state = h->d_task_state;
-  A.N = N; A.H = H; A.time0 = time;
+  A.N = N; A.H = H;
   A.states = h->d_states; A.actions = h->d_actions; A.times = h->d_times; A.residual = h->d_residual;
   A.costs = h->d_costs; A.trace = h->d_trace; A.returns = h->d_returns; A.failure = h->d_failure;
   A.stats = h->d_stats;
@@ -343,9 +377,10 @@ int mjpc_b200_create(const mjpc_model_blob* model, int max_candidates, int max_h
     CREATE_TRY(cudaMemcpy(h->d_pack, f.data(), f.size() * 4, cudaMemcpyHostToDevice));
   }
   const size_t N = max_candidates, H = max_horizon, ds = M.nq + M.nv, n = 2 * M.nv, nu = M.nu, nr = M.num_residual;
-  CREATE_TRY(dalloc(&h->d_state, ds)); CREATE_TRY(dalloc(&h->d_mocap, 7 * (size_t)M.nmocap));
+  // launch inputs: up to max_candidates problems of one candidate each (stage_problems)
+  const size_t in_floats = problem_floats(M, max_candidates, h->maxP) + N * h->maxP * nu;
+  CREATE_TRY(dalloc(&h->d_in, in_floats));
   CREATE_TRY(dalloc(&h->d_task_state, (size_t)M.task_state_size));
-  CREATE_TRY(dalloc(&h->d_knots, N * h->maxP * nu)); CREATE_TRY(dalloc(&h->d_knot_times, (size_t)h->maxP));
   CREATE_TRY(dalloc(&h->d_unom, H * nu)); CREATE_TRY(dalloc(&h->d_xnom, H * ds)); CREATE_TRY(dalloc(&h->d_tnom, H));
   CREATE_TRY(dalloc(&h->d_gains, H * nu * n)); CREATE_TRY(dalloc(&h->d_du, H * nu)); CREATE_TRY(dalloc(&h->d_steps, N));
   CREATE_TRY(dalloc(&h->d_states, N * H * ds)); CREATE_TRY(dalloc(&h->d_actions, N * H * nu));
@@ -354,7 +389,7 @@ int mjpc_b200_create(const mjpc_model_blob* model, int max_candidates, int max_h
   CREATE_TRY(dalloc(&h->d_returns, N)); CREATE_TRY(dalloc(&h->d_failure, N)); CREATE_TRY(dalloc(&h->d_order, N)); CREATE_TRY(dalloc(&h->d_stats, 12 * N));
   CREATE_TRY(dalloc(&h->d_pair_sync, (size_t)256 * 32));
   CREATE_TRY(dalloc(&h->d_dbg, 4 * ds + 2 * nu + (size_t)M.nv * M.nv + nr + 256 + 64 + 7 * (size_t)M.nmocap));
-  h->h_in_floats = ds + 7 * M.nmocap + M.task_state_size + N * h->maxP * nu + h->maxP + H * (nu + ds + 1 + nu * n + nu) + N + 64;
+  h->h_in_floats = in_floats + H * (nu + ds + 1 + nu * n + nu) + N + 64;
   CREATE_TRY(cudaMallocHost((void**)&h->h_in, h->h_in_floats * 4));
   h->h_out_bytes = N * 16 + 64;
   CREATE_TRY(cudaMallocHost((void**)&h->h_out, h->h_out_bytes));
@@ -384,7 +419,7 @@ void mjpc_b200_destroy(mjpc_b200_t* h) {
   if (h->comm && nccl_api().ok) nccl_api().CommDestroy(h->comm);
   void* mbufs[] = {h->d_slot, h->d_gather, h->d_returns_all, h->d_failure_all, h->d_order_all, h->d_bcast};
   for (void* p : mbufs) if (p) cudaFree(p);
-  void* bufs[] = {h->d_pack, h->d_state, h->d_mocap, h->d_task_state, h->d_knots, h->d_knot_times, h->d_unom, h->d_xnom,
+  void* bufs[] = {h->d_pack, h->d_in, h->d_task_state, h->d_unom, h->d_xnom,
                   h->d_tnom, h->d_gains, h->d_du, h->d_steps, h->d_states, h->d_actions, h->d_times, h->d_residual,
                   h->d_costs, h->d_trace, h->d_returns, h->d_failure, h->d_order, h->d_dbg, h->d_stats, h->d_pair_sync};
   for (void* p : bufs) if (p) cudaFree(p);
@@ -439,35 +474,50 @@ int mjpc_b200_set_differentiable(mjpc_b200_t* h, int on) {
   return 0;
 }
 
+// Validate and upload a spline launch of B problems x N candidates; it becomes the resident launch.  B = 1 is the
+// single-problem call.  Nothing is changed on a refusal, so the handle stays usable.
+static int upload_spline(mjpc_b200_t* h, int B, const float* states, const double* times, const float* mocaps,
+                         const double* weights, const double* parameters, const double* task_states, const float* knots,
+                         const double* knot_times, int interp, int P, int N, int H) {
+  const DevModel& M = h->pack.M;
+  if (M.nmocap && !mocaps) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "rollout_spline: mocap required");
+  if (B < 1 || N < 1 || H < 1 || P < 1 || interp < 0 || interp > 2) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "rollout_spline: bad sizes");
+  if ((int64_t)B * N > h->maxN || H > h->maxH || P > h->maxP) return fail(MJPC_B200_ERR_CAPACITY, "rollout_spline: B*N/H/P above capacity");
+  // several candidates per CTA share its shared-memory copy of the task: a CTA must not hold two problems
+  if (B > 1 && N % h->warps_per_cta != 0)
+    return fail(MJPC_B200_ERR_UNSUPPORTED, "rollout_spline_batched: N must be a multiple of MJPC_B200_WARPS_PER_CTA");
+  CUDA_TRY(cudaSetDevice(h->device));
+  RolloutArgs A = base_args(h, B * N, H);
+  size_t end;
+  if (int rc = stage_problems(h, B, states, times, mocaps, weights, parameters, task_states, knots, knot_times, P, N, &A, &end))
+    return rc;
+  A.L = make_layout(h->pack.M, P);
+  A.P = P; A.interp = interp; A.policy_kind = 0;
+  h->resident = A;
+  h->resident_ok = true;
+  return 0;
+}
+
 int mjpc_b200_upload_spline_inputs(mjpc_b200_t* h, const float* state, double time, const float* mocap,
                                    const float* userdata, const float* knots, const double* knot_times, int interp,
                                    int P, int N, int H) {
   if (!h || !state || !knots || !knot_times) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "rollout_spline: null pointer");
-  const DevModel& M = h->pack.M;
   // mjData::userdata: none of the implemented residuals reads it; a model that declares nuserdata > 0 is rejected at
   // create(), so a non-NULL pointer here can only be a caller error - refuse rather than silently ignore it
   if (userdata && h->nuserdata == 0) return fail(MJPC_B200_ERR_UNSUPPORTED, "rollout_spline: the model has nuserdata = 0, userdata must be NULL");
-  if (M.nmocap && !mocap) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "rollout_spline: mocap required");
-  if (N < 1 || H < 1 || P < 1 || interp < 0 || interp > 2) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "rollout_spline: bad sizes");
-  if (N > h->maxN || H > h->maxH || P > h->maxP) return fail(MJPC_B200_ERR_CAPACITY, "rollout_spline: N/H/P above capacity");
-  CUDA_TRY(cudaSetDevice(h->device));
-  Staged s = stage_common(h, state, time, mocap);
-  size_t o = s.end;
-  const size_t ok = o; std::memcpy(h->h_in + o, knots, (size_t)N * P * M.nu * 4); o += (size_t)N * P * M.nu;
-  const size_t ot = o;
-  for (int i = 0; i < P; i++) h->h_in[o + i] = (float)(knot_times[i] - time);
-  o += P;
-  CUDA_TRY(cudaMemcpyAsync(h->d_state, h->h_in + s.state, (M.nq + M.nv) * 4, cudaMemcpyHostToDevice, h->stream));
-  if (M.nmocap) CUDA_TRY(cudaMemcpyAsync(h->d_mocap, h->h_in + s.mocap, 7 * M.nmocap * 4, cudaMemcpyHostToDevice, h->stream));
-  if (M.task_state_size) CUDA_TRY(cudaMemcpyAsync(h->d_task_state, h->h_in + s.tstate, M.task_state_size * 4, cudaMemcpyHostToDevice, h->stream));
-  CUDA_TRY(cudaMemcpyAsync(h->d_knots, h->h_in + ok, (size_t)N * P * M.nu * 4, cudaMemcpyHostToDevice, h->stream));
-  CUDA_TRY(cudaMemcpyAsync(h->d_knot_times, h->h_in + ot, (size_t)P * 4, cudaMemcpyHostToDevice, h->stream));
-  RolloutArgs A = base_args(h, time, N, H);
-  A.L = make_layout(h->pack.M, P);
-  A.knots = h->d_knots; A.knot_times = h->d_knot_times; A.P = P; A.interp = interp; A.policy_kind = 0;
-  h->resident = A;
-  h->resident_ok = true;
-  return 0;
+  return upload_spline(h, 1, state, &time, mocap, nullptr, nullptr, nullptr, knots, knot_times, interp, P, N, H);
+}
+
+int mjpc_b200_rollout_spline_batched(mjpc_b200_t* h, int B, const float* states, const double* times, const float* mocaps,
+                                     const double* weights, const double* parameters, const double* task_states,
+                                     const float* knots, const double* knot_times, int interp, int P, int N, int H,
+                                     float* returns, uint8_t* failure, int* order) {
+  if (!h || !states || !times || !knots || !knot_times) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "rollout_spline_batched: null pointer");
+  int rc = upload_spline(h, B, states, times, mocaps, weights, parameters, task_states, knots, knot_times, interp, P, N, H);
+  if (rc) return rc;
+  rc = launch_rollout(h, h->resident);
+  if (rc) return rc;
+  return read_back(h, B * N, returns, failure, order);
 }
 
 int mjpc_b200_launch_resident(mjpc_b200_t* h) {
@@ -513,8 +563,9 @@ int mjpc_b200_rollout_feedback(mjpc_b200_t* h, const float* state, double time, 
   if (K > h->maxN || H > h->maxH) return fail(MJPC_B200_ERR_CAPACITY, "rollout_feedback: K/H above capacity");
   CUDA_TRY(cudaSetDevice(h->device));
   const size_t ds = M.nq + M.nv, n = 2 * M.nv, nu = M.nu;
-  Staged s = stage_common(h, state, time, mocap);
-  size_t o = s.end;
+  RolloutArgs A = base_args(h, K, H);
+  size_t o;
+  if (int rc = stage_problems(h, 1, state, &time, mocap, nullptr, nullptr, nullptr, nullptr, nullptr, 0, K, &A, &o)) return rc;
   auto put = [&](const float* src, size_t cnt) { size_t at = o; if (src) std::memcpy(h->h_in + o, src, cnt * 4); o += cnt; return at; };
   const size_t ou = put(u_nom, H * nu), ox = put(x_nom, H * ds);
   const size_t ot = o;
@@ -522,14 +573,10 @@ int mjpc_b200_rollout_feedback(mjpc_b200_t* h, const float* state, double time, 
   o += H;
   const size_t og = put(gains, H * nu * n), od = put(du, H * nu), os = put(step_sizes, K);
   auto up = [&](float* dst, size_t at, size_t cnt) { return cudaMemcpyAsync(dst, h->h_in + at, cnt * 4, cudaMemcpyHostToDevice, h->stream); };
-  CUDA_TRY(up(h->d_state, s.state, ds));
-  if (M.nmocap) CUDA_TRY(up(h->d_mocap, s.mocap, 7 * M.nmocap));
-  if (M.task_state_size) CUDA_TRY(up(h->d_task_state, s.tstate, M.task_state_size));
   CUDA_TRY(up(h->d_unom, ou, H * nu)); CUDA_TRY(up(h->d_xnom, ox, H * ds)); CUDA_TRY(up(h->d_tnom, ot, H));
   CUDA_TRY(up(h->d_gains, og, H * nu * n));
   if (du) CUDA_TRY(up(h->d_du, od, H * nu));
   CUDA_TRY(up(h->d_steps, os, K));
-  RolloutArgs A = base_args(h, time, K, H);
   A.L = make_layout(h->pack.M, 1);
   A.P = 1; A.policy_kind = 1;
   A.fb.u_nom = h->d_unom; A.fb.x_nom = h->d_xnom; A.fb.t_nom = h->d_tnom; A.fb.gains = h->d_gains;
@@ -680,7 +727,7 @@ int mjpc_b200_rollout_spline_sharded(mjpc_b200_t* h, const float* state, double 
   pack_slot_kernel<<<(width + 255) / 256, 256, 0, h->stream>>>(h->d_returns, h->d_failure, n, width, h->d_slot);
   NCCL_TRY(api.AllGather(h->d_slot, h->d_gather, 2 * (size_t)width, ncclFloat, h->comm, h->stream));
   compact_gather_kernel<<<(N + 255) / 256, 256, 0, h->stream>>>(h->d_gather, N, h->nranks, width, h->d_returns_all, h->d_failure_all);
-  rank_kernel<<<(N + 255) / 256, 256, 0, h->stream>>>(h->d_returns_all, N, h->d_order_all);
+  rank_kernel<<<(N + 255) / 256, 256, 0, h->stream>>>(h->d_returns_all, N, 1, h->d_order_all);
   CUDA_TRY(cudaEventRecord(h->ev1, h->stream));   // the timed span now covers rollout + exchange + ranking
   CUDA_TRY(cudaGetLastError());
   h->launches += 3;

@@ -81,14 +81,18 @@ void LogScale(double* values, double max_value, double min_value, int steps) {
 
 // ------------------------------------------------------------------------------------------ SamplingPlanner
 SamplingPlanner::~SamplingPlanner() {
-  if (gpu_) mjpc_b200_destroy(gpu_);
+  if (gpu_ && owns_gpu_) mjpc_b200_destroy(gpu_);
 }
 
 int SamplingPlanner::Initialize(const mjpc_model_blob* model, int num_trajectory, int num_spline_points, int interpolation,
                                 double exploration, double exploration2, double timestep, const double* ctrlrange,
-                                uint32_t seed, int max_candidates, int max_horizon, int device) {
-  int rc = mjpc_b200_create(model, max_candidates, max_horizon, device, &gpu_);
-  if (rc) return rc;
+                                uint32_t seed, int max_candidates, int max_horizon, int device, mjpc_b200_t* engine) {
+  owns_gpu_ = engine == nullptr;
+  if (engine) {
+    gpu_ = engine;
+  } else if (int rc = mjpc_b200_create(model, max_candidates, max_horizon, device, &gpu_)) {
+    return rc;
+  }
   mjpc_b200_get_info(gpu_, &info_);
   nu_ = info_.nu;
   num_trajectory_ = num_trajectory;
@@ -160,10 +164,8 @@ void SamplingPlanner::AddNoiseToPolicy(int i) {
   }
 }
 
-int SamplingPlanner::Rollouts(int num_trajectory, int horizon) {
+int SamplingPlanner::PrepareCandidates(int num_trajectory, float* knots, double* knot_times) {
   const int P = policy.plan.Size();
-  knots_.resize((size_t)num_trajectory * P * nu_);
-  knot_times_.resize(P);
   for (int i = 0; i < num_trajectory; i++) {
     {
       const std::shared_lock<std::shared_mutex> lock(mtx_);
@@ -172,12 +174,29 @@ int SamplingPlanner::Rollouts(int num_trajectory, int horizon) {
     if (i != 0) AddNoiseToPolicy(i);
     for (int k = 0; k < P; k++) {
       const double* node = candidate_policy[i].plan.NodeValues(k);
-      for (int d = 0; d < nu_; d++) knots_[((size_t)i * P + k) * nu_ + d] = (float)node[d];
+      for (int d = 0; d < nu_; d++) knots[((size_t)i * P + k) * nu_ + d] = (float)node[d];
     }
   }
-  for (int k = 0; k < P; k++) knot_times_[k] = policy.plan.NodeTime(k);
+  for (int k = 0; k < P; k++) knot_times[k] = policy.plan.NodeTime(k);
+  return P;
+}
+
+void SamplingPlanner::InstallRollouts(int num_trajectory, const float* returns, const uint8_t* failure, const int* order,
+                                      int offset) {
+  std::copy(returns, returns + num_trajectory, returns_.begin());
+  std::copy(failure, failure + num_trajectory, failure_.begin());
+  trajectory_order.assign(order, order + num_trajectory);
+  offset_ = offset;
+}
+
+int SamplingPlanner::Rollouts(int num_trajectory, int horizon) {
+  const int P = policy.plan.Size();
+  knots_.resize((size_t)num_trajectory * P * nu_);
+  knot_times_.resize(P);
+  PrepareCandidates(num_trajectory, knots_.data(), knot_times_.data());
   std::vector<float> state_f(state_.begin(), state_.end()), mocap_f(mocap_.begin(), mocap_.end());
   trajectory_order.resize(num_trajectory);
+  offset_ = 0;
   return mjpc_b200_rollout_spline(gpu_, state_f.data(), time_, mocap_f.empty() ? nullptr : mocap_f.data(), nullptr,
                                   knots_.data(), knot_times_.data(), (int)interpolation_, P, num_trajectory, horizon,
                                   returns_.data(), failure_.data(), trajectory_order.data());
@@ -194,11 +213,15 @@ int SamplingPlanner::OptimizePolicyCandidates(int ncandidates, int horizon) {
 
 int SamplingPlanner::OptimizePolicy(int horizon) {
   if (OptimizePolicyCandidates(1, horizon) < 0) return -1;
+  InstallBest();
+  return 0;
+}
+
+void SamplingPlanner::InstallBest() {
   CopyCandidateToPolicy(0);
   const double best_return = returns_[0];   // candidate 0 is the un-noised nominal
   improvement = std::max(best_return - (double)returns_[winner], 0.0);
   iteration++;
-  return 0;
 }
 
 void SamplingPlanner::CopyCandidateToPolicy(int candidate) {
@@ -220,7 +243,7 @@ int SamplingPlanner::FetchTrajectory(int candidate, int horizon, Trajectory* t) 
   t->dim_trace = 3 * in.num_trace;
   t->states.resize(H * in.dim_state); t->actions.resize(H * in.nu); t->times.resize(H);
   t->residual.resize(H * in.num_residual); t->costs.resize(H); t->trace.resize(H * t->dim_trace);
-  if (mjpc_b200_fetch_trajectory(gpu_, candidate, t->states.data(), t->actions.data(), t->times.data(), t->residual.data(),
+  if (mjpc_b200_fetch_trajectory(gpu_, offset_ + candidate, t->states.data(), t->actions.data(), t->times.data(), t->residual.data(),
                                  t->costs.data(), t->trace.data()))
     return -1;
   t->total_return = returns_[candidate];
@@ -241,7 +264,7 @@ const Trajectory* SamplingPlanner::BestTrajectory() {
   best_.dim_trace = 3 * in.num_trace;
   best_.states.resize((size_t)H * in.dim_state); best_.actions.resize((size_t)H * in.nu); best_.times.resize(H);
   best_.residual.resize((size_t)H * in.num_residual); best_.costs.resize(H); best_.trace.resize((size_t)H * best_.dim_trace);
-  if (mjpc_b200_fetch_trajectory(gpu_, winner, best_.states.data(), best_.actions.data(), best_.times.data(),
+  if (mjpc_b200_fetch_trajectory(gpu_, offset_ + winner, best_.states.data(), best_.actions.data(), best_.times.data(),
                                  best_.residual.data(), best_.costs.data(), best_.trace.data()))
     return nullptr;
   best_.total_return = returns_[winner];

@@ -20,6 +20,10 @@ _bp = C.POINTER(C.c_uint8)
 
 EXPORTS = ["mjpc_b200_version", "mjpc_b200_last_error", "mjpc_b200_create", "mjpc_b200_destroy",
            "mjpc_b200_get_info", "mjpc_b200_set_task", "mjpc_b200_set_differentiable", "mjpc_b200_set_xfrc_noise", "mjpc_b200_rollout_spline", "mjpc_b200_rollout_feedback",
+           "mjpc_b200_rollout_spline_batched", "mjpc_b200_batch_planner_create", "mjpc_b200_batch_planner_destroy",
+           "mjpc_b200_batch_planner_reset", "mjpc_b200_batch_planner_set_state", "mjpc_b200_batch_planner_set_task",
+           "mjpc_b200_batch_planner_optimize_policy", "mjpc_b200_batch_planner_action_from_policy",
+           "mjpc_b200_batch_planner_get_result",
            "mjpc_b200_fetch_trajectory", "mjpc_b200_fetch_all", "mjpc_b200_model_derivatives",
            "mjpc_b200_cost_derivatives", "mjpc_b200_backward_pass", "mjpc_b200_step_debug", "mjpc_b200_step_batch", "mjpc_b200_comm_unique_id", "mjpc_b200_comm_init",
            "mjpc_b200_comm_info", "mjpc_b200_rollout_spline_sharded", "mjpc_b200_fetch_trajectory_sharded",
@@ -92,6 +96,7 @@ def load_library():
         lib.mjpc_b200_device_returns.restype = C.c_void_p
         lib.mjpc_b200_host_philox_normal.restype = C.c_double
         lib.mjpc_b200_planner_destroy.argtypes = [C.c_void_p]
+        lib.mjpc_b200_batch_planner_destroy.argtypes = [C.c_void_p]
         lib.mjpc_b200_planner_set_exploration.argtypes = [C.c_void_p, C.c_double, C.c_double]
         lib.mjpc_b200_ce_planner_destroy.argtypes = [C.c_void_p]
         lib.mjpc_b200_sg_planner_destroy.argtypes = [C.c_void_p]
@@ -210,6 +215,24 @@ class Engine:
                                                       _pd(kt), int(interp), P, N, int(H), _pf(ret),
                                                       fail.ctypes.data_as(_bp), order.ctypes.data_as(_ip)))
         self.lastN, self.lastH = N, H
+        return ret, fail, order
+
+    def rollout_spline_batched(self, states, times, mocaps, knots, knot_times, interp, H, weights=None, parameters=None,
+                               task_states=None):
+        """B independent problems in one launch (mjpc_b200_rollout_spline_batched): states [B, dim_state], times [B]
+        (absolute), mocaps [B, 7 nmocap], knots [B, N, P, nu], knot_times [B, P] (absolute); weights [B, num_term],
+        parameters [B, num_parameters], task_states [B, task_state_size] or None for the set_task values.  Returns
+        returns [B, N], failure [B, N] and order [B, N] (indices local to each problem); fetch_* then take the flat
+        index b * N + i."""
+        knots = _f(knots)
+        B, N, P, nu = knots.shape
+        st, t, mc, kt = _f(states), _d(times), _f(mocaps), _d(knot_times)
+        w, p, s = _d(weights), _d(parameters), _d(task_states)
+        ret = np.zeros((B, N), np.float32); fail = np.zeros((B, N), np.uint8); order = np.zeros((B, N), np.int32)
+        self._check(self.lib.mjpc_b200_rollout_spline_batched(self.h, int(B), _pf(st), _pd(t), _pf(mc), _pd(w), _pd(p), _pd(s),
+                                                              _pf(knots), _pd(kt), int(interp), int(P), int(N), int(H),
+                                                              _pf(ret), fail.ctypes.data_as(_bp), order.ctypes.data_as(_ip)))
+        self.lastN, self.lastH = B * N, H
         return ret, fail, order
 
     # ---- multi-GPU: one planning problem sharded over an NCCL communicator owned by the handle
@@ -460,6 +483,76 @@ class CppSamplingPlanner:
     def action_from_policy(self, time, use_previous=False):
         a = np.zeros(self.nu)
         self.lib.mjpc_b200_planner_action_from_policy(self.h, _pd(a), C.c_double(time), int(use_previous))
+        return a
+
+
+class CppBatchSamplingPlanner:
+    """num_problems independent Predictive Sampling problems planned with one rollout launch per iteration
+    (csrc/host/batch_sampling_planner.cc); each method that concerns one problem takes its index."""
+
+    def __init__(self, model, num_problems, num_trajectory, horizon, seeds=None, device=0):
+        self.lib = load_library()
+        m = self.m = model
+        self._blob = to_blob(model)
+        self._buf = C.create_string_buffer(self._blob, len(self._blob))
+        mb = ModelBlob(C.cast(self._buf, C.c_void_p), len(self._blob))
+        num = m.numeric
+        self.P = int(num.get("sampling_spline_points", [3])[0])
+        self.B, self.horizon, self.N, self.nu = int(num_problems), int(horizon), int(num_trajectory), m.nu
+        sd = np.ascontiguousarray([0x5EED + b for b in range(self.B)] if seeds is None else seeds, np.uint32)
+        cr = _d(np.asarray(m.actuator_ctrlrange, float).reshape(-1))
+        h = C.c_void_p()
+        rc = self.lib.mjpc_b200_batch_planner_create(C.byref(mb), self.B, self.N, self.P,
+                                                     int(num.get("sampling_representation", [2])[0]),
+                                                     C.c_double(float(num.get("sampling_exploration", [0.1])[0])),
+                                                     C.c_double(float(m.opt_timestep)), _pd(cr),
+                                                     sd.ctypes.data_as(C.POINTER(C.c_uint32)), self.horizon, int(device),
+                                                     C.byref(h))
+        if rc != 0:
+            raise EngineError(f"mjpc_b200_batch_planner_create failed ({rc}): {self.lib.mjpc_b200_last_error().decode()}")
+        self.h = h
+
+    def close(self):
+        if getattr(self, "h", None):
+            self.lib.mjpc_b200_batch_planner_destroy(self.h)
+            self.h = None
+
+    __del__ = close
+
+    def _check(self, rc, what):
+        if rc < 0:
+            raise EngineError(f"batch_planner_{what} failed ({rc}): {self.lib.mjpc_b200_last_error().decode()}")
+        return rc
+
+    def reset(self, problem, initial_repeated_action=None):
+        a = _d(initial_repeated_action)
+        self._check(self.lib.mjpc_b200_batch_planner_reset(self.h, int(problem), self.horizon, _pd(a)), "reset")
+
+    def set_state(self, problem, state, time, mocap):
+        s, mc = _d(state), _d(mocap)
+        self._check(self.lib.mjpc_b200_batch_planner_set_state(self.h, int(problem), _pd(s), C.c_double(time), _pd(mc)),
+                    "set_state")
+
+    def set_task(self, problem, weight=None, parameters=None, task_state=None):
+        w, p, s = _d(weight), _d(parameters), _d(task_state)
+        self._check(self.lib.mjpc_b200_batch_planner_set_task(self.h, int(problem), _pd(w), _pd(p), _pd(s)), "set_task")
+
+    def optimize_policy(self):
+        """One planning iteration of every problem; returns the per-problem results."""
+        self._check(self.lib.mjpc_b200_batch_planner_optimize_policy(self.h, self.horizon), "optimize_policy")
+        return [self.result(b) for b in range(self.B)]
+
+    def result(self, problem):
+        winner, imp = C.c_int(), C.c_double()
+        ret = np.zeros(self.N, np.float32); knots = np.zeros((self.P, self.nu)); kt = np.zeros(self.P)
+        self._check(self.lib.mjpc_b200_batch_planner_get_result(self.h, int(problem), C.byref(winner), C.byref(imp), _pf(ret),
+                                                                _pd(knots), _pd(kt)), "get_result")
+        return dict(winner=winner.value, improvement=imp.value, returns=ret, knots=knots, knot_times=kt)
+
+    def action_from_policy(self, problem, time, use_previous=False):
+        a = np.zeros(self.nu)
+        self._check(self.lib.mjpc_b200_batch_planner_action_from_policy(self.h, int(problem), _pd(a), C.c_double(time),
+                                                                        int(use_previous)), "action_from_policy")
         return a
 
 
