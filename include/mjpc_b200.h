@@ -17,6 +17,8 @@
  *   mjpc_b200_cost_derivatives  <- CostDerivatives::Compute             mjpc/planners/cost_derivatives.cc:112-230
  *   mjpc_b200_backward_pass     <- RiccatiStep recursion                mjpc/planners/ilqg/planner.cc:429-520,
  *                                                                       mjpc/planners/ilqg/backward_pass.cc:65-250
+ *   mjpc_b200_*_batched         <- the calls above for B independent problems in one launch (rollout_spline,
+ *                                  rollout_feedback, model_derivatives, cost_derivatives, backward_pass)
  *   mjpc_b200_set_task          <- residual_fn_ snapshot per PlanIteration  mjpc/agent.cc:316-319, task.cc:112-128
  *   mjpc_b200_fetch_trajectory  <- fills a mjpc::Trajectory             mjpc/trajectory.h:74-86
  *   create / destroy            <- Planner::Initialize/Allocate + ResizeMjData  mjpc/planners/planner.cc:23-33;
@@ -137,6 +139,19 @@ int mjpc_b200_rollout_feedback(mjpc_b200_t* h, const float* state, double time, 
                                const float* gains, const float* du, const float* step_sizes, int mode, int K, int H,
                                float* returns, uint8_t* failure, int* order);
 
+/* B independent problems of K line-search rollouts each in ONE launch (mjpc_b200_rollout_feedback is the case B = 1).
+ * Conventions as mjpc_b200_rollout_spline_batched: states [B][dim_state], times [B] (absolute), mocaps [B][7 nmocap],
+ * weights / parameters / task_states [B][..] or NULL for the handle's set_task values; per problem u_nom [B][H][nu],
+ * x_nom [B][H][dim_state], t_nom [B][H] (absolute; rebased to times[b]), gains [B][H][nu][dim_dstate], du [B][H][nu]
+ * (may be NULL), step_sizes [B][K]; mode, K and H are common.  returns / failure / order [B][K], order local to the
+ * problem.  B*K > max_candidates or H > max_horizon: MJPC_B200_ERR_CAPACITY; with MJPC_B200_WARPS_PER_CTA > 1 and
+ * B > 1, K must be a multiple of it (MJPC_B200_ERR_UNSUPPORTED).  fetch_* then take the flat index b*K + i. */
+int mjpc_b200_rollout_feedback_batched(mjpc_b200_t* h, int B, const float* states, const double* times, const float* mocaps,
+                                       const double* weights, const double* parameters, const double* task_states,
+                                       const float* u_nom, const float* x_nom, const double* t_nom, const float* gains,
+                                       const float* du, const float* step_sizes, int mode, int K, int H, float* returns,
+                                       uint8_t* failure, int* order);
+
 /* Copy candidate i of the last rollout into Trajectory-shaped host arrays (any pointer may be NULL):
  * states [H][dim_state], actions [H][nu], times [H], residual [H][num_residual], costs [H], trace [H][3*num_trace] */
 int mjpc_b200_fetch_trajectory(mjpc_b200_t* h, int candidate, float* states, float* actions, double* times,
@@ -169,6 +184,24 @@ int mjpc_b200_backward_pass(mjpc_b200_t* h, const float* A, const float* B, cons
                             const float* cxx, const float* cxu, const float* cuu, const float* actions, int H,
                             float mu, int reg_type, int limits, float* K, float* du, float* dV, float* Vx,
                             float* Vxx, int* status_out);
+
+/* The three iLQG sweeps for B independent problems in one launch each (the single-problem calls above are B = 1).
+ * Every per-problem array gains a leading [B] dimension; H, skip, tol, mode, reg_type and limits are common, the risk
+ * is the handle's.  weights [B][num_term], parameters [B][num_parameters], task_states [B][task_state_size] may each
+ * be NULL for the handle's set_task values; problem b's time-like task state is rebased to its own t[b][0].
+ * backward_pass_batched: mu [B], dV [B][2], status [B] (1 success, 0 failure; a failure ends only that problem's
+ * sweep); Vx / Vxx may be NULL.  B < 1 or a NULL required pointer: MJPC_B200_ERR_BAD_ARGUMENT; H > max_horizon:
+ * MJPC_B200_ERR_CAPACITY.  The handle's iLQG buffers grow on demand to the largest B seen. */
+int mjpc_b200_model_derivatives_batched(mjpc_b200_t* h, int B, const float* x, const float* u, const double* t,
+                                        const float* mocaps, const double* weights, const double* parameters,
+                                        const double* task_states, int H, int skip, float tol, int mode, float* A,
+                                        float* B_, float* C, float* D);
+int mjpc_b200_cost_derivatives_batched(mjpc_b200_t* h, int B, const double* weights, const float* residual, const float* C,
+                                       const float* D, int H, float* cx, float* cu, float* cxx, float* cuu, float* cxu);
+int mjpc_b200_backward_pass_batched(mjpc_b200_t* h, int B, const float* A, const float* B_, const float* cx,
+                                    const float* cu, const float* cxx, const float* cxu, const float* cuu,
+                                    const float* actions, int H, const float* mu, int reg_type, int limits, float* K,
+                                    float* du, float* dV, float* Vx, float* Vxx, int* status);
 
 /* Debug / parity hook: one forward-dynamics evaluation + Euler step for a single state through the same
  * device code the rollout kernel runs. qacc[nv], residual[nr], next_qpos[nq], next_qvel[nv], counts[4] =
@@ -382,6 +415,29 @@ int mjpc_b200_host_ilqg_policy_action(const mjpc_model_blob* model, const float*
 /* scalars[6] = {total_return, regularization, improvement, expected, surprise, winner}; nominal states [H][dim_state],
  * actions [H][nu], times [H] (any pointer may be NULL); returns H */
 int mjpc_b200_ilqg_planner_get_result(void* planner, double* scalars, float* states, float* actions, double* times);
+
+/* ---- Batched iLQG (csrc/host/batch_ilqg_planner.{h,cc}): num_problems independent iLQGPlanners (each with its own
+ * state, mocap, task snapshot, policy and regularisation) on ONE engine handle.  optimize_policy makes one batched
+ * launch per sweep for all problems - backward passes are retried in batches of the problems still failing - and each
+ * problem's result equals that of an iLQGPlanner with the same inputs.  The task snapshot of every problem starts as
+ * the model's; set_task replaces its non-NULL members.  Settings (set_fd) are shared.  Calls that take a problem index
+ * return MJPC_B200_ERR_BAD_ARGUMENT when it is outside [0, num_problems). */
+int mjpc_b200_batch_ilqg_planner_create(const mjpc_model_blob* model, int num_problems, int num_rollouts, int representation,
+                                        double fd_tolerance, int max_horizon, int device, void** out);
+void mjpc_b200_batch_ilqg_planner_destroy(void* planner);
+void mjpc_b200_batch_ilqg_planner_set_fd(void* planner, double tolerance, int mode, int derivative_skip);
+int mjpc_b200_batch_ilqg_planner_reset(void* planner, int problem, int horizon, const double* initial_repeated_action);
+int mjpc_b200_batch_ilqg_planner_set_state(void* planner, int problem, const double* state, double time, const double* mocap);
+int mjpc_b200_batch_ilqg_planner_set_task(void* planner, int problem, const double* weight, const double* parameters,
+                                          const double* task_state);
+int mjpc_b200_batch_ilqg_planner_nominal_trajectory(void* planner, int horizon);   /* every problem, one launch */
+/* every problem: iLQGPlanner::OptimizePolicy; updated [num_problems] (may be NULL) receives each problem's 1/0 */
+int mjpc_b200_batch_ilqg_planner_optimize_policy(void* planner, int horizon, int* updated);
+int mjpc_b200_batch_ilqg_planner_action_from_policy(void* planner, int problem, double* action, const double* state,
+                                                    double time);
+/* as mjpc_b200_ilqg_planner_get_result for one problem; returns H */
+int mjpc_b200_batch_ilqg_planner_get_result(void* planner, int problem, double* scalars, float* states, float* actions,
+                                            double* times);
 
 /* ---- Gradient planner (csrc/host/gradient_planner.{h,cc}; mjpc/planners/gradient/planner.cc:159-383, gradient.cc:44-107,
  * spline_mapping.cc): ResamplePolicy, nominal rollout, {model derivatives, cost derivatives, gradient sweep, total derivative

@@ -35,6 +35,7 @@ def _compile(verbose):
                                                                            os.path.join(CSRC, "host", "cross_entropy_planner.cc"),
                                                                            os.path.join(CSRC, "host", "sample_gradient_planner.cc"),
                                                                            os.path.join(CSRC, "host", "ilqg_planner.cc"),
+                                                                           os.path.join(CSRC, "host", "batch_ilqg_planner.cc"),
                                                                            os.path.join(CSRC, "host", "robust_planner.cc"),
                                                                            os.path.join(CSRC, "host", "gradient_planner.cc"),
                                                                            os.path.join(CSRC, "host", "agent.cc"),

@@ -191,32 +191,41 @@ __device__ __forceinline__ void sub_quat(float* res, const float* qa, const floa
 }
 
 struct FeedbackArgs {
-  const float* u_nom;   // [H][nu]
-  const float* x_nom;   // [H][dim_state]
-  const float* t_nom;   // [H] relative to rollout start
-  const float* gains;   // [H][nu][n]
-  const float* du;      // [H][nu] or nullptr
+  const float* u_nom;   // [B][H][nu]
+  const float* x_nom;   // [B][H][dim_state]
+  const float* t_nom;   // [B][H] relative to the problem's rollout start
+  const float* gains;   // [B][H][nu][n]
+  const float* du;      // [B][H][nu] or nullptr
   int mode;             // 0/1/2 time-indexed, 3 step-indexed
   int H;
+  int nper;             // candidates per problem: candidate `cand` follows problem cand / nper's policy
 };
 
-// ctrl <- clamp(u + scale * K * (x (-) x_nom)); global-memory reads are lane-strided (coalesced)
+// ctrl <- clamp(u + scale * K * (x (-) x_nom)) with the policy of candidate `cand`'s problem; global-memory reads are
+// lane-strided (coalesced).  The problem's slices are resolved here, from the candidate index the caller keeps live
+// anyway, so the step loop of the rollout kernels holds no extra register for them.
 template <class SP>
-__device__ __noinline__ void k_policy_feedback(Ctx& c, const FeedbackArgs& fa, float step, int index) {
+__device__ __noinline__ void k_policy_feedback(Ctx& c, const FeedbackArgs& fa, float step, int index, int cand) {
   auto&& M = SP::model(c);
   const int lane = c.lane, nq = M.nq, nv = M.nv, nu = M.nu, ds = nq + nv, n = 2 * nv, H = fa.H;
+  const size_t pH = (size_t)(cand / fa.nper) * H;
+  const float* u_nom = fa.u_nom + pH * nu;
+  const float* x_nom = fa.x_nom + pH * ds;
+  const float* t_nom = fa.t_nom + pH;
+  const float* gains = fa.gains + pH * nu * n;
+  const float* du = fa.du ? fa.du + pH * nu : nullptr;
   float *xn = DF(xnom), *dx = DF(dx), *ctrl = DF(ctrl);
   int rep = 0;
   float scale = 1.f;
   if (fa.mode == 3) {
-    for (int i = lane; i < ds; i += 32) xn[i] = fa.x_nom[index * ds + i];
-    for (int i = lane; i < nu; i += 32) ctrl[i] = fa.u_nom[index * nu + i] + (fa.du ? step * fa.du[index * nu + i] : 0.f);
+    for (int i = lane; i < ds; i += 32) xn[i] = x_nom[index * ds + i];
+    for (int i = lane; i < nu; i += 32) ctrl[i] = u_nom[index * nu + i] + (du ? step * du[index * nu + i] : 0.f);
   } else {
     int b[2];
-    find_interval(b, fa.t_nom, c.time, H);
+    find_interval(b, t_nom, c.time, H);
     rep = (b[0] == b[1]) ? 0 : fa.mode;
-    for (int i = lane; i < ds; i += 32) xn[i] = interp1(c.time, fa.t_nom, fa.x_nom, ds, H, rep, i);
-    for (int i = lane; i < nu; i += 32) ctrl[i] = interp1(c.time, fa.t_nom, fa.u_nom, nu, H - 1, rep, i);
+    for (int i = lane; i < ds; i += 32) xn[i] = interp1(c.time, t_nom, x_nom, ds, H, rep, i);
+    for (int i = lane; i < nu; i += 32) ctrl[i] = interp1(c.time, t_nom, u_nom, nu, H - 1, rep, i);
     scale = step;
   }
   __syncwarp();
@@ -245,10 +254,10 @@ __device__ __noinline__ void k_policy_feedback(Ctx& c, const FeedbackArgs& fa, f
   for (int i = lane; i < nu; i += 32) {
     float a = 0;
     if (fa.mode == 3) {
-      const float* K = fa.gains + ((size_t)index * nu + i) * n;
+      const float* K = gains + ((size_t)index * nu + i) * n;
       for (int j = 0; j < n; j++) a += K[j] * dx[j];
     } else {
-      for (int j = 0; j < n; j++) a += interp1(c.time, fa.t_nom, fa.gains, nu * n, H - 1, rep, i * n + j) * dx[j];
+      for (int j = 0; j < n; j++) a += interp1(c.time, t_nom, gains, nu * n, H - 1, rep, i * n + j) * dx[j];
     }
     const float u = ctrl[i] + scale * a;
     ctrl[i] = fmaxf(range[2 * i], fminf(range[2 * i + 1], u));

@@ -51,7 +51,9 @@ struct mjpc_b200 {
   float* d_pack = nullptr;
   // inputs: d_in holds the per-problem inputs and the knots of the last rollout launch (stage_problems)
   float *d_in = nullptr, *d_task_state = nullptr;
+  // feedback policy of each problem of the last feedback launch ([fb_nprob][max_horizon][..]; grown on demand)
   float *d_unom = nullptr, *d_xnom = nullptr, *d_tnom = nullptr, *d_gains = nullptr, *d_du = nullptr, *d_steps = nullptr;
+  int fb_nprob = 1;
   // outputs
   float *d_states = nullptr, *d_actions = nullptr, *d_residual = nullptr, *d_costs = nullptr, *d_trace = nullptr,
         *d_returns = nullptr;
@@ -175,6 +177,37 @@ int stage_problems(mjpc_b200* h, int B, const float* states, const double* times
   A->weight = weights ? d + o_w : nullptr; A->parameters = parameters ? d + o_p : nullptr;
   A->knot_times = knots ? d + o_kt : nullptr; A->knots = knots ? d + o_k : nullptr;
   *end = o;
+  return 0;
+}
+
+// grow the pinned staging buffer to at least `floats` (never shrinks); on failure the old buffer stays
+int reserve_h_in(mjpc_b200* h, size_t floats) {
+  if (floats <= h->h_in_floats) return 0;
+  float* p = nullptr;
+  CUDA_TRY(cudaStreamSynchronize(h->stream));   // earlier copies may still read the old buffer
+  CUDA_TRY(cudaMallocHost((void**)&p, floats * 4));
+  cudaFreeHost(h->h_in);
+  h->h_in = p; h->h_in_floats = floats;
+  return 0;
+}
+
+// grow the feedback-policy buffers to B problems (never shrinks); on failure the old buffers stay
+int reserve_feedback(mjpc_b200* h, int B) {
+  if (B <= h->fb_nprob) return 0;
+  const DevModel& M = h->pack.M;
+  const size_t H = h->maxH, ds = M.nq + M.nv, n = 2 * M.nv, nu = M.nu, P = B;
+  float* nb[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
+  const size_t cnt[5] = {P * H * nu, P * H * ds, P * H, P * H * nu * n, P * H * nu};
+  for (int i = 0; i < 5; i++)
+    if (cudaMalloc((void**)&nb[i], cnt[i] * 4) != cudaSuccess) {
+      cudaGetLastError();
+      for (float* q : nb) if (q) cudaFree(q);
+      return fail(MJPC_B200_ERR_CUDA, "rollout_feedback_batched: out of device memory for the feedback policies");
+    }
+  CUDA_TRY(cudaStreamSynchronize(h->stream));
+  float** old[5] = {&h->d_unom, &h->d_xnom, &h->d_tnom, &h->d_gains, &h->d_du};
+  for (int i = 0; i < 5; i++) { cudaFree(*old[i]); *old[i] = nb[i]; }
+  h->fb_nprob = B;
   return 0;
 }
 
@@ -550,6 +583,51 @@ int mjpc_b200_rollout_spline(mjpc_b200_t* h, const float* state, double time, co
   return read_back(h, N, returns, failure, order);
 }
 
+// Feedback rollouts of B problems x K candidates in one launch; B = 1 is the single-problem call.  Every problem's
+// nominal times and time-like task state are rebased to its own start time.  Nothing is changed on a refusal.
+static int rollout_feedback_impl(mjpc_b200_t* h, int B, const float* states, const double* times, const float* mocaps,
+                                 const double* weights, const double* parameters, const double* task_states,
+                                 const float* u_nom, const float* x_nom, const double* t_nom, const float* gains,
+                                 const float* du, const float* step_sizes, int mode, int K, int H, float* returns,
+                                 uint8_t* failure, int* order) {
+  const DevModel& M = h->pack.M;
+  if (M.nmocap && !mocaps) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "rollout_feedback: mocap required");
+  if (B < 1 || K < 1 || H < 1 || mode < 0 || mode > 3) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "rollout_feedback: bad sizes");
+  if ((int64_t)B * K > h->maxN || H > h->maxH) return fail(MJPC_B200_ERR_CAPACITY, "rollout_feedback: B*K/H above capacity");
+  // several candidates per CTA share its shared-memory copy of the task: a CTA must not hold two problems
+  if (B > 1 && K % h->warps_per_cta != 0)
+    return fail(MJPC_B200_ERR_UNSUPPORTED, "rollout_feedback_batched: K must be a multiple of MJPC_B200_WARPS_PER_CTA");
+  CUDA_TRY(cudaSetDevice(h->device));
+  const size_t ds = M.nq + M.nv, n = 2 * M.nv, nu = M.nu, Hs = H, P = B;
+  if (int rc = reserve_feedback(h, B)) return rc;
+  if (int rc = reserve_h_in(h, problem_floats(M, B, 0) + P * Hs * (nu + ds + 1 + nu * n + nu) + P * K + 64)) return rc;
+  RolloutArgs A = base_args(h, B * K, H);
+  size_t o;
+  if (int rc = stage_problems(h, B, states, times, mocaps, weights, parameters, task_states, nullptr, nullptr, 0, K, &A, &o))
+    return rc;
+  auto put = [&](const float* src, size_t cnt) { size_t at = o; if (src) std::memcpy(h->h_in + o, src, cnt * 4); o += cnt; return at; };
+  const size_t ou = put(u_nom, P * Hs * nu), ox = put(x_nom, P * Hs * ds);
+  const size_t ot = o;
+  for (int b = 0; b < B; b++)
+    for (int i = 0; i < H; i++) h->h_in[o + (size_t)b * H + i] = (float)(t_nom[(size_t)b * H + i] - times[b]);
+  o += P * Hs;
+  const size_t og = put(gains, P * Hs * nu * n), od = put(du, P * Hs * nu), os = put(step_sizes, P * K);
+  auto up = [&](float* dst, size_t at, size_t cnt) { return cudaMemcpyAsync(dst, h->h_in + at, cnt * 4, cudaMemcpyHostToDevice, h->stream); };
+  CUDA_TRY(up(h->d_unom, ou, P * Hs * nu)); CUDA_TRY(up(h->d_xnom, ox, P * Hs * ds)); CUDA_TRY(up(h->d_tnom, ot, P * Hs));
+  CUDA_TRY(up(h->d_gains, og, P * Hs * nu * n));
+  if (du) CUDA_TRY(up(h->d_du, od, P * Hs * nu));
+  CUDA_TRY(up(h->d_steps, os, P * K));
+  A.L = make_layout(h->pack.M, 1);
+  A.P = 1; A.policy_kind = 1;
+  A.fb.u_nom = h->d_unom; A.fb.x_nom = h->d_xnom; A.fb.t_nom = h->d_tnom; A.fb.gains = h->d_gains;
+  A.fb.du = du ? h->d_du : nullptr; A.fb.mode = mode; A.fb.H = H; A.fb.nper = K;
+  A.step_sizes = h->d_steps;
+  h->resident_ok = false;
+  int rc = launch_rollout(h, A);
+  if (rc) return rc;
+  return read_back(h, B * K, returns, failure, order);
+}
+
 int mjpc_b200_rollout_feedback(mjpc_b200_t* h, const float* state, double time, const float* mocap,
                                const float* userdata, const float* u_nom, const float* x_nom, const double* t_nom,
                                const float* gains, const float* du, const float* step_sizes, int mode, int K, int H,
@@ -557,35 +635,19 @@ int mjpc_b200_rollout_feedback(mjpc_b200_t* h, const float* state, double time, 
   if (!h || !state || !u_nom || !x_nom || !t_nom || !gains || !step_sizes)
     return fail(MJPC_B200_ERR_BAD_ARGUMENT, "rollout_feedback: null pointer");
   if (userdata && h->nuserdata == 0) return fail(MJPC_B200_ERR_UNSUPPORTED, "rollout_feedback: the model has nuserdata = 0, userdata must be NULL");
-  const DevModel& M = h->pack.M;
-  if (M.nmocap && !mocap) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "rollout_feedback: mocap required");
-  if (K < 1 || H < 1 || mode < 0 || mode > 3) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "rollout_feedback: bad sizes");
-  if (K > h->maxN || H > h->maxH) return fail(MJPC_B200_ERR_CAPACITY, "rollout_feedback: K/H above capacity");
-  CUDA_TRY(cudaSetDevice(h->device));
-  const size_t ds = M.nq + M.nv, n = 2 * M.nv, nu = M.nu;
-  RolloutArgs A = base_args(h, K, H);
-  size_t o;
-  if (int rc = stage_problems(h, 1, state, &time, mocap, nullptr, nullptr, nullptr, nullptr, nullptr, 0, K, &A, &o)) return rc;
-  auto put = [&](const float* src, size_t cnt) { size_t at = o; if (src) std::memcpy(h->h_in + o, src, cnt * 4); o += cnt; return at; };
-  const size_t ou = put(u_nom, H * nu), ox = put(x_nom, H * ds);
-  const size_t ot = o;
-  for (int i = 0; i < H; i++) h->h_in[o + i] = (float)(t_nom[i] - time);
-  o += H;
-  const size_t og = put(gains, H * nu * n), od = put(du, H * nu), os = put(step_sizes, K);
-  auto up = [&](float* dst, size_t at, size_t cnt) { return cudaMemcpyAsync(dst, h->h_in + at, cnt * 4, cudaMemcpyHostToDevice, h->stream); };
-  CUDA_TRY(up(h->d_unom, ou, H * nu)); CUDA_TRY(up(h->d_xnom, ox, H * ds)); CUDA_TRY(up(h->d_tnom, ot, H));
-  CUDA_TRY(up(h->d_gains, og, H * nu * n));
-  if (du) CUDA_TRY(up(h->d_du, od, H * nu));
-  CUDA_TRY(up(h->d_steps, os, K));
-  A.L = make_layout(h->pack.M, 1);
-  A.P = 1; A.policy_kind = 1;
-  A.fb.u_nom = h->d_unom; A.fb.x_nom = h->d_xnom; A.fb.t_nom = h->d_tnom; A.fb.gains = h->d_gains;
-  A.fb.du = du ? h->d_du : nullptr; A.fb.mode = mode; A.fb.H = H;
-  A.step_sizes = h->d_steps;
-  h->resident_ok = false;
-  int rc = launch_rollout(h, A);
-  if (rc) return rc;
-  return read_back(h, K, returns, failure, order);
+  return rollout_feedback_impl(h, 1, state, &time, mocap, nullptr, nullptr, nullptr, u_nom, x_nom, t_nom, gains, du,
+                               step_sizes, mode, K, H, returns, failure, order);
+}
+
+int mjpc_b200_rollout_feedback_batched(mjpc_b200_t* h, int B, const float* states, const double* times, const float* mocaps,
+                                       const double* weights, const double* parameters, const double* task_states,
+                                       const float* u_nom, const float* x_nom, const double* t_nom, const float* gains,
+                                       const float* du, const float* step_sizes, int mode, int K, int H, float* returns,
+                                       uint8_t* failure, int* order) {
+  if (!h || !states || !times || !u_nom || !x_nom || !t_nom || !gains || !step_sizes)
+    return fail(MJPC_B200_ERR_BAD_ARGUMENT, "rollout_feedback_batched: null pointer");
+  return rollout_feedback_impl(h, B, states, times, mocaps, weights, parameters, task_states, u_nom, x_nom, t_nom, gains,
+                               du, step_sizes, mode, K, H, returns, failure, order);
 }
 
 static int fetch_impl(mjpc_b200_t* h, int first, int count, float* states, float* actions, double* times,
@@ -879,28 +941,79 @@ int mjpc_b200_spec_words(const mjpc_model_blob* model, int* out, int capacity) {
 void* mjpc_b200_stream(mjpc_b200_t* h) { return h ? (void*)h->stream : nullptr; }
 float* mjpc_b200_device_returns(mjpc_b200_t* h) { return h ? h->d_returns : nullptr; }
 
-// ---- iLQG entry points (kernels in ilqg_kernels.cuh)
+// ---- iLQG entry points (kernels in ilqg_kernels.cuh).  Each single-problem call is the B = 1 case of its batched
+// twin: one staging path and one launch path per sweep.
+
+// B rows of a double task array converted to float, as upload_task converts the handle's; empty for NULL
+static std::vector<float> to_float(const double* v, size_t count) {
+  return v ? std::vector<float>(v, v + count) : std::vector<float>();
+}
+
+static int model_derivatives_impl(mjpc_b200_t* h, int B, const float* x, const float* u, const double* t,
+                                  const float* mocaps, const double* weights, const double* parameters,
+                                  const double* task_states, int H, int skip, float tol, int mode, float* A, float* B_,
+                                  float* C, float* D) {
+  const DevModel& M = h->pack.M;
+  CUDA_TRY(cudaSetDevice(h->device));
+  const size_t nts = M.task_state_size;
+  std::vector<float> ts((size_t)B * nts), trel((size_t)B * H);
+  // derivative sweeps use absolute-time task state rebased to each problem's own t[0]
+  for (int b = 0; b < B; b++) {
+    const double* src = task_states ? task_states + b * nts : h->task_state.data();
+    const double t0 = t[(size_t)b * H];
+    for (size_t i = 0; i < nts; i++) {
+      double v = src[i];
+      if (std::find(h->time_idx.begin(), h->time_idx.end(), (int)i) != h->time_idx.end()) v -= t0;
+      ts[b * nts + i] = (float)v;
+    }
+    for (int i = 0; i < H; i++) trel[(size_t)b * H + i] = (float)(t[(size_t)b * H + i] - t0);
+  }
+  const std::vector<float> w = to_float(weights, (size_t)B * M.num_term), p = to_float(parameters, (size_t)B * M.num_parameters);
+  const size_t smem = h->smem_bytes(1, 1);
+  if (ilqg_reserve(h->ilqg, M, B, smem, h->stream)) return fail(MJPC_B200_ERR_CUDA, "model_derivatives: out of device memory");
+  int launches = 0;
+  int rc = ilqg_model_derivatives(h->ilqg, M, h->d_pack, h->stream, B, x, u, trel.data(), mocaps, ts.data(),
+                                  weights ? w.data() : nullptr, parameters ? p.data() : nullptr, H, tol, A, B_, C, D,
+                                  smem, &launches, h->ev0, h->ev1, skip, mode);
+  h->launches += launches;
+  if (rc == 0 && cudaEventElapsedTime(&h->last_ms, h->ev0, h->ev1) != cudaSuccess) cudaGetLastError();
+  if (rc) return fail(rc, "model_derivatives: CUDA failure");
+  return 0;
+}
+
 int mjpc_b200_model_derivatives(mjpc_b200_t* h, const float* x, const float* u, const double* t, const float* mocap,
                                 int H, int skip, float tol, int mode, float* A, float* B, float* C, float* D) {
   if (!h || !x || !u || !t || !A || !B || !C || !D) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "model_derivatives: null");
   if (H < 1 || H > h->maxH || !(tol > 0)) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "model_derivatives: bad H or tol");
   if (skip < 0 || mode < 0 || mode > 1) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "model_derivatives: bad skip or mode");
   if (h->pack.M.nmocap && !mocap) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "model_derivatives: mocap required");
+  return model_derivatives_impl(h, 1, x, u, t, mocap, nullptr, nullptr, nullptr, H, skip, tol, mode, A, B, C, D);
+}
+
+int mjpc_b200_model_derivatives_batched(mjpc_b200_t* h, int B, const float* x, const float* u, const double* t,
+                                        const float* mocaps, const double* weights, const double* parameters,
+                                        const double* task_states, int H, int skip, float tol, int mode, float* A,
+                                        float* B_, float* C, float* D) {
+  if (!h || !x || !u || !t || !A || !B_ || !C || !D) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "model_derivatives_batched: null");
+  if (B < 1 || H < 1 || !(tol > 0)) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "model_derivatives_batched: bad B, H or tol");
+  if (H > h->maxH) return fail(MJPC_B200_ERR_CAPACITY, "model_derivatives_batched: H above max_horizon");
+  if (skip < 0 || mode < 0 || mode > 1) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "model_derivatives_batched: bad skip or mode");
+  if (h->pack.M.nmocap && !mocaps) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "model_derivatives_batched: mocap required");
+  return model_derivatives_impl(h, B, x, u, t, mocaps, weights, parameters, task_states, H, skip, tol, mode, A, B_, C, D);
+}
+
+static int cost_derivatives_impl(mjpc_b200_t* h, int B, const double* weights, const float* residual, const float* C,
+                                 const float* D, int H, float* cx, float* cu, float* cxx, float* cuu, float* cxu) {
+  const DevModel& M = h->pack.M;
   CUDA_TRY(cudaSetDevice(h->device));
-  std::vector<float> ts(h->pack.M.task_state_size), trel(H);
-  // derivative sweeps use absolute-time task state rebased to t[0]
-  for (size_t i = 0; i < ts.size(); i++) {
-    double v = h->task_state[i];
-    if (std::find(h->time_idx.begin(), h->time_idx.end(), (int)i) != h->time_idx.end()) v -= t[0];
-    ts[i] = (float)v;
-  }
-  for (int i = 0; i < H; i++) trel[i] = (float)(t[i] - t[0]);
+  const std::vector<float> w = to_float(weights, (size_t)B * M.num_term);
+  if (ilqg_reserve(h->ilqg, M, B, h->smem_bytes(1, 1), h->stream)) return fail(MJPC_B200_ERR_CUDA, "cost_derivatives: out of device memory");
   int launches = 0;
-  int rc = ilqg_model_derivatives(h->ilqg, h->pack.M, h->d_pack, h->stream, x, u, trel.data(), mocap, ts.data(), H, tol,
-                                  A, B, C, D, h->smem_bytes(1, 1), &launches, h->ev0, h->ev1, skip, mode);
+  int rc = ilqg_cost_derivatives(h->ilqg, M, h->d_pack, h->stream, B, weights ? w.data() : nullptr, residual, C, D, H,
+                                 cx, cu, cxx, cuu, cxu, &launches, h->ev0, h->ev1);
   h->launches += launches;
   if (rc == 0 && cudaEventElapsedTime(&h->last_ms, h->ev0, h->ev1) != cudaSuccess) cudaGetLastError();
-  if (rc) return fail(rc, "model_derivatives: CUDA failure");
+  if (rc) return fail(rc, "cost_derivatives: CUDA failure");
   return 0;
 }
 
@@ -909,12 +1022,30 @@ int mjpc_b200_cost_derivatives(mjpc_b200_t* h, const float* residual, const floa
   if (!h || !residual || !C || !D || !cx || !cu || !cxx || !cuu || !cxu)
     return fail(MJPC_B200_ERR_BAD_ARGUMENT, "cost_derivatives: null");
   if (H < 1 || H > h->maxH) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "cost_derivatives: bad H");
+  return cost_derivatives_impl(h, 1, nullptr, residual, C, D, H, cx, cu, cxx, cuu, cxu);
+}
+
+int mjpc_b200_cost_derivatives_batched(mjpc_b200_t* h, int B, const double* weights, const float* residual, const float* C,
+                                       const float* D, int H, float* cx, float* cu, float* cxx, float* cuu, float* cxu) {
+  if (!h || !residual || !C || !D || !cx || !cu || !cxx || !cuu || !cxu)
+    return fail(MJPC_B200_ERR_BAD_ARGUMENT, "cost_derivatives_batched: null");
+  if (B < 1 || H < 1) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "cost_derivatives_batched: bad B or H");
+  if (H > h->maxH) return fail(MJPC_B200_ERR_CAPACITY, "cost_derivatives_batched: H above max_horizon");
+  return cost_derivatives_impl(h, B, weights, residual, C, D, H, cx, cu, cxx, cuu, cxu);
+}
+
+static int backward_pass_impl(mjpc_b200_t* h, int B, const float* A, const float* B_, const float* cx, const float* cu,
+                              const float* cxx, const float* cxu, const float* cuu, const float* actions, int H,
+                              const float* mu, int reg_type, int limits, float* K, float* du, float* dV, float* Vx,
+                              float* Vxx, int* status_out) {
   CUDA_TRY(cudaSetDevice(h->device));
+  if (ilqg_reserve(h->ilqg, h->pack.M, B, h->smem_bytes(1, 1), h->stream)) return fail(MJPC_B200_ERR_CUDA, "backward_pass: out of device memory");
   int launches = 0;
-  int rc = ilqg_cost_derivatives(h->ilqg, h->pack.M, h->d_pack, h->stream, residual, C, D, H, cx, cu, cxx, cuu, cxu, &launches, h->ev0, h->ev1);
+  int rc = ilqg_backward_pass(h->ilqg, h->pack.M, h->d_pack, h->stream, B, A, B_, cx, cu, cxx, cxu, cuu, actions, H, mu,
+                              reg_type, limits, K, du, dV, Vx, Vxx, status_out, &launches, h->ev0, h->ev1);
   h->launches += launches;
   if (rc == 0 && cudaEventElapsedTime(&h->last_ms, h->ev0, h->ev1) != cudaSuccess) cudaGetLastError();
-  if (rc) return fail(rc, "cost_derivatives: CUDA failure");
+  if (rc) return fail(rc, "backward_pass: CUDA failure");
   return 0;
 }
 
@@ -925,14 +1056,19 @@ int mjpc_b200_backward_pass(mjpc_b200_t* h, const float* A, const float* B, cons
   if (!h || !A || !B || !cx || !cu || !cxx || !cxu || !cuu || !actions || !K || !du || !dV || !status_out)
     return fail(MJPC_B200_ERR_BAD_ARGUMENT, "backward_pass: null");
   if (H < 2 || H > h->maxH) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "backward_pass: bad H");
-  CUDA_TRY(cudaSetDevice(h->device));
-  int launches = 0;
-  int rc = ilqg_backward_pass(h->ilqg, h->pack.M, h->d_pack, h->stream, A, B, cx, cu, cxx, cxu, cuu, actions, H, mu,
-                              reg_type, limits, K, du, dV, Vx, Vxx, status_out, &launches, h->ev0, h->ev1);
-  h->launches += launches;
-  if (rc == 0 && cudaEventElapsedTime(&h->last_ms, h->ev0, h->ev1) != cudaSuccess) cudaGetLastError();
-  if (rc) return fail(rc, "backward_pass: CUDA failure");
-  return 0;
+  return backward_pass_impl(h, 1, A, B, cx, cu, cxx, cxu, cuu, actions, H, &mu, reg_type, limits, K, du, dV, Vx, Vxx,
+                            status_out);
+}
+
+int mjpc_b200_backward_pass_batched(mjpc_b200_t* h, int B, const float* A, const float* B_, const float* cx,
+                                    const float* cu, const float* cxx, const float* cxu, const float* cuu,
+                                    const float* actions, int H, const float* mu, int reg_type, int limits, float* K,
+                                    float* du, float* dV, float* Vx, float* Vxx, int* status) {
+  if (!h || !A || !B_ || !cx || !cu || !cxx || !cxu || !cuu || !actions || !mu || !K || !du || !dV || !status)
+    return fail(MJPC_B200_ERR_BAD_ARGUMENT, "backward_pass_batched: null");
+  if (B < 1 || H < 2) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "backward_pass_batched: bad B or H");
+  if (H > h->maxH) return fail(MJPC_B200_ERR_CAPACITY, "backward_pass_batched: H above max_horizon");
+  return backward_pass_impl(h, B, A, B_, cx, cu, cxx, cxu, cuu, actions, H, mu, reg_type, limits, K, du, dV, Vx, Vxx, status);
 }
 
 }  // extern "C"

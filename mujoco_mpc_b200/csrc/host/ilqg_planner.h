@@ -3,6 +3,8 @@
 // Every sweep is one call of the C ABI: NominalTrajectory / ActionRollouts -> mjpc_b200_rollout_feedback,
 // ModelDerivatives::Compute -> mjpc_b200_model_derivatives, CostDerivatives::Compute -> mjpc_b200_cost_derivatives,
 // the Riccati loop -> mjpc_b200_backward_pass (the regularisation retry loop, planner.cc:429-520, stays here).
+// The host work around each call is split into prepare / install halves, so BatchILQGPlanner (batch_ilqg_planner.h)
+// can run the same halves for several planners around one batched call.
 #pragma once
 #include <cstdint>
 #include <shared_mutex>
@@ -49,7 +51,9 @@ void iLQGPolicyAction(const iLQGPolicyModel& m, const float* u_nom, const float*
 class iLQGPlanner {
  public:
   ~iLQGPlanner();
-  int Initialize(const mjpc_model_blob* model, int num_rollouts, int representation, int max_horizon, int device);
+  // borrowed != nullptr: plan on that engine handle (not owned; it must hold max_horizon and num_rollouts candidates)
+  int Initialize(const mjpc_model_blob* model, int num_rollouts, int representation, int max_horizon, int device,
+                 mjpc_b200_t* borrowed = nullptr);
   void Reset(int horizon, const double* initial_repeated_action);
   void SetState(const double* state, double time, const double* mocap);
   int OptimizePolicy(int horizon);       // planner.cc:156-165: NominalTrajectory + Iteration; 1 = policy updated
@@ -78,12 +82,25 @@ class iLQGPlanner {
   int dim_action() const { return nu_; }
 
  private:
+  friend class BatchILQGPlanner;
   std::vector<float> StepSizes() const;                                   // LogScale (utilities.cc:819-825) + trailing 0
-  static int BestRollout(const std::vector<float>& ret, const std::vector<uint8_t>& fail, int K);   // :727-740
-  int FetchCandidate(int candidate, double ret);                          // candidate_policy[0].trajectory = trajectory[i]
+  static int BestRollout(const float* ret, const uint8_t* fail, int K);  // :727-740
+  // candidate_policy[0].trajectory = trajectory[candidate]; candidate is the flat index of the last launch
+  int FetchCandidate(int candidate, double ret);
+  // NominalTrajectory = PrepareNominal (policy snapshot, staging) + feedback launch + InstallNominal (winner, copy)
+  int PrepareNominal(int horizon);
+  int InstallNominal(const float* ret, const uint8_t* fail, int cand0);
+  // Iteration = PrepareIteration + derivatives + cost derivatives + {BackwardPending -> backward pass ->
+  // AfterBackward}* + InstallGains + action rollouts + InstallActions (winner, UpdateRegularization, publish)
+  int PrepareIteration(int horizon);
+  bool BackwardPending(int status) const { return reg_iter_ < settings.max_regularization_iterations && status == 0; }
+  void AfterBackward(int status);
+  bool InstallGains(int status);
+  int InstallActions(const float* ret, const uint8_t* fail, int cand0);
   void ScaleRegularization(double factor);                                // backward_pass.cc:327-343
   void UpdateRegularization(double z, double s);                          // :345-356
   mjpc_b200_t* gpu_ = nullptr;
+  bool owns_gpu_ = true;
   mjpc_b200_info info_{};
   iLQGPolicyModel pm_;
   mutable std::shared_mutex mtx_;   // the policy is read by the physics thread while a plan installs a new one
@@ -95,6 +112,11 @@ class iLQGPlanner {
   int live_H_ = 0;
   std::vector<double> state_, mocap_;
   double time_ = 0;
+  // staged by the prepare halves: the launch inputs of this planner's problem
+  std::vector<float> steps_, st_, mc_;
+  double previous_return_ = 0;
+  int reg_iter_ = 0, iter_H_ = 0;
+  float dV_[2] = {0, 0};
   std::vector<float> A_, B_, C_, D_, cx_, cu_, cxx_, cuu_, cxu_, Kbuf_, dubuf_, ret_;
   std::vector<uint8_t> fail_;
   std::vector<int> order_;

@@ -240,7 +240,7 @@ __device__ __forceinline__ void rollout_body(const RolloutArgs& A) {
     // (with a task warp the spline action of step t > 0 was evaluated by it during step t-1's constraint solve)
     if (!last) {
       if (A.policy_kind == 0) { if (!kTask || t == 0) k_policy_spline<SP>(c, A.P, A.interp); }
-      else k_policy_feedback<SP>(c, A.fb, step_size, t);
+      else k_policy_feedback<SP>(c, A.fb, step_size, t, cand);
     }
     // action record (the last row repeats the previous action; H == 1 -> zeros; trajectory.cc:190-196)
     for (int i = lane; i < nu; i += 32) {

@@ -25,7 +25,14 @@ EXPORTS = ["mjpc_b200_version", "mjpc_b200_last_error", "mjpc_b200_create", "mjp
            "mjpc_b200_batch_planner_optimize_policy", "mjpc_b200_batch_planner_action_from_policy",
            "mjpc_b200_batch_planner_get_result",
            "mjpc_b200_fetch_trajectory", "mjpc_b200_fetch_all", "mjpc_b200_model_derivatives",
-           "mjpc_b200_cost_derivatives", "mjpc_b200_backward_pass", "mjpc_b200_step_debug", "mjpc_b200_step_batch", "mjpc_b200_comm_unique_id", "mjpc_b200_comm_init",
+           "mjpc_b200_cost_derivatives", "mjpc_b200_backward_pass", "mjpc_b200_rollout_feedback_batched",
+           "mjpc_b200_model_derivatives_batched", "mjpc_b200_cost_derivatives_batched", "mjpc_b200_backward_pass_batched",
+           "mjpc_b200_batch_ilqg_planner_create", "mjpc_b200_batch_ilqg_planner_destroy",
+           "mjpc_b200_batch_ilqg_planner_set_fd", "mjpc_b200_batch_ilqg_planner_reset",
+           "mjpc_b200_batch_ilqg_planner_set_state", "mjpc_b200_batch_ilqg_planner_set_task",
+           "mjpc_b200_batch_ilqg_planner_nominal_trajectory", "mjpc_b200_batch_ilqg_planner_optimize_policy",
+           "mjpc_b200_batch_ilqg_planner_action_from_policy", "mjpc_b200_batch_ilqg_planner_get_result",
+           "mjpc_b200_step_debug", "mjpc_b200_step_batch", "mjpc_b200_comm_unique_id", "mjpc_b200_comm_init",
            "mjpc_b200_comm_info", "mjpc_b200_rollout_spline_sharded", "mjpc_b200_fetch_trajectory_sharded",
            "mjpc_b200_fetch_stats", "mjpc_b200_launch_count", "mjpc_b200_last_kernel_ms", "mjpc_b200_last_kernel_static",
            "mjpc_b200_spec_words", "mjpc_b200_upload_spline_inputs",
@@ -101,6 +108,9 @@ def load_library():
         lib.mjpc_b200_ce_planner_destroy.argtypes = [C.c_void_p]
         lib.mjpc_b200_sg_planner_destroy.argtypes = [C.c_void_p]
         lib.mjpc_b200_ilqg_planner_destroy.argtypes = [C.c_void_p]
+        lib.mjpc_b200_batch_ilqg_planner_destroy.argtypes = [C.c_void_p]
+        lib.mjpc_b200_batch_ilqg_planner_set_fd.argtypes = [C.c_void_p, C.c_double, C.c_int, C.c_int]
+        lib.mjpc_b200_batch_ilqg_planner_set_fd.restype = None
         for n in ("mjpc_b200_ilqg_planner_set_fd", "mjpc_b200_gradient_planner_set_fd", "mjpc_b200_ilqs_planner_set_fd"):
             getattr(lib, n).argtypes = [C.c_void_p, C.c_double, C.c_int, C.c_int]
             getattr(lib, n).restype = None
@@ -318,6 +328,25 @@ class Engine:
         self.lastN, self.lastH = K, H
         return ret, fail, order
 
+    def rollout_feedback_batched(self, states, times, mocaps, u_nom, x_nom, t_nom, gains, du, step_sizes, mode,
+                                 weights=None, parameters=None, task_states=None):
+        """B problems of K feedback rollouts in one launch (mjpc_b200_rollout_feedback_batched): states [B, dim_state],
+        times [B] (absolute), mocaps [B, 7 nmocap], u_nom [B, H, nu], x_nom [B, H, dim_state], t_nom [B, H] (absolute),
+        gains [B, H, nu, n], du [B, H, nu] or None, step_sizes [B, K]; task arrays [B, ..] or None for the set_task
+        values.  Returns returns / failure / order [B, K] (order local to each problem); fetch_* then take b * K + i."""
+        u, x, t, g, dd, ss = _f(u_nom), _f(x_nom), _d(t_nom), _f(gains), _f(du), _f(step_sizes)
+        B, K = ss.shape
+        H = u.shape[1]
+        st, tm, mc = _f(states), _d(times), _f(mocaps)
+        w, p, s = _d(weights), _d(parameters), _d(task_states)
+        ret = np.zeros((B, K), np.float32); fail = np.zeros((B, K), np.uint8); order = np.zeros((B, K), np.int32)
+        self._check(self.lib.mjpc_b200_rollout_feedback_batched(self.h, int(B), _pf(st), _pd(tm), _pf(mc), _pd(w), _pd(p), _pd(s),
+                                                                _pf(u), _pf(x), _pd(t), _pf(g), _pf(dd), _pf(ss), int(mode),
+                                                                int(K), int(H), _pf(ret), fail.ctypes.data_as(_bp),
+                                                                order.ctypes.data_as(_ip)))
+        self.lastN, self.lastH = B * K, H
+        return ret, fail, order
+
     def fetch_trajectory(self, i):
         H = self.lastH
         o = dict(states=np.zeros((H, self.ds), np.float32), actions=np.zeros((H, self.nu), np.float32),
@@ -398,6 +427,47 @@ class Engine:
                                                      int(limits), _pf(K), _pf(du), _pf(dV), _pf(Vx), _pf(Vxx),
                                                      C.byref(status)))
         return dict(K=K, du=du, dV=dV, Vx=Vx, Vxx=Vxx, status=status.value)
+
+    def model_derivatives_batched(self, x, u, t, mocaps, tol, skip=0, mode=0, weights=None, parameters=None,
+                                  task_states=None):
+        """B problems in one sweep (mjpc_b200_model_derivatives_batched): x [B, H, dim_state], u [B, H, nu], t [B, H]
+        (absolute), mocaps [B, 7 nmocap]; task arrays [B, ..] or None.  Returns A, B, C, D with a leading [B]."""
+        x, u, t, mc = _f(x), _f(u), _d(t), _f(mocaps)
+        w, p, s = _d(weights), _d(parameters), _d(task_states)
+        Bn, H = x.shape[:2]
+        n, nu, nr = self.n, self.nu, self.nr
+        A = np.zeros((Bn, H, n, n), np.float32); B = np.zeros((Bn, H, n, nu), np.float32)
+        Cm = np.zeros((Bn, H, nr, n), np.float32); D = np.zeros((Bn, H, nr, nu), np.float32)
+        self._check(self.lib.mjpc_b200_model_derivatives_batched(self.h, int(Bn), _pf(x), _pf(u), _pd(t), _pf(mc), _pd(w), _pd(p),
+                                                                 _pd(s), int(H), int(skip), C.c_float(tol), int(mode),
+                                                                 _pf(A), _pf(B), _pf(Cm), _pf(D)))
+        return A, B, Cm, D
+
+    def cost_derivatives_batched(self, residual, Cm, D, weights=None):
+        """B problems in one launch: residual [B, H, nr], C, D [B, H, ..]; weights [B, num_term] or None."""
+        r, c, d, w = _f(residual), _f(Cm), _f(D), _d(weights)
+        Bn, H = r.shape[:2]
+        n, nu = self.n, self.nu
+        cx = np.zeros((Bn, H, n), np.float32); cu = np.zeros((Bn, H, nu), np.float32)
+        cxx = np.zeros((Bn, H, n, n), np.float32); cuu = np.zeros((Bn, H, nu, nu), np.float32)
+        cxu = np.zeros((Bn, H, n, nu), np.float32)
+        self._check(self.lib.mjpc_b200_cost_derivatives_batched(self.h, int(Bn), _pd(w), _pf(r), _pf(c), _pf(d), int(H), _pf(cx),
+                                                                _pf(cu), _pf(cxx), _pf(cuu), _pf(cxu)))
+        return cx, cu, cxx, cuu, cxu
+
+    def backward_pass_batched(self, A, B, cx, cu, cxx, cxu, cuu, actions, mu, reg_type=0, limits=1):
+        """B problems, one CTA each (mjpc_b200_backward_pass_batched): every array [B, H, ..], mu [B].  Returns the
+        backward_pass dict with a leading [B] on every entry (status [B])."""
+        a = [_f(v) for v in (A, B, cx, cu, cxx, cxu, cuu, actions)]
+        Bn, H, n, nu = a[1].shape
+        mus = _f(np.broadcast_to(np.asarray(mu, np.float32), (Bn,)))
+        K = np.zeros((Bn, H, nu, n), np.float32); du = np.zeros((Bn, H, nu), np.float32); dV = np.zeros((Bn, 2), np.float32)
+        Vx = np.zeros((Bn, H, n), np.float32); Vxx = np.zeros((Bn, H, n, n), np.float32)
+        status = np.zeros(Bn, np.int32)
+        self._check(self.lib.mjpc_b200_backward_pass_batched(self.h, int(Bn), *[_pf(v) for v in a], int(H), _pf(mus),
+                                                             int(reg_type), int(limits), _pf(K), _pf(du), _pf(dV), _pf(Vx),
+                                                             _pf(Vxx), status.ctypes.data_as(_ip)))
+        return dict(K=K, du=du, dV=dV, Vx=Vx, Vxx=Vxx, status=status)
 
     def fetch_stats(self):
         st = np.zeros((self.lastN, 12), np.int64)
@@ -735,6 +805,77 @@ class CppILQGPlanner:
         a = np.zeros(self.nu)
         s = _d(state)
         self.lib.mjpc_b200_ilqg_planner_action_from_policy(self.h, _pd(a), _pd(s), C.c_double(time))
+        return a
+
+
+class CppBatchILQGPlanner:
+    """The batched C++ iLQG planner (csrc/host/batch_ilqg_planner.cc): B problems, one launch per sweep.  Mirrors
+    CppILQGPlanner with a problem argument."""
+
+    def __init__(self, model, num_problems, horizon, num_rollouts=10, representation=1, fd_tolerance=3e-4, device=0,
+                 fd_mode=1, derivative_skip=0):
+        self.lib = load_library()
+        m = self.m = model
+        self._blob = to_blob(model)
+        self._buf = C.create_string_buffer(self._blob, len(self._blob))
+        mb = ModelBlob(C.cast(self._buf, C.c_void_p), len(self._blob))
+        self.B, self.H, self.nu, self.ds = int(num_problems), int(horizon), m.nu, m.nq + m.nv
+        h = C.c_void_p()
+        rc = self.lib.mjpc_b200_batch_ilqg_planner_create(C.byref(mb), self.B, int(num_rollouts), int(representation),
+                                                          C.c_double(fd_tolerance), self.H, int(device), C.byref(h))
+        if rc != 0:
+            raise EngineError(f"mjpc_b200_batch_ilqg_planner_create failed ({rc}): {self.lib.mjpc_b200_last_error().decode()}")
+        self.h = h
+        self.lib.mjpc_b200_batch_ilqg_planner_set_fd(self.h, C.c_double(fd_tolerance), int(fd_mode), int(derivative_skip))
+
+    def close(self):
+        if getattr(self, "h", None):
+            self.lib.mjpc_b200_batch_ilqg_planner_destroy(self.h)
+            self.h = None
+
+    __del__ = close
+
+    def _check(self, rc, what):
+        if rc < 0:
+            raise EngineError(f"batch_ilqg_planner_{what} failed ({rc}): {self.lib.mjpc_b200_last_error().decode()}")
+        return rc
+
+    def reset(self, problem, initial_repeated_action=None):
+        a = _d(initial_repeated_action)
+        self._check(self.lib.mjpc_b200_batch_ilqg_planner_reset(self.h, int(problem), self.H, _pd(a)), "reset")
+
+    def set_state(self, problem, state, time, mocap):
+        s, mc = _d(state), _d(mocap)
+        self._check(self.lib.mjpc_b200_batch_ilqg_planner_set_state(self.h, int(problem), _pd(s), C.c_double(time), _pd(mc)),
+                    "set_state")
+
+    def set_task(self, problem, weight=None, parameters=None, task_state=None):
+        w, p, s = _d(weight), _d(parameters), _d(task_state)
+        self._check(self.lib.mjpc_b200_batch_ilqg_planner_set_task(self.h, int(problem), _pd(w), _pd(p), _pd(s)), "set_task")
+
+    def nominal_trajectory(self):
+        return self._check(self.lib.mjpc_b200_batch_ilqg_planner_nominal_trajectory(self.h, self.H), "nominal_trajectory")
+
+    def optimize_policy(self):
+        """Every problem's iLQGPlanner::OptimizePolicy; returns updated [B] (1: the policy was updated)."""
+        up = np.zeros(self.B, np.int32)
+        self._check(self.lib.mjpc_b200_batch_ilqg_planner_optimize_policy(self.h, self.H, up.ctypes.data_as(_ip)),
+                    "optimize_policy")
+        return up
+
+    def result(self, problem):
+        sc = np.zeros(6); st = np.zeros((self.H, self.ds), np.float32); ac = np.zeros((self.H, self.nu), np.float32)
+        tm = np.zeros(self.H)
+        self._check(self.lib.mjpc_b200_batch_ilqg_planner_get_result(self.h, int(problem), _pd(sc), _pf(st), _pf(ac), _pd(tm)),
+                    "get_result")
+        return dict(total_return=sc[0], regularization=sc[1], improvement=sc[2], expected=sc[3], surprise=sc[4],
+                    winner=int(sc[5]), states=st, actions=ac, times=tm)
+
+    def action_from_policy(self, problem, time, state=None):
+        a = np.zeros(self.nu)
+        s = _d(state)
+        self._check(self.lib.mjpc_b200_batch_ilqg_planner_action_from_policy(self.h, int(problem), _pd(a), _pd(s),
+                                                                             C.c_double(time)), "action_from_policy")
         return a
 
 
