@@ -25,6 +25,10 @@ enum { kModeQuadruped = 0, kModeBiped, kModeWalk, kModeScramble, kModeFlip };
 enum { kFootFL = 0, kFootHL, kFootFR, kFootHR };
 
 // ------------------------------------------------------------------------------------------ norms (value)
+// Rectify: p * softplus(x / p), written so that no intermediate overflows.  log(1 + e^z) = max(z, 0) + log1p(e^-|z|);
+// the naive form's e^z is inf in fp32 above z ~ 88.7 where the fp64 reference is still finite (e.g. p = 0.01, x = 1)
+__device__ __forceinline__ float softplus_stable(float z) { return fmaxf(z, 0.f) + log1pf(expf(-fabsf(z))); }
+
 __device__ __forceinline__ float norm_value(const float* x, const float* params, int n, int type) {
   float y = 0;
   const float p = params[0], q = params[1];
@@ -68,7 +72,7 @@ __device__ __forceinline__ float norm_value(const float* x, const float* params,
       break;
     case kRectifyLoss:
       MJPC_ROLL
-      for (int i = 0; i < n; i++) y += p > 0 ? p * logf(1 + expf(x[i] / p)) : fmaxf(x[i], 0.f);
+      for (int i = 0; i < n; i++) y += p > 0 ? p * softplus_stable(x[i] / p) : fmaxf(x[i], 0.f);
       break;
   }
   return y;
@@ -98,7 +102,9 @@ __device__ __noinline__ float k_cost_value(Ctx& c) {
     for (int q = 0; q < cnt; q++) cost += __shfl_sync(kFull, term, q);
   }
   if (fabsf(CM(c).risk) < 1e-6f) return cost;
-  return (expf(CM(c).risk * cost) - 1.0f) / CM(c).risk;
+  // expm1f, not expf(.) - 1: near zero cost the difference cancels (fast-math expf is good to ~1e-7 absolute near 1,
+  // an O(1) relative error once |risk * cost| ~ 1e-7).  -use_fast_math does not remap expm1f.
+  return expm1f(CM(c).risk * cost) / CM(c).risk;
 }
 
 // ------------------------------------------------------------------------------------------ spline policy

@@ -47,6 +47,8 @@ struct mjpc_b200 {
   int maxN = 0, maxH = 0, maxP = 64;
   int warps_per_cta = 1;
   int num_sms = 132;
+  size_t smem_optin = 0;   // the device's opt-in limit of dynamic shared memory per block
+  int max_term_dim = 1;    // widest cost term (task_dim_norm_residual): sizes cost_derivatives_kernel's scratch
   int static_spec = 0;   // 1 / 2: the model equals spec_quadruped.h / spec_humanoid_track.h -> static rollout kernel
   float* d_pack = nullptr;
   // inputs: d_in holds the per-problem inputs and the knots of the last rollout launch (stage_problems)
@@ -384,6 +386,7 @@ int mjpc_b200_create(const mjpc_model_blob* model, int max_candidates, int max_h
     if (h->nuserdata != 0) { delete h; return fail(MJPC_B200_ERR_UNSUPPORTED, "create: mjData::userdata (nuserdata > 0) is not supported"); }
     h->weight = b.reals("task_weight"); h->parameters = b.reals("task_parameters");
     h->task_state = b.reals("task_state"); h->risk = b.r("task_risk");
+    for (int d : b.ints("task_dim_norm_residual")) h->max_term_dim = std::max(h->max_term_dim, d);
   }
   h->time_idx = time_like_state(M.residual_id);
   CREATE_TRY(cudaSetDevice(device));
@@ -393,6 +396,7 @@ int mjpc_b200_create(const mjpc_model_blob* model, int max_candidates, int max_h
   cudaDeviceProp prop;
   CREATE_TRY(cudaGetDeviceProperties(&prop, device));
   h->num_sms = prop.multiProcessorCount;
+  h->smem_optin = prop.sharedMemPerBlockOptin;
   const size_t smem_need = h->smem_bytes(h->maxP, 1);
   if (smem_need > (size_t)prop.sharedMemPerBlockOptin) {
     mjpc_b200_destroy(h);
@@ -1006,11 +1010,13 @@ static int cost_derivatives_impl(mjpc_b200_t* h, int B, const double* weights, c
                                  const float* D, int H, float* cx, float* cu, float* cxx, float* cuu, float* cxu) {
   const DevModel& M = h->pack.M;
   CUDA_TRY(cudaSetDevice(h->device));
+  if (cost_derivatives_smem(M, h->max_term_dim) > h->smem_optin)
+    return fail(MJPC_B200_ERR_CAPACITY, "cost_derivatives: the widest cost term does not fit in shared memory");
   const std::vector<float> w = to_float(weights, (size_t)B * M.num_term);
   if (ilqg_reserve(h->ilqg, M, B, h->smem_bytes(1, 1), h->stream)) return fail(MJPC_B200_ERR_CUDA, "cost_derivatives: out of device memory");
   int launches = 0;
   int rc = ilqg_cost_derivatives(h->ilqg, M, h->d_pack, h->stream, B, weights ? w.data() : nullptr, residual, C, D, H,
-                                 cx, cu, cxx, cuu, cxu, &launches, h->ev0, h->ev1);
+                                 cx, cu, cxx, cuu, cxu, h->max_term_dim, &launches, h->ev0, h->ev1);
   h->launches += launches;
   if (rc == 0 && cudaEventElapsedTime(&h->last_ms, h->ev0, h->ev1) != cudaSuccess) cudaGetLastError();
   if (rc) return fail(rc, "cost_derivatives: CUDA failure");

@@ -26,6 +26,11 @@
 namespace mjpc_dev {
 
 // ------------------------------------------------------------------------------------------ norms with derivatives
+// a^b for the exponents of the derivative formulas that can be exactly zero (L22 q/2 - 1, PowerLoss p - 1 and p - 2,
+// SmoothAbs2 q - 2).  Under -use_fast_math powf is ex2(b * lg2(a)), so 0^0 = ex2(0 * -inf) = NaN where IEEE and the fp64
+// reference give 1; every other input takes the unchanged powf path.
+__device__ __forceinline__ float pow_zero_exp(float a, float b) { return b == 0.f ? 1.f : powf(a, b); }
+
 // value; g[n]; H[n*n] (mjpc/norm.cc:50-210). Executed by ONE thread (n <= 16 per term in practice).
 __device__ inline float norm_full(float* g, float* Hn, const float* x, const float* params, int n, int type) {
   float y = 0;
@@ -43,7 +48,7 @@ __device__ inline float norm_full(float* g, float* Hn, const float* x, const flo
       const float a = powf(cc, q / 2) + powf(p, q);
       const float s = powf(a, 1 / q);
       y = s - p;
-      const float dd = powf(cc, q / 2 - 1);
+      const float dd = pow_zero_exp(cc, q / 2 - 1);
       const float b = s / a * dd;
       for (int i = 0; i < n; i++) g[i] = b * x[i];
       const float c2 = (1 - q) * dd / a + (q - 2) / fmaxf(cc, 1e-15f);
@@ -73,8 +78,8 @@ __device__ inline float norm_full(float* g, float* Hn, const float* x, const flo
       for (int i = 0; i < n; i++) {
         const float s = fabsf(x[i]);
         y += powf(s, p);
-        g[i] = (x[i] > 0 ? 1.f : (x[i] < 0 ? -1.f : 0.f)) * p * powf(s, p - 1);
-        Hn[i * n + i] = (p - 1) * p * powf(s, p - 2);
+        g[i] = (x[i] > 0 ? 1.f : (x[i] < 0 ? -1.f : 0.f)) * p * pow_zero_exp(s, p - 1);
+        Hn[i * n + i] = (p - 1) * p * pow_zero_exp(s, p - 2);
       }
       break;
     case kSmoothAbsLoss:
@@ -92,7 +97,7 @@ __device__ inline float norm_full(float* g, float* Hn, const float* x, const flo
         const float e = dd + powf(p, q);
         const float s = powf(e, 1 / q);
         y += s - p;
-        const float c2 = s * powf(a, q - 2) / e;
+        const float c2 = s * pow_zero_exp(a, q - 2) / e;
         g[i] = c2 * x[i];
         Hn[i * n + i] = c2 * (q - 1) * (1 - dd / e);
       }
@@ -100,10 +105,11 @@ __device__ inline float norm_full(float* g, float* Hn, const float* x, const flo
     case kRectifyLoss:
       for (int i = 0; i < n; i++) {
         if (p > 0) {
-          const float s = expf(x[i] / p);
-          y += p * logf(1 + s);
-          g[i] = s / (1 + s);
-          Hn[i * n + i] = s / (p * (1 + s) * (1 + s));
+          // overflow-safe softplus / sigmoid (softplus_stable, dev_task.cuh): e = e^-|z| lies in (0, 1]
+          const float z = x[i] / p, e = expf(-fabsf(z));
+          y += p * softplus_stable(z);
+          g[i] = z >= 0 ? 1 / (1 + e) : e / (1 + e);
+          Hn[i * n + i] = e / (p * (1 + e) * (1 + e));
         } else {
           y += x[i] > 0 ? x[i] : 0.f;
           g[i] = x[i] > 0 ? 1.f : 0.f;
@@ -976,11 +982,18 @@ inline int ilqg_model_derivatives(IlqgBuffers& b, const DevModel& M, const float
   return 0;
 }
 
-// nprob problems; w [nprob][num_term] (float) or nullptr for the packed Task::weight
+// dynamic shared memory of cost_derivatives_kernel for a model whose widest cost term has kmax residuals
+inline size_t cost_derivatives_smem(const DevModel& M, int kmax) {
+  const size_t n = 2 * (size_t)M.nv, m = M.nu, nr = M.num_residual, k = kmax;
+  return (nr + k * k + k * n + k * m + n + m + n * n + m * m + n * m + 8) * 4;
+}
+
+// nprob problems; w [nprob][num_term] (float) or nullptr for the packed Task::weight; kmax = the widest cost term
+// (the kernel lays its scratch out with it: the caller checks cost_derivatives_smem against the device limit)
 inline int ilqg_cost_derivatives(IlqgBuffers& b, const DevModel& M, const float* d_pack, cudaStream_t st, int nprob,
                                  const float* w, const float* residual, const float* C, const float* D, int H, float* cx,
-                                 float* cu, float* cxx, float* cuu, float* cxu, int* launches, cudaEvent_t e0 = nullptr,
-                                 cudaEvent_t e1 = nullptr) {
+                                 float* cu, float* cxx, float* cuu, float* cxu, int kmax, int* launches,
+                                 cudaEvent_t e0 = nullptr, cudaEvent_t e1 = nullptr) {
   const size_t n = b.n, m = b.nu, nr = b.nr, P = nprob;
   ILQG_TRY(cudaMemcpyAsync(b.res, residual, P * H * nr * 4, cudaMemcpyHostToDevice, st));
   ILQG_TRY(cudaMemcpyAsync(b.C, C, P * H * nr * n * 4, cudaMemcpyHostToDevice, st));
@@ -991,8 +1004,7 @@ inline int ilqg_cost_derivatives(IlqgBuffers& b, const DevModel& M, const float*
   a.M = M; a.pack = d_pack; a.residual = b.res; a.C = b.C; a.D = b.D; a.H = H; a.n = (int)n; a.m = (int)m;
   a.weight = (w && M.num_term) ? b.w : nullptr;
   a.cx = b.cx; a.cu = b.cu; a.cxx = b.cxx; a.cuu = b.cuu; a.cxu = b.cxu;
-  const size_t kmax = 32;
-  const size_t smem = (nr + kmax * kmax + kmax * n + kmax * m + n + m + n * n + m * m + n * m + 8) * 4;
+  const size_t smem = cost_derivatives_smem(M, kmax);
   ILQG_TRY(raise_smem_limit((const void*)cost_derivatives_kernel, smem));
   if (e0) ILQG_TRY(cudaEventRecord(e0, st));
   cost_derivatives_kernel<<<dim3(H, nprob), 256, smem, st>>>(a);
