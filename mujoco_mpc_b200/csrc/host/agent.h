@@ -56,15 +56,8 @@ class Agent {
   AgentSettings settings;
 
  private:
-  std::vector<mjpc_b200_t*> Handles();
   int steps_ = 1, differentiable_ = 0;
-  std::unique_ptr<SamplingPlanner> sampling_;
-  std::unique_ptr<GradientPlanner> gradient_;
-  std::unique_ptr<iLQGPlanner> ilqg_;
-  std::unique_ptr<iLQSPlanner> ilqs_;
-  std::unique_ptr<RobustPlanner> robust_;
-  std::unique_ptr<CrossEntropyPlanner> ce_;
-  std::unique_ptr<SampleGradientPlanner> sg_;
+  std::unique_ptr<Planner> planner_;
   std::vector<double> state_, mocap_, weight_, parameters_, task_state_;
   double time_ = 0, risk_ = 0;
   bool have_task_ = false;

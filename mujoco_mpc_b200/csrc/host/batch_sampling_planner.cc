@@ -88,7 +88,7 @@ int BatchSamplingPlanner::OptimizePolicy(int horizon) {
   // per problem, as SamplingPlanner::OptimizePolicy after its launch
   for (int b = 0; b < B; b++) {
     const size_t o = (size_t)b * N;
-    problems_[b]->InstallRollouts(N, returns_.data() + o, failure_.data() + o, order_.data() + o, (int)o);
+    problems_[b]->InstallRollouts(N, horizon, returns_.data() + o, failure_.data() + o, order_.data() + o, (int)o);
     problems_[b]->InstallBest();
   }
   return 0;
@@ -147,7 +147,7 @@ int mjpc_b200_batch_planner_optimize_policy(void* p, int horizon) {
 int mjpc_b200_batch_planner_action_from_policy(void* p, int problem, double* action, double time, int use_previous) {
   BatchSamplingPlanner* bp = problem_of(p, problem);
   if (!bp || !action) return MJPC_B200_ERR_BAD_ARGUMENT;
-  bp->problem(problem).ActionFromPolicy(action, time, use_previous != 0);
+  bp->problem(problem).ActionFromPolicy(action, nullptr, time, use_previous != 0);
   return 0;
 }
 int mjpc_b200_batch_planner_get_result(void* p, int problem, int* winner, double* improvement, float* returns,

@@ -8,17 +8,11 @@
 
 namespace mjpc_b200_host {
 
-CrossEntropyPlanner::~CrossEntropyPlanner() {
-  if (gpu_) mjpc_b200_destroy(gpu_);
-}
-
 int CrossEntropyPlanner::Initialize(const mjpc_model_blob* model, int num_trajectory, int n_elite, int num_spline_points,
                                     int interpolation, double std_initial, double std_min, double explore_fraction,
                                     double timestep, const double* ctrlrange, uint32_t seed, int max_horizon, int device) {
   // N noisy candidates + the nominal trajectory share one launch
-  int rc = mjpc_b200_create(model, num_trajectory + 1, max_horizon, device, &gpu_);
-  if (rc) return rc;
-  mjpc_b200_get_info(gpu_, &info_);
+  if (int rc = AttachEngine(model, num_trajectory + 1, max_horizon, device)) return rc;
   nu_ = info_.nu;
   num_trajectory_ = num_trajectory;
   n_elite_ = n_elite > 0 ? n_elite : std::max(num_trajectory / 10, 2);   // planner.cc:69-71
@@ -30,7 +24,6 @@ int CrossEntropyPlanner::Initialize(const mjpc_model_blob* model, int num_trajec
   policy.ctrlrange.assign(ctrlrange, ctrlrange + 2 * nu_);
   resampled_policy = policy; previous_policy = policy;
   candidate_policy.assign(num_trajectory, policy);
-  state_.assign(info_.dim_state, 0.0); mocap_.assign(7 * info_.nmocap, 0.0);
   returns_.assign(num_trajectory + 1, 0.f); failure_.assign(num_trajectory + 1, 0);
   trajectory_order.resize(num_trajectory);
   std::iota(trajectory_order.begin(), trajectory_order.end(), 0);
@@ -46,12 +39,6 @@ void CrossEntropyPlanner::Reset(int, const double* initial_repeated_action) {
   variance.assign((size_t)policy.num_spline_points * nu_, std_initial_ * std_initial_);
   times_scratch_.assign(policy.num_spline_points, 0.0);
   improvement = 0; iteration = 0;
-}
-
-void CrossEntropyPlanner::SetState(const double* state, double time, const double* mocap) {
-  std::copy(state, state + state_.size(), state_.begin());
-  if (!mocap_.empty()) std::copy(mocap, mocap + mocap_.size(), mocap_.begin());
-  time_ = time;
 }
 
 void CrossEntropyPlanner::ResamplePolicy(int horizon) {
@@ -97,11 +84,9 @@ int CrossEntropyPlanner::Rollouts(int num_trajectory, int horizon) {
       for (int d = 0; d < nu_; d++) knots_[((size_t)i * P + k) * nu_ + d] = (float)node[d];
     }
   }
-  std::vector<float> state_f(state_.begin(), state_.end()), mocap_f(mocap_.begin(), mocap_.end());
   order_all_.resize(num_trajectory + 1);
-  return mjpc_b200_rollout_spline(gpu_, state_f.data(), time_, mocap_f.empty() ? nullptr : mocap_f.data(), nullptr,
-                                  knots_.data(), times_scratch_.data(), (int)interpolation_, P, num_trajectory + 1,
-                                  horizon, returns_.data(), failure_.data(), order_all_.data());
+  return RolloutSpline(knots_.data(), times_scratch_.data(), (int)interpolation_, P, num_trajectory + 1, horizon,
+                       returns_.data(), failure_.data(), order_all_.data());
 }
 
 int CrossEntropyPlanner::OptimizePolicy(int horizon) {
@@ -151,22 +136,13 @@ int CrossEntropyPlanner::OptimizePolicy(int horizon) {
   return 0;
 }
 
-void CrossEntropyPlanner::ActionFromPolicy(double* action, double time, bool use_previous) {
+void CrossEntropyPlanner::ActionFromPolicy(double* action, const double*, double time, bool use_previous) {
   const std::shared_lock<std::shared_mutex> lock(mtx_);
   (use_previous ? previous_policy : policy).Action(action, time);
 }
 
 const Trajectory* CrossEntropyPlanner::BestTrajectory() {
-  const mjpc_b200_info& in = info_;
-  const int H = in.max_horizon;
-  nominal_.dim_state = in.dim_state; nominal_.dim_action = in.nu; nominal_.dim_residual = in.num_residual;
-  nominal_.dim_trace = 3 * in.num_trace;
-  nominal_.states.resize((size_t)H * in.dim_state); nominal_.actions.resize((size_t)H * in.nu); nominal_.times.resize(H);
-  nominal_.residual.resize((size_t)H * in.num_residual); nominal_.costs.resize(H);
-  nominal_.trace.resize((size_t)H * nominal_.dim_trace);
-  if (mjpc_b200_fetch_trajectory(gpu_, num_trajectory_, nominal_.states.data(), nominal_.actions.data(),
-                                 nominal_.times.data(), nominal_.residual.data(), nominal_.costs.data(), nominal_.trace.data()))
-    return nullptr;
+  if (FetchTrajectory(num_trajectory_, horizon_, &nominal_)) return nullptr;
   nominal_.total_return = returns_[num_trajectory_];
   nominal_.failure = failure_[num_trajectory_];
   return &nominal_;
@@ -200,7 +176,7 @@ void mjpc_b200_ce_planner_set_state(void* p, const double* state, double time, c
 }
 int mjpc_b200_ce_planner_optimize_policy(void* p, int horizon) { return ((CrossEntropyPlanner*)p)->OptimizePolicy(horizon); }
 void mjpc_b200_ce_planner_action_from_policy(void* p, double* action, double time, int use_previous) {
-  ((CrossEntropyPlanner*)p)->ActionFromPolicy(action, time, use_previous != 0);
+  ((CrossEntropyPlanner*)p)->ActionFromPolicy(action, nullptr, time, use_previous != 0);
 }
 // improvement, returns [N+1] (the last one is the nominal), elite order [N], installed policy knots/times, variance
 int mjpc_b200_ce_planner_get_result(void* pv, double* improvement, float* returns, int* order, double* knots,
@@ -210,12 +186,7 @@ int mjpc_b200_ce_planner_get_result(void* pv, double* improvement, float* return
   if (returns) std::copy(p->returns().begin(), p->returns().end(), returns);
   if (order) std::copy(p->trajectory_order.begin(), p->trajectory_order.end(), order);
   if (variance) std::copy(p->variance.begin(), p->variance.end(), variance);
-  const auto& plan = p->policy.plan;
-  for (int k = 0; k < plan.Size(); k++) {
-    if (knot_times) knot_times[k] = plan.NodeTime(k);
-    if (knots) std::copy(plan.NodeValues(k), plan.NodeValues(k) + plan.Dim(), knots + (size_t)k * plan.Dim());
-  }
-  return plan.Size();
+  return p->policy.plan.Export(knots, knot_times);
 }
 
 }  // extern "C"

@@ -8,22 +8,22 @@
 
 namespace mjpc_b200_host {
 
-class CrossEntropyPlanner {
+class CrossEntropyPlanner : public Planner {
  public:
-  ~CrossEntropyPlanner();
   // settings the reference reads from <custom> numerics (planner.cc:55-71): sampling_exploration (initial std),
   // std_min, explore_fraction, sampling_trajectories, n_elite (default max(N/10, 2))
   int Initialize(const mjpc_model_blob* model, int num_trajectory, int n_elite, int num_spline_points, int interpolation,
                  double std_initial, double std_min, double explore_fraction, double timestep, const double* ctrlrange,
                  uint32_t seed, int max_horizon, int device);
-  void Reset(int horizon, const double* initial_repeated_action);   // :121-150 (variance = std_initial^2)
-  void SetState(const double* state, double time, const double* mocap);
-  int OptimizePolicy(int horizon);                    // :153-292
+  void Reset(int horizon, const double* initial_repeated_action) override;   // :121-150 (variance = std_initial^2)
+  int OptimizePolicy(int horizon) override;           // :153-292
+  int NominalTrajectory(int) override { return 0; }   // not restated: planning disabled leaves the plan as it is
   void ResamplePolicy(int horizon);                   // :343-371
   void AddNoiseToPolicy(int i, double std_min);       // :374-411
   int Rollouts(int num_trajectory, int horizon);      // :414-459
-  void ActionFromPolicy(double* action, double time, bool use_previous = false);   // :331-340
-  const Trajectory* BestTrajectory();                 // the NOMINAL trajectory (:462-464)
+  // :331-340; the policy does not depend on the state
+  void ActionFromPolicy(double* action, const double* state, double time, bool use_previous = false) override;
+  const Trajectory* BestTrajectory() override;        // the NOMINAL trajectory (:462-464)
 
   SamplingPolicy policy, resampled_policy, previous_policy;
   std::vector<SamplingPolicy> candidate_policy;
@@ -33,17 +33,13 @@ class CrossEntropyPlanner {
   int iteration = 0;
   int n_elite() const { return n_elite_; }
   const std::vector<float>& returns() const { return returns_; }
-  mjpc_b200_t* gpu() { return gpu_; }
 
  private:
-  mjpc_b200_t* gpu_ = nullptr;
-  mjpc_b200_info info_{};
   int num_trajectory_ = 0, n_elite_ = 2, nu_ = 0;
   SplineInterpolation interpolation_ = kCubicSpline;
   double std_initial_ = 0.1, std_min_ = 0.01, explore_fraction_ = 0.0, timestep_ = 0.01;
   uint32_t seed_ = 0x5EED;
-  std::vector<double> state_, mocap_, times_scratch_;
-  double time_ = 0;
+  std::vector<double> times_scratch_;
   std::vector<float> knots_, returns_;
   std::vector<uint8_t> failure_;
   std::vector<int> order_all_;

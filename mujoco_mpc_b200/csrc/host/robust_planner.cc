@@ -5,6 +5,12 @@
 
 namespace mjpc_b200_host {
 
+int RobustPlanner::Initialize(std::unique_ptr<SamplingPlanner> delegate, const mjpc_model_blob* model,
+                              int noisy_candidates, int max_horizon, int device) {
+  delegate_ = std::move(delegate);
+  return AttachEngine(model, noisy_candidates, max_horizon, device);
+}
+
 void RobustPlanner::Configure(int sampling_trajectories, int ncandidates, int nrepetitions, double xfrc_std,
                               double xfrc_rate, uint32_t seed) {
   nrepetitions_ = nrepetitions > 0 ? nrepetitions : 5;
@@ -14,11 +20,7 @@ void RobustPlanner::Configure(int sampling_trajectories, int ncandidates, int nr
 
 void RobustPlanner::SetState(const double* state, double time, const double* mocap) {
   delegate_->SetState(state, time, mocap);
-  mjpc_b200_info info;
-  mjpc_b200_get_info(noisy_, &info);
-  state_.assign(state, state + info.dim_state);
-  mocap_.assign(mocap, mocap + (mocap ? 7 * info.nmocap : 0));
-  time_ = time;
+  Planner::SetState(state, time, mocap);
 }
 
 int RobustPlanner::OptimizePolicy(int horizon) {
@@ -47,11 +49,9 @@ int RobustPlanner::OptimizePolicy(int horizon) {
         const double* node = d.candidate_policy[order[c]].plan.NodeValues(k);
         for (int a = 0; a < nu; a++) knots[(((size_t)c * rep + j) * P + k) * nu + a] = (float)node[a];
       }
-  std::vector<float> st(state_.begin(), state_.end()), mc(mocap_.begin(), mocap_.end());
-  if (mjpc_b200_set_xfrc_noise(noisy_, xfrc_std_, xfrc_rate_, seed_ + (uint32_t)d.iteration)) return -1;
-  if (mjpc_b200_rollout_spline(noisy_, st.data(), time_, mc.empty() ? nullptr : mc.data(), nullptr, knots.data(),
-                               knot_times.data(), (int)nominal.Interpolation(), P, ncandidates * rep, horizon, ret.data(),
-                               fail.data(), nullptr))
+  if (mjpc_b200_set_xfrc_noise(gpu_, xfrc_std_, xfrc_rate_, seed_ + (uint32_t)d.iteration)) return -1;
+  if (RolloutSpline(knots.data(), knot_times.data(), (int)nominal.Interpolation(), P, ncandidates * rep, horizon,
+                    ret.data(), fail.data(), nullptr))
     return -1;
   // for each candidate the mean of its valid noisy returns; pick the best mean (robust_planner.cc:131-154)
   int best_candidate = -1;
@@ -92,10 +92,9 @@ int mjpc_b200_robust_planner_create(const mjpc_model_blob* model, int num_trajec
   int rc = d->Initialize(model, num_trajectory, num_spline_points, interpolation, exploration, 0.0, timestep, ctrlrange,
                          seed, num_trajectory, max_horizon, device);
   if (rc) { *out = nullptr; return rc; }
-  mjpc_b200_t* noisy = nullptr;
-  rc = mjpc_b200_create(model, std::max(nc * rep, 1), max_horizon, device, &noisy);
-  if (rc) { *out = nullptr; return rc; }
-  auto* p = new RobustPlanner(std::move(d), noisy);
+  auto* p = new RobustPlanner;
+  rc = p->Initialize(std::move(d), model, std::max(nc * rep, 1), max_horizon, device);
+  if (rc) { delete p; *out = nullptr; return rc; }
   p->Configure(num_trajectory, ncandidates, nrepetitions, xfrc_std, xfrc_rate, seed);
   *out = p;
   return 0;
@@ -109,7 +108,7 @@ void mjpc_b200_robust_planner_set_state(void* p, const double* state, double tim
 }
 int mjpc_b200_robust_planner_optimize_policy(void* p, int horizon) { return ((RobustPlanner*)p)->OptimizePolicy(horizon); }
 void mjpc_b200_robust_planner_action_from_policy(void* p, double* action, double time, int use_previous) {
-  ((RobustPlanner*)p)->ActionFromPolicy(action, time, use_previous != 0);
+  ((RobustPlanner*)p)->ActionFromPolicy(action, nullptr, time, use_previous != 0);
 }
 // winner (candidate index of the clean launch), robust scores [ncandidates] (mean noisy return per top candidate),
 // clean returns [num_trajectory], installed knots / times; returns the number of scores written
@@ -120,11 +119,7 @@ int mjpc_b200_robust_planner_get_result(void* pv, int* winner, double* scores, f
   if (winner) *winner = d->winner;
   if (scores) std::copy(p->scores().begin(), p->scores().end(), scores);
   if (returns) std::copy(d->returns().begin(), d->returns().end(), returns);
-  const auto& plan = d->policy.plan;
-  for (int k = 0; k < plan.Size(); k++) {
-    if (knot_times) knot_times[k] = plan.NodeTime(k);
-    if (knots) std::copy(plan.NodeValues(k), plan.NodeValues(k) + plan.Dim(), knots + (size_t)k * plan.Dim());
-  }
+  d->policy.plan.Export(knots, knot_times);
   return (int)p->scores().size();
 }
 

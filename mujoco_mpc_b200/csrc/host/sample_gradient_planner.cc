@@ -8,19 +8,13 @@
 
 namespace mjpc_b200_host {
 
-SampleGradientPlanner::~SampleGradientPlanner() {
-  if (gpu_) mjpc_b200_destroy(gpu_);
-}
-
 int SampleGradientPlanner::Initialize(const mjpc_model_blob* model, int num_trajectory, int num_gradient,
                                       int num_spline_points, int interpolation, double exploration,
                                       double gradient_filter, double timestep, const double* ctrlrange, uint32_t seed,
                                       int max_horizon, int device) {
   if (num_trajectory < 1 || num_spline_points < 2) return MJPC_B200_ERR_BAD_ARGUMENT;   // ResamplePolicy divides by P - 1
   // the nominal, the noisy samples and the gradient candidates share one launch
-  int rc = mjpc_b200_create(model, num_trajectory, max_horizon, device, &gpu_);
-  if (rc) return rc;
-  mjpc_b200_get_info(gpu_, &info_);
+  if (int rc = AttachEngine(model, num_trajectory, max_horizon, device)) return rc;
   nu_ = info_.nu;
   num_trajectory_ = num_trajectory;
   num_gradient_ = std::max(num_gradient, 0);
@@ -31,7 +25,6 @@ int SampleGradientPlanner::Initialize(const mjpc_model_blob* model, int num_traj
   policy.num_spline_points = num_spline_points;
   policy.ctrlrange.assign(ctrlrange, ctrlrange + 2 * nu_);
   candidate_policy.assign(num_trajectory, policy);
-  state_.assign(info_.dim_state, 0.0); mocap_.assign(7 * info_.nmocap, 0.0);
   returns_.assign(num_trajectory, 0.f); failure_.assign(num_trajectory, 0);
   trajectory_order.resize(num_trajectory);
   std::iota(trajectory_order.begin(), trajectory_order.end(), 0);
@@ -48,12 +41,6 @@ void SampleGradientPlanner::Reset(int, const double* initial_repeated_action) {
   noise.assign((size_t)num_trajectory_ * num_parameters, 0.0);
   gradient.assign(num_parameters, 0.0); gradient_previous.assign(num_parameters, 0.0);
   improvement = 0; winner = 0; winner_type = kNominal; iteration = 0;
-}
-
-void SampleGradientPlanner::SetState(const double* state, double time, const double* mocap) {
-  std::copy(state, state + state_.size(), state_.begin());
-  if (!mocap_.empty()) std::copy(mocap, mocap + mocap_.size(), mocap_.begin());
-  time_ = time;
 }
 
 void SampleGradientPlanner::ResamplePolicy(SamplingPolicy& p, int horizon, int num_spline_points) {
@@ -99,11 +86,9 @@ int SampleGradientPlanner::Rollouts(int num_trajectory, int num_gradient, int ho
       for (int d = 0; d < nu_; d++) knots_[((size_t)i * P + k) * nu_ + d] = (float)node[d];
     }
   }
-  std::vector<float> state_f(state_.begin(), state_.end()), mocap_f(mocap_.begin(), mocap_.end());
   // the device ranks all N (lower index first on ties): replaces the partial_sort of OptimizePolicy (:219-229)
-  return mjpc_b200_rollout_spline(gpu_, state_f.data(), time_, mocap_f.empty() ? nullptr : mocap_f.data(), nullptr,
-                                  knots_.data(), knot_times_.data(), (int)interpolation_, P, num_trajectory, horizon,
-                                  returns_.data(), failure_.data(), trajectory_order.data());
+  return RolloutSpline(knots_.data(), knot_times_.data(), (int)interpolation_, P, num_trajectory, horizon,
+                       returns_.data(), failure_.data(), trajectory_order.data());
 }
 
 int SampleGradientPlanner::OptimizePolicy(int horizon) {
@@ -196,29 +181,18 @@ int SampleGradientPlanner::NominalTrajectory(int horizon) {
     const double* node = resampled_policy.plan.NodeValues(k);
     std::copy(node, node + nu_, knots_.begin() + (size_t)k * nu_);
   }
-  std::vector<float> state_f(state_.begin(), state_.end()), mocap_f(mocap_.begin(), mocap_.end());
-  return mjpc_b200_rollout_spline(gpu_, state_f.data(), time_, mocap_f.empty() ? nullptr : mocap_f.data(), nullptr,
-                                  knots_.data(), knot_times_.data(), (int)resampled_policy.plan.Interpolation(), P, 1,
-                                  horizon, returns_.data(), failure_.data(), trajectory_order.data());
+  return RolloutSpline(knots_.data(), knot_times_.data(), (int)resampled_policy.plan.Interpolation(), P, 1, horizon,
+                       returns_.data(), failure_.data(), trajectory_order.data());
 }
 
-void SampleGradientPlanner::ActionFromPolicy(double* action, double time, bool use_previous) {
+void SampleGradientPlanner::ActionFromPolicy(double* action, const double*, double time, bool use_previous) {
   // previous_policy is set only by Reset, as in the reference
   const std::shared_lock<std::shared_mutex> lock(mtx_);
   (use_previous ? previous_policy : policy).Action(action, time);
 }
 
 const Trajectory* SampleGradientPlanner::BestTrajectory() {
-  const mjpc_b200_info& in = info_;
-  const int H = in.max_horizon;
-  best_.dim_state = in.dim_state; best_.dim_action = in.nu; best_.dim_residual = in.num_residual;
-  best_.dim_trace = 3 * in.num_trace;
-  best_.states.resize((size_t)H * in.dim_state); best_.actions.resize((size_t)H * in.nu); best_.times.resize(H);
-  best_.residual.resize((size_t)H * in.num_residual); best_.costs.resize(H);
-  best_.trace.resize((size_t)H * best_.dim_trace);
-  if (mjpc_b200_fetch_trajectory(gpu_, winner, best_.states.data(), best_.actions.data(), best_.times.data(),
-                                 best_.residual.data(), best_.costs.data(), best_.trace.data()))
-    return nullptr;
+  if (FetchTrajectory(winner, horizon_, &best_)) return nullptr;
   best_.total_return = returns_[winner];
   best_.failure = failure_[winner];
   return &best_;
@@ -256,7 +230,7 @@ int mjpc_b200_sg_planner_nominal_trajectory(void* p, int horizon) {
   return ((SampleGradientPlanner*)p)->NominalTrajectory(horizon);
 }
 void mjpc_b200_sg_planner_action_from_policy(void* p, double* action, double time, int use_previous) {
-  ((SampleGradientPlanner*)p)->ActionFromPolicy(action, time, use_previous != 0);
+  ((SampleGradientPlanner*)p)->ActionFromPolicy(action, nullptr, time, use_previous != 0);
 }
 int mjpc_b200_sg_planner_get_result(void* pv, int* winner, int* winner_type, double* improvement, float* returns,
                                     int* order, double* knots, double* knot_times, double* gradient_knots,
@@ -269,19 +243,14 @@ int mjpc_b200_sg_planner_get_result(void* pv, int* winner, int* winner_type, dou
   if (returns) std::copy(p->returns().begin(), p->returns().end(), returns);
   if (order) std::copy(p->trajectory_order.begin(), p->trajectory_order.end(), order);
   if (gradient) std::copy(p->gradient.begin(), p->gradient.end(), gradient);
-  const auto& plan = p->policy.plan;
-  const int P = p->policy.num_spline_points, nu = plan.Dim();
-  for (int k = 0; k < plan.Size(); k++) {
-    if (knot_times) knot_times[k] = plan.NodeTime(k);
-    if (knots) std::copy(plan.NodeValues(k), plan.NodeValues(k) + nu, knots + (size_t)k * nu);
-  }
+  const int P = p->policy.num_spline_points, nu = p->policy.plan.Dim();
   for (int j = 0; gradient_knots && j < G; j++) {
     const auto& gp = p->candidate_policy[N - G + j].plan;
     std::fill(gradient_knots + (size_t)j * P * nu, gradient_knots + (size_t)(j + 1) * P * nu, 0.0);
     for (int k = 0; k < std::min(gp.Size(), P); k++)
       std::copy(gp.NodeValues(k), gp.NodeValues(k) + nu, gradient_knots + ((size_t)j * P + k) * nu);
   }
-  return plan.Size();
+  return p->policy.plan.Export(knots, knot_times);
 }
 
 }  // extern "C"

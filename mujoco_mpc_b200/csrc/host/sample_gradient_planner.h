@@ -13,28 +13,27 @@
 
 namespace mjpc_b200_host {
 
-class SampleGradientPlanner {
+class SampleGradientPlanner : public Planner {
  public:
   enum WinnerType : int { kNominal = 0, kPerturb = 1, kGradient = 2 };
   static constexpr double gradient_max_step_size = 2.0;    // planner.h
   static constexpr double gradient_min_step_size = 1.0e-3;
 
-  ~SampleGradientPlanner();
   // settings the reference reads from <custom> numerics (planner.cc:57-69): sampling_trajectories (N),
   // sampling_exploration, sampling_representation, sample_gradient_trajectories (G), sample_gradient_filter
   int Initialize(const mjpc_model_blob* model, int num_trajectory, int num_gradient, int num_spline_points,
                  int interpolation, double exploration, double gradient_filter, double timestep,
                  const double* ctrlrange, uint32_t seed, int max_horizon, int device);
-  void Reset(int horizon, const double* initial_repeated_action);   // :121-160
-  void SetState(const double* state, double time, const double* mocap);
-  int OptimizePolicy(int horizon);                                  // :169-273
-  int NominalTrajectory(int horizon);                               // :276-287
-  void ActionFromPolicy(double* action, double time, bool use_previous = false);   // :290-299
+  void Reset(int horizon, const double* initial_repeated_action) override;   // :121-160
+  int OptimizePolicy(int horizon) override;                         // :169-273
+  int NominalTrajectory(int horizon) override;                      // :276-287
+  // :290-299; the policy does not depend on the state
+  void ActionFromPolicy(double* action, const double* state, double time, bool use_previous = false) override;
   void ResamplePolicy(SamplingPolicy& p, int horizon, int num_spline_points);     // :302-326
   void AddNoiseToPolicy(int i);                                     // :329-355
   int Rollouts(int num_trajectory, int num_gradient, int horizon);  // :358-398
   void GradientCandidates(int num_trajectory, int num_gradient);    // :401-493
-  const Trajectory* BestTrajectory();                               // trajectory[winner] (:496-498)
+  const Trajectory* BestTrajectory() override;                      // trajectory[winner] (:496-498)
 
   SamplingPolicy policy, resampled_policy, previous_policy;
   std::vector<SamplingPolicy> candidate_policy;
@@ -46,17 +45,13 @@ class SampleGradientPlanner {
   int num_trajectory() const { return num_trajectory_; }
   int num_gradient() const { return num_gradient_; }
   const std::vector<float>& returns() const { return returns_; }
-  mjpc_b200_t* gpu() { return gpu_; }
 
  private:
-  mjpc_b200_t* gpu_ = nullptr;
-  mjpc_b200_info info_{};
   int num_trajectory_ = 10, num_gradient_ = 0, nu_ = 0;
   SplineInterpolation interpolation_ = kCubicSpline;
   double noise_exploration_ = 0.1, gradient_filter_ = 1.0, timestep_ = 0.01;
   uint32_t seed_ = 0x5EED;
-  std::vector<double> state_, mocap_, knot_times_;
-  double time_ = 0;
+  std::vector<double> knot_times_;
   std::vector<double> return_weight_, step_size_;   // cached on size, as in the reference; Reset keeps them
   std::vector<float> knots_, returns_;
   std::vector<uint8_t> failure_;

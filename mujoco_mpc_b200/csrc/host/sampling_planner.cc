@@ -48,6 +48,14 @@ void TimeSpline::Sample(double time, double* out) const {
   }
 }
 
+int TimeSpline::Export(double* values, double* times) const {
+  for (int k = 0; k < Size(); k++) {
+    if (times) times[k] = times_[k];
+    if (values) std::copy(NodeValues(k), NodeValues(k) + dim_, values + (size_t)k * dim_);
+  }
+  return Size();
+}
+
 void SamplingPolicy::Action(double* action, double time) const {
   plan.Sample(time, action);
   for (int i = 0; i < plan.Dim(); i++) action[i] = std::max(ctrlrange[2 * i], std::min(ctrlrange[2 * i + 1], action[i]));
@@ -80,20 +88,10 @@ void LogScale(double* values, double max_value, double min_value, int steps) {
 }
 
 // ------------------------------------------------------------------------------------------ SamplingPlanner
-SamplingPlanner::~SamplingPlanner() {
-  if (gpu_ && owns_gpu_) mjpc_b200_destroy(gpu_);
-}
-
 int SamplingPlanner::Initialize(const mjpc_model_blob* model, int num_trajectory, int num_spline_points, int interpolation,
                                 double exploration, double exploration2, double timestep, const double* ctrlrange,
                                 uint32_t seed, int max_candidates, int max_horizon, int device, mjpc_b200_t* engine) {
-  owns_gpu_ = engine == nullptr;
-  if (engine) {
-    gpu_ = engine;
-  } else if (int rc = mjpc_b200_create(model, max_candidates, max_horizon, device, &gpu_)) {
-    return rc;
-  }
-  mjpc_b200_get_info(gpu_, &info_);
+  if (int rc = AttachEngine(model, max_candidates, max_horizon, device, engine)) return rc;
   nu_ = info_.nu;
   num_trajectory_ = num_trajectory;
   interpolation_ = (SplineInterpolation)interpolation;
@@ -104,7 +102,6 @@ int SamplingPlanner::Initialize(const mjpc_model_blob* model, int num_trajectory
   policy.ctrlrange.assign(ctrlrange, ctrlrange + 2 * nu_);
   previous_policy = policy;
   candidate_policy.assign(max_candidates, policy);
-  state_.assign(info_.dim_state, 0.0); mocap_.assign(7 * info_.nmocap, 0.0);
   returns_.assign(max_candidates, 0.f); failure_.assign(max_candidates, 0);
   winner = 0;
   return 0;
@@ -116,12 +113,6 @@ void SamplingPlanner::Reset(int, const double* initial_repeated_action) {
   previous_policy = policy;
   for (auto& cp : candidate_policy) cp = policy;
   winner = 0; iteration = 0; improvement = 0;
-}
-
-void SamplingPlanner::SetState(const double* state, double time, const double* mocap) {
-  std::copy(state, state + state_.size(), state_.begin());
-  if (!mocap_.empty()) std::copy(mocap, mocap + mocap_.size(), mocap_.begin());
-  time_ = time;
 }
 
 void SamplingPlanner::UpdateNominalPolicy(int horizon) {
@@ -181,12 +172,12 @@ int SamplingPlanner::PrepareCandidates(int num_trajectory, float* knots, double*
   return P;
 }
 
-void SamplingPlanner::InstallRollouts(int num_trajectory, const float* returns, const uint8_t* failure, const int* order,
-                                      int offset) {
+void SamplingPlanner::InstallRollouts(int num_trajectory, int horizon, const float* returns, const uint8_t* failure,
+                                      const int* order, int offset) {
   std::copy(returns, returns + num_trajectory, returns_.begin());
   std::copy(failure, failure + num_trajectory, failure_.begin());
   trajectory_order.assign(order, order + num_trajectory);
-  offset_ = offset;
+  offset_ = offset; horizon_ = horizon;
 }
 
 int SamplingPlanner::Rollouts(int num_trajectory, int horizon) {
@@ -194,12 +185,10 @@ int SamplingPlanner::Rollouts(int num_trajectory, int horizon) {
   knots_.resize((size_t)num_trajectory * P * nu_);
   knot_times_.resize(P);
   PrepareCandidates(num_trajectory, knots_.data(), knot_times_.data());
-  std::vector<float> state_f(state_.begin(), state_.end()), mocap_f(mocap_.begin(), mocap_.end());
   trajectory_order.resize(num_trajectory);
   offset_ = 0;
-  return mjpc_b200_rollout_spline(gpu_, state_f.data(), time_, mocap_f.empty() ? nullptr : mocap_f.data(), nullptr,
-                                  knots_.data(), knot_times_.data(), (int)interpolation_, P, num_trajectory, horizon,
-                                  returns_.data(), failure_.data(), trajectory_order.data());
+  return RolloutSpline(knots_.data(), knot_times_.data(), (int)interpolation_, P, num_trajectory, horizon,
+                       returns_.data(), failure_.data(), trajectory_order.data());
 }
 
 int SamplingPlanner::OptimizePolicyCandidates(int ncandidates, int horizon) {
@@ -217,6 +206,11 @@ int SamplingPlanner::OptimizePolicy(int horizon) {
   return 0;
 }
 
+int SamplingPlanner::NominalTrajectory(int horizon) {
+  UpdateNominalPolicy(horizon);
+  return Rollouts(1, horizon);
+}
+
 void SamplingPlanner::InstallBest() {
   CopyCandidateToPolicy(0);
   const double best_return = returns_[0];   // candidate 0 is the un-noised nominal
@@ -231,21 +225,13 @@ void SamplingPlanner::CopyCandidateToPolicy(int candidate) {
   policy = candidate_policy[winner];
 }
 
-void SamplingPlanner::ActionFromPolicy(double* action, double time, bool use_previous) {
+void SamplingPlanner::ActionFromPolicy(double* action, const double*, double time, bool use_previous) {
   const std::shared_lock<std::shared_mutex> lock(mtx_);
   (use_previous ? previous_policy : policy).Action(action, time);
 }
 
-int SamplingPlanner::FetchTrajectory(int candidate, int horizon, Trajectory* t) {
-  const mjpc_b200_info& in = info_;
-  const size_t H = horizon;
-  t->horizon = horizon; t->dim_state = in.dim_state; t->dim_action = in.nu; t->dim_residual = in.num_residual;
-  t->dim_trace = 3 * in.num_trace;
-  t->states.resize(H * in.dim_state); t->actions.resize(H * in.nu); t->times.resize(H);
-  t->residual.resize(H * in.num_residual); t->costs.resize(H); t->trace.resize(H * t->dim_trace);
-  if (mjpc_b200_fetch_trajectory(gpu_, offset_ + candidate, t->states.data(), t->actions.data(), t->times.data(), t->residual.data(),
-                                 t->costs.data(), t->trace.data()))
-    return -1;
+int SamplingPlanner::CandidateTrajectory(int candidate, int horizon, Trajectory* t) {
+  if (FetchTrajectory(offset_ + candidate, horizon, t)) return -1;
   t->total_return = returns_[candidate];
   t->failure = failure_[candidate];
   return 0;
@@ -258,18 +244,7 @@ void SamplingPlanner::SetPolicy(const double* times, const double* parameters, i
 }
 
 const Trajectory* SamplingPlanner::BestTrajectory() {
-  mjpc_b200_info& in = info_;
-  const int H = in.max_horizon;
-  best_.dim_state = in.dim_state; best_.dim_action = in.nu; best_.dim_residual = in.num_residual;
-  best_.dim_trace = 3 * in.num_trace;
-  best_.states.resize((size_t)H * in.dim_state); best_.actions.resize((size_t)H * in.nu); best_.times.resize(H);
-  best_.residual.resize((size_t)H * in.num_residual); best_.costs.resize(H); best_.trace.resize((size_t)H * best_.dim_trace);
-  if (mjpc_b200_fetch_trajectory(gpu_, offset_ + winner, best_.states.data(), best_.actions.data(), best_.times.data(),
-                                 best_.residual.data(), best_.costs.data(), best_.trace.data()))
-    return nullptr;
-  best_.total_return = returns_[winner];
-  best_.failure = failure_[winner];
-  return &best_;
+  return CandidateTrajectory(winner, horizon_, &best_) ? nullptr : &best_;
 }
 
 }  // namespace mjpc_b200_host
@@ -315,7 +290,7 @@ void mjpc_b200_planner_set_state(void* p, const double* state, double time, cons
 }
 int mjpc_b200_planner_optimize_policy(void* p, int horizon) { return ((SamplingPlanner*)p)->OptimizePolicy(horizon); }
 void mjpc_b200_planner_action_from_policy(void* p, double* action, double time, int use_previous) {
-  ((SamplingPlanner*)p)->ActionFromPolicy(action, time, use_previous != 0);
+  ((SamplingPlanner*)p)->ActionFromPolicy(action, nullptr, time, use_previous != 0);
 }
 // winner index, improvement, returns [num_trajectory], policy knots [P][nu] and times [P] of the installed policy
 int mjpc_b200_planner_get_result(void* pv, int* winner, double* improvement, float* returns, double* knots, double* knot_times) {
@@ -323,12 +298,7 @@ int mjpc_b200_planner_get_result(void* pv, int* winner, double* improvement, flo
   if (winner) *winner = p->winner;
   if (improvement) *improvement = p->improvement;
   if (returns) std::copy(p->returns().begin(), p->returns().end(), returns);
-  const auto& plan = p->policy.plan;
-  for (int k = 0; k < plan.Size(); k++) {
-    if (knot_times) knot_times[k] = plan.NodeTime(k);
-    if (knots) std::copy(plan.NodeValues(k), plan.NodeValues(k) + plan.Dim(), knots + (size_t)k * plan.Dim());
-  }
-  return plan.Size();
+  return p->policy.plan.Export(knots, knot_times);
 }
 
 }  // extern "C"

@@ -137,12 +137,47 @@ class EngineError(RuntimeError):
     pass
 
 
+def _model_blob(model):
+    """The model's blob in a ctypes buffer and the ModelBlob that points at it: keep the buffer while C reads it."""
+    blob = to_blob(model)
+    buf = C.create_string_buffer(blob, len(blob))
+    return buf, ModelBlob(C.cast(buf, C.c_void_p), len(blob))
+
+
+class _CppObject:
+    """A C++ host object behind its `<prefix>_*` entry points: created from the model blob, destroyed by close()."""
+
+    def _create(self, prefix, model, *args):
+        self.lib = load_library()
+        self.m = model
+        self._prefix = prefix
+        self._buf, mb = _model_blob(model)
+        h = C.c_void_p()
+        rc = getattr(self.lib, f"{prefix}_create")(C.byref(mb), *args, C.byref(h))
+        if rc != 0:
+            raise EngineError(f"{prefix}_create failed ({rc}): {self.lib.mjpc_b200_last_error().decode()}")
+        self.h = h
+
+    def close(self):
+        if getattr(self, "h", None):
+            getattr(self.lib, f"{self._prefix}_destroy")(self.h)
+            self.h = None
+
+    __del__ = close
+
+    def reset(self, initial_repeated_action=None):
+        a = _d(initial_repeated_action)
+        getattr(self.lib, f"{self._prefix}_reset")(self.h, self.horizon, _pd(a))
+
+    def set_state(self, state, time, mocap):
+        s, mc = _d(state), _d(mocap)
+        getattr(self.lib, f"{self._prefix}_set_state")(self.h, _pd(s), C.c_double(time), _pd(mc))
+
+
 def host_ilqg_policy_action(model, u_nom, x_nom, t_nom, gains, representation, feedback_scaling, state, time):
     """iLQGPolicy::Action (ilqg/policy.cc:82-161) on the host through mjpc_b200_host_ilqg_policy_action (no device)."""
     lib = load_library()
-    blob = to_blob(model)
-    buf = C.create_string_buffer(blob, len(blob))
-    mb = ModelBlob(C.cast(buf, C.c_void_p), len(blob))
+    buf, mb = _model_blob(model)
     u, x, t, g = _f(u_nom), _f(x_nom), _d(t_nom), _f(gains)
     st = _d(state)
     out = np.zeros(model.nu)
@@ -175,9 +210,7 @@ class Engine:
     def __init__(self, model, max_candidates=256, max_horizon=64, device=0):
         self.lib = load_library()
         self.m = model
-        self._blob = to_blob(model)
-        self._buf = C.create_string_buffer(self._blob, len(self._blob))
-        mb = ModelBlob(C.cast(self._buf, C.c_void_p), len(self._blob))
+        self._buf, mb = _model_blob(model)
         h = C.c_void_p()
         rc = self.lib.mjpc_b200_create(C.byref(mb), int(max_candidates), int(max_horizon), int(device), C.byref(h))
         if rc != 0:
@@ -498,45 +531,20 @@ class Engine:
         return int(self.lib.mjpc_b200_last_kernel_static(self.h))
 
 
-class CppSamplingPlanner:
+class CppSamplingPlanner(_CppObject):
     """The C++ host planner (csrc/host/sampling_planner.cc) through its C wrappers."""
 
     def __init__(self, model, num_trajectory, horizon, seed=0x5EED, device=0):
-        self.lib = load_library()
-        m = self.m = model
-        self._blob = to_blob(model)
-        self._buf = C.create_string_buffer(self._blob, len(self._blob))
-        mb = ModelBlob(C.cast(self._buf, C.c_void_p), len(self._blob))
-        num = m.numeric
+        m, num = model, model.numeric
         self.P = int(num.get("sampling_spline_points", [3])[0])
         self.horizon, self.N, self.nu = int(horizon), int(num_trajectory), m.nu
         cr = _d(np.asarray(m.actuator_ctrlrange, float).reshape(-1))
-        h = C.c_void_p()
-        rc = self.lib.mjpc_b200_planner_create(C.byref(mb), self.N, self.P, int(num.get("sampling_representation", [2])[0]),
-                                               C.c_double(float(num.get("sampling_exploration", [0.1])[0])),
-                                               C.c_double(float(m.opt_timestep)), _pd(cr), C.c_uint32(seed), self.horizon,
-                                               int(device), C.byref(h))
-        if rc != 0:
-            raise EngineError(f"mjpc_b200_planner_create failed ({rc}): {self.lib.mjpc_b200_last_error().decode()}")
-        self.h = h
-
-    def close(self):
-        if getattr(self, "h", None):
-            self.lib.mjpc_b200_planner_destroy(self.h)
-            self.h = None
-
-    __del__ = close
+        self._create("mjpc_b200_planner", m, self.N, self.P, int(num.get("sampling_representation", [2])[0]),
+                     C.c_double(float(num.get("sampling_exploration", [0.1])[0])), C.c_double(float(m.opt_timestep)),
+                     _pd(cr), C.c_uint32(seed), self.horizon, int(device))
 
     def set_exploration(self, exploration, exploration2=0.0):
         self.lib.mjpc_b200_planner_set_exploration(self.h, C.c_double(exploration), C.c_double(exploration2))
-
-    def reset(self, initial_repeated_action=None):
-        a = _d(initial_repeated_action)
-        self.lib.mjpc_b200_planner_reset(self.h, self.horizon, _pd(a))
-
-    def set_state(self, state, time, mocap):
-        s, mc = _d(state), _d(mocap)
-        self.lib.mjpc_b200_planner_set_state(self.h, _pd(s), C.c_double(time), _pd(mc))
 
     def optimize_policy(self):
         rc = self.lib.mjpc_b200_planner_optimize_policy(self.h, self.horizon)
@@ -556,38 +564,19 @@ class CppSamplingPlanner:
         return a
 
 
-class CppBatchSamplingPlanner:
+class CppBatchSamplingPlanner(_CppObject):
     """num_problems independent Predictive Sampling problems planned with one rollout launch per iteration
     (csrc/host/batch_sampling_planner.cc); each method that concerns one problem takes its index."""
 
     def __init__(self, model, num_problems, num_trajectory, horizon, seeds=None, device=0):
-        self.lib = load_library()
-        m = self.m = model
-        self._blob = to_blob(model)
-        self._buf = C.create_string_buffer(self._blob, len(self._blob))
-        mb = ModelBlob(C.cast(self._buf, C.c_void_p), len(self._blob))
-        num = m.numeric
+        m, num = model, model.numeric
         self.P = int(num.get("sampling_spline_points", [3])[0])
         self.B, self.horizon, self.N, self.nu = int(num_problems), int(horizon), int(num_trajectory), m.nu
         sd = np.ascontiguousarray([0x5EED + b for b in range(self.B)] if seeds is None else seeds, np.uint32)
         cr = _d(np.asarray(m.actuator_ctrlrange, float).reshape(-1))
-        h = C.c_void_p()
-        rc = self.lib.mjpc_b200_batch_planner_create(C.byref(mb), self.B, self.N, self.P,
-                                                     int(num.get("sampling_representation", [2])[0]),
-                                                     C.c_double(float(num.get("sampling_exploration", [0.1])[0])),
-                                                     C.c_double(float(m.opt_timestep)), _pd(cr),
-                                                     sd.ctypes.data_as(C.POINTER(C.c_uint32)), self.horizon, int(device),
-                                                     C.byref(h))
-        if rc != 0:
-            raise EngineError(f"mjpc_b200_batch_planner_create failed ({rc}): {self.lib.mjpc_b200_last_error().decode()}")
-        self.h = h
-
-    def close(self):
-        if getattr(self, "h", None):
-            self.lib.mjpc_b200_batch_planner_destroy(self.h)
-            self.h = None
-
-    __del__ = close
+        self._create("mjpc_b200_batch_planner", m, self.B, self.N, self.P, int(num.get("sampling_representation", [2])[0]),
+                     C.c_double(float(num.get("sampling_exploration", [0.1])[0])), C.c_double(float(m.opt_timestep)),
+                     _pd(cr), sd.ctypes.data_as(C.POINTER(C.c_uint32)), self.horizon, int(device))
 
     def _check(self, rc, what):
         if rc < 0:
@@ -626,43 +615,19 @@ class CppBatchSamplingPlanner:
         return a
 
 
-class CppCrossEntropyPlanner:
+class CppCrossEntropyPlanner(_CppObject):
     """The C++ Cross-Entropy planner (csrc/host/cross_entropy_planner.cc) through its C wrappers."""
 
     def __init__(self, model, num_trajectory, horizon, n_elite=0, seed=0x5EED, device=0):
-        self.lib = load_library()
-        m = self.m = model
-        self._blob = to_blob(model)
-        self._buf = C.create_string_buffer(self._blob, len(self._blob))
-        mb = ModelBlob(C.cast(self._buf, C.c_void_p), len(self._blob))
-        num = m.numeric
+        m, num = model, model.numeric
         self.P = int(num.get("sampling_spline_points", [3])[0])
         self.horizon, self.N, self.nu = int(horizon), int(num_trajectory), m.nu
         cr = _d(np.asarray(m.actuator_ctrlrange, float).reshape(-1))
-        h = C.c_void_p()
-        rc = self.lib.mjpc_b200_ce_planner_create(
-            C.byref(mb), self.N, int(n_elite), self.P, int(num.get("sampling_representation", [2])[0]),
+        self._create(
+            "mjpc_b200_ce_planner", m, self.N, int(n_elite), self.P, int(num.get("sampling_representation", [2])[0]),
             C.c_double(float(num.get("sampling_exploration", [0.1])[0])), C.c_double(float(num.get("std_min", [0.01])[0])),
             C.c_double(float(num.get("explore_fraction", [0.0])[0])), C.c_double(float(m.opt_timestep)), _pd(cr),
-            C.c_uint32(seed), self.horizon, int(device), C.byref(h))
-        if rc != 0:
-            raise EngineError(f"mjpc_b200_ce_planner_create failed ({rc}): {self.lib.mjpc_b200_last_error().decode()}")
-        self.h = h
-
-    def close(self):
-        if getattr(self, "h", None):
-            self.lib.mjpc_b200_ce_planner_destroy(self.h)
-            self.h = None
-
-    __del__ = close
-
-    def reset(self, initial_repeated_action=None):
-        a = _d(initial_repeated_action)
-        self.lib.mjpc_b200_ce_planner_reset(self.h, self.horizon, _pd(a))
-
-    def set_state(self, state, time, mocap):
-        s, mc = _d(state), _d(mocap)
-        self.lib.mjpc_b200_ce_planner_set_state(self.h, _pd(s), C.c_double(time), _pd(mc))
+            C.c_uint32(seed), self.horizon, int(device))
 
     def optimize_policy(self):
         rc = self.lib.mjpc_b200_ce_planner_optimize_policy(self.h, self.horizon)
@@ -684,45 +649,21 @@ class CppCrossEntropyPlanner:
         return a
 
 
-class CppSampleGradientPlanner:
+class CppSampleGradientPlanner(_CppObject):
     """The C++ Sample Gradient planner (csrc/host/sample_gradient_planner.cc) through its C wrappers."""
 
     def __init__(self, model, num_trajectory, horizon, num_gradient=None, gradient_filter=None, seed=0x5EED, device=0):
-        self.lib = load_library()
-        m = self.m = model
-        self._blob = to_blob(model)
-        self._buf = C.create_string_buffer(self._blob, len(self._blob))
-        mb = ModelBlob(C.cast(self._buf, C.c_void_p), len(self._blob))
-        num = m.numeric
+        m, num = model, model.numeric
         self.P = int(num.get("sampling_spline_points", [3])[0])
         self.horizon, self.N, self.nu = int(horizon), int(num_trajectory), m.nu
         G = int(num_gradient if num_gradient is not None else num.get("sample_gradient_trajectories", [0])[0])
         self.G = max(min(G, self.N - 1), 0)                  # the clamp OptimizePolicy applies
         f = float(gradient_filter if gradient_filter is not None else num.get("sample_gradient_filter", [1.0])[0])
         cr = _d(np.asarray(m.actuator_ctrlrange, float).reshape(-1))
-        h = C.c_void_p()
-        rc = self.lib.mjpc_b200_sg_planner_create(
-            C.byref(mb), self.N, G, self.P, int(num.get("sampling_representation", [2])[0]),
+        self._create(
+            "mjpc_b200_sg_planner", m, self.N, G, self.P, int(num.get("sampling_representation", [2])[0]),
             C.c_double(float(num.get("sampling_exploration", [0.1])[0])), C.c_double(f), C.c_double(float(m.opt_timestep)),
-            _pd(cr), C.c_uint32(seed), self.horizon, int(device), C.byref(h))
-        if rc != 0:
-            raise EngineError(f"mjpc_b200_sg_planner_create failed ({rc}): {self.lib.mjpc_b200_last_error().decode()}")
-        self.h = h
-
-    def close(self):
-        if getattr(self, "h", None):
-            self.lib.mjpc_b200_sg_planner_destroy(self.h)
-            self.h = None
-
-    __del__ = close
-
-    def reset(self, initial_repeated_action=None):
-        a = _d(initial_repeated_action)
-        self.lib.mjpc_b200_sg_planner_reset(self.h, self.horizon, _pd(a))
-
-    def set_state(self, state, time, mocap):
-        s, mc = _d(state), _d(mocap)
-        self.lib.mjpc_b200_sg_planner_set_state(self.h, _pd(s), C.c_double(time), _pd(mc))
+            _pd(cr), C.c_uint32(seed), self.horizon, int(device))
 
     def optimize_policy(self):
         rc = self.lib.mjpc_b200_sg_planner_optimize_policy(self.h, self.horizon)
@@ -752,38 +693,15 @@ class CppSampleGradientPlanner:
         return a
 
 
-class CppILQGPlanner:
+class CppILQGPlanner(_CppObject):
     """The C++ iLQG planner (csrc/host/ilqg_planner.cc) through its C wrappers."""
 
     def __init__(self, model, horizon, num_rollouts=10, representation=1, fd_tolerance=3e-4, device=0, fd_mode=1, derivative_skip=0):
-        self.lib = load_library()
-        m = self.m = model
-        self._blob = to_blob(model)
-        self._buf = C.create_string_buffer(self._blob, len(self._blob))
-        mb = ModelBlob(C.cast(self._buf, C.c_void_p), len(self._blob))
-        self.H, self.nu, self.ds = int(horizon), m.nu, m.nq + m.nv
-        h = C.c_void_p()
-        rc = self.lib.mjpc_b200_ilqg_planner_create(C.byref(mb), int(num_rollouts), int(representation),
-                                                    C.c_double(fd_tolerance), self.H, int(device), C.byref(h))
-        if rc != 0:
-            raise EngineError(f"mjpc_b200_ilqg_planner_create failed ({rc}): {self.lib.mjpc_b200_last_error().decode()}")
-        self.h = h
+        self.H = self.horizon = int(horizon)
+        self.nu, self.ds = model.nu, model.nq + model.nv
+        self._create("mjpc_b200_ilqg_planner", model, int(num_rollouts), int(representation), C.c_double(fd_tolerance),
+                     self.H, int(device))
         self.lib.mjpc_b200_ilqg_planner_set_fd(self.h, C.c_double(fd_tolerance), int(fd_mode), int(derivative_skip))
-
-    def close(self):
-        if getattr(self, "h", None):
-            self.lib.mjpc_b200_ilqg_planner_destroy(self.h)
-            self.h = None
-
-    __del__ = close
-
-    def reset(self, initial_repeated_action=None):
-        a = _d(initial_repeated_action)
-        self.lib.mjpc_b200_ilqg_planner_reset(self.h, self.H, _pd(a))
-
-    def set_state(self, state, time, mocap):
-        s, mc = _d(state), _d(mocap)
-        self.lib.mjpc_b200_ilqg_planner_set_state(self.h, _pd(s), C.c_double(time), _pd(mc))
 
     def nominal_trajectory(self):
         return self.lib.mjpc_b200_ilqg_planner_nominal_trajectory(self.h, self.H)
@@ -808,32 +726,16 @@ class CppILQGPlanner:
         return a
 
 
-class CppBatchILQGPlanner:
+class CppBatchILQGPlanner(_CppObject):
     """The batched C++ iLQG planner (csrc/host/batch_ilqg_planner.cc): B problems, one launch per sweep.  Mirrors
     CppILQGPlanner with a problem argument."""
 
     def __init__(self, model, num_problems, horizon, num_rollouts=10, representation=1, fd_tolerance=3e-4, device=0,
                  fd_mode=1, derivative_skip=0):
-        self.lib = load_library()
-        m = self.m = model
-        self._blob = to_blob(model)
-        self._buf = C.create_string_buffer(self._blob, len(self._blob))
-        mb = ModelBlob(C.cast(self._buf, C.c_void_p), len(self._blob))
-        self.B, self.H, self.nu, self.ds = int(num_problems), int(horizon), m.nu, m.nq + m.nv
-        h = C.c_void_p()
-        rc = self.lib.mjpc_b200_batch_ilqg_planner_create(C.byref(mb), self.B, int(num_rollouts), int(representation),
-                                                          C.c_double(fd_tolerance), self.H, int(device), C.byref(h))
-        if rc != 0:
-            raise EngineError(f"mjpc_b200_batch_ilqg_planner_create failed ({rc}): {self.lib.mjpc_b200_last_error().decode()}")
-        self.h = h
+        self.B, self.H, self.nu, self.ds = int(num_problems), int(horizon), model.nu, model.nq + model.nv
+        self._create("mjpc_b200_batch_ilqg_planner", model, self.B, int(num_rollouts), int(representation),
+                     C.c_double(fd_tolerance), self.H, int(device))
         self.lib.mjpc_b200_batch_ilqg_planner_set_fd(self.h, C.c_double(fd_tolerance), int(fd_mode), int(derivative_skip))
-
-    def close(self):
-        if getattr(self, "h", None):
-            self.lib.mjpc_b200_batch_ilqg_planner_destroy(self.h)
-            self.h = None
-
-    __del__ = close
 
     def _check(self, rc, what):
         if rc < 0:
@@ -879,45 +781,21 @@ class CppBatchILQGPlanner:
         return a
 
 
-class CppRobustPlanner:
+class CppRobustPlanner(_CppObject):
     """The C++ Robust planner (csrc/host/robust_planner.cc) through its C wrappers."""
 
     def __init__(self, model, num_trajectory, horizon, ncandidates=-1, nrepetitions=5, xfrc_std=0.1, xfrc_rate=0.1,
                  seed=0x5EED, device=0):
-        self.lib = load_library()
-        m = self.m = model
-        self._blob = to_blob(model)
-        self._buf = C.create_string_buffer(self._blob, len(self._blob))
-        mb = ModelBlob(C.cast(self._buf, C.c_void_p), len(self._blob))
-        num = m.numeric
+        m, num = model, model.numeric
         self.P = int(num.get("sampling_spline_points", [3])[0])
         self.horizon, self.N, self.nu = int(horizon), int(num_trajectory), m.nu
         self.nc = int(ncandidates if ncandidates != -1 else num_trajectory // nrepetitions)
         cr = _d(np.asarray(m.actuator_ctrlrange, float).reshape(-1))
-        h = C.c_void_p()
-        rc = self.lib.mjpc_b200_robust_planner_create(
-            C.byref(mb), self.N, self.P, int(num.get("sampling_representation", [2])[0]),
+        self._create(
+            "mjpc_b200_robust_planner", m, self.N, self.P, int(num.get("sampling_representation", [2])[0]),
             C.c_double(float(num.get("sampling_exploration", [0.1])[0])), C.c_double(float(m.opt_timestep)), _pd(cr),
             C.c_uint32(seed), int(ncandidates), int(nrepetitions), C.c_double(xfrc_std), C.c_double(xfrc_rate),
-            self.horizon, int(device), C.byref(h))
-        if rc != 0:
-            raise EngineError(f"mjpc_b200_robust_planner_create failed ({rc}): {self.lib.mjpc_b200_last_error().decode()}")
-        self.h = h
-
-    def close(self):
-        if getattr(self, "h", None):
-            self.lib.mjpc_b200_robust_planner_destroy(self.h)
-            self.h = None
-
-    __del__ = close
-
-    def reset(self, initial_repeated_action=None):
-        a = _d(initial_repeated_action)
-        self.lib.mjpc_b200_robust_planner_reset(self.h, self.horizon, _pd(a))
-
-    def set_state(self, state, time, mocap):
-        s, mc = _d(state), _d(mocap)
-        self.lib.mjpc_b200_robust_planner_set_state(self.h, _pd(s), C.c_double(time), _pd(mc))
+            self.horizon, int(device))
 
     def optimize_policy(self):
         rc = self.lib.mjpc_b200_robust_planner_optimize_policy(self.h, self.horizon)
@@ -947,40 +825,15 @@ def host_spline_mapping(representation, input_times, output_times):
     return W
 
 
-class CppGradientPlanner:
+class CppGradientPlanner(_CppObject):
     """The C++ GradientPlanner (csrc/host/gradient_planner.cc) through its C wrappers."""
 
     def __init__(self, model, horizon, num_trajectory=8, num_spline_points=5, representation=1, fd_tolerance=3e-4, device=0, fd_mode=1):
-        self.lib = load_library()
-        self.m = model
-        self._blob = to_blob(model)
-        self._buf = C.create_string_buffer(self._blob, len(self._blob))
-        mb = ModelBlob(C.cast(self._buf, C.c_void_p), len(self._blob))
         cr = _d(np.asarray(model.actuator_ctrlrange, float).reshape(-1))
         self.horizon, self.P, self.nu = int(horizon), int(num_spline_points), model.nu
-        h = C.c_void_p()
-        rc = self.lib.mjpc_b200_gradient_planner_create(C.byref(mb), int(num_trajectory), self.P, int(representation),
-                                                        C.c_double(fd_tolerance), C.c_double(float(model.opt_timestep)), _pd(cr),
-                                                        self.horizon, int(device), C.byref(h))
-        if rc != 0:
-            raise EngineError(f"gradient_planner_create failed ({rc}): {self.lib.mjpc_b200_last_error().decode()}")
-        self.h = h
+        self._create("mjpc_b200_gradient_planner", model, int(num_trajectory), self.P, int(representation),
+                     C.c_double(fd_tolerance), C.c_double(float(model.opt_timestep)), _pd(cr), self.horizon, int(device))
         self.lib.mjpc_b200_gradient_planner_set_fd(self.h, C.c_double(fd_tolerance), int(fd_mode), -1)
-
-    def close(self):
-        if getattr(self, "h", None):
-            self.lib.mjpc_b200_gradient_planner_destroy(self.h)
-            self.h = None
-
-    __del__ = close
-
-    def reset(self, initial_repeated_action=None):
-        a = _d(initial_repeated_action)
-        self.lib.mjpc_b200_gradient_planner_reset(self.h, self.horizon, _pd(a))
-
-    def set_state(self, state, time, mocap):
-        s, mc = _d(state), _d(mocap)
-        self.lib.mjpc_b200_gradient_planner_set_state(self.h, _pd(s), C.c_double(time), _pd(mc))
 
     def optimize_policy(self):
         rc = self.lib.mjpc_b200_gradient_planner_optimize_policy(self.h, self.horizon)
@@ -1000,44 +853,19 @@ class CppGradientPlanner:
         return a
 
 
-class CppILQSPlanner:
+class CppILQSPlanner(_CppObject):
     """The C++ iLQSPlanner (csrc/host/gradient_planner.cc) through its C wrappers."""
 
     def __init__(self, model, horizon, num_trajectory=8, num_rollouts=6, fd_tolerance=3e-4, seed=0x5EED, device=0, fd_mode=1):
-        self.lib = load_library()
-        m = self.m = model
-        self._blob = to_blob(model)
-        self._buf = C.create_string_buffer(self._blob, len(self._blob))
-        mb = ModelBlob(C.cast(self._buf, C.c_void_p), len(self._blob))
-        num = m.numeric
+        m, num = model, model.numeric
         cr = _d(np.asarray(m.actuator_ctrlrange, float).reshape(-1))
         self.horizon, self.nu = int(horizon), m.nu
-        h = C.c_void_p()
-        rc = self.lib.mjpc_b200_ilqs_planner_create(C.byref(mb), int(num_trajectory), int(num.get("sampling_spline_points", [3])[0]),
-                                                    int(num.get("sampling_representation", [2])[0]),
-                                                    C.c_double(float(num.get("sampling_exploration", [0.1])[0])),
-                                                    C.c_double(float(m.opt_timestep)), _pd(cr), C.c_uint32(seed), int(num_rollouts),
-                                                    int(num.get("ilqg_representation", [1])[0]), C.c_double(fd_tolerance),
-                                                    self.horizon, int(device), C.byref(h))
-        if rc != 0:
-            raise EngineError(f"ilqs_planner_create failed ({rc}): {self.lib.mjpc_b200_last_error().decode()}")
-        self.h = h
+        self._create("mjpc_b200_ilqs_planner", m, int(num_trajectory), int(num.get("sampling_spline_points", [3])[0]),
+                     int(num.get("sampling_representation", [2])[0]),
+                     C.c_double(float(num.get("sampling_exploration", [0.1])[0])), C.c_double(float(m.opt_timestep)),
+                     _pd(cr), C.c_uint32(seed), int(num_rollouts), int(num.get("ilqg_representation", [1])[0]),
+                     C.c_double(fd_tolerance), self.horizon, int(device))
         self.lib.mjpc_b200_ilqs_planner_set_fd(self.h, C.c_double(fd_tolerance), int(fd_mode), -1)
-
-    def close(self):
-        if getattr(self, "h", None):
-            self.lib.mjpc_b200_ilqs_planner_destroy(self.h)
-            self.h = None
-
-    __del__ = close
-
-    def reset(self, initial_repeated_action=None):
-        a = _d(initial_repeated_action)
-        self.lib.mjpc_b200_ilqs_planner_reset(self.h, self.horizon, _pd(a))
-
-    def set_state(self, state, time, mocap):
-        s, mc = _d(state), _d(mocap)
-        self.lib.mjpc_b200_ilqs_planner_set_state(self.h, _pd(s), C.c_double(time), _pd(mc))
 
     def set_exploration(self, sigma):
         self.lib.mjpc_b200_ilqs_planner_set_exploration(self.h, C.c_double(sigma))
@@ -1059,19 +887,14 @@ class CppILQSPlanner:
         return a
 
 
-class CppAgent:
+class CppAgent(_CppObject):
     """Agent::PlanIteration glue (csrc/host/agent.cc) through its C wrappers; settings mirror the task XML numerics."""
     PLANNERS = {"sampling": 0, "gradient": 1, "ilqg": 2, "ilqs": 3, "robust": 4, "cross_entropy": 5, "sample_gradient": 6}
 
     def __init__(self, model, planner="sampling", horizon=None, timestep=None, integrator=0, differentiable=-1, num_trajectory=None,
                  num_spline_points=None, representation=None, exploration=None, ilqg_num_rollouts=10, ilqg_representation=1,
                  fd_tolerance=3e-4, seed=0x5EED, device=0, num_gradient=None, gradient_filter=None):
-        self.lib = load_library()
-        m = self.m = model
-        num = m.numeric
-        self._blob = to_blob(model)
-        self._buf = C.create_string_buffer(self._blob, len(self._blob))
-        mb = ModelBlob(C.cast(self._buf, C.c_void_p), len(self._blob))
+        m, num = model, model.numeric
         g = lambda k, d: float(num.get(k, [d])[0])
         st = np.array([self.PLANNERS[planner] if isinstance(planner, str) else planner,
                        g("agent_horizon", 0.5) if horizon is None else horizon,
@@ -1086,18 +909,8 @@ class CppAgent:
                        g("sample_gradient_trajectories", 0) if num_gradient is None else num_gradient,
                        g("sample_gradient_filter", 1.0) if gradient_filter is None else gradient_filter], float)
         cr = _d(np.asarray(m.actuator_ctrlrange, float).reshape(-1))
-        h = C.c_void_p()
-        rc = self.lib.mjpc_b200_agent_create(C.byref(mb), _pd(st), _pd(cr), int(device), C.byref(h))
-        if rc != 0:
-            raise EngineError(f"agent_create failed ({rc}): {self.lib.mjpc_b200_last_error().decode()}")
-        self.h, self.nu = h, m.nu
-
-    def close(self):
-        if getattr(self, "h", None):
-            self.lib.mjpc_b200_agent_destroy(self.h)
-            self.h = None
-
-    __del__ = close
+        self._create("mjpc_b200_agent", m, _pd(st), _pd(cr), int(device))
+        self.nu = m.nu
 
     @property
     def steps(self):
@@ -1106,10 +919,6 @@ class CppAgent:
     def reset(self, initial_repeated_action=None):
         a = _d(initial_repeated_action)
         self.lib.mjpc_b200_agent_reset(self.h, _pd(a))
-
-    def set_state(self, state, time, mocap):
-        s, mc = _d(state), _d(mocap)
-        self.lib.mjpc_b200_agent_set_state(self.h, _pd(s), C.c_double(time), _pd(mc))
 
     def set_task(self, weight=None, parameters=None, task_state=None, risk=None):
         w, p, s = _d(weight), _d(parameters), _d(task_state)
