@@ -107,15 +107,29 @@ struct Ctx {
   unsigned* sync;        // HBM: this SM's record (32 words)
   int sync_slot;         // 0 / 1: which of the SM's two candidates this one is; -1: not paired
   int sync_mode;         // bit 0: meet at every time step, bit 1: also before every constraint solve
+  int wide_pending;      // helper-warp kernels: a posted phase has not been met yet (wide_settle)
 #ifdef MJPC_PHASE_TIMING
-  long long tph[8], tlast;   // profiling build only: SM cycles per pipeline phase
+  long long tph[9], tlast;   // profiling build only: SM cycles per pipeline phase (slots 0-7 are reported, 8 is "elsewhere")
 #endif
 };
-#ifdef MJPC_PHASE_TIMING
-#define PHASE(c, i) do { const long long t_ = clock64(); (c).tph[i] += t_ - (c).tlast; (c).tlast = t_; } while (0)
-#else
-#define PHASE(c, i) do { } while (0)
+// Profiling build (-DMJPC_PHASE_TIMING): PHASE_AT(c, map, i) adds the SM cycles since the previous timer call to slot i
+// when the build records timer mapping `map` (-DMJPC_PHASE_MAP=<map>, profiles/phase_times.py --map):
+//   0  pipeline phases: kinematics + com (+ CRB), collision, constraint rows, velocities + smooth forces + reference,
+//      solve (rest), Hessian assembly, Cholesky factor + solve, policy + residual + cost + Euler + output
+//   1  the Newton solve: J^T f + gradient + termination, M/J products, line search, step + constraint update, warm-start
+//      evaluations, Hessian (one warp: the assembly; helper warps: the post and the wait at the join), Cholesky factor +
+//      solve; slot 7 counts line-search evaluations (everything outside the solve is total - slots 0..6)
+//   2  the first fork of a task-warp CTA: kinematics + com, collision, constraint rows, the main warp's wait at join 1,
+//      reference + solve, the task warp's fork interval (CRB, velocities, smooth forces), -, the rest of the step
+#ifndef MJPC_PHASE_MAP
+#define MJPC_PHASE_MAP 0
 #endif
+#ifdef MJPC_PHASE_TIMING
+#define PHASE_AT(c, m, i) do { if (MJPC_PHASE_MAP == (m)) { const long long t_ = clock64(); (c).tph[i] += t_ - (c).tlast; (c).tlast = t_; } } while (0)
+#else
+#define PHASE_AT(c, m, i) do { } while (0)
+#endif
+#define PHASE(c, i) PHASE_AT(c, 0, i)
 // ---- model / state accessors.  Every device function is a template over a "spec" SP:
 //   DynSpec          sizes and offsets are read from the header copy in shared memory (any model)
 //   StaticSpec<K>    sizes and offsets are compile-time constants taken from a generated table K (spec_*.h):
@@ -182,8 +196,19 @@ struct StaticSpec {
 // are therefore spread over W warps of the same CTA: the main warp posts a command and its scalar context to a
 // mailbox, all W warps meet on a named barrier, run the phase with a stride of 32*W items, and meet again.  The
 // per-item arithmetic is unchanged, so results are bitwise those of the one-warp kernel.
+// The Newton Hessian assembly (WIDE_HESSIAN) runs on the helper warps alone while the main warp forms J^T f, the
+// gradient and the termination test (k_solve): the main warp posts without waiting (wide_post_async) and meets the
+// helpers again before the Cholesky factor (wide_join).
+//   named barriers: 1 = post (main arrives / helpers wait, 32*W), 3 = join (helpers arrive / main waits, 32*W),
+//   4 = between the helpers' own passes (32*(W-1)).  Post and join are separate barriers: a helper that has arrived at
+//   the join and goes on to wait for the next post must not be counted twice in one barrier generation.
 enum { WIDE_EXIT = 0, WIDE_HESSIAN = 1 };
-struct WideBox { int cmd, ncon, nlim, ndrow, nefc; int task_exit, task_warn; float task_cost; };
+struct WideBox {
+  int cmd, ncon, nlim, ndrow, nefc; int task_exit, task_warn; float task_cost;
+#ifdef MJPC_PHASE_TIMING
+  long long task_fork_cycles;   // timer mapping 2: the task warp's fork intervals, summed over the steps
+#endif
+};
 __device__ __forceinline__ WideBox& wide_box() { __shared__ WideBox box; return box; }
 template <class SP>
 __device__ __forceinline__ void wide_bar() {
@@ -194,6 +219,18 @@ __device__ __forceinline__ void wide_bar() {
 __device__ __forceinline__ void task_bar() { asm volatile("bar.sync 2, 64;" ::: "memory"); }
 // lane index / lane count of the trajectory's thread group
 template <class SP> __device__ __forceinline__ int wide_lane(const Ctx& c) { return SP::kWide > 1 ? (int)threadIdx.x : c.lane; }
+// The thread group a wide phase runs on: all W warps of the trajectory (kHelpers = false; W = 1: the warp itself), or
+// the W-1 helper warps alone (warps 1..W-1 of the CTA)
+template <class SP, bool kHelpers>
+struct WideGroup {
+  static constexpr int kWarps = kHelpers ? SP::kWide - 1 : SP::kWide;
+  static __device__ __forceinline__ int lane(const Ctx& c) { return kHelpers ? (int)threadIdx.x - 32 : wide_lane<SP>(c); }
+  static __device__ __forceinline__ void bar() {
+    if constexpr (!kHelpers) wide_bar<SP>();
+    else if constexpr (kWarps > 1) asm volatile("bar.sync 4, %0;" ::"n"(32 * kWarps) : "memory");
+    else __syncwarp();
+  }
+};
 // main warp: publish the command and the scalar context the phase reads, then release the helpers
 template <class SP>
 __device__ __forceinline__ void wide_post(const Ctx& c, int cmd) {
@@ -201,6 +238,27 @@ __device__ __forceinline__ void wide_post(const Ctx& c, int cmd) {
     WideBox& b = wide_box();
     if (c.lane == 0) { b.cmd = cmd; b.ncon = c.ncon; b.nlim = c.nlim; b.ndrow = c.ndrow; b.nefc = c.nefc; }
     wide_bar<SP>();
+  }
+}
+// ... the same without waiting for the helpers (bar.arrive: the mailbox writes are visible to them once they pass)
+template <class SP>
+__device__ __forceinline__ void wide_post_async(const Ctx& c, int cmd) {
+  static_assert(SP::kWide > 1, "a one-warp trajectory has no helpers to post to");
+  WideBox& b = wide_box();
+  if (c.lane == 0) { b.cmd = cmd; b.ncon = c.ncon; b.nlim = c.nlim; b.ndrow = c.ndrow; b.nefc = c.nefc; }
+  asm volatile("bar.arrive 1, %0;" ::"n"(32 * SP::kWide) : "memory");
+}
+// main warp: wait until the helpers have finished the posted phase; helpers: report it finished
+template <class SP>
+__device__ __forceinline__ void wide_join() { asm volatile("bar.sync 3, %0;" ::"n"(32 * SP::kWide) : "memory"); }
+template <class SP>
+__device__ __forceinline__ void wide_done() { asm volatile("bar.arrive 3, %0;" ::"n"(32 * SP::kWide) : "memory"); }
+// main warp: meet a phase that is still in flight (an assembly the solve no longer needs is left running while the step
+// ends; this is called before the next step touches what it reads or writes, and before the helpers are released)
+template <class SP>
+__device__ __forceinline__ void wide_settle(Ctx& c) {
+  if constexpr (SP::kWide > 1) {
+    if (c.wide_pending) { wide_join<SP>(); c.wide_pending = 0; }
   }
 }
 

@@ -1210,11 +1210,12 @@ __device__ __noinline__ float k_update_constraint(Ctx& c, bool hess) {
 // e = lane + 32 q (hpair tables, NQ per lane) and keeps them in registers; every active constraint row (weight
 // hw != 0) and every cone effective row is one rank-1 update read as a dense row from shared memory
 // (broadcast loads, no bank conflicts, no branches inside).
-template <class SP, int NV, int NQ>
+template <class SP, int NV, int NQ, bool kHelpers = false>
 __device__ __forceinline__ void hessian_dense_reg(Ctx& c) {
   auto&& M = SP::model(c);
-  const int lane = wide_lane<SP>(c);   // index within the trajectory's thread group (the warp, or W warps: dev_data.cuh)
-  constexpr int WN = 32 * SP::kWide;
+  using G = WideGroup<SP, kHelpers>;   // the thread group that assembles (the warp, all W warps, or the helpers: dev_data.cuh)
+  const int lane = G::lane(c);         // index within that group
+  constexpr int WN = 32 * G::kWarps;
   constexpr int NVP = (NV + 3) / 4 * 4;
   const float *qM = DF(qM), *hw = DF(efc_hw), *Jd = DF(efc_Jd), *Xd = DF(efc_Xd), *xw = DF(efc_hc);
   float* H = DF(qH);
@@ -1242,7 +1243,7 @@ __device__ __forceinline__ void hessian_dense_reg(Ctx& c) {
       }
       xwm[36 * ci + 14 + p] = v; xwm[36 * ci + 20 + p] = u;   // zeros for non-cone contacts: read (times 0) below
     }
-    wide_bar<SP>();
+    G::bar();
     // (straight-line: clamped indices, weights selected to zero instead of branches - every taken branch costs a
     // reconvergence (BSSY/BSYNC ~30 cycles) with a single resident warp)
     constexpr int kMaxRows = 10;   // pyramidal condim 6; elliptic contacts have <= 6 rows
@@ -1275,7 +1276,7 @@ __device__ __forceinline__ void hessian_dense_reg(Ctx& c) {
       acc += (on && state[a0] == STATE_CONE) ? tc : 0.f;
       if (base + lane < nwork) Wc[w] = acc;
     }
-    wide_bar<SP>();
+    G::bar();
     // g_i = (sum of W_c over the contacts on bodies in the subtree of dof i's body) cdof_i, one (dof, component) per lane
     const int *subend = MI(body_subtreeend), *cmb = DI(con_mbody), *dbody = MI(dof_bodyid);
     const float* cdof = DF(cdof);
@@ -1299,7 +1300,7 @@ __device__ __forceinline__ void hessian_dense_reg(Ctx& c) {
       }
       g[w] = a;
     }
-    wide_bar<SP>();
+    G::bar();
   }
 #ifdef MJPC_HESS_ROLLED
   // experiment (code footprint): one rolled loop over the pattern entries, H written directly, the rare rank-1 rows
@@ -1307,7 +1308,7 @@ __device__ __forceinline__ void hessian_dense_reg(Ctx& c) {
   if (NE != NV * (NV + 1) / 2) {   // entries outside the pattern (the dense factor reads them); nothing to clear for a full pattern
     MJPC_ROLL
     for (int w = lane; w < NV * NV; w += WN) H[w] = 0.f;
-    wide_bar<SP>();
+    G::bar();
   }
   {
     const float* cdof = DF(cdof);
@@ -1352,7 +1353,7 @@ __device__ __forceinline__ void hessian_dense_reg(Ctx& c) {
       if (e0 + lane < NE) { H[r * NV + sdof] = a; H[sdof * NV + r] = a; }
     }
   }
-  wide_bar<SP>();
+  G::bar();
 }
 #else
   int er[NQ], es[NQ];
@@ -1534,18 +1535,22 @@ __device__ __noinline__ float k_total_cost(Ctx& c, const float* qacc, bool hess,
 // Newton Hessian H = M + J^T diag(hw) J + cone blocks at the point last evaluated by k_total_cost(.., hess=true)
 // (which leaves the row weights hw and the per-cone coefficients in efc_hc).  Kept apart from the cost evaluation
 // so that the solver only assembles and factorises H when another iteration is actually taken.
-// ONE out-of-line copy of the static-spec assembly: the main warp (k_hessian) and the helper warps (wide_helper_loop)
-// execute the very same instructions, so which warp computes an entry cannot change its value.
+// ONE out-of-line copy of the static-spec assembly per kernel: the one-warp kernel runs it on its warp (k_hessian), the
+// helper-warp kernel on its helper warps alone (wide_helper_loop) while the main warp forms the gradient (k_solve).
+// Every work item is computed by one thread in a fixed order whatever the group's size, so the values are the same.
 template <class SP>
 __device__ __noinline__ void hessian_static(Ctx& c) {
-  hessian_dense_reg<SP, SP::kNV, (SP::kNHPair + 31) / 32>(c);
+  hessian_dense_reg<SP, SP::kNV, (SP::kNHPair + 31) / 32, (SP::kWide > 1)>(c);
 }
 
+// The main warp's part of the assembly: the effective rows of cone contacts that the dense rank-1 pass reads (only
+// present with contacts between two moving bodies / tendon limits on the register-blocked path).  Reads efc_J, efc_hc
+// [36 ci + 0 .. 13], efc_state, con_*; writes efc_W, efc_Xd.
 template <class SP>
-__device__ __noinline__ void k_hessian(Ctx& c) {
+__device__ __forceinline__ void hessian_cone_rows(Ctx& c) {
   auto&& M = SP::model(c);
   const int lane = c.lane, nv = M.nv;
-  const float *qM = DF(qM), *J = DF(efc_J);
+  const float* J = DF(efc_J);
   float *X = DF(efc_W);
   const int *state = DI(efc_state), *cdim = DI(con_dim);
   const float* xw = DF(efc_hc);
@@ -1585,8 +1590,16 @@ __device__ __noinline__ void k_hessian(Ctx& c) {
     }
     __syncwarp();
   }
+}
+
+template <class SP>
+__device__ __noinline__ void k_hessian(Ctx& c) {
+  auto&& M = SP::model(c);
+  const int lane = c.lane, nv = M.nv;
+  const float *qM = DF(qM), *J = DF(efc_J);
+  hessian_cone_rows<SP>(c);
   if constexpr (SP::kNV > 0) {
-    wide_post<SP>(c, WIDE_HESSIAN);   // helper warps (if the kernel has them) join for the assembly
+    static_assert(SP::kWide == 1, "helper-warp kernels assemble on the helpers (k_solve)");
     hessian_static<SP>(c);
     return;
   }
@@ -1670,7 +1683,8 @@ __device__ __noinline__ void k_hessian(Ctx& c) {
   }
 }
 
-// Helper warps of a W-warp trajectory group (dev_data.cuh): wait for the main warp's command, run the phase with it.
+// Helper warps of a W-warp trajectory group (dev_data.cuh): wait for the main warp's command, run the phase among
+// themselves and report it done; the main warp meets them at the join when it needs the result.
 template <class SP>
 __device__ __noinline__ void wide_helper_loop(Ctx& c) {
   if constexpr (SP::kWide > 1) {
@@ -1684,6 +1698,7 @@ __device__ __noinline__ void wide_helper_loop(Ctx& c) {
       if (cmd == WIDE_EXIT) return;
       c.ncon = b.ncon; c.nlim = b.nlim; c.ndrow = b.ndrow; c.nefc = b.nefc;
       if (cmd == WIDE_HESSIAN) hessian_static<SP>(c);
+      wide_done<SP>();
     }
   }
 }
@@ -1845,7 +1860,12 @@ __device__ __noinline__ float k_line_search(Ctx& c, float g0, float g1, float g2
   if (snorm < kMinVal) return 0.f;
   const bool cached = c.nitem <= 32;   // one work item per lane: the usual case
   const LsItem item = ls_load_item<SP>(c);
-  auto ev = [&](float alpha) { return cached ? LS_EVAL_CACHED(item, g0, g1, g2, alpha) : k_ls_eval<SP>(c, g0, g1, g2, alpha); };
+  auto ev = [&](float alpha) {
+#if defined(MJPC_PHASE_TIMING) && MJPC_PHASE_MAP == 1
+    c.tph[7]++;   // timer mapping 1: slot 7 counts the evaluations
+#endif
+    return cached ? LS_EVAL_CACHED(item, g0, g1, g2, alpha) : k_ls_eval<SP>(c, g0, g1, g2, alpha);
+  };
   const LsPoint p0 = ev(0.f);
   const float gtol = fmaxf(fmaxf(CM(c).tolerance, kTolFloor) * CM(c).ls_tolerance * snorm * scale_inv, 64 * 1.1920929e-7f * fabsf(p0.d1));
   if (p0.d2 <= kMinVal) return 0.f;
@@ -1942,6 +1962,7 @@ __device__ __noinline__ void k_solve(Ctx& c) {
     __syncwarp();
     return;
   }
+  PHASE_AT(c, 1, 8);
   float gauss, cost;
   if (!M.disable_warmstart) {
     // warm start (engine_forward: the better of qacc_warmstart and qacc_smooth).  The smooth point is evaluated
@@ -1957,6 +1978,7 @@ __device__ __noinline__ void k_solve(Ctx& c) {
     __syncwarp();
     cost = k_total_cost<SP>(c, qacc, true, &gauss);
   }
+  PHASE_AT(c, 1, 4);
   const float scale_inv = CM(c).meaninertia * (float)max(1, nv);
   const float tol = fmaxf(CM(c).tolerance, kTolFloor);
   const int nsimple = M.nfloss + c.nlim;
@@ -1965,7 +1987,22 @@ __device__ __noinline__ void k_solve(Ctx& c) {
   float old = cost, prev_gradient = 3.0e38f, alpha = 0.f;
   int stalls = 0;
   bool qfc_current = false;
+  // Helper-warp kernels: the Hessian at the current point is assembled by the helper warps while this warp forms the
+  // gradient and the termination test.  The assembly reads only what the last k_total_cost(.., hess=true) and the
+  // constraint rows left (qM, efc_hw, efc_hc, efc_w, efc_Jd, efc_Xd, efc_state, con_*, efc_dof, efc_drow, cdof) and
+  // writes efc_hc[36 ci + 14 ..], efc_blk, dofbuf and qH, none of which J^T f, the gradient and the test touch (they
+  // write qfrc_constraint and grad).  An assembly in flight when the test stops the solve is dropped: it is left
+  // running while the step ends (Euler, outputs: they touch none of its arrays) and met by wide_settle before the next
+  // step's kinematics, which rewrite what it reads.
   for (int iter = 0; iter <= M.iterations; iter++) {
+    if constexpr (SP::kWide > 1) {
+      if (iter < M.iterations) {
+        hessian_cone_rows<SP>(c);
+        wide_post_async<SP>(c, WIDE_HESSIAN);
+        c.wide_pending = 1;
+        PHASE_AT(c, 1, 5);
+      }
+    }
     // gradient at the current point; qfc doubles as the J^T force scratch and is the output when we stop here
     jt_force_any<SP>(c, qfc, nv);
     qfc_current = true;
@@ -1993,13 +2030,18 @@ __device__ __noinline__ void k_solve(Ctx& c) {
       else if (gradient > 0.5f * prev_gradient && (alpha > 0.5f || ++stalls >= 3)) break;
       prev_gradient = gradient;
     }
+    PHASE_AT(c, 1, 0);
     if (iter == M.iterations) break;
-    // Newton direction: assemble + factorise the Hessian only now that another iteration is taken
+    // Newton direction: assemble (or meet the helpers' assembly) + factorise the Hessian only now that another
+    // iteration is taken
     PHASE(c, 4);
-    k_hessian<SP>(c);
+    if constexpr (SP::kWide > 1) wide_settle<SP>(c);
+    else k_hessian<SP>(c);
     PHASE(c, 5);
+    PHASE_AT(c, 1, 5);
     warp_chol_factor_solve<SP::kNV>(DF(qH), DF(hinv), search, grad, nv, lane);
     PHASE(c, 6);
+    PHASE_AT(c, 1, 6);
     for (int b0 = 0; b0 < nv; b0 += 32) { const int i = min(b0 + lane, nv - 1); const float v = -search[i]; __syncwarp(); if (b0 + lane < nv) search[i] = v; }
     __syncwarp();
     float q1 = 0, q2 = 0, sn = 0;
@@ -2020,7 +2062,9 @@ __device__ __noinline__ void k_solve(Ctx& c) {
     }
     q1 = warp_sum(q1); q2 = warp_sum(q2); sn = sqrtf(warp_sum(sn));
     __syncwarp();
+    PHASE_AT(c, 1, 1);
     alpha = k_line_search<SP>(c, gauss, q1, q2, sn, scale_inv);
+    PHASE_AT(c, 1, 2);
     if (alpha == 0.f) break;
     for (int b0 = 0; b0 < nv; b0 += 32) { const int i = min(b0 + lane, nv - 1); const float v = qacc[i] + alpha * search[i]; __syncwarp(); if (b0 + lane < nv) qacc[i] = v; }
     __syncwarp();
@@ -2028,8 +2072,11 @@ __device__ __noinline__ void k_solve(Ctx& c) {
     cost = k_total_cost<SP>(c, qacc, true, &gauss, alpha);
     qfc_current = false;
     c.niter = iter + 1;
+    PHASE_AT(c, 1, 3);
   }
+  PHASE_AT(c, 1, 0);
   if (!qfc_current) jt_force_any<SP>(c, qfc, nv);
+  PHASE_AT(c, 1, 0);
 }
 
 // ------------------------------------------------------------------------------------------ pipeline pieces
@@ -2068,7 +2115,9 @@ __device__ __noinline__ void k_euler(Ctx& c) {
   float *qacc = DF(qacc), *qvel = DF(qvel), *qpos = DF(qpos), *vt = DF(vtmp);
   const float* acc = qacc;
   if (M.any_damping && !M.disable_eulerdamp) {
-    float *H = DF(qH), *qM = DF(qM), *smooth = DF(qfrc_smooth), *qfc = DF(qfrc_constraint);
+    // (helper-warp kernels: an abandoned Hessian assembly may still be writing qH; qLD is free after join 1 until the
+    // next step's k_crb)
+    float *H = SP::kWide > 1 ? DF(qLD) : DF(qH), *qM = DF(qM), *smooth = DF(qfrc_smooth), *qfc = DF(qfrc_constraint);
     const float* damping = MF(dof_damping);
     MJPC_ROLL
     for (int w = lane; w < nv * nv; w += 32) {

@@ -95,9 +95,9 @@ __device__ __forceinline__ void init_ctx(Ctx& c, const DevModel* M, const DevLay
   c.lane = lane;
   c.gkey = pack + M->nf + M->ni;   // the keyframe table follows the staged part of the pack in HBM
   c.ncon = 0; c.npseudo = 0; c.xfrc_on = 0; c.nefc = 0; c.ndrow = 0; c.nitem = 0; c.niter = 0; c.nlim = 0; c.warn = 0; c.time = 0.f;
-  c.sync = nullptr; c.sync_slot = -1; c.sync_mode = 0;
+  c.sync = nullptr; c.sync_slot = -1; c.sync_mode = 0; c.wide_pending = 0;
 #ifdef MJPC_PHASE_TIMING
-  for (int k = 0; k < 8; k++) c.tph[k] = 0;
+  for (int k = 0; k < 9; k++) c.tph[k] = 0;
   c.tlast = clock64();
 #endif
 }
@@ -143,13 +143,23 @@ __device__ __noinline__ void task_warp_loop(Ctx& c, const RolloutArgs& A, int ca
   c.xfrc_on = A.xfrc_std > 0.f ? 1 : 0;
   float* o_res = A.residual + (size_t)cand * H * nr;
   float* o_trace = A.trace + (size_t)cand * H * ntr;
+#ifdef MJPC_PHASE_TIMING
+  long long fork_cycles = 0;   // timer mapping 2: this warp's fork intervals, reported by the main warp
+#endif
   for (int t = 0; t < H; t++) {
     const bool last = t == H - 1;
     task_bar();   // fork (the main warp has written the state, the action and the poses of step t)
     if (wide_box().task_exit) return;
+#ifdef MJPC_PHASE_TIMING
+    const long long t_fork = clock64();
+#endif
     k_crb<SP>(c);
     k_com_vel<SP>(c);
     k_smooth_forces<SP>(c);
+#ifdef MJPC_PHASE_TIMING
+    fork_cycles += clock64() - t_fork;
+    if (lane == 0) wide_box().task_fork_cycles = fork_cycles;
+#endif
     task_bar();   // join 1
     k_residual<SP>(c);
     for (int i = lane; i < nr; i += 32) o_res[(size_t)t * nr + i] = DF(residual)[i];
@@ -263,21 +273,23 @@ __device__ __forceinline__ void rollout_body(const RolloutArgs& A) {
       // the step as a fork / join graph (the one-warp order is k_forward, dev_physics.cuh):
       //   main: kinematics, com | collision, constraint rows        | reference, Newton solve           | Euler
       //   task:                 | CRB, velocities, smooth forces    | residual, cost, next spline action |
-      PHASE(c, 7);
+      PHASE(c, 7); PHASE_AT(c, 2, 7);
+      wide_settle<SP>(c);   // the last step's abandoned Hessian assembly reads poses, cdof, qM and the contacts
       k_kinematics<SP>(c);
       k_com_pos<SP>(c);
-      PHASE(c, 0);
+      PHASE(c, 0); PHASE_AT(c, 2, 0);
       task_bar();   // fork
       k_collision<SP>(c);
-      PHASE(c, 1);
+      PHASE(c, 1); PHASE_AT(c, 2, 1);
       k_make_constraint<SP>(c);
-      PHASE(c, 2);
+      PHASE(c, 2); PHASE_AT(c, 2, 2);
       task_bar();   // join: qM, qfrc_smooth, qacc_smooth are in place
+      PHASE_AT(c, 2, 3);
       k_reference<SP>(c);
       PHASE(c, 3);
       if (c.sync_mode & 2) pair_sync_meet(c, 2 * t + 1);
       k_solve<SP>(c);
-      PHASE(c, 4);
+      PHASE(c, 4); PHASE_AT(c, 2, 4);
       n_newton += c.niter; n_con += c.ncon - c.npseudo; n_efc += c.nefc;
       if (!last && k_bad(c, DF(qacc), nv)) c.warn = 1;
       task_bar();   // join: residual, trace and cost of this step are written, ctrl holds the next action
@@ -307,6 +319,7 @@ __device__ __forceinline__ void rollout_body(const RolloutArgs& A) {
     if (lane == 0) o_times[t + 1] = time0 + (double)c.time;
   }
   pair_sync_done(c);
+  wide_settle<SP>(c);
   wide_post<SP>(c, WIDE_EXIT);   // releases the helper warps
   if (lane == 0) {
     A.returns[cand] = failed ? 1.0e6f : total / (float)max(H, 1);
@@ -314,6 +327,9 @@ __device__ __forceinline__ void rollout_body(const RolloutArgs& A) {
     if (A.stats) {
       A.stats[12 * cand] = clock64() - clk0; A.stats[12 * cand + 1] = n_newton;
       A.stats[12 * cand + 2] = n_con; A.stats[12 * cand + 3] = n_efc;
+#if defined(MJPC_PHASE_TIMING) && MJPC_PHASE_MAP == 2
+      if constexpr (kTask) c.tph[5] = wide_box().task_fork_cycles;
+#endif
       for (int k = 0; k < 8; k++) {
 #ifdef MJPC_PHASE_TIMING
         A.stats[12 * cand + 4 + k] = c.tph[k];
@@ -337,11 +353,12 @@ extern "C" __global__ void __launch_bounds__(128) rollout_kernel(const __grid_co
 }
 // statically specialised instance for the Quadruped (flat) task model (spec_quadruped.h); one warp per CTA
 // Static instances: the shipped one holds kRolloutWide + kRolloutTask warps per candidate (main warp, Hessian helper warps,
-// task warp: DESIGN.md section 5 "helper warps"; 6 + 1 measured best at 128 and at 256 candidates).  The *_plain instance is
+// task warp: DESIGN.md section 5 "helper warps"; 7 + 1 since the Hessian runs on the helpers alone: 6 helpers cover the
+// 171 Hessian entries of the A1 in one round, measured faster than 6 + 1 at 256 candidates).  The *_plain instance is
 // the same source with ONE warp per candidate: the reference the helper-warp kernel must equal bit for bit
 // (tests/test_gpu_parity.py, MJPC_B200_SHAPE=plain) and the baseline of the profiles.
 #ifndef MJPC_WIDE
-#define MJPC_WIDE 6
+#define MJPC_WIDE 7
 #endif
 #ifndef MJPC_TASK
 #define MJPC_TASK 1

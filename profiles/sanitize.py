@@ -15,6 +15,8 @@ if which in ("all", "rollout"):
         e.rollout_spline(state, 0.0, mocap, knots, kt, 2, 10)
         assert e.last_kernel_shape == (1 if shape == "wide" else 2)
     del os.environ["MJPC_B200_SHAPE"]
+    mt = type(m)(m); mt.opt_tolerance = 1.0                                    # solves stop with a Hessian assembly in flight
+    et = Engine(mt, 8, 12); et.rollout_spline(state, 0.0, mocap, knots, kt, 2, 10); et.close()
     os.environ["MJPC_B200_NO_STATIC"] = "1"
     e.rollout_spline(state, 0.0, mocap, knots, kt, 2, 10)                      # generic instance
     del os.environ["MJPC_B200_NO_STATIC"]
