@@ -37,6 +37,27 @@ std::vector<int> time_like_state(int residual_id) {
   if (residual_id == RESIDUAL_HUMANOID_TRACK) return {1};   // reference_time
   return {};
 }
+
+// The compiled kernel instances for one task model: the generic (DynSpec) ones, or those statically specialised for a
+// model table (spec_*.h), which create() selects with spec_matches.
+struct KernelSet {
+  const void* rollout;         // shipped shape, rollout_threads threads per candidate
+  const void* rollout_plain;   // one warp per candidate: the bitwise reference of the shipped shape
+  const void* step;
+  const void* fd_center;
+  const void* fd_column;
+  int rollout_threads;
+};
+const KernelSet kGenericKernels = {(const void*)rollout_kernel, (const void*)rollout_kernel, (const void*)step_batch_kernel,
+                                   (const void*)fd_center_kernel, (const void*)fd_column_kernel, 32};
+const KernelSet kQuadrupedKernels = {(const void*)rollout_kernel_quadruped, (const void*)rollout_kernel_quadruped_plain,
+                                     (const void*)step_batch_kernel_quadruped, (const void*)fd_center_kernel_quadruped,
+                                     (const void*)fd_column_kernel_quadruped, kRolloutThreads};
+// (no static fd instances: the Humanoid Track's derivative sweeps run the generic ones)
+const KernelSet kHumanoidTrackKernels = {(const void*)rollout_kernel_humanoid_track,
+                                         (const void*)rollout_kernel_humanoid_track_plain,
+                                         (const void*)step_batch_kernel_humanoid_track, (const void*)fd_center_kernel,
+                                         (const void*)fd_column_kernel, kRolloutThreads};
 }  // namespace
 
 struct mjpc_b200 {
@@ -49,10 +70,10 @@ struct mjpc_b200 {
   int num_sms = 132;
   size_t smem_optin = 0;   // the device's opt-in limit of dynamic shared memory per block
   int max_term_dim = 1;    // widest cost term (task_dim_norm_residual): sizes cost_derivatives_kernel's scratch
-  int static_spec = 0;   // 1 / 2: the model equals spec_quadruped.h / spec_humanoid_track.h -> static rollout kernel
+  const KernelSet* kernels = &kGenericKernels;   // chosen at create: the model's static instances, if it has them
   float* d_pack = nullptr;
   // inputs: d_in holds the per-problem inputs and the knots of the last rollout launch (stage_problems)
-  float *d_in = nullptr, *d_task_state = nullptr;
+  float* d_in = nullptr;
   // feedback policy of each problem of the last feedback launch ([fb_nprob][max_horizon][..]; grown on demand)
   float *d_unom = nullptr, *d_xnom = nullptr, *d_tnom = nullptr, *d_gains = nullptr, *d_du = nullptr, *d_steps = nullptr;
   int fb_nprob = 1;
@@ -64,10 +85,9 @@ struct mjpc_b200 {
   int* d_order = nullptr;
   long long* d_stats = nullptr;
   unsigned* d_pair_sync = nullptr;   // [256][32]: per-SM records of the co-resident pair synchronisation (dev_data.cuh)
-  // debug + ilqg scratch
-  float* d_dbg = nullptr;
-  int dbg_ncon = -1;                 // geometric contacts of the last step_debug (-1: none run yet)
-  float* d_dbg_contact = nullptr;    // their [ncon][8] rows, inside d_dbg
+  // geometric contacts of the last step_debug (-1: none run yet) and their [maxcon][8] rows
+  int dbg_ncon = -1;
+  std::vector<float> dbg_contact;
   IlqgBuffers ilqg;
   // pinned staging
   float* h_in = nullptr;
@@ -124,10 +144,25 @@ int upload_task(mjpc_b200* h) {
   return 0;
 }
 
-// the dynamic shared-memory opt-in is per kernel (process-wide): only ever raise it, several handles may coexist
-int set_smem(const void* fn, size_t bytes) {
-  CUDA_TRY(mjpc_dev::raise_smem_limit(fn, bytes));
-  return 0;
+// The instance a launch runs from the handle's row, and what mjpc_b200_last_kernel_static reports for it (0 generic,
+// 1 static, 2 static one-warp rollout).  Read per launch, so that tests and profiles can switch them on a live engine:
+// MJPC_B200_NO_STATIC=1 forces the generic row, MJPC_B200_SHAPE=plain the one-warp rollout.
+int pick_kernels(const mjpc_b200* h, bool allow_static, const KernelSet** k) {
+  const char* ns = std::getenv("MJPC_B200_NO_STATIC");
+  const char* sh = std::getenv("MJPC_B200_SHAPE");
+  if (h->kernels == &kGenericKernels || !allow_static || (ns && ns[0] == '1')) { *k = &kGenericKernels; return 0; }
+  *k = h->kernels;
+  return sh && sh[0] == 'p' && sh[1] == 'l' ? 2 : 1;
+}
+
+// src (NULL: the handle's task state) as floats, with its time-like entries made relative to t0
+void rebase_task_state(const mjpc_b200* h, const double* src, double t0, float* dst) {
+  if (!src) src = h->task_state.data();
+  for (int i = 0; i < h->pack.M.task_state_size; i++) {
+    double v = src[i];
+    if (std::find(h->time_idx.begin(), h->time_idx.end(), i) != h->time_idx.end()) v -= t0;
+    dst[i] = (float)v;
+  }
 }
 
 // floats of the per-problem block of stage_problems for B problems and P knots (knots excluded)
@@ -153,15 +188,7 @@ int stage_problems(mjpc_b200* h, int B, const float* states, const double* times
   const size_t o_state = o; std::memcpy(in + o, states, B * ds * 4); o += B * ds;
   const size_t o_mocap = o; if (nm) std::memcpy(in + o, mocaps, B * nm * 4); o += B * nm;
   const size_t o_ts = o;
-  for (int b = 0; b < B; b++) {
-    const double* src = task_states ? task_states + b * nts : h->task_state.data();
-    for (size_t i = 0; i < nts; i++) {
-      double v = src[i];
-      if (std::find(h->time_idx.begin(), h->time_idx.end(), (int)i) != h->time_idx.end()) v -= times[b];
-      in[o + i] = (float)v;
-    }
-    o += nts;
-  }
+  for (int b = 0; b < B; b++, o += nts) rebase_task_state(h, task_states ? task_states + b * nts : nullptr, times[b], in + o);
   const size_t o_w = o;
   if (weights) for (size_t i = 0; i < B * nw; i++) in[o++] = (float)weights[i];
   const size_t o_p = o;
@@ -221,9 +248,6 @@ int launch_rollout(mjpc_b200* h, const RolloutArgs& A_in) {
   const size_t smem = h->smem_bytes(A.P, wpc);
   const int grid = (A.N + wpc - 1) / wpc;
   CUDA_TRY(cudaEventRecord(h->ev0, h->stream));
-  // static instance: same arguments, same shared-memory image; MJPC_B200_NO_STATIC=1 forces the generic kernel
-  const char* ns = std::getenv("MJPC_B200_NO_STATIC");
-  const bool use_static = h->static_spec != 0 && wpc == 1 && !(ns && ns[0] == '1');
   // co-resident pair synchronisation: only when at most two candidates can ever be resident per SM and all are resident
   // at once (one wave); MJPC_B200_PAIR_SYNC=0 switches it off (profiling)
   {
@@ -233,19 +257,11 @@ int launch_rollout(mjpc_b200* h, const RolloutArgs& A_in) {
     A.pair_sync_mode = (ps && ps[0] >= '1' && ps[0] <= '9') ? std::atoi(ps) : 1;   // 1: meet per step (default), 3: and before the solve; + 16 k: only at steps with (t & k) == 0
     if (on) CUDA_TRY(cudaMemsetAsync(h->d_pair_sync, 0, (size_t)256 * 32 * sizeof(unsigned), h->stream));
   }
-  // MJPC_B200_SHAPE=plain selects the one-warp-per-candidate static instance (tests / profiling: the bitwise reference)
-  const char* sh = std::getenv("MJPC_B200_SHAPE");
-  const bool plain = sh && sh[0] == 'p' && sh[1] == 'l';
-  if (use_static && h->static_spec == 1) {
-    if (plain) rollout_kernel_quadruped_plain<<<grid, 32, smem, h->stream>>>(A);
-    else rollout_kernel_quadruped<<<grid, kRolloutThreads, smem, h->stream>>>(A);
-  } else if (use_static && h->static_spec == 2) {
-    if (plain) rollout_kernel_humanoid_track_plain<<<grid, 32, smem, h->stream>>>(A);
-    else rollout_kernel_humanoid_track<<<grid, kRolloutThreads, smem, h->stream>>>(A);
-  } else {
-    rollout_kernel<<<grid, 32 * wpc, smem, h->stream>>>(A);
-  }
-  h->last_static = use_static ? (plain ? 2 : 1) : 0;
+  // static instance: same arguments, same shared-memory image, one candidate per CTA
+  const KernelSet* k;
+  h->last_static = pick_kernels(h, wpc == 1, &k);
+  const bool plain = h->last_static == 2;
+  launch_kernel(plain ? k->rollout_plain : k->rollout, grid, (plain ? 32 : k->rollout_threads) * wpc, smem, h->stream, A);
   rank_kernel<<<(A.N + 255) / 256, 256, 0, h->stream>>>(A.returns, A.nper, A.nprob, h->d_order);
   CUDA_TRY(cudaEventRecord(h->ev1, h->stream));
   CUDA_TRY(cudaGetLastError());
@@ -419,7 +435,6 @@ int mjpc_b200_create(const mjpc_model_blob* model, int max_candidates, int max_h
   // launch inputs: up to max_candidates problems of one candidate each (stage_problems)
   const size_t in_floats = problem_floats(M, max_candidates, h->maxP) + N * h->maxP * nu;
   CREATE_TRY(dalloc(&h->d_in, in_floats));
-  CREATE_TRY(dalloc(&h->d_task_state, (size_t)M.task_state_size));
   CREATE_TRY(dalloc(&h->d_unom, H * nu)); CREATE_TRY(dalloc(&h->d_xnom, H * ds)); CREATE_TRY(dalloc(&h->d_tnom, H));
   CREATE_TRY(dalloc(&h->d_gains, H * nu * n)); CREATE_TRY(dalloc(&h->d_du, H * nu)); CREATE_TRY(dalloc(&h->d_steps, N));
   CREATE_TRY(dalloc(&h->d_states, N * H * ds)); CREATE_TRY(dalloc(&h->d_actions, N * H * nu));
@@ -427,24 +442,22 @@ int mjpc_b200_create(const mjpc_model_blob* model, int max_candidates, int max_h
   CREATE_TRY(dalloc(&h->d_costs, N * H)); CREATE_TRY(dalloc(&h->d_trace, N * H * 3 * (size_t)M.num_trace));
   CREATE_TRY(dalloc(&h->d_returns, N)); CREATE_TRY(dalloc(&h->d_failure, N)); CREATE_TRY(dalloc(&h->d_order, N)); CREATE_TRY(dalloc(&h->d_stats, 12 * N));
   CREATE_TRY(dalloc(&h->d_pair_sync, (size_t)256 * 32));
-  CREATE_TRY(dalloc(&h->d_dbg, 4 * ds + 2 * nu + (size_t)M.nv * M.nv + nr + 256 + 64 + 8 * (size_t)M.maxcon +
-                               7 * (size_t)M.nmocap));
   h->h_in_floats = in_floats + H * (nu + ds + 1 + nu * n + nu) + N + 64;
   CREATE_TRY(cudaMallocHost((void**)&h->h_in, h->h_in_floats * 4));
   h->h_out_bytes = N * 16 + 64;
   CREATE_TRY(cudaMallocHost((void**)&h->h_out, h->h_out_bytes));
-  if (int rc = set_smem((const void*)rollout_kernel, h->smem_bytes(h->maxP, h->warps_per_cta))) { mjpc_b200_destroy(h); return rc; }
-  if (int rc = set_smem((const void*)step_debug_kernel, h->smem_bytes(1, 1))) { mjpc_b200_destroy(h); return rc; }
-  if (spec_matches<SpecQuadruped>(M, make_layout(M, 1))) {
-    h->static_spec = 1;
-    if (int rc = set_smem((const void*)rollout_kernel_quadruped, h->smem_bytes(h->maxP, 1))) { mjpc_b200_destroy(h); return rc; }
-    if (int rc = set_smem((const void*)rollout_kernel_quadruped_plain, h->smem_bytes(h->maxP, 1))) { mjpc_b200_destroy(h); return rc; }
-  } else if (spec_matches<SpecHumanoidTrack>(M, make_layout(M, 1))) {
-    h->static_spec = 2;
-    if (int rc = set_smem((const void*)rollout_kernel_humanoid_track, h->smem_bytes(h->maxP, 1))) { mjpc_b200_destroy(h); return rc; }
-    if (int rc = set_smem((const void*)rollout_kernel_humanoid_track_plain, h->smem_bytes(h->maxP, 1))) { mjpc_b200_destroy(h); return rc; }
+  const DevLayout L1 = make_layout(M, 1);
+  if (spec_matches<SpecQuadruped>(M, L1)) h->kernels = &kQuadrupedKernels;
+  else if (spec_matches<SpecHumanoidTrack>(M, L1)) h->kernels = &kHumanoidTrackKernels;
+  // the dynamic shared-memory opt-in is per kernel and process-wide (raise_smem_limit only ever raises it: several
+  // handles may coexist); a launch may fall back to the generic row (pick_kernels), so both rows get theirs
+  const size_t smem_rollout = h->smem_bytes(h->maxP, h->warps_per_cta), smem_step = h->smem_bytes(1, 1);
+  for (const KernelSet* k : {h->kernels, &kGenericKernels}) {
+    CREATE_TRY(raise_smem_limit(k->rollout, smem_rollout)); CREATE_TRY(raise_smem_limit(k->rollout_plain, smem_rollout));
+    CREATE_TRY(raise_smem_limit(k->step, smem_step)); CREATE_TRY(raise_smem_limit(k->fd_center, smem_step));
+    CREATE_TRY(raise_smem_limit(k->fd_column, smem_step));
   }
-  if (int rc = ilqg_init(h->ilqg, h->pack.M, (int)H, h->smem_bytes(1, 1))) {
+  if (int rc = ilqg_init(h->ilqg, h->pack.M, (int)H)) {
     mjpc_b200_destroy(h);
     return fail(rc, "ilqg buffer allocation failed");
   }
@@ -459,9 +472,9 @@ void mjpc_b200_destroy(mjpc_b200_t* h) {
   if (h->comm && nccl_api().ok) nccl_api().CommDestroy(h->comm);
   void* mbufs[] = {h->d_slot, h->d_gather, h->d_returns_all, h->d_failure_all, h->d_order_all, h->d_bcast};
   for (void* p : mbufs) if (p) cudaFree(p);
-  void* bufs[] = {h->d_pack, h->d_in, h->d_task_state, h->d_unom, h->d_xnom,
+  void* bufs[] = {h->d_pack, h->d_in, h->d_unom, h->d_xnom,
                   h->d_tnom, h->d_gains, h->d_du, h->d_steps, h->d_states, h->d_actions, h->d_times, h->d_residual,
-                  h->d_costs, h->d_trace, h->d_returns, h->d_failure, h->d_order, h->d_dbg, h->d_stats, h->d_pair_sync};
+                  h->d_costs, h->d_trace, h->d_returns, h->d_failure, h->d_order, h->d_stats, h->d_pair_sync};
   for (void* p : bufs) if (p) cudaFree(p);
   ilqg_free(h->ilqg);
   if (h->h_in) cudaFreeHost(h->h_in);
@@ -685,48 +698,80 @@ int mjpc_b200_fetch_all(mjpc_b200_t* h, float* states, float* actions, double* t
   return fetch_impl(h, 0, h->lastN, states, actions, times, residual, costs, trace);
 }
 
+// B single steps (see step_batch_kernel) on instance `fn`.  times are absolute; the task state is rebased to time0
+// (device time = times[b] - time0).  Outputs may be NULL; qM [B][nv nv], efc_force [B][maxefc] and contact
+// [B][maxcon][8] are the optional ones, their rows past each problem's counts read as zeros.  e0 / e1, when given,
+// time the kernel.
+static int step_impl(mjpc_b200_t* h, const void* fn, int B, const float* qpos, const float* qvel, const float* ctrl,
+                     const float* warmstart, const float* mocap, double time0, const double* times, float* qacc,
+                     float* next_qpos, float* next_qvel, float* residual, float* cost, int* counts, float* qM,
+                     float* efc_force, float* contact, cudaEvent_t e0, cudaEvent_t e1) {
+  const DevModel& M = h->pack.M;
+  CUDA_TRY(cudaSetDevice(h->device));
+  const size_t Bs = B, nq = M.nq, nv = M.nv, nu = M.nu, nr = std::max(M.num_residual, 1), nm = 7 * (size_t)M.nmocap,
+               nts = (size_t)M.task_state_size;
+  size_t words = 0;
+  auto take = [&](size_t n) { const size_t at = words; words += n; return at; };
+  const size_t o_qpos = take(Bs * nq), o_qvel = take(Bs * nv), o_ctrl = take(Bs * nu), o_warm = take(Bs * nv),
+               o_time = take(Bs), o_mocap = take(nm), o_ts = take(nts), o_qacc = take(Bs * nv), o_nq = take(Bs * nq),
+               o_nv = take(Bs * nv), o_res = take(Bs * nr), o_cost = take(Bs), o_counts = take(4 * Bs),
+               o_qM = take(qM ? Bs * nv * nv : 0), o_efc = take(efc_force ? Bs * M.maxefc : 0),
+               o_con = take(contact ? Bs * M.maxcon * 8 : 0);
+  float* d = nullptr;
+  CUDA_TRY(dalloc(&d, words));
+  struct Guard { float* p; ~Guard() { cudaFree(p); } } guard{d};
+  std::vector<float> trel(B), ts(nts);
+  for (int i = 0; i < B; i++) trel[i] = (float)(times[i] - time0);
+  rebase_task_state(h, nullptr, time0, ts.data());
+  // every transfer on the engine stream, ordered with the kernel
+  auto put = [&](size_t at, const void* src, size_t floats) {
+    return cudaMemcpyAsync(d + at, src, floats * 4, cudaMemcpyHostToDevice, h->stream);
+  };
+  CUDA_TRY(cudaMemsetAsync(d, 0, words * 4, h->stream));
+  CUDA_TRY(put(o_qpos, qpos, Bs * nq)); CUDA_TRY(put(o_qvel, qvel, Bs * nv)); CUDA_TRY(put(o_ctrl, ctrl, Bs * nu));
+  if (warmstart) CUDA_TRY(put(o_warm, warmstart, Bs * nv));
+  CUDA_TRY(put(o_time, trel.data(), Bs));
+  if (nm) CUDA_TRY(put(o_mocap, mocap, nm));
+  if (nts) CUDA_TRY(put(o_ts, ts.data(), nts));
+  StepBatchArgs A;
+  std::memset(&A, 0, sizeof(A));
+  A.M = h->pack.M; A.L = make_layout(h->pack.M, 1); A.pack = h->d_pack;
+  A.qpos = d + o_qpos; A.qvel = d + o_qvel; A.ctrl = d + o_ctrl; A.warmstart = warmstart ? d + o_warm : nullptr;
+  A.mocap = d + o_mocap; A.task_state = nts ? d + o_ts : nullptr; A.time = d + o_time; A.B = B;
+  A.qacc = d + o_qacc; A.next_qpos = d + o_nq; A.next_qvel = d + o_nv; A.residual = d + o_res; A.cost = d + o_cost;
+  A.counts = (int*)(d + o_counts);
+  A.qM = qM ? d + o_qM : nullptr; A.efc_force = efc_force ? d + o_efc : nullptr; A.contact = contact ? d + o_con : nullptr;
+  if (e0) CUDA_TRY(cudaEventRecord(e0, h->stream));
+  launch_kernel(fn, B, 32, h->smem_bytes(1, 1), h->stream, A);
+  if (e1) CUDA_TRY(cudaEventRecord(e1, h->stream));
+  CUDA_TRY(cudaGetLastError());
+  h->launches += 1;
+  CUDA_TRY(cudaStreamSynchronize(h->stream));
+  if (e0 && cudaEventElapsedTime(&h->last_ms, e0, e1) != cudaSuccess) cudaGetLastError();
+  auto get = [&](void* dst, size_t at, size_t bytes) {
+    return dst ? cudaMemcpy(dst, d + at, bytes, cudaMemcpyDeviceToHost) : cudaSuccess;
+  };
+  CUDA_TRY(get(qacc, o_qacc, Bs * nv * 4)); CUDA_TRY(get(next_qpos, o_nq, Bs * nq * 4));
+  CUDA_TRY(get(next_qvel, o_nv, Bs * nv * 4)); CUDA_TRY(get(residual, o_res, Bs * M.num_residual * 4));
+  CUDA_TRY(get(cost, o_cost, Bs * 4)); CUDA_TRY(get(counts, o_counts, Bs * 16));
+  CUDA_TRY(get(qM, o_qM, Bs * nv * nv * 4)); CUDA_TRY(get(efc_force, o_efc, Bs * M.maxefc * 4));
+  CUDA_TRY(get(contact, o_con, Bs * M.maxcon * 8 * 4));
+  return 0;
+}
+
+// One step of the generic instance at device time (float)time, with the task state as set_task left it: step_impl
+// with B = 1 and time0 = 0.  Not timed: last_kernel_ms and last_kernel_static keep describing the last planning launch.
 int mjpc_b200_step_debug(mjpc_b200_t* h, const float* qpos, const float* qvel, const float* ctrl,
                          const float* mocap, double time, const float* warmstart, float* qacc, float* residual,
                          float* next_qpos, float* next_qvel, float* qM, float* efc_force, int* counts) {
   if (!h || !qpos || !qvel || !ctrl) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "step_debug: null");
-  const DevModel& M = h->pack.M;
-  CUDA_TRY(cudaSetDevice(h->device));
-  const size_t nq = M.nq, nv = M.nv, nu = M.nu, nr = M.num_residual;
-  float* d = h->d_dbg;
-  float *d_qpos = d, *d_qvel = d_qpos + nq, *d_ctrl = d_qvel + nv, *d_mocap = d_ctrl + nu, *d_warm = d_mocap + 7 * M.nmocap,
-        *d_qacc = d_warm + nv, *d_res = d_qacc + nv, *d_nq = d_res + nr, *d_nv = d_nq + nq, *d_qM = d_nv + nv,
-        *d_force = d_qM + nv * nv;
-  int* d_counts = (int*)(d_force + 256);
-  float* d_contact = d_force + 256 + 64;
-  h->dbg_ncon = -1; h->d_dbg_contact = d_contact;
-  CUDA_TRY(cudaMemcpy(d_qpos, qpos, nq * 4, cudaMemcpyHostToDevice));
-  CUDA_TRY(cudaMemcpy(d_qvel, qvel, nv * 4, cudaMemcpyHostToDevice));
-  CUDA_TRY(cudaMemcpy(d_ctrl, ctrl, nu * 4, cudaMemcpyHostToDevice));
-  if (M.nmocap) CUDA_TRY(cudaMemcpy(d_mocap, mocap, 7 * M.nmocap * 4, cudaMemcpyHostToDevice));
-  if (warmstart) CUDA_TRY(cudaMemcpy(d_warm, warmstart, nv * 4, cudaMemcpyHostToDevice));
-  std::vector<float> ts(M.task_state_size);
-  for (int i = 0; i < M.task_state_size; i++) ts[i] = (float)h->task_state[i];
-  if (M.task_state_size) CUDA_TRY(cudaMemcpy(h->d_task_state, ts.data(), ts.size() * 4, cudaMemcpyHostToDevice));
-  DebugArgs A;
-  std::memset(&A, 0, sizeof(A));
-  A.M = h->pack.M; A.L = make_layout(h->pack.M, 1); A.pack = h->d_pack;
-  A.qpos = d_qpos; A.qvel = d_qvel; A.ctrl = d_ctrl; A.mocap = d_mocap; A.warmstart = warmstart ? d_warm : nullptr;
-  A.task_state = M.task_state_size ? h->d_task_state : nullptr;
-  A.time = (float)time;
-  A.qacc = d_qacc; A.residual = d_res; A.next_qpos = d_nq; A.next_qvel = d_nv; A.qM = d_qM; A.efc_force = d_force;
-  A.counts = d_counts; A.contact = d_contact;
-  step_debug_kernel<<<1, 32, h->smem_bytes(1, 1), h->stream>>>(A);
-  h->launches += 1;
-  CUDA_TRY(cudaGetLastError());
-  CUDA_TRY(cudaStreamSynchronize(h->stream));
-  if (qacc) CUDA_TRY(cudaMemcpy(qacc, d_qacc, nv * 4, cudaMemcpyDeviceToHost));
-  if (residual) CUDA_TRY(cudaMemcpy(residual, d_res, nr * 4, cudaMemcpyDeviceToHost));
-  if (next_qpos) CUDA_TRY(cudaMemcpy(next_qpos, d_nq, nq * 4, cudaMemcpyDeviceToHost));
-  if (next_qvel) CUDA_TRY(cudaMemcpy(next_qvel, d_nv, nv * 4, cudaMemcpyDeviceToHost));
-  if (qM) CUDA_TRY(cudaMemcpy(qM, d_qM, nv * nv * 4, cudaMemcpyDeviceToHost));
-  if (efc_force) CUDA_TRY(cudaMemcpy(efc_force, d_force, 256 * 4, cudaMemcpyDeviceToHost));
+  h->dbg_ncon = -1;
+  h->dbg_contact.resize((size_t)h->pack.M.maxcon * 8);
+  if (efc_force) std::fill_n(efc_force, 256, 0.f);   // the caller's efc_force holds 256 floats, the first maxefc are rows
   int cnt[4];
-  CUDA_TRY(cudaMemcpy(cnt, d_counts, 16, cudaMemcpyDeviceToHost));
+  if (int rc = step_impl(h, kGenericKernels.step, 1, qpos, qvel, ctrl, warmstart, mocap, 0.0, &time, qacc, next_qpos,
+                         next_qvel, residual, nullptr, cnt, qM, efc_force, h->dbg_contact.data(), nullptr, nullptr))
+    return rc;
   if (counts) std::memcpy(counts, cnt, 16);
   h->dbg_ncon = cnt[0];
   return 0;
@@ -736,10 +781,9 @@ int mjpc_b200_step_debug_contacts(mjpc_b200_t* h, int capacity, float* contact, 
   if (!h || capacity < 0 || (capacity > 0 && !contact) || !ncon)
     return fail(MJPC_B200_ERR_BAD_ARGUMENT, "step_debug_contacts: bad argument");
   if (h->dbg_ncon < 0) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "step_debug_contacts: no step_debug call to report");
-  CUDA_TRY(cudaSetDevice(h->device));
   *ncon = h->dbg_ncon;
   const int n = std::min(h->dbg_ncon, capacity);
-  if (n > 0) CUDA_TRY(cudaMemcpy(contact, h->d_dbg_contact, (size_t)n * 8 * 4, cudaMemcpyDeviceToHost));
+  if (n > 0) std::memcpy(contact, h->dbg_contact.data(), (size_t)n * 8 * 4);
   return 0;
 }
 
@@ -817,10 +861,9 @@ int mjpc_b200_rollout_spline_sharded(mjpc_b200_t* h, const float* state, double 
   CUDA_TRY(cudaGetLastError());
   h->launches += 3;
   h->totalN = N; h->shard_lo = lo; h->shard_hi = hi;
-  float* hr = (float*)h->h_out;   // h_out holds maxN * 16 bytes: read back in chunks through pageable copies instead
-  (void)hr;
   CUDA_TRY(cudaStreamSynchronize(h->stream));
   if (cudaEventElapsedTime(&h->last_ms, h->ev0, h->ev1) != cudaSuccess) cudaGetLastError();
+  // N may exceed max_candidates, which sizes the pinned h_out: pageable copies straight into the caller's arrays
   if (returns) CUDA_TRY(cudaMemcpy(returns, h->d_returns_all, (size_t)N * 4, cudaMemcpyDeviceToHost));
   if (failure) CUDA_TRY(cudaMemcpy(failure, h->d_failure_all, (size_t)N, cudaMemcpyDeviceToHost));
   if (order) CUDA_TRY(cudaMemcpy(order, h->d_order_all, (size_t)N * 4, cudaMemcpyDeviceToHost));
@@ -860,67 +903,18 @@ int mjpc_b200_fetch_trajectory_sharded(mjpc_b200_t* h, int candidate, float* sta
   return 0;
 }
 
-// Batched single-step parity hook (see step_batch_kernel): B tuples -> one mj_step each.  times are absolute; the task
-// state is rebased to `time0` exactly as a rollout starting at time0 would (device time = times[b] - time0).
+// Batched single-step parity hook (step_impl) on the instance a rollout of this handle runs
 int mjpc_b200_step_batch(mjpc_b200_t* h, int B, const float* qpos, const float* qvel, const float* ctrl,
                          const float* warmstart, const float* mocap, double time0, const double* times, float* qacc,
                          float* next_qpos, float* next_qvel, float* residual, float* cost, int* counts) {
   if (!h || B < 1 || !qpos || !qvel || !ctrl || !times) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "step_batch: bad argument");
-  const DevModel& M = h->pack.M;
-  if (M.nmocap && !mocap) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "step_batch: mocap required");
-  CUDA_TRY(cudaSetDevice(h->device));
-  const size_t nq = M.nq, nv = M.nv, nu = M.nu, nr = std::max(M.num_residual, 1), nm = 7 * (size_t)M.nmocap,
-               nts = (size_t)M.task_state_size;
-  const size_t per = nq + nv + nu + nv + 1 + nv + nq + nv + nr + 1 + 4;
-  const size_t words = per * (size_t)B + nm + nts + 16;
-  float* d = nullptr;
-  CUDA_TRY(dalloc(&d, words));
-  struct Guard { float* p; ~Guard() { cudaFree(p); } } guard{d};
-  float *d_qpos = d, *d_qvel = d_qpos + B * nq, *d_ctrl = d_qvel + B * nv, *d_warm = d_ctrl + B * nu, *d_time = d_warm + B * nv,
-        *d_qacc = d_time + B, *d_nq = d_qacc + B * nv, *d_nv = d_nq + B * nq, *d_res = d_nv + B * nv, *d_cost = d_res + B * nr,
-        *d_counts = d_cost + B, *d_mocap = d_counts + 4 * (size_t)B, *d_ts = d_mocap + nm;
-  std::vector<float> trel(B), ts(nts);
-  for (int i = 0; i < B; i++) trel[i] = (float)(times[i] - time0);
-  for (size_t i = 0; i < nts; i++) {
-    double v = h->task_state[i];
-    if (std::find(h->time_idx.begin(), h->time_idx.end(), (int)i) != h->time_idx.end()) v -= time0;
-    ts[i] = (float)v;
-  }
-  CUDA_TRY(cudaMemcpy(d_qpos, qpos, B * nq * 4, cudaMemcpyHostToDevice));
-  CUDA_TRY(cudaMemcpy(d_qvel, qvel, B * nv * 4, cudaMemcpyHostToDevice));
-  CUDA_TRY(cudaMemcpy(d_ctrl, ctrl, B * nu * 4, cudaMemcpyHostToDevice));
-  if (warmstart) CUDA_TRY(cudaMemcpy(d_warm, warmstart, B * nv * 4, cudaMemcpyHostToDevice));
-  CUDA_TRY(cudaMemcpy(d_time, trel.data(), (size_t)B * 4, cudaMemcpyHostToDevice));
-  if (nm) CUDA_TRY(cudaMemcpy(d_mocap, mocap, nm * 4, cudaMemcpyHostToDevice));
-  if (nts) CUDA_TRY(cudaMemcpy(d_ts, ts.data(), nts * 4, cudaMemcpyHostToDevice));
-  StepBatchArgs A;
-  std::memset(&A, 0, sizeof(A));
-  A.M = h->pack.M; A.L = make_layout(h->pack.M, 1); A.pack = h->d_pack;
-  A.qpos = d_qpos; A.qvel = d_qvel; A.ctrl = d_ctrl; A.warmstart = warmstart ? d_warm : nullptr; A.mocap = d_mocap;
-  A.task_state = nts ? d_ts : nullptr; A.time = d_time; A.B = B;
-  A.qacc = d_qacc; A.next_qpos = d_nq; A.next_qvel = d_nv; A.residual = d_res; A.cost = d_cost; A.counts = (int*)d_counts;
-  const size_t smem = h->smem_bytes(1, 1);
-  const char* ns = std::getenv("MJPC_B200_NO_STATIC");
-  const bool use_static = h->static_spec != 0 && !(ns && ns[0] == '1');
-  const void* fn = use_static ? (h->static_spec == 1 ? (const void*)step_batch_kernel_quadruped : (const void*)step_batch_kernel_humanoid_track)
-                              : (const void*)step_batch_kernel;
-  if (int rc = set_smem(fn, smem)) return rc;
-  CUDA_TRY(cudaEventRecord(h->ev0, h->stream));
-  if (use_static && h->static_spec == 1) step_batch_kernel_quadruped<<<B, 32, smem, h->stream>>>(A);
-  else if (use_static) step_batch_kernel_humanoid_track<<<B, 32, smem, h->stream>>>(A);
-  else step_batch_kernel<<<B, 32, smem, h->stream>>>(A);
-  CUDA_TRY(cudaEventRecord(h->ev1, h->stream));
-  CUDA_TRY(cudaGetLastError());
-  h->launches += 1;
-  h->last_static = use_static ? 1 : 0;
-  CUDA_TRY(cudaStreamSynchronize(h->stream));
-  if (cudaEventElapsedTime(&h->last_ms, h->ev0, h->ev1) != cudaSuccess) cudaGetLastError();
-  if (qacc) CUDA_TRY(cudaMemcpy(qacc, d_qacc, B * nv * 4, cudaMemcpyDeviceToHost));
-  if (next_qpos) CUDA_TRY(cudaMemcpy(next_qpos, d_nq, B * nq * 4, cudaMemcpyDeviceToHost));
-  if (next_qvel) CUDA_TRY(cudaMemcpy(next_qvel, d_nv, B * nv * 4, cudaMemcpyDeviceToHost));
-  if (residual) CUDA_TRY(cudaMemcpy(residual, d_res, B * (size_t)M.num_residual * 4, cudaMemcpyDeviceToHost));
-  if (cost) CUDA_TRY(cudaMemcpy(cost, d_cost, (size_t)B * 4, cudaMemcpyDeviceToHost));
-  if (counts) CUDA_TRY(cudaMemcpy(counts, d_counts, (size_t)B * 16, cudaMemcpyDeviceToHost));
+  if (h->pack.M.nmocap && !mocap) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "step_batch: mocap required");
+  const KernelSet* k;
+  const int kind = pick_kernels(h, true, &k);
+  if (int rc = step_impl(h, k->step, B, qpos, qvel, ctrl, warmstart, mocap, time0, times, qacc, next_qpos, next_qvel,
+                         residual, cost, counts, nullptr, nullptr, nullptr, h->ev0, h->ev1))
+    return rc;
+  h->last_static = kind ? 1 : 0;
   return 0;
 }
 
@@ -982,20 +976,17 @@ static int model_derivatives_impl(mjpc_b200_t* h, int B, const float* x, const f
   std::vector<float> ts((size_t)B * nts), trel((size_t)B * H);
   // derivative sweeps use absolute-time task state rebased to each problem's own t[0]
   for (int b = 0; b < B; b++) {
-    const double* src = task_states ? task_states + b * nts : h->task_state.data();
     const double t0 = t[(size_t)b * H];
-    for (size_t i = 0; i < nts; i++) {
-      double v = src[i];
-      if (std::find(h->time_idx.begin(), h->time_idx.end(), (int)i) != h->time_idx.end()) v -= t0;
-      ts[b * nts + i] = (float)v;
-    }
+    rebase_task_state(h, task_states ? task_states + b * nts : nullptr, t0, ts.data() + b * nts);
     for (int i = 0; i < H; i++) trel[(size_t)b * H + i] = (float)(t[(size_t)b * H + i] - t0);
   }
   const std::vector<float> w = to_float(weights, (size_t)B * M.num_term), p = to_float(parameters, (size_t)B * M.num_parameters);
   const size_t smem = h->smem_bytes(1, 1);
-  if (ilqg_reserve(h->ilqg, M, B, smem, h->stream)) return fail(MJPC_B200_ERR_CUDA, "model_derivatives: out of device memory");
+  if (ilqg_reserve(h->ilqg, M, B, h->stream)) return fail(MJPC_B200_ERR_CUDA, "model_derivatives: out of device memory");
+  const KernelSet* k;
+  pick_kernels(h, true, &k);
   int launches = 0;
-  int rc = ilqg_model_derivatives(h->ilqg, M, h->d_pack, h->stream, B, x, u, trel.data(), mocaps, ts.data(),
+  int rc = ilqg_model_derivatives(h->ilqg, M, h->d_pack, h->stream, k->fd_center, k->fd_column, B, x, u, trel.data(), mocaps, ts.data(),
                                   weights ? w.data() : nullptr, parameters ? p.data() : nullptr, H, tol, A, B_, C, D,
                                   smem, &launches, h->ev0, h->ev1, skip, mode);
   h->launches += launches;
@@ -1032,7 +1023,7 @@ static int cost_derivatives_impl(mjpc_b200_t* h, int B, const double* weights, c
   if (cost_derivatives_smem(M, h->max_term_dim) > h->smem_optin)
     return fail(MJPC_B200_ERR_CAPACITY, "cost_derivatives: the widest cost term does not fit in shared memory");
   const std::vector<float> w = to_float(weights, (size_t)B * M.num_term);
-  if (ilqg_reserve(h->ilqg, M, B, h->smem_bytes(1, 1), h->stream)) return fail(MJPC_B200_ERR_CUDA, "cost_derivatives: out of device memory");
+  if (ilqg_reserve(h->ilqg, M, B, h->stream)) return fail(MJPC_B200_ERR_CUDA, "cost_derivatives: out of device memory");
   int launches = 0;
   int rc = ilqg_cost_derivatives(h->ilqg, M, h->d_pack, h->stream, B, weights ? w.data() : nullptr, residual, C, D, H,
                                  cx, cu, cxx, cuu, cxu, h->max_term_dim, &launches, h->ev0, h->ev1);
@@ -1064,7 +1055,7 @@ static int backward_pass_impl(mjpc_b200_t* h, int B, const float* A, const float
                               const float* mu, int reg_type, int limits, float* K, float* du, float* dV, float* Vx,
                               float* Vxx, int* status_out) {
   CUDA_TRY(cudaSetDevice(h->device));
-  if (ilqg_reserve(h->ilqg, h->pack.M, B, h->smem_bytes(1, 1), h->stream)) return fail(MJPC_B200_ERR_CUDA, "backward_pass: out of device memory");
+  if (ilqg_reserve(h->ilqg, h->pack.M, B, h->stream)) return fail(MJPC_B200_ERR_CUDA, "backward_pass: out of device memory");
   int launches = 0;
   int rc = ilqg_backward_pass(h->ilqg, h->pack.M, h->d_pack, h->stream, B, A, B_, cx, cu, cxx, cxu, cuu, actions, H, mu,
                               reg_type, limits, K, du, dV, Vx, Vxx, status_out, &launches, h->ev0, h->ev1);

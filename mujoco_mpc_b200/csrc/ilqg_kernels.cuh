@@ -167,32 +167,14 @@ __device__ __forceinline__ FdProb fd_problem(const Ctx& c, const FdArgs& A, int 
   return P;
 }
 
-// the problem's task snapshot overwrites the CTA's shared-memory pack copy (one problem per CTA), as in the rollout
-// prologue; then the state, control and mocap of step t
+// the problem's task snapshot, as in the rollout prologue; then the state, control and mocap of step t and the warm
+// start (NULL: zeros)
 template <class SP>
-__device__ __forceinline__ void fd_load_state(Ctx& c, const FdProb& P, int t) {
+__device__ __forceinline__ void fd_load_state(Ctx& c, const FdProb& P, int t, const float* warmstart) {
   auto&& M = SP::model(c);
-  const int lane = c.lane, nq = M.nq, nv = M.nv, ds = nq + nv;
-  if (P.task_state) {
-    float* ts = const_cast<float*>(MF(task_state));
-    for (int i = lane; i < M.task_state_size; i += 32) ts[i] = P.task_state[i];
-  }
-  if (P.weight) {
-    float* w = const_cast<float*>(MF(task_weight));
-    for (int i = lane; i < M.num_term; i += 32) w[i] = P.weight[i];
-  }
-  if (P.parameters) {
-    float* pr = const_cast<float*>(MF(task_parameters));
-    for (int i = lane; i < M.num_parameters; i += 32) pr[i] = P.parameters[i];
-  }
-  for (int i = lane; i < nq; i += 32) DF(qpos)[i] = P.x[(size_t)t * ds + i];
-  for (int i = lane; i < nv; i += 32) DF(qvel)[i] = P.x[(size_t)t * ds + nq + i];
-  for (int i = lane; i < M.nu; i += 32) DF(ctrl)[i] = P.u[(size_t)t * M.nu + i];
-  for (int i = lane; i < 7 * M.nmocap; i += 32) {
-    const int k = i / 7, q = i - 7 * k;
-    if (q < 3) DF(mocap_pos)[3 * k + q] = P.mocap[i]; else DF(mocap_quat)[4 * k + q - 3] = P.mocap[i];
-  }
-  for (int i = lane; i < nv * nv; i += 32) DF(qM)[i] = 0;
+  const size_t x = (size_t)t * (M.nq + M.nv);
+  load_task<SP>(c, 0, P.task_state, P.weight, P.parameters);
+  load_state<SP>(c, P.x + x, P.x + x + M.nq, P.u + (size_t)t * M.nu, warmstart, P.mocap);
   c.time = P.t[t];
   __syncwarp();
 }
@@ -206,9 +188,7 @@ __device__ __forceinline__ void fd_center_body(const FdArgs& A) {
   auto&& M = SP::model(c);
   const int lane = c.lane, t = A.eval_t[blockIdx.x], nq = M.nq, nv = M.nv, ds = nq + nv, nr = M.num_residual;
   const FdProb P = fd_problem<SP>(c, A, blockIdx.y);
-  fd_load_state<SP>(c, P, t);
-  for (int i = lane; i < nv; i += 32) DF(qacc_warmstart)[i] = 0;
-  __syncwarp();
+  fd_load_state<SP>(c, P, t, nullptr);
   k_forward<SP>(c);
   k_residual<SP>(c);
   for (int i = lane; i < nr; i += 32) P.r0[(size_t)t * nr + i] = DF(residual)[i];
@@ -263,9 +243,7 @@ __device__ __forceinline__ void fd_column_body(const FdArgs& A) {
   const bool last = t == A.H - 1;
   if (last && col < nu) return;  // only C is computed at the final time step (model_derivatives.cc:89-93)
   const FdProb P = fd_problem<SP>(c, A, blockIdx.y);
-  fd_load_state<SP>(c, P, t);
-  for (int i = lane; i < nv; i += 32) DF(qacc_warmstart)[i] = P.q0[(size_t)t * nv + i];
-  __syncwarp();
+  fd_load_state<SP>(c, P, t, P.q0 + (size_t)t * nv);
   float h = A.eps;  // signed step of a one-sided difference
   bool centred = A.mode == 1;
   if (col < nu) {
@@ -298,9 +276,7 @@ __device__ __forceinline__ void fd_column_body(const FdArgs& A) {
       for (int i = lane; i < nv; i += 32) yp[nq + i] = DF(qvel)[i];
     }
     __syncwarp();
-    fd_load_state<SP>(c, P, t);
-    for (int i = lane; i < nv; i += 32) DF(qacc_warmstart)[i] = P.q0[(size_t)t * nv + i];
-    __syncwarp();
+    fd_load_state<SP>(c, P, t, P.q0 + (size_t)t * nv);
     fd_perturb<SP>(c, col, nu, nv, -A.eps);
     k_forward<SP>(c);
     k_residual<SP>(c);
@@ -830,10 +806,18 @@ inline cudaError_t raise_smem_limit(const void* fn, size_t bytes) {
   return r;
 }
 
+// fn(A) on grid x block threads, as fn<<<grid, block, smem, st>>>(A) would launch it (a launch error surfaces at the
+// caller's cudaGetLastError)
+template <class Args>
+inline void launch_kernel(const void* fn, dim3 grid, int block, size_t smem, cudaStream_t st, const Args& A) {
+  void* args[] = {const_cast<Args*>(&A)};
+  cudaLaunchKernel(fn, grid, dim3(block), args, smem, st);
+}
+
 // Device buffers of the iLQG sweeps for up to `nprob` problems of max_horizon rows each (per-problem arrays are
 // [nprob][H][..]); sized for one problem at create, grown by ilqg_reserve when a batched sweep needs more.
 struct IlqgBuffers {
-  int H = 0, ds = 0, n = 0, nu = 0, nr = 0, nv = 0, static_spec = 0, nprob = 0;
+  int H = 0, ds = 0, n = 0, nu = 0, nr = 0, nv = 0, nprob = 0;
   float *x = nullptr, *u = nullptr, *t = nullptr, *mocap = nullptr, *ts = nullptr, *w = nullptr, *prm = nullptr,
         *y0 = nullptr, *r0 = nullptr, *q0 = nullptr, *A = nullptr, *B = nullptr, *C = nullptr, *D = nullptr,
         *res = nullptr, *cx = nullptr, *cu = nullptr, *cxx = nullptr, *cuu = nullptr, *cxu = nullptr, *act = nullptr,
@@ -854,7 +838,7 @@ inline void ilqg_free(IlqgBuffers& b) {
 }
 
 // allocates everything for nprob problems; on failure the partly allocated buffers are freed and -4 returned
-inline int ilqg_init(IlqgBuffers& b, const DevModel& M, int H, size_t smem_fd, int nprob = 1) {
+inline int ilqg_init(IlqgBuffers& b, const DevModel& M, int H, int nprob = 1) {
   b.H = H; b.nv = M.nv; b.ds = M.nq + M.nv; b.n = 2 * M.nv; b.nu = M.nu; b.nr = M.num_residual; b.nprob = nprob;
   const size_t Hs = H, n = b.n, m = b.nu, nr = b.nr, ds = b.ds, P = nprob;
   struct { float** p; size_t cnt; } plan[] = {
@@ -870,22 +854,15 @@ inline int ilqg_init(IlqgBuffers& b, const DevModel& M, int H, size_t smem_fd, i
     ok = ok && cudaMalloc((void**)e.p, (e.cnt ? e.cnt : 1) * sizeof(float)) == cudaSuccess;
   ok = ok && cudaMalloc((void**)&b.status, P * sizeof(int)) == cudaSuccess;
   ok = ok && cudaMalloc((void**)&b.idx, (4 * Hs + 8) * sizeof(int)) == cudaSuccess;
-  ok = ok && raise_smem_limit((const void*)fd_center_kernel, smem_fd) == cudaSuccess;
-  ok = ok && raise_smem_limit((const void*)fd_column_kernel, smem_fd) == cudaSuccess;
-  b.static_spec = spec_matches<SpecQuadruped>(M, make_layout(M, 1)) ? 1 : 0;
-  if (b.static_spec) {
-    ok = ok && raise_smem_limit((const void*)fd_center_kernel_quadruped, smem_fd) == cudaSuccess;
-    ok = ok && raise_smem_limit((const void*)fd_column_kernel_quadruped, smem_fd) == cudaSuccess;
-  }
   if (!ok) { cudaGetLastError(); ilqg_free(b); return -4; }
   return 0;
 }
 
 // grow b to hold nprob problems (never shrinks).  On an allocation failure b keeps its old buffers and stays usable.
-inline int ilqg_reserve(IlqgBuffers& b, const DevModel& M, int nprob, size_t smem_fd, cudaStream_t st) {
+inline int ilqg_reserve(IlqgBuffers& b, const DevModel& M, int nprob, cudaStream_t st) {
   if (nprob <= b.nprob) return 0;
   IlqgBuffers nb;
-  if (int rc = ilqg_init(nb, M, b.H, smem_fd, nprob)) return rc;
+  if (int rc = ilqg_init(nb, M, b.H, nprob)) return rc;
   if (cudaStreamSynchronize(st) != cudaSuccess) { cudaGetLastError(); ilqg_free(nb); return -4; }
   ilqg_free(b);
   b = nb;
@@ -894,9 +871,11 @@ inline int ilqg_reserve(IlqgBuffers& b, const DevModel& M, int nprob, size_t sme
 
 #define ILQG_TRY(e) do { if ((e) != cudaSuccess) { cudaGetLastError(); return -4; } } while (0)
 
-// nprob problems with common H / skip / mode.  Host inputs are [nprob][..]: x, u, trel (relative to each problem's
-// t[0]), mocap, ts (rebased likewise); w / prm (float weights / parameters) may be nullptr for the packed values.
-inline int ilqg_model_derivatives(IlqgBuffers& b, const DevModel& M, const float* d_pack, cudaStream_t st, int nprob,
+// nprob problems with common H / skip / mode, on the fd_center / fd_column instances given.  Host inputs are [nprob][..]:
+// x, u, trel (relative to each problem's t[0]), mocap, ts (rebased likewise); w / prm (float weights / parameters) may
+// be nullptr for the packed values.
+inline int ilqg_model_derivatives(IlqgBuffers& b, const DevModel& M, const float* d_pack, cudaStream_t st,
+                                  const void* fd_center, const void* fd_column, int nprob,
                                   const float* x, const float* u, const float* trel, const float* mocap, const float* ts,
                                   const float* w, const float* prm, int H, float eps, float* A, float* B, float* C,
                                   float* D, size_t smem, int* launches, cudaEvent_t e0 = nullptr, cudaEvent_t e1 = nullptr,
@@ -953,16 +932,9 @@ inline int ilqg_model_derivatives(IlqgBuffers& b, const DevModel& M, const float
   a.task_state = M.task_state_size ? b.ts : nullptr; a.H = H; a.eps = eps; a.y0 = b.y0; a.r0 = b.r0; a.q0 = b.q0;
   a.weight = (w && M.num_term) ? b.w : nullptr; a.parameters = (prm && M.num_parameters) ? b.prm : nullptr;
   a.A = b.A; a.B = b.B; a.C = b.C; a.D = b.D;
-  const char* ns = std::getenv("MJPC_B200_NO_STATIC");
-  const dim3 gc(neval, nprob), gk(neval * (M.nu + 2 * M.nv), nprob);
   if (e0) ILQG_TRY(cudaEventRecord(e0, st));   // kernel-only span (copies and memsets stay outside)
-  if (b.static_spec == 1 && !(ns && ns[0] == '1')) {
-    fd_center_kernel_quadruped<<<gc, 32, smem, st>>>(a);
-    fd_column_kernel_quadruped<<<gk, 32, smem, st>>>(a);
-  } else {
-    fd_center_kernel<<<gc, 32, smem, st>>>(a);
-    fd_column_kernel<<<gk, 32, smem, st>>>(a);
-  }
+  launch_kernel(fd_center, dim3(neval, nprob), 32, smem, st, a);
+  launch_kernel(fd_column, dim3(neval * (M.nu + 2 * M.nv), nprob), 32, smem, st, a);
   *launches += 2;
   if (ninterp) {
     FdInterpArgs ia;

@@ -4,7 +4,7 @@
 //                       (Trajectory::Rollout / RolloutDiscrete,
 //                       mjpc/trajectory.cc:92-309) incl. policy, mj_step restatement, residual, cost, return
 //   rank_kernel         order of each problem's candidates by return (partial_sort, sampling/planner.cc:184-188)
-//   step_debug_kernel   a single forward+Euler step through the same device functions (parity hook)
+//   step_batch_kernel   independent single forward+Euler steps through the same device functions (parity hooks)
 //   fd_*_kernel         finite-difference transition/residual Jacobians (model_derivatives.cc:45-165)
 //
 // Shared memory per CTA: [model pack (floats | ints)] [warp 0 data] [warp 1 data] ...
@@ -102,6 +102,44 @@ __device__ __forceinline__ void init_ctx(Ctx& c, const DevModel* M, const DevLay
 #endif
 }
 
+// row `prob` of a problem's task snapshot over the CTA's shared-memory copy of the pack; a NULL array keeps the packed
+// values.  The copy is per CTA and a CTA never holds two problems, so every warp of it may write the same values.
+template <class SP>
+__device__ __forceinline__ void load_task(Ctx& c, int prob, const float* task_state, const float* weight,
+                                          const float* parameters) {
+  auto&& M = SP::model(c);
+  const int lane = c.lane;
+  if (task_state) {
+    float* ts = const_cast<float*>(MF(task_state));
+    for (int i = lane; i < M.task_state_size; i += 32) ts[i] = task_state[(size_t)prob * M.task_state_size + i];
+  }
+  if (weight) {
+    float* w = const_cast<float*>(MF(task_weight));
+    for (int i = lane; i < M.num_term; i += 32) w[i] = weight[(size_t)prob * M.num_term + i];
+  }
+  if (parameters) {
+    float* pr = const_cast<float*>(MF(task_parameters));
+    for (int i = lane; i < M.num_parameters; i += 32) pr[i] = parameters[(size_t)prob * M.num_parameters + i];
+  }
+}
+
+// the state a single step starts from: qpos, qvel, ctrl, the warm start (NULL: zeros) and the mocap poses ([nmocap][7]
+// split into pos and quat); qM is zeroed
+template <class SP>
+__device__ __forceinline__ void load_state(Ctx& c, const float* qpos, const float* qvel, const float* ctrl,
+                                           const float* warmstart, const float* mocap) {
+  auto&& M = SP::model(c);
+  const int lane = c.lane, nv = M.nv;
+  for (int i = lane; i < M.nq; i += 32) DF(qpos)[i] = qpos[i];
+  for (int i = lane; i < nv; i += 32) { DF(qvel)[i] = qvel[i]; DF(qacc_warmstart)[i] = warmstart ? warmstart[i] : 0.f; }
+  for (int i = lane; i < M.nu; i += 32) DF(ctrl)[i] = ctrl[i];
+  for (int i = lane; i < 7 * M.nmocap; i += 32) {
+    const int k = i / 7, q = i - 7 * k;
+    if (q < 3) DF(mocap_pos)[3 * k + q] = mocap[i]; else DF(mocap_quat)[4 * k + q - 3] = mocap[i];
+  }
+  for (int i = lane; i < nv * nv; i += 32) DF(qM)[i] = 0;
+}
+
 // write the trace points (GetTraces, mjpc/utilities.cc:268-285)
 template <class SP>
 __device__ __forceinline__ void write_traces(Ctx& c, float* out) {
@@ -196,22 +234,11 @@ __device__ __forceinline__ void rollout_body(const RolloutArgs& A) {
   const double time0 = A.time0[prob];
   const float* state = A.state + (size_t)prob * ds;
   const float* mocap = A.mocap + (size_t)prob * 7 * M.nmocap;
-  // the problem's task snapshot (task state time-rebased) overrides the packed copy: the pack in shared memory is per
-  // CTA and a CTA never holds two problems, so every warp of it writes the same values.  With a task warp this happens
+  // the problem's task snapshot (task state time-rebased) overrides the packed copy.  With a task warp this happens
   // before its first fork, where it starts to read them.
-  if (A.task_state) {
-    float* ts = const_cast<float*>(MF(task_state));
-    for (int i = lane; i < M.task_state_size; i += 32) ts[i] = A.task_state[(size_t)prob * M.task_state_size + i];
-  }
-  if (A.weight) {
-    float* w = const_cast<float*>(MF(task_weight));
-    for (int i = lane; i < M.num_term; i += 32) w[i] = A.weight[(size_t)prob * M.num_term + i];
-  }
-  if (A.parameters) {
-    float* pr = const_cast<float*>(MF(task_parameters));
-    for (int i = lane; i < M.num_parameters; i += 32) pr[i] = A.parameters[(size_t)prob * M.num_parameters + i];
-  }
+  load_task<SP>(c, prob, A.task_state, A.weight, A.parameters);
   // ---- initial conditions (trajectory.cc:108-137)
+  // (written out rather than through load_state: through the helper the rollout kernels compile to different SASS)
   for (int i = lane; i < nq; i += 32) DF(qpos)[i] = state[i];
   for (int i = lane; i < nv; i += 32) { DF(qvel)[i] = state[nq + i]; DF(qacc_warmstart)[i] = 0; }
   for (int i = lane; i < 7 * M.nmocap; i += 32) {
@@ -408,63 +435,10 @@ extern "C" __global__ void rank_kernel(const float* __restrict__ ret, int N, int
   }
 }
 
-struct DebugArgs {
-  DevModel M;
-  DevLayout L;
-  const float* pack;
-  const float* qpos; const float* qvel; const float* ctrl; const float* mocap; const float* warmstart;
-  const float* task_state;
-  float time;
-  float* qacc; float* residual; float* next_qpos; float* next_qvel; float* qM; float* efc_force; int* counts;
-  float* contact;   // [maxcon][8]: dist, pos[3], normal[3], dim of the geometric contacts
-};
-
-extern "C" __global__ void __launch_bounds__(32) step_debug_kernel(const __grid_constant__ DebugArgs A) {
-  using SP = DynSpec;
-  extern __shared__ __align__(16) float smem[];
-  const DevModel& M = A.M;
-  stage_model_pack(smem, A.pack, (unsigned)((M.nf + M.ni) * 4));
-  Ctx c;
-  init_ctx(c, &A.M, &A.L, smem, 0, threadIdx.x, A.pack);
-  const int lane = c.lane, nq = M.nq, nv = M.nv;
-  if (A.task_state) {
-    float* ts = const_cast<float*>(MF(task_state));
-    for (int i = lane; i < M.task_state_size; i += 32) ts[i] = A.task_state[i];
-  }
-  for (int i = lane; i < nq; i += 32) DF(qpos)[i] = A.qpos[i];
-  for (int i = lane; i < nv; i += 32) { DF(qvel)[i] = A.qvel[i]; DF(qacc_warmstart)[i] = A.warmstart ? A.warmstart[i] : 0.f; }
-  for (int i = lane; i < M.nu; i += 32) DF(ctrl)[i] = A.ctrl[i];
-  for (int i = lane; i < 7 * M.nmocap; i += 32) {
-    const int k = i / 7, q = i - 7 * k;
-    if (q < 3) DF(mocap_pos)[3 * k + q] = A.mocap[i]; else DF(mocap_quat)[4 * k + q - 3] = A.mocap[i];
-  }
-  for (int i = lane; i < nv * nv; i += 32) DF(qM)[i] = 0;
-  c.time = A.time;
-  __syncwarp();
-  k_forward<SP>(c);
-  k_residual<SP>(c);
-  if (k_bad(c, DF(qacc), nv)) c.warn = 1;
-  for (int i = lane; i < nv; i += 32) A.qacc[i] = DF(qacc)[i];
-  for (int i = lane; i < nv * nv; i += 32) A.qM[i] = DF(qM)[i];
-  for (int i = lane; i < M.num_residual; i += 32) A.residual[i] = DF(residual)[i];
-  for (int i = lane; i < c.nefc; i += 32) A.efc_force[i] = DF(efc_force)[i];
-  if (lane == 0) { A.counts[0] = c.ncon - c.npseudo; A.counts[1] = c.nefc; A.counts[2] = c.niter; A.counts[3] = c.warn; }
-  for (int i = lane; i < c.ncon - c.npseudo; i += 32) {
-    float* o = A.contact + 8 * i;
-    o[0] = DF(con_dist)[i];
-    for (int q = 0; q < 3; q++) { o[1 + q] = DF(con_pos)[3 * i + q]; o[4 + q] = DF(con_frame)[9 * i + q]; }
-    const int d = DI(con_dim)[i];   // the pyramidal constraint phase rewrites it as the row count 2 (dim - 1)
-    o[7] = (float)(M.cone == CONE_PYRAMIDAL && d > 1 ? d / 2 + 1 : d);
-  }
-  k_euler<SP>(c);
-  for (int i = lane; i < nq; i += 32) A.next_qpos[i] = DF(qpos)[i];
-  for (int i = lane; i < nv; i += 32) A.next_qvel[i] = DF(qvel)[i];
-}
-
-
-// Batched parity hook: B independent (qpos, qvel, ctrl, warm start, time) tuples, each advanced by ONE mj_step through
-// the same device functions - and the same static / generic instances - the rollout kernel runs.  Teacher-forced
-// per-step parity tests feed it the oracle's own states, so a mismatch cannot be blamed on trajectory divergence.
+// Single-step parity hook: B independent (qpos, qvel, ctrl, warm start, time) tuples, each advanced by ONE mj_step
+// through the same device functions - and the same static / generic instances - the rollout kernel runs.
+// Teacher-forced per-step parity tests feed it the oracle's own states, so a mismatch cannot be blamed on trajectory
+// divergence.
 struct StepBatchArgs {
   DevModel M;
   DevLayout L;
@@ -474,6 +448,9 @@ struct StepBatchArgs {
   const float* time;    // [B], relative to the rollout start the task state was rebased to
   int B;
   float* qacc; float* next_qpos; float* next_qvel; float* residual; float* cost; int* counts;   // counts [B][4]
+  // optional (NULL: not written): qM [B][nv nv], efc_force [B][maxefc], contact [B][maxcon][8] = dist, pos[3],
+  // normal[3], dim of the geometric contacts
+  float* qM; float* efc_force; float* contact;
 };
 
 template <class SP>
@@ -486,21 +463,9 @@ __device__ __forceinline__ void step_batch_body(const StepBatchArgs& A) {
   const int lane = c.lane, nq = M.nq, nv = M.nv, nu = M.nu, nr = M.num_residual;
   const int b = blockIdx.x;
   if (b >= A.B) return;
-  if (A.task_state) {
-    float* ts = const_cast<float*>(MF(task_state));
-    for (int i = lane; i < M.task_state_size; i += 32) ts[i] = A.task_state[i];
-  }
-  for (int i = lane; i < nq; i += 32) DF(qpos)[i] = A.qpos[(size_t)b * nq + i];
-  for (int i = lane; i < nv; i += 32) {
-    DF(qvel)[i] = A.qvel[(size_t)b * nv + i];
-    DF(qacc_warmstart)[i] = A.warmstart ? A.warmstart[(size_t)b * nv + i] : 0.f;
-  }
-  for (int i = lane; i < nu; i += 32) DF(ctrl)[i] = A.ctrl[(size_t)b * nu + i];
-  for (int i = lane; i < 7 * M.nmocap; i += 32) {
-    const int k = i / 7, q = i - 7 * k;
-    if (q < 3) DF(mocap_pos)[3 * k + q] = A.mocap[i]; else DF(mocap_quat)[4 * k + q - 3] = A.mocap[i];
-  }
-  for (int i = lane; i < nv * nv; i += 32) DF(qM)[i] = 0;
+  load_task<SP>(c, 0, A.task_state, nullptr, nullptr);
+  load_state<SP>(c, A.qpos + (size_t)b * nq, A.qvel + (size_t)b * nv, A.ctrl + (size_t)b * nu,
+                 A.warmstart ? A.warmstart + (size_t)b * nv : nullptr, A.mocap);
   for (int i = lane; i < 6 * M.nbody; i += 32) DF(xfrc)[i] = 0;
   c.time = A.time[b];
   __syncwarp();
@@ -508,12 +473,25 @@ __device__ __forceinline__ void step_batch_body(const StepBatchArgs& A) {
   k_residual<SP>(c);
   if (k_bad(c, DF(qacc), nv)) c.warn = 1;
   const float cost = k_cost_value<SP>(c);
+  const int ncon = c.ncon - c.npseudo;
   for (int i = lane; i < nv; i += 32) A.qacc[(size_t)b * nv + i] = DF(qacc)[i];
   for (int i = lane; i < nr; i += 32) A.residual[(size_t)b * nr + i] = DF(residual)[i];
   if (lane == 0) {
     A.cost[b] = cost;
-    A.counts[4 * b] = c.ncon - c.npseudo; A.counts[4 * b + 1] = c.nefc; A.counts[4 * b + 2] = c.niter; A.counts[4 * b + 3] = c.warn;
+    A.counts[4 * b] = ncon; A.counts[4 * b + 1] = c.nefc; A.counts[4 * b + 2] = c.niter; A.counts[4 * b + 3] = c.warn;
   }
+  if (A.qM)
+    for (int i = lane; i < nv * nv; i += 32) A.qM[(size_t)b * nv * nv + i] = DF(qM)[i];
+  if (A.efc_force)
+    for (int i = lane; i < c.nefc; i += 32) A.efc_force[(size_t)b * M.maxefc + i] = DF(efc_force)[i];
+  if (A.contact)
+    for (int i = lane; i < ncon; i += 32) {
+      float* o = A.contact + ((size_t)b * M.maxcon + i) * 8;
+      o[0] = DF(con_dist)[i];
+      for (int q = 0; q < 3; q++) { o[1 + q] = DF(con_pos)[3 * i + q]; o[4 + q] = DF(con_frame)[9 * i + q]; }
+      const int d = DI(con_dim)[i];   // the pyramidal constraint phase rewrites it as the row count 2 (dim - 1)
+      o[7] = (float)(M.cone == CONE_PYRAMIDAL && d > 1 ? d / 2 + 1 : d);
+    }
   for (int i = lane; i < nv; i += 32) DF(qacc_warmstart)[i] = DF(qacc)[i];
   k_euler<SP>(c);
   for (int i = lane; i < nq; i += 32) A.next_qpos[(size_t)b * nq + i] = DF(qpos)[i];
