@@ -224,6 +224,46 @@ int mjpc_b200_step_batch(mjpc_b200_t* h, int B, const float* qpos, const float* 
                          const float* warmstart, const float* mocap, double time0, const double* times, float* qacc,
                          float* next_qpos, float* next_qvel, float* residual, float* cost, int* counts);
 
+/* The sigma-point step of a state estimator: B states [B][dim_state], all from the same ctrl [nu], mocap and absolute
+ * time, are each advanced by one mj_step through the kernel instance mjpc_b200_step_batch runs, and the measurement
+ * sensors [sensor_start, sensor_start + nsensor) of each PRE-step state are evaluated after the constraint solve
+ * (positions, velocities and touch forces of the state the step starts from, as mj_step's sensor stage sees them).
+ * Evaluated: jointpos / jointvel of slide and hinge joints, framepos of a site, body (xipos), xbody (xpos) or geom,
+ * and touch with a sphere site zone.  warmstart [B][nv] may be NULL (zeros); mocap [7 nmocap] is required when
+ * nmocap > 0.  Outputs: next_states [B][dim_state], sensordata [B][dim] (dim = the range's total sensor dimension),
+ * and, when not NULL, qacc [B][nv] and counts [B][4] = {ncon, nefc, solver iterations, warning}, all equal to what
+ * mjpc_b200_step_batch returns for the same inputs.  last_kernel_ms times the launch.  A range outside the model's
+ * sensors: MJPC_B200_ERR_BAD_ARGUMENT; a sensor in it that is not evaluated: MJPC_B200_ERR_UNSUPPORTED;
+ * B > max_candidates: MJPC_B200_ERR_CAPACITY.  Device and pinned buffers are the handle's (no allocation per call
+ * once the largest B has been seen). */
+int mjpc_b200_step_sensors(mjpc_b200_t* h, int B, const float* states, const float* ctrl, const float* warmstart,
+                           const float* mocap, double time, int sensor_start, int nsensor, float* next_states,
+                           float* sensordata, float* qacc, int* counts);
+
+/* MJPC's Unscented state estimator (mjpc/estimators/unscented.cc, class mjpc_b200_host::Unscented in
+ * csrc/host/unscented.h): the filter in double precision on the host, its 2 ndstate + 1 sigma-point steps as one
+ * mjpc_b200_step_sensors launch on an engine handle it owns (max_candidates = nsigma).  Settings are explicit (the
+ * reference's defaults: alpha 1, beta 2, timestep = estimator_timestep or opt.timestep, the three noise scales 1e-4).
+ * create: measured sensors [sensor_start, sensor_start + nsensor) of the blob.  reset: state NULL -> the model's
+ * first keyframe, else qpos0 and zero qvel; covariance = covariance_scale I, diagonal process / sensor noise.
+ * set_noise: process [ndstate], sensor [nsensordata] (NULL keeps one).  set: state, covariance [ndstate^2] (NULL keeps
+ * one) and time.  update: ctrl [nu], the measured sensor slice [nsensordata], mocap [7 nmocap] or NULL (the model's);
+ * a failed covariance or sensor-covariance factorisation returns MJPC_B200_ERR_BAD_ARGUMENT and leaves state,
+ * covariance and time untouched (unscented_last_error names the factor).  get: state [nq+nv], covariance, time and
+ * scalars[5] = {ndstate, nsigma, nsensordata, sigma-point steps that raised a warning since reset, timestep}. */
+typedef struct mjpc_b200_unscented mjpc_b200_unscented_t;
+int mjpc_b200_unscented_create(const mjpc_model_blob* model, int sensor_start, int nsensor, double timestep,
+                               double alpha, double beta, int device, mjpc_b200_unscented_t** out);
+void mjpc_b200_unscented_destroy(mjpc_b200_unscented_t* u);
+int mjpc_b200_unscented_reset(mjpc_b200_unscented_t* u, const double* state, double time, double covariance_scale,
+                              double process_scale, double sensor_scale);
+int mjpc_b200_unscented_set_noise(mjpc_b200_unscented_t* u, const double* process, const double* sensor);
+int mjpc_b200_unscented_set(mjpc_b200_unscented_t* u, const double* state, const double* covariance, double time);
+int mjpc_b200_unscented_update(mjpc_b200_unscented_t* u, const double* ctrl, const double* sensor, const float* mocap);
+int mjpc_b200_unscented_get(const mjpc_b200_unscented_t* u, double* state, double* covariance, double* time,
+                            double* scalars);
+const char* mjpc_b200_unscented_last_error(const mjpc_b200_unscented_t* u);
+
 /* Per-candidate execution statistics of the last rollout, stats [N][12] = {SM cycles, Newton iterations, contacts,
  * constraint rows (summed over steps), 8 per-phase cycle counters (zero unless built with -DMJPC_PHASE_TIMING)}. */
 int mjpc_b200_fetch_stats(mjpc_b200_t* h, int64_t* stats);

@@ -24,7 +24,7 @@ _INT_SCALARS = ["nq", "nv", "nu", "na", "nbody", "njnt", "ngeom", "nsite", "nmoc
                 "nsensordata", "npair", "ntendon", "opt_cone", "opt_iterations", "opt_ls_iterations", "opt_integrator",
                 "opt_disable_contact", "opt_disable_eulerdamp", "opt_disable_frictionloss", "opt_disable_limit",
                 "opt_disable_refsafe", "opt_disable_warmstart", "task_num_term", "task_num_residual",
-                "task_num_trace", "task_residual_id"]
+                "task_num_trace", "task_residual_id", "nsensor"]
 _F_SCALARS = ["opt_timestep", "opt_impratio", "opt_tolerance", "opt_ls_tolerance", "stat_meaninertia", "task_risk"]
 _INT_ARRAYS = ["body_parentid", "body_rootid", "body_weldid", "body_jntnum", "body_jntadr", "body_dofnum",
                "body_dofadr", "body_mocapid", "body_depth", "jnt_type", "jnt_qposadr", "jnt_dofadr", "jnt_bodyid",
@@ -33,7 +33,7 @@ _INT_ARRAYS = ["body_parentid", "body_rootid", "body_weldid", "body_jntnum", "bo
                "actuator_biastype", "actuator_ctrllimited", "actuator_forcelimited", "pair_geom1", "pair_geom2",
                "task_dim_norm_residual", "task_norm", "task_num_norm_parameter", "task_trace_objtype",
                "task_trace_objid", "task_ids", "ray_geoms", "tendon_adr", "tendon_num", "tendon_limited", "wrap_dof",
-               "wrap_qposadr"]
+               "wrap_qposadr", "sensor_type", "sensor_objtype", "sensor_objid", "sensor_dim", "sensor_adr", "site_type"]
 _F_ARRAYS = ["opt_gravity", "body_pos", "body_quat", "body_ipos", "body_iquat", "body_mass", "body_inertia",
              "body_subtreemass", "body_invweight0", "jnt_pos", "jnt_axis", "jnt_range", "jnt_stiffness",
              "jnt_margin", "jnt_solref", "jnt_solimp", "qpos0", "qpos_spring", "dof_damping", "dof_armature",
@@ -42,7 +42,7 @@ _F_ARRAYS = ["opt_gravity", "body_pos", "body_quat", "body_ipos", "body_iquat", 
              "geom_rbound", "site_pos", "site_quat", "actuator_gear", "actuator_gainprm", "actuator_biasprm",
              "actuator_ctrlrange", "actuator_forcerange", "key_qpos", "key_qvel", "key_ctrl", "key_mpos",
              "key_mquat", "task_weight", "task_norm_parameter", "task_parameters", "task_state", "wrap_coef",
-             "tendon_range", "tendon_margin", "tendon_solref", "tendon_solimp", "tendon_invweight0"]
+             "tendon_range", "tendon_margin", "tendon_solref", "tendon_solimp", "tendon_invweight0", "site_size", "sensor_cutoff"]
 
 
 def to_blob(model) -> bytes:

@@ -40,7 +40,8 @@ def _compile(verbose):
                                                                            os.path.join(CSRC, "host", "robust_planner.cc"),
                                                                            os.path.join(CSRC, "host", "gradient_planner.cc"),
                                                                            os.path.join(CSRC, "host", "agent.cc"),
-                                                                           os.path.join(CSRC, "host", "task_transition.cc")]
+                                                                           os.path.join(CSRC, "host", "task_transition.cc"),
+                                                                           os.path.join(CSRC, "host", "unscented.cc")]
     subprocess.check_call(cmd, cwd=CSRC)
 
 

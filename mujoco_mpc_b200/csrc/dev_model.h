@@ -64,7 +64,8 @@ enum { JNT_FREE = 0, JNT_BALL, JNT_SLIDE, JNT_HINGE };
 enum { OBJ_BODY = 0, OBJ_XBODY, OBJ_GEOM, OBJ_SITE };
 enum { CONE_PYRAMIDAL = 0, CONE_ELLIPTIC = 1 };
 enum { RESIDUAL_PARTICLE = 0, RESIDUAL_PARTICLE_COPY = 1, RESIDUAL_CARTPOLE = 2, RESIDUAL_QUADRUPED_FLAT = 3,
-       RESIDUAL_HUMANOID_STAND = 4, RESIDUAL_HUMANOID_TRACK = 5, RESIDUAL_SHADOW_REORIENT = 6 };
+       RESIDUAL_HUMANOID_STAND = 4, RESIDUAL_HUMANOID_TRACK = 5, RESIDUAL_SHADOW_REORIENT = 6,
+       RESIDUAL_NONE = 7 /* no cost terms: k_residual writes nothing */ };
 
 // integer fields of the header (sizes, option flags, task dimensions, pack sizes).  A statically specialised
 // kernel (spec_*.h) turns every one of them, and the offset tables below, into compile-time constants.

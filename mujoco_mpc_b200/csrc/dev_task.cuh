@@ -660,4 +660,63 @@ __device__ __noinline__ void k_residual(Ctx& c) {
   }
 }
 
+// ------------------------------------------------------------------------------------------ measurement sensors
+// MuJoCo's sensor types the estimators measure (codes of mujoco_mpc_b200/mjcf.py SENS_*).  One row of the handle's
+// sensor table per sensor (built on the host from the blob's sensor_* / site_* entries, never part of the model pack):
+// adr is the sensor's sensordata address, radius the sphere zone of a touch sensor's site.
+enum { SENS_FRAMEPOS = 1, SENS_JOINTPOS = 2, SENS_TOUCH = 3, SENS_JOINTVEL = 9 };
+struct DevSensor { int type, objtype, objid, adr; float radius; };
+
+// Sensors [0, n) of `tab`, written to out[adr - adr0 ..].  Runs after k_forward and before k_euler: positions and
+// velocities are those of the pre-step state, touch reads the constraint forces of that state's solve (as mj_step's
+// sensor stage does).  One sensor per lane.
+//   jointpos / jointvel  qpos[jnt_qposadr] / qvel[jnt_dofadr] of a slide or hinge joint
+//   framepos             site_xpos, xipos (body), xpos (xbody) or geom_xpos, world frame
+//   touch                the normal forces of the contacts with constraint rows that involve a geom of the site's
+//                        body, counted when the contact point lies in the site's sphere or the ray from the point
+//                        along the contact normal, oriented into the site's body, hits it.  The normal force is the
+//                        normal row's force (elliptic, frictionless) or the sum of the 2 (condim - 1) pyramid edge
+//                        forces; the constraint phase has rewritten con_dim of a pyramidal contact as that row count.
+template <class SP>
+__device__ __noinline__ void k_sensors(Ctx& c, const DevSensor* __restrict__ tab, int n, int adr0, float* out) {
+  auto&& M = SP::model(c);
+  const int ncon = c.ncon - c.npseudo;
+  for (int s = c.lane; s < n; s += 32) {
+    const DevSensor S = tab[s];
+    float* o = out + (S.adr - adr0);
+    if (S.type == SENS_JOINTPOS) {
+      o[0] = DF(qpos)[MI(jnt_qposadr)[S.objid]];
+    } else if (S.type == SENS_JOINTVEL) {
+      o[0] = DF(qvel)[MI(jnt_dofadr)[S.objid]];
+    } else if (S.type == SENS_FRAMEPOS) {
+      const float* p = S.objtype == OBJ_SITE ? DF(site_xpos) : S.objtype == OBJ_GEOM ? DF(geom_xpos)
+                       : S.objtype == OBJ_XBODY ? DF(xpos) : DF(xipos);
+      for (int q = 0; q < 3; q++) o[q] = p[3 * S.objid + q];
+    } else if (S.type == SENS_TOUCH) {
+      const int body = MI(site_bodyid)[S.objid];
+      const float* ctr = DF(site_xpos) + 3 * S.objid;
+      const float r2 = S.radius * S.radius;
+      float sum = 0.f;
+      for (int i = 0; i < ncon; i++) {
+        const int adr = DI(con_adr)[i];
+        const int b1 = MI(geom_bodyid)[DI(con_g1)[i]], b2 = MI(geom_bodyid)[DI(con_g2)[i]];
+        if (adr < 0 || (b1 != body && b2 != body)) continue;
+        float f = DF(efc_force)[adr];
+        if (M.cone == CONE_PYRAMIDAL)
+          for (int k = 1; k < DI(con_dim)[i]; k++) f += DF(efc_force)[adr + k];
+        if (!(f > 0.f)) continue;
+        // the normal points from geom 1 into geom 2: into the site's body when that body is geom 2's
+        const float sg = b2 == body ? 1.f : -1.f;
+        float oc[3], dir[3];
+        for (int q = 0; q < 3; q++) { oc[q] = DF(con_pos)[3 * i + q] - ctr[q]; dir[q] = sg * DF(con_frame)[9 * i + q]; }
+        const float cc = dot3(oc, oc) - r2, b = dot3(oc, dir);
+        // inside the sphere, or the ray p + t dir (t >= 0, |dir| = 1) enters it
+        if (cc <= 0.f || (b < 0.f && b * b - cc >= 0.f)) sum += f;
+      }
+      o[0] = sum;
+    }
+  }
+  __syncwarp();
+}
+
 }  // namespace mjpc_dev

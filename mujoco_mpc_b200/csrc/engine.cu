@@ -117,6 +117,15 @@ struct mjpc_b200 {
   int maxTotal = 0;
   int nuserdata = 0;
   int differentiable = 0;   // MakeDifferentiable (utilities.cc:60-75) for the following launches (DevModel::differentiable)
+  // measurement sensors (k_sensors): one table row per model sensor; sensor_why[i] is empty when sensor i is one the
+  // device evaluates, else the reason it is not
+  std::vector<DevSensor> sensors;
+  std::vector<std::string> sensor_why;
+  DevSensor* d_sensors = nullptr;
+  // persistent scratch of step_impl: device buffer and its pinned host staging, grown on demand
+  float* d_step = nullptr;
+  float* h_step = nullptr;
+  size_t step_words = 0;
   // resident-input launch description
   RolloutArgs resident;
   bool resident_ok = false;
@@ -407,6 +416,38 @@ int mjpc_b200_create(const mjpc_model_blob* model, int max_candidates, int max_h
     for (int d : b.ints("task_dim_norm_residual")) h->max_term_dim = std::max(h->max_term_dim, d);
   }
   h->time_idx = time_like_state(M.residual_id);
+  {
+    // the measurement-sensor table; a blob without the sensor / site entries has no measurable sensors
+    Blob b(model->data, model->nbytes);
+    int dt, cnt; int64_t off;
+    if (b.find("nsensor", &dt, &cnt, &off) && b.find("site_size", &dt, &cnt, &off)) {
+      const std::vector<int> ty = b.ints("sensor_type"), ot = b.ints("sensor_objtype"), oid = b.ints("sensor_objid"),
+                             dim = b.ints("sensor_dim"), adr = b.ints("sensor_adr"), st = b.ints("site_type"),
+                             jt = b.ints("jnt_type");
+      const std::vector<double> ss = b.reals("site_size");
+      std::vector<double> cutoff(ty.size(), 0.0);
+      if (b.find("sensor_cutoff", &dt, &cnt, &off)) cutoff = b.reals("sensor_cutoff");
+      const int ns = b.i("nsensor");
+      for (int i = 0; i < ns; i++) {
+        DevSensor S = {ty[i], ot[i], oid[i], adr[i], 0.f};
+        std::string why;
+        if (ty[i] == SENS_JOINTPOS || ty[i] == SENS_JOINTVEL) {
+          if (jt[oid[i]] != JNT_SLIDE && jt[oid[i]] != JNT_HINGE) why = "jointpos / jointvel of a free or ball joint";
+        } else if (ty[i] == SENS_FRAMEPOS) {
+          if (ot[i] < OBJ_BODY || ot[i] > OBJ_SITE) why = "framepos of an unknown object type";
+        } else if (ty[i] == SENS_TOUCH) {
+          if (st[oid[i]] != GEOM_SPHERE) why = "touch zone other than a sphere site";
+          S.radius = (float)ss[3 * oid[i]];
+        } else {
+          why = "sensor type " + std::to_string(ty[i]) + " (only jointpos, jointvel, framepos and touch are evaluated)";
+        }
+        if (why.empty() && dim[i] != (ty[i] == SENS_FRAMEPOS ? 3 : 1)) why = "unexpected sensor dimension";
+        if (why.empty() && cutoff[i] != 0.0) why = "cutoff is not modelled";
+        h->sensors.push_back(S);
+        h->sensor_why.push_back(why);
+      }
+    }
+  }
   CREATE_TRY(cudaSetDevice(device));
   CREATE_TRY(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
   CREATE_TRY(cudaEventCreate(&h->ev0));
@@ -442,6 +483,9 @@ int mjpc_b200_create(const mjpc_model_blob* model, int max_candidates, int max_h
   CREATE_TRY(dalloc(&h->d_costs, N * H)); CREATE_TRY(dalloc(&h->d_trace, N * H * 3 * (size_t)M.num_trace));
   CREATE_TRY(dalloc(&h->d_returns, N)); CREATE_TRY(dalloc(&h->d_failure, N)); CREATE_TRY(dalloc(&h->d_order, N)); CREATE_TRY(dalloc(&h->d_stats, 12 * N));
   CREATE_TRY(dalloc(&h->d_pair_sync, (size_t)256 * 32));
+  CREATE_TRY(dalloc(&h->d_sensors, h->sensors.size()));
+  if (!h->sensors.empty())
+    CREATE_TRY(cudaMemcpy(h->d_sensors, h->sensors.data(), h->sensors.size() * sizeof(DevSensor), cudaMemcpyHostToDevice));
   h->h_in_floats = in_floats + H * (nu + ds + 1 + nu * n + nu) + N + 64;
   CREATE_TRY(cudaMallocHost((void**)&h->h_in, h->h_in_floats * 4));
   h->h_out_bytes = N * 16 + 64;
@@ -474,11 +518,13 @@ void mjpc_b200_destroy(mjpc_b200_t* h) {
   for (void* p : mbufs) if (p) cudaFree(p);
   void* bufs[] = {h->d_pack, h->d_in, h->d_unom, h->d_xnom,
                   h->d_tnom, h->d_gains, h->d_du, h->d_steps, h->d_states, h->d_actions, h->d_times, h->d_residual,
-                  h->d_costs, h->d_trace, h->d_returns, h->d_failure, h->d_order, h->d_stats, h->d_pair_sync};
+                  h->d_costs, h->d_trace, h->d_returns, h->d_failure, h->d_order, h->d_stats, h->d_pair_sync,
+                  h->d_sensors, h->d_step};
   for (void* p : bufs) if (p) cudaFree(p);
   ilqg_free(h->ilqg);
   if (h->h_in) cudaFreeHost(h->h_in);
   if (h->h_out) cudaFreeHost(h->h_out);
+  if (h->h_step) cudaFreeHost(h->h_step);
   if (h->ev0) cudaEventDestroy(h->ev0);
   if (h->ev1) cudaEventDestroy(h->ev1);
   if (h->stream) cudaStreamDestroy(h->stream);
@@ -698,41 +744,56 @@ int mjpc_b200_fetch_all(mjpc_b200_t* h, float* states, float* actions, double* t
   return fetch_impl(h, 0, h->lastN, states, actions, times, residual, costs, trace);
 }
 
+// grow step_impl's device scratch and pinned staging to `words` floats each (never shrinks); on failure the old ones stay
+int reserve_step(mjpc_b200_t* h, size_t words) {
+  if (words <= h->step_words) return 0;
+  float *d = nullptr, *p = nullptr;
+  CUDA_TRY(cudaStreamSynchronize(h->stream));
+  CUDA_TRY(dalloc(&d, words));
+  if (cudaMallocHost((void**)&p, words * 4) != cudaSuccess) {
+    cudaGetLastError();
+    cudaFree(d);
+    return fail(MJPC_B200_ERR_CUDA, "step: out of pinned host memory");
+  }
+  cudaFree(h->d_step); cudaFreeHost(h->h_step);
+  h->d_step = d; h->h_step = p; h->step_words = words;
+  return 0;
+}
+
 // B single steps (see step_batch_kernel) on instance `fn`.  times are absolute; the task state is rebased to time0
 // (device time = times[b] - time0).  Outputs may be NULL; qM [B][nv nv], efc_force [B][maxefc] and contact
-// [B][maxcon][8] are the optional ones, their rows past each problem's counts read as zeros.  e0 / e1, when given,
-// time the kernel.
+// [B][maxcon][8] are the optional ones, their rows past each problem's counts read as zeros.  sensordata [B][dim]
+// (NULL: not evaluated) receives sensors [s0, s0 + ns) of the handle's table, dim = their total dimension.  e0 / e1,
+// when given, time the kernel.  Inputs go up in one copy from the handle's pinned staging, outputs come back in one.
 static int step_impl(mjpc_b200_t* h, const void* fn, int B, const float* qpos, const float* qvel, const float* ctrl,
                      const float* warmstart, const float* mocap, double time0, const double* times, float* qacc,
                      float* next_qpos, float* next_qvel, float* residual, float* cost, int* counts, float* qM,
-                     float* efc_force, float* contact, cudaEvent_t e0, cudaEvent_t e1) {
+                     float* efc_force, float* contact, cudaEvent_t e0, cudaEvent_t e1, int s0 = 0, int ns = 0,
+                     float* sensordata = nullptr) {
   const DevModel& M = h->pack.M;
   CUDA_TRY(cudaSetDevice(h->device));
   const size_t Bs = B, nq = M.nq, nv = M.nv, nu = M.nu, nr = std::max(M.num_residual, 1), nm = 7 * (size_t)M.nmocap,
                nts = (size_t)M.task_state_size;
+  const int adr0 = ns ? h->sensors[s0].adr : 0;
+  const size_t nsd = ns ? (size_t)(h->sensors[s0 + ns - 1].adr - adr0 + (h->sensors[s0 + ns - 1].type == SENS_FRAMEPOS ? 3 : 1)) : 0;
   size_t words = 0;
   auto take = [&](size_t n) { const size_t at = words; words += n; return at; };
   const size_t o_qpos = take(Bs * nq), o_qvel = take(Bs * nv), o_ctrl = take(Bs * nu), o_warm = take(Bs * nv),
-               o_time = take(Bs), o_mocap = take(nm), o_ts = take(nts), o_qacc = take(Bs * nv), o_nq = take(Bs * nq),
-               o_nv = take(Bs * nv), o_res = take(Bs * nr), o_cost = take(Bs), o_counts = take(4 * Bs),
-               o_qM = take(qM ? Bs * nv * nv : 0), o_efc = take(efc_force ? Bs * M.maxefc : 0),
-               o_con = take(contact ? Bs * M.maxcon * 8 : 0);
-  float* d = nullptr;
-  CUDA_TRY(dalloc(&d, words));
-  struct Guard { float* p; ~Guard() { cudaFree(p); } } guard{d};
-  std::vector<float> trel(B), ts(nts);
-  for (int i = 0; i < B; i++) trel[i] = (float)(times[i] - time0);
-  rebase_task_state(h, nullptr, time0, ts.data());
+               o_time = take(Bs), o_mocap = take(nm), o_ts = take(nts), in_words = words, o_qacc = take(Bs * nv),
+               o_nq = take(Bs * nq), o_nv = take(Bs * nv), o_res = take(Bs * nr), o_cost = take(Bs),
+               o_counts = take(4 * Bs), o_qM = take(qM ? Bs * nv * nv : 0), o_efc = take(efc_force ? Bs * M.maxefc : 0),
+               o_con = take(contact ? Bs * M.maxcon * 8 : 0), o_sens = take(sensordata ? Bs * nsd : 0);
+  if (int rc = reserve_step(h, words)) return rc;
+  float *d = h->d_step, *p = h->h_step;
+  std::memcpy(p + o_qpos, qpos, Bs * nq * 4); std::memcpy(p + o_qvel, qvel, Bs * nv * 4);
+  std::memcpy(p + o_ctrl, ctrl, Bs * nu * 4);
+  if (warmstart) std::memcpy(p + o_warm, warmstart, Bs * nv * 4);
+  for (int i = 0; i < B; i++) p[o_time + i] = (float)(times[i] - time0);
+  if (nm) std::memcpy(p + o_mocap, mocap, nm * 4);
+  rebase_task_state(h, nullptr, time0, p + o_ts);
   // every transfer on the engine stream, ordered with the kernel
-  auto put = [&](size_t at, const void* src, size_t floats) {
-    return cudaMemcpyAsync(d + at, src, floats * 4, cudaMemcpyHostToDevice, h->stream);
-  };
-  CUDA_TRY(cudaMemsetAsync(d, 0, words * 4, h->stream));
-  CUDA_TRY(put(o_qpos, qpos, Bs * nq)); CUDA_TRY(put(o_qvel, qvel, Bs * nv)); CUDA_TRY(put(o_ctrl, ctrl, Bs * nu));
-  if (warmstart) CUDA_TRY(put(o_warm, warmstart, Bs * nv));
-  CUDA_TRY(put(o_time, trel.data(), Bs));
-  if (nm) CUDA_TRY(put(o_mocap, mocap, nm));
-  if (nts) CUDA_TRY(put(o_ts, ts.data(), nts));
+  CUDA_TRY(cudaMemsetAsync(d + in_words, 0, (words - in_words) * 4, h->stream));
+  CUDA_TRY(cudaMemcpyAsync(d, p, in_words * 4, cudaMemcpyHostToDevice, h->stream));
   StepBatchArgs A;
   std::memset(&A, 0, sizeof(A));
   A.M = h->pack.M; A.L = make_layout(h->pack.M, 1); A.pack = h->d_pack;
@@ -741,21 +802,24 @@ static int step_impl(mjpc_b200_t* h, const void* fn, int B, const float* qpos, c
   A.qacc = d + o_qacc; A.next_qpos = d + o_nq; A.next_qvel = d + o_nv; A.residual = d + o_res; A.cost = d + o_cost;
   A.counts = (int*)(d + o_counts);
   A.qM = qM ? d + o_qM : nullptr; A.efc_force = efc_force ? d + o_efc : nullptr; A.contact = contact ? d + o_con : nullptr;
+  if (sensordata) {
+    A.sensors = h->d_sensors + s0; A.nsensor = ns; A.sensor_adr0 = adr0; A.sensor_dim = (int)nsd;
+    A.sensordata = d + o_sens;
+  }
   if (e0) CUDA_TRY(cudaEventRecord(e0, h->stream));
   launch_kernel(fn, B, 32, h->smem_bytes(1, 1), h->stream, A);
   if (e1) CUDA_TRY(cudaEventRecord(e1, h->stream));
   CUDA_TRY(cudaGetLastError());
   h->launches += 1;
+  CUDA_TRY(cudaMemcpyAsync(p + in_words, d + in_words, (words - in_words) * 4, cudaMemcpyDeviceToHost, h->stream));
   CUDA_TRY(cudaStreamSynchronize(h->stream));
   if (e0 && cudaEventElapsedTime(&h->last_ms, e0, e1) != cudaSuccess) cudaGetLastError();
-  auto get = [&](void* dst, size_t at, size_t bytes) {
-    return dst ? cudaMemcpy(dst, d + at, bytes, cudaMemcpyDeviceToHost) : cudaSuccess;
-  };
-  CUDA_TRY(get(qacc, o_qacc, Bs * nv * 4)); CUDA_TRY(get(next_qpos, o_nq, Bs * nq * 4));
-  CUDA_TRY(get(next_qvel, o_nv, Bs * nv * 4)); CUDA_TRY(get(residual, o_res, Bs * M.num_residual * 4));
-  CUDA_TRY(get(cost, o_cost, Bs * 4)); CUDA_TRY(get(counts, o_counts, Bs * 16));
-  CUDA_TRY(get(qM, o_qM, Bs * nv * nv * 4)); CUDA_TRY(get(efc_force, o_efc, Bs * M.maxefc * 4));
-  CUDA_TRY(get(contact, o_con, Bs * M.maxcon * 8 * 4));
+  auto get = [&](void* dst, size_t at, size_t bytes) { if (dst) std::memcpy(dst, p + at, bytes); };
+  get(qacc, o_qacc, Bs * nv * 4); get(next_qpos, o_nq, Bs * nq * 4);
+  get(next_qvel, o_nv, Bs * nv * 4); get(residual, o_res, Bs * M.num_residual * 4);
+  get(cost, o_cost, Bs * 4); get(counts, o_counts, Bs * 16);
+  get(qM, o_qM, Bs * nv * nv * 4); get(efc_force, o_efc, Bs * M.maxefc * 4);
+  get(contact, o_con, Bs * M.maxcon * 8 * 4); get(sensordata, o_sens, Bs * nsd * 4);
   return 0;
 }
 
@@ -914,6 +978,44 @@ int mjpc_b200_step_batch(mjpc_b200_t* h, int B, const float* qpos, const float* 
   if (int rc = step_impl(h, k->step, B, qpos, qvel, ctrl, warmstart, mocap, time0, times, qacc, next_qpos, next_qvel,
                          residual, cost, counts, nullptr, nullptr, nullptr, h->ev0, h->ev1))
     return rc;
+  h->last_static = kind ? 1 : 0;
+  return 0;
+}
+
+// The sigma-point step of a state estimator (Unscented::EvaluateSigmaPoints, unscented.cc:353-394): B states, one
+// ctrl, mocap and time, each advanced by one step_batch step with the measurement sensors of its pre-step state.
+int mjpc_b200_step_sensors(mjpc_b200_t* h, int B, const float* states, const float* ctrl, const float* warmstart,
+                           const float* mocap, double time, int sensor_start, int nsensor, float* next_states,
+                           float* sensordata, float* qacc, int* counts) {
+  if (!h || B < 1 || !states || (!ctrl && h->pack.M.nu) || !next_states || !sensordata)
+    return fail(MJPC_B200_ERR_BAD_ARGUMENT, "step_sensors: bad argument");
+  const DevModel& M = h->pack.M;
+  if (M.nmocap && !mocap) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "step_sensors: mocap required");
+  const int nsens = (int)h->sensors.size();
+  if (sensor_start < 0 || nsensor < 1 || sensor_start > nsens - nsensor)
+    return fail(MJPC_B200_ERR_BAD_ARGUMENT, "step_sensors: sensor range [" + std::to_string(sensor_start) + ", " +
+                                                std::to_string((long long)sensor_start + nsensor) + ") outside the model's " +
+                                                std::to_string(nsens) + " sensors");
+  for (int i = sensor_start; i < sensor_start + nsensor; i++)
+    if (!h->sensor_why[i].empty())
+      return fail(MJPC_B200_ERR_UNSUPPORTED, "step_sensors: sensor " + std::to_string(i) + ": " + h->sensor_why[i]);
+  if (B > h->maxN) return fail(MJPC_B200_ERR_CAPACITY, "step_sensors: B > max_candidates");
+  const KernelSet* k;
+  const int kind = pick_kernels(h, true, &k);
+  const size_t nq = M.nq, nv = M.nv, nu = M.nu, ds = nq + nv;
+  std::vector<float> q(B * nq), v(B * nv), u(B * nu), nq_out(B * nq), nv_out(B * nv);
+  std::vector<double> t(B, time);
+  for (int b = 0; b < B; b++) {
+    std::memcpy(&q[b * nq], states + b * ds, nq * 4); std::memcpy(&v[b * nv], states + b * ds + nq, nv * 4);
+    std::memcpy(&u[b * nu], ctrl, nu * 4);
+  }
+  if (int rc = step_impl(h, k->step, B, q.data(), v.data(), u.data(), warmstart, mocap, time, t.data(), qacc,
+                         nq_out.data(), nv_out.data(), nullptr, nullptr, counts, nullptr, nullptr, nullptr, h->ev0,
+                         h->ev1, sensor_start, nsensor, sensordata))
+    return rc;
+  for (int b = 0; b < B; b++) {
+    std::memcpy(next_states + b * ds, &nq_out[b * nq], nq * 4); std::memcpy(next_states + b * ds + nq, &nv_out[b * nv], nv * 4);
+  }
   h->last_static = kind ? 1 : 0;
   return 0;
 }

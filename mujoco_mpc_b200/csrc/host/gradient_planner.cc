@@ -256,14 +256,7 @@ int iLQSPlanner::OptimizePolicy(int horizon) {
         for (int q = 0; q < P; q++) M[(size_t)p * P + q] += w * W[(size_t)t * P + q];
         for (int j = 0; j < nu_; j++) rhs[(size_t)p * nu_ + j] += w * (double)ilqg.candidate_actions()[(size_t)t * nu_ + j];
       }
-    for (int j = 0; j < P; j++) {                                   // in-place Cholesky (mju_cholFactor)
-      for (int k = 0; k < j; k++) M[(size_t)j * P + j] -= M[(size_t)j * P + k] * M[(size_t)j * P + k];
-      M[(size_t)j * P + j] = std::sqrt(std::max(M[(size_t)j * P + j], 1e-15));
-      for (int i = j + 1; i < P; i++) {
-        for (int k = 0; k < j; k++) M[(size_t)i * P + j] -= M[(size_t)i * P + k] * M[(size_t)j * P + k];
-        M[(size_t)i * P + j] /= M[(size_t)j * P + j];
-      }
-    }
+    CholFactor(M.data(), P, 1e-15);                                 // in-place Cholesky (mju_cholFactor)
     for (int j = 0; j < nu_; j++) {                                 // L L' x = rhs, column by column
       for (int i = 0; i < P; i++) { double a = rhs[(size_t)i * nu_ + j]; for (int k = 0; k < i; k++) a -= M[(size_t)i * P + k] * rhs[(size_t)k * nu_ + j]; rhs[(size_t)i * nu_ + j] = a / M[(size_t)i * P + i]; }
       for (int i = P - 1; i >= 0; i--) { double a = rhs[(size_t)i * nu_ + j]; for (int k = i + 1; k < P; k++) a -= M[(size_t)k * P + i] * rhs[(size_t)k * nu_ + j]; rhs[(size_t)i * nu_ + j] = a / M[(size_t)i * P + i]; }

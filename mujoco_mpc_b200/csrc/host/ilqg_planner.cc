@@ -68,6 +68,21 @@ int iLQGPolicyModel::Load(const mjpc_model_blob* blob) {
   return 0;
 }
 
+void StateDiff(const iLQGPolicyModel& m, double* dx, const double* x_to, const double* x_from) {
+  for (size_t j = 0; j < m.jnt_type.size(); j++) {
+    const int qa = m.jnt_qposadr[j], da = m.jnt_dofadr[j];
+    if (m.jnt_type[j] == 0) {
+      for (int c = 0; c < 3; c++) dx[da + c] = x_to[qa + c] - x_from[qa + c];
+      SubQuat(&dx[da + 3], x_to + qa + 3, &x_from[qa + 3]);
+    } else if (m.jnt_type[j] == 1) {
+      SubQuat(&dx[da], x_to + qa, &x_from[qa]);
+    } else {
+      dx[da] = x_to[qa] - x_from[qa];
+    }
+  }
+  for (int i = 0; i < m.nv; i++) dx[m.nv + i] = x_to[m.nq + i] - x_from[m.nq + i];
+}
+
 void iLQGPolicyAction(const iLQGPolicyModel& m, const float* u_nom, const float* x_nom, const double* t_nom,
                       const float* gains, int H, int representation, double feedback_scaling, const double* state,
                       double time, double* action) {
@@ -86,18 +101,7 @@ void iLQGPolicyAction(const iLQGPolicyModel& m, const float* u_nom, const float*
       }
     Interpolate(K.data(), time, t_nom, gains, nu * n, H - 1, rep);
     // StateDiff(model, dx, x_interp, state, 1): tangent-space difference state (-) x_interp
-    for (size_t j = 0; j < m.jnt_type.size(); j++) {
-      const int qa = m.jnt_qposadr[j], da = m.jnt_dofadr[j];
-      if (m.jnt_type[j] == 0) {
-        for (int c = 0; c < 3; c++) dx[da + c] = state[qa + c] - xi[qa + c];
-        SubQuat(&dx[da + 3], state + qa + 3, &xi[qa + 3]);
-      } else if (m.jnt_type[j] == 1) {
-        SubQuat(&dx[da], state + qa, &xi[qa]);
-      } else {
-        dx[da] = state[qa] - xi[qa];
-      }
-    }
-    for (int i = 0; i < m.nv; i++) dx[m.nv + i] = state[m.nq + i] - xi[m.nq + i];
+    StateDiff(m, dx.data(), state, xi.data());
     for (int i = 0; i < nu; i++) {
       double a = 0;
       for (int j = 0; j < n; j++) a += K[(size_t)i * n + j] * dx[j];

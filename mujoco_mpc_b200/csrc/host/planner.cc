@@ -1,6 +1,8 @@
 // planner.cc - see planner.h.
 #include "planner.h"
 
+#include <cmath>
+
 #include <algorithm>
 
 namespace mjpc_b200_host {
@@ -50,6 +52,26 @@ int Planner::FetchTrajectory(int candidate, int horizon, Trajectory* t) {
   t->residual.resize(H * t->dim_residual); t->costs.resize(H); t->trace.resize(H * t->dim_trace);
   return mjpc_b200_fetch_trajectory(gpu_, candidate, t->states.data(), t->actions.data(), t->times.data(),
                                     t->residual.data(), t->costs.data(), t->trace.data());
+}
+
+int CholFactor(double* M, int n, double mindiag) {
+  int rank = 0;
+  for (int j = 0; j < n; j++) {
+    for (int k = 0; k < j; k++) M[(size_t)j * n + j] -= M[(size_t)j * n + k] * M[(size_t)j * n + k];
+    double d = M[(size_t)j * n + j];
+    if (d < mindiag) d = mindiag; else rank++;
+    M[(size_t)j * n + j] = std::sqrt(d);
+    for (int i = j + 1; i < n; i++) {
+      for (int k = 0; k < j; k++) M[(size_t)i * n + j] -= M[(size_t)i * n + k] * M[(size_t)j * n + k];
+      M[(size_t)i * n + j] /= M[(size_t)j * n + j];
+    }
+  }
+  return rank;
+}
+
+void CholSolve(const double* L, int n, double* x) {
+  for (int i = 0; i < n; i++) { double a = x[i]; for (int k = 0; k < i; k++) a -= L[(size_t)i * n + k] * x[k]; x[i] = a / L[(size_t)i * n + i]; }
+  for (int i = n - 1; i >= 0; i--) { double a = x[i]; for (int k = i + 1; k < n; k++) a -= L[(size_t)k * n + i] * x[k]; x[i] = a / L[(size_t)i * n + i]; }
 }
 
 }  // namespace mjpc_b200_host

@@ -17,6 +17,12 @@ struct Trajectory {                                   // mjpc/trajectory.h:74-86
   bool failure = false;
 };
 
+// mju_cholFactor: in-place lower Cholesky factor of the row-major n x n matrix M (upper triangle left as it was); a
+// pivot below mindiag is raised to mindiag.  Returns the rank, the number of pivots that were not raised.
+int CholFactor(double* M, int n, double mindiag);
+// mju_cholSolve: x = (L L')^-1 x with the factor of CholFactor
+void CholSolve(const double* L, int n, double* x);
+
 // FindInterval (mjpc/utilities.cc:303-330): the indices of the entries of a non-decreasing sequence around `value`,
 // clamped to the sequence
 void FindInterval(int* bounds, const double* sequence, double value, int length);

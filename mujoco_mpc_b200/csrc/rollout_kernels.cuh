@@ -451,6 +451,9 @@ struct StepBatchArgs {
   // optional (NULL: not written): qM [B][nv nv], efc_force [B][maxefc], contact [B][maxcon][8] = dist, pos[3],
   // normal[3], dim of the geometric contacts
   float* qM; float* efc_force; float* contact;
+  // optional (NULL: not evaluated): the measurement sensors sensors[0, nsensor) (k_sensors), sensordata [B][sensor_dim]
+  // from address sensor_adr0 on
+  const DevSensor* sensors; int nsensor, sensor_adr0, sensor_dim; float* sensordata;
 };
 
 template <class SP>
@@ -492,6 +495,7 @@ __device__ __forceinline__ void step_batch_body(const StepBatchArgs& A) {
       const int d = DI(con_dim)[i];   // the pyramidal constraint phase rewrites it as the row count 2 (dim - 1)
       o[7] = (float)(M.cone == CONE_PYRAMIDAL && d > 1 ? d / 2 + 1 : d);
     }
+  if (A.sensordata) k_sensors<SP>(c, A.sensors, A.nsensor, A.sensor_adr0, A.sensordata + (size_t)b * A.sensor_dim);
   for (int i = lane; i < nv; i += 32) DF(qacc_warmstart)[i] = DF(qacc)[i];
   k_euler<SP>(c);
   for (int i = lane; i < nq; i += 32) A.next_qpos[(size_t)b * nq + i] = DF(qpos)[i];

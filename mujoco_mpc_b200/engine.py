@@ -32,7 +32,10 @@ EXPORTS = ["mjpc_b200_version", "mjpc_b200_last_error", "mjpc_b200_create", "mjp
            "mjpc_b200_batch_ilqg_planner_set_state", "mjpc_b200_batch_ilqg_planner_set_task",
            "mjpc_b200_batch_ilqg_planner_nominal_trajectory", "mjpc_b200_batch_ilqg_planner_optimize_policy",
            "mjpc_b200_batch_ilqg_planner_action_from_policy", "mjpc_b200_batch_ilqg_planner_get_result",
-           "mjpc_b200_step_debug", "mjpc_b200_step_debug_contacts", "mjpc_b200_step_batch","mjpc_b200_comm_unique_id", "mjpc_b200_comm_init",
+           "mjpc_b200_step_debug", "mjpc_b200_step_debug_contacts", "mjpc_b200_step_batch", "mjpc_b200_step_sensors",
+           "mjpc_b200_unscented_create", "mjpc_b200_unscented_destroy", "mjpc_b200_unscented_reset",
+           "mjpc_b200_unscented_set_noise", "mjpc_b200_unscented_set", "mjpc_b200_unscented_update",
+           "mjpc_b200_unscented_get", "mjpc_b200_unscented_last_error", "mjpc_b200_comm_unique_id", "mjpc_b200_comm_init",
            "mjpc_b200_comm_info", "mjpc_b200_rollout_spline_sharded", "mjpc_b200_fetch_trajectory_sharded",
            "mjpc_b200_fetch_stats", "mjpc_b200_launch_count", "mjpc_b200_last_kernel_ms", "mjpc_b200_last_kernel_static",
            "mjpc_b200_spec_words", "mjpc_b200_upload_spline_inputs",
@@ -131,6 +134,14 @@ def load_library():
             getattr(lib, n).argtypes = [C.c_void_p]
         _LIB = lib
     return _LIB
+
+
+def sensor_dim(m, sensor_start, nsensor):
+    """Total dimension of the model's sensors [sensor_start, sensor_start + nsensor) (0 for a range outside them: the
+    engine refuses it)."""
+    if sensor_start < 0 or nsensor < 1 or sensor_start + nsensor > m.nsensor:
+        return 0
+    return int(np.sum(m.sensor_dim[sensor_start:sensor_start + nsensor]))
 
 
 class EngineError(RuntimeError):
@@ -429,6 +440,23 @@ class Engine:
         self._check(self.lib.mjpc_b200_step_batch(self.h, B, _pf(q), _pf(v), _pf(u), _pf(ws), _pf(mc), C.c_double(time0),
                                                   _pd(t), _pf(o["qacc"]), _pf(o["next_qpos"]), _pf(o["next_qvel"]),
                                                   _pf(o["residual"]), _pf(o["cost"]), counts.ctypes.data_as(_ip)))
+        o.update(ncon=counts[:, 0], nefc=counts[:, 1], niter=counts[:, 2], warning=counts[:, 3])
+        return o
+
+    def step_sensors(self, states, ctrl, mocap, time, sensor_start, nsensor, warmstart=None):
+        """One step of each of B states from one (ctrl, mocap, time) with the measurement sensors
+        [sensor_start, sensor_start + nsensor) of each pre-step state (mjpc_b200_step_sensors): the sigma-point step
+        of the Unscented filter (mujoco_mpc_b200.estimator).  Returns dict(next_states [B][nq+nv],
+        sensordata [B][dim], qacc [B][nv], ncon, nefc, niter, warning [B])."""
+        x, u, mc, ws = _f(np.atleast_2d(states)), _f(ctrl), _f(mocap), _f(warmstart)
+        B, nv = x.shape[0], self.info.nv
+        dim = sensor_dim(self.m, sensor_start, nsensor)
+        o = dict(next_states=np.zeros((B, self.info.dim_state), np.float32), sensordata=np.zeros((B, dim), np.float32),
+                 qacc=np.zeros((B, nv), np.float32))
+        counts = np.zeros((B, 4), np.int32)
+        self._check(self.lib.mjpc_b200_step_sensors(self.h, B, _pf(x), _pf(u), _pf(ws), _pf(mc), C.c_double(time),
+                                                    int(sensor_start), int(nsensor), _pf(o["next_states"]),
+                                                    _pf(o["sensordata"]), _pf(o["qacc"]), counts.ctypes.data_as(_ip)))
         o.update(ncon=counts[:, 0], nefc=counts[:, 1], niter=counts[:, 2], warning=counts[:, 3])
         return o
 

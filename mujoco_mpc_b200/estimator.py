@@ -1,0 +1,403 @@
+"""MJPC's Unscented state estimator (mjpc/estimators/unscented.cc) with its sigma-point steps on a step backend.
+
+The filter arithmetic is double precision on the host: a Cholesky factor of the covariance, weighted means and
+covariances of at most 2 ndstate + 1 points and one Cholesky factor of the sensor covariance.  The sigma-point steps
+(one mj_step per point, EvaluateSigmaPoints, unscented.cc:353-394) are what costs: the backend runs them all in one
+call.  ``EngineBackend`` runs them as one launch of the CUDA engine (``Engine.step_sensors``); anything with the same
+``step_sensors`` method can stand in for it.
+
+Reference semantics restated (unscented.cc):
+  settings      :31-168, Reset :171-290 (every setting through GetNumberOrDefault)
+  SigmaPoints   :293-349   lower Cholesky factor L of P; point i = x (+) step L[:, i], point i + ndstate = x (-) step
+                           L[:, i] (positions through mj_integratePos, velocities added); the nominal state is LAST
+  Evaluate      :353-394   every point steps from the same time and ctrl; y_i = h(sigma_i) (sensors of the pre-step
+                           state, after the constraint solve), s_i = f(sigma_i); means weight the last point w_mean0
+  QuaternionMean:578-626   per free / ball joint the principal eigenvector of sum 4 w q q^T - (sum w) I, with the
+                           COVARIANCE weights (as the reference does)
+  Differences / Covariances / Update :397-574
+
+Documented differences from the reference:
+  * a failed factorisation (covariance or sensor covariance) raises ``EstimatorError`` naming the factor and leaves
+    state, covariance and time untouched (the reference calls mju_error);
+  * every sigma point warm-starts the constraint solver from the nominal point's qacc of the previous update (zeros
+    after reset); the reference reuses one mjData, so each point starts from the previous point's qacc.  The Newton
+    solution is unique to the solver tolerance, so this changes results only at that level;
+  * ``update`` takes mocap (default: the model's), the reference's mjData keeps the model's;
+  * ``update`` takes the measured slice [nsensordata] of the sensors, not the whole sensordata.
+"""
+from __future__ import annotations
+
+import numpy as np
+
+from .mjcf import JNT_BALL, JNT_FREE, SENS_MEASURED
+
+
+class EstimatorError(RuntimeError):
+    pass
+
+
+def _number(m, name, default):
+    """GetNumberOrDefault (utilities.cc): the model's custom numeric `name`, else `default`."""
+    v = m.numeric.get(name) if hasattr(m, "numeric") else None
+    return float(v[0]) if v is not None and len(v) else default
+
+
+# ------------------------------------------------------------------------------------------- quaternions / positions
+def _quat_mul(a, b):
+    return np.array([a[0] * b[0] - a[1] * b[1] - a[2] * b[2] - a[3] * b[3],
+                     a[0] * b[1] + a[1] * b[0] + a[2] * b[3] - a[3] * b[2],
+                     a[0] * b[2] - a[1] * b[3] + a[2] * b[0] + a[3] * b[1],
+                     a[0] * b[3] + a[1] * b[2] - a[2] * b[1] + a[3] * b[0]])
+
+
+def quat_integrate(q, v, scale):
+    """mju_quatIntegrate: q * exp(scale v / 2), normalised."""
+    w = np.asarray(v, float) * scale
+    a = np.linalg.norm(w)
+    if a < 1e-15:
+        return np.asarray(q, float) / np.linalg.norm(q)
+    r = np.concatenate([[np.cos(a / 2)], np.sin(a / 2) * w / a])
+    out = _quat_mul(q, r)
+    return out / np.linalg.norm(out)
+
+
+def quat_sub(qa, qb):
+    """mju_subQuat: the 3-vector v with qb * exp(v / 2) = qa (shortest arc)."""
+    qb_inv = np.array([qb[0], -qb[1], -qb[2], -qb[3]])
+    d = _quat_mul(qb_inv, qa)
+    d = d / np.linalg.norm(d)
+    if d[0] < 0:
+        d = -d
+    s = np.linalg.norm(d[1:])
+    if s < 1e-15:
+        return np.zeros(3)
+    return 2 * np.arctan2(s, d[0]) * d[1:] / s
+
+
+def integrate_pos(m, qpos, dq, scale=1.0):
+    """mj_integratePos: qpos (+) scale dq, quaternions in the tangent space."""
+    q = np.array(qpos, float)
+    for j in range(m.njnt):
+        a, d, t = m.jnt_qposadr[j], m.jnt_dofadr[j], m.jnt_type[j]
+        if t == JNT_FREE:
+            q[a:a + 3] += scale * dq[d:d + 3]
+            q[a + 3:a + 7] = quat_integrate(q[a + 3:a + 7], dq[d + 3:d + 6], scale)
+        elif t == JNT_BALL:
+            q[a:a + 4] = quat_integrate(q[a:a + 4], dq[d:d + 3], scale)
+        else:
+            q[a] += scale * dq[d]
+    return q
+
+
+def differentiate_pos(m, q1, q2):
+    """mj_differentiatePos with dt = 1: the tangent vector from q1 to q2."""
+    out = np.zeros(m.nv)
+    for j in range(m.njnt):
+        a, d, t = m.jnt_qposadr[j], m.jnt_dofadr[j], m.jnt_type[j]
+        if t == JNT_FREE:
+            out[d:d + 3] = q2[a:a + 3] - q1[a:a + 3]
+            out[d + 3:d + 6] = quat_sub(q2[a + 3:a + 7], q1[a + 3:a + 7])
+        elif t == JNT_BALL:
+            out[d:d + 3] = quat_sub(q2[a:a + 4], q1[a:a + 4])
+        else:
+            out[d] = q2[a] - q1[a]
+    return out
+
+
+def principal_eigenvector4(K, reference):
+    """Principal eigenvector of a symmetric 4 x 4 matrix by cyclic Jacobi rotations, converged to rounding, with the
+    sign that agrees with `reference` (stands for PrincipalEigenVector4, utilities.cc:1476+; the C++ filter runs the
+    same rotations)."""
+    A = np.array(K, float)
+    V = np.eye(4)
+    for _ in range(50):
+        if sum(A[p, q] ** 2 for p in range(4) for q in range(p + 1, 4)) < 1e-300:
+            break
+        for p in range(4):
+            for q in range(p + 1, 4):
+                if A[p, q] == 0:
+                    continue
+                th = (float(A[q, q]) - float(A[p, p])) / (2 * float(A[p, q]))
+                t = 0.5 / th if abs(th) > 1e150 else (1.0 if th >= 0 else -1.0) / (abs(th) + np.sqrt(th * th + 1))
+                c = 1 / np.sqrt(t * t + 1)
+                s = t * c
+                J = np.eye(4)
+                J[p, p] = J[q, q] = c
+                J[p, q], J[q, p] = s, -s
+                A = J.T @ A @ J
+                V = V @ J
+    v = V[:, int(np.argmax(np.diag(A)))]
+    v = v / np.linalg.norm(v)
+    return v if np.dot(v, reference) >= 0 else -v
+
+
+def quaternion_mean(quats, weights, reference):
+    """Principal eigenvector of K = sum 4 w_i q_i q_i^T - (sum w) I (QuaternionMeans, unscented.cc:578-626), with the
+    sign that agrees with `reference` (the nominal point's quaternion)."""
+    Q = np.asarray(quats, float)
+    w = np.asarray(weights, float)
+    K = 4.0 * np.einsum("i,ij,ik->jk", w, Q, Q) - w.sum() * np.eye(4)
+    return principal_eigenvector4(K, reference)
+
+
+# ------------------------------------------------------------------------------------------------------- backends
+class EngineBackend:
+    """The sigma-point steps as one launch of the CUDA engine (mjpc_b200_step_sensors)."""
+
+    def __init__(self, engine, sensor_start, nsensor, timestep):
+        self.engine, self.sensor_start, self.nsensor = engine, int(sensor_start), int(nsensor)
+        engine.set_options(timestep)   # the estimator's own timestep (estimator_timestep), as Reset sets it
+
+    def step_sensors(self, states, ctrl, mocap, time, warmstart):
+        o = self.engine.step_sensors(states, ctrl, mocap, time, self.sensor_start, self.nsensor, warmstart=warmstart)
+        return (o["next_states"].astype(float), o["sensordata"].astype(float), o["qacc"].astype(float),
+                int(np.count_nonzero(o["warning"])))
+
+    @property
+    def last_kernel_ms(self):
+        return self.engine.last_kernel_ms
+
+
+def measured_range(m, sensor_start, nsensor):
+    """Check that sensors [sensor_start, sensor_start + nsensor) are ones the measurement path evaluates; returns the
+    dimension of their sensordata slice."""
+    if sensor_start < 0 or nsensor < 1 or sensor_start + nsensor > m.nsensor:
+        raise EstimatorError("sensor range [%d, %d) outside the model's %d sensors"
+                             % (sensor_start, sensor_start + nsensor, m.nsensor))
+    for i in range(sensor_start, sensor_start + nsensor):
+        if int(m.sensor_type[i]) not in SENS_MEASURED:
+            raise EstimatorError("sensor %d (%s) is not a measured sensor type (jointpos, jointvel, framepos, touch)"
+                                 % (i, m.sensor_names[i]))
+        if float(m.sensor_cutoff[i]) != 0.0:
+            raise EstimatorError("sensor %d (%s): cutoff is not modelled" % (i, m.sensor_names[i]))
+    return int(np.sum(m.sensor_dim[sensor_start:sensor_start + nsensor]))
+
+
+# ------------------------------------------------------------------------------------------------------- the filter
+def settings(m, sensor_start=None, nsensor=None, timestep=None, alpha=None, beta=None):
+    """The filter settings, each left None defaulting from the model's numerics as GetNumberOrDefault does
+    (unscented.cc:31-168): (sensor_start, nsensor, timestep, alpha, beta)."""
+    return (int(_number(m, "estimator_sensor_start", 0) if sensor_start is None else sensor_start),
+            int(_number(m, "estimator_number_sensor", m.nsensor) if nsensor is None else nsensor),
+            float(_number(m, "estimator_timestep", float(m.opt_timestep)) if timestep is None else timestep),
+            float(_number(m, "unscented_alpha", 1.0) if alpha is None else alpha),
+            float(_number(m, "unscented_beta", 2.0) if beta is None else beta))
+
+
+def reset_values(m, state=None, covariance_scale=None, process_scale=None, sensor_scale=None):
+    """Reset's state (the home keyframe if the model has one, else qpos0 and zero qvel) and noise scales."""
+    if state is None:
+        if m.nkey and "home" in m.key_names:
+            k = m.key_names.index("home")
+            state = np.concatenate([m.key_qpos[k], m.key_qvel[k]])
+        else:
+            state = np.concatenate([m.qpos0, np.zeros(m.nv)])
+    cs = _number(m, "estimator_covariance_initial_scale", 1e-4) if covariance_scale is None else covariance_scale
+    ps = _number(m, "estimator_process_noise_scale", 1e-4) if process_scale is None else process_scale
+    ss = _number(m, "estimator_sensor_noise_scale", 1e-4) if sensor_scale is None else sensor_scale
+    return np.array(state, float), float(cs), float(ps), float(ss)
+
+
+class Unscented:
+    """mjpc::Unscented.  `backend(sensor_start, nsensor, timestep)` returns the object that runs the sigma-point steps (see
+    EngineBackend); settings left None default from the model's numerics as GetNumberOrDefault does."""
+
+    def __init__(self, m, backend, sensor_start=None, nsensor=None, timestep=None, alpha=None, beta=None):
+        self.m = m
+        self.sensor_start, self.nsensor, self.timestep, self.alpha, self.beta = settings(m, sensor_start, nsensor,
+                                                                                         timestep, alpha, beta)
+        self.nsensordata = measured_range(m, self.sensor_start, self.nsensor)
+        self.backend = backend(self.sensor_start, self.nsensor, self.timestep)
+        nv = m.nv
+        self.ndstate = 2 * nv
+        self.nsigma = 2 * self.ndstate + 1
+        # derived weights (unscented.cc:171-290)
+        lam = self.ndstate * (self.alpha ** 2 - 1.0)
+        self.sigma_step = np.sqrt(self.ndstate + lam)
+        self.weight_mean0 = lam / (self.ndstate + lam)
+        self.weight_covariance0 = self.weight_mean0 + 1.0 - self.alpha ** 2 + self.beta
+        self.weight_sigma = 1.0 / (2.0 * (self.ndstate + lam))
+        self.warnings = 0
+        self.reset()
+
+    def reset(self, state=None, time=0.0, covariance_scale=None, process_scale=None, sensor_scale=None):
+        """Reset (unscented.cc:171-290): state = the home keyframe if the model has one, else qpos0 and zero qvel."""
+        m = self.m
+        self.state, cs, ps, ss = reset_values(m, state, covariance_scale, process_scale, sensor_scale)
+        self.time = float(time)
+        self.covariance = cs * np.eye(self.ndstate)
+        self.noise_process = np.full(self.ndstate, float(ps))
+        self.noise_sensor = np.full(self.nsensordata, float(ss))
+        self.qacc_warmstart = np.zeros(m.nv)
+        self.warnings = 0
+
+    def set_noise(self, process=None, sensor=None):
+        """Diagonal process [ndstate] / sensor [nsensordata] noise; None keeps one."""
+        if process is not None:
+            self.noise_process = np.array(process, float)
+        if sensor is not None:
+            self.noise_sensor = np.array(sensor, float)
+
+    def sigma_points(self):
+        """SigmaPoints (unscented.cc:293-349): [nsigma][nq+nv], nominal last."""
+        m = self.m
+        nq, nv = m.nq, m.nv
+        try:
+            L = np.linalg.cholesky(self.covariance)
+        except np.linalg.LinAlgError:
+            raise EstimatorError("covariance factorisation failed") from None
+        pts = np.zeros((self.nsigma, nq + nv))
+        pts[-1] = self.state
+        for i in range(self.ndstate):
+            col = self.sigma_step * L[:, i]
+            pts[i, :nq] = integrate_pos(m, self.state[:nq], col[:nv], 1.0)
+            pts[i, nq:] = self.state[nq:] + col[nv:]
+            pts[i + self.ndstate, :nq] = integrate_pos(m, self.state[:nq], col[:nv], -1.0)
+            pts[i + self.ndstate, nq:] = self.state[nq:] - col[nv:]
+        return pts
+
+    def _weights(self, w0):
+        w = np.full(self.nsigma, self.weight_sigma)
+        w[-1] = w0
+        return w
+
+    def state_mean(self, states):
+        """Weighted mean of the stepped states, quaternions by QuaternionMeans."""
+        m = self.m
+        mean = self._weights(self.weight_mean0) @ states
+        wc = self._weights(self.weight_covariance0)
+        for j in range(m.njnt):
+            if m.jnt_type[j] in (JNT_FREE, JNT_BALL):
+                a = m.jnt_qposadr[j] + (3 if m.jnt_type[j] == JNT_FREE else 0)
+                mean[a:a + 4] = quaternion_mean(states[:, a:a + 4], wc, states[-1, a:a + 4])
+        return mean
+
+    def update(self, ctrl, sensor, mocap=None):
+        """One filter update from the measured sensor slice [nsensordata]; advances time by the timestep."""
+        m = self.m
+        nq, nv = m.nq, m.nv
+        if mocap is None:
+            mocap = np.concatenate([m.mocap_pos0, m.mocap_quat0], axis=1).reshape(-1) if m.nmocap else np.zeros(0)
+        sigma = self.sigma_points()
+        warm = np.tile(self.qacc_warmstart, (self.nsigma, 1))
+        states, sensors, qacc, nwarn = self.backend.step_sensors(sigma, np.asarray(ctrl, float), mocap, self.time, warm)
+        wm = self._weights(self.weight_mean0)
+        wc = self._weights(self.weight_covariance0)
+        s_mean = self.state_mean(states)
+        y_mean = wm @ sensors
+        ds = np.zeros((self.nsigma, self.ndstate))
+        for i in range(self.nsigma):
+            ds[i, :nv] = differentiate_pos(m, s_mean[:nq], states[i, :nq])
+            ds[i, nv:] = states[i, nq:] - s_mean[nq:]
+        dy = sensors - y_mean
+        cov_yy = np.diag(self.noise_sensor) + (dy.T * wc) @ dy
+        cov_sy = (ds.T * wc) @ dy
+        cov_ss = np.diag(self.noise_process) + (ds.T * wc) @ ds
+        try:
+            Ly = np.linalg.cholesky(cov_yy)
+        except np.linalg.LinAlgError:
+            raise EstimatorError("sensor covariance factorisation failed") from None
+        solve = lambda b: np.linalg.solve(Ly.T, np.linalg.solve(Ly, b))
+        err = np.asarray(sensor, float) - y_mean
+        corr = cov_sy @ solve(err)
+        new = np.empty_like(self.state)
+        new[:nq] = integrate_pos(m, s_mean[:nq], corr[:nv], 1.0)
+        new[nq:] = s_mean[nq:] + corr[nv:]
+        P = cov_ss - cov_sy @ solve(cov_sy.T)
+        self.state = new
+        self.covariance = 0.5 * (P + P.T)
+        self.time = self.time + self.timestep
+        self.qacc_warmstart = qacc[-1].copy()
+        self.warnings += nwarn
+        return self.state
+
+
+class CppUnscented:
+    """The C++ filter (csrc/host/unscented.{h,cc}, mjpc_b200_unscented_*) behind the same attributes as Unscented;
+    settings resolve from the model's numerics exactly as Unscented's do."""
+
+    def __init__(self, m, sensor_start=None, nsensor=None, timestep=None, alpha=None, beta=None, device=0):
+        import ctypes as C
+        from .engine import EngineError, _model_blob, load_library
+        self.C, self.Error = C, EngineError
+        self.lib = load_library()
+        self.lib.mjpc_b200_unscented_last_error.restype = C.c_char_p
+        self.lib.mjpc_b200_unscented_last_error.argtypes = [C.c_void_p]
+        self.lib.mjpc_b200_unscented_destroy.argtypes = [C.c_void_p]
+        self.m = m
+        self.sensor_start, self.nsensor, self.timestep, self.alpha, self.beta = settings(m, sensor_start, nsensor,
+                                                                                         timestep, alpha, beta)
+        self.nsensordata = measured_range(m, self.sensor_start, self.nsensor)
+        self._buf, mb = _model_blob(m)
+        h = C.c_void_p()
+        rc = self.lib.mjpc_b200_unscented_create(C.byref(mb), self.sensor_start, self.nsensor, C.c_double(self.timestep),
+                                                 C.c_double(self.alpha), C.c_double(self.beta), int(device), C.byref(h))
+        if rc != 0:
+            raise EngineError(f"mjpc_b200_unscented_create failed ({rc}): {self.lib.mjpc_b200_last_error().decode()}")
+        self.h = h
+        self.ndstate, self.nsigma = 2 * m.nv, 4 * m.nv + 1
+        self.reset()
+
+    def close(self):
+        if getattr(self, "h", None):
+            self.lib.mjpc_b200_unscented_destroy(self.h)
+            self.h = None
+
+    __del__ = close
+
+    def _pd(self, a):
+        return None if a is None else np.ascontiguousarray(a, np.float64).ctypes.data_as(self.C.POINTER(self.C.c_double))
+
+    def _check(self, rc):
+        if rc != 0:
+            msg = self.lib.mjpc_b200_unscented_last_error(self.h).decode()
+            if "factorisation" in msg:
+                raise EstimatorError(msg)
+            raise self.Error(f"mjpc_b200_unscented error {rc}: {msg}")
+
+    def reset(self, state=None, time=0.0, covariance_scale=None, process_scale=None, sensor_scale=None):
+        x, cs, ps, ss = reset_values(self.m, state, covariance_scale, process_scale, sensor_scale)
+        self._check(self.lib.mjpc_b200_unscented_reset(self.h, self._pd(x), self.C.c_double(time), self.C.c_double(cs),
+                                                       self.C.c_double(ps), self.C.c_double(ss)))
+
+    def set_noise(self, process=None, sensor=None):
+        self._check(self.lib.mjpc_b200_unscented_set_noise(self.h, self._pd(process), self._pd(sensor)))
+
+    def set(self, state, covariance, time):
+        self._check(self.lib.mjpc_b200_unscented_set(self.h, self._pd(state), self._pd(covariance),
+                                                     self.C.c_double(time)))
+
+    def update(self, ctrl, sensor, mocap=None):
+        C = self.C
+        mc = None if mocap is None or len(mocap) == 0 else np.ascontiguousarray(mocap, np.float32)
+        u = np.ascontiguousarray(np.atleast_1d(np.asarray(ctrl, float)))
+        y = np.ascontiguousarray(sensor, np.float64)
+        self._check(self.lib.mjpc_b200_unscented_update(self.h, u.ctypes.data_as(C.POINTER(C.c_double)),
+                                                        y.ctypes.data_as(C.POINTER(C.c_double)),
+                                                        None if mc is None else mc.ctypes.data_as(C.POINTER(C.c_float))))
+        return self.state
+
+    def _get(self):
+        C = self.C
+        x, P = np.zeros(self.m.nq + self.m.nv), np.zeros((self.ndstate, self.ndstate))
+        t, sc = C.c_double(), np.zeros(5)
+        self._check(self.lib.mjpc_b200_unscented_get(self.h, x.ctypes.data_as(C.POINTER(C.c_double)),
+                                                     P.ctypes.data_as(C.POINTER(C.c_double)), C.byref(t),
+                                                     sc.ctypes.data_as(C.POINTER(C.c_double))))
+        return x, P, t.value, sc
+
+    @property
+    def state(self):
+        return self._get()[0]
+
+    @property
+    def covariance(self):
+        return self._get()[1]
+
+    @property
+    def time(self):
+        return self._get()[2]
+
+    @property
+    def warnings(self):
+        return int(self._get()[3][3])

@@ -31,9 +31,11 @@ JNT_FREE, JNT_BALL, JNT_SLIDE, JNT_HINGE = range(4)
 JNT_TYPES = {"free": 0, "ball": 1, "slide": 2, "hinge": 3}
 # sensor types (own enum; only what the residuals / traces read is evaluated)
 SENS_USER, SENS_FRAMEPOS, SENS_JOINTPOS, SENS_TOUCH, SENS_SUBTREECOM, SENS_SUBTREELINVEL, \
-    SENS_FRAMELINVEL, SENS_FRAMEQUAT, SENS_OTHER = range(9)
+    SENS_FRAMELINVEL, SENS_FRAMEQUAT, SENS_OTHER, SENS_JOINTVEL = range(10)
 SENS_TYPES = {"user": 0, "framepos": 1, "jointpos": 2, "touch": 3, "subtreecom": 4,
-              "subtreelinvel": 5, "framelinvel": 6, "framequat": 7}
+              "subtreelinvel": 5, "framelinvel": 6, "framequat": 7, "jointvel": 9}
+# what the measurement path (engine step_sensors, estimators) evaluates
+SENS_MEASURED = (SENS_FRAMEPOS, SENS_JOINTPOS, SENS_TOUCH, SENS_JOINTVEL)
 SENS_DIM = {"framepos": 3, "jointpos": 1, "touch": 1, "subtreecom": 3, "subtreelinvel": 3,
             "framelinvel": 3, "framequat": 4, "jointvel": 1, "frameangvel": 3, "subtreeangmom": 3,
             "actuatorfrc": 1, "framexaxis": 3, "frameyaxis": 3, "framezaxis": 3, "velocimeter": 3,
@@ -414,6 +416,9 @@ class Compiler:
         m.site_bodyid = np.array([a["_body"] for a in self.sites], np.int32).reshape(ns)
         m.site_pos = np.array([_f(a.get("pos"), default=[0, 0, 0]) for a in self.sites]).reshape(ns, 3)
         m.site_quat = np.array([self._orient(a) for a in self.sites]).reshape(ns, 4)
+        # the zone of touch sensors: mjtGeom type and size, MuJoCo's defaults (sphere, 0.005)
+        m.site_type = np.array([GEOM_TYPES[a.get("type", "sphere")] for a in self.sites], np.int32).reshape(ns)
+        m.site_size = np.array([_f(a.get("size"), 3, [0.005, 0.005, 0.005]) for a in self.sites]).reshape(ns, 3)
         m.site_names = [a.get("name", "") for a in self.sites]
 
         # ---------------- bodies
@@ -644,7 +649,7 @@ class Compiler:
                 sens.append(ch)
         n = len(sens)
         s_type = np.zeros(n, np.int32); s_dim = np.zeros(n, np.int32); s_adr = np.zeros(n, np.int32)
-        s_objtype = np.full(n, -1, np.int32); s_objid = np.full(n, -1, np.int32)
+        s_objtype = np.full(n, -1, np.int32); s_objid = np.full(n, -1, np.int32); cutoff = np.zeros(n)
         users, adr = [], 0
         for i, ch in enumerate(sens):
             tag = ch.tag
@@ -665,10 +670,11 @@ class Compiler:
                     s_objid[i] = m.body_names.index(nm)
             elif tag in ("subtreecom", "subtreelinvel"):
                 s_objtype[i], s_objid[i] = OBJ_BODY, m.body_names.index(ch.get("body"))
-            elif tag == "jointpos":
+            elif tag in ("jointpos", "jointvel"):
                 s_objid[i] = m.jnt_names.index(ch.get("joint"))
             elif tag == "touch":
                 s_objtype[i], s_objid[i] = OBJ_SITE, m.site_names.index(ch.get("site"))
+            cutoff[i] = float(ch.get("cutoff", 0))
         nuser = max([len(u) for u in users] + [0])
         s_user = np.zeros((n, max(nuser, 1)))
         for i, u in enumerate(users):
@@ -676,6 +682,7 @@ class Compiler:
         m.nsensor, m.nsensordata, m.nuser_sensor = n, adr, nuser
         m.sensor_type, m.sensor_dim, m.sensor_adr, m.sensor_objtype, m.sensor_objid = s_type, s_dim, s_adr, s_objtype, s_objid
         m.sensor_user = s_user
+        m.sensor_cutoff = cutoff
         m.sensor_names = [ch.get("name", "") for ch in sens]
 
     def _parse_custom(self, m):
@@ -813,6 +820,9 @@ class Compiler:
         m.task_num_norm_parameter = np.array(nparams, np.int32).reshape(-1)
         m.task_norm_parameter = np.array(params, float).reshape(-1)
         m.task_weight_names = m.sensor_names[:num_term]
+        if num_term == 0:   # the particle residual (id 0) would write nq + nv entries into an empty residual
+            from .task import RESIDUAL_NONE
+            m.task_residual_id = RESIDUAL_NONE
         m.task_risk = float(m.numeric.get("task_risk", [0.0])[0])
         # residual parameters: every numeric whose name starts with residual_ (task.cc:38-64)
         pars, pnames = [], []

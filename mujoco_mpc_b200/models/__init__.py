@@ -93,6 +93,11 @@ def cartpole_xml() -> str:
     <numeric name="sampling_exploration" data="0.5"/>
     <numeric name="sampling_trajectories" data="8"/>
     <numeric name="residual_Goal" data="0.0 -1.5 1.5"/>
+    <!-- estimator (cartpole/task.xml:20-24) -->
+    <numeric name="estimator" data="0"/>
+    <numeric name="estimator_sensor_start" data="4"/>
+    <numeric name="estimator_number_sensor" data="2"/>
+    <numeric name="estimator_timestep" data="0.005"/>
   </custom>
   <worldbody>
     <geom name="floor" pos="0 0 -.05" size="4 4 .2" type="plane"/>
@@ -194,6 +199,11 @@ def quadruped_flat_xml(horizon=0.63, trajectories=256) -> str:
     <numeric name="residual_select_Biped type" data="0"/>
     <numeric name="residual_Heading" data="0 -3.14 3.14"/>
     <numeric name="residual_Arm posture" data=".03 0 1"/>
+    <!-- estimator (task_flat.xml:34-38) -->
+    <numeric name="estimator" data="0"/>
+    <numeric name="estimator_sensor_start" data="9"/>
+    <numeric name="estimator_number_sensor" data="21"/>
+    <numeric name="estimator_timestep" data="0.005"/>
   </custom>
   <default>
     <default class="torque">

@@ -32,6 +32,7 @@ SI_GRASP_SITE, SI_CUBE_BODY, SI_GOAL_BODY, SI_KEY_GRASP, SI_SIZE = 0, 1, 2, 3, 4
 TRACK_MOTION_LENGTHS = (121, 154, 115, 78, 145, 188, 260, 279, 39, 510)   # tracking.cc:43-54
 TRACK_FPS = 30.0
 TS_MODE, TS_REFERENCE_TIME, TS_SIZE = 0, 1, 2
+RESIDUAL_NONE = 7            # a model without cost terms (the reference's estimator test models): no residual is evaluated
 
 # quadruped task-state block layout (doubles); ResidualFn members, quadruped.h:160-225
 QS_MODE, QS_MODE_START_TIME, QS_POSITION, QS_HEADING, QS_SPEED, QS_ANGVEL, QS_GROUND = 0, 1, 2, 5, 7, 8, 9
