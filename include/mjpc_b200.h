@@ -229,7 +229,7 @@ int mjpc_b200_step_batch(mjpc_b200_t* h, int B, const float* qpos, const float* 
  * sensors [sensor_start, sensor_start + nsensor) of each PRE-step state are evaluated after the constraint solve
  * (positions, velocities and touch forces of the state the step starts from, as mj_step's sensor stage sees them).
  * Evaluated: jointpos / jointvel of slide and hinge joints, framepos of a site, body (xipos), xbody (xpos) or geom,
- * and touch with a sphere site zone.  warmstart [B][nv] may be NULL (zeros); mocap [7 nmocap] is required when
+ * touch with a sphere site zone, and accelerometer / velocimeter / gyro of a site (in the site frame).  warmstart [B][nv] may be NULL (zeros); mocap [7 nmocap] is required when
  * nmocap > 0.  Outputs: next_states [B][dim_state], sensordata [B][dim] (dim = the range's total sensor dimension),
  * and, when not NULL, qacc [B][nv] and counts [B][4] = {ncon, nefc, solver iterations, warning}, all equal to what
  * mjpc_b200_step_batch returns for the same inputs.  last_kernel_ms times the launch.  A range outside the model's
@@ -263,6 +263,38 @@ int mjpc_b200_unscented_update(mjpc_b200_unscented_t* u, const double* ctrl, con
 int mjpc_b200_unscented_get(const mjpc_b200_unscented_t* u, double* state, double* covariance, double* time,
                             double* scalars);
 const char* mjpc_b200_unscented_last_error(const mjpc_b200_unscented_t* u);
+
+/* MJPC's Kalman state estimator (mjpc/estimators/kalman.cc, class mjpc_b200_host::Kalman in csrc/host/kalman.h): the
+ * filter in double precision on the host, its finite-difference Jacobians as one mjpc_b200_step_sensors launch each
+ * (the centre state and its ndstate tangent-space perturbations x (+) eps e_i, then x (+) -eps e_i when centered) on an
+ * engine handle it owns (max_candidates = 2 ndstate + 1).  Settings are explicit (timestep = estimator_timestep or
+ * opt.timestep, the three noise scales 1e-4; the reference's finite differences are 1e-6 one-sided, an fp64 setting:
+ * mujoco_mpc_b200.estimator.KALMAN_EPSILON / KALMAN_CENTERED are the engine's).  create: measured sensors
+ * [sensor_start, sensor_start + nsensor) of the blob; it steps the reset state once, so a range outside the model's
+ * sensors returns MJPC_B200_ERR_BAD_ARGUMENT and a sensor the engine does not evaluate MJPC_B200_ERR_UNSUPPORTED.
+ * reset / set_noise / set: as for the Unscented filter.  update_measurement: ctrl [nu], the measured sensor slice
+ * [nsensordata], mocap [7 nmocap] or NULL (the model's); C and the predicted sensors come from one launch at the current
+ * state, then the gain, correction and covariance update.  A failed sensor-covariance factorisation returns
+ * MJPC_B200_ERR_BAD_ARGUMENT and leaves state, covariance and time untouched (kalman_last_error names the factor).
+ * update_prediction: A and the next state from one launch with the ctrl and mocap of the last measurement (zeros and
+ * the model's mocap after reset), P = A P A' + diag(process noise), time += timestep.  update: both.  get: state
+ * [nq+nv], covariance, time and scalars[6] = {ndstate, states per launch, nsensordata, steps that raised a warning
+ * since reset, timestep, epsilon}. */
+typedef struct mjpc_b200_kalman mjpc_b200_kalman_t;
+int mjpc_b200_kalman_create(const mjpc_model_blob* model, int sensor_start, int nsensor, double timestep,
+                            double epsilon, int centered, int device, mjpc_b200_kalman_t** out);
+void mjpc_b200_kalman_destroy(mjpc_b200_kalman_t* k);
+int mjpc_b200_kalman_reset(mjpc_b200_kalman_t* k, const double* state, double time, double covariance_scale,
+                           double process_scale, double sensor_scale);
+int mjpc_b200_kalman_set_noise(mjpc_b200_kalman_t* k, const double* process, const double* sensor);
+int mjpc_b200_kalman_set(mjpc_b200_kalman_t* k, const double* state, const double* covariance, double time);
+int mjpc_b200_kalman_update_measurement(mjpc_b200_kalman_t* k, const double* ctrl, const double* sensor,
+                                        const float* mocap);
+int mjpc_b200_kalman_update_prediction(mjpc_b200_kalman_t* k);
+int mjpc_b200_kalman_update(mjpc_b200_kalman_t* k, const double* ctrl, const double* sensor, const float* mocap);
+int mjpc_b200_kalman_get(const mjpc_b200_kalman_t* k, double* state, double* covariance, double* time,
+                         double* scalars);
+const char* mjpc_b200_kalman_last_error(const mjpc_b200_kalman_t* k);
 
 /* Per-candidate execution statistics of the last rollout, stats [N][12] = {SM cycles, Newton iterations, contacts,
  * constraint rows (summed over steps), 8 per-phase cycle counters (zero unless built with -DMJPC_PHASE_TIMING)}. */

@@ -664,8 +664,13 @@ __device__ __noinline__ void k_residual(Ctx& c) {
 // MuJoCo's sensor types the estimators measure (codes of mujoco_mpc_b200/mjcf.py SENS_*).  One row of the handle's
 // sensor table per sensor (built on the host from the blob's sensor_* / site_* entries, never part of the model pack):
 // adr is the sensor's sensordata address, radius the sphere zone of a touch sensor's site.
-enum { SENS_FRAMEPOS = 1, SENS_JOINTPOS = 2, SENS_TOUCH = 3, SENS_JOINTVEL = 9 };
+enum { SENS_FRAMEPOS = 1, SENS_JOINTPOS = 2, SENS_TOUCH = 3, SENS_JOINTVEL = 9, SENS_ACCELEROMETER = 10,
+       SENS_VELOCIMETER = 11, SENS_GYRO = 12 };
 struct DevSensor { int type, objtype, objid, adr; float radius; };
+// sensordata entries of one measured sensor
+__host__ __device__ inline int sensor_dim(int type) {
+  return type == SENS_FRAMEPOS || type == SENS_ACCELEROMETER || type == SENS_VELOCIMETER || type == SENS_GYRO ? 3 : 1;
+}
 
 // Sensors [0, n) of `tab`, written to out[adr - adr0 ..].  Runs after k_forward and before k_euler: positions and
 // velocities are those of the pre-step state, touch reads the constraint forces of that state's solve (as mj_step's
@@ -677,6 +682,14 @@ struct DevSensor { int type, objtype, objid, adr; float radius; };
 //                        along the contact normal, oriented into the site's body, hits it.  The normal force is the
 //                        normal row's force (elliptic, frictionless) or the sum of the 2 (condim - 1) pyramid edge
 //                        forces; the constraint phase has rewritten con_dim of a pyramidal contact as that row count.
+//   gyro / velocimeter   the angular / linear velocity of the site in the site frame (mj_objectVelocity, flg_local):
+//                        R' w and R' (v - (site_xpos - subtree_com[root]) x w) with (w, v) = cvel of the site's body
+//                        and R = site_xmat = quat2mat(xquat[body] site_quat) (the device keeps no site_xmat)
+//   accelerometer        the linear acceleration of the site in the site frame (mj_objectAcceleration, flg_local):
+//                        the post-constraint com-based acceleration a of the site's body (mj_rnePostConstraint's cacc,
+//                        which is additive along the tree: [0, -gravity] + sum of cdof_dot qvel + cdof qacc over the
+//                        dofs on the path from the body to the world, walked here by the sensor's lane instead of
+//                        written to cacc), shifted to the site like the velocity, rotated, plus (R' w) x (R' v_site)
 template <class SP>
 __device__ __noinline__ void k_sensors(Ctx& c, const DevSensor* __restrict__ tab, int n, int adr0, float* out) {
   auto&& M = SP::model(c);
@@ -714,6 +727,39 @@ __device__ __noinline__ void k_sensors(Ctx& c, const DevSensor* __restrict__ tab
         if (cc <= 0.f || (b < 0.f && b * b - cc >= 0.f)) sum += f;
       }
       o[0] = sum;
+    } else if (S.type == SENS_GYRO || S.type == SENS_VELOCIMETER || S.type == SENS_ACCELEROMETER) {
+      // the world-frame vector first, rotated once at the end: (R' w) x (R' v) = R' (w x v)
+      const int body = MI(site_bodyid)[S.objid];
+      const float* cv = DF(cvel) + 6 * body;
+      const float* com = DF(subtree_com) + 3 * MI(body_rootid)[body];
+      float off[3], w[3], t[3], vec[3];
+      for (int q = 0; q < 3; q++) { off[q] = DF(site_xpos)[3 * S.objid + q] - com[q]; w[q] = cv[q]; }
+      if (S.type == SENS_GYRO) {
+        for (int q = 0; q < 3; q++) vec[q] = w[q];
+      } else {
+        cross3(t, off, w);
+        for (int q = 0; q < 3; q++) vec[q] = cv[3 + q] - t[q];   // the site's linear velocity
+        if (S.type == SENS_ACCELEROMETER) {
+          const int *parent = MI(body_parentid), *dofadr = MI(body_dofadr), *dofnum = MI(body_dofnum);
+          const float *cdof = DF(cdof), *cdof_dot = DF(cdof_dot), *qvel = DF(qvel), *qacc = DF(qacc);
+          float a[6] = {0.f, 0.f, 0.f, -CM(c).gravity[0], -CM(c).gravity[1], -CM(c).gravity[2]};
+          MJPC_ROLL
+          for (int b = body; b > 0; b = parent[b]) {
+            MJPC_ROLL
+            for (int i = dofadr[b]; i < dofadr[b] + dofnum[b]; i++)
+              for (int q = 0; q < 6; q++) a[q] += cdof_dot[6 * i + q] * qvel[i] + cdof[6 * i + q] * qacc[i];
+          }
+          float wv[3];
+          cross3(wv, w, vec);
+          cross3(t, off, a);
+          for (int q = 0; q < 3; q++) vec[q] = a[3 + q] - t[q] + wv[q];
+        }
+      }
+      // site_xmat = quat2mat(xquat[body] site_quat), as mj_kinematics forms it
+      float qs[4], R[9];
+      quat_mul(qs, DF(xquat) + 4 * body, MF(site_quat) + 4 * S.objid);
+      quat2mat(R, qs);
+      rot_vec_T(o, R, vec);
     }
   }
   __syncwarp();

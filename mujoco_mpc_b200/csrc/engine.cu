@@ -438,10 +438,13 @@ int mjpc_b200_create(const mjpc_model_blob* model, int max_candidates, int max_h
         } else if (ty[i] == SENS_TOUCH) {
           if (st[oid[i]] != GEOM_SPHERE) why = "touch zone other than a sphere site";
           S.radius = (float)ss[3 * oid[i]];
+        } else if (ty[i] == SENS_ACCELEROMETER || ty[i] == SENS_VELOCIMETER || ty[i] == SENS_GYRO) {
+          if (ot[i] != OBJ_SITE) why = "accelerometer / velocimeter / gyro of an object other than a site";
         } else {
-          why = "sensor type " + std::to_string(ty[i]) + " (only jointpos, jointvel, framepos and touch are evaluated)";
+          why = "sensor type " + std::to_string(ty[i]) +
+                " (only jointpos, jointvel, framepos, touch, accelerometer, velocimeter and gyro are evaluated)";
         }
-        if (why.empty() && dim[i] != (ty[i] == SENS_FRAMEPOS ? 3 : 1)) why = "unexpected sensor dimension";
+        if (why.empty() && dim[i] != sensor_dim(ty[i])) why = "unexpected sensor dimension";
         if (why.empty() && cutoff[i] != 0.0) why = "cutoff is not modelled";
         h->sensors.push_back(S);
         h->sensor_why.push_back(why);
@@ -775,7 +778,7 @@ static int step_impl(mjpc_b200_t* h, const void* fn, int B, const float* qpos, c
   const size_t Bs = B, nq = M.nq, nv = M.nv, nu = M.nu, nr = std::max(M.num_residual, 1), nm = 7 * (size_t)M.nmocap,
                nts = (size_t)M.task_state_size;
   const int adr0 = ns ? h->sensors[s0].adr : 0;
-  const size_t nsd = ns ? (size_t)(h->sensors[s0 + ns - 1].adr - adr0 + (h->sensors[s0 + ns - 1].type == SENS_FRAMEPOS ? 3 : 1)) : 0;
+  const size_t nsd = ns ? (size_t)(h->sensors[s0 + ns - 1].adr - adr0 + sensor_dim(h->sensors[s0 + ns - 1].type)) : 0;
   size_t words = 0;
   auto take = [&](size_t n) { const size_t at = words; words += n; return at; };
   const size_t o_qpos = take(Bs * nq), o_qvel = take(Bs * nv), o_ctrl = take(Bs * nu), o_warm = take(Bs * nv),

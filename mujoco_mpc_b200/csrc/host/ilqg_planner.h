@@ -46,6 +46,8 @@ struct iLQGPolicyModel {       // the few mjModel fields the policy needs, read 
 };
 // StateDiff (utilities.cc:543-553): dx [2 nv] = x_to (-) x_from, positions in the tangent space (mj_differentiatePos)
 void StateDiff(const iLQGPolicyModel& m, double* dx, const double* x_to, const double* x_from);
+// mj_integratePos: qpos (+) scale dq, quaternions through mju_quatIntegrate (q exp(scale v / 2), normalised)
+void IntegratePos(const iLQGPolicyModel& m, double* qpos, const double* dq, double scale);
 void iLQGPolicyAction(const iLQGPolicyModel& m, const float* u_nom, const float* x_nom, const double* t_nom,
                       const float* gains, int horizon, int representation, double feedback_scaling, const double* state,
                       double time, double* action);

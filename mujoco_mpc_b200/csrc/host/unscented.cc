@@ -12,38 +12,6 @@ namespace mjpc_b200_host {
 
 namespace {
 
-// mju_quatIntegrate: q * exp(scale v / 2), normalised
-void QuatIntegrate(double* q, const double* v, double scale) {
-  const double w[3] = {v[0] * scale, v[1] * scale, v[2] * scale};
-  const double a = std::sqrt(w[0] * w[0] + w[1] * w[1] + w[2] * w[2]);
-  double r[4] = {1, 0, 0, 0};
-  if (a >= 1e-15) {
-    const double s = std::sin(a / 2) / a;
-    r[0] = std::cos(a / 2); r[1] = s * w[0]; r[2] = s * w[1]; r[3] = s * w[2];
-  }
-  const double o[4] = {q[0] * r[0] - q[1] * r[1] - q[2] * r[2] - q[3] * r[3],
-                       q[0] * r[1] + q[1] * r[0] + q[2] * r[3] - q[3] * r[2],
-                       q[0] * r[2] - q[1] * r[3] + q[2] * r[0] + q[3] * r[1],
-                       q[0] * r[3] + q[1] * r[2] - q[2] * r[1] + q[3] * r[0]};
-  const double n = std::sqrt(o[0] * o[0] + o[1] * o[1] + o[2] * o[2] + o[3] * o[3]);
-  for (int k = 0; k < 4; k++) q[k] = o[k] / n;
-}
-
-// mj_integratePos: qpos (+) scale dq
-void IntegratePos(const iLQGPolicyModel& m, double* qpos, const double* dq, double scale) {
-  for (size_t j = 0; j < m.jnt_type.size(); j++) {
-    const int a = m.jnt_qposadr[j], d = m.jnt_dofadr[j];
-    if (m.jnt_type[j] == 0) {
-      for (int c = 0; c < 3; c++) qpos[a + c] += scale * dq[d + c];
-      QuatIntegrate(qpos + a + 3, dq + d + 3, scale);
-    } else if (m.jnt_type[j] == 1) {
-      QuatIntegrate(qpos + a, dq + d, scale);
-    } else {
-      qpos[a] += scale * dq[d];
-    }
-  }
-}
-
 // Principal eigenvector of a symmetric 4 x 4 matrix by cyclic Jacobi rotations (converged to rounding), with the sign
 // that agrees with `ref`.  Stands for PrincipalEigenVector4 (utilities.cc:1476+) in QuaternionMeans.
 void PrincipalEigenVector4(double* out, const double* K, const double* ref) {
@@ -86,6 +54,35 @@ void PrincipalEigenVector4(double* out, const double* K, const double* ref) {
 
 }  // namespace
 
+int LoadEstimatorBlob(const mjpc_model_blob* model, const iLQGPolicyModel& m, std::vector<int>* dims, int* nmocap,
+                      std::vector<float>* mocap0, std::vector<double>* key_state) {
+  try {
+    mjpc_dev::Blob b(model->data, model->nbytes);
+    *dims = b.ints("sensor_dim");
+    *nmocap = b.i("nmocap");
+    const std::vector<int> mid = b.ints("body_mocapid");
+    const std::vector<double> bp = b.reals("body_pos"), bq = b.reals("body_quat"), q0 = b.reals("qpos0");
+    mocap0->assign(7 * (size_t)*nmocap, 0.f);
+    for (size_t i = 0; i < mid.size(); i++)
+      if (mid[i] >= 0) {
+        for (int c = 0; c < 3; c++) (*mocap0)[7 * mid[i] + c] = (float)bp[3 * i + c];
+        for (int c = 0; c < 4; c++) (*mocap0)[7 * mid[i] + 3 + c] = (float)bq[4 * i + c];
+      }
+    const int nkey = b.i("nkey");
+    key_state->assign(m.nq + m.nv, 0.0);
+    if (nkey > 0) {
+      const std::vector<double> kq = b.reals("key_qpos"), kv = b.reals("key_qvel");
+      std::copy(kq.begin(), kq.begin() + m.nq, key_state->begin());
+      std::copy(kv.begin(), kv.begin() + m.nv, key_state->begin() + m.nq);
+    } else {
+      std::copy(q0.begin(), q0.end(), key_state->begin());
+    }
+  } catch (const std::exception&) {
+    return MJPC_B200_ERR_BAD_BLOB;
+  }
+  return 0;
+}
+
 Unscented::~Unscented() { if (engine_) mjpc_b200_destroy(engine_); }
 
 int Unscented::Initialize(const mjpc_model_blob* model, int sensor_start, int nsensor, double timestep_,
@@ -93,28 +90,7 @@ int Unscented::Initialize(const mjpc_model_blob* model, int sensor_start, int ns
   if (!model || !(timestep_ > 0)) { error = "unscented: bad argument"; return MJPC_B200_ERR_BAD_ARGUMENT; }
   if (int rc = m_.Load(model)) { error = "unscented: bad blob"; return rc; }
   std::vector<int> dims;
-  try {
-    mjpc_dev::Blob b(model->data, model->nbytes);
-    dims = b.ints("sensor_dim");
-    nmocap_ = b.i("nmocap");
-    const std::vector<int> mid = b.ints("body_mocapid");
-    const std::vector<double> bp = b.reals("body_pos"), bq = b.reals("body_quat"), q0 = b.reals("qpos0");
-    mocap0_.assign(7 * (size_t)nmocap_, 0.f);
-    for (size_t i = 0; i < mid.size(); i++)
-      if (mid[i] >= 0) {
-        for (int c = 0; c < 3; c++) mocap0_[7 * mid[i] + c] = (float)bp[3 * i + c];
-        for (int c = 0; c < 4; c++) mocap0_[7 * mid[i] + 3 + c] = (float)bq[4 * i + c];
-      }
-    const int nkey = b.i("nkey");
-    key_state_.assign(m_.nq + m_.nv, 0.0);
-    if (nkey > 0) {
-      const std::vector<double> kq = b.reals("key_qpos"), kv = b.reals("key_qvel");
-      std::copy(kq.begin(), kq.begin() + m_.nq, key_state_.begin());
-      std::copy(kv.begin(), kv.begin() + m_.nv, key_state_.begin() + m_.nq);
-    } else {
-      std::copy(q0.begin(), q0.end(), key_state_.begin());
-    }
-  } catch (const std::exception&) {
+  if (LoadEstimatorBlob(model, m_, &dims, &nmocap_, &mocap0_, &key_state_)) {
     error = "unscented: blob without sensor entries";
     return MJPC_B200_ERR_BAD_BLOB;
   }

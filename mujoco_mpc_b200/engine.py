@@ -35,7 +35,10 @@ EXPORTS = ["mjpc_b200_version", "mjpc_b200_last_error", "mjpc_b200_create", "mjp
            "mjpc_b200_step_debug", "mjpc_b200_step_debug_contacts", "mjpc_b200_step_batch", "mjpc_b200_step_sensors",
            "mjpc_b200_unscented_create", "mjpc_b200_unscented_destroy", "mjpc_b200_unscented_reset",
            "mjpc_b200_unscented_set_noise", "mjpc_b200_unscented_set", "mjpc_b200_unscented_update",
-           "mjpc_b200_unscented_get", "mjpc_b200_unscented_last_error", "mjpc_b200_comm_unique_id", "mjpc_b200_comm_init",
+           "mjpc_b200_unscented_get", "mjpc_b200_unscented_last_error", "mjpc_b200_kalman_create", "mjpc_b200_kalman_destroy",
+           "mjpc_b200_kalman_reset", "mjpc_b200_kalman_set_noise", "mjpc_b200_kalman_set",
+           "mjpc_b200_kalman_update_measurement", "mjpc_b200_kalman_update_prediction", "mjpc_b200_kalman_update",
+           "mjpc_b200_kalman_get", "mjpc_b200_kalman_last_error", "mjpc_b200_comm_unique_id", "mjpc_b200_comm_init",
            "mjpc_b200_comm_info", "mjpc_b200_rollout_spline_sharded", "mjpc_b200_fetch_trajectory_sharded",
            "mjpc_b200_fetch_stats", "mjpc_b200_launch_count", "mjpc_b200_last_kernel_ms", "mjpc_b200_last_kernel_static",
            "mjpc_b200_spec_words", "mjpc_b200_upload_spline_inputs",

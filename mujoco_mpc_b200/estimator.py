@@ -1,4 +1,5 @@
-"""MJPC's Unscented state estimator (mjpc/estimators/unscented.cc) with its sigma-point steps on a step backend.
+"""MJPC's Unscented (mjpc/estimators/unscented.cc) and Kalman (mjpc/estimators/kalman.cc) state estimators with their
+steps on a step backend.
 
 The filter arithmetic is double precision on the host: a Cholesky factor of the covariance, weighted means and
 covariances of at most 2 ndstate + 1 points and one Cholesky factor of the sensor covariance.  The sigma-point steps
@@ -24,6 +25,18 @@ Documented differences from the reference:
     solution is unique to the solver tolerance, so this changes results only at that level;
   * ``update`` takes mocap (default: the model's), the reference's mjData keeps the model's;
   * ``update`` takes the measured slice [nsensordata] of the sensors, not the whole sensordata.
+
+The Kalman filter (``Kalman``, kalman.cc) linearises by finite differences instead: the centre state and its
+tangent-space perturbations x (+) eps e_i (then x (+) -eps e_i when centred) are one backend call per Jacobian, the
+sensor Jacobian C from the pre-step sensors at the current state (UpdateMeasurement, :188-276), the dynamics Jacobian A
+from the next states at the corrected state (UpdatePrediction, :279-323).  Its documented differences from the
+reference are the Unscented filter's (the warm start is the centre state's qacc of the previous call), plus:
+  * a failed sensor-covariance factorisation raises ``EstimatorError`` and leaves state, covariance and time untouched;
+  * ``update_prediction`` uses the ctrl and mocap of the last measurement, as the reference's mjData does;
+  * time: both calls run at ``time`` and ``update_prediction`` advances it by the timestep (the reference leaves its
+    ``time`` member alone and its mjData's clock advances inside mj_step);
+  * the finite differences default to KALMAN_CENTERED with KALMAN_EPSILON: the reference's 1e-6 one-sided is an fp64
+    setting, and the engine steps in fp32 (DESIGN.md, "Kalman filter", has the sweep that chose them).
 """
 from __future__ import annotations
 
@@ -142,7 +155,8 @@ def quaternion_mean(quats, weights, reference):
 
 # ------------------------------------------------------------------------------------------------------- backends
 class EngineBackend:
-    """The sigma-point steps as one launch of the CUDA engine (mjpc_b200_step_sensors)."""
+    """The sigma-point (Unscented) or finite-difference (Kalman) steps as one launch of the CUDA engine
+    (mjpc_b200_step_sensors)."""
 
     def __init__(self, engine, sensor_start, nsensor, timestep):
         self.engine, self.sensor_start, self.nsensor = engine, int(sensor_start), int(nsensor)
@@ -166,8 +180,8 @@ def measured_range(m, sensor_start, nsensor):
                              % (sensor_start, sensor_start + nsensor, m.nsensor))
     for i in range(sensor_start, sensor_start + nsensor):
         if int(m.sensor_type[i]) not in SENS_MEASURED:
-            raise EstimatorError("sensor %d (%s) is not a measured sensor type (jointpos, jointvel, framepos, touch)"
-                                 % (i, m.sensor_names[i]))
+            raise EstimatorError("sensor %d (%s) is not a measured sensor type (jointpos, jointvel, framepos, touch, "
+                                 "accelerometer, velocimeter, gyro)" % (i, m.sensor_names[i]))
         if float(m.sensor_cutoff[i]) != 0.0:
             raise EstimatorError("sensor %d (%s): cutoff is not modelled" % (i, m.sensor_names[i]))
     return int(np.sum(m.sensor_dim[sensor_start:sensor_start + nsensor]))
@@ -384,6 +398,226 @@ class CppUnscented:
         self._check(self.lib.mjpc_b200_unscented_get(self.h, x.ctypes.data_as(C.POINTER(C.c_double)),
                                                      P.ctypes.data_as(C.POINTER(C.c_double)), C.byref(t),
                                                      sc.ctypes.data_as(C.POINTER(C.c_double))))
+        return x, P, t.value, sc
+
+    @property
+    def state(self):
+        return self._get()[0]
+
+    @property
+    def covariance(self):
+        return self._get()[1]
+
+    @property
+    def time(self):
+        return self._get()[2]
+
+    @property
+    def warnings(self):
+        return int(self._get()[3][3])
+
+
+# ------------------------------------------------------------------------------------------------------ Kalman
+KALMAN_EPSILON = 1e-3    # the engine's finite differences (profiles/kalman_epsilon_sweep.py, DESIGN.md)
+KALMAN_CENTERED = True
+
+
+def _default_mocap(m):
+    return np.concatenate([m.mocap_pos0, m.mocap_quat0], axis=1).reshape(-1) if m.nmocap else np.zeros(0)
+
+
+class Kalman:
+    """mjpc::Kalman.  `backend(sensor_start, nsensor, timestep)` returns the object that runs the steps (see
+    EngineBackend); settings left None default from the model's numerics as GetNumberOrDefault does."""
+
+    def __init__(self, m, backend, sensor_start=None, nsensor=None, timestep=None, epsilon=KALMAN_EPSILON,
+                 centered=KALMAN_CENTERED):
+        self.m = m
+        self.sensor_start, self.nsensor, self.timestep = settings(m, sensor_start, nsensor, timestep)[:3]
+        self.nsensordata = measured_range(m, self.sensor_start, self.nsensor)
+        self.backend = backend(self.sensor_start, self.nsensor, self.timestep)
+        self.epsilon, self.centered = float(epsilon), bool(centered)
+        self.ndstate = 2 * m.nv
+        self.nstates = (2 if self.centered else 1) * self.ndstate + 1
+        self.warnings = 0
+        self.reset()
+
+    def reset(self, state=None, time=0.0, covariance_scale=None, process_scale=None, sensor_scale=None):
+        """Reset (kalman.cc:113-185): state = the home keyframe if the model has one, else qpos0 and zero qvel."""
+        m = self.m
+        self.state, cs, ps, ss = reset_values(m, state, covariance_scale, process_scale, sensor_scale)
+        self.time = float(time)
+        self.covariance = cs * np.eye(self.ndstate)
+        self.noise_process = np.full(self.ndstate, float(ps))
+        self.noise_sensor = np.full(self.nsensordata, float(ss))
+        self.qacc_warmstart = np.zeros(m.nv)
+        self.ctrl, self.mocap = np.zeros(m.nu), _default_mocap(m)
+        self.warnings = 0
+
+    def set_noise(self, process=None, sensor=None):
+        """Diagonal process [ndstate] / sensor [nsensordata] noise; None keeps one."""
+        if process is not None:
+            self.noise_process = np.array(process, float)
+        if sensor is not None:
+            self.noise_sensor = np.array(sensor, float)
+
+    def perturbed(self):
+        """[nstates][nq+nv]: the state, then x (+) eps e_i for i < ndstate, then (centred) x (+) -eps e_i; positions
+        through mj_integratePos, as mjd_transitionFD perturbs them."""
+        m = self.m
+        nq, nv, n = m.nq, m.nv, self.ndstate
+        X = np.tile(self.state, (self.nstates, 1))
+        for r in range(1, self.nstates):
+            i, e = (r - 1) % n, self.epsilon if r - 1 < n else -self.epsilon
+            if i < nv:
+                d = np.zeros(nv)
+                d[i] = 1.0
+                X[r, :nq] = integrate_pos(m, self.state[:nq], d, e)
+            else:
+                X[r, nq + i - nv] += e
+        return X
+
+    def _step(self, ctrl, mocap):
+        warm = np.tile(self.qacc_warmstart, (self.nstates, 1))
+        return self.backend.step_sensors(self.perturbed(), np.asarray(ctrl, float), mocap, self.time, warm)
+
+    def _column(self, plus, r):
+        """Finite-difference column r of a Jacobian from the rows [nstates][...] of one step (difference `plus`)."""
+        n, h = self.ndstate, (2 * self.epsilon if self.centered else self.epsilon)
+        return plus(r + 1, r + 1 + n if self.centered else 0) / h
+
+    def update_measurement(self, ctrl, sensor, mocap=None):
+        """UpdateMeasurement (kalman.cc:188-276) from the measured sensor slice [nsensordata]."""
+        m = self.m
+        nq, nv = m.nq, m.nv
+        mocap = _default_mocap(m) if mocap is None else np.asarray(mocap, float)
+        nxt, y, qacc, nwarn = self._step(ctrl, mocap)
+        C = np.stack([self._column(lambda a, b: y[a] - y[b], i) for i in range(self.ndstate)], axis=1)
+        P = self.covariance
+        PCt = P @ C.T
+        S = C @ PCt + np.diag(self.noise_sensor)
+        try:
+            L = np.linalg.cholesky(S)
+        except np.linalg.LinAlgError:
+            raise EstimatorError("sensor covariance factorisation failed") from None
+        solve = lambda b: np.linalg.solve(L.T, np.linalg.solve(L, b))
+        corr = PCt @ solve(np.asarray(sensor, float) - y[0])
+        new = np.empty_like(self.state)
+        new[:nq] = integrate_pos(m, self.state[:nq], corr[:nv], 1.0)
+        new[nq:] = self.state[nq:] + corr[nv:]
+        P = P - PCt @ solve(PCt.T)
+        self.state, self.covariance = new, 0.5 * (P + P.T)
+        self.ctrl, self.mocap = np.atleast_1d(np.asarray(ctrl, float)).copy(), mocap
+        self.qacc_warmstart = qacc[0].copy()
+        self.warnings += nwarn
+        return self.state
+
+    def update_prediction(self):
+        """UpdatePrediction (kalman.cc:279-323) with the ctrl and mocap of the last measurement; advances time."""
+        m = self.m
+        nq = m.nq
+        nxt, _, qacc, nwarn = self._step(self.ctrl, self.mocap)
+
+        def diff(a, b):
+            return np.concatenate([differentiate_pos(m, nxt[b, :nq], nxt[a, :nq]), nxt[a, nq:] - nxt[b, nq:]])
+        A = np.stack([self._column(diff, i) for i in range(self.ndstate)], axis=1)
+        P = A @ self.covariance @ A.T + np.diag(self.noise_process)
+        self.state, self.covariance = nxt[0].copy(), 0.5 * (P + P.T)
+        self.time = self.time + self.timestep
+        self.qacc_warmstart = qacc[0].copy()
+        self.warnings += nwarn
+        return self.state
+
+    def update(self, ctrl, sensor, mocap=None):
+        """update_measurement, then update_prediction: the state predicted for the next step."""
+        self.update_measurement(ctrl, sensor, mocap)
+        return self.update_prediction()
+
+
+class CppKalman:
+    """The C++ filter (csrc/host/kalman.{h,cc}, mjpc_b200_kalman_*) behind the same attributes as Kalman; settings
+    resolve from the model's numerics exactly as Kalman's do."""
+
+    def __init__(self, m, sensor_start=None, nsensor=None, timestep=None, epsilon=KALMAN_EPSILON,
+                 centered=KALMAN_CENTERED, device=0):
+        import ctypes as C
+        from .engine import EngineError, _model_blob, load_library
+        self.C, self.Error = C, EngineError
+        self.lib = load_library()
+        self.lib.mjpc_b200_kalman_last_error.restype = C.c_char_p
+        self.lib.mjpc_b200_kalman_last_error.argtypes = [C.c_void_p]
+        self.lib.mjpc_b200_kalman_destroy.argtypes = [C.c_void_p]
+        self.m = m
+        self.sensor_start, self.nsensor, self.timestep = settings(m, sensor_start, nsensor, timestep)[:3]
+        self.nsensordata = measured_range(m, self.sensor_start, self.nsensor)
+        self.epsilon, self.centered = float(epsilon), bool(centered)
+        self._buf, mb = _model_blob(m)
+        h = C.c_void_p()
+        rc = self.lib.mjpc_b200_kalman_create(C.byref(mb), self.sensor_start, self.nsensor, C.c_double(self.timestep),
+                                              C.c_double(self.epsilon), int(self.centered), int(device), C.byref(h))
+        if rc != 0:
+            raise EngineError(f"mjpc_b200_kalman_create failed ({rc}): {self.lib.mjpc_b200_last_error().decode()}")
+        self.h = h
+        self.ndstate = 2 * m.nv
+        self.nstates = (2 if self.centered else 1) * self.ndstate + 1
+        self.reset()
+
+    def close(self):
+        if getattr(self, "h", None):
+            self.lib.mjpc_b200_kalman_destroy(self.h)
+            self.h = None
+
+    __del__ = close
+
+    def _pd(self, a):
+        return None if a is None else np.ascontiguousarray(a, np.float64).ctypes.data_as(self.C.POINTER(self.C.c_double))
+
+    def _check(self, rc):
+        if rc != 0:
+            msg = self.lib.mjpc_b200_kalman_last_error(self.h).decode()
+            if "factorisation" in msg:
+                raise EstimatorError(msg)
+            raise self.Error(f"mjpc_b200_kalman error {rc}: {msg}")
+
+    def reset(self, state=None, time=0.0, covariance_scale=None, process_scale=None, sensor_scale=None):
+        x, cs, ps, ss = reset_values(self.m, state, covariance_scale, process_scale, sensor_scale)
+        self._check(self.lib.mjpc_b200_kalman_reset(self.h, self._pd(x), self.C.c_double(time), self.C.c_double(cs),
+                                                    self.C.c_double(ps), self.C.c_double(ss)))
+
+    def set_noise(self, process=None, sensor=None):
+        self._check(self.lib.mjpc_b200_kalman_set_noise(self.h, self._pd(process), self._pd(sensor)))
+
+    def set(self, state, covariance, time):
+        self._check(self.lib.mjpc_b200_kalman_set(self.h, self._pd(state), self._pd(covariance), self.C.c_double(time)))
+
+    def _args(self, ctrl, sensor, mocap):
+        C = self.C
+        mc = None if mocap is None or len(mocap) == 0 else np.ascontiguousarray(mocap, np.float32)
+        u = np.ascontiguousarray(np.atleast_1d(np.asarray(ctrl, float)))
+        y = np.ascontiguousarray(sensor, np.float64)
+        self._keep = (u, y, mc)
+        return (u.ctypes.data_as(C.POINTER(C.c_double)), y.ctypes.data_as(C.POINTER(C.c_double)),
+                None if mc is None else mc.ctypes.data_as(C.POINTER(C.c_float)))
+
+    def update_measurement(self, ctrl, sensor, mocap=None):
+        self._check(self.lib.mjpc_b200_kalman_update_measurement(self.h, *self._args(ctrl, sensor, mocap)))
+        return self.state
+
+    def update_prediction(self):
+        self._check(self.lib.mjpc_b200_kalman_update_prediction(self.h))
+        return self.state
+
+    def update(self, ctrl, sensor, mocap=None):
+        self._check(self.lib.mjpc_b200_kalman_update(self.h, *self._args(ctrl, sensor, mocap)))
+        return self.state
+
+    def _get(self):
+        C = self.C
+        x, P = np.zeros(self.m.nq + self.m.nv), np.zeros((self.ndstate, self.ndstate))
+        t, sc = C.c_double(), np.zeros(6)
+        self._check(self.lib.mjpc_b200_kalman_get(self.h, x.ctypes.data_as(C.POINTER(C.c_double)),
+                                                  P.ctypes.data_as(C.POINTER(C.c_double)), C.byref(t),
+                                                  sc.ctypes.data_as(C.POINTER(C.c_double))))
         return x, P, t.value, sc
 
     @property

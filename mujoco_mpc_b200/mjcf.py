@@ -31,11 +31,16 @@ JNT_FREE, JNT_BALL, JNT_SLIDE, JNT_HINGE = range(4)
 JNT_TYPES = {"free": 0, "ball": 1, "slide": 2, "hinge": 3}
 # sensor types (own enum; only what the residuals / traces read is evaluated)
 SENS_USER, SENS_FRAMEPOS, SENS_JOINTPOS, SENS_TOUCH, SENS_SUBTREECOM, SENS_SUBTREELINVEL, \
-    SENS_FRAMELINVEL, SENS_FRAMEQUAT, SENS_OTHER, SENS_JOINTVEL = range(10)
+    SENS_FRAMELINVEL, SENS_FRAMEQUAT, SENS_OTHER, SENS_JOINTVEL, SENS_ACCELEROMETER, SENS_VELOCIMETER, \
+    SENS_GYRO = range(13)
 SENS_TYPES = {"user": 0, "framepos": 1, "jointpos": 2, "touch": 3, "subtreecom": 4,
-              "subtreelinvel": 5, "framelinvel": 6, "framequat": 7, "jointvel": 9}
+              "subtreelinvel": 5, "framelinvel": 6, "framequat": 7, "jointvel": 9, "accelerometer": 10,
+              "velocimeter": 11, "gyro": 12}
 # what the measurement path (engine step_sensors, estimators) evaluates
-SENS_MEASURED = (SENS_FRAMEPOS, SENS_JOINTPOS, SENS_TOUCH, SENS_JOINTVEL)
+SENS_MEASURED = (SENS_FRAMEPOS, SENS_JOINTPOS, SENS_TOUCH, SENS_JOINTVEL, SENS_ACCELEROMETER, SENS_VELOCIMETER,
+                 SENS_GYRO)
+# the IMU sensors: 3-vectors in the frame of their site
+SENS_IMU = (SENS_ACCELEROMETER, SENS_VELOCIMETER, SENS_GYRO)
 SENS_DIM = {"framepos": 3, "jointpos": 1, "touch": 1, "subtreecom": 3, "subtreelinvel": 3,
             "framelinvel": 3, "framequat": 4, "jointvel": 1, "frameangvel": 3, "subtreeangmom": 3,
             "actuatorfrc": 1, "framexaxis": 3, "frameyaxis": 3, "framezaxis": 3, "velocimeter": 3,
@@ -672,7 +677,7 @@ class Compiler:
                 s_objtype[i], s_objid[i] = OBJ_BODY, m.body_names.index(ch.get("body"))
             elif tag in ("jointpos", "jointvel"):
                 s_objid[i] = m.jnt_names.index(ch.get("joint"))
-            elif tag == "touch":
+            elif tag in ("touch", "accelerometer", "velocimeter", "gyro"):
                 s_objtype[i], s_objid[i] = OBJ_SITE, m.site_names.index(ch.get("site"))
             cutoff[i] = float(ch.get("cutoff", 0))
         nuser = max([len(u) for u in users] + [0])

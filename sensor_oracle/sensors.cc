@@ -10,6 +10,12 @@
 //                        ray from the point along the contact normal, oriented into the site's body, hits the zone.
 //                        Normal force: the normal row (elliptic / frictionless) or the sum of the 2 (condim - 1)
 //                        pyramid edges.
+//   gyro / velocimeter   mj_objectVelocity of the site with flg_local: the body's com-based velocity cvel = (w, v)
+//                        moved to the site (v - (site_xpos - subtree_com[root]) x w) and rotated by site_xmat'
+//   accelerometer        mj_objectAcceleration of the site with flg_local: the body's post-constraint com-based
+//                        acceleration (mj_rnePostConstraint's recursion cacc[b] = cacc[parent] + cdof_dot qvel +
+//                        cdof qacc from cacc[world] = (0, -gravity)), moved and rotated like the velocity, plus
+//                        (R' w) x (R' v_site)
 // The sensor table is read from the blob's sensor_* / site_* entries.  Written from the definition, independently of
 // the device's k_sensors; the oracle itself is not modified.
 #include <cmath>
@@ -24,7 +30,8 @@ using namespace oracle;
 
 namespace {
 
-enum { SENS_FRAMEPOS = 1, SENS_JOINTPOS = 2, SENS_TOUCH = 3, SENS_JOINTVEL = 9 };
+enum { SENS_FRAMEPOS = 1, SENS_JOINTPOS = 2, SENS_TOUCH = 3, SENS_JOINTVEL = 9, SENS_ACCELEROMETER = 10,
+       SENS_VELOCIMETER = 11, SENS_GYRO = 12 };
 enum { OBJ_BODY = 0, OBJ_XBODY = 1, OBJ_GEOM = 2, OBJ_SITE = 3 };
 
 struct Table {
@@ -75,9 +82,46 @@ double touch(const Model<T>& m, const Data<T>& d, const Table& tab, int site) {
   return sum;
 }
 
+// site_xmat' (vec moved from subtree_com[root] to the site) for a com-based motion vector vec = (angular, linear);
+// out = (angular, linear) in the site frame
+template <class T>
+void site_motion(const Model<T>& m, const Data<T>& d, int site, const double* vec, double* out) {
+  const int b = m.site_bodyid[site], root = m.body_rootid[b];
+  double off[3], lin[3];
+  for (int q = 0; q < 3; q++) off[q] = (double)d.site_xpos[3 * site + q] - (double)d.subtree_com[3 * root + q];
+  lin[0] = vec[3] - (off[1] * vec[2] - off[2] * vec[1]);
+  lin[1] = vec[4] - (off[2] * vec[0] - off[0] * vec[2]);
+  lin[2] = vec[5] - (off[0] * vec[1] - off[1] * vec[0]);
+  const T* R = &d.site_xmat[9 * site];
+  for (int r = 0; r < 3; r++) {
+    out[r] = out[3 + r] = 0;
+    for (int k = 0; k < 3; k++) {
+      out[r] += (double)R[3 * k + r] * vec[k];
+      out[3 + r] += (double)R[3 * k + r] * lin[k];
+    }
+  }
+}
+
+// mj_rnePostConstraint's com-based body accelerations without contact or applied forces: cacc [nbody][6]
+template <class T>
+std::vector<double> post_constraint_acc(const Model<T>& m, const Data<T>& d) {
+  std::vector<double> cacc(6 * (size_t)m.nbody, 0.0);
+  for (int q = 0; q < 3; q++) cacc[3 + q] = -(double)m.gravity[q];
+  for (int b = 1; b < m.nbody; b++) {
+    double* a = &cacc[6 * (size_t)b];
+    const double* ap = &cacc[6 * (size_t)m.body_parentid[b]];
+    for (int q = 0; q < 6; q++) a[q] = ap[q];
+    for (int i = m.body_dofadr[b]; i < m.body_dofadr[b] + m.body_dofnum[b]; i++)
+      for (int q = 0; q < 6; q++)
+        a[q] += (double)d.cdof_dot[6 * i + q] * (double)d.qvel[i] + (double)d.cdof[6 * i + q] * (double)d.qacc[i];
+  }
+  return cacc;
+}
+
 template <class T>
 void sensors(const Model<T>& m, const Data<T>& d, const Table& tab, int start, int count, double* out) {
   const int adr0 = tab.adr[start];
+  std::vector<double> cacc;
   for (int s = start; s < start + count; s++) {
     double* o = out + (tab.adr[s] - adr0);
     const int id = tab.objid[s];
@@ -91,6 +135,22 @@ void sensors(const Model<T>& m, const Data<T>& d, const Table& tab, int start, i
         break;
       }
       case SENS_TOUCH: o[0] = touch(m, d, tab, id); break;
+      case SENS_GYRO: case SENS_VELOCIMETER: case SENS_ACCELEROMETER: {
+        if (tab.objtype[s] != OBJ_SITE) throw std::runtime_error("IMU sensor of an object other than a site");
+        const int b = m.site_bodyid[id];
+        double vel[6], v[6];
+        for (int q = 0; q < 6; q++) vel[q] = d.cvel[6 * b + q];
+        site_motion(m, d, id, vel, v);
+        if (tab.type[s] == SENS_GYRO) { for (int q = 0; q < 3; q++) o[q] = v[q]; break; }
+        if (tab.type[s] == SENS_VELOCIMETER) { for (int q = 0; q < 3; q++) o[q] = v[3 + q]; break; }
+        if (cacc.empty()) cacc = post_constraint_acc(m, d);
+        double a[6];
+        site_motion(m, d, id, &cacc[6 * (size_t)b], a);
+        o[0] = a[3] + v[1] * v[5] - v[2] * v[4];
+        o[1] = a[4] + v[2] * v[3] - v[0] * v[5];
+        o[2] = a[5] + v[0] * v[4] - v[1] * v[3];
+        break;
+      }
       default: throw std::runtime_error("sensor type not evaluated");
     }
   }
