@@ -241,11 +241,11 @@ int mjpc_b200_step_sensors(mjpc_b200_t* h, int B, const float* states, const flo
                            float* sensordata, float* qacc, int* counts);
 
 /* MJPC's Unscented state estimator (mjpc/estimators/unscented.cc, class mjpc_b200_host::Unscented in
- * csrc/host/unscented.h): the filter in double precision on the host, its 2 ndstate + 1 sigma-point steps as one
- * mjpc_b200_step_sensors launch on an engine handle it owns (max_candidates = nsigma).  Settings are explicit (the
- * reference's defaults: alpha 1, beta 2, timestep = estimator_timestep or opt.timestep, the three noise scales 1e-4).
- * create: measured sensors [sensor_start, sensor_start + nsensor) of the blob.  reset: state NULL -> the model's
- * first keyframe, else qpos0 and zero qvel; covariance = covariance_scale I, diagonal process / sensor noise.
+ * csrc/host/unscented.h on the Estimator base): the filter in double on the host, its 2 ndstate + 1 sigma-point steps
+ * as one mjpc_b200_step_sensors launch on a handle it owns (max_candidates = nsigma).  Settings are explicit (alpha 1,
+ * beta 2, timestep = estimator_timestep or opt.timestep, noise scales 1e-4 by default).  create: measured sensors
+ * [sensor_start, sensor_start + nsensor) of the blob, refused as kalman_create refuses them.  reset: state NULL -> the
+ * model's first keyframe, else qpos0 and zero qvel; covariance = covariance_scale I, diagonal process / sensor noise.
  * set_noise: process [ndstate], sensor [nsensordata] (NULL keeps one).  set: state, covariance [ndstate^2] (NULL keeps
  * one) and time.  update: ctrl [nu], the measured sensor slice [nsensordata], mocap [7 nmocap] or NULL (the model's);
  * a failed covariance or sensor-covariance factorisation returns MJPC_B200_ERR_BAD_ARGUMENT and leaves state,

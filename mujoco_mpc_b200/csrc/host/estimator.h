@@ -1,0 +1,68 @@
+// estimator.h - the base every host state estimator derives from (the reference's virtual Estimator,
+// mjpc/estimators/estimator.h, limited to what exists here) and the engine plumbing the estimators share: the engine
+// handle holding 2 ndstate + 1 states (the most any filter steps in one launch), the blob's sensor range, mocap and
+// Reset state, the float staging of one mjpc_b200_step_sensors launch with its warm start, and the double-precision
+// gain step, symmetrisation and tangent-space state addition.
+#pragma once
+#include <string>
+#include <vector>
+
+#include "planner.h"
+
+namespace mjpc_b200_host {
+
+class Estimator {
+ public:
+  virtual ~Estimator();
+  // state NULL -> the model's first keyframe if it has one, else qpos0 and zero qvel; covariance = covariance_scale I,
+  // diagonal process / sensor noise, zero warm start and warnings
+  virtual void Reset(const double* state, double time, double covariance_scale, double process_scale,
+                     double sensor_scale);
+  // one filter update from ctrl [nu], the measured sensor slice [nsensordata] and mocap [7 nmocap] (NULL: the model's)
+  virtual int Update(const double* ctrl, const double* sensor, const float* mocap) = 0;
+
+  std::vector<double> state, covariance, noise_process, noise_sensor;
+  double time = 0;
+  int warnings = 0;   // steps that raised a warning since Reset
+  int ndstate = 0, nsensordata = 0;
+  double timestep = 0;
+  std::string error;
+
+ protected:
+  explicit Estimator(const char* name) : name_(name) {}
+  // Loads the blob, checks the sensor range, creates the engine handle, sets the timestep and Resets.  Then it steps
+  // the reset state once, so a range with a sensor the engine does not evaluate is refused here
+  // (MJPC_B200_ERR_UNSUPPORTED) rather than at the first update, and Resets again.
+  int InitializeBase(const mjpc_model_blob* model, int sensor_start, int nsensor, double timestep, int device);
+  // steps the first n rows of states_ [n][nq+nv] from ctrl [nu] and mocap (NULL: the model's) at `time`, each
+  // warm-started from qacc_warmstart_, into fnext_ / fsensor_ / fqacc_ / counts_
+  int StepSensors(int n, const double* ctrl, const float* mocap);
+  // after a successful update: the warm start from row `centre` of the last launch, and that launch's warnings
+  void Commit(int centre);
+  // corr [ndstate] = X S^-1 innovation and P = P0 - X S^-1 X', symmetrised, for X [ndstate][nsensordata] and
+  // S [nsensordata]^2.  S is overwritten by its Cholesky factor and innovation by S^-1 innovation.  A factor that is
+  // not full rank: MJPC_B200_ERR_BAD_ARGUMENT with corr and P untouched.  P may alias P0.
+  int GainUpdate(const double* X, double* S, double* innovation, const double* P0, double* corr, double* P);
+  void Symmetrize(double* P) const;                                 // P [ndstate]^2 = (P + P') / 2
+  void StateAdd(double* x, const double* dx, double scale) const;   // x (+) scale dx: IntegratePos, velocities added
+
+  const char* name_;   // the prefix of every error message
+  mjpc_b200_t* engine_ = nullptr;
+  HostModel m_;
+  int sensor_start_ = 0, nsensor_ = 0, nmocap_ = 0, nstepped_ = 0;
+  std::vector<double> key_state_, qacc_warmstart_, states_;
+  std::vector<float> fstates_, fnext_, fsensor_, fqacc_, fwarm_, mocap0_;
+  std::vector<int> counts_;
+};
+
+// The bodies of the mjpc_b200_{unscented,kalman}_* entry points every filter shares; a NULL filter returns
+// MJPC_B200_ERR_BAD_ARGUMENT (last_error: "").  Get fills state, covariance and time; each filter fills its scalars.
+void EstimatorDestroy(Estimator* f);
+int EstimatorReset(Estimator* f, const double* state, double time, double covariance_scale, double process_scale,
+                   double sensor_scale);
+int EstimatorSetNoise(Estimator* f, const double* process, const double* sensor);
+int EstimatorSet(Estimator* f, const double* state, const double* covariance, double time);
+int EstimatorGet(const Estimator* f, double* state, double* covariance, double* time);
+const char* EstimatorLastError(const Estimator* f);
+
+}  // namespace mjpc_b200_host

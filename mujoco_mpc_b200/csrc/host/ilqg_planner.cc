@@ -5,8 +5,6 @@
 #include <cmath>
 #include <mutex>
 
-#include "../dev_model.h"   // Blob reader (plain C++)
-
 namespace mjpc_b200_host {
 
 // ------------------------------------------------------------------------------------------ iLQGPolicy::Action
@@ -41,79 +39,9 @@ void NormalizeQuat(double* q) {
   if (n < 1e-15) { q[0] = 1; q[1] = q[2] = q[3] = 0; return; }
   for (int k = 0; k < 4; k++) q[k] /= n;
 }
-void SubQuat(double* res, const double* qa, const double* qb) {   // qb * quat(res) = qa  (mju_subQuat)
-  const double n[4] = {qb[0], -qb[1], -qb[2], -qb[3]};
-  const double d[4] = {n[0] * qa[0] - n[1] * qa[1] - n[2] * qa[2] - n[3] * qa[3],
-                       n[0] * qa[1] + n[1] * qa[0] + n[2] * qa[3] - n[3] * qa[2],
-                       n[0] * qa[2] - n[1] * qa[3] + n[2] * qa[0] + n[3] * qa[1],
-                       n[0] * qa[3] + n[1] * qa[2] - n[2] * qa[1] + n[3] * qa[0]};
-  double axis[3] = {d[1], d[2], d[3]};
-  const double s = std::sqrt(axis[0] * axis[0] + axis[1] * axis[1] + axis[2] * axis[2]);
-  if (s < 1e-15) { axis[0] = 1; axis[1] = axis[2] = 0; } else { for (double& a : axis) a /= s; }
-  double speed = 2 * std::atan2(s, d[0]);
-  if (speed > M_PI) speed -= 2 * M_PI;
-  for (int c = 0; c < 3; c++) res[c] = axis[c] * speed;
-}
-// mju_quatIntegrate: q * exp(scale v / 2), normalised
-void QuatIntegrate(double* q, const double* v, double scale) {
-  const double w[3] = {v[0] * scale, v[1] * scale, v[2] * scale};
-  const double a = std::sqrt(w[0] * w[0] + w[1] * w[1] + w[2] * w[2]);
-  double r[4] = {1, 0, 0, 0};
-  if (a >= 1e-15) {
-    const double s = std::sin(a / 2) / a;
-    r[0] = std::cos(a / 2); r[1] = s * w[0]; r[2] = s * w[1]; r[3] = s * w[2];
-  }
-  const double o[4] = {q[0] * r[0] - q[1] * r[1] - q[2] * r[2] - q[3] * r[3],
-                       q[0] * r[1] + q[1] * r[0] + q[2] * r[3] - q[3] * r[2],
-                       q[0] * r[2] - q[1] * r[3] + q[2] * r[0] + q[3] * r[1],
-                       q[0] * r[3] + q[1] * r[2] - q[2] * r[1] + q[3] * r[0]};
-  const double n = std::sqrt(o[0] * o[0] + o[1] * o[1] + o[2] * o[2] + o[3] * o[3]);
-  for (int k = 0; k < 4; k++) q[k] = o[k] / n;
-}
 }  // namespace
 
-int iLQGPolicyModel::Load(const mjpc_model_blob* blob) {
-  try {
-    mjpc_dev::Blob b(blob->data, blob->nbytes);
-    nq = b.i("nq"); nv = b.i("nv"); nu = b.i("nu");
-    jnt_type = b.ints("jnt_type"); jnt_qposadr = b.ints("jnt_qposadr"); jnt_dofadr = b.ints("jnt_dofadr");
-    ctrlrange = b.reals("actuator_ctrlrange");
-  } catch (const std::exception&) {
-    return MJPC_B200_ERR_BAD_BLOB;
-  }
-  return 0;
-}
-
-void StateDiff(const iLQGPolicyModel& m, double* dx, const double* x_to, const double* x_from) {
-  for (size_t j = 0; j < m.jnt_type.size(); j++) {
-    const int qa = m.jnt_qposadr[j], da = m.jnt_dofadr[j];
-    if (m.jnt_type[j] == 0) {
-      for (int c = 0; c < 3; c++) dx[da + c] = x_to[qa + c] - x_from[qa + c];
-      SubQuat(&dx[da + 3], x_to + qa + 3, &x_from[qa + 3]);
-    } else if (m.jnt_type[j] == 1) {
-      SubQuat(&dx[da], x_to + qa, &x_from[qa]);
-    } else {
-      dx[da] = x_to[qa] - x_from[qa];
-    }
-  }
-  for (int i = 0; i < m.nv; i++) dx[m.nv + i] = x_to[m.nq + i] - x_from[m.nq + i];
-}
-
-void IntegratePos(const iLQGPolicyModel& m, double* qpos, const double* dq, double scale) {
-  for (size_t j = 0; j < m.jnt_type.size(); j++) {
-    const int a = m.jnt_qposadr[j], d = m.jnt_dofadr[j];
-    if (m.jnt_type[j] == 0) {
-      for (int c = 0; c < 3; c++) qpos[a + c] += scale * dq[d + c];
-      QuatIntegrate(qpos + a + 3, dq + d + 3, scale);
-    } else if (m.jnt_type[j] == 1) {
-      QuatIntegrate(qpos + a, dq + d, scale);
-    } else {
-      qpos[a] += scale * dq[d];
-    }
-  }
-}
-
-void iLQGPolicyAction(const iLQGPolicyModel& m, const float* u_nom, const float* x_nom, const double* t_nom,
+void iLQGPolicyAction(const HostModel& m, const float* u_nom, const float* x_nom, const double* t_nom,
                       const float* gains, int H, int representation, double feedback_scaling, const double* state,
                       double time, double* action) {
   const int ds = m.nq + m.nv, n = 2 * m.nv, nu = m.nu;
@@ -414,7 +342,7 @@ int mjpc_b200_host_ilqg_policy_action(const mjpc_model_blob* model, const float*
                                       const double* t_nom, const float* gains, int horizon, int representation,
                                       double feedback_scaling, const double* state, double time, double* action) {
   if (!model || !u_nom || !x_nom || !t_nom || !gains || !action || horizon < 2) return MJPC_B200_ERR_BAD_ARGUMENT;
-  mjpc_b200_host::iLQGPolicyModel pm;
+  mjpc_b200_host::HostModel pm;
   if (int rc = pm.Load(model)) return rc;
   mjpc_b200_host::iLQGPolicyAction(pm, u_nom, x_nom, t_nom, gains, horizon, representation, feedback_scaling, state, time,
                                    action);

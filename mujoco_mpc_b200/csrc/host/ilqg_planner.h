@@ -38,17 +38,7 @@ struct iLQGSettings {                    // mjpc/planners/ilqg/settings.h:21-36
 // Interpolates the nominal actions / states / gains at `time` (representation 0 zero-order, 1 linear, 2 cubic with
 // finite-difference slopes; mjpc/utilities.cc:303-422), adds feedback_scaling * K (x (-) x_nominal) with the
 // tangent-space state difference (StateDiff, utilities.cc:543-553) when a state is given, clamps to ctrlrange.
-struct iLQGPolicyModel {       // the few mjModel fields the policy needs, read from the blob
-  int nq = 0, nv = 0, nu = 0;
-  std::vector<int> jnt_type, jnt_qposadr, jnt_dofadr;
-  std::vector<double> ctrlrange;
-  int Load(const mjpc_model_blob* blob);
-};
-// StateDiff (utilities.cc:543-553): dx [2 nv] = x_to (-) x_from, positions in the tangent space (mj_differentiatePos)
-void StateDiff(const iLQGPolicyModel& m, double* dx, const double* x_to, const double* x_from);
-// mj_integratePos: qpos (+) scale dq, quaternions through mju_quatIntegrate (q exp(scale v / 2), normalised)
-void IntegratePos(const iLQGPolicyModel& m, double* qpos, const double* dq, double scale);
-void iLQGPolicyAction(const iLQGPolicyModel& m, const float* u_nom, const float* x_nom, const double* t_nom,
+void iLQGPolicyAction(const HostModel& m, const float* u_nom, const float* x_nom, const double* t_nom,
                       const float* gains, int horizon, int representation, double feedback_scaling, const double* state,
                       double time, double* action);
 
@@ -101,7 +91,7 @@ class iLQGPlanner : public Planner {
   int InstallActions(const float* ret, const uint8_t* fail, int cand0);
   void ScaleRegularization(double factor);                                // backward_pass.cc:327-343
   void UpdateRegularization(double z, double s);                          // :345-356
-  iLQGPolicyModel pm_;
+  HostModel pm_;
   mutable std::shared_mutex mtx_;   // the policy is read by the physics thread while a plan installs a new one
   int K_ = 10, representation_ = 1, H_ = 0, Hmax_ = 0, nu_ = 0, ds_ = 0, n_ = 0, nr_ = 0;
   // candidate_policy[0]: the working copy NominalTrajectory / Iteration operate on (planner.cc:190-222,392-560)

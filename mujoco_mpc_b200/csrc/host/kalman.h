@@ -1,7 +1,7 @@
 // kalman.h - MJPC's Kalman state estimator (mjpc/estimators/kalman.{h,cc}) on the engine: the finite-difference
 // Jacobians are one mjpc_b200_step_sensors launch each (the centre state and its ndstate, or 2 ndstate when centred,
 // tangent-space perturbations); the filter arithmetic is double precision on the host.  Method names are the
-// reference's.
+// reference's; the engine plumbing is Estimator's (estimator.h).
 //
 //   UpdateMeasurement (kalman.cc:188-276)  C = d sensors / d state of the pre-step states and y_hat = the centre's
 //                                          sensors from one launch; gain P C' (C P C' + R)^-1, correction, P -= ...,
@@ -24,42 +24,34 @@
 //    the engine default for the finite differences is centred with a larger epsilon than the reference's fp64 1e-6
 //    one-sided (DESIGN.md, "Kalman filter").
 #pragma once
-#include <string>
 #include <vector>
 
-#include "ilqg_planner.h"
+#include "estimator.h"
 
 namespace mjpc_b200_host {
 
-class Kalman {
+class Kalman : public Estimator {
  public:
-  ~Kalman();
-  // kalman.cc:31-110: timestep, sensor range, finite-difference settings; the engine handle holds 2 ndstate + 1 states
+  Kalman() : Estimator("kalman") {}
+  // kalman.cc:31-110: timestep, sensor range (Estimator::InitializeBase), finite-difference settings
   int Initialize(const mjpc_model_blob* model, int sensor_start, int nsensor, double timestep, double epsilon,
                  bool centered, int device);
-  // kalman.cc:113-185: state NULL -> the model's first keyframe if it has one, else qpos0 and zero qvel
-  void Reset(const double* state, double time, double covariance_scale, double process_scale, double sensor_scale);
+  // kalman.cc:113-185: Estimator::Reset, and the ctrl and mocap of the last measurement = zeros and the model's mocap
+  void Reset(const double* state, double time, double covariance_scale, double process_scale,
+             double sensor_scale) override;
   int UpdateMeasurement(const double* ctrl, const double* sensor, const float* mocap);   // kalman.cc:188-276
   int UpdatePrediction();                                                                 // kalman.cc:279-323
-  int Update(const double* ctrl, const double* sensor, const float* mocap);   // UpdateMeasurement, UpdatePrediction
+  int Update(const double* ctrl, const double* sensor, const float* mocap) override;   // UpdateMeasurement, UpdatePrediction
 
-  std::vector<double> state, covariance, noise_process, noise_sensor;
-  double time = 0;
-  int warnings = 0;   // steps that raised a warning since Reset
-  int ndstate = 0, nstates = 0, nsensordata = 0;
-  double timestep = 0, epsilon = 0;
+  int nstates = 0;
+  double epsilon = 0;
   bool centered = false;
-  std::string error;
 
  private:
   // the centre state and its perturbations x (+) eps e_i (then x (+) -eps e_i when centred) stepped in one launch
   int Perturbed(const double* ctrl, const float* mocap);
-  mjpc_b200_t* engine_ = nullptr;
-  iLQGPolicyModel m_;
-  int sensor_start_ = 0, nsensor_ = 0, nmocap_ = 0;
-  std::vector<double> key_state_, ctrl_, jacobian_, qacc_warmstart_;
-  std::vector<float> fstates_, fnext_, fsensor_, fqacc_, fwarm_, mocap0_, mocap_;
-  std::vector<int> counts_;
+  std::vector<double> ctrl_, jacobian_;
+  std::vector<float> mocap_;
 };
 
 }  // namespace mjpc_b200_host

@@ -1,6 +1,7 @@
 // planner.h - the interface every host planner implements (the reference's virtual Planner,
 // mjpc/planners/planner.h:33-77, limited to what exists here) and the engine plumbing they share: the engine handle,
-// the planning state, the spline launch and the trajectory fetch.
+// the planning state, the spline launch and the trajectory fetch.  Also the host maths the planners and the
+// estimators share: the Cholesky factor, FindInterval and the host model's state arithmetic.
 #pragma once
 #include <cstdint>
 #include <vector>
@@ -26,6 +27,17 @@ void CholSolve(const double* L, int n, double* x);
 // FindInterval (mjpc/utilities.cc:303-330): the indices of the entries of a non-decreasing sequence around `value`,
 // clamped to the sequence
 void FindInterval(int* bounds, const double* sequence, double value, int length);
+
+struct HostModel {             // the few mjModel fields the host-side state arithmetic needs, read from the blob
+  int nq = 0, nv = 0, nu = 0;
+  std::vector<int> jnt_type, jnt_qposadr, jnt_dofadr;
+  std::vector<double> ctrlrange;
+  int Load(const mjpc_model_blob* blob);
+};
+// StateDiff (utilities.cc:543-553): dx [2 nv] = x_to (-) x_from, positions in the tangent space (mj_differentiatePos)
+void StateDiff(const HostModel& m, double* dx, const double* x_to, const double* x_from);
+// mj_integratePos: qpos (+) scale dq, quaternions through mju_quatIntegrate (q exp(scale v / 2), normalised)
+void IntegratePos(const HostModel& m, double* qpos, const double* dq, double scale);
 
 // MakeDifferentiable while planning, restored afterwards (agent.cc:296-309,346-356)
 struct DifferentiableScope {

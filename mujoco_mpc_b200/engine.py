@@ -132,6 +132,10 @@ def load_library():
             getattr(lib, n).restype = C.c_void_p
         lib.mjpc_b200_quadruped_transition_destroy.argtypes = [C.c_void_p]
         lib.mjpc_b200_track_transition_destroy.argtypes = [C.c_void_p]
+        for n in ("mjpc_b200_unscented", "mjpc_b200_kalman"):
+            getattr(lib, n + "_destroy").argtypes = [C.c_void_p]
+            getattr(lib, n + "_last_error").argtypes = [C.c_void_p]
+            getattr(lib, n + "_last_error").restype = C.c_char_p
         for n in ("mjpc_b200_destroy", "mjpc_b200_fetch_stats", "mjpc_b200_launch_count", "mjpc_b200_last_kernel_ms", "mjpc_b200_stream",
                   "mjpc_b200_device_returns", "mjpc_b200_sync", "mjpc_b200_launch_resident"):
             getattr(lib, n).argtypes = [C.c_void_p]

@@ -1,5 +1,6 @@
 """MJPC's Unscented (mjpc/estimators/unscented.cc) and Kalman (mjpc/estimators/kalman.cc) state estimators with their
-steps on a step backend.
+steps on a step backend.  Both derive from ``_Filter`` (the reference's Estimator base), and their C++ wrappers from
+``_CppFilter``.
 
 The filter arithmetic is double precision on the host: a Cholesky factor of the covariance, weighted means and
 covariances of at most 2 ndstate + 1 points and one Cholesky factor of the sensor covariance.  The sigma-point steps
@@ -40,8 +41,11 @@ reference are the Unscented filter's (the warm start is the centre state's qacc 
 """
 from __future__ import annotations
 
+import ctypes as C
+
 import numpy as np
 
+from .engine import EngineError, _CppObject, _d, _pd, _pf
 from .mjcf import JNT_BALL, JNT_FREE, SENS_MEASURED
 
 
@@ -212,37 +216,30 @@ def reset_values(m, state=None, covariance_scale=None, process_scale=None, senso
     return np.array(state, float), float(cs), float(ps), float(ss)
 
 
-class Unscented:
-    """mjpc::Unscented.  `backend(sensor_start, nsensor, timestep)` returns the object that runs the sigma-point steps (see
-    EngineBackend); settings left None default from the model's numerics as GetNumberOrDefault does."""
+def _default_mocap(m):
+    return np.concatenate([m.mocap_pos0, m.mocap_quat0], axis=1).reshape(-1) if m.nmocap else np.zeros(0)
 
-    def __init__(self, m, backend, sensor_start=None, nsensor=None, timestep=None, alpha=None, beta=None):
+
+class _Filter:
+    """What the Unscented and Kalman filters share: the settings, sensor range and backend, reset, the noise, the
+    warm-started backend step and its commit, the gain update and the tangent-space state addition."""
+
+    def __init__(self, m, backend, sensor_start, nsensor, timestep):
         self.m = m
-        self.sensor_start, self.nsensor, self.timestep, self.alpha, self.beta = settings(m, sensor_start, nsensor,
-                                                                                         timestep, alpha, beta)
+        self.sensor_start, self.nsensor, self.timestep = settings(m, sensor_start, nsensor, timestep)[:3]
         self.nsensordata = measured_range(m, self.sensor_start, self.nsensor)
         self.backend = backend(self.sensor_start, self.nsensor, self.timestep)
-        nv = m.nv
-        self.ndstate = 2 * nv
-        self.nsigma = 2 * self.ndstate + 1
-        # derived weights (unscented.cc:171-290)
-        lam = self.ndstate * (self.alpha ** 2 - 1.0)
-        self.sigma_step = np.sqrt(self.ndstate + lam)
-        self.weight_mean0 = lam / (self.ndstate + lam)
-        self.weight_covariance0 = self.weight_mean0 + 1.0 - self.alpha ** 2 + self.beta
-        self.weight_sigma = 1.0 / (2.0 * (self.ndstate + lam))
+        self.ndstate = 2 * m.nv
         self.warnings = 0
-        self.reset()
 
     def reset(self, state=None, time=0.0, covariance_scale=None, process_scale=None, sensor_scale=None):
-        """Reset (unscented.cc:171-290): state = the home keyframe if the model has one, else qpos0 and zero qvel."""
-        m = self.m
-        self.state, cs, ps, ss = reset_values(m, state, covariance_scale, process_scale, sensor_scale)
+        """Reset: state = the home keyframe if the model has one, else qpos0 and zero qvel."""
+        self.state, cs, ps, ss = reset_values(self.m, state, covariance_scale, process_scale, sensor_scale)
         self.time = float(time)
         self.covariance = cs * np.eye(self.ndstate)
         self.noise_process = np.full(self.ndstate, float(ps))
         self.noise_sensor = np.full(self.nsensordata, float(ss))
-        self.qacc_warmstart = np.zeros(m.nv)
+        self.qacc_warmstart = np.zeros(self.m.nv)
         self.warnings = 0
 
     def set_noise(self, process=None, sensor=None):
@@ -251,6 +248,52 @@ class Unscented:
             self.noise_process = np.array(process, float)
         if sensor is not None:
             self.noise_sensor = np.array(sensor, float)
+
+    def _step(self, states, ctrl, mocap):
+        """One backend call: every state from `time`, ctrl and mocap, warm-started from the committed qacc."""
+        warm = np.tile(self.qacc_warmstart, (len(states), 1))
+        return self.backend.step_sensors(states, np.asarray(ctrl, float), mocap, self.time, warm)
+
+    def _commit(self, qacc, nwarn):
+        """After a successful update: the warm start from the centre's qacc and the call's warnings."""
+        self.qacc_warmstart = qacc.copy()
+        self.warnings += nwarn
+
+    @staticmethod
+    def _gain(X, S, P0, innovation):
+        """(X S^-1 innovation, the symmetrised P0 - X S^-1 X'); EstimatorError when S does not factor."""
+        try:
+            L = np.linalg.cholesky(S)
+        except np.linalg.LinAlgError:
+            raise EstimatorError("sensor covariance factorisation failed") from None
+        solve = lambda b: np.linalg.solve(L.T, np.linalg.solve(L, b))
+        P = P0 - X @ solve(X.T)
+        return X @ solve(innovation), 0.5 * (P + P.T)
+
+    def _state_add(self, x, dx):
+        """x (+) dx: positions through mj_integratePos, velocities added."""
+        nq, nv = self.m.nq, self.m.nv
+        new = np.empty_like(x)
+        new[:nq] = integrate_pos(self.m, x[:nq], dx[:nv], 1.0)
+        new[nq:] = x[nq:] + dx[nv:]
+        return new
+
+
+class Unscented(_Filter):
+    """mjpc::Unscented.  `backend(sensor_start, nsensor, timestep)` returns the object that runs the sigma-point steps (see
+    EngineBackend); settings left None default from the model's numerics as GetNumberOrDefault does."""
+
+    def __init__(self, m, backend, sensor_start=None, nsensor=None, timestep=None, alpha=None, beta=None):
+        super().__init__(m, backend, sensor_start, nsensor, timestep)
+        self.alpha, self.beta = settings(m, alpha=alpha, beta=beta)[3:]
+        self.nsigma = 2 * self.ndstate + 1
+        # derived weights (unscented.cc:171-290)
+        lam = self.ndstate * (self.alpha ** 2 - 1.0)
+        self.sigma_step = np.sqrt(self.ndstate + lam)
+        self.weight_mean0 = lam / (self.ndstate + lam)
+        self.weight_covariance0 = self.weight_mean0 + 1.0 - self.alpha ** 2 + self.beta
+        self.weight_sigma = 1.0 / (2.0 * (self.ndstate + lam))
+        self.reset()
 
     def sigma_points(self):
         """SigmaPoints (unscented.cc:293-349): [nsigma][nq+nv], nominal last."""
@@ -291,10 +334,8 @@ class Unscented:
         m = self.m
         nq, nv = m.nq, m.nv
         if mocap is None:
-            mocap = np.concatenate([m.mocap_pos0, m.mocap_quat0], axis=1).reshape(-1) if m.nmocap else np.zeros(0)
-        sigma = self.sigma_points()
-        warm = np.tile(self.qacc_warmstart, (self.nsigma, 1))
-        states, sensors, qacc, nwarn = self.backend.step_sensors(sigma, np.asarray(ctrl, float), mocap, self.time, warm)
+            mocap = _default_mocap(m)
+        states, sensors, qacc, nwarn = self._step(self.sigma_points(), ctrl, mocap)
         wm = self._weights(self.weight_mean0)
         wc = self._weights(self.weight_covariance0)
         s_mean = self.state_mean(states)
@@ -307,97 +348,48 @@ class Unscented:
         cov_yy = np.diag(self.noise_sensor) + (dy.T * wc) @ dy
         cov_sy = (ds.T * wc) @ dy
         cov_ss = np.diag(self.noise_process) + (ds.T * wc) @ ds
-        try:
-            Ly = np.linalg.cholesky(cov_yy)
-        except np.linalg.LinAlgError:
-            raise EstimatorError("sensor covariance factorisation failed") from None
-        solve = lambda b: np.linalg.solve(Ly.T, np.linalg.solve(Ly, b))
-        err = np.asarray(sensor, float) - y_mean
-        corr = cov_sy @ solve(err)
-        new = np.empty_like(self.state)
-        new[:nq] = integrate_pos(m, s_mean[:nq], corr[:nv], 1.0)
-        new[nq:] = s_mean[nq:] + corr[nv:]
-        P = cov_ss - cov_sy @ solve(cov_sy.T)
-        self.state = new
-        self.covariance = 0.5 * (P + P.T)
+        corr, self.covariance = self._gain(cov_sy, cov_yy, cov_ss, np.asarray(sensor, float) - y_mean)
+        self.state = self._state_add(s_mean, corr)
         self.time = self.time + self.timestep
-        self.qacc_warmstart = qacc[-1].copy()
-        self.warnings += nwarn
+        self._commit(qacc[-1], nwarn)
         return self.state
 
 
-class CppUnscented:
-    """The C++ filter (csrc/host/unscented.{h,cc}, mjpc_b200_unscented_*) behind the same attributes as Unscented;
-    settings resolve from the model's numerics exactly as Unscented's do."""
-
-    def __init__(self, m, sensor_start=None, nsensor=None, timestep=None, alpha=None, beta=None, device=0):
-        import ctypes as C
-        from .engine import EngineError, _model_blob, load_library
-        self.C, self.Error = C, EngineError
-        self.lib = load_library()
-        self.lib.mjpc_b200_unscented_last_error.restype = C.c_char_p
-        self.lib.mjpc_b200_unscented_last_error.argtypes = [C.c_void_p]
-        self.lib.mjpc_b200_unscented_destroy.argtypes = [C.c_void_p]
-        self.m = m
-        self.sensor_start, self.nsensor, self.timestep, self.alpha, self.beta = settings(m, sensor_start, nsensor,
-                                                                                         timestep, alpha, beta)
-        self.nsensordata = measured_range(m, self.sensor_start, self.nsensor)
-        self._buf, mb = _model_blob(m)
-        h = C.c_void_p()
-        rc = self.lib.mjpc_b200_unscented_create(C.byref(mb), self.sensor_start, self.nsensor, C.c_double(self.timestep),
-                                                 C.c_double(self.alpha), C.c_double(self.beta), int(device), C.byref(h))
-        if rc != 0:
-            raise EngineError(f"mjpc_b200_unscented_create failed ({rc}): {self.lib.mjpc_b200_last_error().decode()}")
-        self.h = h
-        self.ndstate, self.nsigma = 2 * m.nv, 4 * m.nv + 1
-        self.reset()
-
-    def close(self):
-        if getattr(self, "h", None):
-            self.lib.mjpc_b200_unscented_destroy(self.h)
-            self.h = None
-
-    __del__ = close
-
-    def _pd(self, a):
-        return None if a is None else np.ascontiguousarray(a, np.float64).ctypes.data_as(self.C.POINTER(self.C.c_double))
+class _CppFilter(_CppObject):
+    """What CppUnscented and CppKalman share: the C++ filter behind its `<prefix>_*` entry points, its reset, noise,
+    set and get, the ctrl / sensor / mocap marshalling and the EstimatorError of a failed factorisation."""
 
     def _check(self, rc):
         if rc != 0:
-            msg = self.lib.mjpc_b200_unscented_last_error(self.h).decode()
+            msg = getattr(self.lib, f"{self._prefix}_last_error")(self.h).decode()
             if "factorisation" in msg:
                 raise EstimatorError(msg)
-            raise self.Error(f"mjpc_b200_unscented error {rc}: {msg}")
+            raise EngineError(f"{self._prefix} error {rc}: {msg}")
+
+    def _call(self, name, *args):
+        self._check(getattr(self.lib, f"{self._prefix}_{name}")(self.h, *args))
 
     def reset(self, state=None, time=0.0, covariance_scale=None, process_scale=None, sensor_scale=None):
         x, cs, ps, ss = reset_values(self.m, state, covariance_scale, process_scale, sensor_scale)
-        self._check(self.lib.mjpc_b200_unscented_reset(self.h, self._pd(x), self.C.c_double(time), self.C.c_double(cs),
-                                                       self.C.c_double(ps), self.C.c_double(ss)))
+        self._call("reset", _pd(_d(x)), C.c_double(time), C.c_double(cs), C.c_double(ps), C.c_double(ss))
 
     def set_noise(self, process=None, sensor=None):
-        self._check(self.lib.mjpc_b200_unscented_set_noise(self.h, self._pd(process), self._pd(sensor)))
+        self._call("set_noise", _pd(_d(process)), _pd(_d(sensor)))
 
     def set(self, state, covariance, time):
-        self._check(self.lib.mjpc_b200_unscented_set(self.h, self._pd(state), self._pd(covariance),
-                                                     self.C.c_double(time)))
+        self._call("set", _pd(_d(state)), _pd(_d(covariance)), C.c_double(time))
 
-    def update(self, ctrl, sensor, mocap=None):
-        C = self.C
+    def _args(self, ctrl, sensor, mocap):
         mc = None if mocap is None or len(mocap) == 0 else np.ascontiguousarray(mocap, np.float32)
         u = np.ascontiguousarray(np.atleast_1d(np.asarray(ctrl, float)))
         y = np.ascontiguousarray(sensor, np.float64)
-        self._check(self.lib.mjpc_b200_unscented_update(self.h, u.ctypes.data_as(C.POINTER(C.c_double)),
-                                                        y.ctypes.data_as(C.POINTER(C.c_double)),
-                                                        None if mc is None else mc.ctypes.data_as(C.POINTER(C.c_float))))
-        return self.state
+        self._keep = (u, y, mc)
+        return _pd(u), _pd(y), _pf(mc)
 
     def _get(self):
-        C = self.C
         x, P = np.zeros(self.m.nq + self.m.nv), np.zeros((self.ndstate, self.ndstate))
-        t, sc = C.c_double(), np.zeros(5)
-        self._check(self.lib.mjpc_b200_unscented_get(self.h, x.ctypes.data_as(C.POINTER(C.c_double)),
-                                                     P.ctypes.data_as(C.POINTER(C.c_double)), C.byref(t),
-                                                     sc.ctypes.data_as(C.POINTER(C.c_double))))
+        t, sc = C.c_double(), np.zeros(self._nscalars)
+        self._call("get", _pd(x), _pd(P), C.byref(t), _pd(sc))
         return x, P, t.value, sc
 
     @property
@@ -417,49 +409,45 @@ class CppUnscented:
         return int(self._get()[3][3])
 
 
+class CppUnscented(_CppFilter):
+    """The C++ filter (csrc/host/unscented.{h,cc}, mjpc_b200_unscented_*) behind the same attributes as Unscented;
+    settings resolve from the model's numerics exactly as Unscented's do."""
+    _nscalars = 5
+
+    def __init__(self, m, sensor_start=None, nsensor=None, timestep=None, alpha=None, beta=None, device=0):
+        self.sensor_start, self.nsensor, self.timestep, self.alpha, self.beta = settings(m, sensor_start, nsensor,
+                                                                                         timestep, alpha, beta)
+        self.nsensordata = measured_range(m, self.sensor_start, self.nsensor)
+        self._create("mjpc_b200_unscented", m, self.sensor_start, self.nsensor, C.c_double(self.timestep),
+                     C.c_double(self.alpha), C.c_double(self.beta), int(device))
+        self.ndstate, self.nsigma = 2 * m.nv, 4 * m.nv + 1
+        self.reset()
+
+    def update(self, ctrl, sensor, mocap=None):
+        self._call("update", *self._args(ctrl, sensor, mocap))
+        return self.state
+
+
 # ------------------------------------------------------------------------------------------------------ Kalman
 KALMAN_EPSILON = 1e-3    # the engine's finite differences (profiles/kalman_epsilon_sweep.py, DESIGN.md)
 KALMAN_CENTERED = True
 
 
-def _default_mocap(m):
-    return np.concatenate([m.mocap_pos0, m.mocap_quat0], axis=1).reshape(-1) if m.nmocap else np.zeros(0)
-
-
-class Kalman:
+class Kalman(_Filter):
     """mjpc::Kalman.  `backend(sensor_start, nsensor, timestep)` returns the object that runs the steps (see
     EngineBackend); settings left None default from the model's numerics as GetNumberOrDefault does."""
 
     def __init__(self, m, backend, sensor_start=None, nsensor=None, timestep=None, epsilon=KALMAN_EPSILON,
                  centered=KALMAN_CENTERED):
-        self.m = m
-        self.sensor_start, self.nsensor, self.timestep = settings(m, sensor_start, nsensor, timestep)[:3]
-        self.nsensordata = measured_range(m, self.sensor_start, self.nsensor)
-        self.backend = backend(self.sensor_start, self.nsensor, self.timestep)
+        super().__init__(m, backend, sensor_start, nsensor, timestep)
         self.epsilon, self.centered = float(epsilon), bool(centered)
-        self.ndstate = 2 * m.nv
         self.nstates = (2 if self.centered else 1) * self.ndstate + 1
-        self.warnings = 0
         self.reset()
 
     def reset(self, state=None, time=0.0, covariance_scale=None, process_scale=None, sensor_scale=None):
-        """Reset (kalman.cc:113-185): state = the home keyframe if the model has one, else qpos0 and zero qvel."""
-        m = self.m
-        self.state, cs, ps, ss = reset_values(m, state, covariance_scale, process_scale, sensor_scale)
-        self.time = float(time)
-        self.covariance = cs * np.eye(self.ndstate)
-        self.noise_process = np.full(self.ndstate, float(ps))
-        self.noise_sensor = np.full(self.nsensordata, float(ss))
-        self.qacc_warmstart = np.zeros(m.nv)
-        self.ctrl, self.mocap = np.zeros(m.nu), _default_mocap(m)
-        self.warnings = 0
-
-    def set_noise(self, process=None, sensor=None):
-        """Diagonal process [ndstate] / sensor [nsensordata] noise; None keeps one."""
-        if process is not None:
-            self.noise_process = np.array(process, float)
-        if sensor is not None:
-            self.noise_sensor = np.array(sensor, float)
+        """Reset (kalman.cc:113-185), and the ctrl and mocap of the last measurement = zeros and the model's mocap."""
+        super().reset(state, time, covariance_scale, process_scale, sensor_scale)
+        self.ctrl, self.mocap = np.zeros(self.m.nu), _default_mocap(self.m)
 
     def perturbed(self):
         """[nstates][nq+nv]: the state, then x (+) eps e_i for i < ndstate, then (centred) x (+) -eps e_i; positions
@@ -477,10 +465,6 @@ class Kalman:
                 X[r, nq + i - nv] += e
         return X
 
-    def _step(self, ctrl, mocap):
-        warm = np.tile(self.qacc_warmstart, (self.nstates, 1))
-        return self.backend.step_sensors(self.perturbed(), np.asarray(ctrl, float), mocap, self.time, warm)
-
     def _column(self, plus, r):
         """Finite-difference column r of a Jacobian from the rows [nstates][...] of one step (difference `plus`)."""
         n, h = self.ndstate, (2 * self.epsilon if self.centered else self.epsilon)
@@ -488,35 +472,23 @@ class Kalman:
 
     def update_measurement(self, ctrl, sensor, mocap=None):
         """UpdateMeasurement (kalman.cc:188-276) from the measured sensor slice [nsensordata]."""
-        m = self.m
-        nq, nv = m.nq, m.nv
-        mocap = _default_mocap(m) if mocap is None else np.asarray(mocap, float)
-        nxt, y, qacc, nwarn = self._step(ctrl, mocap)
+        mocap = _default_mocap(self.m) if mocap is None else np.asarray(mocap, float)
+        nxt, y, qacc, nwarn = self._step(self.perturbed(), ctrl, mocap)
         C = np.stack([self._column(lambda a, b: y[a] - y[b], i) for i in range(self.ndstate)], axis=1)
         P = self.covariance
         PCt = P @ C.T
         S = C @ PCt + np.diag(self.noise_sensor)
-        try:
-            L = np.linalg.cholesky(S)
-        except np.linalg.LinAlgError:
-            raise EstimatorError("sensor covariance factorisation failed") from None
-        solve = lambda b: np.linalg.solve(L.T, np.linalg.solve(L, b))
-        corr = PCt @ solve(np.asarray(sensor, float) - y[0])
-        new = np.empty_like(self.state)
-        new[:nq] = integrate_pos(m, self.state[:nq], corr[:nv], 1.0)
-        new[nq:] = self.state[nq:] + corr[nv:]
-        P = P - PCt @ solve(PCt.T)
-        self.state, self.covariance = new, 0.5 * (P + P.T)
+        corr, self.covariance = self._gain(PCt, S, P, np.asarray(sensor, float) - y[0])
+        self.state = self._state_add(self.state, corr)
         self.ctrl, self.mocap = np.atleast_1d(np.asarray(ctrl, float)).copy(), mocap
-        self.qacc_warmstart = qacc[0].copy()
-        self.warnings += nwarn
+        self._commit(qacc[0], nwarn)
         return self.state
 
     def update_prediction(self):
         """UpdatePrediction (kalman.cc:279-323) with the ctrl and mocap of the last measurement; advances time."""
         m = self.m
         nq = m.nq
-        nxt, _, qacc, nwarn = self._step(self.ctrl, self.mocap)
+        nxt, _, qacc, nwarn = self._step(self.perturbed(), self.ctrl, self.mocap)
 
         def diff(a, b):
             return np.concatenate([differentiate_pos(m, nxt[b, :nq], nxt[a, :nq]), nxt[a, nq:] - nxt[b, nq:]])
@@ -524,8 +496,7 @@ class Kalman:
         P = A @ self.covariance @ A.T + np.diag(self.noise_process)
         self.state, self.covariance = nxt[0].copy(), 0.5 * (P + P.T)
         self.time = self.time + self.timestep
-        self.qacc_warmstart = qacc[0].copy()
-        self.warnings += nwarn
+        self._commit(qacc[0], nwarn)
         return self.state
 
     def update(self, ctrl, sensor, mocap=None):
@@ -534,104 +505,30 @@ class Kalman:
         return self.update_prediction()
 
 
-class CppKalman:
+class CppKalman(_CppFilter):
     """The C++ filter (csrc/host/kalman.{h,cc}, mjpc_b200_kalman_*) behind the same attributes as Kalman; settings
     resolve from the model's numerics exactly as Kalman's do."""
+    _nscalars = 6
 
     def __init__(self, m, sensor_start=None, nsensor=None, timestep=None, epsilon=KALMAN_EPSILON,
                  centered=KALMAN_CENTERED, device=0):
-        import ctypes as C
-        from .engine import EngineError, _model_blob, load_library
-        self.C, self.Error = C, EngineError
-        self.lib = load_library()
-        self.lib.mjpc_b200_kalman_last_error.restype = C.c_char_p
-        self.lib.mjpc_b200_kalman_last_error.argtypes = [C.c_void_p]
-        self.lib.mjpc_b200_kalman_destroy.argtypes = [C.c_void_p]
-        self.m = m
         self.sensor_start, self.nsensor, self.timestep = settings(m, sensor_start, nsensor, timestep)[:3]
         self.nsensordata = measured_range(m, self.sensor_start, self.nsensor)
         self.epsilon, self.centered = float(epsilon), bool(centered)
-        self._buf, mb = _model_blob(m)
-        h = C.c_void_p()
-        rc = self.lib.mjpc_b200_kalman_create(C.byref(mb), self.sensor_start, self.nsensor, C.c_double(self.timestep),
-                                              C.c_double(self.epsilon), int(self.centered), int(device), C.byref(h))
-        if rc != 0:
-            raise EngineError(f"mjpc_b200_kalman_create failed ({rc}): {self.lib.mjpc_b200_last_error().decode()}")
-        self.h = h
+        self._create("mjpc_b200_kalman", m, self.sensor_start, self.nsensor, C.c_double(self.timestep),
+                     C.c_double(self.epsilon), int(self.centered), int(device))
         self.ndstate = 2 * m.nv
         self.nstates = (2 if self.centered else 1) * self.ndstate + 1
         self.reset()
 
-    def close(self):
-        if getattr(self, "h", None):
-            self.lib.mjpc_b200_kalman_destroy(self.h)
-            self.h = None
-
-    __del__ = close
-
-    def _pd(self, a):
-        return None if a is None else np.ascontiguousarray(a, np.float64).ctypes.data_as(self.C.POINTER(self.C.c_double))
-
-    def _check(self, rc):
-        if rc != 0:
-            msg = self.lib.mjpc_b200_kalman_last_error(self.h).decode()
-            if "factorisation" in msg:
-                raise EstimatorError(msg)
-            raise self.Error(f"mjpc_b200_kalman error {rc}: {msg}")
-
-    def reset(self, state=None, time=0.0, covariance_scale=None, process_scale=None, sensor_scale=None):
-        x, cs, ps, ss = reset_values(self.m, state, covariance_scale, process_scale, sensor_scale)
-        self._check(self.lib.mjpc_b200_kalman_reset(self.h, self._pd(x), self.C.c_double(time), self.C.c_double(cs),
-                                                    self.C.c_double(ps), self.C.c_double(ss)))
-
-    def set_noise(self, process=None, sensor=None):
-        self._check(self.lib.mjpc_b200_kalman_set_noise(self.h, self._pd(process), self._pd(sensor)))
-
-    def set(self, state, covariance, time):
-        self._check(self.lib.mjpc_b200_kalman_set(self.h, self._pd(state), self._pd(covariance), self.C.c_double(time)))
-
-    def _args(self, ctrl, sensor, mocap):
-        C = self.C
-        mc = None if mocap is None or len(mocap) == 0 else np.ascontiguousarray(mocap, np.float32)
-        u = np.ascontiguousarray(np.atleast_1d(np.asarray(ctrl, float)))
-        y = np.ascontiguousarray(sensor, np.float64)
-        self._keep = (u, y, mc)
-        return (u.ctypes.data_as(C.POINTER(C.c_double)), y.ctypes.data_as(C.POINTER(C.c_double)),
-                None if mc is None else mc.ctypes.data_as(C.POINTER(C.c_float)))
-
     def update_measurement(self, ctrl, sensor, mocap=None):
-        self._check(self.lib.mjpc_b200_kalman_update_measurement(self.h, *self._args(ctrl, sensor, mocap)))
+        self._call("update_measurement", *self._args(ctrl, sensor, mocap))
         return self.state
 
     def update_prediction(self):
-        self._check(self.lib.mjpc_b200_kalman_update_prediction(self.h))
+        self._call("update_prediction")
         return self.state
 
     def update(self, ctrl, sensor, mocap=None):
-        self._check(self.lib.mjpc_b200_kalman_update(self.h, *self._args(ctrl, sensor, mocap)))
+        self._call("update", *self._args(ctrl, sensor, mocap))
         return self.state
-
-    def _get(self):
-        C = self.C
-        x, P = np.zeros(self.m.nq + self.m.nv), np.zeros((self.ndstate, self.ndstate))
-        t, sc = C.c_double(), np.zeros(6)
-        self._check(self.lib.mjpc_b200_kalman_get(self.h, x.ctypes.data_as(C.POINTER(C.c_double)),
-                                                  P.ctypes.data_as(C.POINTER(C.c_double)), C.byref(t),
-                                                  sc.ctypes.data_as(C.POINTER(C.c_double))))
-        return x, P, t.value, sc
-
-    @property
-    def state(self):
-        return self._get()[0]
-
-    @property
-    def covariance(self):
-        return self._get()[1]
-
-    @property
-    def time(self):
-        return self._get()[2]
-
-    @property
-    def warnings(self):
-        return int(self._get()[3][3])

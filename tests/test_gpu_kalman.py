@@ -19,7 +19,8 @@ from estimator_backends import OracleSigmaBackend, load_estimator_model, mocap_v
 from quadruped_filtering import plant, run_filter  # noqa: E402
 from test_kalman_cpu import IMU_CHAIN_XML, IMU_FREE_XML, load_task_imu  # noqa: E402
 
-from mujoco_mpc_b200.estimator import (CppKalman, EngineBackend, EstimatorError, Kalman, Unscented)  # noqa: E402
+from mujoco_mpc_b200.estimator import (CppKalman, CppUnscented, EngineBackend, EstimatorError, Kalman,  # noqa: E402
+                                       Unscented)
 from mujoco_mpc_b200.mjcf import SENS_ACCELEROMETER, compile_xml  # noqa: E402
 
 pytestmark = pytest.mark.gpu
@@ -210,10 +211,10 @@ def test_kalman_quadruped_filtering_against_the_oracle_plant():
     e.close()
 
 
-def test_kalman_create_refusals():
-    """kalman_create itself refuses a range outside the model's sensors and one with a sensor the engine does not
+def _create_refusals(kind, cpp_filter):
+    """<kind>_create itself refuses a range outside the model's sensors and one with a sensor the engine does not
     evaluate (the Python wrapper's measured_range check is bypassed to reach it); a failed sensor-covariance
-    factorisation through CppKalman leaves state, covariance and time untouched."""
+    factorisation through the C++ filter leaves state, covariance and time untouched."""
     import ctypes as C
     from mujoco_mpc_b200 import models
     from mujoco_mpc_b200.engine import _model_blob, load_library
@@ -221,12 +222,14 @@ def test_kalman_create_refusals():
     m = models.load("quadruped")
     _, mb = _model_blob(m)
     h = C.c_void_p()
-    args = (C.c_double(0.005), C.c_double(1e-3), 1, 0, C.byref(h))
-    assert lib.mjpc_b200_kalman_create(C.byref(mb), 0, 10, *args) == -5 and not h.value      # user sensors
-    assert lib.mjpc_b200_kalman_create(C.byref(mb), 9, m.nsensor, *args) == -1 and not h.value
-    assert lib.mjpc_b200_kalman_create(C.byref(mb), -1, 2, *args) == -1 and not h.value
+    create = getattr(lib, "mjpc_b200_%s_create" % kind)
+    settings = (C.c_double(1e-3), 1) if kind == "kalman" else (C.c_double(1.0), C.c_double(2.0))
+    args = (C.c_double(0.005), *settings, 0, C.byref(h))
+    assert create(C.byref(mb), 0, 10, *args) == -5 and not h.value      # user sensors
+    assert create(C.byref(mb), 9, m.nsensor, *args) == -1 and not h.value
+    assert create(C.byref(mb), -1, 2, *args) == -1 and not h.value
     p = load_task_imu()
-    f = CppKalman(p)
+    f = cpp_filter(p)
     f.reset(state=[0.25, 0.0], time=0.3)
     f.set_noise(sensor=np.full(f.nsensordata, -1.0))
     before = (f.state, f.covariance, f.time)
@@ -234,6 +237,15 @@ def test_kalman_create_refusals():
         f.update(np.zeros(p.nu), [0.25, 0.0, 0.0, 0.0])
     assert np.array_equal(f.state, before[0]) and np.array_equal(f.covariance, before[1]) and f.time == before[2]
     f.close()
+
+
+def test_kalman_create_refusals():
+    _create_refusals("kalman", CppKalman)
+
+
+def test_unscented_create_refusals():
+    """The Unscented filter's create refuses the same inputs as the Kalman filter's: both step the reset state once."""
+    _create_refusals("unscented", CppUnscented)
 
 
 def test_unscented_on_task_imu_through_the_new_sensors():
