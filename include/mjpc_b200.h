@@ -240,61 +240,55 @@ int mjpc_b200_step_sensors(mjpc_b200_t* h, int B, const float* states, const flo
                            const float* mocap, double time, int sensor_start, int nsensor, float* next_states,
                            float* sensordata, float* qacc, int* counts);
 
-/* MJPC's Unscented state estimator (mjpc/estimators/unscented.cc, class mjpc_b200_host::Unscented in
- * csrc/host/unscented.h on the Estimator base): the filter in double on the host, its 2 ndstate + 1 sigma-point steps
- * as one mjpc_b200_step_sensors launch on a handle it owns (max_candidates = nsigma).  Settings are explicit (alpha 1,
- * beta 2, timestep = estimator_timestep or opt.timestep, noise scales 1e-4 by default).  create: measured sensors
- * [sensor_start, sensor_start + nsensor) of the blob, refused as kalman_create refuses them.  reset: state NULL -> the
- * model's first keyframe, else qpos0 and zero qvel; covariance = covariance_scale I, diagonal process / sensor noise.
- * set_noise: process [ndstate], sensor [nsensordata] (NULL keeps one).  set: state, covariance [ndstate^2] (NULL keeps
- * one) and time.  update: ctrl [nu], the measured sensor slice [nsensordata], mocap [7 nmocap] or NULL (the model's);
- * a failed covariance or sensor-covariance factorisation returns MJPC_B200_ERR_BAD_ARGUMENT and leaves state,
- * covariance and time untouched (unscented_last_error names the factor).  get: state [nq+nv], covariance, time and
- * scalars[5] = {ndstate, nsigma, nsensordata, sigma-point steps that raised a warning since reset, timestep}. */
-typedef struct mjpc_b200_unscented mjpc_b200_unscented_t;
-int mjpc_b200_unscented_create(const mjpc_model_blob* model, int sensor_start, int nsensor, double timestep,
-                               double alpha, double beta, int device, mjpc_b200_unscented_t** out);
-void mjpc_b200_unscented_destroy(mjpc_b200_unscented_t* u);
-int mjpc_b200_unscented_reset(mjpc_b200_unscented_t* u, const double* state, double time, double covariance_scale,
+/* ---- State estimators (csrc/host/estimator.h, the reference's Estimator base mjpc/estimators/estimator.h): the filter
+ * in double on the host, its steps as mjpc_b200_step_sensors launches on an engine handle it owns (max_candidates =
+ * 2 ndstate + 1).  Each kind has its own create (its settings); every other call is one of the generic
+ * mjpc_b200_estimator_* below, which take a filter of any kind and return MJPC_B200_ERR_BAD_ARGUMENT for a NULL one
+ * (last_error: "").  create measures the sensors [sensor_start, sensor_start + nsensor) of the blob; it steps the reset
+ * state once, so a range outside the model's sensors returns MJPC_B200_ERR_BAD_ARGUMENT and a sensor the engine does
+ * not evaluate MJPC_B200_ERR_UNSUPPORTED.  Settings are explicit (timestep = estimator_timestep or opt.timestep, noise
+ * scales 1e-4 by default).
+ *   reset      state NULL -> the model's first keyframe, else qpos0 and zero qvel; covariance = covariance_scale I,
+ *              diagonal process / sensor noise
+ *   set_noise  process [ndstate], sensor [nsensordata] (NULL keeps one)
+ *   set        state, covariance [ndstate^2] (NULL keeps one) and time
+ *   update     one filter update from ctrl [nu], the measured sensor slice [nsensordata] and mocap [7 nmocap] or NULL
+ *              (the model's).  A failed factorisation returns MJPC_B200_ERR_BAD_ARGUMENT and leaves state, covariance
+ *              and time untouched; last_error names the factor.
+ *   get        state [nq+nv], covariance, time and the kind's scalars (any pointer may be NULL) */
+typedef struct mjpc_b200_estimator mjpc_b200_estimator_t;
+int mjpc_b200_estimator_destroy(mjpc_b200_estimator_t* f);
+int mjpc_b200_estimator_reset(mjpc_b200_estimator_t* f, const double* state, double time, double covariance_scale,
                               double process_scale, double sensor_scale);
-int mjpc_b200_unscented_set_noise(mjpc_b200_unscented_t* u, const double* process, const double* sensor);
-int mjpc_b200_unscented_set(mjpc_b200_unscented_t* u, const double* state, const double* covariance, double time);
-int mjpc_b200_unscented_update(mjpc_b200_unscented_t* u, const double* ctrl, const double* sensor, const float* mocap);
-int mjpc_b200_unscented_get(const mjpc_b200_unscented_t* u, double* state, double* covariance, double* time,
+int mjpc_b200_estimator_set_noise(mjpc_b200_estimator_t* f, const double* process, const double* sensor);
+int mjpc_b200_estimator_set(mjpc_b200_estimator_t* f, const double* state, const double* covariance, double time);
+int mjpc_b200_estimator_update(mjpc_b200_estimator_t* f, const double* ctrl, const double* sensor, const float* mocap);
+int mjpc_b200_estimator_get(const mjpc_b200_estimator_t* f, double* state, double* covariance, double* time,
                             double* scalars);
-const char* mjpc_b200_unscented_last_error(const mjpc_b200_unscented_t* u);
+const char* mjpc_b200_estimator_last_error(const mjpc_b200_estimator_t* f);
 
-/* MJPC's Kalman state estimator (mjpc/estimators/kalman.cc, class mjpc_b200_host::Kalman in csrc/host/kalman.h): the
- * filter in double precision on the host, its finite-difference Jacobians as one mjpc_b200_step_sensors launch each
- * (the centre state and its ndstate tangent-space perturbations x (+) eps e_i, then x (+) -eps e_i when centered) on an
- * engine handle it owns (max_candidates = 2 ndstate + 1).  Settings are explicit (timestep = estimator_timestep or
- * opt.timestep, the three noise scales 1e-4; the reference's finite differences are 1e-6 one-sided, an fp64 setting:
- * mujoco_mpc_b200.estimator.KALMAN_EPSILON / KALMAN_CENTERED are the engine's).  create: measured sensors
- * [sensor_start, sensor_start + nsensor) of the blob; it steps the reset state once, so a range outside the model's
- * sensors returns MJPC_B200_ERR_BAD_ARGUMENT and a sensor the engine does not evaluate MJPC_B200_ERR_UNSUPPORTED.
- * reset / set_noise / set: as for the Unscented filter.  update_measurement: ctrl [nu], the measured sensor slice
- * [nsensordata], mocap [7 nmocap] or NULL (the model's); C and the predicted sensors come from one launch at the current
- * state, then the gain, correction and covariance update.  A failed sensor-covariance factorisation returns
- * MJPC_B200_ERR_BAD_ARGUMENT and leaves state, covariance and time untouched (kalman_last_error names the factor).
- * update_prediction: A and the next state from one launch with the ctrl and mocap of the last measurement (zeros and
- * the model's mocap after reset), P = A P A' + diag(process noise), time += timestep.  update: both.  get: state
- * [nq+nv], covariance, time and scalars[6] = {ndstate, states per launch, nsensordata, steps that raised a warning
+/* MJPC's Unscented state estimator (mjpc/estimators/unscented.cc, class mjpc_b200_host::Unscented in
+ * csrc/host/unscented.h): its 2 ndstate + 1 sigma-point steps are one launch (alpha 1, beta 2 by default).  update can
+ * fail on the covariance or the sensor-covariance factor.  get: scalars[5] = {ndstate, nsigma, nsensordata, sigma-point
+ * steps that raised a warning since reset, timestep}. */
+int mjpc_b200_unscented_create(const mjpc_model_blob* model, int sensor_start, int nsensor, double timestep,
+                               double alpha, double beta, int device, mjpc_b200_estimator_t** out);
+
+/* MJPC's Kalman state estimator (mjpc/estimators/kalman.cc, class mjpc_b200_host::Kalman in csrc/host/kalman.h): its
+ * finite-difference Jacobians are one launch each (the centre state and its ndstate tangent-space perturbations
+ * x (+) eps e_i, then x (+) -eps e_i when centered).  The reference's finite differences are 1e-6 one-sided, an fp64
+ * setting: mujoco_mpc_b200.estimator.KALMAN_EPSILON / KALMAN_CENTERED are the engine's.  update_measurement (the same
+ * arguments as update): C and the predicted sensors from one launch at the current state, then the gain, correction and
+ * covariance update; it can fail on the sensor-covariance factor.  update_prediction: A and the next state from one
+ * launch with the ctrl and mocap of the last measurement (zeros and the model's mocap after reset),
+ * P = A P A' + diag(process noise), time += timestep.  update: both.  Both return MJPC_B200_ERR_BAD_ARGUMENT for a
+ * filter that is not a Kalman filter.  get: scalars[6] = {ndstate, states per launch, nsensordata, steps that raised a warning
  * since reset, timestep, epsilon}. */
-typedef struct mjpc_b200_kalman mjpc_b200_kalman_t;
 int mjpc_b200_kalman_create(const mjpc_model_blob* model, int sensor_start, int nsensor, double timestep,
-                            double epsilon, int centered, int device, mjpc_b200_kalman_t** out);
-void mjpc_b200_kalman_destroy(mjpc_b200_kalman_t* k);
-int mjpc_b200_kalman_reset(mjpc_b200_kalman_t* k, const double* state, double time, double covariance_scale,
-                           double process_scale, double sensor_scale);
-int mjpc_b200_kalman_set_noise(mjpc_b200_kalman_t* k, const double* process, const double* sensor);
-int mjpc_b200_kalman_set(mjpc_b200_kalman_t* k, const double* state, const double* covariance, double time);
-int mjpc_b200_kalman_update_measurement(mjpc_b200_kalman_t* k, const double* ctrl, const double* sensor,
+                            double epsilon, int centered, int device, mjpc_b200_estimator_t** out);
+int mjpc_b200_kalman_update_measurement(mjpc_b200_estimator_t* f, const double* ctrl, const double* sensor,
                                         const float* mocap);
-int mjpc_b200_kalman_update_prediction(mjpc_b200_kalman_t* k);
-int mjpc_b200_kalman_update(mjpc_b200_kalman_t* k, const double* ctrl, const double* sensor, const float* mocap);
-int mjpc_b200_kalman_get(const mjpc_b200_kalman_t* k, double* state, double* covariance, double* time,
-                         double* scalars);
-const char* mjpc_b200_kalman_last_error(const mjpc_b200_kalman_t* k);
+int mjpc_b200_kalman_update_prediction(mjpc_b200_estimator_t* f);
 
 /* Per-candidate execution statistics of the last rollout, stats [N][12] = {SM cycles, Newton iterations, contacts,
  * constraint rows (summed over steps), 8 per-phase cycle counters (zero unless built with -DMJPC_PHASE_TIMING)}. */
@@ -347,24 +341,50 @@ int mjpc_b200_fetch_trajectory_sharded(mjpc_b200_t* h, int candidate, float* sta
 void* mjpc_b200_stream(mjpc_b200_t* h);
 float* mjpc_b200_device_returns(mjpc_b200_t* h);
 
-/* ---- C++ host layer above the ABI (csrc/host/sampling_planner.{h,cc}): SamplingPlanner with the reference's
- * method names (mjpc/planners/sampling/planner.h:40-160); these C wrappers are what ctypes / a test harness binds.
+/* ---- C++ host layer above the ABI (csrc/host): the reference's planners with its method names; these C wrappers are
+ * what ctypes / a test harness binds.
  * mjpc_b200_host_spline_sample = TimeSpline::Sample (mjpc/spline/spline.cc:103-156), usable without a GPU. */
 void mjpc_b200_host_spline_sample(const double* times, const double* values, int P, int dim, int interp, double t,
                                   double* out);
 double mjpc_b200_host_philox_normal(uint32_t seed, uint32_t iteration, uint32_t candidate, uint32_t knot, uint32_t dof);
-int mjpc_b200_planner_create(const mjpc_model_blob* model, int num_trajectory, int num_spline_points, int interpolation,
-                             double exploration, double timestep, const double* ctrlrange, uint32_t seed,
-                             int max_horizon, int device, void** out);
-void mjpc_b200_planner_destroy(void* planner);
+
+/* ---- Planners (csrc/host/planner.h, the reference's Planner interface mjpc/planners/planner.h:33-77).  Each kind has
+ * its own create (its settings) and get_result (its result shape), and the sampling and iLQS planners a
+ * set_exploration; these return MJPC_B200_ERR_BAD_ARGUMENT for a NULL handle or one of another kind.  Every other call
+ * is one of the generic mjpc_b200_planner_* below, which take a planner of any kind and return
+ * MJPC_B200_ERR_BAD_ARGUMENT for a NULL one.
+ *   reset               Planner::Reset to horizon steps; initial_repeated_action [nu] may be NULL
+ *   set_state           state [dim_state], absolute time, mocap [7 nmocap] (NULL keeps the previous one)
+ *   optimize_policy     Planner::OptimizePolicy: <0 on error.  The sampling, Cross-Entropy, Sample Gradient and Robust
+ *                       planners return 0; iLQG and iLQS 1 when the policy was updated, 0 when the iteration was
+ *                       rejected; Gradient 1 when the return improved, 0 when the nominal was kept
+ *   nominal_trajectory  Planner::NominalTrajectory, what planning does while it is disabled
+ *   action_from_policy  action [nu] of the policy at `time`.  state [dim_state] (may be NULL: open loop) is read by the
+ *                       iLQG policy (iLQG, iLQS); use_previous != 0 reads the previous policy of the sampling-based
+ *                       planners (the others ignore it)
+ *   set_fd              finite-difference settings of the derivative-based planners (ilqg/settings.h:23-24,
+ *                       iLQGPlanner::derivative_skip_): tolerance <= 0 / mode < 0 / skip < 0 keep the current value.
+ *                       Defaults 3e-4, centred, 0 (the reference's 1e-6 one-sided is an fp64 setting, ilqg_planner.h).
+ *                       Gradient, iLQG and the iLQG half of iLQS; the others return MJPC_B200_ERR_UNSUPPORTED */
+typedef struct mjpc_b200_planner mjpc_b200_planner_t;
+int mjpc_b200_planner_destroy(mjpc_b200_planner_t* p);
+int mjpc_b200_planner_reset(mjpc_b200_planner_t* p, int horizon, const double* initial_repeated_action);
+int mjpc_b200_planner_set_state(mjpc_b200_planner_t* p, const double* state, double time, const double* mocap);
+int mjpc_b200_planner_optimize_policy(mjpc_b200_planner_t* p, int horizon);
+int mjpc_b200_planner_nominal_trajectory(mjpc_b200_planner_t* p, int horizon);
+int mjpc_b200_planner_action_from_policy(mjpc_b200_planner_t* p, double* action, const double* state, double time,
+                                         int use_previous);
+int mjpc_b200_planner_set_fd(mjpc_b200_planner_t* p, double tolerance, int mode, int derivative_skip);
+
+/* ---- Predictive Sampling (csrc/host/sampling_planner.{h,cc}; mjpc/planners/sampling/planner.h:40-160). */
+int mjpc_b200_sampling_planner_create(const mjpc_model_blob* model, int num_trajectory, int num_spline_points,
+                                      int interpolation, double exploration, double timestep, const double* ctrlrange,
+                                      uint32_t seed, int max_horizon, int device, mjpc_b200_planner_t** out);
 /* noise_exploration[0..1] (sampling/planner.cc:85-88, 334-338): exploration2 > 0 replaces the std with probability 0.2 */
-void mjpc_b200_planner_set_exploration(void* planner, double exploration, double exploration2);
-void mjpc_b200_planner_reset(void* planner, int horizon, const double* initial_repeated_action);
-void mjpc_b200_planner_set_state(void* planner, const double* state, double time, const double* mocap);
-int mjpc_b200_planner_optimize_policy(void* planner, int horizon);          /* SamplingPlanner::OptimizePolicy */
-void mjpc_b200_planner_action_from_policy(void* planner, double* action, double time, int use_previous);
-int mjpc_b200_planner_get_result(void* planner, int* winner, double* improvement, float* returns, double* knots,
-                                 double* knot_times);
+int mjpc_b200_sampling_planner_set_exploration(mjpc_b200_planner_t* p, double exploration, double exploration2);
+/* winner, improvement, returns [num_trajectory], installed knots [P][nu] / times [P]; returns the number of knots */
+int mjpc_b200_sampling_planner_get_result(mjpc_b200_planner_t* p, int* winner, double* improvement, float* returns,
+                                          double* knots, double* knot_times);
 
 /* ---- Batched Predictive Sampling (csrc/host/batch_sampling_planner.{h,cc}): num_problems independent SamplingPlanners
  * (each with its own seed, state, mocap, task snapshot and policy) on ONE engine handle; optimize_policy makes one
@@ -382,7 +402,8 @@ int mjpc_b200_batch_planner_set_task(void* planner, int problem, const double* w
                                      const double* task_state);
 int mjpc_b200_batch_planner_optimize_policy(void* planner, int horizon);   /* every problem: SamplingPlanner::OptimizePolicy */
 int mjpc_b200_batch_planner_action_from_policy(void* planner, int problem, double* action, double time, int use_previous);
-/* as mjpc_b200_planner_get_result for one problem (returns [num_trajectory]); returns the number of installed knots */
+/* as mjpc_b200_sampling_planner_get_result for one problem (returns [num_trajectory]); returns the number of installed
+ * knots */
 int mjpc_b200_batch_planner_get_result(void* planner, int problem, int* winner, double* improvement, float* returns,
                                        double* knots, double* knot_times);
 
@@ -393,38 +414,29 @@ int mjpc_b200_batch_planner_get_result(void* planner, int problem, int* winner, 
 int mjpc_b200_ce_planner_create(const mjpc_model_blob* model, int num_trajectory, int n_elite, int num_spline_points,
                                 int interpolation, double std_initial, double std_min, double explore_fraction,
                                 double timestep, const double* ctrlrange, uint32_t seed, int max_horizon, int device,
-                                void** out);
-void mjpc_b200_ce_planner_destroy(void* planner);
-void mjpc_b200_ce_planner_reset(void* planner, int horizon, const double* initial_repeated_action);
-void mjpc_b200_ce_planner_set_state(void* planner, const double* state, double time, const double* mocap);
-int mjpc_b200_ce_planner_optimize_policy(void* planner, int horizon);       /* CrossEntropyPlanner::OptimizePolicy */
-void mjpc_b200_ce_planner_action_from_policy(void* planner, double* action, double time, int use_previous);
+                                mjpc_b200_planner_t** out);
 /* improvement, returns [N+1] (last = nominal), elite order [N], installed knots [P][nu] / times [P], variance [P][nu];
  * returns the number of spline points */
-int mjpc_b200_ce_planner_get_result(void* planner, double* improvement, float* returns, int* order, double* knots,
-                                    double* knot_times, double* variance);
+int mjpc_b200_ce_planner_get_result(mjpc_b200_planner_t* p, double* improvement, float* returns, int* order,
+                                    double* knots, double* knot_times, double* variance);
 
 /* ---- Sample Gradient planner (csrc/host/sample_gradient_planner.{h,cc}; mjpc/planners/sample_gradient/planner.cc).
  * One rollout launch covers candidate 0 (the resampled nominal), the noisy samples 1 .. N-G-1 (knot += exploration * z,
  * not scaled by the control range) and the G gradient candidates N-G .. N-1 computed by the previous iteration; the
  * fitness-shaped gradient estimate and the log-spaced steps (1e-3 .. 2) along it are host arithmetic in double.
- * num_gradient is clamped to N - 1 on every optimize_policy.  Requires num_trajectory >= 1, num_spline_points >= 2. */
+ * num_gradient is clamped to N - 1 on every optimize_policy; nominal_trajectory rolls out the resampled nominal alone.
+ * Requires num_trajectory >= 1, num_spline_points >= 2. */
 int mjpc_b200_sg_planner_create(const mjpc_model_blob* model, int num_trajectory, int num_gradient, int num_spline_points,
                                 int interpolation, double exploration, double gradient_filter, double timestep,
-                                const double* ctrlrange, uint32_t seed, int max_horizon, int device, void** out);
-void mjpc_b200_sg_planner_destroy(void* planner);
-void mjpc_b200_sg_planner_reset(void* planner, int horizon, const double* initial_repeated_action);
-void mjpc_b200_sg_planner_set_state(void* planner, const double* state, double time, const double* mocap);
-int mjpc_b200_sg_planner_optimize_policy(void* planner, int horizon);       /* SampleGradientPlanner::OptimizePolicy */
-int mjpc_b200_sg_planner_nominal_trajectory(void* planner, int horizon);    /* rolls out the resampled nominal alone */
-void mjpc_b200_sg_planner_action_from_policy(void* planner, double* action, double time, int use_previous);
+                                const double* ctrlrange, uint32_t seed, int max_horizon, int device,
+                                mjpc_b200_planner_t** out);
 /* winner, winner_type (0 nominal, 1 noisy, 2 gradient), improvement, returns [N], order [N] (as trajectory_order holds
  * it: the ranking of all N, or of the N-G noisy samples in its first N-G entries on the call that computed the
  * fitness weights), installed knots [P][nu] / times [P], gradient candidates' knots [G][P][nu] as the next iteration
  * resamples and rolls them out, gradient [P][nu].  Any pointer may be NULL; returns the number of installed knots. */
-int mjpc_b200_sg_planner_get_result(void* planner, int* winner, int* winner_type, double* improvement, float* returns,
-                                    int* order, double* knots, double* knot_times, double* gradient_knots,
-                                    double* gradient);
+int mjpc_b200_sg_planner_get_result(mjpc_b200_planner_t* p, int* winner, int* winner_type, double* improvement,
+                                    float* returns, int* order, double* knots, double* knot_times,
+                                    double* gradient_knots, double* gradient);
 
 /* ---- Robust planner (csrc/host/robust_planner.{h,cc}; mjpc/planners/robust/robust_planner.cc:40-160) over the
  * sampling planner: the best `ncandidates` of the clean launch are re-rolled `nrepetitions` times each with
@@ -433,15 +445,10 @@ int mjpc_b200_sg_planner_get_result(void* planner, int* winner, int* winner_type
 int mjpc_b200_robust_planner_create(const mjpc_model_blob* model, int num_trajectory, int num_spline_points,
                                     int interpolation, double exploration, double timestep, const double* ctrlrange,
                                     uint32_t seed, int ncandidates, int nrepetitions, double xfrc_std, double xfrc_rate,
-                                    int max_horizon, int device, void** out);
-void mjpc_b200_robust_planner_destroy(void* planner);
-void mjpc_b200_robust_planner_reset(void* planner, int horizon, const double* initial_repeated_action);
-void mjpc_b200_robust_planner_set_state(void* planner, const double* state, double time, const double* mocap);
-int mjpc_b200_robust_planner_optimize_policy(void* planner, int horizon);
-void mjpc_b200_robust_planner_action_from_policy(void* planner, double* action, double time, int use_previous);
+                                    int max_horizon, int device, mjpc_b200_planner_t** out);
 /* winner, robust scores [ncandidates], clean returns [num_trajectory], installed knots/times; returns #scores */
-int mjpc_b200_robust_planner_get_result(void* planner, int* winner, double* scores, float* returns, double* knots,
-                                        double* knot_times);
+int mjpc_b200_robust_planner_get_result(mjpc_b200_planner_t* p, int* winner, double* scores, float* returns,
+                                        double* knots, double* knot_times);
 
 /* ---- Task::Transition of the config tasks on the host (csrc/host/task_transition.{h,cc}): the state machines that
  * produce the task-state block the kernels consume (QuadrupedFlat::TransitionLocked quadruped.cc:228-395,
@@ -471,27 +478,19 @@ int mjpc_b200_shadow_transition_step(void* transition, double* qpos, double* qve
 /* ---- iLQG planner (csrc/host/ilqg_planner.{h,cc}; mjpc/planners/ilqg/planner.h, planner.cc:156-740).
  * OptimizePolicy = NominalTrajectory (feedback-scaling line search) + Iteration (model derivatives, cost derivatives,
  * backward pass with the regularisation retry loop, K action rollouts, winner, regularisation update); each sweep is
- * one call of the ABI above.  Returns 1 when the policy was updated, 0 when the iteration was rejected, <0 on error. */
+ * one call of the ABI above.  fd_tolerance <= 0 keeps the default (set_fd).  action_from_policy is iLQGPolicy::Action
+ * (ilqg/policy.cc:82-161): with a state the time-varying feedback feedback_scaling * K (state (-) x_nominal) is added
+ * before clamping. */
 int mjpc_b200_ilqg_planner_create(const mjpc_model_blob* model, int num_rollouts, int representation, double fd_tolerance,
-                                  int max_horizon, int device, void** out);
-void mjpc_b200_ilqg_planner_destroy(void* planner);
-/* finite-difference settings (ilqg/settings.h:23-24, iLQGPlanner::derivative_skip_): tolerance <= 0 / mode < 0 / skip < 0 keep
- * the current value.  Defaults here: 3e-4, centred, 0 - the reference's 1e-6 one-sided is an fp64 setting (ilqg_planner.h). */
-void mjpc_b200_ilqg_planner_set_fd(void* planner, double tolerance, int mode, int derivative_skip);
-void mjpc_b200_ilqg_planner_reset(void* planner, int horizon, const double* initial_repeated_action);
-void mjpc_b200_ilqg_planner_set_state(void* planner, const double* state, double time, const double* mocap);
-int mjpc_b200_ilqg_planner_nominal_trajectory(void* planner, int horizon);
-int mjpc_b200_ilqg_planner_optimize_policy(void* planner, int horizon);
-/* iLQGPolicy::Action (ilqg/policy.cc:82-161): state may be NULL (open loop), otherwise the time-varying feedback
- * feedback_scaling * K (state (-) x_nominal) is added before clamping */
-void mjpc_b200_ilqg_planner_action_from_policy(void* planner, double* action, const double* state, double time);
-/* the same, stateless and host only: u_nom [H][nu], x_nom [H][dim_state], t_nom [H], gains [H][nu][2 nv] */
+                                  int max_horizon, int device, mjpc_b200_planner_t** out);
+/* iLQGPolicy::Action, stateless and host only: u_nom [H][nu], x_nom [H][dim_state], t_nom [H], gains [H][nu][2 nv] */
 int mjpc_b200_host_ilqg_policy_action(const mjpc_model_blob* model, const float* u_nom, const float* x_nom,
                                       const double* t_nom, const float* gains, int horizon, int representation,
                                       double feedback_scaling, const double* state, double time, double* action);
 /* scalars[6] = {total_return, regularization, improvement, expected, surprise, winner}; nominal states [H][dim_state],
  * actions [H][nu], times [H] (any pointer may be NULL); returns H */
-int mjpc_b200_ilqg_planner_get_result(void* planner, double* scalars, float* states, float* actions, double* times);
+int mjpc_b200_ilqg_planner_get_result(mjpc_b200_planner_t* p, double* scalars, float* states, float* actions,
+                                      double* times);
 
 /* ---- Batched iLQG (csrc/host/batch_ilqg_planner.{h,cc}): num_problems independent iLQGPlanners (each with its own
  * state, mocap, task snapshot, policy and regularisation) on ONE engine handle.  optimize_policy makes one batched
@@ -519,18 +518,12 @@ int mjpc_b200_batch_ilqg_planner_get_result(void* planner, int problem, double* 
 /* ---- Gradient planner (csrc/host/gradient_planner.{h,cc}; mjpc/planners/gradient/planner.cc:159-383, gradient.cc:44-107,
  * spline_mapping.cc): ResamplePolicy, nominal rollout, {model derivatives, cost derivatives, gradient sweep, total derivative
  * through the spline mapping, K line-search rollouts (ONE mjpc_b200_rollout_spline launch)} x max_rollout.
- * optimize_policy returns 1 when the return improved, 0 when the nominal was kept, <0 on error. */
+ * fd_tolerance <= 0 keeps the default (set_fd). */
 int mjpc_b200_gradient_planner_create(const mjpc_model_blob* model, int num_trajectory, int num_spline_points, int representation,
                                       double fd_tolerance, double timestep, const double* ctrlrange, int max_horizon, int device,
-                                      void** out);
-void mjpc_b200_gradient_planner_destroy(void* planner);
-void mjpc_b200_gradient_planner_set_fd(void* planner, double tolerance, int mode, int derivative_skip);   /* as for the iLQG planner */
-void mjpc_b200_gradient_planner_reset(void* planner, int horizon, const double* initial_repeated_action);
-void mjpc_b200_gradient_planner_set_state(void* planner, const double* state, double time, const double* mocap);
-int mjpc_b200_gradient_planner_optimize_policy(void* planner, int horizon);
-void mjpc_b200_gradient_planner_action_from_policy(void* planner, double* action, double time, int use_previous);
+                                      mjpc_b200_planner_t** out);
 /* scalars[6] = {total_return, winner, action_step, expected, improvement, surprise}; parameters [P][nu], times [P] */
-int mjpc_b200_gradient_planner_get_result(void* planner, double* scalars, double* parameters, double* times);
+int mjpc_b200_gradient_planner_get_result(mjpc_b200_planner_t* p, double* scalars, double* parameters, double* times);
 /* SplineMapping::Compute (gradient/spline_mapping.cc) as scalar weights W [num_output][num_input]; host only */
 void mjpc_b200_host_spline_mapping(int representation, const double* input_times, int num_input, const double* output_times,
                                    int num_output, double* W);
@@ -541,16 +534,10 @@ void mjpc_b200_host_spline_mapping(int representation, const double* input_times
 int mjpc_b200_ilqs_planner_create(const mjpc_model_blob* model, int num_trajectory, int num_spline_points, int interpolation,
                                   double exploration, double timestep, const double* ctrlrange, uint32_t seed,
                                   int ilqg_num_rollouts, int ilqg_representation, double fd_tolerance, int max_horizon, int device,
-                                  void** out);
-void mjpc_b200_ilqs_planner_destroy(void* planner);
-void mjpc_b200_ilqs_planner_set_fd(void* planner, double tolerance, int mode, int derivative_skip);       /* its iLQG half */
-void mjpc_b200_ilqs_planner_reset(void* planner, int horizon, const double* initial_repeated_action);
-void mjpc_b200_ilqs_planner_set_state(void* planner, const double* state, double time, const double* mocap);
-void mjpc_b200_ilqs_planner_set_exploration(void* planner, double exploration);
-int mjpc_b200_ilqs_planner_optimize_policy(void* planner, int horizon);
-void mjpc_b200_ilqs_planner_action_from_policy(void* planner, double* action, const double* state, double time, int use_previous);
+                                  mjpc_b200_planner_t** out);
+int mjpc_b200_ilqs_planner_set_exploration(mjpc_b200_planner_t* p, double exploration);   /* its sampling half */
 /* scalars[4] = {active_policy (0 sampling, 1 iLQG), sampling winner return, iLQG total_return, sampling winner}; returns active_policy */
-int mjpc_b200_ilqs_planner_get_result(void* planner, double* scalars);
+int mjpc_b200_ilqs_planner_get_result(mjpc_b200_planner_t* p, double* scalars);
 
 /* ---- Agent::PlanIteration glue (csrc/host/agent.{h,cc}; mjpc/agent.cc:85-107,150-164,283-357): owns the planner selected
  * by agent_planner (0 Sampling, 1 Gradient, 2 iLQG, 3 iLQS, 4 Robust, 5 Cross-Entropy; mjpc/planners/include.h:26-34) and does

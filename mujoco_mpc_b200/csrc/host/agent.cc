@@ -30,14 +30,14 @@ int Agent::Initialize(const mjpc_model_blob* model, const AgentSettings& s, cons
       auto* p = new GradientPlanner;
       planner_.reset(p);
       rc = p->Initialize(model, s.num_trajectory, s.num_spline_points, s.representation, s.timestep, ctrlrange, Hmax, device);
-      if (!rc) { p->settings.fd_tolerance = s.fd_tolerance; p->settings.differentiable = 0; }   // the Agent owns the switch
+      if (!rc) { p->SetFD(s.fd_tolerance, -1, -1); p->settings.differentiable = 0; }   // the Agent owns the switch
       break;
     }
     case kILQGPlanner: {
       auto* p = new iLQGPlanner;
       planner_.reset(p);
       rc = p->Initialize(model, s.ilqg_num_rollouts, s.ilqg_representation, Hmax, device);
-      if (!rc) { p->settings.fd_tolerance = s.fd_tolerance; p->settings.differentiable = 0; }
+      if (!rc) { p->SetFD(s.fd_tolerance, -1, -1); p->settings.differentiable = 0; }
       break;
     }
     case kILQSPlanner: {

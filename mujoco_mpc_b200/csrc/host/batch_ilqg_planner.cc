@@ -257,7 +257,8 @@ int mjpc_b200_batch_ilqg_planner_get_result(void* p, int problem, double* scalar
                                             double* times) {
   BatchILQGPlanner* bp = ilqg_problem_of(p, problem);
   if (!bp) return MJPC_B200_ERR_BAD_ARGUMENT;
-  return mjpc_b200_ilqg_planner_get_result(&bp->problem(problem), scalars, states, actions, times);
+  return mjpc_b200_ilqg_planner_get_result(mjpc_b200_host::ToHandle(&bp->problem(problem)), scalars, states, actions,
+                                           times);
 }
 
 }  // extern "C"

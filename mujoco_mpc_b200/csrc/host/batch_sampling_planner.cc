@@ -154,7 +154,8 @@ int mjpc_b200_batch_planner_get_result(void* p, int problem, int* winner, double
                                        double* knots, double* knot_times) {
   BatchSamplingPlanner* bp = problem_of(p, problem);
   if (!bp) return MJPC_B200_ERR_BAD_ARGUMENT;
-  return mjpc_b200_planner_get_result(&bp->problem(problem), winner, improvement, returns, knots, knot_times);
+  return mjpc_b200_sampling_planner_get_result(mjpc_b200_host::ToHandle(&bp->problem(problem)), winner, improvement,
+                                               returns, knots, knot_times);
 }
 
 }  // extern "C"

@@ -152,36 +152,27 @@ const Trajectory* CrossEntropyPlanner::BestTrajectory() {
 
 // ------------------------------------------------------------------------------------------ C entry points
 using mjpc_b200_host::CrossEntropyPlanner;
+using mjpc_b200_host::PlannerOf;
 
 extern "C" {
 
 int mjpc_b200_ce_planner_create(const mjpc_model_blob* model, int num_trajectory, int n_elite, int num_spline_points,
                                 int interpolation, double std_initial, double std_min, double explore_fraction,
                                 double timestep, const double* ctrlrange, uint32_t seed, int max_horizon, int device,
-                                void** out) {
+                                mjpc_b200_planner_t** out) {
   if (!model || !ctrlrange || !out || num_trajectory < 2 || num_spline_points < 2) return MJPC_B200_ERR_BAD_ARGUMENT;
   auto* p = new CrossEntropyPlanner;
   int rc = p->Initialize(model, num_trajectory, n_elite, num_spline_points, interpolation, std_initial, std_min,
                          explore_fraction, timestep, ctrlrange, seed, max_horizon, device);
   if (rc) { delete p; *out = nullptr; return rc; }
-  *out = p;
+  *out = mjpc_b200_host::ToHandle(p);
   return 0;
 }
-void mjpc_b200_ce_planner_destroy(void* p) { delete (CrossEntropyPlanner*)p; }
-void mjpc_b200_ce_planner_reset(void* p, int horizon, const double* initial_repeated_action) {
-  ((CrossEntropyPlanner*)p)->Reset(horizon, initial_repeated_action);
-}
-void mjpc_b200_ce_planner_set_state(void* p, const double* state, double time, const double* mocap) {
-  ((CrossEntropyPlanner*)p)->SetState(state, time, mocap);
-}
-int mjpc_b200_ce_planner_optimize_policy(void* p, int horizon) { return ((CrossEntropyPlanner*)p)->OptimizePolicy(horizon); }
-void mjpc_b200_ce_planner_action_from_policy(void* p, double* action, double time, int use_previous) {
-  ((CrossEntropyPlanner*)p)->ActionFromPolicy(action, nullptr, time, use_previous != 0);
-}
 // improvement, returns [N+1] (the last one is the nominal), elite order [N], installed policy knots/times, variance
-int mjpc_b200_ce_planner_get_result(void* pv, double* improvement, float* returns, int* order, double* knots,
-                                    double* knot_times, double* variance) {
-  auto* p = (CrossEntropyPlanner*)pv;
+int mjpc_b200_ce_planner_get_result(mjpc_b200_planner_t* h, double* improvement, float* returns, int* order,
+                                    double* knots, double* knot_times, double* variance) {
+  auto* p = PlannerOf<CrossEntropyPlanner>(h);
+  if (!p) return MJPC_B200_ERR_BAD_ARGUMENT;
   if (improvement) *improvement = p->improvement;
   if (returns) std::copy(p->returns().begin(), p->returns().end(), returns);
   if (order) std::copy(p->trajectory_order.begin(), p->trajectory_order.end(), order);

@@ -146,23 +146,40 @@ void Estimator::StateAdd(double* x, const double* dx, double scale) const {
   for (int k = 0; k < m_.nv; k++) x[m_.nq + k] += scale * dx[m_.nv + k];
 }
 
-void EstimatorDestroy(Estimator* f) { delete f; }
+}  // namespace mjpc_b200_host
 
-int EstimatorReset(Estimator* f, const double* state, double time, double covariance_scale, double process_scale,
-                   double sensor_scale) {
+// ------------------------------------------------------------------------------------------------------------ C ABI
+// (the generic estimator family of include/mjpc_b200.h: every kind's handle, a NULL one refused)
+using mjpc_b200_host::Estimator;
+using mjpc_b200_host::EstimatorOf;
+
+extern "C" {
+
+int mjpc_b200_estimator_destroy(mjpc_b200_estimator_t* h) {
+  Estimator* f = EstimatorOf<Estimator>(h);
+  if (!f) return MJPC_B200_ERR_BAD_ARGUMENT;
+  delete f;
+  return 0;
+}
+
+int mjpc_b200_estimator_reset(mjpc_b200_estimator_t* h, const double* state, double time, double covariance_scale,
+                              double process_scale, double sensor_scale) {
+  Estimator* f = EstimatorOf<Estimator>(h);
   if (!f) return MJPC_B200_ERR_BAD_ARGUMENT;
   f->Reset(state, time, covariance_scale, process_scale, sensor_scale);
   return 0;
 }
 
-int EstimatorSetNoise(Estimator* f, const double* process, const double* sensor) {
+int mjpc_b200_estimator_set_noise(mjpc_b200_estimator_t* h, const double* process, const double* sensor) {
+  Estimator* f = EstimatorOf<Estimator>(h);
   if (!f) return MJPC_B200_ERR_BAD_ARGUMENT;
   if (process) f->noise_process.assign(process, process + f->ndstate);
   if (sensor) f->noise_sensor.assign(sensor, sensor + f->nsensordata);
   return 0;
 }
 
-int EstimatorSet(Estimator* f, const double* state, const double* covariance, double time) {
+int mjpc_b200_estimator_set(mjpc_b200_estimator_t* h, const double* state, const double* covariance, double time) {
+  Estimator* f = EstimatorOf<Estimator>(h);
   if (!f) return MJPC_B200_ERR_BAD_ARGUMENT;
   if (state) f->state.assign(state, state + f->state.size());
   if (covariance) f->covariance.assign(covariance, covariance + f->covariance.size());
@@ -170,14 +187,25 @@ int EstimatorSet(Estimator* f, const double* state, const double* covariance, do
   return 0;
 }
 
-int EstimatorGet(const Estimator* f, double* state, double* covariance, double* time) {
+int mjpc_b200_estimator_update(mjpc_b200_estimator_t* h, const double* ctrl, const double* sensor, const float* mocap) {
+  Estimator* f = EstimatorOf<Estimator>(h);
+  return f ? f->Update(ctrl, sensor, mocap) : MJPC_B200_ERR_BAD_ARGUMENT;
+}
+
+int mjpc_b200_estimator_get(const mjpc_b200_estimator_t* h, double* state, double* covariance, double* time,
+                            double* scalars) {
+  const Estimator* f = reinterpret_cast<const Estimator*>(h);
   if (!f) return MJPC_B200_ERR_BAD_ARGUMENT;
   if (state) std::copy(f->state.begin(), f->state.end(), state);
   if (covariance) std::copy(f->covariance.begin(), f->covariance.end(), covariance);
   if (time) *time = f->time;
+  if (scalars) f->GetScalars(scalars);
   return 0;
 }
 
-const char* EstimatorLastError(const Estimator* f) { return f ? f->error.c_str() : ""; }
+const char* mjpc_b200_estimator_last_error(const mjpc_b200_estimator_t* h) {
+  const Estimator* f = reinterpret_cast<const Estimator*>(h);
+  return f ? f->error.c_str() : "";
+}
 
-}  // namespace mjpc_b200_host
+}  // extern "C"

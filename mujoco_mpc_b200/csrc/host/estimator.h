@@ -20,6 +20,8 @@ class Estimator {
                      double sensor_scale);
   // one filter update from ctrl [nu], the measured sensor slice [nsensordata] and mocap [7 nmocap] (NULL: the model's)
   virtual int Update(const double* ctrl, const double* sensor, const float* mocap) = 0;
+  // the filter's scalars of mjpc_b200_estimator_get
+  virtual void GetScalars(double* scalars) const = 0;
 
   std::vector<double> state, covariance, noise_process, noise_sensor;
   double time = 0;
@@ -55,14 +57,10 @@ class Estimator {
   std::vector<int> counts_;
 };
 
-// The bodies of the mjpc_b200_{unscented,kalman}_* entry points every filter shares; a NULL filter returns
-// MJPC_B200_ERR_BAD_ARGUMENT (last_error: "").  Get fills state, covariance and time; each filter fills its scalars.
-void EstimatorDestroy(Estimator* f);
-int EstimatorReset(Estimator* f, const double* state, double time, double covariance_scale, double process_scale,
-                   double sensor_scale);
-int EstimatorSetNoise(Estimator* f, const double* process, const double* sensor);
-int EstimatorSet(Estimator* f, const double* state, const double* covariance, double time);
-int EstimatorGet(const Estimator* f, double* state, double* covariance, double* time);
-const char* EstimatorLastError(const Estimator* f);
+// mjpc_b200_estimator_t* is the Estimator base of the filter, whatever its kind
+inline mjpc_b200_estimator_t* ToHandle(Estimator* f) { return reinterpret_cast<mjpc_b200_estimator_t*>(f); }
+// the filter behind a handle if it is a T, else nullptr (a NULL handle, or one of another kind)
+template <class T>
+T* EstimatorOf(mjpc_b200_estimator_t* h) { return dynamic_cast<T*>(reinterpret_cast<Estimator*>(h)); }
 
 }  // namespace mjpc_b200_host

@@ -221,7 +221,7 @@ int iLQSPlanner::Initialize(const mjpc_model_blob* model, int num_trajectory, in
   if (rc) return rc;
   rc = ilqg.Initialize(model, ilqg_num_rollouts, ilqg_representation, max_horizon, device);
   if (rc) return rc;
-  if (fd_tolerance > 0) ilqg.settings.fd_tolerance = fd_tolerance;
+  ilqg.SetFD(fd_tolerance, -1, -1);
   nu_ = sampling.NumParameters() / std::max(sampling.policy.num_spline_points, 1);
   timestep_ = timestep;
   return 0;
@@ -304,6 +304,7 @@ void iLQSPlanner::ActionFromPolicy(double* action, const double* state, double t
 // ------------------------------------------------------------------------------------------ C entry points
 using mjpc_b200_host::GradientPlanner;
 using mjpc_b200_host::iLQSPlanner;
+using mjpc_b200_host::PlannerOf;
 
 extern "C" {
 
@@ -316,33 +317,19 @@ void mjpc_b200_host_spline_mapping(int representation, const double* input_times
 
 int mjpc_b200_gradient_planner_create(const mjpc_model_blob* model, int num_trajectory, int num_spline_points, int representation,
                                       double fd_tolerance, double timestep, const double* ctrlrange, int max_horizon, int device,
-                                      void** out) {
+                                      mjpc_b200_planner_t** out) {
   if (!model || !ctrlrange || !out || num_trajectory < 1 || num_spline_points < 1 || max_horizon < 2) return MJPC_B200_ERR_BAD_ARGUMENT;
   auto* p = new GradientPlanner;
   int rc = p->Initialize(model, num_trajectory, num_spline_points, representation, timestep, ctrlrange, max_horizon, device);
   if (rc) { delete p; *out = nullptr; return rc; }
-  if (fd_tolerance > 0) p->settings.fd_tolerance = fd_tolerance;
-  *out = p;
+  p->SetFD(fd_tolerance, -1, -1);
+  *out = mjpc_b200_host::ToHandle(p);
   return 0;
 }
-void mjpc_b200_gradient_planner_destroy(void* p) { delete (GradientPlanner*)p; }
-void mjpc_b200_gradient_planner_set_fd(void* p, double tolerance, int mode, int derivative_skip) {
-  auto& s = ((GradientPlanner*)p)->settings;
-  if (tolerance > 0) s.fd_tolerance = tolerance;
-  if (mode >= 0) s.fd_mode = mode ? 1 : 0;
-  if (derivative_skip >= 0) s.derivative_skip = derivative_skip;
-}
-void mjpc_b200_gradient_planner_reset(void* p, int horizon, const double* a) { ((GradientPlanner*)p)->Reset(horizon, a); }
-void mjpc_b200_gradient_planner_set_state(void* p, const double* state, double time, const double* mocap) {
-  ((GradientPlanner*)p)->SetState(state, time, mocap);
-}
-int mjpc_b200_gradient_planner_optimize_policy(void* p, int horizon) { return ((GradientPlanner*)p)->OptimizePolicy(horizon); }
-void mjpc_b200_gradient_planner_action_from_policy(void* p, double* action, double time, int use_previous) {
-  ((GradientPlanner*)p)->ActionFromPolicy(action, nullptr, time, use_previous != 0);
-}
 // scalars[6] = {total_return, winner, action_step, expected, improvement, surprise}; parameters [P][nu], times [P]
-int mjpc_b200_gradient_planner_get_result(void* pv, double* scalars, double* parameters, double* times) {
-  auto* p = (GradientPlanner*)pv;
+int mjpc_b200_gradient_planner_get_result(mjpc_b200_planner_t* h, double* scalars, double* parameters, double* times) {
+  auto* p = PlannerOf<GradientPlanner>(h);
+  if (!p) return MJPC_B200_ERR_BAD_ARGUMENT;
   if (scalars) {
     scalars[0] = p->total_return; scalars[1] = p->winner; scalars[2] = p->action_step; scalars[3] = p->expected;
     scalars[4] = p->improvement; scalars[5] = p->surprise;
@@ -355,34 +342,25 @@ int mjpc_b200_gradient_planner_get_result(void* pv, double* scalars, double* par
 int mjpc_b200_ilqs_planner_create(const mjpc_model_blob* model, int num_trajectory, int num_spline_points, int interpolation,
                                   double exploration, double timestep, const double* ctrlrange, uint32_t seed,
                                   int ilqg_num_rollouts, int ilqg_representation, double fd_tolerance, int max_horizon, int device,
-                                  void** out) {
+                                  mjpc_b200_planner_t** out) {
   if (!model || !ctrlrange || !out || num_trajectory < 1 || ilqg_num_rollouts < 1 || max_horizon < 2) return MJPC_B200_ERR_BAD_ARGUMENT;
   auto* p = new iLQSPlanner;
   int rc = p->Initialize(model, num_trajectory, num_spline_points, interpolation, exploration, timestep, ctrlrange, seed,
                          ilqg_num_rollouts, ilqg_representation, fd_tolerance, max_horizon, device);
   if (rc) { delete p; *out = nullptr; return rc; }
-  *out = p;
+  *out = mjpc_b200_host::ToHandle(p);
   return 0;
 }
-void mjpc_b200_ilqs_planner_destroy(void* p) { delete (iLQSPlanner*)p; }
-void mjpc_b200_ilqs_planner_set_fd(void* p, double tolerance, int mode, int derivative_skip) {
-  auto& s = ((iLQSPlanner*)p)->ilqg.settings;
-  if (tolerance > 0) s.fd_tolerance = tolerance;
-  if (mode >= 0) s.fd_mode = mode ? 1 : 0;
-  if (derivative_skip >= 0) s.derivative_skip = derivative_skip;
-}
-void mjpc_b200_ilqs_planner_reset(void* p, int horizon, const double* a) { ((iLQSPlanner*)p)->Reset(horizon, a); }
-void mjpc_b200_ilqs_planner_set_state(void* p, const double* state, double time, const double* mocap) {
-  ((iLQSPlanner*)p)->SetState(state, time, mocap);
-}
-void mjpc_b200_ilqs_planner_set_exploration(void* p, double exploration) { ((iLQSPlanner*)p)->sampling.SetExploration(exploration, 0.0); }
-int mjpc_b200_ilqs_planner_optimize_policy(void* p, int horizon) { return ((iLQSPlanner*)p)->OptimizePolicy(horizon); }
-void mjpc_b200_ilqs_planner_action_from_policy(void* p, double* action, const double* state, double time, int use_previous) {
-  ((iLQSPlanner*)p)->ActionFromPolicy(action, state, time, use_previous != 0);
+int mjpc_b200_ilqs_planner_set_exploration(mjpc_b200_planner_t* h, double exploration) {
+  auto* p = PlannerOf<iLQSPlanner>(h);
+  if (!p) return MJPC_B200_ERR_BAD_ARGUMENT;
+  p->sampling.SetExploration(exploration, 0.0);
+  return 0;
 }
 // scalars[4] = {active_policy (0 sampling, 1 iLQG), sampling winner return, iLQG total_return, sampling winner}
-int mjpc_b200_ilqs_planner_get_result(void* pv, double* scalars) {
-  auto* p = (iLQSPlanner*)pv;
+int mjpc_b200_ilqs_planner_get_result(mjpc_b200_planner_t* h, double* scalars) {
+  auto* p = PlannerOf<iLQSPlanner>(h);
+  if (!p) return MJPC_B200_ERR_BAD_ARGUMENT;
   if (scalars) {
     scalars[0] = p->active_policy; scalars[1] = p->sampling.returns()[p->sampling.winner]; scalars[2] = p->ilqg.total_return;
     scalars[3] = p->sampling.winner;

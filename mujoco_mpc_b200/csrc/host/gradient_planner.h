@@ -55,6 +55,9 @@ class GradientPlanner : public Planner {
   // the policy does not depend on the state
   void ActionFromPolicy(double* action, const double* state, double time, bool use_previous = false) override;
   const Trajectory* BestTrajectory() override { return winner >= 0 ? &best_ : nullptr; }
+  int SetFD(double tolerance, int mode, int derivative_skip) override {
+    return SetFiniteDifferences(&settings, tolerance, mode, derivative_skip);
+  }
 
   GradientPlannerSettings settings;
   GradientPolicy policy, previous_policy;
@@ -90,6 +93,9 @@ class iLQSPlanner : public Planner {
     return active_policy == kSampling ? sampling.BestTrajectory() : ilqg.BestTrajectory();
   }
   std::vector<mjpc_b200_t*> Handles() override { return {sampling.gpu(), ilqg.gpu()}; }
+  int SetFD(double tolerance, int mode, int derivative_skip) override {   // its iLQG half
+    return ilqg.SetFD(tolerance, mode, derivative_skip);
+  }
   SamplingPlanner sampling;
   iLQGPlanner ilqg;
   int active_policy = kSampling, previous_active_policy = kSampling;

@@ -305,36 +305,19 @@ void iLQGPlanner::ActionFromPolicy(double* action, const double* state, double t
 
 // ------------------------------------------------------------------------------------------ C entry points
 using mjpc_b200_host::iLQGPlanner;
+using mjpc_b200_host::PlannerOf;
 
 extern "C" {
 
 int mjpc_b200_ilqg_planner_create(const mjpc_model_blob* model, int num_rollouts, int representation, double fd_tolerance,
-                                  int max_horizon, int device, void** out) {
+                                  int max_horizon, int device, mjpc_b200_planner_t** out) {
   if (!model || !out || num_rollouts < 1 || max_horizon < 2) return MJPC_B200_ERR_BAD_ARGUMENT;
   auto* p = new iLQGPlanner;
   int rc = p->Initialize(model, num_rollouts, representation, max_horizon, device);
   if (rc) { delete p; *out = nullptr; return rc; }
-  if (fd_tolerance > 0) p->settings.fd_tolerance = fd_tolerance;
-  *out = p;
+  p->SetFD(fd_tolerance, -1, -1);
+  *out = mjpc_b200_host::ToHandle(p);
   return 0;
-}
-void mjpc_b200_ilqg_planner_destroy(void* p) { delete (iLQGPlanner*)p; }
-void mjpc_b200_ilqg_planner_set_fd(void* p, double tolerance, int mode, int derivative_skip) {
-  auto& s = ((iLQGPlanner*)p)->settings;
-  if (tolerance > 0) s.fd_tolerance = tolerance;
-  if (mode >= 0) s.fd_mode = mode ? 1 : 0;
-  if (derivative_skip >= 0) s.derivative_skip = derivative_skip;
-}
-void mjpc_b200_ilqg_planner_reset(void* p, int horizon, const double* initial_repeated_action) {
-  ((iLQGPlanner*)p)->Reset(horizon, initial_repeated_action);
-}
-void mjpc_b200_ilqg_planner_set_state(void* p, const double* state, double time, const double* mocap) {
-  ((iLQGPlanner*)p)->SetState(state, time, mocap);
-}
-int mjpc_b200_ilqg_planner_nominal_trajectory(void* p, int horizon) { return ((iLQGPlanner*)p)->NominalTrajectory(horizon); }
-int mjpc_b200_ilqg_planner_optimize_policy(void* p, int horizon) { return ((iLQGPlanner*)p)->OptimizePolicy(horizon); }
-void mjpc_b200_ilqg_planner_action_from_policy(void* p, double* action, const double* state, double time) {
-  ((iLQGPlanner*)p)->ActionFromPolicy(action, state, time, false);
 }
 // stateless form of iLQGPolicy::Action (host only, no device): u_nom [H][nu], x_nom [H][dim_state], t_nom [H],
 // gains [H][nu][2nv]; state may be NULL (open loop)
@@ -350,8 +333,10 @@ int mjpc_b200_host_ilqg_policy_action(const mjpc_model_blob* model, const float*
 }
 // scalars[6] = {total_return, regularization, improvement, expected, surprise, winner}; nominal states [H][dim_state],
 // actions [H][nu], times [H]; any pointer may be NULL
-int mjpc_b200_ilqg_planner_get_result(void* pv, double* scalars, float* states, float* actions, double* times) {
-  auto* p = (iLQGPlanner*)pv;
+int mjpc_b200_ilqg_planner_get_result(mjpc_b200_planner_t* h, double* scalars, float* states, float* actions,
+                                      double* times) {
+  auto* p = PlannerOf<iLQGPlanner>(h);
+  if (!p) return MJPC_B200_ERR_BAD_ARGUMENT;
   if (scalars) {
     scalars[0] = p->total_return; scalars[1] = p->regularization; scalars[2] = p->improvement;
     scalars[3] = p->expected; scalars[4] = p->surprise; scalars[5] = p->winner;

@@ -54,6 +54,9 @@ class iLQGPlanner : public Planner {
   // ilqg/policy.cc:82-161; there is no previous policy, so use_previous is ignored
   void ActionFromPolicy(double* action, const double* state, double time, bool use_previous = false) override;
   const Trajectory* BestTrajectory() override { return &best_; }
+  int SetFD(double tolerance, int mode, int derivative_skip) override {
+    return SetFiniteDifferences(&settings, tolerance, mode, derivative_skip);
+  }
 
   iLQGSettings settings;
   // the LIVE policy (iLQGPolicy policy): nominal trajectory, feedback gains, open-loop improvement.  Only written

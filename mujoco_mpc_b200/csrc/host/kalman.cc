@@ -125,6 +125,11 @@ int Kalman::Update(const double* ctrl, const double* sensor, const float* mocap)
   return UpdatePrediction();
 }
 
+void Kalman::GetScalars(double* scalars) const {
+  scalars[0] = ndstate; scalars[1] = nstates; scalars[2] = nsensordata; scalars[3] = warnings; scalars[4] = timestep;
+  scalars[5] = epsilon;
+}
+
 }  // namespace mjpc_b200_host
 
 // ------------------------------------------------------------------------------------------------------------ C ABI
@@ -133,7 +138,7 @@ using namespace mjpc_b200_host;
 extern "C" {
 
 int mjpc_b200_kalman_create(const mjpc_model_blob* model, int sensor_start, int nsensor, double timestep,
-                            double epsilon, int centered, int device, mjpc_b200_kalman_t** out) {
+                            double epsilon, int centered, int device, mjpc_b200_estimator_t** out) {
   if (!out) return MJPC_B200_ERR_BAD_ARGUMENT;
   *out = nullptr;
   auto* k = new Kalman;
@@ -141,54 +146,19 @@ int mjpc_b200_kalman_create(const mjpc_model_blob* model, int sensor_start, int 
     delete k;
     return rc;
   }
-  *out = reinterpret_cast<mjpc_b200_kalman_t*>(k);
+  *out = ToHandle(k);
   return 0;
 }
 
-void mjpc_b200_kalman_destroy(mjpc_b200_kalman_t* k) { EstimatorDestroy(reinterpret_cast<Kalman*>(k)); }
-
-int mjpc_b200_kalman_reset(mjpc_b200_kalman_t* k, const double* state, double time, double covariance_scale,
-                           double process_scale, double sensor_scale) {
-  return EstimatorReset(reinterpret_cast<Kalman*>(k), state, time, covariance_scale, process_scale, sensor_scale);
-}
-
-int mjpc_b200_kalman_set_noise(mjpc_b200_kalman_t* k, const double* process, const double* sensor) {
-  return EstimatorSetNoise(reinterpret_cast<Kalman*>(k), process, sensor);
-}
-
-int mjpc_b200_kalman_set(mjpc_b200_kalman_t* k, const double* state, const double* covariance, double time) {
-  return EstimatorSet(reinterpret_cast<Kalman*>(k), state, covariance, time);
-}
-
-int mjpc_b200_kalman_update_measurement(mjpc_b200_kalman_t* k, const double* ctrl, const double* sensor,
+int mjpc_b200_kalman_update_measurement(mjpc_b200_estimator_t* h, const double* ctrl, const double* sensor,
                                         const float* mocap) {
-  if (!k) return MJPC_B200_ERR_BAD_ARGUMENT;
-  return reinterpret_cast<Kalman*>(k)->UpdateMeasurement(ctrl, sensor, mocap);
+  Kalman* k = EstimatorOf<Kalman>(h);
+  return k ? k->UpdateMeasurement(ctrl, sensor, mocap) : MJPC_B200_ERR_BAD_ARGUMENT;
 }
 
-int mjpc_b200_kalman_update_prediction(mjpc_b200_kalman_t* k) {
-  if (!k) return MJPC_B200_ERR_BAD_ARGUMENT;
-  return reinterpret_cast<Kalman*>(k)->UpdatePrediction();
-}
-
-int mjpc_b200_kalman_update(mjpc_b200_kalman_t* k, const double* ctrl, const double* sensor, const float* mocap) {
-  if (!k) return MJPC_B200_ERR_BAD_ARGUMENT;
-  return reinterpret_cast<Kalman*>(k)->Update(ctrl, sensor, mocap);
-}
-
-int mjpc_b200_kalman_get(const mjpc_b200_kalman_t* k, double* state, double* covariance, double* time,
-                         double* scalars) {
-  const Kalman* f = reinterpret_cast<const Kalman*>(k);
-  if (int rc = EstimatorGet(f, state, covariance, time)) return rc;
-  if (scalars) {
-    scalars[0] = f->ndstate; scalars[1] = f->nstates; scalars[2] = f->nsensordata; scalars[3] = f->warnings;
-    scalars[4] = f->timestep; scalars[5] = f->epsilon;
-  }
-  return 0;
-}
-
-const char* mjpc_b200_kalman_last_error(const mjpc_b200_kalman_t* k) {
-  return EstimatorLastError(reinterpret_cast<const Kalman*>(k));
+int mjpc_b200_kalman_update_prediction(mjpc_b200_estimator_t* h) {
+  Kalman* k = EstimatorOf<Kalman>(h);
+  return k ? k->UpdatePrediction() : MJPC_B200_ERR_BAD_ARGUMENT;
 }
 
 }  // extern "C"

@@ -42,6 +42,8 @@ class Kalman : public Estimator {
   int UpdateMeasurement(const double* ctrl, const double* sensor, const float* mocap);   // kalman.cc:188-276
   int UpdatePrediction();                                                                 // kalman.cc:279-323
   int Update(const double* ctrl, const double* sensor, const float* mocap) override;   // UpdateMeasurement, UpdatePrediction
+  // {ndstate, nstates, nsensordata, warnings, timestep, epsilon}
+  void GetScalars(double* scalars) const override;
 
   int nstates = 0;
   double epsilon = 0;

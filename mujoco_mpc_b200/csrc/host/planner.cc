@@ -150,3 +150,50 @@ void CholSolve(const double* L, int n, double* x) {
 }
 
 }  // namespace mjpc_b200_host
+
+// ------------------------------------------------------------------------------------------ C entry points
+// (the generic planner family of include/mjpc_b200.h: every kind's handle, a NULL one refused)
+using mjpc_b200_host::Planner;
+using mjpc_b200_host::PlannerOf;
+
+extern "C" {
+
+int mjpc_b200_planner_destroy(mjpc_b200_planner_t* h) {
+  Planner* p = PlannerOf<Planner>(h);
+  if (!p) return MJPC_B200_ERR_BAD_ARGUMENT;
+  delete p;
+  return 0;
+}
+int mjpc_b200_planner_reset(mjpc_b200_planner_t* h, int horizon, const double* initial_repeated_action) {
+  Planner* p = PlannerOf<Planner>(h);
+  if (!p) return MJPC_B200_ERR_BAD_ARGUMENT;
+  p->Reset(horizon, initial_repeated_action);
+  return 0;
+}
+int mjpc_b200_planner_set_state(mjpc_b200_planner_t* h, const double* state, double time, const double* mocap) {
+  Planner* p = PlannerOf<Planner>(h);
+  if (!p) return MJPC_B200_ERR_BAD_ARGUMENT;
+  p->SetState(state, time, mocap);
+  return 0;
+}
+int mjpc_b200_planner_optimize_policy(mjpc_b200_planner_t* h, int horizon) {
+  Planner* p = PlannerOf<Planner>(h);
+  return p ? p->OptimizePolicy(horizon) : MJPC_B200_ERR_BAD_ARGUMENT;
+}
+int mjpc_b200_planner_nominal_trajectory(mjpc_b200_planner_t* h, int horizon) {
+  Planner* p = PlannerOf<Planner>(h);
+  return p ? p->NominalTrajectory(horizon) : MJPC_B200_ERR_BAD_ARGUMENT;
+}
+int mjpc_b200_planner_action_from_policy(mjpc_b200_planner_t* h, double* action, const double* state, double time,
+                                         int use_previous) {
+  Planner* p = PlannerOf<Planner>(h);
+  if (!p) return MJPC_B200_ERR_BAD_ARGUMENT;
+  p->ActionFromPolicy(action, state, time, use_previous != 0);
+  return 0;
+}
+int mjpc_b200_planner_set_fd(mjpc_b200_planner_t* h, double tolerance, int mode, int derivative_skip) {
+  Planner* p = PlannerOf<Planner>(h);
+  return p ? p->SetFD(tolerance, mode, derivative_skip) : MJPC_B200_ERR_BAD_ARGUMENT;
+}
+
+}  // extern "C"

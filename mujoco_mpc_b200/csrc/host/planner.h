@@ -56,6 +56,9 @@ class Planner {
   virtual int NominalTrajectory(int horizon) = 0;
   virtual void ActionFromPolicy(double* action, const double* state, double time, bool use_previous) = 0;
   virtual const Trajectory* BestTrajectory() = 0;
+  // finite-difference settings of the planners that take derivatives (SetFiniteDifferences); the others:
+  // MJPC_B200_ERR_UNSUPPORTED
+  virtual int SetFD(double tolerance, int mode, int derivative_skip) { return MJPC_B200_ERR_UNSUPPORTED; }
   // every engine handle the planner plans on: Agent applies the planning-model options and the task snapshot to each
   virtual std::vector<mjpc_b200_t*> Handles() { return {gpu_}; }
   mjpc_b200_t* gpu() { return gpu_; }
@@ -79,5 +82,21 @@ class Planner {
   double time_ = 0;
   int horizon_ = 0;                                   // of the last spline launch: the rows a fetch fills
 };
+
+// SetFD for a settings struct with fd_tolerance, fd_mode and derivative_skip: tolerance <= 0, mode < 0 and
+// derivative_skip < 0 keep the current value
+template <class Settings>
+int SetFiniteDifferences(Settings* s, double tolerance, int mode, int derivative_skip) {
+  if (tolerance > 0) s->fd_tolerance = tolerance;
+  if (mode >= 0) s->fd_mode = mode ? 1 : 0;
+  if (derivative_skip >= 0) s->derivative_skip = derivative_skip;
+  return 0;
+}
+
+// mjpc_b200_planner_t* is the Planner base of the planner, whatever its kind
+inline mjpc_b200_planner_t* ToHandle(Planner* p) { return reinterpret_cast<mjpc_b200_planner_t*>(p); }
+// the planner behind a handle if it is a T, else nullptr (a NULL handle, or one of another kind)
+template <class T>
+T* PlannerOf(mjpc_b200_planner_t* h) { return dynamic_cast<T*>(reinterpret_cast<Planner*>(h)); }
 
 }  // namespace mjpc_b200_host

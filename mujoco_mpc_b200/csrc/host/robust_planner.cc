@@ -76,6 +76,7 @@ int RobustPlanner::OptimizePolicy(int horizon) {
 }  // namespace mjpc_b200_host
 
 // ------------------------------------------------------------------------------------------ C entry points
+using mjpc_b200_host::PlannerOf;
 using mjpc_b200_host::RobustPlanner;
 using mjpc_b200_host::SamplingPlanner;
 
@@ -84,7 +85,7 @@ extern "C" {
 int mjpc_b200_robust_planner_create(const mjpc_model_blob* model, int num_trajectory, int num_spline_points,
                                     int interpolation, double exploration, double timestep, const double* ctrlrange,
                                     uint32_t seed, int ncandidates, int nrepetitions, double xfrc_std, double xfrc_rate,
-                                    int max_horizon, int device, void** out) {
+                                    int max_horizon, int device, mjpc_b200_planner_t** out) {
   if (!model || !ctrlrange || !out) return MJPC_B200_ERR_BAD_ARGUMENT;
   const int rep = nrepetitions > 0 ? nrepetitions : 5;
   const int nc = ncandidates != -1 ? ncandidates : num_trajectory / rep;
@@ -96,25 +97,15 @@ int mjpc_b200_robust_planner_create(const mjpc_model_blob* model, int num_trajec
   rc = p->Initialize(std::move(d), model, std::max(nc * rep, 1), max_horizon, device);
   if (rc) { delete p; *out = nullptr; return rc; }
   p->Configure(num_trajectory, ncandidates, nrepetitions, xfrc_std, xfrc_rate, seed);
-  *out = p;
+  *out = mjpc_b200_host::ToHandle(p);
   return 0;
-}
-void mjpc_b200_robust_planner_destroy(void* p) { delete (RobustPlanner*)p; }
-void mjpc_b200_robust_planner_reset(void* p, int horizon, const double* initial_repeated_action) {
-  ((RobustPlanner*)p)->Reset(horizon, initial_repeated_action);
-}
-void mjpc_b200_robust_planner_set_state(void* p, const double* state, double time, const double* mocap) {
-  ((RobustPlanner*)p)->SetState(state, time, mocap);
-}
-int mjpc_b200_robust_planner_optimize_policy(void* p, int horizon) { return ((RobustPlanner*)p)->OptimizePolicy(horizon); }
-void mjpc_b200_robust_planner_action_from_policy(void* p, double* action, double time, int use_previous) {
-  ((RobustPlanner*)p)->ActionFromPolicy(action, nullptr, time, use_previous != 0);
 }
 // winner (candidate index of the clean launch), robust scores [ncandidates] (mean noisy return per top candidate),
 // clean returns [num_trajectory], installed knots / times; returns the number of scores written
-int mjpc_b200_robust_planner_get_result(void* pv, int* winner, double* scores, float* returns, double* knots,
-                                        double* knot_times) {
-  auto* p = (RobustPlanner*)pv;
+int mjpc_b200_robust_planner_get_result(mjpc_b200_planner_t* h, int* winner, double* scores, float* returns,
+                                        double* knots, double* knot_times) {
+  auto* p = PlannerOf<RobustPlanner>(h);
+  if (!p) return MJPC_B200_ERR_BAD_ARGUMENT;
   SamplingPlanner* d = p->delegate();
   if (winner) *winner = d->winner;
   if (scores) std::copy(p->scores().begin(), p->scores().end(), scores);

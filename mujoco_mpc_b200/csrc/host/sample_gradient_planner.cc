@@ -201,41 +201,28 @@ const Trajectory* SampleGradientPlanner::BestTrajectory() {
 }  // namespace mjpc_b200_host
 
 // ------------------------------------------------------------------------------------------ C entry points
+using mjpc_b200_host::PlannerOf;
 using mjpc_b200_host::SampleGradientPlanner;
 
 extern "C" {
 
 int mjpc_b200_sg_planner_create(const mjpc_model_blob* model, int num_trajectory, int num_gradient, int num_spline_points,
                                 int interpolation, double exploration, double gradient_filter, double timestep,
-                                const double* ctrlrange, uint32_t seed, int max_horizon, int device, void** out) {
+                                const double* ctrlrange, uint32_t seed, int max_horizon, int device,
+                                mjpc_b200_planner_t** out) {
   if (!model || !ctrlrange || !out || num_trajectory < 1 || num_spline_points < 2) return MJPC_B200_ERR_BAD_ARGUMENT;
   auto* p = new SampleGradientPlanner;
   int rc = p->Initialize(model, num_trajectory, num_gradient, num_spline_points, interpolation, exploration,
                          gradient_filter, timestep, ctrlrange, seed, max_horizon, device);
   if (rc) { delete p; *out = nullptr; return rc; }
-  *out = p;
+  *out = mjpc_b200_host::ToHandle(p);
   return 0;
 }
-void mjpc_b200_sg_planner_destroy(void* p) { delete (SampleGradientPlanner*)p; }
-void mjpc_b200_sg_planner_reset(void* p, int horizon, const double* initial_repeated_action) {
-  ((SampleGradientPlanner*)p)->Reset(horizon, initial_repeated_action);
-}
-void mjpc_b200_sg_planner_set_state(void* p, const double* state, double time, const double* mocap) {
-  ((SampleGradientPlanner*)p)->SetState(state, time, mocap);
-}
-int mjpc_b200_sg_planner_optimize_policy(void* p, int horizon) {
-  return ((SampleGradientPlanner*)p)->OptimizePolicy(horizon);
-}
-int mjpc_b200_sg_planner_nominal_trajectory(void* p, int horizon) {
-  return ((SampleGradientPlanner*)p)->NominalTrajectory(horizon);
-}
-void mjpc_b200_sg_planner_action_from_policy(void* p, double* action, double time, int use_previous) {
-  ((SampleGradientPlanner*)p)->ActionFromPolicy(action, nullptr, time, use_previous != 0);
-}
-int mjpc_b200_sg_planner_get_result(void* pv, int* winner, int* winner_type, double* improvement, float* returns,
-                                    int* order, double* knots, double* knot_times, double* gradient_knots,
-                                    double* gradient) {
-  auto* p = (SampleGradientPlanner*)pv;
+int mjpc_b200_sg_planner_get_result(mjpc_b200_planner_t* h, int* winner, int* winner_type, double* improvement,
+                                    float* returns, int* order, double* knots, double* knot_times,
+                                    double* gradient_knots, double* gradient) {
+  auto* p = PlannerOf<SampleGradientPlanner>(h);
+  if (!p) return MJPC_B200_ERR_BAD_ARGUMENT;
   const int N = p->num_trajectory(), G = p->num_gradient();
   if (winner) *winner = p->winner;
   if (winner_type) *winner_type = p->winner_type;

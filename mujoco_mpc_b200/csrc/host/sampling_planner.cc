@@ -251,6 +251,7 @@ const Trajectory* SamplingPlanner::BestTrajectory() {
 
 // ------------------------------------------------------------------------------------------ C entry points
 // (declared in include/mjpc_b200.h; what a ctypes / test harness binds)
+using mjpc_b200_host::PlannerOf;
 using mjpc_b200_host::SamplingPlanner;
 
 extern "C" {
@@ -266,35 +267,29 @@ double mjpc_b200_host_philox_normal(uint32_t seed, uint32_t iteration, uint32_t 
   return mjpc_b200_host::PhiloxNormal(seed, iteration, candidate, knot, dof);
 }
 
-int mjpc_b200_planner_create(const mjpc_model_blob* model, int num_trajectory, int num_spline_points, int interpolation,
-                             double exploration, double timestep, const double* ctrlrange, uint32_t seed, int max_horizon,
-                             int device, void** out) {
+int mjpc_b200_sampling_planner_create(const mjpc_model_blob* model, int num_trajectory, int num_spline_points,
+                                      int interpolation, double exploration, double timestep, const double* ctrlrange,
+                                      uint32_t seed, int max_horizon, int device, mjpc_b200_planner_t** out) {
   if (!model || !ctrlrange || !out) return MJPC_B200_ERR_BAD_ARGUMENT;
   auto* p = new SamplingPlanner;
   int rc = p->Initialize(model, num_trajectory, num_spline_points, interpolation, exploration, 0.0, timestep, ctrlrange,
                          seed, num_trajectory, max_horizon, device);
   if (rc) { delete p; *out = nullptr; return rc; }
-  *out = p;
+  *out = mjpc_b200_host::ToHandle(p);
   return 0;
 }
-void mjpc_b200_planner_destroy(void* p) { delete (SamplingPlanner*)p; }
 // noise_exploration[0..1] (sampling/planner.cc:85-88): the second std, when > 0, replaces the first with probability 0.2
-void mjpc_b200_planner_set_exploration(void* p, double exploration, double exploration2) {
-  ((SamplingPlanner*)p)->SetExploration(exploration, exploration2);
-}
-void mjpc_b200_planner_reset(void* p, int horizon, const double* initial_repeated_action) {
-  ((SamplingPlanner*)p)->Reset(horizon, initial_repeated_action);
-}
-void mjpc_b200_planner_set_state(void* p, const double* state, double time, const double* mocap) {
-  ((SamplingPlanner*)p)->SetState(state, time, mocap);
-}
-int mjpc_b200_planner_optimize_policy(void* p, int horizon) { return ((SamplingPlanner*)p)->OptimizePolicy(horizon); }
-void mjpc_b200_planner_action_from_policy(void* p, double* action, double time, int use_previous) {
-  ((SamplingPlanner*)p)->ActionFromPolicy(action, nullptr, time, use_previous != 0);
+int mjpc_b200_sampling_planner_set_exploration(mjpc_b200_planner_t* h, double exploration, double exploration2) {
+  auto* p = PlannerOf<SamplingPlanner>(h);
+  if (!p) return MJPC_B200_ERR_BAD_ARGUMENT;
+  p->SetExploration(exploration, exploration2);
+  return 0;
 }
 // winner index, improvement, returns [num_trajectory], policy knots [P][nu] and times [P] of the installed policy
-int mjpc_b200_planner_get_result(void* pv, int* winner, double* improvement, float* returns, double* knots, double* knot_times) {
-  auto* p = (SamplingPlanner*)pv;
+int mjpc_b200_sampling_planner_get_result(mjpc_b200_planner_t* h, int* winner, double* improvement, float* returns,
+                                          double* knots, double* knot_times) {
+  auto* p = PlannerOf<SamplingPlanner>(h);
+  if (!p) return MJPC_B200_ERR_BAD_ARGUMENT;
   if (winner) *winner = p->winner;
   if (improvement) *improvement = p->improvement;
   if (returns) std::copy(p->returns().begin(), p->returns().end(), returns);

@@ -171,6 +171,10 @@ int Unscented::Update(const double* ctrl, const double* sensor, const float* moc
   return 0;
 }
 
+void Unscented::GetScalars(double* scalars) const {
+  scalars[0] = ndstate; scalars[1] = nsigma; scalars[2] = nsensordata; scalars[3] = warnings; scalars[4] = timestep;
+}
+
 }  // namespace mjpc_b200_host
 
 // ------------------------------------------------------------------------------------------------------------ C ABI
@@ -179,7 +183,7 @@ using namespace mjpc_b200_host;
 extern "C" {
 
 int mjpc_b200_unscented_create(const mjpc_model_blob* model, int sensor_start, int nsensor, double timestep,
-                               double alpha, double beta, int device, mjpc_b200_unscented_t** out) {
+                               double alpha, double beta, int device, mjpc_b200_estimator_t** out) {
   if (!out) return MJPC_B200_ERR_BAD_ARGUMENT;
   *out = nullptr;
   auto* u = new Unscented;
@@ -187,43 +191,8 @@ int mjpc_b200_unscented_create(const mjpc_model_blob* model, int sensor_start, i
     delete u;
     return rc;
   }
-  *out = reinterpret_cast<mjpc_b200_unscented_t*>(u);
+  *out = ToHandle(u);
   return 0;
-}
-
-void mjpc_b200_unscented_destroy(mjpc_b200_unscented_t* u) { EstimatorDestroy(reinterpret_cast<Unscented*>(u)); }
-
-int mjpc_b200_unscented_reset(mjpc_b200_unscented_t* u, const double* state, double time, double covariance_scale,
-                              double process_scale, double sensor_scale) {
-  return EstimatorReset(reinterpret_cast<Unscented*>(u), state, time, covariance_scale, process_scale, sensor_scale);
-}
-
-int mjpc_b200_unscented_set_noise(mjpc_b200_unscented_t* u, const double* process, const double* sensor) {
-  return EstimatorSetNoise(reinterpret_cast<Unscented*>(u), process, sensor);
-}
-
-int mjpc_b200_unscented_set(mjpc_b200_unscented_t* u, const double* state, const double* covariance, double time) {
-  return EstimatorSet(reinterpret_cast<Unscented*>(u), state, covariance, time);
-}
-
-int mjpc_b200_unscented_update(mjpc_b200_unscented_t* u, const double* ctrl, const double* sensor, const float* mocap) {
-  if (!u) return MJPC_B200_ERR_BAD_ARGUMENT;
-  return reinterpret_cast<Unscented*>(u)->Update(ctrl, sensor, mocap);
-}
-
-int mjpc_b200_unscented_get(const mjpc_b200_unscented_t* u, double* state, double* covariance, double* time,
-                            double* scalars) {
-  const Unscented* f = reinterpret_cast<const Unscented*>(u);
-  if (int rc = EstimatorGet(f, state, covariance, time)) return rc;
-  if (scalars) {
-    scalars[0] = f->ndstate; scalars[1] = f->nsigma; scalars[2] = f->nsensordata; scalars[3] = f->warnings;
-    scalars[4] = f->timestep;
-  }
-  return 0;
-}
-
-const char* mjpc_b200_unscented_last_error(const mjpc_b200_unscented_t* u) {
-  return EstimatorLastError(reinterpret_cast<const Unscented*>(u));
 }
 
 }  // extern "C"

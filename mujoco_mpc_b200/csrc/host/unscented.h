@@ -23,6 +23,8 @@ class Unscented : public Estimator {
   int Initialize(const mjpc_model_blob* model, int sensor_start, int nsensor, double timestep, double alpha,
                  double beta, int device);
   int Update(const double* ctrl, const double* sensor, const float* mocap) override;   // unscented.cc:496-574
+  // {ndstate, nsigma, nsensordata, warnings, timestep}
+  void GetScalars(double* scalars) const override;
   void SigmaPoints();                                                           // :293-349 (factor checked by Update)
   int EvaluateSigmaPoints(const double* ctrl, const float* mocap);             // :353-394
   void QuaternionMeans();                                                       // :578-626

@@ -33,42 +33,26 @@ EXPORTS = ["mjpc_b200_version", "mjpc_b200_last_error", "mjpc_b200_create", "mjp
            "mjpc_b200_batch_ilqg_planner_nominal_trajectory", "mjpc_b200_batch_ilqg_planner_optimize_policy",
            "mjpc_b200_batch_ilqg_planner_action_from_policy", "mjpc_b200_batch_ilqg_planner_get_result",
            "mjpc_b200_step_debug", "mjpc_b200_step_debug_contacts", "mjpc_b200_step_batch", "mjpc_b200_step_sensors",
-           "mjpc_b200_unscented_create", "mjpc_b200_unscented_destroy", "mjpc_b200_unscented_reset",
-           "mjpc_b200_unscented_set_noise", "mjpc_b200_unscented_set", "mjpc_b200_unscented_update",
-           "mjpc_b200_unscented_get", "mjpc_b200_unscented_last_error", "mjpc_b200_kalman_create", "mjpc_b200_kalman_destroy",
-           "mjpc_b200_kalman_reset", "mjpc_b200_kalman_set_noise", "mjpc_b200_kalman_set",
-           "mjpc_b200_kalman_update_measurement", "mjpc_b200_kalman_update_prediction", "mjpc_b200_kalman_update",
-           "mjpc_b200_kalman_get", "mjpc_b200_kalman_last_error", "mjpc_b200_comm_unique_id", "mjpc_b200_comm_init",
+           "mjpc_b200_estimator_destroy", "mjpc_b200_estimator_reset", "mjpc_b200_estimator_set_noise",
+           "mjpc_b200_estimator_set", "mjpc_b200_estimator_update", "mjpc_b200_estimator_get",
+           "mjpc_b200_estimator_last_error", "mjpc_b200_unscented_create", "mjpc_b200_kalman_create",
+           "mjpc_b200_kalman_update_measurement", "mjpc_b200_kalman_update_prediction",
+           "mjpc_b200_comm_unique_id", "mjpc_b200_comm_init",
            "mjpc_b200_comm_info", "mjpc_b200_rollout_spline_sharded", "mjpc_b200_fetch_trajectory_sharded",
            "mjpc_b200_fetch_stats", "mjpc_b200_launch_count", "mjpc_b200_last_kernel_ms", "mjpc_b200_last_kernel_static",
            "mjpc_b200_spec_words", "mjpc_b200_upload_spline_inputs",
            "mjpc_b200_launch_resident", "mjpc_b200_sync", "mjpc_b200_read_returns", "mjpc_b200_stream",
            "mjpc_b200_device_returns", "mjpc_b200_host_spline_sample", "mjpc_b200_host_philox_normal",
-           "mjpc_b200_planner_create", "mjpc_b200_planner_destroy", "mjpc_b200_planner_set_exploration", "mjpc_b200_planner_reset",
-           "mjpc_b200_planner_set_state", "mjpc_b200_planner_optimize_policy",
-           "mjpc_b200_planner_action_from_policy", "mjpc_b200_planner_get_result",
-           "mjpc_b200_ce_planner_create", "mjpc_b200_ce_planner_destroy", "mjpc_b200_ce_planner_reset",
-           "mjpc_b200_ce_planner_set_state", "mjpc_b200_ce_planner_optimize_policy",
-           "mjpc_b200_ce_planner_action_from_policy", "mjpc_b200_ce_planner_get_result",
-           "mjpc_b200_sg_planner_create", "mjpc_b200_sg_planner_destroy", "mjpc_b200_sg_planner_reset",
-           "mjpc_b200_sg_planner_set_state", "mjpc_b200_sg_planner_optimize_policy",
-           "mjpc_b200_sg_planner_nominal_trajectory", "mjpc_b200_sg_planner_action_from_policy",
-           "mjpc_b200_sg_planner_get_result",
-           "mjpc_b200_ilqg_planner_create", "mjpc_b200_ilqg_planner_destroy", "mjpc_b200_ilqg_planner_set_fd",
-           "mjpc_b200_gradient_planner_set_fd", "mjpc_b200_ilqs_planner_set_fd", "mjpc_b200_ilqg_planner_reset",
-           "mjpc_b200_ilqg_planner_set_state", "mjpc_b200_ilqg_planner_nominal_trajectory",
-           "mjpc_b200_ilqg_planner_optimize_policy", "mjpc_b200_ilqg_planner_action_from_policy",
-           "mjpc_b200_ilqg_planner_get_result", "mjpc_b200_host_ilqg_policy_action",
-           "mjpc_b200_robust_planner_create", "mjpc_b200_robust_planner_destroy", "mjpc_b200_robust_planner_reset",
-           "mjpc_b200_robust_planner_set_state", "mjpc_b200_robust_planner_optimize_policy",
-           "mjpc_b200_robust_planner_action_from_policy", "mjpc_b200_robust_planner_get_result",
-           "mjpc_b200_gradient_planner_create", "mjpc_b200_gradient_planner_destroy", "mjpc_b200_gradient_planner_reset",
-           "mjpc_b200_gradient_planner_set_state", "mjpc_b200_gradient_planner_optimize_policy",
-           "mjpc_b200_gradient_planner_action_from_policy", "mjpc_b200_gradient_planner_get_result",
-           "mjpc_b200_host_spline_mapping", "mjpc_b200_ilqs_planner_create", "mjpc_b200_ilqs_planner_destroy",
-           "mjpc_b200_ilqs_planner_reset", "mjpc_b200_ilqs_planner_set_state", "mjpc_b200_ilqs_planner_set_exploration",
-           "mjpc_b200_ilqs_planner_optimize_policy", "mjpc_b200_ilqs_planner_action_from_policy",
-           "mjpc_b200_ilqs_planner_get_result",
+           "mjpc_b200_planner_destroy", "mjpc_b200_planner_reset", "mjpc_b200_planner_set_state",
+           "mjpc_b200_planner_optimize_policy", "mjpc_b200_planner_nominal_trajectory",
+           "mjpc_b200_planner_action_from_policy", "mjpc_b200_planner_set_fd",
+           "mjpc_b200_sampling_planner_create", "mjpc_b200_sampling_planner_set_exploration",
+           "mjpc_b200_sampling_planner_get_result", "mjpc_b200_ce_planner_create", "mjpc_b200_ce_planner_get_result",
+           "mjpc_b200_sg_planner_create", "mjpc_b200_sg_planner_get_result", "mjpc_b200_ilqg_planner_create",
+           "mjpc_b200_ilqg_planner_get_result", "mjpc_b200_host_ilqg_policy_action", "mjpc_b200_robust_planner_create",
+           "mjpc_b200_robust_planner_get_result", "mjpc_b200_gradient_planner_create",
+           "mjpc_b200_gradient_planner_get_result", "mjpc_b200_host_spline_mapping", "mjpc_b200_ilqs_planner_create",
+           "mjpc_b200_ilqs_planner_set_exploration", "mjpc_b200_ilqs_planner_get_result",
            "mjpc_b200_set_options", "mjpc_b200_agent_steps", "mjpc_b200_agent_create", "mjpc_b200_agent_destroy",
            "mjpc_b200_agent_reset", "mjpc_b200_agent_set_state", "mjpc_b200_agent_set_task", "mjpc_b200_agent_set_plan_enabled",
            "mjpc_b200_agent_plan_iteration", "mjpc_b200_agent_get_steps", "mjpc_b200_agent_action_from_policy",
@@ -108,34 +92,35 @@ def load_library():
         lib.mjpc_b200_stream.restype = C.c_void_p
         lib.mjpc_b200_device_returns.restype = C.c_void_p
         lib.mjpc_b200_host_philox_normal.restype = C.c_double
-        lib.mjpc_b200_planner_destroy.argtypes = [C.c_void_p]
+        # the generic planner and estimator families: the first argument is the handle
+        for f, args in ((lib.mjpc_b200_planner_destroy, []), (lib.mjpc_b200_planner_reset, [C.c_int, _dp]),
+                        (lib.mjpc_b200_planner_set_state, [_dp, C.c_double, _dp]),
+                        (lib.mjpc_b200_planner_optimize_policy, [C.c_int]),
+                        (lib.mjpc_b200_planner_nominal_trajectory, [C.c_int]),
+                        (lib.mjpc_b200_planner_action_from_policy, [_dp, _dp, C.c_double, C.c_int]),
+                        (lib.mjpc_b200_planner_set_fd, [C.c_double, C.c_int, C.c_int]),
+                        (lib.mjpc_b200_estimator_destroy, []),
+                        (lib.mjpc_b200_estimator_reset, [_dp] + [C.c_double] * 4),
+                        (lib.mjpc_b200_estimator_set_noise, [_dp, _dp]),
+                        (lib.mjpc_b200_estimator_set, [_dp, _dp, C.c_double]),
+                        (lib.mjpc_b200_estimator_update, [_dp, _dp, _fp]), (lib.mjpc_b200_estimator_get, [_dp] * 4),
+                        (lib.mjpc_b200_estimator_last_error, [])):
+            f.argtypes, f.restype = [C.c_void_p] + args, C.c_int
+        lib.mjpc_b200_estimator_last_error.restype = C.c_char_p
         lib.mjpc_b200_batch_planner_destroy.argtypes = [C.c_void_p]
-        lib.mjpc_b200_planner_set_exploration.argtypes = [C.c_void_p, C.c_double, C.c_double]
-        lib.mjpc_b200_ce_planner_destroy.argtypes = [C.c_void_p]
-        lib.mjpc_b200_sg_planner_destroy.argtypes = [C.c_void_p]
-        lib.mjpc_b200_ilqg_planner_destroy.argtypes = [C.c_void_p]
+        lib.mjpc_b200_sampling_planner_set_exploration.argtypes = [C.c_void_p, C.c_double, C.c_double]
         lib.mjpc_b200_batch_ilqg_planner_destroy.argtypes = [C.c_void_p]
         lib.mjpc_b200_batch_ilqg_planner_set_fd.argtypes = [C.c_void_p, C.c_double, C.c_int, C.c_int]
         lib.mjpc_b200_batch_ilqg_planner_set_fd.restype = None
-        for n in ("mjpc_b200_ilqg_planner_set_fd", "mjpc_b200_gradient_planner_set_fd", "mjpc_b200_ilqs_planner_set_fd"):
-            getattr(lib, n).argtypes = [C.c_void_p, C.c_double, C.c_int, C.c_int]
-            getattr(lib, n).restype = None
-        lib.mjpc_b200_robust_planner_destroy.argtypes = [C.c_void_p]
-        lib.mjpc_b200_gradient_planner_destroy.argtypes = [C.c_void_p]
         lib.mjpc_b200_agent_destroy.argtypes = [C.c_void_p]
         lib.mjpc_b200_agent_steps.argtypes = [C.c_double, C.c_double]
         lib.mjpc_b200_set_options.argtypes = [C.c_void_p, C.c_double, C.c_int]
-        lib.mjpc_b200_ilqs_planner_destroy.argtypes = [C.c_void_p]
         lib.mjpc_b200_ilqs_planner_set_exploration.argtypes = [C.c_void_p, C.c_double]
         lib.mjpc_b200_shadow_transition_destroy.argtypes = [C.c_void_p]
         for n in ("mjpc_b200_quadruped_transition_create", "mjpc_b200_track_transition_create", "mjpc_b200_shadow_transition_create"):
             getattr(lib, n).restype = C.c_void_p
         lib.mjpc_b200_quadruped_transition_destroy.argtypes = [C.c_void_p]
         lib.mjpc_b200_track_transition_destroy.argtypes = [C.c_void_p]
-        for n in ("mjpc_b200_unscented", "mjpc_b200_kalman"):
-            getattr(lib, n + "_destroy").argtypes = [C.c_void_p]
-            getattr(lib, n + "_last_error").argtypes = [C.c_void_p]
-            getattr(lib, n + "_last_error").restype = C.c_char_p
         for n in ("mjpc_b200_destroy", "mjpc_b200_fetch_stats", "mjpc_b200_launch_count", "mjpc_b200_last_kernel_ms", "mjpc_b200_stream",
                   "mjpc_b200_device_returns", "mjpc_b200_sync", "mjpc_b200_launch_resident"):
             getattr(lib, n).argtypes = [C.c_void_p]
@@ -163,7 +148,8 @@ def _model_blob(model):
 
 
 class _CppObject:
-    """A C++ host object behind its `<prefix>_*` entry points: created from the model blob, destroyed by close()."""
+    """A C++ host object created from the model blob by `<prefix>_create` and destroyed by close() through
+    `<prefix>_destroy` (the planners and estimators through their family's generic destroy)."""
 
     def _create(self, prefix, model, *args):
         self.lib = load_library()
@@ -183,13 +169,66 @@ class _CppObject:
 
     __del__ = close
 
+
+class _CppPlanner(_CppObject):
+    """A C++ host planner (csrc/host/planner.h): `<prefix>_create` makes it and `<prefix>_get_result` reads result();
+    every other call is one of the generic mjpc_b200_planner_* entry points.  The sampling-based planners'
+    optimize_policy returns result() and raises on any non-zero code; those with _RETURNS_CODE (Gradient, iLQG, iLQS)
+    return the code (1 improved / updated, 0 not) and raise on a negative one."""
+    _RETURNS_CODE = False
+
+    def close(self):
+        if getattr(self, "h", None):
+            self.lib.mjpc_b200_planner_destroy(self.h)
+            self.h = None
+
+    __del__ = close
+
+    def _fail(self, what):
+        raise EngineError(f"{self._prefix}_{what} failed: {self.lib.mjpc_b200_last_error().decode()}")
+
+    def _set_fd(self, tolerance, mode, derivative_skip):
+        if self.lib.mjpc_b200_planner_set_fd(self.h, tolerance, mode, derivative_skip):
+            self._fail("set_fd")
+
     def reset(self, initial_repeated_action=None):
         a = _d(initial_repeated_action)
-        getattr(self.lib, f"{self._prefix}_reset")(self.h, self.horizon, _pd(a))
+        self.lib.mjpc_b200_planner_reset(self.h, self.horizon, _pd(a))
 
     def set_state(self, state, time, mocap):
         s, mc = _d(state), _d(mocap)
-        getattr(self.lib, f"{self._prefix}_set_state")(self.h, _pd(s), C.c_double(time), _pd(mc))
+        self.lib.mjpc_b200_planner_set_state(self.h, _pd(s), time, _pd(mc))
+
+    def optimize_policy(self):
+        rc = self.lib.mjpc_b200_planner_optimize_policy(self.h, self.horizon)
+        if rc < 0 or (rc and not self._RETURNS_CODE):
+            self._fail("optimize_policy")
+        return rc if self._RETURNS_CODE else self.result()
+
+    def nominal_trajectory(self):
+        """NominalTrajectory: what planning does while it is disabled.  The code is returned (iLQG: 1 / 0 / < 0) or,
+        for the sampling-based planners, raises when it is not 0."""
+        rc = self.lib.mjpc_b200_planner_nominal_trajectory(self.h, self.horizon)
+        if self._RETURNS_CODE:
+            return rc
+        if rc:
+            self._fail("nominal_trajectory")
+
+    def _action(self, time, state, use_previous):
+        a, s = np.zeros(self.nu), _d(state)
+        self.lib.mjpc_b200_planner_action_from_policy(self.h, _pd(a), _pd(s), time, int(use_previous))
+        return a
+
+    def action_from_policy(self, time, use_previous=False):
+        return self._action(time, None, use_previous)
+
+
+class _CppFeedbackPlanner(_CppPlanner):
+    """iLQG and iLQS: the policy reads the state (time-varying feedback); the code of optimize_policy is returned."""
+    _RETURNS_CODE = True
+
+    def action_from_policy(self, time, state=None, use_previous=False):
+        return self._action(time, state, use_previous)
 
 
 def host_ilqg_policy_action(model, u_nom, x_nom, t_nom, gains, representation, feedback_scaling, state, time):
@@ -570,7 +609,7 @@ class Engine:
         return int(self.lib.mjpc_b200_last_kernel_static(self.h))
 
 
-class CppSamplingPlanner(_CppObject):
+class CppSamplingPlanner(_CppPlanner):
     """The C++ host planner (csrc/host/sampling_planner.cc) through its C wrappers."""
 
     def __init__(self, model, num_trajectory, horizon, seed=0x5EED, device=0):
@@ -578,29 +617,19 @@ class CppSamplingPlanner(_CppObject):
         self.P = int(num.get("sampling_spline_points", [3])[0])
         self.horizon, self.N, self.nu = int(horizon), int(num_trajectory), m.nu
         cr = _d(np.asarray(m.actuator_ctrlrange, float).reshape(-1))
-        self._create("mjpc_b200_planner", m, self.N, self.P, int(num.get("sampling_representation", [2])[0]),
+        self._create("mjpc_b200_sampling_planner", m, self.N, self.P, int(num.get("sampling_representation", [2])[0]),
                      C.c_double(float(num.get("sampling_exploration", [0.1])[0])), C.c_double(float(m.opt_timestep)),
                      _pd(cr), C.c_uint32(seed), self.horizon, int(device))
 
     def set_exploration(self, exploration, exploration2=0.0):
-        self.lib.mjpc_b200_planner_set_exploration(self.h, C.c_double(exploration), C.c_double(exploration2))
-
-    def optimize_policy(self):
-        rc = self.lib.mjpc_b200_planner_optimize_policy(self.h, self.horizon)
-        if rc != 0:
-            raise EngineError(f"planner_optimize_policy failed: {self.lib.mjpc_b200_last_error().decode()}")
-        return self.result()
+        self.lib.mjpc_b200_sampling_planner_set_exploration(self.h, C.c_double(exploration), C.c_double(exploration2))
 
     def result(self):
         winner, imp = C.c_int(), C.c_double()
         ret = np.zeros(self.N, np.float32); knots = np.zeros((self.P, self.nu)); kt = np.zeros(self.P)
-        self.lib.mjpc_b200_planner_get_result(self.h, C.byref(winner), C.byref(imp), _pf(ret), _pd(knots), _pd(kt))
+        self.lib.mjpc_b200_sampling_planner_get_result(self.h, C.byref(winner), C.byref(imp), _pf(ret), _pd(knots),
+                                                       _pd(kt))
         return dict(winner=winner.value, improvement=imp.value, returns=ret, knots=knots, knot_times=kt)
-
-    def action_from_policy(self, time, use_previous=False):
-        a = np.zeros(self.nu)
-        self.lib.mjpc_b200_planner_action_from_policy(self.h, _pd(a), C.c_double(time), int(use_previous))
-        return a
 
 
 class CppBatchSamplingPlanner(_CppObject):
@@ -654,7 +683,7 @@ class CppBatchSamplingPlanner(_CppObject):
         return a
 
 
-class CppCrossEntropyPlanner(_CppObject):
+class CppCrossEntropyPlanner(_CppPlanner):
     """The C++ Cross-Entropy planner (csrc/host/cross_entropy_planner.cc) through its C wrappers."""
 
     def __init__(self, model, num_trajectory, horizon, n_elite=0, seed=0x5EED, device=0):
@@ -668,12 +697,6 @@ class CppCrossEntropyPlanner(_CppObject):
             C.c_double(float(num.get("explore_fraction", [0.0])[0])), C.c_double(float(m.opt_timestep)), _pd(cr),
             C.c_uint32(seed), self.horizon, int(device))
 
-    def optimize_policy(self):
-        rc = self.lib.mjpc_b200_ce_planner_optimize_policy(self.h, self.horizon)
-        if rc != 0:
-            raise EngineError(f"ce_planner_optimize_policy failed: {self.lib.mjpc_b200_last_error().decode()}")
-        return self.result()
-
     def result(self):
         imp = C.c_double()
         ret = np.zeros(self.N + 1, np.float32); order = np.zeros(self.N, np.int32)
@@ -682,13 +705,8 @@ class CppCrossEntropyPlanner(_CppObject):
                                                  _pd(knots), _pd(kt), _pd(var))
         return dict(improvement=imp.value, returns=ret, order=order, knots=knots, knot_times=kt, variance=var)
 
-    def action_from_policy(self, time, use_previous=False):
-        a = np.zeros(self.nu)
-        self.lib.mjpc_b200_ce_planner_action_from_policy(self.h, _pd(a), C.c_double(time), int(use_previous))
-        return a
 
-
-class CppSampleGradientPlanner(_CppObject):
+class CppSampleGradientPlanner(_CppPlanner):
     """The C++ Sample Gradient planner (csrc/host/sample_gradient_planner.cc) through its C wrappers."""
 
     def __init__(self, model, num_trajectory, horizon, num_gradient=None, gradient_filter=None, seed=0x5EED, device=0):
@@ -704,17 +722,6 @@ class CppSampleGradientPlanner(_CppObject):
             C.c_double(float(num.get("sampling_exploration", [0.1])[0])), C.c_double(f), C.c_double(float(m.opt_timestep)),
             _pd(cr), C.c_uint32(seed), self.horizon, int(device))
 
-    def optimize_policy(self):
-        rc = self.lib.mjpc_b200_sg_planner_optimize_policy(self.h, self.horizon)
-        if rc != 0:
-            raise EngineError(f"sg_planner_optimize_policy failed: {self.lib.mjpc_b200_last_error().decode()}")
-        return self.result()
-
-    def nominal_trajectory(self):
-        rc = self.lib.mjpc_b200_sg_planner_nominal_trajectory(self.h, self.horizon)
-        if rc != 0:
-            raise EngineError(f"sg_planner_nominal_trajectory failed: {self.lib.mjpc_b200_last_error().decode()}")
-
     def result(self):
         winner, wtype, imp = C.c_int(), C.c_int(), C.c_double()
         ret = np.zeros(self.N, np.float32); order = np.zeros(self.N, np.int32)
@@ -726,13 +733,8 @@ class CppSampleGradientPlanner(_CppObject):
         return dict(winner=winner.value, winner_type=wtype.value, improvement=imp.value, returns=ret, order=order,
                     knots=knots[:n], knot_times=kt[:n], gradient_knots=gk, gradient=grad)
 
-    def action_from_policy(self, time, use_previous=False):
-        a = np.zeros(self.nu)
-        self.lib.mjpc_b200_sg_planner_action_from_policy(self.h, _pd(a), C.c_double(time), int(use_previous))
-        return a
 
-
-class CppILQGPlanner(_CppObject):
+class CppILQGPlanner(_CppFeedbackPlanner):
     """The C++ iLQG planner (csrc/host/ilqg_planner.cc) through its C wrappers."""
 
     def __init__(self, model, horizon, num_rollouts=10, representation=1, fd_tolerance=3e-4, device=0, fd_mode=1, derivative_skip=0):
@@ -740,16 +742,7 @@ class CppILQGPlanner(_CppObject):
         self.nu, self.ds = model.nu, model.nq + model.nv
         self._create("mjpc_b200_ilqg_planner", model, int(num_rollouts), int(representation), C.c_double(fd_tolerance),
                      self.H, int(device))
-        self.lib.mjpc_b200_ilqg_planner_set_fd(self.h, C.c_double(fd_tolerance), int(fd_mode), int(derivative_skip))
-
-    def nominal_trajectory(self):
-        return self.lib.mjpc_b200_ilqg_planner_nominal_trajectory(self.h, self.H)
-
-    def optimize_policy(self):
-        rc = self.lib.mjpc_b200_ilqg_planner_optimize_policy(self.h, self.H)
-        if rc < 0:
-            raise EngineError(f"ilqg_planner_optimize_policy failed: {self.lib.mjpc_b200_last_error().decode()}")
-        return rc
+        self._set_fd(fd_tolerance, fd_mode, derivative_skip)
 
     def result(self):
         sc = np.zeros(6); st = np.zeros((self.H, self.ds), np.float32); ac = np.zeros((self.H, self.nu), np.float32)
@@ -757,12 +750,6 @@ class CppILQGPlanner(_CppObject):
         self.lib.mjpc_b200_ilqg_planner_get_result(self.h, _pd(sc), _pf(st), _pf(ac), _pd(tm))
         return dict(total_return=sc[0], regularization=sc[1], improvement=sc[2], expected=sc[3], surprise=sc[4],
                     winner=int(sc[5]), states=st, actions=ac, times=tm)
-
-    def action_from_policy(self, time, state=None):
-        a = np.zeros(self.nu)
-        s = _d(state)
-        self.lib.mjpc_b200_ilqg_planner_action_from_policy(self.h, _pd(a), _pd(s), C.c_double(time))
-        return a
 
 
 class CppBatchILQGPlanner(_CppObject):
@@ -820,7 +807,7 @@ class CppBatchILQGPlanner(_CppObject):
         return a
 
 
-class CppRobustPlanner(_CppObject):
+class CppRobustPlanner(_CppPlanner):
     """The C++ Robust planner (csrc/host/robust_planner.cc) through its C wrappers."""
 
     def __init__(self, model, num_trajectory, horizon, ncandidates=-1, nrepetitions=5, xfrc_std=0.1, xfrc_rate=0.1,
@@ -836,23 +823,12 @@ class CppRobustPlanner(_CppObject):
             C.c_uint32(seed), int(ncandidates), int(nrepetitions), C.c_double(xfrc_std), C.c_double(xfrc_rate),
             self.horizon, int(device))
 
-    def optimize_policy(self):
-        rc = self.lib.mjpc_b200_robust_planner_optimize_policy(self.h, self.horizon)
-        if rc != 0:
-            raise EngineError(f"robust_planner_optimize_policy failed: {self.lib.mjpc_b200_last_error().decode()}")
-        return self.result()
-
     def result(self):
         winner = C.c_int()
         scores = np.zeros(max(self.nc, 1)); ret = np.zeros(self.N, np.float32)
         knots = np.zeros((self.P, self.nu)); kt = np.zeros(self.P)
         n = self.lib.mjpc_b200_robust_planner_get_result(self.h, C.byref(winner), _pd(scores), _pf(ret), _pd(knots), _pd(kt))
         return dict(winner=winner.value, scores=scores[:n], returns=ret, knots=knots, knot_times=kt)
-
-    def action_from_policy(self, time, use_previous=False):
-        a = np.zeros(self.nu)
-        self.lib.mjpc_b200_robust_planner_action_from_policy(self.h, _pd(a), C.c_double(time), int(use_previous))
-        return a
 
 
 def host_spline_mapping(representation, input_times, output_times):
@@ -864,21 +840,16 @@ def host_spline_mapping(representation, input_times, output_times):
     return W
 
 
-class CppGradientPlanner(_CppObject):
+class CppGradientPlanner(_CppPlanner):
     """The C++ GradientPlanner (csrc/host/gradient_planner.cc) through its C wrappers."""
+    _RETURNS_CODE = True
 
     def __init__(self, model, horizon, num_trajectory=8, num_spline_points=5, representation=1, fd_tolerance=3e-4, device=0, fd_mode=1):
         cr = _d(np.asarray(model.actuator_ctrlrange, float).reshape(-1))
         self.horizon, self.P, self.nu = int(horizon), int(num_spline_points), model.nu
         self._create("mjpc_b200_gradient_planner", model, int(num_trajectory), self.P, int(representation),
                      C.c_double(fd_tolerance), C.c_double(float(model.opt_timestep)), _pd(cr), self.horizon, int(device))
-        self.lib.mjpc_b200_gradient_planner_set_fd(self.h, C.c_double(fd_tolerance), int(fd_mode), -1)
-
-    def optimize_policy(self):
-        rc = self.lib.mjpc_b200_gradient_planner_optimize_policy(self.h, self.horizon)
-        if rc < 0:
-            raise EngineError(f"gradient_planner_optimize_policy failed: {self.lib.mjpc_b200_last_error().decode()}")
-        return rc
+        self._set_fd(fd_tolerance, fd_mode, -1)
 
     def result(self):
         sc = np.zeros(6); p = np.zeros((self.P, self.nu)); t = np.zeros(self.P)
@@ -886,13 +857,8 @@ class CppGradientPlanner(_CppObject):
         return dict(total_return=sc[0], winner=int(sc[1]), action_step=sc[2], expected=sc[3], improvement=sc[4],
                     surprise=sc[5], parameters=p, times=t)
 
-    def action_from_policy(self, time, use_previous=False):
-        a = np.zeros(self.nu)
-        self.lib.mjpc_b200_gradient_planner_action_from_policy(self.h, _pd(a), C.c_double(time), int(use_previous))
-        return a
 
-
-class CppILQSPlanner(_CppObject):
+class CppILQSPlanner(_CppFeedbackPlanner):
     """The C++ iLQSPlanner (csrc/host/gradient_planner.cc) through its C wrappers."""
 
     def __init__(self, model, horizon, num_trajectory=8, num_rollouts=6, fd_tolerance=3e-4, seed=0x5EED, device=0, fd_mode=1):
@@ -904,26 +870,15 @@ class CppILQSPlanner(_CppObject):
                      C.c_double(float(num.get("sampling_exploration", [0.1])[0])), C.c_double(float(m.opt_timestep)),
                      _pd(cr), C.c_uint32(seed), int(num_rollouts), int(num.get("ilqg_representation", [1])[0]),
                      C.c_double(fd_tolerance), self.horizon, int(device))
-        self.lib.mjpc_b200_ilqs_planner_set_fd(self.h, C.c_double(fd_tolerance), int(fd_mode), -1)
+        self._set_fd(fd_tolerance, fd_mode, -1)
 
     def set_exploration(self, sigma):
         self.lib.mjpc_b200_ilqs_planner_set_exploration(self.h, C.c_double(sigma))
-
-    def optimize_policy(self):
-        rc = self.lib.mjpc_b200_ilqs_planner_optimize_policy(self.h, self.horizon)
-        if rc < 0:
-            raise EngineError(f"ilqs_planner_optimize_policy failed: {self.lib.mjpc_b200_last_error().decode()}")
-        return rc
 
     def result(self):
         sc = np.zeros(4)
         self.lib.mjpc_b200_ilqs_planner_get_result(self.h, _pd(sc))
         return dict(active_policy=int(sc[0]), sampling_return=sc[1], ilqg_return=sc[2], sampling_winner=int(sc[3]))
-
-    def action_from_policy(self, time, state=None, use_previous=False):
-        a = np.zeros(self.nu); st = _d(state)
-        self.lib.mjpc_b200_ilqs_planner_action_from_policy(self.h, _pd(a), _pd(st), C.c_double(time), int(use_previous))
-        return a
 
 
 class CppAgent(_CppObject):
@@ -958,6 +913,10 @@ class CppAgent(_CppObject):
     def reset(self, initial_repeated_action=None):
         a = _d(initial_repeated_action)
         self.lib.mjpc_b200_agent_reset(self.h, _pd(a))
+
+    def set_state(self, state, time, mocap):
+        s, mc = _d(state), _d(mocap)
+        self.lib.mjpc_b200_agent_set_state(self.h, _pd(s), C.c_double(time), _pd(mc))
 
     def set_task(self, weight=None, parameters=None, task_state=None, risk=None):
         w, p, s = _d(weight), _d(parameters), _d(task_state)

@@ -356,28 +356,37 @@ class Unscented(_Filter):
 
 
 class _CppFilter(_CppObject):
-    """What CppUnscented and CppKalman share: the C++ filter behind its `<prefix>_*` entry points, its reset, noise,
-    set and get, the ctrl / sensor / mocap marshalling and the EstimatorError of a failed factorisation."""
+    """What CppUnscented and CppKalman share: the C++ filter behind the generic mjpc_b200_estimator_* entry points (its
+    reset, noise, set, update and get), the ctrl / sensor / mocap marshalling and the EstimatorError of a failed
+    factorisation."""
+
+    def close(self):
+        if getattr(self, "h", None):
+            self.lib.mjpc_b200_estimator_destroy(self.h)
+            self.h = None
+
+    __del__ = close
 
     def _check(self, rc):
         if rc != 0:
-            msg = getattr(self.lib, f"{self._prefix}_last_error")(self.h).decode()
+            msg = self.lib.mjpc_b200_estimator_last_error(self.h).decode()
             if "factorisation" in msg:
                 raise EstimatorError(msg)
             raise EngineError(f"{self._prefix} error {rc}: {msg}")
 
-    def _call(self, name, *args):
-        self._check(getattr(self.lib, f"{self._prefix}_{name}")(self.h, *args))
-
     def reset(self, state=None, time=0.0, covariance_scale=None, process_scale=None, sensor_scale=None):
         x, cs, ps, ss = reset_values(self.m, state, covariance_scale, process_scale, sensor_scale)
-        self._call("reset", _pd(_d(x)), C.c_double(time), C.c_double(cs), C.c_double(ps), C.c_double(ss))
+        self._check(self.lib.mjpc_b200_estimator_reset(self.h, _pd(_d(x)), time, cs, ps, ss))
 
     def set_noise(self, process=None, sensor=None):
-        self._call("set_noise", _pd(_d(process)), _pd(_d(sensor)))
+        self._check(self.lib.mjpc_b200_estimator_set_noise(self.h, _pd(_d(process)), _pd(_d(sensor))))
 
     def set(self, state, covariance, time):
-        self._call("set", _pd(_d(state)), _pd(_d(covariance)), C.c_double(time))
+        self._check(self.lib.mjpc_b200_estimator_set(self.h, _pd(_d(state)), _pd(_d(covariance)), time))
+
+    def update(self, ctrl, sensor, mocap=None):
+        self._check(self.lib.mjpc_b200_estimator_update(self.h, *self._args(ctrl, sensor, mocap)))
+        return self.state
 
     def _args(self, ctrl, sensor, mocap):
         mc = None if mocap is None or len(mocap) == 0 else np.ascontiguousarray(mocap, np.float32)
@@ -389,7 +398,7 @@ class _CppFilter(_CppObject):
     def _get(self):
         x, P = np.zeros(self.m.nq + self.m.nv), np.zeros((self.ndstate, self.ndstate))
         t, sc = C.c_double(), np.zeros(self._nscalars)
-        self._call("get", _pd(x), _pd(P), C.byref(t), _pd(sc))
+        self._check(self.lib.mjpc_b200_estimator_get(self.h, _pd(x), _pd(P), C.byref(t), _pd(sc)))
         return x, P, t.value, sc
 
     @property
@@ -410,7 +419,7 @@ class _CppFilter(_CppObject):
 
 
 class CppUnscented(_CppFilter):
-    """The C++ filter (csrc/host/unscented.{h,cc}, mjpc_b200_unscented_*) behind the same attributes as Unscented;
+    """The C++ filter (csrc/host/unscented.{h,cc}, mjpc_b200_unscented_create) behind the same attributes as Unscented;
     settings resolve from the model's numerics exactly as Unscented's do."""
     _nscalars = 5
 
@@ -422,10 +431,6 @@ class CppUnscented(_CppFilter):
                      C.c_double(self.alpha), C.c_double(self.beta), int(device))
         self.ndstate, self.nsigma = 2 * m.nv, 4 * m.nv + 1
         self.reset()
-
-    def update(self, ctrl, sensor, mocap=None):
-        self._call("update", *self._args(ctrl, sensor, mocap))
-        return self.state
 
 
 # ------------------------------------------------------------------------------------------------------ Kalman
@@ -507,7 +512,8 @@ class Kalman(_Filter):
 
 class CppKalman(_CppFilter):
     """The C++ filter (csrc/host/kalman.{h,cc}, mjpc_b200_kalman_*) behind the same attributes as Kalman; settings
-    resolve from the model's numerics exactly as Kalman's do."""
+    resolve from the model's numerics exactly as Kalman's do.  update is the generic one: the measurement, then the
+    prediction."""
     _nscalars = 6
 
     def __init__(self, m, sensor_start=None, nsensor=None, timestep=None, epsilon=KALMAN_EPSILON,
@@ -522,13 +528,9 @@ class CppKalman(_CppFilter):
         self.reset()
 
     def update_measurement(self, ctrl, sensor, mocap=None):
-        self._call("update_measurement", *self._args(ctrl, sensor, mocap))
+        self._check(self.lib.mjpc_b200_kalman_update_measurement(self.h, *self._args(ctrl, sensor, mocap)))
         return self.state
 
     def update_prediction(self):
-        self._call("update_prediction")
-        return self.state
-
-    def update(self, ctrl, sensor, mocap=None):
-        self._call("update", *self._args(ctrl, sensor, mocap))
+        self._check(self.lib.mjpc_b200_kalman_update_prediction(self.h))
         return self.state
