@@ -580,6 +580,8 @@ constexpr int kL = 16;  // width of a compact constraint-Jacobian row (dofs of t
 // fully unrolled, predicated loops: straight-line code with no taken branches, which is what a single
 // resident warp per scheduler needs (every loop back-edge is an exposed fetch bubble).
 #define FOR_DIM(j, start, dim) _Pragma("unroll") for (int j = (start); j < 6; j++) if (j < (dim))
+// the rows of one contact: dim <= 6 for an elliptic cone, 2 (condim - 1) <= 10 for a pyramidal one
+#define FOR_ROWS(j, nrow) _Pragma("unroll") for (int j = 0; j < 10; j++) if (j < (nrow))
 #define FOR_KL(l, nd) _Pragma("unroll") for (int l = 0; l < kL; l++) if (l < (nd))
 
 // J row (compact) dot a dof-indexed vector: friction-loss / limit rows touch one dof, contact rows their chain
@@ -1926,8 +1928,8 @@ __device__ __forceinline__ void jt_force(Ctx& c, float* out_or_null) {
     const int a0 = cadr[ci];
     float a = 0.f;
     if (a0 >= 0 && l < cnd[ci]) {
-      const int dim = cdim[ci];
-      FOR_DIM(k, 0, dim) a += J[(a0 + k) * kL + l] * force[a0 + k];
+      const int nrow = cdim[ci];   // the row count (pyramidal: 2 (condim - 1), up to 10)
+      FOR_ROWS(k, nrow) a += J[(a0 + k) * kL + l] * force[a0 + k];
     }
     xf[w] = a;
   }

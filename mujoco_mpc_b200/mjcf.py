@@ -129,6 +129,12 @@ def z2quat(vec):
     return axisangle2quat(axis / s, ang)
 
 
+# <option><flag> switches the device and the oracle implement; every other flag must keep MuJoCo's default (the enable
+# flags below default to "disable"; energy / fwdinv / invdiscrete only add diagnostics, so either value is accepted)
+_FLAGS_HANDLED = ("contact", "eulerdamp", "frictionloss", "limit", "refsafe", "warmstart")
+_FLAGS_ENABLE = ("override", "multiccd", "island", "sensornoise")
+_FLAGS_DIAGNOSTIC = ("energy", "fwdinv", "invdiscrete")
+
 # ----------------------------------------------------------------------------- defaults
 _ACT_TAGS = ("general", "motor", "position", "velocity")
 _DEF_TAGS = ("geom", "joint", "site", "tendon") + _ACT_TAGS
@@ -302,9 +308,12 @@ class Compiler:
             if "integrator" in o.attrib:
                 opt["integrator"] = {"Euler": 0, "RK4": 1, "implicit": 2, "implicitfast": 3}[o.get("integrator")]
             for fl in o.findall("flag"):
-                for k in ("contact", "eulerdamp", "frictionloss", "limit", "refsafe", "warmstart"):
-                    if fl.get(k) == "disable":
-                        opt["disable_" + k] = 1
+                for k, v in fl.attrib.items():
+                    if k in _FLAGS_HANDLED:
+                        opt["disable_" + k] = int(v == "disable")
+                    elif k not in _FLAGS_DIAGNOSTIC and v != ("disable" if k in _FLAGS_ENABLE else "enable"):
+                        raise NotImplementedError(f'<flag {k}="{v}"/> is not supported (only {", ".join(_FLAGS_HANDLED)} '
+                                                  "can be switched)")
         self.opt = opt
 
         # ---- body tree
@@ -502,6 +511,18 @@ class Compiler:
             else:
                 j_limited[j] = 1 if (self.autolimits and "range" in a) else 0
             j_stiff[j] = float(a.get("stiffness", 0)); j_margin[j] = float(a.get("margin", 0))
+            if t in (JNT_FREE, JNT_BALL):
+                # the limit rows (dev_model.h, oracle make_constraint) and the spring (k_smooth_forces, oracle passive)
+                # are implemented for slide and hinge joints only: a quaternion limit or spring would be dropped
+                kind = "ball" if t == JNT_BALL else "free"
+                if j_limited[j]:
+                    raise NotImplementedError(f"joint limits on a {kind} joint ({a.get('name', j)}) are not supported")
+                if j_stiff[j] != 0:
+                    raise NotImplementedError(f"stiffness on a {kind} joint ({a.get('name', j)}) is not supported")
+            if "actuatorfrcrange" in a and a.get("actuatorfrclimited", "auto") != "false":
+                raise NotImplementedError(f"actuatorfrcrange on joint {a.get('name', j)} is not supported")
+            if a.get("actuatorgravcomp", "false") == "true":
+                raise NotImplementedError(f"actuatorgravcomp on joint {a.get('name', j)} is not supported")
             j_solref[j] = _f(a.get("solreflimit"), 2, [0.02, 1])
             j_solimp[j] = _f(a.get("solimplimit"), 5, [0.9, 0.95, 0.001, 0.5, 2])
             ndof = {JNT_FREE: 6, JNT_BALL: 3, JNT_SLIDE: 1, JNT_HINGE: 1}[t]
@@ -561,11 +582,12 @@ class Compiler:
         acts = []
         for sec in self.root.findall("actuator"):
             for ch in sec:
-                if ch.tag in _ACT_TAGS:
-                    a = self.defaults.get(ch.tag, ch.get("class"))
-                    a.update(ch.attrib)
-                    a["_tag"] = ch.tag
-                    acts.append(a)
+                if ch.tag not in _ACT_TAGS:
+                    raise NotImplementedError(f"<{ch.tag}> actuators are not supported (only {', '.join(_ACT_TAGS)})")
+                a = self.defaults.get(ch.tag, ch.get("class"))
+                a.update(ch.attrib)
+                a["_tag"] = ch.tag
+                acts.append(a)
         nu = len(acts)
         m.nu, m.na = nu, 0
         trntype = np.zeros(nu, np.int32)        # 0 joint, 1 fixed tendon (mjTRN_JOINT / mjTRN_TENDON)
@@ -573,14 +595,40 @@ class Compiler:
         biastype = np.zeros(nu, np.int32); ctrllim = np.zeros(nu, np.int32); ctrlrange = np.zeros((nu, 2))
         frclim = np.zeros(nu, np.int32); frcrange = np.zeros((nu, 2))
         for i, a in enumerate(acts):
+            tag = a["_tag"]
+            name = a.get("name", str(i))
+            # what the device and the oracle implement: a scalar gear on a slide / hinge joint or a fixed tendon, a
+            # fixed gain, no activation dynamics, bias none or affine.  Anything else would simulate a different model.
             if "tendon" in a:
                 trntype[i], trnid[i] = 1, m.tendon_names.index(a["tendon"])
-            else:
+            elif "joint" in a:
                 trnid[i] = m.jnt_names.index(a["joint"])
-            gear[i] = _f(a.get("gear"), default=[1])[0]
-            tag = a["_tag"]
+                if m.jnt_type[trnid[i]] not in (JNT_SLIDE, JNT_HINGE):
+                    raise NotImplementedError(f"actuator {name}: actuation of a ball or free joint is not supported")
+            else:
+                raise NotImplementedError(f"actuator {name}: only joint and tendon transmissions are supported")
+            g = _f(a.get("gear"), default=[1])
+            if np.any(g[1:] != 0):
+                raise NotImplementedError(f"actuator {name}: a gear vector (gear=\"{a['gear']}\") is not supported, "
+                                          "only a scalar gear")
+            gear[i] = g[0]
+            if tag == "general":
+                for key, ok in (("gaintype", "fixed"), ("dyntype", "none")):
+                    if a.get(key, ok) != ok:
+                        raise NotImplementedError(f"actuator {name}: {key}=\"{a[key]}\" is not supported (only {ok})")
+                if a.get("biastype", "none") not in ("none", "affine"):
+                    raise NotImplementedError(f"actuator {name}: biastype=\"{a['biastype']}\" is not supported "
+                                              "(only none and affine)")
+            if tag == "position" and float(a.get("timeconst", 0)) > 0:
+                raise NotImplementedError(f"actuator {name}: position timeconst (activation dynamics) is not supported")
+            if tag == "position" and "dampratio" in a:
+                raise NotImplementedError(f"actuator {name}: position dampratio is not supported")
+            if float(a.get("inheritrange", 0)) != 0:
+                raise NotImplementedError(f"actuator {name}: inheritrange is not supported (give ctrlrange explicitly)")
+            if int(a.get("actdim", 0)) != 0 or a.get("actlimited", "false") == "true":
+                raise NotImplementedError(f"actuator {name}: activation state (actdim / actlimited) is not supported")
             gp = _f(a.get("gainprm"), 3, [1, 0, 0]); bp = _f(a.get("biasprm"), 3, [0, 0, 0])
-            bt = {"none": 0, "affine": 1}[a.get("biastype", "none")]
+            bt = 1 if a.get("biastype", "none") == "affine" else 0
             if tag == "motor":
                 gp, bp, bt = np.array([1.0, 0, 0]), np.zeros(3), 0
             elif tag == "position":

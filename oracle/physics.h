@@ -698,7 +698,10 @@ void make_constraint(const Model<T>& m, Data<T>& d) {
   d.efc_J.clear(); d.efc_pos.clear(); d.efc_margin.clear(); d.efc_diagApprox.clear(); d.efc_type.clear();
   d.efc_id.clear(); d.efc_frictionloss.clear();
   std::vector<T> row(nv), jp1(3 * nv), jr1(3 * nv), jp2(3 * nv), jr2(3 * nv);
+  // every row is checked against the constraint buffer (the device's hard limit maxefc): a row that does not fit is
+  // dropped and raises the warning (mjWARN_CNSTRFULL), which fails a rollout
   auto add_row = [&](const T* J, T pos, T margin, T diag, int type, int id, T floss) {
+    if ((int)d.efc_pos.size() >= d.maxefc) { d.warning = true; return; }
     d.efc_J.insert(d.efc_J.end(), J, J + nv);
     d.efc_pos.push_back(pos); d.efc_margin.push_back(margin); d.efc_diagApprox.push_back(diag);
     d.efc_type.push_back(type); d.efc_id.push_back(id); d.efc_frictionloss.push_back(floss);
