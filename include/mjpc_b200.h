@@ -290,6 +290,44 @@ int mjpc_b200_kalman_update_measurement(mjpc_b200_estimator_t* f, const double* 
                                         const float* mocap);
 int mjpc_b200_kalman_update_prediction(mjpc_b200_estimator_t* f);
 
+/* ---- Batched state estimators (csrc/host/batch_estimator.{h,cc}): num_filters independent filters of one kind on ONE
+ * engine handle, each with its own state, covariance, time, noise, warm start, ctrl, sensors and mocap.  kind is the
+ * reference's `estimator` numeric: 1 Kalman (settings {epsilon, centered}), 2 Unscented (settings {alpha, beta}).
+ * Every update runs on the device: the filter arithmetic in fp64 (csrc/estimator_kernels.cuh) around one step launch of
+ * all filters' rows per sigma-point set / Jacobian (Unscented one, Kalman two), the instance mjpc_b200_step_batch runs.
+ * The host uploads ctrl, sensors and mocap once and downloads one status per filter; state and covariance stay on the
+ * device until get.  Filter b computes what the single filter of its kind computes from the same state, covariance,
+ * time, noise and warm start, with the same documented differences from the reference (the fp64 sums are the host's,
+ * in the host's order; sin, cos and atan2 of the quaternion maps may differ in the last bits).
+ *   create     refuses what the single creates refuse: a bad argument or a sensor range outside the model's sensors
+ *              (MJPC_B200_ERR_BAD_ARGUMENT), a bad blob (MJPC_B200_ERR_BAD_BLOB), a sensor the engine does not
+ *              evaluate (MJPC_B200_ERR_UNSUPPORTED); and num_filters x rows per filter above 65536 step rows
+ *              (MJPC_B200_ERR_CAPACITY; rows: Unscented 2 ndstate + 1, Kalman ndstate + 1, or 2 ndstate + 1 centred).
+ *              Every filter starts as reset (NULL state, time 0, scales 1e-4) leaves it.
+ *   reset      filter b as mjpc_b200_estimator_reset, zero warm start and warnings
+ *   set_noise  filter b's process [ndstate] / sensor [nsensordata] noise (NULL keeps one)
+ *   set        filter b's state, covariance [ndstate^2] (NULL keeps one) and time
+ *   update     every filter from ctrl [num_filters][nu], sensor [num_filters][nsensordata] and mocap
+ *              [num_filters][7 nmocap] (NULL: the model's for every filter).  status [num_filters]: 0, or
+ *              MJPC_B200_ERR_BAD_ARGUMENT where a factorisation failed, which leaves that filter's state, covariance,
+ *              time, warm start and warnings untouched; the other filters update normally
+ *   get        filter b's state [nq+nv], covariance, time and the scalars of the single filter of its kind (Unscented
+ *              5, Kalman 6; any pointer may be NULL)
+ * Calls that take a filter index return MJPC_B200_ERR_BAD_ARGUMENT when it is outside [0, num_filters), and every call
+ * returns it for a NULL handle (last_error: ""). */
+int mjpc_b200_batch_estimator_create(const mjpc_model_blob* model, int kind, int num_filters, int sensor_start,
+                                     int nsensor, double timestep, const double* settings, int device, void** out);
+int mjpc_b200_batch_estimator_destroy(void* f);
+int mjpc_b200_batch_estimator_reset(void* f, int filter, const double* state, double time, double covariance_scale,
+                                    double process_scale, double sensor_scale);
+int mjpc_b200_batch_estimator_set_noise(void* f, int filter, const double* process, const double* sensor);
+int mjpc_b200_batch_estimator_set(void* f, int filter, const double* state, const double* covariance, double time);
+int mjpc_b200_batch_estimator_update(void* f, const double* ctrl, const double* sensor, const float* mocap,
+                                     int* status);
+int mjpc_b200_batch_estimator_get(void* f, int filter, double* state, double* covariance, double* time,
+                                  double* scalars);
+const char* mjpc_b200_batch_estimator_last_error(const void* f);
+
 /* Per-candidate execution statistics of the last rollout, stats [N][12] = {SM cycles, Newton iterations, contacts,
  * constraint rows (summed over steps), 8 per-phase cycle counters (zero unless built with -DMJPC_PHASE_TIMING)}. */
 int mjpc_b200_fetch_stats(mjpc_b200_t* h, int64_t* stats);

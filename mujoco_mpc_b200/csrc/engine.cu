@@ -1,6 +1,6 @@
 // engine.cu - host side of libmjpc_b200.so: the C ABI declared in include/mjpc_b200.h.
 // Owns the device buffers, the stream and the pinned staging areas; validates arguments; launches the
-// kernels in rollout_kernels.cuh / ilqg_kernels.cuh.  There is deliberately NO CPU fallback: without a
+// kernels in rollout_kernels.cuh / ilqg_kernels.cuh / estimator_kernels.cuh.  There is deliberately NO CPU fallback: without a
 // usable CUDA device every entry point returns MJPC_B200_ERR_CUDA.
 #include <cuda_runtime.h>
 #include <dlfcn.h>
@@ -15,6 +15,8 @@
 #include <vector>
 
 #include "../../include/mjpc_b200.h"
+#include "estimator_kernels.cuh"
+#include "filter_bank.h"
 #include "ilqg_kernels.cuh"
 #include "rollout_kernels.cuh"
 
@@ -60,6 +62,23 @@ const KernelSet kHumanoidTrackKernels = {(const void*)rollout_kernel_humanoid_tr
                                          (const void*)fd_column_kernel, kRolloutThreads};
 }  // namespace
 
+// The device filter bank of the batched estimators (filter_bank.h): one allocation carved into the filters' fields, the
+// per-update inputs, the rows of the step launch and its outputs, and the filters' scratch; pinned staging for the
+// update's inputs and statuses.
+struct FilterBank {
+  FilterBankArgs a;
+  int s0 = 0, nsens = 0, adr0 = 0, nsd = 0;
+  void* d_mem = nullptr;
+  float *d_rtime = nullptr, *d_task = nullptr, *d_res = nullptr, *d_cost = nullptr;
+  unsigned char* d_in = nullptr;   // sensor [B][ny] doubles, ctrl [B][nu] and mocap [B][7 nmocap] floats
+  unsigned char* h_stage = nullptr;
+  size_t in_bytes = 0;
+  ~FilterBank() {
+    if (d_mem) cudaFree(d_mem);
+    if (h_stage) cudaFreeHost(h_stage);
+  }
+};
+
 struct mjpc_b200 {
   int device = 0;
   cudaStream_t stream = nullptr;
@@ -89,6 +108,7 @@ struct mjpc_b200 {
   int dbg_ncon = -1;
   std::vector<float> dbg_contact;
   IlqgBuffers ilqg;
+  FilterBank* bank = nullptr;   // the batched estimators' filters (filter_bank.h), made by mjpc_b200_bank::Init
   // pinned staging
   float* h_in = nullptr;
   size_t h_in_floats = 0;
@@ -525,6 +545,7 @@ void mjpc_b200_destroy(mjpc_b200_t* h) {
                   h->d_sensors, h->d_step};
   for (void* p : bufs) if (p) cudaFree(p);
   ilqg_free(h->ilqg);
+  delete h->bank;
   if (h->h_in) cudaFreeHost(h->h_in);
   if (h->h_out) cudaFreeHost(h->h_out);
   if (h->h_step) cudaFreeHost(h->h_step);
@@ -1193,3 +1214,167 @@ int mjpc_b200_backward_pass_batched(mjpc_b200_t* h, int B, const float* A, const
 }
 
 }  // extern "C"
+
+// ---- the batched estimators' filter bank (filter_bank.h, kernels in estimator_kernels.cuh)
+namespace mjpc_b200_bank {
+
+int Init(mjpc_b200_t* h, const Desc& d) {
+  if (!h || (d.kind != kFilterKalman && d.kind != kFilterUnscented) || d.num_filters < 1 || d.rows < 1 || d.njnt < 0)
+    return fail(MJPC_B200_ERR_BAD_ARGUMENT, "filter bank: bad argument");
+  const DevModel& M = h->pack.M;
+  const int nsens = (int)h->sensors.size();
+  if (d.sensor_start < 0 || d.nsensor < 1 || d.sensor_start > nsens - d.nsensor)
+    return fail(MJPC_B200_ERR_BAD_ARGUMENT, "filter bank: sensor range outside the model's sensors");
+  for (int i = d.sensor_start; i < d.sensor_start + d.nsensor; i++)
+    if (!h->sensor_why[i].empty())
+      return fail(MJPC_B200_ERR_UNSUPPORTED, "filter bank: sensor " + std::to_string(i) + ": " + h->sensor_why[i]);
+  if ((int64_t)d.num_filters * d.rows > h->maxN) return fail(MJPC_B200_ERR_CAPACITY, "filter bank: rows above max_candidates");
+  CUDA_TRY(cudaSetDevice(h->device));
+  delete h->bank;
+  h->bank = nullptr;
+  FilterBank* k = new FilterBank;
+  FilterBankArgs& a = k->a;
+  std::memset(&a, 0, sizeof(a));
+  a.nq = M.nq; a.nv = M.nv; a.nu = M.nu; a.nmocap = M.nmocap; a.njnt = d.njnt;
+  a.kind = d.kind; a.B = d.num_filters; a.rows = d.rows;
+  a.timestep = d.timestep; a.sigma_step = d.sigma_step; a.weight_mean0 = d.weight_mean0;
+  a.weight_covariance0 = d.weight_covariance0; a.weight_sigma = d.weight_sigma; a.epsilon = d.epsilon;
+  a.centered = d.centered;
+  k->s0 = d.sensor_start; k->nsens = d.nsensor;
+  k->adr0 = h->sensors[d.sensor_start].adr;
+  const DevSensor& last = h->sensors[d.sensor_start + d.nsensor - 1];
+  k->nsd = last.adr - k->adr0 + sensor_dim(last.type);
+  a.ny = k->nsd;
+  const size_t B = a.B, R = (size_t)a.B * a.rows, nq = a.nq, nv = a.nv, nx = nq + nv, ns = 2 * nv, ny = a.ny,
+               nu = a.nu, nm = 7 * (size_t)a.nmocap, nr = std::max(M.num_residual, 1), nts = M.task_state_size;
+  const size_t scratch = filter_scratch_layout(a);
+  // carve one allocation, every piece 256-byte aligned
+  size_t bytes = 0;
+  auto take = [&](size_t n) { const size_t at = bytes; bytes += (n + 255) & ~(size_t)255; return at; };
+  const size_t o_jnt = take(3 * (size_t)d.njnt * 4), o_state = take(B * nx * 8), o_P = take(B * ns * ns * 8),
+               o_time = take(B * 8), o_np = take(B * ns * 8), o_ns = take(B * ny * 8), o_warm = take(B * nv * 4),
+               o_warn = take(B * 4), o_status = take(B * 4);
+  k->in_bytes = B * ny * 8 + B * nu * 4 + B * nm * 4;
+  const size_t o_in = take(k->in_bytes), o_qpos = take(R * nq * 4), o_qvel = take(R * nv * 4),
+               o_rctrl = take(R * nu * 4), o_rwarm = take(R * nv * 4), o_rmocap = take(R * nm * 4),
+               o_rtime = take(R * 4), o_task = take(nts * 4), o_qacc = take(R * nv * 4), o_nq = take(R * nq * 4),
+               o_nv = take(R * nv * 4), o_res = take(R * nr * 4), o_cost = take(R * 4), o_counts = take(4 * R * 4),
+               o_sens = take(R * ny * 4), o_scratch = take(B * scratch * 8);
+  auto fail_k = [&](cudaError_t e) {
+    delete k;
+    return fail(MJPC_B200_ERR_CUDA, std::string("filter bank: ") + cudaGetErrorString(e));
+  };
+  if (cudaError_t e = cudaMalloc(&k->d_mem, bytes)) return fail_k(e);
+  if (cudaError_t e = cudaMemset(k->d_mem, 0, bytes)) return fail_k(e);
+  if (cudaError_t e = cudaMallocHost((void**)&k->h_stage, k->in_bytes + B * 4)) return fail_k(e);
+  unsigned char* base = (unsigned char*)k->d_mem;
+  auto at = [&](size_t o) { return (void*)(base + o); };
+  a.jnt = (const int*)at(o_jnt);
+  a.state = (double*)at(o_state); a.P = (double*)at(o_P); a.time = (double*)at(o_time);
+  a.noise_process = (double*)at(o_np); a.noise_sensor = (double*)at(o_ns); a.warm = (float*)at(o_warm);
+  a.warnings = (int*)at(o_warn); a.status = (int*)at(o_status);
+  k->d_in = (unsigned char*)at(o_in);
+  a.sensor = (const double*)k->d_in; a.ctrl = (const float*)(k->d_in + B * ny * 8);
+  a.mocap = (const float*)(k->d_in + B * ny * 8 + B * nu * 4);
+  a.qpos = (float*)at(o_qpos); a.qvel = (float*)at(o_qvel); a.rctrl = (float*)at(o_rctrl); a.rwarm = (float*)at(o_rwarm);
+  a.rmocap = (float*)at(o_rmocap); k->d_rtime = (float*)at(o_rtime); k->d_task = (float*)at(o_task);
+  a.qacc = (const float*)at(o_qacc); a.next_qpos = (const float*)at(o_nq); a.next_qvel = (const float*)at(o_nv);
+  k->d_res = (float*)at(o_res); k->d_cost = (float*)at(o_cost); a.counts = (const int*)at(o_counts);
+  a.sensordata = (const float*)at(o_sens); a.scratch = (double*)at(o_scratch);
+  // the joints, and the task state at time 0: every row steps at device time 0 (the residual, which reads them, does
+  // not feed the filters)
+  std::vector<int> jnt(3 * (size_t)d.njnt);
+  for (int j = 0; j < d.njnt; j++) {
+    jnt[j] = d.jnt_type[j]; jnt[d.njnt + j] = d.jnt_qposadr[j]; jnt[2 * d.njnt + j] = d.jnt_dofadr[j];
+  }
+  std::vector<float> ts(nts);
+  rebase_task_state(h, nullptr, 0.0, ts.data());
+  if (cudaError_t e = cudaMemcpy((void*)a.jnt, jnt.data(), jnt.size() * 4, cudaMemcpyHostToDevice)) return fail_k(e);
+  if (nts)
+    if (cudaError_t e = cudaMemcpy(k->d_task, ts.data(), nts * 4, cudaMemcpyHostToDevice)) return fail_k(e);
+  h->bank = k;
+  return 0;
+}
+
+int Access(mjpc_b200_t* h, int b, int field, void* data, int write) {
+  if (!h || !h->bank || !data || b < 0 || b >= h->bank->a.B) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "filter bank: bad access");
+  const FilterBankArgs& a = h->bank->a;
+  const size_t nx = a.nq + a.nv, ns = 2 * a.nv;
+  void* p;
+  size_t n;
+  switch (field) {
+    case STATE: p = a.state + b * nx; n = nx * 8; break;
+    case COVARIANCE: p = a.P + b * ns * ns; n = ns * ns * 8; break;
+    case TIME: p = a.time + b; n = 8; break;
+    case NOISE_PROCESS: p = a.noise_process + b * ns; n = ns * 8; break;
+    case NOISE_SENSOR: p = a.noise_sensor + (size_t)b * a.ny; n = (size_t)a.ny * 8; break;
+    case WARMSTART: p = a.warm + b * (size_t)a.nv; n = (size_t)a.nv * 4; break;
+    case WARNINGS: p = a.warnings + b; n = 4; break;
+    default: return fail(MJPC_B200_ERR_BAD_ARGUMENT, "filter bank: bad field");
+  }
+  CUDA_TRY(cudaSetDevice(h->device));
+  CUDA_TRY(cudaStreamSynchronize(h->stream));
+  CUDA_TRY(write ? cudaMemcpy(p, data, n, cudaMemcpyHostToDevice) : cudaMemcpy(data, p, n, cudaMemcpyDeviceToHost));
+  return 0;
+}
+
+// the step launch of every filter's rows, as step_impl launches one (inputs and outputs already on the device)
+static int step_rows(mjpc_b200_t* h, const KernelSet* ks) {
+  FilterBank& k = *h->bank;
+  const FilterBankArgs& a = k.a;
+  StepBatchArgs A;
+  std::memset(&A, 0, sizeof(A));
+  A.M = h->pack.M; A.L = make_layout(h->pack.M, 1); A.pack = h->d_pack;
+  A.qpos = a.qpos; A.qvel = a.qvel; A.ctrl = a.rctrl; A.warmstart = a.rwarm;
+  A.mocap = a.rmocap; A.mocap_stride = 7 * a.nmocap;
+  A.task_state = h->pack.M.task_state_size ? k.d_task : nullptr; A.time = k.d_rtime; A.B = a.B * a.rows;
+  A.qacc = (float*)a.qacc; A.next_qpos = (float*)a.next_qpos; A.next_qvel = (float*)a.next_qvel;
+  A.residual = k.d_res; A.cost = k.d_cost; A.counts = (int*)a.counts;
+  A.sensors = h->d_sensors + k.s0; A.nsensor = k.nsens; A.sensor_adr0 = k.adr0; A.sensor_dim = k.nsd;
+  A.sensordata = (float*)a.sensordata;
+  launch_kernel(ks->step, A.B, 32, h->smem_bytes(1, 1), h->stream, A);
+  h->launches += 1;
+  return 0;
+}
+
+int Update(mjpc_b200_t* h, const float* ctrl, const double* sensor, const float* mocap, int* status) {
+  if (!h || !h->bank || (!ctrl && h->pack.M.nu) || !sensor || (!mocap && h->pack.M.nmocap) || !status)
+    return fail(MJPC_B200_ERR_BAD_ARGUMENT, "filter bank update: bad argument");
+  FilterBank& k = *h->bank;
+  FilterBankArgs a = k.a;
+  const size_t B = a.B, ny = a.ny, nu = a.nu, nm = 7 * (size_t)a.nmocap;
+  CUDA_TRY(cudaSetDevice(h->device));
+  CUDA_TRY(cudaStreamSynchronize(h->stream));   // the staging may still feed an earlier copy
+  std::memcpy(k.h_stage, sensor, B * ny * 8);
+  if (nu) std::memcpy(k.h_stage + B * ny * 8, ctrl, B * nu * 4);
+  if (nm) std::memcpy(k.h_stage + B * ny * 8 + B * nu * 4, mocap, B * nm * 4);
+  CUDA_TRY(cudaMemcpyAsync(k.d_in, k.h_stage, k.in_bytes, cudaMemcpyHostToDevice, h->stream));
+  const KernelSet* ks;
+  const int kind = pick_kernels(h, true, &ks);
+  auto run = [&](const void* fn) {
+    void* args[] = {&a};
+    cudaLaunchKernel(fn, dim3(a.B), dim3(kFilterThreads), args, 0, h->stream);
+    h->launches += 1;
+  };
+  if (a.kind == kFilterUnscented) {
+    a.phase = 0; run((const void*)estimator_rows_kernel);
+    step_rows(h, ks);
+    run((const void*)unscented_update_kernel);
+  } else {
+    a.phase = 1; run((const void*)estimator_rows_kernel);
+    step_rows(h, ks);
+    run((const void*)kalman_measurement_kernel);
+    a.phase = 2; run((const void*)estimator_rows_kernel);
+    step_rows(h, ks);
+    run((const void*)kalman_prediction_kernel);
+  }
+  CUDA_TRY(cudaGetLastError());
+  int* st = (int*)(k.h_stage + k.in_bytes);
+  CUDA_TRY(cudaMemcpyAsync(st, a.status, B * 4, cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(cudaStreamSynchronize(h->stream));
+  for (size_t b = 0; b < B; b++) status[b] = st[b] == kFilterFailed ? MJPC_B200_ERR_BAD_ARGUMENT : st[b];
+  h->last_static = kind ? 1 : 0;
+  return 0;
+}
+
+}  // namespace mjpc_b200_bank

@@ -1,0 +1,37 @@
+// filter_bank.h - the engine side of the batched state estimators (csrc/host/batch_estimator.h): B filters of one kind
+// whose state, covariance, time, noise, warm start and warnings live in device memory of an engine handle, and whose
+// update is the kernels of estimator_kernels.cuh around step_batch launches of all their rows.  Internal to
+// libmjpc_b200.so: engine.cu implements it, batch_estimator.cc calls it.
+#pragma once
+#include "../../include/mjpc_b200.h"
+
+namespace mjpc_b200_bank {
+
+struct Desc {
+  int kind;          // 1 Kalman, 2 Unscented
+  int num_filters;
+  int rows;          // step rows per filter: Unscented nsigma, Kalman nstates
+  int sensor_start, nsensor;
+  double timestep;
+  double sigma_step, weight_mean0, weight_covariance0, weight_sigma;   // Unscented
+  double epsilon;                                                      // Kalman
+  int centered;
+  int njnt;                                                    // the model's joints, for the state arithmetic
+  const int *jnt_type, *jnt_qposadr, *jnt_dofadr;
+};
+
+// one filter's field: STATE [nq+nv], COVARIANCE [ndstate^2], TIME [1], NOISE_PROCESS [ndstate], NOISE_SENSOR
+// [nsensordata] (double); WARMSTART [nv] (float); WARNINGS [1] (int)
+enum Field { STATE, COVARIANCE, TIME, NOISE_PROCESS, NOISE_SENSOR, WARMSTART, WARNINGS };
+
+// The handle's filter bank for d (replacing any earlier one), every field zero.  A sensor range outside the model's
+// sensors: MJPC_B200_ERR_BAD_ARGUMENT; a sensor the engine does not evaluate: MJPC_B200_ERR_UNSUPPORTED;
+// num_filters x rows above the handle's max_candidates: MJPC_B200_ERR_CAPACITY.
+int Init(mjpc_b200_t* h, const Desc& d);
+// copies filter b's field to (write = 0) or from (write = 1) `data`
+int Access(mjpc_b200_t* h, int b, int field, void* data, int write);
+// one update of every filter from ctrl [B][nu], sensor [B][nsensordata] and mocap [B][7 nmocap]; status [B] = 0 or
+// MJPC_B200_ERR_BAD_ARGUMENT for a failed factorisation
+int Update(mjpc_b200_t* h, const float* ctrl, const double* sensor, const float* mocap, int* status);
+
+}  // namespace mjpc_b200_bank

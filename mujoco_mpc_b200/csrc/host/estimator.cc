@@ -7,11 +7,6 @@
 
 namespace mjpc_b200_host {
 
-namespace {
-
-// What the estimators read from the blob besides HostModel: every sensor's dimension, the model's mocap poses
-// [7 nmocap] and the Reset state (the first keyframe, else qpos0 and zero qvel).  0, or MJPC_B200_ERR_BAD_BLOB for a
-// blob without sensor entries.
 int LoadEstimatorBlob(const mjpc_model_blob* model, const HostModel& m, std::vector<int>* dims, int* nmocap,
                       std::vector<float>* mocap0, std::vector<double>* key_state) {
   try {
@@ -40,8 +35,6 @@ int LoadEstimatorBlob(const mjpc_model_blob* model, const HostModel& m, std::vec
   }
   return 0;
 }
-
-}  // namespace
 
 Estimator::~Estimator() { if (engine_) mjpc_b200_destroy(engine_); }
 

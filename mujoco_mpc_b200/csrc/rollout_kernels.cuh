@@ -454,6 +454,8 @@ struct StepBatchArgs {
   // optional (NULL: not evaluated): the measurement sensors sensors[0, nsensor) (k_sensors), sensordata [B][sensor_dim]
   // from address sensor_adr0 on
   const DevSensor* sensors; int nsensor, sensor_adr0, sensor_dim; float* sensordata;
+  // row b's mocap poses start at mocap + b mocap_stride: 0 shares one set, 7 nmocap gives each row its own
+  int mocap_stride;
 };
 
 template <class SP>
@@ -468,7 +470,7 @@ __device__ __forceinline__ void step_batch_body(const StepBatchArgs& A) {
   if (b >= A.B) return;
   load_task<SP>(c, 0, A.task_state, nullptr, nullptr);
   load_state<SP>(c, A.qpos + (size_t)b * nq, A.qvel + (size_t)b * nv, A.ctrl + (size_t)b * nu,
-                 A.warmstart ? A.warmstart + (size_t)b * nv : nullptr, A.mocap);
+                 A.warmstart ? A.warmstart + (size_t)b * nv : nullptr, A.mocap + (size_t)b * A.mocap_stride);
   for (int i = lane; i < 6 * M.nbody; i += 32) DF(xfrc)[i] = 0;
   c.time = A.time[b];
   __syncwarp();

@@ -37,6 +37,9 @@ EXPORTS = ["mjpc_b200_version", "mjpc_b200_last_error", "mjpc_b200_create", "mjp
            "mjpc_b200_estimator_set", "mjpc_b200_estimator_update", "mjpc_b200_estimator_get",
            "mjpc_b200_estimator_last_error", "mjpc_b200_unscented_create", "mjpc_b200_kalman_create",
            "mjpc_b200_kalman_update_measurement", "mjpc_b200_kalman_update_prediction",
+           "mjpc_b200_batch_estimator_create", "mjpc_b200_batch_estimator_destroy", "mjpc_b200_batch_estimator_reset",
+           "mjpc_b200_batch_estimator_set_noise", "mjpc_b200_batch_estimator_set", "mjpc_b200_batch_estimator_update",
+           "mjpc_b200_batch_estimator_get", "mjpc_b200_batch_estimator_last_error",
            "mjpc_b200_comm_unique_id", "mjpc_b200_comm_init",
            "mjpc_b200_comm_info", "mjpc_b200_rollout_spline_sharded", "mjpc_b200_fetch_trajectory_sharded",
            "mjpc_b200_fetch_stats", "mjpc_b200_launch_count", "mjpc_b200_last_kernel_ms", "mjpc_b200_last_kernel_static",

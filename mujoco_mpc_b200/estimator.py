@@ -45,7 +45,7 @@ import ctypes as C
 
 import numpy as np
 
-from .engine import EngineError, _CppObject, _d, _pd, _pf
+from .engine import EngineError, _CppObject, _d, _dp, _fp, _pd, _pf
 from .mjcf import JNT_BALL, JNT_FREE, SENS_MEASURED
 
 
@@ -534,3 +534,91 @@ class CppKalman(_CppFilter):
     def update_prediction(self):
         self._check(self.lib.mjpc_b200_kalman_update_prediction(self.h))
         return self.state
+
+
+# ------------------------------------------------------------------------------------------------------ batched
+class CppBatchEstimator(_CppObject):
+    """num_filters independent filters of one kind on one engine handle, every update on the device
+    (csrc/host/batch_estimator.{h,cc}, mjpc_b200_batch_estimator_*).  kind: "kalman" or "unscented"; settings resolve
+    from the model's numerics exactly as CppKalman's / CppUnscented's do.  Each filter starts as reset() leaves it.
+    update returns the per-filter status (0, or MJPC_B200_ERR_BAD_ARGUMENT = -1 where a factorisation failed and the
+    filter was left as it was); state / covariance / time / warnings take the filter index."""
+    KINDS = {"kalman": 1, "unscented": 2}
+
+    def __init__(self, m, kind, num_filters, sensor_start=None, nsensor=None, timestep=None, alpha=None, beta=None,
+                 epsilon=KALMAN_EPSILON, centered=KALMAN_CENTERED, device=0):
+        if kind not in self.KINDS:
+            raise ValueError("kind must be one of %s" % sorted(self.KINDS))
+        self.kind, self.num_filters = kind, int(num_filters)
+        self.sensor_start, self.nsensor, self.timestep, self.alpha, self.beta = settings(m, sensor_start, nsensor,
+                                                                                         timestep, alpha, beta)
+        self.nsensordata = measured_range(m, self.sensor_start, self.nsensor)
+        self.epsilon, self.centered = float(epsilon), bool(centered)
+        self.ndstate = 2 * m.nv
+        if kind == "unscented":
+            prm, self._nscalars = (self.alpha, self.beta), 5
+            self.rows = 2 * self.ndstate + 1
+        else:
+            prm, self._nscalars = (self.epsilon, float(self.centered)), 6
+            self.rows = (2 if self.centered else 1) * self.ndstate + 1
+        self._settings = np.array(prm, float)
+        self._create("mjpc_b200_batch_estimator", m, self.KINDS[kind], self.num_filters, self.sensor_start,
+                     self.nsensor, C.c_double(self.timestep), _pd(self._settings), int(device))
+        for f, args in ((self.lib.mjpc_b200_batch_estimator_reset, [C.c_int, _dp] + [C.c_double] * 4),
+                        (self.lib.mjpc_b200_batch_estimator_set_noise, [C.c_int, _dp, _dp]),
+                        (self.lib.mjpc_b200_batch_estimator_set, [C.c_int, _dp, _dp, C.c_double]),
+                        (self.lib.mjpc_b200_batch_estimator_update, [_dp, _dp, _fp, C.POINTER(C.c_int)]),
+                        (self.lib.mjpc_b200_batch_estimator_get, [C.c_int] + [_dp] * 4),
+                        (self.lib.mjpc_b200_batch_estimator_destroy, [])):
+            f.argtypes, f.restype = [C.c_void_p] + args, C.c_int
+        self.lib.mjpc_b200_batch_estimator_last_error.argtypes = [C.c_void_p]
+        self.lib.mjpc_b200_batch_estimator_last_error.restype = C.c_char_p
+        for b in range(self.num_filters):
+            self.reset(b)
+
+    def _check(self, rc):
+        if rc != 0:
+            raise EngineError(f"{self._prefix} error {rc}: "
+                              f"{self.lib.mjpc_b200_batch_estimator_last_error(self.h).decode()}")
+
+    def reset(self, b, state=None, time=0.0, covariance_scale=None, process_scale=None, sensor_scale=None):
+        x, cs, ps, ss = reset_values(self.m, state, covariance_scale, process_scale, sensor_scale)
+        self._check(self.lib.mjpc_b200_batch_estimator_reset(self.h, b, _pd(_d(x)), time, cs, ps, ss))
+
+    def set_noise(self, b, process=None, sensor=None):
+        self._check(self.lib.mjpc_b200_batch_estimator_set_noise(self.h, b, _pd(_d(process)), _pd(_d(sensor))))
+
+    def set(self, b, state, covariance, time):
+        self._check(self.lib.mjpc_b200_batch_estimator_set(self.h, b, _pd(_d(state)), _pd(_d(covariance)), time))
+
+    def update(self, ctrl, sensor, mocap=None):
+        """One update of every filter from ctrl [B][nu], sensor [B][nsensordata] and mocap [B][7 nmocap] (None: the
+        model's); returns status [B]."""
+        B = self.num_filters
+        u = np.ascontiguousarray(np.asarray(ctrl, float).reshape(B, self.m.nu))
+        y = np.ascontiguousarray(np.asarray(sensor, float).reshape(B, self.nsensordata))
+        mc = None if mocap is None or np.size(mocap) == 0 else \
+            np.ascontiguousarray(np.asarray(mocap, np.float32).reshape(B, -1))
+        status = np.zeros(B, np.int32)
+        self._check(self.lib.mjpc_b200_batch_estimator_update(self.h, _pd(u), _pd(y), _pf(mc),
+                                                              status.ctypes.data_as(C.POINTER(C.c_int))))
+        return status
+
+    def get(self, b):
+        """(state, covariance, time, scalars) of filter b."""
+        x, P = np.zeros(self.m.nq + self.m.nv), np.zeros((self.ndstate, self.ndstate))
+        t, sc = C.c_double(), np.zeros(self._nscalars)
+        self._check(self.lib.mjpc_b200_batch_estimator_get(self.h, b, _pd(x), _pd(P), C.byref(t), _pd(sc)))
+        return x, P, t.value, sc
+
+    def state(self, b):
+        return self.get(b)[0]
+
+    def covariance(self, b):
+        return self.get(b)[1]
+
+    def time(self, b):
+        return self.get(b)[2]
+
+    def warnings(self, b):
+        return int(self.get(b)[3][3])
