@@ -240,13 +240,13 @@ int mjpc_b200_step_sensors(mjpc_b200_t* h, int B, const float* states, const flo
                            const float* mocap, double time, int sensor_start, int nsensor, float* next_states,
                            float* sensordata, float* qacc, int* counts);
 
-/* ---- State estimators (csrc/host/estimator.h, the reference's Estimator base mjpc/estimators/estimator.h): the filter
- * in double on the host, its steps as mjpc_b200_step_sensors launches on an engine handle it owns (max_candidates =
- * 2 ndstate + 1).  Each kind has its own create (its settings); every other call is one of the generic
+/* ---- State estimators (csrc/host/estimator.h, the reference's Estimator base mjpc/estimators/estimator.h): a single
+ * filter is the batched estimators' bank of one filter below, on an engine handle it owns, with the same device
+ * arithmetic.  Each kind has its own create (its settings); every other call is one of the generic
  * mjpc_b200_estimator_* below, which take a filter of any kind and return MJPC_B200_ERR_BAD_ARGUMENT for a NULL one
- * (last_error: "").  create measures the sensors [sensor_start, sensor_start + nsensor) of the blob; it steps the reset
- * state once, so a range outside the model's sensors returns MJPC_B200_ERR_BAD_ARGUMENT and a sensor the engine does
- * not evaluate MJPC_B200_ERR_UNSUPPORTED.  Settings are explicit (timestep = estimator_timestep or opt.timestep, noise
+ * (last_error: "").  create measures the sensors [sensor_start, sensor_start + nsensor) of the blob; a range outside
+ * the model's sensors returns MJPC_B200_ERR_BAD_ARGUMENT and a sensor the engine does not evaluate
+ * MJPC_B200_ERR_UNSUPPORTED.  Settings are explicit (timestep = estimator_timestep or opt.timestep, noise
  * scales 1e-4 by default).
  *   reset      state NULL -> the model's first keyframe, else qpos0 and zero qvel; covariance = covariance_scale I,
  *              diagonal process / sensor noise
@@ -267,20 +267,20 @@ int mjpc_b200_estimator_get(const mjpc_b200_estimator_t* f, double* state, doubl
                             double* scalars);
 const char* mjpc_b200_estimator_last_error(const mjpc_b200_estimator_t* f);
 
-/* MJPC's Unscented state estimator (mjpc/estimators/unscented.cc, class mjpc_b200_host::Unscented in
- * csrc/host/unscented.h): its 2 ndstate + 1 sigma-point steps are one launch (alpha 1, beta 2 by default).  update can
+/* MJPC's Unscented state estimator (mjpc/estimators/unscented.cc, kind 2 of class mjpc_b200_host::Estimator in
+ * csrc/host/estimator.h): its 2 ndstate + 1 sigma-point steps are one launch (alpha 1, beta 2 by default).  update can
  * fail on the covariance or the sensor-covariance factor.  get: scalars[5] = {ndstate, nsigma, nsensordata, sigma-point
  * steps that raised a warning since reset, timestep}. */
 int mjpc_b200_unscented_create(const mjpc_model_blob* model, int sensor_start, int nsensor, double timestep,
                                double alpha, double beta, int device, mjpc_b200_estimator_t** out);
 
-/* MJPC's Kalman state estimator (mjpc/estimators/kalman.cc, class mjpc_b200_host::Kalman in csrc/host/kalman.h): its
+/* MJPC's Kalman state estimator (mjpc/estimators/kalman.cc, kind 1 of class mjpc_b200_host::Estimator): its
  * finite-difference Jacobians are one launch each (the centre state and its ndstate tangent-space perturbations
  * x (+) eps e_i, then x (+) -eps e_i when centered).  The reference's finite differences are 1e-6 one-sided, an fp64
  * setting: mujoco_mpc_b200.estimator.KALMAN_EPSILON / KALMAN_CENTERED are the engine's.  update_measurement (the same
  * arguments as update): C and the predicted sensors from one launch at the current state, then the gain, correction and
  * covariance update; it can fail on the sensor-covariance factor.  update_prediction: A and the next state from one
- * launch with the ctrl and mocap of the last measurement (zeros and the model's mocap after reset),
+ * launch with the ctrl and mocap of the last successful measurement (zeros and the model's mocap after reset),
  * P = A P A' + diag(process noise), time += timestep.  update: both.  Both return MJPC_B200_ERR_BAD_ARGUMENT for a
  * filter that is not a Kalman filter.  get: scalars[6] = {ndstate, states per launch, nsensordata, steps that raised a warning
  * since reset, timestep, epsilon}. */
@@ -290,15 +290,15 @@ int mjpc_b200_kalman_update_measurement(mjpc_b200_estimator_t* f, const double* 
                                         const float* mocap);
 int mjpc_b200_kalman_update_prediction(mjpc_b200_estimator_t* f);
 
-/* ---- Batched state estimators (csrc/host/batch_estimator.{h,cc}): num_filters independent filters of one kind on ONE
+/* ---- Batched state estimators (csrc/host/estimator.{h,cc}): num_filters independent filters of one kind on ONE
  * engine handle, each with its own state, covariance, time, noise, warm start, ctrl, sensors and mocap.  kind is the
  * reference's `estimator` numeric: 1 Kalman (settings {epsilon, centered}), 2 Unscented (settings {alpha, beta}).
  * Every update runs on the device: the filter arithmetic in fp64 (csrc/estimator_kernels.cuh) around one step launch of
  * all filters' rows per sigma-point set / Jacobian (Unscented one, Kalman two), the instance mjpc_b200_step_batch runs.
  * The host uploads ctrl, sensors and mocap once and downloads one status per filter; state and covariance stay on the
  * device until get.  Filter b computes what the single filter of its kind computes from the same state, covariance,
- * time, noise and warm start, with the same documented differences from the reference (the fp64 sums are the host's,
- * in the host's order; sin, cos and atan2 of the quaternion maps may differ in the last bits).
+ * time, noise and warm start (bitwise: the single filter is the same code), with the same documented differences from
+ * the reference.
  *   create     refuses what the single creates refuse: a bad argument or a sensor range outside the model's sensors
  *              (MJPC_B200_ERR_BAD_ARGUMENT), a bad blob (MJPC_B200_ERR_BAD_BLOB), a sensor the engine does not
  *              evaluate (MJPC_B200_ERR_UNSUPPORTED); and num_filters x rows per filter above 65536 step rows

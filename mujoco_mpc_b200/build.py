@@ -41,10 +41,7 @@ def _compile(verbose):
                                                                            os.path.join(CSRC, "host", "gradient_planner.cc"),
                                                                            os.path.join(CSRC, "host", "agent.cc"),
                                                                            os.path.join(CSRC, "host", "task_transition.cc"),
-                                                                           os.path.join(CSRC, "host", "estimator.cc"),
-                                                                           os.path.join(CSRC, "host", "unscented.cc"),
-                                                                           os.path.join(CSRC, "host", "kalman.cc"),
-                                                                           os.path.join(CSRC, "host", "batch_estimator.cc")]
+                                                                           os.path.join(CSRC, "host", "estimator.cc")]
     subprocess.check_call(cmd, cwd=CSRC)
 
 

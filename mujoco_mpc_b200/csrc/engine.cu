@@ -62,7 +62,7 @@ const KernelSet kHumanoidTrackKernels = {(const void*)rollout_kernel_humanoid_tr
                                          (const void*)fd_column_kernel, kRolloutThreads};
 }  // namespace
 
-// The device filter bank of the batched estimators (filter_bank.h): one allocation carved into the filters' fields, the
+// The device filter bank of the state estimators (filter_bank.h): one allocation carved into the filters' fields, the
 // per-update inputs, the rows of the step launch and its outputs, and the filters' scratch; pinned staging for the
 // update's inputs and statuses.
 struct FilterBank {
@@ -108,7 +108,7 @@ struct mjpc_b200 {
   int dbg_ncon = -1;
   std::vector<float> dbg_contact;
   IlqgBuffers ilqg;
-  FilterBank* bank = nullptr;   // the batched estimators' filters (filter_bank.h), made by mjpc_b200_bank::Init
+  FilterBank* bank = nullptr;   // the state estimators' filters (filter_bank.h), made by mjpc_b200_bank::Init
   // pinned staging
   float* h_in = nullptr;
   size_t h_in_floats = 0;
@@ -1215,7 +1215,7 @@ int mjpc_b200_backward_pass_batched(mjpc_b200_t* h, int B, const float* A, const
 
 }  // extern "C"
 
-// ---- the batched estimators' filter bank (filter_bank.h, kernels in estimator_kernels.cuh)
+// ---- the state estimators' filter bank (filter_bank.h, kernels in estimator_kernels.cuh)
 namespace mjpc_b200_bank {
 
 int Init(mjpc_b200_t* h, const Desc& d) {
@@ -1337,15 +1337,17 @@ static int step_rows(mjpc_b200_t* h, const KernelSet* ks) {
   return 0;
 }
 
-int Update(mjpc_b200_t* h, const float* ctrl, const double* sensor, const float* mocap, int* status) {
-  if (!h || !h->bank || (!ctrl && h->pack.M.nu) || !sensor || (!mocap && h->pack.M.nmocap) || !status)
+int Update(mjpc_b200_t* h, const float* ctrl, const double* sensor, const float* mocap, int phases, int* status) {
+  if (!h || !h->bank || phases < MEASUREMENT || phases > MEASUREMENT_AND_PREDICTION || (!ctrl && h->pack.M.nu) ||
+      (!sensor && (h->bank->a.kind == kFilterUnscented || (phases & MEASUREMENT))) || (!mocap && h->pack.M.nmocap) ||
+      !status)
     return fail(MJPC_B200_ERR_BAD_ARGUMENT, "filter bank update: bad argument");
   FilterBank& k = *h->bank;
   FilterBankArgs a = k.a;
   const size_t B = a.B, ny = a.ny, nu = a.nu, nm = 7 * (size_t)a.nmocap;
   CUDA_TRY(cudaSetDevice(h->device));
   CUDA_TRY(cudaStreamSynchronize(h->stream));   // the staging may still feed an earlier copy
-  std::memcpy(k.h_stage, sensor, B * ny * 8);
+  if (sensor) std::memcpy(k.h_stage, sensor, B * ny * 8);
   if (nu) std::memcpy(k.h_stage + B * ny * 8, ctrl, B * nu * 4);
   if (nm) std::memcpy(k.h_stage + B * ny * 8 + B * nu * 4, mocap, B * nm * 4);
   CUDA_TRY(cudaMemcpyAsync(k.d_in, k.h_stage, k.in_bytes, cudaMemcpyHostToDevice, h->stream));
@@ -1361,18 +1363,24 @@ int Update(mjpc_b200_t* h, const float* ctrl, const double* sensor, const float*
     step_rows(h, ks);
     run((const void*)unscented_update_kernel);
   } else {
-    a.phase = 1; run((const void*)estimator_rows_kernel);
-    step_rows(h, ks);
-    run((const void*)kalman_measurement_kernel);
-    a.phase = 2; run((const void*)estimator_rows_kernel);
-    step_rows(h, ks);
-    run((const void*)kalman_prediction_kernel);
+    if (phases & MEASUREMENT) {
+      a.phase = 1; run((const void*)estimator_rows_kernel);
+      step_rows(h, ks);
+      run((const void*)kalman_measurement_kernel);
+    } else {   // the prediction skips a failed filter: clear the statuses an earlier update left
+      CUDA_TRY(cudaMemsetAsync(a.status, 0, B * 4, h->stream));
+    }
+    if (phases & PREDICTION) {
+      a.phase = 2; run((const void*)estimator_rows_kernel);
+      step_rows(h, ks);
+      run((const void*)kalman_prediction_kernel);
+    }
   }
   CUDA_TRY(cudaGetLastError());
   int* st = (int*)(k.h_stage + k.in_bytes);
   CUDA_TRY(cudaMemcpyAsync(st, a.status, B * 4, cudaMemcpyDeviceToHost, h->stream));
   CUDA_TRY(cudaStreamSynchronize(h->stream));
-  for (size_t b = 0; b < B; b++) status[b] = st[b] == kFilterFailed ? MJPC_B200_ERR_BAD_ARGUMENT : st[b];
+  std::copy(st, st + B, status);
   h->last_static = kind ? 1 : 0;
   return 0;
 }

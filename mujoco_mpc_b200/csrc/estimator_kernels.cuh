@@ -1,10 +1,10 @@
-// estimator_kernels.cuh - the batched Kalman and Unscented filters (csrc/host/batch_estimator.h) on the device: B
-// filters of one kind, one CTA per filter, in fp64.  The kernels restate the host filters (csrc/host/unscented.cc,
-// kalman.cc, estimator.cc, planner.cc) operation for operation: each output is summed in the host's order, and every
-// product that feeds a sum is rounded on its own (__dmul_rn / __dadd_rn: the build's -use_fast_math contracts plain
-// a * b + c into an FMA), so the arithmetic matches the host's except for the last bits of sin, cos and atan2 in the
-// quaternion maps.  Rows of the step launch: filter b owns rows [b rows, (b + 1) rows), laid out as the single
-// filter's launch (Unscented: the 2 ndstate sigma points, nominal last; Kalman: the centre, then the perturbations).
+// estimator_kernels.cuh - the Kalman and Unscented filters (csrc/host/estimator.h) on the device: B filters of one
+// kind, one CTA per filter, in fp64.  The kernels restate the reference's filters (mjpc/estimators/unscented.cc,
+// kalman.cc) as the Python mirror mujoco_mpc_b200/estimator.py (Unscented, Kalman) writes them, with each output summed
+// in a fixed serial order and every product that feeds a sum rounded on its own (__dmul_rn / __dadd_rn: the build's
+// -use_fast_math contracts plain a * b + c into an FMA), so results do not depend on the compiler's contractions.
+// Rows of the step launch: filter b owns rows [b rows, (b + 1) rows), laid out as the mirror's backend call
+// (Unscented: the 2 ndstate sigma points, nominal last; Kalman: the centre, then the perturbations).
 //
 //   estimator_rows_kernel      the step inputs of every row: state, ctrl, warm start and mocap of its filter
 //                              (Unscented: the Cholesky factor of P first; a factor that is not full rank fails the
@@ -14,16 +14,17 @@
 //   kalman_measurement_kernel  C, S = C P C' + R, gain update, correction
 //   kalman_prediction_kernel   A, P = A P A' + Q, the centre's next state, time
 //
-// A failed factorisation sets status[b] = MJPC_B200_ERR_BAD_ARGUMENT and leaves filter b's state, covariance, time,
-// warm start and warnings untouched; the other filters do not depend on it.
+// A failed factorisation sets status[b] to the factor's mjpc_b200_bank::Status and leaves filter b's state,
+// covariance, time, warm start and warnings untouched; the other filters do not depend on it.
 #pragma once
 #include <cuda_runtime.h>
+
+#include "filter_bank.h"
 
 namespace mjpc_dev {
 
 constexpr int kFilterThreads = 128;
 constexpr int kFilterKalman = 1, kFilterUnscented = 2;   // the reference's `estimator` numeric (estimators/include.cc)
-constexpr int kFilterFailed = -1;                        // MJPC_B200_ERR_BAD_ARGUMENT
 
 struct FilterBankArgs {
   int nq, nv, nu, nmocap, njnt;
@@ -61,12 +62,12 @@ inline size_t filter_scratch_layout(FilterBankArgs& a) {
   return w;
 }
 
-// ------------------------------------------------------------------------------------ fp64 in the host's rounding
+// ------------------------------------------------------------------------- fp64, every product rounded on its own
 __device__ __forceinline__ double dmul(double a, double b) { return __dmul_rn(a, b); }
 __device__ __forceinline__ double dadd(double a, double b) { return __dadd_rn(a, b); }
 __device__ __forceinline__ double dsub(double a, double b) { return __dsub_rn(a, b); }
 
-// o = a * b (quaternions), each component summed left to right as the host writes it
+// o = a * b (quaternions), each component summed left to right as mju_mulQuat writes it
 __device__ inline void fb_quat_mul(double* o, const double* a, const double* b) {
   o[0] = dsub(dsub(dsub(dmul(a[0], b[0]), dmul(a[1], b[1])), dmul(a[2], b[2])), dmul(a[3], b[3]));
   o[1] = dsub(dadd(dadd(dmul(a[0], b[1]), dmul(a[1], b[0])), dmul(a[2], b[3])), dmul(a[3], b[2]));
@@ -87,7 +88,7 @@ __device__ inline void fb_sub_quat(double* res, const double* qa, const double* 
   for (int c = 0; c < 3; c++) res[c] = dmul(axis[c], speed);
 }
 
-// mju_quatIntegrate: q * exp(scale v / 2), normalised (planner.cc QuatIntegrate)
+// mju_quatIntegrate: q * exp(scale v / 2), normalised (estimator.py quat_integrate)
 __device__ inline void fb_quat_integrate(double* q, const double* v, double scale) {
   const double w[3] = {dmul(v[0], scale), dmul(v[1], scale), dmul(v[2], scale)};
   const double a = sqrt(dadd(dadd(dmul(w[0], w[0]), dmul(w[1], w[1])), dmul(w[2], w[2])));
@@ -102,7 +103,7 @@ __device__ inline void fb_quat_integrate(double* q, const double* v, double scal
   for (int k = 0; k < 4; k++) q[k] = o[k] / n;
 }
 
-// mj_integratePos: qpos (+) scale dq, dq(k) the tangent vector's entry k (planner.cc IntegratePos)
+// mj_integratePos: qpos (+) scale dq, dq(k) the tangent vector's entry k (estimator.py integrate_pos)
 template <class DQ>
 __device__ inline void fb_integrate_pos(const FilterBankArgs& A, double* qpos, DQ dq, double scale) {
   for (int j = 0; j < A.njnt; j++) {
@@ -119,7 +120,7 @@ __device__ inline void fb_integrate_pos(const FilterBankArgs& A, double* qpos, D
   }
 }
 
-// StateAdd: x (+) scale dx, positions through fb_integrate_pos, velocities added (estimator.cc)
+// x (+) scale dx, positions through fb_integrate_pos, velocities added (estimator.py _Filter._state_add)
 template <class DQ>
 __device__ inline void fb_state_add(const FilterBankArgs& A, double* x, DQ dx, double scale) {
   fb_integrate_pos(A, x, dx, scale);
@@ -144,7 +145,7 @@ __device__ inline void fb_state_diff(const FilterBankArgs& A, double* dx, const 
 
 // ------------------------------------------------------------------------------------------ block-wide linear algebra
 // CholFactor (mju_cholFactor) of the row-major n x n M in place, pivots below mindiag raised to it; every thread gets
-// the rank.  Column j: thread 0 forms the pivot, then the rows below it in parallel, each summed in the host's order.
+// the rank.  Column j: thread 0 forms the pivot, then the rows below it in parallel, each summed serially.
 __device__ inline int fb_chol_factor(double* M, int n, double mindiag) {
   __shared__ int rank;
   if (threadIdx.x == 0) rank = 0;
@@ -194,7 +195,7 @@ __device__ inline void fb_symmetrize(double* P, int n) {
   __syncthreads();
 }
 
-// Estimator::GainUpdate: corr = X S^-1 e, P = P0 - X S^-1 X' symmetrised (P may alias P0), with X [ns][ny] and S
+// The gain update (estimator.py _Filter._gain): corr = X S^-1 e, P = P0 - X S^-1 X' symmetrised (P may alias P0), with X [ns][ny] and S
 // [ny]^2 (overwritten by its factor), e (overwritten by S^-1 e) and T [ns][ny] scratch.  false, with corr and P
 // untouched, when S is not full rank.
 __device__ inline bool fb_gain_update(const double* X, double* S, double* e, const double* P0, double* corr, double* P,
@@ -222,8 +223,8 @@ __device__ inline bool fb_gain_update(const double* X, double* S, double* e, con
   return true;
 }
 
-// Principal eigenvector of a symmetric 4 x 4 matrix by cyclic Jacobi rotations, signed to agree with ref (unscented.cc
-// PrincipalEigenVector4), by one thread
+// Principal eigenvector of a symmetric 4 x 4 matrix by cyclic Jacobi rotations, signed to agree with ref (estimator.py
+// principal_eigenvector4), by one thread
 __device__ inline void fb_principal_eigenvector4(double* out, const double* K, const double* ref) {
   double Am[16], V[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
   for (int k = 0; k < 16; k++) Am[k] = K[k];
@@ -275,7 +276,7 @@ __device__ inline void fb_load_next(const FilterBankArgs& A, int b, double* rows
   __syncthreads();
 }
 
-// Estimator::Commit after a successful update: the warm start from row `centre`, the rows' warnings
+// After a successful update (estimator.py _Filter._commit): the warm start from row `centre`, the rows' warnings
 __device__ inline void fb_commit(const FilterBankArgs& A, int b, int centre) {
   const size_t row0 = (size_t)b * A.rows;
   for (int k = threadIdx.x; k < A.nv; k += blockDim.x) A.warm[(size_t)b * A.nv + k] = A.qacc[(row0 + centre) * A.nv + k];
@@ -289,7 +290,7 @@ __device__ inline void fb_commit(const FilterBankArgs& A, int b, int centre) {
 // -------------------------------------------------------------------------------------------------------- kernels
 // The step rows of every filter.  phase 0: Unscented sigma points from the Cholesky factor of P (a factor that is not
 // full rank fails the filter; its rows then repeat its state).  phase 1: Kalman measurement rows, phase 2: Kalman
-// prediction rows, both the centre state and its +-epsilon tangent-space perturbations (Kalman::Perturbed).
+// prediction rows, both the centre state and its +-epsilon tangent-space perturbations (estimator.py Kalman.perturbed).
 extern "C" __global__ void __launch_bounds__(kFilterThreads) estimator_rows_kernel(const __grid_constant__ FilterBankArgs A) {
   const int b = blockIdx.x, nq = A.nq, nv = A.nv, nx = nq + nv, ns = 2 * nv, R = A.rows;
   double* W = A.scratch + (size_t)b * A.scratch_words;
@@ -302,7 +303,8 @@ extern "C" __global__ void __launch_bounds__(kFilterThreads) estimator_rows_kern
     __syncthreads();
     ok = fb_chol_factor(F, ns, 1e-15) == ns;
   }
-  if (A.phase < 2 && threadIdx.x == 0) A.status[b] = ok ? 0 : kFilterFailed;
+  if (A.phase < 2 && threadIdx.x == 0)
+    A.status[b] = ok ? mjpc_b200_bank::UPDATED : mjpc_b200_bank::COVARIANCE_FACTOR_FAILED;
   for (int r = threadIdx.x; r < R; r += blockDim.x) {
     double* xr = rows + (size_t)r * nx;
     for (int k = 0; k < nx; k++) xr[k] = x[k];
@@ -332,7 +334,7 @@ extern "C" __global__ void __launch_bounds__(kFilterThreads) estimator_rows_kern
   for (int i = threadIdx.x; i < R * nm; i += blockDim.x) A.rmocap[row0 * nm + i] = A.mocap[(size_t)b * nm + i % nm];
 }
 
-// Unscented::Update after the sigma-point launch (unscented.cc EvaluateSigmaPoints .. Update)
+// Unscented.update after the sigma-point launch (unscented.cc EvaluateSigmaPoints .. Update)
 extern "C" __global__ void __launch_bounds__(kFilterThreads) unscented_update_kernel(const __grid_constant__ FilterBankArgs A) {
   const int b = blockIdx.x, nq = A.nq, nv = A.nv, nx = nq + nv, ns = 2 * nv, ny = A.ny, R = A.rows;
   if (A.status[b] != 0) return;
@@ -396,7 +398,7 @@ extern "C" __global__ void __launch_bounds__(kFilterThreads) unscented_update_ke
   __syncthreads();
   double* P = A.P + (size_t)b * ns * ns;
   if (!fb_gain_update(csy, cyy, e, css, corr, P, W + A.o_T, ns, ny)) {
-    if (threadIdx.x == 0) A.status[b] = kFilterFailed;
+    if (threadIdx.x == 0) A.status[b] = mjpc_b200_bank::SENSOR_FACTOR_FAILED;
     return;
   }
   if (threadIdx.x == 0) {
@@ -408,7 +410,7 @@ extern "C" __global__ void __launch_bounds__(kFilterThreads) unscented_update_ke
   fb_commit(A, b, R - 1);
 }
 
-// Kalman::UpdateMeasurement after the measurement launch
+// Kalman.update_measurement (kalman.cc UpdateMeasurement) after the measurement launch
 extern "C" __global__ void __launch_bounds__(kFilterThreads) kalman_measurement_kernel(const __grid_constant__ FilterBankArgs A) {
   const int b = blockIdx.x, nv = A.nv, nx = A.nq + nv, ns = 2 * nv, ny = A.ny;
   double* W = A.scratch + (size_t)b * A.scratch_words;
@@ -440,14 +442,14 @@ extern "C" __global__ void __launch_bounds__(kFilterThreads) kalman_measurement_
   for (int k = threadIdx.x; k < ny; k += blockDim.x) e[k] = dsub(A.sensor[(size_t)b * ny + k], (double)y[k]);
   __syncthreads();
   if (!fb_gain_update(PCt, S, e, P, corr, P, W + A.o_T, ns, ny)) {
-    if (threadIdx.x == 0) A.status[b] = kFilterFailed;
+    if (threadIdx.x == 0) A.status[b] = mjpc_b200_bank::SENSOR_FACTOR_FAILED;
     return;
   }
   if (threadIdx.x == 0) fb_state_add(A, A.state + (size_t)b * nx, [&](int j) { return corr[j]; }, 1.0);
   fb_commit(A, b, 0);
 }
 
-// Kalman::UpdatePrediction after the prediction launch
+// Kalman.update_prediction (kalman.cc UpdatePrediction) after the prediction launch
 extern "C" __global__ void __launch_bounds__(kFilterThreads) kalman_prediction_kernel(const __grid_constant__ FilterBankArgs A) {
   const int b = blockIdx.x, nv = A.nv, nx = A.nq + nv, ns = 2 * nv;
   if (A.status[b] != 0) return;

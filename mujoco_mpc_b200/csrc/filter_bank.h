@@ -1,7 +1,7 @@
-// filter_bank.h - the engine side of the batched state estimators (csrc/host/batch_estimator.h): B filters of one kind
-// whose state, covariance, time, noise, warm start and warnings live in device memory of an engine handle, and whose
-// update is the kernels of estimator_kernels.cuh around step_batch launches of all their rows.  Internal to
-// libmjpc_b200.so: engine.cu implements it, batch_estimator.cc calls it.
+// filter_bank.h - the engine side of the state estimators (csrc/host/estimator.h): B filters of one kind whose state,
+// covariance, time, noise, warm start and warnings live in device memory of an engine handle, and whose update is the
+// kernels of estimator_kernels.cuh around step_batch launches of all their rows.  Internal to libmjpc_b200.so:
+// engine.cu implements it, estimator.cc calls it.
 #pragma once
 #include "../../include/mjpc_b200.h"
 
@@ -24,14 +24,20 @@ struct Desc {
 // [nsensordata] (double); WARMSTART [nv] (float); WARNINGS [1] (int)
 enum Field { STATE, COVARIANCE, TIME, NOISE_PROCESS, NOISE_SENSOR, WARMSTART, WARNINGS };
 
+// the steps of a Kalman update; the Unscented kind has one step and ignores the choice
+enum Phases { MEASUREMENT = 1, PREDICTION = 2, MEASUREMENT_AND_PREDICTION = 3 };
+
+// a filter's status after an update: updated, or the factorisation that failed and left it untouched
+enum Status { UPDATED = 0, SENSOR_FACTOR_FAILED = 1, COVARIANCE_FACTOR_FAILED = 2 };
+
 // The handle's filter bank for d (replacing any earlier one), every field zero.  A sensor range outside the model's
 // sensors: MJPC_B200_ERR_BAD_ARGUMENT; a sensor the engine does not evaluate: MJPC_B200_ERR_UNSUPPORTED;
 // num_filters x rows above the handle's max_candidates: MJPC_B200_ERR_CAPACITY.
 int Init(mjpc_b200_t* h, const Desc& d);
 // copies filter b's field to (write = 0) or from (write = 1) `data`
 int Access(mjpc_b200_t* h, int b, int field, void* data, int write);
-// one update of every filter from ctrl [B][nu], sensor [B][nsensordata] and mocap [B][7 nmocap]; status [B] = 0 or
-// MJPC_B200_ERR_BAD_ARGUMENT for a failed factorisation
-int Update(mjpc_b200_t* h, const float* ctrl, const double* sensor, const float* mocap, int* status);
+// one update of every filter from ctrl [B][nu], sensor [B][nsensordata] and mocap [B][7 nmocap]; status [B] = Status.
+// phases: Phases.  A Kalman prediction alone reads no sensor (it may be NULL) and steps with the ctrl and mocap given.
+int Update(mjpc_b200_t* h, const float* ctrl, const double* sensor, const float* mocap, int phases, int* status);
 
 }  // namespace mjpc_b200_bank

@@ -2,11 +2,20 @@
 #include "estimator.h"
 
 #include <algorithm>
+#include <cmath>
 
 #include "../dev_model.h"   // Blob reader (plain C++)
+#include "../filter_bank.h"
 
 namespace mjpc_b200_host {
 
+using mjpc_b200_bank::Access;
+
+namespace {
+
+// What the estimators read from the blob besides HostModel: every sensor's dimension, the model's mocap poses
+// [7 nmocap] and the Reset state (the first keyframe, else qpos0 and zero qvel).  0, or MJPC_B200_ERR_BAD_BLOB for a
+// blob without sensor entries.
 int LoadEstimatorBlob(const mjpc_model_blob* model, const HostModel& m, std::vector<int>* dims, int* nmocap,
                       std::vector<float>* mocap0, std::vector<double>* key_state) {
   try {
@@ -36,169 +45,287 @@ int LoadEstimatorBlob(const mjpc_model_blob* model, const HostModel& m, std::vec
   return 0;
 }
 
+}  // namespace
+
 Estimator::~Estimator() { if (engine_) mjpc_b200_destroy(engine_); }
 
-int Estimator::InitializeBase(const mjpc_model_blob* model, int sensor_start, int nsensor, double timestep_,
-                              int device) {
-  const std::string name(name_);
-  if (!model || !(timestep_ > 0)) { error = name + ": bad argument"; return MJPC_B200_ERR_BAD_ARGUMENT; }
-  if (int rc = m_.Load(model)) { error = name + ": bad blob"; return rc; }
+int Estimator::Fail(int rc, const std::string& what) {
+  error = std::string(Name()) + ": " + what;
+  return rc;
+}
+
+int Estimator::Initialize(const mjpc_model_blob* model, int kind_, int num_filters_, int sensor_start, int nsensor,
+                          double timestep_, const double* settings, int device) {
+  if (!model || (kind_ != kKalman && kind_ != kUnscented) || num_filters_ < 1 || !settings || !(timestep_ > 0))
+    return Fail(MJPC_B200_ERR_BAD_ARGUMENT, "bad argument");
+  kind = kind_;
+  if (kind == kKalman && !(settings[0] > 0)) return Fail(MJPC_B200_ERR_BAD_ARGUMENT, "bad argument");
+  if (int rc = m_.Load(model)) return Fail(rc, "bad blob");
   std::vector<int> dims;
-  if (LoadEstimatorBlob(model, m_, &dims, &nmocap_, &mocap0_, &key_state_)) {
-    error = name + ": blob without sensor entries";
-    return MJPC_B200_ERR_BAD_BLOB;
-  }
-  if (sensor_start < 0 || nsensor < 1 || sensor_start > (int)dims.size() - nsensor) {
-    error = name + ": sensor range outside the model's sensors";
-    return MJPC_B200_ERR_BAD_ARGUMENT;
-  }
-  sensor_start_ = sensor_start; nsensor_ = nsensor;
+  if (LoadEstimatorBlob(model, m_, &dims, &nmocap_, &mocap0_, &key_state_))
+    return Fail(MJPC_B200_ERR_BAD_BLOB, "blob without sensor entries");
+  if (sensor_start < 0 || nsensor < 1 || sensor_start > (int)dims.size() - nsensor)
+    return Fail(MJPC_B200_ERR_BAD_ARGUMENT, "sensor range outside the model's sensors");
+  num_filters = num_filters_; timestep = timestep_;
+  ndstate = 2 * m_.nv;
   nsensordata = 0;
   for (int i = sensor_start; i < sensor_start + nsensor; i++) nsensordata += dims[i];
-  timestep = timestep_;
-  ndstate = 2 * m_.nv;
-  const size_t ns = 2 * ndstate + 1, nx = m_.nq + m_.nv;
-  if (int rc = mjpc_b200_create(model, (int)ns, 1, device, &engine_)) { error = mjpc_b200_last_error(); return rc; }
-  if (int rc = mjpc_b200_set_options(engine_, timestep, 0)) { error = mjpc_b200_last_error(); return rc; }
-  states_.resize(ns * nx); fstates_.resize(ns * nx); fnext_.resize(ns * nx); fsensor_.resize(ns * nsensordata);
-  fqacc_.resize(ns * m_.nv); fwarm_.resize(ns * m_.nv); counts_.resize(4 * ns);
-  Reset(nullptr, 0.0, 1e-4, 1e-4, 1e-4);
-  std::copy(key_state_.begin(), key_state_.end(), states_.begin());
-  if (int rc = StepSensors(1, std::vector<double>(m_.nu, 0.0).data(), nullptr)) return rc;
-  Reset(nullptr, 0.0, 1e-4, 1e-4, 1e-4);
+  mjpc_b200_bank::Desc d = {};
+  d.kind = kind; d.num_filters = num_filters; d.sensor_start = sensor_start; d.nsensor = nsensor; d.timestep = timestep;
+  if (kind == kUnscented) {   // the derived settings (unscented.cc:171-290)
+    const double alpha = settings[0], beta = settings[1];
+    rows = 2 * ndstate + 1;
+    const double lambda = ndstate * (alpha * alpha - 1.0);
+    d.sigma_step = std::sqrt(ndstate + lambda);
+    d.weight_mean0 = lambda / (ndstate + lambda);
+    d.weight_covariance0 = d.weight_mean0 + 1.0 - alpha * alpha + beta;
+    d.weight_sigma = 1.0 / (2.0 * (ndstate + lambda));
+  } else {
+    epsilon = settings[0];
+    d.epsilon = epsilon; d.centered = settings[1] != 0;
+    rows = (d.centered ? 2 : 1) * ndstate + 1;
+  }
+  d.rows = rows;
+  if ((long long)num_filters * rows > kEstimatorMaxRows)
+    return Fail(MJPC_B200_ERR_CAPACITY, "num_filters x rows per filter above " + std::to_string(kEstimatorMaxRows));
+  d.njnt = (int)m_.jnt_type.size();
+  d.jnt_type = m_.jnt_type.data(); d.jnt_qposadr = m_.jnt_qposadr.data(); d.jnt_dofadr = m_.jnt_dofadr.data();
+  if (int rc = mjpc_b200_create(model, num_filters * rows, 1, device, &engine_))
+    return Fail(rc, mjpc_b200_last_error());
+  if (int rc = mjpc_b200_set_options(engine_, timestep, 0)) return Fail(rc, mjpc_b200_last_error());
+  if (int rc = mjpc_b200_bank::Init(engine_, d)) return Fail(rc, mjpc_b200_last_error());
+  fctrl_.resize((size_t)num_filters * m_.nu); ctrl_.resize(fctrl_.size());
+  fmocap_.resize((size_t)num_filters * mocap0_.size()); mocap_.resize(fmocap_.size());
+  for (int b = 0; b < num_filters; b++)
+    if (int rc = Reset(b, nullptr, 0.0, 1e-4, 1e-4, 1e-4)) return rc;
   return 0;
 }
 
-void Estimator::Reset(const double* s, double t, double covariance_scale, double process_scale, double sensor_scale) {
-  state.assign(s ? s : key_state_.data(), (s ? s : key_state_.data()) + m_.nq + m_.nv);
-  time = t;
-  covariance.assign((size_t)ndstate * ndstate, 0.0);
-  for (int i = 0; i < ndstate; i++) covariance[(size_t)i * ndstate + i] = covariance_scale;
-  noise_process.assign(ndstate, process_scale);
-  noise_sensor.assign(nsensordata, sensor_scale);
-  qacc_warmstart_.assign(m_.nv, 0.0);
-  warnings = 0;
-}
-
-int Estimator::StepSensors(int n, const double* ctrl, const float* mocap) {
-  const int nv = m_.nv;
-  for (size_t i = 0; i < (size_t)n * (m_.nq + nv); i++) fstates_[i] = (float)states_[i];
-  for (int i = 0; i < n; i++)
-    for (int k = 0; k < nv; k++) fwarm_[(size_t)i * nv + k] = (float)qacc_warmstart_[k];
-  std::vector<float> u(m_.nu);
-  for (int k = 0; k < m_.nu; k++) u[k] = (float)ctrl[k];
-  if (int rc = mjpc_b200_step_sensors(engine_, n, fstates_.data(), u.data(), fwarm_.data(),
-                                      mocap ? mocap : mocap0_.data(), time, sensor_start_, nsensor_, fnext_.data(),
-                                      fsensor_.data(), fqacc_.data(), counts_.data())) {
-    error = mjpc_b200_last_error();
-    return rc;
-  }
-  nstepped_ = n;
+int Estimator::Reset(int b, const double* state, double time, double covariance_scale, double process_scale,
+                     double sensor_scale) {
+  if (b < 0 || b >= num_filters) return Fail(MJPC_B200_ERR_BAD_ARGUMENT, "filter index outside [0, num_filters)");
+  std::vector<double> P((size_t)ndstate * ndstate, 0.0), np(ndstate, process_scale), ns(nsensordata, sensor_scale);
+  for (int i = 0; i < ndstate; i++) P[(size_t)i * ndstate + i] = covariance_scale;
+  std::vector<float> warm(m_.nv, 0.f);
+  int warnings = 0;
+  const void* fields[] = {state ? state : key_state_.data(), P.data(), &time, np.data(), ns.data(), warm.data(),
+                          &warnings};
+  for (int f = mjpc_b200_bank::STATE; f <= mjpc_b200_bank::WARNINGS; f++)
+    if (int rc = Access(engine_, b, f, const_cast<void*>(fields[f]), 1)) return Fail(rc, mjpc_b200_last_error());
+  std::fill_n(ctrl_.begin() + (size_t)b * m_.nu, m_.nu, 0.f);
+  std::copy(mocap0_.begin(), mocap0_.end(), mocap_.begin() + (size_t)b * mocap0_.size());
   return 0;
 }
 
-void Estimator::Commit(int centre) {
-  for (int k = 0; k < m_.nv; k++) qacc_warmstart_[k] = fqacc_[(size_t)centre * m_.nv + k];
-  for (int i = 0; i < nstepped_; i++) warnings += counts_[4 * i + 3] != 0;
+int Estimator::SetNoise(int b, const double* process, const double* sensor) {
+  if (b < 0 || b >= num_filters) return Fail(MJPC_B200_ERR_BAD_ARGUMENT, "filter index outside [0, num_filters)");
+  if (process)
+    if (int rc = Access(engine_, b, mjpc_b200_bank::NOISE_PROCESS, const_cast<double*>(process), 1))
+      return Fail(rc, mjpc_b200_last_error());
+  if (sensor)
+    if (int rc = Access(engine_, b, mjpc_b200_bank::NOISE_SENSOR, const_cast<double*>(sensor), 1))
+      return Fail(rc, mjpc_b200_last_error());
+  return 0;
 }
 
-int Estimator::GainUpdate(const double* X, double* S, double* e, const double* P0, double* corr, double* P) {
-  const int ns = ndstate, ny = nsensordata;
-  if (CholFactor(S, ny, 1e-15) < ny) {
-    error = std::string(name_) + " update: sensor covariance factorisation failed";
-    return MJPC_B200_ERR_BAD_ARGUMENT;
+int Estimator::Set(int b, const double* state, const double* covariance, double time) {
+  if (b < 0 || b >= num_filters) return Fail(MJPC_B200_ERR_BAD_ARGUMENT, "filter index outside [0, num_filters)");
+  if (state)
+    if (int rc = Access(engine_, b, mjpc_b200_bank::STATE, const_cast<double*>(state), 1))
+      return Fail(rc, mjpc_b200_last_error());
+  if (covariance)
+    if (int rc = Access(engine_, b, mjpc_b200_bank::COVARIANCE, const_cast<double*>(covariance), 1))
+      return Fail(rc, mjpc_b200_last_error());
+  if (int rc = Access(engine_, b, mjpc_b200_bank::TIME, &time, 1)) return Fail(rc, mjpc_b200_last_error());
+  return 0;
+}
+
+int Estimator::Update(const double* ctrl, const double* sensor, const float* mocap, int phases, int* status) {
+  const bool measure = kind == kUnscented || phases != mjpc_b200_bank::PREDICTION;
+  if ((measure && ((!ctrl && m_.nu) || !sensor)) || !status)
+    return Fail(MJPC_B200_ERR_BAD_ARGUMENT, "update: bad argument");
+  if (!measure) {
+    if (int rc = mjpc_b200_bank::Update(engine_, ctrl_.data(), nullptr, mocap_.data(), phases, status))
+      return Fail(rc, mjpc_b200_last_error());
+    return 0;
   }
-  CholSolve(S, ny, e);
-  for (int r = 0; r < ns; r++) {
-    corr[r] = 0.0;
-    for (int c = 0; c < ny; c++) corr[r] += X[(size_t)r * ny + c] * e[c];
-  }
-  std::vector<double> T(X, X + (size_t)ns * ny);   // rows S^-1 X[r]
-  for (int r = 0; r < ns; r++) CholSolve(S, ny, &T[(size_t)r * ny]);
-  for (int r = 0; r < ns; r++)
-    for (int c = 0; c < ns; c++) {
-      double a = 0;
-      for (int k = 0; k < ny; k++) a += X[(size_t)r * ny + k] * T[(size_t)c * ny + k];
-      P[(size_t)r * ns + c] = P0[(size_t)r * ns + c] - a;
+  // ctrl in the engine's float; a NULL mocap is the model's for every filter
+  const size_t nu = m_.nu, nm = mocap0_.size();
+  for (size_t i = 0; i < fctrl_.size(); i++) fctrl_[i] = (float)ctrl[i];
+  for (int b = 0; b < num_filters; b++)
+    std::copy_n(mocap ? mocap + b * nm : mocap0_.data(), nm, fmocap_.begin() + b * nm);
+  if (int rc = mjpc_b200_bank::Update(engine_, fctrl_.data(), sensor, fmocap_.data(), phases, status))
+    return Fail(rc, mjpc_b200_last_error());
+  for (int b = 0; b < num_filters; b++)
+    if (status[b] == mjpc_b200_bank::UPDATED) {
+      std::copy_n(fctrl_.begin() + b * nu, nu, ctrl_.begin() + b * nu);
+      std::copy_n(fmocap_.begin() + b * nm, nm, mocap_.begin() + b * nm);
     }
-  Symmetrize(P);
   return 0;
 }
 
-void Estimator::Symmetrize(double* P) const {
-  const int n = ndstate;
-  for (int r = 0; r < n; r++)
-    for (int c = r + 1; c < n; c++) {
-      const double s = 0.5 * (P[(size_t)r * n + c] + P[(size_t)c * n + r]);
-      P[(size_t)r * n + c] = P[(size_t)c * n + r] = s;
-    }
-}
-
-void Estimator::StateAdd(double* x, const double* dx, double scale) const {
-  IntegratePos(m_, x, dx, scale);
-  for (int k = 0; k < m_.nv; k++) x[m_.nq + k] += scale * dx[m_.nv + k];
+int Estimator::Get(int b, double* state, double* covariance, double* time, double* scalars) {
+  if (b < 0 || b >= num_filters) return Fail(MJPC_B200_ERR_BAD_ARGUMENT, "filter index outside [0, num_filters)");
+  if (state)
+    if (int rc = Access(engine_, b, mjpc_b200_bank::STATE, state, 0)) return Fail(rc, mjpc_b200_last_error());
+  if (covariance)
+    if (int rc = Access(engine_, b, mjpc_b200_bank::COVARIANCE, covariance, 0)) return Fail(rc, mjpc_b200_last_error());
+  if (time)
+    if (int rc = Access(engine_, b, mjpc_b200_bank::TIME, time, 0)) return Fail(rc, mjpc_b200_last_error());
+  if (scalars) {
+    int warnings = 0;
+    if (int rc = Access(engine_, b, mjpc_b200_bank::WARNINGS, &warnings, 0)) return Fail(rc, mjpc_b200_last_error());
+    scalars[0] = ndstate; scalars[1] = rows; scalars[2] = nsensordata; scalars[3] = warnings; scalars[4] = timestep;
+    if (kind == kKalman) scalars[5] = epsilon;
+  }
+  return 0;
 }
 
 }  // namespace mjpc_b200_host
 
 // ------------------------------------------------------------------------------------------------------------ C ABI
-// (the generic estimator family of include/mjpc_b200.h: every kind's handle, a NULL one refused)
-using mjpc_b200_host::Estimator;
-using mjpc_b200_host::EstimatorOf;
+using namespace mjpc_b200_host;
+
+namespace {
+
+int Create(const mjpc_model_blob* model, int kind, int num_filters, int sensor_start, int nsensor, double timestep,
+           const double* settings, int device, Estimator** out) {
+  if (!out) return MJPC_B200_ERR_BAD_ARGUMENT;
+  *out = nullptr;
+  auto* f = new Estimator;
+  if (int rc = f->Initialize(model, kind, num_filters, sensor_start, nsensor, timestep, settings, device)) {
+    delete f;
+    return rc;
+  }
+  *out = f;
+  return 0;
+}
+
+// the single filter behind a handle of the mjpc_b200_estimator_* family (nullptr for a NULL handle); non-const
+// because get, which takes a const handle, reads through the filter's engine and may record an error
+Estimator* Single(const mjpc_b200_estimator_t* h) {
+  return reinterpret_cast<Estimator*>(const_cast<mjpc_b200_estimator_t*>(h));
+}
+
+// one update of a single filter; a failed factorisation is MJPC_B200_ERR_BAD_ARGUMENT with last_error naming the factor
+int UpdateSingle(Estimator* f, const double* ctrl, const double* sensor, const float* mocap, int phases) {
+  if (!f) return MJPC_B200_ERR_BAD_ARGUMENT;
+  int status = 0;
+  if (int rc = f->Update(ctrl, sensor, mocap, phases, &status)) return rc;
+  if (status == mjpc_b200_bank::UPDATED) return 0;
+  f->error = std::string(f->Name()) + " update: " +
+             (status == mjpc_b200_bank::COVARIANCE_FACTOR_FAILED ? "covariance" : "sensor covariance") +
+             " factorisation failed";
+  return MJPC_B200_ERR_BAD_ARGUMENT;
+}
+
+}  // namespace
 
 extern "C" {
 
+// ---- single filters: filter 0 of a one-filter bank
+int mjpc_b200_unscented_create(const mjpc_model_blob* model, int sensor_start, int nsensor, double timestep,
+                               double alpha, double beta, int device, mjpc_b200_estimator_t** out) {
+  const double settings[2] = {alpha, beta};
+  return Create(model, kUnscented, 1, sensor_start, nsensor, timestep, settings, device,
+                reinterpret_cast<Estimator**>(out));
+}
+
+int mjpc_b200_kalman_create(const mjpc_model_blob* model, int sensor_start, int nsensor, double timestep,
+                            double epsilon, int centered, int device, mjpc_b200_estimator_t** out) {
+  const double settings[2] = {epsilon, centered != 0 ? 1.0 : 0.0};
+  return Create(model, kKalman, 1, sensor_start, nsensor, timestep, settings, device,
+                reinterpret_cast<Estimator**>(out));
+}
+
 int mjpc_b200_estimator_destroy(mjpc_b200_estimator_t* h) {
-  Estimator* f = EstimatorOf<Estimator>(h);
-  if (!f) return MJPC_B200_ERR_BAD_ARGUMENT;
-  delete f;
+  if (!h) return MJPC_B200_ERR_BAD_ARGUMENT;
+  delete Single(h);
   return 0;
 }
 
 int mjpc_b200_estimator_reset(mjpc_b200_estimator_t* h, const double* state, double time, double covariance_scale,
                               double process_scale, double sensor_scale) {
-  Estimator* f = EstimatorOf<Estimator>(h);
-  if (!f) return MJPC_B200_ERR_BAD_ARGUMENT;
-  f->Reset(state, time, covariance_scale, process_scale, sensor_scale);
-  return 0;
+  return h ? Single(h)->Reset(0, state, time, covariance_scale, process_scale, sensor_scale)
+           : MJPC_B200_ERR_BAD_ARGUMENT;
 }
 
 int mjpc_b200_estimator_set_noise(mjpc_b200_estimator_t* h, const double* process, const double* sensor) {
-  Estimator* f = EstimatorOf<Estimator>(h);
-  if (!f) return MJPC_B200_ERR_BAD_ARGUMENT;
-  if (process) f->noise_process.assign(process, process + f->ndstate);
-  if (sensor) f->noise_sensor.assign(sensor, sensor + f->nsensordata);
-  return 0;
+  return h ? Single(h)->SetNoise(0, process, sensor) : MJPC_B200_ERR_BAD_ARGUMENT;
 }
 
 int mjpc_b200_estimator_set(mjpc_b200_estimator_t* h, const double* state, const double* covariance, double time) {
-  Estimator* f = EstimatorOf<Estimator>(h);
-  if (!f) return MJPC_B200_ERR_BAD_ARGUMENT;
-  if (state) f->state.assign(state, state + f->state.size());
-  if (covariance) f->covariance.assign(covariance, covariance + f->covariance.size());
-  f->time = time;
-  return 0;
+  return h ? Single(h)->Set(0, state, covariance, time) : MJPC_B200_ERR_BAD_ARGUMENT;
 }
 
 int mjpc_b200_estimator_update(mjpc_b200_estimator_t* h, const double* ctrl, const double* sensor, const float* mocap) {
-  Estimator* f = EstimatorOf<Estimator>(h);
-  return f ? f->Update(ctrl, sensor, mocap) : MJPC_B200_ERR_BAD_ARGUMENT;
+  return UpdateSingle(Single(h), ctrl, sensor, mocap, mjpc_b200_bank::MEASUREMENT_AND_PREDICTION);
 }
 
 int mjpc_b200_estimator_get(const mjpc_b200_estimator_t* h, double* state, double* covariance, double* time,
                             double* scalars) {
-  const Estimator* f = reinterpret_cast<const Estimator*>(h);
+  return h ? Single(h)->Get(0, state, covariance, time, scalars) : MJPC_B200_ERR_BAD_ARGUMENT;
+}
+
+const char* mjpc_b200_estimator_last_error(const mjpc_b200_estimator_t* h) { return h ? Single(h)->error.c_str() : ""; }
+
+int mjpc_b200_kalman_update_measurement(mjpc_b200_estimator_t* h, const double* ctrl, const double* sensor,
+                                        const float* mocap) {
+  Estimator* f = Single(h);
+  return f && f->kind == kKalman ? UpdateSingle(f, ctrl, sensor, mocap, mjpc_b200_bank::MEASUREMENT)
+                                 : MJPC_B200_ERR_BAD_ARGUMENT;
+}
+
+int mjpc_b200_kalman_update_prediction(mjpc_b200_estimator_t* h) {
+  Estimator* f = Single(h);
+  return f && f->kind == kKalman ? UpdateSingle(f, nullptr, nullptr, nullptr, mjpc_b200_bank::PREDICTION)
+                                 : MJPC_B200_ERR_BAD_ARGUMENT;
+}
+
+// ---- filter banks
+int mjpc_b200_batch_estimator_create(const mjpc_model_blob* model, int kind, int num_filters, int sensor_start,
+                                     int nsensor, double timestep, const double* settings, int device, void** out) {
+  return Create(model, kind, num_filters, sensor_start, nsensor, timestep, settings, device,
+                reinterpret_cast<Estimator**>(out));
+}
+
+int mjpc_b200_batch_estimator_destroy(void* f) {
   if (!f) return MJPC_B200_ERR_BAD_ARGUMENT;
-  if (state) std::copy(f->state.begin(), f->state.end(), state);
-  if (covariance) std::copy(f->covariance.begin(), f->covariance.end(), covariance);
-  if (time) *time = f->time;
-  if (scalars) f->GetScalars(scalars);
+  delete static_cast<Estimator*>(f);
   return 0;
 }
 
-const char* mjpc_b200_estimator_last_error(const mjpc_b200_estimator_t* h) {
-  const Estimator* f = reinterpret_cast<const Estimator*>(h);
-  return f ? f->error.c_str() : "";
+int mjpc_b200_batch_estimator_reset(void* f, int filter, const double* state, double time, double covariance_scale,
+                                    double process_scale, double sensor_scale) {
+  return f ? static_cast<Estimator*>(f)->Reset(filter, state, time, covariance_scale, process_scale, sensor_scale)
+           : MJPC_B200_ERR_BAD_ARGUMENT;
+}
+
+int mjpc_b200_batch_estimator_set_noise(void* f, int filter, const double* process, const double* sensor) {
+  return f ? static_cast<Estimator*>(f)->SetNoise(filter, process, sensor) : MJPC_B200_ERR_BAD_ARGUMENT;
+}
+
+int mjpc_b200_batch_estimator_set(void* f, int filter, const double* state, const double* covariance, double time) {
+  return f ? static_cast<Estimator*>(f)->Set(filter, state, covariance, time) : MJPC_B200_ERR_BAD_ARGUMENT;
+}
+
+int mjpc_b200_batch_estimator_update(void* f, const double* ctrl, const double* sensor, const float* mocap,
+                                     int* status) {
+  if (!f) return MJPC_B200_ERR_BAD_ARGUMENT;
+  Estimator* e = static_cast<Estimator*>(f);
+  if (int rc = e->Update(ctrl, sensor, mocap, mjpc_b200_bank::MEASUREMENT_AND_PREDICTION, status)) return rc;
+  for (int b = 0; b < e->num_filters; b++)
+    if (status[b] != mjpc_b200_bank::UPDATED) status[b] = MJPC_B200_ERR_BAD_ARGUMENT;
+  return 0;
+}
+
+int mjpc_b200_batch_estimator_get(void* f, int filter, double* state, double* covariance, double* time,
+                                  double* scalars) {
+  return f ? static_cast<Estimator*>(f)->Get(filter, state, covariance, time, scalars) : MJPC_B200_ERR_BAD_ARGUMENT;
+}
+
+const char* mjpc_b200_batch_estimator_last_error(const void* f) {
+  return f ? static_cast<const Estimator*>(f)->error.c_str() : "";
 }
 
 }  // extern "C"

@@ -1,8 +1,33 @@
-// estimator.h - the base every host state estimator derives from (the reference's virtual Estimator,
-// mjpc/estimators/estimator.h, limited to what exists here) and the engine plumbing the estimators share: the engine
-// handle holding 2 ndstate + 1 states (the most any filter steps in one launch), the blob's sensor range, mocap and
-// Reset state, the float staging of one mjpc_b200_step_sensors launch with its warm start, and the double-precision
-// gain step, symmetrisation and tangent-space state addition.
+// estimator.h - MJPC's Unscented and Kalman state estimators (mjpc/estimators/unscented.{h,cc}, kalman.{h,cc}; the
+// reference's Estimator base, mjpc/estimators/estimator.h) as a bank of num_filters independent filters of one kind
+// and one model on one engine handle, each with its own state, covariance, time, noise, warm start, ctrl, sensors and
+// mocap.  A single filter (mjpc_b200_unscented_create, mjpc_b200_kalman_create) is the bank of one.  Every update runs
+// on the device: the filter arithmetic in fp64 (estimator_kernels.cuh) and the rows of all filters as one step_batch
+// launch per sigma-point set or Jacobian (filter_bank.h).  The host uploads ctrl, sensors and mocap once per update and
+// downloads one status per filter; state and covariance stay on the device until Get.
+//
+//   Unscented          the 2 ndstate + 1 sigma points (nominal last) stepped with their measurement sensors in one
+//                      launch; means (QuaternionMeans for free and ball joints), differences, covariances, gain update
+//   Kalman measurement (kalman.cc:188-276)  C = d sensors / d state of the pre-step states and y_hat = the centre's
+//                      sensors from one launch; gain P C' (C P C' + R)^-1, correction, P -= ..., symmetrised
+//   Kalman prediction  (kalman.cc:279-323)  A = d next state / d state (tangent-space differences) and the new state
+//                      = the centre's next state from one launch; P = A P A' + diag(process noise), symmetrised
+//
+// Documented differences from the reference:
+//  * a failed factorisation (the Unscented covariance, or either kind's sensor covariance) reports which factor failed
+//    and leaves the filter's state, covariance, time, warm start and warnings untouched (the reference calls
+//    mju_error);
+//  * every row of a launch warm-starts the constraint solver from the centre (Kalman) or nominal (Unscented) row's qacc
+//    of the filter's previous successful launch (zeros after Reset); the reference reuses one mjData, so each row
+//    starts from the previous row's qacc;
+//  * updates take mocap (the reference's mjData keeps the model's) and the measured sensor slice [nsensordata], not the
+//    whole sensordata;
+//  * Kalman: the prediction uses the ctrl and mocap of the last successful measurement, as the reference's mjData does;
+//    both launches run at `time` and the prediction advances it by the timestep (the reference leaves its `time` member
+//    alone and its mjData's clock advances inside mj_step);
+//  * settings are arguments: the blob carries no custom numerics (mujoco_mpc_b200.estimator reads them), and the
+//    engine default for the Kalman finite differences is centred with a larger epsilon than the reference's fp64 1e-6
+//    one-sided (DESIGN.md, "Kalman filter").
 #pragma once
 #include <string>
 #include <vector>
@@ -11,62 +36,46 @@
 
 namespace mjpc_b200_host {
 
-// What the estimators read from the blob besides HostModel: every sensor's dimension, the model's mocap poses
-// [7 nmocap] and the Reset state (the first keyframe, else qpos0 and zero qvel).  0, or MJPC_B200_ERR_BAD_BLOB for a
-// blob without sensor entries.
-int LoadEstimatorBlob(const mjpc_model_blob* model, const HostModel& m, std::vector<int>* dims, int* nmocap,
-                      std::vector<float>* mocap0, std::vector<double>* key_state);
+constexpr int kKalman = 1, kUnscented = 2;   // the reference's `estimator` numeric
+// step rows of one handle: num_filters x (rows per filter) above it is refused at create (MJPC_B200_ERR_CAPACITY)
+constexpr int kEstimatorMaxRows = 65536;
 
 class Estimator {
  public:
-  virtual ~Estimator();
-  // state NULL -> the model's first keyframe if it has one, else qpos0 and zero qvel; covariance = covariance_scale I,
-  // diagonal process / sensor noise, zero warm start and warnings
-  virtual void Reset(const double* state, double time, double covariance_scale, double process_scale,
-                     double sensor_scale);
-  // one filter update from ctrl [nu], the measured sensor slice [nsensordata] and mocap [7 nmocap] (NULL: the model's)
-  virtual int Update(const double* ctrl, const double* sensor, const float* mocap) = 0;
-  // the filter's scalars of mjpc_b200_estimator_get
-  virtual void GetScalars(double* scalars) const = 0;
+  ~Estimator();
+  // kKalman (settings {epsilon, centered}) or kUnscented (settings {alpha, beta}), measuring the sensors
+  // [sensor_start, sensor_start + nsensor); every filter starts as Reset(b, NULL, 0, 1e-4, 1e-4, 1e-4) leaves it
+  int Initialize(const mjpc_model_blob* model, int kind, int num_filters, int sensor_start, int nsensor,
+                 double timestep, const double* settings, int device);
+  // filter b: state NULL -> the model's first keyframe if it has one, else qpos0 and zero qvel; covariance =
+  // covariance_scale I, diagonal process / sensor noise, zero warm start and warnings; the ctrl and mocap of the last
+  // measurement = zeros and the model's mocap
+  int Reset(int b, const double* state, double time, double covariance_scale, double process_scale,
+            double sensor_scale);
+  int SetNoise(int b, const double* process, const double* sensor);             // NULL keeps one
+  int Set(int b, const double* state, const double* covariance, double time);   // NULL keeps one
+  // every filter from ctrl [B][nu], sensor [B][nsensordata] and mocap [B][7 nmocap] (NULL: the model's for every
+  // filter); status [B] = mjpc_b200_bank::Status.  phases: the Kalman kind's steps (mjpc_b200_bank::Phases); a
+  // prediction alone ignores ctrl, sensor and mocap and steps each filter with those of its last successful measurement
+  int Update(const double* ctrl, const double* sensor, const float* mocap, int phases, int* status);
+  // filter b's state, covariance, time and scalars {ndstate, rows, nsensordata, warnings, timestep} (Kalman: then
+  // epsilon); any pointer may be NULL
+  int Get(int b, double* state, double* covariance, double* time, double* scalars);
+  const char* Name() const { return kind == kKalman ? "kalman" : kind == kUnscented ? "unscented" : "estimator"; }
 
-  std::vector<double> state, covariance, noise_process, noise_sensor;
-  double time = 0;
-  int warnings = 0;   // steps that raised a warning since Reset
-  int ndstate = 0, nsensordata = 0;
-  double timestep = 0;
+  int kind = 0, num_filters = 0, ndstate = 0, nsensordata = 0, rows = 0;
+  double timestep = 0, epsilon = 0;
   std::string error;
 
- protected:
-  explicit Estimator(const char* name) : name_(name) {}
-  // Loads the blob, checks the sensor range, creates the engine handle, sets the timestep and Resets.  Then it steps
-  // the reset state once, so a range with a sensor the engine does not evaluate is refused here
-  // (MJPC_B200_ERR_UNSUPPORTED) rather than at the first update, and Resets again.
-  int InitializeBase(const mjpc_model_blob* model, int sensor_start, int nsensor, double timestep, int device);
-  // steps the first n rows of states_ [n][nq+nv] from ctrl [nu] and mocap (NULL: the model's) at `time`, each
-  // warm-started from qacc_warmstart_, into fnext_ / fsensor_ / fqacc_ / counts_
-  int StepSensors(int n, const double* ctrl, const float* mocap);
-  // after a successful update: the warm start from row `centre` of the last launch, and that launch's warnings
-  void Commit(int centre);
-  // corr [ndstate] = X S^-1 innovation and P = P0 - X S^-1 X', symmetrised, for X [ndstate][nsensordata] and
-  // S [nsensordata]^2.  S is overwritten by its Cholesky factor and innovation by S^-1 innovation.  A factor that is
-  // not full rank: MJPC_B200_ERR_BAD_ARGUMENT with corr and P untouched.  P may alias P0.
-  int GainUpdate(const double* X, double* S, double* innovation, const double* P0, double* corr, double* P);
-  void Symmetrize(double* P) const;                                 // P [ndstate]^2 = (P + P') / 2
-  void StateAdd(double* x, const double* dx, double scale) const;   // x (+) scale dx: IntegratePos, velocities added
-
-  const char* name_;   // the prefix of every error message
+ private:
+  int Fail(int rc, const std::string& what);
   mjpc_b200_t* engine_ = nullptr;
   HostModel m_;
-  int sensor_start_ = 0, nsensor_ = 0, nmocap_ = 0, nstepped_ = 0;
-  std::vector<double> key_state_, qacc_warmstart_, states_;
-  std::vector<float> fstates_, fnext_, fsensor_, fqacc_, fwarm_, mocap0_;
-  std::vector<int> counts_;
+  int nmocap_ = 0;
+  std::vector<double> key_state_;
+  std::vector<float> mocap0_;
+  std::vector<float> fctrl_, fmocap_;   // [B][nu], [B][7 nmocap]: the inputs of the update being made
+  std::vector<float> ctrl_, mocap_;     // [B][nu], [B][7 nmocap]: those of each filter's last successful measurement
 };
-
-// mjpc_b200_estimator_t* is the Estimator base of the filter, whatever its kind
-inline mjpc_b200_estimator_t* ToHandle(Estimator* f) { return reinterpret_cast<mjpc_b200_estimator_t*>(f); }
-// the filter behind a handle if it is a T, else nullptr (a NULL handle, or one of another kind)
-template <class T>
-T* EstimatorOf(mjpc_b200_estimator_t* h) { return dynamic_cast<T*>(reinterpret_cast<Estimator*>(h)); }
 
 }  // namespace mjpc_b200_host

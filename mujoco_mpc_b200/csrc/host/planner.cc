@@ -23,22 +23,6 @@ void SubQuat(double* res, const double* qa, const double* qb) {   // qb * quat(r
   if (speed > M_PI) speed -= 2 * M_PI;
   for (int c = 0; c < 3; c++) res[c] = axis[c] * speed;
 }
-// mju_quatIntegrate: q * exp(scale v / 2), normalised
-void QuatIntegrate(double* q, const double* v, double scale) {
-  const double w[3] = {v[0] * scale, v[1] * scale, v[2] * scale};
-  const double a = std::sqrt(w[0] * w[0] + w[1] * w[1] + w[2] * w[2]);
-  double r[4] = {1, 0, 0, 0};
-  if (a >= 1e-15) {
-    const double s = std::sin(a / 2) / a;
-    r[0] = std::cos(a / 2); r[1] = s * w[0]; r[2] = s * w[1]; r[3] = s * w[2];
-  }
-  const double o[4] = {q[0] * r[0] - q[1] * r[1] - q[2] * r[2] - q[3] * r[3],
-                       q[0] * r[1] + q[1] * r[0] + q[2] * r[3] - q[3] * r[2],
-                       q[0] * r[2] - q[1] * r[3] + q[2] * r[0] + q[3] * r[1],
-                       q[0] * r[3] + q[1] * r[2] - q[2] * r[1] + q[3] * r[0]};
-  const double n = std::sqrt(o[0] * o[0] + o[1] * o[1] + o[2] * o[2] + o[3] * o[3]);
-  for (int k = 0; k < 4; k++) q[k] = o[k] / n;
-}
 }  // namespace
 
 int HostModel::Load(const mjpc_model_blob* blob) {
@@ -66,20 +50,6 @@ void StateDiff(const HostModel& m, double* dx, const double* x_to, const double*
     }
   }
   for (int i = 0; i < m.nv; i++) dx[m.nv + i] = x_to[m.nq + i] - x_from[m.nq + i];
-}
-
-void IntegratePos(const HostModel& m, double* qpos, const double* dq, double scale) {
-  for (size_t j = 0; j < m.jnt_type.size(); j++) {
-    const int a = m.jnt_qposadr[j], d = m.jnt_dofadr[j];
-    if (m.jnt_type[j] == 0) {
-      for (int c = 0; c < 3; c++) qpos[a + c] += scale * dq[d + c];
-      QuatIntegrate(qpos + a + 3, dq + d + 3, scale);
-    } else if (m.jnt_type[j] == 1) {
-      QuatIntegrate(qpos + a, dq + d, scale);
-    } else {
-      qpos[a] += scale * dq[d];
-    }
-  }
 }
 
 void FindInterval(int* b, const double* seq, double value, int length) {
@@ -142,11 +112,6 @@ int CholFactor(double* M, int n, double mindiag) {
     }
   }
   return rank;
-}
-
-void CholSolve(const double* L, int n, double* x) {
-  for (int i = 0; i < n; i++) { double a = x[i]; for (int k = 0; k < i; k++) a -= L[(size_t)i * n + k] * x[k]; x[i] = a / L[(size_t)i * n + i]; }
-  for (int i = n - 1; i >= 0; i--) { double a = x[i]; for (int k = i + 1; k < n; k++) a -= L[(size_t)k * n + i] * x[k]; x[i] = a / L[(size_t)i * n + i]; }
 }
 
 }  // namespace mjpc_b200_host

@@ -1,7 +1,7 @@
 // planner.h - the interface every host planner implements (the reference's virtual Planner,
 // mjpc/planners/planner.h:33-77, limited to what exists here) and the engine plumbing they share: the engine handle,
-// the planning state, the spline launch and the trajectory fetch.  Also the host maths the planners and the
-// estimators share: the Cholesky factor, FindInterval and the host model's state arithmetic.
+// the planning state, the spline launch and the trajectory fetch.  Also the host maths the planners share: the Cholesky
+// factor, FindInterval and the host model's state difference.
 #pragma once
 #include <cstdint>
 #include <vector>
@@ -21,8 +21,6 @@ struct Trajectory {                                   // mjpc/trajectory.h:74-86
 // mju_cholFactor: in-place lower Cholesky factor of the row-major n x n matrix M (upper triangle left as it was); a
 // pivot below mindiag is raised to mindiag.  Returns the rank, the number of pivots that were not raised.
 int CholFactor(double* M, int n, double mindiag);
-// mju_cholSolve: x = (L L')^-1 x with the factor of CholFactor
-void CholSolve(const double* L, int n, double* x);
 
 // FindInterval (mjpc/utilities.cc:303-330): the indices of the entries of a non-decreasing sequence around `value`,
 // clamped to the sequence
@@ -36,8 +34,6 @@ struct HostModel {             // the few mjModel fields the host-side state ari
 };
 // StateDiff (utilities.cc:543-553): dx [2 nv] = x_to (-) x_from, positions in the tangent space (mj_differentiatePos)
 void StateDiff(const HostModel& m, double* dx, const double* x_to, const double* x_from);
-// mj_integratePos: qpos (+) scale dq, quaternions through mju_quatIntegrate (q exp(scale v / 2), normalised)
-void IntegratePos(const HostModel& m, double* qpos, const double* dq, double scale);
 
 // MakeDifferentiable while planning, restored afterwards (agent.cc:296-309,346-356)
 struct DifferentiableScope {

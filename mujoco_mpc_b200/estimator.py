@@ -123,8 +123,8 @@ def differentiate_pos(m, q1, q2):
 
 def principal_eigenvector4(K, reference):
     """Principal eigenvector of a symmetric 4 x 4 matrix by cyclic Jacobi rotations, converged to rounding, with the
-    sign that agrees with `reference` (stands for PrincipalEigenVector4, utilities.cc:1476+; the C++ filter runs the
-    same rotations)."""
+    sign that agrees with `reference` (stands for PrincipalEigenVector4, utilities.cc:1476+; the device filters run
+    the same rotations)."""
     A = np.array(K, float)
     V = np.eye(4)
     for _ in range(50):
@@ -419,8 +419,9 @@ class _CppFilter(_CppObject):
 
 
 class CppUnscented(_CppFilter):
-    """The C++ filter (csrc/host/unscented.{h,cc}, mjpc_b200_unscented_create) behind the same attributes as Unscented;
-    settings resolve from the model's numerics exactly as Unscented's do."""
+    """The C++ filter (mjpc_b200_unscented_create: csrc/host/estimator.{h,cc}, a one-filter bank whose arithmetic runs
+    on the device) behind the same attributes as Unscented; settings resolve from the model's numerics exactly as
+    Unscented's do."""
     _nscalars = 5
 
     def __init__(self, m, sensor_start=None, nsensor=None, timestep=None, alpha=None, beta=None, device=0):
@@ -511,9 +512,9 @@ class Kalman(_Filter):
 
 
 class CppKalman(_CppFilter):
-    """The C++ filter (csrc/host/kalman.{h,cc}, mjpc_b200_kalman_*) behind the same attributes as Kalman; settings
-    resolve from the model's numerics exactly as Kalman's do.  update is the generic one: the measurement, then the
-    prediction."""
+    """The C++ filter (mjpc_b200_kalman_*: csrc/host/estimator.{h,cc}, a one-filter bank whose arithmetic runs on the
+    device) behind the same attributes as Kalman; settings resolve from the model's numerics exactly as Kalman's do.
+    update is the generic one: the measurement, then the prediction."""
     _nscalars = 6
 
     def __init__(self, m, sensor_start=None, nsensor=None, timestep=None, epsilon=KALMAN_EPSILON,
@@ -539,7 +540,7 @@ class CppKalman(_CppFilter):
 # ------------------------------------------------------------------------------------------------------ batched
 class CppBatchEstimator(_CppObject):
     """num_filters independent filters of one kind on one engine handle, every update on the device
-    (csrc/host/batch_estimator.{h,cc}, mjpc_b200_batch_estimator_*).  kind: "kalman" or "unscented"; settings resolve
+    (csrc/host/estimator.{h,cc}, mjpc_b200_batch_estimator_*).  kind: "kalman" or "unscented"; settings resolve
     from the model's numerics exactly as CppKalman's / CppUnscented's do.  Each filter starts as reset() leaves it.
     update returns the per-filter status (0, or MJPC_B200_ERR_BAD_ARGUMENT = -1 where a factorisation failed and the
     filter was left as it was); state / covariance / time / warnings take the filter index."""

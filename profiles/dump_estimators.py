@@ -5,9 +5,11 @@ and warnings after every update, and the error of a failed sensor-covariance fac
   python profiles/dump_estimators.py --cmp a.npz b.npz
 
 Filters: Unscented, Kalman centred and Kalman one-sided.  --backend oracle runs the Python mirrors on the fp64 CPU
-oracle (OracleSigmaBackend, no GPU); --backend engine runs CppUnscented / CppKalman and the Python mirrors on
-EngineBackend.  Scenes: the reference's particle1d and box3drot, task_imu, and the Quadruped filtering scenario of
-tests/quadruped_filtering.py.  The archive is written with fixed zip timestamps, so equal outputs give equal files.
+oracle (OracleSigmaBackend, no GPU); --backend engine runs CppUnscented / CppKalman, the Python mirrors on
+EngineBackend and a CppBatchEstimator of 3 filters with distinct start velocities, sensor noises and sensors (its
+failure path: filter 1's sensor noise negative, the statuses and every filter after the update).  Scenes: the
+reference's particle1d and box3drot, task_imu, and the Quadruped filtering scenario of tests/quadruped_filtering.py.
+The archive is written with fixed zip timestamps, so equal outputs give equal files.
 """
 import argparse
 import os
@@ -84,6 +86,29 @@ def record(out, key, f, m, X, Y, U, mocap, sensor_variance, updates):
     out[key + "/after_error"] = np.concatenate([f.state, f.covariance.ravel(), [f.time, f.warnings]])
 
 
+def record_batch(out, key, f, m, X, Y, U, mocap, sensor_variance, updates):
+    B = f.num_filters
+    var = 1e-4 if sensor_variance is None else sensor_variance
+    for b in range(B):
+        x0 = X[0].copy()
+        x0[m.nq:] += 1e-3 * b
+        f.reset(b, state=x0)
+        f.set_noise(b, sensor=np.full(f.nsensordata, var * (1 + b)))
+    mc = np.tile(mocap, (B, 1)) if mocap.size else None
+    S, P, T, W = [], [], [], []
+    for t in range(updates + 1):
+        if t == updates:   # the failure path: filter 1's sensor noise negative
+            f.set_noise(1, sensor=np.full(f.nsensordata, -1.0))
+        y = np.stack([Y[t] + 1e-4 * b for b in range(B)])
+        status = f.update(np.tile(U[t], (B, 1)), y, mc)
+        got = [f.get(b) for b in range(B)]
+        S.append([g[0] for g in got]); P.append([g[1] for g in got])
+        T.append([g[2] for g in got]); W.append([g[3][3] for g in got])
+    out[key + "/state"], out[key + "/covariance"] = np.array(S), np.array(P)
+    out[key + "/time"], out[key + "/warnings"] = np.array(T), np.array(W)
+    out[key + "/status_after_error"] = status
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("out", nargs="?")
@@ -106,13 +131,16 @@ def main():
                 record(out, "python/%s/%s" % (fname, name), f, m, X, Y, U, mocap, var, a.updates)
             continue
         from mujoco_mpc_b200.engine import Engine
-        from mujoco_mpc_b200.estimator import CppKalman, CppUnscented, EngineBackend
+        from mujoco_mpc_b200.estimator import CppBatchEstimator, CppKalman, CppUnscented, EngineBackend
         e = Engine(m, 2 * 2 * m.nv + 1, 8, device=0)
         for fname, cls, kw in kinds:
             f = cls(m, lambda s, n, ts: EngineBackend(e, s, n, ts), **kw)
             record(out, "python/%s/%s" % (fname, name), f, m, X, Y, U, mocap, var, a.updates)
             f = (CppUnscented if cls is Unscented else CppKalman)(m, **kw)
             record(out, "cpp/%s/%s" % (fname, name), f, m, X, Y, U, mocap, var, a.updates)
+            f.close()
+            f = CppBatchEstimator(m, "unscented" if cls is Unscented else "kalman", 3, **kw)
+            record_batch(out, "batch/%s/%s" % (fname, name), f, m, X, Y, U, mocap, var, a.updates)
             f.close()
         e.close()
     save(a.out, out)

@@ -5,7 +5,8 @@ B in {1, 8, 32, 64} filters.
 Per kind and B, in one process:
   * batched: the wall time of one `update` of all B filters (host clock around the call, which ends in a stream
     synchronise), median over the timed updates of a free-running run along the plant;
-  * single: the wall time of B `update`s of B single C++ filters (CppUnscented / CppKalman) over the same updates;
+  * single: the wall time of B `update`s of B single C++ filters (CppUnscented / CppKalman) over the same updates,
+    and of the first filter's alone (`update` returns the state: one update plus one state read);
   * kernels: in a separate profiled pass (torch.profiler, CUDA activities), the mean kernel time of each launch of one
     batched update by kernel name, and the launches of each name per update.
 The GPU's name and power limit are read in the same run.
@@ -55,26 +56,30 @@ def time_kind(m, kind, B, X, Y, U, updates, warmup):
     for s in singles:
         s.reset(state=X[0])
         s.set_noise(sensor=np.full(s.nsensordata, SENSOR_SD ** 2))
-    batch_ms, single_ms = [], []
+    batch_ms, single_ms, one_ms = [], [], []
     for t in range(warmup + updates):
         u, y, mcs = (np.tile(a, (B, 1)) for a in (U[t], Y[t], mc))
         t0 = time.perf_counter()
         status = f.update(u, y, mcs)
         t1 = time.perf_counter()
-        for s in singles:
+        singles[0].update(U[t], Y[t], mc)
+        t1a = time.perf_counter()
+        for s in singles[1:]:
             s.update(U[t], Y[t], mc)
         t2 = time.perf_counter()
         assert (status == 0).all()
         if t >= warmup:
             batch_ms.append((t1 - t0) * 1e3)
             single_ms.append((t2 - t1) * 1e3)
+            one_ms.append((t1a - t1) * 1e3)
     f.close()
     for s in singles:
         s.close()
     return dict(batched_update_ms_median=float(np.median(batch_ms)),
                 batched_update_ms_p90=float(np.percentile(batch_ms, 90)),
                 single_updates_ms_median=float(np.median(single_ms)),
-                single_updates_ms_p90=float(np.percentile(single_ms, 90)))
+                single_updates_ms_p90=float(np.percentile(single_ms, 90)),
+                one_single_update_and_state_ms_median=float(np.median(one_ms)))
 
 
 def kernel_times(m, kind, B, X, Y, U, updates):

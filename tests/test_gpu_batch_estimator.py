@@ -1,13 +1,13 @@
 """The batched Kalman and Unscented filters (mujoco_mpc_b200.estimator.CppBatchEstimator): B filters per update, the
 filter arithmetic in fp64 on the device, every filter's rows in one step launch per sigma-point set / Jacobian.
 
-Bars.  The device restates the single C++ filters' fp64 arithmetic in the host's summation order with every product
-rounded on its own, and its step rows are the single filter's rows, so from the same state, covariance, time, noise
-and warm start the two differ only where sin, cos or atan2 of a quaternion map differ in the last bits: the
-teacher-forced bar is the 1e-9 relative that test_cpp_filter_against_python_mirror holds two double-precision
-implementations of the same launches to.  Free running, every filter of the batch meets the RMS bars the existing GPU
-tests set for the single filter of its kind.  A filter's rows and its CTA read only its own inputs, so its results are
-bitwise the same at any position of any batch, and a failed factorisation leaves its filter bitwise unchanged.
+Bars.  The device restates the Python mirror filters' fp64 arithmetic (mujoco_mpc_b200.estimator.Unscented / Kalman)
+and its step rows are the rows the mirror steps through EngineBackend, so from the same state, covariance, time, noise
+and warm start the two are held to the 1e-9 relative that test_cpp_filter_against_python_mirror holds the single C++
+filters to.  Free running, every filter of the batch meets the RMS bars the existing GPU tests set for the single filter
+of its kind.  A filter's rows and its CTA read only its own inputs, so its results are bitwise the same at any position
+of any batch, a failed factorisation leaves its filter bitwise unchanged, and a single C++ filter, the bank of one, is
+bitwise the batch's filter given the same inputs.
 """
 import os
 import sys
@@ -20,13 +20,15 @@ from estimator_backends import OracleSigmaBackend, load_estimator_model, mocap_v
 from quadruped_filtering import SENSOR_SD, STEPS, plant, run_filter  # noqa: E402
 from test_kalman_cpu import load_task_imu  # noqa: E402
 
-from mujoco_mpc_b200.engine import EngineError  # noqa: E402
-from mujoco_mpc_b200.estimator import CppBatchEstimator, CppKalman, CppUnscented, Kalman, Unscented  # noqa: E402
+from mujoco_mpc_b200.engine import Engine, EngineError  # noqa: E402
+from mujoco_mpc_b200.estimator import (CppBatchEstimator, CppKalman, CppUnscented, EngineBackend,  # noqa: E402
+                                       EstimatorError, Kalman, Unscented)
 
 pytestmark = pytest.mark.gpu
 
 KINDS = ["unscented", "kalman"]
 SINGLE = {"unscented": CppUnscented, "kalman": CppKalman}
+MIRROR = {"unscented": Unscented, "kalman": Kalman}
 BAD_ARGUMENT, BAD_BLOB, CAPACITY, UNSUPPORTED = -1, -2, -3, -5
 
 
@@ -54,17 +56,24 @@ def _tile(a, B):
     return np.tile(np.asarray(a, float).reshape(1, -1), (B, 1))
 
 
+def _relative(x, P, f):
+    """Largest relative differences of state x and covariance P from filter f's."""
+    return (np.max(np.abs(x - f.state)) / max(1.0, np.abs(f.state).max()),
+            np.max(np.abs(P - f.covariance)) / np.abs(f.covariance).max())
+
+
 @pytest.mark.parametrize("kind", KINDS)
 @pytest.mark.parametrize("name", ["box3drot", "task_imu", "quadruped"])
-def test_teacher_forced_against_the_single_filter(kind, name):
+def test_teacher_forced_against_the_python_mirror(kind, name):
     """Per update from an identical (state, covariance, time): each of 3 batched filters, fed its own state and its
-    own sensor noise, agrees with a single C++ filter of its kind to 1e-9 relative in state and covariance; time and
-    warnings are equal."""
+    own sensor noise, agrees with a Python mirror filter of its kind on EngineBackend to 1e-9 relative in state and
+    covariance; time and warnings are equal."""
     m, X, Y, U, T = _scenario(name)
     mc = mocap_vector(m)
     B = 3
     batch = CppBatchEstimator(m, kind, B)
-    singles = [SINGLE[kind](m) for _ in range(B)]
+    e = Engine(m, batch.rows, 8, device=0)
+    singles = [MIRROR[kind](m, lambda s, n, ts: EngineBackend(e, s, n, ts)) for _ in range(B)]
     for b, f in enumerate(singles):
         x0 = X[0].copy()
         x0[m.nq:] += 1e-3 * b            # each filter starts from its own velocity
@@ -82,19 +91,16 @@ def test_teacher_forced_against_the_single_filter(kind, name):
         for b, f in enumerate(singles):
             f.update(U[t], Y[t], mc)
             x, P, tb, sc = batch.get(b)
-            dx = np.max(np.abs(x - f.state)) / max(1.0, np.abs(f.state).max())
-            dP = np.max(np.abs(P - f.covariance)) / np.abs(f.covariance).max()
+            dx, dP = _relative(x, P, f)
             worst = max(worst, dx, dP)
             assert dx <= 1e-9 and dP <= 1e-9, (t, b, dx, dP)
             assert tb == f.time and int(sc[3]) == f.warnings
             assert np.array_equal(P, P.T)
-    print("%s %s: largest relative difference from the single filter %.3g" % (kind, name, worst))
+    print("%s %s: largest relative difference from the Python mirror %.3g" % (kind, name, worst))
     expected = [2 * m.nv, batch.rows, batch.nsensordata, 0, batch.timestep] + ([batch.epsilon] if kind == "kalman" else [])
     assert list(batch.get(0)[3][[0, 1, 2, 4]]) == [expected[i] for i in (0, 1, 2, 4)]
     assert batch.rows == (singles[0].nsigma if kind == "unscented" else singles[0].nstates)
-    for f in singles:
-        f.close()
-    batch.close()
+    batch.close(); e.close()
 
 
 @pytest.mark.parametrize("kind", KINDS)
@@ -103,7 +109,7 @@ def test_quadruped_filtering_free_running(kind):
     state, covariance, time and warm start on the device.  Every filter keeps its covariance symmetric and positive
     definite with no step warnings and meets the single filter's RMS bars (tests/test_gpu_estimator.py,
     tests/test_gpu_kalman.py: within 5 % of the fp32-oracle filter, for the Kalman filter widened by the fp32 / fp64
-    spread).  The largest per-step state difference from the single C++ filter is printed."""
+    spread).  A single C++ filter fed the same inputs equals filter 0 bitwise at every step."""
     m = _quadruped()
     X, Y, U = plant(m)
     mc = mocap_vector(m)
@@ -124,15 +130,17 @@ def test_quadruped_filtering_free_running(kind):
         batch.reset(b, state=X[0])
         batch.set_noise(b, sensor=np.full(batch.nsensordata, SENSOR_SD ** 2))
     eq, ev = [[] for _ in range(B)], [[] for _ in range(B)]
-    diff, asym, mineig = 0.0, 0.0, np.inf
+    asym, mineig = 0.0, np.inf
     for t in range(STEPS):
         status = batch.update(_tile(U[t], B), _tile(Y[t], B), _tile(mc, B))
         assert (status == 0).all(), (t, status)
         single.update(U[t], Y[t], mc)
         for b in range(B):
             x, P, tb, _ = batch.get(b)
+            if b == 0:
+                assert np.array_equal(x, single.state) and np.array_equal(P, single.covariance), t
+                assert tb == single.time and batch.warnings(0) == single.warnings, t
             eq[b].append(x[:m.nq] - X[t + 1, :m.nq]); ev[b].append(x[m.nq:] - X[t + 1, m.nq:])
-            diff = max(diff, float(np.abs(x - single.state).max()))
             asym = max(asym, float(np.abs(P - P.T).max()))
             mineig = min(mineig, float(np.linalg.eigvalsh(0.5 * (P + P.T)).min()))
             assert tb == pytest.approx((t + 1) * 0.005, abs=1e-12)
@@ -141,10 +149,65 @@ def test_quadruped_filtering_free_running(kind):
         rv = float(np.sqrt(np.mean(np.square(ev[b][50:]))))
         assert rq <= bar[0] and rv <= bar[1], (b, rq, rv, bar)
         assert batch.warnings(b) == 0
-    print("batched %s quadruped: RMS qpos %.4g qvel %.4g (bars %.4g %.4g); largest per-step state difference from the "
-          "single C++ filter %.3g" % (kind, rq, rv, bar[0], bar[1], diff))
+    print("batched %s quadruped: RMS qpos %.4g qvel %.4g (bars %.4g %.4g)" % (kind, rq, rv, bar[0], bar[1]))
     assert asym == 0.0 and mineig > 0
     single.close(); batch.close()
+
+
+@pytest.mark.parametrize("kind", KINDS)
+def test_single_filter_is_the_one_filter_bank(kind):
+    """A single C++ filter and a batch of one, given the same inputs, agree bitwise over 5 Quadruped updates.  The
+    Kalman filter's update_measurement and update_prediction, run separately, follow the Python mirror on EngineBackend
+    teacher-forced to 1e-9 relative, through a prediction straight after reset (the ctrl and mocap of the last
+    measurement are then zeros and the model's) and a prediction after a failed measurement (it steps with the last
+    successful measurement's ctrl and mocap)."""
+    m = _quadruped()
+    X, Y, U = plant(m)
+    mc = mocap_vector(m)
+    single, batch = SINGLE[kind](m), CppBatchEstimator(m, kind, 1)
+    noise = np.full(single.nsensordata, SENSOR_SD ** 2)
+    single.reset(state=X[0]); single.set_noise(sensor=noise)
+    batch.reset(0, state=X[0]); batch.set_noise(0, sensor=noise)
+    for t in range(5):
+        assert (batch.update(U[t][None], Y[t][None], mc[None]) == 0).all()
+        single.update(U[t], Y[t], mc)
+        x, P, tb, sc = batch.get(0)
+        assert np.array_equal(x, single.state) and np.array_equal(P, single.covariance), t
+        assert tb == single.time and int(sc[3]) == single.warnings, t
+    batch.close()
+    if kind == "unscented":
+        single.close()
+        return
+    e = Engine(m, single.nstates, 8, device=0)
+    py = Kalman(m, lambda s, n, ts: EngineBackend(e, s, n, ts))
+    for f in (py, single):
+        f.reset(state=X[0]); f.set_noise(sensor=noise)
+    worst = 0.0
+
+    def step(call, *args):
+        nonlocal worst
+        single.set(py.state, py.covariance, py.time)
+        getattr(py, call)(*args); getattr(single, call)(*args)
+        dx, dP = _relative(single.state, single.covariance, py)
+        worst = max(worst, dx, dP)
+        assert dx <= 1e-9 and dP <= 1e-9, (call, dx, dP)
+        assert single.time == py.time and single.warnings == py.warnings
+
+    step("update_prediction")                           # straight after reset
+    for t in range(3):
+        step("update_measurement", U[t], Y[t], mc)
+        step("update_prediction")
+    for f in (py, single):                              # a measurement that fails, then a prediction
+        f.set_noise(sensor=np.full(single.nsensordata, -1e9))
+        before = (f.state, f.covariance, f.time)
+        with pytest.raises(EstimatorError, match="sensor covariance factorisation"):
+            f.update_measurement(U[3], Y[3], mc)
+        assert np.array_equal(f.state, before[0]) and np.array_equal(f.covariance, before[1]) and f.time == before[2]
+        f.set_noise(sensor=noise)
+    step("update_prediction")
+    step("update_measurement", U[4], Y[4], mc)
+    print("Kalman measurement / prediction: largest relative difference from the Python mirror %.3g" % worst)
+    single.close(); e.close()
 
 
 def _inputs(m, X, Y, U, B, t, rng):

@@ -244,7 +244,7 @@ def test_kalman_create_refusals():
 
 
 def test_unscented_create_refusals():
-    """The Unscented filter's create refuses the same inputs as the Kalman filter's: both step the reset state once."""
+    """The Unscented filter's create refuses the same inputs as the Kalman filter's: both are one-filter banks."""
     _create_refusals("unscented", CppUnscented)
 
 
