@@ -351,7 +351,7 @@ int mjpc_b200_spec_words(const mjpc_model_blob* model, int* out, int capacity);
 int mjpc_b200_upload_spline_inputs(mjpc_b200_t* h, const float* state, double time, const float* mocap,
                                    const float* userdata, const float* knots, const double* knot_times, int interp,
                                    int P, int N, int H);
-int mjpc_b200_launch_resident(mjpc_b200_t* h);          /* async on the engine stream */
+int mjpc_b200_launch_resident(mjpc_b200_t* h);          /* async on the engine stream; refused after a set_options timestep change (upload again) */
 int mjpc_b200_sync(mjpc_b200_t* h);
 int mjpc_b200_read_returns(mjpc_b200_t* h, float* returns, uint8_t* failure, int* order);
 /* ---- Multi-GPU: ONE planning problem, its candidates sharded over the ranks of an NCCL communicator owned by the
@@ -384,6 +384,13 @@ float* mjpc_b200_device_returns(mjpc_b200_t* h);
  * mjpc_b200_host_spline_sample = TimeSpline::Sample (mjpc/spline/spline.cc:103-156), usable without a GPU. */
 void mjpc_b200_host_spline_sample(const double* times, const double* values, int P, int dim, int interp, double t,
                                   double* out);
+/* The step table a rollout launch builds per problem to place its policy in time, usable without a GPU: the rollout
+ * time times[t] (time0 plus t timesteps, accumulated in double as mj_step does), upper[t] = the first of the `count`
+ * non-decreasing absolute node times (spline knot times or the feedback policy's nominal times) above times[t], and
+ * frac[t] = the fraction of times[t] between nodes upper[t] - 1 and upper[t], in double rounded to float (0 when
+ * upper[t] is 0 or count).  The spline samples and FindInterval's bounds of every step follow from upper[t]. */
+void mjpc_b200_host_policy_intervals(const double* nodes, int count, double time0, double timestep, int H, double* times,
+                                     int* upper, float* frac);
 double mjpc_b200_host_philox_normal(uint32_t seed, uint32_t iteration, uint32_t candidate, uint32_t knot, uint32_t dof);
 
 /* ---- Planners (csrc/host/planner.h, the reference's Planner interface mjpc/planners/planner.h:33-77).  Each kind has

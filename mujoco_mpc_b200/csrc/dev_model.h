@@ -132,6 +132,7 @@ struct ModelPack {
   std::vector<float> f;
   std::vector<int> i;
   std::vector<double> key_mpos, key_mquat, qpos0;
+  double timestep = 0;   // opt.timestep in double: the rollout clock of the policy step table (M.timestep is its fp32)
 };
 
 inline ModelPack pack_model(const void* data, size_t nbytes, int maxcon, int maxefc) {
@@ -152,7 +153,8 @@ inline ModelPack pack_model(const void* data, size_t nbytes, int maxcon, int max
   M.maxcon = maxcon + 2 * M.ntendon; M.maxefc = maxefc;
   M.residual_id = b.i("task_residual_id"); M.num_residual = b.i("task_num_residual");
   M.num_term = b.i("task_num_term"); M.num_trace = b.i("task_num_trace");
-  M.timestep = (float)b.r("opt_timestep"); M.impratio = (float)b.r("opt_impratio");
+  P.timestep = b.r("opt_timestep");
+  M.timestep = (float)P.timestep; M.impratio = (float)b.r("opt_impratio");
   M.tolerance = (float)b.r("opt_tolerance"); M.ls_tolerance = (float)b.r("opt_ls_tolerance");
   M.meaninertia = (float)b.r("stat_meaninertia"); M.risk = (float)b.r("task_risk");
   auto g = b.reals("opt_gravity");

@@ -107,6 +107,18 @@ __device__ __noinline__ float k_cost_value(Ctx& c) {
   return expm1f(CM(c).risk * cost) / CM(c).risk;
 }
 
+// ------------------------------------------------------------------------------------------ policy time
+// Where step t of a rollout sits among a problem's policy nodes (spline knot times, or the feedback policy's nominal
+// times), decided as the reference decides it: the rollout time T[0] = time0, T[t+1] = T[t] + timestep accumulated in
+// double (mj_step's d->time += h), and std::upper_bound over the absolute node times in double.  The decision is the
+// same for every candidate of a problem, so the host builds one row of H entries per problem and launch
+// (build_policy_intervals, engine.cu) and the kernels read step t's entry instead of searching in fp32.
+struct __align__(16) PolicyInterval {
+  double time;   // T[t], absolute: the rollout's recorded time of step t
+  int upper;     // first node with node time > T[t] (upper_bound), 0 .. count
+  float frac;    // (T[t] - node[upper-1]) / (node[upper] - node[upper-1]) in double, rounded; 0 outside the nodes
+};
+
 // ------------------------------------------------------------------------------------------ spline policy
 __device__ __forceinline__ float spline_slope(const float* times, const float* values, int P, int dim, int node, int k) {
   if (node == 0) return (values[dim + k] - values[k]) / (times[1] - times[0]);
@@ -114,15 +126,13 @@ __device__ __forceinline__ float spline_slope(const float* times, const float* v
   return 0.5f * (values[(node + 1) * dim + k] - values[node * dim + k]) / (times[node + 1] - times[node]) +
          0.5f * (values[node * dim + k] - values[(node - 1) * dim + k]) / (times[node] - times[node - 1]);
 }
+// TimeSpline::Sample at the step whose interval is (upper, t); times are the knot times relative to the rollout start
 __device__ __forceinline__ float spline_sample1(const float* times, const float* values, int P, int dim, int interp,
-                                                float time, int i) {
+                                                int upper, float t, int i) {
   if (P == 0) return 0.f;
-  int upper = 0;
-  while (upper < P && !(time < times[upper])) upper++;
   if (upper == P) return values[(P - 1) * dim + i];
   if (upper == 0) return values[i];
   const int lower = upper - 1;
-  const float t = (time - times[lower]) / (times[upper] - times[lower]);
   if (interp == 0) return values[lower * dim + i];
   if (interp == 1) return values[lower * dim + i] * (1 - t) + values[upper * dim + i] * t;
   const float dt = times[upper] - times[lower];
@@ -132,31 +142,31 @@ __device__ __forceinline__ float spline_sample1(const float* times, const float*
   const float m0 = spline_slope(times, values, P, dim, lower, i), m1 = spline_slope(times, values, P, dim, upper, i);
   return c0 * p0 + c1 * m0 + c2 * p1 + c3 * m1;
 }
-// ctrl <- clamp(spline(time)); one actuator per lane
+// ctrl <- clamp(spline(T[t])) with (upper, t) = the problem's PolicyInterval of step t; one actuator per lane
 // (out of line: the main warp and the task warp of a rollout CTA must evaluate it with the very same instructions)
 template <class SP>
-__device__ __noinline__ void k_policy_spline(Ctx& c, int P, int interp) {
+__device__ __noinline__ void k_policy_spline(Ctx& c, int P, int interp, int upper, float t) {
   auto&& M = SP::model(c);
   const float* range = MF(actuator_ctrlrange);
   for (int i = c.lane; i < M.nu; i += 32) {
-    float a = spline_sample1(DF(knot_times), DF(knots), P, M.nu, interp, c.time, i);
+    float a = spline_sample1(DF(knot_times), DF(knots), P, M.nu, interp, upper, t, i);
     DF(ctrl)[i] = fmaxf(range[2 * i], fminf(range[2 * i + 1], a));
   }
   __syncwarp();
 }
 
 // ------------------------------------------------------------------------------------------ iLQG policy
-// FindInterval (mjpc/utilities.h:125-144).  Rollout time is accumulated in fp32 on the device while the nominal
-// times arrive as (double - time0): a sample that is meant to coincide with a node may land one ulp below it, which
-// would shift a zero-order hold by a whole step.  Nodes within 1e-5 s above the query therefore count as reached.
+// FindInterval (mjpc/utilities.h:125-144) over the first `length` nodes, given the upper_bound `upper` over all of
+// them (PolicyInterval::upper; the nominal states have H nodes, the actions and gains the first H - 1)
+__device__ __forceinline__ void interval_bounds(int* b, int upper, int length) {
+  if (upper == 0) { b[0] = b[1] = 0; return; }
+  b[0] = min(upper - 1, length - 1); b[1] = min(upper, length - 1);
+}
+// FindInterval at a node's own time (the cubic slopes): exact in fp32, the node times are the same floats
 __device__ __forceinline__ void find_interval(int* b, const float* seq, float value, int length) {
   int upper = 0;
-  value += 1e-5f;
   while (upper < length && !(value < seq[upper])) upper++;
-  const int lower = upper - 1;
-  if (lower < 0) { b[0] = b[1] = 0; }
-  else if (lower > length - 1) { b[0] = b[1] = length - 1; }
-  else { b[0] = max(lower, 0); b[1] = min(upper, length - 1); }
+  interval_bounds(b, upper, length);
 }
 __device__ __forceinline__ float fd_slope(float x, const float* xs, const float* ys, int dim, int length, int i) {
   int b[2];
@@ -173,11 +183,12 @@ __device__ __forceinline__ float fd_slope(float x, const float* xs, const float*
   return 0.5f * (ys[dim * b[1] + i] - ys[dim * b[0] + i]) / (xs[b[1]] - xs[b[0]]) +
          0.5f * (ys[dim * b[0] + i] - ys[dim * (b[0] - 1) + i]) / (xs[b[0]] - xs[b[0] - 1]);
 }
-__device__ __forceinline__ float interp1(float x, const float* xs, const float* ys, int dim, int length, int rep, int i) {
+// Zero/Linear/CubicInterpolation (mjpc/utilities.cc:303-422) at the step whose interval is (upper, t)
+__device__ __forceinline__ float interp1(int upper, float t, const float* xs, const float* ys, int dim, int length, int rep,
+                                         int i) {
   int b[2];
-  find_interval(b, xs, x, length);
+  interval_bounds(b, upper, length);
   if (rep == 0 || b[0] == b[1]) return ys[dim * b[0] + i];
-  const float t = (x - xs[b[0]]) / (xs[b[1]] - xs[b[0]]);
   if (rep == 1) return ys[dim * b[0] + i] * (1 - t) + ys[dim * b[1] + i] * t;
   const float dt = xs[b[1]] - xs[b[0]];
   const float c0 = 2 * t * t * t - 3 * t * t + 1, c1 = (t * t * t - 2 * t * t + t) * dt, c2 = -2 * t * t * t + 3 * t * t,
@@ -202,7 +213,8 @@ struct FeedbackArgs {
   const float* t_nom;   // [B][H] relative to the problem's rollout start
   const float* gains;   // [B][H][nu][n]
   const float* du;      // [B][H][nu] or nullptr
-  int mode;             // 0/1/2 time-indexed, 3 step-indexed
+  const PolicyInterval* iv;   // [B][H]: step t's place among the problem's nominal times (modes 0/1/2)
+  int mode;            // 0/1/2 time-indexed, 3 step-indexed
   int H;
   int nper;             // candidates per problem: candidate `cand` follows problem cand / nper's policy
 };
@@ -221,17 +233,19 @@ __device__ __noinline__ void k_policy_feedback(Ctx& c, const FeedbackArgs& fa, f
   const float* gains = fa.gains + pH * nu * n;
   const float* du = fa.du ? fa.du + pH * nu : nullptr;
   float *xn = DF(xnom), *dx = DF(dx), *ctrl = DF(ctrl);
-  int rep = 0;
-  float scale = 1.f;
+  int rep = 0, upper = 0;
+  float scale = 1.f, t = 0.f;
   if (fa.mode == 3) {
     for (int i = lane; i < ds; i += 32) xn[i] = x_nom[index * ds + i];
     for (int i = lane; i < nu; i += 32) ctrl[i] = u_nom[index * nu + i] + (du ? step * du[index * nu + i] : 0.f);
   } else {
+    const PolicyInterval& iv = fa.iv[pH + index];
+    upper = iv.upper; t = iv.frac;
     int b[2];
-    find_interval(b, t_nom, c.time, H);
+    interval_bounds(b, upper, H);
     rep = (b[0] == b[1]) ? 0 : fa.mode;
-    for (int i = lane; i < ds; i += 32) xn[i] = interp1(c.time, t_nom, x_nom, ds, H, rep, i);
-    for (int i = lane; i < nu; i += 32) ctrl[i] = interp1(c.time, t_nom, u_nom, nu, H - 1, rep, i);
+    for (int i = lane; i < ds; i += 32) xn[i] = interp1(upper, t, t_nom, x_nom, ds, H, rep, i);
+    for (int i = lane; i < nu; i += 32) ctrl[i] = interp1(upper, t, t_nom, u_nom, nu, H - 1, rep, i);
     scale = step;
   }
   __syncwarp();
@@ -263,7 +277,7 @@ __device__ __noinline__ void k_policy_feedback(Ctx& c, const FeedbackArgs& fa, f
       const float* K = gains + ((size_t)index * nu + i) * n;
       for (int j = 0; j < n; j++) a += K[j] * dx[j];
     } else {
-      for (int j = 0; j < n; j++) a += interp1(c.time, t_nom, gains, nu * n, H - 1, rep, i * n + j) * dx[j];
+      for (int j = 0; j < n; j++) a += interp1(upper, t, t_nom, gains, nu * n, H - 1, rep, i * n + j) * dx[j];
     }
     const float u = ctrl[i] + scale * a;
     ctrl[i] = fmaxf(range[2 * i], fminf(range[2 * i + 1], u));

@@ -194,26 +194,43 @@ void rebase_task_state(const mjpc_b200* h, const double* src, double t0, float* 
   }
 }
 
-// floats of the per-problem block of stage_problems for B problems and P knots (knots excluded)
-size_t problem_floats(const DevModel& M, int B, int P) {
-  return (size_t)B * (2 + M.nq + M.nv + 7 * M.nmocap + M.task_state_size + M.num_term + M.num_parameters + P);
+// floats of the per-problem block of stage_problems for B problems, P knots and H steps (knots excluded)
+size_t problem_floats(const DevModel& M, int B, int P, int H) {
+  return (size_t)B * (4 * (size_t)H + M.nq + M.nv + 7 * M.nmocap + M.task_state_size + M.num_term + M.num_parameters + P);
+}
+
+// The policy step table of one problem (PolicyInterval, dev_task.cuh): T[0] = time0, T[t+1] = T[t] + timestep in double,
+// and for each step the upper_bound of T[t] over the `count` absolute node times, with the interval fraction in double.
+void build_policy_intervals(const double* nodes, int count, double time0, double timestep, int H, PolicyInterval* out) {
+  double time = time0;
+  for (int t = 0; t < H; t++) {
+    const int upper = (int)(std::upper_bound(nodes, nodes + count, time) - nodes);
+    double frac = 0;
+    if (upper > 0 && upper < count) frac = (time - nodes[upper - 1]) / (nodes[upper] - nodes[upper - 1]);
+    out[t].time = time; out[t].upper = upper; out[t].frac = (float)frac;
+    time += timestep;
+  }
 }
 
 // Stage the inputs of a rollout launch of B problems back to back in the pinned buffer and upload them with ONE copy
 // into d_in; point A's per-problem inputs at them.  Layout (floats):
-//   [time0: B doubles][state B x ds][mocap B x 7 nmocap][task_state B x size][weight B x num_term, if given]
+//   [step table B x H x 4][state B x ds][mocap B x 7 nmocap][task_state B x size][weight B x num_term, if given]
 //   [parameters B x num_parameters, if given][knot_times B x P][knots B x N x P x nu]   (knot blocks: spline launches)
-// A NULL task_states / weights / parameters stands for the handle's set_task values; the time-like task-state entries
-// and the knot times are made relative to each problem's own start time.  *end: the first h_in float after the block.
+// The step table of problem b is built from its start time times[b] and its `count` absolute policy nodes nodes[b]
+// (the knot times of a spline launch, the nominal times of a feedback launch).  A NULL task_states / weights /
+// parameters stands for the handle's set_task values; the time-like task-state entries and the knot times are made
+// relative to each problem's own start time.  *end: the first h_in float after the block.
 int stage_problems(mjpc_b200* h, int B, const float* states, const double* times, const float* mocaps,
-                   const double* weights, const double* parameters, const double* task_states, const float* knots,
-                   const double* knot_times, int P, int N, RolloutArgs* A, size_t* end) {
+                   const double* weights, const double* parameters, const double* task_states, const double* nodes,
+                   int count, int H, const float* knots, int N, RolloutArgs* A, size_t* end) {
   const DevModel& M = h->pack.M;
   const size_t ds = M.nq + M.nv, nm = 7 * (size_t)M.nmocap, nts = M.task_state_size, nw = M.num_term,
                np = M.num_parameters;
   float* in = h->h_in;
-  std::memcpy(in, times, (size_t)B * sizeof(double));
-  size_t o = 2 * (size_t)B;
+  PolicyInterval* iv = reinterpret_cast<PolicyInterval*>(in);
+  for (int b = 0; b < B; b++)
+    build_policy_intervals(nodes + (size_t)b * count, count, times[b], h->pack.timestep, H, iv + (size_t)b * H);
+  size_t o = 4 * (size_t)B * H;
   const size_t o_state = o; std::memcpy(in + o, states, B * ds * 4); o += B * ds;
   const size_t o_mocap = o; if (nm) std::memcpy(in + o, mocaps, B * nm * 4); o += B * nm;
   const size_t o_ts = o;
@@ -225,14 +242,15 @@ int stage_problems(mjpc_b200* h, int B, const float* states, const double* times
   const size_t o_kt = o;
   if (knots) {
     for (int b = 0; b < B; b++)
-      for (int k = 0; k < P; k++) in[o++] = (float)(knot_times[(size_t)b * P + k] - times[b]);
+      for (int k = 0; k < count; k++) in[o++] = (float)(nodes[(size_t)b * count + k] - times[b]);
   }
   const size_t o_k = o;
-  if (knots) { std::memcpy(in + o, knots, (size_t)B * N * P * M.nu * 4); o += (size_t)B * N * P * M.nu; }
+  if (knots) { std::memcpy(in + o, knots, (size_t)B * N * count * M.nu * 4); o += (size_t)B * N * count * M.nu; }
   CUDA_TRY(cudaMemcpyAsync(h->d_in, in, o * 4, cudaMemcpyHostToDevice, h->stream));
   float* d = h->d_in;
   A->nprob = B; A->nper = N;
-  A->time0 = reinterpret_cast<const double*>(d);
+  A->iv = reinterpret_cast<const PolicyInterval*>(d);
+  A->timestep = h->pack.timestep;
   A->state = d + o_state; A->mocap = d + o_mocap; A->task_state = d + o_ts;
   A->weight = weights ? d + o_w : nullptr; A->parameters = parameters ? d + o_p : nullptr;
   A->knot_times = knots ? d + o_kt : nullptr; A->knots = knots ? d + o_k : nullptr;
@@ -497,7 +515,7 @@ int mjpc_b200_create(const mjpc_model_blob* model, int max_candidates, int max_h
   }
   const size_t N = max_candidates, H = max_horizon, ds = M.nq + M.nv, n = 2 * M.nv, nu = M.nu, nr = M.num_residual;
   // launch inputs: up to max_candidates problems of one candidate each (stage_problems)
-  const size_t in_floats = problem_floats(M, max_candidates, h->maxP) + N * h->maxP * nu;
+  const size_t in_floats = problem_floats(M, max_candidates, h->maxP, max_horizon) + N * h->maxP * nu;
   CREATE_TRY(dalloc(&h->d_in, in_floats));
   CREATE_TRY(dalloc(&h->d_unom, H * nu)); CREATE_TRY(dalloc(&h->d_xnom, H * ds)); CREATE_TRY(dalloc(&h->d_tnom, H));
   CREATE_TRY(dalloc(&h->d_gains, H * nu * n)); CREATE_TRY(dalloc(&h->d_du, H * nu)); CREATE_TRY(dalloc(&h->d_steps, N));
@@ -583,6 +601,7 @@ int mjpc_b200_set_task(mjpc_b200_t* h, const mjpc_task_desc* task) {
 int mjpc_b200_set_options(mjpc_b200_t* h, double timestep, int integrator) {
   if (!h || !(timestep > 0)) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "set_options: bad argument");
   if (integrator != 0) return fail(MJPC_B200_ERR_UNSUPPORTED, "set_options: only the Euler integrator (0) is implemented");
+  h->pack.timestep = timestep;
   h->pack.M.timestep = (float)timestep;
   return 0;
 }
@@ -612,7 +631,8 @@ static int upload_spline(mjpc_b200_t* h, int B, const float* states, const doubl
   CUDA_TRY(cudaSetDevice(h->device));
   RolloutArgs A = base_args(h, B * N, H);
   size_t end;
-  if (int rc = stage_problems(h, B, states, times, mocaps, weights, parameters, task_states, knots, knot_times, P, N, &A, &end))
+  if (int rc = stage_problems(h, B, states, times, mocaps, weights, parameters, task_states, knot_times, P, H, knots, N, &A,
+                              &end))
     return rc;
   A.L = make_layout(h->pack.M, P);
   A.P = P; A.interp = interp; A.policy_kind = 0;
@@ -646,6 +666,9 @@ int mjpc_b200_rollout_spline_batched(mjpc_b200_t* h, int B, const float* states,
 int mjpc_b200_launch_resident(mjpc_b200_t* h) {
   if (!h || !h->resident_ok) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "launch_resident: no uploaded inputs");
   CUDA_TRY(cudaSetDevice(h->device));
+  // the step table was built on the upload's clock; a set_options timestep since then needs a new upload
+  if (h->resident.timestep != h->pack.timestep)
+    return fail(MJPC_B200_ERR_BAD_ARGUMENT, "launch_resident: the timestep changed since the upload");
   h->resident.M = h->pack.M;  // picks up set_task changes (risk)
   return launch_rollout(h, h->resident);
 }
@@ -690,10 +713,10 @@ static int rollout_feedback_impl(mjpc_b200_t* h, int B, const float* states, con
   CUDA_TRY(cudaSetDevice(h->device));
   const size_t ds = M.nq + M.nv, n = 2 * M.nv, nu = M.nu, Hs = H, P = B;
   if (int rc = reserve_feedback(h, B)) return rc;
-  if (int rc = reserve_h_in(h, problem_floats(M, B, 0) + P * Hs * (nu + ds + 1 + nu * n + nu) + P * K + 64)) return rc;
+  if (int rc = reserve_h_in(h, problem_floats(M, B, 0, H) + P * Hs * (nu + ds + 1 + nu * n + nu) + P * K + 64)) return rc;
   RolloutArgs A = base_args(h, B * K, H);
   size_t o;
-  if (int rc = stage_problems(h, B, states, times, mocaps, weights, parameters, task_states, nullptr, nullptr, 0, K, &A, &o))
+  if (int rc = stage_problems(h, B, states, times, mocaps, weights, parameters, task_states, t_nom, H, H, nullptr, K, &A, &o))
     return rc;
   auto put = [&](const float* src, size_t cnt) { size_t at = o; if (src) std::memcpy(h->h_in + o, src, cnt * 4); o += cnt; return at; };
   const size_t ou = put(u_nom, P * Hs * nu), ox = put(x_nom, P * Hs * ds);
@@ -710,7 +733,7 @@ static int rollout_feedback_impl(mjpc_b200_t* h, int B, const float* states, con
   A.L = make_layout(h->pack.M, 1);
   A.P = 1; A.policy_kind = 1;
   A.fb.u_nom = h->d_unom; A.fb.x_nom = h->d_xnom; A.fb.t_nom = h->d_tnom; A.fb.gains = h->d_gains;
-  A.fb.du = du ? h->d_du : nullptr; A.fb.mode = mode; A.fb.H = H; A.fb.nper = K;
+  A.fb.du = du ? h->d_du : nullptr; A.fb.iv = A.iv; A.fb.mode = mode; A.fb.H = H; A.fb.nper = K;
   A.step_sizes = h->d_steps;
   h->resident_ok = false;
   int rc = launch_rollout(h, A);
@@ -738,6 +761,13 @@ int mjpc_b200_rollout_feedback_batched(mjpc_b200_t* h, int B, const float* state
     return fail(MJPC_B200_ERR_BAD_ARGUMENT, "rollout_feedback_batched: null pointer");
   return rollout_feedback_impl(h, B, states, times, mocaps, weights, parameters, task_states, u_nom, x_nom, t_nom, gains,
                                du, step_sizes, mode, K, H, returns, failure, order);
+}
+
+void mjpc_b200_host_policy_intervals(const double* nodes, int count, double time0, double timestep, int H, double* times,
+                                     int* upper, float* frac) {
+  std::vector<PolicyInterval> iv(std::max(H, 0));
+  build_policy_intervals(nodes, count, time0, timestep, H, iv.data());
+  for (int t = 0; t < H; t++) { times[t] = iv[t].time; upper[t] = iv[t].upper; frac[t] = iv[t].frac; }
 }
 
 static int fetch_impl(mjpc_b200_t* h, int first, int count, float* states, float* actions, double* times,
@@ -1100,11 +1130,21 @@ static int model_derivatives_impl(mjpc_b200_t* h, int B, const float* x, const f
   CUDA_TRY(cudaSetDevice(h->device));
   const size_t nts = M.task_state_size;
   std::vector<float> ts((size_t)B * nts), trel((size_t)B * H);
-  // derivative sweeps use absolute-time task state rebased to each problem's own t[0]
+  // derivative sweeps use absolute-time task state rebased to each problem's own t[0].  A time on a rollout's clock
+  // (t[0] plus i timesteps in double: what rollouts record) is evaluated at that rollout step's fp32 relative time,
+  // the sum of i fp32 timesteps the residuals of the rollout read, so that the Jacobians belong to the trajectory's own
+  // residuals; any other time at its rounded offset from t[0].
+  const float h32 = M.timestep;
   for (int b = 0; b < B; b++) {
     const double t0 = t[(size_t)b * H];
     rebase_task_state(h, task_states ? task_states + b * nts : nullptr, t0, ts.data() + b * nts);
-    for (int i = 0; i < H; i++) trel[(size_t)b * H + i] = (float)(t[(size_t)b * H + i] - t0);
+    double clock = t0;
+    float clock32 = 0.f;
+    for (int i = 0; i < H; i++) {
+      const double ti = t[(size_t)b * H + i];
+      trel[(size_t)b * H + i] = ti == clock ? clock32 : (float)(ti - t0);
+      clock += h->pack.timestep; clock32 += h32;
+    }
   }
   const std::vector<float> w = to_float(weights, (size_t)B * M.num_term), p = to_float(parameters, (size_t)B * M.num_parameters);
   const size_t smem = h->smem_bytes(1, 1);

@@ -25,7 +25,6 @@ struct RolloutArgs {
   DevLayout L;
   const float* pack;        // device: nf floats followed by ni ints
   int nprob, nper;
-  const double* time0;      // [nprob] absolute start time of each problem
   const float* state;       // [nprob][dim_state]
   const float* mocap;       // [nprob][7*nmocap]
   const float* task_state;  // [nprob][task_state_size] (times rebased to the problem's start) or nullptr
@@ -33,6 +32,8 @@ struct RolloutArgs {
   const float* parameters;  // [nprob][num_parameters] or nullptr (the packed Task::parameters)
   const float* knots;       // [N][P][nu]
   const float* knot_times;  // [nprob][P], relative to the problem's start
+  const PolicyInterval* iv; // [nprob][H]: each step's absolute time and its place among the policy's nodes
+  double timestep;          // the step table's clock step in double: the recorded times accumulate it
   FeedbackArgs fb;
   const float* step_sizes;  // [N] for the feedback policy
   int policy_kind;          // 0 spline, 1 feedback
@@ -181,6 +182,7 @@ __device__ __noinline__ void task_warp_loop(Ctx& c, const RolloutArgs& A, int ca
   c.xfrc_on = A.xfrc_std > 0.f ? 1 : 0;
   float* o_res = A.residual + (size_t)cand * H * nr;
   float* o_trace = A.trace + (size_t)cand * H * ntr;
+  const PolicyInterval* iv = A.iv + (size_t)(cand / A.nper) * H;
 #ifdef MJPC_PHASE_TIMING
   long long fork_cycles = 0;   // timer mapping 2: this warp's fork intervals, reported by the main warp
 #endif
@@ -188,6 +190,11 @@ __device__ __noinline__ void task_warp_loop(Ctx& c, const RolloutArgs& A, int ca
     const bool last = t == H - 1;
     task_bar();   // fork (the main warp has written the state, the action and the poses of step t)
     if (wide_box().task_exit) return;
+    // step t+1's interval (the last step's twice), issued here, right after the fork, so that the load has landed by
+    // the end of the step where the spline reads it
+    int next_upper, next_frac_bits;
+    asm volatile("ld.global.nc.v2.s32 {%0, %1}, [%2];" : "=r"(next_upper), "=r"(next_frac_bits) : "l"(&iv[min(t + 1, H - 1)].upper));
+    const float next_frac = __int_as_float(next_frac_bits);
 #ifdef MJPC_PHASE_TIMING
     const long long t_fork = clock64();
 #endif
@@ -206,7 +213,7 @@ __device__ __noinline__ void task_warp_loop(Ctx& c, const RolloutArgs& A, int ca
     if (lane == 0) { wide_box().task_cost = cost; wide_box().task_warn = c.warn; }   // (a residual can raise a warning)
     if (!last) {
       c.time += CM(c).timestep;   // the same sum k_euler forms on the main warp
-      if (A.policy_kind == 0 && t + 1 < H - 1) k_policy_spline<SP>(c, A.P, A.interp);
+      if (A.policy_kind == 0 && t + 1 < H - 1) k_policy_spline<SP>(c, A.P, A.interp, next_upper, next_frac);
     }
     task_bar();   // join 2
   }
@@ -229,9 +236,9 @@ __device__ __forceinline__ void rollout_body(const RolloutArgs& A) {
   if constexpr (SP::kWide > 1) pair_sync_init(c, A.pair_sync, A.pair_sync_mode);
   auto&& M = SP::model(c);
   const int nq = M.nq, nv = M.nv, nu = M.nu, ds = nq + nv, nr = M.num_residual, ntr = 3 * M.num_trace, H = A.H;
-  // this candidate's problem: its inputs are resolved here, the step loop below only sees Ctx, time0 and the outputs
+  // this candidate's problem: its inputs are resolved here, the step loop below only sees Ctx, the step table and the outputs
   const int prob = cand / A.nper;
-  const double time0 = A.time0[prob];
+  const PolicyInterval* iv = A.iv + (size_t)prob * A.H;
   const float* state = A.state + (size_t)prob * ds;
   const float* mocap = A.mocap + (size_t)prob * 7 * M.nmocap;
   // the problem's task snapshot (task state time-rebased) overrides the packed copy.  With a task warp this happens
@@ -266,7 +273,11 @@ __device__ __forceinline__ void rollout_body(const RolloutArgs& A) {
   float* o_costs = A.costs + (size_t)cand * H;
   float* o_trace = A.trace + (size_t)cand * H * ntr;
   for (int i = lane; i < ds; i += 32) o_states[i] = state[i];
-  if (lane == 0) o_times[0] = time0;
+  // T[t], the reference's rollout clock, accumulated in double as the step table's (c.time is its fp32 relative twin)
+  double time = iv[0].time;
+  if (lane == 0) o_times[0] = time;
+  int next_upper = iv[0].upper;   // the spline's interval of the coming step
+  float next_frac = iv[0].frac;
   float total = 0.f;
   bool failed = false;
   const long long clk0 = clock64();
@@ -276,7 +287,12 @@ __device__ __forceinline__ void rollout_body(const RolloutArgs& A) {
     if ((c.sync_mode & 1) && (t & (c.sync_mode >> 4)) == 0) pair_sync_meet(c, 2 * t);   // bits 4..: step mask (0 = every step)
     // (with a task warp the spline action of step t > 0 was evaluated by it during step t-1's constraint solve)
     if (!last) {
-      if (A.policy_kind == 0) { if (!kTask || t == 0) k_policy_spline<SP>(c, A.P, A.interp); }
+      if (A.policy_kind == 0) {
+        const int upper = next_upper;
+        const float frac = next_frac;
+        if (!kTask) { next_upper = iv[t + 1].upper; next_frac = iv[t + 1].frac; }   // read a step ahead
+        if (!kTask || t == 0) k_policy_spline<SP>(c, A.P, A.interp, upper, frac);
+      }
       else k_policy_feedback<SP>(c, A.fb, step_size, t, cand);
     }
     // action record (the last row repeats the previous action; H == 1 -> zeros; trajectory.cc:190-196)
@@ -343,7 +359,8 @@ __device__ __forceinline__ void rollout_body(const RolloutArgs& A) {
     k_euler<SP>(c);
     for (int i = lane; i < nq; i += 32) o_states[(size_t)(t + 1) * ds + i] = DF(qpos)[i];
     for (int i = lane; i < nv; i += 32) o_states[(size_t)(t + 1) * ds + nq + i] = DF(qvel)[i];
-    if (lane == 0) o_times[t + 1] = time0 + (double)c.time;
+    time += A.timestep;
+    if (lane == 0) o_times[t + 1] = time;
   }
   pair_sync_done(c);
   wide_settle<SP>(c);

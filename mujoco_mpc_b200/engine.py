@@ -45,7 +45,8 @@ EXPORTS = ["mjpc_b200_version", "mjpc_b200_last_error", "mjpc_b200_create", "mjp
            "mjpc_b200_fetch_stats", "mjpc_b200_launch_count", "mjpc_b200_last_kernel_ms", "mjpc_b200_last_kernel_static",
            "mjpc_b200_spec_words", "mjpc_b200_upload_spline_inputs",
            "mjpc_b200_launch_resident", "mjpc_b200_sync", "mjpc_b200_read_returns", "mjpc_b200_stream",
-           "mjpc_b200_device_returns", "mjpc_b200_host_spline_sample", "mjpc_b200_host_philox_normal",
+           "mjpc_b200_device_returns", "mjpc_b200_host_spline_sample", "mjpc_b200_host_policy_intervals",
+           "mjpc_b200_host_philox_normal",
            "mjpc_b200_planner_destroy", "mjpc_b200_planner_reset", "mjpc_b200_planner_set_state",
            "mjpc_b200_planner_optimize_policy", "mjpc_b200_planner_nominal_trajectory",
            "mjpc_b200_planner_action_from_policy", "mjpc_b200_planner_set_fd",
@@ -246,6 +247,17 @@ def host_ilqg_policy_action(model, u_nom, x_nom, t_nom, gains, representation, f
     if rc != 0:
         raise EngineError(f"host_ilqg_policy_action failed ({rc})")
     return out
+
+
+def host_policy_intervals(nodes, time0, timestep, H):
+    """The step table a rollout launch builds per problem (mjpc_b200_host_policy_intervals, no device): the rollout times
+    accumulated in double from time0, each step's upper_bound among the absolute node times, and the interval fraction."""
+    lib = load_library()
+    x = _d(nodes)
+    times, upper, frac = np.zeros(H), np.zeros(H, np.int32), np.zeros(H, np.float32)
+    lib.mjpc_b200_host_policy_intervals(_pd(x), len(x), C.c_double(time0), C.c_double(timestep), int(H), _pd(times),
+                                        upper.ctypes.data_as(C.POINTER(C.c_int)), _pf(frac))
+    return times, upper, frac
 
 
 def _f(a):

@@ -81,9 +81,11 @@ def test_no_contact_rollouts(engines, oracles, name):
     np.testing.assert_allclose(ret, r["returns"], rtol=1e-4)
     tr = e.fetch_all()
     np.testing.assert_allclose(tr["states"], r["states"], atol=2e-4)
-    np.testing.assert_allclose(tr["actions"], r["actions"], atol=2e-5)   # spline sampled at fp32-accumulated times
+    # each step's knot interval and fraction are chosen in double at the reference's rollout time
+    # (largest cubic-spline error measured 3e-7 on an H100; a step in the wrong interval moves an action far more)
+    np.testing.assert_allclose(tr["actions"], r["actions"], rtol=0, atol=1e-6 * (1 + np.abs(knots).max()))
     np.testing.assert_allclose(tr["residual"], r["residual"], atol=2e-4)
-    np.testing.assert_allclose(tr["times"], r["times"], atol=1e-5)
+    assert np.array_equal(tr["times"], r["times"])
     assert list(order) == list(np.argsort(r["returns"], kind="stable"))
 
 
