@@ -129,8 +129,16 @@ int mjpc_b200_rollout_spline_batched(mjpc_b200_t* h, int B, const float* states,
 /* NoisyRollout (mjpc/trajectory.cc:100-210, used by the Robust planner): the following rollouts of this handle add
  * Ornstein-Uhlenbeck noise to xfrc_applied of every body (stationary std xfrc_std, correlation time xfrc_rate
  * seconds), drawn from Philox4x32-10 with key (seed, 1) and counter (step, candidate, element, 'XFRC') - the
- * reference's absl::BitGen cannot be seeded.  xfrc_std = 0 switches the noise off (the default). */
+ * reference's absl::BitGen cannot be seeded.  xfrc_std = 0 switches the noise off (the default).  Clears the
+ * per-problem keys of set_xfrc_noise_batched. */
 int mjpc_b200_set_xfrc_noise(mjpc_b200_t* h, double xfrc_std, double xfrc_rate, uint32_t seed);
+
+/* The same noise with one key per problem: the following rollout launches must hold exactly B problems (a launch of
+ * another B returns MJPC_B200_ERR_BAD_ARGUMENT and leaves the handle usable; a single-problem launch is B = 1), and
+ * problem b draws with key seeds[b] and its problem-local candidate index as the counter - bitwise what a launch of
+ * problem b alone draws after set_xfrc_noise(seeds[b]).  seeds [B].  mjpc_b200_rollout_spline_sharded refuses
+ * per-problem keys (MJPC_B200_ERR_UNSUPPORTED); set_xfrc_noise clears them. */
+int mjpc_b200_set_xfrc_noise_batched(mjpc_b200_t* h, double xfrc_std, double xfrc_rate, int B, const uint32_t* seeds);
 
 /* K line-search rollouts of the iLQG policy. u_nom [H][nu], x_nom [H][dim_state], t_nom [H] (absolute),
  * gains [H][nu][dim_dstate], du [H][nu] (may be NULL), step_sizes [K]. */
@@ -420,6 +428,8 @@ int mjpc_b200_planner_nominal_trajectory(mjpc_b200_planner_t* p, int horizon);
 int mjpc_b200_planner_action_from_policy(mjpc_b200_planner_t* p, double* action, const double* state, double time,
                                          int use_previous);
 int mjpc_b200_planner_set_fd(mjpc_b200_planner_t* p, double tolerance, int mode, int derivative_skip);
+/* mjpc_b200_set_task on every engine handle the planner plans on (the task snapshot Agent gives it per iteration) */
+int mjpc_b200_planner_set_task(mjpc_b200_planner_t* p, const mjpc_task_desc* task);
 
 /* ---- Predictive Sampling (csrc/host/sampling_planner.{h,cc}; mjpc/planners/sampling/planner.h:40-160). */
 int mjpc_b200_sampling_planner_create(const mjpc_model_blob* model, int num_trajectory, int num_spline_points,
@@ -448,9 +458,40 @@ int mjpc_b200_batch_planner_set_task(void* planner, int problem, const double* w
 int mjpc_b200_batch_planner_optimize_policy(void* planner, int horizon);   /* every problem: SamplingPlanner::OptimizePolicy */
 int mjpc_b200_batch_planner_action_from_policy(void* planner, int problem, double* action, double time, int use_previous);
 /* as mjpc_b200_sampling_planner_get_result for one problem (returns [num_trajectory]); returns the number of installed
- * knots */
+ * knots.  A batch of another kind: MJPC_B200_ERR_BAD_ARGUMENT */
 int mjpc_b200_batch_planner_get_result(void* planner, int problem, int* winner, double* improvement, float* returns,
                                        double* knots, double* knot_times);
+
+/* ---- Batched Cross-Entropy, Sample Gradient and Robust planners (csrc/host/batch_planner.{h,cc}): num_problems
+ * independent planners of one kind on ONE engine handle, with the arguments of the single planner's create plus
+ * num_problems and seeds [num_problems]; each problem's result equals that of the single planner with the same seed and
+ * inputs.  One rollout launch per iteration covers every problem's candidates (Cross-Entropy B x (N + 1), Sample
+ * Gradient B x N); the Robust planner makes a clean launch of B x N, then one noisy launch of
+ * B x ncandidates x nrepetitions on a second handle, each problem drawing its force noise with its own key
+ * seed + iteration (mjpc_b200_set_xfrc_noise_batched).  Settings are common to a batch.  reset / set_state / set_task /
+ * optimize_policy / action_from_policy / destroy are the mjpc_b200_batch_planner_* calls above; each _get_result reads
+ * one problem as the single planner's _get_result does, and returns MJPC_B200_ERR_BAD_ARGUMENT for a batch of another
+ * kind or a problem outside [0, num_problems). */
+int mjpc_b200_batch_ce_planner_create(const mjpc_model_blob* model, int num_problems, int num_trajectory, int n_elite,
+                                      int num_spline_points, int interpolation, double std_initial, double std_min,
+                                      double explore_fraction, double timestep, const double* ctrlrange,
+                                      const uint32_t* seeds, int max_horizon, int device, void** out);
+int mjpc_b200_batch_ce_planner_get_result(void* planner, int problem, double* improvement, float* returns, int* order,
+                                          double* knots, double* knot_times, double* variance);
+int mjpc_b200_batch_sg_planner_create(const mjpc_model_blob* model, int num_problems, int num_trajectory,
+                                      int num_gradient, int num_spline_points, int interpolation, double exploration,
+                                      double gradient_filter, double timestep, const double* ctrlrange,
+                                      const uint32_t* seeds, int max_horizon, int device, void** out);
+int mjpc_b200_batch_sg_planner_get_result(void* planner, int problem, int* winner, int* winner_type, double* improvement,
+                                          float* returns, int* order, double* knots, double* knot_times,
+                                          double* gradient_knots, double* gradient);
+int mjpc_b200_batch_robust_planner_create(const mjpc_model_blob* model, int num_problems, int num_trajectory,
+                                          int num_spline_points, int interpolation, double exploration, double timestep,
+                                          const double* ctrlrange, const uint32_t* seeds, int ncandidates,
+                                          int nrepetitions, double xfrc_std, double xfrc_rate, int max_horizon,
+                                          int device, void** out);
+int mjpc_b200_batch_robust_planner_get_result(void* planner, int problem, int* winner, double* scores, float* returns,
+                                              double* knots, double* knot_times);
 
 /* ---- Cross-Entropy planner (csrc/host/cross_entropy_planner.{h,cc}; mjpc/planners/cross_entropy/planner.h:35-146).
  * One rollout launch covers the N noisy candidates and the un-noised nominal (candidate N); the elite mean and

@@ -122,6 +122,7 @@ struct mjpc_b200 {
   int64_t launches = 0;
   float xfrc_std = 0.f, xfrc_rate = 1.f;   // NoisyRollout settings for the following rollouts (0 = off)
   unsigned noise_seed = 0;
+  std::vector<unsigned> noise_seeds;   // set_xfrc_noise_batched: one key per problem of the following launches (else empty)
   int last_static = 0;
   float last_ms = 0;
   // multi-GPU: one NCCL communicator per handle; the per-iteration exchange (all-gather of returns + failure flags)
@@ -196,7 +197,7 @@ void rebase_task_state(const mjpc_b200* h, const double* src, double t0, float* 
 
 // floats of the per-problem block of stage_problems for B problems, P knots and H steps (knots excluded)
 size_t problem_floats(const DevModel& M, int B, int P, int H) {
-  return (size_t)B * (4 * (size_t)H + M.nq + M.nv + 7 * M.nmocap + M.task_state_size + M.num_term + M.num_parameters + P);
+  return (size_t)B * (4 * (size_t)H + M.nq + M.nv + 7 * M.nmocap + M.task_state_size + M.num_term + M.num_parameters + P + 1);
 }
 
 // The policy step table of one problem (PolicyInterval, dev_task.cuh): T[0] = time0, T[t+1] = T[t] + timestep in double,
@@ -216,13 +217,19 @@ void build_policy_intervals(const double* nodes, int count, double time0, double
 // into d_in; point A's per-problem inputs at them.  Layout (floats):
 //   [step table B x H x 4][state B x ds][mocap B x 7 nmocap][task_state B x size][weight B x num_term, if given]
 //   [parameters B x num_parameters, if given][knot_times B x P][knots B x N x P x nu]   (knot blocks: spline launches)
+//   [noise keys B, if set_xfrc_noise_batched set them]
 // The step table of problem b is built from its start time times[b] and its `count` absolute policy nodes nodes[b]
 // (the knot times of a spline launch, the nominal times of a feedback launch).  A NULL task_states / weights /
 // parameters stands for the handle's set_task values; the time-like task-state entries and the knot times are made
-// relative to each problem's own start time.  *end: the first h_in float after the block.
+// relative to each problem's own start time.  *end: the first h_in float after the block.  Per-problem noise keys for
+// another number of problems are refused before anything is staged.
 int stage_problems(mjpc_b200* h, int B, const float* states, const double* times, const float* mocaps,
                    const double* weights, const double* parameters, const double* task_states, const double* nodes,
                    int count, int H, const float* knots, int N, RolloutArgs* A, size_t* end) {
+  if (!h->noise_seeds.empty() && (int)h->noise_seeds.size() != B)
+    return fail(MJPC_B200_ERR_BAD_ARGUMENT, "rollout: set_xfrc_noise_batched gave keys for " +
+                                                std::to_string(h->noise_seeds.size()) + " problems, the launch has " +
+                                                std::to_string(B));
   const DevModel& M = h->pack.M;
   const size_t ds = M.nq + M.nv, nm = 7 * (size_t)M.nmocap, nts = M.task_state_size, nw = M.num_term,
                np = M.num_parameters;
@@ -246,6 +253,8 @@ int stage_problems(mjpc_b200* h, int B, const float* states, const double* times
   }
   const size_t o_k = o;
   if (knots) { std::memcpy(in + o, knots, (size_t)B * N * count * M.nu * 4); o += (size_t)B * N * count * M.nu; }
+  const size_t o_seed = o;
+  if (!h->noise_seeds.empty()) { std::memcpy(in + o, h->noise_seeds.data(), (size_t)B * 4); o += B; }
   CUDA_TRY(cudaMemcpyAsync(h->d_in, in, o * 4, cudaMemcpyHostToDevice, h->stream));
   float* d = h->d_in;
   A->nprob = B; A->nper = N;
@@ -254,6 +263,7 @@ int stage_problems(mjpc_b200* h, int B, const float* states, const double* times
   A->state = d + o_state; A->mocap = d + o_mocap; A->task_state = d + o_ts;
   A->weight = weights ? d + o_w : nullptr; A->parameters = parameters ? d + o_p : nullptr;
   A->knot_times = knots ? d + o_kt : nullptr; A->knots = knots ? d + o_k : nullptr;
+  A->noise_seeds = h->noise_seeds.empty() ? nullptr : reinterpret_cast<const unsigned*>(d + o_seed);
   *end = o;
   return 0;
 }
@@ -953,6 +963,8 @@ int mjpc_b200_rollout_spline_sharded(mjpc_b200_t* h, const float* state, double 
                                      const float* userdata, const float* knots, const double* knot_times, int interp,
                                      int P, int N, int H, float* returns, uint8_t* failure, int* order) {
   if (!h || !knots) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "rollout_spline_sharded: null");
+  if (!h->noise_seeds.empty())
+    return fail(MJPC_B200_ERR_UNSUPPORTED, "rollout_spline_sharded: per-problem noise keys (set_xfrc_noise_batched)");
   if (h->nranks > 1 && !h->comm) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "rollout_spline_sharded: comm_init first");
   if (h->nranks == 1) {
     int rc = mjpc_b200_rollout_spline(h, state, time, mocap, userdata, knots, knot_times, interp, P, N, H, returns, failure, order);
@@ -1087,6 +1099,18 @@ int mjpc_b200_fetch_stats(mjpc_b200_t* h, int64_t* stats) {
 int mjpc_b200_set_xfrc_noise(mjpc_b200_t* h, double xfrc_std, double xfrc_rate, uint32_t seed) {
   if (!h || xfrc_std < 0 || !(xfrc_rate > 0)) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "set_xfrc_noise: bad argument");
   h->xfrc_std = (float)xfrc_std; h->xfrc_rate = (float)xfrc_rate; h->noise_seed = seed;
+  h->noise_seeds.clear();
+  h->resident_ok = false;
+  return MJPC_B200_OK;
+}
+
+// ... with one key per problem for the following launches of exactly B problems: problem b draws as a launch of it
+// alone after set_xfrc_noise(seeds[b]) does
+int mjpc_b200_set_xfrc_noise_batched(mjpc_b200_t* h, double xfrc_std, double xfrc_rate, int B, const uint32_t* seeds) {
+  if (!h || xfrc_std < 0 || !(xfrc_rate > 0) || B < 1 || !seeds)
+    return fail(MJPC_B200_ERR_BAD_ARGUMENT, "set_xfrc_noise_batched: bad argument");
+  h->xfrc_std = (float)xfrc_std; h->xfrc_rate = (float)xfrc_rate;
+  h->noise_seeds.assign(seeds, seeds + B);
   h->resident_ok = false;
   return MJPC_B200_OK;
 }

@@ -10,9 +10,10 @@ namespace mjpc_b200_host {
 
 int CrossEntropyPlanner::Initialize(const mjpc_model_blob* model, int num_trajectory, int n_elite, int num_spline_points,
                                     int interpolation, double std_initial, double std_min, double explore_fraction,
-                                    double timestep, const double* ctrlrange, uint32_t seed, int max_horizon, int device) {
+                                    double timestep, const double* ctrlrange, uint32_t seed, int max_horizon, int device,
+                                    mjpc_b200_t* engine) {
   // N noisy candidates + the nominal trajectory share one launch
-  if (int rc = AttachEngine(model, num_trajectory + 1, max_horizon, device)) return rc;
+  if (int rc = AttachEngine(model, num_trajectory + 1, max_horizon, device, engine)) return rc;
   nu_ = info_.nu;
   num_trajectory_ = num_trajectory;
   n_elite_ = n_elite > 0 ? n_elite : std::max(num_trajectory / 10, 2);   // planner.cc:69-71
@@ -68,11 +69,22 @@ void CrossEntropyPlanner::AddNoiseToPolicy(int i, double std_min) {
   }
 }
 
-int CrossEntropyPlanner::Rollouts(int num_trajectory, int horizon) {
+const SplineCandidates& CrossEntropyPlanner::PrepareCandidates(int horizon) {
+  resampled_policy.plan.SetInterpolation(interpolation_);
+  const int num_trajectory = num_trajectory_;
+  n_elite_ = std::min(n_elite_, num_trajectory);
+  {
+    const std::shared_lock<std::shared_mutex> lock(mtx_);
+    resampled_policy = policy;
+  }
+  resampled_policy.plan.SetInterpolation(interpolation_);
+  ResamplePolicy(horizon);
+  // Rollouts (:414-459): the N noisy candidates, then the nominal as candidate N (NominalTrajectory, :295-307)
   const int P = resampled_policy.plan.Size();
-  knots_.resize((size_t)(num_trajectory + 1) * P * nu_);
+  cands_.Resize(num_trajectory + 1, P, nu_);
+  cands_.interpolation = (int)interpolation_;
   for (int i = 0; i <= num_trajectory; i++) {
-    const SamplingPolicy* src = &resampled_policy;          // candidate N: the nominal (NominalTrajectory, :295-307)
+    const SamplingPolicy* src = &resampled_policy;
     if (i < num_trajectory) {
       const double std = i < num_trajectory * explore_fraction_ ? std_initial_ : std_min_;
       candidate_policy[i] = resampled_policy;
@@ -81,29 +93,32 @@ int CrossEntropyPlanner::Rollouts(int num_trajectory, int horizon) {
     }
     for (int k = 0; k < P; k++) {
       const double* node = src->plan.NodeValues(k);
-      for (int d = 0; d < nu_; d++) knots_[((size_t)i * P + k) * nu_ + d] = (float)node[d];
+      for (int d = 0; d < nu_; d++) cands_.knots[((size_t)i * P + k) * nu_ + d] = (float)node[d];
     }
   }
-  order_all_.resize(num_trajectory + 1);
-  return RolloutSpline(knots_.data(), times_scratch_.data(), (int)interpolation_, P, num_trajectory + 1, horizon,
-                       returns_.data(), failure_.data(), order_all_.data());
+  std::copy(times_scratch_.begin(), times_scratch_.begin() + P, cands_.knot_times.begin());
+  return cands_;
 }
 
 int CrossEntropyPlanner::OptimizePolicy(int horizon) {
-  resampled_policy.plan.SetInterpolation(interpolation_);
-  const int num_trajectory = num_trajectory_;
-  n_elite_ = std::min(n_elite_, num_trajectory);
-  const int n_elite = n_elite_;
-  {
-    const std::shared_lock<std::shared_mutex> lock(mtx_);
-    resampled_policy = policy;
+  const SplineCandidates& c = PrepareCandidates(horizon);
+  order_all_.resize(c.N);
+  if (RolloutSpline(c, horizon, returns_.data(), failure_.data(), order_all_.data())) return -1;
+  InstallRollouts(horizon, returns_.data(), failure_.data(), order_all_.data(), 0);
+  return 0;
+}
+
+void CrossEntropyPlanner::InstallRollouts(int horizon, const float* returns, const uint8_t* failure, const int* order,
+                                          int offset) {
+  const int num_trajectory = num_trajectory_, n_elite = n_elite_;
+  if (returns != returns_.data()) {
+    std::copy(returns, returns + num_trajectory + 1, returns_.begin());
+    std::copy(failure, failure + num_trajectory + 1, failure_.begin());
   }
-  resampled_policy.plan.SetInterpolation(interpolation_);
-  ResamplePolicy(horizon);
-  if (Rollouts(num_trajectory, horizon)) return -1;
+  launch_offset_ = offset; horizon_ = horizon;
   // the device ranked all N+1 launches; the elite ranking is over the N noisy candidates only (:181-193)
   int r = 0;
-  for (int i : order_all_) if (i < num_trajectory) trajectory_order[r++] = i;
+  for (int k = 0; k <= num_trajectory; k++) if (order[k] < num_trajectory) trajectory_order[r++] = order[k];
   const int P = resampled_policy.num_spline_points, num_parameters = P * nu_;
   std::vector<double> mean(num_parameters, 0.0);
   double avg_return = 0;
@@ -133,7 +148,6 @@ int CrossEntropyPlanner::OptimizePolicy(int horizon) {
   }
   improvement = std::max(avg_return - (double)returns_[trajectory_order[0]], 0.0);
   iteration++;
-  return 0;
 }
 
 void CrossEntropyPlanner::ActionFromPolicy(double* action, const double*, double time, bool use_previous) {

@@ -1,6 +1,6 @@
 // cross_entropy_planner.h - C++ host side of the Cross-Entropy Method planner with the reference's method names
 // (mjpc/planners/cross_entropy/planner.h:35-146, planner.cc:38-470).  Same rollout engine call as the sampling
-// planner: Rollouts() makes ONE mjpc_b200_rollout_spline call over N noisy candidates + the un-noised nominal
+// planner: Rollouts is ONE mjpc_b200_rollout_spline call over N noisy candidates + the un-noised nominal
 // (candidate N) where the reference schedules N+1 closures on its ThreadPool (planner.cc:414-459).
 // Noise comes from the injected Philox stream (sampling_planner.h), counter (iteration, candidate, knot, dof).
 #pragma once
@@ -12,15 +12,21 @@ class CrossEntropyPlanner : public Planner {
  public:
   // settings the reference reads from <custom> numerics (planner.cc:55-71): sampling_exploration (initial std),
   // std_min, explore_fraction, sampling_trajectories, n_elite (default max(N/10, 2))
+  // engine != nullptr: roll out on that handle (shared with other planners, not owned) instead of creating one
   int Initialize(const mjpc_model_blob* model, int num_trajectory, int n_elite, int num_spline_points, int interpolation,
                  double std_initial, double std_min, double explore_fraction, double timestep, const double* ctrlrange,
-                 uint32_t seed, int max_horizon, int device);
+                 uint32_t seed, int max_horizon, int device, mjpc_b200_t* engine = nullptr);
   void Reset(int horizon, const double* initial_repeated_action) override;   // :121-150 (variance = std_initial^2)
-  int OptimizePolicy(int horizon) override;           // :153-292
+  int OptimizePolicy(int horizon) override;           // :153-292: the two halves below around one launch
+  // ... before the launch: ResamplePolicy and the candidates of Rollouts (:414-459), the N noisy ones and the nominal
+  // last (N + 1 in all)
+  const SplineCandidates& PrepareCandidates(int horizon);
+  // ... after it: the launch's horizon, the returns, failure flags and ranking of these N + 1 candidates, which it held
+  // from flat index `offset` on; the elite ranking, mean and variance, the installed policy and improvement
+  void InstallRollouts(int horizon, const float* returns, const uint8_t* failure, const int* order, int offset);
   int NominalTrajectory(int) override { return 0; }   // not restated: planning disabled leaves the plan as it is
   void ResamplePolicy(int horizon);                   // :343-371
   void AddNoiseToPolicy(int i, double std_min);       // :374-411
-  int Rollouts(int num_trajectory, int horizon);      // :414-459
   // :331-340; the policy does not depend on the state
   void ActionFromPolicy(double* action, const double* state, double time, bool use_previous = false) override;
   const Trajectory* BestTrajectory() override;        // the NOMINAL trajectory (:462-464)
@@ -40,7 +46,8 @@ class CrossEntropyPlanner : public Planner {
   double std_initial_ = 0.1, std_min_ = 0.01, explore_fraction_ = 0.0, timestep_ = 0.01;
   uint32_t seed_ = 0x5EED;
   std::vector<double> times_scratch_;
-  std::vector<float> knots_, returns_;
+  SplineCandidates cands_;
+  std::vector<float> returns_;
   std::vector<uint8_t> failure_;
   std::vector<int> order_all_;
   Trajectory nominal_;

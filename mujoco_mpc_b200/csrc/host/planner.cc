@@ -84,7 +84,7 @@ void Planner::SetState(const double* state, double time, const double* mocap) {
 int Planner::RolloutSpline(const float* knots, const double* knot_times, int interpolation, int P, int N, int horizon,
                            float* returns, uint8_t* failure, int* order) {
   const std::vector<float> st(state_.begin(), state_.end()), mc(mocap_.begin(), mocap_.end());
-  horizon_ = horizon;
+  horizon_ = horizon; launch_offset_ = 0;
   return mjpc_b200_rollout_spline(gpu_, st.data(), time_, mc.empty() ? nullptr : mc.data(), nullptr, knots, knot_times,
                                   interpolation, P, N, horizon, returns, failure, order);
 }
@@ -95,7 +95,7 @@ int Planner::FetchTrajectory(int candidate, int horizon, Trajectory* t) {
   t->dim_trace = 3 * info_.num_trace;
   t->states.resize(H * t->dim_state); t->actions.resize(H * t->dim_action); t->times.resize(H);
   t->residual.resize(H * t->dim_residual); t->costs.resize(H); t->trace.resize(H * t->dim_trace);
-  return mjpc_b200_fetch_trajectory(gpu_, candidate, t->states.data(), t->actions.data(), t->times.data(),
+  return mjpc_b200_fetch_trajectory(gpu_, launch_offset_ + candidate, t->states.data(), t->actions.data(), t->times.data(),
                                     t->residual.data(), t->costs.data(), t->trace.data());
 }
 
@@ -159,6 +159,13 @@ int mjpc_b200_planner_action_from_policy(mjpc_b200_planner_t* h, double* action,
 int mjpc_b200_planner_set_fd(mjpc_b200_planner_t* h, double tolerance, int mode, int derivative_skip) {
   Planner* p = PlannerOf<Planner>(h);
   return p ? p->SetFD(tolerance, mode, derivative_skip) : MJPC_B200_ERR_BAD_ARGUMENT;
+}
+int mjpc_b200_planner_set_task(mjpc_b200_planner_t* h, const mjpc_task_desc* task) {
+  Planner* p = PlannerOf<Planner>(h);
+  if (!p || !task) return MJPC_B200_ERR_BAD_ARGUMENT;
+  for (mjpc_b200_t* g : p->Handles())
+    if (int rc = mjpc_b200_set_task(g, task)) return rc;
+  return 0;
 }
 
 }  // extern "C"

@@ -18,6 +18,14 @@ struct Trajectory {                                   // mjpc/trajectory.h:74-86
   bool failure = false;
 };
 
+// the candidates of one spline launch of one planning problem: knots [N][P][nu], knot times [P] (absolute)
+struct SplineCandidates {
+  int N = 0, P = 0, interpolation = 0;
+  std::vector<float> knots;
+  std::vector<double> knot_times;
+  void Resize(int n, int p, int nu) { N = n; P = p; knots.resize((size_t)n * p * nu); knot_times.resize(p); }
+};
+
 // mju_cholFactor: in-place lower Cholesky factor of the row-major n x n matrix M (upper triangle left as it was); a
 // pivot below mindiag is raised to mindiag.  Returns the rank, the number of pivots that were not raised.
 int CholFactor(double* M, int n, double mindiag);
@@ -58,6 +66,9 @@ class Planner {
   // every engine handle the planner plans on: Agent applies the planning-model options and the task snapshot to each
   virtual std::vector<mjpc_b200_t*> Handles() { return {gpu_}; }
   mjpc_b200_t* gpu() { return gpu_; }
+  const std::vector<double>& state() const { return state_; }
+  const std::vector<double>& mocap() const { return mocap_; }
+  double time() const { return time_; }
 
  protected:
   // borrowed != nullptr: plan on that handle (not owned); otherwise create one for max_candidates x max_horizon.
@@ -67,8 +78,11 @@ class Planner {
   // mjpc_b200_rollout_spline from state_, time_ and mocap_ with the handle's task snapshot; sets horizon_
   int RolloutSpline(const float* knots, const double* knot_times, int interpolation, int P, int N, int horizon,
                     float* returns, uint8_t* failure, int* order);
-  // sizes *out to `horizon` rows and fetches trajectory `candidate` (flat index) of the handle's last launch into it;
-  // total_return and failure are the caller's
+  int RolloutSpline(const SplineCandidates& c, int horizon, float* returns, uint8_t* failure, int* order) {
+    return RolloutSpline(c.knots.data(), c.knot_times.data(), c.interpolation, c.P, c.N, horizon, returns, failure, order);
+  }
+  // sizes *out to `horizon` rows and fetches trajectory `candidate` of the handle's last launch into it (flat index
+  // launch_offset_ + candidate); total_return and failure are the caller's
   int FetchTrajectory(int candidate, int horizon, Trajectory* out);
 
   mjpc_b200_t* gpu_ = nullptr;
@@ -77,6 +91,7 @@ class Planner {
   std::vector<double> state_, mocap_;
   double time_ = 0;
   int horizon_ = 0;                                   // of the last spline launch: the rows a fetch fills
+  int launch_offset_ = 0;                             // flat index of this planner's candidate 0 in that launch
 };
 
 // SetFD for a settings struct with fd_tolerance, fd_mode and derivative_skip: tolerance <= 0, mode < 0 and

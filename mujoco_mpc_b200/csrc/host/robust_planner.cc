@@ -6,9 +6,9 @@
 namespace mjpc_b200_host {
 
 int RobustPlanner::Initialize(std::unique_ptr<SamplingPlanner> delegate, const mjpc_model_blob* model,
-                              int noisy_candidates, int max_horizon, int device) {
+                              int noisy_candidates, int max_horizon, int device, mjpc_b200_t* engine) {
   delegate_ = std::move(delegate);
-  return AttachEngine(model, noisy_candidates, max_horizon, device);
+  return AttachEngine(model, noisy_candidates, max_horizon, device, engine);
 }
 
 void RobustPlanner::Configure(int sampling_trajectories, int ncandidates, int nrepetitions, double xfrc_std,
@@ -26,6 +26,18 @@ void RobustPlanner::SetState(const double* state, double time, const double* moc
 int RobustPlanner::OptimizePolicy(int horizon) {
   SamplingPlanner& d = *delegate_;
   const int ncandidates = d.OptimizePolicyCandidates(ncandidates_, horizon);
+  const int noisy = PrepareNoisy(ncandidates);
+  if (noisy <= 0) return noisy;
+  std::vector<float> ret(noisy);
+  std::vector<uint8_t> fail(noisy);
+  if (mjpc_b200_set_xfrc_noise(gpu_, xfrc_std_, xfrc_rate_, NoiseSeed())) return -1;
+  if (RolloutSpline(noisy_, horizon, ret.data(), fail.data(), nullptr)) return -1;
+  InstallNoisy(ret.data(), fail.data());
+  return 0;
+}
+
+int RobustPlanner::PrepareNoisy(int ncandidates) {
+  SamplingPlanner& d = *delegate_;
   scores_.clear();
   if (ncandidates < 0) return -1;
   if (ncandidates == 0) return 0;
@@ -35,24 +47,27 @@ int RobustPlanner::OptimizePolicy(int horizon) {
     return 0;
   }
   const int rep = nrepetitions_;
-  const std::vector<float>& clean = d.returns();         // scores of the clean rollouts, indexed by candidate
-  const std::vector<int>& order = d.trajectory_order;    // ... and their ranking
+  const std::vector<int>& order = d.trajectory_order;    // the ranking of the clean rollouts
   const TimeSpline& nominal = d.policy.plan;
   const int P = nominal.Size(), nu = nominal.Dim();
-  std::vector<float> knots((size_t)ncandidates * rep * P * nu), ret((size_t)ncandidates * rep);
-  std::vector<uint8_t> fail((size_t)ncandidates * rep);
-  std::vector<double> knot_times(P);
-  for (int k = 0; k < P; k++) knot_times[k] = nominal.NodeTime(k);
+  noisy_.Resize(ncandidates * rep, P, nu);
+  noisy_.interpolation = (int)nominal.Interpolation();
+  for (int k = 0; k < P; k++) noisy_.knot_times[k] = nominal.NodeTime(k);
   for (int c = 0; c < ncandidates; c++)
     for (int j = 0; j < rep; j++)
       for (int k = 0; k < P; k++) {
         const double* node = d.candidate_policy[order[c]].plan.NodeValues(k);
-        for (int a = 0; a < nu; a++) knots[(((size_t)c * rep + j) * P + k) * nu + a] = (float)node[a];
+        for (int a = 0; a < nu; a++) noisy_.knots[(((size_t)c * rep + j) * P + k) * nu + a] = (float)node[a];
       }
-  if (mjpc_b200_set_xfrc_noise(gpu_, xfrc_std_, xfrc_rate_, seed_ + (uint32_t)d.iteration)) return -1;
-  if (RolloutSpline(knots.data(), knot_times.data(), (int)nominal.Interpolation(), P, ncandidates * rep, horizon,
-                    ret.data(), fail.data(), nullptr))
-    return -1;
+  ncandidates_now_ = ncandidates;
+  return noisy_.N;
+}
+
+void RobustPlanner::InstallNoisy(const float* ret, const uint8_t* fail) {
+  SamplingPlanner& d = *delegate_;
+  const int ncandidates = ncandidates_now_, rep = nrepetitions_;
+  const std::vector<float>& clean = d.returns();         // scores of the clean rollouts, indexed by candidate
+  const std::vector<int>& order = d.trajectory_order;    // ... and their ranking
   // for each candidate the mean of its valid noisy returns; pick the best mean (robust_planner.cc:131-154)
   int best_candidate = -1;
   double best_score = 0;
@@ -70,7 +85,6 @@ int RobustPlanner::OptimizePolicy(int horizon) {
   d.CopyCandidateToPolicy(best_candidate);
   d.improvement = std::max((double)clean[0] - (double)clean[d.winner], 0.0);
   d.iteration++;
-  return 0;
 }
 
 }  // namespace mjpc_b200_host

@@ -11,10 +11,10 @@ namespace mjpc_b200_host {
 int SampleGradientPlanner::Initialize(const mjpc_model_blob* model, int num_trajectory, int num_gradient,
                                       int num_spline_points, int interpolation, double exploration,
                                       double gradient_filter, double timestep, const double* ctrlrange, uint32_t seed,
-                                      int max_horizon, int device) {
+                                      int max_horizon, int device, mjpc_b200_t* engine) {
   if (num_trajectory < 1 || num_spline_points < 2) return MJPC_B200_ERR_BAD_ARGUMENT;   // ResamplePolicy divides by P - 1
   // the nominal, the noisy samples and the gradient candidates share one launch
-  if (int rc = AttachEngine(model, num_trajectory, max_horizon, device)) return rc;
+  if (int rc = AttachEngine(model, num_trajectory, max_horizon, device, engine)) return rc;
   nu_ = info_.nu;
   num_trajectory_ = num_trajectory;
   num_gradient_ = std::max(num_gradient, 0);
@@ -73,39 +73,57 @@ void SampleGradientPlanner::AddNoiseToPolicy(int i) {
   }
 }
 
-int SampleGradientPlanner::Rollouts(int num_trajectory, int num_gradient, int horizon) {
+const SplineCandidates& SampleGradientPlanner::PrepareCandidates(int horizon) {
+  const int num_trajectory = num_trajectory_;
+  num_gradient_ = std::min(num_gradient_, num_trajectory - 1);
+  const int num_gradient = num_gradient_, num_noisy = num_trajectory - num_gradient;
+  {
+    const int P = policy.num_spline_points;
+    {
+      const std::shared_lock<std::shared_mutex> lock(mtx_);
+      resampled_policy = policy;
+    }
+    // the reference sets the live policy's interpolation here, outside any lock; it is always interpolation_ in this
+    // class, so setting it on the copy has the same effect without racing ActionFromPolicy
+    resampled_policy.plan.SetInterpolation(interpolation_);
+    ResamplePolicy(resampled_policy, horizon, P);
+    for (int i = 0; i < num_gradient; i++) ResamplePolicy(candidate_policy[num_noisy + i], horizon, P);
+  }
+  // Rollouts (:358-398)
   const int P = resampled_policy.plan.Size();
-  knots_.resize((size_t)num_trajectory * P * nu_);
+  cands_.Resize(num_trajectory, P, nu_);
+  cands_.interpolation = (int)interpolation_;
   for (int i = 0; i < num_trajectory; i++) {
-    if (i < num_trajectory - num_gradient) {           // nominal and noisy candidates; gradient ones are ready
+    if (i < num_noisy) {                               // nominal and noisy candidates; gradient ones are ready
       candidate_policy[i] = resampled_policy;
       if (i > 0) AddNoiseToPolicy(i);
     }
     for (int k = 0; k < P; k++) {
       const double* node = candidate_policy[i].plan.NodeValues(k);
-      for (int d = 0; d < nu_; d++) knots_[((size_t)i * P + k) * nu_ + d] = (float)node[d];
+      for (int d = 0; d < nu_; d++) cands_.knots[((size_t)i * P + k) * nu_ + d] = (float)node[d];
     }
   }
-  // the device ranks all N (lower index first on ties): replaces the partial_sort of OptimizePolicy (:219-229)
-  return RolloutSpline(knots_.data(), knot_times_.data(), (int)interpolation_, P, num_trajectory, horizon,
-                       returns_.data(), failure_.data(), trajectory_order.data());
+  std::copy(knot_times_.begin(), knot_times_.begin() + P, cands_.knot_times.begin());
+  return cands_;
 }
 
 int SampleGradientPlanner::OptimizePolicy(int horizon) {
-  const int num_trajectory = num_trajectory_;
-  num_gradient_ = std::min(num_gradient_, num_trajectory - 1);
-  const int num_gradient = num_gradient_, num_noisy = num_trajectory - num_gradient;
-  const int P = policy.num_spline_points;
-  {
-    const std::shared_lock<std::shared_mutex> lock(mtx_);
-    resampled_policy = policy;
+  const SplineCandidates& c = PrepareCandidates(horizon);
+  // the device ranks all N (lower index first on ties): replaces the partial_sort of OptimizePolicy (:219-229)
+  if (RolloutSpline(c, horizon, returns_.data(), failure_.data(), trajectory_order.data())) return -1;
+  InstallRollouts(horizon, returns_.data(), failure_.data(), trajectory_order.data(), 0);
+  return 0;
+}
+
+void SampleGradientPlanner::InstallRollouts(int horizon, const float* returns, const uint8_t* failure, const int* order,
+                                            int offset) {
+  const int num_trajectory = num_trajectory_, num_gradient = num_gradient_, num_noisy = num_trajectory - num_gradient;
+  if (returns != returns_.data()) {
+    std::copy(returns, returns + num_trajectory, returns_.begin());
+    std::copy(failure, failure + num_trajectory, failure_.begin());
+    std::copy(order, order + num_trajectory, trajectory_order.begin());
   }
-  // the reference sets the live policy's interpolation here, outside any lock; it is always interpolation_ in this
-  // class, so setting it on the copy has the same effect without racing ActionFromPolicy
-  resampled_policy.plan.SetInterpolation(interpolation_);
-  ResamplePolicy(resampled_policy, horizon, P);
-  for (int i = 0; i < num_gradient; i++) ResamplePolicy(candidate_policy[num_noisy + i], horizon, P);
-  if (Rollouts(num_trajectory, num_gradient, horizon)) return -1;
+  launch_offset_ = offset; horizon_ = horizon;
   winner = returns_[trajectory_order[0]] < returns_[0] ? trajectory_order[0] : 0;
   winner_type = winner == 0 ? kNominal : (winner < num_noisy ? kPerturb : kGradient);
   {
@@ -117,7 +135,6 @@ int SampleGradientPlanner::OptimizePolicy(int horizon) {
   improvement = std::max((double)returns_[0] - (double)returns_[winner], 0.0);
   GradientCandidates(num_trajectory, num_gradient);
   iteration++;
-  return 0;
 }
 
 void SampleGradientPlanner::GradientCandidates(int num_trajectory, int num_gradient) {

@@ -1,5 +1,5 @@
 // sample_gradient_planner.h - C++ host side of the Sample Gradient planner with the reference's method names
-// (mjpc/planners/sample_gradient/planner.h, planner.cc:43-498).  Rollouts() makes ONE mjpc_b200_rollout_spline call
+// (mjpc/planners/sample_gradient/planner.h, planner.cc:43-498).  Rollouts is ONE mjpc_b200_rollout_spline call
 // over all N candidates where the reference schedules N closures on its ThreadPool (planner.cc:358-398):
 //   0             the resampled nominal
 //   1 .. N-G-1    noisy samples, knot += exploration * z, z from the injected Philox stream (sampling_planner.h),
@@ -23,15 +23,19 @@ class SampleGradientPlanner : public Planner {
   // sampling_exploration, sampling_representation, sample_gradient_trajectories (G), sample_gradient_filter
   int Initialize(const mjpc_model_blob* model, int num_trajectory, int num_gradient, int num_spline_points,
                  int interpolation, double exploration, double gradient_filter, double timestep,
-                 const double* ctrlrange, uint32_t seed, int max_horizon, int device);
+                 const double* ctrlrange, uint32_t seed, int max_horizon, int device, mjpc_b200_t* engine = nullptr);
   void Reset(int horizon, const double* initial_repeated_action) override;   // :121-160
-  int OptimizePolicy(int horizon) override;                         // :169-273
+  int OptimizePolicy(int horizon) override;                         // :169-273: the two halves below around one launch
+  // ... before the launch: the resampled nominal, the noisy samples and the resampled gradient candidates (N in all)
+  const SplineCandidates& PrepareCandidates(int horizon);
+  // ... after it: the launch's horizon, the returns, failure flags and ranking of these N candidates, which it held from
+  // flat index `offset` on; the winner, the installed policy, improvement and GradientCandidates
+  void InstallRollouts(int horizon, const float* returns, const uint8_t* failure, const int* order, int offset);
   int NominalTrajectory(int horizon) override;                      // :276-287
   // :290-299; the policy does not depend on the state
   void ActionFromPolicy(double* action, const double* state, double time, bool use_previous = false) override;
   void ResamplePolicy(SamplingPolicy& p, int horizon, int num_spline_points);     // :302-326
   void AddNoiseToPolicy(int i);                                     // :329-355
-  int Rollouts(int num_trajectory, int num_gradient, int horizon);  // :358-398
   void GradientCandidates(int num_trajectory, int num_gradient);    // :401-493
   const Trajectory* BestTrajectory() override;                      // trajectory[winner] (:496-498)
 
@@ -53,6 +57,7 @@ class SampleGradientPlanner : public Planner {
   uint32_t seed_ = 0x5EED;
   std::vector<double> knot_times_;
   std::vector<double> return_weight_, step_size_;   // cached on size, as in the reference; Reset keeps them
+  SplineCandidates cands_;
   std::vector<float> knots_, returns_;
   std::vector<uint8_t> failure_;
   Trajectory best_;

@@ -177,27 +177,34 @@ void SamplingPlanner::InstallRollouts(int num_trajectory, int horizon, const flo
   std::copy(returns, returns + num_trajectory, returns_.begin());
   std::copy(failure, failure + num_trajectory, failure_.begin());
   trajectory_order.assign(order, order + num_trajectory);
-  offset_ = offset; horizon_ = horizon;
+  launch_offset_ = offset; horizon_ = horizon;
+}
+
+const SplineCandidates& SamplingPlanner::Candidates(int num_trajectory) {
+  cands_.Resize(num_trajectory, policy.plan.Size(), nu_);
+  cands_.interpolation = (int)interpolation_;
+  PrepareCandidates(num_trajectory, cands_.knots.data(), cands_.knot_times.data());
+  return cands_;
 }
 
 int SamplingPlanner::Rollouts(int num_trajectory, int horizon) {
-  const int P = policy.plan.Size();
-  knots_.resize((size_t)num_trajectory * P * nu_);
-  knot_times_.resize(P);
-  PrepareCandidates(num_trajectory, knots_.data(), knot_times_.data());
+  const SplineCandidates& c = Candidates(num_trajectory);
   trajectory_order.resize(num_trajectory);
-  offset_ = 0;
-  return RolloutSpline(knots_.data(), knot_times_.data(), (int)interpolation_, P, num_trajectory, horizon,
-                       returns_.data(), failure_.data(), trajectory_order.data());
+  return RolloutSpline(c, horizon, returns_.data(), failure_.data(), trajectory_order.data());
+}
+
+const SplineCandidates& SamplingPlanner::PrepareOptimize(int horizon) {
+  UpdateNominalPolicy(horizon);
+  policy.plan.SetInterpolation(interpolation_);
+  return Candidates(num_trajectory_);
 }
 
 int SamplingPlanner::OptimizePolicyCandidates(int ncandidates, int horizon) {
-  UpdateNominalPolicy(horizon);
-  const int num_trajectory = num_trajectory_;
-  ncandidates = std::min(ncandidates, num_trajectory);
-  policy.plan.SetInterpolation(interpolation_);
-  if (int rc = Rollouts(num_trajectory, horizon)) return -1;   // device ranking replaces partial_sort (:184-188)
-  return ncandidates;
+  const SplineCandidates& c = PrepareOptimize(horizon);
+  trajectory_order.resize(c.N);
+  // device ranking replaces partial_sort (:184-188)
+  if (RolloutSpline(c, horizon, returns_.data(), failure_.data(), trajectory_order.data())) return -1;
+  return std::min(ncandidates, num_trajectory_);
 }
 
 int SamplingPlanner::OptimizePolicy(int horizon) {
@@ -231,7 +238,7 @@ void SamplingPlanner::ActionFromPolicy(double* action, const double*, double tim
 }
 
 int SamplingPlanner::CandidateTrajectory(int candidate, int horizon, Trajectory* t) {
-  if (FetchTrajectory(offset_ + candidate, horizon, t)) return -1;
+  if (FetchTrajectory(candidate, horizon, t)) return -1;
   t->total_return = returns_[candidate];
   t->failure = failure_[candidate];
   return 0;

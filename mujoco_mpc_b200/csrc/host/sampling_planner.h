@@ -66,24 +66,26 @@ class SamplingPlanner : public Planner {
   void UpdateNominalPolicy(int horizon);              // :240-323 (non-sliding resample)
   void AddNoiseToPolicy(int i);                       // :326-352
   int Rollouts(int num_trajectory, int horizon);      // :355-393 -> one C-ABI call
-  // Rollouts in two halves, for a launch shared with other planners (batch_sampling_planner.h):
+  // Rollouts in two halves, for a launch shared with other planners (batch_planner.h):
   // the candidates (nominal + noise) as knots [num_trajectory][P][nu] and knot times [P]; returns P
   int PrepareCandidates(int num_trajectory, float* knots, double* knot_times);
+  // ... the same into the planner's own SplineCandidates
+  const SplineCandidates& Candidates(int num_trajectory);
+  // OptimizePolicyCandidates up to its launch: the nominal update and the num_trajectory candidates
+  const SplineCandidates& PrepareOptimize(int horizon);
   // the launch's horizon, and the returns, failure flags and ranking of these candidates, which it held from flat
   // index `offset` on
   void InstallRollouts(int num_trajectory, int horizon, const float* returns, const uint8_t* failure, const int* order,
                        int offset);
   void InstallBest();                                 // OptimizePolicy after the rollouts: winner, improvement, iteration
-  const std::vector<double>& state() const { return state_; }
-  const std::vector<double>& mocap() const { return mocap_; }
   // :229-237; the policy does not depend on the state
   void ActionFromPolicy(double* action, const double* state, double time, bool use_previous = false) override;
   void CopyCandidateToPolicy(int candidate);          // :534-543
   const Trajectory* BestTrajectory() override;
   int CandidateTrajectory(int candidate, int horizon, Trajectory* out);   // trajectory[candidate] of the last Rollouts
   void SetPolicy(const double* times, const double* parameters, int num_nodes);   // policy.plan = nodes (ilqs/planner.cc:160-172)
-  double time() const { return time_; }
   double timestep() const { return timestep_; }
+  int num_trajectory() const { return num_trajectory_; }
   SplineInterpolation interpolation() const { return interpolation_; }
   double CandidateScore(int candidate) const { return returns_[trajectory_order[candidate]]; }
   int NumParameters() const { return nu_ * policy.num_spline_points; }
@@ -99,14 +101,13 @@ class SamplingPlanner : public Planner {
   void SetExploration(double e0, double e1) { noise_exploration_[0] = e0; noise_exploration_[1] = e1; }
 
  private:
-  int offset_ = 0;                                    // flat index of candidate 0 in the last launch
   int num_trajectory_ = 0, nu_ = 0;
   SplineInterpolation interpolation_ = kCubicSpline;
   double noise_exploration_[2] = {0.1, 0.0};
   double timestep_ = 0.01;
   uint32_t seed_ = 0x5EED;
-  std::vector<float> knots_, returns_;
-  std::vector<double> knot_times_;
+  SplineCandidates cands_;
+  std::vector<float> returns_;
   std::vector<uint8_t> failure_;
   Trajectory best_;
   mutable std::shared_mutex mtx_;

@@ -40,6 +40,9 @@ struct RolloutArgs {
   float xfrc_std, xfrc_rate;   // NoisyRollout (trajectory.cc:100-210): OU force noise, std 0 = off
   unsigned noise_seed;
   int cand0;                // global index of this launch's first candidate (multi-GPU shards): noise stream = cand0 + local index
+  // [nprob] or nullptr: per-problem noise keys.  Given, problem prob draws with key noise_seeds[prob] and its
+  // problem-local candidate index as the stream, which is what a launch of that problem alone with that seed draws.
+  const unsigned* noise_seeds;
   int P, interp, N, H;
   float* states; float* actions; double* times; float* residual; float* costs; float* trace;
   float* returns; unsigned char* failure;
@@ -256,6 +259,15 @@ __device__ __forceinline__ void rollout_body(const RolloutArgs& A) {
   const bool noisy = A.xfrc_std > 0.f;
   const float ou_rate = noisy ? expf(-CM(c).timestep / A.xfrc_rate) : 0.f;
   const float ou_scale = noisy ? A.xfrc_std * sqrtf(1.f - ou_rate * ou_rate) : 0.f;
+  // the noise key and stream of this candidate, [warp of the CTA][key, stream]: kept in shared memory rather than in
+  // registers across the step loop: two more live registers there made the Quadruped one-warp and Humanoid Track
+  // helper-warp instances spill (static instances hold one candidate per CTA; the generic one up to 4)
+  __shared__ unsigned noise_ks[4][2];
+  const int kw = std::is_same<SP, DynSpec>::value ? warp : 0;
+  if (noisy && lane == 0) {   // (published to the warp by the __syncwarp below)
+    noise_ks[kw][0] = A.noise_seeds ? A.noise_seeds[prob] : A.noise_seed;
+    noise_ks[kw][1] = A.noise_seeds ? (unsigned)(cand - prob * A.nper) : (unsigned)(A.cand0 + cand);
+  }
   for (int i = lane; i < 6 * M.nbody; i += 32) DF(xfrc)[i] = 0;
   c.xfrc_on = noisy ? 1 : 0;
   float step_size = 0.f;
@@ -308,7 +320,7 @@ __device__ __forceinline__ void rollout_body(const RolloutArgs& A) {
     if (noisy && !last) {   // Ornstein-Uhlenbeck perturbation in discrete time (trajectory.cc:147-155)
       float* xf = DF(xfrc);
       for (int i = lane; i < 6 * M.nbody; i += 32)
-        xf[i] = ou_rate * xf[i] + ou_scale * xfrc_normal(A.noise_seed, (unsigned)t, (unsigned)(A.cand0 + cand), (unsigned)i);
+        xf[i] = ou_rate * xf[i] + ou_scale * xfrc_normal(noise_ks[kw][0], (unsigned)t, noise_ks[kw][1], (unsigned)i);
       __syncwarp();
     }
     float cost;

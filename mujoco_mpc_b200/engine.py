@@ -23,7 +23,10 @@ EXPORTS = ["mjpc_b200_version", "mjpc_b200_last_error", "mjpc_b200_create", "mjp
            "mjpc_b200_rollout_spline_batched", "mjpc_b200_batch_planner_create", "mjpc_b200_batch_planner_destroy",
            "mjpc_b200_batch_planner_reset", "mjpc_b200_batch_planner_set_state", "mjpc_b200_batch_planner_set_task",
            "mjpc_b200_batch_planner_optimize_policy", "mjpc_b200_batch_planner_action_from_policy",
-           "mjpc_b200_batch_planner_get_result",
+           "mjpc_b200_batch_planner_get_result", "mjpc_b200_set_xfrc_noise_batched", "mjpc_b200_planner_set_task",
+           "mjpc_b200_batch_ce_planner_create", "mjpc_b200_batch_ce_planner_get_result",
+           "mjpc_b200_batch_sg_planner_create", "mjpc_b200_batch_sg_planner_get_result",
+           "mjpc_b200_batch_robust_planner_create", "mjpc_b200_batch_robust_planner_get_result",
            "mjpc_b200_fetch_trajectory", "mjpc_b200_fetch_all", "mjpc_b200_model_derivatives",
            "mjpc_b200_cost_derivatives", "mjpc_b200_backward_pass", "mjpc_b200_rollout_feedback_batched",
            "mjpc_b200_model_derivatives_batched", "mjpc_b200_cost_derivatives_batched", "mjpc_b200_backward_pass_batched",
@@ -112,6 +115,9 @@ def load_library():
             f.argtypes, f.restype = [C.c_void_p] + args, C.c_int
         lib.mjpc_b200_estimator_last_error.restype = C.c_char_p
         lib.mjpc_b200_batch_planner_destroy.argtypes = [C.c_void_p]
+        lib.mjpc_b200_planner_set_task.argtypes = [C.c_void_p, C.c_void_p]
+        lib.mjpc_b200_set_xfrc_noise_batched.argtypes = [C.c_void_p, C.c_double, C.c_double, C.c_int,
+                                                         C.POINTER(C.c_uint32)]
         lib.mjpc_b200_sampling_planner_set_exploration.argtypes = [C.c_void_p, C.c_double, C.c_double]
         lib.mjpc_b200_batch_ilqg_planner_destroy.argtypes = [C.c_void_p]
         lib.mjpc_b200_batch_ilqg_planner_set_fd.argtypes = [C.c_void_p, C.c_double, C.c_int, C.c_int]
@@ -225,6 +231,13 @@ class _CppPlanner(_CppObject):
 
     def action_from_policy(self, time, use_previous=False):
         return self._action(time, None, use_previous)
+
+    def set_task(self, weight=None, parameters=None, task_state=None, risk=None):
+        """The task snapshot of every engine handle the planner plans on (mjpc_b200_planner_set_task)."""
+        w, p, s = _d(weight), _d(parameters), _d(task_state)
+        td = TaskDesc(_pd(w), _pd(p), _pd(s), float(self.m.task_risk if risk is None else risk))
+        if self.lib.mjpc_b200_planner_set_task(self.h, C.byref(td)):
+            self._fail("set_task")
 
 
 class _CppFeedbackPlanner(_CppPlanner):
@@ -608,6 +621,13 @@ class Engine:
         """NoisyRollout perturbation for the following rollouts (mjpc_b200_set_xfrc_noise); std 0 = off."""
         self._check(self.lib.mjpc_b200_set_xfrc_noise(self.h, C.c_double(std), C.c_double(rate), C.c_uint32(seed)))
 
+    def set_xfrc_noise_batched(self, std, rate, seeds):
+        """The same noise with one key per problem (mjpc_b200_set_xfrc_noise_batched): the following launches must
+        hold len(seeds) problems, and problem b draws as a launch of it alone after set_xfrc_noise(std, rate, seeds[b])."""
+        sd = np.ascontiguousarray(seeds, np.uint32)
+        self._check(self.lib.mjpc_b200_set_xfrc_noise_batched(self.h, C.c_double(std), C.c_double(rate), len(sd),
+                                                              sd.ctypes.data_as(C.POINTER(C.c_uint32))))
+
     @property
     def last_kernel_ms(self):
         return float(self.lib.mjpc_b200_last_kernel_ms(self.h))
@@ -647,19 +667,25 @@ class CppSamplingPlanner(_CppPlanner):
         return dict(winner=winner.value, improvement=imp.value, returns=ret, knots=knots, knot_times=kt)
 
 
-class CppBatchSamplingPlanner(_CppObject):
-    """num_problems independent Predictive Sampling problems planned with one rollout launch per iteration
-    (csrc/host/batch_sampling_planner.cc); each method that concerns one problem takes its index."""
+class _CppBatchPlanner(_CppObject):
+    """A batch of num_problems independent planners of one kind (csrc/host/batch_planner.h): `<prefix>_create` makes it
+    and result(problem) reads one problem; every other call is one of the generic mjpc_b200_batch_planner_* entry
+    points, and each method that concerns one problem takes its index."""
 
-    def __init__(self, model, num_problems, num_trajectory, horizon, seeds=None, device=0):
-        m, num = model, model.numeric
+    def _setup(self, model, num_problems, horizon, num_trajectory, seeds):
+        num = model.numeric
         self.P = int(num.get("sampling_spline_points", [3])[0])
-        self.B, self.horizon, self.N, self.nu = int(num_problems), int(horizon), int(num_trajectory), m.nu
-        sd = np.ascontiguousarray([0x5EED + b for b in range(self.B)] if seeds is None else seeds, np.uint32)
-        cr = _d(np.asarray(m.actuator_ctrlrange, float).reshape(-1))
-        self._create("mjpc_b200_batch_planner", m, self.B, self.N, self.P, int(num.get("sampling_representation", [2])[0]),
-                     C.c_double(float(num.get("sampling_exploration", [0.1])[0])), C.c_double(float(m.opt_timestep)),
-                     _pd(cr), sd.ctypes.data_as(C.POINTER(C.c_uint32)), self.horizon, int(device))
+        self.B, self.horizon, self.N, self.nu = int(num_problems), int(horizon), int(num_trajectory), model.nu
+        self._seeds = np.ascontiguousarray([0x5EED + b for b in range(self.B)] if seeds is None else seeds, np.uint32)
+        self._cr = _d(np.asarray(model.actuator_ctrlrange, float).reshape(-1))
+        return num, _pd(self._cr), self._seeds.ctypes.data_as(C.POINTER(C.c_uint32))
+
+    def close(self):
+        if getattr(self, "h", None):
+            self.lib.mjpc_b200_batch_planner_destroy(self.h)
+            self.h = None
+
+    __del__ = close
 
     def _check(self, rc, what):
         if rc < 0:
@@ -684,6 +710,23 @@ class CppBatchSamplingPlanner(_CppObject):
         self._check(self.lib.mjpc_b200_batch_planner_optimize_policy(self.h, self.horizon), "optimize_policy")
         return [self.result(b) for b in range(self.B)]
 
+    def action_from_policy(self, problem, time, use_previous=False):
+        a = np.zeros(self.nu)
+        self._check(self.lib.mjpc_b200_batch_planner_action_from_policy(self.h, int(problem), _pd(a), C.c_double(time),
+                                                                        int(use_previous)), "action_from_policy")
+        return a
+
+
+class CppBatchSamplingPlanner(_CppBatchPlanner):
+    """num_problems independent Predictive Sampling problems planned with one rollout launch per iteration
+    (csrc/host/batch_sampling_planner.cc)."""
+
+    def __init__(self, model, num_problems, num_trajectory, horizon, seeds=None, device=0):
+        num, cr, sd = self._setup(model, num_problems, horizon, num_trajectory, seeds)
+        self._create("mjpc_b200_batch_planner", model, self.B, self.N, self.P, int(num.get("sampling_representation", [2])[0]),
+                     C.c_double(float(num.get("sampling_exploration", [0.1])[0])), C.c_double(float(model.opt_timestep)),
+                     cr, sd, self.horizon, int(device))
+
     def result(self, problem):
         winner, imp = C.c_int(), C.c_double()
         ret = np.zeros(self.N, np.float32); knots = np.zeros((self.P, self.nu)); kt = np.zeros(self.P)
@@ -691,11 +734,77 @@ class CppBatchSamplingPlanner(_CppObject):
                                                                 _pd(knots), _pd(kt)), "get_result")
         return dict(winner=winner.value, improvement=imp.value, returns=ret, knots=knots, knot_times=kt)
 
-    def action_from_policy(self, problem, time, use_previous=False):
-        a = np.zeros(self.nu)
-        self._check(self.lib.mjpc_b200_batch_planner_action_from_policy(self.h, int(problem), _pd(a), C.c_double(time),
-                                                                        int(use_previous)), "action_from_policy")
-        return a
+
+class CppBatchCrossEntropyPlanner(_CppBatchPlanner):
+    """num_problems independent Cross-Entropy problems, one rollout launch of B x (N + 1) per iteration
+    (csrc/host/batch_planner.cc).  Mirrors CppCrossEntropyPlanner with a problem argument."""
+
+    def __init__(self, model, num_problems, num_trajectory, horizon, n_elite=0, seeds=None, device=0):
+        num, cr, sd = self._setup(model, num_problems, horizon, num_trajectory, seeds)
+        self._create(
+            "mjpc_b200_batch_ce_planner", model, self.B, self.N, int(n_elite), self.P,
+            int(num.get("sampling_representation", [2])[0]), C.c_double(float(num.get("sampling_exploration", [0.1])[0])),
+            C.c_double(float(num.get("std_min", [0.01])[0])), C.c_double(float(num.get("explore_fraction", [0.0])[0])),
+            C.c_double(float(model.opt_timestep)), cr, sd, self.horizon, int(device))
+
+    def result(self, problem):
+        imp = C.c_double()
+        ret = np.zeros(self.N + 1, np.float32); order = np.zeros(self.N, np.int32)
+        knots = np.zeros((self.P, self.nu)); kt = np.zeros(self.P); var = np.zeros((self.P, self.nu))
+        self._check(self.lib.mjpc_b200_batch_ce_planner_get_result(self.h, int(problem), C.byref(imp), _pf(ret),
+                                                                   order.ctypes.data_as(_ip), _pd(knots), _pd(kt), _pd(var)),
+                    "get_result")
+        return dict(improvement=imp.value, returns=ret, order=order, knots=knots, knot_times=kt, variance=var)
+
+
+class CppBatchSampleGradientPlanner(_CppBatchPlanner):
+    """num_problems independent Sample Gradient problems, one rollout launch of B x N per iteration
+    (csrc/host/batch_planner.cc).  Mirrors CppSampleGradientPlanner with a problem argument."""
+
+    def __init__(self, model, num_problems, num_trajectory, horizon, num_gradient=None, gradient_filter=None, seeds=None,
+                 device=0):
+        num, cr, sd = self._setup(model, num_problems, horizon, num_trajectory, seeds)
+        G = int(num_gradient if num_gradient is not None else num.get("sample_gradient_trajectories", [0])[0])
+        self.G = max(min(G, self.N - 1), 0)                  # the clamp OptimizePolicy applies
+        f = float(gradient_filter if gradient_filter is not None else num.get("sample_gradient_filter", [1.0])[0])
+        self._create(
+            "mjpc_b200_batch_sg_planner", model, self.B, self.N, G, self.P, int(num.get("sampling_representation", [2])[0]),
+            C.c_double(float(num.get("sampling_exploration", [0.1])[0])), C.c_double(f),
+            C.c_double(float(model.opt_timestep)), cr, sd, self.horizon, int(device))
+
+    def result(self, problem):
+        winner, wtype, imp = C.c_int(), C.c_int(), C.c_double()
+        ret = np.zeros(self.N, np.float32); order = np.zeros(self.N, np.int32)
+        knots = np.zeros((self.P, self.nu)); kt = np.zeros(self.P)
+        gk = np.zeros((self.G, self.P, self.nu)); grad = np.zeros((self.P, self.nu))
+        n = self._check(self.lib.mjpc_b200_batch_sg_planner_get_result(
+            self.h, int(problem), C.byref(winner), C.byref(wtype), C.byref(imp), _pf(ret), order.ctypes.data_as(_ip),
+            _pd(knots), _pd(kt), _pd(gk) if self.G else None, _pd(grad)), "get_result")
+        return dict(winner=winner.value, winner_type=wtype.value, improvement=imp.value, returns=ret, order=order,
+                    knots=knots[:n], knot_times=kt[:n], gradient_knots=gk, gradient=grad)
+
+
+class CppBatchRobustPlanner(_CppBatchPlanner):
+    """num_problems independent Robust problems (csrc/host/batch_planner.cc): per iteration one clean launch of B x N
+    and one noisy launch of B x ncandidates x nrepetitions, each problem with its own noise key.  Mirrors
+    CppRobustPlanner with a problem argument."""
+
+    def __init__(self, model, num_problems, num_trajectory, horizon, ncandidates=-1, nrepetitions=5, xfrc_std=0.1,
+                 xfrc_rate=0.1, seeds=None, device=0):
+        num, cr, sd = self._setup(model, num_problems, horizon, num_trajectory, seeds)
+        self.nc = int(ncandidates if ncandidates != -1 else num_trajectory // nrepetitions)
+        self._create(
+            "mjpc_b200_batch_robust_planner", model, self.B, self.N, self.P, int(num.get("sampling_representation", [2])[0]),
+            C.c_double(float(num.get("sampling_exploration", [0.1])[0])), C.c_double(float(model.opt_timestep)), cr, sd,
+            int(ncandidates), int(nrepetitions), C.c_double(xfrc_std), C.c_double(xfrc_rate), self.horizon, int(device))
+
+    def result(self, problem):
+        winner = C.c_int()
+        scores = np.zeros(max(self.nc, 1)); ret = np.zeros(self.N, np.float32)
+        knots = np.zeros((self.P, self.nu)); kt = np.zeros(self.P)
+        n = self._check(self.lib.mjpc_b200_batch_robust_planner_get_result(self.h, int(problem), C.byref(winner), _pd(scores),
+                                                                           _pf(ret), _pd(knots), _pd(kt)), "get_result")
+        return dict(winner=winner.value, scores=scores[:n], returns=ret, knots=knots, knot_times=kt)
 
 
 class CppCrossEntropyPlanner(_CppPlanner):
