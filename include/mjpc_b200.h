@@ -19,6 +19,8 @@
  *                                                                       mjpc/planners/ilqg/backward_pass.cc:65-250
  *   mjpc_b200_*_batched         <- the calls above for B independent problems in one launch (rollout_spline,
  *                                  rollout_feedback, model_derivatives, cost_derivatives, backward_pass)
+ *   mjpc_b200_gradient_batched  <- Gradient::Compute with its derivatives   mjpc/planners/gradient/gradient.cc:76-107
+ *                                  (the two derivative sweeps, then the gradient recursion, all on the device)
  *   mjpc_b200_set_task          <- residual_fn_ snapshot per PlanIteration  mjpc/agent.cc:316-319, task.cc:112-128
  *   mjpc_b200_fetch_trajectory  <- fills a mjpc::Trajectory             mjpc/trajectory.h:74-86
  *   create / destroy            <- Planner::Initialize/Allocate + ResizeMjData  mjpc/planners/planner.cc:23-33;
@@ -210,6 +212,17 @@ int mjpc_b200_backward_pass_batched(mjpc_b200_t* h, int B, const float* A, const
                                     const float* cu, const float* cxx, const float* cxu, const float* cuu,
                                     const float* actions, int H, const float* mu, int reg_type, int limits, float* K,
                                     float* du, float* dV, float* Vx, float* Vxx, int* status);
+/* Gradient::Compute (gradient.cc:76-107) for B problems: the FD derivative sweep of mjpc_b200_model_derivatives_batched
+ * and the cost derivatives of mjpc_b200_cost_derivatives_batched on the same inputs, then the gradient recursion, all on
+ * the device; A, B, C, D and the cost derivatives never leave it.  Inputs as model_derivatives_batched, plus
+ * residual [B][H][nr].  k [B][H][nu] (row H-1 repeats row H-2), dV0 [B], both double, bitwise what
+ * mjpc_b200_host_gradient_sweep computes from the A, B, cx and cu the two batched calls return.  B < 1, H < 2, a NULL
+ * required pointer, a bad skip / mode / tol or missing mocaps: MJPC_B200_ERR_BAD_ARGUMENT; H > max_horizon:
+ * MJPC_B200_ERR_CAPACITY.  last_kernel_ms spans the call's kernels (the residual upload between them included). */
+int mjpc_b200_gradient_batched(mjpc_b200_t* h, int B, const float* x, const float* u, const double* t,
+                               const float* mocaps, const double* weights, const double* parameters,
+                               const double* task_states, const float* residual, int H, int skip, float tol, int mode,
+                               double* k, double* dV0);
 
 /* Debug / parity hook: one forward-dynamics evaluation + Euler step for a single state through the same
  * device code the rollout kernel runs. qacc[nv], residual[nr], next_qpos[nq], next_qvel[nv], counts[4] =
@@ -613,6 +626,54 @@ int mjpc_b200_gradient_planner_get_result(mjpc_b200_planner_t* p, double* scalar
 /* SplineMapping::Compute (gradient/spline_mapping.cc) as scalar weights W [num_output][num_input]; host only */
 void mjpc_b200_host_spline_mapping(int representation, const double* input_times, int num_input, const double* output_times,
                                    int num_output, double* W);
+/* Gradient::Compute's recursion on the host in fp64 (the single planner's GradientSweep); host only.  A [T][n][n],
+ * B [T][n][m], cx [T][n], cu [T][m] -> k [T][m] (row T-1 repeats row T-2), *dV0.  The reference of
+ * mjpc_b200_gradient_batched. */
+void mjpc_b200_host_gradient_sweep(const float* A, const float* B, const float* cx, const float* cu, int n, int m, int T,
+                                   double* k, double* dV0);
+
+/* ---- Batched Gradient planner (csrc/host/batch_planner.{h,cc}): num_problems independent GradientPlanners on ONE
+ * engine handle of num_problems x num_trajectory candidates, with the single planner's create arguments plus
+ * num_problems.  Per max_rollout iteration: one spline launch of the B resampled nominals, one
+ * mjpc_b200_gradient_batched on their trajectories (each problem with its own mocap and task snapshot), one spline
+ * launch of the B x num_trajectory line-search candidates.  Each problem's result equals that of a GradientPlanner with
+ * the same inputs.  reset / set_state / set_task / optimize_policy / action_from_policy / destroy are the generic
+ * mjpc_b200_batch_planner_* calls; settings (set_fd) are common to the batch. */
+int mjpc_b200_batch_gradient_planner_create(const mjpc_model_blob* model, int num_problems, int num_trajectory,
+                                            int num_spline_points, int representation, double fd_tolerance,
+                                            double timestep, const double* ctrlrange, int max_horizon, int device,
+                                            void** out);
+/* as mjpc_b200_gradient_planner_get_result for one problem; *improved (may be NULL) = what the single planner's
+ * optimize_policy returned on the last iteration (1 improved, 0 not; 0 after an error).  Returns P; a batch of another kind or a problem
+ * outside [0, num_problems): MJPC_B200_ERR_BAD_ARGUMENT */
+int mjpc_b200_batch_gradient_planner_get_result(void* planner, int problem, double* scalars, double* parameters,
+                                                double* times, int* improved);
+/* the finite-difference settings of a Gradient or iLQS batch (every problem), as mjpc_b200_planner_set_fd: tolerance
+ * <= 0, mode < 0 and derivative_skip < 0 keep the current value.  Other kinds: MJPC_B200_ERR_UNSUPPORTED */
+int mjpc_b200_batch_planner_set_fd(void* planner, double tolerance, int mode, int derivative_skip);
+
+/* ---- Batched iLQS planner (csrc/host/batch_planner.{h,cc}): num_problems independent iLQSPlanners, with the single
+ * planner's create arguments plus num_problems and seeds [num_problems], on two handles as the single planner has:
+ * sampling (num_problems x num_trajectory) and iLQG (num_problems x ilqg_num_rollouts).  Per iteration at most: one
+ * feedback launch of the iLQG nominals of the problems whose active policy was iLQG, one spline launch of every
+ * problem's sampling, then for the problems sampling did not settle one batched derivative sweep, one batched
+ * cost-derivative call, backward-pass rounds of the problems still failing and one action-rollout launch.  Each
+ * problem's result equals that of an iLQSPlanner with the same seed and inputs.  Exploration and the finite-difference
+ * and iLQG settings are common to the batch.  reset / set_state / set_task / optimize_policy / destroy and set_fd are
+ * the generic mjpc_b200_batch_planner_* calls; the generic action_from_policy evaluates the policy without a state. */
+int mjpc_b200_batch_ilqs_planner_create(const mjpc_model_blob* model, int num_problems, int num_trajectory,
+                                        int num_spline_points, int interpolation, double exploration, double timestep,
+                                        const double* ctrlrange, const uint32_t* seeds, int ilqg_num_rollouts,
+                                        int ilqg_representation, double fd_tolerance, int max_horizon, int device,
+                                        void** out);
+/* scalars[4] as mjpc_b200_ilqs_planner_get_result for one problem; *improved (may be NULL) = what the single planner's
+ * optimize_policy returned on the last iteration (1 / 0; 0 after an error).  Returns the active policy.  A batch of
+ * another kind or a problem outside [0, num_problems): MJPC_B200_ERR_BAD_ARGUMENT */
+int mjpc_b200_batch_ilqs_planner_get_result(void* planner, int problem, double* scalars, int* improved);
+int mjpc_b200_batch_ilqs_planner_set_exploration(void* planner, double exploration);   /* every problem */
+/* iLQSPlanner::ActionFromPolicy of one problem: the iLQG half is a feedback policy and reads `state` (may be NULL) */
+int mjpc_b200_batch_ilqs_planner_action_from_policy(void* planner, int problem, double* action, const double* state,
+                                                    double time, int use_previous);
 
 /* ---- iLQS planner (csrc/host/gradient_planner.{h,cc}; mjpc/planners/ilqs/planner.cc:87-215): Predictive Sampling first;
  * when it does not improve, one iLQG iteration seeded with the sampling nominal; when sampling follows iLQG the trajectory

@@ -1146,14 +1146,14 @@ static std::vector<float> to_float(const double* v, size_t count) {
   return v ? std::vector<float>(v, v + count) : std::vector<float>();
 }
 
-static int model_derivatives_impl(mjpc_b200_t* h, int B, const float* x, const float* u, const double* t,
-                                  const float* mocaps, const double* weights, const double* parameters,
-                                  const double* task_states, int H, int skip, float tol, int mode, float* A, float* B_,
-                                  float* C, float* D) {
+// the derivative sweep's per-problem task states ts [B][task_state_size] and relative times trel [B][H]
+static void derivative_times(mjpc_b200_t* h, int B, const double* t, const double* task_states, int H,
+                             std::vector<float>* ts_out, std::vector<float>* trel_out) {
   const DevModel& M = h->pack.M;
-  CUDA_TRY(cudaSetDevice(h->device));
   const size_t nts = M.task_state_size;
-  std::vector<float> ts((size_t)B * nts), trel((size_t)B * H);
+  std::vector<float>& ts = *ts_out;
+  std::vector<float>& trel = *trel_out;
+  ts.resize((size_t)B * nts); trel.resize((size_t)B * H);
   // derivative sweeps use absolute-time task state rebased to each problem's own t[0].  A time on a rollout's clock
   // (t[0] plus i timesteps in double: what rollouts record) is evaluated at that rollout step's fp32 relative time,
   // the sum of i fp32 timesteps the residuals of the rollout read, so that the Jacobians belong to the trajectory's own
@@ -1170,6 +1170,16 @@ static int model_derivatives_impl(mjpc_b200_t* h, int B, const float* x, const f
       clock += h->pack.timestep; clock32 += h32;
     }
   }
+}
+
+static int model_derivatives_impl(mjpc_b200_t* h, int B, const float* x, const float* u, const double* t,
+                                  const float* mocaps, const double* weights, const double* parameters,
+                                  const double* task_states, int H, int skip, float tol, int mode, float* A, float* B_,
+                                  float* C, float* D) {
+  const DevModel& M = h->pack.M;
+  CUDA_TRY(cudaSetDevice(h->device));
+  std::vector<float> ts, trel;
+  derivative_times(h, B, t, task_states, H, &ts, &trel);
   const std::vector<float> w = to_float(weights, (size_t)B * M.num_term), p = to_float(parameters, (size_t)B * M.num_parameters);
   const size_t smem = h->smem_bytes(1, 1);
   if (ilqg_reserve(h->ilqg, M, B, h->stream)) return fail(MJPC_B200_ERR_CUDA, "model_derivatives: out of device memory");
@@ -1238,6 +1248,43 @@ int mjpc_b200_cost_derivatives_batched(mjpc_b200_t* h, int B, const double* weig
   if (B < 1 || H < 1) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "cost_derivatives_batched: bad B or H");
   if (H > h->maxH) return fail(MJPC_B200_ERR_CAPACITY, "cost_derivatives_batched: H above max_horizon");
   return cost_derivatives_impl(h, B, weights, residual, C, D, H, cx, cu, cxx, cuu, cxu);
+}
+
+int mjpc_b200_gradient_batched(mjpc_b200_t* h, int B, const float* x, const float* u, const double* t,
+                               const float* mocaps, const double* weights, const double* parameters,
+                               const double* task_states, const float* residual, int H, int skip, float tol, int mode,
+                               double* k, double* dV0) {
+  if (!h || !x || !u || !t || !residual || !k || !dV0) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "gradient_batched: null");
+  if (B < 1 || H < 2 || !(tol > 0)) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "gradient_batched: bad B, H or tol");
+  if (H > h->maxH) return fail(MJPC_B200_ERR_CAPACITY, "gradient_batched: H above max_horizon");
+  if (skip < 0 || mode < 0 || mode > 1) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "gradient_batched: bad skip or mode");
+  if (h->pack.M.nmocap && !mocaps) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "gradient_batched: mocap required");
+  const DevModel& M = h->pack.M;
+  CUDA_TRY(cudaSetDevice(h->device));
+  if (cost_derivatives_smem(M, h->max_term_dim) > h->smem_optin)
+    return fail(MJPC_B200_ERR_CAPACITY, "gradient_batched: the widest cost term does not fit in shared memory");
+  std::vector<float> ts, trel;
+  derivative_times(h, B, t, task_states, H, &ts, &trel);
+  const std::vector<float> w = to_float(weights, (size_t)B * M.num_term), p = to_float(parameters, (size_t)B * M.num_parameters);
+  if (ilqg_reserve(h->ilqg, M, B, h->stream)) return fail(MJPC_B200_ERR_CUDA, "gradient_batched: out of device memory");
+  const KernelSet* ks;
+  pick_kernels(h, true, &ks);
+  // the two derivative sweeps exactly as their batched entry points stage them, except that A, B, C, D and the cost
+  // derivatives stay on the device; one span from the first kernel to the sweep's end
+  int launches = 0;
+  int rc = ilqg_model_derivatives(h->ilqg, M, h->d_pack, h->stream, ks->fd_center, ks->fd_column, B, x, u, trel.data(),
+                                  mocaps, ts.data(), weights ? w.data() : nullptr, parameters ? p.data() : nullptr, H,
+                                  tol, nullptr, nullptr, nullptr, nullptr, h->smem_bytes(1, 1), &launches, h->ev0,
+                                  nullptr, skip, mode);
+  if (rc == 0)
+    rc = ilqg_cost_derivatives(h->ilqg, M, h->d_pack, h->stream, B, weights ? w.data() : nullptr, residual, nullptr,
+                               nullptr, H, nullptr, nullptr, nullptr, nullptr, nullptr, h->max_term_dim, &launches,
+                               nullptr, nullptr, true);
+  if (rc == 0) rc = ilqg_gradient_sweep(h->ilqg, h->stream, B, H, k, dV0, &launches, h->ev1);
+  h->launches += launches;
+  if (rc == 0 && cudaEventElapsedTime(&h->last_ms, h->ev0, h->ev1) != cudaSuccess) cudaGetLastError();
+  if (rc) return fail(rc, "gradient_batched: CUDA failure");
+  return 0;
 }
 
 static int backward_pass_impl(mjpc_b200_t* h, int B, const float* A, const float* B_, const float* cx, const float* cu,

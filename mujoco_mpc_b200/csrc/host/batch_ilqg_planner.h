@@ -4,7 +4,8 @@
 //   feedback rollouts of every NominalTrajectory -> derivatives -> cost derivatives -> backward passes of the problems
 //   still failing, round by round, each with its own regularisation -> action rollouts of the problems that succeeded.
 // Each problem runs exactly the host steps iLQGPlanner runs around its own calls (the prepare / install halves), so
-// its result is bitwise the one an iLQGPlanner with the same inputs computes with its own launches.
+// its result is bitwise the one an iLQGPlanner with the same inputs computes with its own launches.  The sweeps
+// themselves (ILQGSweeps) run over any subset of planners on a handle; BatchILQSPlanner uses them for its iLQG halves.
 #pragma once
 #include <cstdint>
 #include <memory>
@@ -13,6 +14,41 @@
 #include "ilqg_planner.h"
 
 namespace mjpc_b200_host {
+
+// the task snapshots of a batch's problems: rows [..][nw], [..][np], [..][nts]; a NULL array when the model has none
+struct TaskRows {
+  const double *w = nullptr, *p = nullptr, *ts = nullptr;
+  int nw = 0, np = 0, nts = 0;
+};
+
+// The batched iLQG sweeps over any subset of iLQGPlanners that plan on one handle (the planners need not be owned by
+// it): planner ps[j] reads task snapshot row task[j].  Every planner of a call must have the same settings.
+class ILQGSweeps {
+ public:
+  void Attach(mjpc_b200_t* gpu, int num_rollouts, int representation);
+  // iLQGPlanner::NominalTrajectory of each planner, one feedback launch; <0 on error
+  int Nominal(const std::vector<iLQGPlanner*>& ps, const std::vector<int>& task, const TaskRows& rows, int horizon);
+  // iLQGPlanner::Iteration of each planner; updated[j] (may be NULL) receives its 1/0; <0 on error
+  int Iterate(const std::vector<iLQGPlanner*>& ps, const std::vector<int>& task, const TaskRows& rows, int horizon,
+              int* updated);
+
+ private:
+  // one feedback launch of the candidate policies of ps (flat candidate j*K + i for ps[j])
+  int FeedbackLaunch(const std::vector<iLQGPlanner*>& ps, const std::vector<int>& task, const TaskRows& rows,
+                     int horizon, bool with_du, int mode);
+
+  mjpc_b200_t* gpu_ = nullptr;
+  int K_ = 0, representation_ = 0, nu_ = 0, ds_ = 0, n_ = 0, nr_ = 0, nmocap7_ = 0;
+  // launch staging ([problems of the launch][..])
+  std::vector<float> st_, mc_, x_, u_, g_, du_, steps_, res_;
+  std::vector<double> times_, t_, w_, p_, ts_;
+  std::vector<float> A_, B_, C_, D_, cx_, cu_, cxx_, cuu_, cxu_;           // [J][H][..] of the iteration
+  std::vector<float> sA_, sB_, scx_, scu_, scxx_, scxu_, scuu_, sact_, mu_, K_out_, du_out_, dV_out_;   // retry subset
+  std::vector<int> status_;
+  std::vector<float> ret_;   // [J][K] of the last feedback launch
+  std::vector<uint8_t> fail_;
+  std::vector<int> order_;
+};
 
 class BatchILQGPlanner {
  public:
@@ -32,23 +68,15 @@ class BatchILQGPlanner {
 
  private:
   int Nominal(int horizon);
-  int Iterate(int horizon, int* updated);
-  // inputs of one feedback launch for the problems `idx` (flat candidate j*K + i for problem idx[j])
-  int FeedbackLaunch(const std::vector<int>& idx, int horizon, bool with_du, int mode);
+  TaskRows Rows() const;
 
   mjpc_b200_t* gpu_ = nullptr;
   std::vector<std::unique_ptr<iLQGPlanner>> problems_;
-  int K_ = 0, representation_ = 0, nu_ = 0, ds_ = 0, n_ = 0, nr_ = 0, nmocap7_ = 0;
+  std::vector<iLQGPlanner*> all_;
+  std::vector<int> all_idx_;
   std::vector<double> weight_, parameters_, task_state_;   // [B][num_term], [B][num_parameters], [B][task_state_size]
   int nw_ = 0, np_ = 0, nts_ = 0;
-  // launch staging ([problems of the launch][..])
-  std::vector<float> st_, mc_, x_, u_, g_, du_, steps_, res_, ret_;
-  std::vector<double> times_, t_, w_, p_, ts_;
-  std::vector<uint8_t> fail_;
-  std::vector<int> order_;
-  std::vector<float> A_, B_, C_, D_, cx_, cu_, cxx_, cuu_, cxu_;           // [B][H][..] of the iteration
-  std::vector<float> sA_, sB_, scx_, scu_, scxx_, scxu_, scuu_, sact_, mu_, K_out_, du_out_, dV_out_;   // retry subset
-  std::vector<int> status_;
+  ILQGSweeps sweeps_;
 };
 
 }  // namespace mjpc_b200_host

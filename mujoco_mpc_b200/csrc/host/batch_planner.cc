@@ -50,7 +50,7 @@ int BatchPlanner::LaunchSpline(mjpc_b200_t* gpu, const std::vector<const SplineC
   knots_.resize((size_t)B * nk);
   knot_times_.resize((size_t)B * P);
   for (int b = 0; b < B; b++) {
-    const Planner& pl = *problems_[b];
+    const Planner& pl = launcher(b);
     std::copy(cands[b]->knots.begin(), cands[b]->knots.begin() + nk, knots_.begin() + b * nk);
     std::copy(cands[b]->knot_times.begin(), cands[b]->knot_times.begin() + P, knot_times_.begin() + (size_t)b * P);
     const size_t ds = pl.state().size(), nm = pl.mocap().size();
@@ -63,6 +63,12 @@ int BatchPlanner::LaunchSpline(mjpc_b200_t* gpu, const std::vector<const SplineC
                                           nw_ ? weight_.data() : nullptr, np_ ? parameters_.data() : nullptr,
                                           nts_ ? task_state_.data() : nullptr, knots_.data(), knot_times_.data(), interp,
                                           P, N, horizon, returns_.data(), failure_.data(), order_.data());
+}
+
+TaskRows BatchPlanner::Rows() const {
+  TaskRows r;
+  r.w = weight_.data(); r.p = parameters_.data(); r.ts = task_state_.data(); r.nw = nw_; r.np = np_; r.nts = nts_;
+  return r;
 }
 
 // ------------------------------------------------------------------------------------------ Cross-Entropy
@@ -180,11 +186,146 @@ int BatchRobustPlanner::OptimizePolicy(int horizon) {
   return 0;
 }
 
+// ------------------------------------------------------------------------------------------ Gradient
+int BatchGradientPlanner::Initialize(const mjpc_model_blob* model, int num_problems, int num_trajectory,
+                                     int num_spline_points, int representation, double timestep,
+                                     const double* ctrlrange, int max_horizon, int device) {
+  if (num_problems < 1) return MJPC_B200_ERR_BAD_ARGUMENT;
+  if (int rc = Attach(model, num_problems, num_problems * std::max(num_trajectory, 1), max_horizon, device)) return rc;
+  improved_.assign(num_problems, 0);
+  for (int b = 0; b < num_problems; b++) {
+    auto* p = new GradientPlanner;
+    problems_.emplace_back(p);
+    if (int rc = p->Initialize(model, num_trajectory, num_spline_points, representation, timestep, ctrlrange,
+                               max_horizon, device, gpu_))
+      return rc;
+  }
+  return 0;
+}
+
+int BatchGradientPlanner::OptimizePolicy(int horizon) {
+  const int B = NumProblems();
+  std::fill(improved_.begin(), improved_.end(), 0);
+  const GradientPlannerSettings& s = planner(0).settings;
+  const DifferentiableScope diff(gpu_, s.differentiable != 0);
+  std::vector<const SplineCandidates*> cands(B);
+  for (int b = 0; b < B; b++)
+    if (!(cands[b] = planner(b).PrepareNominal(horizon))) return MJPC_B200_ERR_BAD_ARGUMENT;
+  if (int rc = LaunchSpline(gpu_, cands, horizon)) return rc;
+  for (int b = 0; b < B; b++)
+    if (planner(b).InstallNominal(horizon, returns_.data() + b, failure_.data() + b, b)) return -1;
+  const size_t H = horizon;
+  const Trajectory& t0 = planner(0).nominal();
+  const size_t ds = t0.dim_state, nu = t0.dim_action, nr = t0.dim_residual, nm = planner(0).mocap().size();
+  x_.resize(B * H * ds); u_.resize(B * H * nu); res_.resize(B * H * nr); t_.resize(B * H); mc_.resize(B * nm);
+  k_.resize(B * H * nu); dV0_.resize(B);
+  for (int it = 0; it < s.max_rollout; it++) {
+    for (int b = 0; b < B; b++) {
+      const Trajectory& tr = planner(b).nominal();
+      std::copy(tr.states.begin(), tr.states.begin() + H * ds, x_.begin() + b * H * ds);
+      std::copy(tr.actions.begin(), tr.actions.begin() + H * nu, u_.begin() + b * H * nu);
+      std::copy(tr.residual.begin(), tr.residual.begin() + H * nr, res_.begin() + b * H * nr);
+      std::copy(tr.times.begin(), tr.times.begin() + H, t_.begin() + b * H);
+      const std::vector<double>& mc = planner(b).mocap();
+      std::copy(mc.begin(), mc.end(), mc_.begin() + b * nm);   // float, as the single planner passes it
+    }
+    if (int rc = mjpc_b200_gradient_batched(gpu_, B, x_.data(), u_.data(), t_.data(), nm ? mc_.data() : nullptr,
+                                            weights(), parameters(), task_states(), res_.data(), horizon,
+                                            s.derivative_skip, (float)s.fd_tolerance, s.fd_mode, k_.data(),
+                                            dV0_.data()))
+      return rc;
+    for (int b = 0; b < B; b++) cands[b] = &planner(b).PrepareLineSearch(horizon, k_.data() + b * H * nu, dV0_[b]);
+    if (int rc = LaunchSpline(gpu_, cands, horizon)) return rc;
+    const int K = cands[0]->N;
+    for (int b = 0; b < B; b++) {
+      const size_t o = (size_t)b * K;
+      if (planner(b).InstallLineSearch(horizon, returns_.data() + o, failure_.data() + o, (int)o)) return -1;
+    }
+  }
+  for (int b = 0; b < B; b++) improved_[b] = planner(b).Publish();
+  return 0;
+}
+
+// ------------------------------------------------------------------------------------------ iLQS
+BatchILQSPlanner::~BatchILQSPlanner() {
+  problems_.clear();   // the planners borrow both handles
+  if (ilqg_gpu_) mjpc_b200_destroy(ilqg_gpu_);
+}
+
+int BatchILQSPlanner::Initialize(const mjpc_model_blob* model, int num_problems, int num_trajectory,
+                                 int num_spline_points, int interpolation, double exploration, double timestep,
+                                 const double* ctrlrange, const uint32_t* seeds, int ilqg_num_rollouts,
+                                 int ilqg_representation, double fd_tolerance, int max_horizon, int device) {
+  if (num_problems < 1) return MJPC_B200_ERR_BAD_ARGUMENT;
+  if (int rc = Attach(model, num_problems, num_problems * num_trajectory, max_horizon, device)) return rc;
+  if (int rc = mjpc_b200_create(model, num_problems * ilqg_num_rollouts, max_horizon, device, &ilqg_gpu_)) return rc;
+  sweeps_.Attach(ilqg_gpu_, ilqg_num_rollouts, ilqg_representation);
+  improved_.assign(num_problems, 0);
+  for (int b = 0; b < num_problems; b++) {
+    auto* p = new iLQSPlanner;
+    problems_.emplace_back(p);
+    if (int rc = p->Initialize(model, num_trajectory, num_spline_points, interpolation, exploration, timestep, ctrlrange,
+                               seeds[b], ilqg_num_rollouts, ilqg_representation, fd_tolerance, max_horizon, device, gpu_,
+                               ilqg_gpu_))
+      return rc;
+  }
+  return 0;
+}
+
+int BatchILQSPlanner::OptimizePolicy(int horizon) {
+  const int B = NumProblems();
+  std::fill(improved_.begin(), improved_.end(), 0);
+  const bool diff = planner(0).ilqg.settings.differentiable != 0;
+  auto ilqg_of = [&](const std::vector<int>& idx) {
+    std::vector<iLQGPlanner*> ps;
+    for (int b : idx) ps.push_back(&planner(b).ilqg);
+    return ps;
+  };
+  // the iLQG nominals of the problems whose active policy was iLQG, then their conversion to splines
+  std::vector<int> conv;
+  for (int b = 0; b < B; b++) {
+    planner(b).BeginIteration();
+    if (planner(b).previous_active_policy == iLQSPlanner::kiLQG) conv.push_back(b);
+  }
+  if (!conv.empty()) {
+    const DifferentiableScope d(ilqg_gpu_, diff);
+    if (sweeps_.Nominal(ilqg_of(conv), conv, Rows(), horizon)) return -1;
+  }
+  for (int b : conv) planner(b).ConvertToSpline(horizon);
+  // every problem's sampling: one launch
+  std::vector<const SplineCandidates*> cands(B);
+  for (int b = 0; b < B; b++) cands[b] = &planner(b).sampling.PrepareOptimize(horizon);
+  if (int rc = LaunchSpline(gpu_, cands, horizon)) return rc;
+  const int N = cands[0]->N;
+  std::vector<int> rest;
+  for (int b = 0; b < B; b++) {
+    iLQSPlanner& p = planner(b);
+    const size_t o = (size_t)b * N;
+    p.sampling.InstallRollouts(N, horizon, returns_.data() + o, failure_.data() + o, order_.data() + o, (int)o);
+    p.sampling.InstallBest();
+    const int settled = p.SamplingSettled(horizon);
+    if (settled < 0) return -1;
+    if (settled) improved_[b] = 1;
+    else rest.push_back(b);
+  }
+  // one iLQG iteration of the problems sampling did not settle
+  if (rest.empty()) return 0;
+  std::vector<int> updated(rest.size(), 0);
+  {
+    const DifferentiableScope d(ilqg_gpu_, diff);
+    if (sweeps_.Iterate(ilqg_of(rest), rest, Rows(), horizon, updated.data())) return -1;
+  }
+  for (size_t j = 0; j < rest.size(); j++) improved_[rest[j]] = planner(rest[j]).Accept(updated[j]);
+  return 0;
+}
+
 }  // namespace mjpc_b200_host
 
 // ------------------------------------------------------------------------------------------ C entry points
 // (the generic batch family of include/mjpc_b200.h: every batch kind's handle is its BatchPlanner base)
 using mjpc_b200_host::BatchCrossEntropyPlanner;
+using mjpc_b200_host::BatchGradientPlanner;
+using mjpc_b200_host::BatchILQSPlanner;
 using mjpc_b200_host::BatchPlanner;
 using mjpc_b200_host::BatchRobustPlanner;
 using mjpc_b200_host::BatchSampleGradientPlanner;
@@ -297,6 +438,71 @@ int mjpc_b200_batch_robust_planner_get_result(void* p, int problem, int* winner,
   if (!bp) return MJPC_B200_ERR_BAD_ARGUMENT;
   return mjpc_b200_robust_planner_get_result(mjpc_b200_host::ToHandle(&bp->planner(problem)), winner, scores, returns,
                                              knots, knot_times);
+}
+
+int mjpc_b200_batch_planner_set_fd(void* p, double tolerance, int mode, int derivative_skip) {
+  if (!p) return MJPC_B200_ERR_BAD_ARGUMENT;
+  BatchPlanner* bp = batch_of(p);
+  for (int b = 0; b < bp->NumProblems(); b++)
+    if (int rc = bp->problem(b).SetFD(tolerance, mode, derivative_skip)) return rc;   // the kinds without: UNSUPPORTED
+  return 0;
+}
+
+int mjpc_b200_batch_gradient_planner_create(const mjpc_model_blob* model, int num_problems, int num_trajectory,
+                                            int num_spline_points, int representation, double fd_tolerance,
+                                            double timestep, const double* ctrlrange, int max_horizon, int device,
+                                            void** out) {
+  if (!model || !model->data || !ctrlrange || !out || num_trajectory < 1 || num_spline_points < 1 || max_horizon < 2)
+    return MJPC_B200_ERR_BAD_ARGUMENT;
+  *out = nullptr;
+  auto* p = new BatchGradientPlanner;
+  int rc = p->Initialize(model, num_problems, num_trajectory, num_spline_points, representation, timestep, ctrlrange,
+                         max_horizon, device);
+  if (rc == 0) mjpc_b200_batch_planner_set_fd(static_cast<BatchPlanner*>(p), fd_tolerance, -1, -1);
+  return finish_create(p, rc, out);
+}
+int mjpc_b200_batch_gradient_planner_get_result(void* p, int problem, double* scalars, double* parameters,
+                                                double* times, int* improved) {
+  BatchGradientPlanner* bp = problem_of<BatchGradientPlanner>(p, problem);
+  if (!bp) return MJPC_B200_ERR_BAD_ARGUMENT;
+  if (improved) *improved = bp->improved(problem);
+  return mjpc_b200_gradient_planner_get_result(mjpc_b200_host::ToHandle(&bp->planner(problem)), scalars, parameters,
+                                               times);
+}
+
+int mjpc_b200_batch_ilqs_planner_create(const mjpc_model_blob* model, int num_problems, int num_trajectory,
+                                        int num_spline_points, int interpolation, double exploration, double timestep,
+                                        const double* ctrlrange, const uint32_t* seeds, int ilqg_num_rollouts,
+                                        int ilqg_representation, double fd_tolerance, int max_horizon, int device,
+                                        void** out) {
+  if (!model || !model->data || !ctrlrange || !seeds || !out || num_trajectory < 1 || ilqg_num_rollouts < 1 ||
+      max_horizon < 2)
+    return MJPC_B200_ERR_BAD_ARGUMENT;
+  *out = nullptr;
+  auto* p = new BatchILQSPlanner;
+  return finish_create(p, p->Initialize(model, num_problems, num_trajectory, num_spline_points, interpolation,
+                                        exploration, timestep, ctrlrange, seeds, ilqg_num_rollouts, ilqg_representation,
+                                        fd_tolerance, max_horizon, device), out);
+}
+// scalars[4] as mjpc_b200_ilqs_planner_get_result; *improved (may be NULL) = the problem's 1/0 of the last iteration
+int mjpc_b200_batch_ilqs_planner_get_result(void* p, int problem, double* scalars, int* improved) {
+  BatchILQSPlanner* bp = problem_of<BatchILQSPlanner>(p, problem);
+  if (!bp) return MJPC_B200_ERR_BAD_ARGUMENT;
+  if (improved) *improved = bp->improved(problem);
+  return mjpc_b200_ilqs_planner_get_result(mjpc_b200_host::ToHandle(&bp->planner(problem)), scalars);
+}
+int mjpc_b200_batch_ilqs_planner_set_exploration(void* p, double exploration) {
+  BatchILQSPlanner* bp = problem_of<BatchILQSPlanner>(p, 0);
+  if (!bp) return MJPC_B200_ERR_BAD_ARGUMENT;
+  for (int b = 0; b < bp->NumProblems(); b++) bp->planner(b).sampling.SetExploration(exploration, 0.0);
+  return 0;
+}
+int mjpc_b200_batch_ilqs_planner_action_from_policy(void* p, int problem, double* action, const double* state,
+                                                    double time, int use_previous) {
+  BatchILQSPlanner* bp = problem_of<BatchILQSPlanner>(p, problem);
+  if (!bp || !action) return MJPC_B200_ERR_BAD_ARGUMENT;
+  bp->planner(problem).ActionFromPolicy(action, state, time, use_previous != 0);
+  return 0;
 }
 
 }  // extern "C"

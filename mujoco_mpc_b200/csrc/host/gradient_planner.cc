@@ -93,9 +93,9 @@ void GradientPolicy::Action(double* action, double time) const {
 }
 
 int GradientPlanner::Initialize(const mjpc_model_blob* model, int num_trajectory, int num_spline_points, int representation,
-                                double timestep, const double* ctrlrange, int max_horizon, int device) {
+                                double timestep, const double* ctrlrange, int max_horizon, int device, mjpc_b200_t* borrowed) {
   K_ = std::max(num_trajectory, 1);
-  if (int rc = AttachEngine(model, K_, max_horizon, device)) return rc;
+  if (int rc = AttachEngine(model, K_, max_horizon, device, borrowed)) return rc;
   nu_ = info_.nu; n_ = info_.dim_dstate; nr_ = info_.num_residual; Hmax_ = info_.max_horizon;
   timestep_ = timestep;
   policy.nu = nu_; policy.num_spline_points = num_spline_points; policy.representation = representation;
@@ -124,13 +124,17 @@ void GradientPlanner::ResamplePolicy(int horizon) {
   for (int k = 0; k < P; k++) cand_.times[k] = t[0] + shift * k;     // LinearRange (planner.cc:381-382)
 }
 
-int GradientPlanner::Rollouts(const std::vector<double>& parameters, int count, int horizon) {
+void GradientPlanner::Candidates(const std::vector<double>& parameters, int count, SplineCandidates* c) const {
   const int P = cand_.num_spline_points;
-  knots_.resize((size_t)count * P * nu_);
-  for (size_t i = 0; i < knots_.size(); i++) knots_[i] = (float)parameters[i];
-  ret_.assign(count, 0.f); fail_.assign(count, 0); order_.assign(count, 0);
-  return RolloutSpline(knots_.data(), cand_.times.data(), cand_.representation, P, count, horizon, ret_.data(),
-                       fail_.data(), order_.data());
+  c->Resize(count, P, nu_);
+  c->interpolation = cand_.representation;
+  for (size_t i = 0; i < c->knots.size(); i++) c->knots[i] = (float)parameters[i];
+  std::copy(cand_.times.begin(), cand_.times.end(), c->knot_times.begin());
+}
+
+int GradientPlanner::Launch(const SplineCandidates& c, int horizon) {
+  ret_.assign(c.N, 0.f); fail_.assign(c.N, 0); order_.assign(c.N, 0);
+  return RolloutSpline(c, horizon, ret_.data(), fail_.data(), order_.data());
 }
 
 int GradientPlanner::Fetch(int candidate, int horizon, double ret) {
@@ -139,28 +143,89 @@ int GradientPlanner::Fetch(int candidate, int horizon, double ret) {
   return 0;
 }
 
-int GradientPlanner::OptimizePolicy(int horizon) {
-  if (horizon < 2 || horizon > Hmax_) return -1;
-  const size_t H = horizon, n = n_, m = nu_, nr = nr_;
-  const DifferentiableScope diff(gpu_, settings.differentiable != 0);
+const SplineCandidates* GradientPlanner::PrepareNominal(int horizon) {
+  if (horizon < 2 || horizon > Hmax_) return nullptr;
   {
     const std::shared_lock<std::shared_mutex> lock(mtx_);
     cand_ = policy;
   }
-  const int P = cand_.num_spline_points;
   ResamplePolicy(horizon);
-  // nominal rollout: trajectory[0]
-  if (Rollouts(cand_.parameters, 1, horizon)) return -1;
-  const double c_prev = fail_[0] ? 1.0e6 : (double)ret_[0];
-  if (Fetch(0, horizon, c_prev)) return -1;
-  double c_best = c_prev;
-  const std::vector<double> steps = LogScaleSteps(K_, settings.min_linesearch_step);
+  Candidates(cand_.parameters, 1, &nominal_);   // nominal rollout: trajectory[0]
+  return &nominal_;
+}
+
+int GradientPlanner::InstallNominal(int horizon, const float* returns, const uint8_t* failure, int offset) {
+  launch_offset_ = offset; horizon_ = horizon;
+  c_prev_ = failure[0] ? 1.0e6 : (double)returns[0];
+  if (Fetch(0, horizon, c_prev_)) return -1;
+  c_best_ = c_prev_;
+  steps_ = LogScaleSteps(K_, settings.min_linesearch_step);
+  const size_t Pn = (size_t)cand_.num_spline_points * nu_;
+  update_.resize(Pn); candidates_.resize((size_t)K_ * Pn);
+  for (int c = 0; c < K_; c++) std::copy(cand_.parameters.begin(), cand_.parameters.end(), candidates_.begin() + c * Pn);
+  winner = K_ - 1;
+  return 0;
+}
+
+const SplineCandidates& GradientPlanner::PrepareLineSearch(int horizon, const double* k, double dV0) {
+  const int P = cand_.num_spline_points;
+  dV0_ = dV0;
+  SplineMapping(cand_.representation, cand_.times, best_.times.data(), horizon - 1, &W_);
+  std::fill(update_.begin(), update_.end(), 0.0);                      // parameter_update = mapping^T k (:240-245)
+  for (int t = 0; t < horizon - 1; t++)
+    for (int p = 0; p < P; p++) {
+      const double w = W_[(size_t)t * P + p];
+      if (w == 0.0) continue;
+      for (int j = 0; j < nu_; j++) update_[(size_t)p * nu_ + j] += w * k[(size_t)t * nu_ + j];
+    }
+  for (int c = 0; c < K_; c++)                                        // Rollouts (:386-420): parameters += step * update
+    for (size_t q = 0; q < (size_t)P * nu_; q++) candidates_[(size_t)c * P * nu_ + q] = cand_.parameters[q] + steps_[c] * update_[q];
+  Candidates(candidates_, K_, &lines_);
+  return lines_;
+}
+
+int GradientPlanner::InstallLineSearch(int horizon, const float* returns, const uint8_t* failure, int offset) {
+  const size_t Pn = (size_t)cand_.num_spline_points * nu_;
+  launch_offset_ = offset; horizon_ = horizon;
+  winner = K_ - 1;
+  for (int j = K_ - 1; j >= 0; j--) {
+    const double c_sample = failure[j] ? 1.0e6 : (double)returns[j];
+    if (c_sample < c_best_) { c_best_ = c_sample; winner = j; }
+  }
+  std::copy(candidates_.begin() + winner * Pn, candidates_.begin() + (winner + 1) * Pn, cand_.parameters.begin());
+  if (Fetch(winner, horizon, failure[winner] ? 1.0e6 : (double)returns[winner])) return -1;   // trajectory[0] = trajectory[winner]
+  action_step = steps_[winner];
+  expected = -action_step * dV0_ - 1.0e-16;
+  improvement = c_prev_ - c_best_;
+  surprise = std::min(std::max(0.0, improvement / expected), 2.0);
+  return 0;
+}
+
+int GradientPlanner::Publish() {
+  const size_t Pn = (size_t)cand_.num_spline_points * nu_;
+  if (c_best_ >= c_prev_) {
+    winner = K_ - 1;     // step 0: the resampled nominal
+    std::copy(candidates_.begin() + winner * Pn, candidates_.begin() + (winner + 1) * Pn, cand_.parameters.begin());
+  }
+  {
+    const std::unique_lock<std::shared_mutex> lock(mtx_);
+    previous_policy = policy;
+    policy.parameters = cand_.parameters; policy.times = cand_.times;     // CopyParametersFrom (:319-320)
+  }
+  total_return = c_best_;
+  return c_best_ < c_prev_ ? 1 : 0;
+}
+
+int GradientPlanner::OptimizePolicy(int horizon) {
+  if (horizon < 2 || horizon > Hmax_) return -1;
+  const size_t H = horizon, n = n_, m = nu_, nr = nr_;
+  const DifferentiableScope diff(gpu_, settings.differentiable != 0);
+  const SplineCandidates* nominal = PrepareNominal(horizon);
+  if (Launch(*nominal, horizon) || InstallNominal(horizon, ret_.data(), fail_.data(), 0)) return -1;
   A_.resize(H * n * n); B_.resize(H * n * m); C_.resize(H * nr * n); D_.resize(H * nr * m);
   cx_.resize(H * n); cu_.resize(H * m); cxx_.resize(H * n * n); cuu_.resize(H * m * m); cxu_.resize(H * n * m);
   std::vector<float> mc(mocap_.begin(), mocap_.end());
-  std::vector<double> k, W, update((size_t)P * nu_), candidates((size_t)K_ * P * nu_);
-  for (int c = 0; c < K_; c++) std::copy(cand_.parameters.begin(), cand_.parameters.end(), candidates.begin() + (size_t)c * P * nu_);
-  winner = K_ - 1;
+  std::vector<double> k;
   for (int it = 0; it < settings.max_rollout; it++) {
     if (mjpc_b200_model_derivatives(gpu_, best_.states.data(), best_.actions.data(), best_.times.data(),
                                     mc.empty() ? nullptr : mc.data(), horizon, settings.derivative_skip,
@@ -171,40 +236,10 @@ int GradientPlanner::OptimizePolicy(int horizon) {
       return -1;
     double dV0 = 0;
     GradientSweep(A_.data(), B_.data(), cx_.data(), cu_.data(), (int)n, (int)m, horizon, &k, &dV0);
-    SplineMapping(cand_.representation, cand_.times, best_.times.data(), horizon - 1, &W);
-    std::fill(update.begin(), update.end(), 0.0);                       // parameter_update = mapping^T k (:240-245)
-    for (int t = 0; t < horizon - 1; t++)
-      for (int p = 0; p < P; p++) {
-        const double w = W[(size_t)t * P + p];
-        if (w == 0.0) continue;
-        for (int j = 0; j < nu_; j++) update[(size_t)p * nu_ + j] += w * k[(size_t)t * nu_ + j];
-      }
-    for (int c = 0; c < K_; c++)                                        // Rollouts (:386-420): parameters += step * update
-      for (size_t q = 0; q < (size_t)P * nu_; q++) candidates[(size_t)c * P * nu_ + q] = cand_.parameters[q] + steps[c] * update[q];
-    if (Rollouts(candidates, K_, horizon)) return -1;
-    winner = K_ - 1;
-    for (int j = K_ - 1; j >= 0; j--) {
-      const double c_sample = fail_[j] ? 1.0e6 : (double)ret_[j];
-      if (c_sample < c_best) { c_best = c_sample; winner = j; }
-    }
-    std::copy(candidates.begin() + (size_t)winner * P * nu_, candidates.begin() + (size_t)(winner + 1) * P * nu_, cand_.parameters.begin());
-    if (Fetch(winner, horizon, fail_[winner] ? 1.0e6 : (double)ret_[winner])) return -1;   // trajectory[0] = trajectory[winner]
-    action_step = steps[winner];
-    expected = -action_step * dV0 - 1.0e-16;
-    improvement = c_prev - c_best;
-    surprise = std::min(std::max(0.0, improvement / expected), 2.0);
+    if (Launch(PrepareLineSearch(horizon, k.data(), dV0), horizon)) return -1;
+    if (InstallLineSearch(horizon, ret_.data(), fail_.data(), 0)) return -1;
   }
-  if (c_best >= c_prev) {
-    winner = K_ - 1;     // step 0: the resampled nominal
-    std::copy(candidates.begin() + (size_t)winner * P * nu_, candidates.begin() + (size_t)(winner + 1) * P * nu_, cand_.parameters.begin());
-  }
-  {
-    const std::unique_lock<std::shared_mutex> lock(mtx_);
-    previous_policy = policy;
-    policy.parameters = cand_.parameters; policy.times = cand_.times;     // CopyParametersFrom (:319-320)
-  }
-  total_return = c_best;
-  return c_best < c_prev ? 1 : 0;
+  return Publish();
 }
 
 void GradientPlanner::ActionFromPolicy(double* action, const double*, double time, bool use_previous) {
@@ -215,11 +250,12 @@ void GradientPlanner::ActionFromPolicy(double* action, const double*, double tim
 // ------------------------------------------------------------------------------------------ iLQS
 int iLQSPlanner::Initialize(const mjpc_model_blob* model, int num_trajectory, int num_spline_points, int interpolation,
                             double exploration, double timestep, const double* ctrlrange, uint32_t seed, int ilqg_num_rollouts,
-                            int ilqg_representation, double fd_tolerance, int max_horizon, int device) {
+                            int ilqg_representation, double fd_tolerance, int max_horizon, int device,
+                            mjpc_b200_t* sampling_gpu, mjpc_b200_t* ilqg_gpu) {
   int rc = sampling.Initialize(model, num_trajectory, num_spline_points, interpolation, exploration, 0.0, timestep, ctrlrange,
-                               seed, num_trajectory, max_horizon, device);
+                               seed, num_trajectory, max_horizon, device, sampling_gpu);
   if (rc) return rc;
-  rc = ilqg.Initialize(model, ilqg_num_rollouts, ilqg_representation, max_horizon, device);
+  rc = ilqg.Initialize(model, ilqg_num_rollouts, ilqg_representation, max_horizon, device, ilqg_gpu);
   if (rc) return rc;
   ilqg.SetFD(fd_tolerance, -1, -1);
   nu_ = sampling.NumParameters() / std::max(sampling.policy.num_spline_points, 1);
@@ -236,38 +272,35 @@ void iLQSPlanner::SetState(const double* state, double time, const double* mocap
   sampling.SetState(state, time, mocap); ilqg.SetState(state, time, mocap);
 }
 
-int iLQSPlanner::OptimizePolicy(int horizon) {
-  previous_active_policy = active_policy;
-  if (previous_active_policy == kiLQG) {
-    // the trajectory policy of iLQG (the previous winner) -> spline parameters: least-squares inverse of the
-    // parameter-to-action mapping (ilqs/planner.cc:98-172)
-    if (ilqg.NominalTrajectory(horizon) < 0) return -1;
-    const int P = sampling.policy.num_spline_points, T = horizon - 1;
-    const double shift = std::max((horizon - 1) * timestep_ / std::max(P - 1, 1), 1.0e-5);
-    std::vector<double> times(P), W;
-    for (int t = 0; t < P; t++) times[t] = sampling.time() + shift * t;
-    SplineMapping((int)sampling.interpolation(), times, ilqg.candidate_times().data(), T, &W);
-    // M = W' W (P x P), Cholesky, parameters = M^-1 W' actions
-    std::vector<double> M((size_t)P * P, 0.0), rhs((size_t)P * nu_, 0.0);
-    for (int t = 0; t < T; t++)
-      for (int p = 0; p < P; p++) {
-        const double w = W[(size_t)t * P + p];
-        if (w == 0.0) continue;
-        for (int q = 0; q < P; q++) M[(size_t)p * P + q] += w * W[(size_t)t * P + q];
-        for (int j = 0; j < nu_; j++) rhs[(size_t)p * nu_ + j] += w * (double)ilqg.candidate_actions()[(size_t)t * nu_ + j];
-      }
-    CholFactor(M.data(), P, 1e-15);                                 // in-place Cholesky (mju_cholFactor)
-    for (int j = 0; j < nu_; j++) {                                 // L L' x = rhs, column by column
-      for (int i = 0; i < P; i++) { double a = rhs[(size_t)i * nu_ + j]; for (int k = 0; k < i; k++) a -= M[(size_t)i * P + k] * rhs[(size_t)k * nu_ + j]; rhs[(size_t)i * nu_ + j] = a / M[(size_t)i * P + i]; }
-      for (int i = P - 1; i >= 0; i--) { double a = rhs[(size_t)i * nu_ + j]; for (int k = i + 1; k < P; k++) a -= M[(size_t)k * P + i] * rhs[(size_t)k * nu_ + j]; rhs[(size_t)i * nu_ + j] = a / M[(size_t)i * P + i]; }
+void iLQSPlanner::ConvertToSpline(int horizon) {
+  // the trajectory policy of iLQG (the previous winner) -> spline parameters: least-squares inverse of the
+  // parameter-to-action mapping (ilqs/planner.cc:98-172)
+  const int P = sampling.policy.num_spline_points, T = horizon - 1;
+  const double shift = std::max((horizon - 1) * timestep_ / std::max(P - 1, 1), 1.0e-5);
+  std::vector<double> times(P), W;
+  for (int t = 0; t < P; t++) times[t] = sampling.time() + shift * t;
+  SplineMapping((int)sampling.interpolation(), times, ilqg.candidate_times().data(), T, &W);
+  // M = W' W (P x P), Cholesky, parameters = M^-1 W' actions
+  std::vector<double> M((size_t)P * P, 0.0), rhs((size_t)P * nu_, 0.0);
+  for (int t = 0; t < T; t++)
+    for (int p = 0; p < P; p++) {
+      const double w = W[(size_t)t * P + p];
+      if (w == 0.0) continue;
+      for (int q = 0; q < P; q++) M[(size_t)p * P + q] += w * W[(size_t)t * P + q];
+      for (int j = 0; j < nu_; j++) rhs[(size_t)p * nu_ + j] += w * (double)ilqg.candidate_actions()[(size_t)t * nu_ + j];
     }
-    const std::vector<double>& cr = sampling.policy.ctrlrange;
-    for (int t = 0; t < P; t++)
-      for (int j = 0; j < nu_; j++) rhs[(size_t)t * nu_ + j] = std::max(cr[2 * j], std::min(cr[2 * j + 1], rhs[(size_t)t * nu_ + j]));
-    sampling.SetPolicy(times.data(), rhs.data(), P);
+  CholFactor(M.data(), P, 1e-15);                                 // in-place Cholesky (mju_cholFactor)
+  for (int j = 0; j < nu_; j++) {                                 // L L' x = rhs, column by column
+    for (int i = 0; i < P; i++) { double a = rhs[(size_t)i * nu_ + j]; for (int k = 0; k < i; k++) a -= M[(size_t)i * P + k] * rhs[(size_t)k * nu_ + j]; rhs[(size_t)i * nu_ + j] = a / M[(size_t)i * P + i]; }
+    for (int i = P - 1; i >= 0; i--) { double a = rhs[(size_t)i * nu_ + j]; for (int k = i + 1; k < P; k++) a -= M[(size_t)k * P + i] * rhs[(size_t)k * nu_ + j]; rhs[(size_t)i * nu_ + j] = a / M[(size_t)i * P + i]; }
   }
-  // try sampling
-  if (sampling.OptimizePolicy(horizon) < 0) return -1;
+  const std::vector<double>& cr = sampling.policy.ctrlrange;
+  for (int t = 0; t < P; t++)
+    for (int j = 0; j < nu_; j++) rhs[(size_t)t * nu_ + j] = std::max(cr[2 * j], std::min(cr[2 * j + 1], rhs[(size_t)t * nu_ + j]));
+  sampling.SetPolicy(times.data(), rhs.data(), P);
+}
+
+int iLQSPlanner::SamplingSettled(int horizon) {
   const double ref = previous_active_policy == kSampling ? (double)sampling.returns()[0] : ilqg.candidate_return();
   if (sampling.winner > 0 && (double)sampling.returns()[sampling.winner] < ref) {
     active_policy = kSampling;   // best rollout is from sampling: terminate early (:190-207)
@@ -278,14 +311,30 @@ int iLQSPlanner::OptimizePolicy(int horizon) {
     if (sampling.CandidateTrajectory(0, horizon, &t0)) return -1;
     ilqg.SetCandidateTrajectory(t0);
   }
-  const int ok = ilqg.Iteration(horizon);
-  if (ok < 0) return -1;
+  return 0;
+}
+
+int iLQSPlanner::Accept(int ok) {
   if (ok == 1) {
     // ilqg.trajectory[0] is the action rollout with the SMALLEST non-zero step (LogScale ascends): restated literally (:220-224)
     const double old = previous_active_policy == kSampling ? (double)sampling.returns()[sampling.winner] : (double)ilqg.rollout_return(0);
     if (ilqg.total_return < old) active_policy = kiLQG;
   }
   return ok;
+}
+
+int iLQSPlanner::OptimizePolicy(int horizon) {
+  BeginIteration();
+  if (previous_active_policy == kiLQG) {
+    if (ilqg.NominalTrajectory(horizon) < 0) return -1;
+    ConvertToSpline(horizon);
+  }
+  // try sampling
+  if (sampling.OptimizePolicy(horizon) < 0) return -1;
+  if (const int settled = SamplingSettled(horizon)) return settled;
+  const int ok = ilqg.Iteration(horizon);
+  if (ok < 0) return -1;
+  return Accept(ok);
 }
 
 int iLQSPlanner::NominalTrajectory(int horizon) {
@@ -313,6 +362,13 @@ void mjpc_b200_host_spline_mapping(int representation, const double* input_times
   std::vector<double> ti(input_times, input_times + num_input), w;
   mjpc_b200_host::SplineMapping(representation, ti, output_times, num_output, &w);
   std::copy(w.begin(), w.end(), W);
+}
+
+void mjpc_b200_host_gradient_sweep(const float* A, const float* B, const float* cx, const float* cu, int n, int m, int T,
+                                   double* k, double* dV0) {
+  std::vector<double> kv;
+  mjpc_b200_host::GradientSweep(A, B, cx, cu, n, m, T, &kv, dV0);
+  std::copy(kv.begin(), kv.end(), k);
 }
 
 int mjpc_b200_gradient_planner_create(const mjpc_model_blob* model, int num_trajectory, int num_spline_points, int representation,

@@ -6,7 +6,8 @@
 // = FindInterval + Zero/Linear/CubicInterpolation + Clamp, gradient/policy.cc:80-103, which for >= 3 spline points is the
 // function TimeSpline::Sample evaluates on the device), ModelDerivatives::Compute -> mjpc_b200_model_derivatives,
 // CostDerivatives::Compute -> mjpc_b200_cost_derivatives.  Gradient::Compute (a sequential O(H n^2) recursion) and the
-// spline mappings are host arithmetic in double, as in the reference.
+// spline mappings are host arithmetic in double, as in the reference.  BatchGradientPlanner (batch_planner.h) runs the
+// recursion of all its problems on the device instead (mjpc_b200_gradient_batched), bitwise equal to GradientSweep.
 #pragma once
 #include <memory>
 #include <shared_mutex>
@@ -46,10 +47,20 @@ struct GradientPolicy {                 // gradient/policy.h:29-68
 
 class GradientPlanner : public Planner {
  public:
+  // borrowed != nullptr: plan on that handle (BatchGradientPlanner), else on a handle of its own
   int Initialize(const mjpc_model_blob* model, int num_trajectory, int num_spline_points, int representation,
-                 double timestep, const double* ctrlrange, int max_horizon, int device);
+                 double timestep, const double* ctrlrange, int max_horizon, int device, mjpc_b200_t* borrowed = nullptr);
   void Reset(int horizon, const double* initial_repeated_action) override;
   int OptimizePolicy(int horizon) override;              // planner.cc:159-330; 1 = improved, 0 = not, <0 error
+  // OptimizePolicy in halves around its launches and its gradient, which a batch makes for many planners at once.
+  // Returns / failures are this planner's [N] of a launch, its candidate 0 at flat index `offset`.
+  const SplineCandidates* PrepareNominal(int horizon);   // resample; the nominal (N = 1); nullptr for a bad horizon
+  int InstallNominal(int horizon, const float* returns, const uint8_t* failure, int offset);   // <0: fetch failed
+  // k [horizon][nu] and dV0 of the nominal (Gradient::Compute) -> spline mapping, update, the K line-search candidates
+  const SplineCandidates& PrepareLineSearch(int horizon, const double* k, double dV0);
+  int InstallLineSearch(int horizon, const float* returns, const uint8_t* failure, int offset);   // <0: fetch failed
+  int Publish();                                         // the policy update; 1 = improved, 0 = not
+  const Trajectory& nominal() const { return best_; }    // trajectory[0]: what the derivatives are taken along
   int NominalTrajectory(int) override { return 0; }      // not restated: planning disabled leaves the plan as it is
   void ResamplePolicy(int horizon);                      // :356-383
   // the policy does not depend on the state
@@ -65,12 +76,17 @@ class GradientPlanner : public Planner {
   double action_step = 0, expected = 0, improvement = 0, surprise = 0, total_return = 0;
 
  private:
-  int Rollouts(const std::vector<double>& parameters, int count, int horizon);   // count candidates [count][P][nu]
+  // the first count candidates [count][P][nu] of parameters as float knots on cand_'s times
+  void Candidates(const std::vector<double>& parameters, int count, SplineCandidates* c) const;
+  int Launch(const SplineCandidates& c, int horizon);   // this planner's own launch into ret_ / fail_ / order_
   int Fetch(int candidate, int horizon, double ret);     // trajectory[0] = trajectory[candidate], never a failure
   int K_ = 32, nu_ = 0, n_ = 0, nr_ = 0, Hmax_ = 0;
   double timestep_ = 0.01;
   GradientPolicy cand_;                                   // candidate_policy[0]
-  std::vector<float> A_, B_, C_, D_, cx_, cu_, cxx_, cuu_, cxu_, knots_, ret_;
+  SplineCandidates nominal_, lines_;
+  std::vector<double> steps_, candidates_, update_, W_;   // line search of the iteration
+  double c_prev_ = 0, c_best_ = 0, dV0_ = 0;
+  std::vector<float> A_, B_, C_, D_, cx_, cu_, cxx_, cuu_, cxu_, ret_;
   std::vector<uint8_t> fail_;
   std::vector<int> order_;
   Trajectory best_;                                       // trajectory[0] / trajectory[winner]
@@ -81,12 +97,23 @@ class GradientPlanner : public Planner {
 class iLQSPlanner : public Planner {
  public:
   enum { kSampling = 0, kiLQG = 1 };
+  // sampling_gpu / ilqg_gpu != nullptr: plan the two halves on those handles (BatchILQSPlanner), else on handles of
+  // their own
   int Initialize(const mjpc_model_blob* model, int num_trajectory, int num_spline_points, int interpolation,
                  double exploration, double timestep, const double* ctrlrange, uint32_t seed, int ilqg_num_rollouts,
-                 int ilqg_representation, double fd_tolerance, int max_horizon, int device);
+                 int ilqg_representation, double fd_tolerance, int max_horizon, int device,
+                 mjpc_b200_t* sampling_gpu = nullptr, mjpc_b200_t* ilqg_gpu = nullptr);
   void Reset(int horizon, const double* initial_repeated_action) override;
   void SetState(const double* state, double time, const double* mocap) override;
   int OptimizePolicy(int horizon) override;
+  // OptimizePolicy in halves around its calls, which a batch makes for many planners at once:
+  //   BeginIteration; if previous_active_policy == kiLQG: ilqg.NominalTrajectory, then ConvertToSpline;
+  //   sampling.OptimizePolicy; SamplingSettled (1: sampling won, done; 0: ilqg is seeded; <0 error);
+  //   ilqg.Iteration -> Accept(its code).
+  void BeginIteration() { previous_active_policy = active_policy; }
+  void ConvertToSpline(int horizon);   // the iLQG trajectory policy -> spline parameters of the sampling planner
+  int SamplingSettled(int horizon);
+  int Accept(int ok);                  // acceptance of the iLQG iteration; returns ok
   int NominalTrajectory(int horizon) override;
   void ActionFromPolicy(double* action, const double* state, double time, bool use_previous = false) override;
   const Trajectory* BestTrajectory() override {

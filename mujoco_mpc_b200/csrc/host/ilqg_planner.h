@@ -77,7 +77,7 @@ class iLQGPlanner : public Planner {
   int dim_action() const { return nu_; }
 
  private:
-  friend class BatchILQGPlanner;
+  friend class ILQGSweeps;
   std::vector<float> StepSizes() const;                                   // LogScale (utilities.cc:819-825) + trailing 0
   static int BestRollout(const float* ret, const uint8_t* fail, int K);  // :727-740
   // candidate_policy[0].trajectory = trajectory[candidate]; candidate is the flat index of the last launch

@@ -780,6 +780,63 @@ extern "C" __global__ void __launch_bounds__(MJPC_BP_THREADS) backward_pass_kern
   if (tid == 0) { P.dV[0] = s_dV[0]; P.dV[1] = s_dV[1]; *P.status = s_ok; }
 }
 
+// ------------------------------------------------------------------------------------------ gradient sweep
+// Gradient::Compute (mjpc/planners/gradient/gradient.cc:76-107), the loop of the host GradientSweep
+// (csrc/host/gradient_planner.cc) in fp64, one CTA per problem:
+//   Vx = cx[T-1];  for t = T-1 .. 1:  Qx = cx[t-1] + A[t-1]' Vx,  Qu = cu[t-1] + B[t-1]' Vx,  k[t-1] = -Qu,
+//   dV0 += -Qu . Qu,  Vx = Qx;  k[T-1] = k[T-2].
+// Thread j < n sums Qx[j], thread n + j sums Qu[j], each serially over i in the host's order from (double)cx / cu, so
+// that reads of A[t-1] / B[t-1] rows are coalesced over j.  Thread 0 accumulates dV0 in the host's (t descending,
+// j ascending) order.  Every product and sum is rounded on its own (__dmul_rn / __dadd_rn: -use_fast_math would contract
+// them into DFMA), which makes k and dV0 bitwise the host's (baseline x86-64: no FMA).
+struct GradientArgs {
+  const float *A, *B, *cx, *cu;   // [nprob][H][..] as the derivative sweeps leave them
+  double *k, *dV0;                // [nprob][H][m], [nprob]
+  int n, m, H;
+};
+
+extern "C" __global__ void __launch_bounds__(128) gradient_sweep_kernel(const __grid_constant__ GradientArgs P) {
+  extern __shared__ __align__(16) double gsm[];
+  const int n = P.n, m = P.m, H = P.H, tid = threadIdx.x, nt = blockDim.x, b = blockIdx.x;
+  // smem: Vx [2][n] and Qu [2][m], ping-pong by step parity (cur)
+  const float* A = P.A + (size_t)b * H * n * n;
+  const float* Bm = P.B + (size_t)b * H * n * m;
+  const float* cx = P.cx + (size_t)b * H * n;
+  const float* cu = P.cu + (size_t)b * H * m;
+  double* k = P.k + (size_t)b * H * m;
+  for (int j = tid; j < n; j += nt) gsm[j] = (double)cx[(size_t)(H - 1) * n + j];
+  __syncthreads();
+  double dV0 = 0.0;
+  int cur = 0;
+  for (int t = H - 1; t > 0; t--) {
+    const double* Vx = gsm + cur * n;
+    double* Vn = gsm + (cur ^ 1) * n;
+    double* Qu = gsm + 2 * n + cur * m;
+    for (int j = tid; j < n + m; j += nt) {
+      if (j < n) {
+        const float* At = A + (size_t)(t - 1) * n * n;
+        double a = (double)cx[(size_t)(t - 1) * n + j];
+        for (int i = 0; i < n; i++) a = __dadd_rn(a, __dmul_rn((double)At[(size_t)i * n + j], Vx[i]));
+        Vn[j] = a;
+      } else {
+        const int ju = j - n;
+        const float* Bt = Bm + (size_t)(t - 1) * n * m;
+        double a = (double)cu[(size_t)(t - 1) * m + ju];
+        for (int i = 0; i < n; i++) a = __dadd_rn(a, __dmul_rn((double)Bt[(size_t)i * m + ju], Vx[i]));
+        Qu[ju] = a;
+        k[(size_t)(t - 1) * m + ju] = -a;
+        if (t == H - 1) k[(size_t)(H - 1) * m + ju] = -a;   // row H-1 repeats row H-2
+      }
+    }
+    __syncthreads();
+    // this step's Qu is rewritten two steps later, after the next barrier, which thread 0 reaches only once it has read it
+    if (tid == 0)
+      for (int j = 0; j < m; j++) dV0 = __dadd_rn(dV0, __dmul_rn(-Qu[j], Qu[j]));
+    cur ^= 1;
+  }
+  if (tid == 0) P.dV0[b] = dV0;
+}
+
 // ------------------------------------------------------------------------------------------ host launchers
 // (the dynamic shared-memory opt-in is a per-kernel, process-wide attribute: only ever raised; handles may be created
 // from several threads, hence the lock)
@@ -823,6 +880,7 @@ struct IlqgBuffers {
         *res = nullptr, *cx = nullptr, *cu = nullptr, *cxx = nullptr, *cuu = nullptr, *cxu = nullptr, *act = nullptr,
         *K = nullptr, *du = nullptr, *dV = nullptr, *Vx = nullptr, *Vxx = nullptr, *mu = nullptr, *yp = nullptr,
         *rp = nullptr, *iw = nullptr;
+  double *gk = nullptr, *gdV = nullptr;   // gradient sweep: k [nprob][H][nu], dV0 [nprob]
   int* status = nullptr;
   int* idx = nullptr;   // [4 H]: evaluate list, then interpolate t / e0 / e1 (common to all problems)
   std::vector<float**> all() {
@@ -833,6 +891,7 @@ struct IlqgBuffers {
 
 inline void ilqg_free(IlqgBuffers& b) {
   for (float** p : b.all()) if (*p) { cudaFree(*p); *p = nullptr; }
+  for (double** p : {&b.gk, &b.gdV}) if (*p) { cudaFree(*p); *p = nullptr; }
   if (b.status) { cudaFree(b.status); b.status = nullptr; }
   if (b.idx) { cudaFree(b.idx); b.idx = nullptr; }
 }
@@ -852,6 +911,8 @@ inline int ilqg_init(IlqgBuffers& b, const DevModel& M, int H, int nprob = 1) {
   bool ok = true;
   for (auto& e : plan)
     ok = ok && cudaMalloc((void**)e.p, (e.cnt ? e.cnt : 1) * sizeof(float)) == cudaSuccess;
+  ok = ok && cudaMalloc((void**)&b.gk, P * Hs * m * sizeof(double)) == cudaSuccess;
+  ok = ok && cudaMalloc((void**)&b.gdV, P * sizeof(double)) == cudaSuccess;
   ok = ok && cudaMalloc((void**)&b.status, P * sizeof(int)) == cudaSuccess;
   ok = ok && cudaMalloc((void**)&b.idx, (4 * Hs + 8) * sizeof(int)) == cudaSuccess;
   if (!ok) { cudaGetLastError(); ilqg_free(b); return -4; }
@@ -873,7 +934,7 @@ inline int ilqg_reserve(IlqgBuffers& b, const DevModel& M, int nprob, cudaStream
 
 // nprob problems with common H / skip / mode, on the fd_center / fd_column instances given.  Host inputs are [nprob][..]:
 // x, u, trel (relative to each problem's t[0]), mocap, ts (rebased likewise); w / prm (float weights / parameters) may
-// be nullptr for the packed values.
+// be nullptr for the packed values.  A NULL host output A / B / C / D is not copied back: it stays in b only.
 inline int ilqg_model_derivatives(IlqgBuffers& b, const DevModel& M, const float* d_pack, cudaStream_t st,
                                   const void* fd_center, const void* fd_column, int nprob,
                                   const float* x, const float* u, const float* trel, const float* mocap, const float* ts,
@@ -946,11 +1007,11 @@ inline int ilqg_model_derivatives(IlqgBuffers& b, const DevModel& M, const float
   }
   if (e1) ILQG_TRY(cudaEventRecord(e1, st));
   ILQG_TRY(cudaGetLastError());
-  ILQG_TRY(cudaMemcpyAsync(A, b.A, P * H * n * n * 4, cudaMemcpyDeviceToHost, st));
-  ILQG_TRY(cudaMemcpyAsync(B, b.B, P * H * n * m * 4, cudaMemcpyDeviceToHost, st));
-  ILQG_TRY(cudaMemcpyAsync(C, b.C, P * H * nr * n * 4, cudaMemcpyDeviceToHost, st));
-  ILQG_TRY(cudaMemcpyAsync(D, b.D, P * H * nr * m * 4, cudaMemcpyDeviceToHost, st));
-  ILQG_TRY(cudaStreamSynchronize(st));
+  if (A) ILQG_TRY(cudaMemcpyAsync(A, b.A, P * H * n * n * 4, cudaMemcpyDeviceToHost, st));
+  if (B) ILQG_TRY(cudaMemcpyAsync(B, b.B, P * H * n * m * 4, cudaMemcpyDeviceToHost, st));
+  if (C) ILQG_TRY(cudaMemcpyAsync(C, b.C, P * H * nr * n * 4, cudaMemcpyDeviceToHost, st));
+  if (D) ILQG_TRY(cudaMemcpyAsync(D, b.D, P * H * nr * m * 4, cudaMemcpyDeviceToHost, st));
+  if (A || B || C || D) ILQG_TRY(cudaStreamSynchronize(st));
   return 0;
 }
 
@@ -961,15 +1022,19 @@ inline size_t cost_derivatives_smem(const DevModel& M, int kmax) {
 }
 
 // nprob problems; w [nprob][num_term] (float) or nullptr for the packed Task::weight; kmax = the widest cost term
-// (the kernel lays its scratch out with it: the caller checks cost_derivatives_smem against the device limit)
+// (the kernel lays its scratch out with it: the caller checks cost_derivatives_smem against the device limit).
+// cd_resident: C and D are already in b (the model-derivative sweep just left them there) and are not uploaded.  A NULL
+// host output is not copied back.
 inline int ilqg_cost_derivatives(IlqgBuffers& b, const DevModel& M, const float* d_pack, cudaStream_t st, int nprob,
                                  const float* w, const float* residual, const float* C, const float* D, int H, float* cx,
                                  float* cu, float* cxx, float* cuu, float* cxu, int kmax, int* launches,
-                                 cudaEvent_t e0 = nullptr, cudaEvent_t e1 = nullptr) {
+                                 cudaEvent_t e0 = nullptr, cudaEvent_t e1 = nullptr, bool cd_resident = false) {
   const size_t n = b.n, m = b.nu, nr = b.nr, P = nprob;
   ILQG_TRY(cudaMemcpyAsync(b.res, residual, P * H * nr * 4, cudaMemcpyHostToDevice, st));
-  ILQG_TRY(cudaMemcpyAsync(b.C, C, P * H * nr * n * 4, cudaMemcpyHostToDevice, st));
-  ILQG_TRY(cudaMemcpyAsync(b.D, D, P * H * nr * m * 4, cudaMemcpyHostToDevice, st));
+  if (!cd_resident) {
+    ILQG_TRY(cudaMemcpyAsync(b.C, C, P * H * nr * n * 4, cudaMemcpyHostToDevice, st));
+    ILQG_TRY(cudaMemcpyAsync(b.D, D, P * H * nr * m * 4, cudaMemcpyHostToDevice, st));
+  }
   if (w && M.num_term) ILQG_TRY(cudaMemcpyAsync(b.w, w, P * M.num_term * 4, cudaMemcpyHostToDevice, st));
   CostArgs a;
   std::memset(&a, 0, sizeof(a));
@@ -983,11 +1048,28 @@ inline int ilqg_cost_derivatives(IlqgBuffers& b, const DevModel& M, const float*
   if (e1) ILQG_TRY(cudaEventRecord(e1, st));
   *launches += 1;
   ILQG_TRY(cudaGetLastError());
-  ILQG_TRY(cudaMemcpyAsync(cx, b.cx, P * H * n * 4, cudaMemcpyDeviceToHost, st));
-  ILQG_TRY(cudaMemcpyAsync(cu, b.cu, P * H * m * 4, cudaMemcpyDeviceToHost, st));
-  ILQG_TRY(cudaMemcpyAsync(cxx, b.cxx, P * H * n * n * 4, cudaMemcpyDeviceToHost, st));
-  ILQG_TRY(cudaMemcpyAsync(cuu, b.cuu, P * H * m * m * 4, cudaMemcpyDeviceToHost, st));
-  ILQG_TRY(cudaMemcpyAsync(cxu, b.cxu, P * H * n * m * 4, cudaMemcpyDeviceToHost, st));
+  if (cx) ILQG_TRY(cudaMemcpyAsync(cx, b.cx, P * H * n * 4, cudaMemcpyDeviceToHost, st));
+  if (cu) ILQG_TRY(cudaMemcpyAsync(cu, b.cu, P * H * m * 4, cudaMemcpyDeviceToHost, st));
+  if (cxx) ILQG_TRY(cudaMemcpyAsync(cxx, b.cxx, P * H * n * n * 4, cudaMemcpyDeviceToHost, st));
+  if (cuu) ILQG_TRY(cudaMemcpyAsync(cuu, b.cuu, P * H * m * m * 4, cudaMemcpyDeviceToHost, st));
+  if (cxu) ILQG_TRY(cudaMemcpyAsync(cxu, b.cxu, P * H * n * m * 4, cudaMemcpyDeviceToHost, st));
+  if (cx || cu || cxx || cuu || cxu) ILQG_TRY(cudaStreamSynchronize(st));
+  return 0;
+}
+
+// the gradient sweep of nprob problems on the A, B, cx and cu the derivative sweeps left in b; k [nprob][H][nu] and
+// dV0 [nprob] (double) copied to the host
+inline int ilqg_gradient_sweep(IlqgBuffers& b, cudaStream_t st, int nprob, int H, double* k, double* dV0, int* launches,
+                               cudaEvent_t e1 = nullptr) {
+  const size_t m = b.nu, P = nprob;
+  GradientArgs a;
+  a.A = b.A; a.B = b.B; a.cx = b.cx; a.cu = b.cu; a.k = b.gk; a.dV0 = b.gdV; a.n = b.n; a.m = b.nu; a.H = H;
+  gradient_sweep_kernel<<<nprob, 128, (2 * b.n + 2 * b.nu) * sizeof(double), st>>>(a);
+  if (e1) ILQG_TRY(cudaEventRecord(e1, st));
+  *launches += 1;
+  ILQG_TRY(cudaGetLastError());
+  ILQG_TRY(cudaMemcpyAsync(k, b.gk, P * H * m * sizeof(double), cudaMemcpyDeviceToHost, st));
+  ILQG_TRY(cudaMemcpyAsync(dV0, b.gdV, P * sizeof(double), cudaMemcpyDeviceToHost, st));
   ILQG_TRY(cudaStreamSynchronize(st));
   return 0;
 }

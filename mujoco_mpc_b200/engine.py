@@ -58,7 +58,11 @@ EXPORTS = ["mjpc_b200_version", "mjpc_b200_last_error", "mjpc_b200_create", "mjp
            "mjpc_b200_sg_planner_create", "mjpc_b200_sg_planner_get_result", "mjpc_b200_ilqg_planner_create",
            "mjpc_b200_ilqg_planner_get_result", "mjpc_b200_host_ilqg_policy_action", "mjpc_b200_robust_planner_create",
            "mjpc_b200_robust_planner_get_result", "mjpc_b200_gradient_planner_create",
-           "mjpc_b200_gradient_planner_get_result", "mjpc_b200_host_spline_mapping", "mjpc_b200_ilqs_planner_create",
+           "mjpc_b200_gradient_planner_get_result", "mjpc_b200_host_spline_mapping", "mjpc_b200_host_gradient_sweep",
+           "mjpc_b200_gradient_batched", "mjpc_b200_batch_gradient_planner_create",
+           "mjpc_b200_batch_gradient_planner_get_result", "mjpc_b200_batch_planner_set_fd",
+           "mjpc_b200_batch_ilqs_planner_create", "mjpc_b200_batch_ilqs_planner_get_result",
+           "mjpc_b200_batch_ilqs_planner_set_exploration", "mjpc_b200_batch_ilqs_planner_action_from_policy", "mjpc_b200_ilqs_planner_create",
            "mjpc_b200_ilqs_planner_set_exploration", "mjpc_b200_ilqs_planner_get_result",
            "mjpc_b200_set_options", "mjpc_b200_agent_steps", "mjpc_b200_agent_create", "mjpc_b200_agent_destroy",
            "mjpc_b200_agent_reset", "mjpc_b200_agent_set_state", "mjpc_b200_agent_set_task", "mjpc_b200_agent_set_plan_enabled",
@@ -115,6 +119,7 @@ def load_library():
             f.argtypes, f.restype = [C.c_void_p] + args, C.c_int
         lib.mjpc_b200_estimator_last_error.restype = C.c_char_p
         lib.mjpc_b200_batch_planner_destroy.argtypes = [C.c_void_p]
+        lib.mjpc_b200_batch_planner_set_fd.argtypes = [C.c_void_p, C.c_double, C.c_int, C.c_int]
         lib.mjpc_b200_planner_set_task.argtypes = [C.c_void_p, C.c_void_p]
         lib.mjpc_b200_set_xfrc_noise_batched.argtypes = [C.c_void_p, C.c_double, C.c_double, C.c_int,
                                                          C.POINTER(C.c_uint32)]
@@ -126,6 +131,7 @@ def load_library():
         lib.mjpc_b200_agent_steps.argtypes = [C.c_double, C.c_double]
         lib.mjpc_b200_set_options.argtypes = [C.c_void_p, C.c_double, C.c_int]
         lib.mjpc_b200_ilqs_planner_set_exploration.argtypes = [C.c_void_p, C.c_double]
+        lib.mjpc_b200_batch_ilqs_planner_set_exploration.argtypes = [C.c_void_p, C.c_double]
         lib.mjpc_b200_shadow_transition_destroy.argtypes = [C.c_void_p]
         for n in ("mjpc_b200_quadruped_transition_create", "mjpc_b200_track_transition_create", "mjpc_b200_shadow_transition_create"):
             getattr(lib, n).restype = C.c_void_p
@@ -608,6 +614,19 @@ class Engine:
                                                              _pf(Vxx), status.ctypes.data_as(_ip)))
         return dict(K=K, du=du, dV=dV, Vx=Vx, Vxx=Vxx, status=status)
 
+    def gradient_batched(self, x, u, t, mocaps, residual, tol, skip=0, mode=0, weights=None, parameters=None,
+                         task_states=None):
+        """Gradient::Compute for B problems on the device (mjpc_b200_gradient_batched): the inputs of
+        model_derivatives_batched plus residual [B, H, nr].  Returns k [B, H, nu] and dV0 [B] (double)."""
+        x, u, t, mc, r = _f(x), _f(u), _d(t), _f(mocaps), _f(residual)
+        w, p, s = _d(weights), _d(parameters), _d(task_states)
+        Bn, H = x.shape[:2]
+        k = np.zeros((Bn, H, self.nu)); dV0 = np.zeros(Bn)
+        self._check(self.lib.mjpc_b200_gradient_batched(self.h, int(Bn), _pf(x), _pf(u), _pd(t), _pf(mc), _pd(w), _pd(p),
+                                                        _pd(s), _pf(r), int(H), int(skip), C.c_float(tol), int(mode),
+                                                        _pd(k), _pd(dV0)))
+        return k, dV0
+
     def fetch_stats(self):
         st = np.zeros((self.lastN, 12), np.int64)
         self._check(self.lib.mjpc_b200_fetch_stats(self.h, st.ctypes.data_as(C.POINTER(C.c_int64))))
@@ -962,6 +981,95 @@ def host_spline_mapping(representation, input_times, output_times):
     W = np.zeros((len(to), len(ti)))
     lib.mjpc_b200_host_spline_mapping(int(representation), _pd(ti), len(ti), _pd(to), len(to), _pd(W))
     return W
+
+
+def host_gradient_sweep(A, B, cx, cu):
+    """Gradient::Compute's recursion on the host in fp64 (mjpc_b200_host_gradient_sweep, no device): A [T, n, n],
+    B [T, n, m], cx [T, n], cu [T, m] (float32) -> k [T, m], dV0."""
+    lib = load_library()
+    a, b, x, u = _f(A), _f(B), _f(cx), _f(cu)
+    T, n, m = b.shape
+    k, dV0 = np.zeros((T, m)), C.c_double()
+    lib.mjpc_b200_host_gradient_sweep(_pf(a), _pf(b), _pf(x), _pf(u), int(n), int(m), int(T), _pd(k), C.byref(dV0))
+    return k, dV0.value
+
+
+class _CppBatchCodePlanner(_CppBatchPlanner):
+    """A batch whose optimize_policy returns each problem's code, as the single planner's does (Gradient, iLQS); the
+    kind's _get_result takes _NRESULT output pointers, then the code's."""
+    _NRESULT = 0
+
+    def set_fd(self, tolerance, mode=-1, derivative_skip=-1):
+        self._check(self.lib.mjpc_b200_batch_planner_set_fd(self.h, C.c_double(tolerance), int(mode), int(derivative_skip)),
+                    "set_fd")
+
+    def optimize_policy(self):
+        """One planning iteration of every problem; returns each problem's 1 (improved) / 0."""
+        self._check(self.lib.mjpc_b200_batch_planner_optimize_policy(self.h, self.horizon), "optimize_policy")
+        return [self._improved(b) for b in range(self.B)]
+
+    def _improved(self, problem):
+        imp = C.c_int()
+        self._check(getattr(self.lib, f"{self._prefix}_get_result")(self.h, int(problem), *([None] * self._NRESULT),
+                                                                      C.byref(imp)), "get_result")
+        return imp.value
+
+
+class CppBatchGradientPlanner(_CppBatchCodePlanner):
+    """num_problems independent Gradient problems (csrc/host/batch_planner.cc): per iteration one launch of the B
+    nominals, one mjpc_b200_gradient_batched and one launch of the B x num_trajectory line-search candidates.  Mirrors
+    CppGradientPlanner with a problem argument; optimize_policy returns each problem's 1/0."""
+    _NRESULT = 3
+
+    def __init__(self, model, num_problems, horizon, num_trajectory=8, num_spline_points=5, representation=1,
+                 fd_tolerance=3e-4, device=0, fd_mode=1):
+        cr = _d(np.asarray(model.actuator_ctrlrange, float).reshape(-1))
+        self.B, self.horizon, self.P, self.nu = int(num_problems), int(horizon), int(num_spline_points), model.nu
+        self._create("mjpc_b200_batch_gradient_planner", model, self.B, int(num_trajectory), self.P, int(representation),
+                     C.c_double(fd_tolerance), C.c_double(float(model.opt_timestep)), _pd(cr), self.horizon, int(device))
+        self.set_fd(fd_tolerance, fd_mode, -1)
+
+    def result(self, problem):
+        sc = np.zeros(6); p = np.zeros((self.P, self.nu)); t = np.zeros(self.P); imp = C.c_int()
+        self._check(self.lib.mjpc_b200_batch_gradient_planner_get_result(self.h, int(problem), _pd(sc), _pd(p), _pd(t),
+                                                                         C.byref(imp)), "get_result")
+        return dict(total_return=sc[0], winner=int(sc[1]), action_step=sc[2], expected=sc[3], improvement=sc[4],
+                    surprise=sc[5], parameters=p, times=t, improved=imp.value)
+
+
+class CppBatchILQSPlanner(_CppBatchCodePlanner):
+    """num_problems independent iLQS problems (csrc/host/batch_planner.cc) on two handles: per iteration one feedback
+    launch of the iLQG nominals that need converting, one sampling launch of B x num_trajectory, and one batched iLQG
+    iteration of the problems sampling did not settle.  Mirrors CppILQSPlanner with a problem argument;
+    optimize_policy returns each problem's 1/0."""
+    _NRESULT = 1
+
+    def __init__(self, model, num_problems, horizon, num_trajectory=8, num_rollouts=6, fd_tolerance=3e-4, seeds=None,
+                 device=0, fd_mode=1):
+        num, cr, sd = self._setup(model, num_problems, horizon, num_trajectory, seeds)
+        self._create("mjpc_b200_batch_ilqs_planner", model, self.B, self.N, self.P,
+                     int(num.get("sampling_representation", [2])[0]),
+                     C.c_double(float(num.get("sampling_exploration", [0.1])[0])), C.c_double(float(model.opt_timestep)),
+                     cr, sd, int(num_rollouts), int(num.get("ilqg_representation", [1])[0]), C.c_double(fd_tolerance),
+                     self.horizon, int(device))
+        self.set_fd(fd_tolerance, fd_mode, -1)
+
+    def set_exploration(self, sigma):
+        self._check(self.lib.mjpc_b200_batch_ilqs_planner_set_exploration(self.h, C.c_double(sigma)), "set_exploration")
+
+    def result(self, problem):
+        sc, imp = np.zeros(4), C.c_int()
+        self._check(self.lib.mjpc_b200_batch_ilqs_planner_get_result(self.h, int(problem), _pd(sc), C.byref(imp)),
+                    "get_result")
+        return dict(active_policy=int(sc[0]), sampling_return=sc[1], ilqg_return=sc[2], sampling_winner=int(sc[3]),
+                    improved=imp.value)
+
+    def action_from_policy(self, problem, time, state=None, use_previous=False):
+        a, s = np.zeros(self.nu), _d(state)
+        self._check(self.lib.mjpc_b200_batch_ilqs_planner_action_from_policy(self.h, int(problem), _pd(a), _pd(s),
+                                                                             C.c_double(time), int(use_previous)),
+                    "action_from_policy")
+        return a
 
 
 class CppGradientPlanner(_CppPlanner):
