@@ -33,11 +33,9 @@ def _compile(verbose):
     cmd = [nvcc] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-o", SO, os.path.join(CSRC, "engine.cu"), os.path.join(CSRC, "host", "planner.cc"),
                                                                            os.path.join(CSRC, "host", "sampling_planner.cc"),
                                                                            os.path.join(CSRC, "host", "batch_planner.cc"),
-                                                                           os.path.join(CSRC, "host", "batch_sampling_planner.cc"),
                                                                            os.path.join(CSRC, "host", "cross_entropy_planner.cc"),
                                                                            os.path.join(CSRC, "host", "sample_gradient_planner.cc"),
                                                                            os.path.join(CSRC, "host", "ilqg_planner.cc"),
-                                                                           os.path.join(CSRC, "host", "batch_ilqg_planner.cc"),
                                                                            os.path.join(CSRC, "host", "robust_planner.cc"),
                                                                            os.path.join(CSRC, "host", "gradient_planner.cc"),
                                                                            os.path.join(CSRC, "host", "agent.cc"),

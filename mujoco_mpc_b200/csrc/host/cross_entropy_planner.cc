@@ -100,21 +100,29 @@ const SplineCandidates& CrossEntropyPlanner::PrepareCandidates(int horizon) {
   return cands_;
 }
 
-int CrossEntropyPlanner::OptimizePolicy(int horizon) {
-  const SplineCandidates& c = PrepareCandidates(horizon);
-  order_all_.resize(c.N);
-  if (RolloutSpline(c, horizon, returns_.data(), failure_.data(), order_all_.data())) return -1;
-  InstallRollouts(horizon, returns_.data(), failure_.data(), order_all_.data(), 0);
+int CrossEntropyPlanner::Iterate(const std::vector<CrossEntropyPlanner*>& ps, const TaskRows& rows, int horizon,
+                                 SplineLaunch* launch) {
+  std::vector<const SplineCandidates*> cands;
+  for (CrossEntropyPlanner* p : ps) cands.push_back(&p->PrepareCandidates(horizon));
+  if (int rc = launch->Run(std::vector<const Planner*>(ps.begin(), ps.end()), cands, rows, horizon)) return rc;
+  const int N1 = cands[0]->N;
+  for (size_t b = 0; b < ps.size(); b++) {
+    const size_t o = b * N1;
+    ps[b]->InstallRollouts(horizon, launch->returns.data() + o, launch->failure.data() + o, launch->order.data() + o,
+                           (int)o);
+  }
   return 0;
+}
+
+int CrossEntropyPlanner::OptimizePolicy(int horizon) {
+  return Iterate({this}, TaskRows(), horizon, &launch_) ? -1 : 0;
 }
 
 void CrossEntropyPlanner::InstallRollouts(int horizon, const float* returns, const uint8_t* failure, const int* order,
                                           int offset) {
   const int num_trajectory = num_trajectory_, n_elite = n_elite_;
-  if (returns != returns_.data()) {
-    std::copy(returns, returns + num_trajectory + 1, returns_.begin());
-    std::copy(failure, failure + num_trajectory + 1, failure_.begin());
-  }
+  std::copy(returns, returns + num_trajectory + 1, returns_.begin());
+  std::copy(failure, failure + num_trajectory + 1, failure_.begin());
   launch_offset_ = offset; horizon_ = horizon;
   // the device ranked all N+1 launches; the elite ranking is over the N noisy candidates only (:181-193)
   int r = 0;

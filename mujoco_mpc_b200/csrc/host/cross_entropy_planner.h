@@ -1,6 +1,6 @@
 // cross_entropy_planner.h - C++ host side of the Cross-Entropy Method planner with the reference's method names
 // (mjpc/planners/cross_entropy/planner.h:35-146, planner.cc:38-470).  Same rollout engine call as the sampling
-// planner: Rollouts is ONE mjpc_b200_rollout_spline call over N noisy candidates + the un-noised nominal
+// planner: Rollouts is ONE spline launch over N noisy candidates + the un-noised nominal
 // (candidate N) where the reference schedules N+1 closures on its ThreadPool (planner.cc:414-459).
 // Noise comes from the injected Philox stream (sampling_planner.h), counter (iteration, candidate, knot, dof).
 #pragma once
@@ -17,7 +17,11 @@ class CrossEntropyPlanner : public Planner {
                  double std_initial, double std_min, double explore_fraction, double timestep, const double* ctrlrange,
                  uint32_t seed, int max_horizon, int device, mjpc_b200_t* engine = nullptr);
   void Reset(int horizon, const double* initial_repeated_action) override;   // :121-150 (variance = std_initial^2)
-  int OptimizePolicy(int horizon) override;           // :153-292: the two halves below around one launch
+  int OptimizePolicy(int horizon) override;           // :153-292: Iterate over this planner alone
+  // OptimizePolicy of every planner of ps, which plan on one handle: the two halves below around ONE launch of all
+  // their candidates; problem b reads task row b of `rows`.  0, or the launch's error code
+  static int Iterate(const std::vector<CrossEntropyPlanner*>& ps, const TaskRows& rows, int horizon,
+                     SplineLaunch* launch);
   // ... before the launch: ResamplePolicy and the candidates of Rollouts (:414-459), the N noisy ones and the nominal
   // last (N + 1 in all)
   const SplineCandidates& PrepareCandidates(int horizon);
@@ -49,7 +53,6 @@ class CrossEntropyPlanner : public Planner {
   SplineCandidates cands_;
   std::vector<float> returns_;
   std::vector<uint8_t> failure_;
-  std::vector<int> order_all_;
   Trajectory nominal_;
   mutable std::shared_mutex mtx_;
 };

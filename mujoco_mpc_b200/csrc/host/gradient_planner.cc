@@ -96,7 +96,7 @@ int GradientPlanner::Initialize(const mjpc_model_blob* model, int num_trajectory
                                 double timestep, const double* ctrlrange, int max_horizon, int device, mjpc_b200_t* borrowed) {
   K_ = std::max(num_trajectory, 1);
   if (int rc = AttachEngine(model, K_, max_horizon, device, borrowed)) return rc;
-  nu_ = info_.nu; n_ = info_.dim_dstate; nr_ = info_.num_residual; Hmax_ = info_.max_horizon;
+  nu_ = info_.nu; nr_ = info_.num_residual; Hmax_ = info_.max_horizon;
   timestep_ = timestep;
   policy.nu = nu_; policy.num_spline_points = num_spline_points; policy.representation = representation;
   policy.ctrlrange.assign(ctrlrange, ctrlrange + 2 * nu_);
@@ -130,11 +130,6 @@ void GradientPlanner::Candidates(const std::vector<double>& parameters, int coun
   c->interpolation = cand_.representation;
   for (size_t i = 0; i < c->knots.size(); i++) c->knots[i] = (float)parameters[i];
   std::copy(cand_.times.begin(), cand_.times.end(), c->knot_times.begin());
-}
-
-int GradientPlanner::Launch(const SplineCandidates& c, int horizon) {
-  ret_.assign(c.N, 0.f); fail_.assign(c.N, 0); order_.assign(c.N, 0);
-  return RolloutSpline(c, horizon, ret_.data(), fail_.data(), order_.data());
 }
 
 int GradientPlanner::Fetch(int candidate, int horizon, double ret) {
@@ -216,30 +211,52 @@ int GradientPlanner::Publish() {
   return c_best_ < c_prev_ ? 1 : 0;
 }
 
-int GradientPlanner::OptimizePolicy(int horizon) {
-  if (horizon < 2 || horizon > Hmax_) return -1;
-  const size_t H = horizon, n = n_, m = nu_, nr = nr_;
-  const DifferentiableScope diff(gpu_, settings.differentiable != 0);
-  const SplineCandidates* nominal = PrepareNominal(horizon);
-  if (Launch(*nominal, horizon) || InstallNominal(horizon, ret_.data(), fail_.data(), 0)) return -1;
-  A_.resize(H * n * n); B_.resize(H * n * m); C_.resize(H * nr * n); D_.resize(H * nr * m);
-  cx_.resize(H * n); cu_.resize(H * m); cxx_.resize(H * n * n); cuu_.resize(H * m * m); cxu_.resize(H * n * m);
-  std::vector<float> mc(mocap_.begin(), mocap_.end());
-  std::vector<double> k;
-  for (int it = 0; it < settings.max_rollout; it++) {
-    if (mjpc_b200_model_derivatives(gpu_, best_.states.data(), best_.actions.data(), best_.times.data(),
-                                    mc.empty() ? nullptr : mc.data(), horizon, settings.derivative_skip,
-                                    (float)settings.fd_tolerance, settings.fd_mode, A_.data(), B_.data(), C_.data(), D_.data()))
-      return -1;
-    if (mjpc_b200_cost_derivatives(gpu_, best_.residual.data(), C_.data(), D_.data(), horizon, cx_.data(), cu_.data(),
-                                   cxx_.data(), cuu_.data(), cxu_.data()))
-      return -1;
-    double dV0 = 0;
-    GradientSweep(A_.data(), B_.data(), cx_.data(), cu_.data(), (int)n, (int)m, horizon, &k, &dV0);
-    if (Launch(PrepareLineSearch(horizon, k.data(), dV0), horizon)) return -1;
-    if (InstallLineSearch(horizon, ret_.data(), fail_.data(), 0)) return -1;
+int GradientPlanner::Iterate(const std::vector<GradientPlanner*>& ps, const TaskRows& rows, int horizon,
+                             SplineLaunch* launch, int* improved) {
+  const size_t B = ps.size();
+  std::fill(improved, improved + B, 0);
+  const GradientPlannerSettings& s = ps[0]->settings;
+  const DifferentiableScope diff(ps[0]->gpu_, s.differentiable != 0);
+  const std::vector<const Planner*> from(ps.begin(), ps.end());
+  std::vector<const SplineCandidates*> cands(B);
+  for (size_t b = 0; b < B; b++)
+    if (!(cands[b] = ps[b]->PrepareNominal(horizon))) return MJPC_B200_ERR_BAD_ARGUMENT;
+  if (int rc = launch->Run(from, cands, rows, horizon)) return rc;
+  for (size_t b = 0; b < B; b++)
+    if (ps[b]->InstallNominal(horizon, launch->returns.data() + b, launch->failure.data() + b, (int)b)) return -1;
+  // the nominals' trajectories [B][H][..] and mocaps [B][7 nmocap] (float, as the handle stages its own)
+  const size_t H = horizon, ds = ps[0]->info_.dim_state, nu = ps[0]->nu_, nr = ps[0]->nr_, nm = ps[0]->mocap_.size();
+  std::vector<float> x(B * H * ds), u(B * H * nu), res(B * H * nr), mc(B * nm);
+  std::vector<double> t(B * H), k(B * H * nu), dV0(B);
+  for (int it = 0; it < s.max_rollout; it++) {
+    for (size_t b = 0; b < B; b++) {
+      const Trajectory& tr = ps[b]->best_;
+      std::copy(tr.states.begin(), tr.states.begin() + H * ds, x.begin() + b * H * ds);
+      std::copy(tr.actions.begin(), tr.actions.begin() + H * nu, u.begin() + b * H * nu);
+      std::copy(tr.residual.begin(), tr.residual.begin() + H * nr, res.begin() + b * H * nr);
+      std::copy(tr.times.begin(), tr.times.begin() + H, t.begin() + b * H);
+      std::copy(ps[b]->mocap_.begin(), ps[b]->mocap_.end(), mc.begin() + b * nm);
+    }
+    if (int rc = mjpc_b200_gradient_batched(ps[0]->gpu_, (int)B, x.data(), u.data(), t.data(), nm ? mc.data() : nullptr,
+                                            rows.nw ? rows.w : nullptr, rows.np ? rows.p : nullptr,
+                                            rows.nts ? rows.ts : nullptr, res.data(), horizon, s.derivative_skip,
+                                            (float)s.fd_tolerance, s.fd_mode, k.data(), dV0.data()))
+      return rc;
+    for (size_t b = 0; b < B; b++) cands[b] = &ps[b]->PrepareLineSearch(horizon, k.data() + b * H * nu, dV0[b]);
+    if (int rc = launch->Run(from, cands, rows, horizon)) return rc;
+    const int K = cands[0]->N;
+    for (size_t b = 0; b < B; b++) {
+      const size_t o = b * K;
+      if (ps[b]->InstallLineSearch(horizon, launch->returns.data() + o, launch->failure.data() + o, (int)o)) return -1;
+    }
   }
-  return Publish();
+  for (size_t b = 0; b < B; b++) improved[b] = ps[b]->Publish();
+  return 0;
+}
+
+int GradientPlanner::OptimizePolicy(int horizon) {
+  int improved = 0;
+  return Iterate({this}, TaskRows(), horizon, &launch_, &improved) ? -1 : improved;
 }
 
 void GradientPlanner::ActionFromPolicy(double* action, const double*, double time, bool use_previous) {
@@ -323,18 +340,53 @@ int iLQSPlanner::Accept(int ok) {
   return ok;
 }
 
-int iLQSPlanner::OptimizePolicy(int horizon) {
-  BeginIteration();
-  if (previous_active_policy == kiLQG) {
-    if (ilqg.NominalTrajectory(horizon) < 0) return -1;
-    ConvertToSpline(horizon);
+int iLQSPlanner::Iterate(const std::vector<iLQSPlanner*>& ps, const TaskRows& rows, int horizon, SplineLaunch* launch,
+                         ILQGSweeps* sweeps, int* improved) {
+  const int B = (int)ps.size();
+  std::fill(improved, improved + B, 0);
+  mjpc_b200_t* ilqg_gpu = ps[0]->ilqg.gpu();
+  const bool diff = ps[0]->ilqg.settings.differentiable != 0;
+  auto ilqg_of = [&](const std::vector<int>& idx) {
+    std::vector<iLQGPlanner*> q;
+    for (int b : idx) q.push_back(&ps[b]->ilqg);
+    return q;
+  };
+  // the iLQG nominals of the problems whose active policy was iLQG, then their conversion to splines
+  std::vector<int> conv;
+  for (int b = 0; b < B; b++) {
+    ps[b]->BeginIteration();
+    if (ps[b]->previous_active_policy == kiLQG) conv.push_back(b);
   }
-  // try sampling
-  if (sampling.OptimizePolicy(horizon) < 0) return -1;
-  if (const int settled = SamplingSettled(horizon)) return settled;
-  const int ok = ilqg.Iteration(horizon);
-  if (ok < 0) return -1;
-  return Accept(ok);
+  if (!conv.empty()) {
+    const DifferentiableScope d(ilqg_gpu, diff);
+    if (sweeps->Nominal(ilqg_of(conv), conv, rows, horizon, nullptr)) return -1;
+  }
+  for (int b : conv) ps[b]->ConvertToSpline(horizon);
+  // try sampling: every problem in one launch
+  std::vector<SamplingPlanner*> sampling(B);
+  for (int b = 0; b < B; b++) sampling[b] = &ps[b]->sampling;
+  if (int rc = SamplingPlanner::Iterate(sampling, rows, horizon, launch)) return rc;
+  std::vector<int> rest;
+  for (int b = 0; b < B; b++) {
+    const int settled = ps[b]->SamplingSettled(horizon);
+    if (settled < 0) return -1;
+    if (settled) improved[b] = 1;
+    else rest.push_back(b);
+  }
+  // one iLQG iteration of the problems sampling did not settle
+  if (rest.empty()) return 0;
+  std::vector<int> updated(rest.size(), 0);
+  {
+    const DifferentiableScope d(ilqg_gpu, diff);
+    if (sweeps->Iterate(ilqg_of(rest), rest, rows, horizon, updated.data())) return -1;
+  }
+  for (size_t j = 0; j < rest.size(); j++) improved[rest[j]] = ps[rest[j]]->Accept(updated[j]);
+  return 0;
+}
+
+int iLQSPlanner::OptimizePolicy(int horizon) {
+  int improved = 0;
+  return Iterate({this}, TaskRows(), horizon, &launch_, &sweeps_, &improved) ? -1 : improved;
 }
 
 int iLQSPlanner::NominalTrajectory(int horizon) {

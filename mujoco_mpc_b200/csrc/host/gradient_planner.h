@@ -2,12 +2,12 @@
 // (mjpc/planners/gradient/planner.h:39-168, planner.cc:159-383; gradient.cc:44-107; spline_mapping.cc;
 //  mjpc/planners/ilqs/planner.h:37-117, planner.cc:60-260).
 //
-// Every sweep is one call of the ABI: NominalTrajectory / Rollouts -> mjpc_b200_rollout_spline (GradientPolicy::Action
-// = FindInterval + Zero/Linear/CubicInterpolation + Clamp, gradient/policy.cc:80-103, which for >= 3 spline points is the
-// function TimeSpline::Sample evaluates on the device), ModelDerivatives::Compute -> mjpc_b200_model_derivatives,
-// CostDerivatives::Compute -> mjpc_b200_cost_derivatives.  Gradient::Compute (a sequential O(H n^2) recursion) and the
-// spline mappings are host arithmetic in double, as in the reference.  BatchGradientPlanner (batch_planner.h) runs the
-// recursion of all its problems on the device instead (mjpc_b200_gradient_batched), bitwise equal to GradientSweep.
+// Every sweep is one call of the ABI over all the planners of an iteration (GradientPlanner::Iterate): the nominal and
+// the line-search Rollouts -> one spline launch each (GradientPolicy::Action = FindInterval + Zero/Linear/Cubic
+// Interpolation + Clamp, gradient/policy.cc:80-103, which for >= 3 spline points is the function TimeSpline::Sample
+// evaluates on the device), ModelDerivatives::Compute + CostDerivatives::Compute + Gradient::Compute (a sequential
+// O(H n^2) recursion) -> mjpc_b200_gradient_batched, whose k and dV0 are bitwise GradientSweep, its host reference.
+// The spline mappings are host arithmetic in double, as in the reference.
 #pragma once
 #include <memory>
 #include <shared_mutex>
@@ -25,7 +25,7 @@ void SplineMapping(int representation, const std::vector<double>& input_times, c
                    std::vector<double>* W);
 
 // Gradient::Compute (gradient.cc:76-107): k [T][m] (row T-1 repeats row T-2), dV[0] = sum_t k_t . Qu_t.  A [T][n][n],
-// B [T][n][m], cx [T][n], cu [T][m] as returned by the ABI (float).
+// B [T][n][m], cx [T][n], cu [T][m] as returned by the ABI (float).  The reference of mjpc_b200_gradient_batched.
 void GradientSweep(const float* A, const float* B, const float* cx, const float* cu, int n, int m, int T,
                    std::vector<double>* k, double* dV0);
 
@@ -52,8 +52,14 @@ class GradientPlanner : public Planner {
                  double timestep, const double* ctrlrange, int max_horizon, int device, mjpc_b200_t* borrowed = nullptr);
   void Reset(int horizon, const double* initial_repeated_action) override;
   int OptimizePolicy(int horizon) override;              // planner.cc:159-330; 1 = improved, 0 = not, <0 error
-  // OptimizePolicy in halves around its launches and its gradient, which a batch makes for many planners at once.
-  // Returns / failures are this planner's [N] of a launch, its candidate 0 at flat index `offset`.
+  // OptimizePolicy of every planner of ps, which plan on one handle with common settings: per max_rollout iteration
+  // ONE launch of all their nominals, ONE mjpc_b200_gradient_batched and ONE launch of all their line-search
+  // candidates; problem b reads task row b of `rows`.  improved[b] = planner b's 1/0 (0 after an error).  0, or an
+  // error code
+  static int Iterate(const std::vector<GradientPlanner*>& ps, const TaskRows& rows, int horizon, SplineLaunch* launch,
+                     int* improved);
+  // Iterate's halves around its launches and its gradient.  Returns / failures are this planner's [N] of a launch, its
+  // candidate 0 at flat index `offset`.
   const SplineCandidates* PrepareNominal(int horizon);   // resample; the nominal (N = 1); nullptr for a bad horizon
   int InstallNominal(int horizon, const float* returns, const uint8_t* failure, int offset);   // <0: fetch failed
   // k [horizon][nu] and dV0 of the nominal (Gradient::Compute) -> spline mapping, update, the K line-search candidates
@@ -78,17 +84,13 @@ class GradientPlanner : public Planner {
  private:
   // the first count candidates [count][P][nu] of parameters as float knots on cand_'s times
   void Candidates(const std::vector<double>& parameters, int count, SplineCandidates* c) const;
-  int Launch(const SplineCandidates& c, int horizon);   // this planner's own launch into ret_ / fail_ / order_
   int Fetch(int candidate, int horizon, double ret);     // trajectory[0] = trajectory[candidate], never a failure
-  int K_ = 32, nu_ = 0, n_ = 0, nr_ = 0, Hmax_ = 0;
+  int K_ = 32, nu_ = 0, nr_ = 0, Hmax_ = 0;
   double timestep_ = 0.01;
   GradientPolicy cand_;                                   // candidate_policy[0]
   SplineCandidates nominal_, lines_;
   std::vector<double> steps_, candidates_, update_, W_;   // line search of the iteration
   double c_prev_ = 0, c_best_ = 0, dV0_ = 0;
-  std::vector<float> A_, B_, C_, D_, cx_, cu_, cxx_, cuu_, cxu_, ret_;
-  std::vector<uint8_t> fail_;
-  std::vector<int> order_;
   Trajectory best_;                                       // trajectory[0] / trajectory[winner]
   mutable std::shared_mutex mtx_;
 };
@@ -105,11 +107,17 @@ class iLQSPlanner : public Planner {
                  mjpc_b200_t* sampling_gpu = nullptr, mjpc_b200_t* ilqg_gpu = nullptr);
   void Reset(int horizon, const double* initial_repeated_action) override;
   void SetState(const double* state, double time, const double* mocap) override;
-  int OptimizePolicy(int horizon) override;
-  // OptimizePolicy in halves around its calls, which a batch makes for many planners at once:
-  //   BeginIteration; if previous_active_policy == kiLQG: ilqg.NominalTrajectory, then ConvertToSpline;
-  //   sampling.OptimizePolicy; SamplingSettled (1: sampling won, done; 0: ilqg is seeded; <0 error);
-  //   ilqg.Iteration -> Accept(its code).
+  int OptimizePolicy(int horizon) override;   // Iterate over this planner alone; 1 = improved, 0 = not, <0 error
+  // OptimizePolicy of every planner of ps, whose sampling halves plan on one handle and iLQG halves on another, with
+  // common settings; problem b reads task row b of `rows`.  At most: ONE feedback launch of the iLQG nominals of the
+  // problems whose active policy was iLQG, ONE spline launch of every problem's sampling, and for the problems sampling
+  // did not settle ONE batched iLQG iteration.  improved[b] = planner b's 1/0.  0, or an error code
+  static int Iterate(const std::vector<iLQSPlanner*>& ps, const TaskRows& rows, int horizon, SplineLaunch* launch,
+                     ILQGSweeps* sweeps, int* improved);
+  // Iterate's halves around its calls:
+  //   BeginIteration; if previous_active_policy == kiLQG: the iLQG nominal, then ConvertToSpline;
+  //   sampling's iteration; SamplingSettled (1: sampling won, done; 0: ilqg is seeded; <0 error);
+  //   the iLQG iteration -> Accept(its code).
   void BeginIteration() { previous_active_policy = active_policy; }
   void ConvertToSpline(int horizon);   // the iLQG trajectory policy -> spline parameters of the sampling planner
   int SamplingSettled(int horizon);
@@ -130,6 +138,7 @@ class iLQSPlanner : public Planner {
  private:
   int nu_ = 0;
   double timestep_ = 0.01;
+  ILQGSweeps sweeps_;                  // of the iLQG halves when the planner plans alone
 };
 
 }  // namespace mjpc_b200_host

@@ -94,7 +94,7 @@ void iLQGPlanner::Reset(int horizon, const double* a) {
   c_states_ = states; c_actions_ = actions; c_times_ = times; c_residual_ = residual; c_gains_ = gains; c_du_ = du;
   total_return = c_return_ = 0; regularization = 1.0; regularization_rate = 1.0; regularization_factor = 2.0;
   feedback_scaling = 1.0; winner = 0; improvement = expected = surprise = 0;
-  ret_.assign(K_, 0.f); fail_.assign(K_, 0); order_.assign(K_, 0);
+  ret_.assign(K_, 0.f); fail_.assign(K_, 0);
 }
 
 std::vector<float> iLQGPlanner::StepSizes() const {
@@ -147,8 +147,8 @@ int iLQGPlanner::PrepareNominal(int horizon) {
 
 // ret / fail: this problem's K rollouts, the first of which has the flat index cand0 in the last launch
 int iLQGPlanner::InstallNominal(const float* ret, const uint8_t* fail, int cand0) {
-  if (ret != ret_.data()) std::copy(ret, ret + K_, ret_.begin());
-  if (fail != fail_.data()) std::copy(fail, fail + K_, fail_.begin());
+  std::copy(ret, ret + K_, ret_.begin());
+  std::copy(fail, fail + K_, fail_.begin());
   const int best = BestRollout(ret_.data(), fail_.data(), K_);
   if (best == -1) { feedback_scaling = 0.0; return 0; }   // candidate_policy[0] keeps the live trajectory (:203-211)
   if (FetchCandidate(cand0 + best, ret_[best])) return -1;
@@ -157,13 +157,9 @@ int iLQGPlanner::InstallNominal(const float* ret, const uint8_t* fail, int cand0
 }
 
 int iLQGPlanner::NominalTrajectory(int horizon) {
-  if (PrepareNominal(horizon)) return -1;
   const DifferentiableScope diff(gpu_, settings.differentiable != 0);
-  const int rc = mjpc_b200_rollout_feedback(gpu_, st_.data(), time_, mc_.empty() ? nullptr : mc_.data(), nullptr, c_actions_.data(),
-                                            c_states_.data(), c_times_.data(), c_gains_.data(), nullptr, steps_.data(),
-                                            representation_, K_, horizon, ret_.data(), fail_.data(), order_.data());
-  if (rc) return -1;
-  return InstallNominal(ret_.data(), fail_.data(), 0);
+  int found = 0;
+  return sweeps_.Nominal({this}, {0}, TaskRows(), horizon, &found) ? -1 : found;
 }
 
 void iLQGPlanner::ScaleRegularization(double factor) {
@@ -182,12 +178,10 @@ void iLQGPlanner::UpdateRegularization(double z, double s) {
 
 int iLQGPlanner::PrepareIteration(int horizon) {
   if (horizon < 2 || horizon > Hmax_) return -1;
-  const size_t H = horizon, n = n_, m = nu_, nr = nr_;
+  const size_t H = horizon, n = n_, m = nu_;
   iter_H_ = horizon;
   previous_return_ = c_return_;
   steps_ = StepSizes();
-  A_.resize(H * n * n); B_.resize(H * n * m); C_.resize(H * nr * n); D_.resize(H * nr * m);
-  cx_.resize(H * n); cu_.resize(H * m); cxx_.resize(H * n * n); cuu_.resize(H * m * m); cxu_.resize(H * n * m);
   Kbuf_.resize(H * m * n); dubuf_.resize(H * m);
   st_.assign(state_.begin(), state_.end()); mc_.assign(mocap_.begin(), mocap_.end());
   reg_iter_ = 0;
@@ -214,8 +208,8 @@ bool iLQGPlanner::InstallGains(int status) {
 
 int iLQGPlanner::InstallActions(const float* ret, const uint8_t* fail, int cand0) {
   const size_t H = iter_H_, m = nu_, n = n_, nr = nr_;
-  if (ret != ret_.data()) std::copy(ret, ret + K_, ret_.begin());
-  if (fail != fail_.data()) std::copy(fail, fail + K_, fail_.begin());
+  std::copy(ret, ret + K_, ret_.begin());
+  std::copy(fail, fail + K_, fail_.begin());
   const int best = BestRollout(ret_.data(), fail_.data(), K_);
   if (best == -1) return 0;    // every rollout failed: nothing is published (:548-550)
   winner = best;
@@ -252,33 +246,6 @@ int iLQGPlanner::InstallActions(const float* ret, const uint8_t* fail, int cand0
   return 1;
 }
 
-int iLQGPlanner::Iteration(int horizon) {
-  if (PrepareIteration(horizon)) return -1;
-  const DifferentiableScope diff(gpu_, settings.differentiable != 0);
-  const float* mc = mc_.empty() ? nullptr : mc_.data();
-  if (mjpc_b200_model_derivatives(gpu_, c_states_.data(), c_actions_.data(), c_times_.data(), mc, horizon,
-                                  settings.derivative_skip, (float)settings.fd_tolerance, settings.fd_mode,
-                                  A_.data(), B_.data(), C_.data(), D_.data()))
-    return -1;
-  if (mjpc_b200_cost_derivatives(gpu_, c_residual_.data(), C_.data(), D_.data(), horizon, cx_.data(), cu_.data(),
-                                 cxx_.data(), cuu_.data(), cxu_.data()))
-    return -1;
-  int status = 0;
-  while (BackwardPending(status)) {
-    if (mjpc_b200_backward_pass(gpu_, A_.data(), B_.data(), cx_.data(), cu_.data(), cxx_.data(), cxu_.data(),
-                                cuu_.data(), c_actions_.data(), horizon, (float)regularization, settings.regularization_type,
-                                settings.action_limits, Kbuf_.data(), dubuf_.data(), dV_, nullptr, nullptr, &status))
-      return -1;
-    AfterBackward(status);
-  }
-  if (!InstallGains(status)) return 0;
-  if (mjpc_b200_rollout_feedback(gpu_, st_.data(), time_, mc, nullptr, c_actions_.data(), c_states_.data(),
-                                 c_times_.data(), c_gains_.data(), c_du_.data(), steps_.data(), 3, K_, horizon,
-                                 ret_.data(), fail_.data(), order_.data()))
-    return -1;
-  return InstallActions(ret_.data(), fail_.data(), 0);
-}
-
 void iLQGPlanner::SetCandidateTrajectory(const Trajectory& tr) {
   const size_t H = std::min<size_t>(tr.horizon, Hmax_);
   H_ = (int)H;
@@ -290,8 +257,12 @@ void iLQGPlanner::SetCandidateTrajectory(const Trajectory& tr) {
 }
 
 int iLQGPlanner::OptimizePolicy(int horizon) {
-  if (NominalTrajectory(horizon) < 0) return -1;
-  return Iteration(horizon);
+  const DifferentiableScope diff(gpu_, settings.differentiable != 0);
+  int updated = 0;
+  if (sweeps_.Nominal({this}, {0}, TaskRows(), horizon, nullptr) ||
+      sweeps_.Iterate({this}, {0}, TaskRows(), horizon, &updated))
+    return -1;
+  return updated;
 }
 
 void iLQGPlanner::ActionFromPolicy(double* action, const double* state, double time, bool) {
@@ -299,6 +270,146 @@ void iLQGPlanner::ActionFromPolicy(double* action, const double* state, double t
   // the live policy's own feedback_scaling is always 1 (planner.cc:603)
   iLQGPolicyAction(pm_, actions.data(), states.data(), times.data(), gains.data(), live_H_, representation_, 1.0,
                    state, time, action);
+}
+
+// ------------------------------------------------------------------------------------------ ILQGSweeps
+namespace {
+// dst[j] = the first `per` values of row(idx[j]), back to back
+template <class T, class F>
+void gather(std::vector<T>& dst, const std::vector<int>& idx, size_t per, F row) {
+  dst.resize(idx.size() * per);
+  for (size_t j = 0; j < idx.size(); j++) {
+    const T* src = row(idx[j]);
+    std::copy(src, src + per, dst.begin() + j * per);
+  }
+}
+}  // namespace
+
+// one rollout_feedback_batched launch of the candidate policies of ps, as each iLQGPlanner makes it
+int ILQGSweeps::FeedbackLaunch(const std::vector<iLQGPlanner*>& ps, const std::vector<int>& task, const TaskRows& rows,
+                               int horizon, bool with_du, int mode) {
+  const iLQGPlanner& p0 = *ps[0];
+  const size_t H = horizon, J = ps.size(), K = p0.K_, ds = p0.ds_, nu = p0.nu_, n = p0.n_, nm = p0.mocap_.size();
+  std::vector<int> idx(J);
+  for (size_t j = 0; j < J; j++) idx[j] = (int)j;
+  auto pl = [&](int j) -> iLQGPlanner& { return *ps[j]; };
+  gather(st_, idx, ds, [&](int j) { return pl(j).st_.data(); });
+  gather(mc_, idx, nm, [&](int j) { return pl(j).mc_.data(); });
+  gather(times_, idx, 1, [&](int j) { return &pl(j).time_; });
+  gather(u_, idx, H * nu, [&](int j) { return pl(j).c_actions_.data(); });
+  gather(x_, idx, H * ds, [&](int j) { return pl(j).c_states_.data(); });
+  gather(t_, idx, H, [&](int j) { return pl(j).c_times_.data(); });
+  gather(g_, idx, H * nu * n, [&](int j) { return pl(j).c_gains_.data(); });
+  if (with_du) gather(du_, idx, H * nu, [&](int j) { return pl(j).c_du_.data(); });
+  gather(steps_, idx, K, [&](int j) { return pl(j).steps_.data(); });
+  gather(w_, task, rows.nw, [&](int r) { return rows.w + (size_t)r * rows.nw; });
+  gather(p_, task, rows.np, [&](int r) { return rows.p + (size_t)r * rows.np; });
+  gather(ts_, task, rows.nts, [&](int r) { return rows.ts + (size_t)r * rows.nts; });
+  ret_.resize(J * K); fail_.resize(J * K); order_.resize(J * K);
+  return mjpc_b200_rollout_feedback_batched(p0.gpu_, (int)J, st_.data(), times_.data(), nm ? mc_.data() : nullptr,
+                                            rows.nw ? w_.data() : nullptr, rows.np ? p_.data() : nullptr,
+                                            rows.nts ? ts_.data() : nullptr, u_.data(), x_.data(), t_.data(), g_.data(),
+                                            with_du ? du_.data() : nullptr, steps_.data(), mode, (int)K, horizon,
+                                            ret_.data(), fail_.data(), order_.data());
+}
+
+int ILQGSweeps::Nominal(const std::vector<iLQGPlanner*>& ps, const std::vector<int>& task, const TaskRows& rows,
+                        int horizon, int* found) {
+  for (iLQGPlanner* p : ps)
+    if (p->PrepareNominal(horizon)) return -1;
+  if (FeedbackLaunch(ps, task, rows, horizon, false, ps[0]->representation_)) return -1;
+  const int K = ps[0]->K_;
+  for (size_t j = 0; j < ps.size(); j++) {
+    const int r = ps[j]->InstallNominal(ret_.data() + j * K, fail_.data() + j * K, (int)j * K);
+    if (r < 0) return -1;
+    if (found) found[j] = r;
+  }
+  return 0;
+}
+
+int ILQGSweeps::Iterate(const std::vector<iLQGPlanner*>& ps, const std::vector<int>& task, const TaskRows& rows,
+                        int horizon, int* updated) {
+  const int J = (int)ps.size();
+  const iLQGPlanner& p0 = *ps[0];
+  const iLQGSettings& settings = p0.settings;
+  const size_t H = horizon, n = p0.n_, m = p0.nu_, nr = p0.nr_, ds = p0.ds_, nm = p0.mocap_.size();
+  std::vector<int> all(J);
+  for (int j = 0; j < J; j++) {
+    all[j] = j;
+    if (updated) updated[j] = 0;
+    if (ps[j]->PrepareIteration(horizon)) return -1;
+  }
+  auto pl = [&](int j) -> iLQGPlanner& { return *ps[j]; };
+  // derivatives and cost derivatives of every problem (ModelDerivatives / CostDerivatives::Compute)
+  gather(x_, all, H * ds, [&](int j) { return pl(j).c_states_.data(); });
+  gather(u_, all, H * m, [&](int j) { return pl(j).c_actions_.data(); });
+  gather(t_, all, H, [&](int j) { return pl(j).c_times_.data(); });
+  gather(mc_, all, nm, [&](int j) { return pl(j).mc_.data(); });
+  gather(res_, all, H * nr, [&](int j) { return pl(j).c_residual_.data(); });
+  gather(w_, task, rows.nw, [&](int r) { return rows.w + (size_t)r * rows.nw; });
+  gather(p_, task, rows.np, [&](int r) { return rows.p + (size_t)r * rows.np; });
+  gather(ts_, task, rows.nts, [&](int r) { return rows.ts + (size_t)r * rows.nts; });
+  A_.resize(J * H * n * n); B_.resize(J * H * n * m); C_.resize(J * H * nr * n); D_.resize(J * H * nr * m);
+  cx_.resize(J * H * n); cu_.resize(J * H * m); cxx_.resize(J * H * n * n); cuu_.resize(J * H * m * m);
+  cxu_.resize(J * H * n * m);
+  if (mjpc_b200_model_derivatives_batched(p0.gpu_, J, x_.data(), u_.data(), t_.data(), nm ? mc_.data() : nullptr,
+                                          rows.nw ? w_.data() : nullptr, rows.np ? p_.data() : nullptr,
+                                          rows.nts ? ts_.data() : nullptr, horizon, settings.derivative_skip,
+                                          (float)settings.fd_tolerance, settings.fd_mode, A_.data(), B_.data(),
+                                          C_.data(), D_.data()))
+    return -1;
+  if (mjpc_b200_cost_derivatives_batched(p0.gpu_, J, rows.nw ? w_.data() : nullptr, res_.data(), C_.data(), D_.data(),
+                                         horizon, cx_.data(), cu_.data(), cxx_.data(), cuu_.data(), cxu_.data()))
+    return -1;
+  // backward passes: round r holds the problems whose pass has not succeeded and whose retry budget is not spent,
+  // each at its own regularisation - every problem follows its own iLQGPlanner retry loop
+  status_.assign(J, 0);
+  for (;;) {
+    std::vector<int> act;
+    for (int j = 0; j < J; j++) if (pl(j).BackwardPending(status_[j])) act.push_back(j);
+    if (act.empty()) break;
+    const size_t JA = act.size();
+    // the rows of the round's problems; when every problem is in the round they are the arrays themselves
+    auto rows_of = [&](std::vector<float>& v, std::vector<float>& sub, size_t per) -> const float* {
+      if (JA == (size_t)J) return v.data();
+      gather(sub, act, per, [&v, per](int j) { return v.data() + (size_t)j * per; });
+      return sub.data();
+    };
+    const float *rA = rows_of(A_, sA_, H * n * n), *rB = rows_of(B_, sB_, H * n * m), *rcx = rows_of(cx_, scx_, H * n),
+                *rcu = rows_of(cu_, scu_, H * m), *rcxx = rows_of(cxx_, scxx_, H * n * n),
+                *rcxu = rows_of(cxu_, scxu_, H * n * m), *rcuu = rows_of(cuu_, scuu_, H * m * m);
+    gather(sact_, act, H * m, [&](int j) { return pl(j).c_actions_.data(); });
+    mu_.resize(JA);
+    for (size_t a = 0; a < JA; a++) mu_[a] = (float)pl(act[a]).regularization;
+    K_out_.resize(JA * H * m * n); du_out_.resize(JA * H * m); dV_out_.resize(2 * JA);
+    std::vector<int> st(JA, 0);
+    if (mjpc_b200_backward_pass_batched(p0.gpu_, (int)JA, rA, rB, rcx, rcu, rcxx, rcxu, rcuu, sact_.data(), horizon,
+                                        mu_.data(), settings.regularization_type, settings.action_limits,
+                                        K_out_.data(), du_out_.data(), dV_out_.data(), nullptr, nullptr, st.data()))
+      return -1;
+    for (size_t a = 0; a < JA; a++) {
+      iLQGPlanner& p = pl(act[a]);
+      std::copy(K_out_.begin() + a * H * m * n, K_out_.begin() + (a + 1) * H * m * n, p.Kbuf_.begin());
+      std::copy(du_out_.begin() + a * H * m, du_out_.begin() + (a + 1) * H * m, p.dubuf_.begin());
+      p.dV_[0] = dV_out_[2 * a]; p.dV_[1] = dV_out_[2 * a + 1];
+      status_[act[a]] = st[a];
+      p.AfterBackward(st[a]);
+    }
+  }
+  // action rollouts of the problems whose backward pass succeeded; the others are left untouched
+  std::vector<iLQGPlanner*> okp;
+  std::vector<int> ok, okt;
+  for (int j = 0; j < J; j++)
+    if (pl(j).InstallGains(status_[j])) { ok.push_back(j); okp.push_back(ps[j]); okt.push_back(task[j]); }
+  if (ok.empty()) return 0;
+  if (FeedbackLaunch(okp, okt, rows, horizon, true, 3)) return -1;
+  const int K = p0.K_;
+  for (size_t j = 0; j < ok.size(); j++) {
+    const int r = okp[j]->InstallActions(ret_.data() + j * K, fail_.data() + j * K, (int)j * K);
+    if (r < 0) return -1;
+    if (updated) updated[ok[j]] = r;
+  }
+  return 0;
 }
 
 }  // namespace mjpc_b200_host

@@ -1,10 +1,10 @@
 // ilqg_planner.h - C++ host side of the iLQG planner with the reference's method names
 // (mjpc/planners/ilqg/planner.h, planner.cc:40-740; settings.h:21-36; backward_pass.cc:327-356 regularisation).
-// Every sweep is one call of the C ABI: NominalTrajectory / ActionRollouts -> mjpc_b200_rollout_feedback,
-// ModelDerivatives::Compute -> mjpc_b200_model_derivatives, CostDerivatives::Compute -> mjpc_b200_cost_derivatives,
-// the Riccati loop -> mjpc_b200_backward_pass (the regularisation retry loop, planner.cc:429-520, stays here).
-// The host work around each call is split into prepare / install halves, so BatchILQGPlanner (batch_ilqg_planner.h)
-// can run the same halves for several planners around one batched call.
+// Every sweep is one batched call of the C ABI over all the planners of an iteration (ILQGSweeps): NominalTrajectory /
+// ActionRollouts -> mjpc_b200_rollout_feedback_batched, ModelDerivatives::Compute ->
+// mjpc_b200_model_derivatives_batched, CostDerivatives::Compute -> mjpc_b200_cost_derivatives_batched, the Riccati loop
+// -> mjpc_b200_backward_pass_batched (the regularisation retry loop, planner.cc:429-520, stays on the host).  The host
+// work around each call is split into prepare / install halves, which the sweeps run for every planner of the call.
 #pragma once
 #include <cstdint>
 #include <shared_mutex>
@@ -14,6 +14,37 @@
 #include "sampling_planner.h"
 
 namespace mjpc_b200_host {
+
+class iLQGPlanner;
+
+// The iLQG sweeps over any subset of iLQGPlanners that plan on one handle with common settings, one batched call per
+// sweep (the planners need not be owned by the caller): planner ps[j] reads task snapshot row task[j] of `rows`.
+// A single planner runs them over itself with empty rows.
+class ILQGSweeps {
+ public:
+  // iLQGPlanner::NominalTrajectory of each planner, one feedback launch; found[j] (may be NULL) receives 1 when a
+  // rollout of ps[j] did not fail, else 0; <0 on error
+  int Nominal(const std::vector<iLQGPlanner*>& ps, const std::vector<int>& task, const TaskRows& rows, int horizon,
+              int* found);
+  // iLQGPlanner::Iteration of each planner; updated[j] (may be NULL) receives its 1/0; <0 on error
+  int Iterate(const std::vector<iLQGPlanner*>& ps, const std::vector<int>& task, const TaskRows& rows, int horizon,
+              int* updated);
+
+ private:
+  // one feedback launch of the candidate policies of ps (flat candidate j*K + i for ps[j])
+  int FeedbackLaunch(const std::vector<iLQGPlanner*>& ps, const std::vector<int>& task, const TaskRows& rows,
+                     int horizon, bool with_du, int mode);
+
+  // launch staging ([problems of the launch][..])
+  std::vector<float> st_, mc_, x_, u_, g_, du_, steps_, res_;
+  std::vector<double> times_, t_, w_, p_, ts_;
+  std::vector<float> A_, B_, C_, D_, cx_, cu_, cxx_, cuu_, cxu_;           // [J][H][..] of the iteration
+  std::vector<float> sA_, sB_, scx_, scu_, scxx_, scxu_, scuu_, sact_, mu_, K_out_, du_out_, dV_out_;   // retry subset
+  std::vector<int> status_;
+  std::vector<float> ret_;   // [J][K] of the last feedback launch
+  std::vector<uint8_t> fail_;
+  std::vector<int> order_;
+};
 
 struct iLQGSettings {                    // mjpc/planners/ilqg/settings.h:21-36
   double min_linesearch_step = 1.0e-3;
@@ -48,9 +79,10 @@ class iLQGPlanner : public Planner {
   int Initialize(const mjpc_model_blob* model, int num_rollouts, int representation, int max_horizon, int device,
                  mjpc_b200_t* borrowed = nullptr);
   void Reset(int horizon, const double* initial_repeated_action) override;
-  int OptimizePolicy(int horizon) override;       // planner.cc:156-165: NominalTrajectory + Iteration; 1 = policy updated
-  int NominalTrajectory(int horizon) override;    // :167-223
-  int Iteration(int horizon);                     // :377-627
+  // planner.cc:156-165: NominalTrajectory (:167-223) + Iteration (:377-627), the sweeps over this planner alone;
+  // 1 = policy updated
+  int OptimizePolicy(int horizon) override;
+  int NominalTrajectory(int horizon) override;    // 1 = a rollout did not fail, 0 = every one failed
   // ilqg/policy.cc:82-161; there is no previous policy, so use_previous is ignored
   void ActionFromPolicy(double* action, const double* state, double time, bool use_previous = false) override;
   const Trajectory* BestTrajectory() override { return &best_; }
@@ -107,10 +139,10 @@ class iLQGPlanner : public Planner {
   double previous_return_ = 0;
   int reg_iter_ = 0, iter_H_ = 0;
   float dV_[2] = {0, 0};
-  std::vector<float> A_, B_, C_, D_, cx_, cu_, cxx_, cuu_, cxu_, Kbuf_, dubuf_, ret_;
+  std::vector<float> Kbuf_, dubuf_, ret_;
   std::vector<uint8_t> fail_;
-  std::vector<int> order_;
   Trajectory best_;
+  ILQGSweeps sweeps_;                               // of the sweeps the planner makes when it plans alone
 };
 
 }  // namespace mjpc_b200_host

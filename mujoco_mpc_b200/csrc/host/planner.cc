@@ -81,12 +81,28 @@ void Planner::SetState(const double* state, double time, const double* mocap) {
   time_ = time;
 }
 
-int Planner::RolloutSpline(const float* knots, const double* knot_times, int interpolation, int P, int N, int horizon,
-                           float* returns, uint8_t* failure, int* order) {
-  const std::vector<float> st(state_.begin(), state_.end()), mc(mocap_.begin(), mocap_.end());
-  horizon_ = horizon; launch_offset_ = 0;
-  return mjpc_b200_rollout_spline(gpu_, st.data(), time_, mc.empty() ? nullptr : mc.data(), nullptr, knots, knot_times,
-                                  interpolation, P, N, horizon, returns, failure, order);
+int SplineLaunch::Run(const std::vector<const Planner*>& from, const std::vector<const SplineCandidates*>& cands,
+                      const TaskRows& rows, int horizon) {
+  const size_t B = from.size(), N = cands[0]->N, P = cands[0]->P, nk = cands[0]->knots.size();   // nk = N P nu
+  const int interp = cands[0]->interpolation;
+  for (const SplineCandidates* c : cands)
+    if (c->N != (int)N || c->P != (int)P || c->interpolation != interp) return MJPC_B200_ERR_BAD_ARGUMENT;
+  const size_t ds = from[0]->state().size(), nm = from[0]->mocap().size();
+  states_.resize(B * ds); mocaps_.resize(B * nm); times_.resize(B);
+  knots_.resize(B * nk); knot_times_.resize(B * P);
+  for (size_t b = 0; b < B; b++) {
+    std::copy(cands[b]->knots.begin(), cands[b]->knots.begin() + nk, knots_.begin() + b * nk);
+    std::copy(cands[b]->knot_times.begin(), cands[b]->knot_times.begin() + P, knot_times_.begin() + b * P);
+    std::copy(from[b]->state().begin(), from[b]->state().end(), states_.begin() + b * ds);
+    std::copy(from[b]->mocap().begin(), from[b]->mocap().end(), mocaps_.begin() + b * nm);
+    times_[b] = from[b]->time();
+  }
+  returns.resize(B * N); failure.resize(B * N); order.resize(B * N);
+  return mjpc_b200_rollout_spline_batched(from[0]->gpu(), (int)B, states_.data(), times_.data(),
+                                          nm ? mocaps_.data() : nullptr, rows.nw ? rows.w : nullptr,
+                                          rows.np ? rows.p : nullptr, rows.nts ? rows.ts : nullptr, knots_.data(),
+                                          knot_times_.data(), interp, (int)P, (int)N, horizon, returns.data(),
+                                          failure.data(), order.data());
 }
 
 int Planner::FetchTrajectory(int candidate, int horizon, Trajectory* t) {

@@ -26,6 +26,31 @@ struct SplineCandidates {
   void Resize(int n, int p, int nu) { N = n; P = p; knots.resize((size_t)n * p * nu); knot_times.resize(p); }
 };
 
+// the task snapshots of the problems of a launch: rows [..][nw], [..][np], [..][nts].  Empty (no rows): every problem
+// reads the handle's set_task snapshot, as the engine does for NULL task arrays
+struct TaskRows {
+  const double *w = nullptr, *p = nullptr, *ts = nullptr;
+  int nw = 0, np = 0, nts = 0;
+};
+
+class Planner;
+
+// The staging and the results of one mjpc_b200_rollout_spline_batched launch.  Run launches, on the handle of from[0],
+// the candidates cands[b] (common N, P and interpolation) of problem b from planner from[b]'s state, time and mocap with
+// task row b of `rows`; every planner of from plans on that handle.  Fills returns, failure and order [B][N].
+class SplineLaunch {
+ public:
+  int Run(const std::vector<const Planner*>& from, const std::vector<const SplineCandidates*>& cands,
+          const TaskRows& rows, int horizon);
+  std::vector<float> returns;
+  std::vector<uint8_t> failure;
+  std::vector<int> order;
+
+ private:
+  std::vector<float> states_, mocaps_, knots_;
+  std::vector<double> times_, knot_times_;
+};
+
 // mju_cholFactor: in-place lower Cholesky factor of the row-major n x n matrix M (upper triangle left as it was); a
 // pivot below mindiag is raised to mindiag.  Returns the rank, the number of pivots that were not raised.
 int CholFactor(double* M, int n, double mindiag);
@@ -65,7 +90,7 @@ class Planner {
   virtual int SetFD(double tolerance, int mode, int derivative_skip) { return MJPC_B200_ERR_UNSUPPORTED; }
   // every engine handle the planner plans on: Agent applies the planning-model options and the task snapshot to each
   virtual std::vector<mjpc_b200_t*> Handles() { return {gpu_}; }
-  mjpc_b200_t* gpu() { return gpu_; }
+  mjpc_b200_t* gpu() const { return gpu_; }
   const std::vector<double>& state() const { return state_; }
   const std::vector<double>& mocap() const { return mocap_; }
   double time() const { return time_; }
@@ -75,12 +100,6 @@ class Planner {
   // Sizes state_ and mocap_ from the handle's model.
   int AttachEngine(const mjpc_model_blob* model, int max_candidates, int max_horizon, int device,
                    mjpc_b200_t* borrowed = nullptr);
-  // mjpc_b200_rollout_spline from state_, time_ and mocap_ with the handle's task snapshot; sets horizon_
-  int RolloutSpline(const float* knots, const double* knot_times, int interpolation, int P, int N, int horizon,
-                    float* returns, uint8_t* failure, int* order);
-  int RolloutSpline(const SplineCandidates& c, int horizon, float* returns, uint8_t* failure, int* order) {
-    return RolloutSpline(c.knots.data(), c.knot_times.data(), c.interpolation, c.P, c.N, horizon, returns, failure, order);
-  }
   // sizes *out to `horizon` rows and fetches trajectory `candidate` of the handle's last launch into it (flat index
   // launch_offset_ + candidate); total_return and failure are the caller's
   int FetchTrajectory(int candidate, int horizon, Trajectory* out);
@@ -92,6 +111,7 @@ class Planner {
   double time_ = 0;
   int horizon_ = 0;                                   // of the last spline launch: the rows a fetch fills
   int launch_offset_ = 0;                             // flat index of this planner's candidate 0 in that launch
+  SplineLaunch launch_;                               // of the spline launches the planner makes when it plans alone
 };
 
 // SetFD for a settings struct with fd_tolerance, fd_mode and derivative_skip: tolerance <= 0, mode < 0 and

@@ -23,17 +23,42 @@ void RobustPlanner::SetState(const double* state, double time, const double* moc
   Planner::SetState(state, time, mocap);
 }
 
-int RobustPlanner::OptimizePolicy(int horizon) {
-  SamplingPlanner& d = *delegate_;
-  const int ncandidates = d.OptimizePolicyCandidates(ncandidates_, horizon);
-  const int noisy = PrepareNoisy(ncandidates);
+int RobustPlanner::Iterate(const std::vector<RobustPlanner*>& ps, const TaskRows& rows, int horizon,
+                           SplineLaunch* launch) {
+  const size_t B = ps.size();
+  // the delegates' OptimizePolicyCandidates: one clean launch on their handle
+  std::vector<const Planner*> from(B);
+  std::vector<const SplineCandidates*> cands(B);
+  for (size_t b = 0; b < B; b++) {
+    from[b] = ps[b]->delegate();
+    cands[b] = &ps[b]->delegate()->PrepareOptimize(horizon);
+  }
+  if (int rc = launch->Run(from, cands, rows, horizon)) return rc;
+  const int N = cands[0]->N;
+  int noisy = 0;
+  std::vector<uint32_t> seeds(B);
+  for (size_t b = 0; b < B; b++) {
+    RobustPlanner& p = *ps[b];
+    const size_t o = b * N;
+    p.delegate()->InstallRollouts(N, horizon, launch->returns.data() + o, launch->failure.data() + o,
+                                  launch->order.data() + o, (int)o);
+    noisy = p.PrepareNoisy(p.TopCandidates());   // the same for every problem: ncandidates and N are common
+    from[b] = &p;                                // the noisy handle
+    cands[b] = &p.noisy_;
+    seeds[b] = p.NoiseSeed();
+  }
   if (noisy <= 0) return noisy;
-  std::vector<float> ret(noisy);
-  std::vector<uint8_t> fail(noisy);
-  if (mjpc_b200_set_xfrc_noise(gpu_, xfrc_std_, xfrc_rate_, NoiseSeed())) return -1;
-  if (RolloutSpline(noisy_, horizon, ret.data(), fail.data(), nullptr)) return -1;
-  InstallNoisy(ret.data(), fail.data());
+  // the noisy re-evaluations: one launch, each problem with its own noise key
+  if (int rc = mjpc_b200_set_xfrc_noise_batched(ps[0]->gpu_, ps[0]->xfrc_std_, ps[0]->xfrc_rate_, (int)B, seeds.data()))
+    return rc;
+  if (int rc = launch->Run(from, cands, rows, horizon)) return rc;
+  for (size_t b = 0; b < B; b++)
+    ps[b]->InstallNoisy(launch->returns.data() + b * noisy, launch->failure.data() + b * noisy);
   return 0;
+}
+
+int RobustPlanner::OptimizePolicy(int horizon) {
+  return Iterate({this}, TaskRows(), horizon, &launch_) ? -1 : 0;
 }
 
 int RobustPlanner::PrepareNoisy(int ncandidates) {

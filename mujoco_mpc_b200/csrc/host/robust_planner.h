@@ -1,7 +1,7 @@
 // robust_planner.h - C++ host side of the Robust planner (mjpc/planners/robust/robust_planner.h:30-76,
 // robust_planner.cc:40-160) over the SamplingPlanner delegate.  The ncandidates x nrepetitions NoisyRollouts the
-// reference schedules on its ThreadPool (robust_planner.cc:110-129) are ONE mjpc_b200_rollout_spline launch with the
-// handle's force noise switched on (mjpc_b200_set_xfrc_noise; injected Philox stream, seed + iteration).
+// reference schedules on its ThreadPool (robust_planner.cc:110-129) are ONE spline launch with the
+// handle's force noise switched on (mjpc_b200_set_xfrc_noise_batched; injected Philox stream, seed + iteration).
 #pragma once
 #include <algorithm>
 #include <memory>
@@ -22,20 +22,20 @@ class RobustPlanner : public Planner {
   void Configure(int sampling_trajectories, int ncandidates, int nrepetitions, double xfrc_std, double xfrc_rate, uint32_t seed);
   void Reset(int horizon, const double* initial_repeated_action) override { delegate_->Reset(horizon, initial_repeated_action); }
   void SetState(const double* state, double time, const double* mocap) override;
-  int OptimizePolicy(int horizon) override;                            // :91-157
-  // OptimizePolicy between the delegate's clean launch (its OptimizePolicyCandidates, or PrepareOptimize +
-  // InstallRollouts) and the noisy one: the top `ncandidates` (its result) each repeated nrepetitions times into the
-  // noisy candidates.  Returns their number, 0 when there is no noisy launch to make (fewer than two candidates: the
-  // policy is installed already) or -1 for a failed clean launch.
+  int OptimizePolicy(int horizon) override;                            // :91-157: Iterate over this planner alone
+  // OptimizePolicy of every planner of ps, which plan on one pair of handles: ONE clean launch of all the delegates'
+  // candidates, then ONE noisy launch where each problem draws its force noise with its own key (NoiseSeed); problem
+  // b reads task row b of `rows`.  0, -1 for ncandidates < 0, or a launch's error code
+  static int Iterate(const std::vector<RobustPlanner*>& ps, const TaskRows& rows, int horizon, SplineLaunch* launch);
+  // OptimizePolicy between the delegate's clean launch (its PrepareOptimize + InstallRollouts) and the noisy one: the
+  // top `ncandidates` each repeated nrepetitions times into the noisy candidates.  Returns their number, 0 when there is
+  // no noisy launch to make (fewer than two candidates: the policy is installed already) or -1 for ncandidates < 0.
   int PrepareNoisy(int ncandidates);
-  const SplineCandidates& noisy() const { return noisy_; }
   uint32_t NoiseSeed() const { return seed_ + (uint32_t)delegate_->iteration; }   // the noisy launch's force-noise key
   int TopCandidates() const { return std::min(ncandidates_, delegate_->num_trajectory()); }
   // ... after the noisy launch: its returns and failure flags [ncandidates][nrepetitions]; the mean-return scores
   // (robust_planner.cc:131-154), the installed policy and improvement
   void InstallNoisy(const float* returns, const uint8_t* failure);
-  double xfrc_std() const { return xfrc_std_; }
-  double xfrc_rate() const { return xfrc_rate_; }
   int NominalTrajectory(int) override { return 0; }   // not restated: planning disabled leaves the plan as it is
   void ActionFromPolicy(double* action, const double* state, double time, bool use_previous = false) override {
     delegate_->ActionFromPolicy(action, state, time, use_previous);

@@ -107,22 +107,31 @@ const SplineCandidates& SampleGradientPlanner::PrepareCandidates(int horizon) {
   return cands_;
 }
 
-int SampleGradientPlanner::OptimizePolicy(int horizon) {
-  const SplineCandidates& c = PrepareCandidates(horizon);
+int SampleGradientPlanner::Iterate(const std::vector<SampleGradientPlanner*>& ps, const TaskRows& rows, int horizon,
+                                   SplineLaunch* launch) {
+  std::vector<const SplineCandidates*> cands;
+  for (SampleGradientPlanner* p : ps) cands.push_back(&p->PrepareCandidates(horizon));
   // the device ranks all N (lower index first on ties): replaces the partial_sort of OptimizePolicy (:219-229)
-  if (RolloutSpline(c, horizon, returns_.data(), failure_.data(), trajectory_order.data())) return -1;
-  InstallRollouts(horizon, returns_.data(), failure_.data(), trajectory_order.data(), 0);
+  if (int rc = launch->Run(std::vector<const Planner*>(ps.begin(), ps.end()), cands, rows, horizon)) return rc;
+  const int N = cands[0]->N;
+  for (size_t b = 0; b < ps.size(); b++) {
+    const size_t o = b * N;
+    ps[b]->InstallRollouts(horizon, launch->returns.data() + o, launch->failure.data() + o, launch->order.data() + o,
+                           (int)o);
+  }
   return 0;
+}
+
+int SampleGradientPlanner::OptimizePolicy(int horizon) {
+  return Iterate({this}, TaskRows(), horizon, &launch_) ? -1 : 0;
 }
 
 void SampleGradientPlanner::InstallRollouts(int horizon, const float* returns, const uint8_t* failure, const int* order,
                                             int offset) {
   const int num_trajectory = num_trajectory_, num_gradient = num_gradient_, num_noisy = num_trajectory - num_gradient;
-  if (returns != returns_.data()) {
-    std::copy(returns, returns + num_trajectory, returns_.begin());
-    std::copy(failure, failure + num_trajectory, failure_.begin());
-    std::copy(order, order + num_trajectory, trajectory_order.begin());
-  }
+  std::copy(returns, returns + num_trajectory, returns_.begin());
+  std::copy(failure, failure + num_trajectory, failure_.begin());
+  std::copy(order, order + num_trajectory, trajectory_order.begin());
   launch_offset_ = offset; horizon_ = horizon;
   winner = returns_[trajectory_order[0]] < returns_[0] ? trajectory_order[0] : 0;
   winner_type = winner == 0 ? kNominal : (winner < num_noisy ? kPerturb : kGradient);
@@ -186,20 +195,24 @@ void SampleGradientPlanner::GradientCandidates(int num_trajectory, int num_gradi
 int SampleGradientPlanner::NominalTrajectory(int horizon) {
   // trajectory[0] <- resampled_policy as it stands; an empty plan is the clamped zero action
   const int P = std::max(resampled_policy.plan.Size(), 1);
-  knots_.assign((size_t)P * nu_, 0.f);
-  knot_times_.assign(P, time_);
+  cands_.Resize(1, P, nu_);
+  cands_.interpolation = (int)resampled_policy.plan.Interpolation();
+  std::fill(cands_.knots.begin(), cands_.knots.end(), 0.f);
+  std::fill(cands_.knot_times.begin(), cands_.knot_times.end(), time_);
   std::vector<double> v(nu_);
   if (resampled_policy.plan.Size() == 0) {
     resampled_policy.Action(v.data(), time_);
-    std::copy(v.begin(), v.end(), knots_.begin());
+    std::copy(v.begin(), v.end(), cands_.knots.begin());
   }
   for (int k = 0; k < resampled_policy.plan.Size(); k++) {
-    knot_times_[k] = resampled_policy.plan.NodeTime(k);
+    cands_.knot_times[k] = resampled_policy.plan.NodeTime(k);
     const double* node = resampled_policy.plan.NodeValues(k);
-    std::copy(node, node + nu_, knots_.begin() + (size_t)k * nu_);
+    std::copy(node, node + nu_, cands_.knots.begin() + (size_t)k * nu_);
   }
-  return RolloutSpline(knots_.data(), knot_times_.data(), (int)resampled_policy.plan.Interpolation(), P, 1, horizon,
-                       returns_.data(), failure_.data(), trajectory_order.data());
+  if (int rc = launch_.Run({this}, {&cands_}, TaskRows(), horizon)) return rc;
+  returns_[0] = launch_.returns[0]; failure_[0] = launch_.failure[0]; trajectory_order[0] = launch_.order[0];
+  launch_offset_ = 0; horizon_ = horizon;
+  return 0;
 }
 
 void SampleGradientPlanner::ActionFromPolicy(double* action, const double*, double time, bool use_previous) {

@@ -1,5 +1,5 @@
 // sample_gradient_planner.h - C++ host side of the Sample Gradient planner with the reference's method names
-// (mjpc/planners/sample_gradient/planner.h, planner.cc:43-498).  Rollouts is ONE mjpc_b200_rollout_spline call
+// (mjpc/planners/sample_gradient/planner.h, planner.cc:43-498).  Rollouts is ONE spline launch
 // over all N candidates where the reference schedules N closures on its ThreadPool (planner.cc:358-398):
 //   0             the resampled nominal
 //   1 .. N-G-1    noisy samples, knot += exploration * z, z from the injected Philox stream (sampling_planner.h),
@@ -25,7 +25,11 @@ class SampleGradientPlanner : public Planner {
                  int interpolation, double exploration, double gradient_filter, double timestep,
                  const double* ctrlrange, uint32_t seed, int max_horizon, int device, mjpc_b200_t* engine = nullptr);
   void Reset(int horizon, const double* initial_repeated_action) override;   // :121-160
-  int OptimizePolicy(int horizon) override;                         // :169-273: the two halves below around one launch
+  int OptimizePolicy(int horizon) override;                         // :169-273: Iterate over this planner alone
+  // OptimizePolicy of every planner of ps, which plan on one handle: the two halves below around ONE launch of all
+  // their candidates; problem b reads task row b of `rows`.  0, or the launch's error code
+  static int Iterate(const std::vector<SampleGradientPlanner*>& ps, const TaskRows& rows, int horizon,
+                     SplineLaunch* launch);
   // ... before the launch: the resampled nominal, the noisy samples and the resampled gradient candidates (N in all)
   const SplineCandidates& PrepareCandidates(int horizon);
   // ... after it: the launch's horizon, the returns, failure flags and ranking of these N candidates, which it held from
@@ -57,8 +61,8 @@ class SampleGradientPlanner : public Planner {
   uint32_t seed_ = 0x5EED;
   std::vector<double> knot_times_;
   std::vector<double> return_weight_, step_size_;   // cached on size, as in the reference; Reset keeps them
-  SplineCandidates cands_;
-  std::vector<float> knots_, returns_;
+  SplineCandidates cands_;                            // of the last launch: the iteration's, or the nominal alone
+  std::vector<float> returns_;
   std::vector<uint8_t> failure_;
   Trajectory best_;
   mutable std::shared_mutex mtx_;

@@ -187,35 +187,35 @@ const SplineCandidates& SamplingPlanner::Candidates(int num_trajectory) {
   return cands_;
 }
 
-int SamplingPlanner::Rollouts(int num_trajectory, int horizon) {
-  const SplineCandidates& c = Candidates(num_trajectory);
-  trajectory_order.resize(num_trajectory);
-  return RolloutSpline(c, horizon, returns_.data(), failure_.data(), trajectory_order.data());
-}
-
 const SplineCandidates& SamplingPlanner::PrepareOptimize(int horizon) {
   UpdateNominalPolicy(horizon);
   policy.plan.SetInterpolation(interpolation_);
   return Candidates(num_trajectory_);
 }
 
-int SamplingPlanner::OptimizePolicyCandidates(int ncandidates, int horizon) {
-  const SplineCandidates& c = PrepareOptimize(horizon);
-  trajectory_order.resize(c.N);
+int SamplingPlanner::Iterate(const std::vector<SamplingPlanner*>& ps, const TaskRows& rows, int horizon,
+                             SplineLaunch* launch) {
+  std::vector<const SplineCandidates*> cands;
+  for (SamplingPlanner* p : ps) cands.push_back(&p->PrepareOptimize(horizon));
   // device ranking replaces partial_sort (:184-188)
-  if (RolloutSpline(c, horizon, returns_.data(), failure_.data(), trajectory_order.data())) return -1;
-  return std::min(ncandidates, num_trajectory_);
-}
-
-int SamplingPlanner::OptimizePolicy(int horizon) {
-  if (OptimizePolicyCandidates(1, horizon) < 0) return -1;
-  InstallBest();
+  if (int rc = launch->Run(std::vector<const Planner*>(ps.begin(), ps.end()), cands, rows, horizon)) return rc;
+  const int N = cands[0]->N;
+  for (size_t b = 0; b < ps.size(); b++) {
+    const size_t o = b * N;
+    ps[b]->InstallRollouts(N, horizon, launch->returns.data() + o, launch->failure.data() + o,
+                           launch->order.data() + o, (int)o);
+    ps[b]->InstallBest();
+  }
   return 0;
 }
 
+int SamplingPlanner::OptimizePolicy(int horizon) { return Iterate({this}, TaskRows(), horizon, &launch_) ? -1 : 0; }
+
 int SamplingPlanner::NominalTrajectory(int horizon) {
   UpdateNominalPolicy(horizon);
-  return Rollouts(1, horizon);
+  if (int rc = launch_.Run({this}, {&Candidates(1)}, TaskRows(), horizon)) return rc;
+  InstallRollouts(1, horizon, launch_.returns.data(), launch_.failure.data(), launch_.order.data(), 0);
+  return 0;
 }
 
 void SamplingPlanner::InstallBest() {

@@ -1,7 +1,7 @@
 // sampling_planner.h - C++ host side above the C ABI: the Predictive Sampling planner with the reference's
 // method names (mjpc/planners/sampling/planner.h:40-160, planner.cc:40-560), TimeSpline (mjpc/spline/spline.h)
-// and SamplingPolicy (mjpc/planners/sampling/policy.cc:52-59).  Only Rollouts() differs from the reference: it
-// makes ONE mjpc_b200_rollout_spline call instead of scheduling N closures on a ThreadPool.
+// and SamplingPolicy (mjpc/planners/sampling/policy.cc:52-59).  Only Rollouts differs from the reference: it
+// is ONE spline launch (SplineLaunch) instead of N closures scheduled on a ThreadPool.
 //
 // The reference's absl::BitGen cannot be seeded (planner.cc:331), so the noise source is injected:
 // Philox4x32-10, key (seed, 0), counter (iteration, candidate, knot, dof), Box-Muller on the first two words.
@@ -60,18 +60,19 @@ class SamplingPlanner : public Planner {
                  double exploration, double exploration2, double timestep, const double* ctrlrange, uint32_t seed,
                  int max_candidates, int max_horizon, int device, mjpc_b200_t* engine = nullptr);
   void Reset(int horizon, const double* initial_repeated_action) override;
-  int OptimizePolicy(int horizon) override;           // planner.cc:197-212
-  int NominalTrajectory(int horizon) override;        // UpdateNominalPolicy + Rollouts(1, horizon)
-  int OptimizePolicyCandidates(int ncandidates, int horizon);   // :155-194
+  int OptimizePolicy(int horizon) override;           // planner.cc:197-212: Iterate over this planner alone
+  // OptimizePolicy of every planner of ps, which plan on one handle, with ONE launch of all their candidates; problem
+  // b reads task row b of `rows`.  0, or the launch's error code
+  static int Iterate(const std::vector<SamplingPlanner*>& ps, const TaskRows& rows, int horizon, SplineLaunch* launch);
+  int NominalTrajectory(int horizon) override;        // UpdateNominalPolicy + the rollout of the nominal alone
   void UpdateNominalPolicy(int horizon);              // :240-323 (non-sliding resample)
   void AddNoiseToPolicy(int i);                       // :326-352
-  int Rollouts(int num_trajectory, int horizon);      // :355-393 -> one C-ABI call
-  // Rollouts in two halves, for a launch shared with other planners (batch_planner.h):
+  // Rollouts (:355-393) in two halves around one launch, which may be shared with other planners:
   // the candidates (nominal + noise) as knots [num_trajectory][P][nu] and knot times [P]; returns P
   int PrepareCandidates(int num_trajectory, float* knots, double* knot_times);
   // ... the same into the planner's own SplineCandidates
   const SplineCandidates& Candidates(int num_trajectory);
-  // OptimizePolicyCandidates up to its launch: the nominal update and the num_trajectory candidates
+  // OptimizePolicyCandidates (:155-194) up to its launch: the nominal update and the num_trajectory candidates
   const SplineCandidates& PrepareOptimize(int horizon);
   // the launch's horizon, and the returns, failure flags and ranking of these candidates, which it held from flat
   // index `offset` on

@@ -195,6 +195,59 @@ def test_kind_checks():
     g.close(); s.close(); q.close()
 
 
+def test_ilqg_batch_kind_checks():
+    """The iLQG batch's own calls refuse another kind's handle (set_fd and destroy leave it alone), the generic calls
+    drive an iLQG batch as its own calls do, and the sampling-only generic get_result refuses it."""
+    from mujoco_mpc_b200.engine import CppBatchILQGPlanner, CppBatchSamplingPlanner, load_library
+    lib = load_library()
+    m = get_model("particle")
+    H = 16
+    dp = C.POINTER(C.c_double)
+    x, mc = np.zeros(4), np.ascontiguousarray(mocap_of(m), np.float64)
+    xp, mcp = x.ctypes.data_as(dp), mc.ctypes.data_as(dp)
+    s = CppBatchSamplingPlanner(m, 2, 8, H)
+    a, sc, up = (C.c_double * 8)(), (C.c_double * 6)(), (C.c_int * 2)()
+    t0 = C.c_double(0.0)
+    assert lib.mjpc_b200_batch_ilqg_planner_reset(s.h, 0, H, None) == BAD_ARGUMENT
+    assert lib.mjpc_b200_batch_ilqg_planner_set_state(s.h, 0, xp, t0, mcp) == BAD_ARGUMENT
+    assert lib.mjpc_b200_batch_ilqg_planner_set_task(s.h, 0, None, None, None) == BAD_ARGUMENT
+    assert lib.mjpc_b200_batch_ilqg_planner_nominal_trajectory(s.h, H) == BAD_ARGUMENT
+    assert lib.mjpc_b200_batch_ilqg_planner_optimize_policy(s.h, H, up) == BAD_ARGUMENT
+    assert lib.mjpc_b200_batch_ilqg_planner_action_from_policy(s.h, 0, a, None, t0) == BAD_ARGUMENT
+    assert lib.mjpc_b200_batch_ilqg_planner_get_result(s.h, 0, sc, None, None, None) == BAD_ARGUMENT
+    lib.mjpc_b200_batch_ilqg_planner_set_fd(s.h, C.c_double(1e-3), 0, 0)
+    lib.mjpc_b200_batch_ilqg_planner_destroy(s.h)
+    for b in range(2):                                                     # the sampling batch is still whole
+        s.reset(b); s.set_state(b, x, 0.0, mc)
+    assert len(s.optimize_policy()) == 2
+    s.close()
+
+    # the same two problems through the generic calls (q) and the iLQG batch's own (ref)
+    q = CppBatchILQGPlanner(m, 2, H)
+    ref = CppBatchILQGPlanner(m, 2, H, fd_tolerance=1e-3, fd_mode=0, derivative_skip=0)
+    assert lib.mjpc_b200_batch_planner_set_fd(q.h, C.c_double(1e-3), 0, 0) == 0
+    for b in range(2):
+        mb = mc.copy(); mb[:2] = (0.1 * (b + 1), -0.05)
+        assert lib.mjpc_b200_batch_planner_reset(q.h, b, H, None) == 0
+        assert lib.mjpc_b200_batch_planner_set_state(q.h, b, xp, t0, mb.ctypes.data_as(dp)) == 0
+        w = np.asarray(m.task_weight, float) * (1.0 + b)
+        assert lib.mjpc_b200_batch_planner_set_task(q.h, b, w.ctypes.data_as(dp), None, None) == 0
+        ref.reset(b); ref.set_state(b, x, 0.0, mb); ref.set_task(b, w)
+    for _ in range(3):
+        assert lib.mjpc_b200_batch_planner_optimize_policy(q.h, H) == 0
+        ref.optimize_policy()
+    for b in range(2):
+        got = (C.c_double * 6)()
+        assert lib.mjpc_b200_batch_ilqg_planner_get_result(q.h, b, got, None, None, None) == H
+        np.testing.assert_array_equal(np.array(got), np.array([ref.result(b)[k] for k in (
+            "total_return", "regularization", "improvement", "expected", "surprise", "winner")]))
+    assert lib.mjpc_b200_batch_planner_get_result(q.h, 0, *([None] * 5)) == BAD_ARGUMENT
+    assert lib.mjpc_b200_batch_planner_set_state(q.h, 2, xp, t0, mcp) == BAD_ARGUMENT
+    lib.mjpc_b200_batch_planner_destroy(q.h)
+    q.h = None
+    ref.close()
+
+
 def test_batch_gradient_particles_descend():
     """The criterion of the single planner's particle test on a batch: four particles with different goals, planned
     together, each descend monotonically to below 0.9 of their first return."""
