@@ -119,10 +119,9 @@ int mjpc_b200_rollout_spline(mjpc_b200_t* h, const float* state, double time, co
  *   returns [B][N], failure [B][N]; order [B][N] (may be NULL): order[b] ranks problem b's candidates by return with
  *     indices local to the problem (0..N-1, ties: lower index first).
  * B*N must not exceed max_candidates (MJPC_B200_ERR_CAPACITY); B, N, H >= 1, H <= max_horizon and P <= 64, otherwise an
- * error is returned and the handle stays usable.  With MJPC_B200_WARPS_PER_CTA > 1 and B > 1, N must be a multiple of it
- * (MJPC_B200_ERR_UNSUPPORTED).  After a batched launch, fetch_trajectory, fetch_all and fetch_stats take the flat index,
- * last_kernel_ms / last_kernel_static describe the one launch, and NoisyRollout force noise (set_xfrc_noise) draws
- * with the flat index as its candidate counter. */
+ * error is returned and the handle stays usable.  After a batched launch, fetch_trajectory, fetch_all and fetch_stats
+ * take the flat index, last_kernel_ms / last_kernel_static describe the one launch, and NoisyRollout force noise
+ * (set_xfrc_noise) draws with the flat index as its candidate counter. */
 int mjpc_b200_rollout_spline_batched(mjpc_b200_t* h, int B, const float* states, const double* times, const float* mocaps,
                                      const double* weights, const double* parameters, const double* task_states,
                                      const float* knots, const double* knot_times, int interp, int P, int N, int H,
@@ -154,8 +153,7 @@ int mjpc_b200_rollout_feedback(mjpc_b200_t* h, const float* state, double time, 
  * weights / parameters / task_states [B][..] or NULL for the handle's set_task values; per problem u_nom [B][H][nu],
  * x_nom [B][H][dim_state], t_nom [B][H] (absolute; rebased to times[b]), gains [B][H][nu][dim_dstate], du [B][H][nu]
  * (may be NULL), step_sizes [B][K]; mode, K and H are common.  returns / failure / order [B][K], order local to the
- * problem.  B*K > max_candidates or H > max_horizon: MJPC_B200_ERR_CAPACITY; with MJPC_B200_WARPS_PER_CTA > 1 and
- * B > 1, K must be a multiple of it (MJPC_B200_ERR_UNSUPPORTED).  fetch_* then take the flat index b*K + i. */
+ * problem.  B*K > max_candidates or H > max_horizon: MJPC_B200_ERR_CAPACITY.  fetch_* then take the flat index b*K + i. */
 int mjpc_b200_rollout_feedback_batched(mjpc_b200_t* h, int B, const float* states, const double* times, const float* mocaps,
                                        const double* weights, const double* parameters, const double* task_states,
                                        const float* u_nom, const float* x_nom, const double* t_nom, const float* gains,
@@ -361,8 +359,8 @@ float mjpc_b200_last_kernel_ms(const mjpc_b200_t* h);
  * csrc/spec_*.h): 1 = the shipped instance (one CTA per candidate: main warp + Hessian helper warps + task warp),
  * 2 = its one-warp-per-candidate twin (same source, selected only by MJPC_B200_SHAPE=plain: the bitwise reference of
  * the tests and the baseline of the profiles); 0 = the generic kernel (MJPC_B200_NO_STATIC=1 forces it).
- * MJPC_B200_PAIR_SYNC=0 disables the step-by-step synchronisation of the two candidates that share an SM when
- * #SMs < N <= 2 #SMs (a scheduling aid: it never changes a result). */
+ * The shipped instance keeps the two candidates that share an SM in step, meeting once per time step, when
+ * #SMs < N <= 2 #SMs; MJPC_B200_PAIR_SYNC=0 disables this (a scheduling aid: it never changes a result). */
 int mjpc_b200_last_kernel_static(const mjpc_b200_t* h);
 /* Host-only: header + state-layout words of a model ({n_model, n_layout, model words, layout offsets}); what
  * mujoco_mpc_b200/gen_spec.py writes into csrc/spec_*.h.  Returns the number of ints written or <0. */

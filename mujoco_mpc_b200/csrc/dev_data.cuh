@@ -9,17 +9,9 @@
 #include "dev_model.h"
 
 // Code-footprint control: with one warp per scheduler every instruction-cache
-// miss is exposed, and the Newton loop's straight-line code (fully unrolled by default) streams from L2 on every
+// miss is exposed, and fully unrolled straight-line code in the Newton loop would stream from L2 on every
 // iteration.  MJPC_ROLL marks loops whose unrolling buys no ILP worth its code size.
-#ifndef MJPC_NO_COMPACT   // -DMJPC_NO_COMPACT restores the fully unrolled build (profiles/footprint.py measures the executed code)
-#define MJPC_COMPACT 1
-#endif
-#ifdef MJPC_COMPACT
 #define MJPC_ROLL _Pragma("unroll 1")
-#define MJPC_HESS_ROLLED 1
-#else
-#define MJPC_ROLL
-#endif
 
 namespace mjpc_dev {
 
@@ -76,16 +68,13 @@ constexpr float kMinVal = 1e-15f;
 constexpr float kCapsuleParallel = 16 * 1.1920929e-7f;   // 16 fp32 eps: collide_capsule_capsule's parallel test
 constexpr float kMaxVal = 1e10f;
 constexpr float kTolFloor = 1e-6f;
-#ifndef MJPC_GRAD_FLOOR
-#define MJPC_GRAD_FLOOR 16.f
-#endif
-constexpr float kGradFloor = MJPC_GRAD_FLOOR;   // the fp32 gradient cannot be driven below kGradFloor * eps * |its terms| (k_solve)  // fp32 floor on opt.tolerance (same rule as the oracle's fp32 instantiation)
+constexpr float kGradFloor = 16.f;   // the fp32 gradient cannot be driven below kGradFloor * eps * |its terms| (k_solve)  // fp32 floor on opt.tolerance (same rule as the oracle's fp32 instantiation)
 constexpr float kMinImp = 0.0001f, kMaxImp = 0.9999f, kMinMu = 1e-5f;
 enum { CNSTR_FRICTION_DOF = 0, CNSTR_LIMIT_JOINT, CNSTR_CONTACT_FRICTIONLESS, CNSTR_CONTACT_ELLIPTIC };
 enum { STATE_SATISFIED = 0, STATE_QUADRATIC, STATE_LINEARNEG, STATE_LINEARPOS, STATE_CONE };
 
 // Everything a trajectory touches lives in the CTA's dynamic shared memory:
-//   [model floats nf][model ints ni][DevModel header][DevLayout][warp 0 state][warp 1 state] ...
+//   [model floats nf][model ints ni][DevModel header][DevLayout][the trajectory's state]
 // All accessors derive their pointers from the g_smem symbol with 32-bit float indices, so the compiler emits
 // LDS/STS with shared-window addressing (pointers kept in a struct degrade to generic LD + 64-bit address
 // arithmetic: that was ~45 % of the executed instructions in the first profile).
@@ -107,7 +96,6 @@ struct Ctx {
   // co-resident pair synchronisation (pair_sync_* below); sync == nullptr: off.  Only lane 0 of the main warp uses these.
   unsigned* sync;        // HBM: this SM's record (32 words)
   int sync_slot;         // 0 / 1: which of the SM's two candidates this one is; -1: not paired
-  int sync_mode;         // bit 0: meet at every time step, bit 1: also before every constraint solve
   int wide_pending;      // helper-warp kernels: a posted phase has not been met yet (wide_settle)
 #ifdef MJPC_PHASE_TIMING
   long long tph[9], tlast;   // profiling build only: SM cycles per pipeline phase (slots 0-7 are reported, 8 is "elsewhere")
@@ -135,7 +123,7 @@ struct Ctx {
 //   DynSpec          sizes and offsets are read from the header copy in shared memory (any model)
 //   StaticSpec<K>    sizes and offsets are compile-time constants taken from a generated table K (spec_*.h):
 //                    every shared-memory address becomes an immediate, size-dependent loops unroll, option
-//                    branches fold.  Requires one warp per CTA (the state block then sits at a fixed address).
+//                    branches fold.  The state block sits at a fixed address: a CTA holds one trajectory.
 // Float options (timestep, tolerance, risk ...) always come from the live header: CM(c).timestep.
 template <int V> struct IntC { static constexpr int v = V; };
 constexpr int kHdrWords = (int)((sizeof(DevModel) + 15) / 16) * 4;
@@ -268,24 +256,21 @@ __device__ __forceinline__ void wide_settle(Ctx& c) {
 // fetch: two candidates at different places of the 124 KB-per-step code evict each other's lines, while two that
 // run the SAME code at the same time cost each other almost nothing (profiles/icache_probe.py).  The main warps of
 // the two candidates of an SM therefore keep in step through a 128-byte record in HBM (they are different CTAs):
-// they start every time step together (and, mode bit 1, every constraint solve); the one that needs more Newton
-// iterations finishes its solve while the other waits at the next meeting point - and a waiting warp fetches nothing.
+// they start every time step together; the one that needs more Newton iterations finishes its solve while the other
+// waits at the next meeting point - and a waiting warp fetches nothing.
 // Timing only: no data crosses, results are bitwise those of unsynchronised runs; every wait is bounded (partner
 // finished / time-out), so nothing can deadlock.  Meeting at every Newton iteration as well was measured and is slower
 // (an HBM flag round trip per iteration plus the waits), profiles/ab_pairsync.py.
 //   record words: [0] registration count | [8 + 8 s + {0, 1}] alive flag, meeting-point sequence number of slot s
-#ifndef MJPC_PAIR_TIMEOUT
-#define MJPC_PAIR_TIMEOUT 400000
-#endif
-constexpr long long kPairTimeout = MJPC_PAIR_TIMEOUT;   // SM cycles (shorter time-outs were measured: profiles/README.md)
+constexpr long long kPairTimeout = 400000;   // SM cycles (shorter time-outs were measured: strict waiting is best)
 __device__ __forceinline__ unsigned ld_vol(const unsigned* p) {
   unsigned v;
   asm volatile("ld.volatile.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
   return v;
 }
 __device__ __forceinline__ void st_vol(unsigned* p, unsigned v) { asm volatile("st.volatile.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory"); }
-__device__ __forceinline__ void pair_sync_init(Ctx& c, unsigned* table, int mode) {
-  c.sync = nullptr; c.sync_slot = -1; c.sync_mode = mode;
+__device__ __forceinline__ void pair_sync_init(Ctx& c, unsigned* table) {
+  c.sync = nullptr; c.sync_slot = -1;
   if (!table) return;
   unsigned smid;
   asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
@@ -510,66 +495,14 @@ __device__ __forceinline__ void warp_chol_factor_solve_reg(float* A, float* x, c
   __syncwarp();
 }
 
-// ---- rolled left-looking variant for compile-time N <= 32 (experiment MJPC_CHOL_ROLLED2, code footprint): lane i owns
-// row i in shared memory; column j is one dot product over the finished columns (8-byte loads when rows are 8-byte
-// aligned), a shuffle broadcast of the pivot and one store per lane.  ~1 KB of code instead of 13 KB.
-template <int N>
-__device__ __forceinline__ void warp_chol_factor_solve_rolled(float* A, float* inv, float* x, const float* b, int lane) {
-  const int li = lane < N ? lane : N - 1;
-  float y = b[li];
-  __syncwarp();   // x == b callers
-  float* rowi = A + li * N;
-#pragma unroll 1
-  for (int j = 0; j < N; j++) {
-    const float* rowj = A + j * N;
-    float s = rowi[j];
-    int k = 0;
-    if (N % 2 == 0) {
-#pragma unroll 2
-      for (; k + 1 < j; k += 2) {
-        const float2 a = *reinterpret_cast<const float2*>(rowi + k), bb = *reinterpret_cast<const float2*>(rowj + k);
-        s -= a.x * bb.x; s -= a.y * bb.y;
-      }
-    }
-#pragma unroll 1
-    for (; k < j; k++) s -= rowi[k] * rowj[k];
-    float p = __shfl_sync(kFull, s, j);
-    if (p < kMinVal) p = kMinVal;
-    const float l = sqrtf(p), il = 1.0f / l;
-    if (lane >= j && lane < N) rowi[j] = (lane == j) ? l : s * il;
-    if (lane == j) inv[j] = il;
-    __syncwarp();
-  }
-#pragma unroll 1
-  for (int i = 0; i < N; i++) {  // forward: L y = b
-    const float yi = __shfl_sync(kFull, y, i) * inv[i];
-    const float lij = rowi[i];
-    y = (lane == i) ? yi : (lane > i ? y - lij * yi : y);
-  }
-#pragma unroll 1
-  for (int i = N - 1; i >= 0; i--) {  // backward: L^T x = y
-    const float xi = __shfl_sync(kFull, y, i) * inv[i];
-    const float lji = A[i * N + li];
-    y = (lane == i) ? xi : (lane < i ? y - lji * xi : y);
-  }
-  if (lane < N) x[lane] = y;
-  __syncwarp();
-}
-
 // factor A (destroyed, holds L afterwards) and solve A x = b; dispatches to the register variant for the
 // dof counts of the built-in models
 // NS > 0: the size is a compile-time constant of a static spec (register-resident path, no dispatch)
 template <int NS>
 __device__ __noinline__ void warp_chol_factor_solve(float* A, float* inv, float* x, const float* b, int n, int lane) {
-#ifdef MJPC_CHOL_ROLLED2
-  if constexpr (NS > 0 && NS <= 32) { warp_chol_factor_solve_rolled<NS>(A, inv, x, b, lane); return; }
-  if (n == 18) { warp_chol_factor_solve_rolled<18>(A, inv, x, b, lane); return; }
-#endif
-#ifndef MJPC_CHOL_ROLLED   // experiment (profiles/README.md, code footprint): rolled shared-memory factorisation everywhere
   if constexpr (NS > 0 && NS <= 32) { warp_chol_factor_solve_reg<NS>(A, x, b, lane); return; }
   if (n == 18) { warp_chol_factor_solve_reg<18>(A, x, b, lane); return; }
   if (n == 2) { warp_chol_factor_solve_reg<2>(A, x, b, lane); return; }
-#endif
   warp_chol(A, inv, n, lane);
   warp_chol_solve(x, A, inv, b, n, lane);
 }

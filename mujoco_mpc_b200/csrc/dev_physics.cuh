@@ -1216,10 +1216,10 @@ __device__ __noinline__ float k_update_constraint(Ctx& c, bool hess) {
   return cost;
 }
 
-// Register-blocked Newton Hessian for compile-time NV: lane owns structurally non-zero lower-triangle entries
-// e = lane + 32 q (hpair tables, NQ per lane) and keeps them in registers; every active constraint row (weight
-// hw != 0) and every cone effective row is one rank-1 update read as a dense row from shared memory
-// (broadcast loads, no bank conflicts, no branches inside).
+// Newton Hessian for compile-time NV: one rolled pass over the structurally non-zero lower-triangle entries (hpair
+// tables), entry e on thread e of the group per round; every active constraint row and every cone effective row adds
+// its rank-1 term, read as a dense row from shared memory (broadcast loads, no bank conflicts).  NQ (entries per lane
+// of one warp) is not read: it only keeps k_hessian's two nv = 18 instances apart.
 template <class SP, int NV, int NQ, bool kHelpers = false>
 __device__ __forceinline__ void hessian_dense_reg(Ctx& c) {
   auto&& M = SP::model(c);
@@ -1270,11 +1270,7 @@ __device__ __forceinline__ void hessian_dense_reg(Ctx& c) {
       const int a0 = max(a0r, 0);
       const int nrows = on ? cdim[ci] : 0;
       float acc = 0.f;
-#ifdef MJPC_HESS_ROLLED
 #pragma unroll 1
-#else
-#pragma unroll
-#endif
       for (int a = 0; a < kMaxRows; a++) {
         if (a >= 6 && !pyr) break;                       // compile-time for a static spec
         const int r = min(a0 + a, M.maxefc - 1);
@@ -1312,9 +1308,7 @@ __device__ __forceinline__ void hessian_dense_reg(Ctx& c) {
     }
     G::bar();
   }
-#ifdef MJPC_HESS_ROLLED
-  // experiment (code footprint): one rolled loop over the pattern entries, H written directly, the rare rank-1 rows
-  // of two-sided contacts added in shared memory afterwards
+  // one rolled loop over the pattern entries (code footprint), H written directly
   if (NE != NV * (NV + 1) / 2) {   // entries outside the pattern (the dense factor reads them); nothing to clear for a full pattern
     MJPC_ROLL
     for (int w = lane; w < NV * NV; w += WN) H[w] = 0.f;
@@ -1329,6 +1323,8 @@ __device__ __forceinline__ void hessian_dense_reg(Ctx& c) {
       const int e = min(e0 + lane, NE - 1);
       const int r = hi[e], sdof = hj[e];
       float a = qM[r * NV + sdof];
+      // the composite form holds for (dof, ancestor dof) pairs only - the pattern of M itself; entries that exist in
+      // the Hessian pattern because a pair of moving bodies CAN touch (e.g. two legs) get nothing from one-sided contacts
       const int br = dbody2[r];
       const unsigned mlo_r = (unsigned)MI(body_dofmask_lo)[br], mhi_r = (unsigned)MI(body_dofmask_hi)[br];
       const bool anc = sdof < 32 ? ((mlo_r >> sdof) & 1u) : ((mhi_r >> (sdof - 32)) & 1u);
@@ -1365,66 +1361,6 @@ __device__ __forceinline__ void hessian_dense_reg(Ctx& c) {
   }
   G::bar();
 }
-#else
-  int er[NQ], es[NQ];
-  float acc[NQ];
-  for (int w = lane; w < NV * NV; w += 32) H[w] = 0.f;   // entries outside the pattern (the factor fills them)
-  {
-    const float* cdof = DF(cdof);
-    const int* dbody2 = MI(dof_bodyid);
-#pragma unroll
-    for (int q = 0; q < NQ; q++) {
-      int e = lane + 32 * q;
-      if (e >= NE) e = NE - 1;
-      const int r = hi[e];
-      er[q] = r; es[q] = hj[e];
-      float a = qM[er[q] * NV + es[q]];
-      // the composite form holds for (dof, ancestor dof) pairs only - the pattern of M itself; entries that exist in
-      // the Hessian pattern because a pair of moving bodies CAN touch (e.g. two legs) get nothing from one-sided contacts
-      const int br = dbody2[r];
-      const unsigned mlo_r = (unsigned)MI(body_dofmask_lo)[br], mhi_r = (unsigned)MI(body_dofmask_hi)[br];
-      const bool anc = es[q] < 32 ? ((mlo_r >> es[q]) & 1u) : ((mhi_r >> (es[q] - 32)) & 1u);
-      const float *gr = g + 6 * r, *cs = cdof + 6 * es[q];
-      float dsum = 0.f;
-#pragma unroll
-      for (int l = 0; l < 6; l++) dsum += gr[l] * cs[l];
-      a += anc ? dsum : 0.f;
-      if (er[q] == es[q]) {
-        const int fr = frow[r];
-        if (fr >= 0) a += hw[fr];
-        for (int k = M.nfloss; k < M.nfloss + c.nlim; k++) { const float hk = hw[k]; a += edof[k] == r ? hk : 0.f; }
-      }
-      acc[q] = a;
-    }
-  }
-  // ---- rows of two-sided contacts and tendon limits: one rank-1 update per active row / cone effective row
-  const int* drow = DI(efc_drow);
-  for (int k = 0; k < c.ndrow; k++) {
-    const int row = drow[k];
-    const float w = hw[row];
-    if (w == 0.f) continue;   // warp-uniform
-    const float* j = Jd + row * NVP;
-#pragma unroll
-    for (int q = 0; q < NQ; q++) acc[q] += w * j[er[q]] * j[es[q]];
-  }
-  if (c.ndrow > 0) {
-    for (int ci = 0; ci < ncon; ci++) {
-      const int a0 = cadr[ci];
-      if (a0 < 0 || cside[ci] != 0 || state[a0] != STATE_CONE) continue;   // warp-uniform
-      const float wv = xw[36 * ci + 12], wu = xw[36 * ci + 13];
-      const float* xv = Xd + (2 * ci) * NVP;
-      const float* xu = xv + NVP;
-#pragma unroll
-      for (int q = 0; q < NQ; q++) acc[q] += wv * xv[er[q]] * xv[es[q]] + wu * xu[er[q]] * xu[es[q]];
-    }
-  }
-  __syncwarp();
-#pragma unroll
-  for (int q = 0; q < NQ; q++)
-    if (lane + 32 * q < NE) { H[er[q] * NV + es[q]] = acc[q]; H[es[q] * NV + er[q]] = acc[q]; }
-  __syncwarp();
-}
-#endif
 
 // row i of (NV x NV row-major matrix) times vector, compile-time NV, 8-byte vector loads (NV even)
 template <int NV>
@@ -1698,9 +1634,6 @@ __device__ __noinline__ void k_hessian(Ctx& c) {
 template <class SP>
 __device__ __noinline__ void wide_helper_loop(Ctx& c) {
   if constexpr (SP::kWide > 1) {
-#ifndef MJPC_HESS_ROLLED
-    static_assert(SP::kWide == 1, "helper warps need the rolled Hessian assembly (MJPC_COMPACT)");
-#endif
     for (;;) {
       wide_bar<SP>();
       const WideBox& b = wide_box();
@@ -1854,15 +1787,10 @@ __device__ __forceinline__ LsPoint ls_eval_cached(const LsItem& it, float g0, fl
   return p;
 }
 
-#ifdef MJPC_COMPACT
 // one shared copy of the evaluation for the ~6 call sites of the line search (the item travels by value in registers)
 __device__ __noinline__ LsPoint ls_eval_cached_shared(LsItem it, float g0, float g1, float g2, float alpha) {
   return ls_eval_cached(it, g0, g1, g2, alpha);
 }
-#define LS_EVAL_CACHED ls_eval_cached_shared
-#else
-#define LS_EVAL_CACHED ls_eval_cached
-#endif
 
 template <class SP>
 __device__ __noinline__ float k_line_search(Ctx& c, float g0, float g1, float g2, float snorm, float scale_inv) {
@@ -1874,7 +1802,7 @@ __device__ __noinline__ float k_line_search(Ctx& c, float g0, float g1, float g2
 #if defined(MJPC_PHASE_TIMING) && MJPC_PHASE_MAP == 1
     c.tph[7]++;   // timer mapping 1: slot 7 counts the evaluations
 #endif
-    return cached ? LS_EVAL_CACHED(item, g0, g1, g2, alpha) : k_ls_eval<SP>(c, g0, g1, g2, alpha);
+    return cached ? ls_eval_cached_shared(item, g0, g1, g2, alpha) : k_ls_eval<SP>(c, g0, g1, g2, alpha);
   };
   const LsPoint p0 = ev(0.f);
   const float gtol = fmaxf(fmaxf(CM(c).tolerance, kTolFloor) * CM(c).ls_tolerance * snorm * scale_inv, 64 * 1.1920929e-7f * fabsf(p0.d1));
@@ -1951,11 +1879,7 @@ __device__ __forceinline__ void jt_force(Ctx& c, float* out_or_null) {
 }
 
 template <class SP>
-#ifdef MJPC_COMPACT
 __device__ __noinline__ void jt_force_any(Ctx& c, float* out, int nv) {
-#else
-__device__ __forceinline__ void jt_force_any(Ctx& c, float* out, int nv) {
-#endif
   if constexpr (SP::kNV > 0) jt_force_dense<SP, SP::kNV>(c, out);
   else { if (nv == 18) jt_force_dense<SP, 18>(c, out); else jt_force<SP>(c, out); }
 }

@@ -85,7 +85,6 @@ struct mjpc_b200 {
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   ModelPack pack;
   int maxN = 0, maxH = 0, maxP = 64;
-  int warps_per_cta = 1;
   int num_sms = 132;
   size_t smem_optin = 0;   // the device's opt-in limit of dynamic shared memory per block
   int max_term_dim = 1;    // widest cost term (task_dim_norm_residual): sizes cost_derivatives_kernel's scratch
@@ -150,9 +149,9 @@ struct mjpc_b200 {
   // resident-input launch description
   RolloutArgs resident;
   bool resident_ok = false;
-  size_t smem_bytes(int P, int wpc) const {
+  size_t smem_bytes(int P) const {
     DevLayout L = make_layout(pack.M, P);
-    return ((size_t)smem_header_words(pack.M) + (size_t)wpc * L.total) * 4;
+    return ((size_t)smem_header_words(pack.M) + (size_t)L.total) * 4;
   }
 };
 
@@ -177,10 +176,10 @@ int upload_task(mjpc_b200* h) {
 // The instance a launch runs from the handle's row, and what mjpc_b200_last_kernel_static reports for it (0 generic,
 // 1 static, 2 static one-warp rollout).  Read per launch, so that tests and profiles can switch them on a live engine:
 // MJPC_B200_NO_STATIC=1 forces the generic row, MJPC_B200_SHAPE=plain the one-warp rollout.
-int pick_kernels(const mjpc_b200* h, bool allow_static, const KernelSet** k) {
+int pick_kernels(const mjpc_b200* h, const KernelSet** k) {
   const char* ns = std::getenv("MJPC_B200_NO_STATIC");
   const char* sh = std::getenv("MJPC_B200_SHAPE");
-  if (h->kernels == &kGenericKernels || !allow_static || (ns && ns[0] == '1')) { *k = &kGenericKernels; return 0; }
+  if (h->kernels == &kGenericKernels || (ns && ns[0] == '1')) { *k = &kGenericKernels; return 0; }
   *k = h->kernels;
   return sh && sh[0] == 'p' && sh[1] == 'l' ? 2 : 1;
 }
@@ -301,9 +300,7 @@ int reserve_feedback(mjpc_b200* h, int B) {
 
 int launch_rollout(mjpc_b200* h, const RolloutArgs& A_in) {
   RolloutArgs A = A_in;
-  const int wpc = h->warps_per_cta;
-  const size_t smem = h->smem_bytes(A.P, wpc);
-  const int grid = (A.N + wpc - 1) / wpc;
+  const size_t smem = h->smem_bytes(A.P);
   CUDA_TRY(cudaEventRecord(h->ev0, h->stream));
   // co-resident pair synchronisation: only when at most two candidates can ever be resident per SM and all are resident
   // at once (one wave); MJPC_B200_PAIR_SYNC=0 switches it off (profiling)
@@ -311,14 +308,13 @@ int launch_rollout(mjpc_b200* h, const RolloutArgs& A_in) {
     const char* ps = std::getenv("MJPC_B200_PAIR_SYNC");
     const bool on = !(ps && ps[0] == '0') && A.N > h->num_sms && A.N <= 2 * h->num_sms;
     A.pair_sync = on ? h->d_pair_sync : nullptr;
-    A.pair_sync_mode = (ps && ps[0] >= '1' && ps[0] <= '9') ? std::atoi(ps) : 1;   // 1: meet per step (default), 3: and before the solve; + 16 k: only at steps with (t & k) == 0
     if (on) CUDA_TRY(cudaMemsetAsync(h->d_pair_sync, 0, (size_t)256 * 32 * sizeof(unsigned), h->stream));
   }
-  // static instance: same arguments, same shared-memory image, one candidate per CTA
+  // one candidate per CTA, whichever instance; the static ones share the generic one's arguments and shared-memory image
   const KernelSet* k;
-  h->last_static = pick_kernels(h, wpc == 1, &k);
+  h->last_static = pick_kernels(h, &k);
   const bool plain = h->last_static == 2;
-  launch_kernel(plain ? k->rollout_plain : k->rollout, grid, (plain ? 32 : k->rollout_threads) * wpc, smem, h->stream, A);
+  launch_kernel(plain ? k->rollout_plain : k->rollout, A.N, plain ? 32 : k->rollout_threads, smem, h->stream, A);
   rank_kernel<<<(A.N + 255) / 256, 256, 0, h->stream>>>(A.returns, A.nper, A.nprob, h->d_order);
   CUDA_TRY(cudaEventRecord(h->ev1, h->stream));
   CUDA_TRY(cudaGetLastError());
@@ -449,10 +445,6 @@ int mjpc_b200_create(const mjpc_model_blob* model, int max_candidates, int max_h
     return fail(MJPC_B200_ERR_BAD_BLOB, std::string("create: ") + e.what());
   }
   h->device = device;
-  if (const char* w = std::getenv("MJPC_B200_WARPS_PER_CTA")) {  // tuning knob (profiles/): candidates per CTA
-    const int v = std::atoi(w);
-    if (v == 1 || v == 2 || v == 4) h->warps_per_cta = v;
-  }
   h->maxN = max_candidates; h->maxH = max_horizon;
   const DevModel& M = h->pack.M;
   {
@@ -507,7 +499,7 @@ int mjpc_b200_create(const mjpc_model_blob* model, int max_candidates, int max_h
   CREATE_TRY(cudaGetDeviceProperties(&prop, device));
   h->num_sms = prop.multiProcessorCount;
   h->smem_optin = prop.sharedMemPerBlockOptin;
-  const size_t smem_need = h->smem_bytes(h->maxP, 1);
+  const size_t smem_need = h->smem_bytes(h->maxP);
   if (smem_need > (size_t)prop.sharedMemPerBlockOptin) {
     mjpc_b200_destroy(h);
     return fail(MJPC_B200_ERR_CAPACITY, "model does not fit in shared memory");
@@ -546,7 +538,7 @@ int mjpc_b200_create(const mjpc_model_blob* model, int max_candidates, int max_h
   else if (spec_matches<SpecHumanoidTrack>(M, L1)) h->kernels = &kHumanoidTrackKernels;
   // the dynamic shared-memory opt-in is per kernel and process-wide (raise_smem_limit only ever raises it: several
   // handles may coexist); a launch may fall back to the generic row (pick_kernels), so both rows get theirs
-  const size_t smem_rollout = h->smem_bytes(h->maxP, h->warps_per_cta), smem_step = h->smem_bytes(1, 1);
+  const size_t smem_rollout = h->smem_bytes(h->maxP), smem_step = h->smem_bytes(1);
   for (const KernelSet* k : {h->kernels, &kGenericKernels}) {
     CREATE_TRY(raise_smem_limit(k->rollout, smem_rollout)); CREATE_TRY(raise_smem_limit(k->rollout_plain, smem_rollout));
     CREATE_TRY(raise_smem_limit(k->step, smem_step)); CREATE_TRY(raise_smem_limit(k->fd_center, smem_step));
@@ -635,9 +627,6 @@ static int upload_spline(mjpc_b200_t* h, int B, const float* states, const doubl
   if (M.nmocap && !mocaps) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "rollout_spline: mocap required");
   if (B < 1 || N < 1 || H < 1 || P < 1 || interp < 0 || interp > 2) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "rollout_spline: bad sizes");
   if ((int64_t)B * N > h->maxN || H > h->maxH || P > h->maxP) return fail(MJPC_B200_ERR_CAPACITY, "rollout_spline: B*N/H/P above capacity");
-  // several candidates per CTA share its shared-memory copy of the task: a CTA must not hold two problems
-  if (B > 1 && N % h->warps_per_cta != 0)
-    return fail(MJPC_B200_ERR_UNSUPPORTED, "rollout_spline_batched: N must be a multiple of MJPC_B200_WARPS_PER_CTA");
   CUDA_TRY(cudaSetDevice(h->device));
   RolloutArgs A = base_args(h, B * N, H);
   size_t end;
@@ -717,9 +706,6 @@ static int rollout_feedback_impl(mjpc_b200_t* h, int B, const float* states, con
   if (M.nmocap && !mocaps) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "rollout_feedback: mocap required");
   if (B < 1 || K < 1 || H < 1 || mode < 0 || mode > 3) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "rollout_feedback: bad sizes");
   if ((int64_t)B * K > h->maxN || H > h->maxH) return fail(MJPC_B200_ERR_CAPACITY, "rollout_feedback: B*K/H above capacity");
-  // several candidates per CTA share its shared-memory copy of the task: a CTA must not hold two problems
-  if (B > 1 && K % h->warps_per_cta != 0)
-    return fail(MJPC_B200_ERR_UNSUPPORTED, "rollout_feedback_batched: K must be a multiple of MJPC_B200_WARPS_PER_CTA");
   CUDA_TRY(cudaSetDevice(h->device));
   const size_t ds = M.nq + M.nv, n = 2 * M.nv, nu = M.nu, Hs = H, P = B;
   if (int rc = reserve_feedback(h, B)) return rc;
@@ -871,7 +857,7 @@ static int step_impl(mjpc_b200_t* h, const void* fn, int B, const float* qpos, c
     A.sensordata = d + o_sens;
   }
   if (e0) CUDA_TRY(cudaEventRecord(e0, h->stream));
-  launch_kernel(fn, B, 32, h->smem_bytes(1, 1), h->stream, A);
+  launch_kernel(fn, B, 32, h->smem_bytes(1), h->stream, A);
   if (e1) CUDA_TRY(cudaEventRecord(e1, h->stream));
   CUDA_TRY(cudaGetLastError());
   h->launches += 1;
@@ -1040,7 +1026,7 @@ int mjpc_b200_step_batch(mjpc_b200_t* h, int B, const float* qpos, const float* 
   if (!h || B < 1 || !qpos || !qvel || !ctrl || !times) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "step_batch: bad argument");
   if (h->pack.M.nmocap && !mocap) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "step_batch: mocap required");
   const KernelSet* k;
-  const int kind = pick_kernels(h, true, &k);
+  const int kind = pick_kernels(h, &k);
   if (int rc = step_impl(h, k->step, B, qpos, qvel, ctrl, warmstart, mocap, time0, times, qacc, next_qpos, next_qvel,
                          residual, cost, counts, nullptr, nullptr, nullptr, h->ev0, h->ev1))
     return rc;
@@ -1067,7 +1053,7 @@ int mjpc_b200_step_sensors(mjpc_b200_t* h, int B, const float* states, const flo
       return fail(MJPC_B200_ERR_UNSUPPORTED, "step_sensors: sensor " + std::to_string(i) + ": " + h->sensor_why[i]);
   if (B > h->maxN) return fail(MJPC_B200_ERR_CAPACITY, "step_sensors: B > max_candidates");
   const KernelSet* k;
-  const int kind = pick_kernels(h, true, &k);
+  const int kind = pick_kernels(h, &k);
   const size_t nq = M.nq, nv = M.nv, nu = M.nu, ds = nq + nv;
   std::vector<float> q(B * nq), v(B * nv), u(B * nu), nq_out(B * nq), nv_out(B * nv);
   std::vector<double> t(B, time);
@@ -1181,10 +1167,10 @@ static int model_derivatives_impl(mjpc_b200_t* h, int B, const float* x, const f
   std::vector<float> ts, trel;
   derivative_times(h, B, t, task_states, H, &ts, &trel);
   const std::vector<float> w = to_float(weights, (size_t)B * M.num_term), p = to_float(parameters, (size_t)B * M.num_parameters);
-  const size_t smem = h->smem_bytes(1, 1);
+  const size_t smem = h->smem_bytes(1);
   if (ilqg_reserve(h->ilqg, M, B, h->stream)) return fail(MJPC_B200_ERR_CUDA, "model_derivatives: out of device memory");
   const KernelSet* k;
-  pick_kernels(h, true, &k);
+  pick_kernels(h, &k);
   int launches = 0;
   int rc = ilqg_model_derivatives(h->ilqg, M, h->d_pack, h->stream, k->fd_center, k->fd_column, B, x, u, trel.data(), mocaps, ts.data(),
                                   weights ? w.data() : nullptr, parameters ? p.data() : nullptr, H, tol, A, B_, C, D,
@@ -1268,13 +1254,13 @@ int mjpc_b200_gradient_batched(mjpc_b200_t* h, int B, const float* x, const floa
   const std::vector<float> w = to_float(weights, (size_t)B * M.num_term), p = to_float(parameters, (size_t)B * M.num_parameters);
   if (ilqg_reserve(h->ilqg, M, B, h->stream)) return fail(MJPC_B200_ERR_CUDA, "gradient_batched: out of device memory");
   const KernelSet* ks;
-  pick_kernels(h, true, &ks);
+  pick_kernels(h, &ks);
   // the two derivative sweeps exactly as their batched entry points stage them, except that A, B, C, D and the cost
   // derivatives stay on the device; one span from the first kernel to the sweep's end
   int launches = 0;
   int rc = ilqg_model_derivatives(h->ilqg, M, h->d_pack, h->stream, ks->fd_center, ks->fd_column, B, x, u, trel.data(),
                                   mocaps, ts.data(), weights ? w.data() : nullptr, parameters ? p.data() : nullptr, H,
-                                  tol, nullptr, nullptr, nullptr, nullptr, h->smem_bytes(1, 1), &launches, h->ev0,
+                                  tol, nullptr, nullptr, nullptr, nullptr, h->smem_bytes(1), &launches, h->ev0,
                                   nullptr, skip, mode);
   if (rc == 0)
     rc = ilqg_cost_derivatives(h->ilqg, M, h->d_pack, h->stream, B, weights ? w.data() : nullptr, residual, nullptr,
@@ -1443,7 +1429,7 @@ static int step_rows(mjpc_b200_t* h, const KernelSet* ks) {
   A.residual = k.d_res; A.cost = k.d_cost; A.counts = (int*)a.counts;
   A.sensors = h->d_sensors + k.s0; A.nsensor = k.nsens; A.sensor_adr0 = k.adr0; A.sensor_dim = k.nsd;
   A.sensordata = (float*)a.sensordata;
-  launch_kernel(ks->step, A.B, 32, h->smem_bytes(1, 1), h->stream, A);
+  launch_kernel(ks->step, A.B, 32, h->smem_bytes(1), h->stream, A);
   h->launches += 1;
   return 0;
 }
@@ -1463,7 +1449,7 @@ int Update(mjpc_b200_t* h, const float* ctrl, const double* sensor, const float*
   if (nm) std::memcpy(k.h_stage + B * ny * 8 + B * nu * 4, mocap, B * nm * 4);
   CUDA_TRY(cudaMemcpyAsync(k.d_in, k.h_stage, k.in_bytes, cudaMemcpyHostToDevice, h->stream));
   const KernelSet* ks;
-  const int kind = pick_kernels(h, true, &ks);
+  const int kind = pick_kernels(h, &ks);
   auto run = [&](const void* fn) {
     void* args[] = {&a};
     cudaLaunchKernel(fn, dim3(a.B), dim3(kFilterThreads), args, 0, h->stream);

@@ -184,7 +184,7 @@ __device__ __forceinline__ void fd_center_body(const FdArgs& A) {
   float* smem = g_smem;
   stage_model_pack(smem, A.pack, (unsigned)((A.M.nf + A.M.ni) * 4));
   Ctx c;
-  init_ctx(c, &A.M, &A.L, smem, 0, threadIdx.x, A.pack);
+  init_ctx(c, &A.M, &A.L, smem, threadIdx.x, A.pack);
   auto&& M = SP::model(c);
   const int lane = c.lane, t = A.eval_t[blockIdx.x], nq = M.nq, nv = M.nv, ds = nq + nv, nr = M.num_residual;
   const FdProb P = fd_problem<SP>(c, A, blockIdx.y);
@@ -234,7 +234,7 @@ __device__ __forceinline__ void fd_column_body(const FdArgs& A) {
   float* smem = g_smem;
   stage_model_pack(smem, A.pack, (unsigned)((A.M.nf + A.M.ni) * 4));
   Ctx c;
-  init_ctx(c, &A.M, &A.L, smem, 0, threadIdx.x, A.pack);
+  init_ctx(c, &A.M, &A.L, smem, threadIdx.x, A.pack);
   auto&& M = SP::model(c);
   const int lane = c.lane, nq = M.nq, nv = M.nv, nu = M.nu, ds = nq + nv, n = 2 * nv, nr = M.num_residual;
   const int ncol = nu + 2 * nv;
@@ -636,10 +636,8 @@ __device__ inline int box_qp_warp(float* res, float* R, int* index, const float*
 // thread count is a latency knob, not a throughput one: with 8 warps (2 per scheduler) the shared-memory load -> FMA
 // chains of the products were exposed; 512 threads measured faster than 256 and 1024 - the rest is the serial box-QP
 // and gain solves between the barriers.
-#ifndef MJPC_BP_THREADS
-#define MJPC_BP_THREADS 512
-#endif
-extern "C" __global__ void __launch_bounds__(MJPC_BP_THREADS) backward_pass_kernel(const __grid_constant__ BackwardArgs P0) {
+constexpr int kBackwardThreads = 512;
+extern "C" __global__ void __launch_bounds__(kBackwardThreads) backward_pass_kernel(const __grid_constant__ BackwardArgs P0) {
   extern __shared__ __align__(16) float sm[];
   const int n = P0.n, m = P0.m, H = P0.H, tid = threadIdx.x, nt = blockDim.x;
   // this CTA's problem: its slices, its regularisation
@@ -1100,7 +1098,7 @@ inline int ilqg_backward_pass(IlqgBuffers& b, const DevModel& M, const float* d_
   const size_t smem = (4 * n * n + 3 * n * m + 3 * m * m + m * n + 2 * n + 12 * m + 9 * m + 16) * 4;
   ILQG_TRY(raise_smem_limit((const void*)backward_pass_kernel, smem));
   if (e0) ILQG_TRY(cudaEventRecord(e0, st));
-  backward_pass_kernel<<<nprob, MJPC_BP_THREADS, smem, st>>>(a);
+  backward_pass_kernel<<<nprob, kBackwardThreads, smem, st>>>(a);
   if (e1) ILQG_TRY(cudaEventRecord(e1, st));
   *launches += 1;
   ILQG_TRY(cudaGetLastError());

@@ -1,13 +1,13 @@
 // rollout_kernels.cuh - the CUDA kernels of the hot path (sm_90a).
 //
-//   rollout_kernel      one candidate trajectory per warp (generic) or per CTA of main + helper warps (static instances)
+//   rollout_kernel      one candidate trajectory per CTA: one warp (generic) or main + helper warps (static instances)
 //                       (Trajectory::Rollout / RolloutDiscrete,
 //                       mjpc/trajectory.cc:92-309) incl. policy, mj_step restatement, residual, cost, return
 //   rank_kernel         order of each problem's candidates by return (partial_sort, sampling/planner.cc:184-188)
 //   step_batch_kernel   independent single forward+Euler steps through the same device functions (parity hooks)
 //   fd_*_kernel         finite-difference transition/residual Jacobians (model_derivatives.cc:45-165)
 //
-// Shared memory per CTA: [model pack (floats | ints)] [warp 0 data] [warp 1 data] ...
+// Shared memory per CTA: [model pack (floats | ints)] [header copies] [the candidate's data]
 // The model pack is staged with ONE 1-D TMA bulk copy (cp.async.bulk -> SASS UBLKCP) signalled on an mbarrier.
 // Trajectory outputs are written time-major per candidate with lane-strided (coalesced) stores.
 #pragma once
@@ -46,7 +46,6 @@ struct RolloutArgs {
   int P, interp, N, H;
   float* states; float* actions; double* times; float* residual; float* costs; float* trace;
   float* returns; unsigned char* failure;
-  int pair_sync_mode;       // bit 0: meet at every time step, bit 1: also before every constraint solve
   unsigned* pair_sync;      // HBM [256][32] zeroed before the launch, or nullptr: co-resident pair synchronisation (dev_data.cuh)
   long long* stats;         // [N][12]: cycles, Newton iterations, contacts, constraint rows (summed over steps), 8 phase timers
 };
@@ -81,7 +80,7 @@ __host__ __device__ inline int smem_header_words(const DevModel& M) {
 }
 
 // copy the DevModel / DevLayout kernel parameters behind the pack and set up this warp's context
-__device__ __forceinline__ void init_ctx(Ctx& c, const DevModel* M, const DevLayout* L, float* smem, int warp, int lane,
+__device__ __forceinline__ void init_ctx(Ctx& c, const DevModel* M, const DevLayout* L, float* smem, int lane,
                                          const float* pack) {
   const int hdr = M->nf + M->ni;
   const int lay = hdr + (int)((sizeof(DevModel) + 15) / 16) * 4;
@@ -95,11 +94,11 @@ __device__ __forceinline__ void init_ctx(Ctx& c, const DevModel* M, const DevLay
   }
   __syncthreads();
   c.hdr = hdr; c.lay = lay; c.ibase = M->nf;
-  c.dbase = data0 + warp * L->total;
+  c.dbase = data0;
   c.lane = lane;
   c.gkey = pack + M->nf + M->ni;   // the keyframe table follows the staged part of the pack in HBM
   c.ncon = 0; c.npseudo = 0; c.xfrc_on = 0; c.nefc = 0; c.ndrow = 0; c.nitem = 0; c.niter = 0; c.nlim = 0; c.warn = 0; c.time = 0.f;
-  c.sync = nullptr; c.sync_slot = -1; c.sync_mode = 0; c.wide_pending = 0;
+  c.sync = nullptr; c.sync_slot = -1; c.wide_pending = 0;
 #ifdef MJPC_PHASE_TIMING
   for (int k = 0; k < 9; k++) c.tph[k] = 0;
   c.tlast = clock64();
@@ -107,7 +106,7 @@ __device__ __forceinline__ void init_ctx(Ctx& c, const DevModel* M, const DevLay
 }
 
 // row `prob` of a problem's task snapshot over the CTA's shared-memory copy of the pack; a NULL array keeps the packed
-// values.  The copy is per CTA and a CTA never holds two problems, so every warp of it may write the same values.
+// values.  The copy is per CTA and a CTA holds one candidate, so every warp of it may write the same values.
 template <class SP>
 __device__ __forceinline__ void load_task(Ctx& c, int prob, const float* task_state, const float* weight,
                                           const float* parameters) {
@@ -227,16 +226,18 @@ __device__ __forceinline__ void rollout_body(const RolloutArgs& A) {
   float* smem = g_smem;
   stage_model_pack(smem, A.pack, (unsigned)((A.M.nf + A.M.ni) * 4));
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  // SP::kWide > 1: the whole CTA is ONE candidate (warp 0 runs the pipeline, the others help with the wide phases)
-  const int cand = (SP::kWide > 1 || SP::kTask > 0) ? (int)blockIdx.x : blockIdx.x * (blockDim.x >> 5) + warp;
+  // the CTA is ONE candidate (SP::kWide > 1: warp 0 runs the pipeline, the others help with the wide phases).  The
+  // one-warp instances add their warp index, 0: with blockIdx.x alone the Humanoid Track one is compiled to 128
+  // registers and spills.
+  const int cand = (SP::kWide > 1 || SP::kTask > 0) ? (int)blockIdx.x : (int)blockIdx.x + warp;
   Ctx c;
-  init_ctx(c, &A.M, &A.L, smem, (SP::kWide > 1 || SP::kTask > 0) ? 0 : warp, lane, A.pack);
+  init_ctx(c, &A.M, &A.L, smem, lane, A.pack);
   if (cand >= A.N) return;
   if (SP::kWide > 1 && warp > 0 && warp < SP::kWide) { wide_helper_loop<SP>(c); return; }
   if (SP::kTask > 0 && warp == SP::kWide) { task_warp_loop<SP>(c, A, cand); return; }
   constexpr bool kTask = SP::kTask > 0;
   if (kTask && lane == 0) wide_box().task_exit = 0;
-  if constexpr (SP::kWide > 1) pair_sync_init(c, A.pair_sync, A.pair_sync_mode);
+  if constexpr (SP::kWide > 1) pair_sync_init(c, A.pair_sync);
   auto&& M = SP::model(c);
   const int nq = M.nq, nv = M.nv, nu = M.nu, ds = nq + nv, nr = M.num_residual, ntr = 3 * M.num_trace, H = A.H;
   // this candidate's problem: its inputs are resolved here, the step loop below only sees Ctx, the step table and the outputs
@@ -259,14 +260,12 @@ __device__ __forceinline__ void rollout_body(const RolloutArgs& A) {
   const bool noisy = A.xfrc_std > 0.f;
   const float ou_rate = noisy ? expf(-CM(c).timestep / A.xfrc_rate) : 0.f;
   const float ou_scale = noisy ? A.xfrc_std * sqrtf(1.f - ou_rate * ou_rate) : 0.f;
-  // the noise key and stream of this candidate, [warp of the CTA][key, stream]: kept in shared memory rather than in
-  // registers across the step loop: two more live registers there made the Quadruped one-warp and Humanoid Track
-  // helper-warp instances spill (static instances hold one candidate per CTA; the generic one up to 4)
-  __shared__ unsigned noise_ks[4][2];
-  const int kw = std::is_same<SP, DynSpec>::value ? warp : 0;
+  // the noise key and stream of this candidate: kept in shared memory rather than in registers across the step loop:
+  // two more live registers there made the Quadruped one-warp and Humanoid Track helper-warp instances spill
+  __shared__ unsigned noise_ks[2];
   if (noisy && lane == 0) {   // (published to the warp by the __syncwarp below)
-    noise_ks[kw][0] = A.noise_seeds ? A.noise_seeds[prob] : A.noise_seed;
-    noise_ks[kw][1] = A.noise_seeds ? (unsigned)(cand - prob * A.nper) : (unsigned)(A.cand0 + cand);
+    noise_ks[0] = A.noise_seeds ? A.noise_seeds[prob] : A.noise_seed;
+    noise_ks[1] = A.noise_seeds ? (unsigned)(cand - prob * A.nper) : (unsigned)(A.cand0 + cand);
   }
   for (int i = lane; i < 6 * M.nbody; i += 32) DF(xfrc)[i] = 0;
   c.xfrc_on = noisy ? 1 : 0;
@@ -296,7 +295,7 @@ __device__ __forceinline__ void rollout_body(const RolloutArgs& A) {
   long long n_newton = 0, n_con = 0, n_efc = 0;
   for (int t = 0; t < H; t++) {
     const bool last = t == H - 1;
-    if ((c.sync_mode & 1) && (t & (c.sync_mode >> 4)) == 0) pair_sync_meet(c, 2 * t);   // bits 4..: step mask (0 = every step)
+    if constexpr (SP::kWide > 1) pair_sync_meet(c, t);
     // (with a task warp the spline action of step t > 0 was evaluated by it during step t-1's constraint solve)
     if (!last) {
       if (A.policy_kind == 0) {
@@ -320,7 +319,7 @@ __device__ __forceinline__ void rollout_body(const RolloutArgs& A) {
     if (noisy && !last) {   // Ornstein-Uhlenbeck perturbation in discrete time (trajectory.cc:147-155)
       float* xf = DF(xfrc);
       for (int i = lane; i < 6 * M.nbody; i += 32)
-        xf[i] = ou_rate * xf[i] + ou_scale * xfrc_normal(noise_ks[kw][0], (unsigned)t, noise_ks[kw][1], (unsigned)i);
+        xf[i] = ou_rate * xf[i] + ou_scale * xfrc_normal(noise_ks[0], (unsigned)t, noise_ks[1], (unsigned)i);
       __syncwarp();
     }
     float cost;
@@ -342,7 +341,6 @@ __device__ __forceinline__ void rollout_body(const RolloutArgs& A) {
       PHASE_AT(c, 2, 3);
       k_reference<SP>(c);
       PHASE(c, 3);
-      if (c.sync_mode & 2) pair_sync_meet(c, 2 * t + 1);
       k_solve<SP>(c);
       PHASE(c, 4); PHASE_AT(c, 2, 4);
       n_newton += c.niter; n_con += c.ncon - c.npseudo; n_efc += c.nefc;
@@ -404,7 +402,7 @@ __device__ __forceinline__ void rollout_body(const RolloutArgs& A) {
   }
 }
 
-extern "C" __global__ void __launch_bounds__(128) rollout_kernel(const __grid_constant__ RolloutArgs A) {
+extern "C" __global__ void __launch_bounds__(32) rollout_kernel(const __grid_constant__ RolloutArgs A) {
   rollout_body<DynSpec>(A);
 }
 // statically specialised instance for the Quadruped (flat) task model (spec_quadruped.h); one warp per CTA
@@ -413,13 +411,7 @@ extern "C" __global__ void __launch_bounds__(128) rollout_kernel(const __grid_co
 // 171 Hessian entries of the A1 in one round, measured faster than 6 + 1 at 256 candidates).  The *_plain instance is
 // the same source with ONE warp per candidate: the reference the helper-warp kernel must equal bit for bit
 // (tests/test_gpu_parity.py, MJPC_B200_SHAPE=plain) and the baseline of the profiles.
-#ifndef MJPC_WIDE
-#define MJPC_WIDE 7
-#endif
-#ifndef MJPC_TASK
-#define MJPC_TASK 1
-#endif
-constexpr int kRolloutWide = MJPC_WIDE, kRolloutTask = MJPC_TASK, kRolloutThreads = 32 * (kRolloutWide + kRolloutTask);
+constexpr int kRolloutWide = 7, kRolloutTask = 1, kRolloutThreads = 32 * (kRolloutWide + kRolloutTask);
 extern "C" __global__ void __launch_bounds__(kRolloutThreads) rollout_kernel_quadruped(const __grid_constant__ RolloutArgs A) {
   rollout_body<StaticSpec<SpecQuadruped, kRolloutWide, kRolloutTask>>(A);
 }
@@ -492,7 +484,7 @@ __device__ __forceinline__ void step_batch_body(const StepBatchArgs& A) {
   float* smem = g_smem;
   stage_model_pack(smem, A.pack, (unsigned)((A.M.nf + A.M.ni) * 4));
   Ctx c;
-  init_ctx(c, &A.M, &A.L, smem, 0, threadIdx.x, A.pack);
+  init_ctx(c, &A.M, &A.L, smem, threadIdx.x, A.pack);
   auto&& M = SP::model(c);
   const int lane = c.lane, nq = M.nq, nv = M.nv, nu = M.nu, nr = M.num_residual;
   const int b = blockIdx.x;

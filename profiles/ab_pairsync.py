@@ -9,7 +9,7 @@ N = int(sys.argv[1]) if len(sys.argv) > 1 else 256
 e = Engine(m, N, 64)
 d = np.load(os.path.join(R, "profiles", "inputs_quadruped_256x64.npz"))
 kn = np.concatenate([d["knots"]] * ((N + 255) // 256))[:N]
-modes = tuple(sys.argv[2].split(",")) if len(sys.argv) > 2 else ("0", "1", "3")   # off, meet per time step, and before every constraint solve; 17 / 49: every 2nd / 4th step
+modes = ("0", "1")   # off, meet at every time step
 ms = {k: [] for k in modes}; ret = {}
 for rep in range(12):
     for on in modes:

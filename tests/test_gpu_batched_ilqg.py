@@ -306,22 +306,6 @@ def test_batched_argument_errors_leave_the_handle_usable():
     e.close()
 
 
-def test_unsupported_warps_per_cta_batch(monkeypatch):
-    from mujoco_mpc_b200.engine import Engine, EngineError
-    m = get_model("cartpole")
-    H, K = 16, 10
-    pr = _problems(m, H)
-    gains, du, steps = _feedback_inputs(m, pr, K, True)
-    monkeypatch.setenv("MJPC_B200_WARPS_PER_CTA", "4")          # read at create: four candidates per CTA
-    e = Engine(m, 4 * K, H)
-    with pytest.raises(EngineError, match="error -5"):          # K = 10 would put two problems in one CTA
-        _fb_batched(e, pr, gains, du, steps, 3)
-    g8, d8, s8 = _feedback_inputs(m, pr, 8, True)
-    ret = _fb_batched(e, pr, g8, d8, s8, 3)["returns"]
-    assert ret.shape == (4, 8) and np.isfinite(ret).all()
-    e.close()
-
-
 @pytest.mark.parametrize("name,B,H,iters", [("quadruped", 3, 32, 5), ("humanoid", 2, 12, 2)])
 def test_batch_ilqg_planner_equals_independent_planners(name, B, H, iters):
     """CppBatchILQGPlanner (one launch per sweep) vs one CppILQGPlanner per problem (its own launches)."""
