@@ -141,6 +141,29 @@ int mjpc_b200_set_xfrc_noise(mjpc_b200_t* h, double xfrc_std, double xfrc_rate, 
  * per-problem keys (MJPC_B200_ERR_UNSUPPORTED); set_xfrc_noise clears them. */
 int mjpc_b200_set_xfrc_noise_batched(mjpc_b200_t* h, double xfrc_std, double xfrc_rate, int B, const uint32_t* seeds);
 
+/* Per-problem model variants: problem b of the following batched launches runs on models[b] instead of the handle's
+ * model, bitwise what a handle created from models[b] computes.  Each variant is a full blob (its own MJCF through
+ * mjcf.py, or its own mjModel after mj_setConst); derived constants are taken from it, never recomputed.  Every
+ * variant must equal the handle's model, as created, in: every integer header field (sizes, option flags, task
+ * dimensions), the whole int section of the pack (so a frictionloss set to 0, a contype change or an extra geom are
+ * refused), timestep, impratio, tolerance, ls_tolerance, gravity and task_risk, the task arrays (task_weight,
+ * task_norm_parameter, task_parameters, task_state), actuator_ctrlrange and the measurement-sensor table; and it must
+ * pass create's own refusals.  The other float arrays (body, joint, dof, geom, site, actuator and tendon parameters,
+ * qpos0, qpos_spring, key_qpos), meaninertia and the keyframe table may differ.  A mismatch is
+ * MJPC_B200_ERR_BAD_ARGUMENT (last_error names the variant and the first field that differs) and leaves the handle as
+ * it was.  set_options, set_differentiable and set_task still apply to the whole handle (set_task to every variant).
+ * count = 0 (or models NULL) clears the variants.  While variants are set:
+ *   rollout_*_batched, model_derivatives_batched, gradient_batched and a filter bank's update must hold exactly count
+ *     problems (MJPC_B200_ERR_BAD_ARGUMENT otherwise, before anything is staged) - or the B of select_model_variants;
+ *   the single-problem calls, rollout_spline_sharded, step_debug*, step_batch and step_sensors return
+ *     MJPC_B200_ERR_UNSUPPORTED naming the call;
+ *   cost_derivatives_batched and backward_pass_batched read only what variants share, and take any B. */
+int mjpc_b200_set_model_variants(mjpc_b200_t* h, const mjpc_model_blob* models, int count);
+/* With variants set: the following launches hold B problems, problem j running on variant index[j] in [0, count)
+ * (index NULL: problem j on variant j, B = count).  For planners that plan a subset of their problems in one launch.
+ * Without variants there is nothing to select: returns 0 and changes nothing. */
+int mjpc_b200_select_model_variants(mjpc_b200_t* h, const int* index, int B);
+
 /* K line-search rollouts of the iLQG policy. u_nom [H][nu], x_nom [H][dim_state], t_nom [H] (absolute),
  * gains [H][nu][dim_dstate], du [H][nu] (may be NULL), step_sizes [K]. */
 int mjpc_b200_rollout_feedback(mjpc_b200_t* h, const float* state, double time, const float* mocap,
@@ -345,6 +368,10 @@ int mjpc_b200_batch_estimator_update(void* f, const double* ctrl, const double* 
                                      int* status);
 int mjpc_b200_batch_estimator_get(void* f, int filter, double* state, double* covariance, double* time,
                                   double* scalars);
+/* Filter b runs on models[b] from now on: mjpc_b200_set_model_variants on the bank's engine handle, with its rule and
+ * refusals; a NULL-state reset and a NULL mocap then use filter b's model's first keyframe / qpos0 and mocap poses.
+ * count must be num_filters, or 0 to run every filter on the bank's model again.  The filters' states are kept. */
+int mjpc_b200_batch_estimator_set_models(void* f, const mjpc_model_blob* models, int count);
 const char* mjpc_b200_batch_estimator_last_error(const void* f);
 
 /* Per-candidate execution statistics of the last rollout, stats [N][12] = {SM cycles, Newton iterations, contacts,
@@ -467,6 +494,12 @@ int mjpc_b200_batch_planner_set_state(void* planner, int problem, const double* 
 int mjpc_b200_batch_planner_set_task(void* planner, int problem, const double* weight, const double* parameters,
                                      const double* task_state);
 int mjpc_b200_batch_planner_optimize_policy(void* planner, int horizon);   /* every problem: SamplingPlanner::OptimizePolicy */
+/* Problem b plans on models[b] from now on: mjpc_b200_set_model_variants, with its rule and refusals, on every engine
+ * handle the batch owns (the Robust batch's noisy handle and the iLQS batch's iLQG handle too).  count must be
+ * num_problems, or 0 to plan every problem on the batch's model again.  Any batch kind, the iLQG batch included; valid
+ * between planning iterations (after an online system identification, for example).  The planners' settings and
+ * ctrlrange stay the batch's: variants must share actuator_ctrlrange. */
+int mjpc_b200_batch_planner_set_models(void* planner, const mjpc_model_blob* models, int count);
 int mjpc_b200_batch_planner_action_from_policy(void* planner, int problem, double* action, double time, int use_previous);
 /* as mjpc_b200_sampling_planner_get_result for one problem (returns [num_trajectory]); returns the number of installed
  * knots.  A batch of another kind: MJPC_B200_ERR_BAD_ARGUMENT */

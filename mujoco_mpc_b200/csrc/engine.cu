@@ -146,6 +146,15 @@ struct mjpc_b200 {
   float* d_step = nullptr;
   float* h_step = nullptr;
   size_t step_words = 0;
+  // model variants (set_model_variants): the model as created, which every variant is checked against; the variant
+  // blocks [nvariants][variant_stride] floats in one allocation; and the variant each problem of the following launches
+  // runs on, d_variant_index [nselected] (the identity over the variants unless select_model_variants chose others)
+  DevModel M0;
+  double timestep0 = 0;
+  std::vector<float> f0;
+  float* d_variants = nullptr;
+  int* d_variant_index = nullptr;
+  int nvariants = 0, variant_stride = 0, nselected = 0;
   // resident-input launch description
   RolloutArgs resident;
   bool resident_ok = false;
@@ -160,8 +169,12 @@ namespace {
 template <class T>
 cudaError_t dalloc(T** p, size_t n) { return cudaMalloc((void**)p, std::max<size_t>(n, 1) * sizeof(T)); }
 
+// the task floats of a pack: task_weight, task_norm_parameter, task_parameters and task_state lie back to back
+size_t task_floats_begin(const DevModel& M) { return M.fo[F_task_weight]; }
+size_t task_floats_count(const DevModel& M) { return M.fo[F_wrap_coef] - M.fo[F_task_weight]; }
+
 int upload_task(mjpc_b200* h) {
-  // weights / parameters / task_state live inside the model pack (float section)
+  // weights / parameters / task_state live inside the model pack (float section), and inside every variant's block
   const DevModel& M = h->pack.M;
   std::vector<float>& f = h->pack.f;
   for (size_t i = 0; i < h->weight.size(); i++) f[M.fo[F_task_weight] + i] = (float)h->weight[i];
@@ -169,8 +182,111 @@ int upload_task(mjpc_b200* h) {
   for (size_t i = 0; i < h->task_state.size(); i++) f[M.fo[F_task_state] + i] = (float)h->task_state[i];
   h->pack.M.risk = (float)h->risk;
   CUDA_TRY(cudaMemcpyAsync(h->d_pack, f.data(), (size_t)(M.nf + M.ni) * 4, cudaMemcpyHostToDevice, h->stream));
+  const size_t t0 = task_floats_begin(M), nt = task_floats_count(M);
+  for (int v = 0; v < h->nvariants; v++)
+    CUDA_TRY(cudaMemcpyAsync(h->d_variants + (size_t)v * h->variant_stride + t0, f.data() + t0, nt * 4,
+                             cudaMemcpyHostToDevice, h->stream));
   CUDA_TRY(cudaStreamSynchronize(h->stream));  // f is pageable
   return 0;
+}
+
+// The model blocks a launch stages from, and their stride (pack_stride of the kernel arguments): the variants when
+// set, else the one pack with stride 0
+const float* launch_pack(const mjpc_b200* h) { return h->nvariants ? h->d_variants : h->d_pack; }
+int launch_stride(const mjpc_b200* h) { return h->nvariants ? h->variant_stride : 0; }
+
+// With model variants set, a launch that reads them holds one problem per selected variant; the calls without a
+// problem index to choose a variant by (single-problem, sharded and step calls: B < 0 here) are refused.  0 otherwise.
+int check_variants(const mjpc_b200* h, int B, const char* call) {
+  if (!h->nvariants) return 0;
+  if (B < 0)
+    return fail(MJPC_B200_ERR_UNSUPPORTED, std::string(call) + ": not available while model variants are set " +
+                                               "(set_model_variants); use the batched call");
+  if (B != h->nselected)
+    return fail(MJPC_B200_ERR_BAD_ARGUMENT, std::string(call) + ": the launch has " + std::to_string(B) +
+                                                " problems, the model variants are for " + std::to_string(h->nselected));
+  return 0;
+}
+
+// The measurement-sensor table of a blob: one row per model sensor; why[i] is empty when sensor i is one the device
+// evaluates, else the reason it is not.  A blob without the sensor / site entries has no measurable sensors.
+void sensor_table(const Blob& b, std::vector<DevSensor>* sensors, std::vector<std::string>* why_out) {
+  int dt, cnt; int64_t off;
+  if (!b.find("nsensor", &dt, &cnt, &off) || !b.find("site_size", &dt, &cnt, &off)) return;
+  const std::vector<int> ty = b.ints("sensor_type"), ot = b.ints("sensor_objtype"), oid = b.ints("sensor_objid"),
+                         dim = b.ints("sensor_dim"), adr = b.ints("sensor_adr"), st = b.ints("site_type"),
+                         jt = b.ints("jnt_type");
+  const std::vector<double> ss = b.reals("site_size");
+  std::vector<double> cutoff(ty.size(), 0.0);
+  if (b.find("sensor_cutoff", &dt, &cnt, &off)) cutoff = b.reals("sensor_cutoff");
+  const int ns = b.i("nsensor");
+  for (int i = 0; i < ns; i++) {
+    DevSensor S = {ty[i], ot[i], oid[i], adr[i], 0.f};
+    std::string why;
+    if (ty[i] == SENS_JOINTPOS || ty[i] == SENS_JOINTVEL) {
+      if (jt[oid[i]] != JNT_SLIDE && jt[oid[i]] != JNT_HINGE) why = "jointpos / jointvel of a free or ball joint";
+    } else if (ty[i] == SENS_FRAMEPOS) {
+      if (ot[i] < OBJ_BODY || ot[i] > OBJ_SITE) why = "framepos of an unknown object type";
+    } else if (ty[i] == SENS_TOUCH) {
+      if (st[oid[i]] != GEOM_SPHERE) why = "touch zone other than a sphere site";
+      S.radius = (float)ss[3 * oid[i]];
+    } else if (ty[i] == SENS_ACCELEROMETER || ty[i] == SENS_VELOCIMETER || ty[i] == SENS_GYRO) {
+      if (ot[i] != OBJ_SITE) why = "accelerometer / velocimeter / gyro of an object other than a site";
+    } else {
+      why = "sensor type " + std::to_string(ty[i]) +
+            " (only jointpos, jointvel, framepos, touch, accelerometer, velocimeter and gyro are evaluated)";
+    }
+    if (why.empty() && dim[i] != sensor_dim(ty[i])) why = "unexpected sensor dimension";
+    if (why.empty() && cutoff[i] != 0.0) why = "cutoff is not modelled";
+    sensors->push_back(S);
+    why_out->push_back(why);
+  }
+}
+
+const char* const kFloatArrayNames[] = {
+#define X(n) #n,
+    MJPC_F_ARRAYS(X)
+#undef X
+};
+const char* const kIntArrayNames[] = {
+#define X(n) #n,
+    MJPC_I_ARRAYS(X) MJPC_I_DERIVED(X)
+#undef X
+};
+
+// set_model_variants' rule: the first field of variant V (packed, with its sensor table) that must equal the handle's
+// model as created and does not, or "" when V may stand in for it.  Floats compare bitwise.
+std::string variant_mismatch(const mjpc_b200* h, const ModelPack& V, const std::vector<DevSensor>& sensors,
+                             const std::vector<std::string>& why) {
+  const DevModel &M = h->M0, &W = V.M;
+#define X(n) if (W.n != M.n) return #n;
+  MJPC_M_INTS(X)
+#undef X
+  for (int k = 0; k < F_COUNT; k++) if (W.fo[k] != M.fo[k]) return std::string("the layout of ") + kFloatArrayNames[k];
+  for (int k = 0; k < I_COUNT; k++) if (W.io[k] != M.io[k]) return std::string("the layout of ") + kIntArrayNames[k];
+  for (int k = 0; k < I_COUNT; k++) {
+    const int a = M.io[k], e = k + 1 < I_COUNT ? M.io[k + 1] : M.ni;
+    if (!std::equal(V.i.begin() + a, V.i.begin() + e, h->pack.i.begin() + a)) return kIntArrayNames[k];
+  }
+  auto same = [](const void* x, const void* y, size_t n) { return std::memcmp(x, y, n) == 0; };
+  if (V.timestep != h->timestep0 || !same(&W.timestep, &M.timestep, 4)) return "timestep";
+  if (!same(&W.impratio, &M.impratio, 4)) return "impratio";
+  if (!same(&W.tolerance, &M.tolerance, 4)) return "tolerance";
+  if (!same(&W.ls_tolerance, &M.ls_tolerance, 4)) return "ls_tolerance";
+  if (!same(W.gravity, M.gravity, 12)) return "gravity";
+  if (!same(&W.risk, &M.risk, 4)) return "task_risk";
+  for (int k : {F_task_weight, F_task_norm_parameter, F_task_parameters, F_task_state, F_actuator_ctrlrange}) {
+    const int a = M.fo[k], e = M.fo[k + 1];
+    if (!same(V.f.data() + a, h->f0.data() + a, (size_t)(e - a) * 4)) return kFloatArrayNames[k];
+  }
+  if (sensors.size() != h->sensors.size()) return "the sensor table";
+  for (size_t k = 0; k < sensors.size(); k++) {
+    const DevSensor &x = sensors[k], &y = h->sensors[k];
+    if (x.type != y.type || x.objtype != y.objtype || x.objid != y.objid || x.adr != y.adr ||
+        !same(&x.radius, &y.radius, 4) || why[k] != h->sensor_why[k])
+      return "sensor " + std::to_string(k);
+  }
+  return "";
 }
 
 // The instance a launch runs from the handle's row, and what mjpc_b200_last_kernel_static reports for it (0 generic,
@@ -225,6 +341,7 @@ void build_policy_intervals(const double* nodes, int count, double time0, double
 int stage_problems(mjpc_b200* h, int B, const float* states, const double* times, const float* mocaps,
                    const double* weights, const double* parameters, const double* task_states, const double* nodes,
                    int count, int H, const float* knots, int N, RolloutArgs* A, size_t* end) {
+  if (int rc = check_variants(h, B, "rollout")) return rc;
   if (!h->noise_seeds.empty() && (int)h->noise_seeds.size() != B)
     return fail(MJPC_B200_ERR_BAD_ARGUMENT, "rollout: set_xfrc_noise_batched gave keys for " +
                                                 std::to_string(h->noise_seeds.size()) + " problems, the launch has " +
@@ -327,7 +444,7 @@ RolloutArgs base_args(mjpc_b200* h, int N, int H) {
   RolloutArgs A;
   std::memset(&A, 0, sizeof(A));
   A.M = h->pack.M;
-  A.pack = h->d_pack;
+  A.pack = launch_pack(h); A.pack_stride = launch_stride(h); A.pack_index = h->d_variant_index;
   A.N = N; A.H = H;
   A.states = h->d_states; A.actions = h->d_actions; A.times = h->d_times; A.residual = h->d_residual;
   A.costs = h->d_costs; A.trace = h->d_trace; A.returns = h->d_returns; A.failure = h->d_failure;
@@ -456,41 +573,8 @@ int mjpc_b200_create(const mjpc_model_blob* model, int max_candidates, int max_h
     for (int d : b.ints("task_dim_norm_residual")) h->max_term_dim = std::max(h->max_term_dim, d);
   }
   h->time_idx = time_like_state(M.residual_id);
-  {
-    // the measurement-sensor table; a blob without the sensor / site entries has no measurable sensors
-    Blob b(model->data, model->nbytes);
-    int dt, cnt; int64_t off;
-    if (b.find("nsensor", &dt, &cnt, &off) && b.find("site_size", &dt, &cnt, &off)) {
-      const std::vector<int> ty = b.ints("sensor_type"), ot = b.ints("sensor_objtype"), oid = b.ints("sensor_objid"),
-                             dim = b.ints("sensor_dim"), adr = b.ints("sensor_adr"), st = b.ints("site_type"),
-                             jt = b.ints("jnt_type");
-      const std::vector<double> ss = b.reals("site_size");
-      std::vector<double> cutoff(ty.size(), 0.0);
-      if (b.find("sensor_cutoff", &dt, &cnt, &off)) cutoff = b.reals("sensor_cutoff");
-      const int ns = b.i("nsensor");
-      for (int i = 0; i < ns; i++) {
-        DevSensor S = {ty[i], ot[i], oid[i], adr[i], 0.f};
-        std::string why;
-        if (ty[i] == SENS_JOINTPOS || ty[i] == SENS_JOINTVEL) {
-          if (jt[oid[i]] != JNT_SLIDE && jt[oid[i]] != JNT_HINGE) why = "jointpos / jointvel of a free or ball joint";
-        } else if (ty[i] == SENS_FRAMEPOS) {
-          if (ot[i] < OBJ_BODY || ot[i] > OBJ_SITE) why = "framepos of an unknown object type";
-        } else if (ty[i] == SENS_TOUCH) {
-          if (st[oid[i]] != GEOM_SPHERE) why = "touch zone other than a sphere site";
-          S.radius = (float)ss[3 * oid[i]];
-        } else if (ty[i] == SENS_ACCELEROMETER || ty[i] == SENS_VELOCIMETER || ty[i] == SENS_GYRO) {
-          if (ot[i] != OBJ_SITE) why = "accelerometer / velocimeter / gyro of an object other than a site";
-        } else {
-          why = "sensor type " + std::to_string(ty[i]) +
-                " (only jointpos, jointvel, framepos, touch, accelerometer, velocimeter and gyro are evaluated)";
-        }
-        if (why.empty() && dim[i] != sensor_dim(ty[i])) why = "unexpected sensor dimension";
-        if (why.empty() && cutoff[i] != 0.0) why = "cutoff is not modelled";
-        h->sensors.push_back(S);
-        h->sensor_why.push_back(why);
-      }
-    }
-  }
+  sensor_table(Blob(model->data, model->nbytes), &h->sensors, &h->sensor_why);
+  h->M0 = M; h->timestep0 = h->pack.timestep; h->f0 = h->pack.f;
   CREATE_TRY(cudaSetDevice(device));
   CREATE_TRY(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
   CREATE_TRY(cudaEventCreate(&h->ev0));
@@ -562,7 +646,7 @@ void mjpc_b200_destroy(mjpc_b200_t* h) {
   void* bufs[] = {h->d_pack, h->d_in, h->d_unom, h->d_xnom,
                   h->d_tnom, h->d_gains, h->d_du, h->d_steps, h->d_states, h->d_actions, h->d_times, h->d_residual,
                   h->d_costs, h->d_trace, h->d_returns, h->d_failure, h->d_order, h->d_stats, h->d_pair_sync,
-                  h->d_sensors, h->d_step};
+                  h->d_sensors, h->d_step, h->d_variants, h->d_variant_index};
   for (void* p : bufs) if (p) cudaFree(p);
   ilqg_free(h->ilqg);
   delete h->bank;
@@ -618,6 +702,93 @@ int mjpc_b200_set_differentiable(mjpc_b200_t* h, int on) {
   return 0;
 }
 
+// Per-problem model variants: validate every blob against the handle's model as created (variant_mismatch), then
+// upload them into one allocation, variant v's block at d_variants + v * variant_stride:
+//   [its nf floats, with the handle's live task floats][its ni ints][its keyframe table (Ctx::gkey)][pad][meaninertia]
+// The blocks are what a handle created from the variant uploads as d_pack, so problem b of a launch computes what such
+// a handle computes.  count = 0 (or NULL) clears them.  Nothing is changed on a refusal.
+int mjpc_b200_set_model_variants(mjpc_b200_t* h, const mjpc_model_blob* models, int count) {
+  if (!h || count < 0 || (count > 0 && !models)) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "set_model_variants: bad argument");
+  if (count > h->maxN)
+    return fail(MJPC_B200_ERR_CAPACITY, "set_model_variants: more variants than max_candidates problems");
+  CUDA_TRY(cudaSetDevice(h->device));
+  const DevModel& M = h->M0;
+  size_t stride = 0;
+  std::vector<ModelPack> packs(count);
+  for (int v = 0; v < count; v++) {
+    const std::string at = "set_model_variants: variant " + std::to_string(v) + ": ";
+    if (!models[v].data) return fail(MJPC_B200_ERR_BAD_ARGUMENT, at + "NULL blob");
+    std::vector<DevSensor> sensors;
+    std::vector<std::string> why;
+    try {
+      packs[v] = pack_model(models[v].data, models[v].nbytes, M.maxcon - 2 * M.ntendon, M.maxefc);
+      Blob b(models[v].data, models[v].nbytes);
+      if (b.i("nuserdata") != 0)
+        return fail(MJPC_B200_ERR_UNSUPPORTED, at + "mjData::userdata (nuserdata > 0) is not supported");
+      sensor_table(b, &sensors, &why);
+    } catch (const std::exception& e) {
+      return fail(MJPC_B200_ERR_BAD_BLOB, at + e.what());
+    }
+    const std::string field = variant_mismatch(h, packs[v], sensors, why);
+    if (!field.empty()) return fail(MJPC_B200_ERR_BAD_ARGUMENT, at + field + " differs from the handle's model");
+    stride = std::max(stride, (size_t)(M.nf + M.ni) + packs[v].key_mpos.size() + 1);
+  }
+  stride = (stride + 31) & ~(size_t)31;   // 128-byte aligned blocks (the TMA copy needs 16)
+  float* d = nullptr;
+  int* di = nullptr;
+  if (count) {
+    std::vector<float> blocks((size_t)count * stride, 0.f);
+    const size_t t0 = task_floats_begin(M), nt = task_floats_count(M);
+    for (int v = 0; v < count; v++) {
+      float* o = blocks.data() + (size_t)v * stride;
+      const ModelPack& P = packs[v];
+      std::copy(P.f.begin(), P.f.end(), o);
+      std::copy(h->pack.f.begin() + t0, h->pack.f.begin() + t0 + nt, o + t0);   // the live task (set_task)
+      std::memcpy(o + M.nf, P.i.data(), P.i.size() * 4);
+      for (size_t k = 0; k < P.key_mpos.size(); k++) o[M.nf + M.ni + k] = (float)P.key_mpos[k];
+      o[stride - 1] = P.M.meaninertia;
+    }
+    std::vector<int> identity(h->maxN);
+    for (int v = 0; v < h->maxN; v++) identity[v] = v < count ? v : 0;
+    if (cudaError_t e = dalloc(&d, blocks.size())) return fail(MJPC_B200_ERR_CUDA, std::string("set_model_variants: ") + cudaGetErrorString(e));
+    cudaError_t e = dalloc(&di, identity.size());
+    if (e == cudaSuccess) e = cudaMemcpy(d, blocks.data(), blocks.size() * 4, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(di, identity.data(), identity.size() * 4, cudaMemcpyHostToDevice);
+    if (e != cudaSuccess) {
+      cudaFree(d); if (di) cudaFree(di);
+      return fail(MJPC_B200_ERR_CUDA, std::string("set_model_variants: ") + cudaGetErrorString(e));
+    }
+  }
+  CUDA_TRY(cudaStreamSynchronize(h->stream));   // launches in flight may still read the old blocks
+  if (h->d_variants) cudaFree(h->d_variants);
+  if (h->d_variant_index) cudaFree(h->d_variant_index);
+  h->d_variants = d; h->d_variant_index = di;
+  h->nvariants = count; h->nselected = count; h->variant_stride = (int)stride;
+  h->resident_ok = false;
+  return 0;
+}
+
+// The variant each problem of the following launches runs on: problem j on variant index[j] (NULL: the identity over
+// all variants), and those launches hold exactly B problems.  Without variants set there is nothing to select.
+int mjpc_b200_select_model_variants(mjpc_b200_t* h, const int* index, int B) {
+  if (!h) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "select_model_variants: null");
+  if (!h->nvariants) return 0;
+  if (!index) B = h->nvariants;
+  if (B < 1 || B > h->maxN) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "select_model_variants: bad B");
+  std::vector<int> sel(B);
+  for (int j = 0; j < B; j++) {
+    sel[j] = index ? index[j] : j;
+    if (sel[j] < 0 || sel[j] >= h->nvariants)
+      return fail(MJPC_B200_ERR_BAD_ARGUMENT, "select_model_variants: variant index outside [0, count)");
+  }
+  CUDA_TRY(cudaSetDevice(h->device));
+  CUDA_TRY(cudaMemcpyAsync(h->d_variant_index, sel.data(), (size_t)B * 4, cudaMemcpyHostToDevice, h->stream));
+  CUDA_TRY(cudaStreamSynchronize(h->stream));   // sel is pageable
+  h->nselected = B;
+  h->resident_ok = false;
+  return 0;
+}
+
 // Validate and upload a spline launch of B problems x N candidates; it becomes the resident launch.  B = 1 is the
 // single-problem call.  Nothing is changed on a refusal, so the handle stays usable.
 static int upload_spline(mjpc_b200_t* h, int B, const float* states, const double* times, const float* mocaps,
@@ -644,6 +815,7 @@ int mjpc_b200_upload_spline_inputs(mjpc_b200_t* h, const float* state, double ti
                                    const float* userdata, const float* knots, const double* knot_times, int interp,
                                    int P, int N, int H) {
   if (!h || !state || !knots || !knot_times) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "rollout_spline: null pointer");
+  if (int rc = check_variants(h, -1, "rollout_spline")) return rc;
   // mjData::userdata: none of the implemented residuals reads it; a model that declares nuserdata > 0 is rejected at
   // create(), so a non-NULL pointer here can only be a caller error - refuse rather than silently ignore it
   if (userdata && h->nuserdata == 0) return fail(MJPC_B200_ERR_UNSUPPORTED, "rollout_spline: the model has nuserdata = 0, userdata must be NULL");
@@ -664,6 +836,7 @@ int mjpc_b200_rollout_spline_batched(mjpc_b200_t* h, int B, const float* states,
 
 int mjpc_b200_launch_resident(mjpc_b200_t* h) {
   if (!h || !h->resident_ok) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "launch_resident: no uploaded inputs");
+  if (int rc = check_variants(h, h->resident.nprob, "launch_resident")) return rc;
   CUDA_TRY(cudaSetDevice(h->device));
   // the step table was built on the upload's clock; a set_options timestep since then needs a new upload
   if (h->resident.timestep != h->pack.timestep)
@@ -743,6 +916,7 @@ int mjpc_b200_rollout_feedback(mjpc_b200_t* h, const float* state, double time, 
                                float* returns, uint8_t* failure, int* order) {
   if (!h || !state || !u_nom || !x_nom || !t_nom || !gains || !step_sizes)
     return fail(MJPC_B200_ERR_BAD_ARGUMENT, "rollout_feedback: null pointer");
+  if (int rc = check_variants(h, -1, "rollout_feedback")) return rc;
   if (userdata && h->nuserdata == 0) return fail(MJPC_B200_ERR_UNSUPPORTED, "rollout_feedback: the model has nuserdata = 0, userdata must be NULL");
   return rollout_feedback_impl(h, 1, state, &time, mocap, nullptr, nullptr, nullptr, u_nom, x_nom, t_nom, gains, du,
                                step_sizes, mode, K, H, returns, failure, order);
@@ -879,6 +1053,7 @@ int mjpc_b200_step_debug(mjpc_b200_t* h, const float* qpos, const float* qvel, c
                          const float* mocap, double time, const float* warmstart, float* qacc, float* residual,
                          float* next_qpos, float* next_qvel, float* qM, float* efc_force, int* counts) {
   if (!h || !qpos || !qvel || !ctrl) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "step_debug: null");
+  if (int rc = check_variants(h, -1, "step_debug")) return rc;
   h->dbg_ncon = -1;
   h->dbg_contact.resize((size_t)h->pack.M.maxcon * 8);
   if (efc_force) std::fill_n(efc_force, 256, 0.f);   // the caller's efc_force holds 256 floats, the first maxefc are rows
@@ -894,6 +1069,7 @@ int mjpc_b200_step_debug(mjpc_b200_t* h, const float* qpos, const float* qvel, c
 int mjpc_b200_step_debug_contacts(mjpc_b200_t* h, int capacity, float* contact, int* ncon) {
   if (!h || capacity < 0 || (capacity > 0 && !contact) || !ncon)
     return fail(MJPC_B200_ERR_BAD_ARGUMENT, "step_debug_contacts: bad argument");
+  if (int rc = check_variants(h, -1, "step_debug_contacts")) return rc;
   if (h->dbg_ncon < 0) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "step_debug_contacts: no step_debug call to report");
   *ncon = h->dbg_ncon;
   const int n = std::min(h->dbg_ncon, capacity);
@@ -949,6 +1125,7 @@ int mjpc_b200_rollout_spline_sharded(mjpc_b200_t* h, const float* state, double 
                                      const float* userdata, const float* knots, const double* knot_times, int interp,
                                      int P, int N, int H, float* returns, uint8_t* failure, int* order) {
   if (!h || !knots) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "rollout_spline_sharded: null");
+  if (int rc = check_variants(h, -1, "rollout_spline_sharded")) return rc;
   if (!h->noise_seeds.empty())
     return fail(MJPC_B200_ERR_UNSUPPORTED, "rollout_spline_sharded: per-problem noise keys (set_xfrc_noise_batched)");
   if (h->nranks > 1 && !h->comm) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "rollout_spline_sharded: comm_init first");
@@ -1024,6 +1201,7 @@ int mjpc_b200_step_batch(mjpc_b200_t* h, int B, const float* qpos, const float* 
                          const float* warmstart, const float* mocap, double time0, const double* times, float* qacc,
                          float* next_qpos, float* next_qvel, float* residual, float* cost, int* counts) {
   if (!h || B < 1 || !qpos || !qvel || !ctrl || !times) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "step_batch: bad argument");
+  if (int rc = check_variants(h, -1, "step_batch")) return rc;
   if (h->pack.M.nmocap && !mocap) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "step_batch: mocap required");
   const KernelSet* k;
   const int kind = pick_kernels(h, &k);
@@ -1041,6 +1219,7 @@ int mjpc_b200_step_sensors(mjpc_b200_t* h, int B, const float* states, const flo
                            float* sensordata, float* qacc, int* counts) {
   if (!h || B < 1 || !states || (!ctrl && h->pack.M.nu) || !next_states || !sensordata)
     return fail(MJPC_B200_ERR_BAD_ARGUMENT, "step_sensors: bad argument");
+  if (int rc = check_variants(h, -1, "step_sensors")) return rc;
   const DevModel& M = h->pack.M;
   if (M.nmocap && !mocap) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "step_sensors: mocap required");
   const int nsens = (int)h->sensors.size();
@@ -1172,7 +1351,8 @@ static int model_derivatives_impl(mjpc_b200_t* h, int B, const float* x, const f
   const KernelSet* k;
   pick_kernels(h, &k);
   int launches = 0;
-  int rc = ilqg_model_derivatives(h->ilqg, M, h->d_pack, h->stream, k->fd_center, k->fd_column, B, x, u, trel.data(), mocaps, ts.data(),
+  int rc = ilqg_model_derivatives(h->ilqg, M, launch_pack(h), launch_stride(h), h->d_variant_index,
+                                  h->stream, k->fd_center, k->fd_column, B, x, u, trel.data(), mocaps, ts.data(),
                                   weights ? w.data() : nullptr, parameters ? p.data() : nullptr, H, tol, A, B_, C, D,
                                   smem, &launches, h->ev0, h->ev1, skip, mode);
   h->launches += launches;
@@ -1184,6 +1364,7 @@ static int model_derivatives_impl(mjpc_b200_t* h, int B, const float* x, const f
 int mjpc_b200_model_derivatives(mjpc_b200_t* h, const float* x, const float* u, const double* t, const float* mocap,
                                 int H, int skip, float tol, int mode, float* A, float* B, float* C, float* D) {
   if (!h || !x || !u || !t || !A || !B || !C || !D) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "model_derivatives: null");
+  if (int rc = check_variants(h, -1, "model_derivatives")) return rc;
   if (H < 1 || H > h->maxH || !(tol > 0)) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "model_derivatives: bad H or tol");
   if (skip < 0 || mode < 0 || mode > 1) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "model_derivatives: bad skip or mode");
   if (h->pack.M.nmocap && !mocap) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "model_derivatives: mocap required");
@@ -1199,6 +1380,7 @@ int mjpc_b200_model_derivatives_batched(mjpc_b200_t* h, int B, const float* x, c
   if (H > h->maxH) return fail(MJPC_B200_ERR_CAPACITY, "model_derivatives_batched: H above max_horizon");
   if (skip < 0 || mode < 0 || mode > 1) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "model_derivatives_batched: bad skip or mode");
   if (h->pack.M.nmocap && !mocaps) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "model_derivatives_batched: mocap required");
+  if (int rc = check_variants(h, B, "model_derivatives_batched")) return rc;
   return model_derivatives_impl(h, B, x, u, t, mocaps, weights, parameters, task_states, H, skip, tol, mode, A, B_, C, D);
 }
 
@@ -1223,6 +1405,7 @@ int mjpc_b200_cost_derivatives(mjpc_b200_t* h, const float* residual, const floa
                                float* cx, float* cu, float* cxx, float* cuu, float* cxu) {
   if (!h || !residual || !C || !D || !cx || !cu || !cxx || !cuu || !cxu)
     return fail(MJPC_B200_ERR_BAD_ARGUMENT, "cost_derivatives: null");
+  if (int rc = check_variants(h, -1, "cost_derivatives")) return rc;
   if (H < 1 || H > h->maxH) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "cost_derivatives: bad H");
   return cost_derivatives_impl(h, 1, nullptr, residual, C, D, H, cx, cu, cxx, cuu, cxu);
 }
@@ -1245,6 +1428,7 @@ int mjpc_b200_gradient_batched(mjpc_b200_t* h, int B, const float* x, const floa
   if (H > h->maxH) return fail(MJPC_B200_ERR_CAPACITY, "gradient_batched: H above max_horizon");
   if (skip < 0 || mode < 0 || mode > 1) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "gradient_batched: bad skip or mode");
   if (h->pack.M.nmocap && !mocaps) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "gradient_batched: mocap required");
+  if (int rc = check_variants(h, B, "gradient_batched")) return rc;
   const DevModel& M = h->pack.M;
   CUDA_TRY(cudaSetDevice(h->device));
   if (cost_derivatives_smem(M, h->max_term_dim) > h->smem_optin)
@@ -1258,7 +1442,8 @@ int mjpc_b200_gradient_batched(mjpc_b200_t* h, int B, const float* x, const floa
   // the two derivative sweeps exactly as their batched entry points stage them, except that A, B, C, D and the cost
   // derivatives stay on the device; one span from the first kernel to the sweep's end
   int launches = 0;
-  int rc = ilqg_model_derivatives(h->ilqg, M, h->d_pack, h->stream, ks->fd_center, ks->fd_column, B, x, u, trel.data(),
+  int rc = ilqg_model_derivatives(h->ilqg, M, launch_pack(h), launch_stride(h), h->d_variant_index,
+                                  h->stream, ks->fd_center, ks->fd_column, B, x, u, trel.data(),
                                   mocaps, ts.data(), weights ? w.data() : nullptr, parameters ? p.data() : nullptr, H,
                                   tol, nullptr, nullptr, nullptr, nullptr, h->smem_bytes(1), &launches, h->ev0,
                                   nullptr, skip, mode);
@@ -1294,6 +1479,7 @@ int mjpc_b200_backward_pass(mjpc_b200_t* h, const float* A, const float* B, cons
                             int* status_out) {
   if (!h || !A || !B || !cx || !cu || !cxx || !cxu || !cuu || !actions || !K || !du || !dV || !status_out)
     return fail(MJPC_B200_ERR_BAD_ARGUMENT, "backward_pass: null");
+  if (int rc = check_variants(h, -1, "backward_pass")) return rc;
   if (H < 2 || H > h->maxH) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "backward_pass: bad H");
   return backward_pass_impl(h, 1, A, B, cx, cu, cxx, cxu, cuu, actions, H, &mu, reg_type, limits, K, du, dV, Vx, Vxx,
                             status_out);
@@ -1421,7 +1607,8 @@ static int step_rows(mjpc_b200_t* h, const KernelSet* ks) {
   const FilterBankArgs& a = k.a;
   StepBatchArgs A;
   std::memset(&A, 0, sizeof(A));
-  A.M = h->pack.M; A.L = make_layout(h->pack.M, 1); A.pack = h->d_pack;
+  A.M = h->pack.M; A.L = make_layout(h->pack.M, 1);
+  A.pack = launch_pack(h); A.pack_stride = launch_stride(h); A.pack_rows = a.rows; A.pack_index = h->d_variant_index;
   A.qpos = a.qpos; A.qvel = a.qvel; A.ctrl = a.rctrl; A.warmstart = a.rwarm;
   A.mocap = a.rmocap; A.mocap_stride = 7 * a.nmocap;
   A.task_state = h->pack.M.task_state_size ? k.d_task : nullptr; A.time = k.d_rtime; A.B = a.B * a.rows;
@@ -1441,6 +1628,7 @@ int Update(mjpc_b200_t* h, const float* ctrl, const double* sensor, const float*
     return fail(MJPC_B200_ERR_BAD_ARGUMENT, "filter bank update: bad argument");
   FilterBank& k = *h->bank;
   FilterBankArgs a = k.a;
+  if (int rc = check_variants(h, a.B, "filter bank update")) return rc;
   const size_t B = a.B, ny = a.ny, nu = a.nu, nm = 7 * (size_t)a.nmocap;
   CUDA_TRY(cudaSetDevice(h->device));
   CUDA_TRY(cudaStreamSynchronize(h->stream));   // the staging may still feed an earlier copy

@@ -36,6 +36,16 @@ void BatchPlanner::SetTask(int b, const double* weight, const double* parameters
   if (task_state) std::copy(task_state, task_state + nts_, task_state_.begin() + (size_t)b * nts_);
 }
 
+int BatchPlanner::SetModels(const mjpc_model_blob* models, int count) {
+  if (count != 0 && count != NumProblems())
+    return MJPC_B200_ERR_BAD_ARGUMENT;
+  // the handles were created from one model, so a variant the rule refuses is refused by the first, before any
+  // handle changed
+  for (mjpc_b200_t* h : Handles())
+    if (int rc = mjpc_b200_set_model_variants(h, models, count)) return rc;
+  return 0;
+}
+
 TaskRows BatchPlanner::Rows() const {
   TaskRows r;
   r.w = weight_.data(); r.p = parameters_.data(); r.ts = task_state_.data(); r.nw = nw_; r.np = np_; r.nts = nts_;
@@ -264,6 +274,10 @@ int mjpc_b200_batch_planner_set_task(void* p, int problem, const double* weight,
   if (!bp) return MJPC_B200_ERR_BAD_ARGUMENT;
   bp->SetTask(problem, weight, parameters, task_state);
   return 0;
+}
+int mjpc_b200_batch_planner_set_models(void* p, const mjpc_model_blob* models, int count) {
+  if (!p || count < 0) return MJPC_B200_ERR_BAD_ARGUMENT;
+  return batch_of(p)->SetModels(models, count);
 }
 int mjpc_b200_batch_planner_optimize_policy(void* p, int horizon) {
   if (!p) return MJPC_B200_ERR_BAD_ARGUMENT;

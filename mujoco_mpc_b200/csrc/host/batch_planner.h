@@ -33,6 +33,9 @@ class BatchPlanner {
   void SetTask(int b, const double* weight, const double* parameters, const double* task_state);
   // Planner::OptimizePolicy of every problem
   virtual int OptimizePolicy(int horizon) = 0;
+  // problem b plans on models[b] from now on (mjpc_b200_set_model_variants on every handle the batch owns); count is
+  // the number of problems, or 0 to plan every problem on the batch's model again
+  int SetModels(const mjpc_model_blob* models, int count);
 
  protected:
   // the task snapshots of num_problems problems, each the model's, and the engine handle of max_candidates (all
@@ -47,6 +50,9 @@ class BatchPlanner {
     for (auto& p : problems_) ps.push_back(static_cast<T*>(p.get()));
     return ps;
   }
+
+  // every engine handle the batch owns: gpu_, and the second handle of the Robust and iLQS batches
+  virtual std::vector<mjpc_b200_t*> Handles() const { return {gpu_}; }
 
   mjpc_b200_t* gpu_ = nullptr;
   std::vector<std::unique_ptr<Planner>> problems_;   // borrow gpu_
@@ -96,6 +102,7 @@ class BatchRobustPlanner : public BatchPlanner {
   int OptimizePolicy(int horizon) override;
 
  private:
+  std::vector<mjpc_b200_t*> Handles() const override { return {gpu_, noisy_gpu_}; }
   mjpc_b200_t* noisy_gpu_ = nullptr;
 };
 
@@ -125,6 +132,7 @@ class BatchILQSPlanner : public BatchPlanner {
   int improved(int b) const { return improved_[b]; }    // iLQSPlanner::OptimizePolicy's 1/0; 0 after an error
 
  private:
+  std::vector<mjpc_b200_t*> Handles() const override { return {gpu_, ilqg_gpu_}; }
   mjpc_b200_t* ilqg_gpu_ = nullptr;
   ILQGSweeps sweeps_;
   std::vector<int> improved_;

@@ -62,7 +62,7 @@ int Estimator::Initialize(const mjpc_model_blob* model, int kind_, int num_filte
   if (kind == kKalman && !(settings[0] > 0)) return Fail(MJPC_B200_ERR_BAD_ARGUMENT, "bad argument");
   if (int rc = m_.Load(model)) return Fail(rc, "bad blob");
   std::vector<int> dims;
-  if (LoadEstimatorBlob(model, m_, &dims, &nmocap_, &mocap0_, &key_state_))
+  if (LoadEstimatorBlob(model, m_, &dims, &nmocap_, &model_mocap0_, &model_key_state_))
     return Fail(MJPC_B200_ERR_BAD_BLOB, "blob without sensor entries");
   if (sensor_start < 0 || nsensor < 1 || sensor_start > (int)dims.size() - nsensor)
     return Fail(MJPC_B200_ERR_BAD_ARGUMENT, "sensor range outside the model's sensors");
@@ -95,7 +95,11 @@ int Estimator::Initialize(const mjpc_model_blob* model, int kind_, int num_filte
   if (int rc = mjpc_b200_set_options(engine_, timestep, 0)) return Fail(rc, mjpc_b200_last_error());
   if (int rc = mjpc_b200_bank::Init(engine_, d)) return Fail(rc, mjpc_b200_last_error());
   fctrl_.resize((size_t)num_filters * m_.nu); ctrl_.resize(fctrl_.size());
-  fmocap_.resize((size_t)num_filters * mocap0_.size()); mocap_.resize(fmocap_.size());
+  fmocap_.resize((size_t)num_filters * model_mocap0_.size()); mocap_.resize(fmocap_.size());
+  for (int b = 0; b < num_filters; b++) {
+    key_state_.insert(key_state_.end(), model_key_state_.begin(), model_key_state_.end());
+    mocap0_.insert(mocap0_.end(), model_mocap0_.begin(), model_mocap0_.end());
+  }
   for (int b = 0; b < num_filters; b++)
     if (int rc = Reset(b, nullptr, 0.0, 1e-4, 1e-4, 1e-4)) return rc;
   return 0;
@@ -108,12 +112,30 @@ int Estimator::Reset(int b, const double* state, double time, double covariance_
   for (int i = 0; i < ndstate; i++) P[(size_t)i * ndstate + i] = covariance_scale;
   std::vector<float> warm(m_.nv, 0.f);
   int warnings = 0;
-  const void* fields[] = {state ? state : key_state_.data(), P.data(), &time, np.data(), ns.data(), warm.data(),
+  const size_t nx = model_key_state_.size(), nm = model_mocap0_.size();
+  const void* fields[] = {state ? state : key_state_.data() + b * nx, P.data(), &time, np.data(), ns.data(), warm.data(),
                           &warnings};
   for (int f = mjpc_b200_bank::STATE; f <= mjpc_b200_bank::WARNINGS; f++)
     if (int rc = Access(engine_, b, f, const_cast<void*>(fields[f]), 1)) return Fail(rc, mjpc_b200_last_error());
   std::fill_n(ctrl_.begin() + (size_t)b * m_.nu, m_.nu, 0.f);
-  std::copy(mocap0_.begin(), mocap0_.end(), mocap_.begin() + (size_t)b * mocap0_.size());
+  std::copy_n(mocap0_.begin() + b * nm, nm, mocap_.begin() + b * nm);
+  return 0;
+}
+
+int Estimator::SetModels(const mjpc_model_blob* models, int count) {
+  if (count != 0 && (count != num_filters || !models)) return Fail(MJPC_B200_ERR_BAD_ARGUMENT, "set_models: count is not num_filters or 0");
+  if (int rc = mjpc_b200_set_model_variants(engine_, models, count)) return Fail(rc, mjpc_b200_last_error());
+  const size_t nx = model_key_state_.size(), nm = model_mocap0_.size();
+  for (int b = 0; b < num_filters; b++) {
+    std::vector<int> dims;
+    int nmocap = 0;
+    std::vector<float> mocap0 = model_mocap0_;
+    std::vector<double> key_state = model_key_state_;
+    if (count && LoadEstimatorBlob(&models[b], m_, &dims, &nmocap, &mocap0, &key_state))
+      return Fail(MJPC_B200_ERR_BAD_BLOB, "set_models: blob without sensor entries");
+    std::copy_n(key_state.begin(), nx, key_state_.begin() + b * nx);
+    std::copy_n(mocap0.begin(), nm, mocap0_.begin() + b * nm);
+  }
   return 0;
 }
 
@@ -150,10 +172,10 @@ int Estimator::Update(const double* ctrl, const double* sensor, const float* moc
     return 0;
   }
   // ctrl in the engine's float; a NULL mocap is the model's for every filter
-  const size_t nu = m_.nu, nm = mocap0_.size();
+  const size_t nu = m_.nu, nm = model_mocap0_.size();
   for (size_t i = 0; i < fctrl_.size(); i++) fctrl_[i] = (float)ctrl[i];
   for (int b = 0; b < num_filters; b++)
-    std::copy_n(mocap ? mocap + b * nm : mocap0_.data(), nm, fmocap_.begin() + b * nm);
+    std::copy_n((mocap ? mocap : mocap0_.data()) + b * nm, nm, fmocap_.begin() + b * nm);
   if (int rc = mjpc_b200_bank::Update(engine_, fctrl_.data(), sensor, fmocap_.data(), phases, status))
     return Fail(rc, mjpc_b200_last_error());
   for (int b = 0; b < num_filters; b++)
@@ -322,6 +344,10 @@ int mjpc_b200_batch_estimator_update(void* f, const double* ctrl, const double* 
 int mjpc_b200_batch_estimator_get(void* f, int filter, double* state, double* covariance, double* time,
                                   double* scalars) {
   return f ? static_cast<Estimator*>(f)->Get(filter, state, covariance, time, scalars) : MJPC_B200_ERR_BAD_ARGUMENT;
+}
+
+int mjpc_b200_batch_estimator_set_models(void* f, const mjpc_model_blob* models, int count) {
+  return f && count >= 0 ? static_cast<Estimator*>(f)->SetModels(models, count) : MJPC_B200_ERR_BAD_ARGUMENT;
 }
 
 const char* mjpc_b200_batch_estimator_last_error(const void* f) {

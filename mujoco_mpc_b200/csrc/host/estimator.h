@@ -61,6 +61,9 @@ class Estimator {
   // filter b's state, covariance, time and scalars {ndstate, rows, nsensordata, warnings, timestep} (Kalman: then
   // epsilon); any pointer may be NULL
   int Get(int b, double* state, double* covariance, double* time, double* scalars);
+  // filter b runs on models[b] from now on (mjpc_b200_set_model_variants), and its Reset state and default mocap are
+  // that model's; count is num_filters, or 0 for the bank's model again.  The filters' states are kept.
+  int SetModels(const mjpc_model_blob* models, int count);
   const char* Name() const { return kind == kKalman ? "kalman" : kind == kUnscented ? "unscented" : "estimator"; }
 
   int kind = 0, num_filters = 0, ndstate = 0, nsensordata = 0, rows = 0;
@@ -72,7 +75,9 @@ class Estimator {
   mjpc_b200_t* engine_ = nullptr;
   HostModel m_;
   int nmocap_ = 0;
-  std::vector<double> key_state_;
+  std::vector<double> model_key_state_;   // the bank's model's Reset state [nq + nv] and mocap [7 nmocap]
+  std::vector<float> model_mocap0_;
+  std::vector<double> key_state_;         // [B][nq + nv], [B][7 nmocap]: those of each filter's model
   std::vector<float> mocap0_;
   std::vector<float> fctrl_, fmocap_;   // [B][nu], [B][7 nmocap]: the inputs of the update being made
   std::vector<float> ctrl_, mocap_;     // [B][nu], [B][7 nmocap]: those of each filter's last successful measurement

@@ -306,6 +306,8 @@ int ILQGSweeps::FeedbackLaunch(const std::vector<iLQGPlanner*>& ps, const std::v
   gather(p_, task, rows.np, [&](int r) { return rows.p + (size_t)r * rows.np; });
   gather(ts_, task, rows.nts, [&](int r) { return rows.ts + (size_t)r * rows.nts; });
   ret_.resize(J * K); fail_.resize(J * K); order_.resize(J * K);
+  // with model variants, sweep problem j runs on the variant of the problem it plans (its task row)
+  if (int rc = mjpc_b200_select_model_variants(p0.gpu_, task.data(), (int)J)) return rc;
   return mjpc_b200_rollout_feedback_batched(p0.gpu_, (int)J, st_.data(), times_.data(), nm ? mc_.data() : nullptr,
                                             rows.nw ? w_.data() : nullptr, rows.np ? p_.data() : nullptr,
                                             rows.nts ? ts_.data() : nullptr, u_.data(), x_.data(), t_.data(), g_.data(),
@@ -352,7 +354,8 @@ int ILQGSweeps::Iterate(const std::vector<iLQGPlanner*>& ps, const std::vector<i
   A_.resize(J * H * n * n); B_.resize(J * H * n * m); C_.resize(J * H * nr * n); D_.resize(J * H * nr * m);
   cx_.resize(J * H * n); cu_.resize(J * H * m); cxx_.resize(J * H * n * n); cuu_.resize(J * H * m * m);
   cxu_.resize(J * H * n * m);
-  if (mjpc_b200_model_derivatives_batched(p0.gpu_, J, x_.data(), u_.data(), t_.data(), nm ? mc_.data() : nullptr,
+  if (mjpc_b200_select_model_variants(p0.gpu_, task.data(), J) ||
+      mjpc_b200_model_derivatives_batched(p0.gpu_, J, x_.data(), u_.data(), t_.data(), nm ? mc_.data() : nullptr,
                                           rows.nw ? w_.data() : nullptr, rows.np ? p_.data() : nullptr,
                                           rows.nts ? ts_.data() : nullptr, horizon, settings.derivative_skip,
                                           (float)settings.fd_tolerance, settings.fd_mode, A_.data(), B_.data(),

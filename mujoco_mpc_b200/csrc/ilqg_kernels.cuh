@@ -127,6 +127,8 @@ struct FdArgs {
   DevModel M;
   DevLayout L;
   const float* pack;
+  int pack_stride;          // model variants: problem b stages its variant block (problem_pack); 0: the one pack
+  const int* pack_index;    // [B]
   const float* x;  // [B][H][ds]
   const float* u;  // [B][H][nu]
   const float* t;  // [B][H] times relative to the problem's t[0]
@@ -182,9 +184,10 @@ __device__ __forceinline__ void fd_load_state(Ctx& c, const FdProb& P, int t, co
 template <class SP>
 __device__ __forceinline__ void fd_center_body(const FdArgs& A) {
   float* smem = g_smem;
-  stage_model_pack(smem, A.pack, (unsigned)((A.M.nf + A.M.ni) * 4));
+  const float* pack = problem_pack(A.pack, A.pack_stride, A.pack_index, (int)blockIdx.y);
+  stage_model_pack(smem, pack, (unsigned)((A.M.nf + A.M.ni) * 4));
   Ctx c;
-  init_ctx(c, &A.M, &A.L, smem, threadIdx.x, A.pack);
+  init_ctx(c, &A.M, &A.L, smem, threadIdx.x, pack, A.pack_stride);
   auto&& M = SP::model(c);
   const int lane = c.lane, t = A.eval_t[blockIdx.x], nq = M.nq, nv = M.nv, ds = nq + nv, nr = M.num_residual;
   const FdProb P = fd_problem<SP>(c, A, blockIdx.y);
@@ -232,9 +235,10 @@ __device__ __forceinline__ void fd_perturb(Ctx& c, int col, int nu, int nv, floa
 template <class SP>
 __device__ __forceinline__ void fd_column_body(const FdArgs& A) {
   float* smem = g_smem;
-  stage_model_pack(smem, A.pack, (unsigned)((A.M.nf + A.M.ni) * 4));
+  const float* pack = problem_pack(A.pack, A.pack_stride, A.pack_index, (int)blockIdx.y);
+  stage_model_pack(smem, pack, (unsigned)((A.M.nf + A.M.ni) * 4));
   Ctx c;
-  init_ctx(c, &A.M, &A.L, smem, threadIdx.x, A.pack);
+  init_ctx(c, &A.M, &A.L, smem, threadIdx.x, pack, A.pack_stride);
   auto&& M = SP::model(c);
   const int lane = c.lane, nq = M.nq, nv = M.nv, nu = M.nu, ds = nq + nv, n = 2 * nv, nr = M.num_residual;
   const int ncol = nu + 2 * nv;
@@ -932,8 +936,10 @@ inline int ilqg_reserve(IlqgBuffers& b, const DevModel& M, int nprob, cudaStream
 
 // nprob problems with common H / skip / mode, on the fd_center / fd_column instances given.  Host inputs are [nprob][..]:
 // x, u, trel (relative to each problem's t[0]), mocap, ts (rebased likewise); w / prm (float weights / parameters) may
-// be nullptr for the packed values.  A NULL host output A / B / C / D is not copied back: it stays in b only.
-inline int ilqg_model_derivatives(IlqgBuffers& b, const DevModel& M, const float* d_pack, cudaStream_t st,
+// be nullptr for the packed values.  A NULL host output A / B / C / D is not copied back: it stays in b only.  With
+// pack_stride != 0, problem p runs on model variant pack_index[p] (FdArgs).
+inline int ilqg_model_derivatives(IlqgBuffers& b, const DevModel& M, const float* d_pack, int pack_stride,
+                                  const int* pack_index, cudaStream_t st,
                                   const void* fd_center, const void* fd_column, int nprob,
                                   const float* x, const float* u, const float* trel, const float* mocap, const float* ts,
                                   const float* w, const float* prm, int H, float eps, float* A, float* B, float* C,
@@ -987,7 +993,7 @@ inline int ilqg_model_derivatives(IlqgBuffers& b, const DevModel& M, const float
   FdArgs a;
   std::memset(&a, 0, sizeof(a));
   a.eval_t = b.idx; a.neval = neval; a.mode = mode; a.yp = b.yp; a.rp = b.rp;
-  a.M = M; a.L = make_layout(M, 1); a.pack = d_pack; a.x = b.x; a.u = b.u; a.t = b.t; a.mocap = b.mocap;
+  a.M = M; a.L = make_layout(M, 1); a.pack = d_pack; a.pack_stride = pack_stride; a.pack_index = pack_index; a.x = b.x; a.u = b.u; a.t = b.t; a.mocap = b.mocap;
   a.task_state = M.task_state_size ? b.ts : nullptr; a.H = H; a.eps = eps; a.y0 = b.y0; a.r0 = b.r0; a.q0 = b.q0;
   a.weight = (w && M.num_term) ? b.w : nullptr; a.parameters = (prm && M.num_parameters) ? b.prm : nullptr;
   a.A = b.A; a.B = b.B; a.C = b.C; a.D = b.D;

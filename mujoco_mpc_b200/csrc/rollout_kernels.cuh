@@ -24,6 +24,10 @@ struct RolloutArgs {
   DevModel M;
   DevLayout L;
   const float* pack;        // device: nf floats followed by ni ints
+  // model variants (set_model_variants): problem prob stages the block pack + pack_index[prob] * pack_stride instead;
+  // pack_stride 0: every problem the one pack (pack_index unread)
+  int pack_stride;
+  const int* pack_index;    // [nprob]
   int nprob, nper;
   const float* state;       // [nprob][dim_state]
   const float* mocap;       // [nprob][7*nmocap]
@@ -79,9 +83,16 @@ __host__ __device__ inline int smem_header_words(const DevModel& M) {
   return M.nf + M.ni + (int)((sizeof(DevModel) + 15) / 16) * 4 + (int)((sizeof(DevLayout) + 15) / 16) * 4;
 }
 
-// copy the DevModel / DevLayout kernel parameters behind the pack and set up this warp's context
+// the model block a CTA of problem `prob` stages: the pack, or with model variants the problem's variant block
+__device__ __forceinline__ const float* problem_pack(const float* pack, int stride, const int* index, int prob) {
+  return stride ? pack + (size_t)index[prob] * stride : pack;
+}
+
+// copy the DevModel / DevLayout kernel parameters behind the pack and set up this warp's context.  `pack` is the block
+// the CTA staged; with model variants (stride != 0) the last word of the variant's block is its meaninertia, which
+// replaces the header's (the one float of the header a variant may change)
 __device__ __forceinline__ void init_ctx(Ctx& c, const DevModel* M, const DevLayout* L, float* smem, int lane,
-                                         const float* pack) {
+                                         const float* pack, int stride = 0) {
   const int hdr = M->nf + M->ni;
   const int lay = hdr + (int)((sizeof(DevModel) + 15) / 16) * 4;
   const int data0 = lay + (int)((sizeof(DevLayout) + 15) / 16) * 4;
@@ -89,7 +100,9 @@ __device__ __forceinline__ void init_ctx(Ctx& c, const DevModel* M, const DevLay
     const int* srcM = reinterpret_cast<const int*>(M);
     const int* srcL = reinterpret_cast<const int*>(L);
     int* dst = reinterpret_cast<int*>(smem);
-    for (int i = threadIdx.x; i < (int)(sizeof(DevModel) / 4); i += blockDim.x) dst[hdr + i] = srcM[i];
+    constexpr int kMeanInertia = (int)(offsetof(DevModel, meaninertia) / 4);
+    for (int i = threadIdx.x; i < (int)(sizeof(DevModel) / 4); i += blockDim.x)
+      dst[hdr + i] = stride && i == kMeanInertia ? __float_as_int(pack[stride - 1]) : srcM[i];
     for (int i = threadIdx.x; i < (int)(sizeof(DevLayout) / 4); i += blockDim.x) dst[lay + i] = srcL[i];
   }
   __syncthreads();
@@ -224,14 +237,16 @@ __device__ __noinline__ void task_warp_loop(Ctx& c, const RolloutArgs& A, int ca
 template <class SP>
 __device__ __forceinline__ void rollout_body(const RolloutArgs& A) {
   float* smem = g_smem;
-  stage_model_pack(smem, A.pack, (unsigned)((A.M.nf + A.M.ni) * 4));
+  // (blockIdx.x is the candidate in every instance: the one-warp ones have one warp)
+  const float* pack = problem_pack(A.pack, A.pack_stride, A.pack_index, (int)blockIdx.x / A.nper);
+  stage_model_pack(smem, pack, (unsigned)((A.M.nf + A.M.ni) * 4));
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   // the CTA is ONE candidate (SP::kWide > 1: warp 0 runs the pipeline, the others help with the wide phases).  The
   // one-warp instances add their warp index, 0: with blockIdx.x alone the Humanoid Track one is compiled to 128
   // registers and spills.
   const int cand = (SP::kWide > 1 || SP::kTask > 0) ? (int)blockIdx.x : (int)blockIdx.x + warp;
   Ctx c;
-  init_ctx(c, &A.M, &A.L, smem, lane, A.pack);
+  init_ctx(c, &A.M, &A.L, smem, lane, pack, A.pack_stride);
   if (cand >= A.N) return;
   if (SP::kWide > 1 && warp > 0 && warp < SP::kWide) { wide_helper_loop<SP>(c); return; }
   if (SP::kTask > 0 && warp == SP::kWide) { task_warp_loop<SP>(c, A, cand); return; }
@@ -477,17 +492,21 @@ struct StepBatchArgs {
   const DevSensor* sensors; int nsensor, sensor_adr0, sensor_dim; float* sensordata;
   // row b's mocap poses start at mocap + b mocap_stride: 0 shares one set, 7 nmocap gives each row its own
   int mocap_stride;
+  // model variants: row b steps on variant pack_index[b / pack_rows] (problem_pack); pack_stride 0: the one pack
+  int pack_stride, pack_rows;
+  const int* pack_index;
 };
 
 template <class SP>
 __device__ __forceinline__ void step_batch_body(const StepBatchArgs& A) {
   float* smem = g_smem;
-  stage_model_pack(smem, A.pack, (unsigned)((A.M.nf + A.M.ni) * 4));
+  const int b = blockIdx.x;
+  const float* pack = problem_pack(A.pack, A.pack_stride, A.pack_index, A.pack_stride ? b / A.pack_rows : 0);
+  stage_model_pack(smem, pack, (unsigned)((A.M.nf + A.M.ni) * 4));
   Ctx c;
-  init_ctx(c, &A.M, &A.L, smem, threadIdx.x, A.pack);
+  init_ctx(c, &A.M, &A.L, smem, threadIdx.x, pack, A.pack_stride);
   auto&& M = SP::model(c);
   const int lane = c.lane, nq = M.nq, nv = M.nv, nu = M.nu, nr = M.num_residual;
-  const int b = blockIdx.x;
   if (b >= A.B) return;
   load_task<SP>(c, 0, A.task_state, nullptr, nullptr);
   load_state<SP>(c, A.qpos + (size_t)b * nq, A.qvel + (size_t)b * nv, A.ctrl + (size_t)b * nu,

@@ -70,7 +70,9 @@ EXPORTS = ["mjpc_b200_version", "mjpc_b200_last_error", "mjpc_b200_create", "mjp
            "mjpc_b200_quadruped_transition_create", "mjpc_b200_quadruped_transition_destroy",
            "mjpc_b200_quadruped_transition_step", "mjpc_b200_quadruped_transition_set", "mjpc_b200_track_transition_create",
            "mjpc_b200_track_transition_destroy", "mjpc_b200_track_transition_step", "mjpc_b200_shadow_transition_create",
-           "mjpc_b200_shadow_transition_destroy", "mjpc_b200_shadow_transition_step"]
+           "mjpc_b200_shadow_transition_destroy", "mjpc_b200_shadow_transition_step", "mjpc_b200_set_model_variants",
+           "mjpc_b200_select_model_variants", "mjpc_b200_batch_planner_set_models",
+           "mjpc_b200_batch_estimator_set_models"]
 
 
 class ModelBlob(C.Structure):
@@ -161,6 +163,24 @@ def _model_blob(model):
     blob = to_blob(model)
     buf = C.create_string_buffer(blob, len(blob))
     return buf, ModelBlob(C.cast(buf, C.c_void_p), len(blob))
+
+
+def _model_blobs(models):
+    """The blobs of a list of models as (buffers, ModelBlob array, count); (None, None, 0) for None or an empty list.
+    Keep the buffers while C reads them."""
+    if not models:
+        return None, None, 0
+    pairs = [_model_blob(m) for m in models]
+    arr = (ModelBlob * len(pairs))(*[mb for _, mb in pairs])
+    return [b for b, _ in pairs], arr, len(pairs)
+
+
+def _set_batch_models(obj, models):
+    """mjpc_b200_batch_planner_set_models on a batch planner of any kind."""
+    bufs, arr, n = _model_blobs(models)
+    rc = obj.lib.mjpc_b200_batch_planner_set_models(obj.h, arr, n)
+    if rc != 0:
+        raise EngineError(f"batch_planner_set_models failed ({rc}): {obj.lib.mjpc_b200_last_error().decode()}")
 
 
 class _CppObject:
@@ -330,6 +350,14 @@ class Engine:
         w, p, s = _d(weight), _d(parameters), _d(task_state)
         td = TaskDesc(_pd(w), _pd(p), _pd(s), float(self.m.task_risk if risk is None else risk))
         self._check(self.lib.mjpc_b200_set_task(self.h, C.byref(td)))
+
+    def set_model_variants(self, models):
+        """Problem b of the following batched launches runs on compiled model models[b] (mjpc_b200_set_model_variants):
+        bitwise what an Engine of models[b] computes.  The variants may differ from this engine's model only in its
+        physical parameters (include/mjpc_b200.h gives the rule); a launch must then hold len(models) problems, and the
+        single-problem, sharded and step calls are refused.  None or [] clears them."""
+        bufs, arr, n = _model_blobs(models)
+        self._check(self.lib.mjpc_b200_set_model_variants(self.h, arr, n))
 
     def set_options(self, timestep, integrator=0):
         """Agent::PlanIteration's planning-model overrides (agent.cc:288-289)."""
@@ -724,6 +752,11 @@ class _CppBatchPlanner(_CppObject):
         w, p, s = _d(weight), _d(parameters), _d(task_state)
         self._check(self.lib.mjpc_b200_batch_planner_set_task(self.h, int(problem), _pd(w), _pd(p), _pd(s)), "set_task")
 
+    def set_models(self, models):
+        """Problem b plans on compiled model models[b] from now on (len(models) == num_problems), on every engine
+        handle the batch owns; None or [] plans every problem on the batch's model again."""
+        _set_batch_models(self, models)
+
     def optimize_policy(self):
         """One planning iteration of every problem; returns the per-problem results."""
         self._check(self.lib.mjpc_b200_batch_planner_optimize_policy(self.h, self.horizon), "optimize_policy")
@@ -923,6 +956,10 @@ class CppBatchILQGPlanner(_CppObject):
     def set_task(self, problem, weight=None, parameters=None, task_state=None):
         w, p, s = _d(weight), _d(parameters), _d(task_state)
         self._check(self.lib.mjpc_b200_batch_ilqg_planner_set_task(self.h, int(problem), _pd(w), _pd(p), _pd(s)), "set_task")
+
+    def set_models(self, models):
+        """Problem b plans on compiled model models[b] from now on; None or [] on the batch's model again."""
+        _set_batch_models(self, models)
 
     def nominal_trajectory(self):
         return self._check(self.lib.mjpc_b200_batch_ilqg_planner_nominal_trajectory(self.h, self.H), "nominal_trajectory")

@@ -45,7 +45,7 @@ import ctypes as C
 
 import numpy as np
 
-from .engine import EngineError, _CppObject, _d, _dp, _fp, _pd, _pf
+from .engine import EngineError, _CppObject, _d, _dp, _fp, _model_blobs, _pd, _pf
 from .mjcf import JNT_BALL, JNT_FREE, SENS_MEASURED
 
 
@@ -585,6 +585,13 @@ class CppBatchEstimator(_CppObject):
     def reset(self, b, state=None, time=0.0, covariance_scale=None, process_scale=None, sensor_scale=None):
         x, cs, ps, ss = reset_values(self.m, state, covariance_scale, process_scale, sensor_scale)
         self._check(self.lib.mjpc_b200_batch_estimator_reset(self.h, b, _pd(_d(x)), time, cs, ps, ss))
+
+    def set_models(self, models):
+        """Filter b runs on compiled model models[b] from now on (len(models) == num_filters; the rule of
+        Engine.set_model_variants); None or [] runs every filter on the bank's model again.  The filters' states are
+        kept."""
+        bufs, arr, n = _model_blobs(models)
+        self._check(self.lib.mjpc_b200_batch_estimator_set_models(self.h, arr, n))
 
     def set_noise(self, b, process=None, sensor=None):
         self._check(self.lib.mjpc_b200_batch_estimator_set_noise(self.h, b, _pd(_d(process)), _pd(_d(sensor))))
