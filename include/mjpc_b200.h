@@ -282,6 +282,51 @@ int mjpc_b200_step_sensors(mjpc_b200_t* h, int B, const float* states, const flo
                            const float* mocap, double time, int sensor_start, int nsensor, float* next_states,
                            float* sensordata, float* qacc, int* counts);
 
+/* ---- Closed-loop plants: num_plants plants on an engine handle, each an mjData-like state (qpos, qvel, warm start,
+ * time) kept in device memory with its running cost sum, step count and warning count, its own mocap and task rows
+ * (weight, parameters, task state in absolute time) and, with model variants set, its own model: plant b steps on
+ * variant b, bitwise what a handle created from that variant steps.  mjpc_b200_plant_step advances every running plant
+ * by one mj_step in one launch, through the device functions and the kernel instance mjpc_b200_step_batch runs: plant
+ * b's step equals step_batch's with time0 = the plant's time, its task rows and its warm start.  The ctrl is applied
+ * as step_batch applies it.  The warm start carries from step to step (qacc_warmstart across mj_step calls).
+ *
+ * A step is committed only when the next qpos, qvel and qacc are finite: the state, the warm start (= qacc), time +=
+ * timestep (double), cost sum += the step's cost (the pre-step residual's CostValue), steps += 1, warnings += the
+ * step's warning (contact or constraint buffer full).  Otherwise the plant's status becomes MJPC_B200_PLANT_DIVERGED
+ * and nothing is committed.  Unlike MuJoCo, which would call mj_resetData, a plant is never reset silently: it is
+ * skipped by later steps until plant_reset.  A plant is MJPC_B200_PLANT_IDLE from plant_init until its first reset.
+ *
+ * Every call returns MJPC_B200_ERR_BAD_ARGUMENT for a NULL handle, a handle without plants (plant_init) or a plant
+ * index outside [0, num_plants), and leaves the bank unchanged on any refusal. */
+enum { MJPC_B200_PLANT_RUNNING = 0, MJPC_B200_PLANT_DIVERGED = 1, MJPC_B200_PLANT_IDLE = 2 };
+
+/* The handle's plants (replacing any earlier ones), every plant idle, with the handle's set_task values as task rows.
+ * nsensor = 0: no sensors; else plant_step returns the measurement sensors [sensor_start, sensor_start + nsensor) of
+ * each pre-step state (the range rules of mjpc_b200_step_sensors: BAD_ARGUMENT outside the model's sensors,
+ * UNSUPPORTED for a sensor the engine does not evaluate).  num_plants above max_candidates: MJPC_B200_ERR_CAPACITY. */
+int mjpc_b200_plant_init(mjpc_b200_t* h, int num_plants, int sensor_start, int nsensor);
+/* Start an episode of plant `plant` (mj_resetData + setting the state): qpos [nq], qvel [nv], time, mocap [7 nmocap]
+ * (required when nmocap > 0).  Warm start, cost sum, steps and warnings become 0 and the plant runs. */
+int mjpc_b200_plant_reset(mjpc_b200_t* h, int plant, const float* qpos, const float* qvel, double time,
+                          const float* mocap);
+/* What a Task::Transition writes into mjData between steps; NULL keeps the current value.  Warm start, time, sums and
+ * status are kept. */
+int mjpc_b200_plant_set(mjpc_b200_t* h, int plant, const float* qpos, const float* qvel, const float* mocap);
+/* The plant's task rows for the following steps (task state in absolute time); NULL keeps the current row. */
+int mjpc_b200_plant_set_task(mjpc_b200_t* h, int plant, const double* weight, const double* parameters,
+                             const double* task_state);
+/* One step of every running plant from ctrl [num_plants][nu].  Outputs (any may be NULL), per plant after the step:
+ * state [num_plants][nq+nv], time [num_plants], cost [num_plants] (the step's cost; 0 for a plant that did not step),
+ * sensordata [num_plants][dim] (the pre-step sensors of plant_init's range; zeros for a plant that did not step) and
+ * status [num_plants].  With model variants set, their count (or select_model_variants' B) must be num_plants
+ * (MJPC_B200_ERR_BAD_ARGUMENT otherwise).  last_kernel_ms times the launch. */
+int mjpc_b200_plant_step(mjpc_b200_t* h, const float* ctrl, float* state_out, double* time_out, float* cost_out,
+                         float* sensordata_out, int* status_out);
+/* Plant `plant`'s fields; any pointer may be NULL: state [nq+nv], warmstart [nv], time, cost_sum, steps, warnings,
+ * status. */
+int mjpc_b200_plant_get(mjpc_b200_t* h, int plant, float* state, float* warmstart, double* time, double* cost_sum,
+                        int* steps, int* warnings, int* status);
+
 /* ---- State estimators (csrc/host/estimator.h, the reference's Estimator base mjpc/estimators/estimator.h): a single
  * filter is the batched estimators' bank of one filter below, on an engine handle it owns, with the same device
  * arithmetic.  Each kind has its own create (its settings); every other call is one of the generic

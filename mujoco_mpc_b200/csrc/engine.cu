@@ -18,6 +18,7 @@
 #include "estimator_kernels.cuh"
 #include "filter_bank.h"
 #include "ilqg_kernels.cuh"
+#include "plant_bank.h"
 #include "rollout_kernels.cuh"
 
 using namespace mjpc_dev;
@@ -49,17 +50,21 @@ struct KernelSet {
   const void* fd_center;
   const void* fd_column;
   int rollout_threads;
+  const void* plant;           // one step of every closed-loop plant (plant_bank.h)
 };
 const KernelSet kGenericKernels = {(const void*)rollout_kernel, (const void*)rollout_kernel, (const void*)step_batch_kernel,
-                                   (const void*)fd_center_kernel, (const void*)fd_column_kernel, 32};
+                                   (const void*)fd_center_kernel, (const void*)fd_column_kernel, 32,
+                                   (const void*)plant_step_kernel};
 const KernelSet kQuadrupedKernels = {(const void*)rollout_kernel_quadruped, (const void*)rollout_kernel_quadruped_plain,
                                      (const void*)step_batch_kernel_quadruped, (const void*)fd_center_kernel_quadruped,
-                                     (const void*)fd_column_kernel_quadruped, kRolloutThreads};
+                                     (const void*)fd_column_kernel_quadruped, kRolloutThreads,
+                                     (const void*)plant_step_kernel_quadruped};
 // (no static fd instances: the Humanoid Track's derivative sweeps run the generic ones)
 const KernelSet kHumanoidTrackKernels = {(const void*)rollout_kernel_humanoid_track,
                                          (const void*)rollout_kernel_humanoid_track_plain,
                                          (const void*)step_batch_kernel_humanoid_track, (const void*)fd_center_kernel,
-                                         (const void*)fd_column_kernel, kRolloutThreads};
+                                         (const void*)fd_column_kernel, kRolloutThreads,
+                                         (const void*)plant_step_kernel_humanoid_track};
 }  // namespace
 
 // The device filter bank of the state estimators (filter_bank.h): one allocation carved into the filters' fields, the
@@ -108,6 +113,7 @@ struct mjpc_b200 {
   std::vector<float> dbg_contact;
   IlqgBuffers ilqg;
   FilterBank* bank = nullptr;   // the state estimators' filters (filter_bank.h), made by mjpc_b200_bank::Init
+  PlantBank* plants = nullptr;  // the closed-loop plants (plant_bank.h), made by mjpc_b200_plant_init
   // pinned staging
   float* h_in = nullptr;
   size_t h_in_floats = 0;
@@ -626,7 +632,7 @@ int mjpc_b200_create(const mjpc_model_blob* model, int max_candidates, int max_h
   for (const KernelSet* k : {h->kernels, &kGenericKernels}) {
     CREATE_TRY(raise_smem_limit(k->rollout, smem_rollout)); CREATE_TRY(raise_smem_limit(k->rollout_plain, smem_rollout));
     CREATE_TRY(raise_smem_limit(k->step, smem_step)); CREATE_TRY(raise_smem_limit(k->fd_center, smem_step));
-    CREATE_TRY(raise_smem_limit(k->fd_column, smem_step));
+    CREATE_TRY(raise_smem_limit(k->fd_column, smem_step)); CREATE_TRY(raise_smem_limit(k->plant, smem_step));
   }
   if (int rc = ilqg_init(h->ilqg, h->pack.M, (int)H)) {
     mjpc_b200_destroy(h);
@@ -650,6 +656,7 @@ void mjpc_b200_destroy(mjpc_b200_t* h) {
   for (void* p : bufs) if (p) cudaFree(p);
   ilqg_free(h->ilqg);
   delete h->bank;
+  delete h->plants;
   if (h->h_in) cudaFreeHost(h->h_in);
   if (h->h_out) cudaFreeHost(h->h_out);
   if (h->h_step) cudaFreeHost(h->h_step);
@@ -1249,6 +1256,202 @@ int mjpc_b200_step_sensors(mjpc_b200_t* h, int B, const float* states, const flo
   }
   h->last_static = kind ? 1 : 0;
   return 0;
+}
+
+// ---- closed-loop plants (plant_bank.h, plant_step_kernel in rollout_kernels.cuh)
+
+int mjpc_b200_plant_init(mjpc_b200_t* h, int num_plants, int sensor_start, int nsensor) {
+  if (!h || num_plants < 1 || nsensor < 0) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "plant_init: bad argument");
+  if (num_plants > h->maxN) return fail(MJPC_B200_ERR_CAPACITY, "plant_init: num_plants > max_candidates");
+  const int nsens = (int)h->sensors.size();
+  if (nsensor && (sensor_start < 0 || sensor_start > nsens - nsensor))
+    return fail(MJPC_B200_ERR_BAD_ARGUMENT, "plant_init: sensor range [" + std::to_string(sensor_start) + ", " +
+                                                std::to_string((long long)sensor_start + nsensor) + ") outside the model's " +
+                                                std::to_string(nsens) + " sensors");
+  for (int i = sensor_start; i < sensor_start + nsensor; i++)
+    if (!h->sensor_why[i].empty())
+      return fail(MJPC_B200_ERR_UNSUPPORTED, "plant_init: sensor " + std::to_string(i) + ": " + h->sensor_why[i]);
+  CUDA_TRY(cudaSetDevice(h->device));
+  CUDA_TRY(cudaStreamSynchronize(h->stream));   // a step in flight may still use the old bank
+  const DevModel& M = h->pack.M;
+  PlantBank* k = new PlantBank;
+  PlantArgs& a = k->a;
+  std::memset(&a, 0, sizeof(a));
+  a.B = num_plants;
+  if (nsensor) {
+    const DevSensor& last = h->sensors[sensor_start + nsensor - 1];
+    a.sensor_adr0 = h->sensors[sensor_start].adr;
+    k->nsd = last.adr - a.sensor_adr0 + sensor_dim(last.type);
+    a.sensors = h->d_sensors + sensor_start; a.nsensor = nsensor; a.sensor_dim = k->nsd;
+  }
+  const size_t B = num_plants, nq = M.nq, nv = M.nv, nu = M.nu, nm = 7 * (size_t)M.nmocap, nts = M.task_state_size,
+               nw = M.num_term, np = M.num_parameters, nsd = k->nsd;
+  size_t bytes = 0;
+  auto take = [&](size_t n) { const size_t at = bytes; bytes += (n + 255) & ~(size_t)255; return at; };
+  const size_t o_qpos = take(B * nq * 4), o_qvel = take(B * nv * 4), o_warm = take(B * nv * 4), o_time = take(B * 8),
+               o_sum = take(B * 8), o_steps = take(B * 4), o_warn = take(B * 4), o_status = take(B * 4);
+  // the upload and the outputs, each one contiguous block laid out as its pinned mirror
+  size_t in = 0, out = 0;
+  auto in_take = [&](size_t n) { const size_t at = in; in += (n + 15) & ~(size_t)15; return at; };
+  auto out_take = [&](size_t n) { const size_t at = out; out += (n + 15) & ~(size_t)15; return at; };
+  k->o_ctrl = in_take(B * nu * 4); k->o_mocap = in_take(B * nm * 4); k->o_ts = in_take(B * nts * 4);
+  k->o_weight = in_take(B * nw * 4); k->o_par = in_take(B * np * 4);
+  k->o_time = out_take(B * 8); k->o_state = out_take(B * (nq + nv) * 4); k->o_cost = out_take(B * 4);
+  k->o_status = out_take(B * 4); k->o_sens = out_take(B * nsd * 4);
+  k->in_bytes = in; k->out_bytes = out;
+  const size_t o_in = take(in), o_out = take(out);
+  auto fail_k = [&](cudaError_t e) {
+    delete k;
+    return fail(MJPC_B200_ERR_CUDA, std::string("plant_init: ") + cudaGetErrorString(e));
+  };
+  if (cudaError_t e = cudaMalloc(&k->d_mem, bytes)) return fail_k(e);
+  if (cudaError_t e = cudaMemset(k->d_mem, 0, bytes)) return fail_k(e);
+  if (cudaError_t e = cudaMallocHost((void**)&k->h_stage, in + out)) return fail_k(e);
+  std::memset(k->h_stage, 0, in + out);
+  unsigned char* base = (unsigned char*)k->d_mem;
+  a.qpos = (float*)(base + o_qpos); a.qvel = (float*)(base + o_qvel); a.warm = (float*)(base + o_warm);
+  a.time = (double*)(base + o_time); a.cost_sum = (double*)(base + o_sum);
+  a.steps = (int*)(base + o_steps); a.warnings = (int*)(base + o_warn); a.status = (int*)(base + o_status);
+  k->d_in = base + o_in; k->d_out = base + o_out;
+  a.ctrl = (const float*)(k->d_in + k->o_ctrl); a.mocap = (const float*)(k->d_in + k->o_mocap);
+  a.task_state = nts ? (const float*)(k->d_in + k->o_ts) : nullptr;
+  a.weight = nw ? (const float*)(k->d_in + k->o_weight) : nullptr;
+  a.parameters = np ? (const float*)(k->d_in + k->o_par) : nullptr;
+  a.time_out = (double*)(k->d_out + k->o_time); a.state_out = (float*)(k->d_out + k->o_state);
+  a.cost_out = (float*)(k->d_out + k->o_cost); a.status_out = (int*)(k->d_out + k->o_status);
+  a.sensordata = nsd ? (float*)(k->d_out + k->o_sens) : nullptr;
+  std::vector<int> idle(B, PLANT_IDLE);
+  if (cudaError_t e = cudaMemcpy(a.status, idle.data(), B * 4, cudaMemcpyHostToDevice)) return fail_k(e);
+  // every plant starts with the handle's task (set_task) and no mocap; plant_reset starts its episode
+  k->mocap.assign(B * nm, 0.f);
+  k->time.assign(B, 0.0);
+  for (size_t b = 0; b < B; b++) {
+    k->weight.insert(k->weight.end(), h->weight.begin(), h->weight.end());
+    k->parameters.insert(k->parameters.end(), h->parameters.begin(), h->parameters.end());
+    k->task_state.insert(k->task_state.end(), h->task_state.begin(), h->task_state.end());
+  }
+  delete h->plants;
+  h->plants = k;
+  return 0;
+}
+
+// the bank and one of its plants, or a refusal naming the call
+static int plant_check(mjpc_b200_t* h, int plant, const char* call) {
+  if (!h) return fail(MJPC_B200_ERR_BAD_ARGUMENT, std::string(call) + ": null handle");
+  if (!h->plants) return fail(MJPC_B200_ERR_BAD_ARGUMENT, std::string(call) + ": no plants (plant_init)");
+  if (plant < 0 || plant >= h->plants->a.B)
+    return fail(MJPC_B200_ERR_BAD_ARGUMENT, std::string(call) + ": plant " + std::to_string(plant) + " outside [0, " +
+                                                std::to_string(h->plants->a.B) + ")");
+  return 0;
+}
+
+// one plant's device fields from (write = 1) or to (write = 0) the host; NULL pointers are skipped
+static int plant_fields(mjpc_b200_t* h, int b, int write, void* qpos, void* qvel, void* warm, void* time, void* cost_sum,
+                        void* steps, void* warnings, void* status) {
+  const PlantArgs& a = h->plants->a;
+  const size_t nq = h->pack.M.nq, nv = h->pack.M.nv;
+  CUDA_TRY(cudaSetDevice(h->device));
+  CUDA_TRY(cudaStreamSynchronize(h->stream));
+  const struct { void* host; void* dev; size_t n; } f[] = {
+      {qpos, a.qpos + b * nq, nq * 4}, {qvel, a.qvel + b * nv, nv * 4}, {warm, a.warm + b * nv, nv * 4},
+      {time, a.time + b, 8}, {cost_sum, a.cost_sum + b, 8}, {steps, a.steps + b, 4}, {warnings, a.warnings + b, 4},
+      {status, a.status + b, 4}};
+  for (const auto& x : f)
+    if (x.host && x.n)
+      CUDA_TRY(write ? cudaMemcpy(x.dev, x.host, x.n, cudaMemcpyHostToDevice) : cudaMemcpy(x.host, x.dev, x.n, cudaMemcpyDeviceToHost));
+  return 0;
+}
+
+int mjpc_b200_plant_reset(mjpc_b200_t* h, int plant, const float* qpos, const float* qvel, double time, const float* mocap) {
+  if (int rc = plant_check(h, plant, "plant_reset")) return rc;
+  const DevModel& M = h->pack.M;
+  if (!qpos || !qvel || (M.nmocap && !mocap)) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "plant_reset: bad argument");
+  std::vector<float> warm(M.nv, 0.f);
+  double zero = 0.0;
+  int izero = 0, running = PLANT_RUNNING;
+  if (int rc = plant_fields(h, plant, 1, (void*)qpos, (void*)qvel, warm.data(), &time, &zero, &izero, &izero, &running))
+    return rc;
+  PlantBank& k = *h->plants;
+  const size_t nm = 7 * (size_t)M.nmocap;
+  if (nm) std::copy(mocap, mocap + nm, k.mocap.begin() + plant * nm);
+  k.time[plant] = time;
+  return 0;
+}
+
+int mjpc_b200_plant_set(mjpc_b200_t* h, int plant, const float* qpos, const float* qvel, const float* mocap) {
+  if (int rc = plant_check(h, plant, "plant_set")) return rc;
+  if (int rc = plant_fields(h, plant, 1, (void*)qpos, (void*)qvel, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr))
+    return rc;
+  const size_t nm = 7 * (size_t)h->pack.M.nmocap;
+  if (mocap && nm) std::copy(mocap, mocap + nm, h->plants->mocap.begin() + plant * nm);
+  return 0;
+}
+
+int mjpc_b200_plant_set_task(mjpc_b200_t* h, int plant, const double* weight, const double* parameters,
+                             const double* task_state) {
+  if (int rc = plant_check(h, plant, "plant_set_task")) return rc;
+  const DevModel& M = h->pack.M;
+  PlantBank& k = *h->plants;
+  const size_t nw = M.num_term, np = M.num_parameters, nts = M.task_state_size;
+  if (weight) std::copy(weight, weight + nw, k.weight.begin() + plant * nw);
+  if (parameters) std::copy(parameters, parameters + np, k.parameters.begin() + plant * np);
+  if (task_state) std::copy(task_state, task_state + nts, k.task_state.begin() + plant * nts);
+  return 0;
+}
+
+// One step of every plant: ONE upload from the pinned staging (ctrl, mocap, the task rows with the task state rebased
+// to each plant's time), ONE plant_step_kernel launch on the handle's instance, ONE download of the outputs.
+int mjpc_b200_plant_step(mjpc_b200_t* h, const float* ctrl, float* state_out, double* time_out, float* cost_out,
+                         float* sensordata_out, int* status_out) {
+  if (!h) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "plant_step: null handle");
+  if (!h->plants) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "plant_step: no plants (plant_init)");
+  const DevModel& M = h->pack.M;
+  if (!ctrl && M.nu) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "plant_step: ctrl required");
+  PlantBank& k = *h->plants;
+  PlantArgs a = k.a;
+  if (int rc = check_variants(h, a.B, "plant step")) return rc;
+  const size_t B = a.B, nu = M.nu, nm = 7 * (size_t)M.nmocap, nts = M.task_state_size, nw = M.num_term,
+               np = M.num_parameters, ds = M.nq + M.nv;
+  CUDA_TRY(cudaSetDevice(h->device));
+  CUDA_TRY(cudaStreamSynchronize(h->stream));   // the staging may still feed an earlier copy
+  unsigned char* in = k.h_stage;
+  if (nu) std::memcpy(in + k.o_ctrl, ctrl, B * nu * 4);
+  if (nm) std::memcpy(in + k.o_mocap, k.mocap.data(), B * nm * 4);
+  for (size_t b = 0; b < B; b++) {
+    rebase_task_state(h, k.task_state.data() + b * nts, k.time[b], (float*)(in + k.o_ts) + b * nts);
+    for (size_t i = 0; i < nw; i++) ((float*)(in + k.o_weight))[b * nw + i] = (float)k.weight[b * nw + i];
+    for (size_t i = 0; i < np; i++) ((float*)(in + k.o_par))[b * np + i] = (float)k.parameters[b * np + i];
+  }
+  CUDA_TRY(cudaMemcpyAsync(k.d_in, in, k.in_bytes, cudaMemcpyHostToDevice, h->stream));
+  const KernelSet* ks;
+  const int kind = pick_kernels(h, &ks);
+  a.M = M; a.L = make_layout(M, 1);
+  a.pack = launch_pack(h); a.pack_stride = launch_stride(h); a.pack_index = h->d_variant_index;
+  a.timestep = h->pack.timestep;
+  CUDA_TRY(cudaEventRecord(h->ev0, h->stream));
+  launch_kernel(ks->plant, a.B, 32, h->smem_bytes(1), h->stream, a);
+  CUDA_TRY(cudaEventRecord(h->ev1, h->stream));
+  CUDA_TRY(cudaGetLastError());
+  h->launches += 1;
+  unsigned char* out = k.h_stage + k.in_bytes;
+  CUDA_TRY(cudaMemcpyAsync(out, k.d_out, k.out_bytes, cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(cudaStreamSynchronize(h->stream));
+  if (cudaEventElapsedTime(&h->last_ms, h->ev0, h->ev1) != cudaSuccess) cudaGetLastError();
+  std::memcpy(k.time.data(), out + k.o_time, B * 8);
+  if (time_out) std::memcpy(time_out, out + k.o_time, B * 8);
+  if (state_out) std::memcpy(state_out, out + k.o_state, B * ds * 4);
+  if (cost_out) std::memcpy(cost_out, out + k.o_cost, B * 4);
+  if (status_out) std::memcpy(status_out, out + k.o_status, B * 4);
+  if (sensordata_out && k.nsd) std::memcpy(sensordata_out, out + k.o_sens, B * k.nsd * 4);
+  h->last_static = kind ? 1 : 0;
+  return 0;
+}
+
+int mjpc_b200_plant_get(mjpc_b200_t* h, int plant, float* state, float* warmstart, double* time, double* cost_sum,
+                        int* steps, int* warnings, int* status) {
+  if (int rc = plant_check(h, plant, "plant_get")) return rc;
+  const size_t nq = h->pack.M.nq;
+  return plant_fields(h, plant, 0, state, state ? state + nq : nullptr, warmstart, time, cost_sum, steps, warnings, status);
 }
 
 int mjpc_b200_fetch_stats(mjpc_b200_t* h, int64_t* stats) {

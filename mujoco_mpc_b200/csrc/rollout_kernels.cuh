@@ -5,6 +5,7 @@
 //                       mjpc/trajectory.cc:92-309) incl. policy, mj_step restatement, residual, cost, return
 //   rank_kernel         order of each problem's candidates by return (partial_sort, sampling/planner.cc:184-188)
 //   step_batch_kernel   independent single forward+Euler steps through the same device functions (parity hooks)
+//   plant_step_kernel   one step of every closed-loop plant, its state kept in device memory (plant_bank.h)
 //   fd_*_kernel         finite-difference transition/residual Jacobians (model_derivatives.cc:45-165)
 //
 // Shared memory per CTA: [model pack (floats | ints)] [header copies] [the candidate's data]
@@ -551,6 +552,103 @@ extern "C" __global__ void __launch_bounds__(32) step_batch_kernel_quadruped(con
 }
 extern "C" __global__ void __launch_bounds__(32) step_batch_kernel_humanoid_track(const __grid_constant__ StepBatchArgs A) {
   step_batch_body<StaticSpec<SpecHumanoidTrack>>(A);
+}
+
+// Closed-loop plants (plant_bank.h): B plants whose state stays in device memory, each advanced by ONE mj_step per
+// launch through the device functions and the order of step_batch_body, on its own model variant and task rows.  The
+// step of a running plant whose next qpos, qvel and qacc are finite is committed in place (state, warm start carried
+// as MuJoCo's qacc_warmstart, time, cost sum, step and warning counts); otherwise the plant becomes PLANT_DIVERGED and
+// keeps what it had.  A plant that is not running is not stepped.  The outputs of a plant that did not step hold its
+// state and time, cost 0 and zero sensors.
+enum PlantStatus { PLANT_RUNNING = 0, PLANT_DIVERGED = 1, PLANT_IDLE = 2 };
+
+struct PlantArgs {
+  DevModel M;
+  DevLayout L;
+  const float* pack;
+  int pack_stride;          // model variants: plant b stages its variant block (problem_pack); 0: the one pack
+  const int* pack_index;
+  int B;
+  double timestep;
+  // the bank, read and committed in place
+  float* qpos; float* qvel; float* warm;   // [B][nq|nv|nv]
+  double* time; double* cost_sum;          // [B]
+  int* steps; int* warnings; int* status;  // [B]
+  // this step's upload: ctrl [B][nu], mocap [B][7 nmocap], and the task rows with the task state rebased to each plant's
+  // time: task_state [B][size] (nullptr when empty), weight [B][num_term], parameters [B][num_parameters] (nullptr: none)
+  const float* ctrl; const float* mocap; const float* task_state; const float* weight; const float* parameters;
+  // this step's outputs: state [B][nq+nv], time [B], cost [B] (the pre-step residual's), status [B]
+  float* state_out; double* time_out; float* cost_out; int* status_out;
+  // optional (sensordata NULL: not evaluated): sensors [0, nsensor) of the pre-step state, [B][sensor_dim]
+  const DevSensor* sensors; int nsensor, sensor_adr0, sensor_dim; float* sensordata;
+};
+
+template <class SP>
+__device__ __forceinline__ void plant_body(const PlantArgs& A) {
+  float* smem = g_smem;
+  const int b = blockIdx.x;
+  if (b >= A.B) return;
+  const bool running = A.status[b] == PLANT_RUNNING;
+  bool stepped = false;
+  float cost = 0.f;
+  Ctx c;
+  if (running) {
+    // (a state set or reset to non-finite values diverges before it is stepped)
+    const float* pack = problem_pack(A.pack, A.pack_stride, A.pack_index, b);
+    stage_model_pack(smem, pack, (unsigned)((A.M.nf + A.M.ni) * 4));
+    init_ctx(c, &A.M, &A.L, smem, threadIdx.x, pack, A.pack_stride);
+    auto&& M = SP::model(c);
+    const int lane = c.lane, nq = M.nq, nv = M.nv;
+    load_task<SP>(c, b, A.task_state, A.weight, A.parameters);
+    load_state<SP>(c, A.qpos + (size_t)b * nq, A.qvel + (size_t)b * nv, A.ctrl + (size_t)b * M.nu,
+                   A.warm + (size_t)b * nv, A.mocap + (size_t)b * 7 * M.nmocap);
+    for (int i = lane; i < 6 * M.nbody; i += 32) DF(xfrc)[i] = 0;
+    __syncwarp();   // c.time stays 0: the task state was rebased to the plant's time
+    if (!(k_bad(c, DF(qpos), nq) || k_bad(c, DF(qvel), nv))) {
+      // step_batch_body's sequence (written out again: through one shared function the step_batch instances compile
+      // to different SASS)
+      k_forward<SP>(c);
+      k_residual<SP>(c);
+      if (k_bad(c, DF(qacc), nv)) c.warn = 1;
+      cost = k_cost_value<SP>(c);
+      if (A.sensordata) k_sensors<SP>(c, A.sensors, A.nsensor, A.sensor_adr0, A.sensordata + (size_t)b * A.sensor_dim);
+      for (int i = lane; i < nv; i += 32) DF(qacc_warmstart)[i] = DF(qacc)[i];
+      k_euler<SP>(c);
+      stepped = !(k_bad(c, DF(qpos), nq) || k_bad(c, DF(qvel), nv) || k_bad(c, DF(qacc), nv));
+    }
+    if (stepped) {
+      for (int i = lane; i < nq; i += 32) A.qpos[(size_t)b * nq + i] = DF(qpos)[i];
+      for (int i = lane; i < nv; i += 32) { A.qvel[(size_t)b * nv + i] = DF(qvel)[i]; A.warm[(size_t)b * nv + i] = DF(qacc)[i]; }
+      if (lane == 0) {
+        A.time[b] += A.timestep;
+        A.cost_sum[b] += (double)cost;
+        A.steps[b] += 1;
+        A.warnings[b] += c.warn;
+      }
+    } else if (lane == 0) {
+      A.status[b] = PLANT_DIVERGED;
+    }
+    __syncwarp();
+  }
+  const int lane = threadIdx.x, nq = A.M.nq, ds = nq + A.M.nv;
+  for (int i = lane; i < ds; i += 32)
+    A.state_out[(size_t)b * ds + i] = i < nq ? A.qpos[(size_t)b * nq + i] : A.qvel[(size_t)b * A.M.nv + i - nq];
+  if (A.sensordata && !stepped)
+    for (int i = lane; i < A.sensor_dim; i += 32) A.sensordata[(size_t)b * A.sensor_dim + i] = 0.f;
+  if (lane == 0) {
+    A.time_out[b] = A.time[b];
+    A.cost_out[b] = stepped ? cost : 0.f;
+    A.status_out[b] = A.status[b];
+  }
+}
+extern "C" __global__ void __launch_bounds__(32) plant_step_kernel(const __grid_constant__ PlantArgs A) {
+  plant_body<DynSpec>(A);
+}
+extern "C" __global__ void __launch_bounds__(32) plant_step_kernel_quadruped(const __grid_constant__ PlantArgs A) {
+  plant_body<StaticSpec<SpecQuadruped>>(A);
+}
+extern "C" __global__ void __launch_bounds__(32) plant_step_kernel_humanoid_track(const __grid_constant__ PlantArgs A) {
+  plant_body<StaticSpec<SpecHumanoidTrack>>(A);
 }
 
 }  // namespace mjpc_dev

@@ -72,7 +72,8 @@ EXPORTS = ["mjpc_b200_version", "mjpc_b200_last_error", "mjpc_b200_create", "mjp
            "mjpc_b200_track_transition_destroy", "mjpc_b200_track_transition_step", "mjpc_b200_shadow_transition_create",
            "mjpc_b200_shadow_transition_destroy", "mjpc_b200_shadow_transition_step", "mjpc_b200_set_model_variants",
            "mjpc_b200_select_model_variants", "mjpc_b200_batch_planner_set_models",
-           "mjpc_b200_batch_estimator_set_models"]
+           "mjpc_b200_batch_estimator_set_models", "mjpc_b200_plant_init", "mjpc_b200_plant_reset",
+           "mjpc_b200_plant_set", "mjpc_b200_plant_set_task", "mjpc_b200_plant_step", "mjpc_b200_plant_get"]
 
 
 class ModelBlob(C.Structure):
@@ -691,6 +692,110 @@ class Engine:
         return int(self.lib.mjpc_b200_last_kernel_static(self.h))
 
 
+PLANT_RUNNING, PLANT_DIVERGED, PLANT_IDLE = 0, 1, 2   # MJPC_B200_PLANT_*
+
+
+class CppPlantBank:
+    """num_plants closed-loop plants whose state stays in device memory (mjpc_b200_plant_*): step() advances every
+    running plant by one mj_step in one launch, each on its own model once set_models gave it one.  A plant is idle
+    until reset(); a plant whose step would leave a non-finite state becomes PLANT_DIVERGED, keeps its last state and
+    is skipped until reset() (MuJoCo would reset it silently).  sensor_start / nsensor (0: none) choose the measurement
+    sensors step() returns for each pre-step state."""
+
+    def __init__(self, model, num_plants, sensor_start=None, nsensor=0, device=0):
+        self.lib = load_library()
+        self.m = model
+        self.num_plants = int(num_plants)
+        self.nsensor = int(nsensor)
+        self.sensor_start = 0 if sensor_start is None else int(sensor_start)
+        self.nsensordata = sensor_dim(model, self.sensor_start, self.nsensor) if self.nsensor else 0
+        self._buf, mb = _model_blob(model)
+        h = C.c_void_p()
+        rc = self.lib.mjpc_b200_create(C.byref(mb), self.num_plants, 1, int(device), C.byref(h))
+        if rc != 0:
+            raise EngineError(f"mjpc_b200_create failed ({rc}): {self.lib.mjpc_b200_last_error().decode()}")
+        self.h = h
+        self.lib.mjpc_b200_plant_reset.argtypes = [C.c_void_p, C.c_int, _fp, _fp, C.c_double, _fp]
+        self._check(self.lib.mjpc_b200_plant_init(self.h, self.num_plants, self.sensor_start, self.nsensor))
+        # each plant's mocap poses as the bank holds them (float), for the planner's set_state
+        self.mocap = np.zeros((self.num_plants, 7 * model.nmocap), np.float32)
+
+    def close(self):
+        if getattr(self, "h", None):
+            self.lib.mjpc_b200_destroy(self.h)
+            self.h = None
+
+    __del__ = close
+
+    def _check(self, rc):
+        if rc != 0:
+            raise EngineError(f"mjpc_b200 plant error {rc}: {self.lib.mjpc_b200_last_error().decode()}")
+
+    def reset(self, plant, qpos, qvel, time=0.0, mocap=None):
+        """Start an episode: the state and time given, warm start, cost sum and counts 0, running.  mocap None: the
+        model's mocap poses."""
+        q, v = _f(qpos), _f(qvel)
+        mc = _f(self._mocap0() if mocap is None else mocap)
+        self._check(self.lib.mjpc_b200_plant_reset(self.h, int(plant), _pf(q), _pf(v), float(time), _pf(mc)))
+        if mc is not None:
+            self.mocap[plant] = mc
+
+    def _mocap0(self):
+        m = self.m
+        if not m.nmocap:
+            return None
+        return np.concatenate([np.asarray(m.mocap_pos0, float).reshape(-1, 3),
+                               np.asarray(m.mocap_quat0, float).reshape(-1, 4)], 1).reshape(-1)
+
+    def set(self, plant, qpos=None, qvel=None, mocap=None):
+        """What a Task::Transition writes between steps; None keeps the current value."""
+        q, v, mc = _f(qpos), _f(qvel), _f(mocap)
+        self._check(self.lib.mjpc_b200_plant_set(self.h, int(plant), _pf(q), _pf(v), _pf(mc)))
+        if mc is not None:
+            self.mocap[plant] = mc
+
+    def set_task(self, plant, weight=None, parameters=None, task_state=None):
+        """The plant's task rows for the following steps (task state in absolute time); None keeps the current row."""
+        w, p, s = _d(weight), _d(parameters), _d(task_state)
+        self._check(self.lib.mjpc_b200_plant_set_task(self.h, int(plant), _pd(w), _pd(p), _pd(s)))
+
+    def set_models(self, models):
+        """Plant b steps on compiled model models[b] from now on (len(models) == num_plants; the rule of
+        Engine.set_model_variants); None or [] steps every plant on the bank's model again.  The plants are kept."""
+        bufs, arr, n = _model_blobs(models)
+        self._check(self.lib.mjpc_b200_set_model_variants(self.h, arr, n))
+
+    def step(self, ctrl):
+        """One step of every running plant from ctrl [num_plants][nu]: dict(state [B][nq+nv], time [B], cost [B] (the
+        pre-step residual's cost; 0 where the plant did not step), sensordata [B][dim], status [B])."""
+        B, m = self.num_plants, self.m
+        u = np.ascontiguousarray(np.asarray(ctrl, np.float32).reshape(B, m.nu))
+        o = dict(state=np.zeros((B, m.nq + m.nv), np.float32), time=np.zeros(B), cost=np.zeros(B, np.float32),
+                 sensordata=np.zeros((B, self.nsensordata), np.float32), status=np.zeros(B, np.int32))
+        self._check(self.lib.mjpc_b200_plant_step(self.h, _pf(u), _pf(o["state"]), _pd(o["time"]), _pf(o["cost"]),
+                                                  _pf(o["sensordata"]) if self.nsensordata else None,
+                                                  o["status"].ctypes.data_as(_ip)))
+        return o
+
+    def get(self, plant):
+        """dict(state, warmstart, time, cost_sum, steps, warnings, status) of one plant."""
+        m = self.m
+        x, w = np.zeros(m.nq + m.nv, np.float32), np.zeros(m.nv, np.float32)
+        t, cs = C.c_double(), C.c_double()
+        st, wn, ss = C.c_int(), C.c_int(), C.c_int()
+        self._check(self.lib.mjpc_b200_plant_get(self.h, int(plant), _pf(x), _pf(w), C.byref(t), C.byref(cs),
+                                                 C.byref(st), C.byref(wn), C.byref(ss)))
+        return dict(state=x, warmstart=w, time=t.value, cost_sum=cs.value, steps=st.value, warnings=wn.value,
+                    status=ss.value)
+
+    def last_kernel_ms(self):
+        """Device time of the last step's launch (CUDA events)."""
+        return float(self.lib.mjpc_b200_last_kernel_ms(self.h))
+
+    def last_kernel_static(self):
+        return int(self.lib.mjpc_b200_last_kernel_static(self.h))
+
+
 class CppSamplingPlanner(_CppPlanner):
     """The C++ host planner (csrc/host/sampling_planner.cc) through its C wrappers."""
 
@@ -931,6 +1036,7 @@ class CppILQGPlanner(_CppFeedbackPlanner):
 class CppBatchILQGPlanner(_CppObject):
     """The batched C++ iLQG planner (csrc/host/batch_ilqg_planner.cc): B problems, one launch per sweep.  Mirrors
     CppILQGPlanner with a problem argument."""
+    action_reads_state = True   # the feedback policy: action_from_policy(problem, time, state)
 
     def __init__(self, model, num_problems, horizon, num_rollouts=10, representation=1, fd_tolerance=3e-4, device=0,
                  fd_mode=1, derivative_skip=0):
@@ -1079,6 +1185,7 @@ class CppBatchILQSPlanner(_CppBatchCodePlanner):
     launch of the iLQG nominals that need converting, one sampling launch of B x num_trajectory, and one batched iLQG
     iteration of the problems sampling did not settle.  Mirrors CppILQSPlanner with a problem argument;
     optimize_policy returns each problem's 1/0."""
+    action_reads_state = True   # the iLQG half's feedback policy: action_from_policy(problem, time, state)
     _NRESULT = 1
 
     def __init__(self, model, num_problems, horizon, num_trajectory=8, num_rollouts=6, fd_tolerance=3e-4, seeds=None,
