@@ -524,64 +524,6 @@ int mjpc_b200_sampling_planner_set_exploration(mjpc_b200_planner_t* p, double ex
 int mjpc_b200_sampling_planner_get_result(mjpc_b200_planner_t* p, int* winner, double* improvement, float* returns,
                                           double* knots, double* knot_times);
 
-/* ---- Batched Predictive Sampling (csrc/host/batch_sampling_planner.{h,cc}): num_problems independent SamplingPlanners
- * (each with its own seed, state, mocap, task snapshot and policy) on ONE engine handle; optimize_policy makes one
- * mjpc_b200_rollout_spline_batched launch for all of them, and each problem's result equals that of a SamplingPlanner
- * with the same seed and inputs.  seeds [num_problems].  The task snapshot of every problem starts as the model's
- * (weight, parameters, task state); set_task replaces its non-NULL members.  Calls that take a problem index return
- * MJPC_B200_ERR_BAD_ARGUMENT when it is outside [0, num_problems). */
-int mjpc_b200_batch_planner_create(const mjpc_model_blob* model, int num_problems, int num_trajectory, int num_spline_points,
-                                   int interpolation, double exploration, double timestep, const double* ctrlrange,
-                                   const uint32_t* seeds, int max_horizon, int device, void** out);
-void mjpc_b200_batch_planner_destroy(void* planner);
-int mjpc_b200_batch_planner_reset(void* planner, int problem, int horizon, const double* initial_repeated_action);
-int mjpc_b200_batch_planner_set_state(void* planner, int problem, const double* state, double time, const double* mocap);
-int mjpc_b200_batch_planner_set_task(void* planner, int problem, const double* weight, const double* parameters,
-                                     const double* task_state);
-int mjpc_b200_batch_planner_optimize_policy(void* planner, int horizon);   /* every problem: SamplingPlanner::OptimizePolicy */
-/* Problem b plans on models[b] from now on: mjpc_b200_set_model_variants, with its rule and refusals, on every engine
- * handle the batch owns (the Robust batch's noisy handle and the iLQS batch's iLQG handle too).  count must be
- * num_problems, or 0 to plan every problem on the batch's model again.  Any batch kind, the iLQG batch included; valid
- * between planning iterations (after an online system identification, for example).  The planners' settings and
- * ctrlrange stay the batch's: variants must share actuator_ctrlrange. */
-int mjpc_b200_batch_planner_set_models(void* planner, const mjpc_model_blob* models, int count);
-int mjpc_b200_batch_planner_action_from_policy(void* planner, int problem, double* action, double time, int use_previous);
-/* as mjpc_b200_sampling_planner_get_result for one problem (returns [num_trajectory]); returns the number of installed
- * knots.  A batch of another kind: MJPC_B200_ERR_BAD_ARGUMENT */
-int mjpc_b200_batch_planner_get_result(void* planner, int problem, int* winner, double* improvement, float* returns,
-                                       double* knots, double* knot_times);
-
-/* ---- Batched Cross-Entropy, Sample Gradient and Robust planners (csrc/host/batch_planner.{h,cc}): num_problems
- * independent planners of one kind on ONE engine handle, with the arguments of the single planner's create plus
- * num_problems and seeds [num_problems]; each problem's result equals that of the single planner with the same seed and
- * inputs.  One rollout launch per iteration covers every problem's candidates (Cross-Entropy B x (N + 1), Sample
- * Gradient B x N); the Robust planner makes a clean launch of B x N, then one noisy launch of
- * B x ncandidates x nrepetitions on a second handle, each problem drawing its force noise with its own key
- * seed + iteration (mjpc_b200_set_xfrc_noise_batched).  Settings are common to a batch.  reset / set_state / set_task /
- * optimize_policy / action_from_policy / destroy are the mjpc_b200_batch_planner_* calls above; each _get_result reads
- * one problem as the single planner's _get_result does, and returns MJPC_B200_ERR_BAD_ARGUMENT for a batch of another
- * kind or a problem outside [0, num_problems). */
-int mjpc_b200_batch_ce_planner_create(const mjpc_model_blob* model, int num_problems, int num_trajectory, int n_elite,
-                                      int num_spline_points, int interpolation, double std_initial, double std_min,
-                                      double explore_fraction, double timestep, const double* ctrlrange,
-                                      const uint32_t* seeds, int max_horizon, int device, void** out);
-int mjpc_b200_batch_ce_planner_get_result(void* planner, int problem, double* improvement, float* returns, int* order,
-                                          double* knots, double* knot_times, double* variance);
-int mjpc_b200_batch_sg_planner_create(const mjpc_model_blob* model, int num_problems, int num_trajectory,
-                                      int num_gradient, int num_spline_points, int interpolation, double exploration,
-                                      double gradient_filter, double timestep, const double* ctrlrange,
-                                      const uint32_t* seeds, int max_horizon, int device, void** out);
-int mjpc_b200_batch_sg_planner_get_result(void* planner, int problem, int* winner, int* winner_type, double* improvement,
-                                          float* returns, int* order, double* knots, double* knot_times,
-                                          double* gradient_knots, double* gradient);
-int mjpc_b200_batch_robust_planner_create(const mjpc_model_blob* model, int num_problems, int num_trajectory,
-                                          int num_spline_points, int interpolation, double exploration, double timestep,
-                                          const double* ctrlrange, const uint32_t* seeds, int ncandidates,
-                                          int nrepetitions, double xfrc_std, double xfrc_rate, int max_horizon,
-                                          int device, void** out);
-int mjpc_b200_batch_robust_planner_get_result(void* planner, int problem, int* winner, double* scores, float* returns,
-                                              double* knots, double* knot_times);
-
 /* ---- Cross-Entropy planner (csrc/host/cross_entropy_planner.{h,cc}; mjpc/planners/cross_entropy/planner.h:35-146).
  * One rollout launch covers the N noisy candidates and the un-noised nominal (candidate N); the elite mean and
  * variance are host arithmetic in double, as in the reference (planner.cc:201-262).  n_elite <= 0 selects the
@@ -667,29 +609,6 @@ int mjpc_b200_host_ilqg_policy_action(const mjpc_model_blob* model, const float*
 int mjpc_b200_ilqg_planner_get_result(mjpc_b200_planner_t* p, double* scalars, float* states, float* actions,
                                       double* times);
 
-/* ---- Batched iLQG (csrc/host/batch_ilqg_planner.{h,cc}): num_problems independent iLQGPlanners (each with its own
- * state, mocap, task snapshot, policy and regularisation) on ONE engine handle.  optimize_policy makes one batched
- * launch per sweep for all problems - backward passes are retried in batches of the problems still failing - and each
- * problem's result equals that of an iLQGPlanner with the same inputs.  The task snapshot of every problem starts as
- * the model's; set_task replaces its non-NULL members.  Settings (set_fd) are shared.  Calls that take a problem index
- * return MJPC_B200_ERR_BAD_ARGUMENT when it is outside [0, num_problems). */
-int mjpc_b200_batch_ilqg_planner_create(const mjpc_model_blob* model, int num_problems, int num_rollouts, int representation,
-                                        double fd_tolerance, int max_horizon, int device, void** out);
-void mjpc_b200_batch_ilqg_planner_destroy(void* planner);
-void mjpc_b200_batch_ilqg_planner_set_fd(void* planner, double tolerance, int mode, int derivative_skip);
-int mjpc_b200_batch_ilqg_planner_reset(void* planner, int problem, int horizon, const double* initial_repeated_action);
-int mjpc_b200_batch_ilqg_planner_set_state(void* planner, int problem, const double* state, double time, const double* mocap);
-int mjpc_b200_batch_ilqg_planner_set_task(void* planner, int problem, const double* weight, const double* parameters,
-                                          const double* task_state);
-int mjpc_b200_batch_ilqg_planner_nominal_trajectory(void* planner, int horizon);   /* every problem, one launch */
-/* every problem: iLQGPlanner::OptimizePolicy; updated [num_problems] (may be NULL) receives each problem's 1/0 */
-int mjpc_b200_batch_ilqg_planner_optimize_policy(void* planner, int horizon, int* updated);
-int mjpc_b200_batch_ilqg_planner_action_from_policy(void* planner, int problem, double* action, const double* state,
-                                                    double time);
-/* as mjpc_b200_ilqg_planner_get_result for one problem; returns H */
-int mjpc_b200_batch_ilqg_planner_get_result(void* planner, int problem, double* scalars, float* states, float* actions,
-                                            double* times);
-
 /* ---- Gradient planner (csrc/host/gradient_planner.{h,cc}; mjpc/planners/gradient/planner.cc:159-383, gradient.cc:44-107,
  * spline_mapping.cc): ResamplePolicy, nominal rollout, {model derivatives, cost derivatives, gradient sweep, total derivative
  * through the spline mapping, K line-search rollouts (ONE mjpc_b200_rollout_spline launch)} x max_rollout.
@@ -708,49 +627,6 @@ void mjpc_b200_host_spline_mapping(int representation, const double* input_times
 void mjpc_b200_host_gradient_sweep(const float* A, const float* B, const float* cx, const float* cu, int n, int m, int T,
                                    double* k, double* dV0);
 
-/* ---- Batched Gradient planner (csrc/host/batch_planner.{h,cc}): num_problems independent GradientPlanners on ONE
- * engine handle of num_problems x num_trajectory candidates, with the single planner's create arguments plus
- * num_problems.  Per max_rollout iteration: one spline launch of the B resampled nominals, one
- * mjpc_b200_gradient_batched on their trajectories (each problem with its own mocap and task snapshot), one spline
- * launch of the B x num_trajectory line-search candidates.  Each problem's result equals that of a GradientPlanner with
- * the same inputs.  reset / set_state / set_task / optimize_policy / action_from_policy / destroy are the generic
- * mjpc_b200_batch_planner_* calls; settings (set_fd) are common to the batch. */
-int mjpc_b200_batch_gradient_planner_create(const mjpc_model_blob* model, int num_problems, int num_trajectory,
-                                            int num_spline_points, int representation, double fd_tolerance,
-                                            double timestep, const double* ctrlrange, int max_horizon, int device,
-                                            void** out);
-/* as mjpc_b200_gradient_planner_get_result for one problem; *improved (may be NULL) = what the single planner's
- * optimize_policy returned on the last iteration (1 improved, 0 not; 0 after an error).  Returns P; a batch of another kind or a problem
- * outside [0, num_problems): MJPC_B200_ERR_BAD_ARGUMENT */
-int mjpc_b200_batch_gradient_planner_get_result(void* planner, int problem, double* scalars, double* parameters,
-                                                double* times, int* improved);
-/* the finite-difference settings of a Gradient or iLQS batch (every problem), as mjpc_b200_planner_set_fd: tolerance
- * <= 0, mode < 0 and derivative_skip < 0 keep the current value.  Other kinds: MJPC_B200_ERR_UNSUPPORTED */
-int mjpc_b200_batch_planner_set_fd(void* planner, double tolerance, int mode, int derivative_skip);
-
-/* ---- Batched iLQS planner (csrc/host/batch_planner.{h,cc}): num_problems independent iLQSPlanners, with the single
- * planner's create arguments plus num_problems and seeds [num_problems], on two handles as the single planner has:
- * sampling (num_problems x num_trajectory) and iLQG (num_problems x ilqg_num_rollouts).  Per iteration at most: one
- * feedback launch of the iLQG nominals of the problems whose active policy was iLQG, one spline launch of every
- * problem's sampling, then for the problems sampling did not settle one batched derivative sweep, one batched
- * cost-derivative call, backward-pass rounds of the problems still failing and one action-rollout launch.  Each
- * problem's result equals that of an iLQSPlanner with the same seed and inputs.  Exploration and the finite-difference
- * and iLQG settings are common to the batch.  reset / set_state / set_task / optimize_policy / destroy and set_fd are
- * the generic mjpc_b200_batch_planner_* calls; the generic action_from_policy evaluates the policy without a state. */
-int mjpc_b200_batch_ilqs_planner_create(const mjpc_model_blob* model, int num_problems, int num_trajectory,
-                                        int num_spline_points, int interpolation, double exploration, double timestep,
-                                        const double* ctrlrange, const uint32_t* seeds, int ilqg_num_rollouts,
-                                        int ilqg_representation, double fd_tolerance, int max_horizon, int device,
-                                        void** out);
-/* scalars[4] as mjpc_b200_ilqs_planner_get_result for one problem; *improved (may be NULL) = what the single planner's
- * optimize_policy returned on the last iteration (1 / 0; 0 after an error).  Returns the active policy.  A batch of
- * another kind or a problem outside [0, num_problems): MJPC_B200_ERR_BAD_ARGUMENT */
-int mjpc_b200_batch_ilqs_planner_get_result(void* planner, int problem, double* scalars, int* improved);
-int mjpc_b200_batch_ilqs_planner_set_exploration(void* planner, double exploration);   /* every problem */
-/* iLQSPlanner::ActionFromPolicy of one problem: the iLQG half is a feedback policy and reads `state` (may be NULL) */
-int mjpc_b200_batch_ilqs_planner_action_from_policy(void* planner, int problem, double* action, const double* state,
-                                                    double time, int use_previous);
-
 /* ---- iLQS planner (csrc/host/gradient_planner.{h,cc}; mjpc/planners/ilqs/planner.cc:87-215): Predictive Sampling first;
  * when it does not improve, one iLQG iteration seeded with the sampling nominal; when sampling follows iLQG the trajectory
  * policy is converted to spline parameters through the least-squares inverse of the spline mapping. */
@@ -761,6 +637,111 @@ int mjpc_b200_ilqs_planner_create(const mjpc_model_blob* model, int num_trajecto
 int mjpc_b200_ilqs_planner_set_exploration(mjpc_b200_planner_t* p, double exploration);   /* its sampling half */
 /* scalars[4] = {active_policy (0 sampling, 1 iLQG), sampling winner return, iLQG total_return, sampling winner}; returns active_policy */
 int mjpc_b200_ilqs_planner_get_result(mjpc_b200_planner_t* p, double* scalars);
+
+/* ---- Batch planners (csrc/host/batch_planner.h): num_problems independent planners of one kind on ONE engine handle
+ * (two for the Robust and iLQS batches, as their single planners have), each problem with its own seed, state, mocap,
+ * task snapshot and policy.  An iteration runs the kind's one iteration over every problem, one batched launch per
+ * sweep, so each problem's result equals that of the kind's single planner with the same seed and inputs.  Settings are
+ * common to a batch.  Each kind has its own create (the single planner's create arguments plus num_problems, and
+ * seeds [num_problems] in place of seed) and get_result (the single planner's get_result of one problem), the iLQS
+ * batch a set_exploration and the iLQG batch a nominal_trajectory; these return MJPC_B200_ERR_BAD_ARGUMENT for a NULL
+ * handle or one of another kind.  Every other call is one of the generic mjpc_b200_batch_planner_* below, which take a
+ * batch of any kind and return MJPC_B200_ERR_BAD_ARGUMENT for a NULL one (destroy ignores it).  A call that takes a
+ * problem index returns MJPC_B200_ERR_BAD_ARGUMENT when it is outside [0, num_problems).
+ *   reset               mjpc_b200_planner_reset of one problem
+ *   set_state           mjpc_b200_planner_set_state of one problem; state must not be NULL
+ *   set_task            one problem's task snapshot (weight, parameters, task state), which starts as the model's; NULL
+ *                       members keep the current value
+ *   set_models          problem b plans on models[b] from now on: mjpc_b200_set_model_variants, with its rule and
+ *                       refusals, on every engine handle the batch owns.  count must be num_problems, or 0 to plan every
+ *                       problem on the batch's model again.  Valid between planning iterations (after an online system
+ *                       identification, for example).  The planners' settings and ctrlrange stay the batch's: variants
+ *                       must share actuator_ctrlrange
+ *   optimize_policy     Planner::OptimizePolicy of every problem: <0 on error.  codes [num_problems] (may be NULL)
+ *                       receives what each problem's single planner's optimize_policy returns: 0 for Sampling,
+ *                       Cross-Entropy, Sample Gradient and Robust, 1 / 0 for Gradient, iLQG and iLQS; all 0 after an
+ *                       error
+ *   action_from_policy  mjpc_b200_planner_action_from_policy of one problem: state (may be NULL) is read by the iLQG
+ *                       policy (iLQG, iLQS)
+ *   set_fd              mjpc_b200_planner_set_fd of every problem: Gradient, iLQG and iLQS; the others return
+ *                       MJPC_B200_ERR_UNSUPPORTED */
+typedef struct mjpc_b200_batch_planner mjpc_b200_batch_planner_t;
+void mjpc_b200_batch_planner_destroy(mjpc_b200_batch_planner_t* p);
+int mjpc_b200_batch_planner_reset(mjpc_b200_batch_planner_t* p, int problem, int horizon,
+                                  const double* initial_repeated_action);
+int mjpc_b200_batch_planner_set_state(mjpc_b200_batch_planner_t* p, int problem, const double* state, double time,
+                                      const double* mocap);
+int mjpc_b200_batch_planner_set_task(mjpc_b200_batch_planner_t* p, int problem, const double* weight,
+                                     const double* parameters, const double* task_state);
+int mjpc_b200_batch_planner_set_models(mjpc_b200_batch_planner_t* p, const mjpc_model_blob* models, int count);
+int mjpc_b200_batch_planner_optimize_policy(mjpc_b200_batch_planner_t* p, int horizon, int* codes);
+int mjpc_b200_batch_planner_action_from_policy(mjpc_b200_batch_planner_t* p, int problem, double* action,
+                                               const double* state, double time, int use_previous);
+int mjpc_b200_batch_planner_set_fd(mjpc_b200_batch_planner_t* p, double tolerance, int mode, int derivative_skip);
+
+/* Predictive Sampling: one mjpc_b200_rollout_spline_batched launch of B x N per iteration. */
+int mjpc_b200_batch_sampling_planner_create(const mjpc_model_blob* model, int num_problems, int num_trajectory,
+                                            int num_spline_points, int interpolation, double exploration,
+                                            double timestep, const double* ctrlrange, const uint32_t* seeds,
+                                            int max_horizon, int device, mjpc_b200_batch_planner_t** out);
+int mjpc_b200_batch_sampling_planner_get_result(mjpc_b200_batch_planner_t* p, int problem, int* winner,
+                                                double* improvement, float* returns, double* knots,
+                                                double* knot_times);
+/* Cross-Entropy: one launch of B x (N + 1). */
+int mjpc_b200_batch_ce_planner_create(const mjpc_model_blob* model, int num_problems, int num_trajectory, int n_elite,
+                                      int num_spline_points, int interpolation, double std_initial, double std_min,
+                                      double explore_fraction, double timestep, const double* ctrlrange,
+                                      const uint32_t* seeds, int max_horizon, int device,
+                                      mjpc_b200_batch_planner_t** out);
+int mjpc_b200_batch_ce_planner_get_result(mjpc_b200_batch_planner_t* p, int problem, double* improvement,
+                                          float* returns, int* order, double* knots, double* knot_times,
+                                          double* variance);
+/* Sample Gradient: one launch of B x N. */
+int mjpc_b200_batch_sg_planner_create(const mjpc_model_blob* model, int num_problems, int num_trajectory,
+                                      int num_gradient, int num_spline_points, int interpolation, double exploration,
+                                      double gradient_filter, double timestep, const double* ctrlrange,
+                                      const uint32_t* seeds, int max_horizon, int device,
+                                      mjpc_b200_batch_planner_t** out);
+int mjpc_b200_batch_sg_planner_get_result(mjpc_b200_batch_planner_t* p, int problem, int* winner, int* winner_type,
+                                          double* improvement, float* returns, int* order, double* knots,
+                                          double* knot_times, double* gradient_knots, double* gradient);
+/* Robust: a clean launch of B x N, then one noisy launch of B x ncandidates x nrepetitions on a second handle, each
+ * problem drawing its force noise with its own key seed + iteration (mjpc_b200_set_xfrc_noise_batched). */
+int mjpc_b200_batch_robust_planner_create(const mjpc_model_blob* model, int num_problems, int num_trajectory,
+                                          int num_spline_points, int interpolation, double exploration, double timestep,
+                                          const double* ctrlrange, const uint32_t* seeds, int ncandidates,
+                                          int nrepetitions, double xfrc_std, double xfrc_rate, int max_horizon,
+                                          int device, mjpc_b200_batch_planner_t** out);
+int mjpc_b200_batch_robust_planner_get_result(mjpc_b200_batch_planner_t* p, int problem, int* winner, double* scores,
+                                              float* returns, double* knots, double* knot_times);
+/* Gradient: per max_rollout iteration one spline launch of the B resampled nominals, one mjpc_b200_gradient_batched on
+ * their trajectories and one spline launch of the B x num_trajectory line-search candidates. */
+int mjpc_b200_batch_gradient_planner_create(const mjpc_model_blob* model, int num_problems, int num_trajectory,
+                                            int num_spline_points, int representation, double fd_tolerance,
+                                            double timestep, const double* ctrlrange, int max_horizon, int device,
+                                            mjpc_b200_batch_planner_t** out);
+int mjpc_b200_batch_gradient_planner_get_result(mjpc_b200_batch_planner_t* p, int problem, double* scalars,
+                                                double* parameters, double* times);
+/* iLQS: sampling on a handle of num_problems x num_trajectory, iLQG on one of num_problems x ilqg_num_rollouts.  Per
+ * iteration at most one feedback launch of the iLQG nominals of the problems whose active policy was iLQG, one spline
+ * launch of every problem's sampling, then, for the problems sampling did not settle, one batched derivative sweep, one
+ * batched cost-derivative call, backward-pass rounds of the problems still failing and one action-rollout launch.
+ * set_exploration sets every problem's. */
+int mjpc_b200_batch_ilqs_planner_create(const mjpc_model_blob* model, int num_problems, int num_trajectory,
+                                        int num_spline_points, int interpolation, double exploration, double timestep,
+                                        const double* ctrlrange, const uint32_t* seeds, int ilqg_num_rollouts,
+                                        int ilqg_representation, double fd_tolerance, int max_horizon, int device,
+                                        mjpc_b200_batch_planner_t** out);
+int mjpc_b200_batch_ilqs_planner_get_result(mjpc_b200_batch_planner_t* p, int problem, double* scalars);
+int mjpc_b200_batch_ilqs_planner_set_exploration(mjpc_b200_batch_planner_t* p, double exploration);
+/* iLQG: one batched launch per sweep for all problems; backward passes are retried in batches of the problems still
+ * failing.  nominal_trajectory is every problem's iLQGPlanner::NominalTrajectory in one launch. */
+int mjpc_b200_batch_ilqg_planner_create(const mjpc_model_blob* model, int num_problems, int num_rollouts,
+                                        int representation, double fd_tolerance, int max_horizon, int device,
+                                        mjpc_b200_batch_planner_t** out);
+int mjpc_b200_batch_ilqg_planner_get_result(mjpc_b200_batch_planner_t* p, int problem, double* scalars, float* states,
+                                            float* actions, double* times);
+int mjpc_b200_batch_ilqg_planner_nominal_trajectory(mjpc_b200_batch_planner_t* p, int horizon);
 
 /* ---- Agent::PlanIteration glue (csrc/host/agent.{h,cc}; mjpc/agent.cc:85-107,150-164,283-357): owns the planner selected
  * by agent_planner (0 Sampling, 1 Gradient, 2 iLQG, 3 iLQS, 4 Robust, 5 Cross-Entropy; mjpc/planners/include.h:26-34) and does

@@ -21,6 +21,7 @@ int BatchPlanner::Attach(const mjpc_model_blob* model, int num_problems, int max
     return MJPC_B200_ERR_BAD_BLOB;
   }
   nw_ = (int)weight_.size(); np_ = (int)parameters_.size(); nts_ = (int)task_state_.size();
+  codes_.assign(num_problems, 0);
   std::vector<double> w(weight_), p(parameters_), s(task_state_);
   for (int b = 1; b < num_problems; b++) {
     weight_.insert(weight_.end(), w.begin(), w.end());
@@ -152,7 +153,6 @@ int BatchGradientPlanner::Initialize(const mjpc_model_blob* model, int num_probl
                                      const double* ctrlrange, int max_horizon, int device) {
   if (num_problems < 1) return MJPC_B200_ERR_BAD_ARGUMENT;
   if (int rc = Attach(model, num_problems, num_problems * std::max(num_trajectory, 1), max_horizon, device)) return rc;
-  improved_.assign(num_problems, 0);
   for (int b = 0; b < num_problems; b++) {
     auto* p = new GradientPlanner;
     problems_.emplace_back(p);
@@ -164,7 +164,7 @@ int BatchGradientPlanner::Initialize(const mjpc_model_blob* model, int num_probl
 }
 
 int BatchGradientPlanner::OptimizePolicy(int horizon) {
-  return GradientPlanner::Iterate(all<GradientPlanner>(), Rows(), horizon, &launch_, improved_.data());
+  return GradientPlanner::Iterate(all<GradientPlanner>(), Rows(), horizon, &launch_, codes_.data());
 }
 
 // ------------------------------------------------------------------------------------------ iLQS
@@ -180,7 +180,6 @@ int BatchILQSPlanner::Initialize(const mjpc_model_blob* model, int num_problems,
   if (num_problems < 1) return MJPC_B200_ERR_BAD_ARGUMENT;
   if (int rc = Attach(model, num_problems, num_problems * num_trajectory, max_horizon, device)) return rc;
   if (int rc = mjpc_b200_create(model, num_problems * ilqg_num_rollouts, max_horizon, device, &ilqg_gpu_)) return rc;
-  improved_.assign(num_problems, 0);
   for (int b = 0; b < num_problems; b++) {
     auto* p = new iLQSPlanner;
     problems_.emplace_back(p);
@@ -193,7 +192,7 @@ int BatchILQSPlanner::Initialize(const mjpc_model_blob* model, int num_problems,
 }
 
 int BatchILQSPlanner::OptimizePolicy(int horizon) {
-  return iLQSPlanner::Iterate(all<iLQSPlanner>(), Rows(), horizon, &launch_, &sweeps_, improved_.data());
+  return iLQSPlanner::Iterate(all<iLQSPlanner>(), Rows(), horizon, &launch_, &sweeps_, codes_.data());
 }
 
 // ------------------------------------------------------------------------------------------ iLQG
@@ -201,7 +200,6 @@ int BatchILQGPlanner::Initialize(const mjpc_model_blob* model, int num_problems,
                                  int max_horizon, int device) {
   if (num_problems < 1 || num_rollouts < 1 || max_horizon < 2) return MJPC_B200_ERR_BAD_ARGUMENT;
   if (int rc = Attach(model, num_problems, num_problems * num_rollouts, max_horizon, device)) return rc;
-  improved_.assign(num_problems, 0);
   for (int b = 0; b < num_problems; b++) {
     auto* p = new iLQGPlanner;
     problems_.emplace_back(p);
@@ -217,17 +215,18 @@ int BatchILQGPlanner::NominalTrajectory(int horizon) {
 }
 
 int BatchILQGPlanner::OptimizePolicy(int horizon) {
-  std::fill(improved_.begin(), improved_.end(), 0);
+  std::fill(codes_.begin(), codes_.end(), 0);
   const DifferentiableScope diff(gpu_, planner(0).settings.differentiable != 0);
   const std::vector<iLQGPlanner*> ps = all<iLQGPlanner>();
   if (sweeps_.Nominal(ps, problem_rows_, Rows(), horizon, nullptr)) return -1;
-  return sweeps_.Iterate(ps, problem_rows_, Rows(), horizon, improved_.data());
+  return sweeps_.Iterate(ps, problem_rows_, Rows(), horizon, codes_.data());
 }
 
 }  // namespace mjpc_b200_host
 
+
 // ------------------------------------------------------------------------------------------ C entry points
-// (the generic batch family of include/mjpc_b200.h: every batch kind's handle is its BatchPlanner base)
+// (the batch family of include/mjpc_b200.h: every batch kind's handle is its BatchPlanner base)
 using mjpc_b200_host::BatchCrossEntropyPlanner;
 using mjpc_b200_host::BatchGradientPlanner;
 using mjpc_b200_host::BatchILQGPlanner;
@@ -236,89 +235,99 @@ using mjpc_b200_host::BatchPlanner;
 using mjpc_b200_host::BatchRobustPlanner;
 using mjpc_b200_host::BatchSampleGradientPlanner;
 using mjpc_b200_host::BatchSamplingPlanner;
+using mjpc_b200_host::ToHandle;
 
 namespace {
-BatchPlanner* batch_of(void* p) { return reinterpret_cast<BatchPlanner*>(p); }
+mjpc_b200_batch_planner_t* batch_handle(BatchPlanner* p) { return reinterpret_cast<mjpc_b200_batch_planner_t*>(p); }
 // the batch planner behind a handle if it is a T and `problem` is one of its problems, else nullptr
 template <class T>
-T* problem_of(void* p, int problem) {
-  T* bp = dynamic_cast<T*>(batch_of(p));
+T* problem_of(mjpc_b200_batch_planner_t* h, int problem) {
+  T* bp = dynamic_cast<T*>(reinterpret_cast<BatchPlanner*>(h));
   return bp && problem >= 0 && problem < bp->NumProblems() ? bp : nullptr;
 }
 template <class T>
-int finish_create(T* p, int rc, void** out) {
+int finish_create(T* p, int rc, mjpc_b200_batch_planner_t** out) {
   if (rc) { delete p; return rc; }
-  *out = static_cast<BatchPlanner*>(p);
+  *out = batch_handle(p);
   return 0;
 }
 }  // namespace
 
 extern "C" {
 
-void mjpc_b200_batch_planner_destroy(void* p) { delete batch_of(p); }
-int mjpc_b200_batch_planner_reset(void* p, int problem, int horizon, const double* initial_repeated_action) {
-  BatchPlanner* bp = problem_of<BatchPlanner>(p, problem);
+void mjpc_b200_batch_planner_destroy(mjpc_b200_batch_planner_t* h) { delete reinterpret_cast<BatchPlanner*>(h); }
+int mjpc_b200_batch_planner_reset(mjpc_b200_batch_planner_t* h, int problem, int horizon,
+                                  const double* initial_repeated_action) {
+  BatchPlanner* bp = problem_of<BatchPlanner>(h, problem);
   if (!bp) return MJPC_B200_ERR_BAD_ARGUMENT;
   bp->problem(problem).Reset(horizon, initial_repeated_action);
   return 0;
 }
-int mjpc_b200_batch_planner_set_state(void* p, int problem, const double* state, double time, const double* mocap) {
-  BatchPlanner* bp = problem_of<BatchPlanner>(p, problem);
+int mjpc_b200_batch_planner_set_state(mjpc_b200_batch_planner_t* h, int problem, const double* state, double time,
+                                      const double* mocap) {
+  BatchPlanner* bp = problem_of<BatchPlanner>(h, problem);
   if (!bp || !state) return MJPC_B200_ERR_BAD_ARGUMENT;
   bp->problem(problem).SetState(state, time, mocap);
   return 0;
 }
-int mjpc_b200_batch_planner_set_task(void* p, int problem, const double* weight, const double* parameters,
-                                     const double* task_state) {
-  BatchPlanner* bp = problem_of<BatchPlanner>(p, problem);
+int mjpc_b200_batch_planner_set_task(mjpc_b200_batch_planner_t* h, int problem, const double* weight,
+                                     const double* parameters, const double* task_state) {
+  BatchPlanner* bp = problem_of<BatchPlanner>(h, problem);
   if (!bp) return MJPC_B200_ERR_BAD_ARGUMENT;
   bp->SetTask(problem, weight, parameters, task_state);
   return 0;
 }
-int mjpc_b200_batch_planner_set_models(void* p, const mjpc_model_blob* models, int count) {
-  if (!p || count < 0) return MJPC_B200_ERR_BAD_ARGUMENT;
-  return batch_of(p)->SetModels(models, count);
+int mjpc_b200_batch_planner_set_models(mjpc_b200_batch_planner_t* h, const mjpc_model_blob* models, int count) {
+  BatchPlanner* bp = problem_of<BatchPlanner>(h, 0);
+  if (!bp || count < 0) return MJPC_B200_ERR_BAD_ARGUMENT;
+  return bp->SetModels(models, count);
 }
-int mjpc_b200_batch_planner_optimize_policy(void* p, int horizon) {
-  if (!p) return MJPC_B200_ERR_BAD_ARGUMENT;
-  return batch_of(p)->OptimizePolicy(horizon);
+int mjpc_b200_batch_planner_optimize_policy(mjpc_b200_batch_planner_t* h, int horizon, int* codes) {
+  BatchPlanner* bp = problem_of<BatchPlanner>(h, 0);
+  if (!bp) return MJPC_B200_ERR_BAD_ARGUMENT;
+  const int rc = bp->OptimizePolicy(horizon);
+  for (int b = 0; codes && b < bp->NumProblems(); b++) codes[b] = rc < 0 ? 0 : bp->codes()[b];
+  return rc;
 }
-int mjpc_b200_batch_planner_action_from_policy(void* p, int problem, double* action, double time, int use_previous) {
-  BatchPlanner* bp = problem_of<BatchPlanner>(p, problem);
+int mjpc_b200_batch_planner_action_from_policy(mjpc_b200_batch_planner_t* h, int problem, double* action,
+                                               const double* state, double time, int use_previous) {
+  BatchPlanner* bp = problem_of<BatchPlanner>(h, problem);
   if (!bp || !action) return MJPC_B200_ERR_BAD_ARGUMENT;
-  bp->problem(problem).ActionFromPolicy(action, nullptr, time, use_previous != 0);
+  bp->problem(problem).ActionFromPolicy(action, state, time, use_previous != 0);
   return 0;
 }
-int mjpc_b200_batch_planner_set_fd(void* p, double tolerance, int mode, int derivative_skip) {
-  if (!p) return MJPC_B200_ERR_BAD_ARGUMENT;
-  BatchPlanner* bp = batch_of(p);
+int mjpc_b200_batch_planner_set_fd(mjpc_b200_batch_planner_t* h, double tolerance, int mode, int derivative_skip) {
+  BatchPlanner* bp = problem_of<BatchPlanner>(h, 0);
+  if (!bp) return MJPC_B200_ERR_BAD_ARGUMENT;
   for (int b = 0; b < bp->NumProblems(); b++)
     if (int rc = bp->problem(b).SetFD(tolerance, mode, derivative_skip)) return rc;   // the kinds without: UNSUPPORTED
   return 0;
 }
 
-int mjpc_b200_batch_planner_create(const mjpc_model_blob* model, int num_problems, int num_trajectory, int num_spline_points,
-                                   int interpolation, double exploration, double timestep, const double* ctrlrange,
-                                   const uint32_t* seeds, int max_horizon, int device, void** out) {
+int mjpc_b200_batch_sampling_planner_create(const mjpc_model_blob* model, int num_problems, int num_trajectory,
+                                            int num_spline_points, int interpolation, double exploration,
+                                            double timestep, const double* ctrlrange, const uint32_t* seeds,
+                                            int max_horizon, int device, mjpc_b200_batch_planner_t** out) {
   if (!model || !model->data || !ctrlrange || !seeds || !out) return MJPC_B200_ERR_BAD_ARGUMENT;
   *out = nullptr;
   auto* p = new BatchSamplingPlanner;
   return finish_create(p, p->Initialize(model, num_problems, num_trajectory, num_spline_points, interpolation,
                                         exploration, timestep, ctrlrange, seeds, max_horizon, device), out);
 }
-// sampling batches only: another kind is refused
-int mjpc_b200_batch_planner_get_result(void* p, int problem, int* winner, double* improvement, float* returns,
-                                       double* knots, double* knot_times) {
-  BatchSamplingPlanner* bp = problem_of<BatchSamplingPlanner>(p, problem);
+int mjpc_b200_batch_sampling_planner_get_result(mjpc_b200_batch_planner_t* h, int problem, int* winner,
+                                                double* improvement, float* returns, double* knots,
+                                                double* knot_times) {
+  BatchSamplingPlanner* bp = problem_of<BatchSamplingPlanner>(h, problem);
   if (!bp) return MJPC_B200_ERR_BAD_ARGUMENT;
-  return mjpc_b200_sampling_planner_get_result(mjpc_b200_host::ToHandle(&bp->planner(problem)), winner, improvement,
-                                               returns, knots, knot_times);
+  return mjpc_b200_sampling_planner_get_result(ToHandle(&bp->planner(problem)), winner, improvement, returns, knots,
+                                               knot_times);
 }
 
 int mjpc_b200_batch_ce_planner_create(const mjpc_model_blob* model, int num_problems, int num_trajectory, int n_elite,
                                       int num_spline_points, int interpolation, double std_initial, double std_min,
                                       double explore_fraction, double timestep, const double* ctrlrange,
-                                      const uint32_t* seeds, int max_horizon, int device, void** out) {
+                                      const uint32_t* seeds, int max_horizon, int device,
+                                      mjpc_b200_batch_planner_t** out) {
   if (!model || !model->data || !ctrlrange || !seeds || !out || num_trajectory < 2 || num_spline_points < 2)
     return MJPC_B200_ERR_BAD_ARGUMENT;
   *out = nullptr;
@@ -327,18 +336,20 @@ int mjpc_b200_batch_ce_planner_create(const mjpc_model_blob* model, int num_prob
                                         std_initial, std_min, explore_fraction, timestep, ctrlrange, seeds, max_horizon,
                                         device), out);
 }
-int mjpc_b200_batch_ce_planner_get_result(void* p, int problem, double* improvement, float* returns, int* order,
-                                          double* knots, double* knot_times, double* variance) {
-  BatchCrossEntropyPlanner* bp = problem_of<BatchCrossEntropyPlanner>(p, problem);
+int mjpc_b200_batch_ce_planner_get_result(mjpc_b200_batch_planner_t* h, int problem, double* improvement,
+                                          float* returns, int* order, double* knots, double* knot_times,
+                                          double* variance) {
+  BatchCrossEntropyPlanner* bp = problem_of<BatchCrossEntropyPlanner>(h, problem);
   if (!bp) return MJPC_B200_ERR_BAD_ARGUMENT;
-  return mjpc_b200_ce_planner_get_result(mjpc_b200_host::ToHandle(&bp->planner(problem)), improvement, returns, order,
-                                         knots, knot_times, variance);
+  return mjpc_b200_ce_planner_get_result(ToHandle(&bp->planner(problem)), improvement, returns, order, knots,
+                                         knot_times, variance);
 }
 
 int mjpc_b200_batch_sg_planner_create(const mjpc_model_blob* model, int num_problems, int num_trajectory,
                                       int num_gradient, int num_spline_points, int interpolation, double exploration,
                                       double gradient_filter, double timestep, const double* ctrlrange,
-                                      const uint32_t* seeds, int max_horizon, int device, void** out) {
+                                      const uint32_t* seeds, int max_horizon, int device,
+                                      mjpc_b200_batch_planner_t** out) {
   if (!model || !model->data || !ctrlrange || !seeds || !out || num_trajectory < 1 || num_spline_points < 2)
     return MJPC_B200_ERR_BAD_ARGUMENT;
   *out = nullptr;
@@ -347,20 +358,20 @@ int mjpc_b200_batch_sg_planner_create(const mjpc_model_blob* model, int num_prob
                                         interpolation, exploration, gradient_filter, timestep, ctrlrange, seeds,
                                         max_horizon, device), out);
 }
-int mjpc_b200_batch_sg_planner_get_result(void* p, int problem, int* winner, int* winner_type, double* improvement,
-                                          float* returns, int* order, double* knots, double* knot_times,
-                                          double* gradient_knots, double* gradient) {
-  BatchSampleGradientPlanner* bp = problem_of<BatchSampleGradientPlanner>(p, problem);
+int mjpc_b200_batch_sg_planner_get_result(mjpc_b200_batch_planner_t* h, int problem, int* winner, int* winner_type,
+                                          double* improvement, float* returns, int* order, double* knots,
+                                          double* knot_times, double* gradient_knots, double* gradient) {
+  BatchSampleGradientPlanner* bp = problem_of<BatchSampleGradientPlanner>(h, problem);
   if (!bp) return MJPC_B200_ERR_BAD_ARGUMENT;
-  return mjpc_b200_sg_planner_get_result(mjpc_b200_host::ToHandle(&bp->planner(problem)), winner, winner_type,
-                                         improvement, returns, order, knots, knot_times, gradient_knots, gradient);
+  return mjpc_b200_sg_planner_get_result(ToHandle(&bp->planner(problem)), winner, winner_type, improvement, returns,
+                                         order, knots, knot_times, gradient_knots, gradient);
 }
 
 int mjpc_b200_batch_robust_planner_create(const mjpc_model_blob* model, int num_problems, int num_trajectory,
                                           int num_spline_points, int interpolation, double exploration, double timestep,
                                           const double* ctrlrange, const uint32_t* seeds, int ncandidates,
                                           int nrepetitions, double xfrc_std, double xfrc_rate, int max_horizon,
-                                          int device, void** out) {
+                                          int device, mjpc_b200_batch_planner_t** out) {
   if (!model || !model->data || !ctrlrange || !seeds || !out) return MJPC_B200_ERR_BAD_ARGUMENT;
   *out = nullptr;
   auto* p = new BatchRobustPlanner;
@@ -368,41 +379,39 @@ int mjpc_b200_batch_robust_planner_create(const mjpc_model_blob* model, int num_
                                         exploration, timestep, ctrlrange, seeds, ncandidates, nrepetitions, xfrc_std,
                                         xfrc_rate, max_horizon, device), out);
 }
-int mjpc_b200_batch_robust_planner_get_result(void* p, int problem, int* winner, double* scores, float* returns,
-                                              double* knots, double* knot_times) {
-  BatchRobustPlanner* bp = problem_of<BatchRobustPlanner>(p, problem);
+int mjpc_b200_batch_robust_planner_get_result(mjpc_b200_batch_planner_t* h, int problem, int* winner, double* scores,
+                                              float* returns, double* knots, double* knot_times) {
+  BatchRobustPlanner* bp = problem_of<BatchRobustPlanner>(h, problem);
   if (!bp) return MJPC_B200_ERR_BAD_ARGUMENT;
-  return mjpc_b200_robust_planner_get_result(mjpc_b200_host::ToHandle(&bp->planner(problem)), winner, scores, returns,
-                                             knots, knot_times);
+  return mjpc_b200_robust_planner_get_result(ToHandle(&bp->planner(problem)), winner, scores, returns, knots,
+                                             knot_times);
 }
 
 int mjpc_b200_batch_gradient_planner_create(const mjpc_model_blob* model, int num_problems, int num_trajectory,
                                             int num_spline_points, int representation, double fd_tolerance,
                                             double timestep, const double* ctrlrange, int max_horizon, int device,
-                                            void** out) {
+                                            mjpc_b200_batch_planner_t** out) {
   if (!model || !model->data || !ctrlrange || !out || num_trajectory < 1 || num_spline_points < 1 || max_horizon < 2)
     return MJPC_B200_ERR_BAD_ARGUMENT;
   *out = nullptr;
   auto* p = new BatchGradientPlanner;
   int rc = p->Initialize(model, num_problems, num_trajectory, num_spline_points, representation, timestep, ctrlrange,
                          max_horizon, device);
-  if (rc == 0) mjpc_b200_batch_planner_set_fd(static_cast<BatchPlanner*>(p), fd_tolerance, -1, -1);
+  if (rc == 0) mjpc_b200_batch_planner_set_fd(batch_handle(p), fd_tolerance, -1, -1);
   return finish_create(p, rc, out);
 }
-int mjpc_b200_batch_gradient_planner_get_result(void* p, int problem, double* scalars, double* parameters,
-                                                double* times, int* improved) {
-  BatchGradientPlanner* bp = problem_of<BatchGradientPlanner>(p, problem);
+int mjpc_b200_batch_gradient_planner_get_result(mjpc_b200_batch_planner_t* h, int problem, double* scalars,
+                                                double* parameters, double* times) {
+  BatchGradientPlanner* bp = problem_of<BatchGradientPlanner>(h, problem);
   if (!bp) return MJPC_B200_ERR_BAD_ARGUMENT;
-  if (improved) *improved = bp->improved(problem);
-  return mjpc_b200_gradient_planner_get_result(mjpc_b200_host::ToHandle(&bp->planner(problem)), scalars, parameters,
-                                               times);
+  return mjpc_b200_gradient_planner_get_result(ToHandle(&bp->planner(problem)), scalars, parameters, times);
 }
 
 int mjpc_b200_batch_ilqs_planner_create(const mjpc_model_blob* model, int num_problems, int num_trajectory,
                                         int num_spline_points, int interpolation, double exploration, double timestep,
                                         const double* ctrlrange, const uint32_t* seeds, int ilqg_num_rollouts,
                                         int ilqg_representation, double fd_tolerance, int max_horizon, int device,
-                                        void** out) {
+                                        mjpc_b200_batch_planner_t** out) {
   if (!model || !model->data || !ctrlrange || !seeds || !out || num_trajectory < 1 || ilqg_num_rollouts < 1 ||
       max_horizon < 2)
     return MJPC_B200_ERR_BAD_ARGUMENT;
@@ -412,81 +421,37 @@ int mjpc_b200_batch_ilqs_planner_create(const mjpc_model_blob* model, int num_pr
                                         exploration, timestep, ctrlrange, seeds, ilqg_num_rollouts, ilqg_representation,
                                         fd_tolerance, max_horizon, device), out);
 }
-// scalars[4] as mjpc_b200_ilqs_planner_get_result; *improved (may be NULL) = the problem's 1/0 of the last iteration
-int mjpc_b200_batch_ilqs_planner_get_result(void* p, int problem, double* scalars, int* improved) {
-  BatchILQSPlanner* bp = problem_of<BatchILQSPlanner>(p, problem);
+int mjpc_b200_batch_ilqs_planner_get_result(mjpc_b200_batch_planner_t* h, int problem, double* scalars) {
+  BatchILQSPlanner* bp = problem_of<BatchILQSPlanner>(h, problem);
   if (!bp) return MJPC_B200_ERR_BAD_ARGUMENT;
-  if (improved) *improved = bp->improved(problem);
-  return mjpc_b200_ilqs_planner_get_result(mjpc_b200_host::ToHandle(&bp->planner(problem)), scalars);
+  return mjpc_b200_ilqs_planner_get_result(ToHandle(&bp->planner(problem)), scalars);
 }
-int mjpc_b200_batch_ilqs_planner_set_exploration(void* p, double exploration) {
-  BatchILQSPlanner* bp = problem_of<BatchILQSPlanner>(p, 0);
+int mjpc_b200_batch_ilqs_planner_set_exploration(mjpc_b200_batch_planner_t* h, double exploration) {
+  BatchILQSPlanner* bp = problem_of<BatchILQSPlanner>(h, 0);
   if (!bp) return MJPC_B200_ERR_BAD_ARGUMENT;
   for (int b = 0; b < bp->NumProblems(); b++) bp->planner(b).sampling.SetExploration(exploration, 0.0);
   return 0;
 }
-int mjpc_b200_batch_ilqs_planner_action_from_policy(void* p, int problem, double* action, const double* state,
-                                                    double time, int use_previous) {
-  BatchILQSPlanner* bp = problem_of<BatchILQSPlanner>(p, problem);
-  if (!bp || !action) return MJPC_B200_ERR_BAD_ARGUMENT;
-  bp->planner(problem).ActionFromPolicy(action, state, time, use_previous != 0);
-  return 0;
-}
 
-// The iLQG batch's own family: each call refuses a batch of another kind (MJPC_B200_ERR_BAD_ARGUMENT; destroy and
-// set_fd, which return nothing, do nothing) and is otherwise the generic call where there is one.
-int mjpc_b200_batch_ilqg_planner_create(const mjpc_model_blob* model, int num_problems, int num_rollouts, int representation,
-                                        double fd_tolerance, int max_horizon, int device, void** out) {
+int mjpc_b200_batch_ilqg_planner_create(const mjpc_model_blob* model, int num_problems, int num_rollouts,
+                                        int representation, double fd_tolerance, int max_horizon, int device,
+                                        mjpc_b200_batch_planner_t** out) {
   if (!model || !model->data || !out) return MJPC_B200_ERR_BAD_ARGUMENT;
   *out = nullptr;
   auto* p = new BatchILQGPlanner;
   int rc = p->Initialize(model, num_problems, num_rollouts, representation, max_horizon, device);
-  if (rc == 0) mjpc_b200_batch_planner_set_fd(static_cast<BatchPlanner*>(p), fd_tolerance, -1, -1);
+  if (rc == 0) mjpc_b200_batch_planner_set_fd(batch_handle(p), fd_tolerance, -1, -1);
   return finish_create(p, rc, out);
 }
-void mjpc_b200_batch_ilqg_planner_destroy(void* p) {
-  if (problem_of<BatchILQGPlanner>(p, 0)) mjpc_b200_batch_planner_destroy(p);
+int mjpc_b200_batch_ilqg_planner_get_result(mjpc_b200_batch_planner_t* h, int problem, double* scalars, float* states,
+                                            float* actions, double* times) {
+  BatchILQGPlanner* bp = problem_of<BatchILQGPlanner>(h, problem);
+  if (!bp) return MJPC_B200_ERR_BAD_ARGUMENT;
+  return mjpc_b200_ilqg_planner_get_result(ToHandle(&bp->planner(problem)), scalars, states, actions, times);
 }
-void mjpc_b200_batch_ilqg_planner_set_fd(void* p, double tolerance, int mode, int derivative_skip) {
-  if (problem_of<BatchILQGPlanner>(p, 0)) mjpc_b200_batch_planner_set_fd(p, tolerance, mode, derivative_skip);
-}
-int mjpc_b200_batch_ilqg_planner_reset(void* p, int problem, int horizon, const double* initial_repeated_action) {
-  if (!problem_of<BatchILQGPlanner>(p, problem)) return MJPC_B200_ERR_BAD_ARGUMENT;
-  return mjpc_b200_batch_planner_reset(p, problem, horizon, initial_repeated_action);
-}
-int mjpc_b200_batch_ilqg_planner_set_state(void* p, int problem, const double* state, double time, const double* mocap) {
-  if (!problem_of<BatchILQGPlanner>(p, problem)) return MJPC_B200_ERR_BAD_ARGUMENT;
-  return mjpc_b200_batch_planner_set_state(p, problem, state, time, mocap);
-}
-int mjpc_b200_batch_ilqg_planner_set_task(void* p, int problem, const double* weight, const double* parameters,
-                                          const double* task_state) {
-  if (!problem_of<BatchILQGPlanner>(p, problem)) return MJPC_B200_ERR_BAD_ARGUMENT;
-  return mjpc_b200_batch_planner_set_task(p, problem, weight, parameters, task_state);
-}
-int mjpc_b200_batch_ilqg_planner_nominal_trajectory(void* p, int horizon) {
-  BatchILQGPlanner* bp = problem_of<BatchILQGPlanner>(p, 0);
+int mjpc_b200_batch_ilqg_planner_nominal_trajectory(mjpc_b200_batch_planner_t* h, int horizon) {
+  BatchILQGPlanner* bp = problem_of<BatchILQGPlanner>(h, 0);
   return bp ? bp->NominalTrajectory(horizon) : MJPC_B200_ERR_BAD_ARGUMENT;
-}
-int mjpc_b200_batch_ilqg_planner_optimize_policy(void* p, int horizon, int* updated) {
-  BatchILQGPlanner* bp = problem_of<BatchILQGPlanner>(p, 0);
-  if (!bp) return MJPC_B200_ERR_BAD_ARGUMENT;
-  const int rc = mjpc_b200_batch_planner_optimize_policy(p, horizon);
-  for (int b = 0; updated && b < bp->NumProblems(); b++) updated[b] = bp->improved(b);
-  return rc;
-}
-int mjpc_b200_batch_ilqg_planner_action_from_policy(void* p, int problem, double* action, const double* state,
-                                                    double time) {
-  BatchILQGPlanner* bp = problem_of<BatchILQGPlanner>(p, problem);
-  if (!bp || !action) return MJPC_B200_ERR_BAD_ARGUMENT;
-  bp->planner(problem).ActionFromPolicy(action, state, time, false);
-  return 0;
-}
-int mjpc_b200_batch_ilqg_planner_get_result(void* p, int problem, double* scalars, float* states, float* actions,
-                                            double* times) {
-  BatchILQGPlanner* bp = problem_of<BatchILQGPlanner>(p, problem);
-  if (!bp) return MJPC_B200_ERR_BAD_ARGUMENT;
-  return mjpc_b200_ilqg_planner_get_result(mjpc_b200_host::ToHandle(&bp->planner(problem)), scalars, states, actions,
-                                           times);
 }
 
 }  // extern "C"

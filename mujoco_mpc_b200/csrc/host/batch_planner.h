@@ -31,8 +31,10 @@ class BatchPlanner {
   Planner& problem(int b) { return *problems_[b]; }
   // Task::weight / parameters / task-state block of problem b; NULL members keep the current value
   void SetTask(int b, const double* weight, const double* parameters, const double* task_state);
-  // Planner::OptimizePolicy of every problem
+  // Planner::OptimizePolicy of every problem; codes()[b] is then what problem b's returned when it succeeded (the
+  // Gradient, iLQG and iLQS 1/0, 0 for the other kinds)
   virtual int OptimizePolicy(int horizon) = 0;
+  const std::vector<int>& codes() const { return codes_; }
   // problem b plans on models[b] from now on (mjpc_b200_set_model_variants on every handle the batch owns); count is
   // the number of problems, or 0 to plan every problem on the batch's model again
   int SetModels(const mjpc_model_blob* models, int count);
@@ -57,6 +59,7 @@ class BatchPlanner {
   mjpc_b200_t* gpu_ = nullptr;
   std::vector<std::unique_ptr<Planner>> problems_;   // borrow gpu_
   SplineLaunch launch_;
+  std::vector<int> codes_;                            // [B], all 0 until a kind's OptimizePolicy fills it
 
  private:
   std::vector<double> weight_, parameters_, task_state_;   // [B][num_term], [B][num_parameters], [B][task_state_size]
@@ -112,10 +115,6 @@ class BatchGradientPlanner : public BatchPlanner {
                  int representation, double timestep, const double* ctrlrange, int max_horizon, int device);
   GradientPlanner& planner(int b) { return at<GradientPlanner>(b); }
   int OptimizePolicy(int horizon) override;
-  int improved(int b) const { return improved_[b]; }    // GradientPlanner::OptimizePolicy's 1/0; 0 after an error
-
- private:
-  std::vector<int> improved_;
 };
 
 // Two handles, as the single iLQS planner has: the sampling halves launch B x N on the base's handle, the iLQG halves
@@ -129,13 +128,11 @@ class BatchILQSPlanner : public BatchPlanner {
                  int ilqg_num_rollouts, int ilqg_representation, double fd_tolerance, int max_horizon, int device);
   iLQSPlanner& planner(int b) { return at<iLQSPlanner>(b); }
   int OptimizePolicy(int horizon) override;
-  int improved(int b) const { return improved_[b]; }    // iLQSPlanner::OptimizePolicy's 1/0; 0 after an error
 
  private:
   std::vector<mjpc_b200_t*> Handles() const override { return {gpu_, ilqg_gpu_}; }
   mjpc_b200_t* ilqg_gpu_ = nullptr;
   ILQGSweeps sweeps_;
-  std::vector<int> improved_;
 };
 
 class BatchILQGPlanner : public BatchPlanner {
@@ -146,12 +143,10 @@ class BatchILQGPlanner : public BatchPlanner {
   // iLQGPlanner::NominalTrajectory of every problem in one launch; <0 on error
   int NominalTrajectory(int horizon);
   int OptimizePolicy(int horizon) override;
-  int improved(int b) const { return improved_[b]; }    // iLQGPlanner::OptimizePolicy's 1/0; 0 after an error
 
  private:
   ILQGSweeps sweeps_;
   std::vector<int> problem_rows_;   // 0 .. B-1: problem b reads task row b
-  std::vector<int> improved_;
 };
 
 }  // namespace mjpc_b200_host

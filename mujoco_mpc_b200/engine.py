@@ -20,21 +20,18 @@ _bp = C.POINTER(C.c_uint8)
 
 EXPORTS = ["mjpc_b200_version", "mjpc_b200_last_error", "mjpc_b200_create", "mjpc_b200_destroy",
            "mjpc_b200_get_info", "mjpc_b200_set_task", "mjpc_b200_set_differentiable", "mjpc_b200_set_xfrc_noise", "mjpc_b200_rollout_spline", "mjpc_b200_rollout_feedback",
-           "mjpc_b200_rollout_spline_batched", "mjpc_b200_batch_planner_create", "mjpc_b200_batch_planner_destroy",
+           "mjpc_b200_rollout_spline_batched", "mjpc_b200_batch_sampling_planner_create", "mjpc_b200_batch_planner_destroy",
            "mjpc_b200_batch_planner_reset", "mjpc_b200_batch_planner_set_state", "mjpc_b200_batch_planner_set_task",
            "mjpc_b200_batch_planner_optimize_policy", "mjpc_b200_batch_planner_action_from_policy",
-           "mjpc_b200_batch_planner_get_result", "mjpc_b200_set_xfrc_noise_batched", "mjpc_b200_planner_set_task",
+           "mjpc_b200_batch_sampling_planner_get_result", "mjpc_b200_set_xfrc_noise_batched", "mjpc_b200_planner_set_task",
            "mjpc_b200_batch_ce_planner_create", "mjpc_b200_batch_ce_planner_get_result",
            "mjpc_b200_batch_sg_planner_create", "mjpc_b200_batch_sg_planner_get_result",
            "mjpc_b200_batch_robust_planner_create", "mjpc_b200_batch_robust_planner_get_result",
            "mjpc_b200_fetch_trajectory", "mjpc_b200_fetch_all", "mjpc_b200_model_derivatives",
            "mjpc_b200_cost_derivatives", "mjpc_b200_backward_pass", "mjpc_b200_rollout_feedback_batched",
            "mjpc_b200_model_derivatives_batched", "mjpc_b200_cost_derivatives_batched", "mjpc_b200_backward_pass_batched",
-           "mjpc_b200_batch_ilqg_planner_create", "mjpc_b200_batch_ilqg_planner_destroy",
-           "mjpc_b200_batch_ilqg_planner_set_fd", "mjpc_b200_batch_ilqg_planner_reset",
-           "mjpc_b200_batch_ilqg_planner_set_state", "mjpc_b200_batch_ilqg_planner_set_task",
-           "mjpc_b200_batch_ilqg_planner_nominal_trajectory", "mjpc_b200_batch_ilqg_planner_optimize_policy",
-           "mjpc_b200_batch_ilqg_planner_action_from_policy", "mjpc_b200_batch_ilqg_planner_get_result",
+           "mjpc_b200_batch_ilqg_planner_create", "mjpc_b200_batch_ilqg_planner_nominal_trajectory",
+           "mjpc_b200_batch_ilqg_planner_get_result",
            "mjpc_b200_step_debug", "mjpc_b200_step_debug_contacts", "mjpc_b200_step_batch", "mjpc_b200_step_sensors",
            "mjpc_b200_estimator_destroy", "mjpc_b200_estimator_reset", "mjpc_b200_estimator_set_noise",
            "mjpc_b200_estimator_set", "mjpc_b200_estimator_update", "mjpc_b200_estimator_get",
@@ -62,7 +59,7 @@ EXPORTS = ["mjpc_b200_version", "mjpc_b200_last_error", "mjpc_b200_create", "mjp
            "mjpc_b200_gradient_batched", "mjpc_b200_batch_gradient_planner_create",
            "mjpc_b200_batch_gradient_planner_get_result", "mjpc_b200_batch_planner_set_fd",
            "mjpc_b200_batch_ilqs_planner_create", "mjpc_b200_batch_ilqs_planner_get_result",
-           "mjpc_b200_batch_ilqs_planner_set_exploration", "mjpc_b200_batch_ilqs_planner_action_from_policy", "mjpc_b200_ilqs_planner_create",
+           "mjpc_b200_batch_ilqs_planner_set_exploration", "mjpc_b200_ilqs_planner_create",
            "mjpc_b200_ilqs_planner_set_exploration", "mjpc_b200_ilqs_planner_get_result",
            "mjpc_b200_set_options", "mjpc_b200_agent_steps", "mjpc_b200_agent_create", "mjpc_b200_agent_destroy",
            "mjpc_b200_agent_reset", "mjpc_b200_agent_set_state", "mjpc_b200_agent_set_task", "mjpc_b200_agent_set_plan_enabled",
@@ -106,13 +103,21 @@ def load_library():
         lib.mjpc_b200_stream.restype = C.c_void_p
         lib.mjpc_b200_device_returns.restype = C.c_void_p
         lib.mjpc_b200_host_philox_normal.restype = C.c_double
-        # the generic planner and estimator families: the first argument is the handle
+        # the generic planner, batch planner and estimator families: the first argument is the handle
         for f, args in ((lib.mjpc_b200_planner_destroy, []), (lib.mjpc_b200_planner_reset, [C.c_int, _dp]),
                         (lib.mjpc_b200_planner_set_state, [_dp, C.c_double, _dp]),
                         (lib.mjpc_b200_planner_optimize_policy, [C.c_int]),
                         (lib.mjpc_b200_planner_nominal_trajectory, [C.c_int]),
                         (lib.mjpc_b200_planner_action_from_policy, [_dp, _dp, C.c_double, C.c_int]),
                         (lib.mjpc_b200_planner_set_fd, [C.c_double, C.c_int, C.c_int]),
+                        (lib.mjpc_b200_batch_planner_destroy, []),
+                        (lib.mjpc_b200_batch_planner_reset, [C.c_int, C.c_int, _dp]),
+                        (lib.mjpc_b200_batch_planner_set_state, [C.c_int, _dp, C.c_double, _dp]),
+                        (lib.mjpc_b200_batch_planner_set_task, [C.c_int, _dp, _dp, _dp]),
+                        (lib.mjpc_b200_batch_planner_set_models, [C.POINTER(ModelBlob), C.c_int]),
+                        (lib.mjpc_b200_batch_planner_optimize_policy, [C.c_int, _ip]),
+                        (lib.mjpc_b200_batch_planner_action_from_policy, [C.c_int, _dp, _dp, C.c_double, C.c_int]),
+                        (lib.mjpc_b200_batch_planner_set_fd, [C.c_double, C.c_int, C.c_int]),
                         (lib.mjpc_b200_estimator_destroy, []),
                         (lib.mjpc_b200_estimator_reset, [_dp] + [C.c_double] * 4),
                         (lib.mjpc_b200_estimator_set_noise, [_dp, _dp]),
@@ -121,15 +126,11 @@ def load_library():
                         (lib.mjpc_b200_estimator_last_error, [])):
             f.argtypes, f.restype = [C.c_void_p] + args, C.c_int
         lib.mjpc_b200_estimator_last_error.restype = C.c_char_p
-        lib.mjpc_b200_batch_planner_destroy.argtypes = [C.c_void_p]
-        lib.mjpc_b200_batch_planner_set_fd.argtypes = [C.c_void_p, C.c_double, C.c_int, C.c_int]
+        lib.mjpc_b200_batch_planner_destroy.restype = None
         lib.mjpc_b200_planner_set_task.argtypes = [C.c_void_p, C.c_void_p]
         lib.mjpc_b200_set_xfrc_noise_batched.argtypes = [C.c_void_p, C.c_double, C.c_double, C.c_int,
                                                          C.POINTER(C.c_uint32)]
         lib.mjpc_b200_sampling_planner_set_exploration.argtypes = [C.c_void_p, C.c_double, C.c_double]
-        lib.mjpc_b200_batch_ilqg_planner_destroy.argtypes = [C.c_void_p]
-        lib.mjpc_b200_batch_ilqg_planner_set_fd.argtypes = [C.c_void_p, C.c_double, C.c_int, C.c_int]
-        lib.mjpc_b200_batch_ilqg_planner_set_fd.restype = None
         lib.mjpc_b200_agent_destroy.argtypes = [C.c_void_p]
         lib.mjpc_b200_agent_steps.argtypes = [C.c_double, C.c_double]
         lib.mjpc_b200_set_options.argtypes = [C.c_void_p, C.c_double, C.c_int]
@@ -822,7 +823,14 @@ class CppSamplingPlanner(_CppPlanner):
 class _CppBatchPlanner(_CppObject):
     """A batch of num_problems independent planners of one kind (csrc/host/batch_planner.h): `<prefix>_create` makes it
     and result(problem) reads one problem; every other call is one of the generic mjpc_b200_batch_planner_* entry
-    points, and each method that concerns one problem takes its index."""
+    points, and each method that concerns one problem takes its index.  The sampling-based batches' optimize_policy
+    returns every problem's result(); those with _RETURNS_CODE (Gradient, iLQG, iLQS) return each problem's code
+    (1 improved / updated, 0 not), as their single planners do."""
+    _RETURNS_CODE = False
+
+    def _create(self, prefix, model, *args):
+        super()._create(prefix, model, *args)
+        self._codes = np.zeros(self.B, np.int32)   # of the last optimize_policy
 
     def _setup(self, model, num_problems, horizon, num_trajectory, seeds):
         num = model.numeric
@@ -862,33 +870,51 @@ class _CppBatchPlanner(_CppObject):
         handle the batch owns; None or [] plans every problem on the batch's model again."""
         _set_batch_models(self, models)
 
+    def set_fd(self, tolerance, mode=-1, derivative_skip=-1):
+        self._check(self.lib.mjpc_b200_batch_planner_set_fd(self.h, C.c_double(tolerance), int(mode), int(derivative_skip)),
+                    "set_fd")
+
     def optimize_policy(self):
-        """One planning iteration of every problem; returns the per-problem results."""
-        self._check(self.lib.mjpc_b200_batch_planner_optimize_policy(self.h, self.horizon), "optimize_policy")
-        return [self.result(b) for b in range(self.B)]
+        """One planning iteration of every problem; returns the per-problem results or codes."""
+        self._check(self.lib.mjpc_b200_batch_planner_optimize_policy(self.h, self.horizon, self._codes.ctypes.data_as(_ip)),
+                    "optimize_policy")
+        return self._codes.tolist() if self._RETURNS_CODE else [self.result(b) for b in range(self.B)]
+
+    def _action(self, problem, time, state, use_previous):
+        a, s = np.zeros(self.nu), _d(state)
+        self._check(self.lib.mjpc_b200_batch_planner_action_from_policy(self.h, int(problem), _pd(a), _pd(s),
+                                                                        C.c_double(time), int(use_previous)),
+                    "action_from_policy")
+        return a
 
     def action_from_policy(self, problem, time, use_previous=False):
-        a = np.zeros(self.nu)
-        self._check(self.lib.mjpc_b200_batch_planner_action_from_policy(self.h, int(problem), _pd(a), C.c_double(time),
-                                                                        int(use_previous)), "action_from_policy")
-        return a
+        return self._action(problem, time, None, use_previous)
+
+
+class _CppBatchFeedbackPlanner(_CppBatchPlanner):
+    """iLQG and iLQS batches: the policy reads the state (time-varying feedback); optimize_policy returns the codes."""
+    _RETURNS_CODE = True
+    action_reads_state = True
+
+    def action_from_policy(self, problem, time, state=None, use_previous=False):
+        return self._action(problem, time, state, use_previous)
 
 
 class CppBatchSamplingPlanner(_CppBatchPlanner):
     """num_problems independent Predictive Sampling problems planned with one rollout launch per iteration
-    (csrc/host/batch_sampling_planner.cc)."""
+    (csrc/host/batch_planner.cc)."""
 
     def __init__(self, model, num_problems, num_trajectory, horizon, seeds=None, device=0):
         num, cr, sd = self._setup(model, num_problems, horizon, num_trajectory, seeds)
-        self._create("mjpc_b200_batch_planner", model, self.B, self.N, self.P, int(num.get("sampling_representation", [2])[0]),
+        self._create("mjpc_b200_batch_sampling_planner", model, self.B, self.N, self.P, int(num.get("sampling_representation", [2])[0]),
                      C.c_double(float(num.get("sampling_exploration", [0.1])[0])), C.c_double(float(model.opt_timestep)),
                      cr, sd, self.horizon, int(device))
 
     def result(self, problem):
         winner, imp = C.c_int(), C.c_double()
         ret = np.zeros(self.N, np.float32); knots = np.zeros((self.P, self.nu)); kt = np.zeros(self.P)
-        self._check(self.lib.mjpc_b200_batch_planner_get_result(self.h, int(problem), C.byref(winner), C.byref(imp), _pf(ret),
-                                                                _pd(knots), _pd(kt)), "get_result")
+        self._check(self.lib.mjpc_b200_batch_sampling_planner_get_result(self.h, int(problem), C.byref(winner), C.byref(imp),
+                                                                         _pf(ret), _pd(knots), _pd(kt)), "get_result")
         return dict(winner=winner.value, improvement=imp.value, returns=ret, knots=knots, knot_times=kt)
 
 
@@ -1033,49 +1059,24 @@ class CppILQGPlanner(_CppFeedbackPlanner):
                     winner=int(sc[5]), states=st, actions=ac, times=tm)
 
 
-class CppBatchILQGPlanner(_CppObject):
-    """The batched C++ iLQG planner (csrc/host/batch_ilqg_planner.cc): B problems, one launch per sweep.  Mirrors
+class CppBatchILQGPlanner(_CppBatchFeedbackPlanner):
+    """The batched C++ iLQG planner (csrc/host/batch_planner.cc): B problems, one launch per sweep.  Mirrors
     CppILQGPlanner with a problem argument."""
-    action_reads_state = True   # the feedback policy: action_from_policy(problem, time, state)
 
     def __init__(self, model, num_problems, horizon, num_rollouts=10, representation=1, fd_tolerance=3e-4, device=0,
                  fd_mode=1, derivative_skip=0):
-        self.B, self.H, self.nu, self.ds = int(num_problems), int(horizon), model.nu, model.nq + model.nv
+        self.B, self.H = int(num_problems), int(horizon)
+        self.horizon, self.nu, self.ds = self.H, model.nu, model.nq + model.nv
         self._create("mjpc_b200_batch_ilqg_planner", model, self.B, int(num_rollouts), int(representation),
                      C.c_double(fd_tolerance), self.H, int(device))
-        self.lib.mjpc_b200_batch_ilqg_planner_set_fd(self.h, C.c_double(fd_tolerance), int(fd_mode), int(derivative_skip))
-
-    def _check(self, rc, what):
-        if rc < 0:
-            raise EngineError(f"batch_ilqg_planner_{what} failed ({rc}): {self.lib.mjpc_b200_last_error().decode()}")
-        return rc
-
-    def reset(self, problem, initial_repeated_action=None):
-        a = _d(initial_repeated_action)
-        self._check(self.lib.mjpc_b200_batch_ilqg_planner_reset(self.h, int(problem), self.H, _pd(a)), "reset")
-
-    def set_state(self, problem, state, time, mocap):
-        s, mc = _d(state), _d(mocap)
-        self._check(self.lib.mjpc_b200_batch_ilqg_planner_set_state(self.h, int(problem), _pd(s), C.c_double(time), _pd(mc)),
-                    "set_state")
-
-    def set_task(self, problem, weight=None, parameters=None, task_state=None):
-        w, p, s = _d(weight), _d(parameters), _d(task_state)
-        self._check(self.lib.mjpc_b200_batch_ilqg_planner_set_task(self.h, int(problem), _pd(w), _pd(p), _pd(s)), "set_task")
-
-    def set_models(self, models):
-        """Problem b plans on compiled model models[b] from now on; None or [] on the batch's model again."""
-        _set_batch_models(self, models)
+        self.set_fd(fd_tolerance, fd_mode, derivative_skip)
 
     def nominal_trajectory(self):
         return self._check(self.lib.mjpc_b200_batch_ilqg_planner_nominal_trajectory(self.h, self.H), "nominal_trajectory")
 
     def optimize_policy(self):
         """Every problem's iLQGPlanner::OptimizePolicy; returns updated [B] (1: the policy was updated)."""
-        up = np.zeros(self.B, np.int32)
-        self._check(self.lib.mjpc_b200_batch_ilqg_planner_optimize_policy(self.h, self.H, up.ctypes.data_as(_ip)),
-                    "optimize_policy")
-        return up
+        return np.array(super().optimize_policy(), np.int32)
 
     def result(self, problem):
         sc = np.zeros(6); st = np.zeros((self.H, self.ds), np.float32); ac = np.zeros((self.H, self.nu), np.float32)
@@ -1084,13 +1085,6 @@ class CppBatchILQGPlanner(_CppObject):
                     "get_result")
         return dict(total_return=sc[0], regularization=sc[1], improvement=sc[2], expected=sc[3], surprise=sc[4],
                     winner=int(sc[5]), states=st, actions=ac, times=tm)
-
-    def action_from_policy(self, problem, time, state=None):
-        a = np.zeros(self.nu)
-        s = _d(state)
-        self._check(self.lib.mjpc_b200_batch_ilqg_planner_action_from_policy(self.h, int(problem), _pd(a), _pd(s),
-                                                                             C.c_double(time)), "action_from_policy")
-        return a
 
 
 class CppRobustPlanner(_CppPlanner):
@@ -1137,32 +1131,11 @@ def host_gradient_sweep(A, B, cx, cu):
     return k, dV0.value
 
 
-class _CppBatchCodePlanner(_CppBatchPlanner):
-    """A batch whose optimize_policy returns each problem's code, as the single planner's does (Gradient, iLQS); the
-    kind's _get_result takes _NRESULT output pointers, then the code's."""
-    _NRESULT = 0
-
-    def set_fd(self, tolerance, mode=-1, derivative_skip=-1):
-        self._check(self.lib.mjpc_b200_batch_planner_set_fd(self.h, C.c_double(tolerance), int(mode), int(derivative_skip)),
-                    "set_fd")
-
-    def optimize_policy(self):
-        """One planning iteration of every problem; returns each problem's 1 (improved) / 0."""
-        self._check(self.lib.mjpc_b200_batch_planner_optimize_policy(self.h, self.horizon), "optimize_policy")
-        return [self._improved(b) for b in range(self.B)]
-
-    def _improved(self, problem):
-        imp = C.c_int()
-        self._check(getattr(self.lib, f"{self._prefix}_get_result")(self.h, int(problem), *([None] * self._NRESULT),
-                                                                      C.byref(imp)), "get_result")
-        return imp.value
-
-
-class CppBatchGradientPlanner(_CppBatchCodePlanner):
+class CppBatchGradientPlanner(_CppBatchPlanner):
     """num_problems independent Gradient problems (csrc/host/batch_planner.cc): per iteration one launch of the B
     nominals, one mjpc_b200_gradient_batched and one launch of the B x num_trajectory line-search candidates.  Mirrors
     CppGradientPlanner with a problem argument; optimize_policy returns each problem's 1/0."""
-    _NRESULT = 3
+    _RETURNS_CODE = True
 
     def __init__(self, model, num_problems, horizon, num_trajectory=8, num_spline_points=5, representation=1,
                  fd_tolerance=3e-4, device=0, fd_mode=1):
@@ -1173,20 +1146,18 @@ class CppBatchGradientPlanner(_CppBatchCodePlanner):
         self.set_fd(fd_tolerance, fd_mode, -1)
 
     def result(self, problem):
-        sc = np.zeros(6); p = np.zeros((self.P, self.nu)); t = np.zeros(self.P); imp = C.c_int()
-        self._check(self.lib.mjpc_b200_batch_gradient_planner_get_result(self.h, int(problem), _pd(sc), _pd(p), _pd(t),
-                                                                         C.byref(imp)), "get_result")
+        sc = np.zeros(6); p = np.zeros((self.P, self.nu)); t = np.zeros(self.P)
+        self._check(self.lib.mjpc_b200_batch_gradient_planner_get_result(self.h, int(problem), _pd(sc), _pd(p), _pd(t)),
+                    "get_result")
         return dict(total_return=sc[0], winner=int(sc[1]), action_step=sc[2], expected=sc[3], improvement=sc[4],
-                    surprise=sc[5], parameters=p, times=t, improved=imp.value)
+                    surprise=sc[5], parameters=p, times=t, improved=int(self._codes[problem]))
 
 
-class CppBatchILQSPlanner(_CppBatchCodePlanner):
+class CppBatchILQSPlanner(_CppBatchFeedbackPlanner):
     """num_problems independent iLQS problems (csrc/host/batch_planner.cc) on two handles: per iteration one feedback
     launch of the iLQG nominals that need converting, one sampling launch of B x num_trajectory, and one batched iLQG
     iteration of the problems sampling did not settle.  Mirrors CppILQSPlanner with a problem argument;
     optimize_policy returns each problem's 1/0."""
-    action_reads_state = True   # the iLQG half's feedback policy: action_from_policy(problem, time, state)
-    _NRESULT = 1
 
     def __init__(self, model, num_problems, horizon, num_trajectory=8, num_rollouts=6, fd_tolerance=3e-4, seeds=None,
                  device=0, fd_mode=1):
@@ -1202,18 +1173,10 @@ class CppBatchILQSPlanner(_CppBatchCodePlanner):
         self._check(self.lib.mjpc_b200_batch_ilqs_planner_set_exploration(self.h, C.c_double(sigma)), "set_exploration")
 
     def result(self, problem):
-        sc, imp = np.zeros(4), C.c_int()
-        self._check(self.lib.mjpc_b200_batch_ilqs_planner_get_result(self.h, int(problem), _pd(sc), C.byref(imp)),
-                    "get_result")
+        sc = np.zeros(4)
+        self._check(self.lib.mjpc_b200_batch_ilqs_planner_get_result(self.h, int(problem), _pd(sc)), "get_result")
         return dict(active_policy=int(sc[0]), sampling_return=sc[1], ilqg_return=sc[2], sampling_winner=int(sc[3]),
-                    improved=imp.value)
-
-    def action_from_policy(self, problem, time, state=None, use_previous=False):
-        a, s = np.zeros(self.nu), _d(state)
-        self._check(self.lib.mjpc_b200_batch_ilqs_planner_action_from_policy(self.h, int(problem), _pd(a), _pd(s),
-                                                                             C.c_double(time), int(use_previous)),
-                    "action_from_policy")
-        return a
+                    improved=int(self._codes[problem]))
 
 
 class CppGradientPlanner(_CppPlanner):

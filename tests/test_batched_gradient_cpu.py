@@ -35,19 +35,19 @@ def test_create_without_a_device_fails_and_leaves_out_null():
     del buf
 
 
-def test_null_handles_are_refused():
+def test_null_batch_handles_are_refused():
     from mujoco_mpc_b200.engine import load_library
     lib = load_library()
     d = C.c_double
     assert lib.mjpc_b200_batch_gradient_planner_create(None, 2, 8, 5, 1, d(1e-3), d(0.01), None, 16, 0, None) == BAD_ARGUMENT
-    assert lib.mjpc_b200_batch_gradient_planner_get_result(None, 0, None, None, None, None) == BAD_ARGUMENT
+    assert lib.mjpc_b200_batch_gradient_planner_get_result(None, 0, None, None, None) == BAD_ARGUMENT
     assert lib.mjpc_b200_batch_planner_set_fd(None, d(1e-3), 0, 0) == BAD_ARGUMENT
     assert lib.mjpc_b200_batch_ilqs_planner_create(None, 2, 8, 3, 2, d(0.1), d(0.01), None, None, 6, 1, d(1e-3), 16, 0,
                                                    None) == BAD_ARGUMENT
-    assert lib.mjpc_b200_batch_ilqs_planner_get_result(None, 0, None, None) == BAD_ARGUMENT
+    assert lib.mjpc_b200_batch_ilqs_planner_get_result(None, 0, None) == BAD_ARGUMENT
     assert lib.mjpc_b200_batch_ilqs_planner_set_exploration(None, d(0.1)) == BAD_ARGUMENT
     a = (C.c_double * 8)()
-    assert lib.mjpc_b200_batch_ilqs_planner_action_from_policy(None, 0, a, None, d(0.0), 0) == BAD_ARGUMENT
+    assert lib.mjpc_b200_batch_planner_action_from_policy(None, 0, a, a, d(0.0), 0) == BAD_ARGUMENT
     v = (C.c_double * 8)()
     f = (C.c_float * 8)()
     assert lib.mjpc_b200_gradient_batched(None, 1, f, f, v, None, None, None, None, f, 2, 0, C.c_float(1e-3), 0, v,

@@ -1,5 +1,6 @@
-"""CPU: the entry points of the batched Cross-Entropy, Robust and Sample Gradient planners and of per-problem noise
-keys, without a device: creates fail with MJPC_B200_ERR_CUDA and leave *out NULL, and NULL handles are refused."""
+"""CPU: the entry points of the batched Predictive Sampling, Cross-Entropy, Robust and Sample Gradient planners, of the
+generic batch family and of per-problem noise keys, without a device: creates fail with MJPC_B200_ERR_CUDA and leave
+*out NULL, and NULL handles are refused."""
 import ctypes as C
 
 import numpy as np
@@ -27,6 +28,7 @@ def test_creates_without_a_device_fail_and_leave_out_null():
     sp = seeds.ctypes.data_as(C.POINTER(C.c_uint32))
     d = C.c_double
     calls = {
+        "sampling": (2, 8, 3, 2, d(0.1), d(0.01), crp, sp, 11, 0),
         "ce": (2, 8, 0, 3, 2, d(0.1), d(0.01), d(0.0), d(0.01), crp, sp, 11, 0),
         "sg": (2, 8, 2, 3, 2, d(0.1), d(0.5), d(0.01), crp, sp, 11, 0),
         "robust": (2, 10, 3, 2, d(0.1), d(0.01), crp, sp, -1, 5, d(0.1), d(0.1), 11, 0),
@@ -39,17 +41,17 @@ def test_creates_without_a_device_fail_and_leave_out_null():
     del buf
 
 
-def test_null_handles_are_refused():
+def test_null_batch_family_handles_are_refused():
     from mujoco_mpc_b200.engine import load_library
     lib = load_library()
     seeds = (C.c_uint32 * 2)(1, 2)
     assert lib.mjpc_b200_set_xfrc_noise_batched(None, C.c_double(0.1), C.c_double(0.1), 2, seeds) == BAD_ARGUMENT
     assert lib.mjpc_b200_planner_set_task(None, None) == BAD_ARGUMENT
-    for kind in ("ce", "sg", "robust"):
+    for kind in ("sampling", "ce", "sg", "robust"):
         assert getattr(lib, f"mjpc_b200_batch_{kind}_planner_get_result")(None, 0, *([None] * 9)) == BAD_ARGUMENT, kind
         assert getattr(lib, f"mjpc_b200_batch_{kind}_planner_create")(None, *([0] * 8), None) == BAD_ARGUMENT, kind
     v = (C.c_double * 8)()
     generic = {"reset": (0, 8, None), "set_state": (0, v, C.c_double(0.0), None), "set_task": (0, None, None, None),
-               "optimize_policy": (8,), "action_from_policy": (0, v, C.c_double(0.0), 0), "get_result": (0,) + (None,) * 5}
+               "optimize_policy": (8, None), "action_from_policy": (0, v, None, C.c_double(0.0), 0)}
     for name, args in generic.items():
         assert getattr(lib, f"mjpc_b200_batch_planner_{name}")(None, *args) == BAD_ARGUMENT, name

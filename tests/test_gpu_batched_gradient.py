@@ -165,39 +165,42 @@ def test_batch_gradient_problems_are_independent():
                 np.testing.assert_array_equal(ra[b][key], rb[b][key], err_msg=key)
 
 
-def test_kind_checks():
+def test_gradient_ilqs_batch_kind_checks():
+    """A Gradient or iLQS batch's own calls refuse a batch of another kind and a problem outside the batch; set_fd
+    reaches the derivative-based kinds only."""
     from mujoco_mpc_b200.engine import CppBatchGradientPlanner, CppBatchILQSPlanner, CppBatchSamplingPlanner, load_library
     lib = load_library()
     m = get_model("particle")
     g = CppBatchGradientPlanner(m, 2, 16)
     s = CppBatchSamplingPlanner(m, 2, 8, 16)
     sc, v = (C.c_double * 6)(), (C.c_double * 64)()
-    assert lib.mjpc_b200_batch_gradient_planner_get_result(s.h, 0, sc, v, v, None) == BAD_ARGUMENT
+    assert lib.mjpc_b200_batch_gradient_planner_get_result(s.h, 0, sc, v, v) == BAD_ARGUMENT
     assert lib.mjpc_b200_batch_ce_planner_get_result(g.h, 0, *([None] * 6)) == BAD_ARGUMENT
-    assert lib.mjpc_b200_batch_planner_get_result(g.h, 0, *([None] * 5)) == BAD_ARGUMENT
+    assert lib.mjpc_b200_batch_sampling_planner_get_result(g.h, 0, *([None] * 5)) == BAD_ARGUMENT
+    assert lib.mjpc_b200_batch_ilqg_planner_nominal_trajectory(g.h, 16) == BAD_ARGUMENT
     for p in (-1, 2):
-        assert lib.mjpc_b200_batch_gradient_planner_get_result(g.h, p, sc, v, v, None) == BAD_ARGUMENT
+        assert lib.mjpc_b200_batch_gradient_planner_get_result(g.h, p, sc, v, v) == BAD_ARGUMENT
     assert lib.mjpc_b200_batch_planner_set_fd(s.h, C.c_double(1e-3), 0, 0) == UNSUPPORTED
     assert lib.mjpc_b200_batch_planner_set_fd(g.h, C.c_double(1e-3), 0, 0) == 0
-    assert lib.mjpc_b200_batch_gradient_planner_get_result(g.h, 1, sc, v, v, None) == 5   # P
+    assert lib.mjpc_b200_batch_gradient_planner_get_result(g.h, 1, sc, v, v) == 5   # P
     q = CppBatchILQSPlanner(m, 2, 16)
     a = (C.c_double * 8)()
     for other in (g.h, s.h):
-        assert lib.mjpc_b200_batch_ilqs_planner_get_result(other, 0, sc, None) == BAD_ARGUMENT
+        assert lib.mjpc_b200_batch_ilqs_planner_get_result(other, 0, sc) == BAD_ARGUMENT
         assert lib.mjpc_b200_batch_ilqs_planner_set_exploration(other, C.c_double(0.1)) == BAD_ARGUMENT
-        assert lib.mjpc_b200_batch_ilqs_planner_action_from_policy(other, 0, a, None, C.c_double(0.0), 0) == BAD_ARGUMENT
-    assert lib.mjpc_b200_batch_gradient_planner_get_result(q.h, 0, sc, v, v, None) == BAD_ARGUMENT
+    assert lib.mjpc_b200_batch_gradient_planner_get_result(q.h, 0, sc, v, v) == BAD_ARGUMENT
     for p in (-1, 2):
-        assert lib.mjpc_b200_batch_ilqs_planner_get_result(q.h, p, sc, None) == BAD_ARGUMENT
-        assert lib.mjpc_b200_batch_ilqs_planner_action_from_policy(q.h, p, a, None, C.c_double(0.0), 0) == BAD_ARGUMENT
+        assert lib.mjpc_b200_batch_ilqs_planner_get_result(q.h, p, sc) == BAD_ARGUMENT
+        assert lib.mjpc_b200_batch_planner_action_from_policy(q.h, p, a, None, C.c_double(0.0), 0) == BAD_ARGUMENT
     assert lib.mjpc_b200_batch_planner_set_fd(q.h, C.c_double(1e-3), 0, 0) == 0
-    assert lib.mjpc_b200_batch_ilqs_planner_get_result(q.h, 1, sc, None) == 0       # the active policy: sampling
+    assert lib.mjpc_b200_batch_ilqs_planner_get_result(q.h, 1, sc) == 0       # the active policy: sampling
     g.close(); s.close(); q.close()
 
 
-def test_ilqg_batch_kind_checks():
-    """The iLQG batch's own calls refuse another kind's handle (set_fd and destroy leave it alone), the generic calls
-    drive an iLQG batch as its own calls do, and the sampling-only generic get_result refuses it."""
+def test_ilqg_batch_generic_calls_and_kind_checks():
+    """The iLQG batch's own calls refuse another kind's handle and leave it whole, the generic calls drive an iLQG
+    batch as the Python class does (codes, results and actions with a state), and the sampling batch's get_result
+    refuses it."""
     from mujoco_mpc_b200.engine import CppBatchILQGPlanner, CppBatchSamplingPlanner, load_library
     lib = load_library()
     m = get_model("particle")
@@ -206,23 +209,16 @@ def test_ilqg_batch_kind_checks():
     x, mc = np.zeros(4), np.ascontiguousarray(mocap_of(m), np.float64)
     xp, mcp = x.ctypes.data_as(dp), mc.ctypes.data_as(dp)
     s = CppBatchSamplingPlanner(m, 2, 8, H)
-    a, sc, up = (C.c_double * 8)(), (C.c_double * 6)(), (C.c_int * 2)()
+    sc = (C.c_double * 6)()
     t0 = C.c_double(0.0)
-    assert lib.mjpc_b200_batch_ilqg_planner_reset(s.h, 0, H, None) == BAD_ARGUMENT
-    assert lib.mjpc_b200_batch_ilqg_planner_set_state(s.h, 0, xp, t0, mcp) == BAD_ARGUMENT
-    assert lib.mjpc_b200_batch_ilqg_planner_set_task(s.h, 0, None, None, None) == BAD_ARGUMENT
     assert lib.mjpc_b200_batch_ilqg_planner_nominal_trajectory(s.h, H) == BAD_ARGUMENT
-    assert lib.mjpc_b200_batch_ilqg_planner_optimize_policy(s.h, H, up) == BAD_ARGUMENT
-    assert lib.mjpc_b200_batch_ilqg_planner_action_from_policy(s.h, 0, a, None, t0) == BAD_ARGUMENT
     assert lib.mjpc_b200_batch_ilqg_planner_get_result(s.h, 0, sc, None, None, None) == BAD_ARGUMENT
-    lib.mjpc_b200_batch_ilqg_planner_set_fd(s.h, C.c_double(1e-3), 0, 0)
-    lib.mjpc_b200_batch_ilqg_planner_destroy(s.h)
     for b in range(2):                                                     # the sampling batch is still whole
         s.reset(b); s.set_state(b, x, 0.0, mc)
     assert len(s.optimize_policy()) == 2
     s.close()
 
-    # the same two problems through the generic calls (q) and the iLQG batch's own (ref)
+    # the same two problems through the C calls (q) and the Python class (ref)
     q = CppBatchILQGPlanner(m, 2, H)
     ref = CppBatchILQGPlanner(m, 2, H, fd_tolerance=1e-3, fd_mode=0, derivative_skip=0)
     assert lib.mjpc_b200_batch_planner_set_fd(q.h, C.c_double(1e-3), 0, 0) == 0
@@ -233,15 +229,21 @@ def test_ilqg_batch_kind_checks():
         w = np.asarray(m.task_weight, float) * (1.0 + b)
         assert lib.mjpc_b200_batch_planner_set_task(q.h, b, w.ctypes.data_as(dp), None, None) == 0
         ref.reset(b); ref.set_state(b, x, 0.0, mb); ref.set_task(b, w)
+    codes = (C.c_int * 2)()
     for _ in range(3):
-        assert lib.mjpc_b200_batch_planner_optimize_policy(q.h, H) == 0
-        ref.optimize_policy()
+        assert lib.mjpc_b200_batch_planner_optimize_policy(q.h, H, codes) == 0
+        np.testing.assert_array_equal(np.array(codes), ref.optimize_policy())
+    state = np.array([0.05, -0.02, 0.1, 0.0])
     for b in range(2):
         got = (C.c_double * 6)()
         assert lib.mjpc_b200_batch_ilqg_planner_get_result(q.h, b, got, None, None, None) == H
         np.testing.assert_array_equal(np.array(got), np.array([ref.result(b)[k] for k in (
             "total_return", "regularization", "improvement", "expected", "surprise", "winner")]))
-    assert lib.mjpc_b200_batch_planner_get_result(q.h, 0, *([None] * 5)) == BAD_ARGUMENT
+        a = np.zeros(m.nu)
+        assert lib.mjpc_b200_batch_planner_action_from_policy(q.h, b, a.ctypes.data_as(dp), state.ctypes.data_as(dp),
+                                                              C.c_double(0.05), 0) == 0
+        np.testing.assert_array_equal(a, ref.action_from_policy(b, 0.05, state))
+    assert lib.mjpc_b200_batch_sampling_planner_get_result(q.h, 0, *([None] * 5)) == BAD_ARGUMENT
     assert lib.mjpc_b200_batch_planner_set_state(q.h, 2, xp, t0, mcp) == BAD_ARGUMENT
     lib.mjpc_b200_batch_planner_destroy(q.h)
     q.h = None

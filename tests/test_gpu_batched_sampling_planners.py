@@ -182,7 +182,7 @@ def test_problems_are_independent(kind):
         _assert_result_equal(out[0][b], out[1][b], f"problem {b}")
 
 
-def test_kind_checks():
+def test_sampling_family_kind_checks():
     """The generic batch entry points drive every kind; a kind-specific get_result refuses another kind and a problem
     outside the batch."""
     from mujoco_mpc_b200 import engine as E
@@ -190,7 +190,7 @@ def test_kind_checks():
     H = 11
     batches = {"sampling": E.CppBatchSamplingPlanner(m, 2, 8, H), "ce": E.CppBatchCrossEntropyPlanner(m, 2, 8, H),
                "robust": E.CppBatchRobustPlanner(m, 2, 10, H), "sg": E.CppBatchSampleGradientPlanner(m, 2, 8, H, num_gradient=2)}
-    getters = {"sampling": "mjpc_b200_batch_planner_get_result", "ce": "mjpc_b200_batch_ce_planner_get_result",
+    getters = {"sampling": "mjpc_b200_batch_sampling_planner_get_result", "ce": "mjpc_b200_batch_ce_planner_get_result",
                "robust": "mjpc_b200_batch_robust_planner_get_result", "sg": "mjpc_b200_batch_sg_planner_get_result"}
     for kind, bp in batches.items():
         for b in range(2):
