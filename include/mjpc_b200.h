@@ -270,8 +270,16 @@ int mjpc_b200_step_batch(mjpc_b200_t* h, int B, const float* qpos, const float* 
  * time, are each advanced by one mj_step through the kernel instance mjpc_b200_step_batch runs, and the measurement
  * sensors [sensor_start, sensor_start + nsensor) of each PRE-step state are evaluated after the constraint solve
  * (positions, velocities and touch forces of the state the step starts from, as mj_step's sensor stage sees them).
- * Evaluated: jointpos / jointvel of slide and hinge joints, framepos of a site, body (xipos), xbody (xpos) or geom,
- * touch with a sphere site zone, and accelerometer / velocimeter / gyro of a site (in the site frame).  warmstart [B][nv] may be NULL (zeros); mocap [7 nmocap] is required when
+ * Evaluated: jointpos / jointvel of slide and hinge joints; the frame sensors framepos, framequat, framexaxis /
+ * frameyaxis / framezaxis, framelinvel / frameangvel and framelinacc / frameangacc (world frame, no reference frame) of a
+ * site, body (inertial frame), xbody or geom; subtreecom / subtreelinvel / subtreeangmom of a body; touch with a sphere
+ * site zone; accelerometer / velocimeter / gyro of a site (in the site frame); ballquat / ballangvel of a ball joint;
+ * jointactuatorfrc of a slide or hinge joint; actuatorpos / actuatorvel (joint or fixed-tendon transmission) and
+ * actuatorfrc; tendonpos / tendonvel of a fixed tendon.  Not evaluated (MJPC_B200_ERR_UNSUPPORTED, the last error
+ * naming the sensor): user, force, torque, rangefinder, magnetometer, camprojection, limit and constraint force,
+ * energy and clock sensors, touch with another zone, and any sensor with a cutoff.  The same set and refusals hold for
+ * plant_init's sensor range and for the estimators' (unscented_create, kalman_create, batch_estimator_create).
+ * warmstart [B][nv] may be NULL (zeros); mocap [7 nmocap] is required when
  * nmocap > 0.  Outputs: next_states [B][dim_state], sensordata [B][dim] (dim = the range's total sensor dimension),
  * and, when not NULL, qacc [B][nv] and counts [B][4] = {ncon, nefc, solver iterations, warning}, all equal to what
  * mjpc_b200_step_batch returns for the same inputs.  last_kernel_ms times the launch.  A range outside the model's

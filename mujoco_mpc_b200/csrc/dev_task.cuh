@@ -678,12 +678,38 @@ __device__ __noinline__ void k_residual(Ctx& c) {
 // MuJoCo's sensor types the estimators measure (codes of mujoco_mpc_b200/mjcf.py SENS_*).  One row of the handle's
 // sensor table per sensor (built on the host from the blob's sensor_* / site_* entries, never part of the model pack):
 // adr is the sensor's sensordata address, radius the sphere zone of a touch sensor's site.
-enum { SENS_FRAMEPOS = 1, SENS_JOINTPOS = 2, SENS_TOUCH = 3, SENS_JOINTVEL = 9, SENS_ACCELEROMETER = 10,
-       SENS_VELOCIMETER = 11, SENS_GYRO = 12 };
+enum { SENS_FRAMEPOS = 1, SENS_JOINTPOS = 2, SENS_TOUCH = 3, SENS_SUBTREECOM = 4, SENS_SUBTREELINVEL = 5,
+       SENS_FRAMELINVEL = 6, SENS_FRAMEQUAT = 7, SENS_JOINTVEL = 9, SENS_ACCELEROMETER = 10, SENS_VELOCIMETER = 11,
+       SENS_GYRO = 12, SENS_FRAMEANGVEL = 13, SENS_FRAMEXAXIS = 14, SENS_FRAMEYAXIS = 15, SENS_FRAMEZAXIS = 16,
+       SENS_FRAMELINACC = 17, SENS_FRAMEANGACC = 18, SENS_SUBTREEANGMOM = 19, SENS_BALLQUAT = 20,
+       SENS_BALLANGVEL = 21, SENS_JOINTACTUATORFRC = 22, SENS_ACTUATORPOS = 23, SENS_ACTUATORVEL = 24,
+       SENS_ACTUATORFRC = 25, SENS_TENDONPOS = 26, SENS_TENDONVEL = 27 };
 struct DevSensor { int type, objtype, objid, adr; float radius; };
 // sensordata entries of one measured sensor
 __host__ __device__ inline int sensor_dim(int type) {
-  return type == SENS_FRAMEPOS || type == SENS_ACCELEROMETER || type == SENS_VELOCIMETER || type == SENS_GYRO ? 3 : 1;
+  if (type == SENS_FRAMEQUAT || type == SENS_BALLQUAT) return 4;
+  return type == SENS_JOINTPOS || type == SENS_JOINTVEL || type == SENS_TOUCH || type == SENS_JOINTACTUATORFRC ||
+                 type == SENS_ACTUATORPOS || type == SENS_ACTUATORVEL || type == SENS_ACTUATORFRC ||
+                 type == SENS_TENDONPOS || type == SENS_TENDONVEL
+             ? 1 : 3;
+}
+
+// The post-constraint com-based acceleration of a body (mj_rnePostConstraint's cacc, without contact or applied
+// forces), which is additive along the tree: [0, -gravity] + the sum of cdof_dot qvel + cdof qacc over the dofs on the
+// path from the body to the world.  Walked by the calling lane instead of written to cacc.
+template <class SP>
+__device__ __forceinline__ void body_post_acc(Ctx& c, int body, float* a) {
+  auto&& M = SP::model(c);
+  const int *parent = MI(body_parentid), *dofadr = MI(body_dofadr), *dofnum = MI(body_dofnum);
+  const float *cdof = DF(cdof), *cdof_dot = DF(cdof_dot), *qvel = DF(qvel), *qacc = DF(qacc);
+  a[0] = a[1] = a[2] = 0.f;
+  for (int q = 0; q < 3; q++) a[3 + q] = -CM(c).gravity[q];
+  MJPC_ROLL
+  for (int b = body; b > 0; b = parent[b]) {
+    MJPC_ROLL
+    for (int i = dofadr[b]; i < dofadr[b] + dofnum[b]; i++)
+      for (int q = 0; q < 6; q++) a[q] += cdof_dot[6 * i + q] * qvel[i] + cdof[6 * i + q] * qacc[i];
+  }
 }
 
 // Sensors [0, n) of `tab`, written to out[adr - adr0 ..].  Runs after k_forward and before k_euler: positions and
@@ -700,10 +726,27 @@ __host__ __device__ inline int sensor_dim(int type) {
 //                        R' w and R' (v - (site_xpos - subtree_com[root]) x w) with (w, v) = cvel of the site's body
 //                        and R = site_xmat = quat2mat(xquat[body] site_quat) (the device keeps no site_xmat)
 //   accelerometer        the linear acceleration of the site in the site frame (mj_objectAcceleration, flg_local):
-//                        the post-constraint com-based acceleration a of the site's body (mj_rnePostConstraint's cacc,
-//                        which is additive along the tree: [0, -gravity] + sum of cdof_dot qvel + cdof qacc over the
-//                        dofs on the path from the body to the world, walked here by the sensor's lane instead of
-//                        written to cacc), shifted to the site like the velocity, rotated, plus (R' w) x (R' v_site)
+//                        the post-constraint com-based acceleration a of the site's body (body_post_acc), shifted to
+//                        the site like the velocity, rotated, plus (R' w) x (R' v_site)
+// The frame sensors read a frame: a site (site_xpos, xquat[site_body] site_quat), a body's inertial frame (xipos,
+// ximat, xquat body_iquat), an xbody (xpos, xmat, xquat) or a geom (geom_xpos, geom_xmat, xquat[geom_body] geom_quat);
+// p below is the frame's position and b its body.
+//   framequat            the frame's quaternion as listed (not normalised beyond what xquat is)
+//   framex/y/zaxis       column 0 / 1 / 2 of the frame's rotation matrix (site: quat2mat of its quaternion)
+//   framelinvel / -angvel  mj_objectVelocity in the world frame: w = the angular part of cvel[b], and
+//                        v = cvel_lin[b] - (p - subtree_com[root of b]) x w
+//   framelinacc / -angacc  mj_objectAcceleration in the world frame: (alpha, a) = body_post_acc(b) shifted to p the
+//                        same way, a - (p - subtree_com[root]) x alpha, plus w x v on the linear part
+//   subtreecom / subtreelinvel  subtree_com[body] / subtree_linvel[body]
+//   subtreeangmom        the angular momentum of the body's subtree about subtree_com[body], world frame: the sum
+//                        over bodies j of [body, body_subtreeend[body]) of ximat_j diag(body_inertia_j) ximat_j' w_j
+//                        + (xipos_j - subtree_com[body]) x (m_j v_j - m_j subtree_linvel[body]), m_j v_j = body_linvel[j]
+//   ballquat / ballangvel  qpos[jnt_qposadr .. +4] of a ball joint, normalised / qvel[jnt_dofadr .. +3]
+//   jointactuatorfrc     qfrc_actuator[jnt_dofadr] of a slide or hinge joint
+//   actuatorpos / -vel   gear[0] times the transmission's length / velocity: qpos / qvel of a slide or hinge joint,
+//                        or a fixed tendon's sum of wrap_coef qpos[wrap_qposadr] / wrap_coef qvel[wrap_dof]
+//   actuatorfrc          actuator_force[id], after the force limit
+//   tendonpos / -vel     the fixed tendon's length / velocity as above
 template <class SP>
 __device__ __noinline__ void k_sensors(Ctx& c, const DevSensor* __restrict__ tab, int n, int adr0, float* out) {
   auto&& M = SP::model(c);
@@ -754,15 +797,8 @@ __device__ __noinline__ void k_sensors(Ctx& c, const DevSensor* __restrict__ tab
         cross3(t, off, w);
         for (int q = 0; q < 3; q++) vec[q] = cv[3 + q] - t[q];   // the site's linear velocity
         if (S.type == SENS_ACCELEROMETER) {
-          const int *parent = MI(body_parentid), *dofadr = MI(body_dofadr), *dofnum = MI(body_dofnum);
-          const float *cdof = DF(cdof), *cdof_dot = DF(cdof_dot), *qvel = DF(qvel), *qacc = DF(qacc);
-          float a[6] = {0.f, 0.f, 0.f, -CM(c).gravity[0], -CM(c).gravity[1], -CM(c).gravity[2]};
-          MJPC_ROLL
-          for (int b = body; b > 0; b = parent[b]) {
-            MJPC_ROLL
-            for (int i = dofadr[b]; i < dofadr[b] + dofnum[b]; i++)
-              for (int q = 0; q < 6; q++) a[q] += cdof_dot[6 * i + q] * qvel[i] + cdof[6 * i + q] * qacc[i];
-          }
+          float a[6];
+          body_post_acc<SP>(c, body, a);
           float wv[3];
           cross3(wv, w, vec);
           cross3(t, off, a);
@@ -774,9 +810,106 @@ __device__ __noinline__ void k_sensors(Ctx& c, const DevSensor* __restrict__ tab
       quat_mul(qs, DF(xquat) + 4 * body, MF(site_quat) + 4 * S.objid);
       quat2mat(R, qs);
       rot_vec_T(o, R, vec);
+    } else if (S.type == SENS_FRAMEQUAT || S.type == SENS_FRAMEXAXIS || S.type == SENS_FRAMEYAXIS ||
+               S.type == SENS_FRAMEZAXIS) {
+      const int id = S.objid;
+      if (S.type == SENS_FRAMEQUAT) {
+        const float* xq = DF(xquat);
+        if (S.objtype == OBJ_XBODY) for (int q = 0; q < 4; q++) o[q] = xq[4 * id + q];
+        else if (S.objtype == OBJ_BODY) quat_mul(o, xq + 4 * id, MF(body_iquat) + 4 * id);
+        else if (S.objtype == OBJ_GEOM) quat_mul(o, xq + 4 * MI(geom_bodyid)[id], MF(geom_quat) + 4 * id);
+        else quat_mul(o, xq + 4 * MI(site_bodyid)[id], MF(site_quat) + 4 * id);
+      } else {
+        const int col = S.type - SENS_FRAMEXAXIS;
+        float R[9];
+        if (S.objtype == OBJ_SITE) {
+          float qs[4];
+          quat_mul(qs, DF(xquat) + 4 * MI(site_bodyid)[id], MF(site_quat) + 4 * id);
+          quat2mat(R, qs);
+        } else {
+          const float* X = S.objtype == OBJ_GEOM ? DF(geom_xmat) : S.objtype == OBJ_XBODY ? DF(xmat) : DF(ximat);
+          for (int q = 0; q < 9; q++) R[q] = X[9 * id + q];
+        }
+        for (int q = 0; q < 3; q++) o[q] = R[3 * q + col];
+      }
+    } else if (S.type == SENS_FRAMELINVEL || S.type == SENS_FRAMEANGVEL || S.type == SENS_FRAMELINACC ||
+               S.type == SENS_FRAMEANGACC) {
+      const int id = S.objid;
+      const int body = S.objtype == OBJ_SITE ? MI(site_bodyid)[id] : S.objtype == OBJ_GEOM ? MI(geom_bodyid)[id] : id;
+      const float* p = S.objtype == OBJ_SITE ? DF(site_xpos) : S.objtype == OBJ_GEOM ? DF(geom_xpos)
+                       : S.objtype == OBJ_XBODY ? DF(xpos) : DF(xipos);
+      const float* cv = DF(cvel) + 6 * body;
+      const float* com = DF(subtree_com) + 3 * MI(body_rootid)[body];
+      float off[3], t[3], v[3];
+      for (int q = 0; q < 3; q++) off[q] = p[3 * id + q] - com[q];
+      cross3(t, off, cv);
+      for (int q = 0; q < 3; q++) v[q] = cv[3 + q] - t[q];
+      if (S.type == SENS_FRAMEANGVEL) {
+        for (int q = 0; q < 3; q++) o[q] = cv[q];
+      } else if (S.type == SENS_FRAMELINVEL) {
+        for (int q = 0; q < 3; q++) o[q] = v[q];
+      } else {
+        float a[6];
+        body_post_acc<SP>(c, body, a);
+        if (S.type == SENS_FRAMEANGACC) {
+          for (int q = 0; q < 3; q++) o[q] = a[q];
+        } else {
+          float wv[3];
+          cross3(wv, cv, v);
+          cross3(t, off, a);
+          for (int q = 0; q < 3; q++) o[q] = a[3 + q] - t[q] + wv[q];
+        }
+      }
+    } else if (S.type == SENS_SUBTREECOM || S.type == SENS_SUBTREELINVEL) {
+      const float* v = S.type == SENS_SUBTREECOM ? DF(subtree_com) : DF(subtree_linvel);
+      for (int q = 0; q < 3; q++) o[q] = v[3 * S.objid + q];
+    } else if (S.type == SENS_SUBTREEANGMOM) {
+      const int body = S.objid;
+      const float *com = DF(subtree_com) + 3 * body, *slin = DF(subtree_linvel) + 3 * body;
+      const float *mass = MF(body_mass), *inertia = MF(body_inertia), *ximat = DF(ximat), *xipos = DF(xipos),
+                  *blin = DF(body_linvel), *cvel = DF(cvel);
+      float L[3] = {0.f, 0.f, 0.f};
+      MJPC_ROLL
+      for (int j = body; j < MI(body_subtreeend)[body]; j++) {
+        float wl[3], hl[3], h[3], r[3], pr[3], t[3];
+        rot_vec_T(wl, ximat + 9 * j, cvel + 6 * j);
+        for (int q = 0; q < 3; q++) hl[q] = inertia[3 * j + q] * wl[q];
+        rot_vec(h, ximat + 9 * j, hl);
+        for (int q = 0; q < 3; q++) { r[q] = xipos[3 * j + q] - com[q]; pr[q] = blin[3 * j + q] - mass[j] * slin[q]; }
+        cross3(t, r, pr);
+        for (int q = 0; q < 3; q++) L[q] += h[q] + t[q];
+      }
+      for (int q = 0; q < 3; q++) o[q] = L[q];
+    } else if (S.type == SENS_BALLQUAT) {
+      float qb[4];
+      for (int q = 0; q < 4; q++) qb[q] = DF(qpos)[MI(jnt_qposadr)[S.objid] + q];
+      quat_normalize(qb);
+      for (int q = 0; q < 4; q++) o[q] = qb[q];
+    } else if (S.type == SENS_BALLANGVEL) {
+      for (int q = 0; q < 3; q++) o[q] = DF(qvel)[MI(jnt_dofadr)[S.objid] + q];
+    } else if (S.type == SENS_JOINTACTUATORFRC) {
+      o[0] = DF(qfrc_actuator)[MI(jnt_dofadr)[S.objid]];
+    } else if (S.type == SENS_ACTUATORFRC) {
+      o[0] = DF(actuator_force)[S.objid];
+    } else if (S.type == SENS_ACTUATORPOS || S.type == SENS_ACTUATORVEL || S.type == SENS_TENDONPOS ||
+               S.type == SENS_TENDONVEL) {
+      const bool act = S.type == SENS_ACTUATORPOS || S.type == SENS_ACTUATORVEL;
+      const bool vel = S.type == SENS_ACTUATORVEL || S.type == SENS_TENDONVEL;
+      const int id = act ? MI(actuator_trnid)[S.objid] : S.objid;
+      float x = 0.f;
+      if (act && MI(actuator_trntype)[S.objid] != 1) {
+        x = vel ? DF(qvel)[MI(jnt_dofadr)[id]] : DF(qpos)[MI(jnt_qposadr)[id]];
+      } else {
+        const int *adr = vel ? MI(wrap_dof) : MI(wrap_qposadr);
+        const float* v = vel ? DF(qvel) : DF(qpos);
+        MJPC_ROLL
+        for (int w = MI(tendon_adr)[id]; w < MI(tendon_adr)[id] + MI(tendon_num)[id]; w++) x += MF(wrap_coef)[w] * v[adr[w]];
+      }
+      o[0] = act ? MF(actuator_gear)[S.objid] * x : x;
     }
   }
   __syncwarp();
 }
+
 
 }  // namespace mjpc_dev

@@ -221,26 +221,56 @@ void sensor_table(const Blob& b, std::vector<DevSensor>* sensors, std::vector<st
   if (!b.find("nsensor", &dt, &cnt, &off) || !b.find("site_size", &dt, &cnt, &off)) return;
   const std::vector<int> ty = b.ints("sensor_type"), ot = b.ints("sensor_objtype"), oid = b.ints("sensor_objid"),
                          dim = b.ints("sensor_dim"), adr = b.ints("sensor_adr"), st = b.ints("site_type"),
-                         jt = b.ints("jnt_type");
+                         jt = b.ints("jnt_type"), trntype = b.ints("actuator_trntype"),
+                         trnid = b.ints("actuator_trnid");
   const std::vector<double> ss = b.reals("site_size");
   std::vector<double> cutoff(ty.size(), 0.0);
   if (b.find("sensor_cutoff", &dt, &cnt, &off)) cutoff = b.reals("sensor_cutoff");
   const int ns = b.i("nsensor");
+  auto slide_or_hinge = [&](int j) { return jt[j] == JNT_SLIDE || jt[j] == JNT_HINGE; };
   for (int i = 0; i < ns; i++) {
     DevSensor S = {ty[i], ot[i], oid[i], adr[i], 0.f};
     std::string why;
-    if (ty[i] == SENS_JOINTPOS || ty[i] == SENS_JOINTVEL) {
-      if (jt[oid[i]] != JNT_SLIDE && jt[oid[i]] != JNT_HINGE) why = "jointpos / jointvel of a free or ball joint";
-    } else if (ty[i] == SENS_FRAMEPOS) {
-      if (ot[i] < OBJ_BODY || ot[i] > OBJ_SITE) why = "framepos of an unknown object type";
-    } else if (ty[i] == SENS_TOUCH) {
-      if (st[oid[i]] != GEOM_SPHERE) why = "touch zone other than a sphere site";
-      S.radius = (float)ss[3 * oid[i]];
-    } else if (ty[i] == SENS_ACCELEROMETER || ty[i] == SENS_VELOCIMETER || ty[i] == SENS_GYRO) {
-      if (ot[i] != OBJ_SITE) why = "accelerometer / velocimeter / gyro of an object other than a site";
-    } else {
-      why = "sensor type " + std::to_string(ty[i]) +
-            " (only jointpos, jointvel, framepos, touch, accelerometer, velocimeter and gyro are evaluated)";
+    switch (ty[i]) {
+      case SENS_JOINTPOS: case SENS_JOINTVEL:
+        if (!slide_or_hinge(oid[i])) why = "jointpos / jointvel of a free or ball joint";
+        break;
+      case SENS_FRAMEPOS:
+        if (ot[i] < OBJ_BODY || ot[i] > OBJ_SITE) why = "framepos of an unknown object type";
+        break;
+      case SENS_FRAMEQUAT: case SENS_FRAMEXAXIS: case SENS_FRAMEYAXIS: case SENS_FRAMEZAXIS: case SENS_FRAMELINVEL:
+      case SENS_FRAMEANGVEL: case SENS_FRAMELINACC: case SENS_FRAMEANGACC:
+        if (ot[i] < OBJ_BODY || ot[i] > OBJ_SITE) why = "frame sensor of an object other than a body, xbody, geom or site";
+        break;
+      case SENS_TOUCH:
+        if (st[oid[i]] != GEOM_SPHERE) why = "touch zone other than a sphere site";
+        S.radius = (float)ss[3 * oid[i]];
+        break;
+      case SENS_ACCELEROMETER: case SENS_VELOCIMETER: case SENS_GYRO:
+        if (ot[i] != OBJ_SITE) why = "accelerometer / velocimeter / gyro of an object other than a site";
+        break;
+      case SENS_SUBTREECOM: case SENS_SUBTREELINVEL: case SENS_SUBTREEANGMOM:
+        if (ot[i] != OBJ_BODY) why = "subtree sensor of an object other than a body";
+        break;
+      case SENS_BALLQUAT: case SENS_BALLANGVEL:
+        if (jt[oid[i]] != JNT_BALL) why = "ballquat / ballangvel of a joint other than a ball joint";
+        break;
+      case SENS_JOINTACTUATORFRC:
+        if (!slide_or_hinge(oid[i])) why = "jointactuatorfrc of a free or ball joint";
+        break;
+      case SENS_ACTUATORPOS: case SENS_ACTUATORVEL:
+        // mjTRN_JOINT (0) on a slide or hinge joint, or mjTRN_TENDON (1): every tendon of the model is fixed
+        if (!(trntype[oid[i]] == 1 || (trntype[oid[i]] == 0 && slide_or_hinge(trnid[oid[i]]))))
+          why = "actuatorpos / actuatorvel of a transmission other than a slide or hinge joint or a fixed tendon";
+        break;
+      case SENS_ACTUATORFRC: case SENS_TENDONPOS: case SENS_TENDONVEL:
+        break;
+      default:
+        why = "sensor type " + std::to_string(ty[i]) +
+              " (only jointpos, jointvel, framepos, framequat, framexaxis, frameyaxis, framezaxis, framelinvel, "
+              "frameangvel, framelinacc, frameangacc, subtreecom, subtreelinvel, subtreeangmom, touch, accelerometer, "
+              "velocimeter, gyro, ballquat, ballangvel, jointactuatorfrc, actuatorpos, actuatorvel, actuatorfrc, "
+              "tendonpos and tendonvel are evaluated)";
     }
     if (why.empty() && dim[i] != sensor_dim(ty[i])) why = "unexpected sensor dimension";
     if (why.empty() && cutoff[i] != 0.0) why = "cutoff is not modelled";

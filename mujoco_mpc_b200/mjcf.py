@@ -33,18 +33,30 @@ JNT_TYPES = {"free": 0, "ball": 1, "slide": 2, "hinge": 3}
 SENS_USER, SENS_FRAMEPOS, SENS_JOINTPOS, SENS_TOUCH, SENS_SUBTREECOM, SENS_SUBTREELINVEL, \
     SENS_FRAMELINVEL, SENS_FRAMEQUAT, SENS_OTHER, SENS_JOINTVEL, SENS_ACCELEROMETER, SENS_VELOCIMETER, \
     SENS_GYRO = range(13)
+# appended after the codes above, which do not move (SENS_OTHER stays the code of every tag not listed here)
+SENS_FRAMEANGVEL, SENS_FRAMEXAXIS, SENS_FRAMEYAXIS, SENS_FRAMEZAXIS, SENS_FRAMELINACC, SENS_FRAMEANGACC, \
+    SENS_SUBTREEANGMOM, SENS_BALLQUAT, SENS_BALLANGVEL, SENS_JOINTACTUATORFRC, SENS_ACTUATORPOS, SENS_ACTUATORVEL, \
+    SENS_ACTUATORFRC, SENS_TENDONPOS, SENS_TENDONVEL = range(13, 28)
 SENS_TYPES = {"user": 0, "framepos": 1, "jointpos": 2, "touch": 3, "subtreecom": 4,
               "subtreelinvel": 5, "framelinvel": 6, "framequat": 7, "jointvel": 9, "accelerometer": 10,
-              "velocimeter": 11, "gyro": 12}
+              "velocimeter": 11, "gyro": 12, "frameangvel": 13, "framexaxis": 14, "frameyaxis": 15,
+              "framezaxis": 16, "framelinacc": 17, "frameangacc": 18, "subtreeangmom": 19, "ballquat": 20,
+              "ballangvel": 21, "jointactuatorfrc": 22, "actuatorpos": 23, "actuatorvel": 24, "actuatorfrc": 25,
+              "tendonpos": 26, "tendonvel": 27}
 # what the measurement path (engine step_sensors, estimators) evaluates
-SENS_MEASURED = (SENS_FRAMEPOS, SENS_JOINTPOS, SENS_TOUCH, SENS_JOINTVEL, SENS_ACCELEROMETER, SENS_VELOCIMETER,
-                 SENS_GYRO)
+SENS_MEASURED = (SENS_FRAMEPOS, SENS_JOINTPOS, SENS_TOUCH, SENS_SUBTREECOM, SENS_SUBTREELINVEL, SENS_FRAMELINVEL,
+                 SENS_FRAMEQUAT, SENS_JOINTVEL, SENS_ACCELEROMETER, SENS_VELOCIMETER, SENS_GYRO) + tuple(range(13, 28))
 # the IMU sensors: 3-vectors in the frame of their site
 SENS_IMU = (SENS_ACCELEROMETER, SENS_VELOCIMETER, SENS_GYRO)
+# the frame sensors: objtype / objname name a body (inertial frame), an xbody, a geom or a site
+SENS_FRAME_TAGS = ("framepos", "framequat", "framexaxis", "frameyaxis", "framezaxis", "framelinvel", "frameangvel",
+                   "framelinacc", "frameangacc")
 SENS_DIM = {"framepos": 3, "jointpos": 1, "touch": 1, "subtreecom": 3, "subtreelinvel": 3,
             "framelinvel": 3, "framequat": 4, "jointvel": 1, "frameangvel": 3, "subtreeangmom": 3,
             "actuatorfrc": 1, "framexaxis": 3, "frameyaxis": 3, "framezaxis": 3, "velocimeter": 3,
-            "gyro": 3, "accelerometer": 3, "actuatorpos": 1, "actuatorvel": 1, "tendonpos": 1}
+            "gyro": 3, "accelerometer": 3, "actuatorpos": 1, "actuatorvel": 1, "tendonpos": 1,
+            "tendonvel": 1, "framelinacc": 3, "frameangacc": 3, "ballquat": 4, "ballangvel": 3,
+            "jointactuatorfrc": 1}
 OBJ_BODY, OBJ_XBODY, OBJ_GEOM, OBJ_SITE = range(4)
 
 MINVAL = 1e-15
@@ -711,9 +723,16 @@ class Compiler:
             s_dim[i], s_adr[i] = dim, adr
             adr += dim
             users.append(_f(ch.get("user"), default=[]) if ch.get("user") else np.zeros(0))
-            if tag in ("framepos", "framelinvel", "framequat"):
+            if tag in SENS_FRAME_TAGS:
                 ot = ch.get("objtype")
                 nm = ch.get("objname")
+                # neither the oracle nor the kernels implement a reference frame or a camera frame: refused here
+                # rather than read as a world-frame body sensor
+                if ch.get("reftype") is not None or ch.get("refname") is not None:
+                    raise ValueError("sensor %d (%s): frame sensors with reftype / refname are not supported"
+                                     % (i, tag))
+                if ot == "camera":
+                    raise ValueError("sensor %d (%s): frame sensors of a camera are not supported" % (i, tag))
                 if ot == "site":
                     s_objtype[i], s_objid[i] = OBJ_SITE, m.site_names.index(nm)
                 elif ot == "geom":
@@ -721,10 +740,14 @@ class Compiler:
                 else:
                     s_objtype[i] = OBJ_XBODY if ot == "xbody" else OBJ_BODY
                     s_objid[i] = m.body_names.index(nm)
-            elif tag in ("subtreecom", "subtreelinvel"):
+            elif tag in ("subtreecom", "subtreelinvel", "subtreeangmom"):
                 s_objtype[i], s_objid[i] = OBJ_BODY, m.body_names.index(ch.get("body"))
-            elif tag in ("jointpos", "jointvel"):
+            elif tag in ("jointpos", "jointvel", "ballquat", "ballangvel", "jointactuatorfrc"):
                 s_objid[i] = m.jnt_names.index(ch.get("joint"))
+            elif tag in ("actuatorpos", "actuatorvel", "actuatorfrc"):
+                s_objid[i] = m.actuator_names.index(ch.get("actuator"))
+            elif tag in ("tendonpos", "tendonvel"):
+                s_objid[i] = m.tendon_names.index(ch.get("tendon"))
             elif tag in ("touch", "accelerometer", "velocimeter", "gyro"):
                 s_objtype[i], s_objid[i] = OBJ_SITE, m.site_names.index(ch.get("site"))
             cutoff[i] = float(ch.get("cutoff", 0))

@@ -16,6 +16,22 @@
 //                        acceleration (mj_rnePostConstraint's recursion cacc[b] = cacc[parent] + cdof_dot qvel +
 //                        cdof qacc from cacc[world] = (0, -gravity)), moved and rotated like the velocity, plus
 //                        (R' w) x (R' v_site)
+// A frame is a site (site_xpos, site_xmat, xquat[site_body] site_quat), a body's inertial frame (xipos, ximat,
+// xquat body_iquat), an xbody (xpos, xmat, xquat) or a geom (geom_xpos, geom_xmat, xquat[geom_body] geom_quat):
+//   framequat            the frame's quaternion as listed
+//   framex/y/zaxis       column 0 / 1 / 2 of the frame's matrix
+//   framelinvel / -angvel  mj_objectVelocity in the world frame: cvel of the frame's body moved to the frame's position
+//   framelinacc / -angacc  mj_objectAcceleration in the world frame: the post-constraint cacc moved the same way, plus
+//                        w x v_frame on the linear part
+//   subtreecom / subtreelinvel  subtree_com / subtree_linvel of the body
+//   subtreeangmom        sum over the body's descendants j (and itself) of the spin ximat_j diag(I_j) ximat_j' w_j and
+//                        the orbital part (xipos_j - subtree_com) x m_j (v_j - subtree_linvel), with v_j the velocity
+//                        of j's centre of mass
+//   ballquat / ballangvel  the ball joint's normalised quaternion / its 3 dof velocities
+//   jointactuatorfrc     qfrc_actuator of a slide or hinge joint's dof
+//   actuatorpos / -vel   gear times the joint's qpos / qvel, or times the fixed tendon's length / velocity
+//   actuatorfrc          actuator_force (after the force limit)
+//   tendonpos / -vel     the fixed tendon's sum coef qpos / sum coef qvel
 // The sensor table is read from the blob's sensor_* / site_* entries.  Written from the definition, independently of
 // the device's k_sensors; the oracle itself is not modified.
 #include <cmath>
@@ -30,8 +46,12 @@ using namespace oracle;
 
 namespace {
 
-enum { SENS_FRAMEPOS = 1, SENS_JOINTPOS = 2, SENS_TOUCH = 3, SENS_JOINTVEL = 9, SENS_ACCELEROMETER = 10,
-       SENS_VELOCIMETER = 11, SENS_GYRO = 12 };
+enum { SENS_FRAMEPOS = 1, SENS_JOINTPOS = 2, SENS_TOUCH = 3, SENS_SUBTREECOM = 4, SENS_SUBTREELINVEL = 5,
+       SENS_FRAMELINVEL = 6, SENS_FRAMEQUAT = 7, SENS_JOINTVEL = 9, SENS_ACCELEROMETER = 10, SENS_VELOCIMETER = 11,
+       SENS_GYRO = 12, SENS_FRAMEANGVEL = 13, SENS_FRAMEXAXIS = 14, SENS_FRAMEYAXIS = 15, SENS_FRAMEZAXIS = 16,
+       SENS_FRAMELINACC = 17, SENS_FRAMEANGACC = 18, SENS_SUBTREEANGMOM = 19, SENS_BALLQUAT = 20,
+       SENS_BALLANGVEL = 21, SENS_JOINTACTUATORFRC = 22, SENS_ACTUATORPOS = 23, SENS_ACTUATORVEL = 24,
+       SENS_ACTUATORFRC = 25, SENS_TENDONPOS = 26, SENS_TENDONVEL = 27 };
 enum { OBJ_BODY = 0, OBJ_XBODY = 1, OBJ_GEOM = 2, OBJ_SITE = 3 };
 
 struct Table {
@@ -118,6 +138,92 @@ std::vector<double> post_constraint_acc(const Model<T>& m, const Data<T>& d) {
   return cacc;
 }
 
+void qmul(double* r, const double* a, const double* b) {
+  r[0] = a[0] * b[0] - a[1] * b[1] - a[2] * b[2] - a[3] * b[3];
+  r[1] = a[0] * b[1] + a[1] * b[0] + a[2] * b[3] - a[3] * b[2];
+  r[2] = a[0] * b[2] - a[1] * b[3] + a[2] * b[0] + a[3] * b[1];
+  r[3] = a[0] * b[3] + a[1] * b[2] - a[2] * b[1] + a[3] * b[0];
+}
+
+void cross(double* r, const double* a, const double* b) {
+  r[0] = a[1] * b[2] - a[2] * b[1];
+  r[1] = a[2] * b[0] - a[0] * b[2];
+  r[2] = a[0] * b[1] - a[1] * b[0];
+}
+
+// a frame sensor's object: position, rotation matrix (row-major), quaternion, and the body it moves with
+struct Frame {
+  double p[3], R[9], q[4];
+  int body;
+};
+
+template <class T>
+Frame frame(const Model<T>& m, const Data<T>& d, int objtype, int id) {
+  Frame f;
+  const T *p, *R, *local = nullptr;
+  switch (objtype) {
+    case OBJ_SITE: f.body = m.site_bodyid[id]; p = &d.site_xpos[3 * id]; R = &d.site_xmat[9 * id]; local = &m.site_quat[4 * id]; break;
+    case OBJ_GEOM: f.body = m.geom_bodyid[id]; p = &d.geom_xpos[3 * id]; R = &d.geom_xmat[9 * id]; local = &m.geom_quat[4 * id]; break;
+    case OBJ_XBODY: f.body = id; p = &d.xpos[3 * id]; R = &d.xmat[9 * id]; break;
+    case OBJ_BODY: f.body = id; p = &d.xipos[3 * id]; R = &d.ximat[9 * id]; local = &m.body_iquat[4 * id]; break;
+    default: throw std::runtime_error("frame sensor of an unknown object type");
+  }
+  double xq[4], lq[4];
+  for (int q = 0; q < 4; q++) xq[q] = d.xquat[4 * f.body + q];
+  for (int q = 0; q < 3; q++) f.p[q] = p[q];
+  for (int q = 0; q < 9; q++) f.R[q] = R[q];
+  if (local) {
+    for (int q = 0; q < 4; q++) lq[q] = local[q];
+    qmul(f.q, xq, lq);
+  } else {
+    for (int q = 0; q < 4; q++) f.q[q] = xq[q];
+  }
+  return f;
+}
+
+// the world-frame angular and linear velocity (w, v) of the point p moving with body b (mj_objectVelocity)
+template <class T>
+void point_velocity(const Model<T>& m, const Data<T>& d, int b, const double* p, double* w, double* v) {
+  double off[3], t[3];
+  for (int q = 0; q < 3; q++) { w[q] = d.cvel[6 * b + q]; off[q] = p[q] - (double)d.subtree_com[3 * m.body_rootid[b] + q]; }
+  cross(t, off, w);
+  for (int q = 0; q < 3; q++) v[q] = (double)d.cvel[6 * b + 3 + q] - t[q];
+}
+
+// a fixed tendon's length (vel false) or velocity
+template <class T>
+double tendon(const Model<T>& m, const Data<T>& d, int t, bool vel) {
+  double x = 0;
+  for (int w = m.tendon_adr[t]; w < m.tendon_adr[t] + m.tendon_num[t]; w++)
+    x += (double)m.wrap_coef[w] * (vel ? (double)d.qvel[m.wrap_dof[w]] : (double)d.qpos[m.wrap_qposadr[w]]);
+  return x;
+}
+
+template <class T>
+void subtree_angmom(const Model<T>& m, const Data<T>& d, int body, double* L) {
+  const T *com = &d.subtree_com[3 * body], *slin = &d.subtree_linvel[3 * body];
+  L[0] = L[1] = L[2] = 0;
+  for (int j = body; j < m.nbody; j++) {
+    int k = j;
+    while (k > body) k = m.body_parentid[k];
+    if (k != body) continue;   // not a descendant
+    double p[3], w[3], v[3], wl[3] = {0, 0, 0}, r[3], mv[3], t[3];
+    for (int q = 0; q < 3; q++) p[q] = d.xipos[3 * j + q];
+    point_velocity(m, d, j, p, w, v);
+    const T* R = &d.ximat[9 * j];
+    for (int a = 0; a < 3; a++)
+      for (int q = 0; q < 3; q++) wl[a] += (double)R[3 * q + a] * w[q];
+    for (int a = 0; a < 3; a++) wl[a] *= (double)m.body_inertia[3 * j + a];
+    for (int q = 0; q < 3; q++) {
+      for (int a = 0; a < 3; a++) L[q] += (double)R[3 * q + a] * wl[a];
+      r[q] = p[q] - (double)com[q];
+      mv[q] = (double)m.body_mass[j] * (v[q] - (double)slin[q]);
+    }
+    cross(t, r, mv);
+    for (int q = 0; q < 3; q++) L[q] += t[q];
+  }
+}
+
 template <class T>
 void sensors(const Model<T>& m, const Data<T>& d, const Table& tab, int start, int count, double* out) {
   const int adr0 = tab.adr[start];
@@ -151,6 +257,59 @@ void sensors(const Model<T>& m, const Data<T>& d, const Table& tab, int start, i
         o[2] = a[5] + v[0] * v[4] - v[1] * v[3];
         break;
       }
+      case SENS_FRAMEQUAT: case SENS_FRAMEXAXIS: case SENS_FRAMEYAXIS: case SENS_FRAMEZAXIS: {
+        const Frame f = frame(m, d, tab.objtype[s], id);
+        if (tab.type[s] == SENS_FRAMEQUAT) { for (int q = 0; q < 4; q++) o[q] = f.q[q]; break; }
+        const int col = tab.type[s] - SENS_FRAMEXAXIS;
+        for (int q = 0; q < 3; q++) o[q] = f.R[3 * q + col];
+        break;
+      }
+      case SENS_FRAMELINVEL: case SENS_FRAMEANGVEL: case SENS_FRAMELINACC: case SENS_FRAMEANGACC: {
+        const Frame f = frame(m, d, tab.objtype[s], id);
+        double w[3], v[3];
+        point_velocity(m, d, f.body, f.p, w, v);
+        if (tab.type[s] == SENS_FRAMEANGVEL) { for (int q = 0; q < 3; q++) o[q] = w[q]; break; }
+        if (tab.type[s] == SENS_FRAMELINVEL) { for (int q = 0; q < 3; q++) o[q] = v[q]; break; }
+        if (cacc.empty()) cacc = post_constraint_acc(m, d);
+        const double* a = &cacc[6 * (size_t)f.body];
+        if (tab.type[s] == SENS_FRAMEANGACC) { for (int q = 0; q < 3; q++) o[q] = a[q]; break; }
+        double off[3], t[3], wv[3];
+        for (int q = 0; q < 3; q++) off[q] = f.p[q] - (double)d.subtree_com[3 * m.body_rootid[f.body] + q];
+        cross(t, off, a);
+        cross(wv, w, v);
+        for (int q = 0; q < 3; q++) o[q] = a[3 + q] - t[q] + wv[q];
+        break;
+      }
+      case SENS_SUBTREECOM: for (int q = 0; q < 3; q++) o[q] = d.subtree_com[3 * id + q]; break;
+      case SENS_SUBTREELINVEL: for (int q = 0; q < 3; q++) o[q] = d.subtree_linvel[3 * id + q]; break;
+      case SENS_SUBTREEANGMOM: subtree_angmom(m, d, id, o); break;
+      case SENS_BALLQUAT: {
+        if (m.jnt_type[id] != 1) throw std::runtime_error("ballquat of a joint other than a ball joint");
+        const int a = m.jnt_qposadr[id];
+        double n = 0;
+        for (int q = 0; q < 4; q++) n += (double)d.qpos[a + q] * (double)d.qpos[a + q];
+        n = std::sqrt(n);
+        for (int q = 0; q < 4; q++) o[q] = d.qpos[a + q] / n;
+        break;
+      }
+      case SENS_BALLANGVEL:
+        if (m.jnt_type[id] != 1) throw std::runtime_error("ballangvel of a joint other than a ball joint");
+        for (int q = 0; q < 3; q++) o[q] = d.qvel[m.jnt_dofadr[id] + q];
+        break;
+      case SENS_JOINTACTUATORFRC: o[0] = d.qfrc_actuator[m.jnt_dofadr[id]]; break;
+      case SENS_ACTUATORFRC: o[0] = d.actuator_force[id]; break;
+      case SENS_ACTUATORPOS: case SENS_ACTUATORVEL: {
+        const bool vel = tab.type[s] == SENS_ACTUATORVEL;
+        const int j = m.actuator_trnid[id];
+        double x;
+        if (m.actuator_trntype[id] == 1) x = tendon(m, d, j, vel);
+        else if (m.actuator_trntype[id] == 0) x = vel ? (double)d.qvel[m.jnt_dofadr[j]] : (double)d.qpos[m.jnt_qposadr[j]];
+        else throw std::runtime_error("actuator transmission not evaluated");
+        o[0] = (double)m.actuator_gear[id] * x;
+        break;
+      }
+      case SENS_TENDONPOS: o[0] = tendon(m, d, id, false); break;
+      case SENS_TENDONVEL: o[0] = tendon(m, d, id, true); break;
       default: throw std::runtime_error("sensor type not evaluated");
     }
   }
