@@ -548,7 +548,7 @@ def shadow_reorient_xml(horizon=0.25, trajectories=60) -> str:
     The reference includes Menagerie's shadow_hand/right_hand.xml with its mesh assets (CMakeLists.txt fetches them at
     configure time; not vendored, not available offline), so the hand below is a primitive-geom stand-in [GUESS: every
     hand length, mass, joint range and gain]: the same kinematic layout and order - 2 wrist + 4 + 4 + 4 + 5 (little)
-    + 5 (thumb) = 24 hinges, 20 position actuators of which five act on fixed tendons coupling the two distal joints
+    + 5 (thumb) = 24 hinges, 20 position actuators of which four act on fixed tendons coupling the two distal joints
     (rh_*J0 = J2 + J1), a grasp_site on the palm - so nq / nv / nu = 35 / 33 / 20 and the qpos layout the residual's
     literal `qpos + 7` / `qvel + 6` offsets assume.  What IS the reference's: the goal body and the cube
     (common_assets/reorientation_cube.xml + cube.xml.patch), the cost terms, the custom numerics, the 35-value grasp
