@@ -164,6 +164,37 @@ int mjpc_b200_set_model_variants(mjpc_b200_t* h, const mjpc_model_blob* models, 
  * Without variants there is nothing to select: returns 0 and changes nothing. */
 int mjpc_b200_select_model_variants(mjpc_b200_t* h, const int* index, int B);
 
+/* A model ensemble: every spline launch of this handle (rollout_spline, rollout_spline_batched, upload_spline_inputs +
+ * launch_resident) scores each candidate on K member models.  Candidate i of problem b is rolled out once per member,
+ * and its return is the mean of its `worst` largest member returns (worst = K: the expected return; worst = 1: the
+ * worst case): the member returns sorted in descending order (ties to the lower member), the first `worst` summed left
+ * to right in double, divided once by worst and rounded to float.  If any member fails, the candidate fails and its
+ * return is exactly 1e6.  returns, failure and order of the launch describe these scores ([B][N], order ranks them), and
+ * fetch_trajectory / fetch_all (flat index b*N + i) return member 0's trajectories; fetch_stats returns the rows of
+ * every launched trajectory [B][K][N].
+ *   Members follow the rule of set_model_variants, with its error naming the member and the first field that differs;
+ *   set_task rewrites every member's task.  1 <= K <= 32 and 1 <= worst <= K, else MJPC_B200_ERR_BAD_ARGUMENT; the
+ *   handle is unchanged on any refusal.  K = 0 (or models NULL) clears the ensemble.
+ *   The launch holds B*K*N trajectories (member k of problem b is launch problem b*K + k); B*N is still bounded by
+ *   max_candidates: the call grows the per-trajectory device buffers to K x max_candidates (never shrinks them;
+ *   MJPC_B200_ERR_CUDA, handle unchanged, if that fails).
+ *   While an ensemble is set, set_model_variants (count > 0), rollout_feedback*, model_derivatives*, gradient_batched,
+ *   rollout_spline_sharded, step_debug*, step_batch, step_sensors, the plant calls, a filter bank's update and a spline
+ *   launch with force noise (set_xfrc_noise*) return MJPC_B200_ERR_UNSUPPORTED naming the call; set_model_ensemble
+ *   while variants are set likewise. */
+int mjpc_b200_set_model_ensemble(mjpc_b200_t* h, const mjpc_model_blob* models, int K, int worst);
+/* The member returns [B][K][N] and failure flags [B][K][N] of the last launch, an ensemble launch (either may be
+ * NULL); MJPC_B200_ERR_BAD_ARGUMENT after any other launch. */
+int mjpc_b200_fetch_ensemble(mjpc_b200_t* h, float* member_returns, uint8_t* member_failure);
+/* Candidate (flat b*N + i) of the last launch as member `member` rolled it out (fetch_trajectory's arrays);
+ * fetch_trajectory is member 0.  After a launch without an ensemble only member 0 exists. */
+int mjpc_b200_fetch_trajectory_member(mjpc_b200_t* h, int candidate, int member, float* states, float* actions,
+                                      double* times, float* residual, float* costs, float* trace);
+/* The score of one candidate from its K member returns [K] and failure flags [K] on the host, bit for bit what the
+ * device computes (for tests).  Nothing is written unless 1 <= K <= 32 and 1 <= worst <= K. */
+void mjpc_b200_host_ensemble_score(const float* member_returns, const uint8_t* member_failure, int K, int worst,
+                                   float* score, uint8_t* failure);
+
 /* K line-search rollouts of the iLQG policy. u_nom [H][nu], x_nom [H][dim_state], t_nom [H] (absolute),
  * gains [H][nu][dim_dstate], du [H][nu] (may be NULL), step_sizes [K]. */
 int mjpc_b200_rollout_feedback(mjpc_b200_t* h, const float* state, double time, const float* mocap,
@@ -519,6 +550,11 @@ int mjpc_b200_planner_nominal_trajectory(mjpc_b200_planner_t* p, int horizon);
 int mjpc_b200_planner_action_from_policy(mjpc_b200_planner_t* p, double* action, const double* state, double time,
                                          int use_previous);
 int mjpc_b200_planner_set_fd(mjpc_b200_planner_t* p, double tolerance, int mode, int derivative_skip);
+/* Plan on a model ensemble: mjpc_b200_set_model_ensemble on the planner's handle, with its rule and refusals (K = 0 or
+ * models NULL clears it).  The planner ranks by the scores; returns and improvement of its get_result are scores, and
+ * the best trajectory is member 0's trajectory of the winner with the winner's score as its return.  Sampling,
+ * Cross-Entropy and Sample Gradient; Robust, Gradient, iLQG and iLQS return MJPC_B200_ERR_UNSUPPORTED. */
+int mjpc_b200_planner_set_ensemble(mjpc_b200_planner_t* p, const mjpc_model_blob* models, int K, int worst);
 /* mjpc_b200_set_task on every engine handle the planner plans on (the task snapshot Agent gives it per iteration) */
 int mjpc_b200_planner_set_task(mjpc_b200_planner_t* p, const mjpc_task_desc* task);
 
@@ -672,7 +708,9 @@ int mjpc_b200_ilqs_planner_get_result(mjpc_b200_planner_t* p, double* scalars);
  *   action_from_policy  mjpc_b200_planner_action_from_policy of one problem: state (may be NULL) is read by the iLQG
  *                       policy (iLQG, iLQS)
  *   set_fd              mjpc_b200_planner_set_fd of every problem: Gradient, iLQG and iLQS; the others return
- *                       MJPC_B200_ERR_UNSUPPORTED */
+ *                       MJPC_B200_ERR_UNSUPPORTED
+ *   set_ensemble        every problem plans on the same model ensemble: mjpc_b200_planner_set_ensemble's kinds and
+ *                       refusals, on the batch's handle */
 typedef struct mjpc_b200_batch_planner mjpc_b200_batch_planner_t;
 void mjpc_b200_batch_planner_destroy(mjpc_b200_batch_planner_t* p);
 int mjpc_b200_batch_planner_reset(mjpc_b200_batch_planner_t* p, int problem, int horizon,
@@ -686,6 +724,7 @@ int mjpc_b200_batch_planner_optimize_policy(mjpc_b200_batch_planner_t* p, int ho
 int mjpc_b200_batch_planner_action_from_policy(mjpc_b200_batch_planner_t* p, int problem, double* action,
                                                const double* state, double time, int use_previous);
 int mjpc_b200_batch_planner_set_fd(mjpc_b200_batch_planner_t* p, double tolerance, int mode, int derivative_skip);
+int mjpc_b200_batch_planner_set_ensemble(mjpc_b200_batch_planner_t* p, const mjpc_model_blob* models, int K, int worst);
 
 /* Predictive Sampling: one mjpc_b200_rollout_spline_batched launch of B x N per iteration. */
 int mjpc_b200_batch_sampling_planner_create(const mjpc_model_blob* model, int num_problems, int num_trajectory,

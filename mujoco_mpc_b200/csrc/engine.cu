@@ -161,6 +161,17 @@ struct mjpc_b200 {
   float* d_variants = nullptr;
   int* d_variant_index = nullptr;
   int nvariants = 0, variant_stride = 0, nselected = 0;
+  // model ensemble (set_model_ensemble): the member blocks [nmembers][member_stride], laid out as the variant blocks;
+  // the member of every launch problem, d_member_index [traj_factor x max_candidates] (problem j on member j % nmembers);
+  // the members' returns and failure flags [B][K][N] of an ensemble launch.  The per-trajectory buffers hold
+  // traj_factor x max_candidates trajectories (grown by set_model_ensemble, never shrunk).
+  float* d_members = nullptr;
+  int* d_member_index = nullptr;
+  float* d_member_returns = nullptr;
+  unsigned char* d_member_failure = nullptr;
+  int nmembers = 0, member_stride = 0, worst = 0, traj_factor = 1;
+  // the members of the resident and of the last launch (0: not an ensemble launch), and the last launch's N per problem
+  int resident_members = 0, last_members = 0, last_nper = 0;
   // resident-input launch description
   RolloutArgs resident;
   bool resident_ok = false;
@@ -192,6 +203,9 @@ int upload_task(mjpc_b200* h) {
   for (int v = 0; v < h->nvariants; v++)
     CUDA_TRY(cudaMemcpyAsync(h->d_variants + (size_t)v * h->variant_stride + t0, f.data() + t0, nt * 4,
                              cudaMemcpyHostToDevice, h->stream));
+  for (int k = 0; k < h->nmembers; k++)
+    CUDA_TRY(cudaMemcpyAsync(h->d_members + (size_t)k * h->member_stride + t0, f.data() + t0, nt * 4,
+                             cudaMemcpyHostToDevice, h->stream));
   CUDA_TRY(cudaStreamSynchronize(h->stream));  // f is pageable
   return 0;
 }
@@ -212,6 +226,13 @@ int check_variants(const mjpc_b200* h, int B, const char* call) {
     return fail(MJPC_B200_ERR_BAD_ARGUMENT, std::string(call) + ": the launch has " + std::to_string(B) +
                                                 " problems, the model variants are for " + std::to_string(h->nselected));
   return 0;
+}
+
+// With a model ensemble set, only the spline launches score on it: every other call that runs the model is refused
+int check_ensemble(const mjpc_b200* h, const char* call) {
+  if (!h->nmembers) return 0;
+  return fail(MJPC_B200_ERR_UNSUPPORTED,
+              std::string(call) + ": not available while a model ensemble is set (set_model_ensemble)");
 }
 
 // The measurement-sensor table of a blob: one row per model sensor; why[i] is empty when sensor i is one the device
@@ -373,10 +394,11 @@ void build_policy_intervals(const double* nodes, int count, double time0, double
 // (the knot times of a spline launch, the nominal times of a feedback launch).  A NULL task_states / weights /
 // parameters stands for the handle's set_task values; the time-like task-state entries and the knot times are made
 // relative to each problem's own start time.  *end: the first h_in float after the block.  Per-problem noise keys for
-// another number of problems are refused before anything is staged.
+// another number of problems are refused before anything is staged.  R > 1 (a model ensemble of R members) stages
+// each problem R times: launch problem b R + k holds problem b's inputs.
 int stage_problems(mjpc_b200* h, int B, const float* states, const double* times, const float* mocaps,
                    const double* weights, const double* parameters, const double* task_states, const double* nodes,
-                   int count, int H, const float* knots, int N, RolloutArgs* A, size_t* end) {
+                   int count, int H, const float* knots, int N, RolloutArgs* A, size_t* end, int R = 1) {
   if (int rc = check_variants(h, B, "rollout")) return rc;
   if (!h->noise_seeds.empty() && (int)h->noise_seeds.size() != B)
     return fail(MJPC_B200_ERR_BAD_ARGUMENT, "rollout: set_xfrc_noise_batched gave keys for " +
@@ -384,32 +406,37 @@ int stage_problems(mjpc_b200* h, int B, const float* states, const double* times
                                                 std::to_string(B));
   const DevModel& M = h->pack.M;
   const size_t ds = M.nq + M.nv, nm = 7 * (size_t)M.nmocap, nts = M.task_state_size, nw = M.num_term,
-               np = M.num_parameters;
+               np = M.num_parameters, nk = (size_t)N * count * M.nu;
+  const int BR = B * R;
   float* in = h->h_in;
   PolicyInterval* iv = reinterpret_cast<PolicyInterval*>(in);
-  for (int b = 0; b < B; b++)
-    build_policy_intervals(nodes + (size_t)b * count, count, times[b], h->pack.timestep, H, iv + (size_t)b * H);
-  size_t o = 4 * (size_t)B * H;
-  const size_t o_state = o; std::memcpy(in + o, states, B * ds * 4); o += B * ds;
-  const size_t o_mocap = o; if (nm) std::memcpy(in + o, mocaps, B * nm * 4); o += B * nm;
+  for (int j = 0; j < BR; j++)
+    build_policy_intervals(nodes + (size_t)(j / R) * count, count, times[j / R], h->pack.timestep, H, iv + (size_t)j * H);
+  size_t o = 4 * (size_t)BR * H;
+  const size_t o_state = o;
+  for (int j = 0; j < BR; j++, o += ds) std::memcpy(in + o, states + (j / R) * ds, ds * 4);
+  const size_t o_mocap = o;
+  if (nm) for (int j = 0; j < BR; j++, o += nm) std::memcpy(in + o, mocaps + (j / R) * nm, nm * 4);
   const size_t o_ts = o;
-  for (int b = 0; b < B; b++, o += nts) rebase_task_state(h, task_states ? task_states + b * nts : nullptr, times[b], in + o);
+  for (int j = 0; j < BR; j++, o += nts)
+    rebase_task_state(h, task_states ? task_states + (j / R) * nts : nullptr, times[j / R], in + o);
   const size_t o_w = o;
-  if (weights) for (size_t i = 0; i < B * nw; i++) in[o++] = (float)weights[i];
+  if (weights) for (int j = 0; j < BR; j++) for (size_t i = 0; i < nw; i++) in[o++] = (float)weights[(j / R) * nw + i];
   const size_t o_p = o;
-  if (parameters) for (size_t i = 0; i < B * np; i++) in[o++] = (float)parameters[i];
+  if (parameters)
+    for (int j = 0; j < BR; j++) for (size_t i = 0; i < np; i++) in[o++] = (float)parameters[(j / R) * np + i];
   const size_t o_kt = o;
   if (knots) {
-    for (int b = 0; b < B; b++)
-      for (int k = 0; k < count; k++) in[o++] = (float)(nodes[(size_t)b * count + k] - times[b]);
+    for (int j = 0; j < BR; j++)
+      for (int k = 0; k < count; k++) in[o++] = (float)(nodes[(size_t)(j / R) * count + k] - times[j / R]);
   }
   const size_t o_k = o;
-  if (knots) { std::memcpy(in + o, knots, (size_t)B * N * count * M.nu * 4); o += (size_t)B * N * count * M.nu; }
+  if (knots) for (int j = 0; j < BR; j++, o += nk) std::memcpy(in + o, knots + (j / R) * nk, nk * 4);
   const size_t o_seed = o;
   if (!h->noise_seeds.empty()) { std::memcpy(in + o, h->noise_seeds.data(), (size_t)B * 4); o += B; }
   CUDA_TRY(cudaMemcpyAsync(h->d_in, in, o * 4, cudaMemcpyHostToDevice, h->stream));
   float* d = h->d_in;
-  A->nprob = B; A->nper = N;
+  A->nprob = BR; A->nper = N;
   A->iv = reinterpret_cast<const PolicyInterval*>(d);
   A->timestep = h->pack.timestep;
   A->state = d + o_state; A->mocap = d + o_mocap; A->task_state = d + o_ts;
@@ -451,7 +478,10 @@ int reserve_feedback(mjpc_b200* h, int B) {
   return 0;
 }
 
-int launch_rollout(mjpc_b200* h, const RolloutArgs& A_in) {
+// The rollout launch A, then the ranking of its candidates.  K > 0: A holds B x K x N trajectories of a model ensemble
+// (stage_problems with R = K) and writes the member returns; ensemble_score_kernel scores the B x N candidates into
+// d_returns / d_failure, which are ranked.
+int launch_rollout(mjpc_b200* h, const RolloutArgs& A_in, int K = 0) {
   RolloutArgs A = A_in;
   const size_t smem = h->smem_bytes(A.P);
   CUDA_TRY(cudaEventRecord(h->ev0, h->stream));
@@ -468,11 +498,19 @@ int launch_rollout(mjpc_b200* h, const RolloutArgs& A_in) {
   h->last_static = pick_kernels(h, &k);
   const bool plain = h->last_static == 2;
   launch_kernel(plain ? k->rollout_plain : k->rollout, A.N, plain ? 32 : k->rollout_threads, smem, h->stream, A);
-  rank_kernel<<<(A.N + 255) / 256, 256, 0, h->stream>>>(A.returns, A.nper, A.nprob, h->d_order);
+  if (K) {
+    const int B = A.nprob / K, n = B * A.nper;
+    ensemble_score_kernel<<<(n + 7) / 8, 256, 0, h->stream>>>(A.returns, A.failure, B, K, A.nper, h->worst,
+                                                              h->d_returns, h->d_failure);
+    rank_kernel<<<(n + 255) / 256, 256, 0, h->stream>>>(h->d_returns, A.nper, B, h->d_order);
+  } else {
+    rank_kernel<<<(A.N + 255) / 256, 256, 0, h->stream>>>(A.returns, A.nper, A.nprob, h->d_order);
+  }
   CUDA_TRY(cudaEventRecord(h->ev1, h->stream));
   CUDA_TRY(cudaGetLastError());
-  h->launches += 2;
-  h->lastN = A.N; h->lastH = A.H;
+  h->launches += K ? 3 : 2;
+  h->lastN = K ? A.N / K : A.N; h->lastH = A.H;
+  h->last_members = K; h->last_nper = A.nper;
   return 0;
 }
 
@@ -682,7 +720,8 @@ void mjpc_b200_destroy(mjpc_b200_t* h) {
   void* bufs[] = {h->d_pack, h->d_in, h->d_unom, h->d_xnom,
                   h->d_tnom, h->d_gains, h->d_du, h->d_steps, h->d_states, h->d_actions, h->d_times, h->d_residual,
                   h->d_costs, h->d_trace, h->d_returns, h->d_failure, h->d_order, h->d_stats, h->d_pair_sync,
-                  h->d_sensors, h->d_step, h->d_variants, h->d_variant_index};
+                  h->d_sensors, h->d_step, h->d_variants, h->d_variant_index, h->d_members, h->d_member_index,
+                  h->d_member_returns, h->d_member_failure};
   for (void* p : bufs) if (p) cudaFree(p);
   ilqg_free(h->ilqg);
   delete h->bank;
@@ -739,21 +778,16 @@ int mjpc_b200_set_differentiable(mjpc_b200_t* h, int on) {
   return 0;
 }
 
-// Per-problem model variants: validate every blob against the handle's model as created (variant_mismatch), then
-// upload them into one allocation, variant v's block at d_variants + v * variant_stride:
-//   [its nf floats, with the handle's live task floats][its ni ints][its keyframe table (Ctx::gkey)][pad][meaninertia]
-// The blocks are what a handle created from the variant uploads as d_pack, so problem b of a launch computes what such
-// a handle computes.  count = 0 (or NULL) clears them.  Nothing is changed on a refusal.
-int mjpc_b200_set_model_variants(mjpc_b200_t* h, const mjpc_model_blob* models, int count) {
-  if (!h || count < 0 || (count > 0 && !models)) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "set_model_variants: bad argument");
-  if (count > h->maxN)
-    return fail(MJPC_B200_ERR_CAPACITY, "set_model_variants: more variants than max_candidates problems");
-  CUDA_TRY(cudaSetDevice(h->device));
+// set_model_variants' and set_model_ensemble's blocks: each of the count blobs validated against the handle's model as
+// created (variant_mismatch; an error names `call`, the `what` and its index), then laid out as one host image of
+// count blocks of *stride floats.  Nothing is changed on a refusal.
+static int model_blocks(mjpc_b200_t* h, const mjpc_model_blob* models, int count, const char* call, const char* what,
+                        std::vector<float>* image, size_t* stride_out) {
   const DevModel& M = h->M0;
   size_t stride = 0;
   std::vector<ModelPack> packs(count);
   for (int v = 0; v < count; v++) {
-    const std::string at = "set_model_variants: variant " + std::to_string(v) + ": ";
+    const std::string at = std::string(call) + ": " + what + " " + std::to_string(v) + ": ";
     if (!models[v].data) return fail(MJPC_B200_ERR_BAD_ARGUMENT, at + "NULL blob");
     std::vector<DevSensor> sensors;
     std::vector<std::string> why;
@@ -771,30 +805,61 @@ int mjpc_b200_set_model_variants(mjpc_b200_t* h, const mjpc_model_blob* models, 
     stride = std::max(stride, (size_t)(M.nf + M.ni) + packs[v].key_mpos.size() + 1);
   }
   stride = (stride + 31) & ~(size_t)31;   // 128-byte aligned blocks (the TMA copy needs 16)
+  std::vector<float>& blocks = *image;
+  blocks.assign((size_t)count * stride, 0.f);
+  const size_t t0 = task_floats_begin(M), nt = task_floats_count(M);
+  for (int v = 0; v < count; v++) {
+    float* o = blocks.data() + (size_t)v * stride;
+    const ModelPack& P = packs[v];
+    std::copy(P.f.begin(), P.f.end(), o);
+    std::copy(h->pack.f.begin() + t0, h->pack.f.begin() + t0 + nt, o + t0);   // the live task (set_task)
+    std::memcpy(o + M.nf, P.i.data(), P.i.size() * 4);
+    for (size_t k = 0; k < P.key_mpos.size(); k++) o[M.nf + M.ni + k] = (float)P.key_mpos[k];
+    o[stride - 1] = P.M.meaninertia;
+  }
+  *stride_out = stride;
+  return 0;
+}
+
+// device copies of a host block image and of a member / variant index, both or neither: on a failure nothing stays
+// allocated
+static cudaError_t upload_blocks(const std::vector<float>& blocks, const std::vector<int>& index, float** d, int** di) {
+  *d = nullptr; *di = nullptr;
+  cudaError_t e = dalloc(d, blocks.size());
+  if (e == cudaSuccess) e = dalloc(di, index.size());
+  if (e == cudaSuccess) e = cudaMemcpy(*d, blocks.data(), blocks.size() * 4, cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) e = cudaMemcpy(*di, index.data(), index.size() * 4, cudaMemcpyHostToDevice);
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    if (*d) cudaFree(*d);
+    if (*di) cudaFree(*di);
+    *d = nullptr; *di = nullptr;
+  }
+  return e;
+}
+
+// Per-problem model variants: validate every blob against the handle's model as created (variant_mismatch), then
+// upload them into one allocation, variant v's block at d_variants + v * variant_stride:
+//   [its nf floats, with the handle's live task floats][its ni ints][its keyframe table (Ctx::gkey)][pad][meaninertia]
+// The blocks are what a handle created from the variant uploads as d_pack, so problem b of a launch computes what such
+// a handle computes.  count = 0 (or NULL) clears them.  Nothing is changed on a refusal.
+int mjpc_b200_set_model_variants(mjpc_b200_t* h, const mjpc_model_blob* models, int count) {
+  if (!h || count < 0 || (count > 0 && !models)) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "set_model_variants: bad argument");
+  if (count > h->maxN)
+    return fail(MJPC_B200_ERR_CAPACITY, "set_model_variants: more variants than max_candidates problems");
+  if (count > 0)
+    if (int rc = check_ensemble(h, "set_model_variants")) return rc;
+  CUDA_TRY(cudaSetDevice(h->device));
+  std::vector<float> blocks;
+  size_t stride = 0;
+  if (int rc = model_blocks(h, models, count, "set_model_variants", "variant", &blocks, &stride)) return rc;
   float* d = nullptr;
   int* di = nullptr;
   if (count) {
-    std::vector<float> blocks((size_t)count * stride, 0.f);
-    const size_t t0 = task_floats_begin(M), nt = task_floats_count(M);
-    for (int v = 0; v < count; v++) {
-      float* o = blocks.data() + (size_t)v * stride;
-      const ModelPack& P = packs[v];
-      std::copy(P.f.begin(), P.f.end(), o);
-      std::copy(h->pack.f.begin() + t0, h->pack.f.begin() + t0 + nt, o + t0);   // the live task (set_task)
-      std::memcpy(o + M.nf, P.i.data(), P.i.size() * 4);
-      for (size_t k = 0; k < P.key_mpos.size(); k++) o[M.nf + M.ni + k] = (float)P.key_mpos[k];
-      o[stride - 1] = P.M.meaninertia;
-    }
     std::vector<int> identity(h->maxN);
     for (int v = 0; v < h->maxN; v++) identity[v] = v < count ? v : 0;
-    if (cudaError_t e = dalloc(&d, blocks.size())) return fail(MJPC_B200_ERR_CUDA, std::string("set_model_variants: ") + cudaGetErrorString(e));
-    cudaError_t e = dalloc(&di, identity.size());
-    if (e == cudaSuccess) e = cudaMemcpy(d, blocks.data(), blocks.size() * 4, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMemcpy(di, identity.data(), identity.size() * 4, cudaMemcpyHostToDevice);
-    if (e != cudaSuccess) {
-      cudaFree(d); if (di) cudaFree(di);
+    if (cudaError_t e = upload_blocks(blocks, identity, &d, &di))
       return fail(MJPC_B200_ERR_CUDA, std::string("set_model_variants: ") + cudaGetErrorString(e));
-    }
   }
   CUDA_TRY(cudaStreamSynchronize(h->stream));   // launches in flight may still read the old blocks
   if (h->d_variants) cudaFree(h->d_variants);
@@ -826,6 +891,91 @@ int mjpc_b200_select_model_variants(mjpc_b200_t* h, const int* index, int B) {
   return 0;
 }
 
+// Grow the per-trajectory buffers (outputs, member returns, launch inputs and their pinned staging) to K x max_candidates
+// trajectories, for the launches of a K-member ensemble; never shrinks.  On an allocation failure the handle keeps its
+// buffers.
+static int reserve_members(mjpc_b200_t* h, int K) {
+  if (K <= h->traj_factor && h->d_member_returns) return 0;
+  K = std::max(K, h->traj_factor);
+  const DevModel& M = h->pack.M;
+  const size_t N = (size_t)K * h->maxN, H = h->maxH, ds = M.nq + M.nv, nu = M.nu, nr = M.num_residual,
+               ntr = 3 * (size_t)M.num_trace;
+  const size_t in_floats = problem_floats(M, (int)N, h->maxP, h->maxH) + N * h->maxP * nu;
+  float *states = nullptr, *actions = nullptr, *residual = nullptr, *costs = nullptr, *trace = nullptr,
+        *mret = nullptr, *din = nullptr, *hin = nullptr;
+  double* times = nullptr;
+  long long* stats = nullptr;
+  unsigned char* mfail = nullptr;
+  cudaError_t e = dalloc(&states, N * H * ds);
+  if (e == cudaSuccess) e = dalloc(&actions, N * H * nu);
+  if (e == cudaSuccess) e = dalloc(&times, N * H);
+  if (e == cudaSuccess) e = dalloc(&residual, N * H * nr);
+  if (e == cudaSuccess) e = dalloc(&costs, N * H);
+  if (e == cudaSuccess) e = dalloc(&trace, N * H * ntr);
+  if (e == cudaSuccess) e = dalloc(&stats, 12 * N);
+  if (e == cudaSuccess) e = dalloc(&mret, N);
+  if (e == cudaSuccess) e = dalloc(&mfail, N);
+  if (e == cudaSuccess) e = dalloc(&din, in_floats);
+  if (e == cudaSuccess && in_floats + 64 > h->h_in_floats) e = cudaMallocHost((void**)&hin, (in_floats + 64) * 4);
+  void* fresh[] = {states, actions, times, residual, costs, trace, stats, mret, mfail, din};
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    for (void* p : fresh) if (p) cudaFree(p);
+    if (hin) cudaFreeHost(hin);
+    return fail(MJPC_B200_ERR_CUDA, std::string("set_model_ensemble: ") + cudaGetErrorString(e));
+  }
+  CUDA_TRY(cudaStreamSynchronize(h->stream));   // launches and copies in flight may still use the old buffers
+  void* old[] = {h->d_states, h->d_actions, h->d_times, h->d_residual, h->d_costs, h->d_trace, h->d_stats,
+                 h->d_member_returns, h->d_member_failure, h->d_in};
+  for (void* p : old) if (p) cudaFree(p);
+  h->d_states = states; h->d_actions = actions; h->d_times = times; h->d_residual = residual; h->d_costs = costs;
+  h->d_trace = trace; h->d_stats = stats; h->d_member_returns = mret; h->d_member_failure = mfail; h->d_in = din;
+  if (hin) { cudaFreeHost(h->h_in); h->h_in = hin; h->h_in_floats = in_floats + 64; }
+  h->traj_factor = K;
+  h->resident_ok = false;
+  h->lastN = 0;   // the last launch's trajectories are gone
+  return 0;
+}
+
+// A model ensemble: every spline launch rolls each candidate out on the K members and scores it (launch_rollout).  The
+// members are validated and laid out as variants are (model_blocks); launch problem j runs on member j % K.
+int mjpc_b200_set_model_ensemble(mjpc_b200_t* h, const mjpc_model_blob* models, int K, int worst) {
+  if (!h) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "set_model_ensemble: null handle");
+  if (K < 0 || K > 32) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "set_model_ensemble: K must be in [1, 32] (0 clears)");
+  if (K == 0 || !models) {
+    CUDA_TRY(cudaSetDevice(h->device));
+    CUDA_TRY(cudaStreamSynchronize(h->stream));
+    if (h->d_members) cudaFree(h->d_members);
+    if (h->d_member_index) cudaFree(h->d_member_index);
+    h->d_members = nullptr; h->d_member_index = nullptr;
+    h->nmembers = 0; h->member_stride = 0; h->worst = 0;
+    h->resident_ok = false;
+    return 0;
+  }
+  if (worst < 1 || worst > K) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "set_model_ensemble: worst must be in [1, K]");
+  if (h->nvariants)
+    return fail(MJPC_B200_ERR_UNSUPPORTED,
+                "set_model_ensemble: not available while model variants are set (set_model_variants)");
+  CUDA_TRY(cudaSetDevice(h->device));
+  std::vector<float> blocks;
+  size_t stride = 0;
+  if (int rc = model_blocks(h, models, K, "set_model_ensemble", "member", &blocks, &stride)) return rc;
+  if (int rc = reserve_members(h, K)) return rc;
+  std::vector<int> index((size_t)h->traj_factor * h->maxN);
+  for (size_t j = 0; j < index.size(); j++) index[j] = (int)(j % K);
+  float* d = nullptr;
+  int* di = nullptr;
+  if (cudaError_t e = upload_blocks(blocks, index, &d, &di))
+    return fail(MJPC_B200_ERR_CUDA, std::string("set_model_ensemble: ") + cudaGetErrorString(e));
+  CUDA_TRY(cudaStreamSynchronize(h->stream));   // launches in flight may still read the old blocks
+  if (h->d_members) cudaFree(h->d_members);
+  if (h->d_member_index) cudaFree(h->d_member_index);
+  h->d_members = d; h->d_member_index = di;
+  h->nmembers = K; h->member_stride = (int)stride; h->worst = worst;
+  h->resident_ok = false;
+  return 0;
+}
+
 // Validate and upload a spline launch of B problems x N candidates; it becomes the resident launch.  B = 1 is the
 // single-problem call.  Nothing is changed on a refusal, so the handle stays usable.
 static int upload_spline(mjpc_b200_t* h, int B, const float* states, const double* times, const float* mocaps,
@@ -835,15 +985,24 @@ static int upload_spline(mjpc_b200_t* h, int B, const float* states, const doubl
   if (M.nmocap && !mocaps) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "rollout_spline: mocap required");
   if (B < 1 || N < 1 || H < 1 || P < 1 || interp < 0 || interp > 2) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "rollout_spline: bad sizes");
   if ((int64_t)B * N > h->maxN || H > h->maxH || P > h->maxP) return fail(MJPC_B200_ERR_CAPACITY, "rollout_spline: B*N/H/P above capacity");
+  const int K = h->nmembers;
+  if (K && (h->xfrc_std > 0.f || !h->noise_seeds.empty()))
+    return fail(MJPC_B200_ERR_UNSUPPORTED, "rollout_spline: force noise (set_xfrc_noise) is not available while a "
+                                           "model ensemble is set (set_model_ensemble)");
   CUDA_TRY(cudaSetDevice(h->device));
-  RolloutArgs A = base_args(h, B * N, H);
+  RolloutArgs A = base_args(h, B * std::max(K, 1) * N, H);
   size_t end;
   if (int rc = stage_problems(h, B, states, times, mocaps, weights, parameters, task_states, knot_times, P, H, knots, N, &A,
-                              &end))
+                              &end, std::max(K, 1)))
     return rc;
+  if (K) {   // launch problem b K + k: problem b on member k; the members' returns are scored by launch_rollout
+    A.pack = h->d_members; A.pack_stride = h->member_stride; A.pack_index = h->d_member_index;
+    A.returns = h->d_member_returns; A.failure = h->d_member_failure;
+  }
   A.L = make_layout(h->pack.M, P);
   A.P = P; A.interp = interp; A.policy_kind = 0;
   h->resident = A;
+  h->resident_members = K;
   h->resident_ok = true;
   return 0;
 }
@@ -866,7 +1025,7 @@ int mjpc_b200_rollout_spline_batched(mjpc_b200_t* h, int B, const float* states,
   if (!h || !states || !times || !knots || !knot_times) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "rollout_spline_batched: null pointer");
   int rc = upload_spline(h, B, states, times, mocaps, weights, parameters, task_states, knots, knot_times, interp, P, N, H);
   if (rc) return rc;
-  rc = launch_rollout(h, h->resident);
+  rc = launch_rollout(h, h->resident, h->resident_members);
   if (rc) return rc;
   return read_back(h, B * N, returns, failure, order);
 }
@@ -879,7 +1038,7 @@ int mjpc_b200_launch_resident(mjpc_b200_t* h) {
   if (h->resident.timestep != h->pack.timestep)
     return fail(MJPC_B200_ERR_BAD_ARGUMENT, "launch_resident: the timestep changed since the upload");
   h->resident.M = h->pack.M;  // picks up set_task changes (risk)
-  return launch_rollout(h, h->resident);
+  return launch_rollout(h, h->resident, h->resident_members);
 }
 
 int mjpc_b200_sync(mjpc_b200_t* h) {
@@ -900,7 +1059,7 @@ int mjpc_b200_rollout_spline(mjpc_b200_t* h, const float* state, double time, co
                              int P, int N, int H, float* returns, uint8_t* failure, int* order) {
   int rc = mjpc_b200_upload_spline_inputs(h, state, time, mocap, userdata, knots, knot_times, interp, P, N, H);
   if (rc) return rc;
-  rc = launch_rollout(h, h->resident);
+  rc = launch_rollout(h, h->resident, h->resident_members);
   if (rc) return rc;
   return read_back(h, N, returns, failure, order);
 }
@@ -954,6 +1113,7 @@ int mjpc_b200_rollout_feedback(mjpc_b200_t* h, const float* state, double time, 
   if (!h || !state || !u_nom || !x_nom || !t_nom || !gains || !step_sizes)
     return fail(MJPC_B200_ERR_BAD_ARGUMENT, "rollout_feedback: null pointer");
   if (int rc = check_variants(h, -1, "rollout_feedback")) return rc;
+  if (int rc = check_ensemble(h, "rollout_feedback")) return rc;
   if (userdata && h->nuserdata == 0) return fail(MJPC_B200_ERR_UNSUPPORTED, "rollout_feedback: the model has nuserdata = 0, userdata must be NULL");
   return rollout_feedback_impl(h, 1, state, &time, mocap, nullptr, nullptr, nullptr, u_nom, x_nom, t_nom, gains, du,
                                step_sizes, mode, K, H, returns, failure, order);
@@ -966,6 +1126,7 @@ int mjpc_b200_rollout_feedback_batched(mjpc_b200_t* h, int B, const float* state
                                        uint8_t* failure, int* order) {
   if (!h || !states || !times || !u_nom || !x_nom || !t_nom || !gains || !step_sizes)
     return fail(MJPC_B200_ERR_BAD_ARGUMENT, "rollout_feedback_batched: null pointer");
+  if (int rc = check_ensemble(h, "rollout_feedback_batched")) return rc;
   return rollout_feedback_impl(h, B, states, times, mocaps, weights, parameters, task_states, u_nom, x_nom, t_nom, gains,
                                du, step_sizes, mode, K, H, returns, failure, order);
 }
@@ -977,14 +1138,17 @@ void mjpc_b200_host_policy_intervals(const double* nodes, int count, double time
   for (int t = 0; t < H; t++) { times[t] = iv[t].time; upper[t] = iv[t].upper; frac[t] = iv[t].frac; }
 }
 
+// trajectories [first, first + count) of the last launch into rows [row, row + count) of the host arrays
 static int fetch_impl(mjpc_b200_t* h, int first, int count, float* states, float* actions, double* times,
-                      float* residual, float* costs, float* trace) {
+                      float* residual, float* costs, float* trace, int row = 0) {
   const DevModel& M = h->pack.M;
   const size_t H = h->lastH, ds = M.nq + M.nv, nu = M.nu, nr = M.num_residual, ntr = 3 * M.num_trace;
   CUDA_TRY(cudaSetDevice(h->device));
   CUDA_TRY(cudaStreamSynchronize(h->stream));
   auto get = [&](void* dst, const void* src, size_t per, size_t elt) {
-    return dst ? cudaMemcpy(dst, (const char*)src + (size_t)first * per * elt, (size_t)count * per * elt, cudaMemcpyDeviceToHost) : cudaSuccess;
+    return dst ? cudaMemcpy((char*)dst + (size_t)row * per * elt, (const char*)src + (size_t)first * per * elt,
+                            (size_t)count * per * elt, cudaMemcpyDeviceToHost)
+               : cudaSuccess;
   };
   CUDA_TRY(get(states, h->d_states, H * ds, 4)); CUDA_TRY(get(actions, h->d_actions, H * nu, 4));
   CUDA_TRY(get(times, h->d_times, H, 8)); CUDA_TRY(get(residual, h->d_residual, H * nr, 4));
@@ -992,17 +1156,69 @@ static int fetch_impl(mjpc_b200_t* h, int first, int count, float* states, float
   return 0;
 }
 
+// the launched trajectory of candidate c (flat b N + i) of the last launch as member k rolled it out
+static int member_trajectory(const mjpc_b200_t* h, int c, int k) {
+  if (!h->last_members) return c;
+  const int b = c / h->last_nper, i = c - b * h->last_nper;
+  return (b * h->last_members + k) * h->last_nper + i;
+}
+
 int mjpc_b200_fetch_trajectory(mjpc_b200_t* h, int candidate, float* states, float* actions, double* times,
                                float* residual, float* costs, float* trace) {
   if (!h || h->lastN < 1 || candidate < 0 || candidate >= h->lastN)
     return fail(MJPC_B200_ERR_BAD_ARGUMENT, "fetch_trajectory: bad candidate");
-  return fetch_impl(h, candidate, 1, states, actions, times, residual, costs, trace);
+  return fetch_impl(h, member_trajectory(h, candidate, 0), 1, states, actions, times, residual, costs, trace);
+}
+
+int mjpc_b200_fetch_trajectory_member(mjpc_b200_t* h, int candidate, int member, float* states, float* actions,
+                                      double* times, float* residual, float* costs, float* trace) {
+  if (!h || h->lastN < 1 || candidate < 0 || candidate >= h->lastN)
+    return fail(MJPC_B200_ERR_BAD_ARGUMENT, "fetch_trajectory_member: bad candidate");
+  if (member < 0 || member >= std::max(h->last_members, 1))
+    return fail(MJPC_B200_ERR_BAD_ARGUMENT, "fetch_trajectory_member: member " + std::to_string(member) +
+                                                " outside the last launch's " + std::to_string(std::max(h->last_members, 1)));
+  return fetch_impl(h, member_trajectory(h, candidate, member), 1, states, actions, times, residual, costs, trace);
 }
 
 int mjpc_b200_fetch_all(mjpc_b200_t* h, float* states, float* actions, double* times, float* residual, float* costs,
                         float* trace) {
   if (!h || h->lastN < 1) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "fetch_all: nothing to fetch");
-  return fetch_impl(h, 0, h->lastN, states, actions, times, residual, costs, trace);
+  if (!h->last_members) return fetch_impl(h, 0, h->lastN, states, actions, times, residual, costs, trace);
+  for (int b = 0; b < h->lastN / h->last_nper; b++)   // member 0 of each problem's candidates
+    if (int rc = fetch_impl(h, member_trajectory(h, b * h->last_nper, 0), h->last_nper, states, actions, times, residual,
+                            costs, trace, b * h->last_nper))
+      return rc;
+  return 0;
+}
+
+int mjpc_b200_fetch_ensemble(mjpc_b200_t* h, float* member_returns, uint8_t* member_failure) {
+  if (!h || h->lastN < 1 || !h->last_members)
+    return fail(MJPC_B200_ERR_BAD_ARGUMENT, "fetch_ensemble: the last launch was not a model-ensemble launch");
+  const size_t n = (size_t)h->lastN * h->last_members;
+  CUDA_TRY(cudaSetDevice(h->device));
+  CUDA_TRY(cudaStreamSynchronize(h->stream));
+  if (member_returns) CUDA_TRY(cudaMemcpy(member_returns, h->d_member_returns, n * 4, cudaMemcpyDeviceToHost));
+  if (member_failure) CUDA_TRY(cudaMemcpy(member_failure, h->d_member_failure, n, cudaMemcpyDeviceToHost));
+  return 0;
+}
+
+void mjpc_b200_host_ensemble_score(const float* member_returns, const uint8_t* member_failure, int K, int worst,
+                                   float* score, uint8_t* failure) {
+  if (K < 1 || K > 32 || worst < 1 || worst > K) return;
+  const float* r = member_returns;
+  bool failed = false;
+  int at[32];
+  for (int k = 0; k < K; k++) {
+    failed |= member_failure[k] != 0;
+    int rank = 0;   // descending, ties to the lower member, NaN first (ensemble_score_kernel)
+    for (int j = 0; j < K; j++)
+      rank += (r[j] > r[k]) || (r[j] == r[k] && j < k) || (r[j] != r[j] && (r[k] == r[k] || j < k));
+    at[rank] = k;
+  }
+  double sum = 0.0;
+  for (int p = 0; p < worst; p++) sum += (double)r[at[p]];
+  *score = failed ? 1.0e6f : (float)(sum / (double)worst);
+  *failure = failed ? 1 : 0;
 }
 
 // grow step_impl's device scratch and pinned staging to `words` floats each (never shrinks); on failure the old ones stay
@@ -1091,6 +1307,7 @@ int mjpc_b200_step_debug(mjpc_b200_t* h, const float* qpos, const float* qvel, c
                          float* next_qpos, float* next_qvel, float* qM, float* efc_force, int* counts) {
   if (!h || !qpos || !qvel || !ctrl) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "step_debug: null");
   if (int rc = check_variants(h, -1, "step_debug")) return rc;
+  if (int rc = check_ensemble(h, "step_debug")) return rc;
   h->dbg_ncon = -1;
   h->dbg_contact.resize((size_t)h->pack.M.maxcon * 8);
   if (efc_force) std::fill_n(efc_force, 256, 0.f);   // the caller's efc_force holds 256 floats, the first maxefc are rows
@@ -1107,6 +1324,7 @@ int mjpc_b200_step_debug_contacts(mjpc_b200_t* h, int capacity, float* contact, 
   if (!h || capacity < 0 || (capacity > 0 && !contact) || !ncon)
     return fail(MJPC_B200_ERR_BAD_ARGUMENT, "step_debug_contacts: bad argument");
   if (int rc = check_variants(h, -1, "step_debug_contacts")) return rc;
+  if (int rc = check_ensemble(h, "step_debug_contacts")) return rc;
   if (h->dbg_ncon < 0) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "step_debug_contacts: no step_debug call to report");
   *ncon = h->dbg_ncon;
   const int n = std::min(h->dbg_ncon, capacity);
@@ -1163,6 +1381,7 @@ int mjpc_b200_rollout_spline_sharded(mjpc_b200_t* h, const float* state, double 
                                      int P, int N, int H, float* returns, uint8_t* failure, int* order) {
   if (!h || !knots) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "rollout_spline_sharded: null");
   if (int rc = check_variants(h, -1, "rollout_spline_sharded")) return rc;
+  if (int rc = check_ensemble(h, "rollout_spline_sharded")) return rc;
   if (!h->noise_seeds.empty())
     return fail(MJPC_B200_ERR_UNSUPPORTED, "rollout_spline_sharded: per-problem noise keys (set_xfrc_noise_batched)");
   if (h->nranks > 1 && !h->comm) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "rollout_spline_sharded: comm_init first");
@@ -1239,6 +1458,7 @@ int mjpc_b200_step_batch(mjpc_b200_t* h, int B, const float* qpos, const float* 
                          float* next_qpos, float* next_qvel, float* residual, float* cost, int* counts) {
   if (!h || B < 1 || !qpos || !qvel || !ctrl || !times) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "step_batch: bad argument");
   if (int rc = check_variants(h, -1, "step_batch")) return rc;
+  if (int rc = check_ensemble(h, "step_batch")) return rc;
   if (h->pack.M.nmocap && !mocap) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "step_batch: mocap required");
   const KernelSet* k;
   const int kind = pick_kernels(h, &k);
@@ -1257,6 +1477,7 @@ int mjpc_b200_step_sensors(mjpc_b200_t* h, int B, const float* states, const flo
   if (!h || B < 1 || !states || (!ctrl && h->pack.M.nu) || !next_states || !sensordata)
     return fail(MJPC_B200_ERR_BAD_ARGUMENT, "step_sensors: bad argument");
   if (int rc = check_variants(h, -1, "step_sensors")) return rc;
+  if (int rc = check_ensemble(h, "step_sensors")) return rc;
   const DevModel& M = h->pack.M;
   if (M.nmocap && !mocap) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "step_sensors: mocap required");
   const int nsens = (int)h->sensors.size();
@@ -1292,6 +1513,7 @@ int mjpc_b200_step_sensors(mjpc_b200_t* h, int B, const float* states, const flo
 
 int mjpc_b200_plant_init(mjpc_b200_t* h, int num_plants, int sensor_start, int nsensor) {
   if (!h || num_plants < 1 || nsensor < 0) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "plant_init: bad argument");
+  if (int rc = check_ensemble(h, "plant_init")) return rc;
   if (num_plants > h->maxN) return fail(MJPC_B200_ERR_CAPACITY, "plant_init: num_plants > max_candidates");
   const int nsens = (int)h->sensors.size();
   if (nsensor && (sensor_start < 0 || sensor_start > nsens - nsensor))
@@ -1369,6 +1591,7 @@ int mjpc_b200_plant_init(mjpc_b200_t* h, int num_plants, int sensor_start, int n
 static int plant_check(mjpc_b200_t* h, int plant, const char* call) {
   if (!h) return fail(MJPC_B200_ERR_BAD_ARGUMENT, std::string(call) + ": null handle");
   if (!h->plants) return fail(MJPC_B200_ERR_BAD_ARGUMENT, std::string(call) + ": no plants (plant_init)");
+  if (int rc = check_ensemble(h, call)) return rc;
   if (plant < 0 || plant >= h->plants->a.B)
     return fail(MJPC_B200_ERR_BAD_ARGUMENT, std::string(call) + ": plant " + std::to_string(plant) + " outside [0, " +
                                                 std::to_string(h->plants->a.B) + ")");
@@ -1440,6 +1663,7 @@ int mjpc_b200_plant_step(mjpc_b200_t* h, const float* ctrl, float* state_out, do
   PlantBank& k = *h->plants;
   PlantArgs a = k.a;
   if (int rc = check_variants(h, a.B, "plant step")) return rc;
+  if (int rc = check_ensemble(h, "plant_step")) return rc;
   const size_t B = a.B, nu = M.nu, nm = 7 * (size_t)M.nmocap, nts = M.task_state_size, nw = M.num_term,
                np = M.num_parameters, ds = M.nq + M.nv;
   CUDA_TRY(cudaSetDevice(h->device));
@@ -1488,7 +1712,8 @@ int mjpc_b200_fetch_stats(mjpc_b200_t* h, int64_t* stats) {
   if (!h || !stats || h->lastN < 1) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "fetch_stats: nothing to fetch");
   CUDA_TRY(cudaSetDevice(h->device));
   CUDA_TRY(cudaStreamSynchronize(h->stream));
-  CUDA_TRY(cudaMemcpy(stats, h->d_stats, (size_t)h->lastN * 12 * sizeof(long long), cudaMemcpyDeviceToHost));
+  const size_t rows = (size_t)h->lastN * std::max(h->last_members, 1);   // every launched trajectory
+  CUDA_TRY(cudaMemcpy(stats, h->d_stats, rows * 12 * sizeof(long long), cudaMemcpyDeviceToHost));
   return 0;
 }
 
@@ -1598,6 +1823,7 @@ int mjpc_b200_model_derivatives(mjpc_b200_t* h, const float* x, const float* u, 
                                 int H, int skip, float tol, int mode, float* A, float* B, float* C, float* D) {
   if (!h || !x || !u || !t || !A || !B || !C || !D) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "model_derivatives: null");
   if (int rc = check_variants(h, -1, "model_derivatives")) return rc;
+  if (int rc = check_ensemble(h, "model_derivatives")) return rc;
   if (H < 1 || H > h->maxH || !(tol > 0)) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "model_derivatives: bad H or tol");
   if (skip < 0 || mode < 0 || mode > 1) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "model_derivatives: bad skip or mode");
   if (h->pack.M.nmocap && !mocap) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "model_derivatives: mocap required");
@@ -1614,6 +1840,7 @@ int mjpc_b200_model_derivatives_batched(mjpc_b200_t* h, int B, const float* x, c
   if (skip < 0 || mode < 0 || mode > 1) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "model_derivatives_batched: bad skip or mode");
   if (h->pack.M.nmocap && !mocaps) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "model_derivatives_batched: mocap required");
   if (int rc = check_variants(h, B, "model_derivatives_batched")) return rc;
+  if (int rc = check_ensemble(h, "model_derivatives_batched")) return rc;
   return model_derivatives_impl(h, B, x, u, t, mocaps, weights, parameters, task_states, H, skip, tol, mode, A, B_, C, D);
 }
 
@@ -1662,6 +1889,7 @@ int mjpc_b200_gradient_batched(mjpc_b200_t* h, int B, const float* x, const floa
   if (skip < 0 || mode < 0 || mode > 1) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "gradient_batched: bad skip or mode");
   if (h->pack.M.nmocap && !mocaps) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "gradient_batched: mocap required");
   if (int rc = check_variants(h, B, "gradient_batched")) return rc;
+  if (int rc = check_ensemble(h, "gradient_batched")) return rc;
   const DevModel& M = h->pack.M;
   CUDA_TRY(cudaSetDevice(h->device));
   if (cost_derivatives_smem(M, h->max_term_dim) > h->smem_optin)
@@ -1862,6 +2090,7 @@ int Update(mjpc_b200_t* h, const float* ctrl, const double* sensor, const float*
   FilterBank& k = *h->bank;
   FilterBankArgs a = k.a;
   if (int rc = check_variants(h, a.B, "filter bank update")) return rc;
+  if (int rc = check_ensemble(h, "filter bank update")) return rc;
   const size_t B = a.B, ny = a.ny, nu = a.nu, nm = 7 * (size_t)a.nmocap;
   CUDA_TRY(cudaSetDevice(h->device));
   CUDA_TRY(cudaStreamSynchronize(h->stream));   // the staging may still feed an earlier copy

@@ -282,6 +282,11 @@ int mjpc_b200_batch_planner_set_models(mjpc_b200_batch_planner_t* h, const mjpc_
   if (!bp || count < 0) return MJPC_B200_ERR_BAD_ARGUMENT;
   return bp->SetModels(models, count);
 }
+int mjpc_b200_batch_planner_set_ensemble(mjpc_b200_batch_planner_t* h, const mjpc_model_blob* models, int K,
+                                         int worst) {
+  BatchPlanner* bp = problem_of<BatchPlanner>(h, 0);
+  return bp ? bp->SetEnsemble(models, K, worst) : MJPC_B200_ERR_BAD_ARGUMENT;
+}
 int mjpc_b200_batch_planner_optimize_policy(mjpc_b200_batch_planner_t* h, int horizon, int* codes) {
   BatchPlanner* bp = problem_of<BatchPlanner>(h, 0);
   if (!bp) return MJPC_B200_ERR_BAD_ARGUMENT;

@@ -38,6 +38,8 @@ class BatchPlanner {
   // problem b plans on models[b] from now on (mjpc_b200_set_model_variants on every handle the batch owns); count is
   // the number of problems, or 0 to plan every problem on the batch's model again
   int SetModels(const mjpc_model_blob* models, int count);
+  // every problem plans on one model ensemble: Planner::SetEnsemble of the problems, which share the batch's handle
+  int SetEnsemble(const mjpc_model_blob* models, int K, int worst) { return problem(0).SetEnsemble(models, K, worst); }
 
  protected:
   // the task snapshots of num_problems problems, each the model's, and the engine handle of max_candidates (all

@@ -34,6 +34,9 @@ class CrossEntropyPlanner : public Planner {
   // :331-340; the policy does not depend on the state
   void ActionFromPolicy(double* action, const double* state, double time, bool use_previous = false) override;
   const Trajectory* BestTrajectory() override;        // the NOMINAL trajectory (:462-464)
+  int SetEnsemble(const mjpc_model_blob* models, int K, int worst) override {
+    return mjpc_b200_set_model_ensemble(gpu_, models, K, worst);
+  }
 
   SamplingPolicy policy, resampled_policy, previous_policy;
   std::vector<SamplingPolicy> candidate_policy;

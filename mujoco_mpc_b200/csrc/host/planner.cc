@@ -176,6 +176,10 @@ int mjpc_b200_planner_set_fd(mjpc_b200_planner_t* h, double tolerance, int mode,
   Planner* p = PlannerOf<Planner>(h);
   return p ? p->SetFD(tolerance, mode, derivative_skip) : MJPC_B200_ERR_BAD_ARGUMENT;
 }
+int mjpc_b200_planner_set_ensemble(mjpc_b200_planner_t* h, const mjpc_model_blob* models, int K, int worst) {
+  Planner* p = PlannerOf<Planner>(h);
+  return p ? p->SetEnsemble(models, K, worst) : MJPC_B200_ERR_BAD_ARGUMENT;
+}
 int mjpc_b200_planner_set_task(mjpc_b200_planner_t* h, const mjpc_task_desc* task) {
   Planner* p = PlannerOf<Planner>(h);
   if (!p || !task) return MJPC_B200_ERR_BAD_ARGUMENT;

@@ -88,6 +88,9 @@ class Planner {
   // finite-difference settings of the planners that take derivatives (SetFiniteDifferences); the others:
   // MJPC_B200_ERR_UNSUPPORTED
   virtual int SetFD(double tolerance, int mode, int derivative_skip) { return MJPC_B200_ERR_UNSUPPORTED; }
+  // plan on a model ensemble (mjpc_b200_set_model_ensemble on the planner's handle): the planners whose iteration ranks
+  // by SplineLaunch's returns, which are then the scores; the others: MJPC_B200_ERR_UNSUPPORTED
+  virtual int SetEnsemble(const mjpc_model_blob* models, int K, int worst) { return MJPC_B200_ERR_UNSUPPORTED; }
   // every engine handle the planner plans on: Agent applies the planning-model options and the task snapshot to each
   virtual std::vector<mjpc_b200_t*> Handles() { return {gpu_}; }
   mjpc_b200_t* gpu() const { return gpu_; }

@@ -42,6 +42,9 @@ class SampleGradientPlanner : public Planner {
   void AddNoiseToPolicy(int i);                                     // :329-355
   void GradientCandidates(int num_trajectory, int num_gradient);    // :401-493
   const Trajectory* BestTrajectory() override;                      // trajectory[winner] (:496-498)
+  int SetEnsemble(const mjpc_model_blob* models, int K, int worst) override {
+    return mjpc_b200_set_model_ensemble(gpu_, models, K, worst);
+  }
 
   SamplingPolicy policy, resampled_policy, previous_policy;
   std::vector<SamplingPolicy> candidate_policy;

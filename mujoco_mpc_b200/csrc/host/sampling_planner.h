@@ -83,6 +83,9 @@ class SamplingPlanner : public Planner {
   void ActionFromPolicy(double* action, const double* state, double time, bool use_previous = false) override;
   void CopyCandidateToPolicy(int candidate);          // :534-543
   const Trajectory* BestTrajectory() override;
+  int SetEnsemble(const mjpc_model_blob* models, int K, int worst) override {
+    return mjpc_b200_set_model_ensemble(gpu_, models, K, worst);
+  }
   int CandidateTrajectory(int candidate, int horizon, Trajectory* out);   // trajectory[candidate] of the last Rollouts
   void SetPolicy(const double* times, const double* parameters, int num_nodes);   // policy.plan = nodes (ilqs/planner.cc:160-172)
   double timestep() const { return timestep_; }

@@ -4,6 +4,7 @@
 //                       (Trajectory::Rollout / RolloutDiscrete,
 //                       mjpc/trajectory.cc:92-309) incl. policy, mj_step restatement, residual, cost, return
 //   rank_kernel         order of each problem's candidates by return (partial_sort, sampling/planner.cc:184-188)
+//   ensemble_score_kernel  each candidate's score over the member models of a model ensemble (set_model_ensemble)
 //   step_batch_kernel   independent single forward+Euler steps through the same device functions (parity hooks)
 //   plant_step_kernel   one step of every closed-loop plant, its state kept in device memory (plant_bank.h)
 //   fd_*_kernel         finite-difference transition/residual Jacobians (model_derivatives.cc:45-165)
@@ -469,6 +470,38 @@ extern "C" __global__ void rank_kernel(const float* __restrict__ ret, int N, int
       rank += (rj < ri) || (rj == ri && j < i) || (ri != ri && rj == rj);
     }
     order[(size_t)b * N + rank] = i;
+  }
+}
+
+// The score of each candidate of a launch rolled out on K member models (set_model_ensemble): one warp per candidate
+// (b, i) of B problems x N candidates, lane k holding member k, which the rollout left at [(b K + k) N + i].  The member
+// returns are sorted in descending order (ties to the lower member, NaN first), the first `worst` summed left to right
+// in double and divided once by worst: ret [B][N].  A candidate that failed on any member fails with return 1e6.
+// mjpc_b200_host_ensemble_score is the host definition, bit for bit.
+extern "C" __global__ void ensemble_score_kernel(const float* __restrict__ member_ret,
+                                                 const unsigned char* __restrict__ member_fail, int B, int K, int N,
+                                                 int worst, float* __restrict__ ret, unsigned char* __restrict__ failure) {
+  const int lane = threadIdx.x & 31;
+  const int c = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5);
+  if (c >= B * N) return;   // (the whole warp)
+  const int b = c / N, i = c - b * N;
+  const bool member = lane < K;
+  const size_t at = ((size_t)b * K + lane) * N + i;
+  const float r = member ? member_ret[at] : 0.f;
+  const unsigned failed = __ballot_sync(~0u, member && member_fail[at]);
+  int rank = 0;   // the members sorted before this one
+  for (int j = 0; j < K; j++) {
+    const float rj = __shfl_sync(~0u, r, j);
+    rank += (rj > r) || (rj == r && j < lane) || (rj != rj && (r == r || j < lane));
+  }
+  double sum = 0.0;
+  for (int p = 0; p < worst; p++) {
+    const int src = __ffs(__ballot_sync(~0u, member && rank == p)) - 1;
+    sum = __dadd_rn(sum, (double)__shfl_sync(~0u, r, src));
+  }
+  if (lane == 0) {
+    ret[c] = failed ? 1.0e6f : __double2float_rn(__ddiv_rn(sum, (double)worst));
+    failure[c] = failed ? 1 : 0;
   }
 }
 

@@ -70,7 +70,9 @@ EXPORTS = ["mjpc_b200_version", "mjpc_b200_last_error", "mjpc_b200_create", "mjp
            "mjpc_b200_shadow_transition_destroy", "mjpc_b200_shadow_transition_step", "mjpc_b200_set_model_variants",
            "mjpc_b200_select_model_variants", "mjpc_b200_batch_planner_set_models",
            "mjpc_b200_batch_estimator_set_models", "mjpc_b200_plant_init", "mjpc_b200_plant_reset",
-           "mjpc_b200_plant_set", "mjpc_b200_plant_set_task", "mjpc_b200_plant_step", "mjpc_b200_plant_get"]
+           "mjpc_b200_plant_set", "mjpc_b200_plant_set_task", "mjpc_b200_plant_step", "mjpc_b200_plant_get",
+           "mjpc_b200_set_model_ensemble", "mjpc_b200_fetch_ensemble", "mjpc_b200_fetch_trajectory_member",
+           "mjpc_b200_host_ensemble_score", "mjpc_b200_planner_set_ensemble", "mjpc_b200_batch_planner_set_ensemble"]
 
 
 class ModelBlob(C.Structure):
@@ -110,6 +112,8 @@ def load_library():
                         (lib.mjpc_b200_planner_nominal_trajectory, [C.c_int]),
                         (lib.mjpc_b200_planner_action_from_policy, [_dp, _dp, C.c_double, C.c_int]),
                         (lib.mjpc_b200_planner_set_fd, [C.c_double, C.c_int, C.c_int]),
+                        (lib.mjpc_b200_planner_set_ensemble, [C.POINTER(ModelBlob), C.c_int, C.c_int]),
+                        (lib.mjpc_b200_batch_planner_set_ensemble, [C.POINTER(ModelBlob), C.c_int, C.c_int]),
                         (lib.mjpc_b200_batch_planner_destroy, []),
                         (lib.mjpc_b200_batch_planner_reset, [C.c_int, C.c_int, _dp]),
                         (lib.mjpc_b200_batch_planner_set_state, [C.c_int, _dp, C.c_double, _dp]),
@@ -175,6 +179,24 @@ def _model_blobs(models):
     pairs = [_model_blob(m) for m in models]
     arr = (ModelBlob * len(pairs))(*[mb for _, mb in pairs])
     return [b for b, _ in pairs], arr, len(pairs)
+
+
+def host_ensemble_score(member_returns, member_failure, worst):
+    """The score of one candidate from its K member returns and failure flags on the host
+    (mjpc_b200_host_ensemble_score, no device): (score, failure), bitwise what an ensemble launch computes."""
+    lib = load_library()
+    r = np.ascontiguousarray(member_returns, np.float32)
+    f = np.ascontiguousarray(member_failure, np.uint8)
+    score, fail = np.zeros(1, np.float32), np.zeros(1, np.uint8)
+    lib.mjpc_b200_host_ensemble_score(_pf(r), f.ctypes.data_as(_bp), len(r), int(worst), _pf(score),
+                                      fail.ctypes.data_as(_bp))
+    return score[0], fail[0]
+
+
+def _ensemble_args(models, worst):
+    """(buffers, ModelBlob array, K, worst) of set_ensemble: worst None is K (the expected return)."""
+    bufs, arr, n = _model_blobs(models)
+    return bufs, arr, n, n if worst is None else int(worst)
 
 
 def _set_batch_models(obj, models):
@@ -260,6 +282,14 @@ class _CppPlanner(_CppObject):
     def action_from_policy(self, time, use_previous=False):
         return self._action(time, None, use_previous)
 
+    def set_ensemble(self, models, worst=None):
+        """Plan on a model ensemble (mjpc_b200_planner_set_ensemble; Engine.set_model_ensemble gives the score):
+        Sampling, Cross-Entropy and Sample Gradient.  None or [] clears it."""
+        bufs, arr, K, worst = _ensemble_args(models, worst)
+        rc = self.lib.mjpc_b200_planner_set_ensemble(self.h, arr, K, worst)
+        if rc:
+            raise EngineError(f"{self._prefix}_set_ensemble failed ({rc}): {self.lib.mjpc_b200_last_error().decode()}")
+
     def set_task(self, weight=None, parameters=None, task_state=None, risk=None):
         """The task snapshot of every engine handle the planner plans on (mjpc_b200_planner_set_task)."""
         w, p, s = _d(weight), _d(parameters), _d(task_state)
@@ -335,6 +365,9 @@ class Engine:
         self.ds, self.n, self.nu, self.nr = info.dim_state, info.dim_dstate, info.nu, info.num_residual
         self.ntr = 3 * info.num_trace
         self.lastN = self.lastH = 0
+        self.members = 0       # K of the model ensemble (set_model_ensemble), 0: none
+        self.last_members = 0  # ... of the last launch
+        self.lastB = 0
 
     def close(self):
         if getattr(self, "h", None):
@@ -361,6 +394,15 @@ class Engine:
         bufs, arr, n = _model_blobs(models)
         self._check(self.lib.mjpc_b200_set_model_variants(self.h, arr, n))
 
+    def set_model_ensemble(self, models, worst=None):
+        """Score every candidate of the following spline launches on the K = len(models) member models
+        (mjpc_b200_set_model_ensemble): the mean of its `worst` largest member returns (None: K, the expected return;
+        1: the worst case), 1e6 and failed if any member fails.  Members follow the rule of set_model_variants.  None or
+        [] clears the ensemble."""
+        bufs, arr, K, worst = _ensemble_args(models, worst)
+        self._check(self.lib.mjpc_b200_set_model_ensemble(self.h, arr, K, worst))
+        self.members = K
+
     def set_options(self, timestep, integrator=0):
         """Agent::PlanIteration's planning-model overrides (agent.cc:288-289)."""
         self._check(self.lib.mjpc_b200_set_options(self.h, C.c_double(timestep), int(integrator)))
@@ -378,7 +420,7 @@ class Engine:
         self._check(self.lib.mjpc_b200_rollout_spline(self.h, _pf(st), C.c_double(time), _pf(mc), None, _pf(knots),
                                                       _pd(kt), int(interp), P, N, int(H), _pf(ret),
                                                       fail.ctypes.data_as(_bp), order.ctypes.data_as(_ip)))
-        self.lastN, self.lastH = N, H
+        self.lastN, self.lastH, self.lastB, self.last_members = N, H, 1, self.members
         return ret, fail, order
 
     def rollout_spline_batched(self, states, times, mocaps, knots, knot_times, interp, H, weights=None, parameters=None,
@@ -396,7 +438,7 @@ class Engine:
         self._check(self.lib.mjpc_b200_rollout_spline_batched(self.h, int(B), _pf(st), _pd(t), _pf(mc), _pd(w), _pd(p), _pd(s),
                                                               _pf(knots), _pd(kt), int(interp), int(P), int(N), int(H),
                                                               _pf(ret), fail.ctypes.data_as(_bp), order.ctypes.data_as(_ip)))
-        self.lastN, self.lastH = B * N, H
+        self.lastN, self.lastH, self.lastB, self.last_members = B * N, H, B, self.members
         return ret, fail, order
 
     # ---- multi-GPU: one planning problem sharded over an NCCL communicator owned by the handle
@@ -435,6 +477,7 @@ class Engine:
                                                               _pd(kt), int(interp), P, N, int(H), _pf(ret),
                                                               fail.ctypes.data_as(_bp), order.ctypes.data_as(_ip)))
         nr, rk = getattr(self, "nranks", 1), getattr(self, "rank", 0)
+        self.last_members = 0
         self.lastN, self.lastH = N // nr + (1 if rk < N % nr else 0), H     # fetch_all / fetch_stats are per shard
         return ret, fail, order
 
@@ -454,7 +497,7 @@ class Engine:
         st, mc, kt = _f(state), _f(mocap), _d(knot_times)
         self._check(self.lib.mjpc_b200_upload_spline_inputs(self.h, _pf(st), C.c_double(time), _pf(mc), None,
                                                             _pf(knots), _pd(kt), int(interp), P, N, int(H)))
-        self.lastN, self.lastH = N, H
+        self.lastN, self.lastH, self.lastB, self.last_members = N, H, 1, self.members
 
     def launch_resident(self):
         self._check(self.lib.mjpc_b200_launch_resident(self.h))
@@ -479,6 +522,7 @@ class Engine:
         self._check(self.lib.mjpc_b200_rollout_feedback(self.h, _pf(st), C.c_double(time), _pf(mc), None, _pf(u), _pf(x),
                                                         _pd(t), _pf(g), _pf(dd), _pf(ss), int(mode), K, H, _pf(ret),
                                                         fail.ctypes.data_as(_bp), order.ctypes.data_as(_ip)))
+        self.last_members = 0
         self.lastN, self.lastH = K, H
         return ret, fail, order
 
@@ -498,6 +542,7 @@ class Engine:
                                                                 _pf(u), _pf(x), _pd(t), _pf(g), _pf(dd), _pf(ss), int(mode),
                                                                 int(K), int(H), _pf(ret), fail.ctypes.data_as(_bp),
                                                                 order.ctypes.data_as(_ip)))
+        self.last_members = 0
         self.lastN, self.lastH = B * K, H
         return ret, fail, order
 
@@ -510,6 +555,25 @@ class Engine:
                                                         _pd(o["times"]), _pf(o["residual"]), _pf(o["costs"]),
                                                         _pf(o["trace"])))
         return o
+
+    def fetch_trajectory_member(self, i, member):
+        """Candidate i (flat b * N + i) of the last launch as ensemble member `member` rolled it out."""
+        H = self.lastH
+        o = dict(states=np.zeros((H, self.ds), np.float32), actions=np.zeros((H, self.nu), np.float32),
+                 times=np.zeros(H), residual=np.zeros((H, self.nr), np.float32), costs=np.zeros(H, np.float32),
+                 trace=np.zeros((H, self.ntr), np.float32))
+        self._check(self.lib.mjpc_b200_fetch_trajectory_member(self.h, int(i), int(member), _pf(o["states"]),
+                                                               _pf(o["actions"]), _pd(o["times"]), _pf(o["residual"]),
+                                                               _pf(o["costs"]), _pf(o["trace"])))
+        return o
+
+    def fetch_ensemble(self):
+        """(member returns [B, K, N], member failure [B, K, N]) of the last launch, an ensemble launch."""
+        B, K = max(self.lastB, 1), max(self.last_members, 1)
+        shape = (B, K, self.lastN // B)
+        ret, fail = np.zeros(shape, np.float32), np.zeros(shape, np.uint8)
+        self._check(self.lib.mjpc_b200_fetch_ensemble(self.h, _pf(ret), fail.ctypes.data_as(_bp)))
+        return ret, fail
 
     def fetch_all(self):
         N, H = self.lastN, self.lastH
@@ -658,7 +722,7 @@ class Engine:
         return k, dV0
 
     def fetch_stats(self):
-        st = np.zeros((self.lastN, 12), np.int64)
+        st = np.zeros((self.lastN * max(self.last_members, 1), 12), np.int64)   # every launched trajectory
         self._check(self.lib.mjpc_b200_fetch_stats(self.h, st.ctypes.data_as(C.POINTER(C.c_int64))))
         return st
 
@@ -869,6 +933,13 @@ class _CppBatchPlanner(_CppObject):
         """Problem b plans on compiled model models[b] from now on (len(models) == num_problems), on every engine
         handle the batch owns; None or [] plans every problem on the batch's model again."""
         _set_batch_models(self, models)
+
+    def set_ensemble(self, models, worst=None):
+        """Every problem plans on one model ensemble (mjpc_b200_batch_planner_set_ensemble); None or [] clears it."""
+        bufs, arr, K, worst = _ensemble_args(models, worst)
+        rc = self.lib.mjpc_b200_batch_planner_set_ensemble(self.h, arr, K, worst)
+        if rc != 0:
+            raise EngineError(f"batch_planner_set_ensemble failed ({rc}): {self.lib.mjpc_b200_last_error().decode()}")
 
     def set_fd(self, tolerance, mode=-1, derivative_skip=-1):
         self._check(self.lib.mjpc_b200_batch_planner_set_fd(self.h, C.c_double(tolerance), int(mode), int(derivative_skip)),
