@@ -336,7 +336,8 @@ int mjpc_b200_step_sensors(mjpc_b200_t* h, int B, const float* states, const flo
  * skipped by later steps until plant_reset.  A plant is MJPC_B200_PLANT_IDLE from plant_init until its first reset.
  *
  * Every call returns MJPC_B200_ERR_BAD_ARGUMENT for a NULL handle, a handle without plants (plant_init) or a plant
- * index outside [0, num_plants), and leaves the bank unchanged on any refusal. */
+ * index outside [0, num_plants), and leaves the bank unchanged on any refusal.  Disturbances (control noise, body-force
+ * noise, a held wrench) are set per plant below plant_get. */
 enum { MJPC_B200_PLANT_RUNNING = 0, MJPC_B200_PLANT_DIVERGED = 1, MJPC_B200_PLANT_IDLE = 2 };
 
 /* The handle's plants (replacing any earlier ones), every plant idle, with the handle's set_task values as task rows.
@@ -365,6 +366,33 @@ int mjpc_b200_plant_step(mjpc_b200_t* h, const float* ctrl, float* state_out, do
  * status. */
 int mjpc_b200_plant_get(mjpc_b200_t* h, int plant, float* state, float* warmstart, double* time, double* cost_sum,
                         int* steps, int* warnings, int* status);
+
+/* Disturbances (the reference app's control noise and force perturbations, app.cc:95-101, 291-304, 323-352).  Before
+ * each step of a running plant:
+ *   control noise  n <- r n + s z per actuator, r = exp(-timestep / ctrl_rate), s = ctrl_std sqrt(1 - r^2), added to the
+ *                  commanded ctrl; actuation clamps the sum to ctrlrange as it clamps any ctrl
+ *   force noise    the same recursion (xfrc_std, xfrc_rate) over the 6 nbody entries of xfrc_applied, as the Robust
+ *                  planner's rollouts draw it
+ *   xfrc_applied   = the held wrench + the force noise: per body force 3 then torque 3, world frame, at the body's
+ *                  centre of mass
+ * z is a standard normal: Philox4x32-10 with key (seed, 2) and counter (the plant's committed step count, 0, element,
+ * 'CTRL' or 'XFRC'), Box-Muller on the first two words.  A plant's noise depends on its seed and its own history only.
+ * The OU states advance only with a committed step.  plant_reset zeroes them (with the step count: the episode replays
+ * its seed's sequence) and keeps the settings and the held wrench; plant_init starts every plant undisturbed.  A plant
+ * without disturbances steps bitwise as before.  Every call below is refused with MJPC_B200_ERR_UNSUPPORTED while a
+ * model ensemble is set. */
+/* Plant `plant`'s noise (std 0: off) and seed; zeroes its OU states.  BAD_ARGUMENT: a negative or non-finite std, or a
+ * rate <= 0 or non-finite where its std is > 0. */
+int mjpc_b200_plant_set_disturbance(mjpc_b200_t* h, int plant, double ctrl_std, double ctrl_rate, double xfrc_std,
+                                    double xfrc_rate, uint32_t seed);
+/* The wrench xfrc [nbody][6] held on plant `plant` until changed (ApplyForcePerturbations headless); NULL clears it.
+ * BAD_ARGUMENT: a non-finite value. */
+int mjpc_b200_plant_set_xfrc(mjpc_b200_t* h, int plant, const float* xfrc);
+/* Plant `plant`'s OU states; either pointer may be NULL: ctrl_noise [nu], xfrc_noise [nbody][6]. */
+int mjpc_b200_plant_get_disturbance(mjpc_b200_t* h, int plant, float* ctrl_noise, float* xfrc_noise);
+/* The ctrl every plant applied in the last plant_step, [num_plants][nu]: commanded + control noise (the commanded ctrl,
+ * bit for bit, without control noise; the commanded ctrl of a plant that was not running; zeros before any step). */
+int mjpc_b200_plant_last_ctrl(mjpc_b200_t* h, float* ctrl_out);
 
 /* ---- State estimators (csrc/host/estimator.h, the reference's Estimator base mjpc/estimators/estimator.h): a single
  * filter is the batched estimators' bank of one filter below, on an engine handle it owns, with the same device

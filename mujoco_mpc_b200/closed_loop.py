@@ -8,7 +8,10 @@ Per physics step i, for every episode b, in the reference's order:
   4. one plant step of every episode; its cost is CostValue of the pre-step residual (testspeed.cc:104);
   5. planner.optimize_policy() when i % steps_per_planning_iteration == 0, from the states set in 2.
 With an estimator (a CppBatchEstimator of B filters on the plants' sensor range), every plant step is followed by one
-filter update from that step's ctrl, the plant's pre-step sensors and its mocap (app.cc:155-197)."""
+filter update from the ctrl the plant applied (the commanded ctrl plus any control noise: the app's estimator reads the
+noisy d->ctrl, app.cc:174), the plant's pre-step sensors and its mocap (app.cc:155-197).  A perturbation (a function of
+the step index and the plants' times) may hold a wrench on every plant before a step, as the app applies the user's
+force perturbation before each physics step (app.cc:323-326, 349-352)."""
 from __future__ import annotations
 
 import time as _time
@@ -18,10 +21,12 @@ import numpy as np
 from .engine import PLANT_RUNNING
 
 
-def synchronous_planning_cost(planner, plant, steps, steps_per_planning_iteration=4, transitions=None, estimator=None):
+def synchronous_planning_cost(planner, plant, steps, steps_per_planning_iteration=4, transitions=None, estimator=None,
+                              perturbation=None):
     """Run `steps` physics steps of plant.num_plants episodes with `planner` (a batch planner of as many problems),
     from the plants as reset() left them.  transitions: None or one Transition per plant (transition(time, qpos,
-    qvel) -> (qpos, qvel, mocap) and task_state(), as transition.HumanoidTrackTransition).
+    qvel) -> (qpos, qvel, mocap) and task_state(), as transition.HumanoidTrackTransition).  perturbation: None or
+    perturbation(i, time [B]) -> None or xfrc [B][nbody][6]; an array is held on plant b (plant.set_xfrc) from step i on.
 
     Returns dict(average_cost [B] (cost sum / steps of each plant), costs [steps][B], states [steps][B][nq+nv] and
     status [steps][B] after each step, final_status [B], wall_time and planning_time [s], x_realtime (B x simulated
@@ -42,6 +47,11 @@ def synchronous_planning_cost(planner, plant, steps, steps_per_planning_iteratio
     planning = 0.0
     start = _time.perf_counter()
     for i in range(steps):
+        xfrc = None if perturbation is None else perturbation(i, t.copy())
+        if xfrc is not None:
+            xfrc = np.asarray(xfrc, np.float32).reshape(B, m.nbody, 6)
+            for b in range(B):
+                plant.set_xfrc(b, xfrc[b])
         for b in range(B):
             if transitions is not None:
                 q, v, mocap = transitions[b].transition(t[b], x[b, :nq].astype(float), x[b, nq:].astype(float))
@@ -68,7 +78,8 @@ def synchronous_planning_cost(planner, plant, steps, steps_per_planning_iteratio
         x, t, status = o["state"].copy(), o["time"].copy(), o["status"].copy()
         states[i], statuses[i] = x, status
         if estimator is not None:
-            estimator.update(ctrl, o["sensordata"].astype(float), plant.mocap if m.nmocap else None)
+            applied = o.get("ctrl", ctrl)   # (a plant that reports no applied ctrl applied the commanded one)
+            estimator.update(applied, o["sensordata"].astype(float), plant.mocap if m.nmocap else None)
         if i % spp == 0:
             t0 = _time.perf_counter()
             planner.optimize_policy()

@@ -1540,8 +1540,11 @@ int mjpc_b200_plant_init(mjpc_b200_t* h, int num_plants, int sensor_start, int n
                nw = M.num_term, np = M.num_parameters, nsd = k->nsd;
   size_t bytes = 0;
   auto take = [&](size_t n) { const size_t at = bytes; bytes += (n + 255) & ~(size_t)255; return at; };
+  const size_t nx = 6 * (size_t)M.nbody;
   const size_t o_qpos = take(B * nq * 4), o_qvel = take(B * nv * 4), o_warm = take(B * nv * 4), o_time = take(B * 8),
-               o_sum = take(B * 8), o_steps = take(B * 4), o_warn = take(B * 4), o_status = take(B * 4);
+               o_sum = take(B * 8), o_steps = take(B * 4), o_warn = take(B * 4), o_status = take(B * 4),
+               o_dist = take(B * sizeof(PlantDisturbance)), o_cnoise = take(B * nu * 4), o_xnoise = take(B * nx * 4),
+               o_held = take(B * nx * 4), o_next = take(B * (nu + nx) * 4);
   // the upload and the outputs, each one contiguous block laid out as its pinned mirror
   size_t in = 0, out = 0;
   auto in_take = [&](size_t n) { const size_t at = in; in += (n + 15) & ~(size_t)15; return at; };
@@ -1549,7 +1552,7 @@ int mjpc_b200_plant_init(mjpc_b200_t* h, int num_plants, int sensor_start, int n
   k->o_ctrl = in_take(B * nu * 4); k->o_mocap = in_take(B * nm * 4); k->o_ts = in_take(B * nts * 4);
   k->o_weight = in_take(B * nw * 4); k->o_par = in_take(B * np * 4);
   k->o_time = out_take(B * 8); k->o_state = out_take(B * (nq + nv) * 4); k->o_cost = out_take(B * 4);
-  k->o_status = out_take(B * 4); k->o_sens = out_take(B * nsd * 4);
+  k->o_status = out_take(B * 4); k->o_sens = out_take(B * nsd * 4); k->o_ctrl_out = out_take(B * nu * 4);
   k->in_bytes = in; k->out_bytes = out;
   const size_t o_in = take(in), o_out = take(out);
   auto fail_k = [&](cudaError_t e) {
@@ -1564,6 +1567,8 @@ int mjpc_b200_plant_init(mjpc_b200_t* h, int num_plants, int sensor_start, int n
   a.qpos = (float*)(base + o_qpos); a.qvel = (float*)(base + o_qvel); a.warm = (float*)(base + o_warm);
   a.time = (double*)(base + o_time); a.cost_sum = (double*)(base + o_sum);
   a.steps = (int*)(base + o_steps); a.warnings = (int*)(base + o_warn); a.status = (int*)(base + o_status);
+  a.dist = (const PlantDisturbance*)(base + o_dist); a.ctrl_noise = (float*)(base + o_cnoise);
+  a.xfrc_noise = (float*)(base + o_xnoise); a.xfrc_held = (const float*)(base + o_held); a.noise_next = (float*)(base + o_next);
   k->d_in = base + o_in; k->d_out = base + o_out;
   a.ctrl = (const float*)(k->d_in + k->o_ctrl); a.mocap = (const float*)(k->d_in + k->o_mocap);
   a.task_state = nts ? (const float*)(k->d_in + k->o_ts) : nullptr;
@@ -1572,10 +1577,13 @@ int mjpc_b200_plant_init(mjpc_b200_t* h, int num_plants, int sensor_start, int n
   a.time_out = (double*)(k->d_out + k->o_time); a.state_out = (float*)(k->d_out + k->o_state);
   a.cost_out = (float*)(k->d_out + k->o_cost); a.status_out = (int*)(k->d_out + k->o_status);
   a.sensordata = nsd ? (float*)(k->d_out + k->o_sens) : nullptr;
+  a.ctrl_out = (float*)(k->d_out + k->o_ctrl_out);
   std::vector<int> idle(B, PLANT_IDLE);
   if (cudaError_t e = cudaMemcpy(a.status, idle.data(), B * 4, cudaMemcpyHostToDevice)) return fail_k(e);
-  // every plant starts with the handle's task (set_task) and no mocap; plant_reset starts its episode
+  // every plant starts with the handle's task (set_task), no mocap and no disturbance (the zeroed allocation);
+  // plant_reset starts its episode
   k->mocap.assign(B * nm, 0.f);
+  k->dist.assign(B, PlantDisturbance{});
   k->time.assign(B, 0.0);
   for (size_t b = 0; b < B; b++) {
     k->weight.insert(k->weight.end(), h->weight.begin(), h->weight.end());
@@ -1615,6 +1623,17 @@ static int plant_fields(mjpc_b200_t* h, int b, int write, void* qpos, void* qvel
   return 0;
 }
 
+// zero plant b's OU states: with the step count at 0 its episode replays its seed's noise (app.cc:428-431)
+static int plant_zero_noise(mjpc_b200_t* h, int b) {
+  const PlantArgs& a = h->plants->a;
+  const size_t nu = h->pack.M.nu, nx = 6 * (size_t)h->pack.M.nbody;
+  CUDA_TRY(cudaSetDevice(h->device));
+  CUDA_TRY(cudaStreamSynchronize(h->stream));
+  if (nu) CUDA_TRY(cudaMemset(a.ctrl_noise + b * nu, 0, nu * 4));
+  CUDA_TRY(cudaMemset(a.xfrc_noise + b * nx, 0, nx * 4));
+  return 0;
+}
+
 int mjpc_b200_plant_reset(mjpc_b200_t* h, int plant, const float* qpos, const float* qvel, double time, const float* mocap) {
   if (int rc = plant_check(h, plant, "plant_reset")) return rc;
   const DevModel& M = h->pack.M;
@@ -1624,6 +1643,7 @@ int mjpc_b200_plant_reset(mjpc_b200_t* h, int plant, const float* qpos, const fl
   int izero = 0, running = PLANT_RUNNING;
   if (int rc = plant_fields(h, plant, 1, (void*)qpos, (void*)qvel, warm.data(), &time, &zero, &izero, &izero, &running))
     return rc;
+  if (int rc = plant_zero_noise(h, plant)) return rc;
   PlantBank& k = *h->plants;
   const size_t nm = 7 * (size_t)M.nmocap;
   if (nm) std::copy(mocap, mocap + nm, k.mocap.begin() + plant * nm);
@@ -1698,6 +1718,69 @@ int mjpc_b200_plant_step(mjpc_b200_t* h, const float* ctrl, float* state_out, do
   if (status_out) std::memcpy(status_out, out + k.o_status, B * 4);
   if (sensordata_out && k.nsd) std::memcpy(sensordata_out, out + k.o_sens, B * k.nsd * 4);
   h->last_static = kind ? 1 : 0;
+  return 0;
+}
+
+static bool finite_f(double x) { return std::isfinite(x) && std::isfinite((float)x); }
+
+int mjpc_b200_plant_set_disturbance(mjpc_b200_t* h, int plant, double ctrl_std, double ctrl_rate, double xfrc_std,
+                                    double xfrc_rate, uint32_t seed) {
+  if (int rc = plant_check(h, plant, "plant_set_disturbance")) return rc;
+  for (const auto& [std_, rate] : {std::pair<double, double>{ctrl_std, ctrl_rate}, {xfrc_std, xfrc_rate}}) {
+    if (!finite_f(std_) || std_ < 0)
+      return fail(MJPC_B200_ERR_BAD_ARGUMENT, "plant_set_disturbance: a std must be finite and >= 0");
+    if (std_ > 0 && (!finite_f(rate) || !((float)rate > 0)))
+      return fail(MJPC_B200_ERR_BAD_ARGUMENT, "plant_set_disturbance: a rate must be finite and > 0 where its std is > 0");
+  }
+  PlantBank& k = *h->plants;
+  PlantDisturbance d = k.dist[plant];
+  d.ctrl_std = (float)ctrl_std; d.ctrl_rate = (float)ctrl_rate; d.xfrc_std = (float)xfrc_std; d.xfrc_rate = (float)xfrc_rate;
+  d.seed = seed;
+  if (int rc = plant_zero_noise(h, plant)) return rc;
+  CUDA_TRY(cudaMemcpy((PlantDisturbance*)k.a.dist + plant, &d, sizeof(d), cudaMemcpyHostToDevice));
+  k.dist[plant] = d;
+  return 0;
+}
+
+int mjpc_b200_plant_set_xfrc(mjpc_b200_t* h, int plant, const float* xfrc) {
+  if (int rc = plant_check(h, plant, "plant_set_xfrc")) return rc;
+  const size_t nx = 6 * (size_t)h->pack.M.nbody;
+  std::vector<float> w(nx, 0.f);
+  if (xfrc) w.assign(xfrc, xfrc + nx);
+  int held = 0;
+  for (float x : w) {
+    if (!std::isfinite(x)) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "plant_set_xfrc: non-finite wrench");
+    held |= x != 0.f;
+  }
+  PlantBank& k = *h->plants;
+  PlantDisturbance d = k.dist[plant];
+  d.held = held;
+  CUDA_TRY(cudaSetDevice(h->device));
+  CUDA_TRY(cudaStreamSynchronize(h->stream));
+  CUDA_TRY(cudaMemcpy((float*)k.a.xfrc_held + plant * nx, w.data(), nx * 4, cudaMemcpyHostToDevice));
+  CUDA_TRY(cudaMemcpy((PlantDisturbance*)k.a.dist + plant, &d, sizeof(d), cudaMemcpyHostToDevice));
+  k.dist[plant] = d;
+  return 0;
+}
+
+int mjpc_b200_plant_get_disturbance(mjpc_b200_t* h, int plant, float* ctrl_noise, float* xfrc_noise) {
+  if (int rc = plant_check(h, plant, "plant_get_disturbance")) return rc;
+  const PlantArgs& a = h->plants->a;
+  const size_t nu = h->pack.M.nu, nx = 6 * (size_t)h->pack.M.nbody;
+  CUDA_TRY(cudaSetDevice(h->device));
+  CUDA_TRY(cudaStreamSynchronize(h->stream));
+  if (ctrl_noise && nu) CUDA_TRY(cudaMemcpy(ctrl_noise, a.ctrl_noise + plant * nu, nu * 4, cudaMemcpyDeviceToHost));
+  if (xfrc_noise) CUDA_TRY(cudaMemcpy(xfrc_noise, a.xfrc_noise + plant * nx, nx * 4, cudaMemcpyDeviceToHost));
+  return 0;
+}
+
+int mjpc_b200_plant_last_ctrl(mjpc_b200_t* h, float* ctrl_out) {
+  if (!h || !ctrl_out) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "plant_last_ctrl: bad argument");
+  if (!h->plants) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "plant_last_ctrl: no plants (plant_init)");
+  if (int rc = check_ensemble(h, "plant_last_ctrl")) return rc;
+  const PlantBank& k = *h->plants;
+  // the last step's outputs, in the pinned staging since its download (zeros before the first step)
+  std::memcpy(ctrl_out, k.h_stage + k.in_bytes + k.o_ctrl_out, (size_t)k.a.B * h->pack.M.nu * 4);
   return 0;
 }
 

@@ -170,10 +170,11 @@ __device__ __forceinline__ void write_traces(Ctx& c, float* out) {
   }
 }
 
-// Injected noise of NoisyRollout: Philox4x32-10, key (seed, 1), counter (step, stream, element, 'XFRC'), Box-Muller on
-// the first two words - the definition of oracle/rollout.h (xfrc_normal), evaluated in fp32 here.
-__device__ __forceinline__ float xfrc_normal(unsigned seed, unsigned step, unsigned stream, unsigned element) {
-  unsigned c0 = step, c1 = stream, c2 = element, c3 = 0x58465243u, k0 = seed, k1 = 1u;
+// A standard normal from Philox4x32-10 with key (k0, k1) on counter (c0, c1, c2, c3), Box-Muller on the first two
+// output words.  Key word 1 names the stream's owner: 0 the knots (host), 1 the rollouts' force noise, 2 the plants'
+// disturbances, so no two of them ever draw the same numbers.
+__device__ __forceinline__ float philox_normal(unsigned c0, unsigned c1, unsigned c2, unsigned c3, unsigned k0,
+                                               unsigned k1) {
 #pragma unroll
   for (int r = 0; r < 10; r++) {
     const unsigned hi0 = __umulhi(0xD2511F53u, c0), lo0 = 0xD2511F53u * c0;
@@ -184,6 +185,12 @@ __device__ __forceinline__ float xfrc_normal(unsigned seed, unsigned step, unsig
   }
   const float u1 = ((float)c0 + 0.5f) * 2.3283064365386963e-10f, u2 = ((float)c1 + 0.5f) * 2.3283064365386963e-10f;
   return sqrtf(-2.0f * logf(fmaxf(u1, 1e-12f))) * cospif(2.0f * u2);
+}
+
+// Injected noise of NoisyRollout: key (seed, 1), counter (step, stream, element, 'XFRC') - the definition of
+// oracle/rollout.h (xfrc_normal), evaluated in fp32 here.
+__device__ __forceinline__ float xfrc_normal(unsigned seed, unsigned step, unsigned stream, unsigned element) {
+  return philox_normal(step, stream, element, 0x58465243u, seed, 1u);
 }
 
 // The task warp of a rollout CTA (StaticSpec<K, W, 1>): per step, between the main warp's fork / join barriers,
@@ -592,8 +599,25 @@ extern "C" __global__ void __launch_bounds__(32) step_batch_kernel_humanoid_trac
 // step of a running plant whose next qpos, qvel and qacc are finite is committed in place (state, warm start carried
 // as MuJoCo's qacc_warmstart, time, cost sum, step and warning counts); otherwise the plant becomes PLANT_DIVERGED and
 // keeps what it had.  A plant that is not running is not stepped.  The outputs of a plant that did not step hold its
-// state and time, cost 0 and zero sensors.
+// state and time, cost 0 and zero sensors; its applied ctrl is the ctrl its step was given (commanded + control noise),
+// or the commanded ctrl when it is not running.  The disturbances' OU states advance only with a committed step.
 enum PlantStatus { PLANT_RUNNING = 0, PLANT_DIVERGED = 1, PLANT_IDLE = 2 };
+
+// A plant's disturbances (mjpc_b200_plant_set_disturbance / _set_xfrc): Ornstein-Uhlenbeck control noise and body-force
+// noise (std 0: off; the rate is the time constant in seconds), the key of its noise stream and whether it holds a
+// non-zero wrench
+struct PlantDisturbance {
+  float ctrl_std, ctrl_rate, xfrc_std, xfrc_rate;
+  unsigned seed;
+  int held;
+};
+
+// Plant noise: Philox key (seed, 2), counter (committed step count, 0, element, tag)
+constexpr unsigned kPlantTagCtrl = 0x4354524Cu;   // 'CTRL'
+constexpr unsigned kPlantTagXfrc = 0x58465243u;   // 'XFRC'
+__device__ __forceinline__ float plant_normal(unsigned seed, unsigned step, unsigned element, unsigned tag) {
+  return philox_normal(step, 0u, element, tag, seed, 2u);
+}
 
 struct PlantArgs {
   DevModel M;
@@ -614,7 +638,59 @@ struct PlantArgs {
   float* state_out; double* time_out; float* cost_out; int* status_out;
   // optional (sensordata NULL: not evaluated): sensors [0, nsensor) of the pre-step state, [B][sensor_dim]
   const DevSensor* sensors; int nsensor, sensor_adr0, sensor_dim; float* sensordata;
+  // disturbances: settings dist [B]; OU states ctrl_noise [B][nu] and xfrc_noise [B][6 nbody]; the held wrench
+  // xfrc_held [B][6 nbody]; noise_next [B][nu + 6 nbody], this step's OU states until the step is committed
+  const PlantDisturbance* dist; float* ctrl_noise; float* xfrc_noise; const float* xfrc_held; float* noise_next;
+  float* ctrl_out;   // output: the applied ctrl [B][nu] (commanded + control noise)
 };
+
+// The disturbances of plant b's coming step, between load_state and k_forward (app.cc:291-304, 95-101, 323-352):
+// control noise n <- r n + s z (r = exp(-timestep / rate), s = std sqrt(1 - r^2)) added to the ctrl, which actuation
+// clamps as any ctrl; xfrc = the held wrench + the force noise's state under the same recursion.  The advanced states go
+// to noise_next; the applied ctrl is written out.
+template <class SP>
+__device__ __forceinline__ void plant_disturb(Ctx& c, const PlantArgs& A, int b) {
+  auto&& M = SP::model(c);
+  const int lane = c.lane, nu = M.nu, nx = 6 * M.nbody;
+  const PlantDisturbance& d = A.dist[b];
+  const unsigned step = (unsigned)A.steps[b];
+  float* next = A.noise_next + (size_t)b * (nu + nx);
+  if (d.ctrl_std > 0.f) {
+    const float r = expf(-CM(c).timestep / d.ctrl_rate), s = d.ctrl_std * sqrtf(1.f - r * r);
+    const float* n = A.ctrl_noise + (size_t)b * nu;
+    for (int i = lane; i < nu; i += 32) {
+      const float v = r * n[i] + s * plant_normal(d.seed, step, (unsigned)i, kPlantTagCtrl);
+      next[i] = v;
+      DF(ctrl)[i] += v;
+    }
+  }
+  for (int i = lane; i < nu; i += 32) A.ctrl_out[(size_t)b * nu + i] = DF(ctrl)[i];
+  const float* held = A.xfrc_held + (size_t)b * nx;
+  if (d.xfrc_std > 0.f) {
+    const float r = expf(-CM(c).timestep / d.xfrc_rate), s = d.xfrc_std * sqrtf(1.f - r * r);
+    const float* n = A.xfrc_noise + (size_t)b * nx;
+    for (int i = lane; i < nx; i += 32) {
+      const float v = r * n[i] + s * plant_normal(d.seed, step, (unsigned)i, kPlantTagXfrc);
+      next[nu + i] = v;
+      DF(xfrc)[i] = held[i] + v;
+    }
+    c.xfrc_on = 1;
+  } else if (d.held) {
+    for (int i = lane; i < nx; i += 32) DF(xfrc)[i] = held[i];
+    c.xfrc_on = 1;
+  }
+}
+
+// a committed step advances plant b's OU states to noise_next (each lane copies what it wrote in plant_disturb)
+__device__ __forceinline__ void plant_commit_noise(const PlantArgs& A, int b, int lane) {
+  const PlantDisturbance& d = A.dist[b];
+  const int nu = A.M.nu, nx = 6 * A.M.nbody;
+  const float* next = A.noise_next + (size_t)b * (nu + nx);
+  if (d.ctrl_std > 0.f)
+    for (int i = lane; i < nu; i += 32) A.ctrl_noise[(size_t)b * nu + i] = next[i];
+  if (d.xfrc_std > 0.f)
+    for (int i = lane; i < nx; i += 32) A.xfrc_noise[(size_t)b * nx + i] = next[nu + i];
+}
 
 template <class SP>
 __device__ __forceinline__ void plant_body(const PlantArgs& A) {
@@ -636,6 +712,7 @@ __device__ __forceinline__ void plant_body(const PlantArgs& A) {
     load_state<SP>(c, A.qpos + (size_t)b * nq, A.qvel + (size_t)b * nv, A.ctrl + (size_t)b * M.nu,
                    A.warm + (size_t)b * nv, A.mocap + (size_t)b * 7 * M.nmocap);
     for (int i = lane; i < 6 * M.nbody; i += 32) DF(xfrc)[i] = 0;
+    plant_disturb<SP>(c, A, b);
     __syncwarp();   // c.time stays 0: the task state was rebased to the plant's time
     if (!(k_bad(c, DF(qpos), nq) || k_bad(c, DF(qvel), nv))) {
       // step_batch_body's sequence (written out again: through one shared function the step_batch instances compile
@@ -650,6 +727,7 @@ __device__ __forceinline__ void plant_body(const PlantArgs& A) {
       stepped = !(k_bad(c, DF(qpos), nq) || k_bad(c, DF(qvel), nv) || k_bad(c, DF(qacc), nv));
     }
     if (stepped) {
+      plant_commit_noise(A, b, lane);
       for (int i = lane; i < nq; i += 32) A.qpos[(size_t)b * nq + i] = DF(qpos)[i];
       for (int i = lane; i < nv; i += 32) { A.qvel[(size_t)b * nv + i] = DF(qvel)[i]; A.warm[(size_t)b * nv + i] = DF(qacc)[i]; }
       if (lane == 0) {
@@ -664,6 +742,8 @@ __device__ __forceinline__ void plant_body(const PlantArgs& A) {
     __syncwarp();
   }
   const int lane = threadIdx.x, nq = A.M.nq, ds = nq + A.M.nv;
+  if (!running)
+    for (int i = lane; i < A.M.nu; i += 32) A.ctrl_out[(size_t)b * A.M.nu + i] = A.ctrl[(size_t)b * A.M.nu + i];
   for (int i = lane; i < ds; i += 32)
     A.state_out[(size_t)b * ds + i] = i < nq ? A.qpos[(size_t)b * nq + i] : A.qvel[(size_t)b * A.M.nv + i - nq];
   if (A.sensordata && !stepped)

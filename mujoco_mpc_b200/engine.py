@@ -71,6 +71,8 @@ EXPORTS = ["mjpc_b200_version", "mjpc_b200_last_error", "mjpc_b200_create", "mjp
            "mjpc_b200_select_model_variants", "mjpc_b200_batch_planner_set_models",
            "mjpc_b200_batch_estimator_set_models", "mjpc_b200_plant_init", "mjpc_b200_plant_reset",
            "mjpc_b200_plant_set", "mjpc_b200_plant_set_task", "mjpc_b200_plant_step", "mjpc_b200_plant_get",
+           "mjpc_b200_plant_set_disturbance", "mjpc_b200_plant_set_xfrc", "mjpc_b200_plant_get_disturbance",
+           "mjpc_b200_plant_last_ctrl",
            "mjpc_b200_set_model_ensemble", "mjpc_b200_fetch_ensemble", "mjpc_b200_fetch_trajectory_member",
            "mjpc_b200_host_ensemble_score", "mjpc_b200_planner_set_ensemble", "mjpc_b200_batch_planner_set_ensemble"]
 
@@ -765,7 +767,8 @@ class CppPlantBank:
     running plant by one mj_step in one launch, each on its own model once set_models gave it one.  A plant is idle
     until reset(); a plant whose step would leave a non-finite state becomes PLANT_DIVERGED, keeps its last state and
     is skipped until reset() (MuJoCo would reset it silently).  sensor_start / nsensor (0: none) choose the measurement
-    sensors step() returns for each pre-step state."""
+    sensors step() returns for each pre-step state.  set_disturbance() and set_xfrc() disturb a plant with the
+    reference app's Ornstein-Uhlenbeck control noise, body-force noise and a held wrench."""
 
     def __init__(self, model, num_plants, sensor_start=None, nsensor=0, device=0):
         self.lib = load_library()
@@ -830,9 +833,30 @@ class CppPlantBank:
         bufs, arr, n = _model_blobs(models)
         self._check(self.lib.mjpc_b200_set_model_variants(self.h, arr, n))
 
+    def set_disturbance(self, plant, ctrl_std=0.0, ctrl_rate=1.0, xfrc_std=0.0, xfrc_rate=1.0, seed=0):
+        """Plant `plant`'s OU control noise and body-force noise (std 0: off; rate: the time constant in seconds) and
+        the seed of its noise stream; its noise states restart from zero."""
+        self._check(self.lib.mjpc_b200_plant_set_disturbance(self.h, int(plant), C.c_double(ctrl_std),
+                                                             C.c_double(ctrl_rate), C.c_double(xfrc_std),
+                                                             C.c_double(xfrc_rate), C.c_uint32(seed)))
+
+    def set_xfrc(self, plant, xfrc=None):
+        """The wrench [nbody][6] (force, torque; world frame, at each body's centre of mass) held on plant `plant` from
+        the next step until changed; None clears it."""
+        w = None if xfrc is None else np.ascontiguousarray(np.asarray(xfrc, np.float32).reshape(self.m.nbody * 6))
+        self._check(self.lib.mjpc_b200_plant_set_xfrc(self.h, int(plant), _pf(w)))
+
+    def disturbance(self, plant):
+        """dict(ctrl_noise [nu], xfrc_noise [nbody][6]): the plant's OU states after its last committed step."""
+        m = self.m
+        u, x = np.zeros(m.nu, np.float32), np.zeros((m.nbody, 6), np.float32)
+        self._check(self.lib.mjpc_b200_plant_get_disturbance(self.h, int(plant), _pf(u), _pf(x)))
+        return dict(ctrl_noise=u, xfrc_noise=x)
+
     def step(self, ctrl):
         """One step of every running plant from ctrl [num_plants][nu]: dict(state [B][nq+nv], time [B], cost [B] (the
-        pre-step residual's cost; 0 where the plant did not step), sensordata [B][dim], status [B])."""
+        pre-step residual's cost; 0 where the plant did not step), sensordata [B][dim], status [B], ctrl [B][nu] (the
+        ctrl each plant applied: commanded + control noise))."""
         B, m = self.num_plants, self.m
         u = np.ascontiguousarray(np.asarray(ctrl, np.float32).reshape(B, m.nu))
         o = dict(state=np.zeros((B, m.nq + m.nv), np.float32), time=np.zeros(B), cost=np.zeros(B, np.float32),
@@ -840,6 +864,8 @@ class CppPlantBank:
         self._check(self.lib.mjpc_b200_plant_step(self.h, _pf(u), _pf(o["state"]), _pd(o["time"]), _pf(o["cost"]),
                                                   _pf(o["sensordata"]) if self.nsensordata else None,
                                                   o["status"].ctypes.data_as(_ip)))
+        o["ctrl"] = np.zeros((B, m.nu), np.float32)
+        self._check(self.lib.mjpc_b200_plant_last_ctrl(self.h, _pf(o["ctrl"])))
         return o
 
     def get(self, plant):

@@ -59,9 +59,11 @@ class SensorOracle:
             lib().sensor_oracle_destroy(self.h)
             self.h = None
 
-    def step(self, qpos, qvel, ctrl, mocap, times, start, count, warmstart=None):
+    def step(self, qpos, qvel, ctrl, mocap, times, start, count, warmstart=None, xfrc=None):
+        """B single steps; xfrc: None or xfrc_applied [B][nbody][6] for the step."""
         m = self.m
         q, v, u, mc, t, ws = _d(qpos), _d(qvel), _d(ctrl), _d(mocap), _d(times), _d(warmstart)
+        xf = None if xfrc is None else np.ascontiguousarray(np.asarray(xfrc, np.float64).reshape(-1, 6 * m.nbody))
         B = q.shape[0]
         dim = int(np.sum(m.sensor_dim[start:start + count])) if count > 0 else 0
         o = dict(next_qpos=np.zeros((B, m.nq)), next_qvel=np.zeros((B, m.nv)), qacc=np.zeros((B, m.nv)),
@@ -69,7 +71,7 @@ class SensorOracle:
         counts = np.zeros((B, 4), np.int32)
         rc = lib().sensor_oracle_step(self.h, B, _p(q), _p(v), _p(u), _p(ws), _p(mc), _p(t), int(start), int(count),
                                       _p(o["next_qpos"]), _p(o["next_qvel"]), _p(o["qacc"]), _p(o["sensordata"]),
-                                      counts.ctypes.data_as(C.POINTER(C.c_int)))
+                                      counts.ctypes.data_as(C.POINTER(C.c_int)), _p(xf))
         if rc != 0:
             raise ValueError("sensor_oracle_step: sensor range [%d, %d) not evaluated" % (start, start + count))
         o.update(ncon=counts[:, 0], nefc=counts[:, 1], niter=counts[:, 2], warning=counts[:, 3])

@@ -1,6 +1,7 @@
 // TEST INFRASTRUCTURE - measurement sensors on the CPU oracle (oracle/physics.h), fp64 or fp32.
 //
-// The same single step as the oracle's step_batch (forward, warning on a bad qacc, warm start from qacc, Euler) plus
+// The same single step as the oracle's step_batch (forward, warning on a bad qacc, warm start from qacc, Euler), with an
+// optional xfrc_applied [B][nbody][6] for the step (mj_xfrcAccumulate, as the plants' disturbances apply it), plus
 // the measurement sensors [start, start + count) of each pre-step state, read after the constraint solve as mj_step's
 // sensor stage reads them:
 //   jointpos / jointvel  qpos[jnt_qposadr] / qvel[jnt_dofadr]
@@ -318,7 +319,7 @@ void sensors(const Model<T>& m, const Data<T>& d, const Table& tab, int start, i
 template <class T>
 int step(Sim<T>& sim, const Table& tab, int B, const double* qpos, const double* qvel, const double* ctrl,
          const double* warmstart, const double* mocap, const double* times, int start, int count, double* next_qpos,
-         double* next_qvel, double* qacc, double* sensordata, int* counts) {
+         double* next_qvel, double* qacc, double* sensordata, int* counts, const double* xfrc) {
   const Model<T>& m = sim.model;
   Data<T>& d = sim.data;
   const int nq = m.nq, nv = m.nv, nu = m.nu;
@@ -333,7 +334,8 @@ int step(Sim<T>& sim, const Table& tab, int B, const double* qpos, const double*
     }
     for (int i = 0; i < nv; i++) d.qacc_warmstart[i] = warmstart ? (T)warmstart[(size_t)b * nv + i] : (T)0;
     std::fill(d.xfrc_applied.begin(), d.xfrc_applied.end(), (T)0);
-    d.xfrc_active = false;
+    d.xfrc_active = xfrc != nullptr;
+    if (xfrc) for (int i = 0; i < 6 * m.nbody; i++) d.xfrc_applied[i] = (T)xfrc[(size_t)b * 6 * m.nbody + i];
     d.time = (T)times[b];
     d.warning = false;
     forward<T>(m, d, nullptr);
@@ -372,18 +374,20 @@ void* sensor_oracle_create(const void* blob, size_t nbytes, int precision) {
 void sensor_oracle_destroy(void* h) { delete (Handle*)h; }
 
 // B single steps; sensordata [B][dim of sensors start .. start + count); returns 0, or -1 when a sensor in the range
-// is not evaluated (type, or a non-sphere touch zone) or the range is outside the model's sensors
+// is not evaluated (type, or a non-sphere touch zone) or the range is outside the model's sensors.  xfrc NULL: no
+// applied wrench.
 int sensor_oracle_step(void* hv, int B, const double* qpos, const double* qvel, const double* ctrl,
                        const double* warmstart, const double* mocap, const double* times, int start, int count,
-                       double* next_qpos, double* next_qvel, double* qacc, double* sensordata, int* counts) {
+                       double* next_qpos, double* next_qvel, double* qacc, double* sensordata, int* counts,
+                       const double* xfrc) {
   Handle* h = (Handle*)hv;
   if (start < 0 || count < 0 || start + count > (int)h->tab.type.size()) return -1;
   try {
     if (h->precision == 64)
       return step(*h->s64, h->tab, B, qpos, qvel, ctrl, warmstart, mocap, times, start, count, next_qpos, next_qvel,
-                  qacc, sensordata, counts);
+                  qacc, sensordata, counts, xfrc);
     return step(*h->s32, h->tab, B, qpos, qvel, ctrl, warmstart, mocap, times, start, count, next_qpos, next_qvel, qacc,
-                sensordata, counts);
+                sensordata, counts, xfrc);
   } catch (const std::exception&) {
     return -1;
   }
