@@ -306,8 +306,11 @@ int mjpc_b200_step_batch(mjpc_b200_t* h, int B, const float* qpos, const float* 
  * site, body (inertial frame), xbody or geom; subtreecom / subtreelinvel / subtreeangmom of a body; touch with a sphere
  * site zone; accelerometer / velocimeter / gyro of a site (in the site frame); ballquat / ballangvel of a ball joint;
  * jointactuatorfrc of a slide or hinge joint; actuatorpos / actuatorvel (joint or fixed-tendon transmission) and
- * actuatorfrc; tendonpos / tendonvel of a fixed tendon.  Not evaluated (MJPC_B200_ERR_UNSUPPORTED, the last error
- * naming the sensor): user, force, torque, rangefinder, magnetometer, camprojection, limit and constraint force,
+ * actuatorfrc; tendonpos / tendonvel of a fixed tendon; magnetometer of a site (site_xmat' opt.magnetic, the blob's
+ * opt_magnetic or MuJoCo's default 0 -0.5 0); rangefinder of a site (mj_ray along the site's z axis over the geoms not
+ * of the site's body whose alpha, the blob's geom_alpha, is not 0: the least distance, or -1; refused when such a geom
+ * is a height field or another type rays are not cast against).  Not evaluated (MJPC_B200_ERR_UNSUPPORTED, the last
+ * error naming the sensor): user, force, torque, camprojection, limit and constraint force,
  * energy and clock sensors, touch with another zone, and any sensor with a cutoff.  The same set and refusals hold for
  * plant_init's sensor range and for the estimators' (unscented_create, kalman_create, batch_estimator_create).
  * warmstart [B][nv] may be NULL (zeros); mocap [7 nmocap] is required when

@@ -45,7 +45,13 @@ _F_ARRAYS = ["opt_gravity", "body_pos", "body_quat", "body_ipos", "body_iquat", 
              "tendon_range", "tendon_margin", "tendon_solref", "tendon_solimp", "tendon_invweight0", "site_size", "sensor_cutoff"]
 
 
+# written only for a model with a magnetometer or a rangefinder, so that every other model's blob stays as it was:
+# opt.magnetic, and the alpha mj_ray reads per geom (its material's when it has one, else its rgba's)
+_F_RAY_FIELD = ["opt_magnetic", "geom_alpha"]
+
+
 def to_blob(model) -> bytes:
+    from .mjcf import SENS_RAY_FIELD
     entries = []
     for k in _INT_SCALARS:
         entries.append((k, 0, np.array([int(model.get(k, 0))], np.int32)))
@@ -55,6 +61,9 @@ def to_blob(model) -> bytes:
         entries.append((k, 0, np.ascontiguousarray(np.asarray(model.get(k, np.zeros(0)), np.int32).reshape(-1))))
     for k in _F_ARRAYS:
         entries.append((k, 1, np.ascontiguousarray(np.asarray(model.get(k, np.zeros(0)), np.float64).reshape(-1))))
+    if np.isin(np.asarray(model.get("sensor_type", np.zeros(0))), SENS_RAY_FIELD).any():
+        for k in _F_RAY_FIELD:
+            entries.append((k, 1, np.ascontiguousarray(np.asarray(model[k], np.float64).reshape(-1))))
     header_size = 16 + len(entries) * 56
     payload = bytearray()
     table = bytearray()

@@ -683,15 +683,83 @@ enum { SENS_FRAMEPOS = 1, SENS_JOINTPOS = 2, SENS_TOUCH = 3, SENS_SUBTREECOM = 4
        SENS_GYRO = 12, SENS_FRAMEANGVEL = 13, SENS_FRAMEXAXIS = 14, SENS_FRAMEYAXIS = 15, SENS_FRAMEZAXIS = 16,
        SENS_FRAMELINACC = 17, SENS_FRAMEANGACC = 18, SENS_SUBTREEANGMOM = 19, SENS_BALLQUAT = 20,
        SENS_BALLANGVEL = 21, SENS_JOINTACTUATORFRC = 22, SENS_ACTUATORPOS = 23, SENS_ACTUATORVEL = 24,
-       SENS_ACTUATORFRC = 25, SENS_TENDONPOS = 26, SENS_TENDONVEL = 27 };
-struct DevSensor { int type, objtype, objid, adr; float radius; };
+       SENS_ACTUATORFRC = 25, SENS_TENDONPOS = 26, SENS_TENDONVEL = 27, SENS_MAGNETOMETER = 28,
+       SENS_RANGEFINDER = 29 };
+// field: a magnetometer's opt.magnetic.  A rangefinder's ngeom eligible geoms (ray_sensor_geoms) are ints stored
+// geom0 ints after the start of its own row, in the same allocation as the table, so a row read from any slice of the
+// table finds them.
+struct DevSensor { int type, objtype, objid, adr; float radius; float field[3]; int geom0, ngeom; };
 // sensordata entries of one measured sensor
 __host__ __device__ inline int sensor_dim(int type) {
   if (type == SENS_FRAMEQUAT || type == SENS_BALLQUAT) return 4;
   return type == SENS_JOINTPOS || type == SENS_JOINTVEL || type == SENS_TOUCH || type == SENS_JOINTACTUATORFRC ||
                  type == SENS_ACTUATORPOS || type == SENS_ACTUATORVEL || type == SENS_ACTUATORFRC ||
-                 type == SENS_TENDONPOS || type == SENS_TENDONVEL
+                 type == SENS_TENDONPOS || type == SENS_TENDONVEL || type == SENS_RANGEFINDER
              ? 1 : 3;
+}
+
+// The distance along the ray pnt + x vec to geom `type` (any type a rangefinder casts against), or -1 when the ray
+// misses it.  Plane, sphere and box are ray_geom's, which stays as it is (the Quadruped residual's Ground inlines it into
+// the rollouts); capsule, ellipsoid and cylinder are added here, in the geom's frame (lp, lv), as mju_rayGeom does:
+//   capsule   size (r, h): the side |z| <= h of the infinite cylinder x^2 + y^2 = r^2, and the cap spheres of radius r
+//             at z = +-h beyond the side (z * s >= h for the cap at s h)
+//   ellipsoid size (a, b, c): the unit sphere in coordinates scaled by 1 / size
+//   cylinder  size (r, h): the side |z| <= h, and the flat ends z = +-h within x^2 + y^2 <= r^2
+// Each quadratic keeps its smallest non-negative root, so a ray starting inside reads the distance to the exit.
+__device__ __forceinline__ float ray_quadratic(float a, float b, float cc) {
+  const float det = b * b - a * cc;
+  if (det < 0 || a < kMinVal) return -1;
+  const float sq = sqrtf(det);
+  const float x0 = (-b - sq) / a, x1 = (-b + sq) / a;
+  return x0 >= 0 ? x0 : x1 >= 0 ? x1 : -1;
+}
+__device__ __forceinline__ float ray_min(float best, float x) { return x >= 0 && (best < 0 || x < best) ? x : best; }
+__device__ float ray_geom_sensor(const float* gpos, const float* gmat, const float* size, int type, const float* pnt,
+                                 const float* vec) {
+  if (type != GEOM_CAPSULE && type != GEOM_ELLIPSOID && type != GEOM_CYLINDER)
+    return ray_geom(gpos, gmat, size, type, pnt, vec);
+  float dp[3] = {pnt[0] - gpos[0], pnt[1] - gpos[1], pnt[2] - gpos[2]};
+  float lp[3], lv[3];
+  rot_vec_T(lp, gmat, dp);
+  rot_vec_T(lv, gmat, vec);
+  if (type == GEOM_ELLIPSOID) {
+    const float sp[3] = {lp[0] / size[0], lp[1] / size[1], lp[2] / size[2]};
+    const float sv[3] = {lv[0] / size[0], lv[1] / size[1], lv[2] / size[2]};
+    return ray_quadratic(dot3(sv, sv), dot3(sv, sp), dot3(sp, sp) - 1);
+  }
+  const float r = size[0], h = size[1];
+  float best = -1;
+  // side: the roots of the infinite cylinder within |z| <= h
+  {
+    const float a = lv[0] * lv[0] + lv[1] * lv[1], b = lv[0] * lp[0] + lv[1] * lp[1];
+    const float cc = lp[0] * lp[0] + lp[1] * lp[1] - r * r, det = b * b - a * cc;
+    if (a >= kMinVal && det >= 0) {
+      const float sq = sqrtf(det);
+      for (int k = -1; k <= 1; k += 2) {
+        const float x = (-b + (float)k * sq) / a;
+        if (x >= 0 && fabsf(lp[2] + x * lv[2]) <= h) best = ray_min(best, x);
+      }
+    }
+  }
+  for (int s = -1; s <= 1; s += 2) {
+    if (type == GEOM_CAPSULE) {
+      // cap sphere centred at z = s h, counted on its outer half only
+      const float q[3] = {lp[0], lp[1], lp[2] - (float)s * h};
+      const float b = dot3(lv, q), cc = dot3(q, q) - r * r, det = b * b - dot3(lv, lv) * cc;
+      if (det < 0) continue;
+      const float sq = sqrtf(det), a = dot3(lv, lv);
+      for (int k = -1; k <= 1; k += 2) {
+        const float x = (-b + (float)k * sq) / a;
+        if (x >= 0 && (float)s * (lp[2] + x * lv[2]) >= h) best = ray_min(best, x);
+      }
+    } else if (fabsf(lv[2]) > kMinVal) {
+      // flat end z = s h
+      const float x = ((float)s * h - lp[2]) / lv[2];
+      const float p0 = lp[0] + x * lv[0], p1 = lp[1] + x * lv[1];
+      if (x >= 0 && p0 * p0 + p1 * p1 <= r * r) best = ray_min(best, x);
+    }
+  }
+  return best;
 }
 
 // The post-constraint com-based acceleration of a body (mj_rnePostConstraint's cacc, without contact or applied
@@ -747,6 +815,12 @@ __device__ __forceinline__ void body_post_acc(Ctx& c, int body, float* a) {
 //                        or a fixed tendon's sum of wrap_coef qpos[wrap_qposadr] / wrap_coef qvel[wrap_dof]
 //   actuatorfrc          actuator_force[id], after the force limit
 //   tendonpos / -vel     the fixed tendon's length / velocity as above
+//   magnetometer         site_xmat' opt.magnetic (mj_sensorPos), opt.magnetic from the row's field
+//   rangefinder          mj_ray from site_xpos along the site's z axis (column 2 of site_xmat, unit length, so the ray
+//                        parameter is the distance) over the row's eligible geoms: every geom except those of the
+//                        site's body and those whose alpha is 0 (mj_ray with flg_static = 1, no group filter,
+//                        bodyexclude = the site's body).  The smallest non-negative distance, or -1 when none is hit.
+//                        Geom sizes and poses are the staged pack's and the data's, so a model variant's sizes count.
 template <class SP>
 __device__ __noinline__ void k_sensors(Ctx& c, const DevSensor* __restrict__ tab, int n, int adr0, float* out) {
   auto&& M = SP::model(c);
@@ -906,6 +980,25 @@ __device__ __noinline__ void k_sensors(Ctx& c, const DevSensor* __restrict__ tab
         for (int w = MI(tendon_adr)[id]; w < MI(tendon_adr)[id] + MI(tendon_num)[id]; w++) x += MF(wrap_coef)[w] * v[adr[w]];
       }
       o[0] = act ? MF(actuator_gear)[S.objid] * x : x;
+    } else if (S.type == SENS_MAGNETOMETER || S.type == SENS_RANGEFINDER) {
+      float qs[4], R[9];
+      quat_mul(qs, DF(xquat) + 4 * MI(site_bodyid)[S.objid], MF(site_quat) + 4 * S.objid);
+      quat2mat(R, qs);
+      if (S.type == SENS_MAGNETOMETER) {
+        rot_vec_T(o, R, S.field);
+      } else {
+        const float dir[3] = {R[2], R[5], R[8]};
+        const float* pnt = DF(site_xpos) + 3 * S.objid;
+        const int* geoms = reinterpret_cast<const int*>(tab + s) + S.geom0;
+        const int* gtype = MI(geom_type);
+        const float *gxpos = DF(geom_xpos), *gxmat = DF(geom_xmat), *gsize = MF(geom_size);
+        float best = -1;
+        for (int k = 0; k < S.ngeom; k++) {
+          const int g = geoms[k];
+          best = ray_min(best, ray_geom_sensor(gxpos + 3 * g, gxmat + 9 * g, gsize + 3 * g, gtype[g], pnt, dir));
+        }
+        o[0] = best;
+      }
     }
   }
   __syncwarp();

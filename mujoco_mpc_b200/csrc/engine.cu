@@ -147,6 +147,7 @@ struct mjpc_b200 {
   // device evaluates, else the reason it is not
   std::vector<DevSensor> sensors;
   std::vector<std::string> sensor_why;
+  std::vector<int> sensor_geoms;   // the rangefinders' eligible geoms, uploaded right after the rows
   DevSensor* d_sensors = nullptr;
   // persistent scratch of step_impl: device buffer and its pinned host staging, grown on demand
   float* d_step = nullptr;
@@ -237,7 +238,11 @@ int check_ensemble(const mjpc_b200* h, const char* call) {
 
 // The measurement-sensor table of a blob: one row per model sensor; why[i] is empty when sensor i is one the device
 // evaluates, else the reason it is not.  A blob without the sensor / site entries has no measurable sensors.
-void sensor_table(const Blob& b, std::vector<DevSensor>* sensors, std::vector<std::string>* why_out) {
+// ray_geoms gets the rangefinders' eligible-geom lists, which the device finds after the rows (DevSensor::geom0).
+// opt_magnetic and geom_alpha are in the blob only when the model has a magnetometer or a rangefinder (MuJoCo's
+// defaults otherwise: magnetic (0, -0.5, 0), every geom visible to rays).
+void sensor_table(const Blob& b, std::vector<DevSensor>* sensors, std::vector<std::string>* why_out,
+                  std::vector<int>* ray_geoms) {
   int dt, cnt; int64_t off;
   if (!b.find("nsensor", &dt, &cnt, &off) || !b.find("site_size", &dt, &cnt, &off)) return;
   const std::vector<int> ty = b.ints("sensor_type"), ot = b.ints("sensor_objtype"), oid = b.ints("sensor_objid"),
@@ -247,10 +252,15 @@ void sensor_table(const Blob& b, std::vector<DevSensor>* sensors, std::vector<st
   const std::vector<double> ss = b.reals("site_size");
   std::vector<double> cutoff(ty.size(), 0.0);
   if (b.find("sensor_cutoff", &dt, &cnt, &off)) cutoff = b.reals("sensor_cutoff");
+  std::vector<double> magnetic = {0.0, -0.5, 0.0};
+  if (b.find("opt_magnetic", &dt, &cnt, &off)) magnetic = b.reals("opt_magnetic");
+  const std::vector<int> gtype = b.ints("geom_type"), gbody = b.ints("geom_bodyid"), sbody = b.ints("site_bodyid");
+  std::vector<double> alpha(gtype.size(), 1.0);
+  if (b.find("geom_alpha", &dt, &cnt, &off)) alpha = b.reals("geom_alpha");
   const int ns = b.i("nsensor");
   auto slide_or_hinge = [&](int j) { return jt[j] == JNT_SLIDE || jt[j] == JNT_HINGE; };
   for (int i = 0; i < ns; i++) {
-    DevSensor S = {ty[i], ot[i], oid[i], adr[i], 0.f};
+    DevSensor S = {ty[i], ot[i], oid[i], adr[i], 0.f, {0.f, 0.f, 0.f}, 0, 0};
     std::string why;
     switch (ty[i]) {
       case SENS_JOINTPOS: case SENS_JOINTVEL:
@@ -286,18 +296,43 @@ void sensor_table(const Blob& b, std::vector<DevSensor>* sensors, std::vector<st
         break;
       case SENS_ACTUATORFRC: case SENS_TENDONPOS: case SENS_TENDONVEL:
         break;
+      case SENS_MAGNETOMETER:
+        if (ot[i] != OBJ_SITE) why = "magnetometer of an object other than a site";
+        for (int q = 0; q < 3; q++) S.field[q] = (float)magnetic[q];
+        break;
+      case SENS_RANGEFINDER: {
+        if (ot[i] != OBJ_SITE) { why = "rangefinder of an object other than a site"; break; }
+        // mj_ray's eligible geoms: not of the site's body, alpha not 0; every group, static geoms included
+        S.geom0 = (int)ray_geoms->size();
+        for (int g = 0; g < (int)gtype.size(); g++) {
+          if (gbody[g] == sbody[oid[i]] || alpha[g] == 0.0) continue;
+          if (gtype[g] != GEOM_PLANE && gtype[g] != GEOM_SPHERE && gtype[g] != GEOM_CAPSULE &&
+              gtype[g] != GEOM_ELLIPSOID && gtype[g] != GEOM_CYLINDER && gtype[g] != GEOM_BOX) {
+            why = "rangefinder: geom " + std::to_string(g) + " is of type " + std::to_string(gtype[g]) +
+                  ", which rays are not cast against (only plane, sphere, capsule, ellipsoid, cylinder and box)";
+            break;
+          }
+          ray_geoms->push_back(g);
+        }
+        S.ngeom = (int)ray_geoms->size() - S.geom0;
+        break;
+      }
       default:
         why = "sensor type " + std::to_string(ty[i]) +
               " (only jointpos, jointvel, framepos, framequat, framexaxis, frameyaxis, framezaxis, framelinvel, "
               "frameangvel, framelinacc, frameangacc, subtreecom, subtreelinvel, subtreeangmom, touch, accelerometer, "
-              "velocimeter, gyro, ballquat, ballangvel, jointactuatorfrc, actuatorpos, actuatorvel, actuatorfrc, "
-              "tendonpos and tendonvel are evaluated)";
+              "velocimeter, gyro, magnetometer, rangefinder, ballquat, ballangvel, jointactuatorfrc, actuatorpos, "
+              "actuatorvel, actuatorfrc, tendonpos and tendonvel are evaluated)";
     }
     if (why.empty() && dim[i] != sensor_dim(ty[i])) why = "unexpected sensor dimension";
     if (why.empty() && cutoff[i] != 0.0) why = "cutoff is not modelled";
     sensors->push_back(S);
     why_out->push_back(why);
   }
+  // geom0 from the start of the list to the start of the row: the list follows the n rows
+  const int row_words = (int)(sizeof(DevSensor) / sizeof(int));
+  for (int i = 0; i < (int)sensors->size(); i++)
+    if ((*sensors)[i].type == SENS_RANGEFINDER) (*sensors)[i].geom0 += ((int)sensors->size() - i) * row_words;
 }
 
 const char* const kFloatArrayNames[] = {
@@ -314,7 +349,7 @@ const char* const kIntArrayNames[] = {
 // set_model_variants' rule: the first field of variant V (packed, with its sensor table) that must equal the handle's
 // model as created and does not, or "" when V may stand in for it.  Floats compare bitwise.
 std::string variant_mismatch(const mjpc_b200* h, const ModelPack& V, const std::vector<DevSensor>& sensors,
-                             const std::vector<std::string>& why) {
+                             const std::vector<std::string>& why, const std::vector<int>& geoms) {
   const DevModel &M = h->M0, &W = V.M;
 #define X(n) if (W.n != M.n) return #n;
   MJPC_M_INTS(X)
@@ -340,9 +375,11 @@ std::string variant_mismatch(const mjpc_b200* h, const ModelPack& V, const std::
   for (size_t k = 0; k < sensors.size(); k++) {
     const DevSensor &x = sensors[k], &y = h->sensors[k];
     if (x.type != y.type || x.objtype != y.objtype || x.objid != y.objid || x.adr != y.adr ||
-        !same(&x.radius, &y.radius, 4) || why[k] != h->sensor_why[k])
+        !same(&x.radius, &y.radius, 4) || !same(x.field, y.field, 12) || x.geom0 != y.geom0 ||
+        x.ngeom != y.ngeom || why[k] != h->sensor_why[k])
       return "sensor " + std::to_string(k);
   }
+  if (geoms != h->sensor_geoms) return "the rangefinders' geoms";
   return "";
 }
 
@@ -647,7 +684,7 @@ int mjpc_b200_create(const mjpc_model_blob* model, int max_candidates, int max_h
     for (int d : b.ints("task_dim_norm_residual")) h->max_term_dim = std::max(h->max_term_dim, d);
   }
   h->time_idx = time_like_state(M.residual_id);
-  sensor_table(Blob(model->data, model->nbytes), &h->sensors, &h->sensor_why);
+  sensor_table(Blob(model->data, model->nbytes), &h->sensors, &h->sensor_why, &h->sensor_geoms);
   h->M0 = M; h->timestep0 = h->pack.timestep; h->f0 = h->pack.f;
   CREATE_TRY(cudaSetDevice(device));
   CREATE_TRY(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
@@ -684,9 +721,15 @@ int mjpc_b200_create(const mjpc_model_blob* model, int max_candidates, int max_h
   CREATE_TRY(dalloc(&h->d_costs, N * H)); CREATE_TRY(dalloc(&h->d_trace, N * H * 3 * (size_t)M.num_trace));
   CREATE_TRY(dalloc(&h->d_returns, N)); CREATE_TRY(dalloc(&h->d_failure, N)); CREATE_TRY(dalloc(&h->d_order, N)); CREATE_TRY(dalloc(&h->d_stats, 12 * N));
   CREATE_TRY(dalloc(&h->d_pair_sync, (size_t)256 * 32));
-  CREATE_TRY(dalloc(&h->d_sensors, h->sensors.size()));
-  if (!h->sensors.empty())
-    CREATE_TRY(cudaMemcpy(h->d_sensors, h->sensors.data(), h->sensors.size() * sizeof(DevSensor), cudaMemcpyHostToDevice));
+  {
+    // the rows, then the rangefinders' geom lists (DevSensor::geom0)
+    const size_t rows = h->sensors.size() * sizeof(DevSensor), list = h->sensor_geoms.size() * sizeof(int);
+    CREATE_TRY(dalloc(&h->d_sensors, h->sensors.size() + (list + sizeof(DevSensor) - 1) / sizeof(DevSensor)));
+    if (rows) CREATE_TRY(cudaMemcpy(h->d_sensors, h->sensors.data(), rows, cudaMemcpyHostToDevice));
+    if (list)
+      CREATE_TRY(cudaMemcpy(reinterpret_cast<char*>(h->d_sensors) + rows, h->sensor_geoms.data(), list,
+                            cudaMemcpyHostToDevice));
+  }
   h->h_in_floats = in_floats + H * (nu + ds + 1 + nu * n + nu) + N + 64;
   CREATE_TRY(cudaMallocHost((void**)&h->h_in, h->h_in_floats * 4));
   h->h_out_bytes = N * 16 + 64;
@@ -791,16 +834,17 @@ static int model_blocks(mjpc_b200_t* h, const mjpc_model_blob* models, int count
     if (!models[v].data) return fail(MJPC_B200_ERR_BAD_ARGUMENT, at + "NULL blob");
     std::vector<DevSensor> sensors;
     std::vector<std::string> why;
+    std::vector<int> geoms;
     try {
       packs[v] = pack_model(models[v].data, models[v].nbytes, M.maxcon - 2 * M.ntendon, M.maxefc);
       Blob b(models[v].data, models[v].nbytes);
       if (b.i("nuserdata") != 0)
         return fail(MJPC_B200_ERR_UNSUPPORTED, at + "mjData::userdata (nuserdata > 0) is not supported");
-      sensor_table(b, &sensors, &why);
+      sensor_table(b, &sensors, &why, &geoms);
     } catch (const std::exception& e) {
       return fail(MJPC_B200_ERR_BAD_BLOB, at + e.what());
     }
-    const std::string field = variant_mismatch(h, packs[v], sensors, why);
+    const std::string field = variant_mismatch(h, packs[v], sensors, why, geoms);
     if (!field.empty()) return fail(MJPC_B200_ERR_BAD_ARGUMENT, at + field + " differs from the handle's model");
     stride = std::max(stride, (size_t)(M.nf + M.ni) + packs[v].key_mpos.size() + 1);
   }

@@ -185,7 +185,7 @@ def measured_range(m, sensor_start, nsensor):
     for i in range(sensor_start, sensor_start + nsensor):
         if int(m.sensor_type[i]) not in SENS_MEASURED:
             raise EstimatorError("sensor %d (%s) is not a measured sensor type (jointpos, jointvel, touch, the frame, "
-                                 "subtree, IMU, ball-joint, actuator and tendon sensors)" % (i, m.sensor_names[i]))
+                                 "subtree, IMU, magnetometer, rangefinder, ball-joint, actuator and tendon sensors)" % (i, m.sensor_names[i]))
         if float(m.sensor_cutoff[i]) != 0.0:
             raise EstimatorError("sensor %d (%s): cutoff is not modelled" % (i, m.sensor_names[i]))
     return int(np.sum(m.sensor_dim[sensor_start:sensor_start + nsensor]))

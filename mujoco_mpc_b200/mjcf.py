@@ -37,15 +37,19 @@ SENS_USER, SENS_FRAMEPOS, SENS_JOINTPOS, SENS_TOUCH, SENS_SUBTREECOM, SENS_SUBTR
 SENS_FRAMEANGVEL, SENS_FRAMEXAXIS, SENS_FRAMEYAXIS, SENS_FRAMEZAXIS, SENS_FRAMELINACC, SENS_FRAMEANGACC, \
     SENS_SUBTREEANGMOM, SENS_BALLQUAT, SENS_BALLANGVEL, SENS_JOINTACTUATORFRC, SENS_ACTUATORPOS, SENS_ACTUATORVEL, \
     SENS_ACTUATORFRC, SENS_TENDONPOS, SENS_TENDONVEL = range(13, 28)
+SENS_MAGNETOMETER, SENS_RANGEFINDER = 28, 29
 SENS_TYPES = {"user": 0, "framepos": 1, "jointpos": 2, "touch": 3, "subtreecom": 4,
               "subtreelinvel": 5, "framelinvel": 6, "framequat": 7, "jointvel": 9, "accelerometer": 10,
               "velocimeter": 11, "gyro": 12, "frameangvel": 13, "framexaxis": 14, "frameyaxis": 15,
               "framezaxis": 16, "framelinacc": 17, "frameangacc": 18, "subtreeangmom": 19, "ballquat": 20,
               "ballangvel": 21, "jointactuatorfrc": 22, "actuatorpos": 23, "actuatorvel": 24, "actuatorfrc": 25,
-              "tendonpos": 26, "tendonvel": 27}
+              "tendonpos": 26, "tendonvel": 27, "magnetometer": 28, "rangefinder": 29}
 # what the measurement path (engine step_sensors, estimators) evaluates
 SENS_MEASURED = (SENS_FRAMEPOS, SENS_JOINTPOS, SENS_TOUCH, SENS_SUBTREECOM, SENS_SUBTREELINVEL, SENS_FRAMELINVEL,
-                 SENS_FRAMEQUAT, SENS_JOINTVEL, SENS_ACCELEROMETER, SENS_VELOCIMETER, SENS_GYRO) + tuple(range(13, 28))
+                 SENS_FRAMEQUAT, SENS_JOINTVEL, SENS_ACCELEROMETER, SENS_VELOCIMETER, SENS_GYRO) + tuple(range(13, 28)) + \
+    (SENS_MAGNETOMETER, SENS_RANGEFINDER)
+# the sensors that read opt.magnetic or cast rays: a model with one gets the blob entries opt_magnetic and geom_alpha
+SENS_RAY_FIELD = (SENS_MAGNETOMETER, SENS_RANGEFINDER)
 # the IMU sensors: 3-vectors in the frame of their site
 SENS_IMU = (SENS_ACCELEROMETER, SENS_VELOCIMETER, SENS_GYRO)
 # the frame sensors: objtype / objname name a body (inertial frame), an xbody, a geom or a site
@@ -56,7 +60,7 @@ SENS_DIM = {"framepos": 3, "jointpos": 1, "touch": 1, "subtreecom": 3, "subtreel
             "actuatorfrc": 1, "framexaxis": 3, "frameyaxis": 3, "framezaxis": 3, "velocimeter": 3,
             "gyro": 3, "accelerometer": 3, "actuatorpos": 1, "actuatorvel": 1, "tendonpos": 1,
             "tendonvel": 1, "framelinacc": 3, "frameangacc": 3, "ballquat": 4, "ballangvel": 3,
-            "jointactuatorfrc": 1}
+            "jointactuatorfrc": 1, "magnetometer": 3, "rangefinder": 1}
 OBJ_BODY, OBJ_XBODY, OBJ_GEOM, OBJ_SITE = range(4)
 
 MINVAL = 1e-15
@@ -305,7 +309,7 @@ class Compiler:
         opt = dict(timestep=0.002, gravity=[0, 0, -9.81], cone=0, impratio=1.0, tolerance=1e-8,
                    ls_tolerance=0.01, iterations=100, ls_iterations=50, integrator=0,
                    disable_contact=0, disable_eulerdamp=0, disable_frictionloss=0, disable_limit=0,
-                   disable_refsafe=0, disable_warmstart=0, o_margin=0.0)
+                   disable_refsafe=0, disable_warmstart=0, o_margin=0.0, magnetic=[0, -0.5, 0])
         for o in root.findall("option"):
             for k in ("timestep", "impratio", "tolerance", "ls_tolerance", "o_margin"):
                 if k in o.attrib:
@@ -313,8 +317,9 @@ class Compiler:
             for k in ("iterations", "ls_iterations"):
                 if k in o.attrib:
                     opt[k] = int(o.get(k))
-            if "gravity" in o.attrib:
-                opt["gravity"] = list(_f(o.get("gravity")))
+            for k in ("gravity", "magnetic"):
+                if k in o.attrib:
+                    opt[k] = list(_f(o.get(k)))
             if "cone" in o.attrib:
                 opt["cone"] = 1 if o.get("cone") == "elliptic" else 0
             if "integrator" in o.attrib:
@@ -343,7 +348,7 @@ class Compiler:
         self._parse_custom(m)
         self._parse_keys(m)
         for k, v in opt.items():
-            m["opt_" + k] = np.array(v, dtype=float) if k == "gravity" else v
+            m["opt_" + k] = np.array(v, dtype=float) if k in ("gravity", "magnetic") else v
         self._constants(m)
         self._pairs(m)
         self._task(m)
@@ -394,6 +399,12 @@ class Compiler:
         g_size = np.zeros((ng, 3)); g_pos = np.zeros((ng, 3)); g_quat = np.zeros((ng, 4))
         g_fric = np.zeros((ng, 3)); g_solmix = np.ones(ng); g_solref = np.zeros((ng, 2)); g_solimp = np.zeros((ng, 5))
         g_margin = np.zeros(ng); g_gap = np.zeros(ng)
+        # what mj_ray reads to skip a geom: the alpha of its material's rgba when it has a material, else of its rgba
+        mat_alpha = {}
+        for sec in self.root.findall("asset"):
+            for mat in sec.findall("material"):
+                mat_alpha[mat.get("name")] = float(_f(mat.get("rgba"), 4, [1, 1, 1, 1])[3])
+        g_alpha = np.ones(ng)
         g_massprops = []
         names = []
         for i, a in enumerate(self.geoms):
@@ -420,6 +431,10 @@ class Compiler:
             g_solmix[i] = float(a.get("solmix", 1)); g_solref[i] = _f(a.get("solref"), 2, [0.02, 1])
             g_solimp[i] = _f(a.get("solimp"), 5, [0.9, 0.95, 0.001, 0.5, 2])
             g_margin[i] = float(a.get("margin", 0)); g_gap[i] = float(a.get("gap", 0))
+            if a.get("material"):
+                g_alpha[i] = mat_alpha[a["material"]]
+            else:
+                g_alpha[i] = float(_f(a.get("rgba"), 4, [0.5, 0.5, 0.5, 1])[3])
             mass = float(a["mass"]) if "mass" in a else None
             g_massprops.append(_geom_inertia(t, size, float(a.get("density", 1000)), mass))
         m.ngeom = ng
@@ -427,6 +442,7 @@ class Compiler:
         m.geom_condim, m.geom_priority, m.geom_group = g_condim, g_prio, g_group
         m.geom_size, m.geom_pos, m.geom_quat, m.geom_friction = g_size, g_pos, g_quat, g_fric
         m.geom_solmix, m.geom_solref, m.geom_solimp, m.geom_margin, m.geom_gap = g_solmix, g_solref, g_solimp, g_margin, g_gap
+        m.geom_alpha = g_alpha
         rb = np.zeros(ng)
         for i in range(ng):
             s = g_size[i]
@@ -748,7 +764,7 @@ class Compiler:
                 s_objid[i] = m.actuator_names.index(ch.get("actuator"))
             elif tag in ("tendonpos", "tendonvel"):
                 s_objid[i] = m.tendon_names.index(ch.get("tendon"))
-            elif tag in ("touch", "accelerometer", "velocimeter", "gyro"):
+            elif tag in ("touch", "accelerometer", "velocimeter", "gyro", "magnetometer", "rangefinder"):
                 s_objtype[i], s_objid[i] = OBJ_SITE, m.site_names.index(ch.get("site"))
             cutoff[i] = float(ch.get("cutoff", 0))
         nuser = max([len(u) for u in users] + [0])

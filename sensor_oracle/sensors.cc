@@ -33,8 +33,14 @@
 //   actuatorpos / -vel   gear times the joint's qpos / qvel, or times the fixed tendon's length / velocity
 //   actuatorfrc          actuator_force (after the force limit)
 //   tendonpos / -vel     the fixed tendon's sum coef qpos / sum coef qvel
+//   magnetometer         site_xmat' opt.magnetic (MuJoCo's mj_sensorPos)
+//   rangefinder          mj_ray(pnt = site_xpos, vec = column 2 of site_xmat, geomgroup NULL, flg_static 1,
+//                        bodyexclude = the site's body): the least non-negative distance to a geom not of the site's
+//                        body whose alpha is not 0, or -1.  The ray-geom distances are restated below from the
+//                        surfaces' equations, in the precision of the model (fp32 arithmetic in the fp32 oracle).
 // The sensor table is read from the blob's sensor_* / site_* entries.  Written from the definition, independently of
 // the device's k_sensors; the oracle itself is not modified.
+#include <algorithm>
 #include <cmath>
 #include <cstring>
 #include <memory>
@@ -52,13 +58,147 @@ enum { SENS_FRAMEPOS = 1, SENS_JOINTPOS = 2, SENS_TOUCH = 3, SENS_SUBTREECOM = 4
        SENS_GYRO = 12, SENS_FRAMEANGVEL = 13, SENS_FRAMEXAXIS = 14, SENS_FRAMEYAXIS = 15, SENS_FRAMEZAXIS = 16,
        SENS_FRAMELINACC = 17, SENS_FRAMEANGACC = 18, SENS_SUBTREEANGMOM = 19, SENS_BALLQUAT = 20,
        SENS_BALLANGVEL = 21, SENS_JOINTACTUATORFRC = 22, SENS_ACTUATORPOS = 23, SENS_ACTUATORVEL = 24,
-       SENS_ACTUATORFRC = 25, SENS_TENDONPOS = 26, SENS_TENDONVEL = 27 };
+       SENS_ACTUATORFRC = 25, SENS_TENDONPOS = 26, SENS_TENDONVEL = 27, SENS_MAGNETOMETER = 28,
+       SENS_RANGEFINDER = 29 };
 enum { OBJ_BODY = 0, OBJ_XBODY = 1, OBJ_GEOM = 2, OBJ_SITE = 3 };
 
 struct Table {
   std::vector<int> type, objtype, objid, dim, adr, site_type;
   std::vector<double> site_size;
+  double magnetic[3] = {0, -0.5, 0};   // opt.magnetic, MuJoCo's default unless the blob has opt_magnetic
+  std::vector<double> geom_alpha;      // empty: every geom has alpha 1
 };
+
+// ----------------------------------------------------------------------------------------------- ray casting
+// t >= 0 of the ray p + t v (v unit) on each geom surface, in the geom's frame; -1: no such t.  A ray that starts
+// inside a closed surface hits it on the way out.
+template <class T>
+T smallest(T a, T b) { return a < 0 ? b : (b < 0 ? a : std::min(a, b)); }
+
+// plane z = 0, hit from its front (+z) side only, within |x| <= size0 and |y| <= size1 when those are positive
+template <class T>
+T ray_plane(const T* p, const T* v, const T* size) {
+  if (!(v[2] < 0)) return -1;
+  const T t = -p[2] / v[2];
+  if (t < 0) return -1;
+  const T x = p[0] + t * v[0], y = p[1] + t * v[1];
+  if ((size[0] > 0 && std::fabs(x) > size[0]) || (size[1] > 0 && std::fabs(y) > size[1])) return -1;
+  return t;
+}
+
+// |p + t v - c|^2 = r^2 in coordinates scaled by s (an ellipsoid of semi-axes s; a sphere: s = r, r = 1)
+template <class T>
+void quadric_roots(const T* p, const T* v, const T* c, const T* s, T* t0, T* t1) {
+  T a = 0, b = 0, cc = -1;
+  for (int k = 0; k < 3; k++) {
+    const T pk = (p[k] - c[k]) / s[k], vk = v[k] / s[k];
+    a += vk * vk; b += pk * vk; cc += pk * pk;
+  }
+  const T disc = b * b - a * cc;
+  *t0 = *t1 = -1;
+  if (disc < 0 || a <= 0) return;
+  *t0 = (-b - std::sqrt(disc)) / a;
+  *t1 = (-b + std::sqrt(disc)) / a;
+}
+
+template <class T>
+T ray_ellipsoid(const T* p, const T* v, const T* size) {
+  const T c[3] = {0, 0, 0};
+  T t0, t1;
+  quadric_roots(p, v, c, size, &t0, &t1);
+  return t0 >= 0 ? t0 : (t1 >= 0 ? t1 : T(-1));
+}
+
+// the lateral surface x^2 + y^2 = r^2, |z| <= h
+template <class T>
+T ray_tube(const T* p, const T* v, T r, T h) {
+  const T a = v[0] * v[0] + v[1] * v[1];
+  if (a <= 0) return -1;
+  const T b = p[0] * v[0] + p[1] * v[1], cc = p[0] * p[0] + p[1] * p[1] - r * r, disc = b * b - a * cc;
+  if (disc < 0) return -1;
+  T best = -1;
+  for (T t : {(-b - std::sqrt(disc)) / a, (-b + std::sqrt(disc)) / a})
+    if (t >= 0 && std::fabs(p[2] + t * v[2]) <= h) best = smallest(best, t);
+  return best;
+}
+
+// capsule: the tube and the two hemispherical caps of radius r centred at z = +-h (each beyond its end)
+template <class T>
+T ray_capsule(const T* p, const T* v, const T* size) {
+  const T r = size[0], h = size[1];
+  T best = ray_tube(p, v, r, h);
+  const T s[3] = {r, r, r};
+  for (int side = -1; side <= 1; side += 2) {
+    const T c[3] = {0, 0, side * h};
+    T t[2];
+    quadric_roots(p, v, c, s, &t[0], &t[1]);
+    for (T x : t)
+      if (x >= 0 && side * (p[2] + x * v[2]) >= h) best = smallest(best, x);
+  }
+  return best;
+}
+
+// cylinder: the tube and the two discs z = +-h of radius r
+template <class T>
+T ray_cylinder(const T* p, const T* v, const T* size) {
+  const T r = size[0], h = size[1];
+  T best = ray_tube(p, v, r, h);
+  if (v[2] != 0)
+    for (int side = -1; side <= 1; side += 2) {
+      const T t = (side * h - p[2]) / v[2], x = p[0] + t * v[0], y = p[1] + t * v[1];
+      if (t >= 0 && x * x + y * y <= r * r) best = smallest(best, t);
+    }
+  return best;
+}
+
+// box |x_k| <= size_k: each face plane x_k = +-size_k, hit inside the face's rectangle
+template <class T>
+T ray_box(const T* p, const T* v, const T* size) {
+  T best = -1;
+  for (int k = 0; k < 3; k++) {
+    if (v[k] == 0) continue;
+    for (int side = -1; side <= 1; side += 2) {
+      const T t = (side * size[k] - p[k]) / v[k];
+      if (t < 0) continue;
+      bool in = true;
+      for (int j = 0; j < 3; j++)
+        if (j != k && std::fabs(p[j] + t * v[j]) > size[j]) in = false;
+      if (in) best = smallest(best, t);
+    }
+  }
+  return best;
+}
+
+template <class T>
+double rangefinder(const Model<T>& m, const Data<T>& d, const Table& tab, int site) {
+  const int body = m.site_bodyid[site];
+  const T* R = &d.site_xmat[9 * site];
+  const T v[3] = {R[2], R[5], R[8]};
+  T best = -1;
+  for (int g = 0; g < m.ngeom; g++) {
+    if (m.geom_bodyid[g] == body || (!tab.geom_alpha.empty() && tab.geom_alpha[g] == 0)) continue;
+    // the ray in the geom's frame: geom_xmat' (pnt - geom_xpos), geom_xmat' vec
+    const T *gp = &d.geom_xpos[3 * g], *gm = &d.geom_xmat[9 * g], *size = &m.geom_size[3 * g];
+    T lp[3] = {0, 0, 0}, lv[3] = {0, 0, 0};
+    for (int a = 0; a < 3; a++)
+      for (int k = 0; k < 3; k++) {
+        lp[a] += gm[3 * k + a] * (d.site_xpos[3 * site + k] - gp[k]);
+        lv[a] += gm[3 * k + a] * v[k];
+      }
+    T t;
+    switch (m.geom_type[g]) {
+      case GEOM_PLANE: t = ray_plane(lp, lv, size); break;
+      case GEOM_SPHERE: { const T s[3] = {size[0], size[0], size[0]}; t = ray_ellipsoid(lp, lv, s); break; }
+      case GEOM_CAPSULE: t = ray_capsule(lp, lv, size); break;
+      case GEOM_ELLIPSOID: t = ray_ellipsoid(lp, lv, size); break;
+      case GEOM_CYLINDER: t = ray_cylinder(lp, lv, size); break;
+      case GEOM_BOX: t = ray_box(lp, lv, size); break;
+      default: throw std::runtime_error("rangefinder: a geom type rays are not cast against");
+    }
+    best = smallest(best, t);
+  }
+  return best;
+}
 
 template <class T>
 struct Sim {
@@ -311,6 +451,20 @@ void sensors(const Model<T>& m, const Data<T>& d, const Table& tab, int start, i
       }
       case SENS_TENDONPOS: o[0] = tendon(m, d, id, false); break;
       case SENS_TENDONVEL: o[0] = tendon(m, d, id, true); break;
+      case SENS_MAGNETOMETER: {
+        if (tab.objtype[s] != OBJ_SITE) throw std::runtime_error("magnetometer of an object other than a site");
+        const T* R = &d.site_xmat[9 * id];
+        for (int r = 0; r < 3; r++) {
+          T x = 0;
+          for (int k = 0; k < 3; k++) x += R[3 * k + r] * (T)tab.magnetic[k];
+          o[r] = x;
+        }
+        break;
+      }
+      case SENS_RANGEFINDER:
+        if (tab.objtype[s] != OBJ_SITE) throw std::runtime_error("rangefinder of an object other than a site");
+        o[0] = rangefinder(m, d, tab, id);
+        break;
       default: throw std::runtime_error("sensor type not evaluated");
     }
   }
@@ -363,6 +517,13 @@ void* sensor_oracle_create(const void* blob, size_t nbytes, int precision) {
     h->tab.type = b.ints("sensor_type"); h->tab.objtype = b.ints("sensor_objtype"); h->tab.objid = b.ints("sensor_objid");
     h->tab.dim = b.ints("sensor_dim"); h->tab.adr = b.ints("sensor_adr"); h->tab.site_type = b.ints("site_type");
     h->tab.site_size = b.reals("site_size");
+    int dt, cnt;
+    int64_t off;
+    if (b.find("opt_magnetic", &dt, &cnt, &off)) {
+      const std::vector<double> mag = b.reals("opt_magnetic");
+      for (int q = 0; q < 3; q++) h->tab.magnetic[q] = mag.at(q);
+    }
+    if (b.find("geom_alpha", &dt, &cnt, &off)) h->tab.geom_alpha = b.reals("geom_alpha");
     if (precision == 64) h->s64.reset(new Sim<double>(blob, nbytes));
     else h->s32.reset(new Sim<float>(blob, nbytes));
     return h;
