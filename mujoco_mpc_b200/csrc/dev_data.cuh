@@ -6,6 +6,8 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include <utility>
+
 #include "dev_model.h"
 
 // Code-footprint control: with one warp per scheduler every instruction-cache
@@ -130,7 +132,7 @@ constexpr int kHdrWords = (int)((sizeof(DevModel) + 15) / 16) * 4;
 constexpr int kLayWords = (int)((sizeof(DevLayout) + 15) / 16) * 4;
 
 struct DynSpec {
-  static constexpr bool kStatic = false;
+  static constexpr bool kStatic = false, kTreeFactor = false;
   static constexpr int kNV = 0, kNHPair = 0;
   static constexpr int kWide = 1, kTask = 0;
   static __device__ __forceinline__ const DevModel& hdr(const Ctx& c) { return *reinterpret_cast<const DevModel*>(g_smem + c.hdr); }
@@ -144,12 +146,38 @@ struct DynSpec {
   }
 };
 
+// The dof tree of a static spec (K::kDofParent, parent before child) as warp_tree_factor_solve reads it: the ancestors
+// of each dof, and the elimination order - by height above the leaves (a dof after all its descendants), within one
+// height by descending index.
+template <class K, int N>
+struct DofTree {
+  static constexpr int kN = N;
+  static __host__ __device__ constexpr unsigned anc(int j) {
+    unsigned m = 0;
+    for (int a = K::kDofParent[j]; a >= 0; a = K::kDofParent[a]) m |= 1u << a;
+    return m;
+  }
+  static __host__ __device__ constexpr int col(int t) {
+    int h[64] = {}, hmax = 0;
+    for (int k = N - 1; k >= 0; k--) {
+      const int p = K::kDofParent[k];
+      if (p >= 0 && h[k] + 1 > h[p]) h[p] = h[k] + 1;
+      if (h[k] > hmax) hmax = h[k];
+    }
+    for (int l = 0; l <= hmax; l++)
+      for (int j = N - 1; j >= 0; j--)
+        if (h[j] == l && t-- == 0) return j;
+    return -1;
+  }
+};
+
 // W > 1: the CTA holds W warps for ONE trajectory - warp 0 runs the pipeline, warps 1..W-1 are helpers that join it for
 // the phases with more independent work items than one warp has lanes (wide_* below)
 // T = 1: one more warp (index W) runs the phases that do not depend on the constraint pipeline concurrently with it
-template <class K, int W = 1, int T = 0>
+// D = true: the SPD solves keep the dense factor (warp_chol_factor_solve) instead of the dof tree's (step_batch_body)
+template <class K, int W = 1, int T = 0, bool D = false>
 struct StaticSpec {
-  static constexpr bool kStatic = true;
+  static constexpr bool kStatic = true, kTreeFactor = !D;
   static constexpr int kWide = W, kTask = T;
   static __host__ __device__ constexpr int w(size_t byte_off, int i = 0) { return K::kModelWords[byte_off / 4 + i]; }
   struct View {
@@ -158,6 +186,7 @@ struct StaticSpec {
 #undef X
   };
   static constexpr int kNV = View::nv, kNHPair = View::nhpair;
+  using Tree = DofTree<K, kNV>;
   static constexpr int kHdr = View::nf + View::ni;
   static constexpr int kData0 = kHdr + kHdrWords + kLayWords;
   static __device__ __forceinline__ const DevModel& hdr(const Ctx&) { return *reinterpret_cast<const DevModel*>(g_smem + kHdr); }
@@ -493,6 +522,70 @@ __device__ __forceinline__ void warp_chol_factor_solve_reg(float* A, float* x, c
   }
   if (lane < N) x[lane] = y;
   __syncwarp();
+}
+
+// ---- leaves-first factorisation along the dof tree, for matrices whose non-zeros all pair a dof with an ancestor (qM,
+// qM + h diag(damping), and the Newton Hessian when every contact is against a body without dofs).  Eliminating a dof
+// only couples its ancestors, which are already coupled, so nothing fills in; dofs in different branches are
+// independent, and the dependent chain is the tree's height instead of nv (Quadruped: 9 levels instead of 18 columns).
+//   A = G G^T, G upper triangular: G[a][j] = A'[a][j] / l_j for every ancestor a of j (A' the matrix as updated by the
+//   eliminations of j's descendants), G[j][j] = l_j.
+// Lane a (< N) holds column a of A's lower triangle (A[k][a], k >= a); lane N holds b as one more row: it is an
+// ancestor of every dof, and its entry j ends as y_j, the solution of G y = b (the forward substitution is part of the
+// elimination and has no dependent chain of its own).  G^T x = y is then solved root-to-leaves on every lane, from G
+// gathered by shuffles off the chain.  Every register access has a compile-time index (no local memory) and every
+// dependence between columns is a real one, so the scheduler overlaps the branches.
+// Tr: the compile-time tree of N dofs (DofTree below): anc(j) bit mask of j's ancestors, col(t) the t-th column
+// eliminated (by height above the leaves, leaves first).  A is read only.  Pivots below kMinVal are clamped as in the
+// dense factor.
+template <int J, int B, class Tr, int N>
+__device__ __forceinline__ void tree_update(float (&row)[N]) {
+  if constexpr (((Tr::anc(J) >> B) & 1u) != 0u) row[B] -= row[J] * __shfl_sync(kFull, row[J], B);
+}
+template <int T, class Tr, int N, int... B>
+__device__ __forceinline__ void tree_column(float (&row)[N], float (&il)[N], std::integer_sequence<int, B...>) {
+  constexpr int J = Tr::col(T);
+  float p = __shfl_sync(kFull, row[J], J);
+  if (p < kMinVal) p = kMinVal;
+  const float l = sqrtf(p);
+  il[J] = 1.0f / l;
+  row[J] *= il[J];
+  (tree_update<J, B, Tr>(row), ...);
+}
+template <int J, int I, class Tr, int N>
+__device__ __forceinline__ void tree_back_update(float& t, const float (&row)[N], const float (&xs)[N]) {
+  if constexpr (((Tr::anc(J) >> I) & 1u) != 0u) t -= __shfl_sync(kFull, row[J], I) * xs[I];
+}
+template <int J, class Tr, int N, int... I>
+__device__ __forceinline__ void tree_back(const float (&row)[N], float (&xs)[N], const float (&il)[N], std::integer_sequence<int, I...>) {
+  float t = xs[J];
+  (tree_back_update<J, I, Tr>(t, row, xs), ...);
+  xs[J] = t * il[J];
+}
+template <class Tr, int N, int... T>
+__device__ __forceinline__ void tree_solve(const float* A, float* x, const float* b, int lane, std::integer_sequence<int, T...> seq) {
+  static_assert(N < 32, "lane N carries the right-hand side");
+  float row[N], il[N], xs[N];
+  const int li = lane < N ? lane : N - 1;
+#pragma unroll
+  for (int k = 0; k < N; k++) row[k] = lane == N ? b[k] : A[k * N + li];
+  __syncwarp();   // x may alias b
+  (tree_column<T, Tr>(row, il, seq), ...);
+  // G^T x = y, root to leaves (a dof's ancestors have smaller indices): x_j = (y_j - sum_{i anc j} G[i][j] x_i) / l_j
+#pragma unroll
+  for (int j = 0; j < N; j++) xs[j] = __shfl_sync(kFull, row[j], N);
+  (tree_back<T, Tr>(row, xs, il, seq), ...);
+  // every lane holds all of x: same-value stores from all lanes (picking x[lane] out of xs would index it by lane,
+  // which puts xs in local memory)
+#pragma unroll
+  for (int k = 0; k < N; k++) x[k] = xs[k];
+  __syncwarp();
+}
+// solve A x = b (x may alias b) for a matrix with Tr's tree pattern.  ONE out-of-line copy per tree: every kernel
+// instance of a model, helper-warp or one-warp, runs this same code.
+template <class Tr>
+__device__ __noinline__ void warp_tree_factor_solve(const float* A, float* x, const float* b, int lane) {
+  tree_solve<Tr, Tr::kN>(A, x, b, lane, std::make_integer_sequence<int, Tr::kN>{});
 }
 
 // factor A (destroyed, holds L afterwards) and solve A x = b; dispatches to the register variant for the

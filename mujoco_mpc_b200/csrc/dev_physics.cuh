@@ -187,7 +187,18 @@ __device__ __noinline__ void k_com_pos(Ctx& c) {
   __syncwarp();
 }
 
-// composite rigid body inertia -> dense joint-space inertia qM, then its Cholesky factor qLD
+// SPD solve A x = b (x may alias b) of qM, qM + h diag(damping) or the Newton Hessian.  Static specs factor along the
+// dof tree when the matrix has the tree's pattern (`tree_pattern`; qM and the Euler matrix always do) and leave A
+// unchanged; otherwise the dense factor overwrites A.
+template <class SP>
+__device__ __forceinline__ void spd_solve(Ctx& c, float* A, float* inv, float* x, const float* b, bool tree_pattern) {
+  if constexpr (SP::kTreeFactor) {
+    if (tree_pattern) { warp_tree_factor_solve<typename SP::Tree>(A, x, b, c.lane); return; }
+  }
+  warp_chol_factor_solve<SP::kNV>(A, inv, x, b, SP::model(c).nv, c.lane);
+}
+
+// composite rigid body inertia -> dense joint-space inertia qM (and qLD, the copy the dense factor overwrites)
 template <class SP>
 __device__ __noinline__ void k_crb(Ctx& c) {
   auto&& M = SP::model(c);
@@ -216,10 +227,12 @@ __device__ __noinline__ void k_crb(Ctx& c) {
     qM[i * nv + j] = s; qM[j * nv + i] = s;
   }
   __syncwarp();
-  // entries of qM outside the (dof, ancestor) pattern stay zero (zeroed once per rollout); the factor
-  // fills in, so the whole matrix is re-copied before every factorisation
-  for (int w = lane; w < nv * nv; w += 32) qLD[w] = qM[w];
-  __syncwarp();
+  // entries of qM outside the (dof, ancestor) pattern stay zero (zeroed once per rollout); the dense factor
+  // fills in, so the whole matrix is re-copied before every factorisation (the tree factor reads qM itself)
+  if constexpr (!SP::kTreeFactor) {
+    for (int w = lane; w < nv * nv; w += 32) qLD[w] = qM[w];
+    __syncwarp();
+  }
 }
 
 // ------------------------------------------------------------------------------------------ collision
@@ -1122,7 +1135,7 @@ __device__ __noinline__ void k_smooth_forces(Ctx& c) {
     }
   }
   __syncwarp();
-  warp_chol_factor_solve<SP::kNV>(DF(qLD), DF(ldinv), DF(qacc_smooth), smooth, nv, lane);
+  spd_solve<SP>(c, SP::kTreeFactor ? DF(qM) : DF(qLD), DF(ldinv), DF(qacc_smooth), smooth, true);
 }
 
 // constraint reference acceleration aref = -B*vel - K*imp*(pos - margin)
@@ -1973,7 +1986,9 @@ __device__ __noinline__ void k_solve(Ctx& c) {
     else k_hessian<SP>(c);
     PHASE(c, 5);
     PHASE_AT(c, 1, 5);
-    warp_chol_factor_solve<SP::kNV>(DF(qH), DF(hinv), search, grad, nv, lane);
+    // fill check: only rows of contacts between two moving bodies and of tendon limits (efc_drow) can couple dofs of
+    // different branches; without them H has qM's (dof, ancestor) pattern
+    spd_solve<SP>(c, DF(qH), DF(hinv), search, grad, c.ndrow == 0);
     PHASE(c, 6);
     PHASE_AT(c, 1, 6);
     for (int b0 = 0; b0 < nv; b0 += 32) { const int i = min(b0 + lane, nv - 1); const float v = -search[i]; __syncwarp(); if (b0 + lane < nv) search[i] = v; }
@@ -2060,7 +2075,7 @@ __device__ __noinline__ void k_euler(Ctx& c) {
     }
     for (int i = lane; i < nv; i += 32) vt[i] = smooth[i] + qfc[i];
     __syncwarp();
-    warp_chol_factor_solve<SP::kNV>(H, DF(hinv), vt, vt, nv, lane);
+    spd_solve<SP>(c, H, DF(hinv), vt, vt, true);
     acc = vt;
   }
   for (int i = lane; i < nv; i += 32) qvel[i] += h * acc[i];

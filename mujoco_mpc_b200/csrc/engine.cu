@@ -735,8 +735,9 @@ int mjpc_b200_create(const mjpc_model_blob* model, int max_candidates, int max_h
   h->h_out_bytes = N * 16 + 64;
   CREATE_TRY(cudaMallocHost((void**)&h->h_out, h->h_out_bytes));
   const DevLayout L1 = make_layout(M, 1);
-  if (spec_matches<SpecQuadruped>(M, L1)) h->kernels = &kQuadrupedKernels;
-  else if (spec_matches<SpecHumanoidTrack>(M, L1)) h->kernels = &kHumanoidTrackKernels;
+  const int* dof_parent = h->pack.i.data() + M.io[I_dof_parentid];
+  if (spec_matches<SpecQuadruped>(M, L1, dof_parent)) h->kernels = &kQuadrupedKernels;
+  else if (spec_matches<SpecHumanoidTrack>(M, L1, dof_parent)) h->kernels = &kHumanoidTrackKernels;
   // the dynamic shared-memory opt-in is per kernel and process-wide (raise_smem_limit only ever raises it: several
   // handles may coexist); a launch may fall back to the generic row (pick_kernels), so both rows get theirs
   const size_t smem_rollout = h->smem_bytes(h->maxP), smem_step = h->smem_bytes(1);
@@ -1869,18 +1870,19 @@ int64_t mjpc_b200_launch_count(const mjpc_b200_t* h) { return h ? h->launches : 
 float mjpc_b200_last_kernel_ms(const mjpc_b200_t* h) { return h ? h->last_ms : 0.f; }
 int mjpc_b200_last_kernel_static(const mjpc_b200_t* h) { return h ? h->last_static : 0; }
 
-// Header + state-layout words of a model, as the static kernel tables (spec_*.h) store them.  Host only.
+// Header + state-layout words and the dof tree of a model, as the static kernel tables (spec_*.h) store them.  Host only.
 int mjpc_b200_spec_words(const mjpc_model_blob* model, int* out, int capacity) {
   if (!model || !model->data || !out) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "spec_words: null");
   try {
     ModelPack P = pack_model(model->data, model->nbytes, 32, 96);
     const DevLayout L = make_layout(P.M, 1);
-    const int nm = (int)(sizeof(DevModel) / 4), nl = (int)D_COUNT;
-    if (capacity < 2 + nm + nl) return fail(MJPC_B200_ERR_CAPACITY, "spec_words: buffer too small");
+    const int nm = (int)(sizeof(DevModel) / 4), nl = (int)D_COUNT, nv = P.M.nv;
+    if (capacity < 2 + nm + nl + nv) return fail(MJPC_B200_ERR_CAPACITY, "spec_words: buffer too small");
     out[0] = nm; out[1] = nl;
     std::memcpy(out + 2, &P.M, sizeof(DevModel));
     for (int i = 0; i < nl; i++) out[2 + nm + i] = L.off[i];
-    return 2 + nm + nl;
+    std::memcpy(out + 2 + nm + nl, P.i.data() + P.M.io[I_dof_parentid], 4 * (size_t)nv);   // the dof tree
+    return 2 + nm + nl + nv;
   } catch (const std::exception& e) {
     return fail(MJPC_B200_ERR_BAD_BLOB, std::string("spec_words: ") + e.what());
   }

@@ -450,10 +450,10 @@ extern "C" __global__ void __launch_bounds__(32) rollout_kernel_humanoid_track_p
   rollout_body<StaticSpec<SpecHumanoidTrack, 1, 0>>(A);
 }
 
-// host: does the live model header / state layout equal the table a static kernel was compiled from?
+// host: do the live model header / state layout / dof tree equal the table a static kernel was compiled from?
 // (float options are not part of the comparison: static kernels read them from the live header)
 template <class K>
-inline bool spec_matches(const DevModel& M, const DevLayout& L) {
+inline bool spec_matches(const DevModel& M, const DevLayout& L, const int* dof_parent) {
   if (K::kNumModelWords != (int)(sizeof(DevModel) / 4) || K::kNumLayout != (int)D_COUNT) return false;
   const int* w = K::kModelWords;
 #define X(n) if (w[offsetof(DevModel, n) / 4] != M.n) return false;
@@ -462,6 +462,7 @@ inline bool spec_matches(const DevModel& M, const DevLayout& L) {
   for (int i = 0; i < F_COUNT; i++) if (w[offsetof(DevModel, fo) / 4 + i] != M.fo[i]) return false;
   for (int i = 0; i < I_COUNT; i++) if (w[offsetof(DevModel, io) / 4 + i] != M.io[i]) return false;
   for (int i = 0; i < D_COUNT; i++) if (K::kLayoutOff[i] != L.off[i]) return false;
+  for (int i = 0; i < M.nv; i++) if (K::kDofParent[i] != dof_parent[i]) return false;
   return true;
 }
 
@@ -587,11 +588,14 @@ __device__ __forceinline__ void step_batch_body(const StepBatchArgs& A) {
 extern "C" __global__ void __launch_bounds__(32) step_batch_kernel(const __grid_constant__ StepBatchArgs A) {
   step_batch_body<DynSpec>(A);
 }
+// The one-step entry points (step_batch, and step_sensors: the estimators' sigma-point and finite-difference steps) and
+// the plant steps, which must equal them, keep the dense factor: the Kalman filter differentiates these steps with 1e-3 differences, and through a hard contact solve
+// a rounding change can move where the Newton iteration stops by its tolerance, which those differences amplify.
 extern "C" __global__ void __launch_bounds__(32) step_batch_kernel_quadruped(const __grid_constant__ StepBatchArgs A) {
-  step_batch_body<StaticSpec<SpecQuadruped>>(A);
+  step_batch_body<StaticSpec<SpecQuadruped, 1, 0, true>>(A);
 }
 extern "C" __global__ void __launch_bounds__(32) step_batch_kernel_humanoid_track(const __grid_constant__ StepBatchArgs A) {
-  step_batch_body<StaticSpec<SpecHumanoidTrack>>(A);
+  step_batch_body<StaticSpec<SpecHumanoidTrack, 1, 0, true>>(A);
 }
 
 // Closed-loop plants (plant_bank.h): B plants whose state stays in device memory, each advanced by ONE mj_step per
@@ -758,10 +762,10 @@ extern "C" __global__ void __launch_bounds__(32) plant_step_kernel(const __grid_
   plant_body<DynSpec>(A);
 }
 extern "C" __global__ void __launch_bounds__(32) plant_step_kernel_quadruped(const __grid_constant__ PlantArgs A) {
-  plant_body<StaticSpec<SpecQuadruped>>(A);
+  plant_body<StaticSpec<SpecQuadruped, 1, 0, true>>(A);
 }
 extern "C" __global__ void __launch_bounds__(32) plant_step_kernel_humanoid_track(const __grid_constant__ PlantArgs A) {
-  plant_body<StaticSpec<SpecHumanoidTrack>>(A);
+  plant_body<StaticSpec<SpecHumanoidTrack, 1, 0, true>>(A);
 }
 
 }  // namespace mjpc_dev
