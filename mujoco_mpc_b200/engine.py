@@ -6,75 +6,21 @@ CPU fallback: if the library is missing or no CUDA device is visible, constructi
 from __future__ import annotations
 
 import ctypes as C
+import functools
 import os
+import re
 
 import numpy as np
 
 from .blob import to_blob
-from .build import SO
+from .build import HERE, SO
+
+HEADER = os.path.join(HERE, "..", "include", "mjpc_b200.h")
 
 _fp = C.POINTER(C.c_float)
 _dp = C.POINTER(C.c_double)
 _ip = C.POINTER(C.c_int)
 _bp = C.POINTER(C.c_uint8)
-
-EXPORTS = ["mjpc_b200_version", "mjpc_b200_last_error", "mjpc_b200_create", "mjpc_b200_destroy",
-           "mjpc_b200_get_info", "mjpc_b200_set_task", "mjpc_b200_set_differentiable", "mjpc_b200_set_xfrc_noise", "mjpc_b200_rollout_spline", "mjpc_b200_rollout_feedback",
-           "mjpc_b200_rollout_spline_batched", "mjpc_b200_batch_sampling_planner_create", "mjpc_b200_batch_planner_destroy",
-           "mjpc_b200_batch_planner_reset", "mjpc_b200_batch_planner_set_state", "mjpc_b200_batch_planner_set_task",
-           "mjpc_b200_batch_planner_optimize_policy", "mjpc_b200_batch_planner_action_from_policy",
-           "mjpc_b200_batch_sampling_planner_get_result", "mjpc_b200_set_xfrc_noise_batched", "mjpc_b200_planner_set_task",
-           "mjpc_b200_batch_ce_planner_create", "mjpc_b200_batch_ce_planner_get_result",
-           "mjpc_b200_batch_sg_planner_create", "mjpc_b200_batch_sg_planner_get_result",
-           "mjpc_b200_batch_robust_planner_create", "mjpc_b200_batch_robust_planner_get_result",
-           "mjpc_b200_fetch_trajectory", "mjpc_b200_fetch_all", "mjpc_b200_model_derivatives",
-           "mjpc_b200_cost_derivatives", "mjpc_b200_backward_pass", "mjpc_b200_rollout_feedback_batched",
-           "mjpc_b200_model_derivatives_batched", "mjpc_b200_cost_derivatives_batched", "mjpc_b200_backward_pass_batched",
-           "mjpc_b200_batch_ilqg_planner_create", "mjpc_b200_batch_ilqg_planner_nominal_trajectory",
-           "mjpc_b200_batch_ilqg_planner_get_result",
-           "mjpc_b200_step_debug", "mjpc_b200_step_debug_contacts", "mjpc_b200_step_batch", "mjpc_b200_step_sensors",
-           "mjpc_b200_estimator_destroy", "mjpc_b200_estimator_reset", "mjpc_b200_estimator_set_noise",
-           "mjpc_b200_estimator_set", "mjpc_b200_estimator_update", "mjpc_b200_estimator_get",
-           "mjpc_b200_estimator_last_error", "mjpc_b200_unscented_create", "mjpc_b200_kalman_create",
-           "mjpc_b200_kalman_update_measurement", "mjpc_b200_kalman_update_prediction",
-           "mjpc_b200_batch_estimator_create", "mjpc_b200_batch_estimator_destroy", "mjpc_b200_batch_estimator_reset",
-           "mjpc_b200_batch_estimator_set_noise", "mjpc_b200_batch_estimator_set", "mjpc_b200_batch_estimator_update",
-           "mjpc_b200_batch_estimator_get", "mjpc_b200_batch_estimator_last_error",
-           "mjpc_b200_comm_unique_id", "mjpc_b200_comm_init",
-           "mjpc_b200_comm_info", "mjpc_b200_rollout_spline_sharded", "mjpc_b200_fetch_trajectory_sharded",
-           "mjpc_b200_fetch_stats", "mjpc_b200_launch_count", "mjpc_b200_last_kernel_ms", "mjpc_b200_last_kernel_static",
-           "mjpc_b200_spec_words", "mjpc_b200_upload_spline_inputs",
-           "mjpc_b200_launch_resident", "mjpc_b200_sync", "mjpc_b200_read_returns", "mjpc_b200_stream",
-           "mjpc_b200_device_returns", "mjpc_b200_host_spline_sample", "mjpc_b200_host_policy_intervals",
-           "mjpc_b200_host_philox_normal",
-           "mjpc_b200_planner_destroy", "mjpc_b200_planner_reset", "mjpc_b200_planner_set_state",
-           "mjpc_b200_planner_optimize_policy", "mjpc_b200_planner_nominal_trajectory",
-           "mjpc_b200_planner_action_from_policy", "mjpc_b200_planner_set_fd",
-           "mjpc_b200_sampling_planner_create", "mjpc_b200_sampling_planner_set_exploration",
-           "mjpc_b200_sampling_planner_get_result", "mjpc_b200_ce_planner_create", "mjpc_b200_ce_planner_get_result",
-           "mjpc_b200_sg_planner_create", "mjpc_b200_sg_planner_get_result", "mjpc_b200_ilqg_planner_create",
-           "mjpc_b200_ilqg_planner_get_result", "mjpc_b200_host_ilqg_policy_action", "mjpc_b200_robust_planner_create",
-           "mjpc_b200_robust_planner_get_result", "mjpc_b200_gradient_planner_create",
-           "mjpc_b200_gradient_planner_get_result", "mjpc_b200_host_spline_mapping", "mjpc_b200_host_gradient_sweep",
-           "mjpc_b200_gradient_batched", "mjpc_b200_batch_gradient_planner_create",
-           "mjpc_b200_batch_gradient_planner_get_result", "mjpc_b200_batch_planner_set_fd",
-           "mjpc_b200_batch_ilqs_planner_create", "mjpc_b200_batch_ilqs_planner_get_result",
-           "mjpc_b200_batch_ilqs_planner_set_exploration", "mjpc_b200_ilqs_planner_create",
-           "mjpc_b200_ilqs_planner_set_exploration", "mjpc_b200_ilqs_planner_get_result",
-           "mjpc_b200_set_options", "mjpc_b200_agent_steps", "mjpc_b200_agent_create", "mjpc_b200_agent_destroy",
-           "mjpc_b200_agent_reset", "mjpc_b200_agent_set_state", "mjpc_b200_agent_set_task", "mjpc_b200_agent_set_plan_enabled",
-           "mjpc_b200_agent_plan_iteration", "mjpc_b200_agent_get_steps", "mjpc_b200_agent_action_from_policy",
-           "mjpc_b200_quadruped_transition_create", "mjpc_b200_quadruped_transition_destroy",
-           "mjpc_b200_quadruped_transition_step", "mjpc_b200_quadruped_transition_set", "mjpc_b200_track_transition_create",
-           "mjpc_b200_track_transition_destroy", "mjpc_b200_track_transition_step", "mjpc_b200_shadow_transition_create",
-           "mjpc_b200_shadow_transition_destroy", "mjpc_b200_shadow_transition_step", "mjpc_b200_set_model_variants",
-           "mjpc_b200_select_model_variants", "mjpc_b200_batch_planner_set_models",
-           "mjpc_b200_batch_estimator_set_models", "mjpc_b200_plant_init", "mjpc_b200_plant_reset",
-           "mjpc_b200_plant_set", "mjpc_b200_plant_set_task", "mjpc_b200_plant_step", "mjpc_b200_plant_get",
-           "mjpc_b200_plant_set_disturbance", "mjpc_b200_plant_set_xfrc", "mjpc_b200_plant_get_disturbance",
-           "mjpc_b200_plant_last_ctrl",
-           "mjpc_b200_set_model_ensemble", "mjpc_b200_fetch_ensemble", "mjpc_b200_fetch_trajectory_member",
-           "mjpc_b200_host_ensemble_score", "mjpc_b200_planner_set_ensemble", "mjpc_b200_batch_planner_set_ensemble"]
 
 
 class ModelBlob(C.Structure):
@@ -91,65 +37,60 @@ class Info(C.Structure):
                                        "max_candidates", "max_horizon", "device", "smem_bytes_per_warp")]
 
 
+_SCALARS = {"int": C.c_int, "double": C.c_double, "float": C.c_float, "uint32_t": C.c_uint32, "size_t": C.c_size_t,
+            "int64_t": C.c_int64, "uint8_t": C.c_uint8}
+_STRUCTS = {"mjpc_model_blob": ModelBlob, "mjpc_task_desc": TaskDesc, "mjpc_b200_info": Info}
+_HANDLES = {"mjpc_b200_t", "mjpc_b200_planner_t", "mjpc_b200_batch_planner_t", "mjpc_b200_estimator_t", "void"}
+
+
+def _ctype(decl, text, is_return):
+    """The ctypes type of one C type as the header writes it (`const` ignored, any spacing around `*`)."""
+    words = text.replace("*", " * ").split()
+    stars = words.count("*")
+    base = " ".join(w for w in words if w not in ("const", "*"))
+    if is_return and base == "void" and not stars:
+        return None
+    if is_return and stars:   # raw addresses, strings aside
+        return C.c_char_p if (base, stars) == ("char", 1) else C.c_void_p
+    if not stars and base in _SCALARS:
+        return _SCALARS[base]
+    if stars == 1 and base in _SCALARS:
+        return C.POINTER(_SCALARS[base])
+    if stars == 1 and base in _STRUCTS:
+        return C.POINTER(_STRUCTS[base])
+    if base in _HANDLES and stars in (1, 2):
+        return C.c_void_p if stars == 1 else C.POINTER(C.c_void_p)
+    raise TypeError(f"include/mjpc_b200.h: no ctypes type for '{text.strip()}' in `{decl}`")
+
+
+def parse_header(text):
+    """{name: (restype, argtypes)} of every `<return type> mjpc_b200_<name>(<parameters>);` the header text declares.
+    A type the binding has no ctypes type for raises TypeError naming the declaration."""
+    text = re.sub(r"/\*.*?\*/|//[^\n]*", " ", text, flags=re.S)
+    text = re.sub(r"^\s*#[^\n]*", " ", text, flags=re.M)
+    protos = {}
+    for m in re.finditer(r"([A-Za-z_][\w\s*]*?)\b(mjpc_b200_\w+)\s*\(([^()]*)\)\s*;", text):
+        decl = " ".join(m.group(0).split())
+        params = [p for p in m.group(3).split(",") if p.split() != ["void"]]
+        argtypes = [_ctype(decl, re.sub(r"\w+\s*$", "", p), False) for p in params]   # `<type> <name>`
+        protos[m.group(2)] = (_ctype(decl, m.group(1), True), argtypes)
+    return protos
+
+
 _LIB = None
 
 
 def load_library():
+    """libmjpc_b200.so with every entry point's argtypes / restype from include/mjpc_b200.h."""
     global _LIB
     if _LIB is None:
         if not os.path.exists(SO):
             raise RuntimeError(f"{SO} not built: run `python -m mujoco_mpc_b200.build` (no fallback path exists)")
         lib = C.CDLL(SO)
-        lib.mjpc_b200_version.restype = C.c_char_p
-        lib.mjpc_b200_last_error.restype = C.c_char_p
-        lib.mjpc_b200_launch_count.restype = C.c_int64
-        lib.mjpc_b200_last_kernel_ms.restype = C.c_float
-        lib.mjpc_b200_stream.restype = C.c_void_p
-        lib.mjpc_b200_device_returns.restype = C.c_void_p
-        lib.mjpc_b200_host_philox_normal.restype = C.c_double
-        # the generic planner, batch planner and estimator families: the first argument is the handle
-        for f, args in ((lib.mjpc_b200_planner_destroy, []), (lib.mjpc_b200_planner_reset, [C.c_int, _dp]),
-                        (lib.mjpc_b200_planner_set_state, [_dp, C.c_double, _dp]),
-                        (lib.mjpc_b200_planner_optimize_policy, [C.c_int]),
-                        (lib.mjpc_b200_planner_nominal_trajectory, [C.c_int]),
-                        (lib.mjpc_b200_planner_action_from_policy, [_dp, _dp, C.c_double, C.c_int]),
-                        (lib.mjpc_b200_planner_set_fd, [C.c_double, C.c_int, C.c_int]),
-                        (lib.mjpc_b200_planner_set_ensemble, [C.POINTER(ModelBlob), C.c_int, C.c_int]),
-                        (lib.mjpc_b200_batch_planner_set_ensemble, [C.POINTER(ModelBlob), C.c_int, C.c_int]),
-                        (lib.mjpc_b200_batch_planner_destroy, []),
-                        (lib.mjpc_b200_batch_planner_reset, [C.c_int, C.c_int, _dp]),
-                        (lib.mjpc_b200_batch_planner_set_state, [C.c_int, _dp, C.c_double, _dp]),
-                        (lib.mjpc_b200_batch_planner_set_task, [C.c_int, _dp, _dp, _dp]),
-                        (lib.mjpc_b200_batch_planner_set_models, [C.POINTER(ModelBlob), C.c_int]),
-                        (lib.mjpc_b200_batch_planner_optimize_policy, [C.c_int, _ip]),
-                        (lib.mjpc_b200_batch_planner_action_from_policy, [C.c_int, _dp, _dp, C.c_double, C.c_int]),
-                        (lib.mjpc_b200_batch_planner_set_fd, [C.c_double, C.c_int, C.c_int]),
-                        (lib.mjpc_b200_estimator_destroy, []),
-                        (lib.mjpc_b200_estimator_reset, [_dp] + [C.c_double] * 4),
-                        (lib.mjpc_b200_estimator_set_noise, [_dp, _dp]),
-                        (lib.mjpc_b200_estimator_set, [_dp, _dp, C.c_double]),
-                        (lib.mjpc_b200_estimator_update, [_dp, _dp, _fp]), (lib.mjpc_b200_estimator_get, [_dp] * 4),
-                        (lib.mjpc_b200_estimator_last_error, [])):
-            f.argtypes, f.restype = [C.c_void_p] + args, C.c_int
-        lib.mjpc_b200_estimator_last_error.restype = C.c_char_p
-        lib.mjpc_b200_batch_planner_destroy.restype = None
-        lib.mjpc_b200_planner_set_task.argtypes = [C.c_void_p, C.c_void_p]
-        lib.mjpc_b200_set_xfrc_noise_batched.argtypes = [C.c_void_p, C.c_double, C.c_double, C.c_int,
-                                                         C.POINTER(C.c_uint32)]
-        lib.mjpc_b200_sampling_planner_set_exploration.argtypes = [C.c_void_p, C.c_double, C.c_double]
-        lib.mjpc_b200_agent_destroy.argtypes = [C.c_void_p]
-        lib.mjpc_b200_agent_steps.argtypes = [C.c_double, C.c_double]
-        lib.mjpc_b200_set_options.argtypes = [C.c_void_p, C.c_double, C.c_int]
-        lib.mjpc_b200_ilqs_planner_set_exploration.argtypes = [C.c_void_p, C.c_double]
-        lib.mjpc_b200_batch_ilqs_planner_set_exploration.argtypes = [C.c_void_p, C.c_double]
-        lib.mjpc_b200_shadow_transition_destroy.argtypes = [C.c_void_p]
-        for n in ("mjpc_b200_quadruped_transition_create", "mjpc_b200_track_transition_create", "mjpc_b200_shadow_transition_create"):
-            getattr(lib, n).restype = C.c_void_p
-        lib.mjpc_b200_quadruped_transition_destroy.argtypes = [C.c_void_p]
-        lib.mjpc_b200_track_transition_destroy.argtypes = [C.c_void_p]
-        for n in ("mjpc_b200_destroy", "mjpc_b200_fetch_stats", "mjpc_b200_launch_count", "mjpc_b200_last_kernel_ms", "mjpc_b200_stream",
-                  "mjpc_b200_device_returns", "mjpc_b200_sync", "mjpc_b200_launch_resident"):
-            getattr(lib, n).argtypes = [C.c_void_p]
+        with open(HEADER) as f:
+            for name, (restype, argtypes) in parse_header(f.read()).items():
+                fn = getattr(lib, name)
+                fn.restype, fn.argtypes = restype, argtypes
         _LIB = lib
     return _LIB
 
@@ -238,6 +179,14 @@ class _CppPlanner(_CppObject):
     optimize_policy returns result() and raises on any non-zero code; those with _RETURNS_CODE (Gradient, iLQG, iLQS)
     return the code (1 improved / updated, 0 not) and raise on a negative one."""
     _RETURNS_CODE = False
+
+    def _start(self, model, horizon, device, args):
+        """mjpc_b200_<kind>_planner_create(model, *args, horizon, device), args from the kind's _args."""
+        self.horizon, self.nu = int(horizon), model.nu
+        self._create(f"mjpc_b200_{self._KIND}_planner", model, *args, self.horizon, int(device))
+
+    def result(self):
+        return self._result(functools.partial(getattr(self.lib, f"{self._prefix}_get_result"), self.h))
 
     def close(self):
         if getattr(self, "h", None):
@@ -484,14 +433,7 @@ class Engine:
         return ret, fail, order
 
     def fetch_trajectory_sharded(self, i):
-        H = self.lastH
-        o = dict(states=np.zeros((H, self.ds), np.float32), actions=np.zeros((H, self.nu), np.float32),
-                 times=np.zeros(H), residual=np.zeros((H, self.nr), np.float32), costs=np.zeros(H, np.float32),
-                 trace=np.zeros((H, self.ntr), np.float32))
-        self._check(self.lib.mjpc_b200_fetch_trajectory_sharded(self.h, int(i), _pf(o["states"]), _pf(o["actions"]),
-                                                                _pd(o["times"]), _pf(o["residual"]), _pf(o["costs"]),
-                                                                _pf(o["trace"])))
-        return o
+        return self._fetch(functools.partial(self.lib.mjpc_b200_fetch_trajectory_sharded, self.h, int(i)))
 
     def upload_spline_inputs(self, state, time, mocap, knots, knot_times, interp, H):
         knots = _f(knots)
@@ -548,26 +490,22 @@ class Engine:
         self.lastN, self.lastH = B * K, H
         return ret, fail, order
 
-    def fetch_trajectory(self, i):
-        H = self.lastH
-        o = dict(states=np.zeros((H, self.ds), np.float32), actions=np.zeros((H, self.nu), np.float32),
-                 times=np.zeros(H), residual=np.zeros((H, self.nr), np.float32), costs=np.zeros(H, np.float32),
-                 trace=np.zeros((H, self.ntr), np.float32))
-        self._check(self.lib.mjpc_b200_fetch_trajectory(self.h, int(i), _pf(o["states"]), _pf(o["actions"]),
-                                                        _pd(o["times"]), _pf(o["residual"]), _pf(o["costs"]),
-                                                        _pf(o["trace"])))
+    def _fetch(self, fetch, *lead):
+        """Trajectory-shaped arrays [*lead][lastH][..] filled by fetch(states, actions, times, residual, costs, trace)."""
+        s = (*lead, self.lastH)
+        o = dict(states=np.zeros((*s, self.ds), np.float32), actions=np.zeros((*s, self.nu), np.float32),
+                 times=np.zeros(s), residual=np.zeros((*s, self.nr), np.float32), costs=np.zeros(s, np.float32),
+                 trace=np.zeros((*s, self.ntr), np.float32))
+        self._check(fetch(_pf(o["states"]), _pf(o["actions"]), _pd(o["times"]), _pf(o["residual"]), _pf(o["costs"]),
+                          _pf(o["trace"])))
         return o
+
+    def fetch_trajectory(self, i):
+        return self._fetch(functools.partial(self.lib.mjpc_b200_fetch_trajectory, self.h, int(i)))
 
     def fetch_trajectory_member(self, i, member):
         """Candidate i (flat b * N + i) of the last launch as ensemble member `member` rolled it out."""
-        H = self.lastH
-        o = dict(states=np.zeros((H, self.ds), np.float32), actions=np.zeros((H, self.nu), np.float32),
-                 times=np.zeros(H), residual=np.zeros((H, self.nr), np.float32), costs=np.zeros(H, np.float32),
-                 trace=np.zeros((H, self.ntr), np.float32))
-        self._check(self.lib.mjpc_b200_fetch_trajectory_member(self.h, int(i), int(member), _pf(o["states"]),
-                                                               _pf(o["actions"]), _pd(o["times"]), _pf(o["residual"]),
-                                                               _pf(o["costs"]), _pf(o["trace"])))
-        return o
+        return self._fetch(functools.partial(self.lib.mjpc_b200_fetch_trajectory_member, self.h, int(i), int(member)))
 
     def fetch_ensemble(self):
         """(member returns [B, K, N], member failure [B, K, N]) of the last launch, an ensemble launch."""
@@ -578,13 +516,7 @@ class Engine:
         return ret, fail
 
     def fetch_all(self):
-        N, H = self.lastN, self.lastH
-        o = dict(states=np.zeros((N, H, self.ds), np.float32), actions=np.zeros((N, H, self.nu), np.float32),
-                 times=np.zeros((N, H)), residual=np.zeros((N, H, self.nr), np.float32),
-                 costs=np.zeros((N, H), np.float32), trace=np.zeros((N, H, self.ntr), np.float32))
-        self._check(self.lib.mjpc_b200_fetch_all(self.h, _pf(o["states"]), _pf(o["actions"]), _pd(o["times"]),
-                                                 _pf(o["residual"]), _pf(o["costs"]), _pf(o["trace"])))
-        return o
+        return self._fetch(functools.partial(self.lib.mjpc_b200_fetch_all, self.h), self.lastN)
 
     def step_debug(self, qpos, qvel, ctrl, mocap, time=0.0, warmstart=None):
         nv, nq = self.info.nv, self.info.nq
@@ -783,7 +715,6 @@ class CppPlantBank:
         if rc != 0:
             raise EngineError(f"mjpc_b200_create failed ({rc}): {self.lib.mjpc_b200_last_error().decode()}")
         self.h = h
-        self.lib.mjpc_b200_plant_reset.argtypes = [C.c_void_p, C.c_int, _fp, _fp, C.c_double, _fp]
         self._check(self.lib.mjpc_b200_plant_init(self.h, self.num_plants, self.sensor_start, self.nsensor))
         # each plant's mocap poses as the bank holds them (float), for the planner's set_state
         self.mocap = np.zeros((self.num_plants, 7 * model.nmocap), np.float32)
@@ -887,27 +818,204 @@ class CppPlantBank:
         return int(self.lib.mjpc_b200_last_kernel_static(self.h))
 
 
-class CppSamplingPlanner(_CppPlanner):
+def _numeric(model, name, default):
+    """The first value of the model's custom numeric `name`, else `default`, as the default's type."""
+    return type(default)(model.numeric.get(name, [default])[0])
+
+
+def _ctrlrange(model):
+    """The model's ctrlrange [nu][2] as a create argument (the pointer keeps its array alive through the call)."""
+    return _pd(_d(np.asarray(model.actuator_ctrlrange, float).reshape(-1)))
+
+
+def _seeds(num_problems, seeds):
+    """The seeds [num_problems] of a batch planner's create, as _ctrlrange: problem b's is 0x5EED + b unless given."""
+    sd = np.ascontiguousarray([0x5EED + b for b in range(int(num_problems))] if seeds is None else seeds, np.uint32)
+    return sd.ctypes.data_as(C.POINTER(C.c_uint32))
+
+
+# ---- The planner kinds, each shared by its single planner and its batch planner.  _args returns the kind's create
+# arguments after the model (and the batch's num_problems) and before (max_horizon, device), with `seed` in the seed's
+# place: the single planner's seed or the batch's seeds.  _result allocates the kind's get_result outputs, calls
+# get_result(*outputs) (bound to the planner, and to the problem of a batch) and decodes them into the result dict.
+def _sampling_args(planner, model, num_trajectory, seed):
+    """The create arguments of the sampling planner, which those of the Robust and iLQS planners begin with."""
+    planner.N, planner.P = int(num_trajectory), _numeric(model, "sampling_spline_points", 3)
+    return (planner.N, planner.P, _numeric(model, "sampling_representation", 2),
+            _numeric(model, "sampling_exploration", 0.1), float(model.opt_timestep), _ctrlrange(model), seed)
+
+
+class _Sampling:
+    _KIND = "sampling"
+
+    def _args(self, model, num_trajectory, seed):
+        return _sampling_args(self, model, num_trajectory, seed)
+
+    def _result(self, get_result):
+        winner, imp = C.c_int(), C.c_double()
+        ret = np.zeros(self.N, np.float32); knots = np.zeros((self.P, self.nu)); kt = np.zeros(self.P)
+        get_result(C.byref(winner), C.byref(imp), _pf(ret), _pd(knots), _pd(kt))
+        return dict(winner=winner.value, improvement=imp.value, returns=ret, knots=knots, knot_times=kt)
+
+
+class _CrossEntropy:
+    _KIND = "ce"
+
+    def _args(self, model, num_trajectory, seed, n_elite):
+        self.N, self.P = int(num_trajectory), _numeric(model, "sampling_spline_points", 3)
+        return (self.N, int(n_elite), self.P, _numeric(model, "sampling_representation", 2),
+                _numeric(model, "sampling_exploration", 0.1), _numeric(model, "std_min", 0.01),
+                _numeric(model, "explore_fraction", 0.0), float(model.opt_timestep), _ctrlrange(model), seed)
+
+    def _result(self, get_result):
+        imp = C.c_double()
+        ret = np.zeros(self.N + 1, np.float32); order = np.zeros(self.N, np.int32)
+        knots = np.zeros((self.P, self.nu)); kt = np.zeros(self.P); var = np.zeros((self.P, self.nu))
+        get_result(C.byref(imp), _pf(ret), order.ctypes.data_as(_ip), _pd(knots), _pd(kt), _pd(var))
+        return dict(improvement=imp.value, returns=ret, order=order, knots=knots, knot_times=kt, variance=var)
+
+
+class _SampleGradient:
+    _KIND = "sg"
+
+    def _args(self, model, num_trajectory, seed, num_gradient, gradient_filter):
+        self.N, self.P = int(num_trajectory), _numeric(model, "sampling_spline_points", 3)
+        G = int(num_gradient if num_gradient is not None else _numeric(model, "sample_gradient_trajectories", 0))
+        self.G = max(min(G, self.N - 1), 0)                  # the clamp OptimizePolicy applies
+        f = float(gradient_filter if gradient_filter is not None else _numeric(model, "sample_gradient_filter", 1.0))
+        return (self.N, G, self.P, _numeric(model, "sampling_representation", 2),
+                _numeric(model, "sampling_exploration", 0.1), f, float(model.opt_timestep), _ctrlrange(model), seed)
+
+    def _result(self, get_result):
+        winner, wtype, imp = C.c_int(), C.c_int(), C.c_double()
+        ret = np.zeros(self.N, np.float32); order = np.zeros(self.N, np.int32)
+        knots = np.zeros((self.P, self.nu)); kt = np.zeros(self.P)
+        gk = np.zeros((self.G, self.P, self.nu)); grad = np.zeros((self.P, self.nu))
+        n = get_result(C.byref(winner), C.byref(wtype), C.byref(imp), _pf(ret), order.ctypes.data_as(_ip), _pd(knots),
+                       _pd(kt), _pd(gk) if self.G else None, _pd(grad))
+        return dict(winner=winner.value, winner_type=wtype.value, improvement=imp.value, returns=ret, order=order,
+                    knots=knots[:n], knot_times=kt[:n], gradient_knots=gk, gradient=grad)
+
+
+class _Robust:
+    _KIND = "robust"
+
+    def _args(self, model, num_trajectory, seed, ncandidates, nrepetitions, xfrc_std, xfrc_rate):
+        self.nc = int(ncandidates if ncandidates != -1 else num_trajectory // nrepetitions)
+        return _sampling_args(self, model, num_trajectory, seed) + (int(ncandidates), int(nrepetitions), xfrc_std,
+                                                                    xfrc_rate)
+
+    def _result(self, get_result):
+        winner = C.c_int()
+        scores = np.zeros(max(self.nc, 1)); ret = np.zeros(self.N, np.float32)
+        knots = np.zeros((self.P, self.nu)); kt = np.zeros(self.P)
+        n = get_result(C.byref(winner), _pd(scores), _pf(ret), _pd(knots), _pd(kt))
+        return dict(winner=winner.value, scores=scores[:n], returns=ret, knots=knots, knot_times=kt)
+
+
+class _Gradient:
+    _KIND = "gradient"
+
+    def _args(self, model, num_trajectory, num_spline_points, representation, fd_tolerance):
+        self.P = int(num_spline_points)
+        return (int(num_trajectory), self.P, int(representation), fd_tolerance, float(model.opt_timestep),
+                _ctrlrange(model))
+
+    def _result(self, get_result):
+        sc = np.zeros(6); p = np.zeros((self.P, self.nu)); t = np.zeros(self.P)
+        get_result(_pd(sc), _pd(p), _pd(t))
+        return dict(total_return=sc[0], winner=int(sc[1]), action_step=sc[2], expected=sc[3], improvement=sc[4],
+                    surprise=sc[5], parameters=p, times=t)
+
+
+class _ILQG:
+    _KIND = "ilqg"
+
+    def _args(self, model, horizon, num_rollouts, representation, fd_tolerance):
+        self.H, self.ds = int(horizon), model.nq + model.nv
+        return int(num_rollouts), int(representation), fd_tolerance
+
+    def _result(self, get_result):
+        sc = np.zeros(6); st = np.zeros((self.H, self.ds), np.float32); ac = np.zeros((self.H, self.nu), np.float32)
+        tm = np.zeros(self.H)
+        get_result(_pd(sc), _pf(st), _pf(ac), _pd(tm))
+        return dict(total_return=sc[0], regularization=sc[1], improvement=sc[2], expected=sc[3], surprise=sc[4],
+                    winner=int(sc[5]), states=st, actions=ac, times=tm)
+
+
+class _ILQS:
+    _KIND = "ilqs"
+
+    def _args(self, model, num_trajectory, seed, num_rollouts, fd_tolerance):
+        return _sampling_args(self, model, num_trajectory, seed) + (
+            int(num_rollouts), _numeric(model, "ilqg_representation", 1), fd_tolerance)
+
+    def _result(self, get_result):
+        sc = np.zeros(4)
+        get_result(_pd(sc))
+        return dict(active_policy=int(sc[0]), sampling_return=sc[1], ilqg_return=sc[2], sampling_winner=int(sc[3]))
+
+
+class CppSamplingPlanner(_Sampling, _CppPlanner):
     """The C++ host planner (csrc/host/sampling_planner.cc) through its C wrappers."""
 
     def __init__(self, model, num_trajectory, horizon, seed=0x5EED, device=0):
-        m, num = model, model.numeric
-        self.P = int(num.get("sampling_spline_points", [3])[0])
-        self.horizon, self.N, self.nu = int(horizon), int(num_trajectory), m.nu
-        cr = _d(np.asarray(m.actuator_ctrlrange, float).reshape(-1))
-        self._create("mjpc_b200_sampling_planner", m, self.N, self.P, int(num.get("sampling_representation", [2])[0]),
-                     C.c_double(float(num.get("sampling_exploration", [0.1])[0])), C.c_double(float(m.opt_timestep)),
-                     _pd(cr), C.c_uint32(seed), self.horizon, int(device))
+        self._start(model, horizon, device, self._args(model, num_trajectory, seed))
 
     def set_exploration(self, exploration, exploration2=0.0):
         self.lib.mjpc_b200_sampling_planner_set_exploration(self.h, C.c_double(exploration), C.c_double(exploration2))
 
-    def result(self):
-        winner, imp = C.c_int(), C.c_double()
-        ret = np.zeros(self.N, np.float32); knots = np.zeros((self.P, self.nu)); kt = np.zeros(self.P)
-        self.lib.mjpc_b200_sampling_planner_get_result(self.h, C.byref(winner), C.byref(imp), _pf(ret), _pd(knots),
-                                                       _pd(kt))
-        return dict(winner=winner.value, improvement=imp.value, returns=ret, knots=knots, knot_times=kt)
+
+class CppCrossEntropyPlanner(_CrossEntropy, _CppPlanner):
+    """The C++ Cross-Entropy planner (csrc/host/cross_entropy_planner.cc) through its C wrappers."""
+
+    def __init__(self, model, num_trajectory, horizon, n_elite=0, seed=0x5EED, device=0):
+        self._start(model, horizon, device, self._args(model, num_trajectory, seed, n_elite))
+
+
+class CppSampleGradientPlanner(_SampleGradient, _CppPlanner):
+    """The C++ Sample Gradient planner (csrc/host/sample_gradient_planner.cc) through its C wrappers."""
+
+    def __init__(self, model, num_trajectory, horizon, num_gradient=None, gradient_filter=None, seed=0x5EED, device=0):
+        self._start(model, horizon, device, self._args(model, num_trajectory, seed, num_gradient, gradient_filter))
+
+
+class CppRobustPlanner(_Robust, _CppPlanner):
+    """The C++ Robust planner (csrc/host/robust_planner.cc) through its C wrappers."""
+
+    def __init__(self, model, num_trajectory, horizon, ncandidates=-1, nrepetitions=5, xfrc_std=0.1, xfrc_rate=0.1,
+                 seed=0x5EED, device=0):
+        self._start(model, horizon, device,
+                    self._args(model, num_trajectory, seed, ncandidates, nrepetitions, xfrc_std, xfrc_rate))
+
+
+class CppGradientPlanner(_Gradient, _CppPlanner):
+    """The C++ GradientPlanner (csrc/host/gradient_planner.cc) through its C wrappers."""
+    _RETURNS_CODE = True
+
+    def __init__(self, model, horizon, num_trajectory=8, num_spline_points=5, representation=1, fd_tolerance=3e-4, device=0, fd_mode=1):
+        self._start(model, horizon, device,
+                    self._args(model, num_trajectory, num_spline_points, representation, fd_tolerance))
+        self._set_fd(fd_tolerance, fd_mode, -1)
+
+
+class CppILQGPlanner(_ILQG, _CppFeedbackPlanner):
+    """The C++ iLQG planner (csrc/host/ilqg_planner.cc) through its C wrappers."""
+
+    def __init__(self, model, horizon, num_rollouts=10, representation=1, fd_tolerance=3e-4, device=0, fd_mode=1, derivative_skip=0):
+        self._start(model, horizon, device, self._args(model, horizon, num_rollouts, representation, fd_tolerance))
+        self._set_fd(fd_tolerance, fd_mode, derivative_skip)
+
+
+class CppILQSPlanner(_ILQS, _CppFeedbackPlanner):
+    """The C++ iLQSPlanner (csrc/host/gradient_planner.cc) through its C wrappers."""
+
+    def __init__(self, model, horizon, num_trajectory=8, num_rollouts=6, fd_tolerance=3e-4, seed=0x5EED, device=0, fd_mode=1):
+        self._start(model, horizon, device, self._args(model, num_trajectory, seed, num_rollouts, fd_tolerance))
+        self._set_fd(fd_tolerance, fd_mode, -1)
+
+    def set_exploration(self, sigma):
+        self.lib.mjpc_b200_ilqs_planner_set_exploration(self.h, C.c_double(sigma))
 
 
 class _CppBatchPlanner(_CppObject):
@@ -918,17 +1026,16 @@ class _CppBatchPlanner(_CppObject):
     (1 improved / updated, 0 not), as their single planners do."""
     _RETURNS_CODE = False
 
-    def _create(self, prefix, model, *args):
-        super()._create(prefix, model, *args)
+    def _start(self, model, num_problems, horizon, device, args):
+        """mjpc_b200_batch_<kind>_planner_create(model, num_problems, *args, horizon, device), args from the kind's
+        _args."""
+        self.B, self.horizon, self.nu = int(num_problems), int(horizon), model.nu
+        self._create(f"mjpc_b200_batch_{self._KIND}_planner", model, self.B, *args, self.horizon, int(device))
         self._codes = np.zeros(self.B, np.int32)   # of the last optimize_policy
 
-    def _setup(self, model, num_problems, horizon, num_trajectory, seeds):
-        num = model.numeric
-        self.P = int(num.get("sampling_spline_points", [3])[0])
-        self.B, self.horizon, self.N, self.nu = int(num_problems), int(horizon), int(num_trajectory), model.nu
-        self._seeds = np.ascontiguousarray([0x5EED + b for b in range(self.B)] if seeds is None else seeds, np.uint32)
-        self._cr = _d(np.asarray(model.actuator_ctrlrange, float).reshape(-1))
-        return num, _pd(self._cr), self._seeds.ctypes.data_as(C.POINTER(C.c_uint32))
+    def result(self, problem):
+        get_result = getattr(self.lib, f"{self._prefix}_get_result")
+        return self._result(lambda *out: self._check(get_result(self.h, int(problem), *out), "get_result"))
 
     def close(self):
         if getattr(self, "h", None):
@@ -997,175 +1104,69 @@ class _CppBatchFeedbackPlanner(_CppBatchPlanner):
         return self._action(problem, time, state, use_previous)
 
 
-class CppBatchSamplingPlanner(_CppBatchPlanner):
+class CppBatchSamplingPlanner(_Sampling, _CppBatchPlanner):
     """num_problems independent Predictive Sampling problems planned with one rollout launch per iteration
     (csrc/host/batch_planner.cc)."""
 
     def __init__(self, model, num_problems, num_trajectory, horizon, seeds=None, device=0):
-        num, cr, sd = self._setup(model, num_problems, horizon, num_trajectory, seeds)
-        self._create("mjpc_b200_batch_sampling_planner", model, self.B, self.N, self.P, int(num.get("sampling_representation", [2])[0]),
-                     C.c_double(float(num.get("sampling_exploration", [0.1])[0])), C.c_double(float(model.opt_timestep)),
-                     cr, sd, self.horizon, int(device))
-
-    def result(self, problem):
-        winner, imp = C.c_int(), C.c_double()
-        ret = np.zeros(self.N, np.float32); knots = np.zeros((self.P, self.nu)); kt = np.zeros(self.P)
-        self._check(self.lib.mjpc_b200_batch_sampling_planner_get_result(self.h, int(problem), C.byref(winner), C.byref(imp),
-                                                                         _pf(ret), _pd(knots), _pd(kt)), "get_result")
-        return dict(winner=winner.value, improvement=imp.value, returns=ret, knots=knots, knot_times=kt)
+        self._start(model, num_problems, horizon, device, self._args(model, num_trajectory, _seeds(num_problems, seeds)))
 
 
-class CppBatchCrossEntropyPlanner(_CppBatchPlanner):
+class CppBatchCrossEntropyPlanner(_CrossEntropy, _CppBatchPlanner):
     """num_problems independent Cross-Entropy problems, one rollout launch of B x (N + 1) per iteration
     (csrc/host/batch_planner.cc).  Mirrors CppCrossEntropyPlanner with a problem argument."""
 
     def __init__(self, model, num_problems, num_trajectory, horizon, n_elite=0, seeds=None, device=0):
-        num, cr, sd = self._setup(model, num_problems, horizon, num_trajectory, seeds)
-        self._create(
-            "mjpc_b200_batch_ce_planner", model, self.B, self.N, int(n_elite), self.P,
-            int(num.get("sampling_representation", [2])[0]), C.c_double(float(num.get("sampling_exploration", [0.1])[0])),
-            C.c_double(float(num.get("std_min", [0.01])[0])), C.c_double(float(num.get("explore_fraction", [0.0])[0])),
-            C.c_double(float(model.opt_timestep)), cr, sd, self.horizon, int(device))
-
-    def result(self, problem):
-        imp = C.c_double()
-        ret = np.zeros(self.N + 1, np.float32); order = np.zeros(self.N, np.int32)
-        knots = np.zeros((self.P, self.nu)); kt = np.zeros(self.P); var = np.zeros((self.P, self.nu))
-        self._check(self.lib.mjpc_b200_batch_ce_planner_get_result(self.h, int(problem), C.byref(imp), _pf(ret),
-                                                                   order.ctypes.data_as(_ip), _pd(knots), _pd(kt), _pd(var)),
-                    "get_result")
-        return dict(improvement=imp.value, returns=ret, order=order, knots=knots, knot_times=kt, variance=var)
+        self._start(model, num_problems, horizon, device,
+                    self._args(model, num_trajectory, _seeds(num_problems, seeds), n_elite))
 
 
-class CppBatchSampleGradientPlanner(_CppBatchPlanner):
+class CppBatchSampleGradientPlanner(_SampleGradient, _CppBatchPlanner):
     """num_problems independent Sample Gradient problems, one rollout launch of B x N per iteration
     (csrc/host/batch_planner.cc).  Mirrors CppSampleGradientPlanner with a problem argument."""
 
     def __init__(self, model, num_problems, num_trajectory, horizon, num_gradient=None, gradient_filter=None, seeds=None,
                  device=0):
-        num, cr, sd = self._setup(model, num_problems, horizon, num_trajectory, seeds)
-        G = int(num_gradient if num_gradient is not None else num.get("sample_gradient_trajectories", [0])[0])
-        self.G = max(min(G, self.N - 1), 0)                  # the clamp OptimizePolicy applies
-        f = float(gradient_filter if gradient_filter is not None else num.get("sample_gradient_filter", [1.0])[0])
-        self._create(
-            "mjpc_b200_batch_sg_planner", model, self.B, self.N, G, self.P, int(num.get("sampling_representation", [2])[0]),
-            C.c_double(float(num.get("sampling_exploration", [0.1])[0])), C.c_double(f),
-            C.c_double(float(model.opt_timestep)), cr, sd, self.horizon, int(device))
-
-    def result(self, problem):
-        winner, wtype, imp = C.c_int(), C.c_int(), C.c_double()
-        ret = np.zeros(self.N, np.float32); order = np.zeros(self.N, np.int32)
-        knots = np.zeros((self.P, self.nu)); kt = np.zeros(self.P)
-        gk = np.zeros((self.G, self.P, self.nu)); grad = np.zeros((self.P, self.nu))
-        n = self._check(self.lib.mjpc_b200_batch_sg_planner_get_result(
-            self.h, int(problem), C.byref(winner), C.byref(wtype), C.byref(imp), _pf(ret), order.ctypes.data_as(_ip),
-            _pd(knots), _pd(kt), _pd(gk) if self.G else None, _pd(grad)), "get_result")
-        return dict(winner=winner.value, winner_type=wtype.value, improvement=imp.value, returns=ret, order=order,
-                    knots=knots[:n], knot_times=kt[:n], gradient_knots=gk, gradient=grad)
+        self._start(model, num_problems, horizon, device,
+                    self._args(model, num_trajectory, _seeds(num_problems, seeds), num_gradient, gradient_filter))
 
 
-class CppBatchRobustPlanner(_CppBatchPlanner):
+class CppBatchRobustPlanner(_Robust, _CppBatchPlanner):
     """num_problems independent Robust problems (csrc/host/batch_planner.cc): per iteration one clean launch of B x N
     and one noisy launch of B x ncandidates x nrepetitions, each problem with its own noise key.  Mirrors
     CppRobustPlanner with a problem argument."""
 
     def __init__(self, model, num_problems, num_trajectory, horizon, ncandidates=-1, nrepetitions=5, xfrc_std=0.1,
                  xfrc_rate=0.1, seeds=None, device=0):
-        num, cr, sd = self._setup(model, num_problems, horizon, num_trajectory, seeds)
-        self.nc = int(ncandidates if ncandidates != -1 else num_trajectory // nrepetitions)
-        self._create(
-            "mjpc_b200_batch_robust_planner", model, self.B, self.N, self.P, int(num.get("sampling_representation", [2])[0]),
-            C.c_double(float(num.get("sampling_exploration", [0.1])[0])), C.c_double(float(model.opt_timestep)), cr, sd,
-            int(ncandidates), int(nrepetitions), C.c_double(xfrc_std), C.c_double(xfrc_rate), self.horizon, int(device))
+        self._start(model, num_problems, horizon, device,
+                    self._args(model, num_trajectory, _seeds(num_problems, seeds), ncandidates, nrepetitions, xfrc_std,
+                               xfrc_rate))
+
+
+class CppBatchGradientPlanner(_Gradient, _CppBatchPlanner):
+    """num_problems independent Gradient problems (csrc/host/batch_planner.cc): per iteration one launch of the B
+    nominals, one mjpc_b200_gradient_batched and one launch of the B x num_trajectory line-search candidates.  Mirrors
+    CppGradientPlanner with a problem argument; optimize_policy returns each problem's 1/0."""
+    _RETURNS_CODE = True
+
+    def __init__(self, model, num_problems, horizon, num_trajectory=8, num_spline_points=5, representation=1,
+                 fd_tolerance=3e-4, device=0, fd_mode=1):
+        self._start(model, num_problems, horizon, device,
+                    self._args(model, num_trajectory, num_spline_points, representation, fd_tolerance))
+        self.set_fd(fd_tolerance, fd_mode, -1)
 
     def result(self, problem):
-        winner = C.c_int()
-        scores = np.zeros(max(self.nc, 1)); ret = np.zeros(self.N, np.float32)
-        knots = np.zeros((self.P, self.nu)); kt = np.zeros(self.P)
-        n = self._check(self.lib.mjpc_b200_batch_robust_planner_get_result(self.h, int(problem), C.byref(winner), _pd(scores),
-                                                                           _pf(ret), _pd(knots), _pd(kt)), "get_result")
-        return dict(winner=winner.value, scores=scores[:n], returns=ret, knots=knots, knot_times=kt)
+        return dict(super().result(problem), improved=int(self._codes[problem]))
 
 
-class CppCrossEntropyPlanner(_CppPlanner):
-    """The C++ Cross-Entropy planner (csrc/host/cross_entropy_planner.cc) through its C wrappers."""
-
-    def __init__(self, model, num_trajectory, horizon, n_elite=0, seed=0x5EED, device=0):
-        m, num = model, model.numeric
-        self.P = int(num.get("sampling_spline_points", [3])[0])
-        self.horizon, self.N, self.nu = int(horizon), int(num_trajectory), m.nu
-        cr = _d(np.asarray(m.actuator_ctrlrange, float).reshape(-1))
-        self._create(
-            "mjpc_b200_ce_planner", m, self.N, int(n_elite), self.P, int(num.get("sampling_representation", [2])[0]),
-            C.c_double(float(num.get("sampling_exploration", [0.1])[0])), C.c_double(float(num.get("std_min", [0.01])[0])),
-            C.c_double(float(num.get("explore_fraction", [0.0])[0])), C.c_double(float(m.opt_timestep)), _pd(cr),
-            C.c_uint32(seed), self.horizon, int(device))
-
-    def result(self):
-        imp = C.c_double()
-        ret = np.zeros(self.N + 1, np.float32); order = np.zeros(self.N, np.int32)
-        knots = np.zeros((self.P, self.nu)); kt = np.zeros(self.P); var = np.zeros((self.P, self.nu))
-        self.lib.mjpc_b200_ce_planner_get_result(self.h, C.byref(imp), _pf(ret), order.ctypes.data_as(C.POINTER(C.c_int)),
-                                                 _pd(knots), _pd(kt), _pd(var))
-        return dict(improvement=imp.value, returns=ret, order=order, knots=knots, knot_times=kt, variance=var)
-
-
-class CppSampleGradientPlanner(_CppPlanner):
-    """The C++ Sample Gradient planner (csrc/host/sample_gradient_planner.cc) through its C wrappers."""
-
-    def __init__(self, model, num_trajectory, horizon, num_gradient=None, gradient_filter=None, seed=0x5EED, device=0):
-        m, num = model, model.numeric
-        self.P = int(num.get("sampling_spline_points", [3])[0])
-        self.horizon, self.N, self.nu = int(horizon), int(num_trajectory), m.nu
-        G = int(num_gradient if num_gradient is not None else num.get("sample_gradient_trajectories", [0])[0])
-        self.G = max(min(G, self.N - 1), 0)                  # the clamp OptimizePolicy applies
-        f = float(gradient_filter if gradient_filter is not None else num.get("sample_gradient_filter", [1.0])[0])
-        cr = _d(np.asarray(m.actuator_ctrlrange, float).reshape(-1))
-        self._create(
-            "mjpc_b200_sg_planner", m, self.N, G, self.P, int(num.get("sampling_representation", [2])[0]),
-            C.c_double(float(num.get("sampling_exploration", [0.1])[0])), C.c_double(f), C.c_double(float(m.opt_timestep)),
-            _pd(cr), C.c_uint32(seed), self.horizon, int(device))
-
-    def result(self):
-        winner, wtype, imp = C.c_int(), C.c_int(), C.c_double()
-        ret = np.zeros(self.N, np.float32); order = np.zeros(self.N, np.int32)
-        knots = np.zeros((self.P, self.nu)); kt = np.zeros(self.P)
-        gk = np.zeros((self.G, self.P, self.nu)); grad = np.zeros((self.P, self.nu))
-        n = self.lib.mjpc_b200_sg_planner_get_result(self.h, C.byref(winner), C.byref(wtype), C.byref(imp), _pf(ret),
-                                                     order.ctypes.data_as(_ip), _pd(knots), _pd(kt),
-                                                     _pd(gk) if self.G else None, _pd(grad))
-        return dict(winner=winner.value, winner_type=wtype.value, improvement=imp.value, returns=ret, order=order,
-                    knots=knots[:n], knot_times=kt[:n], gradient_knots=gk, gradient=grad)
-
-
-class CppILQGPlanner(_CppFeedbackPlanner):
-    """The C++ iLQG planner (csrc/host/ilqg_planner.cc) through its C wrappers."""
-
-    def __init__(self, model, horizon, num_rollouts=10, representation=1, fd_tolerance=3e-4, device=0, fd_mode=1, derivative_skip=0):
-        self.H = self.horizon = int(horizon)
-        self.nu, self.ds = model.nu, model.nq + model.nv
-        self._create("mjpc_b200_ilqg_planner", model, int(num_rollouts), int(representation), C.c_double(fd_tolerance),
-                     self.H, int(device))
-        self._set_fd(fd_tolerance, fd_mode, derivative_skip)
-
-    def result(self):
-        sc = np.zeros(6); st = np.zeros((self.H, self.ds), np.float32); ac = np.zeros((self.H, self.nu), np.float32)
-        tm = np.zeros(self.H)
-        self.lib.mjpc_b200_ilqg_planner_get_result(self.h, _pd(sc), _pf(st), _pf(ac), _pd(tm))
-        return dict(total_return=sc[0], regularization=sc[1], improvement=sc[2], expected=sc[3], surprise=sc[4],
-                    winner=int(sc[5]), states=st, actions=ac, times=tm)
-
-
-class CppBatchILQGPlanner(_CppBatchFeedbackPlanner):
+class CppBatchILQGPlanner(_ILQG, _CppBatchFeedbackPlanner):
     """The batched C++ iLQG planner (csrc/host/batch_planner.cc): B problems, one launch per sweep.  Mirrors
     CppILQGPlanner with a problem argument."""
 
     def __init__(self, model, num_problems, horizon, num_rollouts=10, representation=1, fd_tolerance=3e-4, device=0,
                  fd_mode=1, derivative_skip=0):
-        self.B, self.H = int(num_problems), int(horizon)
-        self.horizon, self.nu, self.ds = self.H, model.nu, model.nq + model.nv
-        self._create("mjpc_b200_batch_ilqg_planner", model, self.B, int(num_rollouts), int(representation),
-                     C.c_double(fd_tolerance), self.H, int(device))
+        self._start(model, num_problems, horizon, device,
+                    self._args(model, horizon, num_rollouts, representation, fd_tolerance))
         self.set_fd(fd_tolerance, fd_mode, derivative_skip)
 
     def nominal_trajectory(self):
@@ -1175,37 +1176,24 @@ class CppBatchILQGPlanner(_CppBatchFeedbackPlanner):
         """Every problem's iLQGPlanner::OptimizePolicy; returns updated [B] (1: the policy was updated)."""
         return np.array(super().optimize_policy(), np.int32)
 
+
+class CppBatchILQSPlanner(_ILQS, _CppBatchFeedbackPlanner):
+    """num_problems independent iLQS problems (csrc/host/batch_planner.cc) on two handles: per iteration one feedback
+    launch of the iLQG nominals that need converting, one sampling launch of B x num_trajectory, and one batched iLQG
+    iteration of the problems sampling did not settle.  Mirrors CppILQSPlanner with a problem argument;
+    optimize_policy returns each problem's 1/0."""
+
+    def __init__(self, model, num_problems, horizon, num_trajectory=8, num_rollouts=6, fd_tolerance=3e-4, seeds=None,
+                 device=0, fd_mode=1):
+        self._start(model, num_problems, horizon, device,
+                    self._args(model, num_trajectory, _seeds(num_problems, seeds), num_rollouts, fd_tolerance))
+        self.set_fd(fd_tolerance, fd_mode, -1)
+
+    def set_exploration(self, sigma):
+        self._check(self.lib.mjpc_b200_batch_ilqs_planner_set_exploration(self.h, C.c_double(sigma)), "set_exploration")
+
     def result(self, problem):
-        sc = np.zeros(6); st = np.zeros((self.H, self.ds), np.float32); ac = np.zeros((self.H, self.nu), np.float32)
-        tm = np.zeros(self.H)
-        self._check(self.lib.mjpc_b200_batch_ilqg_planner_get_result(self.h, int(problem), _pd(sc), _pf(st), _pf(ac), _pd(tm)),
-                    "get_result")
-        return dict(total_return=sc[0], regularization=sc[1], improvement=sc[2], expected=sc[3], surprise=sc[4],
-                    winner=int(sc[5]), states=st, actions=ac, times=tm)
-
-
-class CppRobustPlanner(_CppPlanner):
-    """The C++ Robust planner (csrc/host/robust_planner.cc) through its C wrappers."""
-
-    def __init__(self, model, num_trajectory, horizon, ncandidates=-1, nrepetitions=5, xfrc_std=0.1, xfrc_rate=0.1,
-                 seed=0x5EED, device=0):
-        m, num = model, model.numeric
-        self.P = int(num.get("sampling_spline_points", [3])[0])
-        self.horizon, self.N, self.nu = int(horizon), int(num_trajectory), m.nu
-        self.nc = int(ncandidates if ncandidates != -1 else num_trajectory // nrepetitions)
-        cr = _d(np.asarray(m.actuator_ctrlrange, float).reshape(-1))
-        self._create(
-            "mjpc_b200_robust_planner", m, self.N, self.P, int(num.get("sampling_representation", [2])[0]),
-            C.c_double(float(num.get("sampling_exploration", [0.1])[0])), C.c_double(float(m.opt_timestep)), _pd(cr),
-            C.c_uint32(seed), int(ncandidates), int(nrepetitions), C.c_double(xfrc_std), C.c_double(xfrc_rate),
-            self.horizon, int(device))
-
-    def result(self):
-        winner = C.c_int()
-        scores = np.zeros(max(self.nc, 1)); ret = np.zeros(self.N, np.float32)
-        knots = np.zeros((self.P, self.nu)); kt = np.zeros(self.P)
-        n = self.lib.mjpc_b200_robust_planner_get_result(self.h, C.byref(winner), _pd(scores), _pf(ret), _pd(knots), _pd(kt))
-        return dict(winner=winner.value, scores=scores[:n], returns=ret, knots=knots, knot_times=kt)
+        return dict(super().result(problem), improved=int(self._codes[problem]))
 
 
 def host_spline_mapping(representation, input_times, output_times):
@@ -1226,95 +1214,6 @@ def host_gradient_sweep(A, B, cx, cu):
     k, dV0 = np.zeros((T, m)), C.c_double()
     lib.mjpc_b200_host_gradient_sweep(_pf(a), _pf(b), _pf(x), _pf(u), int(n), int(m), int(T), _pd(k), C.byref(dV0))
     return k, dV0.value
-
-
-class CppBatchGradientPlanner(_CppBatchPlanner):
-    """num_problems independent Gradient problems (csrc/host/batch_planner.cc): per iteration one launch of the B
-    nominals, one mjpc_b200_gradient_batched and one launch of the B x num_trajectory line-search candidates.  Mirrors
-    CppGradientPlanner with a problem argument; optimize_policy returns each problem's 1/0."""
-    _RETURNS_CODE = True
-
-    def __init__(self, model, num_problems, horizon, num_trajectory=8, num_spline_points=5, representation=1,
-                 fd_tolerance=3e-4, device=0, fd_mode=1):
-        cr = _d(np.asarray(model.actuator_ctrlrange, float).reshape(-1))
-        self.B, self.horizon, self.P, self.nu = int(num_problems), int(horizon), int(num_spline_points), model.nu
-        self._create("mjpc_b200_batch_gradient_planner", model, self.B, int(num_trajectory), self.P, int(representation),
-                     C.c_double(fd_tolerance), C.c_double(float(model.opt_timestep)), _pd(cr), self.horizon, int(device))
-        self.set_fd(fd_tolerance, fd_mode, -1)
-
-    def result(self, problem):
-        sc = np.zeros(6); p = np.zeros((self.P, self.nu)); t = np.zeros(self.P)
-        self._check(self.lib.mjpc_b200_batch_gradient_planner_get_result(self.h, int(problem), _pd(sc), _pd(p), _pd(t)),
-                    "get_result")
-        return dict(total_return=sc[0], winner=int(sc[1]), action_step=sc[2], expected=sc[3], improvement=sc[4],
-                    surprise=sc[5], parameters=p, times=t, improved=int(self._codes[problem]))
-
-
-class CppBatchILQSPlanner(_CppBatchFeedbackPlanner):
-    """num_problems independent iLQS problems (csrc/host/batch_planner.cc) on two handles: per iteration one feedback
-    launch of the iLQG nominals that need converting, one sampling launch of B x num_trajectory, and one batched iLQG
-    iteration of the problems sampling did not settle.  Mirrors CppILQSPlanner with a problem argument;
-    optimize_policy returns each problem's 1/0."""
-
-    def __init__(self, model, num_problems, horizon, num_trajectory=8, num_rollouts=6, fd_tolerance=3e-4, seeds=None,
-                 device=0, fd_mode=1):
-        num, cr, sd = self._setup(model, num_problems, horizon, num_trajectory, seeds)
-        self._create("mjpc_b200_batch_ilqs_planner", model, self.B, self.N, self.P,
-                     int(num.get("sampling_representation", [2])[0]),
-                     C.c_double(float(num.get("sampling_exploration", [0.1])[0])), C.c_double(float(model.opt_timestep)),
-                     cr, sd, int(num_rollouts), int(num.get("ilqg_representation", [1])[0]), C.c_double(fd_tolerance),
-                     self.horizon, int(device))
-        self.set_fd(fd_tolerance, fd_mode, -1)
-
-    def set_exploration(self, sigma):
-        self._check(self.lib.mjpc_b200_batch_ilqs_planner_set_exploration(self.h, C.c_double(sigma)), "set_exploration")
-
-    def result(self, problem):
-        sc = np.zeros(4)
-        self._check(self.lib.mjpc_b200_batch_ilqs_planner_get_result(self.h, int(problem), _pd(sc)), "get_result")
-        return dict(active_policy=int(sc[0]), sampling_return=sc[1], ilqg_return=sc[2], sampling_winner=int(sc[3]),
-                    improved=int(self._codes[problem]))
-
-
-class CppGradientPlanner(_CppPlanner):
-    """The C++ GradientPlanner (csrc/host/gradient_planner.cc) through its C wrappers."""
-    _RETURNS_CODE = True
-
-    def __init__(self, model, horizon, num_trajectory=8, num_spline_points=5, representation=1, fd_tolerance=3e-4, device=0, fd_mode=1):
-        cr = _d(np.asarray(model.actuator_ctrlrange, float).reshape(-1))
-        self.horizon, self.P, self.nu = int(horizon), int(num_spline_points), model.nu
-        self._create("mjpc_b200_gradient_planner", model, int(num_trajectory), self.P, int(representation),
-                     C.c_double(fd_tolerance), C.c_double(float(model.opt_timestep)), _pd(cr), self.horizon, int(device))
-        self._set_fd(fd_tolerance, fd_mode, -1)
-
-    def result(self):
-        sc = np.zeros(6); p = np.zeros((self.P, self.nu)); t = np.zeros(self.P)
-        self.lib.mjpc_b200_gradient_planner_get_result(self.h, _pd(sc), _pd(p), _pd(t))
-        return dict(total_return=sc[0], winner=int(sc[1]), action_step=sc[2], expected=sc[3], improvement=sc[4],
-                    surprise=sc[5], parameters=p, times=t)
-
-
-class CppILQSPlanner(_CppFeedbackPlanner):
-    """The C++ iLQSPlanner (csrc/host/gradient_planner.cc) through its C wrappers."""
-
-    def __init__(self, model, horizon, num_trajectory=8, num_rollouts=6, fd_tolerance=3e-4, seed=0x5EED, device=0, fd_mode=1):
-        m, num = model, model.numeric
-        cr = _d(np.asarray(m.actuator_ctrlrange, float).reshape(-1))
-        self.horizon, self.nu = int(horizon), m.nu
-        self._create("mjpc_b200_ilqs_planner", m, int(num_trajectory), int(num.get("sampling_spline_points", [3])[0]),
-                     int(num.get("sampling_representation", [2])[0]),
-                     C.c_double(float(num.get("sampling_exploration", [0.1])[0])), C.c_double(float(m.opt_timestep)),
-                     _pd(cr), C.c_uint32(seed), int(num_rollouts), int(num.get("ilqg_representation", [1])[0]),
-                     C.c_double(fd_tolerance), self.horizon, int(device))
-        self._set_fd(fd_tolerance, fd_mode, -1)
-
-    def set_exploration(self, sigma):
-        self.lib.mjpc_b200_ilqs_planner_set_exploration(self.h, C.c_double(sigma))
-
-    def result(self):
-        sc = np.zeros(4)
-        self.lib.mjpc_b200_ilqs_planner_get_result(self.h, _pd(sc))
-        return dict(active_policy=int(sc[0]), sampling_return=sc[1], ilqg_return=sc[2], sampling_winner=int(sc[3]))
 
 
 class CppAgent(_CppObject):

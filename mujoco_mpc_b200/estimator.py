@@ -42,10 +42,11 @@ reference are the Unscented filter's (the warm start is the centre state's qacc 
 from __future__ import annotations
 
 import ctypes as C
+import functools
 
 import numpy as np
 
-from .engine import EngineError, _CppObject, _d, _dp, _fp, _model_blobs, _pd, _pf
+from .engine import EngineError, _CppObject, _d, _model_blobs, _pd, _pf
 from .mjcf import JNT_BALL, JNT_FREE, SENS_MEASURED
 
 
@@ -355,6 +356,14 @@ class Unscented(_Filter):
         return self.state
 
 
+def _get_filter(f, get):
+    """(state, covariance, time, scalars) of the C++ filter object f, read by get(state, covariance, time, scalars)."""
+    x, P = np.zeros(f.m.nq + f.m.nv), np.zeros((f.ndstate, f.ndstate))
+    t, sc = C.c_double(), np.zeros(f._nscalars)
+    f._check(get(_pd(x), _pd(P), C.byref(t), _pd(sc)))
+    return x, P, t.value, sc
+
+
 class _CppFilter(_CppObject):
     """What CppUnscented and CppKalman share: the C++ filter behind the generic mjpc_b200_estimator_* entry points (its
     reset, noise, set, update and get), the ctrl / sensor / mocap marshalling and the EstimatorError of a failed
@@ -396,10 +405,7 @@ class _CppFilter(_CppObject):
         return _pd(u), _pd(y), _pf(mc)
 
     def _get(self):
-        x, P = np.zeros(self.m.nq + self.m.nv), np.zeros((self.ndstate, self.ndstate))
-        t, sc = C.c_double(), np.zeros(self._nscalars)
-        self._check(self.lib.mjpc_b200_estimator_get(self.h, _pd(x), _pd(P), C.byref(t), _pd(sc)))
-        return x, P, t.value, sc
+        return _get_filter(self, functools.partial(self.lib.mjpc_b200_estimator_get, self.h))
 
     @property
     def state(self):
@@ -565,15 +571,6 @@ class CppBatchEstimator(_CppObject):
         self._settings = np.array(prm, float)
         self._create("mjpc_b200_batch_estimator", m, self.KINDS[kind], self.num_filters, self.sensor_start,
                      self.nsensor, C.c_double(self.timestep), _pd(self._settings), int(device))
-        for f, args in ((self.lib.mjpc_b200_batch_estimator_reset, [C.c_int, _dp] + [C.c_double] * 4),
-                        (self.lib.mjpc_b200_batch_estimator_set_noise, [C.c_int, _dp, _dp]),
-                        (self.lib.mjpc_b200_batch_estimator_set, [C.c_int, _dp, _dp, C.c_double]),
-                        (self.lib.mjpc_b200_batch_estimator_update, [_dp, _dp, _fp, C.POINTER(C.c_int)]),
-                        (self.lib.mjpc_b200_batch_estimator_get, [C.c_int] + [_dp] * 4),
-                        (self.lib.mjpc_b200_batch_estimator_destroy, [])):
-            f.argtypes, f.restype = [C.c_void_p] + args, C.c_int
-        self.lib.mjpc_b200_batch_estimator_last_error.argtypes = [C.c_void_p]
-        self.lib.mjpc_b200_batch_estimator_last_error.restype = C.c_char_p
         for b in range(self.num_filters):
             self.reset(b)
 
@@ -614,10 +611,7 @@ class CppBatchEstimator(_CppObject):
 
     def get(self, b):
         """(state, covariance, time, scalars) of filter b."""
-        x, P = np.zeros(self.m.nq + self.m.nv), np.zeros((self.ndstate, self.ndstate))
-        t, sc = C.c_double(), np.zeros(self._nscalars)
-        self._check(self.lib.mjpc_b200_batch_estimator_get(self.h, b, _pd(x), _pd(P), C.byref(t), _pd(sc)))
-        return x, P, t.value, sc
+        return _get_filter(self, functools.partial(self.lib.mjpc_b200_batch_estimator_get, self.h, b))
 
     def state(self, b):
         return self.get(b)[0]
