@@ -394,13 +394,24 @@ int pick_kernels(const mjpc_b200* h, const KernelSet** k) {
   return sh && sh[0] == 'p' && sh[1] == 'l' ? 2 : 1;
 }
 
-// src (NULL: the handle's task state) as floats, with its time-like entries made relative to t0
+// src (NULL: the handle's task state) as floats, with its time-like entries made relative to t0.  The Quadruped's gait
+// phase start is an absolute phase that grows at 2 pi cadence per second, so it is folded to t0 as well: the phase at
+// t0 in double, less whole periods, and phase start time 0.  Periods come off only while the phase stays >= 2 pi: the
+// gait's fmod(phase + pi - footphase, 2 pi) keeps the sign of its argument, which is negative early in an episode
+// (phase < footphase - pi), and a phase of at least 2 pi keeps it positive.
 void rebase_task_state(const mjpc_b200* h, const double* src, double t0, float* dst) {
   if (!src) src = h->task_state.data();
   for (int i = 0; i < h->pack.M.task_state_size; i++) {
     double v = src[i];
     if (std::find(h->time_idx.begin(), h->time_idx.end(), i) != h->time_idx.end()) v -= t0;
     dst[i] = (float)v;
+  }
+  if (h->pack.M.residual_id == RESIDUAL_QUADRUPED_FLAT) {
+    const double period = 2 * M_PI;
+    const double phase = src[QS_PHASE_START] + (t0 - src[QS_PHASE_START_TIME]) * src[QS_PHASE_VELOCITY];
+    const double k = std::max(0.0, std::floor(phase / period) - 1);
+    dst[QS_PHASE_START] = (float)(phase - k * period);
+    dst[QS_PHASE_START_TIME] = 0.f;
   }
 }
 
