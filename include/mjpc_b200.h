@@ -195,6 +195,48 @@ int mjpc_b200_fetch_trajectory_member(mjpc_b200_t* h, int candidate, int member,
 void mjpc_b200_host_ensemble_score(const float* member_returns, const uint8_t* member_failure, int K, int worst,
                                    float* score, uint8_t* failure);
 
+/* An initial-state ensemble: rollout_spline_batched with every candidate scored over K initial states drawn from each
+ * problem's state covariance, so that a candidate that does well only from the exact mean state does not win when the
+ * state estimate is uncertain.  Arguments as rollout_spline_batched, plus:
+ *   covariances [B][n][n] (double, n = 2 nv: the filters' tangent space, positions then velocities), K members per
+ *   problem, worst (the score is the mean of the `worst` largest member returns: set_model_ensemble's rule, with its
+ *   failure rule), and seed / iteration of the draws.
+ * Member 0 of problem b starts from states[b] itself; member k >= 1 from states[b] (+) L_b z_{b,k}, where L_b is the
+ * lower Cholesky factor of (P_b + P_b') / 2 and (+) is mj_integratePos for the position half (free and ball joints:
+ * the quaternion times exp(w / 2), normalised; a rotation of exactly zero keeps the quaternion bit for bit) and addition
+ * for the velocity half (a zero entry keeps the coordinate bit for bit).  z is a standard normal: Philox4x32-10 with key
+ * (seed + b, 3) and counter (iteration, k, element, 'BELF'), Box-Muller in double on the first two words; key word 3 is
+ * used by no candidate-noise or plant-noise draw.  The factor, L z and (+) are computed in double on the device (one
+ * CTA per problem), and the member states are written as float straight into the launch's state rows.  A pivot of
+ * exactly 0 whose column below is all zero gives a zero column, so a zero covariance gives K copies of the mean and
+ * scores equal to the plain launch's returns.
+ * The launch holds B*K*N trajectories, member k of problem b as launch problem b*K + k (the model ensemble's layout):
+ * returns / failure / order are the scores [B][N], fetch_ensemble gives the member returns [B][K][N],
+ * fetch_trajectory_member any member's trajectory and fetch_trajectory / fetch_all member 0's.  With model variants
+ * set (B must then be their count or select_model_variants' B), every member row of problem b runs on problem b's
+ * variant.  The launch does not become the resident one (launch_resident refuses until the next upload).
+ * Refusals, each before anything is staged and with the handle unchanged: K outside [1, 32], worst outside [1, K], a
+ * non-finite covariance entry (last_error names the problem) or bad sizes: MJPC_B200_ERR_BAD_ARGUMENT; B*N above
+ * max_candidates (or H, P above capacity): MJPC_B200_ERR_CAPACITY; a model ensemble or force noise (set_xfrc_noise*)
+ * set on the handle: MJPC_B200_ERR_UNSUPPORTED naming the call.  As set_model_ensemble does, the call grows the
+ * per-trajectory device buffers to K x max_candidates trajectories (never shrinks them; MJPC_B200_ERR_CUDA if that
+ * fails), so the launch holds up to K x max_candidates trajectories; it also allocates its own tables once.  A
+ * covariance whose factorisation fails (a pivot < 0,
+ * a zero pivot with a non-zero column below, or a non-finite pivot) returns MJPC_B200_ERR_BAD_ARGUMENT with last_error
+ * naming the problem, and no rollout is launched and no returns are written; the handle stays usable. */
+int mjpc_b200_rollout_spline_belief_batched(mjpc_b200_t* h, int B, int K, int worst, uint32_t seed, uint32_t iteration,
+                                            const float* states, const double* covariances, const double* times,
+                                            const float* mocaps, const double* weights, const double* parameters,
+                                            const double* task_states, const float* knots, const double* knot_times,
+                                            int interp, int P, int N, int H, float* returns, uint8_t* failure,
+                                            int* order);
+/* Member `member` (0..31) of problem `problem` of a belief launch on the host, in double (for tests): out [nq + nv] is
+ * state (+) L z with the launch's factor, draw and (+), summed in the same order; the device's member states are this
+ * rounded to float, up to fp64 contractions.  MJPC_B200_ERR_BAD_ARGUMENT for a non-finite covariance or a failed
+ * factorisation (out then holds state), MJPC_B200_ERR_BAD_BLOB for a bad blob. */
+int mjpc_b200_host_state_member(const mjpc_model_blob* model, const double* state, const double* covariance,
+                                uint32_t seed, uint32_t iteration, int problem, int member, double* out);
+
 /* K line-search rollouts of the iLQG policy. u_nom [H][nu], x_nom [H][dim_state], t_nom [H] (absolute),
  * gains [H][nu][dim_dstate], du [H][nu] (may be NULL), step_sizes [K]. */
 int mjpc_b200_rollout_feedback(mjpc_b200_t* h, const float* state, double time, const float* mocap,
@@ -391,6 +433,16 @@ int mjpc_b200_plant_set_disturbance(mjpc_b200_t* h, int plant, double ctrl_std, 
 /* The wrench xfrc [nbody][6] held on plant `plant` until changed (ApplyForcePerturbations headless); NULL clears it.
  * BAD_ARGUMENT: a non-finite value. */
 int mjpc_b200_plant_set_xfrc(mjpc_b200_t* h, int plant, const float* xfrc);
+/* Measurement noise of plant `plant`: std [nsensordata] (one entry per element of plant_init's sensor range; NULL
+ * clears it).  Each committed step of the running plant returns sensordata[e] + std[e] z, z a standard normal from
+ * Philox4x32-10 with key (seed, 2) and counter (the committed step count before the step, 0, e, 'SENS'): it depends on
+ * the plant's seed (set_disturbance) and its own history only, never on its index or the other plants, never repeats
+ * the control or force noise, and plant_reset replays it.  Quaternion sensors (framequat, ballquat) get the noise
+ * added to each component, without renormalisation.  Only the returned measurement changes: the plant's state, cost
+ * and warm start are bitwise what they are without noise, elements whose std is 0 are bitwise unchanged, and a plant
+ * whose stds are all 0 steps exactly as one without the call.  BAD_ARGUMENT: a negative or non-finite entry (the plant
+ * is then unchanged). */
+int mjpc_b200_plant_set_sensor_noise(mjpc_b200_t* h, int plant, const float* std);
 /* Plant `plant`'s OU states; either pointer may be NULL: ctrl_noise [nu], xfrc_noise [nbody][6]. */
 int mjpc_b200_plant_get_disturbance(mjpc_b200_t* h, int plant, float* ctrl_noise, float* xfrc_noise);
 /* The ctrl every plant applied in the last plant_step, [num_plants][nu]: commanded + control noise (the commanded ctrl,
@@ -586,6 +638,19 @@ int mjpc_b200_planner_set_fd(mjpc_b200_planner_t* p, double tolerance, int mode,
  * the best trajectory is member 0's trajectory of the winner with the winner's score as its return.  Sampling,
  * Cross-Entropy and Sample Gradient; Robust, Gradient, iLQG and iLQS return MJPC_B200_ERR_UNSUPPORTED. */
 int mjpc_b200_planner_set_ensemble(mjpc_b200_planner_t* p, const mjpc_model_blob* models, int K, int worst);
+/* Plan over the state estimate's uncertainty: every spline launch of the planner becomes
+ * mjpc_b200_rollout_spline_belief_batched with K members per problem, `worst`, `seed` and the planner's own iteration
+ * counter, from the covariance of set_state_covariance.  The planner ranks by the scores, as with a model ensemble.
+ * K = 0 clears it.  K outside [0, 32] or worst outside [1, K]: MJPC_B200_ERR_BAD_ARGUMENT.  Refused
+ * (MJPC_B200_ERR_UNSUPPORTED) while a model ensemble is set, and set_ensemble (K > 0) is refused while a state ensemble
+ * is set.  Sampling, Cross-Entropy and Sample Gradient; Robust, Gradient, iLQG and iLQS return
+ * MJPC_B200_ERR_UNSUPPORTED. */
+int mjpc_b200_planner_set_state_ensemble(mjpc_b200_planner_t* p, int K, int worst, uint32_t seed);
+/* The state covariance [2 nv][2 nv] (double) the planner's state-ensemble launches draw from until the next call; NULL
+ * is zero, as is a planner's covariance before the first call (its members then all equal the mean and its scores are
+ * the plain returns).  A non-finite entry: MJPC_B200_ERR_BAD_ARGUMENT, nothing changed.  The kinds of
+ * set_state_ensemble. */
+int mjpc_b200_planner_set_state_covariance(mjpc_b200_planner_t* p, const double* covariance);
 /* mjpc_b200_set_task on every engine handle the planner plans on (the task snapshot Agent gives it per iteration) */
 int mjpc_b200_planner_set_task(mjpc_b200_planner_t* p, const mjpc_task_desc* task);
 
@@ -741,7 +806,12 @@ int mjpc_b200_ilqs_planner_get_result(mjpc_b200_planner_t* p, double* scalars);
  *   set_fd              mjpc_b200_planner_set_fd of every problem: Gradient, iLQG and iLQS; the others return
  *                       MJPC_B200_ERR_UNSUPPORTED
  *   set_ensemble        every problem plans on the same model ensemble: mjpc_b200_planner_set_ensemble's kinds and
- *                       refusals, on the batch's handle */
+ *                       refusals, on the batch's handle
+ *   set_state_ensemble  every problem plans over its state covariance with the same K, worst and seed:
+ *                       mjpc_b200_planner_set_state_ensemble's kinds and refusals; the batch's one launch draws problem
+ *                       b with key seed + b (so problem b of a batch draws what a single planner with seed + b draws)
+ *                       and the iteration counter of problem 0 (the problems iterate together)
+ *   set_state_covariance  problem `problem`'s covariance: mjpc_b200_planner_set_state_covariance */
 typedef struct mjpc_b200_batch_planner mjpc_b200_batch_planner_t;
 void mjpc_b200_batch_planner_destroy(mjpc_b200_batch_planner_t* p);
 int mjpc_b200_batch_planner_reset(mjpc_b200_batch_planner_t* p, int problem, int horizon,
@@ -756,6 +826,8 @@ int mjpc_b200_batch_planner_action_from_policy(mjpc_b200_batch_planner_t* p, int
                                                const double* state, double time, int use_previous);
 int mjpc_b200_batch_planner_set_fd(mjpc_b200_batch_planner_t* p, double tolerance, int mode, int derivative_skip);
 int mjpc_b200_batch_planner_set_ensemble(mjpc_b200_batch_planner_t* p, const mjpc_model_blob* models, int K, int worst);
+int mjpc_b200_batch_planner_set_state_ensemble(mjpc_b200_batch_planner_t* p, int K, int worst, uint32_t seed);
+int mjpc_b200_batch_planner_set_state_covariance(mjpc_b200_batch_planner_t* p, int problem, const double* covariance);
 
 /* Predictive Sampling: one mjpc_b200_rollout_spline_batched launch of B x N per iteration. */
 int mjpc_b200_batch_sampling_planner_create(const mjpc_model_blob* model, int num_problems, int num_trajectory,

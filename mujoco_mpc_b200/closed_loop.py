@@ -9,7 +9,8 @@ Per physics step i, for every episode b, in the reference's order:
   5. planner.optimize_policy() when i % steps_per_planning_iteration == 0, from the states set in 2.
 With an estimator (a CppBatchEstimator of B filters on the plants' sensor range), every plant step is followed by one
 filter update from the ctrl the plant applied (the commanded ctrl plus any control noise: the app's estimator reads the
-noisy d->ctrl, app.cc:174), the plant's pre-step sensors and its mocap (app.cc:155-197).  A perturbation (a function of
+noisy d->ctrl, app.cc:174), the plant's pre-step sensors (with the plant's measurement noise, set_sensor_noise) and its
+mocap (app.cc:155-197); a planner with a state ensemble (set_state_ensemble) also gets the filter's covariance in 2.  A perturbation (a function of
 the step index and the plants' times) may hold a wrench on every plant before a step, as the app applies the user's
 force perturbation before each physics step (app.cc:323-326, 349-352)."""
 from __future__ import annotations
@@ -67,6 +68,8 @@ def synchronous_planning_cost(planner, plant, steps, steps_per_planning_iteratio
             state = x[b] if estimator is None else estimator.state(b)
             state = np.asarray(state, float)
             planner.set_state(b, state, t[b], np.asarray(plant.mocap[b], float))
+            if estimator is not None and getattr(planner, "state_members", 0):
+                planner.set_state_covariance(b, estimator.covariance(b))
             if status[b] == PLANT_RUNNING:
                 ctrl[b] = planner.action_from_policy(b, t[b], state) if reads_state else \
                     planner.action_from_policy(b, t[b])

@@ -15,6 +15,7 @@
 #include <vector>
 
 #include "../../include/mjpc_b200.h"
+#include "belief_kernels.cuh"
 #include "estimator_kernels.cuh"
 #include "filter_bank.h"
 #include "ilqg_kernels.cuh"
@@ -173,6 +174,13 @@ struct mjpc_b200 {
   int nmembers = 0, member_stride = 0, worst = 0, traj_factor = 1;
   // the members of the resident and of the last launch (0: not an ensemble launch), and the last launch's N per problem
   int resident_members = 0, last_members = 0, last_nper = 0;
+  // initial-state ensembles (rollout_spline_belief_batched): the covariances of the launch [cov_problems][n][n], the
+  // joint table [3][njnt] (type, qposadr, dofadr), and d_belief [33 max_candidates]: each launch row's variant (up to
+  // 32 rows per problem), then each problem's factorisation status
+  double* d_cov = nullptr;
+  int cov_problems = 0;
+  int* d_jnt = nullptr;
+  int* d_belief = nullptr;
   // resident-input launch description
   RolloutArgs resident;
   bool resident_ok = false;
@@ -527,9 +535,10 @@ int reserve_feedback(mjpc_b200* h, int B) {
 }
 
 // The rollout launch A, then the ranking of its candidates.  K > 0: A holds B x K x N trajectories of a model ensemble
-// (stage_problems with R = K) and writes the member returns; ensemble_score_kernel scores the B x N candidates into
-// d_returns / d_failure, which are ranked.
-int launch_rollout(mjpc_b200* h, const RolloutArgs& A_in, int K = 0) {
+// or an initial-state ensemble (stage_problems with R = K) and writes the member returns; ensemble_score_kernel scores
+// the B x N candidates with the mean of the `worst` largest (worst < 1: the model ensemble's) into d_returns /
+// d_failure, which are ranked.
+int launch_rollout(mjpc_b200* h, const RolloutArgs& A_in, int K = 0, int worst = 0) {
   RolloutArgs A = A_in;
   const size_t smem = h->smem_bytes(A.P);
   CUDA_TRY(cudaEventRecord(h->ev0, h->stream));
@@ -548,8 +557,8 @@ int launch_rollout(mjpc_b200* h, const RolloutArgs& A_in, int K = 0) {
   launch_kernel(plain ? k->rollout_plain : k->rollout, A.N, plain ? 32 : k->rollout_threads, smem, h->stream, A);
   if (K) {
     const int B = A.nprob / K, n = B * A.nper;
-    ensemble_score_kernel<<<(n + 7) / 8, 256, 0, h->stream>>>(A.returns, A.failure, B, K, A.nper, h->worst,
-                                                              h->d_returns, h->d_failure);
+    ensemble_score_kernel<<<(n + 7) / 8, 256, 0, h->stream>>>(A.returns, A.failure, B, K, A.nper,
+                                                              worst > 0 ? worst : h->worst, h->d_returns, h->d_failure);
     rank_kernel<<<(n + 255) / 256, 256, 0, h->stream>>>(h->d_returns, A.nper, B, h->d_order);
   } else {
     rank_kernel<<<(A.N + 255) / 256, 256, 0, h->stream>>>(A.returns, A.nper, A.nprob, h->d_order);
@@ -776,7 +785,7 @@ void mjpc_b200_destroy(mjpc_b200_t* h) {
                   h->d_tnom, h->d_gains, h->d_du, h->d_steps, h->d_states, h->d_actions, h->d_times, h->d_residual,
                   h->d_costs, h->d_trace, h->d_returns, h->d_failure, h->d_order, h->d_stats, h->d_pair_sync,
                   h->d_sensors, h->d_step, h->d_variants, h->d_variant_index, h->d_members, h->d_member_index,
-                  h->d_member_returns, h->d_member_failure};
+                  h->d_member_returns, h->d_member_failure, h->d_cov, h->d_jnt, h->d_belief};
   for (void* p : bufs) if (p) cudaFree(p);
   ilqg_free(h->ilqg);
   delete h->bank;
@@ -1084,6 +1093,153 @@ int mjpc_b200_rollout_spline_batched(mjpc_b200_t* h, int B, const float* states,
   rc = launch_rollout(h, h->resident, h->resident_members);
   if (rc) return rc;
   return read_back(h, B * N, returns, failure, order);
+}
+
+// The buffers of a belief launch of B problems x K members: the per-trajectory buffers for K x max_candidates
+// trajectories and the member returns (set_model_ensemble's reserve_members), and the launch's own tables, grown to B
+// problems (never shrunk): covariances, the joint table (once), and the per-row variant index and per-problem status.
+// On an allocation failure the handle keeps what it had.
+static int reserve_belief(mjpc_b200_t* h, int B, int K) {
+  const DevModel& M = h->pack.M;
+  const size_t n = 2 * (size_t)M.nv;
+  if (int rc = reserve_members(h, K)) return rc;
+  if (!h->d_jnt) {
+    std::vector<int> jnt(3 * (size_t)std::max(M.njnt, 1), 0);
+    for (int j = 0; j < M.njnt; j++) {
+      jnt[j] = h->pack.i[M.io[I_jnt_type] + j];
+      jnt[M.njnt + j] = h->pack.i[M.io[I_jnt_qposadr] + j];
+      jnt[2 * M.njnt + j] = h->pack.i[M.io[I_jnt_dofadr] + j];
+    }
+    int* dj = nullptr;
+    int* db = nullptr;
+    cudaError_t e = dalloc(&dj, jnt.size());
+    if (e == cudaSuccess) e = dalloc(&db, 33 * (size_t)h->maxN);
+    if (e == cudaSuccess) e = cudaMemcpy(dj, jnt.data(), jnt.size() * 4, cudaMemcpyHostToDevice);
+    if (e != cudaSuccess) {
+      cudaGetLastError();
+      if (dj) cudaFree(dj);
+      if (db) cudaFree(db);
+      return fail(MJPC_B200_ERR_CUDA, std::string("rollout_spline_belief_batched: ") + cudaGetErrorString(e));
+    }
+    h->d_jnt = dj; h->d_belief = db;
+  }
+  if (B > h->cov_problems) {
+    double* dc = nullptr;
+    if (cudaError_t e = dalloc(&dc, (size_t)B * n * n)) {
+      cudaGetLastError();
+      return fail(MJPC_B200_ERR_CUDA, std::string("rollout_spline_belief_batched: ") + cudaGetErrorString(e));
+    }
+    CUDA_TRY(cudaStreamSynchronize(h->stream));   // a launch in flight may still read the old covariances
+    if (h->d_cov) cudaFree(h->d_cov);
+    h->d_cov = dc; h->cov_problems = B;
+  }
+  return 0;
+}
+
+// An initial-state ensemble launch: problem b is staged K times (stage_problems with R = K), state_sample_kernel
+// overwrites rows b K + 1 .. b K + K - 1 with member states drawn from covariances[b], the rollout runs the B K N
+// trajectories on the handle's instance (each row on its problem's variant, when variants are set), and
+// ensemble_score_kernel scores them with `worst`.  Every refusal comes before anything is staged.
+int mjpc_b200_rollout_spline_belief_batched(mjpc_b200_t* h, int B, int K, int worst, uint32_t seed, uint32_t iteration,
+                                            const float* states, const double* covariances, const double* times,
+                                            const float* mocaps, const double* weights, const double* parameters,
+                                            const double* task_states, const float* knots, const double* knot_times,
+                                            int interp, int P, int N, int H, float* returns, uint8_t* failure,
+                                            int* order) {
+  static const char* call = "rollout_spline_belief_batched";
+  if (!h || !states || !covariances || !times || !knots || !knot_times)
+    return fail(MJPC_B200_ERR_BAD_ARGUMENT, std::string(call) + ": null pointer");
+  const DevModel& M = h->pack.M;
+  if (M.nmocap && !mocaps) return fail(MJPC_B200_ERR_BAD_ARGUMENT, std::string(call) + ": mocap required");
+  if (K < 1 || K > 32) return fail(MJPC_B200_ERR_BAD_ARGUMENT, std::string(call) + ": K must be in [1, 32]");
+  if (worst < 1 || worst > K) return fail(MJPC_B200_ERR_BAD_ARGUMENT, std::string(call) + ": worst must be in [1, K]");
+  if (B < 1 || N < 1 || H < 1 || P < 1 || interp < 0 || interp > 2)
+    return fail(MJPC_B200_ERR_BAD_ARGUMENT, std::string(call) + ": bad sizes");
+  if ((int64_t)B * N > h->maxN || H > h->maxH || P > h->maxP)
+    return fail(MJPC_B200_ERR_CAPACITY, std::string(call) + ": B*N/H/P above capacity");
+  if (h->nmembers)
+    return fail(MJPC_B200_ERR_UNSUPPORTED, std::string(call) + ": not available while a model ensemble is set "
+                                                               "(set_model_ensemble)");
+  if (h->xfrc_std > 0.f || !h->noise_seeds.empty())
+    return fail(MJPC_B200_ERR_UNSUPPORTED, std::string(call) + ": not available with force noise (set_xfrc_noise)");
+  if (int rc = check_variants(h, B, call)) return rc;
+  const size_t n = 2 * (size_t)M.nv, nn = n * n;
+  for (int b = 0; b < B; b++)
+    for (size_t e = 0; e < nn; e++)
+      if (!std::isfinite(covariances[(size_t)b * nn + e]))
+        return fail(MJPC_B200_ERR_BAD_ARGUMENT, std::string(call) + ": problem " + std::to_string(b) +
+                                                    ": non-finite covariance entry " + std::to_string(e));
+  const size_t smem = belief_smem((int)n, M.nq, M.nv);
+  if (smem > h->smem_optin)
+    return fail(MJPC_B200_ERR_CAPACITY, std::string(call) + ": the covariance does not fit in shared memory");
+  CUDA_TRY(cudaSetDevice(h->device));
+  if (int rc = reserve_belief(h, B, K)) return rc;
+  RolloutArgs A = base_args(h, B * K * N, H);
+  size_t end;
+  if (int rc = stage_problems(h, B, states, times, mocaps, weights, parameters, task_states, knot_times, P, H, knots, N,
+                              &A, &end, K))
+    return rc;
+  h->resident_ok = false;   // d_in now holds this launch, which is not a resident one
+  CUDA_TRY(cudaMemcpyAsync(h->d_cov, covariances, (size_t)B * nn * 8, cudaMemcpyHostToDevice, h->stream));
+  BeliefArgs S;
+  S.B = B; S.K = K; S.n = (int)n; S.nq = M.nq; S.nv = M.nv; S.njnt = M.njnt;
+  S.jnt = h->d_jnt; S.cov = h->d_cov; S.seed = seed; S.iteration = iteration;
+  S.rows = const_cast<float*>(A.state);
+  S.variant_index = h->nvariants ? h->d_variant_index : nullptr;
+  S.row_index = h->d_belief; S.status = h->d_belief + 32 * (size_t)h->maxN;
+  if (smem > 48 * 1024)
+    CUDA_TRY(cudaFuncSetAttribute((const void*)state_sample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  state_sample_kernel<<<B, kBeliefThreads, smem, h->stream>>>(S);
+  CUDA_TRY(cudaGetLastError());
+  std::vector<int> status(B);
+  CUDA_TRY(cudaMemcpyAsync(status.data(), S.status, (size_t)B * 4, cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(cudaStreamSynchronize(h->stream));
+  for (int b = 0; b < B; b++)
+    if (status[b])
+      return fail(MJPC_B200_ERR_BAD_ARGUMENT, std::string(call) + ": problem " + std::to_string(b) +
+                                                  ": the covariance is not positive semi-definite (a pivot <= 0)");
+  if (h->nvariants) A.pack_index = h->d_belief;
+  A.returns = h->d_member_returns; A.failure = h->d_member_failure;
+  A.L = make_layout(M, P);
+  A.P = P; A.interp = interp; A.policy_kind = 0;
+  if (int rc = launch_rollout(h, A, K, worst)) return rc;
+  return read_back(h, B * N, returns, failure, order);
+}
+
+int mjpc_b200_host_state_member(const mjpc_model_blob* model, const double* state, const double* covariance,
+                                uint32_t seed, uint32_t iteration, int problem, int member, double* out) {
+  if (!model || !model->data || !state || !covariance || !out || problem < 0 || member < 0 || member > 31)
+    return fail(MJPC_B200_ERR_BAD_ARGUMENT, "host_state_member: bad argument");
+  std::vector<int> type, qadr, dadr;
+  int nq = 0, nv = 0;
+  try {
+    Blob b(model->data, model->nbytes);
+    nq = b.i("nq"); nv = b.i("nv");
+    type = b.ints("jnt_type"); qadr = b.ints("jnt_qposadr"); dadr = b.ints("jnt_dofadr");
+  } catch (const std::exception& e) {
+    return fail(MJPC_B200_ERR_BAD_BLOB, std::string("host_state_member: ") + e.what());
+  }
+  const int n = 2 * nv;
+  std::copy(state, state + nq + nv, out);
+  for (int e = 0; e < n * n; e++)
+    if (!std::isfinite(covariance[e]))
+      return fail(MJPC_B200_ERR_BAD_ARGUMENT, "host_state_member: non-finite covariance entry " + std::to_string(e));
+  std::vector<double> L((size_t)n * n, 0.0), z(n), dx(n);
+  for (int i = 0; i < n; i++)
+    for (int c = 0; c <= i; c++) L[(size_t)i * n + c] = 0.5 * (covariance[i * n + c] + covariance[c * n + i]);
+  for (int j = 0; j < n; j++) {   // state_sample_kernel's order
+    if (!belief_pivot(L.data(), n, j))
+      return fail(MJPC_B200_ERR_BAD_ARGUMENT, "host_state_member: the covariance is not positive semi-definite");
+    for (int i = j + 1; i < n; i++) belief_column(L.data(), n, j, i);
+    for (int i = j + 1; i < n; i++)
+      for (int c = j + 1; c <= i; c++) belief_update(L.data(), n, j, i, c);
+  }
+  if (member == 0) return 0;
+  for (int e = 0; e < n; e++) z[e] = belief_normal(seed, iteration, problem, member, e);
+  for (int i = 0; i < n; i++) dx[i] = belief_row(L.data(), z.data(), n, i);
+  for (size_t j = 0; j < type.size(); j++) belief_joint(out + qadr[j], dx.data() + dadr[j], type[j]);
+  for (int i = 0; i < nv; i++) out[nq + i] = belief_add(out[nq + i], dx[nv + i]);
+  return 0;
 }
 
 int mjpc_b200_launch_resident(mjpc_b200_t* h) {
@@ -1600,7 +1756,7 @@ int mjpc_b200_plant_init(mjpc_b200_t* h, int num_plants, int sensor_start, int n
   const size_t o_qpos = take(B * nq * 4), o_qvel = take(B * nv * 4), o_warm = take(B * nv * 4), o_time = take(B * 8),
                o_sum = take(B * 8), o_steps = take(B * 4), o_warn = take(B * 4), o_status = take(B * 4),
                o_dist = take(B * sizeof(PlantDisturbance)), o_cnoise = take(B * nu * 4), o_xnoise = take(B * nx * 4),
-               o_held = take(B * nx * 4), o_next = take(B * (nu + nx) * 4);
+               o_held = take(B * nx * 4), o_next = take(B * (nu + nx) * 4), o_sstd = take(B * nsd * 4);
   // the upload and the outputs, each one contiguous block laid out as its pinned mirror
   size_t in = 0, out = 0;
   auto in_take = [&](size_t n) { const size_t at = in; in += (n + 15) & ~(size_t)15; return at; };
@@ -1625,6 +1781,7 @@ int mjpc_b200_plant_init(mjpc_b200_t* h, int num_plants, int sensor_start, int n
   a.steps = (int*)(base + o_steps); a.warnings = (int*)(base + o_warn); a.status = (int*)(base + o_status);
   a.dist = (const PlantDisturbance*)(base + o_dist); a.ctrl_noise = (float*)(base + o_cnoise);
   a.xfrc_noise = (float*)(base + o_xnoise); a.xfrc_held = (const float*)(base + o_held); a.noise_next = (float*)(base + o_next);
+  a.sensor_std = (const float*)(base + o_sstd);
   k->d_in = base + o_in; k->d_out = base + o_out;
   a.ctrl = (const float*)(k->d_in + k->o_ctrl); a.mocap = (const float*)(k->d_in + k->o_mocap);
   a.task_state = nts ? (const float*)(k->d_in + k->o_ts) : nullptr;
@@ -1814,6 +1971,31 @@ int mjpc_b200_plant_set_xfrc(mjpc_b200_t* h, int plant, const float* xfrc) {
   CUDA_TRY(cudaSetDevice(h->device));
   CUDA_TRY(cudaStreamSynchronize(h->stream));
   CUDA_TRY(cudaMemcpy((float*)k.a.xfrc_held + plant * nx, w.data(), nx * 4, cudaMemcpyHostToDevice));
+  CUDA_TRY(cudaMemcpy((PlantDisturbance*)k.a.dist + plant, &d, sizeof(d), cudaMemcpyHostToDevice));
+  k.dist[plant] = d;
+  return 0;
+}
+
+// Measurement noise: the std row of plant `plant` in the bank, and its sens flag on when any entry is > 0, so that a
+// plant without sensor noise steps exactly as before
+int mjpc_b200_plant_set_sensor_noise(mjpc_b200_t* h, int plant, const float* std_) {
+  if (int rc = plant_check(h, plant, "plant_set_sensor_noise")) return rc;
+  PlantBank& k = *h->plants;
+  const size_t nsd = k.nsd;
+  std::vector<float> w(nsd, 0.f);
+  if (std_) w.assign(std_, std_ + nsd);
+  int on = 0;
+  for (size_t e = 0; e < nsd; e++) {
+    if (!std::isfinite(w[e]) || w[e] < 0.f)
+      return fail(MJPC_B200_ERR_BAD_ARGUMENT, "plant_set_sensor_noise: std[" + std::to_string(e) +
+                                                  "] must be finite and >= 0");
+    on |= w[e] > 0.f;
+  }
+  PlantDisturbance d = k.dist[plant];
+  d.sens = on;
+  CUDA_TRY(cudaSetDevice(h->device));
+  CUDA_TRY(cudaStreamSynchronize(h->stream));
+  if (nsd) CUDA_TRY(cudaMemcpy((float*)k.a.sensor_std + plant * nsd, w.data(), nsd * 4, cudaMemcpyHostToDevice));
   CUDA_TRY(cudaMemcpy((PlantDisturbance*)k.a.dist + plant, &d, sizeof(d), cudaMemcpyHostToDevice));
   k.dist[plant] = d;
   return 0;

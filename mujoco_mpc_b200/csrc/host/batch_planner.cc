@@ -47,6 +47,12 @@ int BatchPlanner::SetModels(const mjpc_model_blob* models, int count) {
   return 0;
 }
 
+int BatchPlanner::SetStateEnsemble(int K, int worst, uint32_t seed) {
+  for (int b = 0; b < NumProblems(); b++)
+    if (int rc = problem(b).SetStateEnsemble(K, worst, seed)) return rc;
+  return 0;
+}
+
 TaskRows BatchPlanner::Rows() const {
   TaskRows r;
   r.w = weight_.data(); r.p = parameters_.data(); r.ts = task_state_.data(); r.nw = nw_; r.np = np_; r.nts = nts_;
@@ -286,6 +292,14 @@ int mjpc_b200_batch_planner_set_ensemble(mjpc_b200_batch_planner_t* h, const mjp
                                          int worst) {
   BatchPlanner* bp = problem_of<BatchPlanner>(h, 0);
   return bp ? bp->SetEnsemble(models, K, worst) : MJPC_B200_ERR_BAD_ARGUMENT;
+}
+int mjpc_b200_batch_planner_set_state_ensemble(mjpc_b200_batch_planner_t* h, int K, int worst, uint32_t seed) {
+  BatchPlanner* bp = problem_of<BatchPlanner>(h, 0);
+  return bp ? bp->SetStateEnsemble(K, worst, seed) : MJPC_B200_ERR_BAD_ARGUMENT;
+}
+int mjpc_b200_batch_planner_set_state_covariance(mjpc_b200_batch_planner_t* h, int problem, const double* covariance) {
+  BatchPlanner* bp = problem_of<BatchPlanner>(h, problem);
+  return bp ? bp->SetStateCovariance(problem, covariance) : MJPC_B200_ERR_BAD_ARGUMENT;
 }
 int mjpc_b200_batch_planner_optimize_policy(mjpc_b200_batch_planner_t* h, int horizon, int* codes) {
   BatchPlanner* bp = problem_of<BatchPlanner>(h, 0);

@@ -40,6 +40,10 @@ class BatchPlanner {
   int SetModels(const mjpc_model_blob* models, int count);
   // every problem plans on one model ensemble: Planner::SetEnsemble of the problems, which share the batch's handle
   int SetEnsemble(const mjpc_model_blob* models, int K, int worst) { return problem(0).SetEnsemble(models, K, worst); }
+  // every problem plans over its own state covariance with the same K, worst and seed (Planner::SetStateEnsemble of
+  // each problem; problem 0 first, so a refusal changes nothing); the launch draws problem b with key seed + b
+  int SetStateEnsemble(int K, int worst, uint32_t seed);
+  int SetStateCovariance(int b, const double* covariance) { return problem(b).SetStateCovariance(covariance); }
 
  protected:
   // the task snapshots of num_problems problems, each the model's, and the engine handle of max_candidates (all

@@ -34,9 +34,10 @@ class CrossEntropyPlanner : public Planner {
   // :331-340; the policy does not depend on the state
   void ActionFromPolicy(double* action, const double* state, double time, bool use_previous = false) override;
   const Trajectory* BestTrajectory() override;        // the NOMINAL trajectory (:462-464)
-  int SetEnsemble(const mjpc_model_blob* models, int K, int worst) override {
-    return mjpc_b200_set_model_ensemble(gpu_, models, K, worst);
-  }
+  int SetEnsemble(const mjpc_model_blob* models, int K, int worst) override { return ModelEnsemble(models, K, worst); }
+  int SetStateEnsemble(int K, int worst, uint32_t seed) override { return StateEnsemble(K, worst, seed); }
+  int SetStateCovariance(const double* covariance) override { return StateCovariance(covariance); }
+  uint32_t PlanIteration() const override { return (uint32_t)iteration; }
 
   SamplingPolicy policy, resampled_policy, previous_policy;
   std::vector<SamplingPolicy> candidate_policy;

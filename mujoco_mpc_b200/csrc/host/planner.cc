@@ -72,6 +72,32 @@ int Planner::AttachEngine(const mjpc_model_blob* model, int max_candidates, int 
   else if (int rc = mjpc_b200_create(model, max_candidates, max_horizon, device, &gpu_)) return rc;
   mjpc_b200_get_info(gpu_, &info_);
   state_.assign(info_.dim_state, 0.0); mocap_.assign(7 * info_.nmocap, 0.0);
+  state_cov_.assign((size_t)info_.dim_dstate * info_.dim_dstate, 0.0);
+  return 0;
+}
+
+int Planner::ModelEnsemble(const mjpc_model_blob* models, int K, int worst) {
+  const bool set = K > 0 && models;
+  if (set && state_members_) return MJPC_B200_ERR_UNSUPPORTED;
+  if (int rc = mjpc_b200_set_model_ensemble(gpu_, models, K, worst)) return rc;
+  model_ensemble_ = set;
+  return 0;
+}
+
+int Planner::StateEnsemble(int K, int worst, uint32_t seed) {
+  if (K < 0 || K > 32) return MJPC_B200_ERR_BAD_ARGUMENT;
+  if (K == 0) { state_members_ = state_worst_ = 0; return 0; }
+  if (worst < 1 || worst > K) return MJPC_B200_ERR_BAD_ARGUMENT;
+  if (model_ensemble_) return MJPC_B200_ERR_UNSUPPORTED;
+  state_members_ = K; state_worst_ = worst; state_seed_ = seed;
+  return 0;
+}
+
+int Planner::StateCovariance(const double* covariance) {
+  if (!covariance) { std::fill(state_cov_.begin(), state_cov_.end(), 0.0); return 0; }
+  for (size_t e = 0; e < state_cov_.size(); e++)
+    if (!std::isfinite(covariance[e])) return MJPC_B200_ERR_BAD_ARGUMENT;
+  std::copy(covariance, covariance + state_cov_.size(), state_cov_.begin());
   return 0;
 }
 
@@ -98,6 +124,18 @@ int SplineLaunch::Run(const std::vector<const Planner*>& from, const std::vector
     times_[b] = from[b]->time();
   }
   returns.resize(B * N); failure.resize(B * N); order.resize(B * N);
+  const Planner& p0 = *from[0];
+  if (p0.state_members()) {   // problem b's members from planner b's covariance, the draws on problem 0's counter
+    const size_t nn = p0.state_covariance().size();
+    covariances_.resize(B * nn);
+    for (size_t b = 0; b < B; b++)
+      std::copy(from[b]->state_covariance().begin(), from[b]->state_covariance().end(), covariances_.begin() + b * nn);
+    return mjpc_b200_rollout_spline_belief_batched(
+        p0.gpu(), (int)B, p0.state_members(), p0.state_worst(), p0.state_seed(), p0.PlanIteration(), states_.data(),
+        covariances_.data(), times_.data(), nm ? mocaps_.data() : nullptr, rows.nw ? rows.w : nullptr,
+        rows.np ? rows.p : nullptr, rows.nts ? rows.ts : nullptr, knots_.data(), knot_times_.data(), interp, (int)P,
+        (int)N, horizon, returns.data(), failure.data(), order.data());
+  }
   return mjpc_b200_rollout_spline_batched(from[0]->gpu(), (int)B, states_.data(), times_.data(),
                                           nm ? mocaps_.data() : nullptr, rows.nw ? rows.w : nullptr,
                                           rows.np ? rows.p : nullptr, rows.nts ? rows.ts : nullptr, knots_.data(),
@@ -179,6 +217,14 @@ int mjpc_b200_planner_set_fd(mjpc_b200_planner_t* h, double tolerance, int mode,
 int mjpc_b200_planner_set_ensemble(mjpc_b200_planner_t* h, const mjpc_model_blob* models, int K, int worst) {
   Planner* p = PlannerOf<Planner>(h);
   return p ? p->SetEnsemble(models, K, worst) : MJPC_B200_ERR_BAD_ARGUMENT;
+}
+int mjpc_b200_planner_set_state_ensemble(mjpc_b200_planner_t* h, int K, int worst, uint32_t seed) {
+  Planner* p = PlannerOf<Planner>(h);
+  return p ? p->SetStateEnsemble(K, worst, seed) : MJPC_B200_ERR_BAD_ARGUMENT;
+}
+int mjpc_b200_planner_set_state_covariance(mjpc_b200_planner_t* h, const double* covariance) {
+  Planner* p = PlannerOf<Planner>(h);
+  return p ? p->SetStateCovariance(covariance) : MJPC_B200_ERR_BAD_ARGUMENT;
 }
 int mjpc_b200_planner_set_task(mjpc_b200_planner_t* h, const mjpc_task_desc* task) {
   Planner* p = PlannerOf<Planner>(h);

@@ -48,7 +48,7 @@ class SplineLaunch {
 
  private:
   std::vector<float> states_, mocaps_, knots_;
-  std::vector<double> times_, knot_times_;
+  std::vector<double> times_, knot_times_, covariances_;
 };
 
 // mju_cholFactor: in-place lower Cholesky factor of the row-major n x n matrix M (upper triangle left as it was); a
@@ -91,6 +91,17 @@ class Planner {
   // plan on a model ensemble (mjpc_b200_set_model_ensemble on the planner's handle): the planners whose iteration ranks
   // by SplineLaunch's returns, which are then the scores; the others: MJPC_B200_ERR_UNSUPPORTED
   virtual int SetEnsemble(const mjpc_model_blob* models, int K, int worst) { return MJPC_B200_ERR_UNSUPPORTED; }
+  // plan over the state covariance (mjpc_b200_planner_set_state_ensemble / _set_state_covariance): SplineLaunch then
+  // runs mjpc_b200_rollout_spline_belief_batched; the planners whose iteration ranks by its returns, the others:
+  // MJPC_B200_ERR_UNSUPPORTED
+  virtual int SetStateEnsemble(int K, int worst, uint32_t seed) { return MJPC_B200_ERR_UNSUPPORTED; }
+  virtual int SetStateCovariance(const double* covariance) { return MJPC_B200_ERR_UNSUPPORTED; }
+  // the counter of the planner's iterations, which its state-ensemble draws take (0 for the kinds without them)
+  virtual uint32_t PlanIteration() const { return 0; }
+  int state_members() const { return state_members_; }
+  int state_worst() const { return state_worst_; }
+  uint32_t state_seed() const { return state_seed_; }
+  const std::vector<double>& state_covariance() const { return state_cov_; }
   // every engine handle the planner plans on: Agent applies the planning-model options and the task snapshot to each
   virtual std::vector<mjpc_b200_t*> Handles() { return {gpu_}; }
   mjpc_b200_t* gpu() const { return gpu_; }
@@ -106,6 +117,11 @@ class Planner {
   // sizes *out to `horizon` rows and fetches trajectory `candidate` of the handle's last launch into it (flat index
   // launch_offset_ + candidate); total_return and failure are the caller's
   int FetchTrajectory(int candidate, int horizon, Trajectory* out);
+  // SetEnsemble / SetStateEnsemble / SetStateCovariance of the kinds that support them: a model ensemble and a state
+  // ensemble exclude each other (MJPC_B200_ERR_UNSUPPORTED)
+  int ModelEnsemble(const mjpc_model_blob* models, int K, int worst);
+  int StateEnsemble(int K, int worst, uint32_t seed);
+  int StateCovariance(const double* covariance);
 
   mjpc_b200_t* gpu_ = nullptr;
   bool owns_gpu_ = false;
@@ -115,6 +131,10 @@ class Planner {
   int horizon_ = 0;                                   // of the last spline launch: the rows a fetch fills
   int launch_offset_ = 0;                             // flat index of this planner's candidate 0 in that launch
   SplineLaunch launch_;                               // of the spline launches the planner makes when it plans alone
+  bool model_ensemble_ = false;                       // SetEnsemble set one
+  int state_members_ = 0, state_worst_ = 0;           // SetStateEnsemble (0: none)
+  uint32_t state_seed_ = 0;
+  std::vector<double> state_cov_;                     // [2 nv][2 nv], zero until SetStateCovariance
 };
 
 // SetFD for a settings struct with fd_tolerance, fd_mode and derivative_skip: tolerance <= 0, mode < 0 and

@@ -42,9 +42,10 @@ class SampleGradientPlanner : public Planner {
   void AddNoiseToPolicy(int i);                                     // :329-355
   void GradientCandidates(int num_trajectory, int num_gradient);    // :401-493
   const Trajectory* BestTrajectory() override;                      // trajectory[winner] (:496-498)
-  int SetEnsemble(const mjpc_model_blob* models, int K, int worst) override {
-    return mjpc_b200_set_model_ensemble(gpu_, models, K, worst);
-  }
+  int SetEnsemble(const mjpc_model_blob* models, int K, int worst) override { return ModelEnsemble(models, K, worst); }
+  int SetStateEnsemble(int K, int worst, uint32_t seed) override { return StateEnsemble(K, worst, seed); }
+  int SetStateCovariance(const double* covariance) override { return StateCovariance(covariance); }
+  uint32_t PlanIteration() const override { return (uint32_t)iteration; }
 
   SamplingPolicy policy, resampled_policy, previous_policy;
   std::vector<SamplingPolicy> candidate_policy;

@@ -83,9 +83,10 @@ class SamplingPlanner : public Planner {
   void ActionFromPolicy(double* action, const double* state, double time, bool use_previous = false) override;
   void CopyCandidateToPolicy(int candidate);          // :534-543
   const Trajectory* BestTrajectory() override;
-  int SetEnsemble(const mjpc_model_blob* models, int K, int worst) override {
-    return mjpc_b200_set_model_ensemble(gpu_, models, K, worst);
-  }
+  int SetEnsemble(const mjpc_model_blob* models, int K, int worst) override { return ModelEnsemble(models, K, worst); }
+  int SetStateEnsemble(int K, int worst, uint32_t seed) override { return StateEnsemble(K, worst, seed); }
+  int SetStateCovariance(const double* covariance) override { return StateCovariance(covariance); }
+  uint32_t PlanIteration() const override { return (uint32_t)iteration; }
   int CandidateTrajectory(int candidate, int horizon, Trajectory* out);   // trajectory[candidate] of the last Rollouts
   void SetPolicy(const double* times, const double* parameters, int num_nodes);   // policy.plan = nodes (ilqs/planner.cc:160-172)
   double timestep() const { return timestep_; }

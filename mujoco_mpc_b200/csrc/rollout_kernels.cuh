@@ -172,7 +172,8 @@ __device__ __forceinline__ void write_traces(Ctx& c, float* out) {
 
 // A standard normal from Philox4x32-10 with key (k0, k1) on counter (c0, c1, c2, c3), Box-Muller on the first two
 // output words.  Key word 1 names the stream's owner: 0 the knots (host), 1 the rollouts' force noise, 2 the plants'
-// disturbances, so no two of them ever draw the same numbers.
+// disturbances and measurement noise, 3 the initial-state ensembles (belief_kernels.cuh), so no two of them ever draw
+// the same numbers.
 __device__ __forceinline__ float philox_normal(unsigned c0, unsigned c1, unsigned c2, unsigned c3, unsigned k0,
                                                unsigned k1) {
 #pragma unroll
@@ -607,18 +608,20 @@ extern "C" __global__ void __launch_bounds__(32) step_batch_kernel_humanoid_trac
 // or the commanded ctrl when it is not running.  The disturbances' OU states advance only with a committed step.
 enum PlantStatus { PLANT_RUNNING = 0, PLANT_DIVERGED = 1, PLANT_IDLE = 2 };
 
-// A plant's disturbances (mjpc_b200_plant_set_disturbance / _set_xfrc): Ornstein-Uhlenbeck control noise and body-force
-// noise (std 0: off; the rate is the time constant in seconds), the key of its noise stream and whether it holds a
-// non-zero wrench
+// A plant's disturbances (mjpc_b200_plant_set_disturbance / _set_xfrc / _set_sensor_noise): Ornstein-Uhlenbeck control
+// noise and body-force noise (std 0: off; the rate is the time constant in seconds), the key of its noise stream,
+// whether it holds a non-zero wrench and whether any of its sensor-noise stds is > 0
 struct PlantDisturbance {
   float ctrl_std, ctrl_rate, xfrc_std, xfrc_rate;
   unsigned seed;
   int held;
+  int sens;
 };
 
 // Plant noise: Philox key (seed, 2), counter (committed step count, 0, element, tag)
 constexpr unsigned kPlantTagCtrl = 0x4354524Cu;   // 'CTRL'
 constexpr unsigned kPlantTagXfrc = 0x58465243u;   // 'XFRC'
+constexpr unsigned kPlantTagSens = 0x53454E53u;   // 'SENS'
 __device__ __forceinline__ float plant_normal(unsigned seed, unsigned step, unsigned element, unsigned tag) {
   return philox_normal(step, 0u, element, tag, seed, 2u);
 }
@@ -646,6 +649,7 @@ struct PlantArgs {
   // xfrc_held [B][6 nbody]; noise_next [B][nu + 6 nbody], this step's OU states until the step is committed
   const PlantDisturbance* dist; float* ctrl_noise; float* xfrc_noise; const float* xfrc_held; float* noise_next;
   float* ctrl_out;   // output: the applied ctrl [B][nu] (commanded + control noise)
+  const float* sensor_std;   // measurement noise std [B][sensor_dim] (read only for a plant whose dist.sens is set)
 };
 
 // The disturbances of plant b's coming step, between load_state and k_forward (app.cc:291-304, 95-101, 323-352):
@@ -694,6 +698,17 @@ __device__ __forceinline__ void plant_commit_noise(const PlantArgs& A, int b, in
     for (int i = lane; i < nu; i += 32) A.ctrl_noise[(size_t)b * nu + i] = next[i];
   if (d.xfrc_std > 0.f)
     for (int i = lane; i < nx; i += 32) A.xfrc_noise[(size_t)b * nx + i] = next[nu + i];
+}
+
+// The measurement noise of plant b's committed step, after the step is committed: sensordata[e] += std[e] z on counter
+// (the committed step count before this step, 0, e, 'SENS').  Elements whose std is 0 are not touched.  Only the
+// returned measurement changes.
+__device__ __forceinline__ void plant_sensor_noise(const PlantArgs& A, int b, int lane) {
+  const unsigned seed = A.dist[b].seed, step = (unsigned)A.steps[b] - 1u;
+  const float* sd = A.sensor_std + (size_t)b * A.sensor_dim;
+  float* out = A.sensordata + (size_t)b * A.sensor_dim;
+  for (int e = lane; e < A.sensor_dim; e += 32)
+    if (sd[e] > 0.f) out[e] += sd[e] * plant_normal(seed, step, (unsigned)e, kPlantTagSens);
 }
 
 template <class SP>
@@ -752,6 +767,8 @@ __device__ __forceinline__ void plant_body(const PlantArgs& A) {
     A.state_out[(size_t)b * ds + i] = i < nq ? A.qpos[(size_t)b * nq + i] : A.qvel[(size_t)b * A.M.nv + i - nq];
   if (A.sensordata && !stepped)
     for (int i = lane; i < A.sensor_dim; i += 32) A.sensordata[(size_t)b * A.sensor_dim + i] = 0.f;
+  // (the __syncwarp above made the committed step count and k_sensors' values visible to every lane)
+  if (stepped && A.dist[b].sens) plant_sensor_noise(A, b, lane);
   if (lane == 0) {
     A.time_out[b] = A.time[b];
     A.cost_out[b] = stepped ? cost : 0.f;

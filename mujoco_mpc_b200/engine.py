@@ -136,6 +136,21 @@ def host_ensemble_score(member_returns, member_failure, worst):
     return score[0], fail[0]
 
 
+def host_state_member(model, state, covariance, seed, iteration, problem, member):
+    """Member `member` of problem `problem` of a belief launch (Engine.rollout_spline_belief_batched) on the host, in
+    fp64 (mjpc_b200_host_state_member, no device): state (+) L z, L the Cholesky factor of (P + P') / 2.  The device's
+    member states are this rounded to float."""
+    lib = load_library()
+    buf, mb = _model_blob(model)
+    x, P = _d(state), _d(covariance)
+    out = np.zeros(model.nq + model.nv)
+    rc = lib.mjpc_b200_host_state_member(C.byref(mb), _pd(x), _pd(P), C.c_uint32(seed), C.c_uint32(iteration),
+                                         int(problem), int(member), _pd(out))
+    if rc != 0:
+        raise EngineError(f"host_state_member failed ({rc}): {lib.mjpc_b200_last_error().decode()}")
+    return out
+
+
 def _ensemble_args(models, worst):
     """(buffers, ModelBlob array, K, worst) of set_ensemble: worst None is K (the expected return)."""
     bufs, arr, n = _model_blobs(models)
@@ -240,6 +255,23 @@ class _CppPlanner(_CppObject):
         rc = self.lib.mjpc_b200_planner_set_ensemble(self.h, arr, K, worst)
         if rc:
             raise EngineError(f"{self._prefix}_set_ensemble failed ({rc}): {self.lib.mjpc_b200_last_error().decode()}")
+
+    def set_state_ensemble(self, K, worst=None, seed=0):
+        """Plan over the state covariance (mjpc_b200_planner_set_state_ensemble): every candidate is scored over K
+        initial states drawn from set_state_covariance's covariance, the mean of its `worst` largest member returns
+        (None: K).  Sampling, Cross-Entropy and Sample Gradient.  K = 0 clears it."""
+        K = int(K)
+        rc = self.lib.mjpc_b200_planner_set_state_ensemble(self.h, K, K if worst is None else int(worst), C.c_uint32(seed))
+        if rc:
+            raise EngineError(f"{self._prefix}_set_state_ensemble failed ({rc})")
+        self.state_members = K
+
+    def set_state_covariance(self, covariance):
+        """The state covariance [2 nv][2 nv] the state-ensemble launches draw from (None: zero)."""
+        P = _d(covariance)
+        rc = self.lib.mjpc_b200_planner_set_state_covariance(self.h, _pd(P))
+        if rc:
+            raise EngineError(f"{self._prefix}_set_state_covariance failed ({rc})")
 
     def set_task(self, weight=None, parameters=None, task_state=None, risk=None):
         """The task snapshot of every engine handle the planner plans on (mjpc_b200_planner_set_task)."""
@@ -390,6 +422,25 @@ class Engine:
                                                               _pf(knots), _pd(kt), int(interp), int(P), int(N), int(H),
                                                               _pf(ret), fail.ctypes.data_as(_bp), order.ctypes.data_as(_ip)))
         self.lastN, self.lastH, self.lastB, self.last_members = B * N, H, B, self.members
+        return ret, fail, order
+
+    def rollout_spline_belief_batched(self, states, covariances, times, mocaps, knots, knot_times, interp, H, K,
+                                      worst=None, seed=0, iteration=0, weights=None, parameters=None, task_states=None):
+        """rollout_spline_batched with every candidate scored over K initial states per problem
+        (mjpc_b200_rollout_spline_belief_batched): member 0 the state itself, member k states[b] (+) L_b z drawn from
+        covariances [B, 2 nv, 2 nv]; the score is the mean of the `worst` largest member returns (None: K).  Returns the
+        scores, failure and order [B, N]; fetch_ensemble / fetch_trajectory_member then give the members."""
+        knots = _f(knots)
+        B, N, P, nu = knots.shape
+        K = int(K)
+        st, P_, t, mc, kt = _f(states), _d(covariances), _d(times), _f(mocaps), _d(knot_times)
+        w, p, s = _d(weights), _d(parameters), _d(task_states)
+        ret = np.zeros((B, N), np.float32); fail = np.zeros((B, N), np.uint8); order = np.zeros((B, N), np.int32)
+        self._check(self.lib.mjpc_b200_rollout_spline_belief_batched(
+            self.h, int(B), K, K if worst is None else int(worst), C.c_uint32(seed), C.c_uint32(iteration), _pf(st),
+            _pd(P_), _pd(t), _pf(mc), _pd(w), _pd(p), _pd(s), _pf(knots), _pd(kt), int(interp), int(P), int(N), int(H),
+            _pf(ret), fail.ctypes.data_as(_bp), order.ctypes.data_as(_ip)))
+        self.lastN, self.lastH, self.lastB, self.last_members = B * N, H, B, K
         return ret, fail, order
 
     # ---- multi-GPU: one planning problem sharded over an NCCL communicator owned by the handle
@@ -777,6 +828,15 @@ class CppPlantBank:
         w = None if xfrc is None else np.ascontiguousarray(np.asarray(xfrc, np.float32).reshape(self.m.nbody * 6))
         self._check(self.lib.mjpc_b200_plant_set_xfrc(self.h, int(plant), _pf(w)))
 
+    def set_sensor_noise(self, plant, std=None):
+        """Measurement noise of plant `plant`: std [nsensordata] (a scalar is every element's; None clears it).  step()
+        then returns sensordata + std z, z white Gaussian noise of the plant's seed (set_disturbance) and step count; the
+        plant itself is unaffected."""
+        s = None
+        if std is not None:
+            s = np.ascontiguousarray(np.broadcast_to(np.asarray(std, np.float32), (self.nsensordata,)))
+        self._check(self.lib.mjpc_b200_plant_set_sensor_noise(self.h, int(plant), _pf(s)))
+
     def disturbance(self, plant):
         """dict(ctrl_noise [nu], xfrc_noise [nbody][6]): the plant's OU states after its last committed step."""
         m = self.m
@@ -1073,6 +1133,22 @@ class _CppBatchPlanner(_CppObject):
         rc = self.lib.mjpc_b200_batch_planner_set_ensemble(self.h, arr, K, worst)
         if rc != 0:
             raise EngineError(f"batch_planner_set_ensemble failed ({rc}): {self.lib.mjpc_b200_last_error().decode()}")
+
+    def set_state_ensemble(self, K, worst=None, seed=0):
+        """Every problem plans over its own state covariance with K members (mjpc_b200_batch_planner_set_state_ensemble;
+        problem b draws as a single planner with seed + b).  K = 0 clears it."""
+        K = int(K)
+        rc = self.lib.mjpc_b200_batch_planner_set_state_ensemble(self.h, K, K if worst is None else int(worst),
+                                                                 C.c_uint32(seed))
+        if rc:
+            raise EngineError(f"batch_planner_set_state_ensemble failed ({rc})")
+        self.state_members = K
+
+    def set_state_covariance(self, problem, covariance):
+        """Problem `problem`'s state covariance [2 nv][2 nv] (None: zero)."""
+        P = _d(covariance)
+        self._check(self.lib.mjpc_b200_batch_planner_set_state_covariance(self.h, int(problem), _pd(P)),
+                    "set_state_covariance")
 
     def set_fd(self, tolerance, mode=-1, derivative_skip=-1):
         self._check(self.lib.mjpc_b200_batch_planner_set_fd(self.h, C.c_double(tolerance), int(mode), int(derivative_skip)),
