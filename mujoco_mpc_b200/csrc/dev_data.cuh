@@ -374,13 +374,16 @@ __device__ __forceinline__ void axis_angle_quat(float* q, const float* axis, flo
   sincosf(angle * 0.5f, &s, &co);
   q[0] = co; q[1] = axis[0] * s; q[2] = axis[1] * s; q[3] = axis[2] * s;
 }
+// q <- q * exp(w*h/2).  As mju_quatIntegrate, the result is the normalised q (the identity for an all-zero q) times
+// the rotation, a unit quaternion also when w = 0.
 __device__ __forceinline__ void quat_integrate(float* q, const float* w, float h) {
   float ax[3] = {w[0], w[1], w[2]};
   float n = norm3(ax);
-  if (n < kMinVal) return;
+  if (n < kMinVal) { quat_normalize(q); return; }
   ax[0] /= n; ax[1] /= n; ax[2] /= n;
   float dq[4], r[4];
   axis_angle_quat(dq, ax, n * h);
+  if (sqrtf(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]) < kMinVal) { q[0] = 1; q[1] = q[2] = q[3] = 0; }
   quat_mul(r, q, dq);
   quat_normalize(r);
   q[0] = r[0]; q[1] = r[1]; q[2] = r[2]; q[3] = r[3];

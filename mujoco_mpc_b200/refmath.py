@@ -80,8 +80,8 @@ def body_jacobian(m, kin, b, point):
     return J
 
 
-def mass_matrix_and_jacobians(m, qpos):
-    kin = kinematics(m, qpos)
+def mass_matrix_and_jacobians(m, qpos, mocap_pos=None, mocap_quat=None):
+    kin = kinematics(m, qpos, mocap_pos, mocap_quat)
     M = np.diag(m.dof_armature.astype(float)) if m.nv else np.zeros((0, 0))
     Jb = {}
     for b in range(1, m.nbody):

@@ -96,14 +96,16 @@ template <class T> inline void axis_angle_quat(T* q, const T* axis, T angle) {
   T s = mm::sin(angle * (T)0.5);
   q[0] = mm::cos(angle * (T)0.5); q[1] = axis[0] * s; q[2] = axis[1] * s; q[3] = axis[2] * s;
 }
-// q <- q * exp(w*h/2): integrate body-frame angular velocity
+// q <- q * exp(w*h/2): integrate body-frame angular velocity.  As mju_quatIntegrate, the result is the normalised q
+// (the identity for an all-zero q) times the rotation, a unit quaternion also when w = 0.
 template <class T> inline void quat_integrate(T* q, const T* w, T h) {
   T ax[3] = {w[0], w[1], w[2]};
   T n = norm3(ax);
-  if (n < kMinVal<T>()) return;
+  if (n < kMinVal<T>()) { quat_normalize(q); return; }
   ax[0] /= n; ax[1] /= n; ax[2] /= n;
   T dq[4], r[4];
   axis_angle_quat(dq, ax, n * h);
+  if (mm::sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]) < kMinVal<T>()) { q[0] = 1; q[1] = q[2] = q[3] = 0; }
   quat_mul(r, q, dq);
   quat_normalize(r);
   q[0] = r[0]; q[1] = r[1]; q[2] = r[2]; q[3] = r[3];
