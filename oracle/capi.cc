@@ -180,6 +180,55 @@ int forward_debug(Engine<T>& e, const double* qpos, const double* qvel, const do
   return d.warning ? 1 : 0;
 }
 
+// one mj_forward at (qpos, qvel, ctrl), then the constraint problem the solver was given and its answer: the
+// independent restatement of the convex problem (tests/test_constraint_solve_cpu.py) reads these.  Rows past
+// cap_efc and contacts past cap_con are not written (the counts are).
+//   rows      [nefc]: J [nv], type, id, pos, margin, diagApprox, R, D, aref, force, state, frictionloss
+//   contacts  [ncon]: efc_address, dim, geom1, geom2, mu, friction [5], frame [9], dist, pos [3]
+//   counts    {nefc, ncon, niter, warning}
+template <class T>
+int forward_debug_efc(Engine<T>& e, const double* qpos, const double* qvel, const double* ctrl, const double* mocap,
+                      double time, const double* warmstart, int cap_efc, int cap_con, double* qacc, double* qacc_smooth,
+                      double* qfrc_smooth, double* qM, double* efc_J, int* efc_type, int* efc_id, double* efc_row,
+                      int* con_int, double* con_real, int* counts) {
+  const Model<T>& m = e.model;
+  e.resize(1);
+  Data<T>& d = *e.data[0];
+  for (int i = 0; i < m.nq; i++) d.qpos[i] = (T)qpos[i];
+  for (int i = 0; i < m.nv; i++) d.qvel[i] = (T)qvel[i];
+  for (int i = 0; i < m.nu; i++) d.ctrl[i] = (T)ctrl[i];
+  for (int i = 0; i < m.nmocap; i++) {
+    for (int c = 0; c < 3; c++) d.mocap_pos[3 * i + c] = (T)mocap[7 * i + c];
+    for (int c = 0; c < 4; c++) d.mocap_quat[4 * i + c] = (T)mocap[7 * i + 3 + c];
+  }
+  for (int i = 0; i < m.nv; i++) d.qacc_warmstart[i] = warmstart ? (T)warmstart[i] : 0;
+  d.time = (T)time;
+  d.warning = false;
+  forward<T>(m, d, residual_by_id<T>(m.residual_id));
+  const int nv = m.nv;
+  for (int i = 0; i < nv; i++) { qacc[i] = d.qacc[i]; qacc_smooth[i] = d.qacc_smooth[i]; qfrc_smooth[i] = d.qfrc_smooth[i]; }
+  for (int i = 0; i < nv * nv; i++) qM[i] = d.qM[i];
+  for (int r = 0; r < d.nefc && r < cap_efc; r++) {
+    for (int i = 0; i < nv; i++) efc_J[(size_t)r * nv + i] = d.efc_J[(size_t)r * nv + i];
+    efc_type[r] = d.efc_type[r]; efc_id[r] = d.efc_id[r];
+    const T row[10] = {d.efc_pos[r], d.efc_margin[r], d.efc_diagApprox[r], d.efc_R[r], d.efc_D[r], d.efc_aref[r],
+                       d.efc_force[r], (T)d.efc_state[r], d.efc_frictionloss[r], d.efc_vel[r]};
+    for (int k = 0; k < 10; k++) efc_row[10 * r + k] = row[k];
+  }
+  for (int ci = 0; ci < d.ncon && ci < cap_con; ci++) {
+    const Contact<T>& c = d.contact[ci];
+    con_int[4 * ci] = c.efc_address; con_int[4 * ci + 1] = c.dim; con_int[4 * ci + 2] = c.geom1; con_int[4 * ci + 3] = c.geom2;
+    double* o = con_real + 19 * ci;
+    o[0] = c.mu;
+    for (int k = 0; k < 5; k++) o[1 + k] = c.friction[k];
+    for (int k = 0; k < 9; k++) o[6 + k] = c.frame[k];
+    o[15] = c.dist;
+    for (int k = 0; k < 3; k++) o[16 + k] = c.pos[k];
+  }
+  counts[0] = d.nefc; counts[1] = d.ncon; counts[2] = d.solver_niter; counts[3] = d.warning ? 1 : 0;
+  return d.warning ? 1 : 0;
+}
+
 // B independent single steps (mj_step, trajectory.cc:158) from given (qpos, qvel, ctrl, warm start, time): the CPU
 // side of the teacher-forced per-step parity tests.  counts [B][4] = {ncon, nefc, Newton iterations, warning}.
 template <class T>
@@ -345,6 +394,17 @@ int oracle_forward_debug(void* hv, const double* qpos, const double* qvel, const
   return forward_debug(*h->e32, qpos, qvel, ctrl, mocap, time, warmstart, qacc, qM, qfrc_bias, qfrc_smooth, residual,
                        efc_force, nefc, ncon, niter, xpos, subtree_com, contact_out, qfrc_constraint, next_qpos,
                        next_qvel);
+}
+
+int oracle_forward_debug_efc(void* hv, const double* qpos, const double* qvel, const double* ctrl, const double* mocap,
+                             double time, const double* warmstart, int cap_efc, int cap_con, double* qacc,
+                             double* qacc_smooth, double* qfrc_smooth, double* qM, double* efc_J, int* efc_type,
+                             int* efc_id, double* efc_row, int* con_int, double* con_real, int* counts) {
+  auto* h = (Handle*)hv;
+#define CALL(e) forward_debug_efc(e, qpos, qvel, ctrl, mocap, time, warmstart, cap_efc, cap_con, qacc, qacc_smooth, \
+                                  qfrc_smooth, qM, efc_J, efc_type, efc_id, efc_row, con_int, con_real, counts)
+  return DISPATCH(h, CALL);
+#undef CALL
 }
 
 // ---- exact operation count of one spline rollout batch (instrumented scalar, oracle/counted.h)

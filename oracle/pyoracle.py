@@ -149,6 +149,34 @@ class Oracle:
         o["contact"] = o["contact"][: ncon.value]
         return o
 
+    def efc_debug(self, qpos, qvel, ctrl, mocap, time=0.0, warmstart=None, cap_efc=256, cap_con=64):
+        """The constraint problem of one mj_forward and the solver's answer.  Per row: efc_J [nefc, nv], efc_type,
+        efc_id, efc_pos, efc_margin, efc_diagApprox, efc_R, efc_D, efc_aref, efc_force, efc_state, efc_frictionloss,
+        efc_vel; per contact: efc_address, dim, geom1, geom2, mu, friction [5], frame [3, 3] (rows: normal, t1, t2),
+        dist, pos; and qacc, qacc_smooth, qfrc_smooth, qM, nefc, ncon, niter, warning."""
+        m = self.m
+        nv = m.nv
+        o = dict(qacc=np.zeros(nv), qacc_smooth=np.zeros(nv), qfrc_smooth=np.zeros(nv), qM=np.zeros((nv, nv)))
+        J, ty, idx = np.zeros((cap_efc, nv)), np.zeros(cap_efc, np.int32), np.zeros(cap_efc, np.int32)
+        row, ci, cr, counts = np.zeros((cap_efc, 10)), np.zeros((cap_con, 4), np.int32), np.zeros((cap_con, 19)), \
+            np.zeros(4, np.int32)
+        q, v, u, mc, ws = _d(qpos), _d(qvel), _d(ctrl), _d(mocap), _d(warmstart)
+        ip = lambda a: a.ctypes.data_as(C.POINTER(C.c_int))
+        lib().oracle_forward_debug_efc(self.h, _p(q), _p(v), _p(u), _p(mc), C.c_double(time), _p(ws), int(cap_efc),
+                                       int(cap_con), _p(o["qacc"]), _p(o["qacc_smooth"]), _p(o["qfrc_smooth"]),
+                                       _p(o["qM"]), _p(J), ip(ty), ip(idx), _p(row), ip(ci), _p(cr), ip(counts))
+        ne, nc = int(counts[0]), int(counts[1])
+        assert ne <= cap_efc and nc <= cap_con, (ne, nc)
+        o.update(nefc=ne, ncon=nc, niter=int(counts[2]), warning=int(counts[3]), efc_J=J[:ne], efc_type=ty[:ne],
+                 efc_id=idx[:ne])
+        for k, name in enumerate(("pos", "margin", "diagApprox", "R", "D", "aref", "force", "state", "frictionloss",
+                                  "vel")):
+            o["efc_" + name] = row[:ne, k]
+        o["efc_state"] = o["efc_state"].astype(int)
+        o.update(efc_address=ci[:nc, 0], dim=ci[:nc, 1], geom1=ci[:nc, 2], geom2=ci[:nc, 3], mu=cr[:nc, 0],
+                 friction=cr[:nc, 1:6], frame=cr[:nc, 6:15].reshape(nc, 3, 3), dist=cr[:nc, 15], pos=cr[:nc, 16:19])
+        return o
+
     def ilqg_policy_action(self, u_nom, x_nom, t_nom, gains, mode, step, state, time):
         """iLQGPolicy::Action of the oracle (fp64 handle only)."""
         assert self.precision == 64
