@@ -11,11 +11,13 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 #include <string>
 #include <vector>
 
 #include "../../include/mjpc_b200.h"
 #include "belief_kernels.cuh"
+#include "device_memory.h"
 #include "estimator_kernels.cuh"
 #include "filter_bank.h"
 #include "ilqg_kernels.cuh"
@@ -23,6 +25,8 @@
 #include "rollout_kernels.cuh"
 
 using namespace mjpc_dev;
+using mjpc_mem::DeviceArray;
+using mjpc_mem::PinnedArray;
 
 namespace {
 thread_local std::string g_last_error;
@@ -74,15 +78,11 @@ const KernelSet kHumanoidTrackKernels = {(const void*)rollout_kernel_humanoid_tr
 struct FilterBank {
   FilterBankArgs a;
   int s0 = 0, nsens = 0, adr0 = 0, nsd = 0;
-  void* d_mem = nullptr;
+  DeviceArray<unsigned char> d_mem;
   float *d_rtime = nullptr, *d_task = nullptr, *d_res = nullptr, *d_cost = nullptr;
   unsigned char* d_in = nullptr;   // sensor [B][ny] doubles, ctrl [B][nu] and mocap [B][7 nmocap] floats
-  unsigned char* h_stage = nullptr;
+  PinnedArray<unsigned char> h_stage;
   size_t in_bytes = 0;
-  ~FilterBank() {
-    if (d_mem) cudaFree(d_mem);
-    if (h_stage) cudaFreeHost(h_stage);
-  }
 };
 
 struct mjpc_b200 {
@@ -95,30 +95,29 @@ struct mjpc_b200 {
   size_t smem_optin = 0;   // the device's opt-in limit of dynamic shared memory per block
   int max_term_dim = 1;    // widest cost term (task_dim_norm_residual): sizes cost_derivatives_kernel's scratch
   const KernelSet* kernels = &kGenericKernels;   // chosen at create: the model's static instances, if it has them
-  float* d_pack = nullptr;
+  DeviceArray<float> d_pack;
   // inputs: d_in holds the per-problem inputs and the knots of the last rollout launch (stage_problems)
-  float* d_in = nullptr;
+  DeviceArray<float> d_in;
   // feedback policy of each problem of the last feedback launch ([fb_nprob][max_horizon][..]; grown on demand)
-  float *d_unom = nullptr, *d_xnom = nullptr, *d_tnom = nullptr, *d_gains = nullptr, *d_du = nullptr, *d_steps = nullptr;
+  DeviceArray<float> d_unom, d_xnom, d_tnom, d_gains, d_du, d_steps;
   int fb_nprob = 1;
   // outputs
-  float *d_states = nullptr, *d_actions = nullptr, *d_residual = nullptr, *d_costs = nullptr, *d_trace = nullptr,
-        *d_returns = nullptr;
-  double* d_times = nullptr;
-  unsigned char* d_failure = nullptr;
-  int* d_order = nullptr;
-  long long* d_stats = nullptr;
-  unsigned* d_pair_sync = nullptr;   // [256][32]: per-SM records of the co-resident pair synchronisation (dev_data.cuh)
+  DeviceArray<float> d_states, d_actions, d_residual, d_costs, d_trace, d_returns;
+  DeviceArray<double> d_times;
+  DeviceArray<unsigned char> d_failure;
+  DeviceArray<int> d_order;
+  DeviceArray<long long> d_stats;
+  DeviceArray<unsigned> d_pair_sync;   // [256][32]: per-SM records of the co-resident pair synchronisation (dev_data.cuh)
   // geometric contacts of the last step_debug (-1: none run yet) and their [maxcon][8] rows
   int dbg_ncon = -1;
   std::vector<float> dbg_contact;
   IlqgBuffers ilqg;
-  FilterBank* bank = nullptr;   // the state estimators' filters (filter_bank.h), made by mjpc_b200_bank::Init
-  PlantBank* plants = nullptr;  // the closed-loop plants (plant_bank.h), made by mjpc_b200_plant_init
+  std::unique_ptr<FilterBank> bank;   // the state estimators' filters (filter_bank.h), made by mjpc_b200_bank::Init
+  std::unique_ptr<PlantBank> plants;  // the closed-loop plants (plant_bank.h), made by mjpc_b200_plant_init
   // pinned staging
-  float* h_in = nullptr;
+  PinnedArray<float> h_in;
   size_t h_in_floats = 0;
-  unsigned char* h_out = nullptr;
+  PinnedArray<unsigned char> h_out;
   size_t h_out_bytes = 0;
   // host copies of the live task
   std::vector<double> weight, parameters, task_state;
@@ -136,10 +135,10 @@ struct mjpc_b200 {
   ncclComm_t comm = nullptr;
   int nranks = 1, rank = 0;
   int totalN = 0, shard_lo = 0, shard_hi = 0;   // of the last sharded rollout
-  float *d_slot = nullptr, *d_gather = nullptr, *d_returns_all = nullptr;
-  unsigned char* d_failure_all = nullptr;
-  int* d_order_all = nullptr;
-  float* d_bcast = nullptr;
+  DeviceArray<float> d_slot, d_gather, d_returns_all;
+  DeviceArray<unsigned char> d_failure_all;
+  DeviceArray<int> d_order_all;
+  DeviceArray<float> d_bcast;
   size_t bcast_floats = 0;
   int maxTotal = 0;
   int nuserdata = 0;
@@ -149,10 +148,10 @@ struct mjpc_b200 {
   std::vector<DevSensor> sensors;
   std::vector<std::string> sensor_why;
   std::vector<int> sensor_geoms;   // the rangefinders' eligible geoms, uploaded right after the rows
-  DevSensor* d_sensors = nullptr;
+  DeviceArray<DevSensor> d_sensors;
   // persistent scratch of step_impl: device buffer and its pinned host staging, grown on demand
-  float* d_step = nullptr;
-  float* h_step = nullptr;
+  DeviceArray<float> d_step;
+  PinnedArray<float> h_step;
   size_t step_words = 0;
   // model variants (set_model_variants): the model as created, which every variant is checked against; the variant
   // blocks [nvariants][variant_stride] floats in one allocation; and the variant each problem of the following launches
@@ -160,27 +159,27 @@ struct mjpc_b200 {
   DevModel M0;
   double timestep0 = 0;
   std::vector<float> f0;
-  float* d_variants = nullptr;
-  int* d_variant_index = nullptr;
+  DeviceArray<float> d_variants;
+  DeviceArray<int> d_variant_index;
   int nvariants = 0, variant_stride = 0, nselected = 0;
   // model ensemble (set_model_ensemble): the member blocks [nmembers][member_stride], laid out as the variant blocks;
   // the member of every launch problem, d_member_index [traj_factor x max_candidates] (problem j on member j % nmembers);
   // the members' returns and failure flags [B][K][N] of an ensemble launch.  The per-trajectory buffers hold
   // traj_factor x max_candidates trajectories (grown by set_model_ensemble, never shrunk).
-  float* d_members = nullptr;
-  int* d_member_index = nullptr;
-  float* d_member_returns = nullptr;
-  unsigned char* d_member_failure = nullptr;
+  DeviceArray<float> d_members;
+  DeviceArray<int> d_member_index;
+  DeviceArray<float> d_member_returns;
+  DeviceArray<unsigned char> d_member_failure;
   int nmembers = 0, member_stride = 0, worst = 0, traj_factor = 1;
   // the members of the resident and of the last launch (0: not an ensemble launch), and the last launch's N per problem
   int resident_members = 0, last_members = 0, last_nper = 0;
   // initial-state ensembles (rollout_spline_belief_batched): the covariances of the launch [cov_problems][n][n], the
   // joint table [3][njnt] (type, qposadr, dofadr), and d_belief [33 max_candidates]: each launch row's variant (up to
   // 32 rows per problem), then each problem's factorisation status
-  double* d_cov = nullptr;
+  DeviceArray<double> d_cov;
   int cov_problems = 0;
-  int* d_jnt = nullptr;
-  int* d_belief = nullptr;
+  DeviceArray<int> d_jnt;
+  DeviceArray<int> d_belief;
   // resident-input launch description
   RolloutArgs resident;
   bool resident_ok = false;
@@ -188,12 +187,16 @@ struct mjpc_b200 {
     DevLayout L = make_layout(pack.M, P);
     return ((size_t)smem_header_words(pack.M) + (size_t)L.total) * 4;
   }
+  // the stream is idle here (mjpc_b200_destroy synchronised it; a failed create enqueued nothing on it), and the
+  // owners free the memory after this
+  ~mjpc_b200() {
+    if (ev0) cudaEventDestroy(ev0);
+    if (ev1) cudaEventDestroy(ev1);
+    if (stream) cudaStreamDestroy(stream);
+  }
 };
 
 namespace {
-
-template <class T>
-cudaError_t dalloc(T** p, size_t n) { return cudaMalloc((void**)p, std::max<size_t>(n, 1) * sizeof(T)); }
 
 // the task floats of a pack: task_weight, task_norm_parameter, task_parameters and task_state lie back to back
 size_t task_floats_begin(const DevModel& M) { return M.fo[F_task_weight]; }
@@ -506,11 +509,10 @@ int stage_problems(mjpc_b200* h, int B, const float* states, const double* times
 // grow the pinned staging buffer to at least `floats` (never shrinks); on failure the old buffer stays
 int reserve_h_in(mjpc_b200* h, size_t floats) {
   if (floats <= h->h_in_floats) return 0;
-  float* p = nullptr;
+  PinnedArray<float> p;
+  CUDA_TRY(p.alloc(floats));
   CUDA_TRY(cudaStreamSynchronize(h->stream));   // earlier copies may still read the old buffer
-  CUDA_TRY(cudaMallocHost((void**)&p, floats * 4));
-  cudaFreeHost(h->h_in);
-  h->h_in = p; h->h_in_floats = floats;
+  h->h_in = std::move(p); h->h_in_floats = floats;
   return 0;
 }
 
@@ -519,17 +521,13 @@ int reserve_feedback(mjpc_b200* h, int B) {
   if (B <= h->fb_nprob) return 0;
   const DevModel& M = h->pack.M;
   const size_t H = h->maxH, ds = M.nq + M.nv, n = 2 * M.nv, nu = M.nu, P = B;
-  float* nb[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
-  const size_t cnt[5] = {P * H * nu, P * H * ds, P * H, P * H * nu * n, P * H * nu};
-  for (int i = 0; i < 5; i++)
-    if (cudaMalloc((void**)&nb[i], cnt[i] * 4) != cudaSuccess) {
-      cudaGetLastError();
-      for (float* q : nb) if (q) cudaFree(q);
-      return fail(MJPC_B200_ERR_CUDA, "rollout_feedback_batched: out of device memory for the feedback policies");
-    }
+  DeviceArray<float> unom, xnom, tnom, gains, du;
+  if (unom.alloc(P * H * nu) || xnom.alloc(P * H * ds) || tnom.alloc(P * H) || gains.alloc(P * H * nu * n) ||
+      du.alloc(P * H * nu))
+    return fail(MJPC_B200_ERR_CUDA, "rollout_feedback_batched: out of device memory for the feedback policies");
   CUDA_TRY(cudaStreamSynchronize(h->stream));
-  float** old[5] = {&h->d_unom, &h->d_xnom, &h->d_tnom, &h->d_gains, &h->d_du};
-  for (int i = 0; i < 5; i++) { cudaFree(*old[i]); *old[i] = nb[i]; }
+  h->d_unom = std::move(unom); h->d_xnom = std::move(xnom); h->d_tnom = std::move(tnom);
+  h->d_gains = std::move(gains); h->d_du = std::move(du);
   h->fb_nprob = B;
   return 0;
 }
@@ -547,7 +545,7 @@ int launch_rollout(mjpc_b200* h, const RolloutArgs& A_in, int K = 0, int worst =
   {
     const char* ps = std::getenv("MJPC_B200_PAIR_SYNC");
     const bool on = !(ps && ps[0] == '0') && A.N > h->num_sms && A.N <= 2 * h->num_sms;
-    A.pair_sync = on ? h->d_pair_sync : nullptr;
+    A.pair_sync = on ? h->d_pair_sync.get() : nullptr;
     if (on) CUDA_TRY(cudaMemsetAsync(h->d_pair_sync, 0, (size_t)256 * 32 * sizeof(unsigned), h->stream));
   }
   // one candidate per CTA, whichever instance; the static ones share the generic one's arguments and shared-memory image
@@ -585,7 +583,7 @@ RolloutArgs base_args(mjpc_b200* h, int N, int H) {
 }
 
 int read_back(mjpc_b200* h, int N, float* returns, uint8_t* failure, int* order) {
-  float* hr = (float*)h->h_out;
+  float* hr = (float*)h->h_out.get();
   int* ho = (int*)(h->h_out + (size_t)N * 4);
   unsigned char* hf = h->h_out + (size_t)N * 8;
   CUDA_TRY(cudaMemcpyAsync(hr, h->d_returns, (size_t)N * 4, cudaMemcpyDeviceToHost, h->stream));
@@ -665,16 +663,6 @@ extern "C" {
 const char* mjpc_b200_version(void) { return "mjpc_b200 0.1.0 (sm_90a)"; }
 const char* mjpc_b200_last_error(void) { return g_last_error.c_str(); }
 
-// inside create(): a failing CUDA call must not leak the half-built handle
-#define CREATE_TRY(expr)                                                                                   \
-  do {                                                                                                     \
-    cudaError_t e_ = (expr);                                                                               \
-    if (e_ != cudaSuccess) {                                                                               \
-      mjpc_b200_destroy(h);                                                                                \
-      return fail(MJPC_B200_ERR_CUDA, std::string(#expr) + ": " + cudaGetErrorString(e_));                 \
-    }                                                                                                      \
-  } while (0)
-
 int mjpc_b200_create(const mjpc_model_blob* model, int max_candidates, int max_horizon, int device,
                      mjpc_b200_t** out) {
   if (!model || !model->data || !out || max_candidates < 1 || max_horizon < 1)
@@ -684,12 +672,12 @@ int mjpc_b200_create(const mjpc_model_blob* model, int max_candidates, int max_h
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
     return fail(MJPC_B200_ERR_CUDA, "no CUDA device: the engine has no CPU fallback");
   if (device < 0 || device >= ndev) return fail(MJPC_B200_ERR_BAD_ARGUMENT, "create: bad device ordinal");
-  mjpc_b200* h = new mjpc_b200;
+  // the handle is built here and released to the caller only when complete; a refusal frees whatever it holds
+  std::unique_ptr<mjpc_b200> h(new mjpc_b200);
   try {
     int maxcon = 32, maxefc = 96;
     h->pack = pack_model(model->data, model->nbytes, maxcon, maxefc);
   } catch (const std::exception& e) {
-    delete h;
     return fail(MJPC_B200_ERR_BAD_BLOB, std::string("create: ") + e.what());
   }
   h->device = device;
@@ -698,7 +686,7 @@ int mjpc_b200_create(const mjpc_model_blob* model, int max_candidates, int max_h
   {
     Blob b(model->data, model->nbytes);
     h->nuserdata = b.i("nuserdata");
-    if (h->nuserdata != 0) { delete h; return fail(MJPC_B200_ERR_UNSUPPORTED, "create: mjData::userdata (nuserdata > 0) is not supported"); }
+    if (h->nuserdata != 0) return fail(MJPC_B200_ERR_UNSUPPORTED, "create: mjData::userdata (nuserdata > 0) is not supported");
     h->weight = b.reals("task_weight"); h->parameters = b.reals("task_parameters");
     h->task_state = b.reals("task_state"); h->risk = b.r("task_risk");
     for (int d : b.ints("task_dim_norm_residual")) h->max_term_dim = std::max(h->max_term_dim, d);
@@ -706,19 +694,17 @@ int mjpc_b200_create(const mjpc_model_blob* model, int max_candidates, int max_h
   h->time_idx = time_like_state(M.residual_id);
   sensor_table(Blob(model->data, model->nbytes), &h->sensors, &h->sensor_why, &h->sensor_geoms);
   h->M0 = M; h->timestep0 = h->pack.timestep; h->f0 = h->pack.f;
-  CREATE_TRY(cudaSetDevice(device));
-  CREATE_TRY(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
-  CREATE_TRY(cudaEventCreate(&h->ev0));
-  CREATE_TRY(cudaEventCreate(&h->ev1));
+  CUDA_TRY(cudaSetDevice(device));
+  CUDA_TRY(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
+  CUDA_TRY(cudaEventCreate(&h->ev0));
+  CUDA_TRY(cudaEventCreate(&h->ev1));
   cudaDeviceProp prop;
-  CREATE_TRY(cudaGetDeviceProperties(&prop, device));
+  CUDA_TRY(cudaGetDeviceProperties(&prop, device));
   h->num_sms = prop.multiProcessorCount;
   h->smem_optin = prop.sharedMemPerBlockOptin;
   const size_t smem_need = h->smem_bytes(h->maxP);
-  if (smem_need > (size_t)prop.sharedMemPerBlockOptin) {
-    mjpc_b200_destroy(h);
+  if (smem_need > (size_t)prop.sharedMemPerBlockOptin)
     return fail(MJPC_B200_ERR_CAPACITY, "model does not fit in shared memory");
-  }
   // pack: floats then ints, one buffer (single TMA bulk copy per CTA)
   {
     std::vector<float>& f = h->pack.f;
@@ -727,33 +713,33 @@ int mjpc_b200_create(const mjpc_model_blob* model, int max_candidates, int max_h
     std::memcpy(f.data() + nf, h->pack.i.data(), h->pack.i.size() * 4);
     // not staged to shared memory: keyframe mocap positions, read from HBM by the tracking residual (Ctx::gkey)
     for (double x : h->pack.key_mpos) f.push_back((float)x);
-    CREATE_TRY(dalloc(&h->d_pack, f.size()));
-    CREATE_TRY(cudaMemcpy(h->d_pack, f.data(), f.size() * 4, cudaMemcpyHostToDevice));
+    CUDA_TRY(h->d_pack.alloc(f.size()));
+    CUDA_TRY(cudaMemcpy(h->d_pack, f.data(), f.size() * 4, cudaMemcpyHostToDevice));
   }
   const size_t N = max_candidates, H = max_horizon, ds = M.nq + M.nv, n = 2 * M.nv, nu = M.nu, nr = M.num_residual;
   // launch inputs: up to max_candidates problems of one candidate each (stage_problems)
   const size_t in_floats = problem_floats(M, max_candidates, h->maxP, max_horizon) + N * h->maxP * nu;
-  CREATE_TRY(dalloc(&h->d_in, in_floats));
-  CREATE_TRY(dalloc(&h->d_unom, H * nu)); CREATE_TRY(dalloc(&h->d_xnom, H * ds)); CREATE_TRY(dalloc(&h->d_tnom, H));
-  CREATE_TRY(dalloc(&h->d_gains, H * nu * n)); CREATE_TRY(dalloc(&h->d_du, H * nu)); CREATE_TRY(dalloc(&h->d_steps, N));
-  CREATE_TRY(dalloc(&h->d_states, N * H * ds)); CREATE_TRY(dalloc(&h->d_actions, N * H * nu));
-  CREATE_TRY(dalloc(&h->d_times, N * H)); CREATE_TRY(dalloc(&h->d_residual, N * H * nr));
-  CREATE_TRY(dalloc(&h->d_costs, N * H)); CREATE_TRY(dalloc(&h->d_trace, N * H * 3 * (size_t)M.num_trace));
-  CREATE_TRY(dalloc(&h->d_returns, N)); CREATE_TRY(dalloc(&h->d_failure, N)); CREATE_TRY(dalloc(&h->d_order, N)); CREATE_TRY(dalloc(&h->d_stats, 12 * N));
-  CREATE_TRY(dalloc(&h->d_pair_sync, (size_t)256 * 32));
+  CUDA_TRY(h->d_in.alloc(in_floats));
+  CUDA_TRY(h->d_unom.alloc(H * nu)); CUDA_TRY(h->d_xnom.alloc(H * ds)); CUDA_TRY(h->d_tnom.alloc(H));
+  CUDA_TRY(h->d_gains.alloc(H * nu * n)); CUDA_TRY(h->d_du.alloc(H * nu)); CUDA_TRY(h->d_steps.alloc(N));
+  CUDA_TRY(h->d_states.alloc(N * H * ds)); CUDA_TRY(h->d_actions.alloc(N * H * nu));
+  CUDA_TRY(h->d_times.alloc(N * H)); CUDA_TRY(h->d_residual.alloc(N * H * nr));
+  CUDA_TRY(h->d_costs.alloc(N * H)); CUDA_TRY(h->d_trace.alloc(N * H * 3 * (size_t)M.num_trace));
+  CUDA_TRY(h->d_returns.alloc(N)); CUDA_TRY(h->d_failure.alloc(N)); CUDA_TRY(h->d_order.alloc(N)); CUDA_TRY(h->d_stats.alloc(12 * N));
+  CUDA_TRY(h->d_pair_sync.alloc((size_t)256 * 32));
   {
     // the rows, then the rangefinders' geom lists (DevSensor::geom0)
     const size_t rows = h->sensors.size() * sizeof(DevSensor), list = h->sensor_geoms.size() * sizeof(int);
-    CREATE_TRY(dalloc(&h->d_sensors, h->sensors.size() + (list + sizeof(DevSensor) - 1) / sizeof(DevSensor)));
-    if (rows) CREATE_TRY(cudaMemcpy(h->d_sensors, h->sensors.data(), rows, cudaMemcpyHostToDevice));
+    CUDA_TRY(h->d_sensors.alloc(h->sensors.size() + (list + sizeof(DevSensor) - 1) / sizeof(DevSensor)));
+    if (rows) CUDA_TRY(cudaMemcpy(h->d_sensors, h->sensors.data(), rows, cudaMemcpyHostToDevice));
     if (list)
-      CREATE_TRY(cudaMemcpy(reinterpret_cast<char*>(h->d_sensors) + rows, h->sensor_geoms.data(), list,
-                            cudaMemcpyHostToDevice));
+      CUDA_TRY(cudaMemcpy(reinterpret_cast<char*>(h->d_sensors.get()) + rows, h->sensor_geoms.data(), list,
+                          cudaMemcpyHostToDevice));
   }
   h->h_in_floats = in_floats + H * (nu + ds + 1 + nu * n + nu) + N + 64;
-  CREATE_TRY(cudaMallocHost((void**)&h->h_in, h->h_in_floats * 4));
+  CUDA_TRY(h->h_in.alloc(h->h_in_floats));
   h->h_out_bytes = N * 16 + 64;
-  CREATE_TRY(cudaMallocHost((void**)&h->h_out, h->h_out_bytes));
+  CUDA_TRY(h->h_out.alloc(h->h_out_bytes));
   const DevLayout L1 = make_layout(M, 1);
   const int* dof_parent = h->pack.i.data() + M.io[I_dof_parentid];
   if (spec_matches<SpecQuadruped>(M, L1, dof_parent)) h->kernels = &kQuadrupedKernels;
@@ -762,15 +748,12 @@ int mjpc_b200_create(const mjpc_model_blob* model, int max_candidates, int max_h
   // handles may coexist); a launch may fall back to the generic row (pick_kernels), so both rows get theirs
   const size_t smem_rollout = h->smem_bytes(h->maxP), smem_step = h->smem_bytes(1);
   for (const KernelSet* k : {h->kernels, &kGenericKernels}) {
-    CREATE_TRY(raise_smem_limit(k->rollout, smem_rollout)); CREATE_TRY(raise_smem_limit(k->rollout_plain, smem_rollout));
-    CREATE_TRY(raise_smem_limit(k->step, smem_step)); CREATE_TRY(raise_smem_limit(k->fd_center, smem_step));
-    CREATE_TRY(raise_smem_limit(k->fd_column, smem_step)); CREATE_TRY(raise_smem_limit(k->plant, smem_step));
+    CUDA_TRY(raise_smem_limit(k->rollout, smem_rollout)); CUDA_TRY(raise_smem_limit(k->rollout_plain, smem_rollout));
+    CUDA_TRY(raise_smem_limit(k->step, smem_step)); CUDA_TRY(raise_smem_limit(k->fd_center, smem_step));
+    CUDA_TRY(raise_smem_limit(k->fd_column, smem_step)); CUDA_TRY(raise_smem_limit(k->plant, smem_step));
   }
-  if (int rc = ilqg_init(h->ilqg, h->pack.M, (int)H)) {
-    mjpc_b200_destroy(h);
-    return fail(rc, "ilqg buffer allocation failed");
-  }
-  *out = h;
+  if (int rc = ilqg_init(h->ilqg, h->pack.M, (int)H)) return fail(rc, "ilqg buffer allocation failed");
+  *out = h.release();
   return MJPC_B200_OK;
 }
 
@@ -779,23 +762,6 @@ void mjpc_b200_destroy(mjpc_b200_t* h) {
   cudaSetDevice(h->device);
   if (h->stream) cudaStreamSynchronize(h->stream);
   if (h->comm && nccl_api().ok) nccl_api().CommDestroy(h->comm);
-  void* mbufs[] = {h->d_slot, h->d_gather, h->d_returns_all, h->d_failure_all, h->d_order_all, h->d_bcast};
-  for (void* p : mbufs) if (p) cudaFree(p);
-  void* bufs[] = {h->d_pack, h->d_in, h->d_unom, h->d_xnom,
-                  h->d_tnom, h->d_gains, h->d_du, h->d_steps, h->d_states, h->d_actions, h->d_times, h->d_residual,
-                  h->d_costs, h->d_trace, h->d_returns, h->d_failure, h->d_order, h->d_stats, h->d_pair_sync,
-                  h->d_sensors, h->d_step, h->d_variants, h->d_variant_index, h->d_members, h->d_member_index,
-                  h->d_member_returns, h->d_member_failure, h->d_cov, h->d_jnt, h->d_belief};
-  for (void* p : bufs) if (p) cudaFree(p);
-  ilqg_free(h->ilqg);
-  delete h->bank;
-  delete h->plants;
-  if (h->h_in) cudaFreeHost(h->h_in);
-  if (h->h_out) cudaFreeHost(h->h_out);
-  if (h->h_step) cudaFreeHost(h->h_step);
-  if (h->ev0) cudaEventDestroy(h->ev0);
-  if (h->ev1) cudaEventDestroy(h->ev1);
-  if (h->stream) cudaStreamDestroy(h->stream);
   delete h;
 }
 
@@ -886,20 +852,14 @@ static int model_blocks(mjpc_b200_t* h, const mjpc_model_blob* models, int count
   return 0;
 }
 
-// device copies of a host block image and of a member / variant index, both or neither: on a failure nothing stays
-// allocated
-static cudaError_t upload_blocks(const std::vector<float>& blocks, const std::vector<int>& index, float** d, int** di) {
-  *d = nullptr; *di = nullptr;
-  cudaError_t e = dalloc(d, blocks.size());
-  if (e == cudaSuccess) e = dalloc(di, index.size());
+// device copies of a host block image and of a member / variant index
+static cudaError_t upload_blocks(const std::vector<float>& blocks, const std::vector<int>& index, DeviceArray<float>* d,
+                                 DeviceArray<int>* di) {
+  cudaError_t e = d->alloc(blocks.size());
+  if (e == cudaSuccess) e = di->alloc(index.size());
   if (e == cudaSuccess) e = cudaMemcpy(*d, blocks.data(), blocks.size() * 4, cudaMemcpyHostToDevice);
   if (e == cudaSuccess) e = cudaMemcpy(*di, index.data(), index.size() * 4, cudaMemcpyHostToDevice);
-  if (e != cudaSuccess) {
-    cudaGetLastError();
-    if (*d) cudaFree(*d);
-    if (*di) cudaFree(*di);
-    *d = nullptr; *di = nullptr;
-  }
+  if (e != cudaSuccess) cudaGetLastError();
   return e;
 }
 
@@ -918,8 +878,8 @@ int mjpc_b200_set_model_variants(mjpc_b200_t* h, const mjpc_model_blob* models, 
   std::vector<float> blocks;
   size_t stride = 0;
   if (int rc = model_blocks(h, models, count, "set_model_variants", "variant", &blocks, &stride)) return rc;
-  float* d = nullptr;
-  int* di = nullptr;
+  DeviceArray<float> d;
+  DeviceArray<int> di;
   if (count) {
     std::vector<int> identity(h->maxN);
     for (int v = 0; v < h->maxN; v++) identity[v] = v < count ? v : 0;
@@ -927,9 +887,7 @@ int mjpc_b200_set_model_variants(mjpc_b200_t* h, const mjpc_model_blob* models, 
       return fail(MJPC_B200_ERR_CUDA, std::string("set_model_variants: ") + cudaGetErrorString(e));
   }
   CUDA_TRY(cudaStreamSynchronize(h->stream));   // launches in flight may still read the old blocks
-  if (h->d_variants) cudaFree(h->d_variants);
-  if (h->d_variant_index) cudaFree(h->d_variant_index);
-  h->d_variants = d; h->d_variant_index = di;
+  h->d_variants = std::move(d); h->d_variant_index = std::move(di);
   h->nvariants = count; h->nselected = count; h->variant_stride = (int)stride;
   h->resident_ok = false;
   return 0;
@@ -966,36 +924,30 @@ static int reserve_members(mjpc_b200_t* h, int K) {
   const size_t N = (size_t)K * h->maxN, H = h->maxH, ds = M.nq + M.nv, nu = M.nu, nr = M.num_residual,
                ntr = 3 * (size_t)M.num_trace;
   const size_t in_floats = problem_floats(M, (int)N, h->maxP, h->maxH) + N * h->maxP * nu;
-  float *states = nullptr, *actions = nullptr, *residual = nullptr, *costs = nullptr, *trace = nullptr,
-        *mret = nullptr, *din = nullptr, *hin = nullptr;
-  double* times = nullptr;
-  long long* stats = nullptr;
-  unsigned char* mfail = nullptr;
-  cudaError_t e = dalloc(&states, N * H * ds);
-  if (e == cudaSuccess) e = dalloc(&actions, N * H * nu);
-  if (e == cudaSuccess) e = dalloc(&times, N * H);
-  if (e == cudaSuccess) e = dalloc(&residual, N * H * nr);
-  if (e == cudaSuccess) e = dalloc(&costs, N * H);
-  if (e == cudaSuccess) e = dalloc(&trace, N * H * ntr);
-  if (e == cudaSuccess) e = dalloc(&stats, 12 * N);
-  if (e == cudaSuccess) e = dalloc(&mret, N);
-  if (e == cudaSuccess) e = dalloc(&mfail, N);
-  if (e == cudaSuccess) e = dalloc(&din, in_floats);
-  if (e == cudaSuccess && in_floats + 64 > h->h_in_floats) e = cudaMallocHost((void**)&hin, (in_floats + 64) * 4);
-  void* fresh[] = {states, actions, times, residual, costs, trace, stats, mret, mfail, din};
-  if (e != cudaSuccess) {
-    cudaGetLastError();
-    for (void* p : fresh) if (p) cudaFree(p);
-    if (hin) cudaFreeHost(hin);
-    return fail(MJPC_B200_ERR_CUDA, std::string("set_model_ensemble: ") + cudaGetErrorString(e));
-  }
+  DeviceArray<float> states, actions, residual, costs, trace, mret, din;
+  DeviceArray<double> times;
+  DeviceArray<long long> stats;
+  DeviceArray<unsigned char> mfail;
+  PinnedArray<float> hin;
+  const bool grow_h_in = in_floats + 64 > h->h_in_floats;
+  cudaError_t e = states.alloc(N * H * ds);
+  if (e == cudaSuccess) e = actions.alloc(N * H * nu);
+  if (e == cudaSuccess) e = times.alloc(N * H);
+  if (e == cudaSuccess) e = residual.alloc(N * H * nr);
+  if (e == cudaSuccess) e = costs.alloc(N * H);
+  if (e == cudaSuccess) e = trace.alloc(N * H * ntr);
+  if (e == cudaSuccess) e = stats.alloc(12 * N);
+  if (e == cudaSuccess) e = mret.alloc(N);
+  if (e == cudaSuccess) e = mfail.alloc(N);
+  if (e == cudaSuccess) e = din.alloc(in_floats);
+  if (e == cudaSuccess && grow_h_in) e = hin.alloc(in_floats + 64);
+  if (e != cudaSuccess) return fail(MJPC_B200_ERR_CUDA, std::string("set_model_ensemble: ") + cudaGetErrorString(e));
   CUDA_TRY(cudaStreamSynchronize(h->stream));   // launches and copies in flight may still use the old buffers
-  void* old[] = {h->d_states, h->d_actions, h->d_times, h->d_residual, h->d_costs, h->d_trace, h->d_stats,
-                 h->d_member_returns, h->d_member_failure, h->d_in};
-  for (void* p : old) if (p) cudaFree(p);
-  h->d_states = states; h->d_actions = actions; h->d_times = times; h->d_residual = residual; h->d_costs = costs;
-  h->d_trace = trace; h->d_stats = stats; h->d_member_returns = mret; h->d_member_failure = mfail; h->d_in = din;
-  if (hin) { cudaFreeHost(h->h_in); h->h_in = hin; h->h_in_floats = in_floats + 64; }
+  h->d_states = std::move(states); h->d_actions = std::move(actions); h->d_times = std::move(times);
+  h->d_residual = std::move(residual); h->d_costs = std::move(costs); h->d_trace = std::move(trace);
+  h->d_stats = std::move(stats); h->d_member_returns = std::move(mret); h->d_member_failure = std::move(mfail);
+  h->d_in = std::move(din);
+  if (grow_h_in) { h->h_in = std::move(hin); h->h_in_floats = in_floats + 64; }
   h->traj_factor = K;
   h->resident_ok = false;
   h->lastN = 0;   // the last launch's trajectories are gone
@@ -1010,9 +962,7 @@ int mjpc_b200_set_model_ensemble(mjpc_b200_t* h, const mjpc_model_blob* models, 
   if (K == 0 || !models) {
     CUDA_TRY(cudaSetDevice(h->device));
     CUDA_TRY(cudaStreamSynchronize(h->stream));
-    if (h->d_members) cudaFree(h->d_members);
-    if (h->d_member_index) cudaFree(h->d_member_index);
-    h->d_members = nullptr; h->d_member_index = nullptr;
+    h->d_members.reset(); h->d_member_index.reset();
     h->nmembers = 0; h->member_stride = 0; h->worst = 0;
     h->resident_ok = false;
     return 0;
@@ -1028,14 +978,12 @@ int mjpc_b200_set_model_ensemble(mjpc_b200_t* h, const mjpc_model_blob* models, 
   if (int rc = reserve_members(h, K)) return rc;
   std::vector<int> index((size_t)h->traj_factor * h->maxN);
   for (size_t j = 0; j < index.size(); j++) index[j] = (int)(j % K);
-  float* d = nullptr;
-  int* di = nullptr;
+  DeviceArray<float> d;
+  DeviceArray<int> di;
   if (cudaError_t e = upload_blocks(blocks, index, &d, &di))
     return fail(MJPC_B200_ERR_CUDA, std::string("set_model_ensemble: ") + cudaGetErrorString(e));
   CUDA_TRY(cudaStreamSynchronize(h->stream));   // launches in flight may still read the old blocks
-  if (h->d_members) cudaFree(h->d_members);
-  if (h->d_member_index) cudaFree(h->d_member_index);
-  h->d_members = d; h->d_member_index = di;
+  h->d_members = std::move(d); h->d_member_index = std::move(di);
   h->nmembers = K; h->member_stride = (int)stride; h->worst = worst;
   h->resident_ok = false;
   return 0;
@@ -1110,28 +1058,22 @@ static int reserve_belief(mjpc_b200_t* h, int B, int K) {
       jnt[M.njnt + j] = h->pack.i[M.io[I_jnt_qposadr] + j];
       jnt[2 * M.njnt + j] = h->pack.i[M.io[I_jnt_dofadr] + j];
     }
-    int* dj = nullptr;
-    int* db = nullptr;
-    cudaError_t e = dalloc(&dj, jnt.size());
-    if (e == cudaSuccess) e = dalloc(&db, 33 * (size_t)h->maxN);
+    DeviceArray<int> dj, db;
+    cudaError_t e = dj.alloc(jnt.size());
+    if (e == cudaSuccess) e = db.alloc(33 * (size_t)h->maxN);
     if (e == cudaSuccess) e = cudaMemcpy(dj, jnt.data(), jnt.size() * 4, cudaMemcpyHostToDevice);
     if (e != cudaSuccess) {
       cudaGetLastError();
-      if (dj) cudaFree(dj);
-      if (db) cudaFree(db);
       return fail(MJPC_B200_ERR_CUDA, std::string("rollout_spline_belief_batched: ") + cudaGetErrorString(e));
     }
-    h->d_jnt = dj; h->d_belief = db;
+    h->d_jnt = std::move(dj); h->d_belief = std::move(db);
   }
   if (B > h->cov_problems) {
-    double* dc = nullptr;
-    if (cudaError_t e = dalloc(&dc, (size_t)B * n * n)) {
-      cudaGetLastError();
+    DeviceArray<double> dc;
+    if (cudaError_t e = dc.alloc((size_t)B * n * n))
       return fail(MJPC_B200_ERR_CUDA, std::string("rollout_spline_belief_batched: ") + cudaGetErrorString(e));
-    }
     CUDA_TRY(cudaStreamSynchronize(h->stream));   // a launch in flight may still read the old covariances
-    if (h->d_cov) cudaFree(h->d_cov);
-    h->d_cov = dc; h->cov_problems = B;
+    h->d_cov = std::move(dc); h->cov_problems = B;
   }
   return 0;
 }
@@ -1185,7 +1127,7 @@ int mjpc_b200_rollout_spline_belief_batched(mjpc_b200_t* h, int B, int K, int wo
   S.B = B; S.K = K; S.n = (int)n; S.nq = M.nq; S.nv = M.nv; S.njnt = M.njnt;
   S.jnt = h->d_jnt; S.cov = h->d_cov; S.seed = seed; S.iteration = iteration;
   S.rows = const_cast<float*>(A.state);
-  S.variant_index = h->nvariants ? h->d_variant_index : nullptr;
+  S.variant_index = h->nvariants ? h->d_variant_index.get() : nullptr;
   S.row_index = h->d_belief; S.status = h->d_belief + 32 * (size_t)h->maxN;
   if (smem > 48 * 1024)
     CUDA_TRY(cudaFuncSetAttribute((const void*)state_sample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -1310,7 +1252,7 @@ static int rollout_feedback_impl(mjpc_b200_t* h, int B, const float* states, con
   A.L = make_layout(h->pack.M, 1);
   A.P = 1; A.policy_kind = 1;
   A.fb.u_nom = h->d_unom; A.fb.x_nom = h->d_xnom; A.fb.t_nom = h->d_tnom; A.fb.gains = h->d_gains;
-  A.fb.du = du ? h->d_du : nullptr; A.fb.iv = A.iv; A.fb.mode = mode; A.fb.H = H; A.fb.nper = K;
+  A.fb.du = du ? h->d_du.get() : nullptr; A.fb.iv = A.iv; A.fb.mode = mode; A.fb.H = H; A.fb.nper = K;
   A.step_sizes = h->d_steps;
   h->resident_ok = false;
   int rc = launch_rollout(h, A);
@@ -1436,16 +1378,12 @@ void mjpc_b200_host_ensemble_score(const float* member_returns, const uint8_t* m
 // grow step_impl's device scratch and pinned staging to `words` floats each (never shrinks); on failure the old ones stay
 int reserve_step(mjpc_b200_t* h, size_t words) {
   if (words <= h->step_words) return 0;
-  float *d = nullptr, *p = nullptr;
+  DeviceArray<float> d;
+  PinnedArray<float> p;
+  CUDA_TRY(d.alloc(words));
+  if (p.alloc(words)) return fail(MJPC_B200_ERR_CUDA, "step: out of pinned host memory");
   CUDA_TRY(cudaStreamSynchronize(h->stream));
-  CUDA_TRY(dalloc(&d, words));
-  if (cudaMallocHost((void**)&p, words * 4) != cudaSuccess) {
-    cudaGetLastError();
-    cudaFree(d);
-    return fail(MJPC_B200_ERR_CUDA, "step: out of pinned host memory");
-  }
-  cudaFree(h->d_step); cudaFreeHost(h->h_step);
-  h->d_step = d; h->h_step = p; h->step_words = words;
+  h->d_step = std::move(d); h->h_step = std::move(p); h->step_words = words;
   return 0;
 }
 
@@ -1562,18 +1500,25 @@ int mjpc_b200_comm_init(mjpc_b200_t* h, int nranks, int rank, const void* unique
   NcclApi& api = nccl_api();
   if (!api.ok) return fail(MJPC_B200_ERR_UNSUPPORTED, "libnccl.so.2 not found");
   CUDA_TRY(cudaSetDevice(h->device));
+  // the exchange buffers first, then the communicator, then everything is stored at once: a refusal leaves no
+  // communicator on the handle, so the call can be repeated
+  const DevModel& M = h->pack.M;
+  const size_t width = h->maxN, total = (size_t)nranks * h->maxN,
+               bcast_floats = (size_t)h->maxH * (M.nq + M.nv + M.nu + M.num_residual + 1 + 3 * M.num_trace + 2) + 16;
+  DeviceArray<float> slot, gather, returns_all, bcast;
+  DeviceArray<unsigned char> failure_all;
+  DeviceArray<int> order_all;
+  CUDA_TRY(slot.alloc(2 * width)); CUDA_TRY(gather.alloc(2 * width * nranks));
+  CUDA_TRY(returns_all.alloc(total)); CUDA_TRY(failure_all.alloc(total)); CUDA_TRY(order_all.alloc(total));
+  CUDA_TRY(bcast.alloc(bcast_floats));
   ncclUniqueId id;
   std::memcpy(&id, unique_id, sizeof(id));
-  NCCL_TRY(api.CommInitRank(&h->comm, nranks, id, rank));
-  h->nranks = nranks; h->rank = rank;
-  h->maxTotal = nranks * h->maxN;
-  const DevModel& M = h->pack.M;
-  const size_t width = h->maxN;
-  CUDA_TRY(dalloc(&h->d_slot, 2 * width)); CUDA_TRY(dalloc(&h->d_gather, 2 * width * nranks));
-  CUDA_TRY(dalloc(&h->d_returns_all, (size_t)h->maxTotal)); CUDA_TRY(dalloc(&h->d_failure_all, (size_t)h->maxTotal));
-  CUDA_TRY(dalloc(&h->d_order_all, (size_t)h->maxTotal));
-  h->bcast_floats = (size_t)h->maxH * (M.nq + M.nv + M.nu + M.num_residual + 1 + 3 * M.num_trace + 2) + 16;
-  CUDA_TRY(dalloc(&h->d_bcast, h->bcast_floats));
+  ncclComm_t comm = nullptr;
+  NCCL_TRY(api.CommInitRank(&comm, nranks, id, rank));
+  h->comm = comm; h->nranks = nranks; h->rank = rank;
+  h->maxTotal = (int)total; h->bcast_floats = bcast_floats;
+  h->d_slot = std::move(slot); h->d_gather = std::move(gather); h->d_returns_all = std::move(returns_all);
+  h->d_failure_all = std::move(failure_all); h->d_order_all = std::move(order_all); h->d_bcast = std::move(bcast);
   return 0;
 }
 
@@ -1736,9 +1681,8 @@ int mjpc_b200_plant_init(mjpc_b200_t* h, int num_plants, int sensor_start, int n
     if (!h->sensor_why[i].empty())
       return fail(MJPC_B200_ERR_UNSUPPORTED, "plant_init: sensor " + std::to_string(i) + ": " + h->sensor_why[i]);
   CUDA_TRY(cudaSetDevice(h->device));
-  CUDA_TRY(cudaStreamSynchronize(h->stream));   // a step in flight may still use the old bank
   const DevModel& M = h->pack.M;
-  PlantBank* k = new PlantBank;
+  std::unique_ptr<PlantBank> k(new PlantBank);
   PlantArgs& a = k->a;
   std::memset(&a, 0, sizeof(a));
   a.B = num_plants;
@@ -1768,14 +1712,13 @@ int mjpc_b200_plant_init(mjpc_b200_t* h, int num_plants, int sensor_start, int n
   k->in_bytes = in; k->out_bytes = out;
   const size_t o_in = take(in), o_out = take(out);
   auto fail_k = [&](cudaError_t e) {
-    delete k;
     return fail(MJPC_B200_ERR_CUDA, std::string("plant_init: ") + cudaGetErrorString(e));
   };
-  if (cudaError_t e = cudaMalloc(&k->d_mem, bytes)) return fail_k(e);
+  if (cudaError_t e = k->d_mem.alloc(bytes)) return fail_k(e);
   if (cudaError_t e = cudaMemset(k->d_mem, 0, bytes)) return fail_k(e);
-  if (cudaError_t e = cudaMallocHost((void**)&k->h_stage, in + out)) return fail_k(e);
+  if (cudaError_t e = k->h_stage.alloc(in + out)) return fail_k(e);
   std::memset(k->h_stage, 0, in + out);
-  unsigned char* base = (unsigned char*)k->d_mem;
+  unsigned char* base = k->d_mem;
   a.qpos = (float*)(base + o_qpos); a.qvel = (float*)(base + o_qvel); a.warm = (float*)(base + o_warm);
   a.time = (double*)(base + o_time); a.cost_sum = (double*)(base + o_sum);
   a.steps = (int*)(base + o_steps); a.warnings = (int*)(base + o_warn); a.status = (int*)(base + o_status);
@@ -1803,8 +1746,8 @@ int mjpc_b200_plant_init(mjpc_b200_t* h, int num_plants, int sensor_start, int n
     k->parameters.insert(k->parameters.end(), h->parameters.begin(), h->parameters.end());
     k->task_state.insert(k->task_state.end(), h->task_state.begin(), h->task_state.end());
   }
-  delete h->plants;
-  h->plants = k;
+  CUDA_TRY(cudaStreamSynchronize(h->stream));   // a step in flight may still use the old bank
+  h->plants = std::move(k);
   return 0;
 }
 
@@ -2081,7 +2024,7 @@ int mjpc_b200_spec_words(const mjpc_model_blob* model, int* out, int capacity) {
   }
 }
 void* mjpc_b200_stream(mjpc_b200_t* h) { return h ? (void*)h->stream : nullptr; }
-float* mjpc_b200_device_returns(mjpc_b200_t* h) { return h ? h->d_returns : nullptr; }
+float* mjpc_b200_device_returns(mjpc_b200_t* h) { return h ? h->d_returns.get() : nullptr; }
 
 // ---- iLQG entry points (kernels in ilqg_kernels.cuh).  Each single-problem call is the B = 1 case of its batched
 // twin: one staging path and one launch path per sweep.
@@ -2296,9 +2239,7 @@ int Init(mjpc_b200_t* h, const Desc& d) {
       return fail(MJPC_B200_ERR_UNSUPPORTED, "filter bank: sensor " + std::to_string(i) + ": " + h->sensor_why[i]);
   if ((int64_t)d.num_filters * d.rows > h->maxN) return fail(MJPC_B200_ERR_CAPACITY, "filter bank: rows above max_candidates");
   CUDA_TRY(cudaSetDevice(h->device));
-  delete h->bank;
-  h->bank = nullptr;
-  FilterBank* k = new FilterBank;
+  std::unique_ptr<FilterBank> k(new FilterBank);
   FilterBankArgs& a = k->a;
   std::memset(&a, 0, sizeof(a));
   a.nq = M.nq; a.nv = M.nv; a.nu = M.nu; a.nmocap = M.nmocap; a.njnt = d.njnt;
@@ -2327,13 +2268,12 @@ int Init(mjpc_b200_t* h, const Desc& d) {
                o_nv = take(R * nv * 4), o_res = take(R * nr * 4), o_cost = take(R * 4), o_counts = take(4 * R * 4),
                o_sens = take(R * ny * 4), o_scratch = take(B * scratch * 8);
   auto fail_k = [&](cudaError_t e) {
-    delete k;
     return fail(MJPC_B200_ERR_CUDA, std::string("filter bank: ") + cudaGetErrorString(e));
   };
-  if (cudaError_t e = cudaMalloc(&k->d_mem, bytes)) return fail_k(e);
+  if (cudaError_t e = k->d_mem.alloc(bytes)) return fail_k(e);
   if (cudaError_t e = cudaMemset(k->d_mem, 0, bytes)) return fail_k(e);
-  if (cudaError_t e = cudaMallocHost((void**)&k->h_stage, k->in_bytes + B * 4)) return fail_k(e);
-  unsigned char* base = (unsigned char*)k->d_mem;
+  if (cudaError_t e = k->h_stage.alloc(k->in_bytes + B * 4)) return fail_k(e);
+  unsigned char* base = k->d_mem;
   auto at = [&](size_t o) { return (void*)(base + o); };
   a.jnt = (const int*)at(o_jnt);
   a.state = (double*)at(o_state); a.P = (double*)at(o_P); a.time = (double*)at(o_time);
@@ -2358,7 +2298,8 @@ int Init(mjpc_b200_t* h, const Desc& d) {
   if (cudaError_t e = cudaMemcpy((void*)a.jnt, jnt.data(), jnt.size() * 4, cudaMemcpyHostToDevice)) return fail_k(e);
   if (nts)
     if (cudaError_t e = cudaMemcpy(k->d_task, ts.data(), nts * 4, cudaMemcpyHostToDevice)) return fail_k(e);
-  h->bank = k;
+  CUDA_TRY(cudaStreamSynchronize(h->stream));   // an update in flight may still use the old bank
+  h->bank = std::move(k);
   return 0;
 }
 

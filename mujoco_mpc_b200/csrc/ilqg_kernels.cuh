@@ -16,11 +16,13 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include <type_traits>
 #include <utility>
 #include <vector>
 
 #include <mutex>
 
+#include "device_memory.h"
 #include "rollout_kernels.cuh"
 
 namespace mjpc_dev {
@@ -874,7 +876,8 @@ inline void launch_kernel(const void* fn, dim3 grid, int block, size_t smem, cud
 }
 
 // Device buffers of the iLQG sweeps for up to `nprob` problems of max_horizon rows each (per-problem arrays are
-// [nprob][H][..]); sized for one problem at create, grown by ilqg_reserve when a batched sweep needs more.
+// [nprob][H][..]); sized for one problem at create, grown by ilqg_reserve when a batched sweep needs more.  The arrays
+// are carved from one owned allocation, every piece 256-byte aligned as an allocation of its own would be.
 struct IlqgBuffers {
   int H = 0, ds = 0, n = 0, nu = 0, nr = 0, nv = 0, nprob = 0;
   float *x = nullptr, *u = nullptr, *t = nullptr, *mocap = nullptr, *ts = nullptr, *w = nullptr, *prm = nullptr,
@@ -885,39 +888,36 @@ struct IlqgBuffers {
   double *gk = nullptr, *gdV = nullptr;   // gradient sweep: k [nprob][H][nu], dV0 [nprob]
   int* status = nullptr;
   int* idx = nullptr;   // [4 H]: evaluate list, then interpolate t / e0 / e1 (common to all problems)
-  std::vector<float**> all() {
-    return {&x, &u, &t, &mocap, &ts, &w, &prm, &y0, &r0, &q0, &A, &B, &C, &D, &res, &cx, &cu, &cxx, &cuu, &cxu, &act,
-            &K, &du, &dV, &Vx, &Vxx, &mu, &yp, &rp, &iw};
-  }
+  mjpc_mem::DeviceArray<unsigned char> mem;
 };
 
-inline void ilqg_free(IlqgBuffers& b) {
-  for (float** p : b.all()) if (*p) { cudaFree(*p); *p = nullptr; }
-  for (double** p : {&b.gk, &b.gdV}) if (*p) { cudaFree(*p); *p = nullptr; }
-  if (b.status) { cudaFree(b.status); b.status = nullptr; }
-  if (b.idx) { cudaFree(b.idx); b.idx = nullptr; }
-}
-
-// allocates everything for nprob problems; on failure the partly allocated buffers are freed and -4 returned
+// allocates everything for nprob problems into an empty b; on failure -4
 inline int ilqg_init(IlqgBuffers& b, const DevModel& M, int H, int nprob = 1) {
   b.H = H; b.nv = M.nv; b.ds = M.nq + M.nv; b.n = 2 * M.nv; b.nu = M.nu; b.nr = M.num_residual; b.nprob = nprob;
   const size_t Hs = H, n = b.n, m = b.nu, nr = b.nr, ds = b.ds, P = nprob;
-  struct { float** p; size_t cnt; } plan[] = {
-      {&b.x, P * Hs * ds}, {&b.u, P * Hs * m}, {&b.t, P * Hs}, {&b.mocap, P * 7 * (size_t)M.nmocap + 1},
-      {&b.ts, P * M.task_state_size + 1}, {&b.w, P * M.num_term + 1}, {&b.prm, P * M.num_parameters + 1},
-      {&b.y0, P * Hs * ds}, {&b.r0, P * Hs * nr}, {&b.q0, P * Hs * M.nv}, {&b.A, P * Hs * n * n}, {&b.B, P * Hs * n * m},
-      {&b.C, P * Hs * nr * n}, {&b.D, P * Hs * nr * m}, {&b.res, P * Hs * nr}, {&b.cx, P * Hs * n}, {&b.cu, P * Hs * m},
-      {&b.cxx, P * Hs * n * n}, {&b.cuu, P * Hs * m * m}, {&b.cxu, P * Hs * n * m}, {&b.act, P * Hs * m},
-      {&b.K, P * Hs * m * n}, {&b.du, P * Hs * m}, {&b.dV, 2 * P}, {&b.Vx, P * Hs * n}, {&b.Vxx, P * Hs * n * n},
-      {&b.mu, P}, {&b.yp, P * (Hs + 2) * (m + n) * ds}, {&b.rp, P * (Hs + 2) * (m + n) * nr + 1}, {&b.iw, Hs + 1}};
-  bool ok = true;
-  for (auto& e : plan)
-    ok = ok && cudaMalloc((void**)e.p, (e.cnt ? e.cnt : 1) * sizeof(float)) == cudaSuccess;
-  ok = ok && cudaMalloc((void**)&b.gk, P * Hs * m * sizeof(double)) == cudaSuccess;
-  ok = ok && cudaMalloc((void**)&b.gdV, P * sizeof(double)) == cudaSuccess;
-  ok = ok && cudaMalloc((void**)&b.status, P * sizeof(int)) == cudaSuccess;
-  ok = ok && cudaMalloc((void**)&b.idx, (4 * Hs + 8) * sizeof(int)) == cudaSuccess;
-  if (!ok) { cudaGetLastError(); ilqg_free(b); return -4; }
+  // two passes over the fields: the first sizes the allocation (base null), the second points each field into it
+  unsigned char* base = nullptr;
+  size_t bytes = 0;
+  auto take = [&](auto*& p, size_t count) {
+    using T = std::remove_reference_t<decltype(*p)>;
+    p = base ? reinterpret_cast<T*>(base + bytes) : nullptr;
+    bytes += (std::max<size_t>(count, 1) * sizeof(T) + 255) & ~(size_t)255;
+  };
+  auto carve = [&] {
+    take(b.x, P * Hs * ds); take(b.u, P * Hs * m); take(b.t, P * Hs); take(b.mocap, P * 7 * (size_t)M.nmocap + 1);
+    take(b.ts, P * M.task_state_size + 1); take(b.w, P * M.num_term + 1); take(b.prm, P * M.num_parameters + 1);
+    take(b.y0, P * Hs * ds); take(b.r0, P * Hs * nr); take(b.q0, P * Hs * M.nv); take(b.A, P * Hs * n * n);
+    take(b.B, P * Hs * n * m); take(b.C, P * Hs * nr * n); take(b.D, P * Hs * nr * m); take(b.res, P * Hs * nr);
+    take(b.cx, P * Hs * n); take(b.cu, P * Hs * m); take(b.cxx, P * Hs * n * n); take(b.cuu, P * Hs * m * m);
+    take(b.cxu, P * Hs * n * m); take(b.act, P * Hs * m); take(b.K, P * Hs * m * n); take(b.du, P * Hs * m);
+    take(b.dV, 2 * P); take(b.Vx, P * Hs * n); take(b.Vxx, P * Hs * n * n); take(b.mu, P);
+    take(b.yp, P * (Hs + 2) * (m + n) * ds); take(b.rp, P * (Hs + 2) * (m + n) * nr + 1); take(b.iw, Hs + 1);
+    take(b.gk, P * Hs * m); take(b.gdV, P); take(b.status, P); take(b.idx, 4 * Hs + 8);
+  };
+  carve();
+  if (b.mem.alloc(bytes)) return -4;
+  base = b.mem; bytes = 0;
+  carve();
   return 0;
 }
 
@@ -926,9 +926,8 @@ inline int ilqg_reserve(IlqgBuffers& b, const DevModel& M, int nprob, cudaStream
   if (nprob <= b.nprob) return 0;
   IlqgBuffers nb;
   if (int rc = ilqg_init(nb, M, b.H, nprob)) return rc;
-  if (cudaStreamSynchronize(st) != cudaSuccess) { cudaGetLastError(); ilqg_free(nb); return -4; }
-  ilqg_free(b);
-  b = nb;
+  if (cudaStreamSynchronize(st) != cudaSuccess) { cudaGetLastError(); return -4; }
+  b = std::move(nb);
   return 0;
 }
 

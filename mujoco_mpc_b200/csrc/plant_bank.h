@@ -18,23 +18,20 @@
 
 #include <vector>
 
+#include "device_memory.h"
 #include "rollout_kernels.cuh"
 
 struct PlantBank {
   mjpc_dev::PlantArgs a;   // device pointers into d_mem; the launch fills in the model, the pack and the instance
   int nsd = 0;             // sensor dimension of the plants' sensor range (0: no sensors)
-  void* d_mem = nullptr;
+  mjpc_mem::DeviceArray<unsigned char> d_mem;
   unsigned char* d_in = nullptr;    // the upload
   unsigned char* d_out = nullptr;   // the outputs
-  unsigned char* h_stage = nullptr; // pinned: [upload][outputs]
+  mjpc_mem::PinnedArray<unsigned char> h_stage;   // [upload][outputs]
   size_t in_bytes = 0, out_bytes = 0;
   size_t o_ctrl = 0, o_mocap = 0, o_ts = 0, o_weight = 0, o_par = 0;                   // within the upload
   size_t o_time = 0, o_state = 0, o_cost = 0, o_status = 0, o_sens = 0, o_ctrl_out = 0;  // within the outputs
   std::vector<float> mocap;                                   // [B][7 nmocap]
   std::vector<mjpc_dev::PlantDisturbance> dist;               // [B], as on the device
   std::vector<double> weight, parameters, task_state, time;   // [B][..], task state in absolute time; time [B]
-  ~PlantBank() {
-    if (d_mem) cudaFree(d_mem);
-    if (h_stage) cudaFreeHost(h_stage);
-  }
 };

@@ -39,4 +39,9 @@ if which in ("all", "humanoid"):
     eh.rollout_spline(sh, 0.0, mc, kh, np.arange(16) * 0.003, 2, 8)
     del os.environ["MJPC_B200_NO_STATIC"]
     g = eh.step_debug(mh.qpos0, np.zeros(mh.nv), np.zeros(mh.nu), mc)
+if which in ("all", "growth"):                                               # every grow path; closes its handles
+    import test_gpu_buffer_growth as growth
+    for name in dir(growth):
+        if name.startswith("test_"):
+            getattr(growth, name)()
 print("sanitize run done:", which)
