@@ -194,6 +194,17 @@ int mjpc_b200_fetch_trajectory_member(mjpc_b200_t* h, int candidate, int member,
  * device computes (for tests).  Nothing is written unless 1 <= K <= 32 and 1 <= worst <= K. */
 void mjpc_b200_host_ensemble_score(const float* member_returns, const uint8_t* member_failure, int K, int worst,
                                    float* score, uint8_t* failure);
+/* Test hooks: the device's candidate ranking and ensemble score on caller data, with the launch shapes of a rollout
+ * launch, on the handle's stream; the last launch's returns, order and trajectories are untouched.
+ * debug_rank: returns [nseg][N] -> order [nseg][N], each segment's indices by ascending return (ties to the lower
+ *   index, NaN last); order is filled with -1 before the launch, so a slot the ranking misses reads -1.
+ * debug_ensemble_score: member_returns / member_failure [B][K][N] -> returns / failure [B][N], the score of
+ *   set_model_ensemble with `worst`.
+ * nseg, N, B < 1, K outside [1, 32], worst outside [1, K] or a NULL pointer: MJPC_B200_ERR_BAD_ARGUMENT, nothing
+ * launched and the handle usable. */
+int mjpc_b200_debug_rank(mjpc_b200_t* h, const float* returns, int nseg, int N, int* order);
+int mjpc_b200_debug_ensemble_score(mjpc_b200_t* h, const float* member_returns, const uint8_t* member_failure, int B,
+                                   int K, int N, int worst, float* returns, uint8_t* failure);
 
 /* An initial-state ensemble: rollout_spline_batched with every candidate scored over K initial states drawn from each
  * problem's state covariance, so that a candidate that does well only from the exact mean state does not win when the

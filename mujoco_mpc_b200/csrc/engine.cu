@@ -7,6 +7,7 @@
 #include <nccl.h>   // types only: the NCCL entry points are bound with dlopen at comm_init (no link-time dependency)
 
 #include <algorithm>
+#include <climits>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
@@ -1373,6 +1374,45 @@ void mjpc_b200_host_ensemble_score(const float* member_returns, const uint8_t* m
   for (int p = 0; p < worst; p++) sum += (double)r[at[p]];
   *score = failed ? 1.0e6f : (float)(sum / (double)worst);
   *failure = failed ? 1 : 0;
+}
+
+// Test hooks: rank_kernel and ensemble_score_kernel on the caller's data, launched as launch_rollout launches them, on
+// the handle's stream and in scratch of their own (the last launch's buffers are untouched).
+int mjpc_b200_debug_rank(mjpc_b200_t* h, const float* returns, int nseg, int N, int* order) {
+  if (!h || !returns || !order || nseg < 1 || N < 1 || (long long)nseg * N > INT_MAX / 2)
+    return fail(MJPC_B200_ERR_BAD_ARGUMENT, "debug_rank: bad argument");
+  const size_t n = (size_t)nseg * N;
+  CUDA_TRY(cudaSetDevice(h->device));
+  DeviceArray<float> d_ret;
+  DeviceArray<int> d_order;
+  CUDA_TRY(d_ret.alloc(n)); CUDA_TRY(d_order.alloc(n));
+  CUDA_TRY(cudaMemcpyAsync(d_ret, returns, n * 4, cudaMemcpyHostToDevice, h->stream));
+  CUDA_TRY(cudaMemsetAsync(d_order, 0xFF, n * 4, h->stream));   // -1: a slot the kernel does not write stays visible
+  rank_kernel<<<(int)((n + 255) / 256), 256, 0, h->stream>>>(d_ret, N, nseg, d_order);
+  CUDA_TRY(cudaGetLastError());
+  CUDA_TRY(cudaMemcpyAsync(order, d_order, n * 4, cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(cudaStreamSynchronize(h->stream));
+  return 0;
+}
+
+int mjpc_b200_debug_ensemble_score(mjpc_b200_t* h, const float* member_returns, const uint8_t* member_failure, int B,
+                                   int K, int N, int worst, float* returns, uint8_t* failure) {
+  if (!h || !member_returns || !member_failure || !returns || !failure || B < 1 || N < 1 || K < 1 || K > 32 ||
+      worst < 1 || worst > K || (long long)B * K * N > INT_MAX / 32)
+    return fail(MJPC_B200_ERR_BAD_ARGUMENT, "debug_ensemble_score: bad argument");
+  const size_t n = (size_t)B * N, nm = n * K;
+  CUDA_TRY(cudaSetDevice(h->device));
+  DeviceArray<float> d_mr, d_ret;
+  DeviceArray<unsigned char> d_mf, d_fail;
+  CUDA_TRY(d_mr.alloc(nm)); CUDA_TRY(d_mf.alloc(nm)); CUDA_TRY(d_ret.alloc(n)); CUDA_TRY(d_fail.alloc(n));
+  CUDA_TRY(cudaMemcpyAsync(d_mr, member_returns, nm * 4, cudaMemcpyHostToDevice, h->stream));
+  CUDA_TRY(cudaMemcpyAsync(d_mf, member_failure, nm, cudaMemcpyHostToDevice, h->stream));
+  ensemble_score_kernel<<<(int)((n + 7) / 8), 256, 0, h->stream>>>(d_mr, d_mf, B, K, N, worst, d_ret, d_fail);
+  CUDA_TRY(cudaGetLastError());
+  CUDA_TRY(cudaMemcpyAsync(returns, d_ret, n * 4, cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(cudaMemcpyAsync(failure, d_fail, n, cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(cudaStreamSynchronize(h->stream));
+  return 0;
 }
 
 // grow step_impl's device scratch and pinned staging to `words` floats each (never shrinks); on failure the old ones stay

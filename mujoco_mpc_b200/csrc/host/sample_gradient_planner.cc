@@ -153,12 +153,15 @@ void SampleGradientPlanner::GradientCandidates(int num_trajectory, int num_gradi
   gradient_previous = gradient;
   // fitness shaping (planner.cc:417-450), restated with its quirks (DESIGN.md §8): the weights are cached while the
   // number of noisy samples is unchanged, and on the call that computes them they are indexed by candidate index
-  // (order[i] + 1), not by rank
+  // (order[i] + 1), not by rank.  NaN returns sort after every number, as the device ranking puts them: a bare `<`
+  // is no strict weak ordering once a NaN is present, and left NaN candidates where they stood
   if ((int)return_weight_.size() != num_noisy) {
     return_weight_.resize(num_noisy);
     std::iota(trajectory_order.begin(), trajectory_order.begin() + num_noisy, 0);
-    std::stable_sort(trajectory_order.begin(), trajectory_order.begin() + num_noisy,
-                     [&](int a, int b) { return returns_[a] < returns_[b]; });
+    std::stable_sort(trajectory_order.begin(), trajectory_order.begin() + num_noisy, [&](int a, int b) {
+      const float ra = returns_[a], rb = returns_[b];
+      return ra < rb || (rb != rb && ra == ra);
+    });
     const double f0 = std::log(0.5 * num_noisy + 1.0);
     double den = 0.0;
     for (int i = 0; i < num_noisy; i++) den += std::max(0.0, f0 - std::log(trajectory_order[i] + 1));

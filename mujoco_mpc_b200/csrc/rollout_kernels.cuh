@@ -467,7 +467,8 @@ inline bool spec_matches(const DevModel& M, const DevLayout& L, const int* dof_p
   return true;
 }
 
-// nseg segments of N returns: order[b][rank] = i, the index within segment b, ascending return, ties broken by index
+// nseg segments of N returns: order[b][rank] = i, the index within segment b, ascending return, ties broken by index,
+// NaN after every number and NaNs among themselves by index (numpy's stable argsort), so every segment is a permutation
 extern "C" __global__ void rank_kernel(const float* __restrict__ ret, int N, int nseg, int* __restrict__ order) {
   for (int g = blockIdx.x * blockDim.x + threadIdx.x; g < nseg * N; g += gridDim.x * blockDim.x) {
     const int b = g / N, i = g - b * N;
@@ -476,7 +477,7 @@ extern "C" __global__ void rank_kernel(const float* __restrict__ ret, int N, int
     int rank = 0;
     for (int j = 0; j < N; j++) {
       const float rj = r[j];
-      rank += (rj < ri) || (rj == ri && j < i) || (ri != ri && rj == rj);
+      rank += (rj < ri) || (rj == ri && j < i) || (ri != ri && (rj == rj || j < i));
     }
     order[(size_t)b * N + rank] = i;
   }

@@ -588,6 +588,25 @@ class Engine:
         o["contact"] = con[: min(n.value, 64)]
         return o
 
+    def debug_rank(self, returns):
+        """The device ranking of returns [nseg, N] (mjpc_b200_debug_rank): order [nseg, N], -1 where no index landed."""
+        r = np.ascontiguousarray(np.atleast_2d(returns), np.float32)
+        nseg, N = r.shape
+        order = np.zeros((nseg, N), np.int32)
+        self._check(self.lib.mjpc_b200_debug_rank(self.h, _pf(r), int(nseg), int(N), order.ctypes.data_as(_ip)))
+        return order
+
+    def debug_ensemble_score(self, member_returns, member_failure, worst):
+        """The device ensemble score of member returns / failure flags [B, K, N] (mjpc_b200_debug_ensemble_score):
+        (returns [B, N], failure [B, N])."""
+        r = np.ascontiguousarray(member_returns, np.float32)
+        f = np.ascontiguousarray(member_failure, np.uint8)
+        B, K, N = r.shape
+        ret, fail = np.zeros((B, N), np.float32), np.zeros((B, N), np.uint8)
+        self._check(self.lib.mjpc_b200_debug_ensemble_score(self.h, _pf(r), f.ctypes.data_as(_bp), int(B), int(K), int(N),
+                                                            int(worst), _pf(ret), fail.ctypes.data_as(_bp)))
+        return ret, fail
+
     def step_batch(self, qpos, qvel, ctrl, mocap, times, time0=0.0, warmstart=None):
         """B independent single steps (mjpc_b200_step_batch): teacher-forced per-step parity at planner sizes."""
         q, v, u, mc, ws, t = _f(qpos), _f(qvel), _f(ctrl), _f(mocap), _f(warmstart), _d(times)
