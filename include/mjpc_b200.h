@@ -473,8 +473,11 @@ int mjpc_b200_plant_last_ctrl(mjpc_b200_t* h, float* ctrl_out);
  *   set_noise  process [ndstate], sensor [nsensordata] (NULL keeps one)
  *   set        state, covariance [ndstate^2] (NULL keeps one) and time
  *   update     one filter update from ctrl [nu], the measured sensor slice [nsensordata] and mocap [7 nmocap] or NULL
- *              (the model's).  A failed factorisation returns MJPC_B200_ERR_BAD_ARGUMENT and leaves state, covariance
- *              and time untouched; last_error names the factor.
+ *              (the model's).  A failed factorisation (a pivot below 1e-15 or not finite) or a new state or
+ *              covariance that would not be finite returns MJPC_B200_ERR_BAD_ARGUMENT and leaves state, covariance
+ *              and time untouched; last_error names the factor, or says "non-finite result".
+ * reset, set_noise, set and update refuse a value that is not finite with MJPC_B200_ERR_BAD_ARGUMENT and change
+ * nothing.
  *   get        state [nq+nv], covariance, time and the kind's scalars (any pointer may be NULL) */
 typedef struct mjpc_b200_estimator mjpc_b200_estimator_t;
 int mjpc_b200_estimator_destroy(mjpc_b200_estimator_t* f);
@@ -529,8 +532,10 @@ int mjpc_b200_kalman_update_prediction(mjpc_b200_estimator_t* f);
  *   set        filter b's state, covariance [ndstate^2] (NULL keeps one) and time
  *   update     every filter from ctrl [num_filters][nu], sensor [num_filters][nsensordata] and mocap
  *              [num_filters][7 nmocap] (NULL: the model's for every filter).  status [num_filters]: 0, or
- *              MJPC_B200_ERR_BAD_ARGUMENT where a factorisation failed, which leaves that filter's state, covariance,
- *              time, warm start and warnings untouched; the other filters update normally
+ *              MJPC_B200_ERR_BAD_ARGUMENT where a factorisation failed or the new state or covariance would not be
+ *              finite, which leaves that filter's state, covariance, time, warm start and warnings untouched; the
+ *              other filters update normally.  A ctrl, sensor or mocap value that is not finite refuses the whole call
+ *              (MJPC_B200_ERR_BAD_ARGUMENT, nothing changed), as reset, set_noise and set refuse theirs
  *   get        filter b's state [nq+nv], covariance, time and the scalars of the single filter of its kind (Unscented
  *              5, Kalman 6; any pointer may be NULL)
  * Calls that take a filter index return MJPC_B200_ERR_BAD_ARGUMENT when it is outside [0, num_filters), and every call
@@ -546,6 +551,22 @@ int mjpc_b200_batch_estimator_update(void* f, const double* ctrl, const double* 
                                      int* status);
 int mjpc_b200_batch_estimator_get(void* f, int filter, double* state, double* covariance, double* time,
                                   double* scalars);
+/* Test hooks: the bank's own kernels on the caller's data, with the bank's launch shape and stream.  phase: 0 the
+ * Unscented sigma points, 1 the Kalman measurement, 2 the Kalman prediction (another phase than the kind's:
+ * MJPC_B200_ERR_BAD_ARGUMENT).  status [num_filters] is the raw filter status: 0 updated, 1 sensor-covariance factor
+ * failed, 2 covariance factor failed, 3 non-finite result.
+ *   debug_rows    stages ctrl [num_filters][nu] and mocap (NULL: the model's) as update does and runs the row kernel:
+ *                 qpos [num_filters rows][nq], qvel [num_filters rows][nv] and warm [num_filters rows][nv] are the step
+ *                 launch's input rows and warm starts; phases 0 and 1 set status, phase 2 leaves the last one
+ *   debug_finish  stages sensor [num_filters][nsensordata] (phase 2: may be NULL), clears every status, writes
+ *                 next_qpos, next_qvel, qacc [num_filters rows][nv], sensordata [num_filters rows][nsensordata] and
+ *                 counts [num_filters rows][4] where the step launch writes them and runs the phase's update kernel,
+ *                 which commits into the filters as update does */
+int mjpc_b200_batch_estimator_debug_rows(void* f, int phase, const double* ctrl, const float* mocap, float* qpos,
+                                         float* qvel, float* warm, int* status);
+int mjpc_b200_batch_estimator_debug_finish(void* f, int phase, const double* sensor, const float* next_qpos,
+                                           const float* next_qvel, const float* qacc, const float* sensordata,
+                                           const int* counts, int* status);
 /* Filter b runs on models[b] from now on: mjpc_b200_set_model_variants on the bank's engine handle, with its rule and
  * refusals; a NULL-state reset and a NULL mocap then use filter b's model's first keyframe / qpos0 and mocap poses.
  * count must be num_filters, or 0 to run every filter on the bank's model again.  The filters' states are kept. */

@@ -2385,54 +2385,114 @@ static int step_rows(mjpc_b200_t* h, const KernelSet* ks) {
   return 0;
 }
 
+// the update inputs into the bank: sensor [B][ny], ctrl [B][nu], mocap [B][7 nmocap]; a NULL one keeps what the last
+// staging left
+static int stage_inputs(mjpc_b200_t* h, const float* ctrl, const double* sensor, const float* mocap) {
+  FilterBank& k = *h->bank;
+  const FilterBankArgs& a = k.a;
+  const size_t B = a.B, ny = a.ny, nu = a.nu, nm = 7 * (size_t)a.nmocap;
+  CUDA_TRY(cudaSetDevice(h->device));
+  CUDA_TRY(cudaStreamSynchronize(h->stream));   // the staging may still feed an earlier copy
+  if (sensor) std::memcpy(k.h_stage, sensor, B * ny * 8);
+  if (nu && ctrl) std::memcpy(k.h_stage + B * ny * 8, ctrl, B * nu * 4);
+  if (nm && mocap) std::memcpy(k.h_stage + B * ny * 8 + B * nu * 4, mocap, B * nm * 4);
+  CUDA_TRY(cudaMemcpyAsync(k.d_in, k.h_stage, k.in_bytes, cudaMemcpyHostToDevice, h->stream));
+  return 0;
+}
+
+// The kernels of one phase (0 Unscented, 1 Kalman measurement, 2 Kalman prediction) on every filter: the step rows
+// before the step launch, and the update after it
+static void run_filter_kernel(mjpc_b200_t* h, int phase, const void* fn) {
+  FilterBankArgs a = h->bank->a;
+  a.phase = phase;
+  void* args[] = {&a};
+  cudaLaunchKernel(fn, dim3(a.B), dim3(kFilterThreads), args, 0, h->stream);
+  h->launches += 1;
+}
+static void launch_phase_rows(mjpc_b200_t* h, int phase) { run_filter_kernel(h, phase, (const void*)estimator_rows_kernel); }
+static void launch_phase_update(mjpc_b200_t* h, int phase) {
+  run_filter_kernel(h, phase, phase == 0 ? (const void*)unscented_update_kernel
+                              : phase == 1 ? (const void*)kalman_measurement_kernel : (const void*)kalman_prediction_kernel);
+}
+
+// the statuses [B] of the last kernels, after the stream's work
+static int read_status(mjpc_b200_t* h, int* status) {
+  FilterBank& k = *h->bank;
+  CUDA_TRY(cudaGetLastError());
+  int* st = (int*)(k.h_stage + k.in_bytes);
+  CUDA_TRY(cudaMemcpyAsync(st, k.a.status, k.a.B * 4, cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(cudaStreamSynchronize(h->stream));
+  std::copy(st, st + k.a.B, status);
+  return 0;
+}
+
 int Update(mjpc_b200_t* h, const float* ctrl, const double* sensor, const float* mocap, int phases, int* status) {
   if (!h || !h->bank || phases < MEASUREMENT || phases > MEASUREMENT_AND_PREDICTION || (!ctrl && h->pack.M.nu) ||
       (!sensor && (h->bank->a.kind == kFilterUnscented || (phases & MEASUREMENT))) || (!mocap && h->pack.M.nmocap) ||
       !status)
     return fail(MJPC_B200_ERR_BAD_ARGUMENT, "filter bank update: bad argument");
-  FilterBank& k = *h->bank;
-  FilterBankArgs a = k.a;
+  const FilterBankArgs& a = h->bank->a;
   if (int rc = check_variants(h, a.B, "filter bank update")) return rc;
   if (int rc = check_ensemble(h, "filter bank update")) return rc;
-  const size_t B = a.B, ny = a.ny, nu = a.nu, nm = 7 * (size_t)a.nmocap;
-  CUDA_TRY(cudaSetDevice(h->device));
-  CUDA_TRY(cudaStreamSynchronize(h->stream));   // the staging may still feed an earlier copy
-  if (sensor) std::memcpy(k.h_stage, sensor, B * ny * 8);
-  if (nu) std::memcpy(k.h_stage + B * ny * 8, ctrl, B * nu * 4);
-  if (nm) std::memcpy(k.h_stage + B * ny * 8 + B * nu * 4, mocap, B * nm * 4);
-  CUDA_TRY(cudaMemcpyAsync(k.d_in, k.h_stage, k.in_bytes, cudaMemcpyHostToDevice, h->stream));
+  if (int rc = stage_inputs(h, ctrl, sensor, mocap)) return rc;
   const KernelSet* ks;
   const int kind = pick_kernels(h, &ks);
-  auto run = [&](const void* fn) {
-    void* args[] = {&a};
-    cudaLaunchKernel(fn, dim3(a.B), dim3(kFilterThreads), args, 0, h->stream);
-    h->launches += 1;
+  auto run = [&](int phase) {
+    launch_phase_rows(h, phase);
+    step_rows(h, ks);
+    launch_phase_update(h, phase);
   };
   if (a.kind == kFilterUnscented) {
-    a.phase = 0; run((const void*)estimator_rows_kernel);
-    step_rows(h, ks);
-    run((const void*)unscented_update_kernel);
+    run(0);
   } else {
     if (phases & MEASUREMENT) {
-      a.phase = 1; run((const void*)estimator_rows_kernel);
-      step_rows(h, ks);
-      run((const void*)kalman_measurement_kernel);
+      run(1);
     } else {   // the prediction skips a failed filter: clear the statuses an earlier update left
-      CUDA_TRY(cudaMemsetAsync(a.status, 0, B * 4, h->stream));
+      CUDA_TRY(cudaMemsetAsync(a.status, 0, a.B * 4, h->stream));
     }
-    if (phases & PREDICTION) {
-      a.phase = 2; run((const void*)estimator_rows_kernel);
-      step_rows(h, ks);
-      run((const void*)kalman_prediction_kernel);
-    }
+    if (phases & PREDICTION) run(2);
   }
-  CUDA_TRY(cudaGetLastError());
-  int* st = (int*)(k.h_stage + k.in_bytes);
-  CUDA_TRY(cudaMemcpyAsync(st, a.status, B * 4, cudaMemcpyDeviceToHost, h->stream));
-  CUDA_TRY(cudaStreamSynchronize(h->stream));
-  std::copy(st, st + B, status);
+  if (int rc = read_status(h, status)) return rc;
   h->last_static = kind ? 1 : 0;
   return 0;
+}
+
+// whether the bank's kind runs `phase`
+static bool bank_phase(const mjpc_b200_t* h, int phase) {
+  return h && h->bank && (h->bank->a.kind == kFilterUnscented ? phase == 0 : phase == 1 || phase == 2);
+}
+
+int DebugRows(mjpc_b200_t* h, int phase, const float* ctrl, const float* mocap, float* qpos, float* qvel, float* warm,
+              int* status) {
+  if (!bank_phase(h, phase) || (!ctrl && h->pack.M.nu) || (!mocap && h->pack.M.nmocap) || !qpos || !qvel || !warm ||
+      !status)
+    return fail(MJPC_B200_ERR_BAD_ARGUMENT, "filter bank debug_rows: bad argument");
+  const FilterBankArgs& a = h->bank->a;
+  const size_t R = (size_t)a.B * a.rows;
+  if (int rc = stage_inputs(h, ctrl, nullptr, mocap)) return rc;
+  launch_phase_rows(h, phase);
+  CUDA_TRY(cudaMemcpyAsync(qpos, a.qpos, R * a.nq * 4, cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(cudaMemcpyAsync(qvel, a.qvel, R * a.nv * 4, cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(cudaMemcpyAsync(warm, a.rwarm, R * a.nv * 4, cudaMemcpyDeviceToHost, h->stream));
+  return read_status(h, status);
+}
+
+int DebugFinish(mjpc_b200_t* h, int phase, const double* sensor, const float* next_qpos, const float* next_qvel,
+                const float* qacc, const float* sensordata, const int* counts, int* status) {
+  if (!bank_phase(h, phase) || (!sensor && phase < 2) || !next_qpos || !next_qvel || !qacc || !sensordata || !counts ||
+      !status)
+    return fail(MJPC_B200_ERR_BAD_ARGUMENT, "filter bank debug_finish: bad argument");
+  const FilterBankArgs& a = h->bank->a;
+  const size_t R = (size_t)a.B * a.rows;
+  if (int rc = stage_inputs(h, nullptr, sensor, nullptr)) return rc;
+  CUDA_TRY(cudaMemsetAsync(a.status, 0, a.B * 4, h->stream));
+  CUDA_TRY(cudaMemcpyAsync((void*)a.next_qpos, next_qpos, R * a.nq * 4, cudaMemcpyHostToDevice, h->stream));
+  CUDA_TRY(cudaMemcpyAsync((void*)a.next_qvel, next_qvel, R * a.nv * 4, cudaMemcpyHostToDevice, h->stream));
+  CUDA_TRY(cudaMemcpyAsync((void*)a.qacc, qacc, R * a.nv * 4, cudaMemcpyHostToDevice, h->stream));
+  CUDA_TRY(cudaMemcpyAsync((void*)a.sensordata, sensordata, R * a.ny * 4, cudaMemcpyHostToDevice, h->stream));
+  CUDA_TRY(cudaMemcpyAsync((void*)a.counts, counts, R * 4 * 4, cudaMemcpyHostToDevice, h->stream));
+  launch_phase_update(h, phase);
+  return read_status(h, status);
 }
 
 }  // namespace mjpc_b200_bank

@@ -8,16 +8,20 @@
 //
 //   estimator_rows_kernel      the step inputs of every row: state, ctrl, warm start and mocap of its filter
 //                              (Unscented: the Cholesky factor of P first; a factor that is not full rank fails the
-//                              filter)
+//                              filter: a pivot below 1e-15 or not finite)
 //   step_batch_kernel*         one launch of all B rows (engine.cu), the measurement sensors of each pre-step state
 //   unscented_update_kernel    means, QuaternionMeans, differences, covariances, gain update, state and time
 //   kalman_measurement_kernel  C, S = C P C' + R, gain update, correction
 //   kalman_prediction_kernel   A, P = A P A' + Q, the centre's next state, time
 //
-// A failed factorisation sets status[b] to the factor's mjpc_b200_bank::Status and leaves filter b's state,
-// covariance, time, warm start and warnings untouched; the other filters do not depend on it.
+// A failed factorisation sets status[b] to the factor's mjpc_b200_bank::Status, and an update whose new state or
+// covariance is not finite sets NONFINITE_RESULT; either leaves filter b's state, covariance, time, warm start and
+// warnings untouched, and the other filters do not depend on it.  Every update is formed in scratch (the new state,
+// o_Pn the new covariance) and committed only once all of it is finite.
 #pragma once
 #include <cuda_runtime.h>
+
+#include <cfloat>
 
 #include "filter_bank.h"
 
@@ -46,7 +50,7 @@ struct FilterBankArgs {
   // per filter scratch [scratch_words] and its offsets
   double* scratch;
   size_t scratch_words;
-  int o_F, o_mean, o_ymean, o_ds, o_dy, o_S, o_X, o_P0, o_T, o_C, o_e, o_corr, o_rows;
+  int o_F, o_mean, o_ymean, o_ds, o_dy, o_S, o_X, o_P0, o_T, o_C, o_e, o_corr, o_rows, o_Pn;
 };
 
 // the per-filter scratch offsets (doubles) for ndstate ns, nx = nq + nv, ny sensor values and R rows; returns the total
@@ -57,7 +61,7 @@ inline size_t filter_scratch_layout(FilterBankArgs& a) {
   a.o_F = take((size_t)ns * ns); a.o_mean = take(nx); a.o_ymean = take(ny); a.o_ds = take((size_t)R * ns);
   a.o_dy = take((size_t)R * ny); a.o_S = take((size_t)ny * ny); a.o_X = take((size_t)ns * ny);
   a.o_P0 = take((size_t)ns * ns); a.o_T = take((size_t)ns * ny); a.o_C = take((size_t)ny * ns); a.o_e = take(ny);
-  a.o_corr = take(ns); a.o_rows = take((size_t)R * nx);
+  a.o_corr = take(ns); a.o_rows = take((size_t)R * nx); a.o_Pn = take((size_t)ns * ns);
   a.scratch_words = w;
   return w;
 }
@@ -145,7 +149,8 @@ __device__ inline void fb_state_diff(const FilterBankArgs& A, double* dx, const 
 
 // ------------------------------------------------------------------------------------------ block-wide linear algebra
 // CholFactor (mju_cholFactor) of the row-major n x n M in place, pivots below mindiag raised to it; every thread gets
-// the rank.  Column j: thread 0 forms the pivot, then the rows below it in parallel, each summed serially.
+// the rank, which counts the pivots >= mindiag that are finite (a NaN or infinite pivot is raised to mindiag and not
+// counted).  Column j: thread 0 forms the pivot, then the rows below it in parallel, each summed serially.
 __device__ inline int fb_chol_factor(double* M, int n, double mindiag) {
   __shared__ int rank;
   if (threadIdx.x == 0) rank = 0;
@@ -153,7 +158,7 @@ __device__ inline int fb_chol_factor(double* M, int n, double mindiag) {
     if (threadIdx.x == 0) {
       double d = M[(size_t)j * n + j];
       for (int k = 0; k < j; k++) d = dsub(d, dmul(M[(size_t)j * n + k], M[(size_t)j * n + k]));
-      if (d < mindiag) d = mindiag; else rank++;
+      if (d >= mindiag && d <= DBL_MAX) rank++; else d = mindiag;
       M[(size_t)j * n + j] = sqrt(d);
     }
     __syncthreads();
@@ -182,6 +187,13 @@ __device__ inline void fb_chol_solve(const double* L, int n, double* x) {
     for (int k = i + 1; k < n; k++) a = dsub(a, dmul(L[(size_t)k * n + i], x[k]));
     x[i] = a / L[(size_t)i * n + i];
   }
+}
+
+// true on every thread when the n values v are all finite
+__device__ inline bool fb_all_finite(const double* v, int n) {
+  int bad = 0;
+  for (int i = threadIdx.x; i < n; i += blockDim.x) bad |= !(fabs(v[i]) <= DBL_MAX);
+  return !__syncthreads_or(bad);
 }
 
 // P [n]^2 = (P + P') / 2, each pair by one thread
@@ -276,8 +288,19 @@ __device__ inline void fb_load_next(const FilterBankArgs& A, int b, double* rows
   __syncthreads();
 }
 
-// After a successful update (estimator.py _Filter._commit): the warm start from row `centre`, the rows' warnings
-__device__ inline void fb_commit(const FilterBankArgs& A, int b, int centre) {
+// After a successful update (estimator.py _Filter._commit): the new state x [nq+nv] and covariance Pn [ndstate^2] from
+// scratch when both are finite (else status NONFINITE_RESULT and nothing is written), then time += timestep when
+// `advance`, the warm start from row `centre` and the rows' warnings.  true when committed.
+__device__ inline bool fb_commit(const FilterBankArgs& A, int b, const double* x, const double* Pn, bool advance,
+                                 int centre) {
+  const int nx = A.nq + A.nv, ns = 2 * A.nv;
+  if (!fb_all_finite(x, nx) || !fb_all_finite(Pn, ns * ns)) {
+    if (threadIdx.x == 0) A.status[b] = mjpc_b200_bank::NONFINITE_RESULT;
+    return false;
+  }
+  for (int k = threadIdx.x; k < nx; k += blockDim.x) A.state[(size_t)b * nx + k] = x[k];
+  for (int k = threadIdx.x; k < ns * ns; k += blockDim.x) A.P[(size_t)b * ns * ns + k] = Pn[k];
+  if (advance && threadIdx.x == 0) A.time[b] = dadd(A.time[b], A.timestep);
   const size_t row0 = (size_t)b * A.rows;
   for (int k = threadIdx.x; k < A.nv; k += blockDim.x) A.warm[(size_t)b * A.nv + k] = A.qacc[(row0 + centre) * A.nv + k];
   if (threadIdx.x == 0) {
@@ -285,6 +308,7 @@ __device__ inline void fb_commit(const FilterBankArgs& A, int b, int centre) {
     for (int i = 0; i < A.rows; i++) w += A.counts[4 * (row0 + i) + 3] != 0;
     A.warnings[b] += w;
   }
+  return true;
 }
 
 // -------------------------------------------------------------------------------------------------------- kernels
@@ -396,25 +420,22 @@ extern "C" __global__ void __launch_bounds__(kFilterThreads) unscented_update_ke
   }
   for (int k = threadIdx.x; k < ny; k += blockDim.x) e[k] = dsub(A.sensor[(size_t)b * ny + k], ymean[k]);
   __syncthreads();
-  double* P = A.P + (size_t)b * ns * ns;
-  if (!fb_gain_update(csy, cyy, e, css, corr, P, W + A.o_T, ns, ny)) {
+  double* Pn = W + A.o_Pn;
+  if (!fb_gain_update(csy, cyy, e, css, corr, Pn, W + A.o_T, ns, ny)) {
     if (threadIdx.x == 0) A.status[b] = mjpc_b200_bank::SENSOR_FACTOR_FAILED;
     return;
   }
-  if (threadIdx.x == 0) {
-    double* x = A.state + (size_t)b * nx;
-    for (int k = 0; k < nx; k++) x[k] = mean[k];
-    fb_state_add(A, x, [&](int j) { return corr[j]; }, 1.0);
-    A.time[b] = dadd(A.time[b], A.timestep);
-  }
-  fb_commit(A, b, R - 1);
+  if (threadIdx.x == 0) fb_state_add(A, mean, [&](int j) { return corr[j]; }, 1.0);   // mean becomes the new state
+  __syncthreads();
+  fb_commit(A, b, mean, Pn, true, R - 1);
 }
 
 // Kalman.update_measurement (kalman.cc UpdateMeasurement) after the measurement launch
 extern "C" __global__ void __launch_bounds__(kFilterThreads) kalman_measurement_kernel(const __grid_constant__ FilterBankArgs A) {
   const int b = blockIdx.x, nv = A.nv, nx = A.nq + nv, ns = 2 * nv, ny = A.ny;
   double* W = A.scratch + (size_t)b * A.scratch_words;
-  double *Cm = W + A.o_C, *PCt = W + A.o_X, *S = W + A.o_S, *e = W + A.o_e, *corr = W + A.o_corr;
+  double *Cm = W + A.o_C, *PCt = W + A.o_X, *S = W + A.o_S, *e = W + A.o_e, *corr = W + A.o_corr, *x = W + A.o_mean,
+         *Pn = W + A.o_Pn;
   double* P = A.P + (size_t)b * ns * ns;
   const float* y = A.sensordata + (size_t)b * A.rows * ny;
   const double h = A.centered ? 2 * A.epsilon : A.epsilon;
@@ -440,13 +461,15 @@ extern "C" __global__ void __launch_bounds__(kFilterThreads) kalman_measurement_
     S[k] = dadd(a, r == c ? A.noise_sensor[(size_t)b * ny + r] : 0.0);
   }
   for (int k = threadIdx.x; k < ny; k += blockDim.x) e[k] = dsub(A.sensor[(size_t)b * ny + k], (double)y[k]);
+  for (int k = threadIdx.x; k < nx; k += blockDim.x) x[k] = A.state[(size_t)b * nx + k];
   __syncthreads();
-  if (!fb_gain_update(PCt, S, e, P, corr, P, W + A.o_T, ns, ny)) {
+  if (!fb_gain_update(PCt, S, e, P, corr, Pn, W + A.o_T, ns, ny)) {
     if (threadIdx.x == 0) A.status[b] = mjpc_b200_bank::SENSOR_FACTOR_FAILED;
     return;
   }
-  if (threadIdx.x == 0) fb_state_add(A, A.state + (size_t)b * nx, [&](int j) { return corr[j]; }, 1.0);
-  fb_commit(A, b, 0);
+  if (threadIdx.x == 0) fb_state_add(A, x, [&](int j) { return corr[j]; }, 1.0);
+  __syncthreads();
+  fb_commit(A, b, x, Pn, false, 0);
 }
 
 // Kalman.update_prediction (kalman.cc UpdatePrediction) after the prediction launch
@@ -454,8 +477,8 @@ extern "C" __global__ void __launch_bounds__(kFilterThreads) kalman_prediction_k
   const int b = blockIdx.x, nv = A.nv, nx = A.nq + nv, ns = 2 * nv;
   if (A.status[b] != 0) return;
   double* W = A.scratch + (size_t)b * A.scratch_words;
-  double *rows = W + A.o_rows, *Am = W + A.o_F, *cols = W + A.o_ds, *PAt = W + A.o_P0;
-  double* P = A.P + (size_t)b * ns * ns;
+  double *rows = W + A.o_rows, *Am = W + A.o_F, *cols = W + A.o_ds, *PAt = W + A.o_P0, *Pn = W + A.o_Pn;
+  const double* P = A.P + (size_t)b * ns * ns;
   const double h = A.centered ? 2 * A.epsilon : A.epsilon;
   fb_load_next(A, b, rows);
   // column i of A: (next(x (+) eps e_i) (-) next(x [(+) -eps e_i])) / h
@@ -478,15 +501,11 @@ extern "C" __global__ void __launch_bounds__(kFilterThreads) kalman_prediction_k
     const int r = k / ns, c = k - r * ns;
     double s = 0;
     for (int j = 0; j < ns; j++) s = dadd(s, dmul(Am[(size_t)r * ns + j], PAt[(size_t)j * ns + c]));
-    P[k] = dadd(s, r == c ? A.noise_process[(size_t)b * ns + r] : 0.0);
+    Pn[k] = dadd(s, r == c ? A.noise_process[(size_t)b * ns + r] : 0.0);
   }
   __syncthreads();
-  fb_symmetrize(P, ns);
-  if (threadIdx.x == 0) {
-    for (int k = 0; k < nx; k++) A.state[(size_t)b * nx + k] = rows[k];
-    A.time[b] = dadd(A.time[b], A.timestep);
-  }
-  fb_commit(A, b, 0);
+  fb_symmetrize(Pn, ns);
+  fb_commit(A, b, rows, Pn, true, 0);   // the new state: the centre's next state, row 0
 }
 
 }  // namespace mjpc_dev

@@ -45,6 +45,15 @@ int LoadEstimatorBlob(const mjpc_model_blob* model, const HostModel& m, std::vec
   return 0;
 }
 
+// every one of the n values is finite (a NULL array has none)
+template <class T>
+bool AllFinite(const T* v, size_t n) {
+  if (v)
+    for (size_t i = 0; i < n; i++)
+      if (!std::isfinite(v[i])) return false;
+  return true;
+}
+
 }  // namespace
 
 Estimator::~Estimator() { if (engine_) mjpc_b200_destroy(engine_); }
@@ -108,6 +117,9 @@ int Estimator::Initialize(const mjpc_model_blob* model, int kind_, int num_filte
 int Estimator::Reset(int b, const double* state, double time, double covariance_scale, double process_scale,
                      double sensor_scale) {
   if (b < 0 || b >= num_filters) return Fail(MJPC_B200_ERR_BAD_ARGUMENT, "filter index outside [0, num_filters)");
+  if (!AllFinite(state, model_key_state_.size()) || !std::isfinite(time) || !std::isfinite(covariance_scale) ||
+      !std::isfinite(process_scale) || !std::isfinite(sensor_scale))
+    return Fail(MJPC_B200_ERR_BAD_ARGUMENT, "reset: a value is not finite");
   std::vector<double> P((size_t)ndstate * ndstate, 0.0), np(ndstate, process_scale), ns(nsensordata, sensor_scale);
   for (int i = 0; i < ndstate; i++) P[(size_t)i * ndstate + i] = covariance_scale;
   std::vector<float> warm(m_.nv, 0.f);
@@ -141,6 +153,8 @@ int Estimator::SetModels(const mjpc_model_blob* models, int count) {
 
 int Estimator::SetNoise(int b, const double* process, const double* sensor) {
   if (b < 0 || b >= num_filters) return Fail(MJPC_B200_ERR_BAD_ARGUMENT, "filter index outside [0, num_filters)");
+  if (!AllFinite(process, ndstate) || !AllFinite(sensor, nsensordata))
+    return Fail(MJPC_B200_ERR_BAD_ARGUMENT, "set_noise: a value is not finite");
   if (process)
     if (int rc = Access(engine_, b, mjpc_b200_bank::NOISE_PROCESS, const_cast<double*>(process), 1))
       return Fail(rc, mjpc_b200_last_error());
@@ -152,6 +166,9 @@ int Estimator::SetNoise(int b, const double* process, const double* sensor) {
 
 int Estimator::Set(int b, const double* state, const double* covariance, double time) {
   if (b < 0 || b >= num_filters) return Fail(MJPC_B200_ERR_BAD_ARGUMENT, "filter index outside [0, num_filters)");
+  if (!AllFinite(state, model_key_state_.size()) || !AllFinite(covariance, (size_t)ndstate * ndstate) ||
+      !std::isfinite(time))
+    return Fail(MJPC_B200_ERR_BAD_ARGUMENT, "set: a value is not finite");
   if (state)
     if (int rc = Access(engine_, b, mjpc_b200_bank::STATE, const_cast<double*>(state), 1))
       return Fail(rc, mjpc_b200_last_error());
@@ -171,11 +188,10 @@ int Estimator::Update(const double* ctrl, const double* sensor, const float* moc
       return Fail(rc, mjpc_b200_last_error());
     return 0;
   }
-  // ctrl in the engine's float; a NULL mocap is the model's for every filter
+  if (!AllFinite(sensor, (size_t)num_filters * nsensordata))
+    return Fail(MJPC_B200_ERR_BAD_ARGUMENT, "update: a sensor value is not finite");
+  if (int rc = StageInputs(ctrl, mocap)) return rc;
   const size_t nu = m_.nu, nm = model_mocap0_.size();
-  for (size_t i = 0; i < fctrl_.size(); i++) fctrl_[i] = (float)ctrl[i];
-  for (int b = 0; b < num_filters; b++)
-    std::copy_n((mocap ? mocap : mocap0_.data()) + b * nm, nm, fmocap_.begin() + b * nm);
   if (int rc = mjpc_b200_bank::Update(engine_, fctrl_.data(), sensor, fmocap_.data(), phases, status))
     return Fail(rc, mjpc_b200_last_error());
   for (int b = 0; b < num_filters; b++)
@@ -183,6 +199,34 @@ int Estimator::Update(const double* ctrl, const double* sensor, const float* moc
       std::copy_n(fctrl_.begin() + b * nu, nu, ctrl_.begin() + b * nu);
       std::copy_n(fmocap_.begin() + b * nm, nm, mocap_.begin() + b * nm);
     }
+  return 0;
+}
+
+int Estimator::StageInputs(const double* ctrl, const float* mocap) {
+  const size_t nm = model_mocap0_.size();
+  if (!AllFinite(ctrl, fctrl_.size()) || !AllFinite(mocap, (size_t)num_filters * nm))
+    return Fail(MJPC_B200_ERR_BAD_ARGUMENT, "update: a ctrl or mocap value is not finite");
+  // ctrl in the engine's float; a NULL mocap is the model's for every filter
+  for (size_t i = 0; i < fctrl_.size(); i++) fctrl_[i] = (float)ctrl[i];
+  for (int b = 0; b < num_filters; b++)
+    std::copy_n((mocap ? mocap : mocap0_.data()) + b * nm, nm, fmocap_.begin() + b * nm);
+  return 0;
+}
+
+int Estimator::DebugRows(int phase, const double* ctrl, const float* mocap, float* qpos, float* qvel, float* warm,
+                         int* status) {
+  if (!ctrl && m_.nu) return Fail(MJPC_B200_ERR_BAD_ARGUMENT, "debug_rows: bad argument");
+  if (int rc = StageInputs(ctrl, mocap)) return rc;
+  if (int rc = mjpc_b200_bank::DebugRows(engine_, phase, fctrl_.data(), fmocap_.data(), qpos, qvel, warm, status))
+    return Fail(rc, mjpc_b200_last_error());
+  return 0;
+}
+
+int Estimator::DebugFinish(int phase, const double* sensor, const float* next_qpos, const float* next_qvel,
+                           const float* qacc, const float* sensordata, const int* counts, int* status) {
+  if (int rc = mjpc_b200_bank::DebugFinish(engine_, phase, sensor, next_qpos, next_qvel, qacc, sensordata, counts,
+                                           status))
+    return Fail(rc, mjpc_b200_last_error());
   return 0;
 }
 
@@ -229,15 +273,17 @@ Estimator* Single(const mjpc_b200_estimator_t* h) {
   return reinterpret_cast<Estimator*>(const_cast<mjpc_b200_estimator_t*>(h));
 }
 
-// one update of a single filter; a failed factorisation is MJPC_B200_ERR_BAD_ARGUMENT with last_error naming the factor
+// one update of a single filter; a failed factorisation or a result that is not finite is MJPC_B200_ERR_BAD_ARGUMENT
+// with last_error naming it
 int UpdateSingle(Estimator* f, const double* ctrl, const double* sensor, const float* mocap, int phases) {
   if (!f) return MJPC_B200_ERR_BAD_ARGUMENT;
   int status = 0;
   if (int rc = f->Update(ctrl, sensor, mocap, phases, &status)) return rc;
   if (status == mjpc_b200_bank::UPDATED) return 0;
   f->error = std::string(f->Name()) + " update: " +
-             (status == mjpc_b200_bank::COVARIANCE_FACTOR_FAILED ? "covariance" : "sensor covariance") +
-             " factorisation failed";
+             (status == mjpc_b200_bank::COVARIANCE_FACTOR_FAILED ? "covariance factorisation failed"
+              : status == mjpc_b200_bank::SENSOR_FACTOR_FAILED   ? "sensor covariance factorisation failed"
+                                                                 : "non-finite result (state or covariance)");
   return MJPC_B200_ERR_BAD_ARGUMENT;
 }
 
@@ -348,6 +394,20 @@ int mjpc_b200_batch_estimator_get(void* f, int filter, double* state, double* co
 
 int mjpc_b200_batch_estimator_set_models(void* f, const mjpc_model_blob* models, int count) {
   return f && count >= 0 ? static_cast<Estimator*>(f)->SetModels(models, count) : MJPC_B200_ERR_BAD_ARGUMENT;
+}
+
+int mjpc_b200_batch_estimator_debug_rows(void* f, int phase, const double* ctrl, const float* mocap, float* qpos,
+                                         float* qvel, float* warm, int* status) {
+  return f ? static_cast<Estimator*>(f)->DebugRows(phase, ctrl, mocap, qpos, qvel, warm, status)
+           : MJPC_B200_ERR_BAD_ARGUMENT;
+}
+
+int mjpc_b200_batch_estimator_debug_finish(void* f, int phase, const double* sensor, const float* next_qpos,
+                                           const float* next_qvel, const float* qacc, const float* sensordata,
+                                           const int* counts, int* status) {
+  return f ? static_cast<Estimator*>(f)->DebugFinish(phase, sensor, next_qpos, next_qvel, qacc, sensordata, counts,
+                                                     status)
+           : MJPC_B200_ERR_BAD_ARGUMENT;
 }
 
 const char* mjpc_b200_batch_estimator_last_error(const void* f) {

@@ -17,6 +17,11 @@
 //  * a failed factorisation (the Unscented covariance, or either kind's sensor covariance) reports which factor failed
 //    and leaves the filter's state, covariance, time, warm start and warnings untouched (the reference calls
 //    mju_error);
+//  * a factorisation fails on a pivot below 1e-15 or one that is not finite (the reference's mju_cholFactor(.., 0)
+//    accepts pivots >= 0 and divides by a zero one);
+//  * an update whose new state or covariance would not be finite fails the same way, untouched (status
+//    NONFINITE_RESULT); ctrl, sensor and mocap values, and those of Reset, Set and SetNoise, that are not finite are
+//    refused with MJPC_B200_ERR_BAD_ARGUMENT and nothing changed (the reference takes them);
 //  * every row of a launch warm-starts the constraint solver from the centre (Kalman) or nominal (Unscented) row's qacc
 //    of the filter's previous successful launch (zeros after Reset); the reference reuses one mjData, so each row
 //    starts from the previous row's qacc;
@@ -61,6 +66,12 @@ class Estimator {
   // filter b's state, covariance, time and scalars {ndstate, rows, nsensordata, warnings, timestep} (Kalman: then
   // epsilon); any pointer may be NULL
   int Get(int b, double* state, double* covariance, double* time, double* scalars);
+  // test hooks (mjpc_b200_bank::DebugRows / DebugFinish): the step rows of `phase` from ctrl [B][nu] and mocap
+  // [B][7 nmocap] (NULL: the model's), and that phase's update from the caller's step outputs; status [B] is the raw
+  // mjpc_b200_bank::Status
+  int DebugRows(int phase, const double* ctrl, const float* mocap, float* qpos, float* qvel, float* warm, int* status);
+  int DebugFinish(int phase, const double* sensor, const float* next_qpos, const float* next_qvel, const float* qacc,
+                  const float* sensordata, const int* counts, int* status);
   // filter b runs on models[b] from now on (mjpc_b200_set_model_variants), and its Reset state and default mocap are
   // that model's; count is num_filters, or 0 for the bank's model again.  The filters' states are kept.
   int SetModels(const mjpc_model_blob* models, int count);
@@ -72,6 +83,9 @@ class Estimator {
 
  private:
   int Fail(int rc, const std::string& what);
+  // ctrl [B][nu] in float and mocap [B][7 nmocap] (NULL: each filter's model's) into fctrl_ / fmocap_; refuses values
+  // that are not finite
+  int StageInputs(const double* ctrl, const float* mocap);
   mjpc_b200_t* engine_ = nullptr;
   HostModel m_;
   int nmocap_ = 0;

@@ -20,7 +20,10 @@ Reference semantics restated (unscented.cc):
 
 Documented differences from the reference:
   * a failed factorisation (covariance or sensor covariance) raises ``EstimatorError`` naming the factor and leaves
-    state, covariance and time untouched (the reference calls mju_error);
+    state, covariance and time untouched (the reference calls mju_error).  A factorisation fails on a pivot below
+    CHOL_MIN_PIVOT or one that is not finite (the reference's mju_cholFactor(.., 0) accepts pivots >= 0);
+  * an update whose new state or covariance would not be finite raises ``EstimatorError`` ("non-finite result") and
+    leaves the filter untouched;
   * every sigma point warm-starts the constraint solver from the nominal point's qacc of the previous update (zeros
     after reset); the reference reuses one mjData, so each point starts from the previous point's qacc.  The Newton
     solution is unique to the solver tolerance, so this changes results only at that level;
@@ -52,6 +55,30 @@ from .mjcf import JNT_BALL, JNT_FREE, SENS_MEASURED
 
 class EstimatorError(RuntimeError):
     pass
+
+
+CHOL_MIN_PIVOT = 1e-15   # the device factorisation's pivot threshold (csrc/estimator_kernels.cuh fb_chol_factor)
+
+
+def cholesky(M, what):
+    """Lower Cholesky factor of M; EstimatorError naming `what` when a pivot M_jj - sum_k<j L_jk^2 is below
+    CHOL_MIN_PIVOT or any entry is not finite (LAPACK accepts any positive pivot and may return a NaN factor without
+    raising)."""
+    try:
+        L = np.linalg.cholesky(M)
+    except np.linalg.LinAlgError:
+        L = None
+    if L is None or not np.all(np.isfinite(L)) or \
+            not np.all(np.diag(M) - np.sum(np.tril(L, -1) ** 2, axis=1) >= CHOL_MIN_PIVOT):
+        raise EstimatorError(what + " factorisation failed")
+    return L
+
+
+def _finite_result(state, covariance):
+    """(state, covariance), or EstimatorError when either is not finite (the filter then keeps what it had)."""
+    if not (np.all(np.isfinite(state)) and np.all(np.isfinite(covariance))):
+        raise EstimatorError("non-finite result (state or covariance)")
+    return state, covariance
 
 
 def _number(m, name, default):
@@ -263,10 +290,7 @@ class _Filter:
     @staticmethod
     def _gain(X, S, P0, innovation):
         """(X S^-1 innovation, the symmetrised P0 - X S^-1 X'); EstimatorError when S does not factor."""
-        try:
-            L = np.linalg.cholesky(S)
-        except np.linalg.LinAlgError:
-            raise EstimatorError("sensor covariance factorisation failed") from None
+        L = cholesky(S, "sensor covariance")
         solve = lambda b: np.linalg.solve(L.T, np.linalg.solve(L, b))
         P = P0 - X @ solve(X.T)
         return X @ solve(innovation), 0.5 * (P + P.T)
@@ -300,10 +324,7 @@ class Unscented(_Filter):
         """SigmaPoints (unscented.cc:293-349): [nsigma][nq+nv], nominal last."""
         m = self.m
         nq, nv = m.nq, m.nv
-        try:
-            L = np.linalg.cholesky(self.covariance)
-        except np.linalg.LinAlgError:
-            raise EstimatorError("covariance factorisation failed") from None
+        L = cholesky(self.covariance, "covariance")
         pts = np.zeros((self.nsigma, nq + nv))
         pts[-1] = self.state
         for i in range(self.ndstate):
@@ -349,8 +370,8 @@ class Unscented(_Filter):
         cov_yy = np.diag(self.noise_sensor) + (dy.T * wc) @ dy
         cov_sy = (ds.T * wc) @ dy
         cov_ss = np.diag(self.noise_process) + (ds.T * wc) @ ds
-        corr, self.covariance = self._gain(cov_sy, cov_yy, cov_ss, np.asarray(sensor, float) - y_mean)
-        self.state = self._state_add(s_mean, corr)
+        corr, P = self._gain(cov_sy, cov_yy, cov_ss, np.asarray(sensor, float) - y_mean)
+        self.state, self.covariance = _finite_result(self._state_add(s_mean, corr), P)
         self.time = self.time + self.timestep
         self._commit(qacc[-1], nwarn)
         return self.state
@@ -379,7 +400,7 @@ class _CppFilter(_CppObject):
     def _check(self, rc):
         if rc != 0:
             msg = self.lib.mjpc_b200_estimator_last_error(self.h).decode()
-            if "factorisation" in msg:
+            if "factorisation" in msg or "non-finite result" in msg:
                 raise EstimatorError(msg)
             raise EngineError(f"{self._prefix} error {rc}: {msg}")
 
@@ -490,8 +511,8 @@ class Kalman(_Filter):
         P = self.covariance
         PCt = P @ C.T
         S = C @ PCt + np.diag(self.noise_sensor)
-        corr, self.covariance = self._gain(PCt, S, P, np.asarray(sensor, float) - y[0])
-        self.state = self._state_add(self.state, corr)
+        corr, Pn = self._gain(PCt, S, P, np.asarray(sensor, float) - y[0])
+        self.state, self.covariance = _finite_result(self._state_add(self.state, corr), Pn)
         self.ctrl, self.mocap = np.atleast_1d(np.asarray(ctrl, float)).copy(), mocap
         self._commit(qacc[0], nwarn)
         return self.state
@@ -506,7 +527,7 @@ class Kalman(_Filter):
             return np.concatenate([differentiate_pos(m, nxt[b, :nq], nxt[a, :nq]), nxt[a, nq:] - nxt[b, nq:]])
         A = np.stack([self._column(diff, i) for i in range(self.ndstate)], axis=1)
         P = A @ self.covariance @ A.T + np.diag(self.noise_process)
-        self.state, self.covariance = nxt[0].copy(), 0.5 * (P + P.T)
+        self.state, self.covariance = _finite_result(nxt[0].copy(), 0.5 * (P + P.T))
         self.time = self.time + self.timestep
         self._commit(qacc[0], nwarn)
         return self.state
@@ -612,6 +633,38 @@ class CppBatchEstimator(_CppObject):
     def get(self, b):
         """(state, covariance, time, scalars) of filter b."""
         return _get_filter(self, functools.partial(self.lib.mjpc_b200_batch_estimator_get, self.h, b))
+
+    def debug_rows(self, phase, ctrl=None, mocap=None):
+        """The bank's row kernel alone (mjpc_b200_batch_estimator_debug_rows; phase 0 Unscented, 1 Kalman measurement,
+        2 Kalman prediction) from ctrl [B][nu] (None: zeros) and mocap (None: the model's): (qpos [B][rows][nq],
+        qvel [B][rows][nv], the rows' warm starts [B][rows][nv], status [B])."""
+        B, R, m = self.num_filters, self.rows, self.m
+        u = np.ascontiguousarray(np.zeros((B, m.nu)) if ctrl is None else np.asarray(ctrl, float).reshape(B, m.nu))
+        mc = None if mocap is None or np.size(mocap) == 0 else \
+            np.ascontiguousarray(np.asarray(mocap, np.float32).reshape(B, -1))
+        qpos, qvel = np.zeros((B, R, m.nq), np.float32), np.zeros((B, R, m.nv), np.float32)
+        warm = np.zeros((B, R, m.nv), np.float32)
+        status = np.zeros(B, np.int32)
+        self._check(self.lib.mjpc_b200_batch_estimator_debug_rows(
+            self.h, int(phase), _pd(u), _pf(mc), _pf(qpos), _pf(qvel), _pf(warm),
+            status.ctypes.data_as(C.POINTER(C.c_int))))
+        return qpos, qvel, warm, status
+
+    def debug_finish(self, phase, sensor, next_qpos, next_qvel, qacc, sensordata, counts):
+        """The phase's update kernel on the caller's step outputs (mjpc_b200_batch_estimator_debug_finish):
+        sensor [B][nsensordata] (None for phase 2), next_qpos [B][rows][nq], next_qvel / qacc [B][rows][nv],
+        sensordata [B][rows][nsensordata] (float32) and counts [B][rows][4] (int32); returns the raw status [B]."""
+        B, R, m = self.num_filters, self.rows, self.m
+        f32 = lambda a, n: np.ascontiguousarray(np.asarray(a, np.float32).reshape(B, R, n))
+        nq, nv, ys, qa = f32(next_qpos, m.nq), f32(next_qvel, m.nv), f32(sensordata, self.nsensordata), f32(qacc, m.nv)
+        cn = np.ascontiguousarray(np.asarray(counts, np.int32).reshape(B, R, 4))
+        y = None if sensor is None else np.ascontiguousarray(np.asarray(sensor, float).reshape(B, self.nsensordata))
+        status = np.zeros(B, np.int32)
+        ip = C.POINTER(C.c_int)
+        self._check(self.lib.mjpc_b200_batch_estimator_debug_finish(
+            self.h, int(phase), _pd(y), _pf(nq), _pf(nv), _pf(qa), _pf(ys), cn.ctypes.data_as(ip),
+            status.ctypes.data_as(ip)))
+        return status
 
     def state(self, b):
         return self.get(b)[0]
