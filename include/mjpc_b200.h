@@ -218,9 +218,12 @@ int mjpc_b200_debug_ensemble_score(mjpc_b200_t* h, const float* member_returns, 
  * for the velocity half (a zero entry keeps the coordinate bit for bit).  z is a standard normal: Philox4x32-10 with key
  * (seed + b, 3) and counter (iteration, k, element, 'BELF'), Box-Muller in double on the first two words; key word 3 is
  * used by no candidate-noise or plant-noise draw.  The factor, L z and (+) are computed in double on the device (one
- * CTA per problem), and the member states are written as float straight into the launch's state rows.  A pivot of
- * exactly 0 whose column below is all zero gives a zero column, so a zero covariance gives K copies of the mean and
- * scores equal to the plain launch's returns.
+ * CTA per problem), and the member states are written as float straight into the launch's state rows.  The pivot
+ * of row j within tau_j = n 2^-40 P_jj of 0 whose column below holds only rounded couplings (A_ij^2 <= 4 tau_j
+ * (max(A_ii, 0) + tau_i)) gives a zero column, so a positive semi-definite but rank-deficient covariance draws only
+ * along the directions it spans, and a zero covariance gives K copies of the mean and scores equal to the plain
+ * launch's returns.  A diagonal covariance, and a positive definite one with cond below 2^40 / n, is factored as
+ * without the tolerance.
  * The launch holds B*K*N trajectories, member k of problem b as launch problem b*K + k (the model ensemble's layout):
  * returns / failure / order are the scores [B][N], fetch_ensemble gives the member returns [B][K][N],
  * fetch_trajectory_member any member's trajectory and fetch_trajectory / fetch_all member 0's.  With model variants
@@ -232,8 +235,8 @@ int mjpc_b200_debug_ensemble_score(mjpc_b200_t* h, const float* member_returns, 
  * set on the handle: MJPC_B200_ERR_UNSUPPORTED naming the call.  As set_model_ensemble does, the call grows the
  * per-trajectory device buffers to K x max_candidates trajectories (never shrinks them; MJPC_B200_ERR_CUDA if that
  * fails), so the launch holds up to K x max_candidates trajectories; it also allocates its own tables once.  A
- * covariance whose factorisation fails (a pivot < 0,
- * a zero pivot with a non-zero column below, or a non-finite pivot) returns MJPC_B200_ERR_BAD_ARGUMENT with last_error
+ * covariance whose factorisation fails (a pivot < -tau,
+ * a pivot within tau of 0 with a coupling below it, or a non-finite pivot) returns MJPC_B200_ERR_BAD_ARGUMENT with last_error
  * naming the problem, and no rollout is launched and no returns are written; the handle stays usable. */
 int mjpc_b200_rollout_spline_belief_batched(mjpc_b200_t* h, int B, int K, int worst, uint32_t seed, uint32_t iteration,
                                             const float* states, const double* covariances, const double* times,
@@ -426,7 +429,7 @@ int mjpc_b200_plant_get(mjpc_b200_t* h, int plant, float* state, float* warmstar
 /* Disturbances (the reference app's control noise and force perturbations, app.cc:95-101, 291-304, 323-352).  Before
  * each step of a running plant:
  *   control noise  n <- r n + s z per actuator, r = exp(-timestep / ctrl_rate), s = ctrl_std sqrt(1 - r^2), added to the
- *                  commanded ctrl; actuation clamps the sum to ctrlrange as it clamps any ctrl
+ *                  commanded ctrl (r and s in fp32 as 1 + expm1 and sqrt(-expm1), accurate for any rate > 0); actuation clamps the sum to ctrlrange as it clamps any ctrl
  *   force noise    the same recursion (xfrc_std, xfrc_rate) over the 6 nbody entries of xfrc_applied, as the Robust
  *                  planner's rollouts draw it
  *   xfrc_applied   = the held wrench + the force noise: per body force 3 then torque 3, world frame, at the body's

@@ -2,7 +2,8 @@
 // problem of a launch, drawn on the device from the problem's state covariance, and the same arithmetic on the host
 // (mjpc_b200_host_state_member).
 //
-//   state_sample_kernel   one CTA per problem: the Cholesky factor L of (P + P')/2 in fp64 (shared memory), then for
+//   state_sample_kernel   one CTA per problem: the Cholesky factor L of (P + P')/2 in fp64 (shared memory; pivots
+//                         within belief_tolerance of zero give zero columns), then for
 //                         each member k >= 1 the tangent vector dx = L z and the state mean (+) dx written as float
 //                         into launch row b K + k.  Row b K (member 0) keeps the mean as staged.
 //
@@ -40,15 +41,29 @@ __host__ __device__ inline double belief_normal(unsigned seed, unsigned iteratio
   return sqrt(-2.0 * log(u1)) * cos(6.283185307179586 * u2);
 }
 
-// Step j of the right-looking factorisation of the symmetric lower triangle A (row-major n x n): the pivot.  A pivot
-// > 0 gives L[j][j] = sqrt(pivot); a pivot of exactly 0 whose column below is all zero gives a zero column (a state
-// direction with no uncertainty); anything else (a negative, zero-with-coupling or non-finite pivot) fails: false.
-__host__ __device__ inline bool belief_pivot(double* A, int n, int j) {
+// The pivot tolerances of the factorisation of the symmetric n x n matrix A (row-major, lower triangle read), one per
+// row: tau[i] = n 2^-40 max(A_ii, 0).  The pivot of row j is A_jj minus the squares of row j of L, which sum to A_jj
+// in exact arithmetic, so without pivoting its rounding is about n eps A_jj times the growth that the leading block's
+// conditioning adds; tau allows a growth of 2^12.  A positive definite A has every pivot at or above its smallest
+// eigenvalue and tau[j] <= n 2^-40 times its largest, so with cond(A) below 2^40 / n it is factored exactly as
+// without the tolerance; so is any diagonal A.
+__host__ __device__ inline void belief_tolerance(const double* A, int n, int i, double* tau) {
+  tau[i] = A[i * n + i] > 0.0 ? n * 0x1p-40 * A[i * n + i] : 0.0;
+}
+// Step j of the right-looking factorisation of the symmetric lower triangle A (row-major n x n): the pivot d.
+// d > tau[j] gives L[j][j] = sqrt(d).  |d| <= tau[j] is a rounded zero: the column becomes zero (a state direction
+// with no uncertainty) when every entry below it is a rounded coupling of a positive semi-definite trailing block too,
+// A_ij^2 <= 4 tau[j] (max(A_ii, 0) + tau[i]) (exactly, A_ij^2 <= d A_ii, with d and A_ii each off by up to their
+// tolerance).  Anything else (d < -tau[j], a real coupling below a zero pivot, a non-finite pivot) fails: false.
+__host__ __device__ inline bool belief_pivot(double* A, int n, int j, const double* tau) {
   const double d = A[j * n + j];
-  if (d > 0.0) { A[j * n + j] = sqrt(d); return true; }
-  if (!(d == 0.0)) return false;
-  for (int i = j + 1; i < n; i++)
-    if (A[i * n + j] != 0.0) return false;
+  if (d > tau[j] && d <= 1.7976931348623157e308) { A[j * n + j] = sqrt(d); return true; }
+  if (!(fabs(d) <= tau[j])) return false;
+  for (int i = j + 1; i < n; i++) {
+    const double a = A[i * n + j], aii = A[i * n + i] > 0.0 ? A[i * n + i] : 0.0;
+    if (!(a * a <= 4.0 * tau[j] * (aii + tau[i]))) return false;
+  }
+  A[j * n + j] = 0.0;
   return true;
 }
 // below the pivot of column j: L[i][j] = A[i][j] / L[j][j] (0 for a zero column)
@@ -114,8 +129,9 @@ struct BeliefArgs {
   int* status;                 // out [B]: 0, or 1 when the factorisation failed (no row of the problem is written)
 };
 
-// dynamic shared memory of state_sample_kernel for tangent dimension n: L [n][n], z [n], dx [n], the mean [nq + nv]
-inline size_t belief_smem(int n, int nq, int nv) { return ((size_t)n * n + 2 * (size_t)n + nq + nv) * sizeof(double); }
+// dynamic shared memory of state_sample_kernel for tangent dimension n: L [n][n], z [n], dx [n], the pivot tolerances
+// [n], the mean [nq + nv]
+inline size_t belief_smem(int n, int nq, int nv) { return ((size_t)n * n + 3 * (size_t)n + nq + nv) * sizeof(double); }
 
 extern "C" __global__ void __launch_bounds__(kBeliefThreads) state_sample_kernel(const BeliefArgs A) {
   extern __shared__ double s_belief[];
@@ -123,7 +139,8 @@ extern "C" __global__ void __launch_bounds__(kBeliefThreads) state_sample_kernel
   double* L = s_belief;
   double* z = L + (size_t)n * n;
   double* dx = z + n;
-  double* mean = dx + n;
+  double* tau = dx + n;
+  double* mean = tau + n;
   const int R = b * A.K;
   if (A.variant_index && tid < A.K) A.row_index[R + tid] = A.variant_index[b];
   // (P + P') / 2, lower triangle
@@ -136,8 +153,10 @@ extern "C" __global__ void __launch_bounds__(kBeliefThreads) state_sample_kernel
   __shared__ int ok;
   if (tid == 0) ok = 1;
   __syncthreads();
+  for (int i = tid; i < n; i += blockDim.x) belief_tolerance(L, n, i, tau);
+  __syncthreads();
   for (int j = 0; j < n; j++) {
-    if (tid == 0 && !belief_pivot(L, n, j)) ok = 0;
+    if (tid == 0 && !belief_pivot(L, n, j, tau)) ok = 0;
     __syncthreads();
     if (!ok) break;
     for (int i = j + 1 + tid; i < n; i += blockDim.x) belief_column(L, n, j, i);

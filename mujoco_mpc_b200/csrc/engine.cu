@@ -1140,7 +1140,9 @@ int mjpc_b200_rollout_spline_belief_batched(mjpc_b200_t* h, int B, int K, int wo
   for (int b = 0; b < B; b++)
     if (status[b])
       return fail(MJPC_B200_ERR_BAD_ARGUMENT, std::string(call) + ": problem " + std::to_string(b) +
-                                                  ": the covariance is not positive semi-definite (a pivot <= 0)");
+                                                  ": the covariance is not positive semi-definite (a pivot below -tau, or a "
+                                                  "pivot within tau of 0 with a coupling below it; "
+                                                  "tau = 2 nv 2^-40 P_jj)");
   if (h->nvariants) A.pack_index = h->d_belief;
   A.returns = h->d_member_returns; A.failure = h->d_member_failure;
   A.L = make_layout(M, P);
@@ -1170,8 +1172,10 @@ int mjpc_b200_host_state_member(const mjpc_model_blob* model, const double* stat
   std::vector<double> L((size_t)n * n, 0.0), z(n), dx(n);
   for (int i = 0; i < n; i++)
     for (int c = 0; c <= i; c++) L[(size_t)i * n + c] = 0.5 * (covariance[i * n + c] + covariance[c * n + i]);
+  std::vector<double> tau(n);
+  for (int i = 0; i < n; i++) belief_tolerance(L.data(), n, i, tau.data());
   for (int j = 0; j < n; j++) {   // state_sample_kernel's order
-    if (!belief_pivot(L.data(), n, j))
+    if (!belief_pivot(L.data(), n, j, tau.data()))
       return fail(MJPC_B200_ERR_BAD_ARGUMENT, "host_state_member: the covariance is not positive semi-definite");
     for (int i = j + 1; i < n; i++) belief_column(L.data(), n, j, i);
     for (int i = j + 1; i < n; i++)

@@ -184,8 +184,24 @@ __device__ __forceinline__ float philox_normal(unsigned c0, unsigned c1, unsigne
     c0 = n0; c1 = lo1; c2 = n2; c3 = lo0;
     k0 += 0x9E3779B9u; k1 += 0xBB67AE85u;
   }
-  const float u1 = ((float)c0 + 0.5f) * 2.3283064365386963e-10f, u2 = ((float)c1 + 0.5f) * 2.3283064365386963e-10f;
-  return sqrtf(-2.0f * logf(fmaxf(u1, 1e-12f))) * cospif(2.0f * u2);
+  // log u1, u1 = (c0 + 0.5) 2^-32, without rounding c0 to 24 bits where that matters: above 2^31 as log1p of minus the
+  // complement (~c0 + 0.5) 2^-32, so the top counters keep their distance from u1 = 1 (fp32 u1 would round to 1 and
+  // give z = 0 for the top 128 counters); below it u1 <= 1/2 and logf's relative error is what a rounded c0 adds.
+  // -use_fast_math remaps logf to __logf, not log1pf.
+  const float l1 = c0 >= 0x80000000u ? log1pf(-((float)(~c0) + 0.5f) * 2.3283064365386963e-10f)
+                                     : logf(((float)c0 + 0.5f) * 2.3283064365386963e-10f);
+  const float u2 = ((float)c1 + 0.5f) * 2.3283064365386963e-10f;
+  return sqrtf(-2.0f * l1) * cospif(2.0f * u2);
+}
+
+// The Ornstein-Uhlenbeck coefficients of a noise of stationary std `std_` and time constant `rate` seconds over a step
+// dt: n <- r n + s z with r = exp(-dt / rate) and s = std sqrt(1 - r^2), written as 1 + expm1 and sqrt(-expm1) so that
+// neither cancels when rate >> dt (1 - r r in fp32 loses s entirely from rate ~ 1e6 dt), and r <= 1 always.
+// -use_fast_math does not remap expm1f; the division is the correctly rounded one.
+struct OUCoefficients { float r, s; };
+__device__ __forceinline__ OUCoefficients ou_coefficients(float dt, float std_, float rate) {
+  const float x = __fdiv_rn(-dt, rate);
+  return {1.f + expm1f(x), std_ * sqrtf(-expm1f(2.f * x))};
 }
 
 // Injected noise of NoisyRollout: key (seed, 1), counter (step, stream, element, 'XFRC') - the definition of
@@ -283,8 +299,8 @@ __device__ __forceinline__ void rollout_body(const RolloutArgs& A) {
   }
   for (int i = lane; i < nv * nv; i += 32) DF(qM)[i] = 0;
   const bool noisy = A.xfrc_std > 0.f;
-  const float ou_rate = noisy ? expf(-CM(c).timestep / A.xfrc_rate) : 0.f;
-  const float ou_scale = noisy ? A.xfrc_std * sqrtf(1.f - ou_rate * ou_rate) : 0.f;
+  const OUCoefficients ou = noisy ? ou_coefficients(CM(c).timestep, A.xfrc_std, A.xfrc_rate) : OUCoefficients{0.f, 0.f};
+  const float ou_rate = ou.r, ou_scale = ou.s;
   // the noise key and stream of this candidate: kept in shared memory rather than in registers across the step loop:
   // two more live registers there made the Quadruped one-warp and Humanoid Track helper-warp instances spill
   __shared__ unsigned noise_ks[2];
@@ -654,7 +670,7 @@ struct PlantArgs {
 };
 
 // The disturbances of plant b's coming step, between load_state and k_forward (app.cc:291-304, 95-101, 323-352):
-// control noise n <- r n + s z (r = exp(-timestep / rate), s = std sqrt(1 - r^2)) added to the ctrl, which actuation
+// control noise n <- r n + s z (r = exp(-timestep / rate), s = std sqrt(1 - r^2), ou_coefficients) added to the ctrl, which actuation
 // clamps as any ctrl; xfrc = the held wrench + the force noise's state under the same recursion.  The advanced states go
 // to noise_next; the applied ctrl is written out.
 template <class SP>
@@ -665,7 +681,8 @@ __device__ __forceinline__ void plant_disturb(Ctx& c, const PlantArgs& A, int b)
   const unsigned step = (unsigned)A.steps[b];
   float* next = A.noise_next + (size_t)b * (nu + nx);
   if (d.ctrl_std > 0.f) {
-    const float r = expf(-CM(c).timestep / d.ctrl_rate), s = d.ctrl_std * sqrtf(1.f - r * r);
+    const OUCoefficients ou = ou_coefficients(CM(c).timestep, d.ctrl_std, d.ctrl_rate);
+    const float r = ou.r, s = ou.s;
     const float* n = A.ctrl_noise + (size_t)b * nu;
     for (int i = lane; i < nu; i += 32) {
       const float v = r * n[i] + s * plant_normal(d.seed, step, (unsigned)i, kPlantTagCtrl);
@@ -676,7 +693,8 @@ __device__ __forceinline__ void plant_disturb(Ctx& c, const PlantArgs& A, int b)
   for (int i = lane; i < nu; i += 32) A.ctrl_out[(size_t)b * nu + i] = DF(ctrl)[i];
   const float* held = A.xfrc_held + (size_t)b * nx;
   if (d.xfrc_std > 0.f) {
-    const float r = expf(-CM(c).timestep / d.xfrc_rate), s = d.xfrc_std * sqrtf(1.f - r * r);
+    const OUCoefficients ou = ou_coefficients(CM(c).timestep, d.xfrc_std, d.xfrc_rate);
+    const float r = ou.r, s = ou.s;
     const float* n = A.xfrc_noise + (size_t)b * nx;
     for (int i = lane; i < nx; i += 32) {
       const float v = r * n[i] + s * plant_normal(d.seed, step, (unsigned)i, kPlantTagXfrc);

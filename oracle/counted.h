@@ -42,7 +42,7 @@ ORACLE_BINOP(+) ORACLE_BINOP(-) ORACLE_BINOP(*) ORACLE_BINOP(/)
 ORACLE_CMP(<) ORACLE_CMP(>) ORACLE_CMP(<=) ORACLE_CMP(>=) ORACLE_CMP(==) ORACLE_CMP(!=)
 #undef ORACLE_CMP
 #define ORACLE_FN1(name) inline Counted name(Counted a) { Counted::flops++; return Counted(std::name(a.v)); }
-ORACLE_FN1(sqrt) ORACLE_FN1(exp) ORACLE_FN1(log) ORACLE_FN1(sin) ORACLE_FN1(cos) ORACLE_FN1(cosh) ORACLE_FN1(sinh)
+ORACLE_FN1(sqrt) ORACLE_FN1(exp) ORACLE_FN1(expm1) ORACLE_FN1(log) ORACLE_FN1(sin) ORACLE_FN1(cos) ORACLE_FN1(cosh) ORACLE_FN1(sinh)
 #undef ORACLE_FN1
 inline Counted fabs(Counted a) { return Counted(std::fabs(a.v)); }
 inline Counted pow(Counted a, Counted b) { Counted::flops++; return Counted(std::pow(a.v, b.v)); }
@@ -54,6 +54,7 @@ namespace mm {
 template <class T> inline T sqrt(T x) { using std::sqrt; return sqrt(x); }
 template <class T> inline T fabs(T x) { using std::fabs; return fabs(x); }
 template <class T> inline T exp(T x) { using std::exp; return exp(x); }
+template <class T> inline T expm1(T x) { using std::expm1; return expm1(x); }
 template <class T> inline T log(T x) { using std::log; return log(x); }
 template <class T> inline T sin(T x) { using std::sin; return sin(x); }
 template <class T> inline T cos(T x) { using std::cos; return cos(x); }

@@ -116,8 +116,10 @@ void rollout(Trajectory<T>& tr, const Policy<T>& policy, const Model<T>& m, cons
     policy(&tr.actions[t * nu], &tr.states[t * ds], d.time, t);
     for (int i = 0; i < nu; i++) d.ctrl[i] = tr.actions[t * nu + i];
     if (noise.std > 0) {   // Ornstein-Uhlenbeck perturbation in discrete time (trajectory.cc:147-155)
-      const T rate = mm::exp(-m.timestep / (T)noise.rate);
-      const T scale = (T)noise.std * mm::sqrt(1 - rate * rate);
+      // as 1 + expm1 and sqrt(-expm1), the device's ou_coefficients: 1 - rate^2 cancels in fp32 for rate >> timestep
+      const T x = -m.timestep / (T)noise.rate;
+      const T rate = 1 + mm::expm1(x);
+      const T scale = (T)noise.std * mm::sqrt(-mm::expm1(2 * x));
       for (int i = 0; i < 6 * m.nbody; i++)
         d.xfrc_applied[i] = rate * d.xfrc_applied[i] + scale * (T)xfrc_normal(noise.seed, (uint32_t)t, noise.stream, (uint32_t)i);
     }
